@@ -27,7 +27,7 @@ struct UpdArgs : BatchArrays {
 
 template <typename real>
 __host__ __device__ inline size_t upd_smem_layout(int N, int Mp, int warps, size_t *o_dxi, size_t *o_x, size_t *o_seg, size_t *o_red, size_t *o_ring) {
-    size_t off = sizeof(double) * 12 * (size_t)N;                  // candidate camera poses: Rwc[9], c[3]
+    size_t off = sizeof(FrameSm) * (size_t)N;                      // candidate camera poses
     *o_dxi = off; off += sizeof(double) * 6 * (size_t)N;           // xi = T delta per frame
     *o_x = off; off += sizeof(double) * 3 * (size_t)Mp;            // candidate world points (SoA)
     *o_red = off; off += sizeof(double) * 8;
@@ -86,7 +86,7 @@ update_obs_kernel(UpdArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     size_t o_dxi, o_x, o_seg, o_red, o_ring;
     upd_smem_layout<real>(N, Mp, kWarps, &o_dxi, &o_x, &o_seg, &o_red, &o_ring);
-    double *Fc = reinterpret_cast<double *>(smem_raw);                  // [N][12] candidate state
+    FrameSm *Fc = reinterpret_cast<FrameSm *>(smem_raw);                // [N] candidate camera poses
     double *dxi = reinterpret_cast<double *>(smem_raw + o_dxi);         // [N][6]
     double *xs = reinterpret_cast<double *>(smem_raw + o_x);            // [3][Mp]
     double *red = reinterpret_cast<double *>(smem_raw + o_red);         // [8]
@@ -94,108 +94,117 @@ update_obs_kernel(UpdArgs a) {
 
     const double step_a = kMode == 2 ? ctrl.step_a : a.step_a;
     const double step_b = kMode == 2 ? ctrl.step_b : a.step_b;
-    if (tid < N) {
+    // the candidate poses (warp 0) and the frame steps xi (warp 1) are independent: in separate warps, neither adds to
+    // the other's registers
+    static_assert(kThreads >= 32 + kMaxFrames, "update_obs_kernel: warp 1 computes the frame steps");
+    if (kMode != 1 && tid < N) {
         const double *fs = a.frames + ((size_t)w * a.Ncap + tid) * kFrameStride;
         const double *d = a.dx_pose + ((size_t)w * a.Ncap + tid) * 15;
-        if (kMode != 1) {
-            double fc[kFrameStride];
-            const double *vp = a.v_pose + ((size_t)w * a.Ncap + tid) * 15;
-            double de[15];
+        const double *vp = a.v_pose + ((size_t)w * a.Ncap + tid) * 15;
+        // only the candidate pose stays in registers; the rest of the candidate state goes straight to frames_cand
+        auto step = [&](int i) { return step_b * d[i] - (step_a != 0.0 ? step_a * vp[i] : 0.0); };
+        double fc[7];
+        {
+            const double dr[3] = {step(0), step(1), step(2)};
+            quat_plus(fs, dr, fc);
+        }
 #pragma unroll
-            for (int i = 0; i < 15; ++i) de[i] = step_b * d[i] - (step_a != 0.0 ? step_a * vp[i] : 0.0);
-            quat_plus(fs, de, fc);
+        for (int i = 4; i < 7; ++i) fc[i] = fs[i] + step(i - 1);
+        if (blockIdx.x == 0) {
+            double *o = a.frames_cand + ((size_t)w * a.Ncap + tid) * kFrameStride;
+            double amb = 0.0;
 #pragma unroll
-            for (int i = 0; i < 12; ++i) fc[4 + i] = fs[4 + i] + de[3 + i];
-            FrameSm f;
-            make_frame(fc, wc, f);
-#pragma unroll
-            for (int i = 0; i < 9; ++i) Fc[tid * 12 + i] = f.Rwc[i];
-#pragma unroll
-            for (int i = 0; i < 3; ++i) Fc[tid * 12 + 9 + i] = f.c[i];
-            if (blockIdx.x == 0) {
-                double *o = a.frames_cand + ((size_t)w * a.Ncap + tid) * kFrameStride;
-                double amb = 0.0;
-#pragma unroll
-                for (int i = 0; i < kFrameStride; ++i) {
-                    o[i] = fc[i];
-                    const bool pose = i < 7;
-                    const bool live = pose ? !((H.fixed_mask >> tid) & 1) : (H.use_inertial != 0);
-                    if (live) amb += (fc[i] - fs[i]) * (fc[i] - fs[i]);
-                }
-                atomicAdd(&a.acc[(size_t)w * kAcc + 6], amb);
+            for (int i = 0; i < kFrameStride; ++i) {
+                const double v = i < 7 ? fc[i] : fs[i] + step(i - 1);
+                o[i] = v;
+                const bool pose = i < 7;
+                const bool live = pose ? !((H.fixed_mask >> tid) & 1) : (H.use_inertial != 0);
+                if (live) amb += (v - fs[i]) * (v - fs[i]);
             }
+            atomicAdd(&a.acc[(size_t)w * kAcc + 6], amb);
         }
-        if (kMode != 2) {
-            double R[9], om[3];
-            quat_to_mat(fs, R);
-            mat3_vec(R, d, om);
-            const double p0 = fs[4] - wc.origin[0], p1 = fs[5] - wc.origin[1], p2 = fs[6] - wc.origin[2];
-            dxi[tid * 6 + 0] = om[0]; dxi[tid * 6 + 1] = om[1]; dxi[tid * 6 + 2] = om[2];
-            dxi[tid * 6 + 3] = -(p1 * om[2] - p2 * om[1]) - d[3];
-            dxi[tid * 6 + 4] = -(p2 * om[0] - p0 * om[2]) - d[4];
-            dxi[tid * 6 + 5] = -(p0 * om[1] - p1 * om[0]) - d[5];
-        }
+        make_frame(fc, wc, Fc[tid]);
+    }
+    if (kMode != 2 && tid >= 32 && tid < 32 + N) {
+        const int f = tid - 32;
+        const double *fs = a.frames + ((size_t)w * a.Ncap + f) * kFrameStride;
+        const double *d = a.dx_pose + ((size_t)w * a.Ncap + f) * 15;
+        double R[9], om[3];
+        quat_to_mat(fs, R);
+        mat3_vec(R, d, om);
+        const double p0 = fs[4] - wc.origin[0], p1 = fs[5] - wc.origin[1], p2 = fs[6] - wc.origin[2];
+        dxi[f * 6 + 0] = om[0]; dxi[f * 6 + 1] = om[1]; dxi[f * 6 + 2] = om[2];
+        dxi[f * 6 + 3] = -(p1 * om[2] - p2 * om[1]) - d[3];
+        dxi[f * 6 + 4] = -(p2 * om[0] - p0 * om[2]) - d[4];
+        dxi[f * 6 + 5] = -(p0 * om[1] - p1 * om[0]) - d[5];
     }
     if (tid < 8) red[tid] = 0.0;
     if (kMode == 0) for (int i = tid; i < kSegTab; i += kThreads) sg[i] = a.seg[(size_t)w * kSegTab + i];
     __syncthreads();
 
-    const double mu = a.mu_override >= 0.0 ? a.mu_override : ctrl.mu;
-    const LmRec *lms = a.lms + (size_t)w * a.Mcap;
-    const double *rho = a.rho + (size_t)w * a.Mcap;
-    const double *lm_scale = a.lm_scale + (size_t)w * a.Mcap;
     const size_t bsel = a.loop ? (size_t)ctrl.buf : 0;
-    const LmAux *aux = a.lm_aux + bsel * a.bufs.lm_aux + (size_t)w * a.Mcap;
+    const LmAux *aux = a.lm_aux + bsel * a.bufs.lm_aux;
     const real *hs = reinterpret_cast<const real *>(reinterpret_cast<const char *>(a.hs) + bsel * a.bufs.hs) + (size_t)w * a.Ncap * a.Mcap * 6;
-    double *rho_c = a.rho_cand + (size_t)w * a.Mcap;
-    double *dxl = a.dx_lm + (size_t)w * a.Mcap;
-    double *lmv = a.lm_v + (size_t)w * a.Mcap;
     const unsigned fixed = (unsigned)H.fixed_mask & ((1u << N) - 1u);
 
-    // ---- phase 1: back-substitution, candidate inverse depth and world point
+    // ---- phase 1a: h_l . dxi = sum_t h_lt . (dxi_t - dxi_a) of the thread's landmarks, in frame order, parked in xs[l]
+    // (the slot the landmark's candidate world point takes in phase 1b; the same thread reads it back).  Nothing but
+    // the records in flight is live here.
+    if (kMode != 2) {
+        constexpr int kGroup = 6;       // records in flight: the <= 9 target frames of a 10-frame window in two groups
+        for (int l = tid; l < M; l += kThreads) {
+            const int meta = a.lms[(size_t)w * a.Mcap + l].meta;
+            if (lm_nobs(meta) == 0) continue;
+            const int anchor = lm_anchor(meta);
+            double hdx = 0.0;
+            typedef typename Vec2<real>::type real2;
+            unsigned fm = lm_mask(meta);
+            if ((fixed >> anchor) & 1u) fm &= ~fixed;                  // record not written; both steps are zero
+            const double *da = dxi + anchor * 6;
+            // the loads of a group are independent of each other; the anchor block of a residual is minus its target block
+            while (fm) {
+                int fr[kGroup];
+                real2 h[kGroup][3];
+#pragma unroll
+                for (int q = 0; q < kGroup; ++q) {
+                    fr[q] = fm ? __ffs(fm) - 1 : -1;
+                    fm &= fm - 1;
+                    if (fr[q] >= 0) {
+                        const real2 *hp = reinterpret_cast<const real2 *>(hs + ((size_t)fr[q] * a.Mcap + l) * 6);
+                        h[q][0] = hp[0]; h[q][1] = hp[1]; h[q][2] = hp[2];
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < kGroup; ++q) {
+                    if (fr[q] < 0) continue;
+                    const double *df = dxi + fr[q] * 6;
+                    hdx += (double)h[q][0].x * (df[0] - da[0]) + (double)h[q][0].y * (df[1] - da[1]) + (double)h[q][1].x * (df[2] - da[2]) +
+                           (double)h[q][1].y * (df[3] - da[3]) + (double)h[q][2].x * (df[4] - da[4]) + (double)h[q][2].y * (df[5] - da[5]);
+                }
+            }
+            xs[l] = hdx;
+        }
+    }
+
+    // ---- phase 1b: back-substitution, candidate inverse depth and world point
     double s_gdx = 0.0, s_reg = 0.0, s_gn = 0.0, s_dx2 = 0.0, s_x2 = 0.0, s_g2 = 0.0, s_vrd = 0.0;
     for (int l = tid; l < Mp; l += kThreads) {
         double x0 = 0.0, x1 = 0.0, x2 = 1.0;
         if (l < M) {
-            const LmRec lr = lms[l];
-            const int n_obs = lm_nobs(lr.meta), anchor = lm_anchor(lr.meta);
-            const double rl = rho[l];
+            const size_t gi = (size_t)w * a.Mcap + l;
+            const int meta = a.lms[gi].meta;
+            const int n_obs = lm_nobs(meta), anchor = lm_anchor(meta);
+            const double rl = a.rho[gi];
             const bool mine = ((l >> 5) % (int)gridDim.x) == (int)blockIdx.x;
             double drho = 0.0, vl = 0.0;
             if (n_obs > 0 && kMode != 2) {
-                const LmAux ax = aux[l];
-                // h_l . dxi = sum_t h_lt . (dxi_t - dxi_a): the anchor block of a residual is minus its target block
-                double hdx = 0.0;
-                const bool a_fixed = (fixed >> anchor) & 1u;
-                typedef typename Vec2<real>::type real2;
-                unsigned fm = lm_mask(lr.meta);
-                if (a_fixed) fm &= ~fixed;                              // record not written; both steps are zero
-                const double *da = dxi + anchor * 6;
-                // four records in flight at a time (the loads of a group are independent of each other)
-                while (fm) {
-                    int f4[4];
-                    real2 h[4][3];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        f4[q] = fm ? __ffs(fm) - 1 : -1;
-                        fm &= fm - 1;
-                        if (f4[q] >= 0) {
-                            const real2 *hp = reinterpret_cast<const real2 *>(hs + ((size_t)f4[q] * a.Mcap + l) * 6);
-                            h[q][0] = hp[0]; h[q][1] = hp[1]; h[q][2] = hp[2];
-                        }
-                    }
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (f4[q] < 0) continue;
-                        const double *df = dxi + f4[q] * 6;
-                        hdx += (double)h[q][0].x * (df[0] - da[0]) + (double)h[q][0].y * (df[1] - da[1]) + (double)h[q][1].x * (df[2] - da[2]) +
-                               (double)h[q][1].y * (df[3] - da[3]) + (double)h[q][2].x * (df[4] - da[4]) + (double)h[q][2].y * (df[5] - da[5]);
-                    }
-                }
+                const double hdx = xs[l];
+                const LmAux ax = aux[gi];
                 const double wl = 1.0 / ax.hll_reg;
                 const double hll = ax.hll;
                 drho = isfinite(wl) ? -(ax.gl + hdx) * wl : 0.0;
-                const double sc = lm_scale[l];
+                const double sc = a.lm_scale[gi];
+                const double mu = a.mu_override >= 0.0 ? a.mu_override : ctrl.mu;
                 const double reg = mu > 0.0 ? lm_reg(hll, sc, mu) : 0.0;
                 double d2 = sc * sc * hll;
                 d2 = fmin(fmax(d2, 1.0e-6), 1.0e32);
@@ -209,26 +218,36 @@ update_obs_kernel(UpdArgs a) {
                     s_x2 += rl * rl;
                 }
             }
-            if (kMode == 1) { dxl[l] = drho; lmv[l] = vl; continue; }
-            if (kMode == 2 && n_obs > 0) { drho = dxl[l]; vl = lmv[l]; }
+            if (kMode == 1) { a.dx_lm[gi] = drho; a.lm_v[gi] = vl; continue; }
+            if (kMode == 2 && n_obs > 0) { drho = a.dx_lm[gi]; vl = a.lm_v[gi]; }
             drho = step_b * drho - step_a * vl;
-            if (mine) { s_dx2 += drho * drho; rho_c[l] = rl + drho; dxl[l] = drho; }
+            if (mine) { s_dx2 += drho * drho; a.rho_cand[gi] = rl + drho; a.dx_lm[gi] = drho; }
             if (kMode != 2 && n_obs > 0) {
-                const double *Fa = Fc + anchor * 12;
+                const double *R = Fc[anchor].Rwc, *ca = Fc[anchor].c;
                 const double ir = 1.0 / (rl + drho);
+                const LmRec &lr = a.lms[gi];
                 const double zx = (double)lr.zrx, zy = (double)lr.zry;
-                x0 = (Fa[0] * zx + Fa[1] * zy + Fa[2]) * ir + Fa[9];
-                x1 = (Fa[3] * zx + Fa[4] * zy + Fa[5]) * ir + Fa[10];
-                x2 = (Fa[6] * zx + Fa[7] * zy + Fa[8]) * ir + Fa[11];
+                x0 = (R[0] * zx + R[1] * zy + R[2]) * ir + ca[0];
+                x1 = (R[3] * zx + R[4] * zy + R[5]) * ir + ca[1];
+                x2 = (R[6] * zx + R[7] * zy + R[8]) * ir + ca[2];
             }
         }
         if (kMode == 0) { xs[l] = x0; xs[Mp + l] = x1; xs[2 * Mp + l] = x2; }
     }
+    {   // the back-substitution scalars are complete: reduced here, so that the row walk carries s_cost alone
+        double v[7] = {s_gdx, s_reg, s_gn, s_dx2, s_x2, s_g2, s_vrd};
+#pragma unroll
+        for (int k = 0; k < 7; ++k) {
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], off);
+            if (lane == 0 && v[k] != 0.0) atomicAdd(&red[k + 1], v[k]);
+        }
+    }
     __syncthreads();
 
     // ---- phase 2: candidate cost over the rows of the frame-major table
-    double s_cost = 0.0;
     if (kMode == 0) {
+        double s_cost = 0.0;
         const real W[4] = {(real)wc.sic[0], (real)wc.sic[1], (real)wc.sic[2], (real)wc.sic[3]};
         const real cb = (real)(wc.cauchy_a * wc.cauchy_a), inv_cb = (real)(1.0 / (wc.cauchy_a * wc.cauchy_a));
         const bool diag_w = wc.sic[1] == 0.0 && wc.sic[2] == 0.0;
@@ -248,13 +267,10 @@ update_obs_kernel(UpdArgs a) {
             const int seg_end = sbeg[sp + 1];
             const int r_stop = min(r_end, srow[sp + 1]);
             double Rwc[9], c[3];
-            {
-                const double *Ft = Fc + t * 12;
 #pragma unroll
-                for (int i = 0; i < 9; ++i) Rwc[i] = Ft[i];
+            for (int i = 0; i < 9; ++i) Rwc[i] = Fc[t].Rwc[i];
 #pragma unroll
-                for (int i = 0; i < 3; ++i) c[i] = Ft[9 + i];
-            }
+            for (int i = 0; i < 3; ++i) c[i] = Fc[t].c[i];
             LogAcc<real> la;
             int nfold = 0;
             for (; cs.r < r_stop; cs.advance()) {
@@ -272,13 +288,9 @@ update_obs_kernel(UpdArgs a) {
             s_cost += (double)((real)0.5 * cb * la.total());
         }
         asm volatile("cp.async.wait_all;" ::: "memory");
-    }
-    double v[8] = {s_cost, s_gdx, s_reg, s_gn, s_dx2, s_x2, s_g2, s_vrd};
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], off);
-        if (lane == 0 && v[k] != 0.0) atomicAdd(&red[k], v[k]);
+        for (int off = 16; off > 0; off >>= 1) s_cost += __shfl_xor_sync(0xffffffffu, s_cost, off);
+        if (lane == 0 && s_cost != 0.0) atomicAdd(&red[0], s_cost);
     }
     __syncthreads();
     double *acc = a.acc + (size_t)w * kAcc;
