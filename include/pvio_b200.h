@@ -230,6 +230,17 @@ int pvio_b200_batch_download_state(pvio_b200_handle h, int n, double *frames, in
  * copy buys up to max_iterations iterations per window. */
 int pvio_b200_batch_solve_host(pvio_b200_handle h, int n, const pvio_b200_options *opt, double *frames, int64_t frames_stride,
                                double *inv_depth, int64_t inv_depth_stride, pvio_b200_summary *summaries);
+/* BundleAdjustor::marginalize_frame(map, 0) (bundle_adjustor.cpp:348-599) for each of the first n uploaded windows, at
+ * their device-resident states (e.g. right after pvio_b200_batch_solve).  Every window must carry motion states, have
+ * N >= 2 and 15 (N - 1) <= 165.  The victim's landmarks are the ones flagged lm_in_victim when the slot was packed.
+ * The new prior of window i (S_i, e_i over its frames 1 .. N_i - 1, linearised at those frames' current states) is
+ * written into slot i's prior arrays on the device.  A later pvio_b200_batch_set_window(i, w', ...) of the shifted
+ * window with w'.prior_S == NULL and w'.n_prior == N_i - 1 names that prior, and it is not uploaded again; until the
+ * slot is packed and uploaded again, its old window is not to be solved.  The device states are not modified.
+ * S_out [n][S_stride] (row-major dk_i x dk_i at the start of each row, dk_i = 15 (N_i - 1)) and e_out [n][e_stride]
+ * may be NULL.  Every window is checked before anything runs: on PVIO_B200_EINVAL no slot has changed. */
+int pvio_b200_batch_marginalize(pvio_b200_handle h, int n, double *S_out, int64_t S_stride,
+                                double *e_out, int64_t e_stride);
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */
 int pvio_b200_timer_start(pvio_b200_handle h);

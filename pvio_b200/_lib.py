@@ -76,6 +76,7 @@ EXPORTS = [
     "pvio_b200_window_add_observations", "pvio_b200_window_remove_track", "pvio_b200_window_set_prior",
     "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
     "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
+    "pvio_b200_batch_marginalize",
 ]
 
 _lib = None
@@ -117,6 +118,7 @@ def load():
     lib.pvio_b200_batch_download_state.argtypes = [vp, C.c_int, c_f64p, C.c_int64, c_f64p, C.c_int64, C.POINTER(CSummary)]
     lib.pvio_b200_batch_solve_host.argtypes = [vp, C.c_int, C.POINTER(COptions), c_f64p, C.c_int64, c_f64p, C.c_int64,
                                                C.POINTER(CSummary)]
+    lib.pvio_b200_batch_marginalize.argtypes = [vp, C.c_int, c_f64p, C.c_int64, c_f64p, C.c_int64]
     lib.pvio_b200_selftest_lie.argtypes = [vp, C.c_int, c_f64p, c_f64p]
     lib.pvio_b200_sync.argtypes = [vp]
     lib.pvio_b200_timer_start.argtypes = [vp]

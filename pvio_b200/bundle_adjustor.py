@@ -25,7 +25,9 @@ class BundleAdjustor:
             msg = self.lib.pvio_b200_last_error(self.h).decode() if self.h else ""
             raise PvioB200Error(f"pvio_b200_create failed ({rc}) {msg}: a CUDA device is required, there is no CPU fallback")
         self.max_windows = max_windows
+        self.max_frames = max_frames
         self._keep = {}
+        self._slot_frames = {}          # frame count of the window packed into each slot by batch_set / batch_replicate
 
     def close(self):
         if self.h:
@@ -101,12 +103,36 @@ class BundleAdjustor:
         return err.value
 
     # ---- batched windows -------------------------------------------------------------
-    def batch_set(self, slot, win, st):
+    def batch_set(self, slot, win, st, resident_prior=False):
+        """Pack `win` into slot `slot`.  resident_prior: the window's prior is the one batch_marginalize left in this slot
+        on the device (n_prior and prior_frames are passed, the prior's S, e and linearisation point are not)."""
         pa = _lib.PackedArgs(win, st)
+        if resident_prior:
+            pa.cw.prior_S = pa.cw.prior_e = pa.cw.prior_state0 = None
         self._ck(self.lib.pvio_b200_batch_set_window(self.h, slot, C.byref(pa.cw), C.byref(pa.cs)))
+        self._slot_frames[slot] = win.N
 
     def batch_replicate(self, n):
         self._ck(self.lib.pvio_b200_batch_replicate(self.h, n))
+        for i in range(1, n):
+            self._slot_frames[i] = self._slot_frames.get(0)
+
+    def batch_marginalize(self, n, want=False):
+        """BundleAdjustor::marginalize_frame(0) of each of the first n uploaded windows at its device state; the new priors
+        stay in the slots' device arrays (see batch_set(resident_prior=True)).  want: also return [(S_i, e_i)], shaped by
+        the frame count of the window batch_set packed into slot i."""
+        if not want:
+            self._ck(self.lib.pvio_b200_batch_marginalize(self.h, n, None, 0, None, 0))
+            return None
+        dmax = 15 * (self.max_frames - 1)
+        S, e = np.zeros((n, dmax * dmax)), np.zeros((n, dmax))
+        self._ck(self.lib.pvio_b200_batch_marginalize(self.h, n, _lib._ptr(S, C.c_double), dmax * dmax,
+                                                      _lib._ptr(e, C.c_double), dmax))
+        out = []
+        for i in range(n):
+            d = 15 * (self._slot_frames[i] - 1)
+            out.append((S[i, :d * d].reshape(d, d).copy(), e[i, :d].copy()))
+        return out
 
     def batch_upload(self, n):
         self._ck(self.lib.pvio_b200_batch_upload(self.h, n))

@@ -234,6 +234,10 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
             seen |= 1u << f;
         }
     }
+    // prior_S == NULL names the prior the marginaliser left in this slot's device arrays (pvio_b200_batch_marginalize,
+    // pvio_b200_window_drop_victim); checked before anything of the slot is overwritten
+    if (n_prior > 0 && !w->prior_S && h->prior_resident[slot] != n_prior)
+        return fail(h, PVIO_B200_EINVAL, "prior_S == NULL: no device-resident prior of that size in this slot");
     if (w->n_plane_tracks < 0 || w->n_planes < 0 || w->n_planes > h->Pcap) return fail(h, PVIO_B200_EINVAL, "too many planes");
     if (w->n_plane_tracks > 0) {
         if (!w->pt_obs_begin || !w->pt_plane || !w->pt_obs_frame || !w->pt_obs_z || !w->plane_param || w->pt_obs_begin[0] != 0)
@@ -327,11 +331,8 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
         if (n_imu > 0) memcpy(h->imu_data.h + (size_t)slot * h->Ncap * kImuStride, w->imu_data, sizeof(double) * n_imu * kImuStride);
         const size_t dcap = 15 * (size_t)h->Ncap, d = 15 * (size_t)n_prior;
         for (int n = 0; n < n_prior; ++n) h->prior_frames.h[(size_t)slot * h->Ncap + n] = w->prior_frames[n];
-        if (d > 0 && !w->prior_S) {         // prior left on the device by marginalize_impl(keep_on_device): slot 0 only
-            if (slot != 0 || !h->prior_resident || h->prior_resident_n != n_prior)
-                return fail(h, PVIO_B200_EINVAL, "prior_S == NULL: no device-resident prior of that size");
-        } else if (d > 0) {
-            if (slot == 0) h->prior_resident = false;
+        if (d > 0 && w->prior_S) {          // a host prior replaces a device-resident one
+            h->prior_resident[slot] = 0;
             memcpy(h->prior_S.h + (size_t)slot * dcap * dcap, w->prior_S, sizeof(double) * d * d);   // dense d x d, row-major
             memcpy(h->prior_e.h + (size_t)slot * dcap, w->prior_e, sizeof(double) * d);
             memcpy(h->prior_x0.h + (size_t)slot * h->Ncap * kFrameStride, w->prior_state0, sizeof(double) * n_prior * kFrameStride);
@@ -376,10 +377,14 @@ static int upload_range(Handle *h, int w0, int n, cudaStream_t st) {
         TRY(h2d(h, h->imu_idx, N * 2, w0, n, st));
         TRY(h2d(h, h->imu_data, N * kImuStride, w0, n, st));
         TRY(h2d(h, h->prior_frames, N, w0, n, st));
-        if (!(w0 == 0 && n == 1 && h->prior_resident)) {     // a device-resident prior (marginalize_impl) is never re-uploaded
-            TRY(h2d(h, h->prior_S, dcap * dcap, w0, n, st));
-            TRY(h2d(h, h->prior_e, dcap, w0, n, st));
-            TRY(h2d(h, h->prior_x0, N * kFrameStride, w0, n, st));
+        for (int i = w0; i < w0 + n;) {      // a device-resident prior is never re-uploaded: copy the runs of the other slots
+            if (h->prior_resident[i]) { ++i; continue; }
+            int j = i;
+            while (j < w0 + n && !h->prior_resident[j]) ++j;
+            TRY(h2d(h, h->prior_S, dcap * dcap, i, j - i, st));
+            TRY(h2d(h, h->prior_e, dcap, i, j - i, st));
+            TRY(h2d(h, h->prior_x0, N * kFrameStride, i, j - i, st));
+            i = j;
         }
         for (int i = w0; i < w0 + n; ++i) any_prior |= h->hdr.h[i].n_prior > 0;
         if (any_prior) {
@@ -576,11 +581,11 @@ static int run_linearize(Handle *h, int n, const StepCfg &c, const BatchShape &b
     return 0;
 }
 
-int run_marg_vision(Handle *h) {
+int run_marg_vision(Handle *h, int n) {
     StepCfg c;
     c.mu = 0.0; c.compute_scale = 1;
-    const BatchShape b = batch_shape(h, 0, 1, false);
-    return run_linearize(h, 1, c, b, false, true);
+    const BatchShape b = batch_shape(h, 0, n, false);
+    return run_linearize(h, n, c, b, false, true);
 }
 
 static int run_solve(Handle *h, int n, const StepCfg &c, const BatchShape &b) {
@@ -964,6 +969,7 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
     TRY(alloc(h, h->Hfull, (15 * N) * (15 * N), true)); TRY(alloc(h, h->gfull, 15 * N, true));
     refresh_arrays(h);
     h->perm.resize(W); h->perm_identity.assign(W, 1); h->slot_M.assign(W, 0); h->slot_N.assign(W, 0); h->slot_K.assign(W, 0);
+    h->prior_resident.assign(W, 0);
     {   // opt in to large dynamic shared memory ONCE per kernel with the device limit: the attribute is process-wide, so a
         // per-handle value would be overwritten by the next handle with other capacities
         const int lim = (int)prop.sharedMemPerBlockOptin - 2048;
@@ -1091,8 +1097,11 @@ int pvio_b200_batch_replicate(pvio_b200_handle hh, int n) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
+    if (h->prior_resident[0] && h->hdr.h[0].n_prior > 0)
+        return fail(h, PVIO_B200_EINVAL, "batch_replicate: slot 0's prior is device-resident, its staging does not hold it");
     const size_t N = h->Ncap;
     for (int i = 1; i < n; ++i) {
+        h->prior_resident[i] = 0;          // the slot takes slot 0's host prior from the staging
         h->hdr.h[i] = h->hdr.h[0]; h->cst.h[i] = h->cst.h[0];
         memcpy(h->obs.h + (size_t)i * h->Kcap, h->obs.h, sizeof(ObsRec) * h->slot_K[0]);
         memcpy(h->lms.h + (size_t)i * h->Mcap, h->lms.h, sizeof(LmRec) * h->slot_M[0]);
@@ -1274,6 +1283,12 @@ int pvio_b200_ba_marginalize(pvio_b200_handle hh, const pvio_b200_window *w, con
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h || !w || !s) return PVIO_B200_EINVAL;
     return marginalize_impl(h, w, s, index, false, S_out, e_out, H_out, b_out);
+}
+
+int pvio_b200_batch_marginalize(pvio_b200_handle hh, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return batch_marginalize_impl(h, n, S_out, S_stride, e_out, e_stride);
 }
 
 int pvio_b200_pnp_solve(pvio_b200_handle hh, const pvio_b200_pnp_problem *problem, double *frame,

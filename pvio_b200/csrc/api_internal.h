@@ -36,8 +36,8 @@ struct Handle {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::string err;
     int64_t launches = 0;
-    bool prior_resident = false;                  // slot 0's prior (S, e, x0) was written on the device by the marginaliser
-    int prior_resident_n = 0;                     // its frame count
+    std::vector<int> prior_resident;              // per slot: frame count of the prior (S, e, x0) the marginaliser wrote on the
+                                                  // device (0: none); a pack naming it with prior_S == NULL keeps it, a host prior clears it
     struct ResidentWindow *resident = nullptr;    // resident.cu
     struct DetectState *detect = nullptr;         // detect.cu
     size_t sys_set = 0;                           // elements between the two buffer sets of the reduced-system arrays (LinBufs)
@@ -135,8 +135,8 @@ inline SolveOptions solve_options(const pvio_b200_options *opt) {
 
 // api.cu: pack window into slot 0, copy it to the device, build the frame-major table
 int pack_and_upload(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s);
-// api.cu: linearise + Schur of window 0 with the fp64 pipeline, no loss (the marginaliser's reprojection part)
-int run_marg_vision(Handle *h);
+// api.cu: linearise + Schur of the uploaded windows [0, n) with the fp64 pipeline, no loss (the marginaliser's reprojection part)
+int run_marg_vision(Handle *h, int n);
 void drop_graphs(Handle *h);
 // klt.cu
 int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int width, int height, int stride,
@@ -156,6 +156,7 @@ int klt_clahe_device(Handle *h, const uint8_t *d_src, uint8_t *d_dst, uint8_t *d
 void detect_free(Handle *h);
 int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
                      double *S_out, double *e_out, double *H_out, double *b_out);
+int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride);
 void marg_free(Handle *h);
 // fmat.cu
 int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double threshold, double confidence, int max_iters,

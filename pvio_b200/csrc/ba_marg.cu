@@ -7,6 +7,9 @@
 //   frame Schur with the explicit 15x15 inverse   :547-581   marg_reduce_kernel
 //   eigen factorisation, clamp lambda <= 1e-8     :583-590   marg_eig_kernel (Householder tridiagonalisation + implicit QL)
 // All dense algebra is fp64.  Runs once per keyframe (not per iteration): latency, not bandwidth.
+// Each of the three dense kernels runs one CTA per window: CTA c of a launch works on window w0 + c, with the dense
+// scratch block c of the chunk (MargLayout).  A single window is a grid of 1.
+#include <algorithm>
 #include <cstring>
 #include <vector>
 #include "api_internal.h"
@@ -15,22 +18,38 @@
 
 namespace pvio {
 
-struct MargArgs : BatchArrays {        // window 0; Hred, gred: vision part (xi coordinates) from the linearise + Schur stage
+// Dense fp64 scratch of one window (offsets in doubles from the window's block, sized from the handle's frame capacity;
+// ncap = 15 Ncap, dcap = ncap - 15) and the stride between the blocks of a chunk.
+struct MargLayout {
+    size_t H;                          // [ncap^2] information matrix, row-major with leading dimension 15 N, full symmetric
+    size_t b;                          // [ncap]
+    size_t Hk, bk;                     // [dcap^2], [dcap] after the frame Schur complement (leading dimension 15 (N - 1))
+    size_t S, e;                       // [dcap^2], [dcap] the new prior, when it does not go to the window's prior arrays
+    size_t scr;                        // >= 2048 + 64 Ncap doubles: IMU factor blocks, prior residual / Jacobian
+    size_t stride;
+};
+
+struct MargArgs : BatchArrays {        // Hred, gred: set 0 of the vision part (xi coordinates) from the linearise + Schur stage
     int index;                         // victim frame
-    double *H;                         // [(15N)^2] row-major, full symmetric
-    double *b;                         // [15N]
-    double *scratch;                   // >= 4*(15*30+16) + 4*15*Ncap doubles
+    int w0;                            // window of CTA 0
+    double *buf;                       // chunk scratch: block c belongs to window w0 + c
+    MargLayout L;
 };
 
 __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
-    const WinHdr &Hh = a.hdr[0];
-    const WinConst &wc = a.cst[0];
+    const int w = a.w0 + blockIdx.x;
+    const WinHdr &Hh = a.hdr[w];
+    const WinConst &wc = a.cst[w];
     const int N = Hh.N, n = 15 * N;
     const int tid = threadIdx.x, nt = blockDim.x;
-    const double *frames = a.frames;
+    const size_t Nc = a.Ncap, dcap = 15 * Nc;
+    const double *frames = a.frames + (size_t)w * Nc * kFrameStride;
+    double *const blk = a.buf + blockIdx.x * a.L.stride;
+    double *const Hm = blk + a.L.H, *const bv = blk + a.L.b, *const scratch = blk + a.L.scr;
+    const double *Hred = a.Hred + (size_t)w * (Nc * (Nc + 1) / 2) * 36, *gred = a.gred + (size_t)w * Nc * 6;
     __shared__ double T[kMaxFrames * 36];
-    for (int i = tid; i < n * n; i += nt) a.H[i] = 0.0;
-    for (int i = tid; i < n; i += nt) a.b[i] = 0.0;
+    for (int i = tid; i < n * n; i += nt) Hm[i] = 0.0;
+    for (int i = tid; i < n; i += nt) bv[i] = 0.0;
     if (tid < N) {
         const double *fs = frames + tid * kFrameStride;
         double R[9], Hp[9], B[9];
@@ -55,7 +74,7 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
         int f = 0;
         while ((f + 1) * (f + 2) / 2 <= p) ++f;
         const int gf = p - f * (f + 1) / 2;
-        const double *X = a.Hred + p * 36;
+        const double *X = Hred + p * 36;
         const double *Tf = T + f * 36, *Tg = T + gf * 36;
         double s = 0.0;
         for (int aa = 0; aa < 6; ++aa) {
@@ -64,32 +83,34 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
             s += Tf[aa * 6 + i] * t;
         }
         const int gi = f * 15 + i, gj = gf * 15 + j;
-        a.H[(size_t)gi * n + gj] = s;
-        if (f != gf) a.H[(size_t)gj * n + gi] = s;
+        Hm[(size_t)gi * n + gj] = s;
+        if (f != gf) Hm[(size_t)gj * n + gi] = s;
     }
     for (int e = tid; e < N * 6; e += nt) {
         const int f = e / 6, i = e - f * 6;
         double s = 0.0;
-        for (int aa = 0; aa < 6; ++aa) s += T[f * 36 + aa * 6 + i] * a.gred[f * 6 + aa];
-        a.b[f * 15 + i] = s;
+        for (int aa = 0; aa < 6; ++aa) s += T[f * 36 + aa * 6 + i] * gred[f * 6 + aa];
+        bv[f * 15 + i] = s;
     }
     __syncthreads();
     // ---- prior :369-413  (H += E^T Lambda E, b += E^T S^T (S r0 + e))
     if (Hh.n_prior > 0) {
         const int np = Hh.n_prior, d = 15 * np;
-        double *r0 = a.scratch, *rr = r0 + d, *vv = rr + d, *Ji = vv + d;
-        if (tid < np) prior_frame_raw(frames + a.prior_frames[tid] * kFrameStride, a.prior_x0 + tid * kFrameStride,
+        const int32_t *pfr = a.prior_frames + (size_t)w * Nc;
+        const double *pS = a.prior_S + (size_t)w * dcap * dcap, *pe = a.prior_e + (size_t)w * dcap;
+        double *r0 = scratch, *rr = r0 + d, *vv = rr + d, *Ji = vv + d;
+        if (tid < np) prior_frame_raw(frames + pfr[tid] * kFrameStride, a.prior_x0 + ((size_t)w * Nc + tid) * kFrameStride,
                                       r0 + 15 * tid, Ji + 9 * tid);
         __syncthreads();
         for (int i = tid; i < d; i += nt) {
-            double s = a.prior_e[i];
-            for (int k = 0; k < d; ++k) s += a.prior_S[(size_t)i * d + k] * r0[k];
+            double s = pe[i];
+            for (int k = 0; k < d; ++k) s += pS[(size_t)i * d + k] * r0[k];
             rr[i] = s;
         }
         __syncthreads();
         for (int i = tid; i < d; i += nt) {
             double s = 0.0;
-            for (int k = 0; k < d; ++k) s += a.prior_S[(size_t)k * d + i] * rr[k];
+            for (int k = 0; k < d; ++k) s += pS[(size_t)k * d + i] * rr[k];
             vv[i] = s;
         }
         __syncthreads();
@@ -98,9 +119,9 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
             double s;
             if (ci < 3) { s = 0.0; for (int k = 0; k < 3; ++k) s += Ji[9 * fi + 3 * k + ci] * vv[15 * fi + k]; }
             else s = vv[i];
-            a.b[a.prior_frames[fi] * 15 + ci] += s;
+            bv[pfr[fi] * 15 + ci] += s;
         }
-        const double *L = a.prior_L;
+        const double *L = a.prior_L + (size_t)w * dcap * dcap;
         for (int e = tid; e < d * d; e += nt) {
             const int i = e / d, j = e - i * d;
             const int fi = i / 15, ci = i - fi * 15, fj = j / 15, cj = j - fj * 15;
@@ -116,17 +137,18 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
             } else {
                 s = L[(size_t)i * d + j];
             }
-            a.H[(size_t)(a.prior_frames[fi] * 15 + ci) * n + a.prior_frames[fj] * 15 + cj] += s;
+            Hm[(size_t)(pfr[fi] * 15 + ci) * n + pfr[fj] * 15 + cj] += s;
         }
         __syncthreads();
     }
     // ---- IMU factors with j == index or j == index + 1  :416-450.  The functor reads the bias
     // linearisation point from the very memory passed as the parameter, so dbg = dba = 0.
+    const int32_t *imu_idx = a.imu_idx + (size_t)w * Nc * 2;
     for (int m = 0; m < Hh.n_imu; ++m) {
-        const int fi = a.imu_idx[2 * m], fj = a.imu_idx[2 * m + 1];
+        const int fi = imu_idx[2 * m], fj = imu_idx[2 * m + 1];
         if (fj != a.index && fj != a.index + 1) continue;
-        double *Jraw = a.scratch, *rraw = Jraw + 450, *Jw = rraw + 16, *rw = Jw + 450;
-        const double *rec = a.imu_data + (size_t)m * kImuStride;
+        double *Jraw = scratch, *rraw = Jraw + 450, *Jw = rraw + 16, *rw = Jw + 450;
+        const double *rec = a.imu_data + ((size_t)w * Nc + m) * kImuStride;
         if (tid == 0) imu_factor_raw(frames + fi * kFrameStride, frames + fj * kFrameStride, rec, wc, 1, rraw, Jraw);
         __syncthreads();
         for (int e = tid; e < 15 * 31; e += nt) {
@@ -144,10 +166,10 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
             if (cb_ < 30) {
                 const int gb = (cb_ < 15 ? fi * 15 + cb_ : fj * 15 + cb_ - 15);
                 for (int k = 0; k < 15; ++k) s += Jw[k * 30 + ra] * Jw[k * 30 + cb_];
-                a.H[(size_t)ga * n + gb] += s;
+                Hm[(size_t)ga * n + gb] += s;
             } else {
                 for (int k = 0; k < 15; ++k) s += Jw[k * 30 + ra] * rw[k];
-                a.b[ga] += s;
+                bv[ga] += s;
             }
         }
         __syncthreads();
@@ -156,9 +178,11 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
 
 // Frame Schur complement :547-581.  inv = H[vv]^-1 by Gauss-Jordan with partial pivoting
 // (Eigen's dynamic .inverse() is PartialPivLU based), then Hk = H[kk] - H[kv] inv H[vk].
-__global__ void __launch_bounds__(256) marg_reduce_kernel(const double *H, const double *b, int N, int index,
-                                                         double *Hk, double *bk) {
-    const int n = 15 * N, dk = n - 15, v0 = 15 * index;
+__global__ void __launch_bounds__(256) marg_reduce_kernel(const WinHdr *hdr, int w0, int index, double *buf, MargLayout L) {
+    double *const blk = buf + blockIdx.x * L.stride;
+    const double *H = blk + L.H, *b = blk + L.b;
+    double *Hk = blk + L.Hk, *bk = blk + L.bk;
+    const int n = 15 * hdr[w0 + blockIdx.x].N, dk = n - 15, v0 = 15 * index;
     const int tid = threadIdx.x, nt = blockDim.x;
     __shared__ double M[15][31];
     __shared__ int piv_sm;
@@ -244,9 +268,16 @@ __device__ long long g_marg_stamps[8];
 #define MARG_STAMP(k) do { } while (0)
 #endif
 
-__global__ void __launch_bounds__(256) marg_eig_kernel(const double *Ain, const double *bvec, int n, int ring, double *S, double *evec) {
+// Per window (CTA c: window w0 + c): S [c * S_stride] dense n x n row-major, evec [c * e_stride]; x0 (may be NULL): the
+// linearisation point of the new prior, frames 1 .. N - 1 of the window's state (frames, x0: window w0's, x_stride apart).
+__global__ void __launch_bounds__(256) marg_eig_kernel(const WinHdr *hdr, int w0, const double *buf, MargLayout L, int ring,
+                                                       double *S_all, size_t S_stride, double *e_all, size_t e_stride,
+                                                       const double *frames, double *x0, size_t x_stride) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x, nt = blockDim.x;
+    const int c = blockIdx.x, N = hdr[w0 + c].N, n = 15 * (N - 1);
+    const double *Ain = buf + c * L.stride + L.Hk, *bvec = buf + c * L.stride + L.bk;
+    double *S = S_all + c * S_stride, *evec = e_all + c * e_stride;
     const int ld = n | 1;
     double *a = reinterpret_cast<double *>(smem_raw);       // [n][ld]: matrix -> eigenvectors (columns)
     double *d = a + (size_t)n * ld;                         // [n]
@@ -418,6 +449,8 @@ __global__ void __launch_bounds__(256) marg_eig_kernel(const double *Ain, const 
         }
         evec[i] = il * dot;
     }
+    if (x0)
+        for (int i = tid; i < (N - 1) * kFrameStride; i += nt) x0[c * x_stride + i] = frames[c * x_stride + kFrameStride + i];
     MARG_STAMP(4);
 }
 
@@ -441,62 +474,126 @@ void marg_free(Handle *h) {
     }
 }
 
-// keep_on_device (index 0 only): the new prior -- S, e and its linearisation point, the CURRENT states of the frames that
-// stay -- is written straight into slot 0's prior arrays on the device; the next solve of the shifted window names it
-// with prior_S == NULL (pack_window) and nothing of it crosses PCIe.
+// Windows per pass of the dense kernels.  Their scratch blocks (about 0.4 MB each at N = 9) are allocated for the largest
+// pass a handle has run and reused by every pass.  Two per SM: at D = 135 the eigen-solver's shared memory admits one CTA
+// per SM, so the second half of a pass queues behind the first; at N = 6 several CTAs share an SM.
+constexpr int kMargChunkPerSm = 2;
+constexpr size_t kEigSmemMax = 226 * 1024;
+
+static MargLayout marg_layout(const Handle *h) {
+    const size_t ncap = 15 * (size_t)h->Ncap, dcap = ncap - 15;
+    MargLayout L;
+    L.H = 0; L.b = L.H + ncap * ncap;
+    L.Hk = L.b + ncap; L.bk = L.Hk + dcap * dcap;
+    L.S = L.bk + dcap; L.e = L.S + dcap * dcap;
+    L.scr = L.e + dcap;
+    L.stride = L.scr + 2048 + 64 * (size_t)h->Ncap;
+    return L;
+}
+
+// dynamic shared memory of the eigen-solver: matrix + d, e + the ring of rotation batches
+static size_t eig_smem(int dk, int ring) { return sizeof(double) * ((size_t)dk * (dk | 1) + (2 + 2 * (size_t)ring) * dk); }
+static bool eig_fits(int dk) { return eig_smem(dk, 2) <= kEigSmemMax; }      // 15 (N - 1) <= 165
+
+// The marginaliser of the uploaded windows [0, n) at their device states: the vision part of all n windows, then the dense
+// tail chunk by chunk (assemble -> frame Schur complement -> eigen-solver; a window's three kernels stay in one chunk, so
+// its old prior is consumed before its new one overwrites it).  eig = false stops after the Schur complement.
+// to_slots: S, e and the linearisation point (the CURRENT states of frames 1 .. N - 1) go straight into each window's own
+// prior arrays, where a later pack of the shifted window names them with prior_S == NULL; otherwise (n == 1) into the
+// scratch block of window 0.
+static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLayout &L) {
+    const int chunk = std::min(n, kMargChunkPerSm * h->sm_count);
+    L = marg_layout(h);
+    if (!h->marg) h->marg = new MargScratch();
+    if (h->marg->words < L.stride * chunk) {
+        if (h->marg->buf) cudaFree(h->marg->buf);
+        h->marg->buf = nullptr; h->marg->words = 0;
+        CK(h, cudaMalloc(&h->marg->buf, sizeof(double) * L.stride * chunk));
+        h->marg->words = L.stride * chunk;
+    }
+    static bool attr_set = false;
+    if (eig && !attr_set) { CK(h, cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEigSmemMax)); attr_set = true; }
+    // vision part: no loss, victim-seen landmarks only, mu = 0, fp64 (lin_obs_kernel<false, double> + schur_kernel<double>)
+    TRY(run_marg_vision(h, n));
+    const size_t Nc = h->Ncap, dcap = 15 * Nc, xs = Nc * kFrameStride;
+    MargArgs m = launch_args<MargArgs>(h);
+    m.index = index; m.buf = h->marg->buf; m.L = L;
+    for (int w0 = 0; w0 < n; w0 += chunk) {
+        const int cn = std::min(chunk, n - w0);
+        m.w0 = w0;
+        marg_assemble_kernel<<<cn, 256, 0, h->stream>>>(m);
+        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, h->marg->buf, L);
+        h->launches += 2;
+        if (!eig) continue;
+        int dk = 0;
+        for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[i].N - 1));
+        const int ring = eig_smem(dk, 4) <= kEigSmemMax ? 4 : 2;      // 2 when the matrix leaves no room: dk = 165
+        if (to_slots)
+            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, h->marg->buf, L, ring,
+                h->prior_S.d + w0 * dcap * dcap, dcap * dcap, h->prior_e.d + w0 * dcap, dcap, h->frames.d + w0 * xs,
+                h->prior_x0.d + w0 * xs, xs);
+        else
+            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, h->marg->buf, L, ring,
+                h->marg->buf + L.S, L.stride, h->marg->buf + L.e, L.stride, nullptr, nullptr, 0);
+        ++h->launches;
+    }
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// keep_on_device (index 0 only): the new prior is written straight into slot 0's prior arrays on the device (run_marg's
+// to_slots); the next solve of the shifted window names it with prior_S == NULL (pack_window) and nothing of it crosses PCIe.
 int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
                      double *S_out, double *e_out, double *H_out, double *b_out) {
     const int N = w->n_frames;
     if (index < 0 || index >= N || N < 2) return fail(h, PVIO_B200_EINVAL, "marginalize: bad frame index");
     if (!w->use_inertial) return fail(h, PVIO_B200_EINVAL, "marginalize: the window must carry motion states");
-    const int n = 15 * N, dk = n - 15;
+    const int dk = 15 * (N - 1);
     if (keep_on_device && index != 0) return fail(h, PVIO_B200_EINVAL, "marginalize: the resident prior is defined for index 0");
-    if ((S_out || e_out || keep_on_device) && sizeof(double) * ((size_t)dk * (dk | 1) + 6 * (size_t)dk) > 226 * 1024)
+    const bool eig = S_out || e_out || keep_on_device;
+    if (eig && !eig_fits(dk))
         return fail(h, PVIO_B200_EINVAL, "marginalize: window too large for the shared-memory eigen-solver (15 (N - 1) <= 165)");
-    int rc = pack_and_upload(h, w, s);
-    if (rc != 0) return rc;
-    // dense buffers: sized once from the handle's frame capacity
-    const size_t ncap = 15 * (size_t)h->Ncap, dcap = ncap - 15;
-    const size_t words = ncap * ncap + ncap + 3 * dcap * dcap + 2 * dcap + 2048 + 64 * (size_t)h->Ncap;
-    if (!h->marg) h->marg = new MargScratch();
-    if (h->marg->words < words) {
-        if (h->marg->buf) cudaFree(h->marg->buf);
-        h->marg->buf = nullptr; h->marg->words = 0;
-        CK(h, cudaMalloc(&h->marg->buf, sizeof(double) * words));
-        h->marg->words = words;
+    TRY(pack_and_upload(h, w, s));
+    MargLayout L;
+    TRY(run_marg(h, 1, index, eig, keep_on_device, L));
+    const double *blk = h->marg->buf;
+    if (H_out) CK(h, cudaMemcpyAsync(H_out, blk + L.Hk, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
+    if (b_out) CK(h, cudaMemcpyAsync(b_out, blk + L.bk, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
+    const double *dS = keep_on_device ? h->prior_S.d : blk + L.S, *de = keep_on_device ? h->prior_e.d : blk + L.e;
+    if (S_out) CK(h, cudaMemcpyAsync(S_out, dS, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
+    if (e_out) CK(h, cudaMemcpyAsync(e_out, de, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    CK(h, cudaGetLastError());
+    if (keep_on_device) h->prior_resident[0] = N - 1;
+    return 0;
+}
+
+// pvio_b200_batch_marginalize: every window is checked before anything is launched, so a rejected call changes nothing.
+int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride) {
+    if (n < 1 || n > h->n_uploaded) return fail(h, PVIO_B200_EINVAL, "batch_marginalize: windows not uploaded");
+    for (int i = 0; i < n; ++i) {
+        const WinHdr &H = h->hdr.h[i];
+        const int dk = 15 * (H.N - 1);
+        if (!H.use_inertial) return fail(h, PVIO_B200_EINVAL, "batch_marginalize: every window must carry motion states");
+        if (H.N < 2) return fail(h, PVIO_B200_EINVAL, "batch_marginalize: a window needs at least two frames");
+        if (!eig_fits(dk))
+            return fail(h, PVIO_B200_EINVAL, "batch_marginalize: window too large for the shared-memory eigen-solver (15 (N - 1) <= 165)");
+        if ((S_out && S_stride < (int64_t)dk * dk) || (e_out && e_stride < dk))
+            return fail(h, PVIO_B200_EINVAL, "batch_marginalize: output stride smaller than a window's prior");
     }
-    double *dH = h->marg->buf, *db = dH + ncap * ncap, *dHk = db + ncap, *dV = dHk + dcap * dcap, *dS = dV + dcap * dcap,
-           *dbk = dS + dcap * dcap, *de = dbk + dcap, *dscr = de + dcap;
-    // vision part: no loss, victim-seen landmarks only, mu = 0, fp64 (lin_obs_kernel<false, double> + schur_kernel<double>)
-    rc = run_marg_vision(h);
-    if (rc != 0) return rc;
-    MargArgs m = launch_args<MargArgs>(h);
-    m.index = index; m.H = dH; m.b = db; m.scratch = dscr;
-    marg_assemble_kernel<<<1, 256, 0, h->stream>>>(m);
-    marg_reduce_kernel<<<1, 256, 0, h->stream>>>(dH, db, N, index, dHk, dbk);
-    h->launches += 2;
-    if (H_out) CK(h, cudaMemcpyAsync(H_out, dHk, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
-    if (b_out) CK(h, cudaMemcpyAsync(b_out, dbk, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
-    if (S_out || e_out || keep_on_device) {
-        // matrix + d, e + the ring of rotation batches (4 slots; 2 when the matrix leaves no room: dk = 165)
-        const size_t esm4 = sizeof(double) * ((size_t)dk * (dk | 1) + 10 * (size_t)dk);
-        const int ring = esm4 <= 226 * 1024 ? 4 : 2;
-        const size_t esm = sizeof(double) * ((size_t)dk * (dk | 1) + (2 + 2 * (size_t)ring) * dk);
-        static bool attr_set = false;
-        if (!attr_set) { CK(h, cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024)); attr_set = true; }
-        marg_eig_kernel<<<1, 256, esm, h->stream>>>(dHk, dbk, dk, ring, dS, de);
-        ++h->launches;
-        if (S_out) CK(h, cudaMemcpyAsync(S_out, dS, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
-        if (e_out) CK(h, cudaMemcpyAsync(e_out, de, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
-        if (keep_on_device) {       // slot 0: dense dk x dk S, e, x0 = states of frames 1 .. N - 1 (read by the kernels above: stream order)
-            CK(h, cudaMemcpyAsync(h->prior_S.d, dS, sizeof(double) * dk * dk, cudaMemcpyDeviceToDevice, h->stream));
-            CK(h, cudaMemcpyAsync(h->prior_e.d, de, sizeof(double) * dk, cudaMemcpyDeviceToDevice, h->stream));
-            CK(h, cudaMemcpyAsync(h->prior_x0.d, h->frames.d + kFrameStride, sizeof(double) * (N - 1) * kFrameStride, cudaMemcpyDeviceToDevice, h->stream));
-        }
+    MargLayout L;
+    TRY(run_marg(h, n, 0, true, true, L));
+    const size_t dcap = 15 * (size_t)h->Ncap;
+    for (int i = 0; i < n; ++i) {          // slot i's prior arrays hold the dense dk x dk S and e at their start
+        const size_t dk = 15 * (size_t)(h->hdr.h[i].N - 1);
+        if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.d + i * dcap * dcap, sizeof(double) * dk * dk,
+                                         cudaMemcpyDeviceToHost, h->stream));
+        if (e_out) CK(h, cudaMemcpyAsync(e_out + i * e_stride, h->prior_e.d + i * dcap, sizeof(double) * dk,
+                                         cudaMemcpyDeviceToHost, h->stream));
     }
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    if (keep_on_device) { h->prior_resident = true; h->prior_resident_n = N - 1; }
+    for (int i = 0; i < n; ++i) h->prior_resident[i] = h->hdr.h[i].N - 1;
     return 0;
 }
 

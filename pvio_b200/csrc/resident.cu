@@ -145,7 +145,7 @@ int pvio_b200_window_reset(pvio_b200_handle hh, const pvio_b200_window *constant
     resident_free(h);
     h->resident = new ResidentWindow();
     h->resident->cst = *constants;
-    h->prior_resident = false; h->prior_resident_n = 0;
+    h->prior_resident[0] = 0;
     return 0;
 }
 
