@@ -272,6 +272,16 @@ typedef struct pvio_b200_pnp_problem {
 int pvio_b200_pnp_solve(pvio_b200_handle h, const pvio_b200_pnp_problem *problem, double *frame,
                         const pvio_b200_options *opt, pvio_b200_summary *summary);
 
+/* visual_inertial_pnp (pnp.cpp:32-100) for n independent problems, e.g. the new frame of n sequences, in ONE kernel
+ * launch, one CTA per problem.  problems [n]: as for pvio_b200_pnp_solve; each problem has its own points,
+ * extrinsics, sqrt_inv_cov, last frame and IMU record.  frames: n rows of frames_stride (>= 16) doubles, in/out.
+ * opt: shared by all problems.  summaries [n] (may be NULL): one per problem; solve_seconds = device time of the
+ * batched launch.  Every problem is checked before anything is copied: on PVIO_B200_EINVAL no frame has changed.
+ * n == 0 is a no-op.  Independent of the capacities given to pvio_b200_create.  A problem solved in a batch matches
+ * its pvio_b200_pnp_solve to rounding, not bit for bit (the per-point sums are combined in a different order). */
+int pvio_b200_batch_pnp_solve(pvio_b200_handle h, int n, const pvio_b200_pnp_problem *problems, double *frames,
+                              int64_t frames_stride, const pvio_b200_options *opt, pvio_b200_summary *summaries);
+
 /* Same, from the RAW 8-bit frames: CLAHE (cv::createCLAHE(clahe_clip, Size(tiles_x, tiles_y))->apply,
  * pvio-extra/src/pvio/extra/opencv_image.cpp:138-143: clip 6.0, 8 x 8 tiles) runs on the device between the upload and
  * the pyramid build, bit-exact with OpenCV.  width / height must be multiples of tiles_x / tiles_y (752x480 and

@@ -76,7 +76,7 @@ EXPORTS = [
     "pvio_b200_window_add_observations", "pvio_b200_window_remove_track", "pvio_b200_window_set_prior",
     "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
     "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
-    "pvio_b200_batch_marginalize",
+    "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve",
 ]
 
 _lib = None
@@ -125,6 +125,8 @@ def load():
     lib.pvio_b200_timer_stop.argtypes = [vp, c_f32p]
     lib.pvio_b200_last_kernel_ms.argtypes = [vp, C.c_int, c_f32p]
     lib.pvio_b200_pnp_solve.argtypes = [vp, C.POINTER(CPnpProblem), c_f64p, C.POINTER(COptions), C.POINTER(CSummary)]
+    lib.pvio_b200_batch_pnp_solve.argtypes = [vp, C.c_int, C.POINTER(CPnpProblem), c_f64p, C.c_int64,
+                                              C.POINTER(COptions), C.POINTER(CSummary)]
     lib.pvio_b200_klt_track.argtypes = [vp, c_u8p, c_u8p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p,
                                         C.c_int, C.c_int, C.c_int, C.c_double]
     for name in EXPORTS:

@@ -1298,6 +1298,13 @@ int pvio_b200_pnp_solve(pvio_b200_handle hh, const pvio_b200_pnp_problem *proble
     return pnp_solve_impl(h, problem, frame, opt, summary);
 }
 
+int pvio_b200_batch_pnp_solve(pvio_b200_handle hh, int n, const pvio_b200_pnp_problem *problems, double *frames,
+                              int64_t frames_stride, const pvio_b200_options *opt, pvio_b200_summary *summaries) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return batch_pnp_solve_impl(h, n, problems, frames, frames_stride, opt, summaries);
+}
+
 int pvio_b200_klt_track(pvio_b200_handle hh, const uint8_t *prev, const uint8_t *next, int width, int height, int stride,
                         const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points,
                         int max_level, int max_iter, double eps) {

@@ -92,7 +92,8 @@ struct Handle {
     KltState *klt = nullptr;
     MargScratch *marg = nullptr;
     FmState *fm = nullptr;
-    double *pnp_dev = nullptr, *pnp_host = nullptr;   // pnp.cu: device buffer + pinned staging, grown on demand
+    double *pnp_dev = nullptr, *pnp_host = nullptr;   // pnp.cu: device buffer + pinned staging, grown on demand to the
+                                                      // largest batch (records, points, IMU records, frames) seen
     size_t pnp_words = 0;
 };
 
@@ -148,6 +149,8 @@ void klt_free(Handle *h);
 // pnp.cu
 int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,
                    pvio_b200_summary *summary);
+int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
+                         const pvio_b200_options *opt, pvio_b200_summary *summaries);
 // ba_marg.cu
 void resident_free(Handle *h);     // resident.cu
 // klt.cu / detect.cu

@@ -9,25 +9,34 @@
 // variables in shared memory and runs every iteration of TrustRegionMinimizer + TRADITIONAL_DOGLEG
 // (Ceres 1.14 defaults as PVIO sets them, solver_options.h:26-33) on the device; the host sees one
 // launch and one read-back.  All arithmetic is fp64.
+//
+// A batch of independent problems (the new frame of many sequences) is one launch of the same kernel, one CTA per
+// problem: CTA b copies its record b into shared memory and solves on that copy.  The single call is a batch of one.
+#include <algorithm>
 #include <cstring>
 #include "api_internal.h"
 #include "ba_factors.cuh"
 
 namespace pvio {
 
-struct PnpArgs {
+struct PnpArgs {            // one problem's record, staged in device memory (pointers into the same staging buffer)
     const double *pts;      // [n][3]
     const double *z;        // [n][2]
     int n, inertial, max_iter;
     double radius0;
     WinConst wc;            // extrinsics, sqrt_inv_cov, cauchy_a
     double last[16];
-    const double *imu_rec;  // [288] device
+    const double *imu_rec;  // [288] device (null without inertial)
     double *frame;          // [16] in/out (device)
     double *out;            // [8] iterations, accepted, termination, usable, initial_cost, final_cost, radius, mu
 };
+static_assert(sizeof(PnpArgs) % sizeof(double) == 0, "records are staged as whole 8-byte words");
+constexpr int kPnpRecWords = sizeof(PnpArgs) / sizeof(double);
 
-constexpr int kPnpThreads = 256;
+// The two instantiations of pnp_kernel.  One problem (pvio_b200_pnp_solve, or a batch of one): 256 threads, the
+// whole register file of one SM, the shortest latency of a lone CTA.  n > 1 problems: 128 threads bounded to 4 CTAs
+// per SM (128 registers per thread), so a wave holds 4 problems per SM (DESIGN 4.6).
+constexpr int kPnpSingleThreads = 256, kPnpBatchThreads = 128, kPnpBatchCtasPerSm = 4;
 
 // residual (whitened) and local Jacobian of one pose-only reprojection block, fp64
 __device__ __forceinline__ void pnp_point(const double *R, const double *p, const double *Rcs, const double *pcs,
@@ -68,7 +77,9 @@ struct PnpShared {
 };
 
 // all threads: H, g, cost at state xs (jac) or only the cost
+template <int kPnpThreads>
 __device__ void pnp_evaluate(const PnpArgs &a, PnpShared &S, const double *xs, bool jac, double *cost_out) {
+    static_assert(kPnpThreads >= 64 && kPnpThreads % 32 == 0, "thread 32 evaluates the IMU factor");
     const int tid = threadIdx.x;
     __shared__ double R[9], Rcs[9];
     if (tid == 0) { quat_to_mat(xs, R); quat_to_mat(a.wc.cam_q, Rcs); }
@@ -157,16 +168,24 @@ __device__ bool pnp_chol_solve(const double *Hs, const double *lm2, const double
     return true;
 }
 
-__global__ void __launch_bounds__(kPnpThreads) pnp_kernel(PnpArgs a) {
+template <int kPnpThreads, int kMinCtas>
+__global__ void __launch_bounds__(kPnpThreads, kMinCtas) pnp_kernel(const PnpArgs *recs) {
     __shared__ PnpShared S;
+    __shared__ PnpArgs a;
     const int tid = threadIdx.x;
+    {
+        const unsigned long long *src = reinterpret_cast<const unsigned long long *>(recs + blockIdx.x);
+        unsigned long long *dst = reinterpret_cast<unsigned long long *>(&a);
+        for (int i = tid; i < kPnpRecWords; i += kPnpThreads) dst[i] = src[i];
+    }
+    __syncthreads();
     if (tid < 16) S.x[tid] = a.frame[tid];
     if (tid == 0) {
         S.done = 0; S.term = PVIO_B200_TERM_NO_CONVERGENCE; S.usable = 1; S.it = 0; S.accepted = 0; S.reuse = 0;
         S.radius = a.radius0; S.mu = 1e-8; S.nd = a.inertial ? 15 : 6;
     }
     __syncthreads();
-    pnp_evaluate(a, S, S.x, true, &S.cost);
+    pnp_evaluate<kPnpThreads>(a, S, S.x, true, &S.cost);
     if (tid == 0) {
         a.out[4] = S.cost;
         double gmax = 0.0;
@@ -242,7 +261,7 @@ __global__ void __launch_bounds__(kPnpThreads) pnp_kernel(PnpArgs a) {
         if (S.done) break;
         if (S.action == 0) continue;
         // ---------------- all threads: candidate cost
-        pnp_evaluate(a, S, S.xc, false, &S.cand_cost);
+        pnp_evaluate<kPnpThreads>(a, S, S.xc, false, &S.cand_cost);
         if (tid == 0) {
             S.action = 0;
             const double step_amb = sqrt(pnp_ambient_norm2(S.xc, S.x, a.inertial));
@@ -265,7 +284,7 @@ __global__ void __launch_bounds__(kPnpThreads) pnp_kernel(PnpArgs a) {
         }
         __syncthreads();
         if (S.action == 2) {
-            pnp_evaluate(a, S, S.x, true, &S.cost);
+            pnp_evaluate<kPnpThreads>(a, S, S.x, true, &S.cost);
             if (tid == 0) {
                 double gmax = 0.0;
                 for (int i = 0; i < S.nd; ++i) gmax = fmax(gmax, fabs(S.g[i]));
@@ -281,59 +300,98 @@ __global__ void __launch_bounds__(kPnpThreads) pnp_kernel(PnpArgs a) {
     }
 }
 
-int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,
-                   pvio_b200_summary *summary) {
-    const int n = pb->n_points;
-    if (n < 0 || !frame || !pb->last_frame || (pb->use_inertial && !pb->imu_data))
-        return fail(h, PVIO_B200_EINVAL, "pnp: bad arguments");
-    const size_t words = (size_t)5 * n + 16 + 8 + kImuStride;
-    if (words > h->pnp_words) {                       // this runs on every frame: no allocation in the steady state
+// n problems, frames [n][frames_stride]: every problem is checked before anything is copied; then one H2D copy of the
+// packed staging, one launch between ev0 / ev1, one D2H copy of the frames and summary words, one synchronise.
+int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
+                         const pvio_b200_options *opt, pvio_b200_summary *summaries) {
+    if (n < 0) return fail(h, PVIO_B200_EINVAL, "pnp: negative problem count");
+    if (n == 0) return 0;
+    if (!pbs || !frames || frames_stride < 16) return fail(h, PVIO_B200_EINVAL, "pnp: bad arguments");
+    size_t n_pts = 0, n_imu = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_pnp_problem &pb = pbs[i];
+        if (pb.n_points < 0 || !pb.last_frame || (pb.use_inertial && !pb.imu_data) ||
+            (pb.n_points > 0 && (!pb.points || !pb.z)))
+            return fail(h, PVIO_B200_EINVAL, "pnp: bad problem");
+        n_pts += pb.n_points;
+        n_imu += pb.use_inertial ? 1 : 0;
+    }
+    // staging layout (doubles): records [n][kPnpRecWords] | points [n_pts][3] and z [n_pts][2], problem after problem |
+    // IMU records [n_imu][kImuStride] of the inertial problems | frames [n][16] | summary words [n][8]
+    const size_t o_pts = (size_t)n * kPnpRecWords, o_z = o_pts + 3 * n_pts, o_imu = o_z + 2 * n_pts;
+    const size_t o_frames = o_imu + n_imu * kImuStride, o_out = o_frames + (size_t)16 * n, words = o_out + (size_t)8 * n;
+    if (words > h->pnp_words) {     // this runs on every frame: grown to the largest batch seen, no allocation in the steady state
         if (h->pnp_dev) cudaFree(h->pnp_dev);
         if (h->pnp_host) cudaFreeHost(h->pnp_host);
         h->pnp_dev = nullptr; h->pnp_host = nullptr; h->pnp_words = 0;
-        const size_t cap = std::max<size_t>(words, (size_t)5 * 512 + 16 + 8 + kImuStride);
+        const size_t cap = std::max<size_t>(words, (size_t)kPnpRecWords + 5 * 512 + kImuStride + 24);
         CK(h, cudaMalloc(&h->pnp_dev, sizeof(double) * cap));
         CK(h, cudaMallocHost(&h->pnp_host, sizeof(double) * cap));
         h->pnp_words = cap;
     }
     double *d = h->pnp_dev, *stage = h->pnp_host;
-    memset(stage, 0, sizeof(double) * words);
-    if (n > 0) { memcpy(stage, pb->points, sizeof(double) * 3 * n); memcpy(stage + 3 * n, pb->z, sizeof(double) * 2 * n); }
-    memcpy(stage + 5 * n, frame, sizeof(double) * 16);
-    if (pb->use_inertial) memcpy(stage + 5 * n + 24, pb->imu_data, sizeof(double) * kImuStride);
-    CK(h, cudaMemcpyAsync(d, stage, sizeof(double) * words, cudaMemcpyHostToDevice, h->stream));
-    PnpArgs a;
-    memset(&a, 0, sizeof(a));
-    a.pts = d; a.z = d + 3 * n; a.frame = d + 5 * n; a.out = d + 5 * n + 16; a.imu_rec = d + 5 * n + 24;
-    a.n = n; a.inertial = pb->use_inertial ? 1 : 0;
+    PnpArgs *recs = reinterpret_cast<PnpArgs *>(stage);
     const SolveOptions o = solve_options(opt);
-    a.max_iter = o.max_iter;
-    a.radius0 = o.radius0;
-    memcpy(a.wc.cam_q, pb->cam_q_cs, 32); memcpy(a.wc.cam_p, pb->cam_p_cs, 24);
-    memcpy(a.wc.imu_q, pb->imu_q_cs, 32); memcpy(a.wc.imu_p, pb->imu_p_cs, 24);
-    memcpy(a.wc.sic, pb->sqrt_inv_cov, 32);
-    a.wc.cauchy_a = pb->cauchy_a > 0 ? pb->cauchy_a : 1.0;
-    memcpy(a.last, pb->last_frame, sizeof(double) * 16);
+    size_t p = 0, k = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_pnp_problem &pb = pbs[i];
+        const int m = pb.n_points;
+        PnpArgs &a = recs[i];
+        memset(&a, 0, sizeof(a));
+        if (m > 0) {
+            memcpy(stage + o_pts + 3 * p, pb.points, sizeof(double) * 3 * m);
+            memcpy(stage + o_z + 2 * p, pb.z, sizeof(double) * 2 * m);
+        }
+        a.pts = d + o_pts + 3 * p; a.z = d + o_z + 2 * p;
+        a.n = m; a.inertial = pb.use_inertial ? 1 : 0;
+        a.max_iter = o.max_iter;
+        a.radius0 = o.radius0;
+        memcpy(a.wc.cam_q, pb.cam_q_cs, 32); memcpy(a.wc.cam_p, pb.cam_p_cs, 24);
+        memcpy(a.wc.imu_q, pb.imu_q_cs, 32); memcpy(a.wc.imu_p, pb.imu_p_cs, 24);
+        memcpy(a.wc.sic, pb.sqrt_inv_cov, 32);
+        a.wc.cauchy_a = pb.cauchy_a > 0 ? pb.cauchy_a : 1.0;
+        memcpy(a.last, pb.last_frame, sizeof(double) * 16);
+        if (a.inertial) {
+            memcpy(stage + o_imu + k * kImuStride, pb.imu_data, sizeof(double) * kImuStride);
+            a.imu_rec = d + o_imu + k * kImuStride;
+            ++k;
+        }
+        memcpy(stage + o_frames + 16 * (size_t)i, frames + frames_stride * i, sizeof(double) * 16);
+        a.frame = d + o_frames + 16 * (size_t)i;
+        a.out = d + o_out + 8 * (size_t)i;
+        p += m;
+    }
+    CK(h, cudaMemcpyAsync(d, stage, sizeof(double) * o_out, cudaMemcpyHostToDevice, h->stream));
+    const PnpArgs *d_recs = reinterpret_cast<const PnpArgs *>(d);
     CK(h, cudaEventRecord(h->ev0, h->stream));
-    pnp_kernel<<<1, kPnpThreads, 0, h->stream>>>(a);
+    if (n == 1) pnp_kernel<kPnpSingleThreads, 1><<<1, kPnpSingleThreads, 0, h->stream>>>(d_recs);
+    else pnp_kernel<kPnpBatchThreads, kPnpBatchCtasPerSm><<<n, kPnpBatchThreads, 0, h->stream>>>(d_recs);
     CK(h, cudaEventRecord(h->ev1, h->stream));
     ++h->launches;
-    double *back = stage + 5 * n;                     // the frame + summary words come back into the pinned staging
-    CK(h, cudaMemcpyAsync(back, d + 5 * n, sizeof(double) * 24, cudaMemcpyDeviceToHost, h->stream));
+    // the frames + summary words come back into the pinned staging
+    CK(h, cudaMemcpyAsync(stage + o_frames, d + o_frames, sizeof(double) * 24 * n, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    memcpy(frame, back, sizeof(double) * 16);
-    if (summary) {
+    float ms = 0.f;
+    if (summaries) cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+    for (int i = 0; i < n; ++i) {
+        memcpy(frames + frames_stride * i, stage + o_frames + 16 * (size_t)i, sizeof(double) * 16);
+        if (!summaries) continue;
+        const double *back = stage + o_out + 8 * (size_t)i;
+        pvio_b200_summary *summary = summaries + i;
         memset(summary, 0, sizeof(*summary));
-        summary->iterations = (int)back[16]; summary->accepted_steps = (int)back[17];
-        summary->termination = (int)back[18]; summary->usable = (int)back[19];
-        summary->initial_cost = back[20]; summary->final_cost = back[21];
-        summary->final_radius = back[22]; summary->final_mu = back[23];
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+        summary->iterations = (int)back[0]; summary->accepted_steps = (int)back[1];
+        summary->termination = (int)back[2]; summary->usable = (int)back[3];
+        summary->initial_cost = back[4]; summary->final_cost = back[5];
+        summary->final_radius = back[6]; summary->final_mu = back[7];
         summary->solve_seconds = ms * 1e-3;
     }
     return 0;
+}
+
+int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,
+                   pvio_b200_summary *summary) {
+    return batch_pnp_solve_impl(h, 1, pb, frame, 16, opt, summary);
 }
 
 }  // namespace pvio
