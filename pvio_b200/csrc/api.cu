@@ -63,7 +63,7 @@ static LinBufs lin_bufs(Handle *h) {
 // cached graphs: their launches carry the old view.
 static void refresh_arrays(Handle *h) {
     BatchArrays &a = h->arrays;
-    a.hdr = h->hdr.d; a.cst = h->cst.d; a.obs = h->obs.d; a.fobs = h->fobs.d; a.seg = h->seg.d; a.lms = h->lms.d;
+    a.hdr = h->hdr.d; a.cst = h->cst.d; a.obs = h->obs.d; a.fz = h->fz.d; a.flm = h->flm.d; a.seg = h->seg.d; a.lms = h->lms.d;
     a.rho = h->rho.d; a.frames = h->frames.d; a.ctrl = h->ctrl.d; a.rho_cand = h->rho_cand.d; a.frames_cand = h->frames_cand.d;
     a.lm_scale = h->lm_scale.d; a.lm_aux = h->lm_aux.d; a.lm_w = h->lm_w.d; a.lm_msk = h->lm_msk.d; a.jr = h->jr.d; a.hs = h->hs.d;
     a.Hred = h->Hred.d; a.Hdd = h->Hdd.d; a.gdir = h->gdir.d; a.gred = h->gred.d; a.cost_vis = h->cost_vis.d;
@@ -489,6 +489,9 @@ static int sweep_grid_x(Handle *h, int n) { return n * 2 < h->sm_count ? 16 : 1;
 // slower per step, 3 for either is within the run-to-run spread; the results do not depend on them.  The update sweep at
 // 8 CTAs / SM (64 registers) takes 0.352 ms per step, at 6 (80 registers) 0.361 ms (H100 SXM, 700 W power limit).
 constexpr int kLinWarps = 4, kLinBlocks = 4;
+// the linearise sweep may drop to 3 CTAs / SM for its fp64 shared-memory sums (lin_part_fits); 3 CTAs / SM alone was
+// measured within the run-to-run spread (above)
+constexpr int kLinPartMinBlocks = 3;
 constexpr int kSchurThreads = 128, kSchurBlocks = 4;
 constexpr int kUpdWarps = 4, kUpdBlocks = 8;
 
@@ -518,6 +521,28 @@ static __global__ void zero_system_kernel(PipeArgs a_in, int npairs_cap) {
     if (threadIdx.x == 0) a.cost_vis[w] = 0.0;
 }
 
+// Whether a linearise CTA that owns its window keeps the per-landmark (j.j, j.r) sums in shared memory (PipeArgs::lm_part)
+// at this shape: only when the larger layout fits and leaves at least min(kLinPartMinBlocks, the CTAs / SM without it)
+// resident (occupancy API: registers and shared memory), so that e.g. a large max_landmarks falls back to the jr records
+// instead of failing or losing more occupancy.
+template <typename real>
+static bool lin_part_fits(Handle *h, const void *kernel, int N, int Mp) {
+    const auto key = std::make_tuple((int)sizeof(real), N, Mp);
+    auto it = h->lin_part.find(key);
+    if (it != h->lin_part.end()) return it->second;
+    const size_t with = lin_smem_bytes<real>(N, Mp, kLinWarps, true), without = lin_smem_bytes<real>(N, Mp, kLinWarps, false);
+    int nb_with = 0, nb_without = 0;
+    bool ok = false;
+    if ((int)with <= h->smem_lim) {
+        const cudaError_t e1 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_with, kernel, kLinWarps * 32, with);
+        const cudaError_t e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_without, kernel, kLinWarps * 32, without);
+        if (e1 != cudaSuccess || e2 != cudaSuccess) cudaGetLastError();      // a failed query only means: keep jr
+        else ok = nb_with >= 1 && nb_with >= std::min(nb_without, kLinPartMinBlocks);
+    }
+    h->lin_part[key] = ok;
+    return ok;
+}
+
 // linearise sweep (+ per-landmark completion as its own launch when several CTAs share a window).  spec: the
 // speculative sweep of the trust-region loop over the CANDIDATE, into the window's other buffer set (ba_tr.cuh).
 static int launch_lin(Handle *h, int n, const StepCfg &c, const BatchShape &b, bool loss, bool victim_only, bool spec) {
@@ -534,12 +559,15 @@ static int launch_lin(Handle *h, int n, const StepCfg &c, const BatchShape &b, b
     const int Mp = (b.M + 31) & ~31;
     if (!h->hs_double) {
         if (!loss) return fail(h, PVIO_B200_EINVAL, "the loss-free sweep runs in fp64");
-        lin_obs_kernel<true, float, kLinWarps, kLinBlocks><<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<float>(b.N, Mp, kLinWarps), st>>>(a);
+        auto k = lin_obs_kernel<true, float, kLinWarps, kLinBlocks>;
+        a.lm_part = gx == 1 && lin_part_fits<float>(h, (const void *)k, b.N, Mp) ? 1 : 0;
+        k<<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<float>(b.N, Mp, kLinWarps, a.lm_part), st>>>(a);
         LAUNCH_CK(h, "lin_obs_kernel<float>");
         if (gx > 1) { lm_finish_kernel<float><<<dim3((b.M + 127) / 128, n), 128, 0, st>>>(a); ++h->launches; LAUNCH_CK(h, "lm_finish_kernel<float>"); }
     } else {
-        if (loss) lin_obs_kernel<true, double, kLinWarps, 2><<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<double>(b.N, Mp, kLinWarps), st>>>(a);
-        else lin_obs_kernel<false, double, kLinWarps, 2><<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<double>(b.N, Mp, kLinWarps), st>>>(a);
+        auto k = loss ? lin_obs_kernel<true, double, kLinWarps, 2> : lin_obs_kernel<false, double, kLinWarps, 2>;
+        a.lm_part = gx == 1 && lin_part_fits<double>(h, (const void *)k, b.N, Mp) ? 1 : 0;
+        k<<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<double>(b.N, Mp, kLinWarps, a.lm_part), st>>>(a);
         LAUNCH_CK(h, "lin_obs_kernel<double>");
         if (gx > 1) { lm_finish_kernel<double><<<dim3((b.M + 127) / 128, n), 128, 0, st>>>(a); ++h->launches; LAUNCH_CK(h, "lm_finish_kernel<double>"); }
     }
@@ -940,7 +968,9 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
     const size_t W = h->W, N = h->Ncap, M = h->Mcap, K = h->Kcap, npc = N * (N + 1) / 2;
     TRY(alloc(h, h->hdr, W, true)); TRY(alloc(h, h->cst, W, true));
     TRY(alloc(h, h->obs, W * K, true)); TRY(alloc(h, h->lms, W * M, true));
-    TRY(alloc(h, h->fobs, W * K, false)); TRY(alloc(h, h->seg, W * kSegTab, false));
+    // flm is padded: the update sweep copies five 16-byte granules from the one holding a row's first index (row_prefetch)
+    TRY(alloc(h, h->fz, W * K, false)); TRY(alloc(h, h->flm, W * K + kFlmPad, false));
+    TRY(alloc(h, h->seg, W * kSegTab, false));
     TRY(alloc(h, h->rho, W * M, true)); TRY(alloc(h, h->frames, W * N * kFrameStride, true));
     TRY(alloc(h, h->ctrl, W, true));
     TRY(alloc(h, h->rho_cand, W * M, false)); TRY(alloc(h, h->frames_cand, W * N * kFrameStride, false));
@@ -973,6 +1003,7 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
     {   // opt in to large dynamic shared memory ONCE per kernel with the device limit: the attribute is process-wide, so a
         // per-handle value would be overwritten by the next handle with other capacities
         const int lim = (int)prop.sharedMemPerBlockOptin - 2048;
+        h->smem_lim = lim;
         CK(h, cudaFuncSetAttribute(lin_obs_kernel<true, float, kLinWarps, kLinBlocks>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(lin_obs_kernel<true, double, kLinWarps, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(lin_obs_kernel<false, double, kLinWarps, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
@@ -1008,7 +1039,7 @@ void pvio_b200_destroy(pvio_b200_handle hh) {
     detect_free(h);
     fm_free(h);
     release(h->hdr); release(h->cst); release(h->obs); release(h->lms); release(h->rho); release(h->frames);
-    release(h->fobs); release(h->seg); release(h->jr); release(h->lm_w); release(h->lm_msk); release(h->frames_out); release(h->rho_out); release(h->lm_v); release(h->valid); release(h->quality);
+    release(h->fz); release(h->flm); release(h->seg); release(h->jr); release(h->lm_w); release(h->lm_msk); release(h->frames_out); release(h->rho_out); release(h->lm_v); release(h->valid); release(h->quality);
     release(h->ctrl); release(h->rho_cand); release(h->frames_cand); release(h->lm_scale); release(h->lm_aux); release(h->hs);
     release(h->dx_lm); release(h->dx_pose); release(h->pose_scale); release(h->v_pose); release(h->Hred);
     release(h->acc); release(h->aux_cost);

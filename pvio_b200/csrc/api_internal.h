@@ -42,12 +42,16 @@ struct Handle {
     struct DetectState *detect = nullptr;         // detect.cu
     size_t sys_set = 0;                           // elements between the two buffer sets of the reduced-system arrays (LinBufs)
     int sm_count = 132;                           // set from the device at create
+    int smem_lim = 0;                             // dynamic shared memory the large-layout kernels opt in to (create)
+    std::map<std::tuple<int, int, int>, bool> lin_part;   // (sizeof(real), N, Mp) -> the linearise sweep keeps its
+                                                          // per-landmark sums in shared memory (api.cu: lin_part_fits)
 
     // vision (always allocated)
     DevBuf<WinHdr> hdr;
     DevBuf<WinConst> cst;
     DevBuf<ObsRec> obs;                          // landmark-major table as the shim gathers it (uploaded)
-    DevBuf<FObs> fobs;                           // frame-major table, built on the device after every upload
+    DevBuf<float2> fz;                           // frame-major table, built on the device after every upload: keypoints
+    DevBuf<FLm> flm;                             //   and landmark indices
     DevBuf<int32_t> seg;                         // [W][kSegTab]
     DevBuf<LmRec> lms;
     DevBuf<double> rho, frames;

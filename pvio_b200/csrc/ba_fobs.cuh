@@ -9,7 +9,7 @@
 
 namespace pvio {
 
-struct FobsArgs : BatchArrays {      // obs -> fobs, seg
+struct FobsArgs : BatchArrays {      // obs -> fz, flm, seg
     int w0;
 };
 
@@ -69,7 +69,8 @@ __global__ void __launch_bounds__(256) fobs_build_kernel(FobsArgs a) {
         }
     }
     __syncthreads();
-    FObs *fo = a.fobs + (size_t)w * a.Kcap;
+    float2 *fz = a.fz + (size_t)w * a.Kcap;
+    FLm *flm = a.flm + (size_t)w * a.Kcap;
     for (int ch = wv; ch < nch; ch += 8) {
         const int c = H.chunk_meta[ch] & 0xff;
         const int l = H.chunk_begin[ch] + lane;
@@ -82,9 +83,8 @@ __global__ void __launch_bounds__(256) fobs_build_kernel(FobsArgs a) {
             if ((m >> t) & 1u) {
                 const int pos = cnt[ch][t] + __popc(b & ((1u << lane) - 1u));
                 const ObsRec o = obs[lr.obs_begin + __popc(m & ((1u << t) - 1u))];
-                FObs rec;
-                rec.zx = o.zx; rec.zy = o.zy; rec.lm = l; rec.pad = 0;
-                fo[pos] = rec;
+                fz[pos] = make_float2(o.zx, o.zy);
+                flm[pos] = (FLm)l;
             }
         }
     }

@@ -15,8 +15,10 @@
 //             segment; a warp owns a contiguous range of rows.  Thread = residual block.  The target pose sits
 //             in registers for the whole segment; Y^T Y, Y^T r of the segment are REGISTER sums (float2
 //             pairs of fma.rn.f32), reduced across the warp once per segment; h_t = Y^T j leaves as one coalesced
-//             24-byte store per lane into the frame-major record array hs[t][l][6], (j.j, j.r) as one
-//             8-byte store into jr[t][l][2] (the Schur kernel sums them per landmark, in frame order).
+//             24-byte store per lane into the frame-major record array hs[t][l][6].  (j.j, j.r): when one CTA
+//             owns the window (and the shared layout fits, PipeArgs::lm_part), added into the warp's own
+//             per-landmark partial in shared memory; otherwise one 8-byte store into jr[t][l][2].  lm_finish
+//             sums either per landmark, in frame order.
 //   epilogue  direct blocks -> Hred / gred (the Schur kernel subtracts its sum).
 // real = float: fp32 Jacobians, fp64 residual numerators (the visual-only throughput path);
 // real = double: everything fp64 (inertial windows, whose reduced system is too ill-conditioned for fp32
@@ -37,6 +39,7 @@ struct PipeArgs : BatchArrays {
     int w0;                      // first window of this launch
     int loop;                    // 1: iteration of the device-side trust-region loop (ba_tr.cuh): obey the window's flags
     int spec;                    // loop only. 1: linearise the CANDIDATE (frames_cand, rho_cand) into the window's other buffer set
+    int lm_part;                 // 1 (one CTA per window only): the (j.j, j.r) sums stay in shared memory, jr is not touched
 };
 
 __device__ __forceinline__ void pipe_select(PipeArgs &a, int b) {
@@ -219,6 +222,13 @@ __device__ __forceinline__ void lm_sm_load(unsigned rec, double (&x)[3], double 
     x[2] = bx; xf[0] = x[0]; xf[1] = x[1]; xf[2] = bx;
     c[0] = by; c[1] = dx; c[2] = dy;
 }
+// *addr += v for a (j.j, j.r) partial at a shared-space address (phase 1 of lin_obs_kernel with lm_part)
+__device__ __forceinline__ void part_add(unsigned addr, double2 v) {
+    double x, y;
+    asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(x), "=d"(y) : "r"(addr) : "memory");
+    x = __dadd_rn(x, v.x); y = __dadd_rn(y, v.y);
+    asm volatile("st.shared.v2.f64 [%0], {%1, %2};" :: "r"(addr), "d"(x), "d"(y) : "memory");
+}
 // read-ahead of [p, p + bytes) into L2 by the whole CTA (the sweeps are latency-bound: 16 warps per SM)
 __device__ __forceinline__ void l2_prefetch(const void *p, size_t bytes, int tid, int nthreads) {
     const char *c = reinterpret_cast<const char *>(p);
@@ -288,13 +298,31 @@ struct RowCursor {
     __device__ __forceinline__ int k0() const { return sbeg[sp] + (r - srow[sp]) * 32; }
 };
 
-// request row pf.r (if the warp owns it) into `dst` (32 entries) and move the prefetch cursor on; one commit group per
-// call, empty or not, so that the consumer's wait_group count stays uniform
-__device__ __forceinline__ void row_prefetch(RowCursor &pf, int r_end, const FObs *fobs, FObs *dst, int lane) {
+// One row of the frame-major table in shared memory: the 32 keypoints (lane i copies and reads entry i), then the five
+// 16-byte granules of flm from the one that holds the row's first index (a row starts anywhere in a granule), copied
+// by lanes 0-4 and read by every lane, so the consumer needs __syncwarp around them.
+constexpr int kFlmPad = 40;                     // entries of flm allocated beyond the last table entry
+struct RowSlot {
+    float2 z[32];
+    uint4 lm[5];
+    int off;                                    // halfword of the row's first index in lm[0]
+};
+__device__ __forceinline__ int row_lm(const RowSlot &s, int lane) {
+    return reinterpret_cast<const FLm *>(s.lm)[s.off + lane];
+}
+
+// request row pf.r (if the warp owns it) into `dst` and move the prefetch cursor on; one commit group per call, empty
+// or not, so that the consumer's wait_group count stays uniform
+__device__ __forceinline__ void row_prefetch(RowCursor &pf, int r_end, const float2 *fz, const FLm *flm, RowSlot *dst, int lane) {
     if (pf.r < r_end) {
-        const int k = pf.k0() + lane;
-        if (k < pf.sbeg[pf.sp + 1])
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"((uint32_t)__cvta_generic_to_shared(dst + lane)), "l"(fobs + k) : "memory");
+        const int k0 = pf.k0();
+        if (k0 + lane < pf.sbeg[pf.sp + 1])
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" :: "r"((uint32_t)__cvta_generic_to_shared(dst->z + lane)), "l"(fz + k0 + lane) : "memory");
+        // always all five granules (flm is allocated kFlmPad entries beyond the table for this)
+        const uintptr_t p = reinterpret_cast<uintptr_t>(flm + k0), g0 = p & ~(uintptr_t)15;
+        if (lane < 5)
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"((uint32_t)__cvta_generic_to_shared(dst->lm + lane)), "l"(g0 + 16 * (uintptr_t)lane) : "memory");
+        if (lane == 0) dst->off = (int)(p & 15) >> 1;
         pf.advance();
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
@@ -306,8 +334,11 @@ __device__ __forceinline__ void row_prefetch(RowCursor &pf, int r_end, const FOb
 // Schur complement divides by (bundle_adjustor.cpp:537-538: skipped when not finite) --, the anchor block
 // h_la = -sum_t h_lt when the anchor frame is free, zero blocks for the free frames that do not see the landmark
 // (the Schur tiles then need no per-block predicate).
+// part: the per-warp partial sums [nwarps][Mp] of the CTA's shared memory (lin_obs_kernel with lm_part), each a sum
+// in frame order; summed here in warp order, which is again frame order.  nullptr: the per-block pairs in jr.
 template <typename real>
-__device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N, int M, unsigned fixed, double mu, int compute_scale) {
+__device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N, int M, unsigned fixed, double mu, int compute_scale,
+                                          const double2 *part = nullptr, int nwarps = 0, int Mp = 0) {
     typedef typename Vec2<real>::type real2;
     const LmRec *lms = a.lms + (size_t)w * a.Mcap;
     real2 *wv = reinterpret_cast<real2 *>(a.lm_w) + (size_t)w * a.Mcap;
@@ -323,10 +354,12 @@ __device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N
         if (!a.victim_only) { aux[l].hll_reg = 1.0; aux[l].gl = 0.0; aux[l].hll = 0.0; }
         return;
     }
-    const real2 *jr = reinterpret_cast<const real2 *>(a.jr) + (size_t)w * a.Ncap * a.Mcap;
     real *hs = reinterpret_cast<real *>(a.hs) + (size_t)w * a.Ncap * a.Mcap * 6;
     double hll = 0.0, gl = 0.0;
-    {   // all loads first (independent, predicated), then the sums in frame order
+    if (part) {
+        for (int q = 0; q < nwarps; ++q) { const double2 v = part[q * Mp + l]; hll += v.x; gl += v.y; }
+    } else {   // all loads first (independent, predicated), then the sums in frame order
+        const real2 *jr = reinterpret_cast<const real2 *>(a.jr) + (size_t)w * a.Ncap * a.Mcap;
         real2 v[kMaxFrames];
 #pragma unroll
         for (int f = 0; f < kMaxFrames; ++f) {
@@ -382,22 +415,24 @@ __global__ void __launch_bounds__(128) lm_finish_kernel(PipeArgs a_in) {
 }
 
 template <typename real>
-__host__ __device__ inline size_t lin_smem_layout(int N, int Mp, size_t *o_dta, size_t *o_seg, size_t *o_rec, size_t *o_rs, size_t *o_skip) {
+__host__ __device__ inline size_t lin_smem_layout(int N, int Mp, int warps, bool part, size_t *o_dta, size_t *o_seg, size_t *o_rec,
+                                                  size_t *o_rs, size_t *o_skip, size_t *o_part) {
     const size_t nsp = (size_t)N * (N - 1) / 2;
     size_t off = sizeof(double) * 12 * (size_t)N;                              // frames: Rwc[9], c[3]
     *o_dta = off; off += sizeof(double) * ((nsp + 1 + (size_t)N) * kDta + 8);  // direct blocks (pairs, then per frame), cost
     *o_seg = off; off += sizeof(int32_t) * kSegTab;
     off = (off + 15) & ~(size_t)15;
     *o_rec = off; off += (size_t)kLmSm * Mp;                                   // landmark records (lm_sm_store)
+    *o_part = off; if (part) off += sizeof(double2) * (size_t)warps * Mp;      // per-warp (j.j, j.r) sums (PipeArgs::lm_part)
     *o_rs = off; off += sizeof(real) * 12 * (size_t)N;                         // (real) Rwc of every frame
     *o_skip = off; off += (size_t)Mp;                                          // 1: landmark not linearised (victim-only sweeps)
     return (off + 15) & ~(size_t)15;
 }
 
 template <typename real>
-__host__ __device__ inline size_t lin_smem_bytes(int N, int Mp, int /*warps*/) {
-    size_t a, b, c, d, e;
-    return lin_smem_layout<real>(N, Mp, &a, &b, &c, &d, &e);
+__host__ __device__ inline size_t lin_smem_bytes(int N, int Mp, int warps, bool part) {
+    size_t a, b, c, d, e, f;
+    return lin_smem_layout<real>(N, Mp, warps, part, &a, &b, &c, &d, &e, &f);
 }
 
 template <bool kLoss, typename real, int kWarps, int kMinBlocks>
@@ -419,8 +454,9 @@ lin_obs_kernel(PipeArgs a_in) {
     const int nsp = N * (N - 1) / 2;
 
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    size_t o_dta, o_seg, o_rec, o_rs, o_skip;
-    lin_smem_layout<real>(N, Mp, &o_dta, &o_seg, &o_rec, &o_rs, &o_skip);
+    const bool lpart = a.lm_part != 0;
+    size_t o_dta, o_seg, o_rec, o_rs, o_skip, o_part;
+    lin_smem_layout<real>(N, Mp, kWarps, lpart, &o_dta, &o_seg, &o_rec, &o_rs, &o_skip, &o_part);
     double *Fs = reinterpret_cast<double *>(smem_raw);                       // [N][12]
     double *Dta = reinterpret_cast<double *>(smem_raw + o_dta);              // [nsp + 1][kDta]
     double *Ddg = Dta + (nsp + 1) * kDta;                                    // [N][kDta] sum of the blocks touching frame f (signed gradient)
@@ -429,9 +465,11 @@ lin_obs_kernel(PipeArgs a_in) {
     unsigned char *recs = smem_raw + o_rec;                                  // [Mp] landmark records
     real *Rs = reinterpret_cast<real *>(smem_raw + o_rs);                    // [N][12] (real) Rwc
     unsigned char *skip = smem_raw + o_skip;
+    double2 *part = reinterpret_cast<double2 *>(smem_raw + o_part);         // [kWarps][Mp] when lpart
 
     if (gridDim.x == 1) {          // everything this CTA will read from HBM, requested before the first dependent load
-        l2_prefetch(a.fobs + (size_t)w * a.Kcap, sizeof(FObs) * (size_t)H.K, tid, kThreads);
+        l2_prefetch(a.fz + (size_t)w * a.Kcap, sizeof(float2) * (size_t)H.K, tid, kThreads);
+        l2_prefetch(a.flm + (size_t)w * a.Kcap, sizeof(FLm) * (size_t)H.K, tid, kThreads);
         l2_prefetch(a.lms + (size_t)w * a.Mcap, sizeof(LmRec) * (size_t)M, tid, kThreads);
         l2_prefetch(a.rho + (size_t)w * a.Mcap, sizeof(double) * (size_t)M, tid, kThreads);
     }
@@ -447,6 +485,7 @@ lin_obs_kernel(PipeArgs a_in) {
     }
     for (int i = tid; i < (nsp + 1 + N) * kDta + 8; i += kThreads) Dta[i] = 0.0;
     for (int i = tid; i < kSegTab; i += kThreads) sg[i] = a.seg[(size_t)w * kSegTab + i];
+    if (lpart) for (int i = tid; i < kWarps * Mp; i += kThreads) part[i] = make_double2(0.0, 0.0);
     __syncthreads();
 
     // ---- phase 0: world points (reprojection_error_cost.h:58-60)
@@ -480,7 +519,8 @@ lin_obs_kernel(PipeArgs a_in) {
     const real inv_cb = (real)(1.0 / (wc.cauchy_a * wc.cauchy_a));
     const bool diag_w = wc.sic[1] == 0.0 && wc.sic[2] == 0.0;
     const bool vo = a.victim_only != 0;      // only then can a landmark of the table be left out (skip[])
-    const FObs *fobs = a.fobs + (size_t)w * a.Kcap;
+    const float2 *fz = a.fz + (size_t)w * a.Kcap;
+    const FLm *flm = a.flm + (size_t)w * a.Kcap;
     real *hs = reinterpret_cast<real *>(a.hs) + (size_t)w * a.Ncap * a.Mcap * 6;
     real2 *jr = reinterpret_cast<real2 *>(a.jr) + (size_t)w * a.Ncap * a.Mcap;
     const unsigned fixed = (unsigned)H.fixed_mask & ((1u << N) - 1u);
@@ -491,6 +531,8 @@ lin_obs_kernel(PipeArgs a_in) {
 
     unsigned recs_a = (unsigned)__cvta_generic_to_shared(recs);
     asm volatile("" : "+r"(recs_a));           // opaque: ptxas would otherwise re-derive the base from (N, Mp) in every row
+    unsigned part_w = (unsigned)__cvta_generic_to_shared(part) + (unsigned)(wv * Mp) * (unsigned)sizeof(double2);   // this warp's partial
+    asm volatile("" : "+r"(part_w));
     RowCursor cs(sbeg, srow, r_begin, rows);
     real cost_acc = 0;
     LogAcc<real> la;
@@ -523,31 +565,35 @@ lin_obs_kernel(PipeArgs a_in) {
             if (e >= 0) atomicAdd(&Dta[sp * kDta + e], tot);          // +sum Y^T Y, Y^T r; the epilogue applies the signs
         };
         // the table entry of the NEXT row is requested before the current row is evaluated
-        // (12 of the entry's 16 bytes are loaded: a 16-byte load would tie up a register for the padding word)
         int k = cs.k0() + lane;
-        const FObs *pk = fobs + k;
+        const float2 *pz = fz + k;
+        const FLm *pl = flm + k;
         float2 z_nx = make_float2(0.f, 0.f);
         int l_nx = 0;
-        if (k < seg_end) { z_nx = *reinterpret_cast<const float2 *>(pk); l_nx = pk->lm; }
+        if (k < seg_end) { z_nx = *pz; l_nx = *pl; }
         const int nrow = r_stop - cs.r;
         for (int i = 0; i < nrow; ++i) {
-            FObs o;
-            o.zx = z_nx.x; o.zy = z_nx.y; o.lm = l_nx;
+            const float2 z = z_nx;
+            const int l = l_nx;
             const bool valid = k < seg_end;
-            k += 32; pk += 32;
-            if (i + 1 < nrow && k < seg_end) { z_nx = *reinterpret_cast<const float2 *>(pk); l_nx = pk->lm; }
+            k += 32; pz += 32; pl += 32;
+            if (i + 1 < nrow && k < seg_end) { z_nx = *pz; l_nx = *pl; }
             if (valid) {
-                const int l = o.lm;
                 if (!(vo && skip[l])) {
                     ObsL<real> ol;
                     double x[3];
                     real xf[3], cl[3];
                     lm_sm_load(recs_a + (unsigned)l * kLmSm, x, xf, cl);
-                    linearize_blk<kLoss, real>(F, x[0], x[1], x[2], xf[0], xf[1], xf[2], cl[0], cl[1], cl[2], o.zx, o.zy, W,
+                    linearize_blk<kLoss, real>(F, x[0], x[1], x[2], xf[0], xf[1], xf[2], cl[0], cl[1], cl[2], z.x, z.y, W,
                                                diag_w, inv_cb, ol);
                     if (kLoss) la.add(ol.cost); else cost_acc += ol.cost;
                     const unsigned rec = tM + (unsigned)l;
-                    jr[rec] = mk2(ol.j0 * ol.j0 + ol.j1 * ol.j1, ol.j0 * ol.r0 + ol.j1 * ol.r1);
+                    const real2 jj = mk2(ol.j0 * ol.j0 + ol.j1 * ol.j1, ol.j0 * ol.r0 + ol.j1 * ol.r1);
+                    if (lpart) {        // the warp's own partial; a row holds a landmark at most once: no two lanes collide
+                        part_add(part_w + (unsigned)l * (unsigned)sizeof(double2), make_double2((double)jj.x, (double)jj.y));
+                    } else {
+                        jr[rec] = jj;
+                    }
                     if (need) {
                         real2 h[3];
 #pragma unroll
@@ -593,7 +639,8 @@ lin_obs_kernel(PipeArgs a_in) {
     if (exclusive) {       // this CTA wrote every record of the window: complete the landmarks here
         const double mu = pipe_mu(a, w);
         const int compute_scale = a.loop ? (a.ctrl[w].have_scale == 0) : a.compute_scale;
-        for (int l = tid; l < ((M + 3) & ~3); l += kThreads) lm_finish<real>(a, w, l, N, M, fixed, mu, compute_scale);
+        for (int l = tid; l < ((M + 3) & ~3); l += kThreads)
+            lm_finish<real>(a, w, l, N, M, fixed, mu, compute_scale, lpart ? part : nullptr, kWarps, Mp);
     }
     // direct part of the reduced system (schur_kernel subtracts the Schur sum from Hred / gred).  D(t, a) enters the
     // off-diagonal block (t, a) with a minus sign and BOTH diagonal blocks with a plus sign; its gradient part enters

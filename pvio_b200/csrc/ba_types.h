@@ -4,6 +4,7 @@
 // residual must be evaluated in fp64 to meet the 1e-5 relative tolerance on dx.
 #pragma once
 #include <stdint.h>
+#include <vector_types.h>
 
 namespace pvio {
 
@@ -43,8 +44,10 @@ PVIO_HD int32_t lm_meta(int anchor, int victim, int n_obs, unsigned mask) {
 // Frame-major observation table (built on the device from the landmark-major one, ba_fobs.cuh): the residual
 // blocks sorted by (target frame t, anchor frame a, landmark), segment sp = t (t - 1) / 2 + a.  A warp of the
 // linearise / update sweeps works on 32 consecutive entries of ONE segment ("row"), so the target frame is
-// warp-uniform (held in registers) and the per-(t, a) direct blocks are plain register sums.
-struct __align__(16) FObs { float zx, zy; int32_t lm, pad; };     // keypoint in the target frame, packed landmark index
+// warp-uniform (held in registers) and the per-(t, a) direct blocks are plain register sums.  Stored as two arrays of
+// the same index: fz (keypoint in the target frame, 8 B) and flm (packed landmark index, 2 B: Mcap <= 65536), 10 B
+// per residual block.
+typedef uint16_t FLm;
 
 // per-landmark sums of the linearise sweep (H_ll, g_l), formed by the Schur kernel
 struct LmSum { double hll, gl; };
@@ -119,7 +122,8 @@ struct BatchArrays {
     double *lm_scale;               // [W][Mcap] Jacobi scale of each inverse depth (fixed at iteration 0)
     LmAux *lm_aux;                  // 2x [W][Mcap] H_ll + reg, g_l, H_ll of every landmark (lm_finish -> update sweep)
     void *hs;                       // 2x [W][Ncap][Mcap][6] real: UNSCALED h_lt = Y^T j of every (landmark, target)
-    FObs *fobs;                     // [W][Kcap] frame-major table (ba_fobs.cuh)
+    float2 *fz;                     // [W][Kcap] frame-major table (ba_fobs.cuh): keypoint of each residual block
+    FLm *flm;                       // [W][Kcap]   and its landmark
     int32_t *seg;                   // [W][kSegTab]: seg_begin[sp], then seg_row[sp] (rows of 32 before segment sp)
     double *dx_pose;                // [W][Ncap][15] pose/motion step in delta coordinates
     double *rho_cand;               // [W][Mcap] candidate
@@ -135,8 +139,10 @@ struct BatchArrays {
     LinBufs bufs;
     void *lm_w;                     // 2x [W][Mcap][2] real: w_l = 1 / (H_ll + reg), w_l g_l (lm_finish -> Schur kernel)
     int32_t *lm_msk;                // 2x [W][Mcap] frames of the landmark (targets | anchor), 0: not eliminated
-    void *jr;                       // 2x [W][Ncap][Mcap][2] real: (j.j, j.r) of every (landmark, target) residual block; the
-                                    //    Schur kernel sums them per landmark in frame order (deterministic, no atomics)
+    void *jr;                       // 2x [W][Ncap][Mcap][2] real: (j.j, j.r) of every (landmark, target) residual block;
+                                    //    lm_finish sums them per landmark in frame order (deterministic, no atomics).  Only
+                                    //    written when several CTAs share a window or the shared-memory sums do not fit
+                                    //    (PipeArgs::lm_part)
     double *Hred;                   // 2x [W][npairs_cap][36] block-lower-triangular reduced system (xi coords)
     double *Hdd;                    // 2x [W][Ncap][36] direct (pre-Schur) diagonal blocks
     double *gdir;                   // 2x [W][Ncap][6] direct gradient

@@ -33,7 +33,7 @@ __host__ __device__ inline size_t upd_smem_layout(int N, int Mp, int warps, size
     *o_red = off; off += sizeof(double) * 8;
     *o_seg = off; off += sizeof(int32_t) * kSegTab;
     off = (off + 15) & ~(size_t)15;
-    *o_ring = off; off += sizeof(FObs) * kRing * 32 * (size_t)warps;
+    *o_ring = off; off += sizeof(RowSlot) * kRing * (size_t)warps;
     return off;
 }
 template <typename real>
@@ -251,16 +251,17 @@ update_obs_kernel(UpdArgs a) {
         const real W[4] = {(real)wc.sic[0], (real)wc.sic[1], (real)wc.sic[2], (real)wc.sic[3]};
         const real cb = (real)(wc.cauchy_a * wc.cauchy_a), inv_cb = (real)(1.0 / (wc.cauchy_a * wc.cauchy_a));
         const bool diag_w = wc.sic[1] == 0.0 && wc.sic[2] == 0.0;
-        const FObs *fobs = a.fobs + (size_t)w * a.Kcap;
+        const float2 *fz = a.fz + (size_t)w * a.Kcap;
+        const FLm *flm = a.flm + (size_t)w * a.Kcap;
         const int32_t *sbeg = sg, *srow = sg + kMaxSeg + 1;
         const int rows = srow[nsp];
         const int nwt = gridDim.x * kWarps, wid = blockIdx.x * kWarps + wv;
         const int r_begin = (int)((long long)rows * wid / nwt), r_end = (int)((long long)rows * (wid + 1) / nwt);
-        // rows through the per-warp cp.async ring, as in lin_obs_kernel
-        FObs *ring = reinterpret_cast<FObs *>(smem_raw + o_ring) + (size_t)wv * kRing * 32;
+        // rows through a per-warp cp.async ring of kRing rows
+        RowSlot *ring = reinterpret_cast<RowSlot *>(smem_raw + o_ring) + (size_t)wv * kRing;
         RowCursor pf(sbeg, srow, r_begin, rows), cs(sbeg, srow, r_begin, rows);
 #pragma unroll
-        for (int d = 0; d < kRing; ++d) row_prefetch(pf, r_end, fobs, ring + d * 32, lane);
+        for (int d = 0; d < kRing; ++d) row_prefetch(pf, r_end, fz, flm, ring + d, lane);
         int slot = 0;
         while (cs.r < r_end) {
             const int sp = cs.sp, t = cs.t;
@@ -276,13 +277,14 @@ update_obs_kernel(UpdArgs a) {
             for (; cs.r < r_stop; cs.advance()) {
                 const int k = cs.k0() + lane;
                 asm volatile("cp.async.wait_group %0;" :: "n"(kRing - 1) : "memory");
-                const FObs o = ring[slot * 32 + lane];
-                row_prefetch(pf, r_end, fobs, ring + slot * 32, lane);
+                __syncwarp();                     // the index granules of the row were copied by lanes 0-4
+                const float2 z = ring[slot].z[lane];
+                const int l = row_lm(ring[slot], lane);     // stale past the segment's end, and unused there
+                __syncwarp();                     // every lane has read the slot before it is refilled
+                row_prefetch(pf, r_end, fz, flm, ring + slot, lane);
                 slot = slot + 1 == kRing ? 0 : slot + 1;
-                if (k < seg_end) {
-                    const int l = o.lm;
-                    la.add(residual_cost_blk<real>(Rwc, c, xs[l], xs[Mp + l], xs[2 * Mp + l], o.zx, o.zy, W, diag_w, inv_cb));
-                }
+                if (k < seg_end)
+                    la.add(residual_cost_blk<real>(Rwc, c, xs[l], xs[Mp + l], xs[2 * Mp + l], z.x, z.y, W, diag_w, inv_cb));
                 if ((++nfold & 3) == 0) la.fold();
             }
             s_cost += (double)((real)0.5 * cb * la.total());
