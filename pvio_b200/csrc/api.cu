@@ -25,26 +25,6 @@ int fail(Handle *h, int code, const char *what, cudaError_t e) {
     return code;
 }
 
-template <typename T>
-static int alloc(Handle *h, DevBuf<T> &b, size_t n, bool pinned) {
-    b.n = n;
-    if (n == 0) return 0;
-    CK(h, cudaMalloc(&b.d, n * sizeof(T)));
-    CK(h, cudaMemset(b.d, 0, n * sizeof(T)));
-    if (pinned) {
-        CK(h, cudaMallocHost(&b.h, n * sizeof(T)));
-        memset(b.h, 0, n * sizeof(T));
-    }
-    return 0;
-}
-
-template <typename T>
-static void release(DevBuf<T> &b) {
-    if (b.d) cudaFree(b.d);
-    if (b.h) cudaFreeHost(b.h);
-    b.d = nullptr; b.h = nullptr; b.n = 0;
-}
-
 void drop_graphs(Handle *h) {
     for (auto &kv : h->graphs) cudaGraphExecDestroy(kv.second.first);
     h->graphs.clear();
@@ -59,14 +39,23 @@ static LinBufs lin_bufs(Handle *h) {
     return b;
 }
 
+// pinned staging: slot j of src -> slot i of dst (a slot of the shorter stride; the arrays may differ in stride only)
+template <typename T>
+static void copy_slot(DevBuf<T> &dst, size_t i, const DevBuf<T> &src, size_t j) {
+    memcpy(dst.slot(i), src.slot(j), sizeof(T) * std::min(dst.per, src.per));
+}
+
 // The handle's arrays as the kernels see them (BatchArrays).  Called after every (re)allocation, which also drops the
 // cached graphs: their launches carry the old view.
 static void refresh_arrays(Handle *h) {
     BatchArrays &a = h->arrays;
+    const size_t W = h->W, N = h->Ncap, npc = N * (N + 1) / 2;
     a.hdr = h->hdr.d; a.cst = h->cst.d; a.obs = h->obs.d; a.fz = h->fz.d; a.flm = h->flm.d; a.seg = h->seg.d; a.lms = h->lms.d;
     a.rho = h->rho.d; a.frames = h->frames.d; a.ctrl = h->ctrl.d; a.rho_cand = h->rho_cand.d; a.frames_cand = h->frames_cand.d;
     a.lm_scale = h->lm_scale.d; a.lm_aux = h->lm_aux.d; a.lm_w = h->lm_w.d; a.lm_msk = h->lm_msk.d; a.jr = h->jr.d; a.hs = h->hs.d;
-    a.Hred = h->Hred.d; a.Hdd = h->Hdd.d; a.gdir = h->gdir.d; a.gred = h->gred.d; a.cost_vis = h->cost_vis.d;
+    // the reduced-system outputs of set 0 lie back to back in Hred, set 1 sys_set elements behind them (LinBufs)
+    a.Hred = h->Hred.d; a.Hdd = a.Hred + W * npc * 36; a.gdir = a.Hdd + W * N * 36; a.gred = a.gdir + W * N * 6;
+    a.cost_vis = a.gred + W * N * 6;
     a.dx_pose = h->dx_pose.d; a.dx_lm = h->dx_lm.d; a.v_pose = h->v_pose.d; a.lm_v = h->lm_v.d; a.pose_scale = h->pose_scale.d;
     a.acc = h->acc.d; a.aux_cost = h->aux_cost.d;
     a.imu_idx = h->imu_idx.d; a.imu_data = h->imu_data.d; a.prior_frames = h->prior_frames.d; a.prior_S = h->prior_S.d;
@@ -79,21 +68,20 @@ static void refresh_arrays(Handle *h) {
 
 static int ensure_inertial(Handle *h) {
     if (h->have_inertial) return 0;
-    const size_t W = h->W, N = h->Ncap, dcap = 15 * N;
+    const size_t W = h->W, N = h->Ncap, M = h->Mcap, dcap = 15 * N;
     cudaStreamSynchronize(h->stream);
     drop_graphs(h);                                 // the record array is reallocated below: pointers in cached graphs go stale
-    TRY(alloc(h, h->imu_idx, W * N * 2, true));
-    TRY(alloc(h, h->imu_data, W * N * kImuStride, true));
-    TRY(alloc(h, h->prior_frames, W * N, true));
-    TRY(alloc(h, h->prior_S, W * dcap * dcap, true));
-    TRY(alloc(h, h->prior_L, W * dcap * dcap, false));
-    TRY(alloc(h, h->prior_e, W * dcap, true));
-    TRY(alloc(h, h->prior_x0, W * N * kFrameStride, true));
-    // windows with motion states run the fp64 pipeline: h records of 8-byte elements
-    release(h->hs); release(h->jr); release(h->lm_w);
-    TRY(alloc(h, h->hs, 2 * W * N * (size_t)h->Mcap * 6 * sizeof(double), false));      // two buffer sets (LinBufs)
-    TRY(alloc(h, h->jr, 2 * W * N * (size_t)h->Mcap * 2 * sizeof(double), false));
-    TRY(alloc(h, h->lm_w, 2 * W * (size_t)h->Mcap * 2 * sizeof(double), false));
+    TRY(alloc(h, h->imu_idx, W * N * 2, kBoth, N * 2));
+    TRY(alloc(h, h->imu_data, W * N * kImuStride, kBoth, N * kImuStride));
+    TRY(alloc(h, h->prior_frames, W * N, kBoth, N));
+    TRY(alloc(h, h->prior_S, W * dcap * dcap, kBoth, dcap * dcap));
+    TRY(alloc(h, h->prior_L, W * dcap * dcap, kDevice, dcap * dcap));
+    TRY(alloc(h, h->prior_e, W * dcap, kBoth, dcap));
+    TRY(alloc(h, h->prior_x0, W * N * kFrameStride, kBoth, N * kFrameStride));
+    // windows with motion states run the fp64 pipeline: h records of 8-byte elements, two buffer sets (LinBufs)
+    TRY(alloc(h, h->hs, 2 * W * N * M * 6 * sizeof(double), kDevice));
+    TRY(alloc(h, h->jr, 2 * W * N * M * 2 * sizeof(double), kDevice));
+    TRY(alloc(h, h->lm_w, 2 * W * M * 2 * sizeof(double), kDevice));
     h->hs_double = true;
     h->have_inertial = true;
     refresh_arrays(h);
@@ -108,24 +96,22 @@ static int ensure_planes(Handle *h, int T, int O) {
     const size_t W = h->W;
     cudaStreamSynchronize(h->stream);
     drop_graphs(h);
+    const size_t P4 = (size_t)h->Pcap * 4;
     DevBuf<double> pp; DevBuf<int32_t> tp, tb, tf; DevBuf<float> tz;
-    TRY(alloc(h, pp, W * h->Pcap * 4, true));
-    TRY(alloc(h, tp, W * Tn, true));
-    TRY(alloc(h, tb, W * (Tn + 1), true));
-    TRY(alloc(h, tf, W * On, true));
-    TRY(alloc(h, tz, W * On * 2, true));
+    TRY(alloc(h, pp, W * P4, kBoth, P4));
+    TRY(alloc(h, tp, W * Tn, kBoth, Tn));
+    TRY(alloc(h, tb, W * (Tn + 1), kBoth, Tn + 1));
+    TRY(alloc(h, tf, W * On, kBoth, On));
+    TRY(alloc(h, tz, W * On * 2, kBoth, On * 2));
     if (h->have_planes) {
-        memcpy(pp.h, h->plane_param.h, sizeof(double) * W * h->Pcap * 4);
         for (size_t i = 0; i < W; ++i) {
-            memcpy(tp.h + i * Tn, h->pt_plane.h + i * h->Tcap, sizeof(int32_t) * h->Tcap);
-            memcpy(tb.h + i * (Tn + 1), h->pt_begin.h + i * (h->Tcap + 1), sizeof(int32_t) * (h->Tcap + 1));
-            memcpy(tf.h + i * On, h->pt_frame.h + i * h->Ocap, sizeof(int32_t) * h->Ocap);
-            memcpy(tz.h + i * On * 2, h->pt_z.h + i * h->Ocap * 2, sizeof(float) * h->Ocap * 2);
+            copy_slot(pp, i, h->plane_param, i); copy_slot(tp, i, h->pt_plane, i); copy_slot(tb, i, h->pt_begin, i);
+            copy_slot(tf, i, h->pt_frame, i); copy_slot(tz, i, h->pt_z, i);
         }
     }
-    release(h->plane_param); release(h->pt_plane); release(h->pt_begin); release(h->pt_frame); release(h->pt_z); release(h->pt_J);
-    h->plane_param = pp; h->pt_plane = tp; h->pt_begin = tb; h->pt_frame = tf; h->pt_z = tz;
-    TRY(alloc(h, h->pt_J, W * Tn * (6 * (size_t)h->Ncap + 2), false));      // device scratch of solve_kernel's plane block
+    h->plane_param = std::move(pp); h->pt_plane = std::move(tp); h->pt_begin = std::move(tb); h->pt_frame = std::move(tf);
+    h->pt_z = std::move(tz);
+    TRY(alloc(h, h->pt_J, W * Tn * (6 * (size_t)h->Ncap + 2), kDevice));      // device scratch of solve_kernel's plane block
     h->Tcap = Tn; h->Ocap = On;
     h->have_planes = true;
     refresh_arrays(h);
@@ -262,7 +248,7 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     memcpy(C.sic, w->sqrt_inv_cov, 32);
     C.fx = w->fx; C.fy = w->fy; C.cauchy_a = w->cauchy_a > 0 ? w->cauchy_a : 1.0; C.plane_sic = w->plane_sqrt_inv_cov;
     // frames + origin (mean frame position keeps |x_l| ~ depth in the fp32 Jacobian arithmetic)
-    double *fr = h->frames.h + (size_t)slot * h->Ncap * kFrameStride;
+    double *fr = h->frames.slot(slot);
     memcpy(fr, s->frames, sizeof(double) * N * kFrameStride);
     double o[3] = {0, 0, 0};
     for (int f = 0; f < N; ++f) for (int k = 0; k < 3; ++k) o[k] += fr[f * kFrameStride + 4 + k];
@@ -278,9 +264,9 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
         if (l > 0 && a < w->lm_anchor[l - 1]) sorted = false;
     }
     if (!sorted) std::stable_sort(perm.begin(), perm.end(), [&](int a, int b) { return w->lm_anchor[a] < w->lm_anchor[b]; });
-    ObsRec *ob = h->obs.h + (size_t)slot * h->Kcap;
-    LmRec *lm = h->lms.h + (size_t)slot * h->Mcap;
-    double *rh = h->rho.h + (size_t)slot * h->Mcap;
+    ObsRec *ob = h->obs.slot(slot);
+    LmRec *lm = h->lms.slot(slot);
+    double *rh = h->rho.slot(slot);
     int k_out = 0, nch = 0;
     for (int lp = 0; lp < M; ++lp) {
         const int l = perm[lp];
@@ -326,16 +312,16 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     H.n_imu = n_imu;
     H.n_prior = n_prior;
     if (n_imu > 0 || n_prior > 0) {
-        int32_t *ii = h->imu_idx.h + (size_t)slot * h->Ncap * 2;
+        int32_t *ii = h->imu_idx.slot(slot);
         for (int n = 0; n < n_imu; ++n) { ii[2 * n] = w->imu_frame_i[n]; ii[2 * n + 1] = w->imu_frame_j[n]; }
-        if (n_imu > 0) memcpy(h->imu_data.h + (size_t)slot * h->Ncap * kImuStride, w->imu_data, sizeof(double) * n_imu * kImuStride);
-        const size_t dcap = 15 * (size_t)h->Ncap, d = 15 * (size_t)n_prior;
-        for (int n = 0; n < n_prior; ++n) h->prior_frames.h[(size_t)slot * h->Ncap + n] = w->prior_frames[n];
+        if (n_imu > 0) memcpy(h->imu_data.slot(slot), w->imu_data, sizeof(double) * n_imu * kImuStride);
+        const size_t d = 15 * (size_t)n_prior;
+        for (int n = 0; n < n_prior; ++n) h->prior_frames.slot(slot)[n] = w->prior_frames[n];
         if (d > 0 && w->prior_S) {          // a host prior replaces a device-resident one
             h->prior_resident[slot] = 0;
-            memcpy(h->prior_S.h + (size_t)slot * dcap * dcap, w->prior_S, sizeof(double) * d * d);   // dense d x d, row-major
-            memcpy(h->prior_e.h + (size_t)slot * dcap, w->prior_e, sizeof(double) * d);
-            memcpy(h->prior_x0.h + (size_t)slot * h->Ncap * kFrameStride, w->prior_state0, sizeof(double) * n_prior * kFrameStride);
+            memcpy(h->prior_S.slot(slot), w->prior_S, sizeof(double) * d * d);   // dense d x d, row-major
+            memcpy(h->prior_e.slot(slot), w->prior_e, sizeof(double) * d);
+            memcpy(h->prior_x0.slot(slot), w->prior_state0, sizeof(double) * n_prior * kFrameStride);
         }
     }
     // planes
@@ -343,20 +329,21 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     if (H.n_ptracks > 0) {
         const int O = w->pt_obs_begin[H.n_ptracks];
         TRY(ensure_planes(h, H.n_ptracks, O));
-        memcpy(h->plane_param.h + (size_t)slot * h->Pcap * 4, w->plane_param, sizeof(double) * 4 * H.n_planes);
-        memcpy(h->pt_plane.h + (size_t)slot * h->Tcap, w->pt_plane, sizeof(int32_t) * H.n_ptracks);
-        memcpy(h->pt_begin.h + (size_t)slot * (h->Tcap + 1), w->pt_obs_begin, sizeof(int32_t) * (H.n_ptracks + 1));
-        memcpy(h->pt_frame.h + (size_t)slot * h->Ocap, w->pt_obs_frame, sizeof(int32_t) * O);
-        float *z = h->pt_z.h + (size_t)slot * h->Ocap * 2;
+        memcpy(h->plane_param.slot(slot), w->plane_param, sizeof(double) * 4 * H.n_planes);
+        memcpy(h->pt_plane.slot(slot), w->pt_plane, sizeof(int32_t) * H.n_ptracks);
+        memcpy(h->pt_begin.slot(slot), w->pt_obs_begin, sizeof(int32_t) * (H.n_ptracks + 1));
+        memcpy(h->pt_frame.slot(slot), w->pt_obs_frame, sizeof(int32_t) * O);
+        float *z = h->pt_z.slot(slot);
         for (int i = 0; i < 2 * O; ++i) z[i] = (float)w->pt_obs_z[i];
     }
     return 0;
 }
 
+// pinned staging -> device of window slots [w0, w0 + n)
 template <typename T>
-static int h2d(Handle *h, DevBuf<T> &b, size_t per, int w0, int n, cudaStream_t st) {
-    if (!b.d || !b.h || per == 0) return 0;
-    CK(h, cudaMemcpyAsync(b.d + per * w0, b.h + per * w0, per * n * sizeof(T), cudaMemcpyHostToDevice, st));
+static int h2d(Handle *h, DevBuf<T> &b, int w0, int n, cudaStream_t st) {
+    if (!b.d || !b.h || b.per == 0) return 0;
+    CK(h, cudaMemcpyAsync(b.dslot(w0), b.slot(w0), b.per * n * sizeof(T), cudaMemcpyHostToDevice, st));
     return 0;
 }
 
@@ -364,26 +351,24 @@ static int h2d(Handle *h, DevBuf<T> &b, size_t per, int w0, int n, cudaStream_t 
 // across the iterations of a solve: the frame-major table and Lambda = S^T S of the priors.
 static int upload_range(Handle *h, int w0, int n, cudaStream_t st) {
     if (n < 1 || w0 < 0 || w0 + n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window range");
-    const size_t N = h->Ncap;
-    TRY(h2d(h, h->hdr, 1, w0, n, st));
-    TRY(h2d(h, h->cst, 1, w0, n, st));
-    TRY(h2d(h, h->obs, h->Kcap, w0, n, st));
-    TRY(h2d(h, h->lms, h->Mcap, w0, n, st));
-    TRY(h2d(h, h->rho, h->Mcap, w0, n, st));
-    TRY(h2d(h, h->frames, N * kFrameStride, w0, n, st));
+    TRY(h2d(h, h->hdr, w0, n, st));
+    TRY(h2d(h, h->cst, w0, n, st));
+    TRY(h2d(h, h->obs, w0, n, st));
+    TRY(h2d(h, h->lms, w0, n, st));
+    TRY(h2d(h, h->rho, w0, n, st));
+    TRY(h2d(h, h->frames, w0, n, st));
     bool any_prior = false;
     if (h->have_inertial) {
-        const size_t dcap = 15 * N;
-        TRY(h2d(h, h->imu_idx, N * 2, w0, n, st));
-        TRY(h2d(h, h->imu_data, N * kImuStride, w0, n, st));
-        TRY(h2d(h, h->prior_frames, N, w0, n, st));
+        TRY(h2d(h, h->imu_idx, w0, n, st));
+        TRY(h2d(h, h->imu_data, w0, n, st));
+        TRY(h2d(h, h->prior_frames, w0, n, st));
         for (int i = w0; i < w0 + n;) {      // a device-resident prior is never re-uploaded: copy the runs of the other slots
             if (h->prior_resident[i]) { ++i; continue; }
             int j = i;
             while (j < w0 + n && !h->prior_resident[j]) ++j;
-            TRY(h2d(h, h->prior_S, dcap * dcap, i, j - i, st));
-            TRY(h2d(h, h->prior_e, dcap, i, j - i, st));
-            TRY(h2d(h, h->prior_x0, N * kFrameStride, i, j - i, st));
+            TRY(h2d(h, h->prior_S, i, j - i, st));
+            TRY(h2d(h, h->prior_e, i, j - i, st));
+            TRY(h2d(h, h->prior_x0, i, j - i, st));
             i = j;
         }
         for (int i = w0; i < w0 + n; ++i) any_prior |= h->hdr.h[i].n_prior > 0;
@@ -393,11 +378,11 @@ static int upload_range(Handle *h, int w0, int n, cudaStream_t st) {
         }
     }
     if (h->have_planes) {
-        TRY(h2d(h, h->plane_param, (size_t)h->Pcap * 4, w0, n, st));
-        TRY(h2d(h, h->pt_plane, h->Tcap, w0, n, st));
-        TRY(h2d(h, h->pt_begin, h->Tcap + 1, w0, n, st));
-        TRY(h2d(h, h->pt_frame, h->Ocap, w0, n, st));
-        TRY(h2d(h, h->pt_z, (size_t)h->Ocap * 2, w0, n, st));
+        TRY(h2d(h, h->plane_param, w0, n, st));
+        TRY(h2d(h, h->pt_plane, w0, n, st));
+        TRY(h2d(h, h->pt_begin, w0, n, st));
+        TRY(h2d(h, h->pt_frame, w0, n, st));
+        TRY(h2d(h, h->pt_z, w0, n, st));
     }
     FobsArgs fa = launch_args<FobsArgs>(h);
     fa.w0 = w0;
@@ -788,8 +773,8 @@ static int scatter_dx(Handle *h, int w0, int n, double *dx, int64_t dx_stride, d
         const int N = h->slot_N[i], M = h->slot_M[i];
         if (dx) {
             double *o = dx + (size_t)i * dx_stride;
-            memcpy(o, h->dx_pose.h + (size_t)i * h->Ncap * 15, sizeof(double) * N * 15);
-            const double *dl = h->dx_lm.h + (size_t)i * h->Mcap;
+            memcpy(o, h->dx_pose.slot(i), sizeof(double) * N * 15);
+            const double *dl = h->dx_lm.slot(i);
             if (h->perm_identity[i]) memcpy(o + N * 15, dl, sizeof(double) * M);
             else { const std::vector<int32_t> &perm = h->perm[i]; for (int lp = 0; lp < M; ++lp) o[N * 15 + perm[lp]] = dl[lp]; }
         }
@@ -799,14 +784,18 @@ static int scatter_dx(Handle *h, int w0, int n, double *dx, int64_t dx_stride, d
     return 0;
 }
 
+// device array src -> pinned array dst (same slot stride) of window slots [w0, w0 + n) on stream st (async)
+template <typename T>
+static int d2h(Handle *h, DevBuf<T> &dst, const DevBuf<T> &src, int w0, int n, cudaStream_t st) {
+    CK(h, cudaMemcpyAsync(dst.slot(w0), src.dslot(w0), sizeof(T) * src.per * n, cudaMemcpyDeviceToHost, st));
+    return 0;
+}
+
 // device -> host of the steps + summaries of windows [w0, w0 + n) on stream st (async)
 static int download_dx_async(Handle *h, int w0, int n, cudaStream_t st) {
-    const size_t P = (size_t)h->Ncap * 15;
-    CK(h, cudaMemcpyAsync(h->dx_pose.h + w0 * P, h->dx_pose.d + w0 * P, sizeof(double) * P * n, cudaMemcpyDeviceToHost, st));
-    CK(h, cudaMemcpyAsync(h->dx_lm.h + (size_t)w0 * h->Mcap, h->dx_lm.d + (size_t)w0 * h->Mcap, sizeof(double) * h->Mcap * n,
-                          cudaMemcpyDeviceToHost, st));
-    CK(h, cudaMemcpyAsync(h->ctrl.h + w0, h->ctrl.d + w0, sizeof(WinCtrl) * n, cudaMemcpyDeviceToHost, st));
-    return 0;
+    TRY(d2h(h, h->dx_pose, h->dx_pose, w0, n, st));
+    TRY(d2h(h, h->dx_lm, h->dx_lm, w0, n, st));
+    return d2h(h, h->ctrl, h->ctrl, w0, n, st);
 }
 
 static int download_dx(Handle *h, int n, double *dx, int64_t dx_stride, double *costs) {
@@ -818,13 +807,9 @@ static int download_dx(Handle *h, int n, double *dx, int64_t dx_stride, double *
 
 // device -> host of the solved state + summaries of windows [w0, w0 + n) on stream st (async)
 static int download_state_async(Handle *h, int w0, int n, cudaStream_t st) {
-    const size_t N = h->Ncap;
-    CK(h, cudaMemcpyAsync(h->frames_out.h + (size_t)w0 * N * kFrameStride, h->frames.d + (size_t)w0 * N * kFrameStride,
-                          sizeof(double) * N * kFrameStride * n, cudaMemcpyDeviceToHost, st));
-    CK(h, cudaMemcpyAsync(h->rho_out.h + (size_t)w0 * h->Mcap, h->rho.d + (size_t)w0 * h->Mcap, sizeof(double) * h->Mcap * n,
-                          cudaMemcpyDeviceToHost, st));
-    CK(h, cudaMemcpyAsync(h->ctrl.h + w0, h->ctrl.d + w0, sizeof(WinCtrl) * n, cudaMemcpyDeviceToHost, st));
-    return 0;
+    TRY(d2h(h, h->frames_out, h->frames, w0, n, st));
+    TRY(d2h(h, h->rho_out, h->rho, w0, n, st));
+    return d2h(h, h->ctrl, h->ctrl, w0, n, st);
 }
 
 static void fill_summary(const WinCtrl &c, pvio_b200_summary *sm) {
@@ -835,9 +820,9 @@ static void fill_summary(const WinCtrl &c, pvio_b200_summary *sm) {
 
 static void scatter_state(Handle *h, int i, double *frames, double *inv_depth) {
     const int N = h->slot_N[i], M = h->slot_M[i];
-    if (frames) memcpy(frames, h->frames_out.h + (size_t)i * h->Ncap * kFrameStride, sizeof(double) * N * kFrameStride);
+    if (frames) memcpy(frames, h->frames_out.slot(i), sizeof(double) * N * kFrameStride);
     if (inv_depth) {
-        const double *r = h->rho_out.h + (size_t)i * h->Mcap;
+        const double *r = h->rho_out.slot(i);
         const std::vector<int32_t> &perm = h->perm[i];
         if (h->perm_identity[i]) memcpy(inv_depth, r, sizeof(double) * M);
         else for (int lp = 0; lp < M; ++lp) inv_depth[perm[lp]] = r[lp];
@@ -966,37 +951,29 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
     CK(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     CK(h, cudaEventCreate(&h->ev0)); CK(h, cudaEventCreate(&h->ev1));
     const size_t W = h->W, N = h->Ncap, M = h->Mcap, K = h->Kcap, npc = N * (N + 1) / 2;
-    TRY(alloc(h, h->hdr, W, true)); TRY(alloc(h, h->cst, W, true));
-    TRY(alloc(h, h->obs, W * K, true)); TRY(alloc(h, h->lms, W * M, true));
+    const size_t X = N * kFrameStride;                        // doubles per window of the frame states
+    TRY(alloc(h, h->hdr, W, kBoth, 1)); TRY(alloc(h, h->cst, W, kBoth, 1));
+    TRY(alloc(h, h->obs, W * K, kBoth, K)); TRY(alloc(h, h->lms, W * M, kBoth, M));
     // flm is padded: the update sweep copies five 16-byte granules from the one holding a row's first index (row_prefetch)
-    TRY(alloc(h, h->fz, W * K, false)); TRY(alloc(h, h->flm, W * K + kFlmPad, false));
-    TRY(alloc(h, h->seg, W * kSegTab, false));
-    TRY(alloc(h, h->rho, W * M, true)); TRY(alloc(h, h->frames, W * N * kFrameStride, true));
-    TRY(alloc(h, h->ctrl, W, true));
-    TRY(alloc(h, h->rho_cand, W * M, false)); TRY(alloc(h, h->frames_cand, W * N * kFrameStride, false));
+    TRY(alloc(h, h->fz, W * K, kDevice)); TRY(alloc(h, h->flm, W * K + kFlmPad, kDevice));
+    TRY(alloc(h, h->seg, W * kSegTab, kDevice));
+    TRY(alloc(h, h->rho, W * M, kBoth, M)); TRY(alloc(h, h->frames, W * X, kBoth, X));
+    TRY(alloc(h, h->ctrl, W, kBoth, 1));
+    TRY(alloc(h, h->rho_cand, W * M, kDevice)); TRY(alloc(h, h->frames_cand, W * X, kDevice));
     // the linearisation lives in two buffer sets (LinBufs, ba_types.h): everything below up to the reduced system is doubled
-    TRY(alloc(h, h->lm_scale, W * M, false)); TRY(alloc(h, h->lm_aux, 2 * W * M, false));
-    TRY(alloc(h, h->hs, 2 * W * N * M * 6 * sizeof(float), false)); TRY(alloc(h, h->jr, 2 * W * N * M * 2 * sizeof(float), false));
-    TRY(alloc(h, h->lm_w, 2 * W * M * 2 * sizeof(float), false)); TRY(alloc(h, h->lm_msk, 2 * W * M, false));
-    {   // landing area of downloaded states: host only
-        CK(h, cudaMallocHost(&h->frames_out.h, sizeof(double) * W * N * kFrameStride));
-        CK(h, cudaMallocHost(&h->rho_out.h, sizeof(double) * W * M));
-    }
-    TRY(alloc(h, h->dx_lm, W * M, true)); TRY(alloc(h, h->lm_v, W * M, false)); TRY(alloc(h, h->dx_pose, W * N * 15, true));
-    TRY(alloc(h, h->pose_scale, W * N * 15, false)); TRY(alloc(h, h->v_pose, W * N * 15, false));
-    TRY(alloc(h, h->valid, W * M, true)); TRY(alloc(h, h->quality, W * M, true));
-    {   // the reduced-system outputs of the linearise kernel live in ONE allocation so that the
-        // multi-CTA-per-window mode (atomic accumulation) needs a single memset per launch
-        const size_t n_sys = W * (npc * 36 + N * 36 + N * 6 + N * 6 + 1);
-        TRY(alloc(h, h->Hred, 2 * n_sys, false));
-        h->Hdd.d = h->Hred.d + W * npc * 36; h->Hdd.n = 0;
-        h->gdir.d = h->Hdd.d + W * N * 36; h->gdir.n = 0;
-        h->gred.d = h->gdir.d + W * N * 6; h->gred.n = 0;
-        h->cost_vis.d = h->gred.d + W * N * 6; h->cost_vis.n = 0;
-        h->sys_set = n_sys;                                   // set 1 of each array lies n_sys elements behind set 0
-    }
-    TRY(alloc(h, h->acc, W * kAcc, true)); TRY(alloc(h, h->aux_cost, W, false));
-    TRY(alloc(h, h->Hfull, (15 * N) * (15 * N), true)); TRY(alloc(h, h->gfull, 15 * N, true));
+    TRY(alloc(h, h->lm_scale, W * M, kDevice)); TRY(alloc(h, h->lm_aux, 2 * W * M, kDevice));
+    TRY(alloc(h, h->hs, 2 * W * N * M * 6 * sizeof(float), kDevice)); TRY(alloc(h, h->jr, 2 * W * N * M * 2 * sizeof(float), kDevice));
+    TRY(alloc(h, h->lm_w, 2 * W * M * 2 * sizeof(float), kDevice)); TRY(alloc(h, h->lm_msk, 2 * W * M, kDevice));
+    TRY(alloc(h, h->frames_out, W * X, kPinned, X)); TRY(alloc(h, h->rho_out, W * M, kPinned, M));
+    TRY(alloc(h, h->dx_lm, W * M, kBoth, M)); TRY(alloc(h, h->lm_v, W * M, kDevice)); TRY(alloc(h, h->dx_pose, W * N * 15, kBoth, N * 15));
+    TRY(alloc(h, h->pose_scale, W * N * 15, kDevice)); TRY(alloc(h, h->v_pose, W * N * 15, kDevice));
+    TRY(alloc(h, h->valid, W * M, kBoth, M)); TRY(alloc(h, h->quality, W * M, kBoth, M));
+    // the reduced-system outputs of the linearise kernel (Hred, Hdd, gdir, gred, cost_vis: refresh_arrays) live in ONE
+    // allocation so that the multi-CTA-per-window mode (atomic accumulation) needs a single memset per launch
+    h->sys_set = W * (npc * 36 + N * 36 + N * 6 + N * 6 + 1);   // set 1 of each array lies sys_set elements behind set 0
+    TRY(alloc(h, h->Hred, 2 * h->sys_set, kDevice));
+    TRY(alloc(h, h->acc, W * kAcc, kBoth)); TRY(alloc(h, h->aux_cost, W, kDevice));
+    TRY(alloc(h, h->Hfull, (15 * N) * (15 * N), kBoth)); TRY(alloc(h, h->gfull, 15 * N, kBoth));
     refresh_arrays(h);
     h->perm.resize(W); h->perm_identity.assign(W, 1); h->slot_M.assign(W, 0); h->slot_N.assign(W, 0); h->slot_K.assign(W, 0);
     h->prior_resident.assign(W, 0);
@@ -1031,22 +1008,6 @@ void pvio_b200_destroy(pvio_b200_handle hh) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
-    if (h->pnp_dev) cudaFree(h->pnp_dev);
-    if (h->pnp_host) cudaFreeHost(h->pnp_host);
-    klt_free(h);
-    marg_free(h);
-    resident_free(h);
-    detect_free(h);
-    fm_free(h);
-    release(h->hdr); release(h->cst); release(h->obs); release(h->lms); release(h->rho); release(h->frames);
-    release(h->fz); release(h->flm); release(h->seg); release(h->jr); release(h->lm_w); release(h->lm_msk); release(h->frames_out); release(h->rho_out); release(h->lm_v); release(h->valid); release(h->quality);
-    release(h->ctrl); release(h->rho_cand); release(h->frames_cand); release(h->lm_scale); release(h->lm_aux); release(h->hs);
-    release(h->dx_lm); release(h->dx_pose); release(h->pose_scale); release(h->v_pose); release(h->Hred);
-    release(h->acc); release(h->aux_cost);
-    release(h->Hfull); release(h->gfull);
-    release(h->imu_idx); release(h->imu_data); release(h->prior_frames); release(h->prior_S); release(h->prior_L);
-    release(h->prior_e); release(h->prior_x0);
-    release(h->pt_J); release(h->plane_param); release(h->pt_plane); release(h->pt_begin); release(h->pt_frame); release(h->pt_z);
     drop_graphs(h);
     for (auto &e : h->kev) cudaEventDestroy(e);
     cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1);
@@ -1059,7 +1020,7 @@ void pvio_b200_destroy(pvio_b200_handle hh) {
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->stream_aux) { cudaStreamDestroy(h->stream_aux); cudaEventDestroy(h->ev_aux_fork); cudaEventDestroy(h->ev_aux_join); }
     cudaStreamDestroy(h->stream);
-    delete h;
+    delete h;                        // frees every buffer (DevBuf)
 }
 
 const char *pvio_b200_last_error(pvio_b200_handle hh) {
@@ -1130,31 +1091,13 @@ int pvio_b200_batch_replicate(pvio_b200_handle hh, int n) {
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
     if (h->prior_resident[0] && h->hdr.h[0].n_prior > 0)
         return fail(h, PVIO_B200_EINVAL, "batch_replicate: slot 0's prior is device-resident, its staging does not hold it");
-    const size_t N = h->Ncap;
     for (int i = 1; i < n; ++i) {
+        auto rep = [&](auto &b) { copy_slot(b, i, b, 0); };
         h->prior_resident[i] = 0;          // the slot takes slot 0's host prior from the staging
-        h->hdr.h[i] = h->hdr.h[0]; h->cst.h[i] = h->cst.h[0];
-        memcpy(h->obs.h + (size_t)i * h->Kcap, h->obs.h, sizeof(ObsRec) * h->slot_K[0]);
-        memcpy(h->lms.h + (size_t)i * h->Mcap, h->lms.h, sizeof(LmRec) * h->slot_M[0]);
-        memcpy(h->rho.h + (size_t)i * h->Mcap, h->rho.h, sizeof(double) * h->slot_M[0]);
-        memcpy(h->frames.h + (size_t)i * N * kFrameStride, h->frames.h, sizeof(double) * N * kFrameStride);
+        rep(h->hdr); rep(h->cst); rep(h->obs); rep(h->lms); rep(h->rho); rep(h->frames);
         h->perm[i] = h->perm[0]; h->perm_identity[i] = h->perm_identity[0]; h->slot_M[i] = h->slot_M[0]; h->slot_N[i] = h->slot_N[0]; h->slot_K[i] = h->slot_K[0];
-        if (h->have_inertial) {
-            const size_t dcap = 15 * N;
-            memcpy(h->imu_idx.h + (size_t)i * N * 2, h->imu_idx.h, sizeof(int32_t) * N * 2);
-            memcpy(h->imu_data.h + (size_t)i * N * kImuStride, h->imu_data.h, sizeof(double) * N * kImuStride);
-            memcpy(h->prior_frames.h + (size_t)i * N, h->prior_frames.h, sizeof(int32_t) * N);
-            memcpy(h->prior_S.h + (size_t)i * dcap * dcap, h->prior_S.h, sizeof(double) * dcap * dcap);
-            memcpy(h->prior_e.h + (size_t)i * dcap, h->prior_e.h, sizeof(double) * dcap);
-            memcpy(h->prior_x0.h + (size_t)i * N * kFrameStride, h->prior_x0.h, sizeof(double) * N * kFrameStride);
-        }
-        if (h->have_planes) {
-            memcpy(h->plane_param.h + (size_t)i * h->Pcap * 4, h->plane_param.h, sizeof(double) * h->Pcap * 4);
-            memcpy(h->pt_plane.h + (size_t)i * h->Tcap, h->pt_plane.h, sizeof(int32_t) * h->Tcap);
-            memcpy(h->pt_begin.h + (size_t)i * (h->Tcap + 1), h->pt_begin.h, sizeof(int32_t) * (h->Tcap + 1));
-            memcpy(h->pt_frame.h + (size_t)i * h->Ocap, h->pt_frame.h, sizeof(int32_t) * h->Ocap);
-            memcpy(h->pt_z.h + (size_t)i * h->Ocap * 2, h->pt_z.h, sizeof(float) * h->Ocap * 2);
-        }
+        if (h->have_inertial) { rep(h->imu_idx); rep(h->imu_data); rep(h->prior_frames); rep(h->prior_S); rep(h->prior_e); rep(h->prior_x0); }
+        if (h->have_planes) { rep(h->plane_param); rep(h->pt_plane); rep(h->pt_begin); rep(h->pt_frame); rep(h->pt_z); }
     }
     return 0;
 }

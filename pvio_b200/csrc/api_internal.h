@@ -2,25 +2,112 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <array>
+#include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 #include "../../include/pvio_b200.h"
 #include "ba_types.h"
 
 namespace pvio {
 
+// Owner of one array in device memory, pinned host memory or both (the same element count on each side); move-only,
+// freed with its owner.  Allocated only by alloc / reserve (below), which also record its capacity and slot stride.
 template <typename T>
 struct DevBuf {
     T *d = nullptr;      // device
-    T *h = nullptr;      // pinned host staging (optional)
-    size_t n = 0;
+    T *h = nullptr;      // pinned host
+    size_t n = 0;        // capacity in elements: 0 until an allocation has fully succeeded
+    size_t per = 0;      // arrays indexed by window slot: elements per slot
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept : d(o.d), h(o.h), n(o.n), per(o.per) { o.d = o.h = nullptr; o.n = o.per = 0; }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        DevBuf t(std::move(o));
+        std::swap(d, t.d); std::swap(h, t.h); std::swap(n, t.n); std::swap(per, t.per);
+        return *this;
+    }
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() {
+        if (d) cudaFree(d);
+        if (h) cudaFreeHost(h);
+    }
+    T *slot(size_t i) const { return h + i * per; }      // pinned staging of window slot i
+    T *dslot(size_t i) const { return d + i * per; }     // device array of window slot i
+};
+enum MemSides { kDevice = 1, kPinned = 2, kBoth = 3 };
+
+// klt.cu: the two pyramids of the tracker and their staging.  Rebuilt (which drops the image cache) when the image
+// shape, the level count or the point capacity changes.
+constexpr int kMaxLevels = 8;
+struct KltState {
+    int w = 0, h = 0, levels = 0, cap_pts = 0;
+    DevBuf<uint8_t> pyr[2];                   // both pyramids, levels packed back to back
+    size_t off[kMaxLevels + 1] = {};
+    int lw[kMaxLevels] = {}, lh[kMaxLevels] = {};
+    DevBuf<float> pts;                        // [5][cap_pts] both sides: prev [2] | next [2] | err
+    DevBuf<uint8_t> status;                   // [cap_pts] both sides
+    DevBuf<uint8_t> raw[2];                   // pre-CLAHE level-0 images (raw entry point only)
+    DevBuf<uint8_t> lut;                      // [tiles][256] CLAHE look-up tables
+    DevBuf<uint8_t> img;                      // pinned staging for both level-0 images
+    // image cache: pyr[i] holds the finished pyramid of the frame with id pyr_id[i] (0: none) built with pyr_clahe[i];
+    // the tracker calls with prev = the previous call's next (feature_tracker.cpp:92), so half the uploads and
+    // pyramid builds of a steady-state call are skipped
+    uint64_t pyr_id[2] = {0, 0};
+    double pyr_clahe[2] = {0.0, 0.0};
 };
 
-struct KltState;         // klt.cu
-struct MargScratch;      // ba_marg.cu
-struct FmState;          // fmat.cu
+// detect.cu: per-image-shape buffers of the corner detector
+struct DetectState {
+    int w = 0, h = 0;
+    int cap = 0;                              // candidate capacity
+    size_t cub_bytes = 0;
+    DevBuf<uint8_t> img;                      // own copy of the image when the frame is not in the KLT cache; .h: its staging
+    DevBuf<uint8_t> raw, lut;
+    DevBuf<float> resp;
+    DevBuf<unsigned long long> keys;
+    DevBuf<unsigned long long> keys_sorted;   // both sides
+    DevBuf<int> counters;                     // both sides: [0] max response bits, [1] candidate count
+    DevBuf<uint8_t> cub_tmp;
+};
+
+// fmat.cu: RANSAC buffers, grown to the largest point count / iteration budget seen
+struct FmState {
+    DevBuf<float> pts;                        // [2][n][2] p then q, both sides
+    DevBuf<int> sched;                        // [s][7], both sides
+    DevBuf<int> counts;                       // [s][4] nmodels, count / median bits of each model, both sides
+    DevBuf<double> F;                         // [s][3][9]
+    DevBuf<unsigned> masks;                   // [s][3][words]
+    DevBuf<double> h_F;                       // pinned: the winning model
+    DevBuf<unsigned> h_mask;                  // pinned: its inlier mask
+};
+
+// resident.cu: the sliding window kept between keyframes
+struct ResTrack {
+    std::vector<int32_t> frames;      // window indices, increasing
+    std::vector<double> z;            // [2] per observation
+    double rho = 1.0;
+    bool alive = true;
+};
+
+struct ResidentWindow {
+    pvio_b200_window cst;             // constants (extrinsics, noise model, flags); the array members are rebuilt per call
+    std::vector<std::array<double, kFrameStride>> frames;
+    std::vector<uint8_t> fixed;
+    std::vector<std::array<double, kImuStride>> imu;      // factor k couples frames (k, k + 1)
+    std::vector<ResTrack> tracks;
+    int n_prior = 0;                  // the prior covers frames 0 .. n_prior - 1
+    bool prior_on_device = false;
+    std::vector<double> host_S, host_e, host_x0;          // a prior given by the caller (first window: the gauge prior)
+    // the view handed to pack_window
+    std::vector<int32_t> lm_anchor, lm_obs_begin, obs_frame, imu_i, imu_j, prior_frames, lm_track;
+    std::vector<double> lm_z_ref, obs_z, imu_data, st_frames, st_rho;
+    std::vector<uint8_t> lm_in_victim;
+};
 
 struct Handle {
     int device = 0;
@@ -38,8 +125,8 @@ struct Handle {
     int64_t launches = 0;
     std::vector<int> prior_resident;              // per slot: frame count of the prior (S, e, x0) the marginaliser wrote on the
                                                   // device (0: none); a pack naming it with prior_S == NULL keeps it, a host prior clears it
-    struct ResidentWindow *resident = nullptr;    // resident.cu
-    struct DetectState *detect = nullptr;         // detect.cu
+    std::unique_ptr<ResidentWindow> resident;     // resident.cu (null until pvio_b200_window_reset)
+    DetectState detect;                           // detect.cu
     size_t sys_set = 0;                           // elements between the two buffer sets of the reduced-system arrays (LinBufs)
     int sm_count = 132;                           // set from the device at create
     int smem_lim = 0;                             // dynamic shared memory the large-layout kernels opt in to (create)
@@ -64,7 +151,9 @@ struct Handle {
     DevBuf<int32_t> lm_msk;                      // [W][Mcap] frame mask of each landmark
     bool hs_double = false;
     DevBuf<double> frames_out, rho_out;          // pinned landing area of downloaded states (the upload staging stays intact)
-    DevBuf<double> Hred, Hdd, gdir, gred, cost_vis, acc, aux_cost;
+    DevBuf<double> Hred;                         // reduced-system outputs of the linearise sweep, Hdd, gdir, gred and
+                                                 // cost_vis included, both buffer sets (api.cu: refresh_arrays)
+    DevBuf<double> acc, aux_cost;
     DevBuf<double> Hfull, gfull;                 // debug dump (single window only)
     DevBuf<uint8_t> valid;                       // post-pass results
     DevBuf<double> quality;
@@ -93,12 +182,11 @@ struct Handle {
     std::map<GraphKey, std::pair<cudaGraphExec_t, int>> graphs;
     bool capturing = false;
     BatchArrays arrays;                           // the device arrays above as the kernels see them (api.cu: refresh_arrays)
-    KltState *klt = nullptr;
-    MargScratch *marg = nullptr;
-    FmState *fm = nullptr;
-    double *pnp_dev = nullptr, *pnp_host = nullptr;   // pnp.cu: device buffer + pinned staging, grown on demand to the
-                                                      // largest batch (records, points, IMU records, frames) seen
-    size_t pnp_words = 0;
+    KltState klt;
+    DevBuf<double> marg;                          // ba_marg.cu: scratch blocks of the marginaliser's dense kernels
+    FmState fm;
+    DevBuf<double> pnp;                           // pnp.cu: both sides, grown on demand to the largest batch (records,
+                                                  // points, IMU records, frames) seen
 };
 
 int fail(Handle *h, int code, const char *what, cudaError_t e = cudaSuccess);
@@ -138,6 +226,35 @@ inline SolveOptions solve_options(const pvio_b200_options *opt) {
 
 #define TRY(x) do { int rc__ = (x); if (rc__ != 0) return rc__; } while (0)
 
+// The one allocation routine of the library.  n elements on the given sides (MemSides), per elements per window slot.
+// A buffer being replaced may still be in use by queued work, so the handle's stream is synchronised before it is freed.
+// Every allocation is zeroed: device memory in stream order on the handle's stream (which every kernel of the handle
+// follows), pinned memory here.  The capacity is recorded last, so a failed step leaves an empty buffer that the next
+// alloc / reserve allocates again instead of a half-built one.
+template <typename T>
+int alloc(Handle *h, DevBuf<T> &b, size_t n, int sides, size_t per = 0) {
+    if (b.d || b.h) CK(h, cudaStreamSynchronize(h->stream));
+    b = DevBuf<T>();
+    if (n == 0) return 0;
+    const size_t bytes = n * sizeof(T);
+    if (sides & kDevice) {
+        CK(h, cudaMalloc(&b.d, bytes));
+        CK(h, cudaMemsetAsync(b.d, 0, bytes, h->stream));
+    }
+    if (sides & kPinned) {
+        CK(h, cudaMallocHost(&b.h, bytes));
+        memset(b.h, 0, bytes);
+    }
+    b.n = n; b.per = per;
+    return 0;
+}
+
+// grow-only: allocates only when n exceeds the capacity
+template <typename T>
+int reserve(Handle *h, DevBuf<T> &b, size_t n, int sides) {
+    return n <= b.n ? 0 : alloc(h, b, n, sides);
+}
+
 // api.cu: pack window into slot 0, copy it to the device, build the frame-major table
 int pack_and_upload(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s);
 // api.cu: linearise + Schur of the uploaded windows [0, n) with the fp64 pipeline, no loss (the marginaliser's reprojection part)
@@ -149,26 +266,21 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
                    int max_level, int max_iter, double eps, double clahe_clip = 0.0, int tiles_x = 0, int tiles_y = 0,
                    uint8_t *prev_eq = nullptr, uint8_t *next_eq = nullptr, uint64_t prev_id = 0, uint64_t next_id = 0, int border = 0);
 int clahe_impl(Handle *h, const uint8_t *src, int width, int height, int stride, double clip, int tiles_x, int tiles_y, uint8_t *dst);
-void klt_free(Handle *h);
 // pnp.cu
 int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,
                    pvio_b200_summary *summary);
 int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
                          const pvio_b200_options *opt, pvio_b200_summary *summaries);
-// ba_marg.cu
-void resident_free(Handle *h);     // resident.cu
 // klt.cu / detect.cu
 const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int height, double clahe_clip);
 int klt_clahe_device(Handle *h, const uint8_t *d_src, uint8_t *d_dst, uint8_t *d_lut, int width, int height, double clip, int tiles_x, int tiles_y);
-void detect_free(Handle *h);
+// ba_marg.cu
 int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
                      double *S_out, double *e_out, double *H_out, double *b_out);
 int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride);
-void marg_free(Handle *h);
 // fmat.cu
 int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double threshold, double confidence, int max_iters,
                    const int32_t *schedule, int n_schedule, uint8_t *mask, double *F_out, int32_t *info);
-void fm_free(Handle *h);
 int fm_cv_schedule(int n, const float *p, const float *q, int iters, int32_t *schedule);
 // selftest.cu
 int selftest_lie_impl(Handle *h, int n, const double *w_in, double *out);

@@ -433,22 +433,9 @@ extern "C" int pvio_b200_debug_marg_stamps(long long *out) {
 }
 #endif
 
-// Persistent device scratch of the marginaliser (it runs at every keyframe: nothing is allocated in the steady state).
-struct MargScratch {
-    double *buf = nullptr;
-    size_t words = 0;
-};
-
-void marg_free(Handle *h) {
-    if (h->marg) {
-        if (h->marg->buf) cudaFree(h->marg->buf);
-        delete h->marg;
-        h->marg = nullptr;
-    }
-}
-
-// Windows per pass of the dense kernels.  Their scratch blocks (about 0.4 MB each at N = 9) are allocated for the largest
-// pass a handle has run and reused by every pass.  Two per SM: at D = 135 the eigen-solver's shared memory admits one CTA
+// Windows per pass of the dense kernels.  Their scratch blocks (about 0.4 MB each at N = 9, Handle::marg) are allocated
+// for the largest pass a handle has run and reused by every pass: the marginaliser runs at every keyframe, and nothing
+// is allocated in the steady state.  Two per SM: at D = 135 the eigen-solver's shared memory admits one CTA
 // per SM, so the second half of a pass queues behind the first; at N = 6 several CTAs share an SM.
 constexpr int kMargChunkPerSm = 2;
 constexpr size_t kEigSmemMax = 226 * 1024;
@@ -477,37 +464,31 @@ static bool eig_fits(int dk) { return eig_smem(dk, 2) <= kEigSmemMax; }      // 
 static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLayout &L) {
     const int chunk = std::min(n, kMargChunkPerSm * h->sm_count);
     L = marg_layout(h);
-    if (!h->marg) h->marg = new MargScratch();
-    if (h->marg->words < L.stride * chunk) {
-        if (h->marg->buf) cudaFree(h->marg->buf);
-        h->marg->buf = nullptr; h->marg->words = 0;
-        CK(h, cudaMalloc(&h->marg->buf, sizeof(double) * L.stride * chunk));
-        h->marg->words = L.stride * chunk;
-    }
+    TRY(reserve(h, h->marg, L.stride * chunk, kDevice));
     static bool attr_set = false;
     if (eig && !attr_set) { CK(h, cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEigSmemMax)); attr_set = true; }
     // vision part: no loss, victim-seen landmarks only, mu = 0, fp64 (lin_obs_kernel<false, double> + schur_kernel<double>)
     TRY(run_marg_vision(h, n));
-    const size_t Nc = h->Ncap, dcap = 15 * Nc, xs = Nc * kFrameStride;
+    double *buf = h->marg.d;
     MargArgs m = launch_args<MargArgs>(h);
-    m.index = index; m.buf = h->marg->buf; m.L = L;
+    m.index = index; m.buf = buf; m.L = L;
     for (int w0 = 0; w0 < n; w0 += chunk) {
         const int cn = std::min(chunk, n - w0);
         m.w0 = w0;
         marg_assemble_kernel<<<cn, 256, 0, h->stream>>>(m);
-        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, h->marg->buf, L);
+        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, buf, L);
         h->launches += 2;
         if (!eig) continue;
         int dk = 0;
         for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[i].N - 1));
         const int ring = eig_smem(dk, 4) <= kEigSmemMax ? 4 : 2;      // 2 when the matrix leaves no room: dk = 165
         if (to_slots)
-            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, h->marg->buf, L, ring,
-                h->prior_S.d + w0 * dcap * dcap, dcap * dcap, h->prior_e.d + w0 * dcap, dcap, h->frames.d + w0 * xs,
-                h->prior_x0.d + w0 * xs, xs);
+            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, buf, L, ring,
+                h->prior_S.dslot(w0), h->prior_S.per, h->prior_e.dslot(w0), h->prior_e.per, h->frames.dslot(w0),
+                h->prior_x0.dslot(w0), h->prior_x0.per);
         else
-            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, h->marg->buf, L, ring,
-                h->marg->buf + L.S, L.stride, h->marg->buf + L.e, L.stride, nullptr, nullptr, 0);
+            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, buf, L, ring,
+                buf + L.S, L.stride, buf + L.e, L.stride, nullptr, nullptr, 0);
         ++h->launches;
     }
     CK(h, cudaGetLastError());
@@ -529,7 +510,7 @@ int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state
     TRY(pack_and_upload(h, w, s));
     MargLayout L;
     TRY(run_marg(h, 1, index, eig, keep_on_device, L));
-    const double *blk = h->marg->buf;
+    const double *blk = h->marg.d;
     if (H_out) CK(h, cudaMemcpyAsync(H_out, blk + L.Hk, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
     if (b_out) CK(h, cudaMemcpyAsync(b_out, blk + L.bk, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
     const double *dS = keep_on_device ? h->prior_S.d : blk + L.S, *de = keep_on_device ? h->prior_e.d : blk + L.e;
@@ -556,12 +537,11 @@ int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, do
     }
     MargLayout L;
     TRY(run_marg(h, n, 0, true, true, L));
-    const size_t dcap = 15 * (size_t)h->Ncap;
     for (int i = 0; i < n; ++i) {          // slot i's prior arrays hold the dense dk x dk S and e at their start
         const size_t dk = 15 * (size_t)(h->hdr.h[i].N - 1);
-        if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.d + i * dcap * dcap, sizeof(double) * dk * dk,
+        if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.dslot(i), sizeof(double) * dk * dk,
                                          cudaMemcpyDeviceToHost, h->stream));
-        if (e_out) CK(h, cudaMemcpyAsync(e_out + i * e_stride, h->prior_e.d + i * dcap, sizeof(double) * dk,
+        if (e_out) CK(h, cudaMemcpyAsync(e_out + i * e_stride, h->prior_e.dslot(i), sizeof(double) * dk,
                                          cudaMemcpyDeviceToHost, h->stream));
     }
     CK(h, cudaStreamSynchronize(h->stream));

@@ -27,34 +27,6 @@
 #include "api_internal.h"
 
 namespace pvio {
-
-struct DetectState {
-    int w = 0, h = 0;
-    uint8_t *img = nullptr, *raw = nullptr, *lut = nullptr;   // own copy of the image when the frame is not in the KLT cache
-    int lut_tiles = 0;
-    float *resp = nullptr;
-    unsigned long long *keys = nullptr, *keys_sorted = nullptr;
-    int *counters = nullptr;           // [0] max response bits, [1] candidate count
-    void *cub_tmp = nullptr;
-    size_t cub_bytes = 0;
-    unsigned long long *h_keys = nullptr;   // pinned
-    int *h_counters = nullptr;              // pinned
-    uint8_t *h_img = nullptr;               // pinned
-    int cap = 0;
-};
-
-void detect_free(Handle *h) {
-    DetectState *d = h->detect;
-    if (!d) return;
-    cudaFree(d->img); cudaFree(d->raw); cudaFree(d->lut); cudaFree(d->resp); cudaFree(d->keys); cudaFree(d->keys_sorted);
-    cudaFree(d->counters); cudaFree(d->cub_tmp);
-    if (d->h_keys) cudaFreeHost(d->h_keys);
-    if (d->h_counters) cudaFreeHost(d->h_counters);
-    if (d->h_img) cudaFreeHost(d->h_img);
-    delete d;
-    h->detect = nullptr;
-}
-
 namespace {
 
 __device__ __forceinline__ int refl(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
@@ -192,24 +164,21 @@ struct PoissonFilter {
 };
 
 int ensure(Handle *h, int w, int hgt) {
-    DetectState *d = h->detect;
-    if (d && (d->w != w || d->h != hgt)) { detect_free(h); d = nullptr; }
-    if (d) return 0;
-    d = new DetectState();
-    h->detect = d;
-    d->w = w; d->h = hgt;
+    DetectState &d = h->detect;
     const size_t px = (size_t)w * hgt;
-    d->cap = (int)std::min<size_t>(px / 4 + 1024, (size_t)1 << 22);       // local maxima of a 3x3 test: at most one per 2x2 block
-    CK(h, cudaMalloc(&d->img, px)); CK(h, cudaMalloc(&d->raw, px));
-    CK(h, cudaMalloc(&d->resp, sizeof(float) * px));
-    CK(h, cudaMalloc(&d->keys, sizeof(unsigned long long) * d->cap));
-    CK(h, cudaMalloc(&d->keys_sorted, sizeof(unsigned long long) * d->cap));
-    CK(h, cudaMalloc(&d->counters, sizeof(int) * 2));
-    cub::DeviceRadixSort::SortKeysDescending(nullptr, d->cub_bytes, d->keys, d->keys_sorted, d->cap);
-    CK(h, cudaMalloc(&d->cub_tmp, d->cub_bytes));
-    CK(h, cudaMallocHost(&d->h_keys, sizeof(unsigned long long) * d->cap));
-    CK(h, cudaMallocHost(&d->h_counters, sizeof(int) * 2));
-    CK(h, cudaMallocHost(&d->h_img, px));
+    if (d.w != w || d.h != hgt) {
+        d = DetectState{};
+        d.w = w; d.h = hgt;
+        d.cap = (int)std::min<size_t>(px / 4 + 1024, (size_t)1 << 22);       // local maxima of a 3x3 test: at most one per 2x2 block
+        cub::DeviceRadixSort::SortKeysDescending(nullptr, d.cub_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr, d.cap);
+    }
+    TRY(reserve(h, d.img, px, kBoth));
+    TRY(reserve(h, d.raw, px, kDevice));
+    TRY(reserve(h, d.resp, px, kDevice));
+    TRY(reserve(h, d.keys, d.cap, kDevice));
+    TRY(reserve(h, d.keys_sorted, d.cap, kBoth));
+    TRY(reserve(h, d.counters, 2, kBoth));
+    TRY(reserve(h, d.cub_tmp, d.cub_bytes, kDevice));
     return 0;
 }
 
@@ -230,43 +199,40 @@ extern "C" int pvio_b200_detect_keypoints(pvio_b200_handle hh, uint64_t frame_id
     if (clahe_clip > 0.0 && (tiles_x < 1 || tiles_y < 1 || width % tiles_x || height % tiles_y))
         return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
     TRY(ensure(h, width, height));
-    DetectState *d = h->detect;
+    DetectState &d = h->detect;
     const size_t px = (size_t)width * height;
     const uint8_t *src = klt_cached_level0(h, frame_id, width, height, clahe_clip);
     if (!src) {
         if (!image || stride < width) return fail(h, PVIO_B200_EINVAL, "detect_keypoints: frame not cached and no pixels given");
-        for (int y = 0; y < height; ++y) memcpy(d->h_img + (size_t)y * width, image + (size_t)y * stride, width);
+        for (int y = 0; y < height; ++y) memcpy(d.img.h + (size_t)y * width, image + (size_t)y * stride, width);
         if (clahe_clip > 0.0) {
-            if (d->lut_tiles < tiles_x * tiles_y) {
-                cudaFree(d->lut); d->lut = nullptr;
-                CK(h, cudaMalloc(&d->lut, (size_t)tiles_x * tiles_y * 256));
-                d->lut_tiles = tiles_x * tiles_y;
-            }
-            CK(h, cudaMemcpyAsync(d->raw, d->h_img, px, cudaMemcpyHostToDevice, h->stream));
-            TRY(klt_clahe_device(h, d->raw, d->img, d->lut, width, height, clahe_clip, tiles_x, tiles_y));
+            TRY(reserve(h, d.lut, (size_t)tiles_x * tiles_y * 256, kDevice));
+            CK(h, cudaMemcpyAsync(d.raw.d, d.img.h, px, cudaMemcpyHostToDevice, h->stream));
+            TRY(klt_clahe_device(h, d.raw.d, d.img.d, d.lut.d, width, height, clahe_clip, tiles_x, tiles_y));
         } else {
-            CK(h, cudaMemcpyAsync(d->img, d->h_img, px, cudaMemcpyHostToDevice, h->stream));
+            CK(h, cudaMemcpyAsync(d.img.d, d.img.h, px, cudaMemcpyHostToDevice, h->stream));
         }
-        src = d->img;
+        src = d.img.d;
     }
-    CK(h, cudaMemsetAsync(d->counters, 0, sizeof(int) * 2, h->stream));
+    int *counters = d.counters.d;
+    CK(h, cudaMemsetAsync(counters, 0, sizeof(int) * 2, h->stream));
     harris_response_kernel<<<dim3((width + kTX - 1) / kTX, (height + kTY - 1) / kTY), dim3(kTX, kTY), 0, h->stream>>>(
-        src, width, height, 0.04f, d->resp, d->counters);
+        src, width, height, 0.04f, d.resp.d, counters);
     nms_compact_kernel<<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, h->stream>>>(
-        d->resp, width, height, 1.0e-3, d->counters, d->keys, d->counters + 1, d->cap);
+        d.resp.d, width, height, 1.0e-3, counters, d.keys.d, counters + 1, d.cap);
     h->launches += 2;
-    CK(h, cudaMemcpyAsync(d->h_counters, d->counters, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(d.counters.h, counters, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
-    const int n = std::min(d->h_counters[1], d->cap);
+    const int n = std::min(d.counters.h[1], d.cap);
     std::vector<float> corners;
     if (n > 0) {
-        size_t tmp = d->cub_bytes;
-        cub::DeviceRadixSort::SortKeysDescending(d->cub_tmp, tmp, d->keys, d->keys_sorted, n, 0, 64, h->stream);
+        size_t tmp = d.cub_bytes;
+        cub::DeviceRadixSort::SortKeysDescending(d.cub_tmp.d, tmp, d.keys.d, d.keys_sorted.d, n, 0, 64, h->stream);
         ++h->launches;
-        CK(h, cudaMemcpyAsync(d->h_keys, d->keys_sorted, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost, h->stream));
+        CK(h, cudaMemcpyAsync(d.keys_sorted.h, d.keys_sorted.d, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost, h->stream));
         CK(h, cudaStreamSynchronize(h->stream));
         CK(h, cudaGetLastError());
-        min_distance_select(d->h_keys, n, width, height, 20.0, 1000, corners);          // GFTTDetector::create(1000, 1e-3, 20, 3, true)
+        min_distance_select(d.keys_sorted.h, n, width, height, 20.0, 1000, corners);          // GFTTDetector::create(1000, 1e-3, 20, 3, true)
     }
     const int ng = (int)corners.size() / 2;
     if (n_gftt) *n_gftt = ng;

@@ -32,33 +32,6 @@
 #include "api_internal.h"
 
 namespace pvio {
-
-struct FmState {
-    float *d_pts = nullptr;        // [2][cap_n][2]  p then q
-    int *d_sched = nullptr;        // [cap_s][7]
-    int *d_counts = nullptr;       // [cap_s][4]  nmodels, count / median bits of each model
-    double *d_F = nullptr;         // [cap_s][3][9]
-    unsigned *d_masks = nullptr;   // [cap_s][3][cap_w]
-    float *h_pts = nullptr;        // pinned
-    int *h_sched = nullptr, *h_counts = nullptr;
-    double *h_F = nullptr;
-    unsigned *h_mask = nullptr;
-    int cap_n = 0, cap_s = 0, cap_w = 0;
-};
-
-void fm_free(Handle *h) {
-    FmState *f = h->fm;
-    if (!f) return;
-    cudaFree(f->d_pts); cudaFree(f->d_sched); cudaFree(f->d_counts); cudaFree(f->d_F); cudaFree(f->d_masks);
-    if (f->h_pts) cudaFreeHost(f->h_pts);
-    if (f->h_sched) cudaFreeHost(f->h_sched);
-    if (f->h_counts) cudaFreeHost(f->h_counts);
-    if (f->h_F) cudaFreeHost(f->h_F);
-    if (f->h_mask) cudaFreeHost(f->h_mask);
-    delete f;
-    h->fm = nullptr;
-}
-
 namespace {
 
 // ---- host: OpenCV's sample schedule --------------------------------------------------------------------------------
@@ -363,34 +336,17 @@ __global__ void fm_mask_kernel(const float2 *p, const float2 *q, int n, const do
     if ((threadIdx.x & 31) == 0) mask[i >> 5] = b;
 }
 
+// room for n points and s iterations: at least 1024 points and 1000 iterations, grown on demand
 int fm_reserve(Handle *h, int n, int s) {
-    if (!h->fm) h->fm = new FmState();
-    FmState *f = h->fm;
-    if (n > f->cap_n || s > f->cap_s) {
-        const int cn = std::max(n, std::max(f->cap_n, 1024)), cs = std::max(s, std::max(f->cap_s, 1000));
-        const int cw = (cn + 31) / 32;
-        CK(h, cudaStreamSynchronize(h->stream));
-        cudaFree(f->d_pts); cudaFree(f->d_sched); cudaFree(f->d_counts); cudaFree(f->d_F); cudaFree(f->d_masks);
-        if (f->h_pts) cudaFreeHost(f->h_pts);
-        if (f->h_sched) cudaFreeHost(f->h_sched);
-        if (f->h_counts) cudaFreeHost(f->h_counts);
-        if (f->h_F) cudaFreeHost(f->h_F);
-        if (f->h_mask) cudaFreeHost(f->h_mask);
-        f->d_pts = nullptr; f->d_sched = nullptr; f->d_counts = nullptr; f->d_F = nullptr; f->d_masks = nullptr;
-        f->h_pts = nullptr; f->h_sched = nullptr; f->h_counts = nullptr; f->h_F = nullptr; f->h_mask = nullptr;
-        f->cap_n = f->cap_s = f->cap_w = 0;
-        CK(h, cudaMalloc(&f->d_pts, sizeof(float) * 4 * cn));
-        CK(h, cudaMalloc(&f->d_sched, sizeof(int) * 7 * cs));
-        CK(h, cudaMalloc(&f->d_counts, sizeof(int) * 4 * cs));
-        CK(h, cudaMalloc(&f->d_F, sizeof(double) * 27 * cs));
-        CK(h, cudaMalloc(&f->d_masks, sizeof(unsigned) * 3 * (size_t)cs * cw));
-        CK(h, cudaMallocHost(&f->h_pts, sizeof(float) * 4 * cn));
-        CK(h, cudaMallocHost(&f->h_sched, sizeof(int) * 7 * cs));
-        CK(h, cudaMallocHost(&f->h_counts, sizeof(int) * 4 * cs));
-        CK(h, cudaMallocHost(&f->h_F, sizeof(double) * 27));
-        CK(h, cudaMallocHost(&f->h_mask, sizeof(unsigned) * cw));
-        f->cap_n = cn; f->cap_s = cs; f->cap_w = cw;
-    }
+    FmState &f = h->fm;
+    const size_t cn = std::max(n, 1024), cs = std::max(s, 1000), cw = (cn + 31) / 32;
+    TRY(reserve(h, f.pts, 4 * cn, kBoth));
+    TRY(reserve(h, f.sched, 7 * cs, kBoth));
+    TRY(reserve(h, f.counts, 4 * cs, kBoth));
+    TRY(reserve(h, f.F, 27 * cs, kDevice));
+    TRY(reserve(h, f.masks, 3 * cs * cw, kDevice));
+    TRY(reserve(h, f.h_F, 9, kPinned));
+    TRY(reserve(h, f.h_mask, cw, kPinned));
     return 0;
 }
 
@@ -416,12 +372,12 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
     const bool seven = n == 7, ransac = n >= 15;
     const int budget = seven ? 1 : ransac ? max_iters : ransac_update_num_iters(confidence, 0.45, 7, max_iters);
     TRY(fm_reserve(h, n, budget));
-    FmState *f = h->fm;
-    std::memcpy(f->h_pts, p, sizeof(float) * 2 * n);
-    std::memcpy(f->h_pts + 2 * n, q, sizeof(float) * 2 * n);
+    FmState &f = h->fm;
+    std::memcpy(f.pts.h, p, sizeof(float) * 2 * n);
+    std::memcpy(f.pts.h + 2 * n, q, sizeof(float) * 2 * n);
     int have = budget;                        // iterations that have a subset
     if (seven) {
-        for (int i = 0; i < 7; ++i) f->h_sched[i] = i;
+        for (int i = 0; i < 7; ++i) f.sched.h[i] = i;
     } else if (schedule) {
         if (n_schedule < 1) return fail(h, PVIO_B200_EINVAL, "find_fundamental_mask: empty schedule");
         have = std::min(budget, n_schedule);
@@ -430,11 +386,11 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
             for (int i = 0; i < 7; ++i) {
                 const int v = schedule[7 * it + i];
                 if (v < 0 || v >= n) return fail(h, PVIO_B200_EINVAL, "find_fundamental_mask: schedule index out of range");
-                f->h_sched[7 * it + i] = v;
+                f.sched.h[7 * it + i] = v;
             }
         }
     } else {
-        have = cv_schedule(p, q, n, budget, ransac ? 10000 : 1000, f->h_sched);
+        have = cv_schedule(p, q, n, budget, ransac ? 10000 : 1000, f.sched.h);
     }
     if (have == 0) {                          // getSubset failed at iteration 0: run() returns false, the mask stays as created
         std::memset(mask, 0, n);
@@ -442,30 +398,30 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
     }
     cudaStream_t st = h->stream;
     const int nw = (n + 31) / 32;
-    float2 *dp = (float2 *)f->d_pts, *dq = (float2 *)(f->d_pts + 2 * n);
-    CK(h, cudaMemcpyAsync(f->d_pts, f->h_pts, sizeof(float) * 4 * n, cudaMemcpyHostToDevice, st));
-    CK(h, cudaMemcpyAsync(f->d_sched, f->h_sched, sizeof(int) * 7 * have, cudaMemcpyHostToDevice, st));
+    float2 *dp = (float2 *)f.pts.d, *dq = (float2 *)(f.pts.d + 2 * n);
+    CK(h, cudaMemcpyAsync(f.pts.d, f.pts.h, sizeof(float) * 4 * n, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(f.sched.d, f.sched.h, sizeof(int) * 7 * have, cudaMemcpyHostToDevice, st));
     const float thr2 = (float)(threshold * threshold);
     fm_hypotheses_kernel<<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>(
-        dp, dq, n, f->d_sched, have, thr2, (!ransac && !seven) ? 1 : 0, nw, f->d_counts, f->d_F, f->d_masks);
+        dp, dq, n, f.sched.d, have, thr2, (!ransac && !seven) ? 1 : 0, nw, f.counts.d, f.F.d, f.masks.d);
     h->launches++;
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(f->h_counts, f->d_counts, sizeof(int) * 4 * have, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(f.counts.h, f.counts.d, sizeof(int) * 4 * have, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
 
     int best_it = -1, best_k = -1, it = 0;
     if (seven) {
         inf[3] = 3;
         std::memset(mask, 1, n);              // fundam.cpp: the mask of the 7-point / 8-point call is all ones
-        if (f->h_counts[0] >= 1) { best_it = 0; best_k = 0; }
+        if (f.counts.h[0] >= 1) { best_it = 0; best_k = 0; }
         it = 1;
     } else if (ransac) {
         inf[3] = 1;
         int niters = budget, max_good = 0;
         for (; it < niters && it < have; ++it) {
-            const int nm = f->h_counts[4 * it];
+            const int nm = f.counts.h[4 * it];
             for (int k = 0; k < nm && k < 3; ++k) {
-                const int good = f->h_counts[4 * it + 1 + k];
+                const int good = f.counts.h[4 * it + 1 + k];
                 if (good > std::max(max_good, 6)) {
                     max_good = good; best_it = it; best_k = k;
                     niters = ransac_update_num_iters(confidence, (double)(n - good) / n, 7, niters);
@@ -476,18 +432,18 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
         inf[3] = 2;
         double min_median = DBL_MAX;
         for (; it < have; ++it) {
-            const int nm = f->h_counts[4 * it];
+            const int nm = f.counts.h[4 * it];
             for (int k = 0; k < nm && k < 3; ++k) {
                 float med;
-                std::memcpy(&med, &f->h_counts[4 * it + 1 + k], 4);
+                std::memcpy(&med, &f.counts.h[4 * it + 1 + k], 4);
                 if ((double)med < min_median) { min_median = med; best_it = it; best_k = k; }
             }
         }
         if (best_it >= 0) {
             double sigma = 2.5 * 1.4826 * (1 + 5. / (n - 7)) * std::sqrt(min_median);
             sigma = std::fmax(sigma, 0.001);
-            fm_mask_kernel<<<(n + 31) / 32, 32, 0, st>>>(dp, dq, n, f->d_F + (size_t)(3 * best_it + best_k) * 9, (float)(sigma * sigma),
-                                                        f->d_masks);
+            fm_mask_kernel<<<(n + 31) / 32, 32, 0, st>>>(dp, dq, n, f.F.d + (size_t)(3 * best_it + best_k) * 9, (float)(sigma * sigma),
+                                                        f.masks.d);
             h->launches++;
             CK(h, cudaGetLastError());
         }
@@ -497,15 +453,15 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
         if (!seven) std::memset(mask, 0, n);
         return finish(0);
     }
-    CK(h, cudaMemcpyAsync(f->h_F, f->d_F + (size_t)(3 * best_it + best_k) * 9, sizeof(double) * 9, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(f.h_F.h, f.F.d + (size_t)(3 * best_it + best_k) * 9, sizeof(double) * 9, cudaMemcpyDeviceToHost, st));
     if (!seven) {
-        const unsigned *src = ransac ? f->d_masks + (size_t)(3 * best_it + best_k) * nw : f->d_masks;
-        CK(h, cudaMemcpyAsync(f->h_mask, src, sizeof(unsigned) * nw, cudaMemcpyDeviceToHost, st));
+        const unsigned *src = ransac ? f.masks.d + (size_t)(3 * best_it + best_k) * nw : f.masks.d;
+        CK(h, cudaMemcpyAsync(f.h_mask.h, src, sizeof(unsigned) * nw, cudaMemcpyDeviceToHost, st));
     }
     CK(h, cudaStreamSynchronize(st));
     if (!seven)
-        for (int i = 0; i < n; ++i) mask[i] = (f->h_mask[i >> 5] >> (i & 31)) & 1u;
-    if (F_out) std::memcpy(F_out, f->h_F, 9 * sizeof(double));
+        for (int i = 0; i < n; ++i) mask[i] = (f.h_mask.h[i >> 5] >> (i & 31)) & 1u;
+    if (F_out) std::memcpy(F_out, f.h_F.h, 9 * sizeof(double));
     return finish(0);
 }
 

@@ -203,33 +203,32 @@ extern "C" int pvio_b200_preintegrate(pvio_b200_handle hh, int n_factors, const 
                                       const double *t_end, const double *bias, const double *noise_cov, double *records) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    if (n_factors < 1 || !begin || !samples || !t_end || !bias || !noise_cov || !records) { h->err = "preintegrate: bad argument"; return PVIO_B200_EINVAL; }
+    if (n_factors < 1 || !begin || !samples || !t_end || !bias || !noise_cov || !records)
+        return fail(h, PVIO_B200_EINVAL, "preintegrate: bad argument");
     for (int i = 0; i < n_factors; ++i)
-        if (begin[i + 1] <= begin[i]) { h->err = "preintegrate: a factor without IMU samples (integrate() returns false, preintegrator.cpp:86)"; return PVIO_B200_EINVAL; }
+        if (begin[i + 1] <= begin[i])
+            return fail(h, PVIO_B200_EINVAL, "preintegrate: a factor without IMU samples (integrate() returns false, preintegrator.cpp:86)");
     cudaSetDevice(h->device);
     const size_t total = (size_t)begin[n_factors];
     const size_t nd = total * 7 + (size_t)n_factors * 7 + 36 + (size_t)n_factors * kImuStride;
-    double *d = nullptr;
-    int32_t *db = nullptr;
-    if (cudaMalloc(&d, sizeof(double) * nd) != cudaSuccess || cudaMalloc(&db, sizeof(int32_t) * (n_factors + 1)) != cudaSuccess) {
-        cudaFree(d); h->err = "preintegrate: out of device memory"; return PVIO_B200_ECUDA;
-    }
+    DevBuf<double> d;
+    DevBuf<int32_t> db;
+    TRY(alloc(h, d, nd, kDevice));
+    TRY(alloc(h, db, n_factors + 1, kDevice));
     ImuArgs a;
-    a.n = n_factors; a.begin = db;
-    double *ds = d, *dt = ds + total * 7, *dbias = dt + n_factors, *dn = dbias + (size_t)n_factors * 6, *dr = dn + 36;
+    a.n = n_factors; a.begin = db.d;
+    double *ds = d.d, *dt = ds + total * 7, *dbias = dt + n_factors, *dn = dbias + (size_t)n_factors * 6, *dr = dn + 36;
     a.samples = ds; a.t_end = dt; a.bias = dbias; a.noise = dn; a.rec = dr;
     cudaStream_t st = h->stream;
-    cudaMemcpyAsync(db, begin, sizeof(int32_t) * (n_factors + 1), cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(ds, samples, sizeof(double) * total * 7, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(dt, t_end, sizeof(double) * n_factors, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(dbias, bias, sizeof(double) * n_factors * 6, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(dn, noise_cov, sizeof(double) * 36, cudaMemcpyHostToDevice, st);
+    CK(h, cudaMemcpyAsync(db.d, begin, sizeof(int32_t) * (n_factors + 1), cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(ds, samples, sizeof(double) * total * 7, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(dt, t_end, sizeof(double) * n_factors, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(dbias, bias, sizeof(double) * n_factors * 6, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(dn, noise_cov, sizeof(double) * 36, cudaMemcpyHostToDevice, st));
     preintegrate_kernel<<<(n_factors + 3) / 4, 128, 0, st>>>(a);
     ++h->launches;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(records, dr, sizeof(double) * (size_t)n_factors * kImuStride, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d); cudaFree(db);
-    if (e != cudaSuccess) { h->err = std::string("preintegrate: ") + cudaGetErrorString(e); return PVIO_B200_ECUDA; }
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(records, dr, sizeof(double) * (size_t)n_factors * kImuStride, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaStreamSynchronize(st));
     return PVIO_B200_OK;
 }

@@ -19,27 +19,6 @@ namespace pvio {
 constexpr int kWin = 21;
 constexpr int kWBits = 14;
 constexpr int kKltWarps = 4;
-constexpr int kMaxLevels = 8;
-
-struct KltState {
-    int w = 0, h = 0, levels = 0, cap_pts = 0;
-    uint8_t *pyr[2] = {nullptr, nullptr};     // both pyramids, levels packed back to back
-    size_t off[kMaxLevels + 1];
-    int lw[kMaxLevels], lh[kMaxLevels];
-    float *d_prev = nullptr, *d_next = nullptr, *d_err = nullptr;
-    uint8_t *d_status = nullptr;
-    uint8_t *raw[2] = {nullptr, nullptr};     // pre-CLAHE level-0 images (raw entry point only)
-    uint8_t *lut = nullptr;                   // [2][tiles][256] CLAHE look-up tables
-    int lut_tiles = 0;
-    uint8_t *h_img = nullptr;                 // pinned staging for both level-0 images
-    float *h_pts = nullptr;                   // pinned: prev | next | err
-    uint8_t *h_status = nullptr;
-    // image cache: pyr[i] holds the finished pyramid of the frame with id pyr_id[i] (0: none) built with pyr_clahe[i];
-    // the tracker calls with prev = the previous call's next (feature_tracker.cpp:92), so half the uploads and
-    // pyramid builds of a steady-state call are skipped
-    uint64_t pyr_id[2] = {0, 0};
-    double pyr_clahe[2] = {0.0, 0.0};
-};
 
 // 20-pixel border rejection of OpenCvImage::track_keypoints (opencv_image.cpp:106-108) on the device
 __global__ void klt_border_kernel(const float *pts, uint8_t *status, int n, int w, int h, int border) {
@@ -310,46 +289,24 @@ klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *s
     }
 }
 
-void klt_free(Handle *h) {
-    KltState *k = h->klt;
-    if (!k) return;
-    for (int i = 0; i < 2; ++i) if (k->pyr[i]) cudaFree(k->pyr[i]);
-    if (k->d_prev) cudaFree(k->d_prev);
-    if (k->d_next) cudaFree(k->d_next);
-    if (k->d_err) cudaFree(k->d_err);
-    if (k->d_status) cudaFree(k->d_status);
-    for (int i = 0; i < 2; ++i) if (k->raw[i]) cudaFree(k->raw[i]);
-    if (k->lut) cudaFree(k->lut);
-    if (k->h_img) cudaFreeHost(k->h_img);
-    if (k->h_pts) cudaFreeHost(k->h_pts);
-    if (k->h_status) cudaFreeHost(k->h_status);
-    delete k;
-    h->klt = nullptr;
-}
-
 static int klt_prepare(Handle *h, int w, int hgt, int max_level, int n_points) {
-    KltState *k = h->klt;
-    if (k && (k->w != w || k->h != hgt || k->levels != max_level + 1 || k->cap_pts < n_points)) { klt_free(h); k = nullptr; }   // (drops the image cache)
-    if (k) return 0;
-    k = new KltState();
-    h->klt = k;
-    k->w = w; k->h = hgt; k->levels = max_level + 1; k->cap_pts = std::max(n_points, 1024);
-    size_t off = 0;
-    int lw = w, lh = hgt;
-    for (int l = 0; l <= max_level; ++l) {
-        k->lw[l] = lw; k->lh[l] = lh; k->off[l] = off;
-        off += ((size_t)lw * lh + 255) & ~(size_t)255;
-        lw = (lw + 1) / 2; lh = (lh + 1) / 2;
+    KltState &k = h->klt;
+    if (k.w != w || k.h != hgt || k.levels != max_level + 1 || k.cap_pts < n_points) {   // (drops the image cache)
+        k = KltState{};
+        k.w = w; k.h = hgt; k.levels = max_level + 1; k.cap_pts = std::max(n_points, 1024);
+        size_t off = 0;
+        int lw = w, lh = hgt;
+        for (int l = 0; l <= max_level; ++l) {
+            k.lw[l] = lw; k.lh[l] = lh; k.off[l] = off;
+            off += ((size_t)lw * lh + 255) & ~(size_t)255;
+            lw = (lw + 1) / 2; lh = (lh + 1) / 2;
+        }
+        k.off[max_level + 1] = off;
     }
-    k->off[max_level + 1] = off;
-    for (int i = 0; i < 2; ++i) CK(h, cudaMalloc(&k->pyr[i], off));
-    CK(h, cudaMalloc(&k->d_prev, sizeof(float) * 2 * k->cap_pts));
-    CK(h, cudaMalloc(&k->d_next, sizeof(float) * 2 * k->cap_pts));
-    CK(h, cudaMalloc(&k->d_err, sizeof(float) * k->cap_pts));
-    CK(h, cudaMalloc(&k->d_status, k->cap_pts));
-    CK(h, cudaMallocHost(&k->h_img, (size_t)2 * w * hgt));
-    CK(h, cudaMallocHost(&k->h_pts, sizeof(float) * 5 * k->cap_pts));
-    CK(h, cudaMallocHost(&k->h_status, k->cap_pts));
+    for (auto &p : k.pyr) TRY(reserve(h, p, k.off[k.levels], kDevice));
+    TRY(reserve(h, k.pts, 5 * (size_t)k.cap_pts, kBoth));
+    TRY(reserve(h, k.status, k.cap_pts, kBoth));
+    TRY(reserve(h, k.img, (size_t)2 * w * hgt, kPinned));
     return 0;
 }
 
@@ -371,15 +328,15 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
         ++levels;
     }
     if (levels - 1 < max_level) max_level = levels - 1;
-    int rc = klt_prepare(h, width, height, max_level, n_points);
-    if (rc != 0) return rc;
-    KltState *k = h->klt;
-    const size_t img_bytes = (size_t)width * height;
+    TRY(klt_prepare(h, width, height, max_level, n_points));
+    KltState &k = h->klt;
+    const size_t img_bytes = (size_t)width * height, cap = k.cap_pts;
+    float *h_pts = k.pts.h, *d_prev = k.pts.d, *d_next = k.pts.d + 2 * cap, *d_err = k.pts.d + 4 * cap;
     // which pyramid slot holds which frame: cached frames (same id, same preprocessing) are neither uploaded nor rebuilt
     int sp = -1, sn = -1;
     for (int i = 0; i < 2; ++i) {
-        if (prev_id && k->pyr_id[i] == prev_id && k->pyr_clahe[i] == clahe_clip) sp = i;
-        if (next_id && k->pyr_id[i] == next_id && k->pyr_clahe[i] == clahe_clip && i != sp) sn = i;
+        if (prev_id && k.pyr_id[i] == prev_id && k.pyr_clahe[i] == clahe_clip) sp = i;
+        if (next_id && k.pyr_id[i] == next_id && k.pyr_clahe[i] == clahe_clip && i != sp) sn = i;
     }
     const bool have_prev = sp >= 0, have_next = sn >= 0;
     if (!have_prev) sp = have_next ? 1 - sn : 0;
@@ -390,76 +347,72 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
     const bool have[2] = {have_prev, have_next};
     for (int i = 0; i < 2; ++i) {
         if (have[i]) continue;
-        for (int y = 0; y < height; ++y) memcpy(k->h_img + i * img_bytes + (size_t)y * width, src[i] + (size_t)y * stride, width);
+        for (int y = 0; y < height; ++y) memcpy(k.img.h + i * img_bytes + (size_t)y * width, src[i] + (size_t)y * stride, width);
     }
-    memcpy(k->h_pts, prev_pts, sizeof(float) * 2 * n_points);
-    memcpy(k->h_pts + 2 * k->cap_pts, next_pts, sizeof(float) * 2 * n_points);
+    memcpy(h_pts, prev_pts, sizeof(float) * 2 * n_points);
+    memcpy(h_pts + 2 * cap, next_pts, sizeof(float) * 2 * n_points);
     if (do_clahe) {
         // raw frames -> device, CLAHE on the device into level 0 of the pyramids (opencv_image.cpp:138-143)
-        if (!k->raw[0]) for (int i = 0; i < 2; ++i) CK(h, cudaMalloc(&k->raw[i], img_bytes));
-        if (k->lut_tiles < tiles_x * tiles_y) {
-            if (k->lut) cudaFree(k->lut);
-            CK(h, cudaMalloc(&k->lut, (size_t)tiles_x * tiles_y * 256));
-            k->lut_tiles = tiles_x * tiles_y;
-        }
+        for (auto &r : k.raw) TRY(reserve(h, r, img_bytes, kDevice));
+        TRY(reserve(h, k.lut, (size_t)tiles_x * tiles_y * 256, kDevice));
     }
     for (int i = 0; i < 2; ++i) {
         if (have[i]) continue;
-        uint8_t *P = k->pyr[slot[i]];
+        uint8_t *P = k.pyr[slot[i]].d;
         if (do_clahe) {
-            CK(h, cudaMemcpyAsync(k->raw[i], k->h_img + i * img_bytes, img_bytes, cudaMemcpyHostToDevice, h->stream));
-            clahe_device(h, k->raw[i], P, k->lut, width, height, clahe_clip, tiles_x, tiles_y);
+            CK(h, cudaMemcpyAsync(k.raw[i].d, k.img.h + i * img_bytes, img_bytes, cudaMemcpyHostToDevice, h->stream));
+            clahe_device(h, k.raw[i].d, P, k.lut.d, width, height, clahe_clip, tiles_x, tiles_y);
         } else {
-            CK(h, cudaMemcpyAsync(P, k->h_img + i * img_bytes, img_bytes, cudaMemcpyHostToDevice, h->stream));
+            CK(h, cudaMemcpyAsync(P, k.img.h + i * img_bytes, img_bytes, cudaMemcpyHostToDevice, h->stream));
         }
         for (int l = 1; l <= max_level; ++l) {
-            dim3 b(32, 8), g((k->lw[l] + 31) / 32, (k->lh[l] + 7) / 8);
-            pyrdown_kernel<<<g, b, 0, h->stream>>>(P + k->off[l - 1], k->lw[l - 1], k->lh[l - 1], P + k->off[l], k->lw[l], k->lh[l]);
+            dim3 b(32, 8), g((k.lw[l] + 31) / 32, (k.lh[l] + 7) / 8);
+            pyrdown_kernel<<<g, b, 0, h->stream>>>(P + k.off[l - 1], k.lw[l - 1], k.lh[l - 1], P + k.off[l], k.lw[l], k.lh[l]);
             ++h->launches;
         }
     }
-    k->pyr_id[sp] = prev_id; k->pyr_clahe[sp] = clahe_clip;
-    k->pyr_id[sn] = next_id; k->pyr_clahe[sn] = clahe_clip;
-    CK(h, cudaMemcpyAsync(k->d_prev, k->h_pts, sizeof(float) * 2 * n_points, cudaMemcpyHostToDevice, h->stream));
-    CK(h, cudaMemcpyAsync(k->d_next, k->h_pts + 2 * k->cap_pts, sizeof(float) * 2 * n_points, cudaMemcpyHostToDevice, h->stream));
+    k.pyr_id[sp] = prev_id; k.pyr_clahe[sp] = clahe_clip;
+    k.pyr_id[sn] = next_id; k.pyr_clahe[sn] = clahe_clip;
+    CK(h, cudaMemcpyAsync(d_prev, h_pts, sizeof(float) * 2 * n_points, cudaMemcpyHostToDevice, h->stream));
+    CK(h, cudaMemcpyAsync(d_next, h_pts + 2 * cap, sizeof(float) * 2 * n_points, cudaMemcpyHostToDevice, h->stream));
     KltLevels L;
     L.n = max_level + 1;
     for (int l = 0; l <= max_level; ++l) {
-        L.I[l] = k->pyr[sp] + k->off[l]; L.J[l] = k->pyr[sn] + k->off[l];
-        L.w[l] = k->lw[l]; L.h[l] = k->lh[l];
+        L.I[l] = k.pyr[sp].d + k.off[l]; L.J[l] = k.pyr[sn].d + k.off[l];
+        L.w[l] = k.lw[l]; L.h[l] = k.lh[l];
     }
     const int mi = std::min(std::max(max_iter, 0), 100);
     const double e = std::min(std::max(eps, 0.0), 10.0);
     klt_track_kernel<<<(n_points + kKltWarps - 1) / kKltWarps, 32 * kKltWarps, 0, h->stream>>>(
-        L, k->d_prev, k->d_next, k->d_status, k->d_err, n_points, mi, e * e, 1e-4f);
+        L, d_prev, d_next, k.status.d, d_err, n_points, mi, e * e, 1e-4f);
     ++h->launches;
     if (border > 0) {
-        klt_border_kernel<<<(n_points + 127) / 128, 128, 0, h->stream>>>(k->d_next, k->d_status, n_points, width, height, border);
+        klt_border_kernel<<<(n_points + 127) / 128, 128, 0, h->stream>>>(d_next, k.status.d, n_points, width, height, border);
         ++h->launches;
     }
-    CK(h, cudaMemcpyAsync(k->h_pts + 2 * k->cap_pts, k->d_next, sizeof(float) * 2 * n_points, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaMemcpyAsync(k->h_pts + 4 * k->cap_pts, k->d_err, sizeof(float) * n_points, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaMemcpyAsync(k->h_status, k->d_status, n_points, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(h_pts + 2 * cap, d_next, sizeof(float) * 2 * n_points, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(h_pts + 4 * cap, d_err, sizeof(float) * n_points, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(k.status.h, k.status.d, n_points, cudaMemcpyDeviceToHost, h->stream));
     if (do_clahe && (prev_eq || next_eq)) {
-        CK(h, cudaMemcpyAsync(k->h_img, k->pyr[sp], img_bytes, cudaMemcpyDeviceToHost, h->stream));
-        CK(h, cudaMemcpyAsync(k->h_img + img_bytes, k->pyr[sn], img_bytes, cudaMemcpyDeviceToHost, h->stream));
+        CK(h, cudaMemcpyAsync(k.img.h, k.pyr[sp].d, img_bytes, cudaMemcpyDeviceToHost, h->stream));
+        CK(h, cudaMemcpyAsync(k.img.h + img_bytes, k.pyr[sn].d, img_bytes, cudaMemcpyDeviceToHost, h->stream));
     }
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    memcpy(next_pts, k->h_pts + 2 * k->cap_pts, sizeof(float) * 2 * n_points);
-    if (err) memcpy(err, k->h_pts + 4 * k->cap_pts, sizeof(float) * n_points);
-    memcpy(status, k->h_status, n_points);
-    if (do_clahe && prev_eq) memcpy(prev_eq, k->h_img, img_bytes);
-    if (do_clahe && next_eq) memcpy(next_eq, k->h_img + img_bytes, img_bytes);
+    memcpy(next_pts, h_pts + 2 * cap, sizeof(float) * 2 * n_points);
+    if (err) memcpy(err, h_pts + 4 * cap, sizeof(float) * n_points);
+    memcpy(status, k.status.h, n_points);
+    if (do_clahe && prev_eq) memcpy(prev_eq, k.img.h, img_bytes);
+    if (do_clahe && next_eq) memcpy(next_eq, k.img.h + img_bytes, img_bytes);
     return 0;
 }
 
 // Level 0 (the equalised image) of a frame in the pyramid cache, or nullptr: the detector reads the frame the tracker
 // has just uploaded (frame.cpp:108-130 detects on the image it tracked into)
 const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int height, double clahe_clip) {
-    KltState *k = h->klt;
-    if (!k || !frame_id || k->w != width || k->h != height) return nullptr;
-    for (int i = 0; i < 2; ++i) if (k->pyr_id[i] == frame_id && k->pyr_clahe[i] == clahe_clip) return k->pyr[i];
+    const KltState &k = h->klt;
+    if (!frame_id || k.w != width || k.h != height) return nullptr;
+    for (int i = 0; i < 2; ++i) if (k.pyr_id[i] == frame_id && k.pyr_clahe[i] == clahe_clip) return k.pyr[i].d;
     return nullptr;
 }
 // CLAHE of a device image into a device image (the detector's own upload path)
@@ -473,14 +426,14 @@ int clahe_impl(Handle *h, const uint8_t *src, int width, int height, int stride,
     if (width < 1 || height < 1 || stride < width || clip <= 0.0 || tiles_x < 1 || tiles_y < 1 || width % tiles_x || height % tiles_y)
         return fail(h, PVIO_B200_EINVAL, "clahe: bad arguments (the image size must be a multiple of the tile grid)");
     const size_t bytes = (size_t)width * height;
-    uint8_t *d = nullptr;
-    CK(h, cudaMalloc(&d, 2 * bytes + (size_t)tiles_x * tiles_y * 256));
-    cudaError_t e = cudaMemcpy2DAsync(d, width, src, stride, width, height, cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) { clahe_device(h, d, d + bytes, d + 2 * bytes, width, height, clip, tiles_x, tiles_y); e = cudaGetLastError(); }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dst, d + bytes, bytes, cudaMemcpyDeviceToHost, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    cudaFree(d);
-    if (e != cudaSuccess) { h->err = std::string("clahe: ") + cudaGetErrorString(e); return PVIO_B200_ECUDA; }
+    DevBuf<uint8_t> buf;
+    TRY(alloc(h, buf, 2 * bytes + (size_t)tiles_x * tiles_y * 256, kDevice));
+    uint8_t *d = buf.d;
+    CK(h, cudaMemcpy2DAsync(d, width, src, stride, width, height, cudaMemcpyHostToDevice, h->stream));
+    clahe_device(h, d, d + bytes, d + 2 * bytes, width, height, clip, tiles_x, tiles_y);
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(dst, d + bytes, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
 

@@ -320,16 +320,9 @@ int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, dou
     // IMU records [n_imu][kImuStride] of the inertial problems | frames [n][16] | summary words [n][8]
     const size_t o_pts = (size_t)n * kPnpRecWords, o_z = o_pts + 3 * n_pts, o_imu = o_z + 2 * n_pts;
     const size_t o_frames = o_imu + n_imu * kImuStride, o_out = o_frames + (size_t)16 * n, words = o_out + (size_t)8 * n;
-    if (words > h->pnp_words) {     // this runs on every frame: grown to the largest batch seen, no allocation in the steady state
-        if (h->pnp_dev) cudaFree(h->pnp_dev);
-        if (h->pnp_host) cudaFreeHost(h->pnp_host);
-        h->pnp_dev = nullptr; h->pnp_host = nullptr; h->pnp_words = 0;
-        const size_t cap = std::max<size_t>(words, (size_t)kPnpRecWords + 5 * 512 + kImuStride + 24);
-        CK(h, cudaMalloc(&h->pnp_dev, sizeof(double) * cap));
-        CK(h, cudaMallocHost(&h->pnp_host, sizeof(double) * cap));
-        h->pnp_words = cap;
-    }
-    double *d = h->pnp_dev, *stage = h->pnp_host;
+    // this runs on every frame: grown to the largest batch seen, no allocation in the steady state
+    TRY(reserve(h, h->pnp, std::max<size_t>(words, (size_t)kPnpRecWords + 5 * 512 + kImuStride + 24), kBoth));
+    double *d = h->pnp.d, *stage = h->pnp.h;
     PnpArgs *recs = reinterpret_cast<PnpArgs *>(stage);
     const SolveOptions o = solve_options(opt);
     size_t p = 0, k = 0;

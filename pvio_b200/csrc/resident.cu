@@ -18,34 +18,6 @@
 #include "api_internal.h"
 
 namespace pvio {
-
-struct ResTrack {
-    std::vector<int32_t> frames;      // window indices, increasing
-    std::vector<double> z;            // [2] per observation
-    double rho = 1.0;
-    bool alive = true;
-};
-
-struct ResidentWindow {
-    pvio_b200_window cst;             // constants (extrinsics, noise model, flags); the array members are rebuilt per call
-    std::vector<std::array<double, kFrameStride>> frames;
-    std::vector<uint8_t> fixed;
-    std::vector<std::array<double, kImuStride>> imu;      // factor k couples frames (k, k + 1)
-    std::vector<ResTrack> tracks;
-    int n_prior = 0;                  // the prior covers frames 0 .. n_prior - 1
-    bool prior_on_device = false;
-    std::vector<double> host_S, host_e, host_x0;          // a prior given by the caller (first window: the gauge prior)
-    // the view handed to pack_window
-    std::vector<int32_t> lm_anchor, lm_obs_begin, obs_frame, imu_i, imu_j, prior_frames, lm_track;
-    std::vector<double> lm_z_ref, obs_z, imu_data, st_frames, st_rho;
-    std::vector<uint8_t> lm_in_victim;
-};
-
-void resident_free(Handle *h) {
-    delete h->resident;
-    h->resident = nullptr;
-}
-
 namespace {
 
 // quaternions (x, y, z, w), Hamilton product, q * v = rotate: the reference's Eigen conventions (estimation/state.h)
@@ -129,7 +101,7 @@ void build_view(ResidentWindow &r, pvio_b200_window &w, pvio_b200_state &s) {
 
 ResidentWindow *get(Handle *h) {
     if (!h->resident) fail(h, PVIO_B200_EINVAL, "no resident window: call pvio_b200_window_reset first");
-    return h->resident;
+    return h->resident.get();
 }
 
 }  // namespace
@@ -142,8 +114,7 @@ extern "C" {
 int pvio_b200_window_reset(pvio_b200_handle hh, const pvio_b200_window *constants) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h || !constants) return PVIO_B200_EINVAL;
-    resident_free(h);
-    h->resident = new ResidentWindow();
+    h->resident = std::make_unique<ResidentWindow>();
     h->resident->cst = *constants;
     h->prior_resident[0] = 0;
     return 0;

@@ -27,17 +27,14 @@ __global__ void selftest_lie_kernel(int n, const double *w, double *out) {
 }
 
 int selftest_lie_impl(Handle *h, int n, const double *w_in, double *out) {
-    double *d = nullptr;
-    CK(h, cudaMalloc(&d, sizeof(double) * (size_t)n * 35));
-    cudaError_t e = cudaMemcpyAsync(d, w_in, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) {
-        selftest_lie_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(n, d, d + 3 * (size_t)n);
-        ++h->launches;
-        e = cudaMemcpyAsync(out, d + 3 * (size_t)n, sizeof(double) * 32 * n, cudaMemcpyDeviceToHost, h->stream);
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(h, PVIO_B200_ECUDA, "selftest_lie", e);
+    DevBuf<double> buf;
+    TRY(alloc(h, buf, (size_t)n * 35, kDevice));
+    double *d = buf.d;
+    CK(h, cudaMemcpyAsync(d, w_in, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, h->stream));
+    selftest_lie_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(n, d, d + 3 * (size_t)n);
+    ++h->launches;
+    CK(h, cudaMemcpyAsync(out, d + 3 * (size_t)n, sizeof(double) * 32 * n, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
 

@@ -93,36 +93,36 @@ extern "C" int pvio_b200_triangulate(pvio_b200_handle hh, int n_frames, const do
                                      const int32_t *obs_frame, const double *obs_z, double *points, uint8_t *valid, double *score) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    if (n_frames < 1 || n_tracks < 1 || !P || !begin || !obs_frame || !obs_z || !points || !valid || !score) { h->err = "triangulate: bad argument"; return PVIO_B200_EINVAL; }
+    if (n_frames < 1 || n_tracks < 1 || !P || !begin || !obs_frame || !obs_z || !points || !valid || !score)
+        return fail(h, PVIO_B200_EINVAL, "triangulate: bad argument");
     const int total = begin[n_tracks];
     for (int i = 0; i < n_tracks; ++i)
-        if (begin[i + 1] - begin[i] < 2) { h->err = "triangulate: a track needs at least two views (stereo.h:106)"; return PVIO_B200_EINVAL; }
+        if (begin[i + 1] - begin[i] < 2) return fail(h, PVIO_B200_EINVAL, "triangulate: a track needs at least two views (stereo.h:106)");
     for (int i = 0; i < total; ++i)
-        if (obs_frame[i] < 0 || obs_frame[i] >= n_frames) { h->err = "triangulate: frame index out of range"; return PVIO_B200_EINVAL; }
+        if (obs_frame[i] < 0 || obs_frame[i] >= n_frames) return fail(h, PVIO_B200_EINVAL, "triangulate: frame index out of range");
     cudaSetDevice(h->device);
-    unsigned char *d = nullptr;
     const size_t szP = sizeof(double) * 12 * n_frames, szB = sizeof(int32_t) * (n_tracks + 1), szF = sizeof(int32_t) * total,
                  szZ = sizeof(double) * 2 * total, szO = sizeof(double) * 3 * n_tracks, szS = sizeof(double) * n_tracks, szV = n_tracks;
     auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
     const size_t oP = 0, oZ = oP + al(szP), oO = oZ + al(szZ), oS = oO + al(szO), oB = oS + al(szS), oF = oB + al(szB), oV = oF + al(szF);
-    if (cudaMalloc(&d, oV + al(szV)) != cudaSuccess) { h->err = "triangulate: out of device memory"; return PVIO_B200_ECUDA; }
+    DevBuf<unsigned char> buf;
+    TRY(alloc(h, buf, oV + al(szV), kDevice));
+    unsigned char *d = buf.d;
     cudaStream_t st = h->stream;
-    cudaMemcpyAsync(d + oP, P, szP, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(d + oZ, obs_z, szZ, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(d + oB, begin, szB, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(d + oF, obs_frame, szF, cudaMemcpyHostToDevice, st);
+    CK(h, cudaMemcpyAsync(d + oP, P, szP, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(d + oZ, obs_z, szZ, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(d + oB, begin, szB, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(d + oF, obs_frame, szF, cudaMemcpyHostToDevice, st));
     TriArgs a;
     a.n_tracks = n_tracks; a.P = reinterpret_cast<double *>(d + oP); a.z = reinterpret_cast<double *>(d + oZ);
     a.begin = reinterpret_cast<int32_t *>(d + oB); a.frame = reinterpret_cast<int32_t *>(d + oF);
     a.p_out = reinterpret_cast<double *>(d + oO); a.score = reinterpret_cast<double *>(d + oS); a.valid = d + oV;
     triangulate_kernel<<<(n_tracks + 127) / 128, 128, 0, st>>>(a);
     ++h->launches;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(points, d + oO, szO, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(score, d + oS, szS, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(valid, d + oV, szV, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) { h->err = std::string("triangulate: ") + cudaGetErrorString(e); return PVIO_B200_ECUDA; }
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(points, d + oO, szO, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(score, d + oS, szS, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(valid, d + oV, szV, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaStreamSynchronize(st));
     return PVIO_B200_OK;
 }
