@@ -342,6 +342,41 @@ int pvio_b200_track_keypoints(pvio_b200_handle h, uint64_t prev_id, const uint8_
                               int n_points, int max_level, int max_iter, double eps, double clahe_clip, int tiles_x, int tiles_y,
                               int border, double ransac_threshold, double ransac_confidence);
 
+/* One frame pair of pvio_b200_batch_track_keypoints: the next frame of one sequence. */
+typedef struct pvio_b200_klt_pair {
+    int32_t slot;                  /* the sequence's cache slot, 0 .. 65535, distinct within one call                 */
+    int32_t width, height, stride;
+    uint64_t prev_id, next_id;     /* frame ids WITHIN the sequence, != 0                                             */
+    const uint8_t *prev, *next;    /* pixels (raw when clahe_clip > 0); NULL allowed when the id is cached in this    */
+                                   /* slot                                                                            */
+    int32_t n_points;
+    const float *prev_pts;         /* [n][2]                                                                          */
+    float *next_pts;               /* [n][2] in: initial guess (opencv_image.cpp:91-96), out: tracked positions       */
+    uint8_t *status;               /* [n] out: the matches the reference keeps                                        */
+    float *err;                    /* [n] out, may be NULL: LK error, as pvio_b200_klt_track_cached gives it          */
+    int32_t *info;                 /* [4] out, may be NULL: as pvio_b200_find_fundamental_mask's info;                */
+                                   /* {0, -1, -1, 0} when fewer than 8 matches survive                                */
+} pvio_b200_klt_pair;              /* 96 bytes on LP64 */
+
+/* pvio_b200_track_keypoints for n independent sequences in one call, e.g. the new camera frame of each.  Each pair
+ * gets bit for bit what pvio_b200_track_keypoints gives on a handle whose cache holds that sequence's frames: LK on
+ * the two pyramids, the border test, and findFundamentalMat(FM_RANSAC) with OpenCV's own sample schedule over the
+ * survivors (LMedS below 15) when at least 8 survive.  The options are shared; the image shape may differ per pair,
+ * and each pair's level count follows OpenCV's small-image rule for its own shape.
+ * Cache: slot s keeps the finished pyramids of the last two frames of its sequence, keyed by (id, clahe_clip); ids
+ * are looked up in their own slot only, so two slots may use the same ids for different images.  A slot's buffers
+ * are rebuilt, and its cache dropped, only when its shape or level count changes.  Slots are created on demand,
+ * independent of the window capacities, and separate from the cache of the single calls (which
+ * pvio_b200_detect_keypoints reads): neither path reads or evicts the other's frames.  Unlike the single call, a pair
+ * with n_points == 0 still caches its next frame, so a sequence that lost every track continues with prev = NULL.
+ * Every pair is checked before anything is staged: on PVIO_B200_EINVAL no output and no slot has changed.  n == 0 is
+ * a no-op.  A call whose previous frames are all cached runs CLAHE, pyrDown, LK, the schedules, the hypotheses and
+ * the masks as at most 7 + max_level kernel launches whatever n is, with two synchronisations. */
+int pvio_b200_batch_track_keypoints(pvio_b200_handle h, int n, const pvio_b200_klt_pair *pairs,
+                                    int max_level, int max_iter, double eps, double clahe_clip,
+                                    int tiles_x, int tiles_y, int border,
+                                    double ransac_threshold, double ransac_confidence);
+
 /* CLAHE of one frame (same kernels); dst is [height][width]. */
 int pvio_b200_clahe(pvio_b200_handle h, const uint8_t *src, int width, int height, int stride, double clip_limit,
                     int tiles_x, int tiles_y, uint8_t *dst);

@@ -63,6 +63,13 @@ class CPnpProblem(C.Structure):
                 ("last_frame", c_f64p), ("imu_data", c_f64p)]
 
 
+class CKltPair(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32),
+                ("prev_id", C.c_uint64), ("next_id", C.c_uint64), ("prev", c_u8p), ("next", c_u8p),
+                ("n_points", C.c_int32), ("prev_pts", c_f32p), ("next_pts", c_f32p), ("status", c_u8p),
+                ("err", c_f32p), ("info", c_i32p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -76,7 +83,7 @@ EXPORTS = [
     "pvio_b200_window_add_observations", "pvio_b200_window_remove_track", "pvio_b200_window_set_prior",
     "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
     "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
-    "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve",
+    "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve", "pvio_b200_batch_track_keypoints",
 ]
 
 _lib = None
@@ -127,6 +134,8 @@ def load():
     lib.pvio_b200_pnp_solve.argtypes = [vp, C.POINTER(CPnpProblem), c_f64p, C.POINTER(COptions), C.POINTER(CSummary)]
     lib.pvio_b200_batch_pnp_solve.argtypes = [vp, C.c_int, C.POINTER(CPnpProblem), c_f64p, C.c_int64,
                                               C.POINTER(COptions), C.POINTER(CSummary)]
+    lib.pvio_b200_batch_track_keypoints.argtypes = [vp, C.c_int, C.POINTER(CKltPair), C.c_int, C.c_int, C.c_double,
+                                                    C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
     lib.pvio_b200_klt_track.argtypes = [vp, c_u8p, c_u8p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p,
                                         C.c_int, C.c_int, C.c_int, C.c_double]
     for name in EXPORTS:

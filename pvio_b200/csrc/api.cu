@@ -1352,6 +1352,15 @@ int pvio_b200_track_keypoints(pvio_b200_handle hh, uint64_t prev_id, const uint8
     return 0;
 }
 
+int pvio_b200_batch_track_keypoints(pvio_b200_handle hh, int n, const pvio_b200_klt_pair *pairs, int max_level, int max_iter,
+                                    double eps, double clahe_clip, int tiles_x, int tiles_y, int border,
+                                    double ransac_threshold, double ransac_confidence) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return batch_track_impl(h, n, pairs, max_level, max_iter, eps, clahe_clip, tiles_x, tiles_y, border, ransac_threshold,
+                            ransac_confidence);
+}
+
 int pvio_b200_clahe(pvio_b200_handle hh, const uint8_t *src, int width, int height, int stride, double clip_limit,
                     int tiles_x, int tiles_y, uint8_t *dst) {
     Handle *h = reinterpret_cast<Handle *>(hh);

@@ -41,24 +41,39 @@ struct DevBuf {
 };
 enum MemSides { kDevice = 1, kPinned = 2, kBoth = 3 };
 
-// klt.cu: the two pyramids of the tracker and their staging.  Rebuilt (which drops the image cache) when the image
-// shape, the level count or the point capacity changes.
+// klt.cu: the pyramid cache of one sequence -- the finished pyramids of its last two frames.  Rebuilt (which drops the
+// image cache) when the image shape or the level count changes.
 constexpr int kMaxLevels = 8;
-struct KltState {
-    int w = 0, h = 0, levels = 0, cap_pts = 0;
+struct KltPyramids {
+    int w = 0, h = 0, levels = 0;
     DevBuf<uint8_t> pyr[2];                   // both pyramids, levels packed back to back
     size_t off[kMaxLevels + 1] = {};
     int lw[kMaxLevels] = {}, lh[kMaxLevels] = {};
-    DevBuf<float> pts;                        // [5][cap_pts] both sides: prev [2] | next [2] | err
-    DevBuf<uint8_t> status;                   // [cap_pts] both sides
-    DevBuf<uint8_t> raw[2];                   // pre-CLAHE level-0 images (raw entry point only)
-    DevBuf<uint8_t> lut;                      // [tiles][256] CLAHE look-up tables
-    DevBuf<uint8_t> img;                      // pinned staging for both level-0 images
     // image cache: pyr[i] holds the finished pyramid of the frame with id pyr_id[i] (0: none) built with pyr_clahe[i];
     // the tracker calls with prev = the previous call's next (feature_tracker.cpp:92), so half the uploads and
     // pyramid builds of a steady-state call are skipped
     uint64_t pyr_id[2] = {0, 0};
     double pyr_clahe[2] = {0.0, 0.0};
+};
+
+// the single-call tracker: one sequence's pyramids and the staging of one frame pair.  Also rebuilt when the point
+// capacity changes.
+struct KltState : KltPyramids {
+    int cap_pts = 0;
+    DevBuf<float> pts;                        // [5][cap_pts] both sides: prev [2] | next [2] | err
+    DevBuf<uint8_t> status;                   // [cap_pts] both sides
+    DevBuf<uint8_t> raw[2];                   // pre-CLAHE level-0 images (raw entry point only)
+    DevBuf<uint8_t> lut;                      // [tiles][256] CLAHE look-up tables
+    DevBuf<uint8_t> img;                      // pinned staging for both level-0 images
+};
+
+// the batched tracker (pvio_b200_batch_track_keypoints): one pyramid cache per sequence slot, grown on demand, and
+// the buffers of one call, grown to the largest call seen
+struct KltBatchState {
+    std::vector<KltPyramids> slots;
+    DevBuf<uint8_t> stage;                    // both sides: uploaded descriptors, frames and points | downloaded results |
+                                              // winners' masks; host side only: the mask jobs the device reads in place
+    DevBuf<uint8_t> scratch;                  // device: CLAHE tables, RANSAC matches, schedules, counts, models, masks
 };
 
 // detect.cu: per-image-shape buffers of the corner detector
@@ -183,6 +198,7 @@ struct Handle {
     bool capturing = false;
     BatchArrays arrays;                           // the device arrays above as the kernels see them (api.cu: refresh_arrays)
     KltState klt;
+    KltBatchState kltb;                           // klt.cu: the batched tracker, independent of klt
     DevBuf<double> marg;                          // ba_marg.cu: scratch blocks of the marginaliser's dense kernels
     FmState fm;
     DevBuf<double> pnp;                           // pnp.cu: both sides, grown on demand to the largest batch (records,
@@ -278,10 +294,39 @@ int klt_clahe_device(Handle *h, const uint8_t *d_src, uint8_t *d_dst, uint8_t *d
 int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
                      double *S_out, double *e_out, double *H_out, double *b_out);
 int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride);
+// klt.cu: pvio_b200_batch_track_keypoints
+int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_level, int max_iter, double eps,
+                     double clahe_clip, int tiles_x, int tiles_y, int border, double ransac_threshold,
+                     double ransac_confidence);
 // fmat.cu
 int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double threshold, double confidence, int max_iters,
                    const int32_t *schedule, int n_schedule, uint8_t *mask, double *F_out, int32_t *info);
 int fm_cv_schedule(int n, const float *p, const float *q, int iters, int32_t *schedule);
+// fmat.cu, the F-matrix rejection of a batched tracker call: one problem per frame pair, every pointer on the device
+struct FmBatchProblem {
+    const float *prev_pts, *next_pts;         // [n_pts][2] the pair's LK input and output
+    const uint8_t *status;                    // [n_pts] LK + border status
+    float2 *p, *q;                            // [n_pts] room for the survivors, compacted in order
+    int *sched, *counts;                      // [budget][7], [budget][4] (as fm_hypotheses_kernel writes them)
+    double *F;                                // [budget][3][9]
+    unsigned *masks;                          // [budget][3][words of n_pts]
+    int *surv;                                // [2] written on the device: survivors, iterations that have a subset
+    int n_pts, budget;                        // tracked points; iterations reserved (0: fewer than 8 points)
+};
+struct FmMaskJob {                            // the mask of one pair's winning model (n == 0: none)
+    const float2 *p, *q;
+    const double *F;                          // LMedS: the model, tested against thr2
+    const unsigned *src;                      // RANSAC: the mask as fm_hypotheses_kernel stored it
+    unsigned *out;
+    float thr2;
+    int n;
+};
+void fm_options(double &threshold, double &confidence, int &max_iters);
+int fm_lmeds_iters(double confidence, int max_iters);
+float fm_replay(const int *counts, int n, int have, int max_iters, double confidence, int *info);
+void fm_batch_schedule(Handle *h, const FmBatchProblem *probs, int n, int max_iters, int lmeds_iters);
+void fm_batch_hypotheses(Handle *h, const FmBatchProblem *probs, int n, int max_budget, float thr2);
+void fm_batch_masks(Handle *h, const FmMaskJob *jobs, int n, int max_words);
 // selftest.cu
 int selftest_lie_impl(Handle *h, int n, const double *w_in, double *out);
 

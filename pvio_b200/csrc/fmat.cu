@@ -9,7 +9,8 @@
 //
 // Here: SPECULATIVE evaluation + serial-equivalent replay.
 //   host     the sample schedule: cv::RNG((uint64)-1) and getSubset (7 distinct indices, the collinearity test of the
-//            last point) restated, so the schedule IS OpenCV's -- or the schedule the caller injects
+//            last point) restated, so the schedule IS OpenCV's -- or the schedule the caller injects (the batched
+//            tracker draws the same schedule on the device, fm_schedule_kernel)
 //   device   fm_hypotheses_kernel: one warp per iteration of the schedule, ALL max_iters of them at once (1000 warps):
 //            lane 0 solves the 7-point problem (Hartley normalisation, null space of the 7 x 9 system by a Householder
 //            QR of its transpose, the cubic det(lambda f1 + (1 - lambda) f2) = 0 with cv::solveCubic's branches and
@@ -34,26 +35,28 @@
 namespace pvio {
 namespace {
 
-// ---- host: OpenCV's sample schedule --------------------------------------------------------------------------------
+// ---- host and device: OpenCV's sample schedule ----------------------------------------------------------------------
+// One implementation for both sides: the single call draws it on the host, the batched tracker on the device (one
+// thread per frame pair, fm_schedule_kernel).  Integer RNG and unfused double arithmetic: the two draw the same subsets.
 struct CvRng {                       // cv::RNG (core/operations.hpp): multiply-with-carry
     uint64_t state;
-    explicit CvRng(uint64_t s) : state(s ? s : 0xffffffffULL) {}
-    unsigned next() {
+    __host__ __device__ explicit CvRng(uint64_t s) : state(s ? s : 0xffffffffULL) {}
+    __host__ __device__ unsigned next() {
         state = (uint64_t)(unsigned)state * 4164903690U + (unsigned)(state >> 32);
         return (unsigned)state;
     }
-    int uniform(int a, int b) { return a == b ? a : (int)(next() % (unsigned)(b - a) + a); }
+    __host__ __device__ int uniform(int a, int b) { return a == b ? a : (int)(next() % (unsigned)(b - a) + a); }
 };
 
 // fundam.cpp haveCollinearPoints: the LAST of `count` points against every pair before it
-bool last_point_collinear(const float *pts, const int *idx, int count) {
+__host__ __device__ __forceinline__ bool last_point_collinear(const float *pts, const int *idx, int count) {
     const int i = count - 1;
     const float xi = pts[2 * idx[i]], yi = pts[2 * idx[i] + 1];
     for (int j = 0; j < i; ++j) {
         const double dx1 = pts[2 * idx[j]] - xi, dy1 = pts[2 * idx[j] + 1] - yi;
         for (int k = 0; k < j; ++k) {
             const double dx2 = pts[2 * idx[k]] - xi, dy2 = pts[2 * idx[k] + 1] - yi;
-            if (std::fabs(dx2 * dy1 - dy2 * dx1) <= FLT_EPSILON * (std::fabs(dx1) + std::fabs(dy1) + std::fabs(dx2) + std::fabs(dy2)))
+            if (fabs(dx2 * dy1 - dy2 * dx1) <= FLT_EPSILON * (fabs(dx1) + fabs(dy1) + fabs(dx2) + fabs(dy2)))
                 return true;
         }
     }
@@ -61,25 +64,30 @@ bool last_point_collinear(const float *pts, const int *idx, int count) {
 }
 
 // ptsetreg.cpp getSubset for every iteration the loop could run: iteration `it` always consumes exactly one subset.
-// Returns the number of iterations that have a subset (getSubset giving up ends the loop).
-int cv_schedule(const float *p, const float *q, int n, int iters, int max_attempts, int *sched) {
+// Returns the number of iterations that have a subset (getSubset giving up ends the loop; its row holds the last try).
+// The subset is drawn in a local array, which the unrolled loops keep in registers on the device: the serial chain of
+// draws and collinearity tests then never waits on a load of its own subset from global memory.
+__host__ __device__ int cv_schedule(const float *p, const float *q, int n, int iters, int max_attempts, int *sched) {
     CvRng rng((uint64_t)-1);
     for (int it = 0; it < iters; ++it) {
-        int *idx = sched + 7 * it;
+        int idx[7];
         int attempt = 0;
         for (; attempt < max_attempts; ++attempt) {
+#pragma unroll
             for (int i = 0; i < 7; ++i) {
                 int v;
                 bool dup;
                 do {
                     v = rng.uniform(0, n);
                     dup = false;
+#pragma unroll
                     for (int j = 0; j < i; ++j) dup |= idx[j] == v;
                 } while (dup);
                 idx[i] = v;
             }
             if (!last_point_collinear(p, idx, 7) && !last_point_collinear(q, idx, 7)) break;
         }
+        for (int i = 0; i < 7; ++i) sched[7 * it + i] = idx[i];
         if (attempt == max_attempts) return it;
     }
     return iters;
@@ -274,13 +282,23 @@ constexpr int kWarpsPerCta = 4;
 
 // One warp per iteration of the schedule.  lmeds == 0: counts[it] = {nmodels, inliers of model 0, 1, 2}, masks[it][k][nw];
 // lmeds == 1 (n < 32): counts[it] = {nmodels, float bits of the median error of model 0, 1, 2}.
+// kBatch: problem blockIdx.y of probs[] instead of the arguments; its survivor and iteration counts come from the
+// schedule kernel, and it runs LMedS below 15 survivors as the single call does.
+template <bool kBatch>
 __global__ void __launch_bounds__(32 * kWarpsPerCta) fm_hypotheses_kernel(const float2 *p, const float2 *q, int n, const int *sched,
                                                                           int iters, float thr2, int lmeds, int nw, int *counts,
-                                                                          double *Fout, unsigned *masks) {
+                                                                          double *Fout, unsigned *masks,
+                                                                          const FmBatchProblem *probs) {
     __shared__ double sF[kWarpsPerCta][3][9];
     __shared__ int sN[kWarpsPerCta];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int it = blockIdx.x * kWarpsPerCta + warp;
+    if constexpr (kBatch) {
+        const FmBatchProblem &P = probs[blockIdx.y];
+        n = P.surv[0]; iters = P.surv[1];       // iters == 0 below 8 survivors
+        p = P.p; q = P.q; sched = P.sched; counts = P.counts; Fout = P.F; masks = P.masks;
+        lmeds = n < 15 ? 1 : 0; nw = (n + 31) / 32;
+    }
     if (it >= iters) return;
     if (lane == 0) {
         int idx[7];
@@ -325,15 +343,57 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta) fm_hypotheses_kernel(const 
     }
 }
 
-// mask of one model under one threshold (LMedS: the inliers of the best model under sigma; n == 7: not needed)
-__global__ void fm_mask_kernel(const float2 *p, const float2 *q, int n, const double *Fm, float thr2, unsigned *mask) {
-    double F[9];
-    for (int i = 0; i < 9; ++i) F[i] = Fm[i];
+// mask of one model under one threshold (LMedS: the inliers of the best model under sigma; n == 7: not needed).
+// kBatch: the job jobs[blockIdx.y] instead of the arguments; a RANSAC job copies the mask fm_hypotheses_kernel stored.
+template <bool kBatch>
+__global__ void fm_mask_kernel(const float2 *p, const float2 *q, int n, const double *Fm, float thr2, unsigned *mask,
+                               const FmMaskJob *jobs) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (kBatch) {
+        const FmMaskJob &J = jobs[blockIdx.y];
+        if ((i >> 5) * 32 >= J.n) return;       // whole warps
+        mask = J.out;
+        if (J.src) {
+            if ((threadIdx.x & 31) == 0) mask[i >> 5] = J.src[i >> 5];
+            return;
+        }
+        p = J.p; q = J.q; n = J.n; Fm = J.F; thr2 = J.thr2;
+    }
+    double F[9];
+    for (int k = 0; k < 9; ++k) F[k] = Fm[k];
     bool in = false;
     if (i < n) in = fm_error(F, p[i], q[i]) <= thr2;
     const unsigned b = __ballot_sync(0xffffffffu, in);
     if ((threadIdx.x & 31) == 0) mask[i >> 5] = b;
+}
+
+// The batched tracker's step between LK and the hypotheses, one warp per frame pair (opencv_image.cpp:112-121): the
+// warp compacts the pair's surviving matches in order, then lane 0 draws OpenCV's schedule over them when there are at
+// least 8 -- one serial RNG chain per pair, as cv_schedule on the host.  surv = {survivors, iterations with a subset}.
+__global__ void __launch_bounds__(32) fm_schedule_kernel(const FmBatchProblem *probs, int max_iters, int lmeds_iters) {
+    const FmBatchProblem &P = probs[blockIdx.x];
+    const int lane = threadIdx.x;
+    int s = 0;
+    for (int base = 0; base < P.n_pts; base += 32) {
+        const int i = base + lane;
+        const bool keep = i < P.n_pts && P.status[i];
+        const unsigned b = __ballot_sync(0xffffffffu, keep);
+        if (keep) {
+            const int r = s + __popc(b & ((1u << lane) - 1u));
+            P.p[r] = make_float2(P.prev_pts[2 * i], P.prev_pts[2 * i + 1]);
+            P.q[r] = make_float2(P.next_pts[2 * i], P.next_pts[2 * i + 1]);
+        }
+        s += __popc(b);
+    }
+    __syncwarp();
+    if (lane != 0) return;
+    int have = 0;
+    if (s >= 8) {
+        const bool ransac = s >= 15;
+        have = cv_schedule(reinterpret_cast<const float *>(P.p), reinterpret_cast<const float *>(P.q), s,
+                           ransac ? max_iters : lmeds_iters, ransac ? 10000 : 1000, P.sched);
+    }
+    P.surv[0] = s; P.surv[1] = have;
 }
 
 // room for n points and s iterations: at least 1024 points and 1000 iterations, grown on demand
@@ -357,6 +417,61 @@ int fm_cv_schedule(int n, const float *p, const float *q, int iters, int32_t *sc
     return cv_schedule(p, q, n, iters, n >= 15 ? 10000 : 1000, schedule);
 }
 
+// findFundamentalMat's defaults for out-of-range options
+void fm_options(double &threshold, double &confidence, int &max_iters) {
+    if (threshold <= 0) threshold = 3;
+    if (confidence < DBL_EPSILON || confidence > 1 - DBL_EPSILON) confidence = 0.99;
+    if (max_iters < 1) max_iters = 1;
+}
+
+// the iteration budget of the LMedS branch (8 <= n < 15): RANSACUpdateNumIters at the outlier ratio OpenCV assumes
+int fm_lmeds_iters(double confidence, int max_iters) { return ransac_update_num_iters(confidence, 0.45, 7, max_iters); }
+
+// The serial loop OpenCV runs over the evaluated iterations counts[have][4] of n matches (7: the 7-point solve, 8..14:
+// LMedS, >= 15: RANSAC with at most max_iters iterations), with the host's own log / pow as OpenCV's.  Sets
+// inf = {iterations run, winning iteration (-1: none), winning model, method}; returns the threshold of the LMedS
+// winner's mask (sigma^2), 0 otherwise.
+float fm_replay(const int *counts, int n, int have, int max_iters, double confidence, int *inf) {
+    int best_it = -1, best_k = -1, it = 0;
+    float thr2 = 0.f;
+    if (n == 7) {
+        inf[3] = 3;
+        if (counts[0] >= 1) { best_it = 0; best_k = 0; }
+        it = 1;
+    } else if (n >= 15) {
+        inf[3] = 1;
+        int niters = max_iters, max_good = 0;
+        for (; it < niters && it < have; ++it) {
+            const int nm = counts[4 * it];
+            for (int k = 0; k < nm && k < 3; ++k) {
+                const int good = counts[4 * it + 1 + k];
+                if (good > std::max(max_good, 6)) {
+                    max_good = good; best_it = it; best_k = k;
+                    niters = ransac_update_num_iters(confidence, (double)(n - good) / n, 7, niters);
+                }
+            }
+        }
+    } else {
+        inf[3] = 2;
+        double min_median = DBL_MAX;
+        for (; it < have; ++it) {
+            const int nm = counts[4 * it];
+            for (int k = 0; k < nm && k < 3; ++k) {
+                float med;
+                std::memcpy(&med, &counts[4 * it + 1 + k], 4);
+                if ((double)med < min_median) { min_median = med; best_it = it; best_k = k; }
+            }
+        }
+        if (best_it >= 0) {
+            double sigma = 2.5 * 1.4826 * (1 + 5. / (n - 7)) * std::sqrt(min_median);
+            sigma = std::fmax(sigma, 0.001);
+            thr2 = (float)(sigma * sigma);
+        }
+    }
+    inf[0] = it; inf[1] = best_it; inf[2] = best_k;
+    return thr2;
+}
+
 int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double threshold, double confidence, int max_iters,
                    const int32_t *schedule, int n_schedule, uint8_t *mask, double *F_out, int32_t *info) {
     int inf[4] = {0, -1, -1, 0};              // iterations run, winning iteration, winning model, method (1 RANSAC, 2 LMedS, 3 seven points)
@@ -366,11 +481,9 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
         if (n > 0) std::memset(mask, 0, n);
         return finish(0);
     }
-    if (threshold <= 0) threshold = 3;
-    if (confidence < DBL_EPSILON || confidence > 1 - DBL_EPSILON) confidence = 0.99;
-    if (max_iters < 1) max_iters = 1;
+    fm_options(threshold, confidence, max_iters);
     const bool seven = n == 7, ransac = n >= 15;
-    const int budget = seven ? 1 : ransac ? max_iters : ransac_update_num_iters(confidence, 0.45, 7, max_iters);
+    const int budget = seven ? 1 : ransac ? max_iters : fm_lmeds_iters(confidence, max_iters);
     TRY(fm_reserve(h, n, budget));
     FmState &f = h->fm;
     std::memcpy(f.pts.h, p, sizeof(float) * 2 * n);
@@ -402,56 +515,25 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
     CK(h, cudaMemcpyAsync(f.pts.d, f.pts.h, sizeof(float) * 4 * n, cudaMemcpyHostToDevice, st));
     CK(h, cudaMemcpyAsync(f.sched.d, f.sched.h, sizeof(int) * 7 * have, cudaMemcpyHostToDevice, st));
     const float thr2 = (float)(threshold * threshold);
-    fm_hypotheses_kernel<<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>(
-        dp, dq, n, f.sched.d, have, thr2, (!ransac && !seven) ? 1 : 0, nw, f.counts.d, f.F.d, f.masks.d);
+    fm_hypotheses_kernel<false><<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>(
+        dp, dq, n, f.sched.d, have, thr2, (!ransac && !seven) ? 1 : 0, nw, f.counts.d, f.F.d, f.masks.d, nullptr);
     h->launches++;
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(f.counts.h, f.counts.d, sizeof(int) * 4 * have, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
 
-    int best_it = -1, best_k = -1, it = 0;
-    if (seven) {
-        inf[3] = 3;
-        std::memset(mask, 1, n);              // fundam.cpp: the mask of the 7-point / 8-point call is all ones
-        if (f.counts.h[0] >= 1) { best_it = 0; best_k = 0; }
-        it = 1;
-    } else if (ransac) {
-        inf[3] = 1;
-        int niters = budget, max_good = 0;
-        for (; it < niters && it < have; ++it) {
-            const int nm = f.counts.h[4 * it];
-            for (int k = 0; k < nm && k < 3; ++k) {
-                const int good = f.counts.h[4 * it + 1 + k];
-                if (good > std::max(max_good, 6)) {
-                    max_good = good; best_it = it; best_k = k;
-                    niters = ransac_update_num_iters(confidence, (double)(n - good) / n, 7, niters);
-                }
-            }
-        }
-    } else {
-        inf[3] = 2;
-        double min_median = DBL_MAX;
-        for (; it < have; ++it) {
-            const int nm = f.counts.h[4 * it];
-            for (int k = 0; k < nm && k < 3; ++k) {
-                float med;
-                std::memcpy(&med, &f.counts.h[4 * it + 1 + k], 4);
-                if ((double)med < min_median) { min_median = med; best_it = it; best_k = k; }
-            }
-        }
-        if (best_it >= 0) {
-            double sigma = 2.5 * 1.4826 * (1 + 5. / (n - 7)) * std::sqrt(min_median);
-            sigma = std::fmax(sigma, 0.001);
-            fm_mask_kernel<<<(n + 31) / 32, 32, 0, st>>>(dp, dq, n, f.F.d + (size_t)(3 * best_it + best_k) * 9, (float)(sigma * sigma),
-                                                        f.masks.d);
-            h->launches++;
-            CK(h, cudaGetLastError());
-        }
-    }
-    inf[0] = it; inf[1] = best_it; inf[2] = best_k;
+    const float thr_lmeds = fm_replay(f.counts.h, n, have, max_iters, confidence, inf);
+    const int best_it = inf[1], best_k = inf[2];
+    if (seven) std::memset(mask, 1, n);       // fundam.cpp: the mask of the 7-point / 8-point call is all ones
     if (best_it < 0) {
         if (!seven) std::memset(mask, 0, n);
         return finish(0);
+    }
+    if (!ransac && !seven) {
+        fm_mask_kernel<false><<<(n + 31) / 32, 32, 0, st>>>(dp, dq, n, f.F.d + (size_t)(3 * best_it + best_k) * 9, thr_lmeds,
+                                                            f.masks.d, nullptr);
+        h->launches++;
+        CK(h, cudaGetLastError());
     }
     CK(h, cudaMemcpyAsync(f.h_F.h, f.F.d + (size_t)(3 * best_it + best_k) * 9, sizeof(double) * 9, cudaMemcpyDeviceToHost, st));
     if (!seven) {
@@ -463,6 +545,25 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
         for (int i = 0; i < n; ++i) mask[i] = (f.h_mask.h[i >> 5] >> (i & 31)) & 1u;
     if (F_out) std::memcpy(F_out, f.h_F.h, 9 * sizeof(double));
     return finish(0);
+}
+
+// ---- the batched tracker's launches (klt.cu: batch_track_impl) -----------------------------------------------------
+void fm_batch_schedule(Handle *h, const FmBatchProblem *probs, int n, int max_iters, int lmeds_iters) {
+    fm_schedule_kernel<<<n, 32, 0, h->stream>>>(probs, max_iters, lmeds_iters);
+    h->launches++;
+}
+
+// every iteration of every pair in one launch: blockIdx.y is the pair, warps beyond its schedule exit at once
+void fm_batch_hypotheses(Handle *h, const FmBatchProblem *probs, int n, int max_budget, float thr2) {
+    fm_hypotheses_kernel<true><<<dim3((max_budget + kWarpsPerCta - 1) / kWarpsPerCta, n), 32 * kWarpsPerCta, 0, h->stream>>>(
+        nullptr, nullptr, 0, nullptr, 0, thr2, 0, 0, nullptr, nullptr, nullptr, probs);
+    h->launches++;
+}
+
+// every winner's mask in one launch: one warp per mask word, blockIdx.y the pair
+void fm_batch_masks(Handle *h, const FmMaskJob *jobs, int n, int max_words) {
+    fm_mask_kernel<true><<<dim3((max_words + 3) / 4, n), 128, 0, h->stream>>>(nullptr, nullptr, 0, nullptr, 0.f, nullptr, jobs);
+    h->launches++;
 }
 
 }  // namespace pvio

@@ -10,6 +10,7 @@
 //                    <= max_iter Newton steps with OpenCV's eps / oscillation stopping rules.
 // Compiled with -fmad=false: the float expressions must round like OpenCV's (no contraction),
 // because status flags are compared bit-exactly with cv2.
+#include <algorithm>
 #include <cstring>
 #include <vector>
 #include "api_internal.h"
@@ -35,6 +36,18 @@ struct KltLevels {
     int n;
 };
 
+// one frame a batched call uploads (batch_track_impl): its raw pixels in the staging, CLAHE into level 0 of its
+// pyramid, then pyrDown level by level
+struct KltBatchFrame {
+    const uint8_t *raw;                       // level-0 pixels as uploaded (raw when CLAHE runs)
+    uint8_t *lut;                             // [tiles][256] its CLAHE tables
+    uint8_t *pyr;                             // its pyramid in the sequence's slot
+    int levels, tw, th, clip;
+    float lut_scale;
+    int w[kMaxLevels], h[kMaxLevels];
+    size_t off[kMaxLevels];
+};
+
 __device__ __forceinline__ int reflect101(int i, int n) {
     i = i < 0 ? -i : i;
     return i >= n ? 2 * (n - 1) - i : i;
@@ -45,11 +58,17 @@ __device__ __forceinline__ int reflect101(int i, int n) {
 // of the tile grid only.  Kernel 1: one CTA per tile -- histogram in shared memory, clip + redistribute, prefix
 // sum, LUT = cvRound(cdf * 255 / area).  Kernel 2: one thread per pixel, bilinear blend of the four neighbouring
 // tiles' LUTs in OpenCV's float32 operation order (explicit _rn intrinsics: no FMA contraction).
+// kBatch: frame blockIdx.y of frames[] (lut kernel) / blockIdx.z (apply kernel) instead of the arguments.
+template <bool kBatch>
 __global__ void __launch_bounds__(256) clahe_lut_kernel(const uint8_t *src, int w, int tw, int th, int tiles_x,
-                                                        int clip, float lut_scale, uint8_t *lut) {
+                                                        int clip, float lut_scale, uint8_t *lut, const KltBatchFrame *frames) {
     __shared__ int hist[256];
     __shared__ int wsum[8];
     __shared__ int total_clipped;
+    if constexpr (kBatch) {
+        const KltBatchFrame &f = frames[blockIdx.y];
+        src = f.raw; w = f.w[0]; tw = f.tw; th = f.th; clip = f.clip; lut_scale = f.lut_scale; lut = f.lut;
+    }
     const int t = blockIdx.x, tx = t % tiles_x, ty = t / tiles_x, tid = threadIdx.x;
     hist[tid] = 0;
     __syncthreads();
@@ -87,9 +106,14 @@ __global__ void __launch_bounds__(256) clahe_lut_kernel(const uint8_t *src, int 
     lut[(size_t)t * 256 + tid] = (uint8_t)min(max(__float2int_rn(f), 0), 255);
 }
 
+template <bool kBatch>
 __global__ void clahe_apply_kernel(const uint8_t *src, int w, int h, int tw, int th, int tiles_x, int tiles_y,
-                                   const uint8_t *lut, uint8_t *dst) {
+                                   const uint8_t *lut, uint8_t *dst, const KltBatchFrame *frames) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if constexpr (kBatch) {
+        const KltBatchFrame &f = frames[blockIdx.z];
+        src = f.raw; w = f.w[0]; h = f.h[0]; tw = f.tw; th = f.th; lut = f.lut; dst = f.pyr;
+    }
     if (x >= w || y >= h) return;
     const float inv_tw = __fdiv_rn(1.0f, (float)tw), inv_th = __fdiv_rn(1.0f, (float)th);
     const float txf = __fsub_rn(__fmul_rn((float)x, inv_tw), 0.5f), tyf = __fsub_rn(__fmul_rn((float)y, inv_th), 0.5f);
@@ -107,21 +131,39 @@ __global__ void clahe_apply_kernel(const uint8_t *src, int w, int h, int tw, int
     dst[(size_t)y * w + x] = (uint8_t)min(max(__float2int_rn(res), 0), 255);
 }
 
+// cv::CLAHE's per-tile constants of a w x h image
+static void clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_y, int &tw, int &th, int &clip,
+                         float &lut_scale) {
+    tw = w / tiles_x; th = hgt / tiles_y;
+    const int area = tw * th;
+    clip = std::max((int)(clip_limit * area / 256), 1);
+    lut_scale = 255.0f / (float)area;
+}
+
 // device-resident CLAHE of a w x h image (row stride w)
 static int clahe_device(Handle *h, const uint8_t *src, uint8_t *dst, uint8_t *lut, int w, int hgt, double clip_limit,
                         int tiles_x, int tiles_y) {
-    const int tw = w / tiles_x, th = hgt / tiles_y, area = tw * th;
-    const int clip = std::max((int)(clip_limit * area / 256), 1);
-    const float lut_scale = 255.0f / (float)area;
-    clahe_lut_kernel<<<tiles_x * tiles_y, 256, 0, h->stream>>>(src, w, tw, th, tiles_x, clip, lut_scale, lut);
+    int tw, th, clip;
+    float lut_scale;
+    clahe_params(w, hgt, clip_limit, tiles_x, tiles_y, tw, th, clip, lut_scale);
+    clahe_lut_kernel<false><<<tiles_x * tiles_y, 256, 0, h->stream>>>(src, w, tw, th, tiles_x, clip, lut_scale, lut, nullptr);
     dim3 b(32, 8), g((w + 31) / 32, (hgt + 7) / 8);
-    clahe_apply_kernel<<<g, b, 0, h->stream>>>(src, w, hgt, tw, th, tiles_x, tiles_y, lut, dst);
+    clahe_apply_kernel<false><<<g, b, 0, h->stream>>>(src, w, hgt, tw, th, tiles_x, tiles_y, lut, dst, nullptr);
     h->launches += 2;
     return 0;
 }
 
-__global__ void pyrdown_kernel(const uint8_t *src, int sw, int sh, uint8_t *dst, int dw, int dh) {
+// kBatch: level `level` of frame blockIdx.z of frames[] (frames with fewer levels exit) instead of the arguments
+template <bool kBatch>
+__global__ void pyrdown_kernel(const uint8_t *src, int sw, int sh, uint8_t *dst, int dw, int dh, const KltBatchFrame *frames,
+                               int level) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if constexpr (kBatch) {
+        const KltBatchFrame &f = frames[blockIdx.z];
+        if (level >= f.levels) return;
+        src = f.pyr + f.off[level - 1]; sw = f.w[level - 1]; sh = f.h[level - 1];
+        dst = f.pyr + f.off[level]; dw = f.w[level]; dh = f.h[level];
+    }
     if (x >= dw || y >= dh) return;
     const int k[5] = {1, 4, 6, 4, 1};
     int acc = 0;
@@ -152,9 +194,13 @@ __device__ __forceinline__ void bilinear_weights(float a, float b, int &w00, int
 
 __device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
 
+// kBatch: the points of all pairs of a batched call; point pt belongs to pair pair_of[pt], whose pyramids are
+// pairs[pair_of[pt]] (in device memory) instead of L, and the border test of that pair's frame size (border > 0) runs
+// here rather than in klt_border_kernel.
+template <bool kBatch>
 __global__ void __launch_bounds__(32 * kKltWarps)
 klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points,
-                 int max_iter, double eps2, float min_eig_thr) {
+                 int max_iter, double eps2, float min_eig_thr, const KltLevels *pairs, const int *pair_of, int border) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int pt = blockIdx.x * kKltWarps + warp;
     __shared__ int Ipatch[kKltWarps][24 * 24];
@@ -162,6 +208,7 @@ klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *s
     __shared__ short IWin[kKltWarps][kWin * kWin];
     __shared__ short dIWin[kKltWarps][kWin * kWin * 2];
     if (pt >= n_points) return;
+    const KltLevels &Lv = kBatch ? pairs[pair_of[pt]] : L;
     const float px0 = prev_pts[2 * pt], py0 = prev_pts[2 * pt + 1];
     float nx = next_pts[2 * pt], ny = next_pts[2 * pt + 1];      // OPTFLOW_USE_INITIAL_FLOW
     bool st = true;
@@ -170,12 +217,12 @@ klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *s
     int *Ip = Ipatch[warp];
     short *Dp = Dpatch[warp], *Iw = IWin[warp], *dIw = dIWin[warp];
 
-    for (int level = L.n - 1; level >= 0; --level) {
-        const uint8_t *I = L.I[level], *J = L.J[level];
-        const int cols = L.w[level], rows = L.h[level];
+    for (int level = Lv.n - 1; level >= 0; --level) {
+        const uint8_t *I = Lv.I[level], *J = Lv.J[level];
+        const int cols = Lv.w[level], rows = Lv.h[level];
         const float sc = (float)(1. / (1 << level));
         float ppx = px0 * sc, ppy = py0 * sc;
-        if (level == L.n - 1) { nx = nx * sc; ny = ny * sc; } else { nx = nx * 2.f; ny = ny * 2.f; }
+        if (level == Lv.n - 1) { nx = nx * sc; ny = ny * sc; } else { nx = nx * 2.f; ny = ny * 2.f; }
         ppx -= half; ppy -= half;
         const int ipx = (int)floorf(ppx), ipy = (int)floorf(ppy);
         if (ipx < -kWin || ipx >= cols || ipy < -kWin || ipy >= rows) {
@@ -284,24 +331,61 @@ klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *s
     }
     if (lane == 0) {
         next_pts[2 * pt] = nx; next_pts[2 * pt + 1] = ny;
-        status[pt] = st ? 1 : 0;
+        bool keep = st;
+        if (kBatch && border > 0) {           // klt_border_kernel's test on the pair's level-0 size
+            const int w = Lv.w[0], h = Lv.h[0];
+            if (nx < (float)border || nx >= (float)(w - border) || ny < (float)border || ny >= (float)(h - border)) keep = false;
+        }
+        status[pt] = keep ? 1 : 0;
         if (err) err[pt] = st ? err_out : 0.f;
     }
+}
+
+// cv::buildOpticalFlowPyramid halves first and drops the NEW level if it is not larger than the window: the number of
+// levels (level 0 included) a width x height frame gets for maxLevel max_level
+static int klt_levels(int width, int height, int max_level) {
+    int levels = 1, lw = width, lh = height;
+    while (levels <= max_level) {
+        lw = (lw + 1) / 2; lh = (lh + 1) / 2;
+        if (lw <= kWin || lh <= kWin) break;
+        ++levels;
+    }
+    return levels;
+}
+
+// the level sizes and offsets of an empty cache for w x hgt frames with `levels` levels
+static void klt_layout(KltPyramids &k, int w, int hgt, int levels) {
+    k.w = w; k.h = hgt; k.levels = levels;
+    size_t off = 0;
+    int lw = w, lh = hgt;
+    for (int l = 0; l < levels; ++l) {
+        k.lw[l] = lw; k.lh[l] = lh; k.off[l] = off;
+        off += ((size_t)lw * lh + 255) & ~(size_t)255;
+        lw = (lw + 1) / 2; lh = (lh + 1) / 2;
+    }
+    k.off[levels] = off;
+}
+
+// which pyramid of the cache takes which frame (pyr[slot[0]] prev, pyr[slot[1]] next): cached frames (same id, same
+// preprocessing) are neither uploaded nor rebuilt (have[i])
+static void klt_lookup(const KltPyramids &k, uint64_t prev_id, uint64_t next_id, double clahe_clip, int slot[2], bool have[2]) {
+    int sp = -1, sn = -1;
+    for (int i = 0; i < 2; ++i) {
+        if (prev_id && k.pyr_id[i] == prev_id && k.pyr_clahe[i] == clahe_clip) sp = i;
+        if (next_id && k.pyr_id[i] == next_id && k.pyr_clahe[i] == clahe_clip && i != sp) sn = i;
+    }
+    have[0] = sp >= 0; have[1] = sn >= 0;
+    if (!have[0]) sp = have[1] ? 1 - sn : 0;
+    if (!have[1]) sn = 1 - sp;
+    slot[0] = sp; slot[1] = sn;
 }
 
 static int klt_prepare(Handle *h, int w, int hgt, int max_level, int n_points) {
     KltState &k = h->klt;
     if (k.w != w || k.h != hgt || k.levels != max_level + 1 || k.cap_pts < n_points) {   // (drops the image cache)
         k = KltState{};
-        k.w = w; k.h = hgt; k.levels = max_level + 1; k.cap_pts = std::max(n_points, 1024);
-        size_t off = 0;
-        int lw = w, lh = hgt;
-        for (int l = 0; l <= max_level; ++l) {
-            k.lw[l] = lw; k.lh[l] = lh; k.off[l] = off;
-            off += ((size_t)lw * lh + 255) & ~(size_t)255;
-            lw = (lw + 1) / 2; lh = (lh + 1) / 2;
-        }
-        k.off[max_level + 1] = off;
+        klt_layout(k, w, hgt, max_level + 1);
+        k.cap_pts = std::max(n_points, 1024);
     }
     for (auto &p : k.pyr) TRY(reserve(h, p, k.off[k.levels], kDevice));
     TRY(reserve(h, k.pts, 5 * (size_t)k.cap_pts, kBoth));
@@ -320,31 +404,17 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
     if (do_clahe && (tiles_x < 1 || tiles_y < 1 || width % tiles_x || height % tiles_y))
         return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
     if (n_points == 0) return 0;
-    // cv::buildOpticalFlowPyramid halves first and drops the NEW level if it is not larger than the window
-    int levels = 1, lw = width, lh = height;
-    while (levels <= max_level) {
-        lw = (lw + 1) / 2; lh = (lh + 1) / 2;
-        if (lw <= kWin || lh <= kWin) break;
-        ++levels;
-    }
-    if (levels - 1 < max_level) max_level = levels - 1;
+    max_level = klt_levels(width, height, max_level) - 1;
     TRY(klt_prepare(h, width, height, max_level, n_points));
     KltState &k = h->klt;
     const size_t img_bytes = (size_t)width * height, cap = k.cap_pts;
     float *h_pts = k.pts.h, *d_prev = k.pts.d, *d_next = k.pts.d + 2 * cap, *d_err = k.pts.d + 4 * cap;
-    // which pyramid slot holds which frame: cached frames (same id, same preprocessing) are neither uploaded nor rebuilt
-    int sp = -1, sn = -1;
-    for (int i = 0; i < 2; ++i) {
-        if (prev_id && k.pyr_id[i] == prev_id && k.pyr_clahe[i] == clahe_clip) sp = i;
-        if (next_id && k.pyr_id[i] == next_id && k.pyr_clahe[i] == clahe_clip && i != sp) sn = i;
-    }
-    const bool have_prev = sp >= 0, have_next = sn >= 0;
-    if (!have_prev) sp = have_next ? 1 - sn : 0;
-    if (!have_next) sn = 1 - sp;
-    if ((!have_prev && !prev) || (!have_next && !next)) return fail(h, PVIO_B200_EINVAL, "klt: image not cached and no pixels given");
+    int slot[2];
+    bool have[2];
+    klt_lookup(k, prev_id, next_id, clahe_clip, slot, have);
+    const int sp = slot[0], sn = slot[1];
+    if ((!have[0] && !prev) || (!have[1] && !next)) return fail(h, PVIO_B200_EINVAL, "klt: image not cached and no pixels given");
     const uint8_t *src[2] = {prev, next};
-    const int slot[2] = {sp, sn};
-    const bool have[2] = {have_prev, have_next};
     for (int i = 0; i < 2; ++i) {
         if (have[i]) continue;
         for (int y = 0; y < height; ++y) memcpy(k.img.h + i * img_bytes + (size_t)y * width, src[i] + (size_t)y * stride, width);
@@ -367,7 +437,8 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
         }
         for (int l = 1; l <= max_level; ++l) {
             dim3 b(32, 8), g((k.lw[l] + 31) / 32, (k.lh[l] + 7) / 8);
-            pyrdown_kernel<<<g, b, 0, h->stream>>>(P + k.off[l - 1], k.lw[l - 1], k.lh[l - 1], P + k.off[l], k.lw[l], k.lh[l]);
+            pyrdown_kernel<false><<<g, b, 0, h->stream>>>(P + k.off[l - 1], k.lw[l - 1], k.lh[l - 1], P + k.off[l], k.lw[l], k.lh[l],
+                                                           nullptr, 0);
             ++h->launches;
         }
     }
@@ -383,8 +454,8 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
     }
     const int mi = std::min(std::max(max_iter, 0), 100);
     const double e = std::min(std::max(eps, 0.0), 10.0);
-    klt_track_kernel<<<(n_points + kKltWarps - 1) / kKltWarps, 32 * kKltWarps, 0, h->stream>>>(
-        L, d_prev, d_next, k.status.d, d_err, n_points, mi, e * e, 1e-4f);
+    klt_track_kernel<false><<<(n_points + kKltWarps - 1) / kKltWarps, 32 * kKltWarps, 0, h->stream>>>(
+        L, d_prev, d_next, k.status.d, d_err, n_points, mi, e * e, 1e-4f, nullptr, nullptr, 0);
     ++h->launches;
     if (border > 0) {
         klt_border_kernel<<<(n_points + 127) / 128, 128, 0, h->stream>>>(d_next, k.status.d, n_points, width, height, border);
@@ -404,6 +475,288 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
     memcpy(status, k.status.h, n_points);
     if (do_clahe && prev_eq) memcpy(prev_eq, k.img.h, img_bytes);
     if (do_clahe && next_eq) memcpy(next_eq, k.img.h + img_bytes, img_bytes);
+    return 0;
+}
+
+// ---- the batched tracker (pvio_b200_batch_track_keypoints) --------------------------------------------------------
+// n frame pairs of n sequences, each with its own pyramid cache (h->kltb.slots[pair.slot]).  Every pair is checked before
+// anything changes.  Then: one H2D copy of the packed staging; CLAHE (2 launches) and pyrDown (one launch per level)
+// over every new frame; LK + border over every point of every pair (1); per pair, the survivors compacted and OpenCV's
+// sample schedule drawn on the device (1); every RANSAC iteration of every pair (1); one D2H copy of the results and a
+// synchronise; the host replays each pair as fm_ransac_impl does; one launch writes every winner's mask, one D2H copy,
+// a synchronise.  Without CLAHE each new frame is copied into level 0 of its pyramid (a device copy per frame).
+namespace {
+constexpr int kMaxBatchPairs = 32767;         // grid y / z limits: one block row per pair, per new frame
+constexpr int kMaxBatchSlot = 65535;
+constexpr int kFmIters = 1000;                // findFundamentalMat's maxIters, as pvio_b200_track_keypoints passes it
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+}  // namespace
+
+int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_level, int max_iter, double eps,
+                     double clahe_clip, int tiles_x, int tiles_y, int border, double ransac_threshold,
+                     double ransac_confidence) {
+    if (n < 0 || n > kMaxBatchPairs) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad pair count");
+    if (n == 0) return 0;
+    if (!pairs || max_level < 0 || max_level >= kMaxLevels || border < 0 || !(clahe_clip >= 0.0))
+        return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad arguments");
+    const bool do_clahe = clahe_clip > 0.0;
+    if (do_clahe && (tiles_x < 1 || tiles_y < 1)) return fail(h, PVIO_B200_EINVAL, "clahe: bad tile grid");
+    KltBatchState &B = h->kltb;
+    struct Plan {
+        int levels, slot[2];                  // level count; which pyramid of the slot takes prev / next
+        bool have[2], rebuild;                // prev / next cached; the slot's buffers are rebuilt (its cache dropped)
+    };
+    std::vector<Plan> plan(n);
+    std::vector<uint8_t> taken;
+    const KltPyramids empty;
+    size_t n_pts = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_klt_pair &a = pairs[i];
+        if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: slot out of range");
+        if ((size_t)a.slot >= taken.size()) taken.resize(a.slot + 1, 0);
+        if (taken[a.slot]) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: a slot appears twice");
+        taken[a.slot] = 1;
+        if (a.width < 2 || a.height < 2 || a.stride < a.width || !a.prev_id || !a.next_id)
+            return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad shape, stride or frame id");
+        if (do_clahe && (a.width % tiles_x || a.height % tiles_y))
+            return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
+        if (a.n_points < 0 || (a.n_points > 0 && (!a.prev_pts || !a.next_pts || !a.status)))
+            return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad points");
+        Plan &pl = plan[i];
+        pl.levels = klt_levels(a.width, a.height, max_level);
+        const KltPyramids *c = (size_t)a.slot < B.slots.size() ? &B.slots[a.slot] : nullptr;
+        pl.rebuild = !c || c->w != a.width || c->h != a.height || c->levels != pl.levels;
+        klt_lookup(pl.rebuild ? empty : *c, a.prev_id, a.next_id, clahe_clip, pl.slot, pl.have);
+        if ((!pl.have[0] && !a.prev) || (!pl.have[1] && !a.next))
+            return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: image not cached in its slot and no pixels given");
+        n_pts += a.n_points;
+    }
+    if (n_pts > ((size_t)1 << 28)) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: too many points");
+
+    // the slots: grown on demand, rebuilt on a shape change; per pair its RANSAC budget (iterations reserved)
+    double thr = ransac_threshold, conf = ransac_confidence;
+    int fm_iters = kFmIters;
+    fm_options(thr, conf, fm_iters);
+    const int lmeds_iters = fm_lmeds_iters(conf, fm_iters);
+    if (taken.size() > B.slots.size()) B.slots.resize(taken.size());
+    std::vector<int> budget(n);
+    size_t n_frames = 0, pix_bytes = 0, budget_sum = 0, words_sum = 0, mask_words = 0;
+    int max_budget = 0, max_words = 0, max_levels = 1, lvw[kMaxLevels] = {}, lvh[kMaxLevels] = {};
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_klt_pair &a = pairs[i];
+        const Plan &pl = plan[i];
+        KltPyramids &s = B.slots[a.slot];
+        if (pl.rebuild) {
+            s = KltPyramids{};
+            klt_layout(s, a.width, a.height, pl.levels);
+        }
+        for (auto &p : s.pyr) TRY(reserve(h, p, s.off[s.levels], kDevice));
+        for (int side = 0; side < 2; ++side) {
+            if (pl.have[side]) continue;
+            ++n_frames;
+            pix_bytes += align256((size_t)a.width * a.height);
+            max_levels = std::max(max_levels, s.levels);
+            for (int l = 0; l < s.levels; ++l) { lvw[l] = std::max(lvw[l], s.lw[l]); lvh[l] = std::max(lvh[l], s.lh[l]); }
+        }
+        const int np = a.n_points, nw = (np + 31) / 32;
+        budget[i] = np < 8 ? 0 : np < 15 ? lmeds_iters : std::max(fm_iters, lmeds_iters);
+        budget_sum += budget[i];
+        words_sum += nw;
+        mask_words += (size_t)3 * budget[i] * nw;
+        max_budget = std::max(max_budget, budget[i]);
+        max_words = std::max(max_words, nw);
+    }
+
+    // staging (both sides): upload [o_lv, o_err) | download [o_next, o_mw) | masks [o_mw, o_job) | jobs (host side)
+    const size_t tiles = do_clahe ? (size_t)tiles_x * tiles_y : 0;
+    size_t o = 0;
+    const size_t o_lv = o;   o = align256(o + sizeof(KltLevels) * n);
+    const size_t o_fmp = o;  o = align256(o + sizeof(FmBatchProblem) * n);
+    const size_t o_frm = o;  o = align256(o + sizeof(KltBatchFrame) * n_frames);
+    const size_t o_pof = o;  o = align256(o + sizeof(int) * n_pts);
+    const size_t o_pix = o;  o += pix_bytes;
+    const size_t o_prev = o; o = align256(o + sizeof(float) * 2 * n_pts);
+    const size_t o_next = o; o = align256(o + sizeof(float) * 2 * n_pts);          // guesses in, positions out
+    const size_t o_err = o;  o = align256(o + sizeof(float) * n_pts);
+    const size_t o_st = o;   o = align256(o + n_pts);
+    const size_t o_surv = o; o = align256(o + sizeof(int) * 2 * n);
+    const size_t o_cnt = o;  o = align256(o + sizeof(int) * 4 * budget_sum);
+    const size_t o_mw = o;   o = align256(o + sizeof(unsigned) * words_sum);
+    const size_t o_job = o;  o = align256(o + sizeof(FmMaskJob) * n);
+    // device scratch: CLAHE tables | survivors p, q | schedules | models | per-iteration masks
+    size_t c = 0;
+    const size_t c_lut = c;   c = align256(c + tiles * 256 * n_frames);
+    const size_t c_pq = c;    c = align256(c + sizeof(float2) * 2 * n_pts);
+    const size_t c_sched = c; c = align256(c + sizeof(int) * 7 * budget_sum);
+    const size_t c_F = c;     c = align256(c + sizeof(double) * 27 * budget_sum);
+    const size_t c_masks = c; c = align256(c + sizeof(unsigned) * mask_words);
+    TRY(reserve(h, B.stage, o, kBoth));
+    TRY(reserve(h, B.scratch, std::max<size_t>(c, 256), kDevice));
+    uint8_t *hs = B.stage.h, *ds = B.stage.d, *dc = B.scratch.d;
+    KltLevels *lv = reinterpret_cast<KltLevels *>(hs + o_lv);
+    FmBatchProblem *fmp = reinterpret_cast<FmBatchProblem *>(hs + o_fmp);
+    KltBatchFrame *frm = reinterpret_cast<KltBatchFrame *>(hs + o_frm);
+    int *pof = reinterpret_cast<int *>(hs + o_pof);
+    float *h_prev = reinterpret_cast<float *>(hs + o_prev), *h_next = reinterpret_cast<float *>(hs + o_next);
+    size_t p = 0, f = 0, pix = 0, bsum = 0, msum = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_klt_pair &a = pairs[i];
+        const Plan &pl = plan[i];
+        KltPyramids &s = B.slots[a.slot];
+        KltLevels &L = lv[i];
+        memset(&L, 0, sizeof(L));
+        L.n = s.levels;
+        for (int l = 0; l < s.levels; ++l) {
+            L.I[l] = s.pyr[pl.slot[0]].d + s.off[l]; L.J[l] = s.pyr[pl.slot[1]].d + s.off[l];
+            L.w[l] = s.lw[l]; L.h[l] = s.lh[l];
+        }
+        const uint8_t *src[2] = {a.prev, a.next};
+        for (int side = 0; side < 2; ++side) {
+            if (pl.have[side]) continue;
+            uint8_t *dst = hs + o_pix + pix;
+            for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, src[side] + (size_t)y * a.stride, a.width);
+            KltBatchFrame &F = frm[f];
+            memset(&F, 0, sizeof(F));
+            F.raw = ds + o_pix + pix;
+            F.lut = dc + c_lut + f * tiles * 256;
+            F.pyr = s.pyr[pl.slot[side]].d;
+            F.levels = s.levels;
+            for (int l = 0; l < s.levels; ++l) { F.w[l] = s.lw[l]; F.h[l] = s.lh[l]; F.off[l] = s.off[l]; }
+            if (do_clahe) clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, F.tw, F.th, F.clip, F.lut_scale);
+            pix += align256((size_t)a.width * a.height);
+            ++f;
+        }
+        s.pyr_id[pl.slot[0]] = a.prev_id; s.pyr_clahe[pl.slot[0]] = clahe_clip;
+        s.pyr_id[pl.slot[1]] = a.next_id; s.pyr_clahe[pl.slot[1]] = clahe_clip;
+        const int np = a.n_points;
+        if (np > 0) {
+            memcpy(h_prev + 2 * p, a.prev_pts, sizeof(float) * 2 * np);
+            memcpy(h_next + 2 * p, a.next_pts, sizeof(float) * 2 * np);
+            std::fill(pof + p, pof + p + np, i);
+        }
+        FmBatchProblem &P = fmp[i];
+        P.prev_pts = reinterpret_cast<const float *>(ds + o_prev) + 2 * p;
+        P.next_pts = reinterpret_cast<const float *>(ds + o_next) + 2 * p;
+        P.status = ds + o_st + p;
+        P.p = reinterpret_cast<float2 *>(dc + c_pq) + p;
+        P.q = reinterpret_cast<float2 *>(dc + c_pq) + n_pts + p;
+        P.sched = reinterpret_cast<int *>(dc + c_sched) + 7 * bsum;
+        P.counts = reinterpret_cast<int *>(ds + o_cnt) + 4 * bsum;
+        P.F = reinterpret_cast<double *>(dc + c_F) + 27 * bsum;
+        P.masks = reinterpret_cast<unsigned *>(dc + c_masks) + msum;
+        P.surv = reinterpret_cast<int *>(ds + o_surv) + 2 * i;
+        P.n_pts = np;
+        P.budget = budget[i];
+        p += np;
+        bsum += budget[i];
+        msum += (size_t)3 * budget[i] * ((np + 31) / 32);
+    }
+
+    cudaStream_t st = h->stream;
+    CK(h, cudaMemcpyAsync(ds, hs, o_err, cudaMemcpyHostToDevice, st));
+    const KltBatchFrame *d_frm = reinterpret_cast<const KltBatchFrame *>(ds + o_frm);
+    const dim3 b2(32, 8);
+    if (n_frames > 0) {
+        const int nf = (int)n_frames;
+        if (do_clahe) {
+            clahe_lut_kernel<true><<<dim3((unsigned)tiles, nf), 256, 0, st>>>(nullptr, 0, 0, 0, tiles_x, 0, 0.f, nullptr, d_frm);
+            clahe_apply_kernel<true><<<dim3((lvw[0] + 31) / 32, (lvh[0] + 7) / 8, nf), b2, 0, st>>>(
+                nullptr, 0, 0, 0, 0, tiles_x, tiles_y, nullptr, nullptr, d_frm);
+            h->launches += 2;
+        } else {
+            for (size_t j = 0; j < n_frames; ++j)
+                CK(h, cudaMemcpyAsync(frm[j].pyr, frm[j].raw, (size_t)frm[j].w[0] * frm[j].h[0], cudaMemcpyDeviceToDevice, st));
+        }
+        for (int l = 1; l < max_levels; ++l) {
+            pyrdown_kernel<true><<<dim3((lvw[l] + 31) / 32, (lvh[l] + 7) / 8, nf), b2, 0, st>>>(nullptr, 0, 0, nullptr, 0, 0, d_frm, l);
+            ++h->launches;
+        }
+    }
+    float *d_next = reinterpret_cast<float *>(ds + o_next);
+    uint8_t *d_status = ds + o_st;
+    if (n_pts > 0) {
+        const int mi = std::min(std::max(max_iter, 0), 100);
+        const double e = std::min(std::max(eps, 0.0), 10.0);
+        klt_track_kernel<true><<<(unsigned)((n_pts + kKltWarps - 1) / kKltWarps), 32 * kKltWarps, 0, st>>>(
+            KltLevels{}, reinterpret_cast<const float *>(ds + o_prev), d_next, d_status, reinterpret_cast<float *>(ds + o_err),
+            (int)n_pts, mi, e * e, 1e-4f, reinterpret_cast<const KltLevels *>(ds + o_lv), reinterpret_cast<const int *>(ds + o_pof),
+            border);
+        ++h->launches;
+    }
+    const FmBatchProblem *d_fmp = reinterpret_cast<const FmBatchProblem *>(ds + o_fmp);
+    if (max_budget > 0) {
+        fm_batch_schedule(h, d_fmp, n, fm_iters, lmeds_iters);
+        fm_batch_hypotheses(h, d_fmp, n, max_budget, (float)(thr * thr));
+    }
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(hs + o_next, ds + o_next, o_mw - o_next, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaStreamSynchronize(st));
+
+    // LK results out; each pair's replay (opencv_image.cpp:112-129: findFundamentalMat over >= 8 survivors)
+    const float *r_next = reinterpret_cast<const float *>(hs + o_next), *r_err = reinterpret_cast<const float *>(hs + o_err);
+    const uint8_t *r_st = hs + o_st;
+    const int *r_surv = reinterpret_cast<const int *>(hs + o_surv), *r_cnt = reinterpret_cast<const int *>(hs + o_cnt);
+    FmMaskJob *jobs = reinterpret_cast<FmMaskJob *>(hs + o_job);
+    std::vector<int32_t> info(4 * (size_t)n);
+    bool any_job = false;
+    p = 0; bsum = 0;
+    size_t wsum = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_klt_pair &a = pairs[i];
+        const int np = a.n_points;
+        if (np > 0) {
+            memcpy(a.next_pts, r_next + 2 * p, sizeof(float) * 2 * np);
+            memcpy(a.status, r_st + p, np);
+            if (a.err) memcpy(a.err, r_err + p, sizeof(float) * np);
+        }
+        int32_t *inf = &info[4 * (size_t)i];
+        inf[0] = 0; inf[1] = -1; inf[2] = -1; inf[3] = 0;
+        FmMaskJob &J = jobs[i];
+        memset(&J, 0, sizeof(J));
+        const int s = budget[i] ? r_surv[2 * i] : 0, have = budget[i] ? r_surv[2 * i + 1] : 0;
+        if (s >= 8) {
+            float thr_lmeds = 0.f;
+            if (have > 0) thr_lmeds = fm_replay(r_cnt + 4 * bsum, s, have, fm_iters, conf, inf);
+            const int bi = inf[1], bk = inf[2];
+            if (have > 0 && bi >= 0) {
+                const FmBatchProblem &P = fmp[i];
+                J.p = P.p; J.q = P.q; J.n = s;
+                J.out = reinterpret_cast<unsigned *>(ds + o_mw) + wsum;
+                if (s >= 15) J.src = P.masks + (size_t)(3 * bi + bk) * ((s + 31) / 32);
+                else { J.F = P.F + (size_t)(3 * bi + bk) * 9; J.thr2 = thr_lmeds; }
+                any_job = true;
+            } else {
+                memset(a.status, 0, np);     // getSubset gave up at once, or no model won: the mask is all zero
+            }
+        }
+        p += np;
+        bsum += budget[i];
+        wsum += (np + 31) / 32;
+    }
+    if (any_job) {
+        FmMaskJob *d_jobs = nullptr;          // read in place from the pinned staging (mapped: unified addressing)
+        CK(h, cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_jobs), jobs, 0));
+        fm_batch_masks(h, d_jobs, n, max_words);
+        CK(h, cudaGetLastError());
+        CK(h, cudaMemcpyAsync(hs + o_mw, ds + o_mw, sizeof(unsigned) * words_sum, cudaMemcpyDeviceToHost, st));
+        CK(h, cudaStreamSynchronize(st));
+        const unsigned *r_mw = reinterpret_cast<const unsigned *>(hs + o_mw);
+        wsum = 0;
+        for (int i = 0; i < n; ++i) {
+            const pvio_b200_klt_pair &a = pairs[i];
+            if (jobs[i].n > 0) {
+                const unsigned *m = r_mw + wsum;
+                for (int j = 0, r = 0; j < a.n_points; ++j) {
+                    if (!a.status[j]) continue;
+                    if (!((m[r >> 5] >> (r & 31)) & 1u)) a.status[j] = 0;
+                    ++r;
+                }
+            }
+            wsum += (a.n_points + 31) / 32;
+        }
+    }
+    for (int i = 0; i < n; ++i)
+        if (pairs[i].info) memcpy(pairs[i].info, &info[4 * (size_t)i], sizeof(int32_t) * 4);
     return 0;
 }
 

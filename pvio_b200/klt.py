@@ -127,3 +127,50 @@ def track_keypoints_ransac(ba, prev_img, next_img, curr_keypoints, next_keypoint
               _lib._ptr(status, C.c_uint8), n, max_level, max_iter, eps, float(clahe_clip), clahe_tiles[0], clahe_tiles[1],
               int(border), float(ransac_threshold), float(ransac_confidence)))
     return nxt, status[:n]
+
+
+def pack_pairs(pairs):
+    """The pvio_b200_klt_pair array of a batched call (see batch_track_keypoints) and its output arrays: returns
+    (CKltPair array, outputs [(next_pts, status, err, info)] per pair, the arrays that must stay alive for the call)."""
+    n = len(pairs)
+    cp = (_lib.CKltPair * max(n, 1))()
+    outs, keep = [], []
+    for i, d in enumerate(pairs):
+        imgs = [None if d.get(k) is None else np.ascontiguousarray(d[k], dtype=np.uint8) for k in ("prev", "next")]
+        ref = imgs[1] if imgs[1] is not None else imgs[0]
+        h, w = ref.shape if ref is not None else d["shape"]
+        cur = np.ascontiguousarray(d["pts"], dtype=np.float32).reshape(-1, 2)
+        init = d.get("init")
+        nxt = cur.copy() if init is None or len(init) == 0 else np.array(init, dtype=np.float32, copy=True).reshape(-1, 2)
+        m = len(cur)
+        status = np.zeros(max(m, 1), dtype=np.uint8)
+        err = np.zeros(max(m, 1), dtype=np.float32)
+        info = np.zeros(4, dtype=np.int32)
+        c = cp[i]
+        c.slot, c.width, c.height, c.stride = int(d["slot"]), w, h, w
+        c.prev_id, c.next_id = int(d["prev_id"]), int(d["next_id"])
+        c.prev = None if imgs[0] is None else _lib._ptr(imgs[0], C.c_uint8)
+        c.next = None if imgs[1] is None else _lib._ptr(imgs[1], C.c_uint8)
+        c.n_points = m
+        c.prev_pts, c.next_pts = _lib._ptr(cur, C.c_float), _lib._ptr(nxt, C.c_float)
+        c.status, c.err, c.info = _lib._ptr(status, C.c_uint8), _lib._ptr(err, C.c_float), _lib._ptr(info, C.c_int32)
+        keep += [imgs, cur, nxt, status, err, info]
+        outs.append((nxt, status[:m], err[:m], info))
+    return cp, outs, keep
+
+
+def batch_track_keypoints(ba, pairs, max_level=3, max_iter=30, eps=0.01, clahe_clip=0.0, clahe_tiles=(8, 8), border=20,
+                          ransac_threshold=1.0, ransac_confidence=0.99):
+    """OpenCvImage::track_keypoints (opencv_image.cpp:88-136) for many sequences in one C-ABI call
+    (pvio_b200_batch_track_keypoints).  pairs: one dict per sequence with slot (its cache slot, distinct within the
+    call), prev_id / next_id (frame ids within the sequence, != 0), prev / next (uint8 [h, w] frames, raw when
+    clahe_clip > 0; None when the id is cached in the slot), pts (float32 [n, 2]), optionally init (the initial guess,
+    default pts) and shape ((h, w), needed when both frames are None).
+    Returns one (next_keypoints float32 [n, 2], status uint8 [n], err float32 [n], info int32 [4]) per pair; info as
+    find_fundamental_mask's (iterations, best iteration, best model, method), {0, -1, -1, 0} when RANSAC did not run."""
+    cp, outs, keep = pack_pairs(pairs)
+    ba._ck(ba.lib.pvio_b200_batch_track_keypoints(ba.h, len(pairs), cp, int(max_level), int(max_iter), float(eps),
+                                                  float(clahe_clip), int(clahe_tiles[0]), int(clahe_tiles[1]), int(border),
+                                                  float(ransac_threshold), float(ransac_confidence)))
+    del keep
+    return outs
