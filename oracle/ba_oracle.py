@@ -580,6 +580,26 @@ def landmark_postpass(win, st):
     return valid, quality
 
 
+def reprojection_error(win, st):
+    """BundleAdjustor::compute_reprojection_error (bundle_adjustor.cpp:321-336) over the window's landmarks, which are
+    the TF_VALID tracks the shim packs: the mean pixel error of every observation (anchor included) of every landmark.
+    No depth test: a landmark the post-pass would reject still counts, in the sum and in the count."""
+    fx, fy = win.K_fx, win.K_fy
+    qsum, qn = 0.0, 0
+    for l in range(win.M):
+        a = int(win.lm_anchor[l])
+        qa = qmul(st.q[a], win.cam_q_cs)
+        x = qrot(qa, np.array([win.lm_z_ref[l][0], win.lm_z_ref[l][1], 1.0])) / st.rho[l] + st.p[a] + qrot(st.q[a], win.cam_p_cs)
+        obs = [(a, win.lm_z_ref[l])] + [(int(win.obs_frame[k]), win.obs_z[k])
+                                        for k in range(int(win.lm_obs_begin[l]), int(win.lm_obs_begin[l + 1]))]
+        for f, z in obs:
+            y = qrot(qconj(qmul(st.q[f], win.cam_q_cs)), x - st.p[f] - qrot(st.q[f], win.cam_p_cs))
+            d = np.array([(y[0] / y[2] - z[0]) * fx, (y[1] / y[2] - z[1]) * fy])
+            qsum += np.sqrt(d @ d)
+            qn += 1
+    return qsum / max(qn, 1)
+
+
 # ----------------------------------------------------------------------- marginaliser
 def marginalize(win, st, index=0):
     """bundle_adjustor.cpp:348-599.  `win.lm_in_victim[M]` flags the landmarks observed by

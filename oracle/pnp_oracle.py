@@ -80,8 +80,9 @@ class PnpProblem:
 
 
 def pnp_solve(frame, last, imu, pts, zs, cam_q, cam_p, imu_q, imu_p, W, use_inertial=True, max_iter=10,
-              radius0=1.0e4, verbose=False):
-    """frame / last: 16-vectors (q xyzw, p, v, bg, ba).  Returns (frame', summary)."""
-    prob = PnpProblem(np.asarray(last, float), imu, pts, zs, cam_q, cam_p, imu_q, imu_p, W, use_inertial)
+              radius0=1.0e4, verbose=False, cauchy_a=1.0):
+    """frame / last: 16-vectors (q xyzw, p, v, bg, ba).  cauchy_a: the scale of the reprojection blocks' CauchyLoss.
+    Returns (frame', summary)."""
+    prob = PnpProblem(np.asarray(last, float), imu, pts, zs, cam_q, cam_p, imu_q, imu_p, W, use_inertial, cauchy_a)
     return bo.trust_region(prob.normal, prob.cost, prob.plus, prob.ambient, np.array(frame, float), prob.idx, 15,
                            max_iter, radius0, verbose)

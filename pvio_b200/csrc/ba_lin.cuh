@@ -60,10 +60,18 @@ struct ObsLin {            // linearisation of one observation in xi coordinates
     float cost;            // rho(s) / 2
 };
 
-// Evaluate one observation.  x: world point (fp64), xf: (float)x, cl: d x / d rho (fp32).
+// bt = Rwc_t^T (c_a - c_t): the anchor camera's centre in the target camera's axes (fp64, rounded once)
+__device__ __forceinline__ void baseline_in(const FrameSm &Ft, const FrameSm &Fa, float bt[3]) {
+    const double d0 = Fa.c[0] - Ft.c[0], d1 = Fa.c[1] - Ft.c[1], d2 = Fa.c[2] - Ft.c[2];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) bt[j] = (float)(Ft.Rwc[j] * d0 + Ft.Rwc[3 + j] * d1 + Ft.Rwc[6 + j] * d2);
+}
+
+// Evaluate one observation.  x: world point (fp64), xf: (float)x, ir = 1 / rho, bt = Rwc^T (c_anchor - c_target)
+// (the baseline in the target camera): d r / d rho = ir W dpi bt (see linearize_blk in ba_linearize.cuh).
 template <bool kLoss>
 __device__ __forceinline__ void linearize_obs(const FrameSm &F, const double x[3], const float xf[3],
-                                              const float cl[3], float zx, float zy,
+                                              float ir, const float bt[3], float zx, float zy,
                                               const float W[4], float cauchy_b, ObsLin &o) {
     const double d0 = x[0] - F.c[0], d1 = x[1] - F.c[1], d2 = x[2] - F.c[2];
     const double y0 = F.Rwc[0] * d0 + F.Rwc[3] * d1 + F.Rwc[6] * d2;
@@ -81,6 +89,8 @@ __device__ __forceinline__ void linearize_obs(const FrameSm &F, const double x[3
     const float A10 = W[2] * iz, A11 = W[3] * iz, A12 = -(W[2] * yx + W[3] * yy) * iz;
     // G = A * Rwc^T  ->  G[i][k] = sum_m A[i][m] Rwc[k][m]
     float G0[3], G1[3];
+    const float m0 = iz * ir * (bt[0] - yx * bt[2]), m1 = iz * ir * (bt[1] - yy * bt[2]);     // ir dpi bt
+    float j0 = W[0] * m0 + W[1] * m1, j1 = W[2] * m0 + W[3] * m1;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         G0[k] = A00 * F.R32[3 * k] + A01 * F.R32[3 * k + 1] + A02 * F.R32[3 * k + 2];
@@ -94,7 +104,7 @@ __device__ __forceinline__ void linearize_obs(const FrameSm &F, const double x[3
         const float t = 1.0f + s / cauchy_b;
         const float sc = rsqrtf(t);
         cost = 0.5f * cauchy_b * logf(t);
-        r0 *= sc; r1 *= sc;
+        r0 *= sc; r1 *= sc; j0 *= sc; j1 *= sc;
 #pragma unroll
         for (int k = 0; k < 3; ++k) { G0[k] *= sc; G1[k] *= sc; }
     } else {
@@ -109,8 +119,7 @@ __device__ __forceinline__ void linearize_obs(const FrameSm &F, const double x[3
     o.Y1[2] = G1[0] * xf[1] - G1[1] * xf[0];
 #pragma unroll
     for (int k = 0; k < 3; ++k) { o.Y0[3 + k] = G0[k]; o.Y1[3 + k] = G1[k]; }
-    o.j0 = G0[0] * cl[0] + G0[1] * cl[1] + G0[2] * cl[2];
-    o.j1 = G1[0] * cl[0] + G1[1] * cl[1] + G1[2] * cl[2];
+    o.j0 = j0; o.j1 = j1;
     o.r0 = r0; o.r1 = r1; o.cost = cost;
 }
 

@@ -10,7 +10,7 @@
 //
 // Work decomposition (third generation; the first two walked the table by landmark and paid a 31-shuffle
 // transpose-reduction per observation step):
-//   phase 0   thread per landmark: world point x_l (fp64) and d x / d rho into shared memory.
+//   phase 0   thread per landmark: world point x_l (fp64) and 1 / rho into shared memory.
 //   phase 1   the frame-major table (ba_fobs.cuh) is cut into rows of 32 entries of ONE (target, anchor)
 //             segment; a warp owns a contiguous range of rows.  Thread = residual block.  The target pose sits
 //             in registers for the whole segment; Y^T Y, Y^T r of the segment are REGISTER sums (float2
@@ -106,15 +106,18 @@ template <typename real>
 struct ObsL {                // linearisation of one residual block in xi coordinates (loss-corrected)
     typename Vec2<real>::type Y0[3], Y1[3];   // rows of Y = sqrt(rho') G X_l as pairs (0,1) (2,3) (4,5)
     real r0, r1;             // sqrt(rho') r
-    real j0, j1;             // sqrt(rho') G c_l  (d r / d rho)
+    real j0, j1;             // sqrt(rho') d r / d rho
     real cost;               // with the loss: t = 1 + s / b (the caller accumulates b/2 log t); without: s / 2
 };
 
 // reprojection_error_cost.h:58-117 in xi coordinates (see ba_lin.cuh).  x: world point (fp64), xf = (real)x,
-// cl = d x / d rho.
+// ir = 1 / rho, bt = Rwc^T (c_anchor - c_target) (the baseline in the target camera, fp64 rounded once).
+// d r / d rho = G d x / d rho = -ir W dpi Rwc^T (x - c_anchor) = ir W dpi bt, because dpi y = 0: the form
+// G . (d x / d rho) cancels to |bt| / depth of its terms and loses eps * depth / baseline in `real` (1e-4 of the
+// inverse-depth Jacobian at a 1/1000 baseline in fp32); dpi bt has no such cancellation.
 template <bool kLoss, typename real>
 __device__ __forceinline__ void linearize_blk(const FrameR<real> &F, double x0, double x1, double x2, real xf0, real xf1,
-                                              real xf2, real c0, real c1, real c2, float zx, float zy, const real (&W)[4],
+                                              real xf2, real ir, const real (&bt)[3], float zx, float zy, const real (&W)[4],
                                               bool diag_w, real inv_cauchy_b, ObsL<real> &o) {
     const double d0 = x0 - F.c[0], d1 = x1 - F.c[1], d2 = x2 - F.c[2];
     const double y0 = F.Rwc[0] * d0 + F.Rwc[3] * d1 + F.Rwc[6] * d2;
@@ -127,9 +130,11 @@ __device__ __forceinline__ void linearize_blk(const FrameR<real> &F, double x0, 
     const real yx = (real)y0 * iz, yy = (real)y1 * iz;
     // A = W dpi, dpi = [[iz, 0, -yx iz], [0, iz, -yy iz]];  G = A Rwc^T.  W = sqrt_inv_cov is diag(fx, fy) / sigma in the
     // reference (core/core.cpp:114-116): the diagonal case (uniform per window) skips the zero products
-    real r0, r1, G0[3], G1[3];
+    real r0, r1, G0[3], G1[3], j0, j1;
+    const real m0 = iz * ir * (bt[0] - yx * bt[2]), m1 = iz * ir * (bt[1] - yy * bt[2]);     // ir dpi bt
     if (diag_w) {
         r0 = W[0] * u0; r1 = W[3] * u1;
+        j0 = W[0] * m0; j1 = W[3] * m1;
         const real A00 = W[0] * iz, A02 = -A00 * yx, A11 = W[3] * iz, A12 = -A11 * yy;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
@@ -139,6 +144,8 @@ __device__ __forceinline__ void linearize_blk(const FrameR<real> &F, double x0, 
     } else {
         r0 = W[0] * u0 + W[1] * u1;
         r1 = W[2] * u0 + W[3] * u1;
+        j0 = W[0] * m0 + W[1] * m1;
+        j1 = W[2] * m0 + W[3] * m1;
         const real A00 = W[0] * iz, A01 = W[1] * iz, A02 = -(W[0] * yx + W[1] * yy) * iz;
         const real A10 = W[2] * iz, A11 = W[3] * iz, A12 = -(W[2] * yx + W[3] * yy) * iz;
 #pragma unroll
@@ -154,7 +161,7 @@ __device__ __forceinline__ void linearize_blk(const FrameR<real> &F, double x0, 
         const real t = (real)1 + s * inv_cauchy_b;
         const real sc = rsqrt_r(t);
         o.cost = t;
-        r0 *= sc; r1 *= sc;
+        r0 *= sc; r1 *= sc; j0 *= sc; j1 *= sc;
 #pragma unroll
         for (int k = 0; k < 3; ++k) { G0[k] *= sc; G1[k] *= sc; }
     } else {
@@ -167,8 +174,7 @@ __device__ __forceinline__ void linearize_blk(const FrameR<real> &F, double x0, 
     o.Y1[0] = mk2(G1[1] * xf2 - G1[2] * xf1, G1[2] * xf0 - G1[0] * xf2);
     o.Y1[1] = mk2(G1[0] * xf1 - G1[1] * xf0, G1[0]);
     o.Y1[2] = mk2(G1[1], G1[2]);
-    o.j0 = G0[0] * c0 + G0[1] * c1 + G0[2] * c2;
-    o.j1 = G1[0] * c0 + G1[1] * c1 + G1[2] * c2;
+    o.j0 = j0; o.j1 = j1;
     o.r0 = r0; o.r1 = r1;
 }
 
@@ -190,7 +196,7 @@ template <> struct LogAcc<double> {
 };
 
 // Per-landmark record of the linearise sweep in shared memory, 48 bytes = three 16-byte loads by the lane that owns an
-// observation of the landmark: world point x (fp64), (real) x, c = d x / d rho.
+// observation of the landmark: world point x (fp64), (real) x, c = (1 / rho, 0, 0).
 constexpr int kLmSm = 48;
 __device__ __forceinline__ void lm_sm_store(unsigned char *rec, double x0, double x1, double x2, float c0, float c1, float c2) {
     reinterpret_cast<double2 *>(rec)[0] = make_double2(x0, x1);
@@ -505,7 +511,7 @@ lin_obs_kernel(PipeArgs a_in) {
                 const double v1 = (Fa[3] * zx + Fa[4] * zy + Fa[5]) * ir;
                 const double v2 = (Fa[6] * zx + Fa[7] * zy + Fa[8]) * ir;
                 x0 = v0 + Fa[9]; x1 = v1 + Fa[10]; x2 = v2 + Fa[11];
-                c0 = (real)(-v0 * ir); c1 = (real)(-v1 * ir); c2 = (real)(-v2 * ir);
+                c0 = (real)ir;          // linearize_blk forms d r / d rho from 1 / rho and the segment's baseline
                 sk = 0;
             }
         }
@@ -542,13 +548,17 @@ lin_obs_kernel(PipeArgs a_in) {
         const int r_stop = min(min(r_end, srow[sp + 1]), cs.r + 64);      // pieces of <= 64 rows: <= 64 terms per thread in `real`
         const bool need = (((fixed >> t) & (fixed >> an)) & 1u) == 0u;    // both blocks constant: only H_ll, g_l, cost
         FrameR<real> F;
+        real bt[3];                   // Rwc_t^T (c_an - c_t): the segment's baseline in the target camera
         {
-            const double *Ft = Fs + t * 12;
+            const double *Ft = Fs + t * 12, *Fa = Fs + an * 12;
             const real *Rt = Rs + t * 12;
 #pragma unroll
             for (int i = 0; i < 9; ++i) { F.Rwc[i] = Ft[i]; F.R[i] = Rt[i]; }
 #pragma unroll
             for (int i = 0; i < 3; ++i) F.c[i] = Ft[9 + i];
+            const double d0 = Fa[9] - Ft[9], d1 = Fa[10] - Ft[10], d2 = Fa[11] - Ft[11];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) bt[j] = (real)(Ft[j] * d0 + Ft[3 + j] * d1 + Ft[6 + j] * d2);
         }
         const unsigned tM = (unsigned)t * (unsigned)a.Mcap;       // this segment's slice of the record arrays
         real2 q[15];
@@ -582,9 +592,9 @@ lin_obs_kernel(PipeArgs a_in) {
                 if (!(vo && skip[l])) {
                     ObsL<real> ol;
                     double x[3];
-                    real xf[3], cl[3];
-                    lm_sm_load(recs_a + (unsigned)l * kLmSm, x, xf, cl);
-                    linearize_blk<kLoss, real>(F, x[0], x[1], x[2], xf[0], xf[1], xf[2], cl[0], cl[1], cl[2], z.x, z.y, W,
+                    real xf[3], ir[3];             // ir = (1 / rho, 0, 0)
+                    lm_sm_load(recs_a + (unsigned)l * kLmSm, x, xf, ir);
+                    linearize_blk<kLoss, real>(F, x[0], x[1], x[2], xf[0], xf[1], xf[2], ir[0], bt, z.x, z.y, W,
                                                diag_w, inv_cb, ol);
                     if (kLoss) la.add(ol.cost); else cost_acc += ol.cost;
                     const unsigned rec = tM + (unsigned)l;

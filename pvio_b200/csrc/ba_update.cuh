@@ -363,13 +363,16 @@ jv_vision_kernel(UpdArgs a) {
         double x[3];
         float xf[3], cl[3];
         world_point(F[anchor], lr.zrx, lr.zry, rho[l], x, xf, cl);
+        const float ir = (float)(1.0 / rho[l]);
         // first pass: H_ll for the landmark's scaled direction, second pass: the products
         double hll = 0.0;
         for (unsigned j = 0, fm = lm_mask(lr.meta); j < (unsigned)n_obs; ++j, fm &= fm - 1) {
             const ObsRec o = obs[lr.obs_begin + j];
             const int of = __ffs(fm) - 1;
+            float bt[3];
+            baseline_in(F[of], F[anchor], bt);
             ObsLin ol;
-            linearize_obs<true>(F[of], x, xf, cl, o.zx, o.zy, W, cb, ol);
+            linearize_obs<true>(F[of], x, xf, ir, bt, o.zx, o.zy, W, cb, ol);
             hll += (double)(ol.j0 * ol.j0 + ol.j1 * ol.j1);
         }
         const double sc = lm_scale[l];
@@ -379,8 +382,10 @@ jv_vision_kernel(UpdArgs a) {
         for (unsigned j = 0, fm = lm_mask(lr.meta); j < (unsigned)n_obs; ++j, fm &= fm - 1) {
             const ObsRec o = obs[lr.obs_begin + j];
             const int of = __ffs(fm) - 1;
+            float bt[3];
+            baseline_in(F[of], F[anchor], bt);
             ObsLin ol;
-            linearize_obs<true>(F[of], x, xf, cl, o.zx, o.zy, W, cb, ol);
+            linearize_obs<true>(F[of], x, xf, ir, bt, o.zx, o.zy, W, cb, ol);
             double r0 = (double)ol.j0 * vl, r1 = (double)ol.j1 * vl;
 #pragma unroll
             for (int i = 0; i < 6; ++i) {

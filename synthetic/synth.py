@@ -77,14 +77,29 @@ def _sample_landmark(rng, cal, w, q_t, p_t, frames, dmin=2.0, dmax=10.0):
     raise RuntimeError("could not place a landmark")
 
 
-def _fill_observations(rng, cal, w, q_t, p_t, lm_frames):
+def _depth_ranges(M, depth_mix):
+    """Per-landmark (dmin, dmax) of a depth mixture [(fraction, dmin, dmax), ...]: the groups take consecutive
+    landmark indices in proportion to their fractions (no random draw, so the mixture leaves the RNG stream alone).
+    None: every landmark at 2-10 m."""
+    if depth_mix is None:
+        return [(2.0, 10.0)] * M
+    fr = np.array([g[0] for g in depth_mix], dtype=float)
+    edges = np.rint(np.cumsum(fr) / fr.sum() * M)
+    return [depth_mix[min(int(np.searchsorted(edges, l, side='right')), len(depth_mix) - 1)][1:] for l in range(M)]
+
+
+# 70 % of the landmarks at 2-10 m, 20 % at 20-60 m, 10 % at 60-400 m (beyond the post-pass's 50 m: rejected)
+DEPTH_MIX_OUTDOOR = ((0.7, 2.0, 10.0), (0.2, 20.0, 60.0), (0.1, 60.0, 400.0))
+
+
+def _fill_observations(rng, cal, w, q_t, p_t, lm_frames, depth_mix=None):
     """lm_frames: per-landmark sorted frame lists (anchor first).  Adds pixel noise."""
     fx, fy = cal['K'][0], cal['K'][1]
     s = np.sqrt(cal['noise_px2'])
     M = len(lm_frames)
     anchors, zrefs, begins, of, oz, rho_t = [], [], [0], [], [], []
-    for frames in lm_frames:
-        x, zr, d = _sample_landmark(rng, cal, w, q_t, p_t, frames)
+    for frames, (dmin, dmax) in zip(lm_frames, _depth_ranges(M, depth_mix)):
+        x, zr, d = _sample_landmark(rng, cal, w, q_t, p_t, frames, dmin, dmax)
         anchors.append(frames[0])
         zrefs.append(zr + rng.normal(0, s, 2) / np.array([fx, fy]))
         for f in frames[1:]:
@@ -119,11 +134,12 @@ def _perturb(rng, w, truth, sig_p=0.01, sig_th=np.deg2rad(0.5), sig_rho=0.05, si
     return st
 
 
-def make_cfg2(seed=648, N=10, M=500, staggered=False, cal=EUROC):
+def make_cfg2(seed=648, N=10, M=500, staggered=False, cal=EUROC, depth_mix=None, baseline=1.0):
     """BASELINE config 2: N keyframes x M landmarks, reprojection-only GN, frames 0 and 1
     FF_FIX_POSE (gauge + scale), every landmark anchored in frame 0 and seen in all frames
     (K_res = M(N-1)).  staggered=True is config 2b: landmark l first observed in frame
-    l mod 5, last in frame N-1."""
+    l mod 5, last in frame N-1.  depth_mix: landmark depths (see _depth_ranges); baseline
+    scales the frame positions (1e-3: a camera hovering at start-up)."""
     rng = np.random.default_rng(seed)
     w = _base_window(cal, N, use_inertial=False)
     w.frame_fixed[:2] = 1
@@ -134,12 +150,12 @@ def make_cfg2(seed=648, N=10, M=500, staggered=False, cal=EUROC):
         yaw = np.deg2rad(10.0) * k / max(N - 1, 1)
         Rz = np.array([[np.cos(yaw), -np.sin(yaw), 0.], [np.sin(yaw), np.cos(yaw), 0.], [0., 0., 1.]])
         q_t[k] = so3.mat2quat(Rz @ R_wb0)
-        p_t[k] = np.array([0.3 * np.sin(yaw) * 4.0, -0.25 * k, 0.02 * np.sin(0.7 * k)])
+        p_t[k] = baseline * np.array([0.3 * np.sin(yaw) * 4.0, -0.25 * k, 0.02 * np.sin(0.7 * k)])
     lm_frames = []
     for l in range(M):
         a = (l % min(5, N - 1)) if staggered else 0
         lm_frames.append(list(range(a, N)))
-    rho_t = _fill_observations(rng, cal, w, q_t, p_t, lm_frames)
+    rho_t = _fill_observations(rng, cal, w, q_t, p_t, lm_frames, depth_mix)
     truth = State(q_t, p_t, np.zeros((N, 3)), np.zeros((N, 3)), np.zeros((N, 3)), rho_t)
     w.validate()
     return w, _perturb(rng, w, truth), truth
@@ -200,9 +216,10 @@ def gauge_prior(w, st):
 
 
 def make_cfg3(seed=649, N=9, M=300, cal=EUROC, planes=0, tracks_per_plane=40, prior='synthetic',
-              kf_dt=0.25, imu_hz=200.0):
+              kf_dt=0.25, imu_hz=200.0, depth_mix=None):
     """BASELINE config 3 (planes=0) / config 4 (planes=2, TUM-VI calibration): full window
-    with reprojection + IMU pre-integration + marginalisation prior (+ plane factors)."""
+    with reprojection + IMU pre-integration + marginalisation prior (+ plane factors).
+    depth_mix: landmark depths (see _depth_ranges)."""
     rng = np.random.default_rng(seed)
     w = _base_window(cal, N, use_inertial=True)
     R_wb0 = R_WC0 @ so3.qmat(w.cam_q_cs).T
@@ -224,7 +241,7 @@ def make_cfg3(seed=649, N=9, M=300, cal=EUROC, planes=0, tracks_per_plane=40, pr
             a = 0               # plenty of victim-frame tracks for the marginaliser
             L = min(L, N)
         lm_frames.append(list(range(a, a + L)))
-    rho_t = _fill_observations(rng, cal, w, q_t, p_t, lm_frames)
+    rho_t = _fill_observations(rng, cal, w, q_t, p_t, lm_frames, depth_mix)
     truth = State(q_t, p_t, v_t, bg_t, ba_t, rho_t)
     st = _perturb(rng, w, truth)
     # IMU factors: synthetic gyro/accel at imu_hz, pre-integrated at the GUESS biases
@@ -320,6 +337,191 @@ def make_cfg4(seed=650, **kw):
     return make_cfg3(seed=seed, cal=TUMVI, planes=2, **kw)
 
 
+# ------------------------------------------------------------------ hard windows: post-transforms
+# Each takes a generated (Window, State guess, State truth) and returns new copies; the inputs are left alone.
+def _copies(w, st, truth):
+    import copy
+    return copy.deepcopy(w), st.copy(), copy.deepcopy(truth)
+
+
+def _px_offsets(rng, n, px, fx, fy):
+    """n displacements of uniform direction and a length uniform in px = (lo, hi) pixels, in normalised coordinates."""
+    ang = rng.uniform(0.0, 2.0 * np.pi, n)
+    r = rng.uniform(px[0], px[1], n)
+    return np.stack([r * np.cos(ang) / fx, r * np.sin(ang) / fy], axis=1)
+
+
+def with_outliers(w, st, truth, seed=0, frac=0.07, px=(15.0, 300.0), n_tracks=2):
+    """Mismatched keypoints: a fraction `frac` of the observations displaced by px pixels, and n_tracks whole tracks
+    with a wrong keypoint (a different one) in every observing frame.  Returns (w, st, truth, outlier observation mask)."""
+    w, st, truth = _copies(w, st, truth)
+    rng = np.random.default_rng(seed)
+    bad = np.zeros(w.K, dtype=bool)
+    bad[rng.choice(w.K, int(round(frac * w.K)), replace=False)] = True
+    nobs = np.diff(w.lm_obs_begin)
+    for l in rng.choice(np.nonzero(nobs >= 2)[0], n_tracks, replace=False):
+        bad[w.lm_obs_begin[l]:w.lm_obs_begin[l + 1]] = True
+    w.obs_z = w.obs_z.copy()
+    w.obs_z[bad] += _px_offsets(rng, int(bad.sum()), px, w.K_fx, w.K_fy)
+    return w, st, truth, bad
+
+
+def general_sqrt_info(w, sigma_px=None, ratio=1.6, corr=0.55, angle=0.5):
+    """A full 2x2 square-root information of correlated keypoint noise: the upper Cholesky factor U of
+    Lambda = Sigma^-1 (Sigma: sigma_px and ratio * sigma_px pixel deviations with correlation corr) turned by `angle`,
+    W = Rot(angle) U.  W^T W = Lambda as for U, but W is not symmetric and its two off-diagonals are non-zero and
+    different, so a transposed or swapped entry changes every residual."""
+    if sigma_px is None:
+        sigma_px = w.K_fx / w.sqrt_inv_cov[0, 0]
+    sx, sy = sigma_px / w.K_fx, ratio * sigma_px / w.K_fy
+    Sig = np.array([[sx * sx, corr * sx * sy], [corr * sx * sy, sy * sy]])
+    U = np.linalg.cholesky(np.linalg.inv(Sig)).T
+    c, s = np.cos(angle), np.sin(angle)
+    return np.array([[c, -s], [s, c]]) @ U
+
+
+def with_general_w(w, st, truth, **kw):
+    w, st, truth = _copies(w, st, truth)
+    w.sqrt_inv_cov = general_sqrt_info(w, **kw)
+    return w, st, truth
+
+
+def with_cauchy(w, st, truth, a):
+    w, st, truth = _copies(w, st, truth)
+    w.cauchy_a = float(a)
+    return w, st, truth
+
+
+FAR_OFFSET = np.array([4000.0, -3000.0, 120.0])      # 5.0 km from the world origin
+
+
+def with_offset(w, st, truth, offset=FAR_OFFSET):
+    """The whole window translated by `offset` (a long sequence far from its start): frame positions of the guess and
+    the truth, the prior's linearisation point, and each plane's distance (n.x = d becomes n.x = d + n.offset).  The
+    inverse-depth landmarks move with their anchors; IMU factors are translation invariant.  The plane factors are not:
+    the reference's functor regularises its point towards n.x = -d and measures n.x - d, so their cost changes."""
+    w, st, truth = _copies(w, st, truth)
+    o = np.asarray(offset, dtype=float)
+    st.p = st.p + o
+    truth.p = truth.p + o
+    if w.n_prior > 0:
+        w.prior_p0 = w.prior_p0 + o
+    if w.n_planes > 0:
+        w.plane_distance = w.plane_distance + w.plane_normal @ o
+    return w, st, truth
+
+
+def _anchor_point(w, st, l, rho):
+    a = int(w.lm_anchor[l])
+    qc, pc = _cam_pose(st.q[a], st.p[a], w)
+    return so3.qrot(qc, np.array([w.lm_z_ref[l][0], w.lm_z_ref[l][1], 1.0])) / rho + pc
+
+
+def with_rejected_landmarks(w, st, truth, seed=0, n_behind=3, n_far=3, far=(55.0, 90.0)):
+    """Landmarks the post-pass rejects: n_behind with an inverse depth of the wrong sign in the guess (behind the
+    anchor camera), n_far moved to far = (lo, hi) metres along their anchor ray, observations re-projected from the truth
+    poses with their pixel noise kept.  Returns (w, st, truth, behind indices, far indices)."""
+    w, st, truth = _copies(w, st, truth)
+    rng = np.random.default_rng(seed)
+    nobs = np.diff(w.lm_obs_begin)
+    pick = rng.choice(np.nonzero(nobs >= 1)[0], n_behind + n_far, replace=False)
+    behind, farl = np.sort(pick[:n_behind]), np.sort(pick[n_behind:])
+    st.rho[behind] = -st.rho[behind]
+    w.obs_z = w.obs_z.copy()
+    for l in farl:
+        d = rng.uniform(*far)
+        x_old, x_new = _anchor_point(w, truth, l, truth.rho[l]), _anchor_point(w, truth, l, 1.0 / d)
+        for k in range(int(w.lm_obs_begin[l]), int(w.lm_obs_begin[l + 1])):
+            f = int(w.obs_frame[k])
+            z_old, _ = _project(truth.q[f], truth.p[f], w, x_old)
+            z_new, _ = _project(truth.q[f], truth.p[f], w, x_new)
+            w.obs_z[k] = z_new + (w.obs_z[k] - z_old)
+        st.rho[l] = st.rho[l] / truth.rho[l] / d
+        truth.rho[l] = 1.0 / d
+    return w, st, truth, behind, farl
+
+
+def with_offplane_tracks(w, st, truth, seed=0, frac=0.3, dist=(0.3, 1.0)):
+    """Plane tracks of points off their plane (a wrong plane association): a fraction `frac` of the tracks moved by
+    dist = (lo, hi) metres along the plane normal, either side; the point is triangulated from the truth poses and the
+    observations, the observations are re-projected with their pixel noise kept.  Returns (w, st, truth, moved tracks,
+    signed displacements)."""
+    w, st, truth = _copies(w, st, truth)
+    rng = np.random.default_rng(seed)
+    n = int(round(frac * w.n_ptracks))
+    tracks = np.sort(rng.choice(w.n_ptracks, n, replace=False))
+    shift = rng.uniform(*dist, n) * rng.choice([-1.0, 1.0], n)
+    w.pt_obs_z = w.pt_obs_z.copy()
+    for t, dd in zip(tracks, shift):
+        ks = range(int(w.pt_obs_begin[t]), int(w.pt_obs_begin[t + 1]))
+        A, b = np.zeros((3, 3)), np.zeros(3)
+        for k in ks:                                         # least-squares intersection of the observation rays
+            qc, pc = _cam_pose(truth.q[w.pt_obs_frame[k]], truth.p[w.pt_obs_frame[k]], w)
+            u = so3.qrot(qc, np.array([w.pt_obs_z[k][0], w.pt_obs_z[k][1], 1.0]))
+            P = np.eye(3) - np.outer(u, u) / (u @ u)
+            A += P
+            b += P @ pc
+        x = np.linalg.solve(A, b)
+        x_new = x + dd * w.plane_normal[w.pt_plane[t]]
+        for k in ks:
+            f = int(w.pt_obs_frame[k])
+            z_old, _ = _project(truth.q[f], truth.p[f], w, x)
+            z_new, _ = _project(truth.q[f], truth.p[f], w, x_new)
+            w.pt_obs_z[k] = z_new + (w.pt_obs_z[k] - z_old)
+    return w, st, truth, tracks, shift
+
+
+
+def f32_keypoints(w):
+    """The keypoints rounded to fp32, as the device keeps them (the oracle then sees the values the kernels see)."""
+    w.obs_z = w.obs_z.astype(np.float32).astype(np.float64)
+    w.lm_z_ref = w.lm_z_ref.astype(np.float32).astype(np.float64)
+    w.pt_obs_z = w.pt_obs_z.astype(np.float32).astype(np.float64)
+    return w
+
+
+HARD_KINDS_VISUAL = ("far_depths", "low_baseline", "outliers", "general_w", "cauchy_0.3", "cauchy_0.01", "offset",
+                     "rejected", "all")
+HARD_KINDS_INERTIAL = ("far_depths", "outliers", "general_w", "cauchy_0.01", "offset", "rejected", "all")
+
+
+def hard_base(inertial, kind, N, M, seed):
+    """The generated window a hard kind starts from: cfg3 (inertial) or cfg2, with the outdoor depth mixture for
+    far_depths / all and a 1/1000 baseline for low_baseline."""
+    mix = DEPTH_MIX_OUTDOOR if kind in ("far_depths", "all") else None
+    if inertial:
+        return make_cfg3(N=N, M=M, seed=seed, depth_mix=mix)
+    return make_cfg2(N=N, M=M, seed=seed, depth_mix=mix, baseline=1e-3 if kind == "low_baseline" else 1.0)
+
+
+def hard_window(kind, inertial=False, N=8, M=200, seed=800):
+    """(Window, State) of one hard kind: plain, far_depths, low_baseline, outliers, general_w, cauchy_0.3,
+    cauchy_0.01, offset, rejected, or all (outliers, full W, Cauchy 0.3, rejected landmarks, 5 km offset on the
+    outdoor depth mixture), keypoints rounded to fp32."""
+    w, st, truth = hard_base(inertial, kind, N, M, seed)
+    if kind in ("plain", "far_depths", "low_baseline"):
+        pass                                    # made by the generator itself
+    elif kind == "outliers":
+        w, st, truth, _ = with_outliers(w, st, truth, seed=1)
+    elif kind == "general_w":
+        w, st, truth = with_general_w(w, st, truth)
+    elif kind in ("cauchy_0.3", "cauchy_0.01"):
+        w, st, truth, _ = with_outliers(w, st, truth, seed=2)
+        w, st, truth = with_cauchy(w, st, truth, float(kind.split("_")[1]))
+    elif kind == "offset":
+        w, st, truth = with_offset(w, st, truth)
+    elif kind == "rejected":
+        w, st, truth, _, _ = with_rejected_landmarks(w, st, truth, seed=3)
+    elif kind == "all":
+        w, st, truth, _ = with_outliers(w, st, truth, seed=4)
+        w, st, truth = with_general_w(w, st, truth)
+        w, st, truth = with_cauchy(w, st, truth, 0.3)
+        w, st, truth, _, _ = with_rejected_landmarks(w, st, truth, seed=5)
+        w, st, truth = with_offset(w, st, truth)
+    else:
+        raise ValueError(kind)
+    return f32_keypoints(w), st
+
 # ----------------------------------------------------------------------------- KLT inputs
 def _texture(rng, w, h):
     """Band-limited noise (sum of octaves), 8-bit, with good corners everywhere."""
@@ -375,10 +577,14 @@ def make_klt_pair(seed=648, size=(752, 480), n_points=500, max_shift=8.0):
 
 
 # ----------------------------------------------------------------------------- PnP inputs
-def make_pnp(seed=651, n_points=150, cal=EUROC, use_inertial=True, kf_dt=0.05, imu_hz=200.0):
+def make_pnp(seed=651, n_points=150, cal=EUROC, use_inertial=True, kf_dt=0.05, imu_hz=200.0, depth=(2.0, 10.0),
+             outlier_frac=0.0, outlier_px=(15.0, 300.0), W=None, cauchy_a=1.0, offset=None):
     """Inputs of visual_inertial_pnp (estimation/pnp.cpp:32-100): the last frame (constant), the new
     frame's predicted state, the IMU pre-integration between them and the world points of the tracks
-    both frames see, with pixel noise.  Returns a dict of arrays (16-vectors: q xyzw, p, v, bg, ba)."""
+    both frames see, with pixel noise.  Returns a dict of arrays (16-vectors: q xyzw, p, v, bg, ba).
+    Hard inputs: depth = (dmin, dmax) of the points; a fraction outlier_frac of the keypoints displaced by
+    outlier_px pixels; W a full 2x2 square-root information (general_sqrt_info); cauchy_a of the loss (the dict
+    carries it only when it is not 1); offset translates the scene (frames and points)."""
     rng = np.random.default_rng(seed)
     w = _base_window(cal, 2, use_inertial)
     R_wb0 = R_WC0 @ so3.qmat(w.cam_q_cs).T
@@ -407,7 +613,7 @@ def make_pnp(seed=651, n_points=150, cal=EUROC, use_inertial=True, kf_dt=0.05, i
     s_px = np.sqrt(cal['noise_px2'])
     pts, zs = [], []
     for _ in range(n_points):
-        x, _, _ = _sample_landmark(rng, cal, w, q_t, p_t, [0, 1])
+        x, _, _ = _sample_landmark(rng, cal, w, q_t, p_t, [0, 1], depth[0], depth[1])
         z, _ = _project(q_t[1], p_t[1], w, x)
         pts.append(x + rng.normal(0, 0.02, 3))                 # landmark estimate, not the true point
         zs.append(z + rng.normal(0, s_px, 2) / np.array([fx, fy]))
@@ -415,9 +621,22 @@ def make_pnp(seed=651, n_points=150, cal=EUROC, use_inertial=True, kf_dt=0.05, i
     guess[0:4] = so3.qnormalize(so3.qmul(truth[0:4], so3.qexp(rng.normal(0, np.deg2rad(0.7), 3))))
     guess[4:7] += rng.normal(0, 0.03, 3)
     guess[7:10] += rng.normal(0, 0.05, 3)
-    return dict(frame=guess, last=last, truth=truth, imu=imu, pts=np.array(pts), zs=np.array(zs),
-                cam_q=w.cam_q_cs, cam_p=w.cam_p_cs, imu_q=w.imu_q_cs, imu_p=w.imu_p_cs, W=w.sqrt_inv_cov,
-                use_inertial=use_inertial)
+    pts, zs = np.array(pts), np.array(zs)
+    if outlier_frac > 0:                                       # own stream: the draws above do not move
+        r2 = np.random.default_rng(seed + 7919)
+        bad = r2.choice(n_points, int(round(outlier_frac * n_points)), replace=False)
+        zs[bad] += _px_offsets(r2, len(bad), outlier_px, fx, fy)
+    if offset is not None:
+        o = np.asarray(offset, dtype=float)
+        for v in (guess, last, truth):
+            v[4:7] += o
+        pts = pts + o
+    d = dict(frame=guess, last=last, truth=truth, imu=imu, pts=pts, zs=zs,
+             cam_q=w.cam_q_cs, cam_p=w.cam_p_cs, imu_q=w.imu_q_cs, imu_p=w.imu_p_cs,
+             W=w.sqrt_inv_cov if W is None else np.asarray(W, dtype=float), use_inertial=use_inertial)
+    if cauchy_a != 1.0:
+        d['cauchy_a'] = float(cauchy_a)
+    return d
 
 
 def make_fm_matches(seed=652, n=300, outlier_frac=0.2, noise=0.3, planar=False, cal=EUROC):

@@ -283,9 +283,7 @@ def test_solve_matches_oracle_loop(ba, maker, kw):
 
 def test_reprojection_error(ba):
     w, st, _ = synth.make_cfg2(N=6, M=80)
-    valid, quality = bo.landmark_postpass(w, st)
-    n = np.diff(w.lm_obs_begin) + 1
-    ref = np.sum(quality * n) / np.sum(n)
+    ref = bo.reprojection_error(w, st)
     assert abs(ba.compute_reprojection_error(w, st) - ref) < 1e-6 * ref
 
 
