@@ -377,6 +377,38 @@ int pvio_b200_batch_track_keypoints(pvio_b200_handle h, int n, const pvio_b200_k
                                     int tiles_x, int tiles_y, int border,
                                     double ransac_threshold, double ransac_confidence);
 
+/* One frame of pvio_b200_batch_detect_keypoints: the arguments of one pvio_b200_detect_keypoints call. */
+typedef struct pvio_b200_detect_request {
+    int32_t slot;                  /* a sequence slot of pvio_b200_batch_track_keypoints, 0 .. 65535                  */
+    int32_t width, height, stride; /* width, height >= 8; stride >= width when the pixels are uploaded                */
+    uint64_t frame_id;             /* the frame's id within its slot's sequence (0: never cached)                     */
+    const uint8_t *image;          /* pixels (raw when clahe_clip > 0); NULL allowed when frame_id is cached in slot  */
+    const double *existing;        /* [n_existing][2] the frame's existing keypoints, pixels                          */
+    int32_t n_existing;
+    int32_t max_out;
+    double keypoint_distance;      /* Poisson-disk radius, > 0                                                        */
+    double *keypoints_out;         /* [max_out][2] out: the new keypoints in the reference's order                    */
+    int32_t *n_out;                /* out: their number                                                               */
+    float *gftt_out;               /* [1000][2] out, may be NULL: the GFTT corners before the Poisson filter          */
+    int32_t *n_gftt;               /* out, may be NULL: their number                                                  */
+} pvio_b200_detect_request;        /* 88 bytes on LP64 */
+
+/* pvio_b200_detect_keypoints for n frames in one call, e.g. the frame each sequence of a batched tracker call has just
+ * tracked into.  Each request gets bit for bit what pvio_b200_detect_keypoints gives for that frame: the same keypoints
+ * and GFTT corners in the same order.  clahe_clip and the tile grid are shared.
+ * Frame source: level 0 of the pyramid in the request's slot of pvio_b200_batch_track_keypoints is used when
+ * (frame_id, clahe_clip) is cached in that slot -- either of the slot's two cached frames -- and the shape matches;
+ * otherwise `image` is uploaded, and equalised on the device when clahe_clip > 0 (the size must then be a multiple of
+ * the tile grid).  The call changes no cache, neither the slots nor the single calls' cache, so several requests may
+ * name the same slot.
+ * Every request is checked before anything is staged: on an argument error PVIO_B200_EINVAL is returned and no output
+ * has changed.  A request whose keypoints do not fit gets its first max_out keypoints and *n_out = its full count (at
+ * most 1000), as the single call, and the call returns PVIO_B200_EINVAL after every request has its results.  n == 0 is
+ * a no-op.  A call runs CLAHE (uploaded frames only), Harris, non-maximum suppression, a segmented sort and the two
+ * greedy passes as at most 6 kernel launches whatever n is, with one upload, one download and one synchronisation. */
+int pvio_b200_batch_detect_keypoints(pvio_b200_handle h, int n, const pvio_b200_detect_request *requests,
+                                     double clahe_clip, int tiles_x, int tiles_y);
+
 /* CLAHE of one frame (same kernels); dst is [height][width]. */
 int pvio_b200_clahe(pvio_b200_handle h, const uint8_t *src, int width, int height, int stride, double clip_limit,
                     int tiles_x, int tiles_y, uint8_t *dst);

@@ -70,6 +70,13 @@ class CKltPair(C.Structure):
                 ("err", c_f32p), ("info", c_i32p)]
 
 
+class CDetectRequest(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32),
+                ("frame_id", C.c_uint64), ("image", c_u8p), ("existing", c_f64p), ("n_existing", C.c_int32),
+                ("max_out", C.c_int32), ("keypoint_distance", C.c_double), ("keypoints_out", c_f64p), ("n_out", c_i32p),
+                ("gftt_out", c_f32p), ("n_gftt", c_i32p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -84,6 +91,7 @@ EXPORTS = [
     "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
     "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
     "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve", "pvio_b200_batch_track_keypoints",
+    "pvio_b200_batch_detect_keypoints",
 ]
 
 _lib = None
@@ -136,6 +144,7 @@ def load():
                                               C.POINTER(COptions), C.POINTER(CSummary)]
     lib.pvio_b200_batch_track_keypoints.argtypes = [vp, C.c_int, C.POINTER(CKltPair), C.c_int, C.c_int, C.c_double,
                                                     C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
+    lib.pvio_b200_batch_detect_keypoints.argtypes = [vp, C.c_int, C.POINTER(CDetectRequest), C.c_double, C.c_int, C.c_int]
     lib.pvio_b200_klt_track.argtypes = [vp, c_u8p, c_u8p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p,
                                         C.c_int, C.c_int, C.c_int, C.c_double]
     for name in EXPORTS:

@@ -1361,6 +1361,13 @@ int pvio_b200_batch_track_keypoints(pvio_b200_handle hh, int n, const pvio_b200_
                             ransac_confidence);
 }
 
+int pvio_b200_batch_detect_keypoints(pvio_b200_handle hh, int n, const pvio_b200_detect_request *requests, double clahe_clip,
+                                     int tiles_x, int tiles_y) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return batch_detect_impl(h, n, requests, clahe_clip, tiles_x, tiles_y);
+}
+
 int pvio_b200_clahe(pvio_b200_handle hh, const uint8_t *src, int width, int height, int stride, double clip_limit,
                     int tiles_x, int tiles_y, uint8_t *dst) {
     Handle *h = reinterpret_cast<Handle *>(hh);

@@ -67,6 +67,19 @@ struct KltState : KltPyramids {
     DevBuf<uint8_t> img;                      // pinned staging for both level-0 images
 };
 
+// one frame a batched call equalises or downsamples on the device (klt.cu: batch_track_impl, detect.cu:
+// batch_detect_impl): its raw pixels, CLAHE into level 0 of `pyr`, then pyrDown level by level
+struct KltBatchFrame {
+    const uint8_t *raw;                       // level-0 pixels as uploaded (raw when CLAHE runs)
+    uint8_t *lut;                             // [tiles][256] its CLAHE tables
+    uint8_t *pyr;                             // its pyramid (the detector: level 0 only, in its scratch)
+    int levels, tw, th, clip;
+    float lut_scale;
+    int w[kMaxLevels], h[kMaxLevels];
+    size_t off[kMaxLevels];
+};
+constexpr int kMaxBatchSlot = 65535;          // the sequence slots of the batched calls: 0 .. kMaxBatchSlot
+
 // the batched tracker (pvio_b200_batch_track_keypoints): one pyramid cache per sequence slot, grown on demand, and
 // the buffers of one call, grown to the largest call seen
 struct KltBatchState {
@@ -88,6 +101,14 @@ struct DetectState {
     DevBuf<unsigned long long> keys_sorted;   // both sides
     DevBuf<int> counters;                     // both sides: [0] max response bits, [1] candidate count
     DevBuf<uint8_t> cub_tmp;
+};
+
+// detect.cu: the batched detector (pvio_b200_batch_detect_keypoints); both grown to the largest call seen
+struct DetectBatchState {
+    DevBuf<uint8_t> stage;                    // both sides: descriptors, counters, existing points, uploaded pixels |
+                                              // per-request results
+    DevBuf<uint8_t> scratch;                  // device: responses, keys, sorted keys, equalised frames, CLAHE tables,
+                                              // sort temporaries, select working areas that do not fit on chip
 };
 
 // fmat.cu: RANSAC buffers, grown to the largest point count / iteration budget seen
@@ -142,6 +163,7 @@ struct Handle {
                                                   // device (0: none); a pack naming it with prior_S == NULL keeps it, a host prior clears it
     std::unique_ptr<ResidentWindow> resident;     // resident.cu (null until pvio_b200_window_reset)
     DetectState detect;                           // detect.cu
+    DetectBatchState detectb;                     // detect.cu: the batched detector, independent of detect
     size_t sys_set = 0;                           // elements between the two buffer sets of the reduced-system arrays (LinBufs)
     int sm_count = 132;                           // set from the device at create
     int smem_lim = 0;                             // dynamic shared memory the large-layout kernels opt in to (create)
@@ -290,6 +312,12 @@ int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, dou
 // klt.cu / detect.cu
 const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int height, double clahe_clip);
 int klt_clahe_device(Handle *h, const uint8_t *d_src, uint8_t *d_dst, uint8_t *d_lut, int width, int height, double clip, int tiles_x, int tiles_y);
+// klt.cu, used by detect.cu: cv::CLAHE's per-tile constants of a w x h frame, and CLAHE of n_frames frames (frames in
+// device memory; each equalises raw into level 0 of pyr) as 2 launches whose grids cover max_w x max_h
+void klt_clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_y, int &tw, int &th, int &clip, float &lut_scale);
+void klt_batch_clahe(Handle *h, const KltBatchFrame *frames, int n_frames, int tiles_x, int tiles_y, int max_w, int max_h);
+// detect.cu: pvio_b200_batch_detect_keypoints
+int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, double clahe_clip, int tiles_x, int tiles_y);
 // ba_marg.cu
 int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
                      double *S_out, double *e_out, double *H_out, double *b_out);

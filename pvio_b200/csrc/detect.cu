@@ -18,11 +18,16 @@
 // ~4e-7 relative, and the SELECTED corner set is compared with cv2.goodFeaturesToTrack(useHarrisDetector=True) as a set:
 // identical on every test image; a difference could only arise where two responses lie within that rounding.
 #include <algorithm>
+#include <cassert>
+#include <climits>
+#include <cmath>
 #include <cstring>
 #include <unordered_map>
 #include <vector>
 
 #include <cub/cub.cuh>
+#include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 
 #include "api_internal.h"
 
@@ -32,12 +37,42 @@ namespace {
 __device__ __forceinline__ int refl(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 constexpr int kTX = 32, kTY = 16;
+constexpr int kMaxCorners = 1000;             // GFTTDetector::create(1000, ...)
+
+// the per-request results of a batched call (batch_detect_impl), downloaded in one copy
+struct DetectResult {
+    int n_gftt, pad;
+    unsigned mask[(kMaxCorners + 31) / 32];   // bit j: corner j passes the Poisson filter and the 20-pixel border
+    unsigned corner[kMaxCorners];             // the GFTT corners in order, as pixel indices y * w + x
+};
+
+// one frame of a batched call, as the kernels read it
+struct DetectBatchFrame {
+    const uint8_t *img;                       // the equalised frame (a cached level 0, uploaded pixels, or CLAHE output)
+    float *resp;                              // [h][w] Harris response
+    unsigned long long *keys, *sorted;        // its segment of the candidate keys, unsorted / sorted descending
+    int *counters;                            // [2] max response bits, candidate count
+    const double2 *pre;                       // [n_pre] the existing keypoints a corner's Poisson walk can meet, in order
+    uint8_t *work;                            // the select kernel's working area in global memory, or nullptr: on chip
+    DetectResult *res;
+    double gs, r2;                            // Poisson cell size r / sqrt(2) and r^2
+    int w, h, cap, key_off;                   // key_off: the segment's first key
+    int n_pre, gw, gh, hbits;                 // min-distance grid gw x gh; Poisson hash table of 2^hbits cells
+};
 
 // one thread per pixel; the (kTX + 2) x (kTY + 2) tile of the three products in shared memory.  Every operation is a
 // separately rounded fp32 operation except the one fused multiply-add of the Sobel-x column pass (this file is
-// compiled with -fmad=false).
-__global__ void __launch_bounds__(kTX *kTY) harris_response_kernel(const uint8_t *img, int w, int h, float k, float *resp, int *max_bits) {
+// compiled with -fmad=false).  kBatch: frame blockIdx.z of frames[] instead of the arguments (blocks outside a smaller
+// frame exit).
+template <bool kBatch>
+__global__ void __launch_bounds__(kTX *kTY) harris_response_kernel(const uint8_t *img, int w, int h, float k, float *resp, int *max_bits,
+                                                                   const DetectBatchFrame *frames) {
     __shared__ float cxx[kTY + 2][kTX + 2], cxy[kTY + 2][kTX + 2], cyy[kTY + 2][kTX + 2];
+    if constexpr (kBatch) {
+        const DetectBatchFrame &f = frames[blockIdx.z];
+        img = f.img; w = f.w; h = f.h; resp = f.resp; max_bits = f.counters;
+        if ((int)blockIdx.x * kTX >= w || (int)blockIdx.y * kTY >= h) return;     // block-uniform
+    }
     const int x0 = blockIdx.x * kTX, y0 = blockIdx.y * kTY, tid = threadIdx.y * kTX + threadIdx.x;
     // the box filter's border pixel is the product AT the mirror pixel: evaluate the products at reflected coordinates
     for (int e = tid; e < (kTY + 2) * (kTX + 2); e += kTX * kTY) {
@@ -84,8 +119,14 @@ __global__ void __launch_bounds__(kTX *kTY) harris_response_kernel(const uint8_t
     if (r > 0.0f) atomicMax(max_bits, __float_as_int(r));       // positive floats order like their bit patterns
 }
 
+// kBatch: frame blockIdx.z of frames[] instead of the arguments; its keys go to its own segment
+template <bool kBatch>
 __global__ void nms_compact_kernel(const float *resp, int w, int h, double quality, const int *max_bits, unsigned long long *keys,
-                                   int *count, int cap) {
+                                   int *count, int cap, const DetectBatchFrame *frames) {
+    if constexpr (kBatch) {
+        const DetectBatchFrame &f = frames[blockIdx.z];
+        resp = f.resp; w = f.w; h = f.h; max_bits = f.counters; keys = f.keys; count = f.counters + 1; cap = f.cap;
+    }
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x < 1 || y < 1 || x >= w - 1 || y >= h - 1) return;      // goodFeaturesToTrack visits interior pixels only
     const float mx = __int_as_float(*max_bits);
@@ -163,13 +204,16 @@ struct PoissonFilter {
     }
 };
 
+// local maxima of a 3x3 test: at most one per 2x2 block
+int candidate_cap(size_t px) { return (int)std::min<size_t>(px / 4 + 1024, (size_t)1 << 22); }
+
 int ensure(Handle *h, int w, int hgt) {
     DetectState &d = h->detect;
     const size_t px = (size_t)w * hgt;
     if (d.w != w || d.h != hgt) {
         d = DetectState{};
         d.w = w; d.h = hgt;
-        d.cap = (int)std::min<size_t>(px / 4 + 1024, (size_t)1 << 22);       // local maxima of a 3x3 test: at most one per 2x2 block
+        d.cap = candidate_cap(px);
         cub::DeviceRadixSort::SortKeysDescending(nullptr, d.cub_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr, d.cap);
     }
     TRY(reserve(h, d.img, px, kBoth));
@@ -182,7 +226,389 @@ int ensure(Handle *h, int w, int hgt) {
     return 0;
 }
 
+// ---- the batched detector (pvio_b200_batch_detect_keypoints) -------------------------------------------------------
+// n frames, each cached in a slot of the batched tracker or uploaded.  Every request is checked before anything is
+// staged.  Then: one H2D copy of the packed staging (descriptors, zeroed counters, existing points, uploaded pixels);
+// CLAHE over the uploaded frames (2 launches, clahe_clip > 0 only); Harris and NMS over every frame, grid z = frame
+// (2); a segmented descending radix sort of each frame's keys, whose segment ends are read on the device (1);
+// detect_select_kernel, one CTA per frame running both greedy passes (1); one D2H copy of the results, a synchronise.
+constexpr int kMinDist = 20;                  // GFTT's minDistance, and the cell of its grid (lround(20))
+constexpr int kCellEmpty = -(1 << 30);        // x of an empty min-distance slot: farther than 20 px from every pixel
+constexpr unsigned long long kHashEmpty = ~0ull;
+constexpr double kCellLimit = 1073741824.0;   // 2^30: the Poisson cell indices the host pass forms without int overflow
+constexpr int kSelectThreads = 128;
+constexpr size_t kSelectSmem = 96 * 1024;     // larger working areas go to global memory
+constexpr int kMaxBatchDetect = 65535;        // grid z: one layer per frame
+
+// min_distance_select's distance test: float dx^2 + dy^2 against 20^2
+__device__ __forceinline__ bool md_close(int x, int y, int px, int py) {
+    const float dx = (float)x - (float)px, dy = (float)y - (float)py;
+    return dx * dx + dy * dy < 400.0f;
+}
+
+// Poisson cells (ix, iy) >= (-2, -2) as hash keys; never kHashEmpty
+__device__ __forceinline__ unsigned long long cell_key(long long ix, long long iy) {
+    return ((unsigned long long)(ix + 8) << 32) | (unsigned long long)(iy + 8);
+}
+__device__ __forceinline__ unsigned long long hash_slot(unsigned long long key, int hbits) {
+    return (key * 0x9E3779B97F4A7C15ull) >> (64 - hbits);
+}
+__device__ int hash_find(const unsigned long long *hk, const int *hv, int hbits, unsigned long long key) {
+    const unsigned long long m = (1ull << hbits) - 1;
+    for (unsigned long long s = hash_slot(key, hbits);; s = (s + 1) & m) {
+        const unsigned long long k = hk[s];
+        if (k == key) return hv[s];
+        if (k == kHashEmpty) return -1;
+    }
+}
+
+// The two greedy passes of pvio_b200_detect_keypoints (min_distance_select, PoissonFilter, the border) for frame
+// blockIdx.x, with exactly their semantics.  Working area (shared memory, or f.work when it does not fit there):
+//   grid     [gh][gw] int4: the min-distance grid, two (x, y) slots per 20 x 20 cell.  Two slots suffice: accepted
+//            corners are >= 20 px apart, the integer pixels of one cell differ by <= 19 per axis, and 3 points in a
+//            square of side 19 are at most (sqrt(6) - sqrt(2)) * 19 = 19.67 px apart.
+//   corners  [1000] float2: the accepted corners in order
+//   hk, hv   the Poisson grid as an open-addressing hash table of 2^hbits cells (>= twice the points it can hold):
+//            cell -> index of the LAST point inserted into it (presets: their index; corner j: n_pre + j)
+// All warps initialise the area and insert the presets; warp 0 then runs the passes.
+//   min distance  32 sorted candidates per step: each lane tests its candidate against the grid, the chunk is then
+//                 resolved in lane order (the host's order) with shuffles: lane k is accepted if it passed and no
+//                 accepted earlier lane of the chunk is closer than 20 px.  Within 20 px means within the 3 x 3 cells
+//                 the host examines, so the two tests agree.  Stops at 1000 corners.
+//   Poisson       corner by corner: lane t examines cell t + 1 of the reference's walk over the 5 x 5 block (which
+//                 skips the block's first cell and examines the one past its end), then a vote; an accepted corner
+//                 overwrites its cell and is kept if it lies inside the 20-px border.
+__global__ void __launch_bounds__(kSelectThreads) detect_select_kernel(const DetectBatchFrame *frames) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const DetectBatchFrame &f = frames[blockIdx.x];
+    uint8_t *work = f.work ? f.work : smem;
+    const int ncell = f.gw * f.gh, tid = threadIdx.x;
+    const unsigned long long hcap = 1ull << f.hbits;
+    int4 *grid = reinterpret_cast<int4 *>(work);
+    float2 *corners = reinterpret_cast<float2 *>(work + sizeof(int4) * (size_t)ncell);
+    unsigned long long *hk = reinterpret_cast<unsigned long long *>(corners + kMaxCorners);
+    int *hv = reinterpret_cast<int *>(hk + hcap);
+    DetectResult *res = f.res;
+    for (int c = tid; c < ncell; c += kSelectThreads) grid[c] = make_int4(kCellEmpty, 0, kCellEmpty, 0);
+    for (unsigned long long s = tid; s < hcap; s += kSelectThreads) { hk[s] = kHashEmpty; hv[s] = -1; }
+    for (int j = tid; j < (kMaxCorners + 31) / 32; j += kSelectThreads) res->mask[j] = 0;
+    __syncthreads();
+    const unsigned long long hm = hcap - 1;
+    const double gs = f.gs;
+    for (int i = tid; i < f.n_pre; i += kSelectThreads) {          // the last preset of a cell holds it: the largest index
+        const double2 p = f.pre[i];
+        const unsigned long long key = cell_key((long long)floor(p.x / gs), (long long)floor(p.y / gs));
+        for (unsigned long long s = hash_slot(key, f.hbits);; s = (s + 1) & hm) {
+            const unsigned long long k = atomicCAS(&hk[s], kHashEmpty, key);
+            if (k == kHashEmpty || k == key) { atomicMax(&hv[s], i); break; }
+        }
+    }
+    __syncthreads();
+    if (tid >= 32) return;
+    const int lane = tid, w = f.w, hgt = f.h, gw = f.gw, gh = f.gh;
+
+    // cv::goodFeaturesToTrack's minimum-distance pass over the sorted candidates
+    const int nk = min(f.counters[1], f.cap);
+    const unsigned long long *keys = f.sorted;
+    int ng = 0;
+    for (int base = 0; base < nk && ng < kMaxCorners; base += 32) {
+        const int i = base + lane;
+        int x = 0, y = 0;
+        unsigned idx = 0;
+        bool ok = false;
+        if (i < nk) {
+            idx = (unsigned)(keys[i] & 0xffffffffull);
+            y = (int)(idx / (unsigned)w); x = (int)(idx - (unsigned)y * (unsigned)w);
+            const int xc = x / kMinDist, yc = y / kMinDist;
+            ok = true;
+            for (int yy = max(0, yc - 1); yy <= min(gh - 1, yc + 1); ++yy)
+                for (int xx = max(0, xc - 1); xx <= min(gw - 1, xc + 1); ++xx) {
+                    const int4 c = grid[yy * gw + xx];
+                    if (md_close(x, y, c.x, c.y) || md_close(x, y, c.z, c.w)) ok = false;
+                }
+        }
+        const unsigned passed = __ballot_sync(0xffffffffu, ok);
+        if (!passed) continue;
+        unsigned conf = 0;                                          // passed earlier lanes closer than 20 px
+        for (int k = 0; k < 31; ++k) {
+            const int xk = __shfl_sync(0xffffffffu, x, k), yk = __shfl_sync(0xffffffffu, y, k);
+            if (k < lane && ((passed >> k) & 1u) && md_close(x, y, xk, yk)) conf |= 1u << k;
+        }
+        unsigned acc = 0;
+        int nacc = 0;
+        const int room = kMaxCorners - ng;
+        for (int k = 0; k < 32 && nacc < room; ++k) {
+            const unsigned ck = __shfl_sync(0xffffffffu, conf, k);
+            if (((passed >> k) & 1u) && !(ck & acc)) { acc |= 1u << k; ++nacc; }
+        }
+        if ((acc >> lane) & 1u) {
+            const int pos = ng + __popc(acc & ((1u << lane) - 1u));
+            corners[pos] = make_float2((float)x, (float)y);
+            res->corner[pos] = idx;
+            int4 &c = grid[(y / kMinDist) * gw + x / kMinDist];
+            if (atomicCAS(&c.x, kCellEmpty, x) == kCellEmpty) {
+                c.y = y;
+            } else {
+                const int old = atomicCAS(&c.z, kCellEmpty, x);
+                assert(old == kCellEmpty);                           // two slots per cell (above)
+                c.w = y;
+            }
+        }
+        ng += nacc;
+        __syncwarp();
+    }
+    if (lane == 0) res->n_gftt = ng;
+    __syncwarp();
+
+    // PoissonDiskFilter against the presets, then the 20-pixel border (opencv_image.cpp:69-84)
+    const double r2 = f.r2;
+    unsigned word = 0;
+    for (int i = 0; i < ng; ++i) {
+        const double x = corners[i].x, y = corners[i].y;
+        const double fx = floor(x / gs), fy = floor(y / gs);
+        // beyond 2^30 (or a NaN radius) the host's cell arithmetic overflows and its walk meets no point: no test
+        const bool regular = fx <= kCellLimit && fy <= kCellLimit;
+        bool near = false;
+        if (regular && lane < 25) {
+            const int t = lane + 1;
+            const int v = hash_find(hk, hv, f.hbits, cell_key((long long)fx - 2 + t % 5, (long long)fy - 2 + t / 5));
+            if (v >= 0) {
+                const double px = v < f.n_pre ? f.pre[v].x : (double)corners[v - f.n_pre].x;
+                const double py = v < f.n_pre ? f.pre[v].y : (double)corners[v - f.n_pre].y;
+                const double dx = x - px, dy = y - py;
+                near = dx * dx + dy * dy < r2;
+            }
+        }
+        const bool take = !__any_sync(0xffffffffu, near);
+        if (lane == 0) {
+            if (take && regular) {
+                const unsigned long long key = cell_key((long long)fx, (long long)fy);
+                unsigned long long s = hash_slot(key, f.hbits);
+                while (hk[s] != kHashEmpty && hk[s] != key) s = (s + 1) & hm;
+                hk[s] = key; hv[s] = f.n_pre + i;
+            }
+            if (take && !(x < 20 || y < 20 || x >= w - 20 || y >= hgt - 20)) word |= 1u << (i & 31);
+            if ((i & 31) == 31 || i == ng - 1) { res->mask[i >> 5] = word; word = 0; }
+        }
+        __syncwarp();
+    }
+}
+
+// the segment [begin, end) of frame i's keys; end read on the device after the NMS kernel has counted them
+struct SegBegin {
+    const DetectBatchFrame *f;
+    __host__ __device__ int operator()(int i) const { return f[i].key_off; }
+};
+struct SegEnd {
+    const DetectBatchFrame *f;
+    __host__ __device__ int operator()(int i) const {
+        const int c = f[i].counters[1];
+        return f[i].key_off + (c < f[i].cap ? c : f[i].cap);
+    }
+};
+
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
 }  // namespace
+
+int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, double clahe_clip, int tiles_x, int tiles_y) {
+    if (n < 0 || n > kMaxBatchDetect) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: bad request count");
+    if (n == 0) return 0;
+    if (!reqs || clahe_clip < 0.0) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: bad arguments");
+    const bool do_clahe = clahe_clip > 0.0;
+    const KltBatchState &B = h->kltb;
+    std::vector<const uint8_t *> cached(n, nullptr);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_detect_request &a = reqs[i];
+        if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: slot out of range");
+        if (a.width < 8 || a.height < 8 || a.n_existing < 0 || a.max_out < 0 || a.keypoint_distance <= 0.0 || !a.n_out ||
+            (a.n_existing > 0 && !a.existing) || (a.max_out > 0 && !a.keypoints_out))
+            return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: bad arguments");
+        if (a.frame_id && (size_t)a.slot < B.slots.size()) {
+            const KltPyramids &s = B.slots[a.slot];
+            if (s.w == a.width && s.h == a.height)
+                for (int k = 0; k < 2; ++k)
+                    if (s.pyr_id[k] == a.frame_id && s.pyr_clahe[k] == clahe_clip) cached[i] = s.pyr[k].d;
+        }
+        if (cached[i]) continue;
+        if (!a.image) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: frame not cached in its slot and no pixels given");
+        if (a.stride < a.width) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: bad stride");
+        if (do_clahe && (tiles_x < 1 || tiles_y < 1 || a.width % tiles_x || a.height % tiles_y))
+            return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
+    }
+
+    // sizes: per frame its key segment, the existing points its Poisson walks can meet (cells [-2, cx + 2] x
+    // [-2, cy + 3] around the cells of its pixels), its working area; the staging and the scratch of the call
+    struct Plan {
+        size_t pix_off, eq_off, resp_off, work, work_off;
+        int cap, key_off, n_pre, gw, gh, hbits;
+        double gs, cxmax, cymax;
+    };
+    std::vector<Plan> plan(n);
+    auto keep = [](const Plan &P, double x, double y) {
+        const double fx = std::floor(x / P.gs), fy = std::floor(y / P.gs);
+        return fx >= -2.0 && fx <= P.cxmax + 2.0 && fy >= -2.0 && fy <= P.cymax + 3.0;
+    };
+    size_t n_keys = 0, n_pre = 0, pix_bytes = 0, eq_bytes = 0, resp_bytes = 0, smem = 0;
+    int n_eq = 0, max_w = 0, max_h = 0, eq_w = 0, eq_h = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_detect_request &a = reqs[i];
+        Plan &P = plan[i];
+        const size_t px = (size_t)a.width * a.height;
+        P.cap = candidate_cap(px);
+        P.key_off = (int)std::min<size_t>(n_keys, INT_MAX);
+        n_keys += P.cap;
+        P.gs = a.keypoint_distance / std::sqrt(2.0);                // PoissonFilter's cell size
+        P.cxmax = std::min(std::floor((a.width - 1) / P.gs), kCellLimit);
+        P.cymax = std::min(std::floor((a.height - 1) / P.gs), kCellLimit);
+        P.n_pre = 0;
+        for (int j = 0; j < a.n_existing; ++j) P.n_pre += keep(P, a.existing[2 * j], a.existing[2 * j + 1]);
+        n_pre += P.n_pre;
+        P.gw = (a.width + kMinDist - 1) / kMinDist;
+        P.gh = (a.height + kMinDist - 1) / kMinDist;
+        P.hbits = 1;
+        while (((size_t)1 << P.hbits) < 2 * ((size_t)P.n_pre + kMaxCorners)) ++P.hbits;
+        P.work = align256(sizeof(int4) * P.gw * P.gh + sizeof(float2) * kMaxCorners + 12 * ((size_t)1 << P.hbits));
+        if (P.work <= kSelectSmem) smem = std::max(smem, P.work);
+        P.resp_off = resp_bytes;
+        resp_bytes += align256(sizeof(float) * px);
+        max_w = std::max(max_w, a.width); max_h = std::max(max_h, a.height);
+        if (!cached[i]) {
+            P.pix_off = pix_bytes;
+            pix_bytes += align256(px);
+            if (do_clahe) {
+                P.eq_off = eq_bytes;
+                eq_bytes += align256(px);
+                ++n_eq;
+                eq_w = std::max(eq_w, a.width); eq_h = std::max(eq_h, a.height);
+            }
+        }
+    }
+    if (n_keys > (size_t)INT_MAX) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: too many pixels in one call");
+    size_t work_bytes = 0;
+    for (auto &P : plan)
+        if (P.work > smem) { P.work_off = work_bytes; work_bytes += P.work; }
+
+    // staging (both sides): upload [0, o_up) | download [o_res, o)
+    size_t o = 0;
+    const size_t o_frm = o; o = align256(o + sizeof(DetectBatchFrame) * n);
+    const size_t o_kf = o;  o = align256(o + sizeof(KltBatchFrame) * n_eq);
+    const size_t o_cnt = o; o = align256(o + sizeof(int) * 2 * n);
+    const size_t o_pre = o; o = align256(o + sizeof(double2) * n_pre);
+    const size_t o_pix = o; o += pix_bytes;
+    const size_t o_up = o;  o = align256(o);
+    const size_t o_res = o; o = align256(o + sizeof(DetectResult) * n);
+    // device scratch: responses | keys | sorted keys | equalised frames | CLAHE tables | working areas | sort temporaries
+    const size_t tiles = do_clahe ? (size_t)tiles_x * tiles_y : 0;
+    auto begin_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{nullptr});
+    auto end_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{nullptr});
+    size_t cub_bytes = 0;
+    CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(nullptr, cub_bytes, (const unsigned long long *)nullptr,
+                                                            (unsigned long long *)nullptr, (int)n_keys, n, begin_it, end_it, 0, 64));
+    size_t c = 0;
+    const size_t c_resp = c;   c += resp_bytes;
+    const size_t c_keys = c;   c = align256(c + sizeof(unsigned long long) * n_keys);
+    const size_t c_sorted = c; c = align256(c + sizeof(unsigned long long) * n_keys);
+    const size_t c_eq = c;     c += eq_bytes;
+    const size_t c_lut = c;    c = align256(c + tiles * 256 * n_eq);
+    const size_t c_work = c;   c += work_bytes;
+    const size_t c_cub = c;    c = align256(c + cub_bytes);
+    DetectBatchState &D = h->detectb;
+    TRY(reserve(h, D.stage, o, kBoth));
+    TRY(reserve(h, D.scratch, c, kDevice));
+
+    uint8_t *hs = D.stage.h, *ds = D.stage.d, *dc = D.scratch.d;
+    DetectBatchFrame *frm = reinterpret_cast<DetectBatchFrame *>(hs + o_frm);
+    KltBatchFrame *kf = reinterpret_cast<KltBatchFrame *>(hs + o_kf);
+    double2 *pre = reinterpret_cast<double2 *>(hs + o_pre);
+    memset(hs + o_cnt, 0, sizeof(int) * 2 * n);
+    size_t p = 0;
+    int q = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_detect_request &a = reqs[i];
+        const Plan &P = plan[i];
+        const uint8_t *img = cached[i];
+        if (!img) {
+            uint8_t *dst = hs + o_pix + P.pix_off;
+            for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, a.image + (size_t)y * a.stride, a.width);
+            img = ds + o_pix + P.pix_off;
+            if (do_clahe) {                   // raw pixels: CLAHE into the detector's scratch
+                KltBatchFrame &K = kf[q];
+                memset(&K, 0, sizeof(K));
+                K.raw = img;
+                K.lut = dc + c_lut + (size_t)q * tiles * 256;
+                K.pyr = dc + c_eq + P.eq_off;
+                K.levels = 1;
+                K.w[0] = a.width; K.h[0] = a.height;
+                klt_clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, K.tw, K.th, K.clip, K.lut_scale);
+                img = K.pyr;
+                ++q;
+            }
+        }
+        DetectBatchFrame &F = frm[i];
+        memset(&F, 0, sizeof(F));
+        F.img = img;
+        F.resp = reinterpret_cast<float *>(dc + c_resp + P.resp_off);
+        F.keys = reinterpret_cast<unsigned long long *>(dc + c_keys) + P.key_off;
+        F.sorted = reinterpret_cast<unsigned long long *>(dc + c_sorted) + P.key_off;
+        F.counters = reinterpret_cast<int *>(ds + o_cnt) + 2 * i;
+        F.pre = reinterpret_cast<const double2 *>(ds + o_pre) + p;
+        for (int j = 0; j < a.n_existing; ++j) {
+            const double x = a.existing[2 * j], y = a.existing[2 * j + 1];
+            if (keep(P, x, y)) pre[p++] = make_double2(x, y);
+        }
+        F.work = P.work > smem ? dc + c_work + P.work_off : nullptr;
+        F.res = reinterpret_cast<DetectResult *>(ds + o_res) + i;
+        F.gs = P.gs; F.r2 = a.keypoint_distance * a.keypoint_distance;
+        F.w = a.width; F.h = a.height; F.cap = P.cap; F.key_off = P.key_off;
+        F.n_pre = P.n_pre; F.gw = P.gw; F.gh = P.gh; F.hbits = P.hbits;
+    }
+
+    cudaStream_t st = h->stream;
+    CK(h, cudaMemcpyAsync(ds, hs, o_up, cudaMemcpyHostToDevice, st));
+    const DetectBatchFrame *d_frm = reinterpret_cast<const DetectBatchFrame *>(ds + o_frm);
+    if (n_eq > 0) klt_batch_clahe(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_eq, tiles_x, tiles_y, eq_w, eq_h);
+    harris_response_kernel<true><<<dim3((max_w + kTX - 1) / kTX, (max_h + kTY - 1) / kTY, n), dim3(kTX, kTY), 0, st>>>(
+        nullptr, 0, 0, 0.04f, nullptr, nullptr, d_frm);
+    nms_compact_kernel<true><<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n), dim3(32, 8), 0, st>>>(
+        nullptr, 0, 0, 1.0e-3, nullptr, nullptr, nullptr, 0, d_frm);
+    h->launches += 2;
+    size_t tmp = cub_bytes;
+    CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(
+              dc + c_cub, tmp, reinterpret_cast<const unsigned long long *>(dc + c_keys), reinterpret_cast<unsigned long long *>(dc + c_sorted),
+              (int)n_keys, n, thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{d_frm}),
+              thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{d_frm}), 0, 64, st));
+    ++h->launches;
+    if (smem > 48 * 1024)
+        CK(h, cudaFuncSetAttribute(detect_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    detect_select_kernel<<<n, kSelectThreads, smem, st>>>(d_frm);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(hs + o_res, ds + o_res, sizeof(DetectResult) * n, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaStreamSynchronize(st));
+
+    // per request: the corners, and the keypoints the mask keeps, in order
+    const DetectResult *rr = reinterpret_cast<const DetectResult *>(hs + o_res);
+    bool overflow = false;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_detect_request &a = reqs[i];
+        const DetectResult &R = rr[i];
+        const int ng = R.n_gftt;
+        if (a.n_gftt) *a.n_gftt = ng;
+        int m = 0;
+        for (int j = 0; j < ng; ++j) {
+            const unsigned idx = R.corner[j], y = idx / (unsigned)a.width, x = idx - y * (unsigned)a.width;
+            if (a.gftt_out) { a.gftt_out[2 * j] = (float)x; a.gftt_out[2 * j + 1] = (float)y; }
+            if (!((R.mask[j >> 5] >> (j & 31)) & 1u)) continue;
+            if (m < a.max_out) { a.keypoints_out[2 * m] = (double)x; a.keypoints_out[2 * m + 1] = (double)y; }
+            ++m;
+        }
+        *a.n_out = m;
+        overflow |= m > a.max_out;
+    }
+    return overflow ? fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: an output array is too small") : 0;
+}
+
 }  // namespace pvio
 
 using namespace pvio;
@@ -216,10 +642,10 @@ extern "C" int pvio_b200_detect_keypoints(pvio_b200_handle hh, uint64_t frame_id
     }
     int *counters = d.counters.d;
     CK(h, cudaMemsetAsync(counters, 0, sizeof(int) * 2, h->stream));
-    harris_response_kernel<<<dim3((width + kTX - 1) / kTX, (height + kTY - 1) / kTY), dim3(kTX, kTY), 0, h->stream>>>(
-        src, width, height, 0.04f, d.resp.d, counters);
-    nms_compact_kernel<<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, h->stream>>>(
-        d.resp.d, width, height, 1.0e-3, counters, d.keys.d, counters + 1, d.cap);
+    harris_response_kernel<false><<<dim3((width + kTX - 1) / kTX, (height + kTY - 1) / kTY), dim3(kTX, kTY), 0, h->stream>>>(
+        src, width, height, 0.04f, d.resp.d, counters, nullptr);
+    nms_compact_kernel<false><<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, h->stream>>>(
+        d.resp.d, width, height, 1.0e-3, counters, d.keys.d, counters + 1, d.cap, nullptr);
     h->launches += 2;
     CK(h, cudaMemcpyAsync(d.counters.h, counters, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));

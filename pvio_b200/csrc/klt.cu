@@ -36,18 +36,6 @@ struct KltLevels {
     int n;
 };
 
-// one frame a batched call uploads (batch_track_impl): its raw pixels in the staging, CLAHE into level 0 of its
-// pyramid, then pyrDown level by level
-struct KltBatchFrame {
-    const uint8_t *raw;                       // level-0 pixels as uploaded (raw when CLAHE runs)
-    uint8_t *lut;                             // [tiles][256] its CLAHE tables
-    uint8_t *pyr;                             // its pyramid in the sequence's slot
-    int levels, tw, th, clip;
-    float lut_scale;
-    int w[kMaxLevels], h[kMaxLevels];
-    size_t off[kMaxLevels];
-};
-
 __device__ __forceinline__ int reflect101(int i, int n) {
     i = i < 0 ? -i : i;
     return i >= n ? 2 * (n - 1) - i : i;
@@ -132,12 +120,21 @@ __global__ void clahe_apply_kernel(const uint8_t *src, int w, int h, int tw, int
 }
 
 // cv::CLAHE's per-tile constants of a w x h image
-static void clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_y, int &tw, int &th, int &clip,
-                         float &lut_scale) {
+void klt_clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_y, int &tw, int &th, int &clip,
+                      float &lut_scale) {
     tw = w / tiles_x; th = hgt / tiles_y;
     const int area = tw * th;
     clip = std::max((int)(clip_limit * area / 256), 1);
     lut_scale = 255.0f / (float)area;
+}
+
+// CLAHE of the frames of a batched call, each into level 0 of its f.pyr
+void klt_batch_clahe(Handle *h, const KltBatchFrame *frames, int n_frames, int tiles_x, int tiles_y, int max_w, int max_h) {
+    clahe_lut_kernel<true><<<dim3((unsigned)(tiles_x * tiles_y), n_frames), 256, 0, h->stream>>>(nullptr, 0, 0, 0, tiles_x, 0, 0.f,
+                                                                                               nullptr, frames);
+    clahe_apply_kernel<true><<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n_frames), dim3(32, 8), 0, h->stream>>>(
+        nullptr, 0, 0, 0, 0, tiles_x, tiles_y, nullptr, nullptr, frames);
+    h->launches += 2;
 }
 
 // device-resident CLAHE of a w x h image (row stride w)
@@ -145,7 +142,7 @@ static int clahe_device(Handle *h, const uint8_t *src, uint8_t *dst, uint8_t *lu
                         int tiles_x, int tiles_y) {
     int tw, th, clip;
     float lut_scale;
-    clahe_params(w, hgt, clip_limit, tiles_x, tiles_y, tw, th, clip, lut_scale);
+    klt_clahe_params(w, hgt, clip_limit, tiles_x, tiles_y, tw, th, clip, lut_scale);
     clahe_lut_kernel<false><<<tiles_x * tiles_y, 256, 0, h->stream>>>(src, w, tw, th, tiles_x, clip, lut_scale, lut, nullptr);
     dim3 b(32, 8), g((w + 31) / 32, (hgt + 7) / 8);
     clahe_apply_kernel<false><<<g, b, 0, h->stream>>>(src, w, hgt, tw, th, tiles_x, tiles_y, lut, dst, nullptr);
@@ -487,7 +484,6 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
 // a synchronise.  Without CLAHE each new frame is copied into level 0 of its pyramid (a device copy per frame).
 namespace {
 constexpr int kMaxBatchPairs = 32767;         // grid y / z limits: one block row per pair, per new frame
-constexpr int kMaxBatchSlot = 65535;
 constexpr int kFmIters = 1000;                // findFundamentalMat's maxIters, as pvio_b200_track_keypoints passes it
 inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 }  // namespace
@@ -622,7 +618,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
             F.pyr = s.pyr[pl.slot[side]].d;
             F.levels = s.levels;
             for (int l = 0; l < s.levels; ++l) { F.w[l] = s.lw[l]; F.h[l] = s.lh[l]; F.off[l] = s.off[l]; }
-            if (do_clahe) clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, F.tw, F.th, F.clip, F.lut_scale);
+            if (do_clahe) klt_clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, F.tw, F.th, F.clip, F.lut_scale);
             pix += align256((size_t)a.width * a.height);
             ++f;
         }
@@ -659,10 +655,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     if (n_frames > 0) {
         const int nf = (int)n_frames;
         if (do_clahe) {
-            clahe_lut_kernel<true><<<dim3((unsigned)tiles, nf), 256, 0, st>>>(nullptr, 0, 0, 0, tiles_x, 0, 0.f, nullptr, d_frm);
-            clahe_apply_kernel<true><<<dim3((lvw[0] + 31) / 32, (lvh[0] + 7) / 8, nf), b2, 0, st>>>(
-                nullptr, 0, 0, 0, 0, tiles_x, tiles_y, nullptr, nullptr, d_frm);
-            h->launches += 2;
+            klt_batch_clahe(h, d_frm, nf, tiles_x, tiles_y, lvw[0], lvh[0]);
         } else {
             for (size_t j = 0; j < n_frames; ++j)
                 CK(h, cudaMemcpyAsync(frm[j].pyr, frm[j].raw, (size_t)frm[j].w[0] * frm[j].h[0], cudaMemcpyDeviceToDevice, st));

@@ -26,3 +26,53 @@ def detect_keypoints(ba, image, keypoints=(), keypoint_distance=25.0, clahe_clip
               clahe_tiles[0], clahe_tiles[1], _lib._ptr(ex, C.c_double) if len(ex) else None, len(ex), float(keypoint_distance),
               max_out, _lib._ptr(out, C.c_double), C.byref(n), _lib._ptr(gftt, C.c_float), C.byref(ng)))
     return (out[:n.value].copy(), gftt[:ng.value].copy()) if want_gftt else out[:n.value].copy()
+
+
+def pack_requests(requests, want_gftt=False):
+    """The pvio_b200_detect_request array of a batched call (see batch_detect_keypoints) and its output arrays: returns
+    (CDetectRequest array, outputs [(keypoints, n_out, gftt, n_gftt)] per request, the arrays that must stay alive)."""
+    n = len(requests)
+    cr = (_lib.CDetectRequest * max(n, 1))()
+    outs, keep = [], []
+    for i, d in enumerate(requests):
+        img = None if d.get("image") is None else np.ascontiguousarray(d["image"], dtype=np.uint8)
+        h, w = img.shape if img is not None else d["shape"]
+        ex = np.ascontiguousarray(d.get("keypoints", ()), dtype=np.float64).reshape(-1, 2)
+        max_out = int(d.get("max_out", 2048))
+        out = np.zeros((max(max_out, 1), 2))
+        cnt = np.zeros(2, dtype=np.int32)                  # n_out, n_gftt
+        gftt = np.zeros((1000, 2), dtype=np.float32) if want_gftt else None
+        c = cr[i]
+        c.slot, c.width, c.height, c.stride = int(d["slot"]), w, h, w
+        c.frame_id = int(d.get("frame_id", 0))
+        c.image = None if img is None else _lib._ptr(img, C.c_uint8)
+        c.existing = _lib._ptr(ex, C.c_double) if len(ex) else None
+        c.n_existing = len(ex)
+        c.max_out = max_out
+        c.keypoint_distance = float(d.get("keypoint_distance", 25.0))
+        c.keypoints_out = _lib._ptr(out, C.c_double)
+        c.n_out = _lib._ptr(cnt, C.c_int32)
+        c.gftt_out = None if gftt is None else _lib._ptr(gftt, C.c_float)
+        c.n_gftt = C.cast(cnt.ctypes.data + 4, C.POINTER(C.c_int32))
+        keep += [img, ex, out, cnt, gftt]
+        outs.append((out, cnt, gftt))
+    return cr, outs, keep
+
+
+def batch_detect_keypoints(ba, requests, clahe_clip=0.0, clahe_tiles=(8, 8), want_gftt=False):
+    """OpenCvImage::detect_keypoints (opencv_image.cpp:54-86) for many frames in one C-ABI call
+    (pvio_b200_batch_detect_keypoints).  requests: one dict per frame with slot (a sequence slot of
+    klt.batch_track_keypoints), frame_id (its id in that slot; 0 or not cached: `image` is uploaded), image (uint8 [h, w],
+    raw when clahe_clip > 0; None when frame_id is cached in the slot, `shape` (h, w) then names the size), keypoints
+    (the frame's existing keypoints [n, 2]), keypoint_distance (default 25) and max_out (default 2048).
+    Returns per request the new keypoints [m, 2] in the reference's order (and the GFTT corners if want_gftt), each as
+    detect.detect_keypoints gives it."""
+    cr, outs, keep = pack_requests(requests, want_gftt)
+    ba._ck(ba.lib.pvio_b200_batch_detect_keypoints(ba.h, len(requests), cr, float(clahe_clip), int(clahe_tiles[0]),
+                                                   int(clahe_tiles[1])))
+    del keep
+    res = []
+    for out, cnt, gftt in outs:
+        kp = out[:cnt[0]].copy()
+        res.append((kp, gftt[:cnt[1]].copy()) if want_gftt else kp)
+    return res
