@@ -440,6 +440,14 @@ int pvio_b200_triangulate(pvio_b200_handle h, int n_frames, const double *P, int
  * logmap(expmap(w)) (3), right_jacobian(w) (9, row-major), its inverse (9), Plus(expmap(w), w) (4), 3 spare.
  * Not part of the reference interface. */
 int pvio_b200_selftest_lie(pvio_b200_handle h, int n, const double *w, double *out);
+/* Device self-test of the marginaliser's eigen-solver (the factorisation of bundle_adjustor.cpp:583-590): n problems in
+ * one launch of the same kernel, with the launch shape pvio_b200_ba_marginalize gives a window of the largest dk.
+ * Problem i: dk[i] in {15, 30, ..., 165}, a dk[i] x dk[i] symmetric row-major matrix A_i and a vector b_i, stored back to
+ * back in A and b.  Out, in the same layout: S_i = sqrt(lambda+) V^T and e_i = sqrt(1 / lambda+) V^T b_i, where lambda+
+ * keeps the eigenvalues above 1e-8 (the rows of the others are 0).  PVIO_B200_EINVAL for n < 1 or a dk outside that set.
+ * Not part of the reference interface. */
+int pvio_b200_selftest_eig(pvio_b200_handle h, int n, const int32_t *dk, const double *A, const double *b, double *S_out,
+                           double *e_out);
 
 /* ---- KLT ----------------------------------------------------------------------------- */
 /* Pyramidal Lucas-Kanade with OpenCV's semantics: winSize 21x21, maxLevel levels above

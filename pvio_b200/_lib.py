@@ -91,7 +91,7 @@ EXPORTS = [
     "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
     "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
     "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve", "pvio_b200_batch_track_keypoints",
-    "pvio_b200_batch_detect_keypoints",
+    "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig",
 ]
 
 _lib = None
@@ -135,6 +135,7 @@ def load():
                                                C.POINTER(CSummary)]
     lib.pvio_b200_batch_marginalize.argtypes = [vp, C.c_int, c_f64p, C.c_int64, c_f64p, C.c_int64]
     lib.pvio_b200_selftest_lie.argtypes = [vp, C.c_int, c_f64p, c_f64p]
+    lib.pvio_b200_selftest_eig.argtypes = [vp, C.c_int, c_i32p, c_f64p, c_f64p, c_f64p, c_f64p]
     lib.pvio_b200_sync.argtypes = [vp]
     lib.pvio_b200_timer_start.argtypes = [vp]
     lib.pvio_b200_timer_stop.argtypes = [vp, c_f32p]

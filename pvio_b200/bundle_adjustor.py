@@ -185,6 +185,21 @@ class BundleAdjustor:
         self._ck(self.lib.pvio_b200_selftest_lie(self.h, len(w), _lib._ptr(w, C.c_double), _lib._ptr(out, C.c_double)))
         return out
 
+    def selftest_eig(self, problems):
+        """The marginaliser's eigen-solver on [(A, b)] in one launch (see the header) -> [(S, e)]."""
+        dk = np.array([len(b) for _, b in problems], dtype=np.int32)
+        A = np.concatenate([np.ascontiguousarray(a, dtype=np.float64).ravel() for a, _ in problems])
+        b = np.concatenate([np.asarray(v, dtype=np.float64) for _, v in problems])
+        S, e = np.zeros_like(A), np.zeros_like(b)
+        self._ck(self.lib.pvio_b200_selftest_eig(self.h, len(dk), _lib._ptr(dk, C.c_int32), _lib._ptr(A, C.c_double),
+                                                 _lib._ptr(b, C.c_double), _lib._ptr(S, C.c_double), _lib._ptr(e, C.c_double)))
+        out, oa, ob = [], 0, 0
+        for d in dk:
+            out.append((S[oa:oa + d * d].reshape(d, d), e[ob:ob + d]))
+            oa += d * d
+            ob += d
+        return out
+
     def sync(self):
         self._ck(self.lib.pvio_b200_sync(self.h))
 

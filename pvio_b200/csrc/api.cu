@@ -996,6 +996,7 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
         CK(h, cudaFuncSetAttribute(update_obs_kernel<double, kUpdWarps, 4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
         CK(h, cudaFuncSetAttribute(solve_kernel_visual, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024));
+        TRY(marg_opt_in(h));
     }
     init_ctrl_kernel<<<(int)W, 32, 0, h->stream>>>(h->ctrl.d, 1e-8, 1e4, 10, 0.0, 0);
     ++h->launches;
@@ -1379,6 +1380,13 @@ int pvio_b200_selftest_lie(pvio_b200_handle hh, int n, const double *w, double *
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h || !w || !out || n < 1) return PVIO_B200_EINVAL;
     return selftest_lie_impl(h, n, w, out);
+}
+
+int pvio_b200_selftest_eig(pvio_b200_handle hh, int n, const int32_t *dk, const double *A, const double *b, double *S_out,
+                           double *e_out) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h || !dk || !A || !b || !S_out || !e_out) return PVIO_B200_EINVAL;
+    return selftest_eig_impl(h, n, dk, A, b, S_out, e_out);
 }
 
 #ifdef PVIO_SOLVE_STAMPS

@@ -322,6 +322,8 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
 int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
                      double *S_out, double *e_out, double *H_out, double *b_out);
 int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride);
+int selftest_eig_impl(Handle *h, int n, const int32_t *dk, const double *A, const double *b, double *S_out, double *e_out);
+int marg_opt_in(Handle *h);        // the eigen-solver's dynamic shared memory, for the current device (pvio_b200_create)
 // klt.cu: pvio_b200_batch_track_keypoints
 int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_level, int max_iter, double eps,
                      double clahe_clip, int tiles_x, int tiles_y, int border, double ransac_threshold,

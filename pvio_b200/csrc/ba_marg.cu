@@ -455,6 +455,21 @@ static MargLayout marg_layout(const Handle *h) {
 static size_t eig_smem(int dk, int ring) { return sizeof(double) * ((size_t)dk * (dk | 1) + (2 + 2 * (size_t)ring) * dk); }
 static bool eig_fits(int dk) { return eig_smem(dk, 2) <= kEigSmemMax; }      // 15 (N - 1) <= 165
 
+// The launch shape of marg_eig_kernel for a grid whose largest matrix is dk_max: a ring of 4 rotation batches, or 2 when
+// the matrix leaves no room for 4.  Every CTA of the launch gets the ring and the shared memory of the largest.  Every
+// accepted size takes 4: at dk = 165 the 4-slot ring needs 231000 bytes of the 231424 opted in.
+struct EigLaunch { int ring; size_t smem; };
+static EigLaunch eig_launch(int dk_max) {
+    const int ring = eig_smem(dk_max, 4) <= kEigSmemMax ? 4 : 2;
+    return {ring, eig_smem(dk_max, ring)};
+}
+
+// once per handle, for the handle's device (pvio_b200_create): function attributes belong to the current device
+int marg_opt_in(Handle *h) {
+    CK(h, cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEigSmemMax));
+    return 0;
+}
+
 // The marginaliser of the uploaded windows [0, n) at their device states: the vision part of all n windows, then the dense
 // tail chunk by chunk (assemble -> frame Schur complement -> eigen-solver; a window's three kernels stay in one chunk, so
 // its old prior is consumed before its new one overwrites it).  eig = false stops after the Schur complement.
@@ -465,8 +480,6 @@ static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLa
     const int chunk = std::min(n, kMargChunkPerSm * h->sm_count);
     L = marg_layout(h);
     TRY(reserve(h, h->marg, L.stride * chunk, kDevice));
-    static bool attr_set = false;
-    if (eig && !attr_set) { CK(h, cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEigSmemMax)); attr_set = true; }
     // vision part: no loss, victim-seen landmarks only, mu = 0, fp64 (lin_obs_kernel<false, double> + schur_kernel<double>)
     TRY(run_marg_vision(h, n));
     double *buf = h->marg.d;
@@ -481,13 +494,13 @@ static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLa
         if (!eig) continue;
         int dk = 0;
         for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[i].N - 1));
-        const int ring = eig_smem(dk, 4) <= kEigSmemMax ? 4 : 2;      // 2 when the matrix leaves no room: dk = 165
+        const EigLaunch el = eig_launch(dk);
         if (to_slots)
-            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, buf, L, ring,
+            marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring,
                 h->prior_S.dslot(w0), h->prior_S.per, h->prior_e.dslot(w0), h->prior_e.per, h->frames.dslot(w0),
                 h->prior_x0.dslot(w0), h->prior_x0.per);
         else
-            marg_eig_kernel<<<cn, 256, eig_smem(dk, ring), h->stream>>>(h->hdr.d, w0, buf, L, ring,
+            marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring,
                 buf + L.S, L.stride, buf + L.e, L.stride, nullptr, nullptr, 0);
         ++h->launches;
     }
@@ -547,6 +560,53 @@ int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, do
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
     for (int i = 0; i < n; ++i) h->prior_resident[i] = h->hdr.h[i].N - 1;
+    return 0;
+}
+
+// pvio_b200_selftest_eig: the unchanged marg_eig_kernel in one launch over n given symmetric matrices, so that tests can
+// pin the eigen-solver against a reference on spectra no window produces.  Problem c is staged as block c of a
+// MargLayout-shaped scratch (Hk, bk; the kernel reads nothing else) with a WinHdr of its own whose N = dk_c / 15 + 1 (the
+// only field the kernel reads); the launch shape is the marginaliser's, eig_launch of the largest dk.  A, b, S_out and
+// e_out hold the problems back to back: dk_c x dk_c row-major matrices, dk_c vectors.
+int selftest_eig_impl(Handle *h, int n, const int32_t *dk, const double *A, const double *b, double *S_out, double *e_out) {
+    if (n < 1) return fail(h, PVIO_B200_EINVAL, "selftest_eig: n < 1");
+    int dmax = 0;
+    for (int c = 0; c < n; ++c) {
+        if (dk[c] < 15 || dk[c] % 15 != 0 || !eig_fits(dk[c]))
+            return fail(h, PVIO_B200_EINVAL, "selftest_eig: every dk must be a multiple of 15 in [15, 165]");
+        dmax = std::max(dmax, (int)dk[c]);
+    }
+    MargLayout L{};
+    L.Hk = 0; L.bk = (size_t)dmax * dmax; L.stride = L.bk + dmax;
+    DevBuf<double> buf;                    // n input blocks, then n output blocks (S at the block's start, e at its bk)
+    DevBuf<WinHdr> hdr;
+    TRY(alloc(h, buf, 2 * n * L.stride, kBoth));
+    TRY(alloc(h, hdr, n, kBoth));
+    size_t oa = 0, ob = 0;
+    for (int c = 0; c < n; ++c) {
+        const size_t d = dk[c];
+        memcpy(buf.h + c * L.stride + L.Hk, A + oa, sizeof(double) * d * d);
+        memcpy(buf.h + c * L.stride + L.bk, b + ob, sizeof(double) * d);
+        hdr.h[c].N = dk[c] / 15 + 1;
+        oa += d * d; ob += d;
+    }
+    double *out = buf.d + n * L.stride;
+    CK(h, cudaMemcpyAsync(buf.d, buf.h, sizeof(double) * n * L.stride, cudaMemcpyHostToDevice, h->stream));
+    CK(h, cudaMemcpyAsync(hdr.d, hdr.h, sizeof(WinHdr) * n, cudaMemcpyHostToDevice, h->stream));
+    const EigLaunch el = eig_launch(dmax);
+    marg_eig_kernel<<<n, 256, el.smem, h->stream>>>(hdr.d, 0, buf.d, L, el.ring, out, L.stride, out + L.bk, L.stride,
+                                                   nullptr, nullptr, 0);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(buf.h, out, sizeof(double) * n * L.stride, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    oa = ob = 0;
+    for (int c = 0; c < n; ++c) {
+        const size_t d = dk[c];
+        memcpy(S_out + oa, buf.h + c * L.stride, sizeof(double) * d * d);
+        memcpy(e_out + ob, buf.h + c * L.stride + L.bk, sizeof(double) * d);
+        oa += d * d; ob += d;
+    }
     return 0;
 }
 

@@ -287,11 +287,14 @@ def test_reprojection_error(ba):
     assert abs(ba.compute_reprojection_error(w, st) - ref) < 1e-6 * ref
 
 
-@pytest.mark.parametrize("index", [0])
+@pytest.mark.parametrize("index", [0, 1, 4, 7, 8])
 def test_marginalize_matches_oracle(ba, index):
     """bundle_adjustor.cpp:348-599 on the GPU vs the oracle.  S is unique only up to the sign /
-    order of eigenvectors, so compare the information S^T S, S^T e and the pre-factorisation H, b."""
+    order of eigenvectors, so compare the information S^T S, S^T e and the pre-factorisation H, b.
+    The victim's landmarks are the ones anchored in it or observed by it."""
+    from test_marginalize_oracle_shapes import victim_flags
     w, st, _ = synth.make_cfg3()
+    w.lm_in_victim = victim_flags(w, index)
     S, e, H, b = ba.marginalize_frame(w, st, index=index, want_info=True)
     S0, e0, H0, b0 = bo.marginalize(w, st, index=index)
     hs = np.maximum(np.sqrt(np.abs(np.diag(H0))), 1e-3)
@@ -528,33 +531,37 @@ def test_sequence_of_20_keyframes_marginalise_shift_solve(ba):
     """Sequence-level parity (the plumbing of BASELINE config 1 without its images): 20 keyframes of
     solve -> marginalize_frame(0) -> drop the oldest frame / append the next (core/sliding_window_tracker.cpp:79-125),
     a GPU chain and a CPU-oracle chain side by side, each feeding its own states, re-anchored inverse depths
-    (map/track.cpp:42-49) and its own prior (S, e, linearisation point) forward.  The chains must not drift apart."""
+    (map/track.cpp:42-49) and its own prior (S, e, linearisation point) forward.  The chains must not drift apart.
+    Windows of N = 6 and of N = 11, the reference's default (Config::sliding_window_size() = 10, marginalised at 11
+    frames)."""
     from oracle import c_oracle
     from synthetic.sequence import Run, Chain
     from pvio_b200.window import State
-    run = Run(F=26, N=6, M=260, seed=700)
-    gpu, ref = Chain(run), Chain(run)
-    worst_cost = 0.0
-    for k in range(20):
-        wg, sg, ids_g = gpu.window(k)
-        wr, sr, ids_r = ref.window(k)
-        assert ids_g == ids_r
-        out, summ = ba.solve(wg, sg, max_iterations=6)
-        fr, rho, rsum = c_oracle.solve(wr, sr, max_iter=6)
-        ref_state = State(fr[:, 0:4], fr[:, 4:7], fr[:, 7:10], fr[:, 10:13], fr[:, 13:16], rho)
-        assert summ['iterations'] == rsum['iterations'] and summ['accepted_steps'] == rsum['accepted_steps'], k
-        worst_cost = max(worst_cost, abs(summ['final_cost'] - rsum['final_cost']) / rsum['final_cost'])
-        Sg, eg = ba.marginalize_frame(wg, out, index=0)
-        Sr, er, _, _ = c_oracle.marginalize(wr, ref_state, 0)
-        gpu.store(k, out, ids_g); gpu.set_prior(k, Sg, eg, out)
-        ref.store(k, ref_state, ids_r); ref.set_prior(k, Sr, er, ref_state)
-    path = np.linalg.norm(np.diff(run.truth.p[:26], axis=0), axis=1).sum()
-    drift_p = np.max(np.linalg.norm(gpu.p[:25] - ref.p[:25], axis=1))
-    drift_v = np.max(np.linalg.norm(gpu.v[:25] - ref.v[:25], axis=1))
-    drift_rho = np.max(np.abs(gpu.rho - ref.rho) / np.abs(ref.rho))
-    print(f"20 keyframes: path {path:.2f} m, max |dp| {drift_p:.3e} m, max |dv| {drift_v:.3e} m/s, max rel d rho {drift_rho:.3e}, "
-          f"worst final-cost rel diff {worst_cost:.3e}")
-    assert drift_p < 1e-5 * path and drift_v < 1e-4 and drift_rho < 1e-4 and worst_cost < 1e-5
+    for N in (6, 11):
+        run = Run(F=20 + N, N=N, M=260, seed=700)
+        gpu, ref = Chain(run), Chain(run)
+        worst_cost = 0.0
+        for k in range(20):
+            wg, sg, ids_g = gpu.window(k)
+            wr, sr, ids_r = ref.window(k)
+            assert ids_g == ids_r
+            out, summ = ba.solve(wg, sg, max_iterations=6)
+            fr, rho, rsum = c_oracle.solve(wr, sr, max_iter=6)
+            ref_state = State(fr[:, 0:4], fr[:, 4:7], fr[:, 7:10], fr[:, 10:13], fr[:, 13:16], rho)
+            assert summ['iterations'] == rsum['iterations'] and summ['accepted_steps'] == rsum['accepted_steps'], (N, k)
+            worst_cost = max(worst_cost, abs(summ['final_cost'] - rsum['final_cost']) / rsum['final_cost'])
+            Sg, eg = ba.marginalize_frame(wg, out, index=0)
+            Sr, er, _, _ = c_oracle.marginalize(wr, ref_state, 0)
+            gpu.store(k, out, ids_g); gpu.set_prior(k, Sg, eg, out)
+            ref.store(k, ref_state, ids_r); ref.set_prior(k, Sr, er, ref_state)
+        F = run.F
+        path = np.linalg.norm(np.diff(run.truth.p[:F], axis=0), axis=1).sum()
+        drift_p = np.max(np.linalg.norm(gpu.p[:F - 1] - ref.p[:F - 1], axis=1))
+        drift_v = np.max(np.linalg.norm(gpu.v[:F - 1] - ref.v[:F - 1], axis=1))
+        drift_rho = np.max(np.abs(gpu.rho - ref.rho) / np.abs(ref.rho))
+        print(f"N={N}, 20 keyframes: path {path:.2f} m, max |dp| {drift_p:.3e} m, max |dv| {drift_v:.3e} m/s, "
+              f"max rel d rho {drift_rho:.3e}, worst final-cost rel diff {worst_cost:.3e}")
+        assert drift_p < 1e-5 * path and drift_v < 1e-4 and drift_rho < 1e-4 and worst_cost < 1e-5, N
 
 
 @pytest.mark.gpu

@@ -32,12 +32,12 @@ def _rel(a, b):
 NOISE_ABS = 1.0e-7
 
 
-def _info_err(S, e, S1, e1, hs, tol):
-    """(max |S^T S - S1^T S1| / (tol hs hs^T + NOISE_ABS), relative max |S^T e - S1^T e1|).  S is unique only up to the
+def _info_err(S, e, S1, e1, hs, tol, noise_abs=NOISE_ABS):
+    """(max |S^T S - S1^T S1| / (tol hs hs^T + noise_abs), relative max |S^T e - S1^T e1|).  S is unique only up to the
     sign / order of its rows."""
     L, L1 = S.T @ S, S1.T @ S1
     v, v1 = S.T @ e, S1.T @ e1
-    return np.max(np.abs(L - L1) / (tol * np.outer(hs, hs) + NOISE_ABS)), np.max(np.abs(v - v1)) / np.max(np.abs(v1))
+    return np.max(np.abs(L - L1) / (tol * np.outer(hs, hs) + noise_abs)), np.max(np.abs(v - v1)) / np.max(np.abs(v1))
 
 
 def _n_pos(S):
@@ -50,9 +50,9 @@ def _n_noise(H):
     return int(np.sum((np.abs(ev) > 1e-10) & (np.abs(ev) < 1e-6)))
 
 
-def _check_prior(S, e, S1, e1, H1, tol):
+def _check_prior(S, e, S1, e1, H1, tol, noise_abs=NOISE_ABS):
     hs = np.maximum(np.sqrt(np.abs(np.diag(H1))), 1e-3)
-    eL, ev = _info_err(S, e, S1, e1, hs, tol)
+    eL, ev = _info_err(S, e, S1, e1, hs, tol, noise_abs)
     assert eL < 1.0 and ev < tol, (eL, ev)
     assert abs(_n_pos(S) - _n_pos(S1)) <= _n_noise(H1), (_n_pos(S), _n_pos(S1), _n_noise(H1))
     return eL, ev
@@ -216,7 +216,7 @@ def _same(a, b):
 
 
 def test_rejected_calls_change_nothing(kinds):
-    b = BundleAdjustor(max_windows=4, max_frames=9, max_landmarks=320, max_obs=3000)
+    b = BundleAdjustor(max_windows=4, max_frames=13, max_landmarks=320, max_obs=3000)
     (w0, s0), (w1, s1) = kinds[0], kinds[1]
     wv, sv, _ = synth.make_cfg2(N=6, M=80, seed=661)
     for i, (w, st) in enumerate(((w0, s0), (w1, s1), (wv, sv))):
@@ -253,6 +253,17 @@ def test_rejected_calls_change_nothing(kinds):
     dx, _ = b.batch_download(2, 15 * 9 + 320)
     assert np.all(np.isfinite(dx))
     assert len(S_all) == 2
+    # 13 frames (dk = 180) are more than the shared-memory eigen-solver takes: rejected alone and inside a batch
+    w13, s13, _ = synth.make_cfg3(N=13, M=120, seed=662)
+    b.batch_set(2, w13, s13)
+    b.batch_upload(3)
+    snap = _unchanged(b, 3, 13, 320)
+    with pytest.raises(PvioB200Error, match=EINVAL):
+        b.marginalize_frame(w13, s13, 0)
+    assert _same(_unchanged(b, 3, 13, 320), snap)
+    with pytest.raises(PvioB200Error, match=EINVAL):
+        b.batch_marginalize(3)
+    assert _same(_unchanged(b, 3, 13, 320), snap)
     b.close()
 
 
