@@ -241,6 +241,83 @@ int pvio_b200_batch_solve_host(pvio_b200_handle h, int n, const pvio_b200_option
  * may be NULL.  Every window is checked before anything runs: on PVIO_B200_EINVAL no slot has changed. */
 int pvio_b200_batch_marginalize(pvio_b200_handle h, int n, double *S_out, int64_t S_stride,
                                 double *e_out, int64_t e_stride);
+
+/* ---- resident batched windows: many sequences' sliding windows kept on the device --------------------------------- */
+/* A slot made resident by pvio_b200_batch_window_reset holds its sequence's whole window on the device between camera
+ * frames: frame states, IMU records, the prior and every live track (frame mask, fp64 keypoint per frame, inverse depth).
+ * The caller sends only what changed; the packed tables the solve kernels read are rebuilt on the device exactly as
+ * pvio_b200_batch_set_window would pack the window pvio_b200_window_* keeps (tracks with >= 2 observations, in id order,
+ * stably sorted by anchor).  Frame arguments are window indices (0 = oldest).
+ * Rules:
+ *  - Every call checks all its inputs before it stages or launches anything: on PVIO_B200_EINVAL no slot has changed.
+ *    Rejected: a slot out of range or not resident, a slot named twice, an unknown or dead track, observations out of
+ *    frame order, more than max_frames frames, more live tracks than max_landmarks (rounded up to a multiple of 4; one-
+ *    observation tracks count), more than max_obs observations, a landmark with 16 or more observations, more than 96
+ *    landmark chunks, a drop on a window without motion states or with 15 (N - 1) > 165.
+ *  - Track ids are per slot, increasing, never reused until the slot is reset; the storage of dead tracks is reused, so a
+ *    sequence is limited by its live tracks only.
+ *  - A resident slot changes through these calls only.  pvio_b200_batch_set_window on it, and any single-window call
+ *    that packs into slot 0 (ba_solve, ba_gn_step, ba_marginalize, reprojection_error, window_*), end its residency;
+ *    then these calls return PVIO_B200_EINVAL for it until it is reset.  batch_upload, batch_replicate, batch_gn_step,
+ *    batch_solve, batch_marginalize and the *_host calls over a range holding a resident slot return PVIO_B200_EINVAL.
+ *  - The kernel-launch count of a call does not depend on n.  An edit call makes one host -> device and one
+ *    device -> host copy. */
+/* Start an empty resident window in `slot`.  Of `constants` the scalar members are kept (as pvio_b200_window_reset);
+ * n_planes > 0 is rejected. */
+int pvio_b200_batch_window_reset(pvio_b200_handle h, int slot, const pvio_b200_window *constants);
+/* A prior given by the caller over frames 0 .. n_prior-1 (the 1e15 gauge prior of the first window,
+ * sliding_window_tracker.cpp:100-112).  S [(15 n_prior)^2] row-major, e [15 n_prior], state0 [n_prior][16]. */
+int pvio_b200_batch_window_set_prior(pvio_b200_handle h, int slot, int n_prior, const double *S, const double *e,
+                                     const double *state0);
+/* One camera frame of one sequence, applied in this order:
+ *  1. replace_last: drop the newest frame, its IMU factor and its observations (map->erase_frame(frame_num - 1));
+ *     a track left without observations dies;
+ *  2. state != NULL: a new frame (state [16], fixed), imu_record [PVIO_B200_IMU_STRIDE] the factor (previous frame,
+ *     new frame), NULL for the first frame or a visual-only window;
+ *  3. new tracks: first frame, keypoint z [n][2] and initial inverse depth; their ids go to new_ids (may be NULL);
+ *  4. observations (track id, frame, z [n][2]) in increasing frame order per track;
+ *  5. track removals (Map::prune_tracks). */
+typedef struct pvio_b200_window_edit {
+    int32_t slot;
+    int32_t replace_last;
+    const double *state;
+    int32_t fixed;
+    const double *imu_record;
+    int32_t n_new_tracks;
+    const int32_t *new_frame;
+    const double *new_z;
+    const double *new_inv_depth;
+    int32_t *new_ids;
+    int32_t n_obs;
+    const int32_t *obs_track;
+    const int32_t *obs_frame;
+    const double *obs_z;
+    int32_t n_remove;
+    const int32_t *remove;
+} pvio_b200_window_edit;           /* 120 bytes on LP64 */
+/* n edits, each naming a different resident slot. */
+int pvio_b200_batch_window_edit(pvio_b200_handle h, int n, const pvio_b200_window_edit *edits);
+/* BundleAdjustor::solve on the named slots: the trust-region chain of pvio_b200_batch_solve (per-window termination),
+ * then the landmark post-pass (unless opt->run_postpass == 0); solved states and inverse depths stay in the slots and the
+ * post-pass flags in the tracks.  Slots not named keep their windows bit for bit and run no iteration (their solver
+ * records are marked finished).  summaries [n] (may be NULL), in the order of `slots`. */
+int pvio_b200_batch_window_solve(pvio_b200_handle h, int n, const int32_t *slots, const pvio_b200_options *opt,
+                                 pvio_b200_summary *summaries);
+/* Map::marginalize_frame(0) on the named slots: the marginaliser of pvio_b200_batch_marginalize with the new prior
+ * left in the slot, then the victim leaves: a track anchored in it is re-anchored in its next frame from the current
+ * states (track.cpp:42-49), its observations leave their tracks, frames, IMU factors and fixed flags shift by one.
+ * S_out [n][S_stride], e_out [n][e_stride] (may be NULL): the new priors, as pvio_b200_batch_marginalize returns them. */
+int pvio_b200_batch_window_drop_victim(pvio_b200_handle h, int n, const int32_t *slots, double *S_out, int64_t S_stride,
+                                       double *e_out, int64_t e_stride);
+/* Device -> host in one copy, per named slot i: n_frames [n], frames [n][frames_stride] ([N][16]), n_tracks [n] (live
+ * tracks), and for each live track in id order at [i * track_stride + r]: id, inverse depth, anchor frame, observation
+ * count, and the post-pass valid / quality of the last solve (0 / 0 for a track that did not take part in it).  Any
+ * output pointer may be NULL. */
+int pvio_b200_batch_window_download(pvio_b200_handle h, int n, const int32_t *slots, int32_t *n_frames, double *frames,
+                                    int64_t frames_stride, int32_t *n_tracks, int64_t track_stride, int32_t *track_id,
+                                    double *inv_depth, int32_t *anchor_frame, int32_t *n_observations, uint8_t *valid,
+                                    double *quality);
+
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */
 int pvio_b200_timer_start(pvio_b200_handle h);

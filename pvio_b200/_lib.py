@@ -77,6 +77,13 @@ class CDetectRequest(C.Structure):
                 ("gftt_out", c_f32p), ("n_gftt", c_i32p)]
 
 
+class CWindowEdit(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("replace_last", C.c_int32), ("state", c_f64p), ("fixed", C.c_int32),
+                ("imu_record", c_f64p), ("n_new_tracks", C.c_int32), ("new_frame", c_i32p), ("new_z", c_f64p),
+                ("new_inv_depth", c_f64p), ("new_ids", c_i32p), ("n_obs", C.c_int32), ("obs_track", c_i32p),
+                ("obs_frame", c_i32p), ("obs_z", c_f64p), ("n_remove", C.c_int32), ("remove", c_i32p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -91,7 +98,9 @@ EXPORTS = [
     "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
     "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
     "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve", "pvio_b200_batch_track_keypoints",
-    "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig",
+    "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig", "pvio_b200_batch_window_reset",
+    "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
+    "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download",
 ]
 
 _lib = None

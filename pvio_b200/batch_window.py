@@ -1,0 +1,139 @@
+"""Resident sliding windows of many sequences (include/pvio_b200.h "resident batched windows", csrc/batch_window.cu): each
+slot keeps one sequence's window on the device; per camera frame the caller sends only the edits, solves and
+marginalises the slots that take a keyframe, and reads back states, inverse depths and post-pass flags in one copy."""
+import ctypes as C
+
+import numpy as np
+
+from . import _lib
+
+_i32p, _f64p, _u8p = C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_uint8)
+
+
+def _argtypes(L):
+    vp = C.c_void_p
+    L.pvio_b200_batch_window_reset.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindow)]
+    L.pvio_b200_batch_window_set_prior.argtypes = [vp, C.c_int, C.c_int, _f64p, _f64p, _f64p]
+    L.pvio_b200_batch_window_edit.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowEdit)]
+    L.pvio_b200_batch_window_solve.argtypes = [vp, C.c_int, _i32p, C.POINTER(_lib.COptions), C.POINTER(_lib.CSummary)]
+    L.pvio_b200_batch_window_drop_victim.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64, _f64p, C.c_int64]
+    L.pvio_b200_batch_window_download.argtypes = [vp, C.c_int, _i32p, _i32p, _f64p, C.c_int64, _i32p, C.c_int64, _i32p,
+                                                  _f64p, _i32p, _i32p, _u8p, _f64p]
+
+
+def _constants(win):
+    cw = _lib.CWindow()
+    cw.use_inertial = 1 if win.use_inertial else 0
+    cw.cam_q_cs[:] = list(win.cam_q_cs); cw.cam_p_cs[:] = list(win.cam_p_cs)
+    cw.imu_q_cs[:] = list(win.imu_q_cs); cw.imu_p_cs[:] = list(win.imu_p_cs)
+    cw.sqrt_inv_cov[:] = list(np.asarray(win.sqrt_inv_cov, dtype=np.float64).reshape(4))
+    cw.fx, cw.fy, cw.cauchy_a = win.K_fx, win.K_fy, win.cauchy_a
+    cw.plane_sqrt_inv_cov = getattr(win, "plane_sqrt_inv_cov", 0.0)
+    return cw
+
+
+class Edit:
+    """One camera frame of one slot (pvio_b200_window_edit), built up by the caller:
+    replace_last, frame(state16, fixed, imu_record), new tracks (frame, z, inv_depth), observations (id, frame, z),
+    removals (ids)."""
+
+    def __init__(self, slot, replace_last=False):
+        self.slot, self.replace_last = int(slot), bool(replace_last)
+        self.state, self.fixed, self.imu = None, False, None
+        self.new, self.obs, self.remove = [], [], []
+
+    def frame(self, state16, fixed=False, imu_record=None):
+        self.state, self.fixed = np.ascontiguousarray(state16, dtype=np.float64), bool(fixed)
+        self.imu = None if imu_record is None else np.ascontiguousarray(imu_record, dtype=np.float64)
+        return self
+
+
+class BatchWindows:
+    def __init__(self, ba):
+        """ba: a BundleAdjustor (owns the device handle and its max_windows slots)."""
+        self.ba, self.lib, self.h = ba, ba.lib, ba.h
+        _argtypes(self.lib)
+
+    def reset(self, slot, win):
+        """Start an empty resident window in `slot`; `win` carries the constants (its arrays are not used)."""
+        self.ba._ck(self.lib.pvio_b200_batch_window_reset(self.h, int(slot), C.byref(_constants(win))))
+
+    def set_prior(self, slot, S, e, state0):
+        S = np.ascontiguousarray(S, dtype=np.float64); e = np.ascontiguousarray(e, dtype=np.float64)
+        x0 = np.ascontiguousarray(state0, dtype=np.float64).reshape(-1, 16)
+        self.ba._ck(self.lib.pvio_b200_batch_window_set_prior(self.h, int(slot), len(x0), _lib._ptr(S, C.c_double),
+                                                              _lib._ptr(e, C.c_double), _lib._ptr(x0, C.c_double)))
+
+    def edit(self, edits):
+        """Apply a list of Edit (distinct slots) in one call; returns the new track ids of each edit."""
+        keep, recs = [], (_lib.CWindowEdit * max(len(edits), 1))()
+        ids = []
+        for i, e in enumerate(edits):
+            r = recs[i]
+            r.slot, r.replace_last = e.slot, 1 if e.replace_last else 0
+            if e.state is not None:
+                keep.append(e.state); r.state = _lib._ptr(e.state, C.c_double); r.fixed = 1 if e.fixed else 0
+                if e.imu is not None:
+                    keep.append(e.imu); r.imu_record = _lib._ptr(e.imu, C.c_double)
+            out = np.zeros(max(len(e.new), 1), dtype=np.int32)
+            ids.append(out)
+            if e.new:
+                f = np.array([t[0] for t in e.new], dtype=np.int32)
+                z = np.ascontiguousarray([t[1] for t in e.new], dtype=np.float64).reshape(-1, 2)
+                rho = np.array([t[2] for t in e.new], dtype=np.float64)
+                keep += [f, z, rho]
+                r.n_new_tracks = len(e.new)
+                r.new_frame, r.new_z = _lib._ptr(f, C.c_int32), _lib._ptr(z, C.c_double)
+                r.new_inv_depth, r.new_ids = _lib._ptr(rho, C.c_double), _lib._ptr(out, C.c_int32)
+            if e.obs:
+                t = np.array([o[0] for o in e.obs], dtype=np.int32)
+                f = np.array([o[1] for o in e.obs], dtype=np.int32)
+                z = np.ascontiguousarray([o[2] for o in e.obs], dtype=np.float64).reshape(-1, 2)
+                keep += [t, f, z]
+                r.n_obs = len(e.obs)
+                r.obs_track, r.obs_frame, r.obs_z = _lib._ptr(t, C.c_int32), _lib._ptr(f, C.c_int32), _lib._ptr(z, C.c_double)
+            if e.remove:
+                rm = np.array(e.remove, dtype=np.int32)
+                keep.append(rm)
+                r.n_remove, r.remove = len(rm), _lib._ptr(rm, C.c_int32)
+        self.ba._ck(self.lib.pvio_b200_batch_window_edit(self.h, len(edits), recs))
+        return [o[:len(e.new)].copy() for o, e in zip(ids, edits)]
+
+    def solve(self, slots, max_iterations=10, max_time=1e6, alias_bias=True, postpass=True):
+        s = np.ascontiguousarray(slots, dtype=np.int32)
+        opt = _lib.COptions(max_iterations, max_time, 1 if alias_bias else 0, 1 if postpass else 0, 0.0)
+        sm = (_lib.CSummary * max(len(s), 1))()
+        self.ba._ck(self.lib.pvio_b200_batch_window_solve(self.h, len(s), _lib._ptr(s, C.c_int32), C.byref(opt), sm))
+        return [{k: getattr(sm[i], k) for k, _ in _lib.CSummary._fields_} for i in range(len(s))]
+
+    def drop_victim(self, slots, want=False, max_frames=None):
+        """Map::marginalize_frame(0) on the slots; want: also return each slot's new prior (S, e)."""
+        s = np.ascontiguousarray(slots, dtype=np.int32)
+        if not want:
+            self.ba._ck(self.lib.pvio_b200_batch_window_drop_victim(self.h, len(s), _lib._ptr(s, C.c_int32), None, 0, None, 0))
+            return None
+        d = 15 * ((max_frames or self.ba.max_frames) - 1)
+        S = np.zeros((max(len(s), 1), d * d)); e = np.zeros((max(len(s), 1), d))
+        self.ba._ck(self.lib.pvio_b200_batch_window_drop_victim(self.h, len(s), _lib._ptr(s, C.c_int32), _lib._ptr(S, C.c_double),
+                                                                d * d, _lib._ptr(e, C.c_double), d))
+        return S, e
+
+    def download(self, slots, track_stride):
+        """Per slot a dict: frames [N, 16], and per live track in id order: id, inv_depth, anchor, n_obs, valid, quality."""
+        s = np.ascontiguousarray(slots, dtype=np.int32)
+        n, fs = len(s), 16 * self.ba.max_frames
+        nf = np.zeros(max(n, 1), dtype=np.int32); nt = np.zeros(max(n, 1), dtype=np.int32)
+        fr = np.zeros((max(n, 1), fs))
+        T = max(int(track_stride), 1)
+        ids = np.zeros((max(n, 1), T), dtype=np.int32); rho = np.zeros((max(n, 1), T)); an = np.zeros_like(ids)
+        cnt = np.zeros_like(ids); val = np.zeros((max(n, 1), T), dtype=np.uint8); q = np.zeros((max(n, 1), T))
+        p = _lib._ptr
+        self.ba._ck(self.lib.pvio_b200_batch_window_download(
+            self.h, n, p(s, C.c_int32), p(nf, C.c_int32), p(fr, C.c_double), fs, p(nt, C.c_int32), T, p(ids, C.c_int32),
+            p(rho, C.c_double), p(an, C.c_int32), p(cnt, C.c_int32), p(val, C.c_uint8), p(q, C.c_double)))
+        out = []
+        for i in range(n):
+            N, k = int(nf[i]), int(nt[i])
+            out.append(dict(frames=fr[i, :16 * N].reshape(N, 16).copy(), ids=ids[i, :k].copy(), inv_depth=rho[i, :k].copy(),
+                            anchor=an[i, :k].copy(), n_obs=cnt[i, :k].copy(), valid=val[i, :k].copy(), quality=q[i, :k].copy()))
+        return out

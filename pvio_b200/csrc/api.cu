@@ -66,7 +66,7 @@ static void refresh_arrays(Handle *h) {
     a.bufs = lin_bufs(h);
 }
 
-static int ensure_inertial(Handle *h) {
+int ensure_inertial(Handle *h) {
     if (h->have_inertial) return 0;
     const size_t W = h->W, N = h->Ncap, M = h->Mcap, dcap = 15 * N;
     cudaStreamSynchronize(h->stream);
@@ -120,8 +120,9 @@ static int ensure_planes(Handle *h, int T, int O) {
 
 // ------------------------------------------------------------------------ small kernels
 // Lambda = S^T S of the marginalisation prior (once per upload; constant across iterations)
-__global__ void prior_lambda_kernel(const WinHdr *hdr, const double *S, double *L, int Ncap, int w0) {
-    const int w = blockIdx.x + w0;
+// slots (may be NULL): CTA row b works on window slots[b] instead of w0 + b
+__global__ void prior_lambda_kernel(const WinHdr *hdr, const double *S, double *L, int Ncap, int w0, const int32_t *slots) {
+    const int w = slots ? slots[blockIdx.x] : blockIdx.x + w0;
     const int d = 15 * hdr[w].n_prior, dcap = 15 * Ncap;
     const double *Sw = S + (size_t)w * dcap * dcap;
     double *Lw = L + (size_t)w * dcap * dcap;
@@ -138,8 +139,8 @@ __global__ void prior_lambda_kernel(const WinHdr *hdr, const double *S, double *
 // (anchor included) and mean pixel reprojection error.  One group of 16 lanes per landmark.
 __global__ void postpass_kernel(const WinHdr *hdr, const WinConst *cst, const ObsRec *obs, const LmRec *lms,
                                 const double *rho, const double *frames, uint8_t *valid, double *quality,
-                                double *err_acc, int Ncap, int Mcap, int Kcap, int w0) {
-    const int w = blockIdx.y + w0;
+                                double *err_acc, int Ncap, int Mcap, int Kcap, int w0, const int32_t *slots) {
+    const int w = slots ? slots[blockIdx.y] : blockIdx.y + w0;
     const WinHdr &H = hdr[w];
     const WinConst &wc = cst[w];
     __shared__ FrameSm F[kMaxFrames];
@@ -238,6 +239,7 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
             if (w->pt_obs_frame[i] < 0 || w->pt_obs_frame[i] >= N) return fail(h, PVIO_B200_EINVAL, "pt_obs_frame out of range");
     }
     if (n_imu > 0 || n_prior > 0 || inertial) TRY(ensure_inertial(h));
+    if (slot < (int)h->bw.slot.size()) h->bw.slot[slot].on = false;     // a packed slot is no longer a resident window
     WinHdr &H = h->hdr.h[slot];
     WinConst &C = h->cst.h[slot];
     memset(&H, 0, sizeof(H));
@@ -373,7 +375,7 @@ static int upload_range(Handle *h, int w0, int n, cudaStream_t st) {
         }
         for (int i = w0; i < w0 + n; ++i) any_prior |= h->hdr.h[i].n_prior > 0;
         if (any_prior) {
-            prior_lambda_kernel<<<dim3(n, n < 64 ? 32 : 1), 256, 0, st>>>(h->hdr.d, h->prior_S.d, h->prior_L.d, h->Ncap, w0);
+            prior_lambda_kernel<<<dim3(n, n < 64 ? 32 : 1), 256, 0, st>>>(h->hdr.d, h->prior_S.d, h->prior_L.d, h->Ncap, w0, nullptr);
             ++h->launches;
         }
     }
@@ -415,6 +417,7 @@ struct StepCfg {
     int w0 = 0;                    // first window (sub-batch pipelining)
     int fork_aux = 0;              // latency path: the non-vision candidate cost runs beside the candidate's linearisation sweep
     cudaStream_t stream = nullptr; // nullptr: the handle's stream
+    const int32_t *slots = nullptr;// device list of the windows of the sweeps (PipeArgs::slots); nullptr: [w0, w0 + n)
 };
 
 // what the windows [w0, w0 + n) need from the launch: worst case over the batch
@@ -438,10 +441,10 @@ static size_t solve_smem_one(const WinHdr &H, bool lean) {
     return sizeof(double) * ((nb + 1) * (nb + 2) / 2 * 18 + 4 * Dp + (size_t)H.N * 36 + scr);   // tiles of kTP = 18 doubles (ba_solve.cuh)
 }
 
-static BatchShape batch_shape(Handle *h, int w0, int n, bool by_capacity) {
+static BatchShape batch_shape(Handle *h, int w0, int n, bool by_capacity, const int32_t *h_slots = nullptr) {
     BatchShape b;
-    for (int i = w0; i < w0 + n; ++i) {
-        const WinHdr &H = h->hdr.h[i];
+    for (int k = w0; k < w0 + n; ++k) {
+        const WinHdr &H = h->hdr.h[h_slots ? h_slots[k - w0] : k];
         b.N = std::max(b.N, H.N); b.M = std::max(b.M, H.M);
         const unsigned allm = (1u << H.N) - 1u, freem = ~(unsigned)H.fixed_mask & allm;
         b.nfree = std::max(b.nfree, __builtin_popcount(freem));
@@ -462,7 +465,7 @@ static BatchShape batch_shape(Handle *h, int w0, int n, bool by_capacity) {
 
 static PipeArgs pipe_args(Handle *h, const StepCfg &c) {
     PipeArgs a = launch_args<PipeArgs>(h);
-    a.compute_scale = c.compute_scale; a.mu_override = c.mu; a.w0 = c.w0; a.loop = c.loop;
+    a.compute_scale = c.compute_scale; a.mu_override = c.mu; a.w0 = c.w0; a.loop = c.loop; a.slots = c.slots;
     return a;
 }
 
@@ -494,7 +497,7 @@ static size_t schur_launch_smem(int N, int nfree) { return schur_smem_bytes<real
 // per window: the latency path)
 static __global__ void zero_system_kernel(PipeArgs a_in, int npairs_cap) {
     PipeArgs a = a_in;
-    const int w = blockIdx.x + a.w0;
+    const int w = a.slots ? a.slots[blockIdx.x] : blockIdx.x + a.w0;
     const int bsel = pipe_buffer(a, w);
     if (bsel < 0) return;
     pipe_select(a, bsel);
@@ -594,10 +597,10 @@ static int run_linearize(Handle *h, int n, const StepCfg &c, const BatchShape &b
     return 0;
 }
 
-int run_marg_vision(Handle *h, int n) {
+int run_marg_vision(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots) {
     StepCfg c;
-    c.mu = 0.0; c.compute_scale = 1;
-    const BatchShape b = batch_shape(h, 0, n, false);
+    c.mu = 0.0; c.compute_scale = 1; c.slots = d_slots;
+    const BatchShape b = batch_shape(h, 0, n, false, h_slots);
     return run_linearize(h, n, c, b, false, true);
 }
 
@@ -713,15 +716,17 @@ static int iteration_body(Handle *h, int n, const StepCfg &c, const BatchShape &
 // bodies.  For the latency path (a few windows from window 0) the sequence is captured once into a CUDA graph keyed by
 // (n, max_iter, flags) with capacity-sized launch shapes, and replayed: ONE launch per solve, no device -> host traffic
 // inside.  The graphs bake in w0 = 0.
-static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaStream_t st) {
+static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaStream_t st, bool init = true) {
     StepCfg c;
     c.mu = -1.0; c.loop = 1; c.alias_bias = o.alias_bias; c.compute_scale = 0; c.w0 = w0; c.stream = st;
     const bool graphable = w0 == 0 && n * 2 < h->sm_count;
     const BatchShape b = batch_shape(h, w0, n, graphable);
     const int bodies = o.max_iter + 2;               // spare bodies absorb retries of a failed linear solve (mu *= 10)
-    init_ctrl_kernel<<<n, 32, 0, st>>>(h->ctrl.d, 1e-8, o.radius0, o.max_iter, o.max_time, w0);
-    ++h->launches;
-    LAUNCH_CK(h, "init_ctrl_kernel");
+    if (init) {
+        init_ctrl_kernel<<<n, 32, 0, st>>>(h->ctrl.d, 1e-8, o.radius0, o.max_iter, o.max_time, w0);
+        ++h->launches;
+        LAUNCH_CK(h, "init_ctrl_kernel");
+    }
     if (!graphable) {
         for (int it = 0; it < bodies; ++it) TRY(iteration_body(h, n, c, b, it == 0));
         return 0;
@@ -758,10 +763,33 @@ static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaS
     return 0;
 }
 
-static int run_postpass(Handle *h, int n, bool want_flags, double *err_acc) {
+static int run_postpass(Handle *h, int n, bool want_flags, double *err_acc, const int32_t *slots = nullptr) {
     postpass_kernel<<<dim3(n * 2 < h->sm_count ? 8 : 1, n), 256, 0, h->stream>>>(
         h->hdr.d, h->cst.d, h->obs.d, h->lms.d, h->rho.d, h->frames.d, want_flags ? h->valid.d : nullptr,
-        want_flags ? h->quality.d : nullptr, err_acc, h->Ncap, h->Mcap, h->Kcap, 0);
+        want_flags ? h->quality.d : nullptr, err_acc, h->Ncap, h->Mcap, h->Kcap, 0, slots);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+int run_postpass_slots(Handle *h, int n, const int32_t *slots) { return run_postpass(h, n, true, nullptr, slots); }
+
+int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named) {
+    const SolveOptions o = solve_options(opt);
+    init_ctrl_kernel<<<n, 32, 0, h->stream>>>(h->ctrl.d, 1e-8, o.radius0, o.max_iter, o.max_time, 0, named);
+    ++h->launches;
+    LAUNCH_CK(h, "init_ctrl_kernel");
+    return run_solve_loop(h, o, 0, n, h->stream, false);
+}
+
+int launch_layout_tail(Handle *h, const int32_t *slots, int n, bool prior) {
+    if (prior) {
+        prior_lambda_kernel<<<dim3(n, n < 64 ? 32 : 1), 256, 0, h->stream>>>(h->hdr.d, h->prior_S.d, h->prior_L.d, h->Ncap, 0, slots);
+        ++h->launches;
+    }
+    FobsArgs fa = launch_args<FobsArgs>(h);
+    fa.slots = slots;
+    fobs_build_kernel<<<n, 256, 0, h->stream>>>(fa);
     ++h->launches;
     CK(h, cudaGetLastError());
     return 0;
@@ -885,6 +913,7 @@ static int ensure_pipeline_streams(Handle *h, int nsub) {
 template <typename Work, typename Download, typename Scatter>
 static int run_host_pipeline(Handle *h, int n, Work work, Download download, Scatter scatter) {
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
+    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "upload: the range holds a resident window (pvio_b200_batch_window_*)");
     const std::vector<int> sizes = sub_batches(n);
     const int nsub = (int)sizes.size();
     if (nsub == 1) {
@@ -1090,6 +1119,7 @@ int pvio_b200_batch_replicate(pvio_b200_handle hh, int n) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
+    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_replicate: the range holds a resident window (pvio_b200_batch_window_*)");
     if (h->prior_resident[0] && h->hdr.h[0].n_prior > 0)
         return fail(h, PVIO_B200_EINVAL, "batch_replicate: slot 0's prior is device-resident, its staging does not hold it");
     for (int i = 1; i < n; ++i) {
@@ -1106,6 +1136,7 @@ int pvio_b200_batch_replicate(pvio_b200_handle hh, int n) {
 int pvio_b200_batch_upload(pvio_b200_handle hh, int n) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
+    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_upload: the range holds a resident window (pvio_b200_batch_window_*)");
     return upload(h, n);
 }
 
@@ -1113,6 +1144,7 @@ int pvio_b200_batch_gn_step(pvio_b200_handle hh, int n, double mu, int apply) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->n_uploaded) return fail(h, PVIO_B200_EINVAL, "windows not uploaded");
+    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_gn_step: the range holds a resident window (pvio_b200_batch_window_*)");
     StepCfg c;
     c.mu = mu; c.apply = apply; c.compute_scale = 1;
     return run_gn_step(h, n, c, batch_shape(h, 0, n, false));
@@ -1121,6 +1153,7 @@ int pvio_b200_batch_gn_step(pvio_b200_handle hh, int n, double mu, int apply) {
 int pvio_b200_batch_download(pvio_b200_handle hh, int n, double *dx, int64_t dx_stride, double *costs) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
+    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_download: the range holds a resident window (pvio_b200_batch_window_*)");
     return download_dx(h, n, dx, dx_stride, costs);
 }
 
@@ -1144,6 +1177,7 @@ int pvio_b200_batch_solve(pvio_b200_handle hh, int n, const pvio_b200_options *o
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->n_uploaded) return fail(h, PVIO_B200_EINVAL, "windows not uploaded");
+    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_solve: the range holds a resident window (pvio_b200_batch_window_*)");
     return run_solve_loop(h, solve_options(opt), 0, n, h->stream);
 }
 
@@ -1152,6 +1186,8 @@ int pvio_b200_batch_download_state(pvio_b200_handle hh, int n, double *frames, i
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
+    if (any_resident(h, 0, n))
+        return fail(h, PVIO_B200_EINVAL, "batch_download_state: the range holds a resident window (pvio_b200_batch_window_*)");
     TRY(download_state_async(h, 0, n, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     scatter_states(h, 0, n, frames, frames_stride, inv_depth, inv_depth_stride, summaries);
@@ -1263,6 +1299,8 @@ int pvio_b200_ba_marginalize(pvio_b200_handle hh, const pvio_b200_window *w, con
 int pvio_b200_batch_marginalize(pvio_b200_handle hh, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
+    if (n >= 1 && n <= h->W && any_resident(h, 0, n))
+        return fail(h, PVIO_B200_EINVAL, "batch_marginalize: the range holds a resident window (pvio_b200_batch_window_*)");
     return batch_marginalize_impl(h, n, S_out, S_stride, e_out, e_stride);
 }
 

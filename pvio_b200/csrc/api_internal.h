@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <algorithm>
 #include <array>
 #include <cstring>
 #include <map>
@@ -145,6 +146,29 @@ struct ResidentWindow {
     std::vector<uint8_t> lm_in_victim;
 };
 
+// batch_window.cu: the resident windows of the batched slots.  Per slot the host keeps integers only: the frame count,
+// the prior's frame count, the fixed mask, and for every live track (rows in id order) its id and frame mask; the device
+// keeps the track table (frame mask, inverse depth, fp64 keypoint per window frame, post-pass flags) and the packed window.
+struct BwSlot {
+    bool on = false;                  // resident: the slot changes through pvio_b200_batch_window_* only
+    int N = 0, n_prior = 0, fixed = 0, inertial = 0;
+    int32_t next_id = 0;
+    std::vector<int32_t> ids;         // live tracks, increasing: row r of the device table holds track ids[r]
+    std::vector<uint32_t> mask;       // frame mask of each row
+};
+struct BatchWindows {
+    std::vector<BwSlot> slot;                    // [W]
+    DevBuf<int32_t> tid;                         // [W][Mcap] track id of each row
+    DevBuf<uint32_t> tmask;                      // [W][Mcap] frames observing it (0: free row)
+    DevBuf<double> trho;                         // [W][Mcap] inverse depth in its anchor (lowest) frame
+    DevBuf<double2> tz;                          // [W][Mcap][Ncap] fp64 keypoint per window frame
+    DevBuf<uint8_t> tvalid;                      // [W][Mcap] post-pass result of the last solve
+    DevBuf<double> tqual;                        // [W][Mcap]
+    DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
+    DevBuf<uint8_t> named;                       // [W] device: 1 for the slots a solve names
+    DevBuf<uint8_t> stage;                       // both sides, grown: the one upload / download of a call
+};
+
 struct Handle {
     int device = 0;
     int W = 1, Ncap = 0, Mcap = 0, Kcap = 0;
@@ -225,7 +249,15 @@ struct Handle {
     FmState fm;
     DevBuf<double> pnp;                           // pnp.cu: both sides, grown on demand to the largest batch (records,
                                                   // points, IMU records, frames) seen
+    BatchWindows bw;                              // batch_window.cu (empty until the first pvio_b200_batch_window_reset)
 };
+
+// whether any of the slots [w0, w0 + n) holds a resident window (batch_window.cu)
+inline bool any_resident(const Handle *h, int w0, int n) {
+    for (int i = std::max(w0, 0); i < w0 + n && i < (int)h->bw.slot.size(); ++i)
+        if (h->bw.slot[i].on) return true;
+    return false;
+}
 
 int fail(Handle *h, int code, const char *what, cudaError_t e = cudaSuccess);
 
@@ -296,8 +328,21 @@ int reserve(Handle *h, DevBuf<T> &b, size_t n, int sides) {
 // api.cu: pack window into slot 0, copy it to the device, build the frame-major table
 int pack_and_upload(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s);
 // api.cu: linearise + Schur of the uploaded windows [0, n) with the fp64 pipeline, no loss (the marginaliser's reprojection part)
-int run_marg_vision(Handle *h, int n);
+// h_slots / d_slots (may be NULL): host / device copies of a list of the n windows, instead of [0, n)
+int run_marg_vision(Handle *h, int n, const int32_t *h_slots = nullptr, const int32_t *d_slots = nullptr);
 void drop_graphs(Handle *h);
+// api.cu, for the resident batched windows (batch_window.cu)
+int ensure_inertial(Handle *h);
+// the trust-region solve of windows [0, n); named (device, [n], may be NULL): only windows with named[w] != 0 are solved,
+// the others are marked finished before the first body and cost no iteration
+int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named);
+int run_postpass_slots(Handle *h, int n, const int32_t *slots);   // post-pass of the n windows of a device list
+// the frame-major table of the n windows slots[0 .. n) (device list), and Lambda = S^T S of their priors when prior
+int launch_layout_tail(Handle *h, const int32_t *slots, int n, bool prior);
+// ba_marg.cu: the marginaliser (index 0, new prior into the slots) of the n windows h_slots / d_slots (host / device
+// copies of one list)
+int named_marginalize_impl(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots);
+bool marg_eig_fits(int dk);
 // klt.cu
 int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int width, int height, int stride,
                    const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points,

@@ -11,12 +11,13 @@ namespace pvio {
 
 struct FobsArgs : BatchArrays {      // obs -> fz, flm, seg
     int w0;
+    const int32_t *slots;            // may be NULL: CTA b builds window slots[b] instead of w0 + b
 };
 
 __host__ __device__ __forceinline__ int seg_index(int t, int a) { return t * (t - 1) / 2 + a; }
 
 __global__ void __launch_bounds__(256) fobs_build_kernel(FobsArgs a) {
-    const int w = blockIdx.x + a.w0;
+    const int w = a.slots ? a.slots[blockIdx.x] : blockIdx.x + a.w0;
     const WinHdr &H = a.hdr[w];
     const int N = H.N, nch = H.n_chunks;
     const int tid = threadIdx.x, lane = tid & 31, wv = tid >> 5;

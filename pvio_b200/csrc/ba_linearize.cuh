@@ -40,6 +40,7 @@ struct PipeArgs : BatchArrays {
     int loop;                    // 1: iteration of the device-side trust-region loop (ba_tr.cuh): obey the window's flags
     int spec;                    // loop only. 1: linearise the CANDIDATE (frames_cand, rho_cand) into the window's other buffer set
     int lm_part;                 // 1 (one CTA per window only): the (j.j, j.r) sums stay in shared memory, jr is not touched
+    const int32_t *slots;        // may be NULL: CTA row b works on window slots[b] instead of w0 + b (a named-slot list)
 };
 
 __device__ __forceinline__ void pipe_select(PipeArgs &a, int b) {
@@ -408,7 +409,7 @@ __device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N
 template <typename real>
 __global__ void __launch_bounds__(128) lm_finish_kernel(PipeArgs a_in) {
     PipeArgs a = a_in;
-    const int w = blockIdx.y + a.w0;
+    const int w = a.slots ? a.slots[blockIdx.y] : blockIdx.y + a.w0;
     const int bsel = pipe_buffer(a, w);
     if (bsel < 0) return;
     pipe_select(a, bsel);
@@ -447,7 +448,7 @@ lin_obs_kernel(PipeArgs a_in) {
     typedef typename Vec2<real>::type real2;
     constexpr int kThreads = kWarps * 32;
     PipeArgs a = a_in;
-    const int w = blockIdx.y + a.w0;
+    const int w = a.slots ? a.slots[blockIdx.y] : blockIdx.y + a.w0;
     const int bsel = pipe_buffer(a, w);
     if (bsel < 0) return;
     pipe_select(a, bsel);

@@ -33,10 +33,11 @@ struct MargArgs : BatchArrays {        // Hred, gred: set 0 of the vision part (
     int w0;                            // window of CTA 0
     double *buf;                       // chunk scratch: block c belongs to window w0 + c
     MargLayout L;
+    const int32_t *slots;              // may be NULL: block c belongs to window slots[w0 + c] instead
 };
 
 __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
-    const int w = a.w0 + blockIdx.x;
+    const int w = a.slots ? a.slots[a.w0 + blockIdx.x] : a.w0 + blockIdx.x;
     const WinHdr &Hh = a.hdr[w];
     const WinConst &wc = a.cst[w];
     const int N = Hh.N, n = 15 * N;
@@ -151,11 +152,12 @@ __global__ void __launch_bounds__(256) marg_assemble_kernel(MargArgs a) {
 
 // Frame Schur complement :547-581.  inv = H[vv]^-1 by Gauss-Jordan with partial pivoting
 // (Eigen's dynamic .inverse() is PartialPivLU based), then Hk = H[kk] - H[kv] inv H[vk].
-__global__ void __launch_bounds__(256) marg_reduce_kernel(const WinHdr *hdr, int w0, int index, double *buf, MargLayout L) {
+__global__ void __launch_bounds__(256) marg_reduce_kernel(const WinHdr *hdr, int w0, int index, double *buf, MargLayout L,
+                                                          const int32_t *slots) {
     double *const blk = buf + blockIdx.x * L.stride;
     const double *H = blk + L.H, *b = blk + L.b;
     double *Hk = blk + L.Hk, *bk = blk + L.bk;
-    const int n = 15 * hdr[w0 + blockIdx.x].N, dk = n - 15, v0 = 15 * index;
+    const int n = 15 * hdr[slots ? slots[w0 + blockIdx.x] : w0 + blockIdx.x].N, dk = n - 15, v0 = 15 * index;
     const int tid = threadIdx.x, nt = blockDim.x;
     __shared__ double M[15][31];
     __shared__ int piv_sm;
@@ -243,14 +245,17 @@ __device__ long long g_marg_stamps[8];
 
 // Per window (CTA c: window w0 + c): S [c * S_stride] dense n x n row-major, evec [c * e_stride]; x0 (may be NULL): the
 // linearisation point of the new prior, frames 1 .. N - 1 of the window's state (frames, x0: window w0's, x_stride apart).
+// slots (may be NULL): CTA c works on window w = slots[w0 + c] and its outputs are at [w * stride] instead.
 __global__ void __launch_bounds__(256) marg_eig_kernel(const WinHdr *hdr, int w0, const double *buf, MargLayout L, int ring,
                                                        double *S_all, size_t S_stride, double *e_all, size_t e_stride,
-                                                       const double *frames, double *x0, size_t x_stride) {
+                                                       const double *frames, double *x0, size_t x_stride,
+                                                       const int32_t *slots) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x, nt = blockDim.x;
-    const int c = blockIdx.x, N = hdr[w0 + c].N, n = 15 * (N - 1);
+    const int c = blockIdx.x, w = slots ? slots[w0 + c] : w0 + c, N = hdr[w].N, n = 15 * (N - 1);
+    const size_t o = slots ? (size_t)w : (size_t)c;
     const double *Ain = buf + c * L.stride + L.Hk, *bvec = buf + c * L.stride + L.bk;
-    double *S = S_all + c * S_stride, *evec = e_all + c * e_stride;
+    double *S = S_all + o * S_stride, *evec = e_all + o * e_stride;
     const int ld = n | 1;
     double *a = reinterpret_cast<double *>(smem_raw);       // [n][ld]: matrix -> eigenvectors (columns)
     double *d = a + (size_t)n * ld;                         // [n]
@@ -423,7 +428,7 @@ __global__ void __launch_bounds__(256) marg_eig_kernel(const WinHdr *hdr, int w0
         evec[i] = il * dot;
     }
     if (x0)
-        for (int i = tid; i < (N - 1) * kFrameStride; i += nt) x0[c * x_stride + i] = frames[c * x_stride + kFrameStride + i];
+        for (int i = tid; i < (N - 1) * kFrameStride; i += nt) x0[o * x_stride + i] = frames[o * x_stride + kFrameStride + i];
     MARG_STAMP(4);
 }
 
@@ -489,7 +494,7 @@ static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLa
         const int cn = std::min(chunk, n - w0);
         m.w0 = w0;
         marg_assemble_kernel<<<cn, 256, 0, h->stream>>>(m);
-        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, buf, L);
+        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, buf, L, nullptr);
         h->launches += 2;
         if (!eig) continue;
         int dk = 0;
@@ -498,10 +503,10 @@ static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLa
         if (to_slots)
             marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring,
                 h->prior_S.dslot(w0), h->prior_S.per, h->prior_e.dslot(w0), h->prior_e.per, h->frames.dslot(w0),
-                h->prior_x0.dslot(w0), h->prior_x0.per);
+                h->prior_x0.dslot(w0), h->prior_x0.per, nullptr);
         else
             marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring,
-                buf + L.S, L.stride, buf + L.e, L.stride, nullptr, nullptr, 0);
+                buf + L.S, L.stride, buf + L.e, L.stride, nullptr, nullptr, 0, nullptr);
         ++h->launches;
     }
     CK(h, cudaGetLastError());
@@ -532,6 +537,35 @@ int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
     if (keep_on_device) h->prior_resident[0] = N - 1;
+    return 0;
+}
+
+bool marg_eig_fits(int dk) { return eig_fits(dk); }
+
+// The marginaliser of frame 0 for the n resident windows of a list (batch_window.cu: pvio_b200_batch_window_drop_victim),
+// checked by the caller: every kernel, the vision sweeps included, works on the listed windows only, each new prior into
+// its own slot.
+int named_marginalize_impl(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots) {
+    const int chunk = std::min(n, kMargChunkPerSm * h->sm_count);
+    const MargLayout L = marg_layout(h);
+    TRY(reserve(h, h->marg, L.stride * chunk, kDevice));
+    TRY(run_marg_vision(h, n, h_slots, d_slots));
+    double *buf = h->marg.d;
+    MargArgs m = launch_args<MargArgs>(h);
+    m.index = 0; m.buf = buf; m.L = L; m.slots = d_slots;
+    for (int w0 = 0; w0 < n; w0 += chunk) {
+        const int cn = std::min(chunk, n - w0);
+        m.w0 = w0;
+        marg_assemble_kernel<<<cn, 256, 0, h->stream>>>(m);
+        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, 0, buf, L, d_slots);
+        int dk = 0;
+        for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[h_slots[i]].N - 1));
+        const EigLaunch el = eig_launch(dk);
+        marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring, h->prior_S.d, h->prior_S.per,
+            h->prior_e.d, h->prior_e.per, h->frames.d, h->prior_x0.d, h->prior_x0.per, d_slots);
+        h->launches += 3;
+    }
+    CK(h, cudaGetLastError());
     return 0;
 }
 
@@ -595,7 +629,7 @@ int selftest_eig_impl(Handle *h, int n, const int32_t *dk, const double *A, cons
     CK(h, cudaMemcpyAsync(hdr.d, hdr.h, sizeof(WinHdr) * n, cudaMemcpyHostToDevice, h->stream));
     const EigLaunch el = eig_launch(dmax);
     marg_eig_kernel<<<n, 256, el.smem, h->stream>>>(hdr.d, 0, buf.d, L, el.ring, out, L.stride, out + L.bk, L.stride,
-                                                   nullptr, nullptr, 0);
+                                                   nullptr, nullptr, 0, nullptr);
     ++h->launches;
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(buf.h, out, sizeof(double) * n * L.stride, cudaMemcpyDeviceToHost, h->stream));

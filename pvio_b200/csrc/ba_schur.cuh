@@ -61,7 +61,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks)
 schur_kernel(PipeArgs a_in) {
     typedef typename Vec2<real>::type real2;
     PipeArgs a = a_in;
-    const int w = blockIdx.y + a.w0;
+    const int w = a.slots ? a.slots[blockIdx.y] : blockIdx.y + a.w0;
     if (a.loop) {
         const WinCtrl &c = a.ctrl[w];
         if (c.done || c.reuse) return;

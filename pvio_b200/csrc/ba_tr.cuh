@@ -122,8 +122,11 @@ __device__ inline bool tr_decide(WinCtrl &c, const double *acc, double cand_vis,
     return accept;
 }
 
-static __global__ void init_ctrl_kernel(WinCtrl *ctrl, double mu, double radius, int max_iter, double max_time_s, int w0) {
+// named (may be NULL): a window with named[w] == 0 is only marked finished, so that every kernel of the loop skips it
+static __global__ void init_ctrl_kernel(WinCtrl *ctrl, double mu, double radius, int max_iter, double max_time_s, int w0,
+                                        const uint8_t *named = nullptr) {
     WinCtrl &c = ctrl[blockIdx.x + w0];
+    if (named && !named[blockIdx.x + w0]) { if (threadIdx.x == 0) c.done = 1; return; }
     if (threadIdx.x == 0) {
         c.mu = mu; c.radius = radius; c.iteration = 0; c.accepted = 0; c.done = 0;
         c.termination = PVIO_B200_TERM_NO_CONVERGENCE; c.solve_failed = 0; c.have_scale = 0; c.usable = 1;

@@ -1,0 +1,804 @@
+// Resident sliding windows of the batched slots (pvio_b200_batch_window_*): the many-sequence counterpart of resident.cu.
+// A resident slot keeps its whole window on the device -- frame states, IMU records, the prior, and a TRACK TABLE with
+// every live track's frame mask, inverse depth and fp64 keypoint per window frame.  Per camera frame the host sends only
+// what changed (edit records); the packed tables the solve kernels read (LmRec, ObsRec, rho, WinHdr, the frame-major
+// table) are rebuilt from the track table on the device, exactly as pack_window builds them from resident.cu's
+// build_view: tracks with >= 2 observations in id order, stably sorted by anchor (their lowest frame).
+//
+// The host keeps integers only (frame count, prior size, fixed mask, the id and frame mask of every live row), enough to
+// check every call completely before anything is staged, and to know the launch shapes.  The rows of a slot's table are
+// its live tracks in id order: removals compact the table (the storage of dead tracks is reused), new tracks append.
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
+#include "api_internal.h"
+
+namespace pvio {
+
+// ------------------------------------------------------------------------ staged records (host -> device)
+struct BwEdit {                       // one slot's edit, applied by bw_edit_kernel
+    int32_t slot, N_old, T_old, replace_last;
+    int32_t n_rm, rm_off;             // rows of the table BEFORE compaction
+    int32_t frame, has_imu, x_off;    // new frame index (-1: none); its state [16] (+ IMU record) at doubles x_off
+    int32_t n_new, new_off, n_obs, obs_off;
+    int32_t out_off;                  // ints of the result: live rows after the edit, then the new ids
+};
+struct BwNew { int32_t row, id, frame, pad; double zx, zy, rho; };
+struct BwObs { int32_t row, frame; double zx, zy; };
+struct BwLayout { int32_t slot, N, T, fixed, n_prior, inertial; };     // a slot's window as the kernels rebuild it
+struct BwDl { int32_t slot, N, T, pad; int64_t off; };                  // download: bytes into the result area
+
+struct BwArgs {
+    WinHdr *hdr;
+    WinConst *cst;
+    LmRec *lms;
+    ObsRec *obs;
+    double *rho, *frames, *imu_data;
+    int32_t *imu_idx, *prior_frames;
+    int32_t *tid;
+    uint32_t *tmask;
+    double *trho;
+    double2 *tz;
+    uint8_t *tvalid;
+    double *tqual;
+    int32_t *lm_row;
+    const uint8_t *valid;
+    const double *quality;
+    int Ncap, Mcap, Kcap;
+};
+
+constexpr int kBwThreads = 256;
+constexpr int kBwWarps = kBwThreads / 32;
+
+// exclusive scan of one int per thread over the CTA (kBwThreads); total: the sum
+__device__ int bw_block_scan(int v, int *sh, int &total) {
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) sh[wv] = x;
+    __syncthreads();
+    if (threadIdx.x == 0) { int s = 0; for (int k = 0; k < kBwWarps; ++k) { const int t = sh[k]; sh[k] = s; s += t; } sh[kBwWarps] = s; }
+    __syncthreads();
+    const int r = sh[wv] + x - v;
+    total = sh[kBwWarps];
+    __syncthreads();
+    return r;
+}
+
+// stable compaction of rows [0, T) of window w to the rows whose frame mask is not 0; returns the live count.  A row only
+// moves down, chunk by chunk: each chunk is read completely before it is written.
+__device__ int bw_compact(const BwArgs &a, int w, int T, int *sh) {
+    const size_t base = (size_t)w * a.Mcap;
+    int carry = 0;
+    for (int c0 = 0; c0 < T; c0 += kBwThreads) {
+        const int r = c0 + threadIdx.x;
+        const bool live = r < T && a.tmask[base + r] != 0u;
+        int tot;
+        const int d = carry + bw_block_scan(live ? 1 : 0, sh, tot);
+        int32_t id = 0; uint32_t m = 0; double rho = 0.0, q = 0.0; uint8_t v = 0;
+        if (live) { id = a.tid[base + r]; m = a.tmask[base + r]; rho = a.trho[base + r]; v = a.tvalid[base + r]; q = a.tqual[base + r]; }
+        __syncthreads();
+        if (live && d != r) { a.tid[base + d] = id; a.tmask[base + d] = m; a.trho[base + d] = rho; a.tvalid[base + d] = v; a.tqual[base + d] = q; }
+        __syncthreads();
+        for (int f = 0; f < a.Ncap; ++f) {
+            double2 z = make_double2(0.0, 0.0);
+            if (live) z = a.tz[(base + r) * a.Ncap + f];
+            __syncthreads();
+            if (live && d != r) a.tz[(base + d) * a.Ncap + f] = z;
+            __syncthreads();
+        }
+        carry += tot;
+    }
+    for (int r = carry + threadIdx.x; r < T; r += kBwThreads) a.tmask[base + r] = 0u;
+    __syncthreads();
+    return carry;
+}
+
+// One CTA per edit (each names a different slot): replace_last and removals clear mask bits, the table is compacted, then
+// the new frame, the new tracks (appended) and the observations are written.  out: live rows, then the ids stored.
+__global__ void __launch_bounds__(kBwThreads) bw_edit_kernel(BwArgs a, const BwEdit *eds, const int32_t *rm, const BwNew *nw,
+                                                              const BwObs *ob, const double *x, int32_t *out) {
+    __shared__ int sh[kBwWarps + 1];
+    const BwEdit e = eds[blockIdx.x];
+    const int w = e.slot;
+    const size_t base = (size_t)w * a.Mcap;
+    if (e.replace_last)
+        for (int r = threadIdx.x; r < e.T_old; r += kBwThreads) a.tmask[base + r] &= ~(1u << (e.N_old - 1));
+    __syncthreads();
+    for (int i = threadIdx.x; i < e.n_rm; i += kBwThreads) a.tmask[base + rm[e.rm_off + i]] = 0u;
+    __syncthreads();
+    const int T = bw_compact(a, w, e.T_old, sh);
+    if (e.frame >= 0) {
+        double *fr = a.frames + ((size_t)w * a.Ncap + e.frame) * kFrameStride;
+        for (int i = threadIdx.x; i < kFrameStride; i += kBwThreads) fr[i] = x[e.x_off + i];
+        if (e.has_imu) {
+            double *rec = a.imu_data + ((size_t)w * a.Ncap + e.frame - 1) * kImuStride;
+            for (int i = threadIdx.x; i < kImuStride; i += kBwThreads) rec[i] = x[e.x_off + kFrameStride + i];
+        }
+    }
+    for (int i = threadIdx.x; i < e.n_new; i += kBwThreads) {
+        const BwNew t = nw[e.new_off + i];
+        const size_t R = base + t.row;
+        a.tid[R] = t.id; a.tmask[R] = 1u << t.frame; a.trho[R] = t.rho; a.tvalid[R] = 0; a.tqual[R] = 0.0;
+        a.tz[R * a.Ncap + t.frame] = make_double2(t.zx, t.zy);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < e.n_obs; i += kBwThreads) {      // distinct frames per row: the masks meet in atomicOr only
+        const BwObs o = ob[e.obs_off + i];
+        atomicOr(&a.tmask[base + o.row], 1u << o.frame);
+        a.tz[(base + o.row) * a.Ncap + o.frame] = make_double2(o.zx, o.zy);
+    }
+    __syncthreads();
+    int live = 0;
+    for (int r = threadIdx.x; r < T + e.n_new; r += kBwThreads) live += a.tmask[base + r] != 0u ? 1 : 0;
+    for (int o = 16; o > 0; o >>= 1) live += __shfl_xor_sync(0xffffffffu, live, o);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = live;
+    __syncthreads();
+    if (threadIdx.x == 0) { int s = 0; for (int k = 0; k < kBwWarps; ++k) s += sh[k]; out[e.out_off] = s; }
+    for (int i = threadIdx.x; i < e.n_new; i += kBwThreads) out[e.out_off + 1 + i] = a.tid[base + nw[e.new_off + i].row];
+}
+
+// One CTA per slot: the packed window from the track table, as pack_window builds it from build_view's window.
+__global__ void __launch_bounds__(kBwThreads) bw_layout_kernel(BwArgs a, const BwLayout *lay) {
+    __shared__ int sh[kBwWarps + 1];
+    __shared__ int cnt[kMaxFrames], first[kMaxFrames], run[kMaxFrames];
+    __shared__ int wcnt[kBwWarps][kMaxFrames + 1];
+    const BwLayout L = lay[blockIdx.x];
+    const int w = L.slot, N = L.N, T = L.T;
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const size_t base = (size_t)w * a.Mcap;
+    if (threadIdx.x < kMaxFrames) { cnt[threadIdx.x] = 0; run[threadIdx.x] = 0; }
+    __syncthreads();
+    for (int r = threadIdx.x; r < T; r += kBwThreads) {
+        const uint32_t m = a.tmask[base + r];
+        if (__popc(m) >= 2) atomicAdd(&cnt[__ffs(m) - 1], 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { int s = 0; for (int k = 0; k < kMaxFrames; ++k) { first[k] = s; s += cnt[k]; } sh[kBwWarps] = s; }
+    __syncthreads();
+    const int M = sh[kBwWarps];
+    __syncthreads();
+    // landmark order: anchor, then row (= id) -- a counting sort, stable chunk by chunk
+    for (int c0 = 0; c0 < T; c0 += kBwThreads) {
+        const int r = c0 + threadIdx.x;
+        const uint32_t m = r < T ? a.tmask[base + r] : 0u;
+        const int an = __popc(m) >= 2 ? __ffs(m) - 1 : kMaxFrames;
+        for (int i = threadIdx.x; i < kBwWarps * (kMaxFrames + 1); i += kBwThreads) (&wcnt[0][0])[i] = 0;
+        __syncthreads();
+        const unsigned peers = __match_any_sync(0xffffffffu, an);
+        const int rank = __popc(peers & ((1u << lane) - 1u));
+        if (rank == 0) wcnt[wv][an] = __popc(peers);
+        __syncthreads();
+        if (threadIdx.x < kMaxFrames) {
+            int s = run[threadIdx.x];
+            for (int k = 0; k < kBwWarps; ++k) { const int c = wcnt[k][threadIdx.x]; wcnt[k][threadIdx.x] = s; s += c; }
+            run[threadIdx.x] = s;
+        }
+        __syncthreads();
+        if (an < kMaxFrames) a.lm_row[base + first[an] + wcnt[wv][an] + rank] = r;
+        __syncthreads();
+    }
+    // records: LmRec, rho, ObsRec in increasing frame order per landmark
+    int carry = 0;
+    for (int c0 = 0; c0 < M; c0 += kBwThreads) {
+        const int lp = c0 + threadIdx.x;
+        const bool ok = lp < M;
+        const int row = ok ? a.lm_row[base + lp] : 0;
+        const uint32_t m = ok ? a.tmask[base + row] : 0u;
+        const int an = ok ? __ffs(m) - 1 : 0;
+        const uint32_t seen = m & ~(1u << an);
+        const int n = ok ? __popc(seen) : 0;
+        int tot;
+        const int ob = carry + bw_block_scan(n, sh, tot);
+        if (ok) {
+            const double2 *z = a.tz + (base + row) * a.Ncap;
+            LmRec lr;
+            lr.zrx = (float)z[an].x; lr.zry = (float)z[an].y;
+            lr.meta = lm_meta(an, an == 0 ? 1 : 0, n, seen);
+            lr.obs_begin = ob;
+            a.lms[base + lp] = lr;
+            a.rho[base + lp] = a.trho[base + row];
+            ObsRec *o = a.obs + (size_t)w * a.Kcap + ob;
+            int k = 0;
+            for (uint32_t s = seen; s; s &= s - 1) {
+                const int f = __ffs(s) - 1;
+                o[k].zx = (float)z[f].x; o[k].zy = (float)z[f].y;
+                ++k;
+            }
+        }
+        carry += tot;
+    }
+    WinHdr &H = a.hdr[w];
+    for (int i = threadIdx.x; i < kMaxChunks; i += kBwThreads) { H.chunk_begin[i] = 0; H.chunk_meta[i] = 0; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const int n_imu = L.inertial ? max(N - 1, 0) : 0;
+        H.N = N; H.M = M; H.K = carry; H.use_inertial = L.inertial;
+        H.n_imu = n_imu; H.n_prior = L.inertial ? L.n_prior : 0; H.n_planes = 0; H.n_ptracks = 0;
+        H.fixed_mask = L.fixed; H.pad0 = 0; H.pad1 = 0;
+        int nch = 0;
+        for (int an = 0; an < N; ++an)
+            for (int j = 0; j < cnt[an]; j += 32) {
+                H.chunk_begin[nch] = first[an] + j;
+                H.chunk_meta[nch] = (an << 8) + min(32, cnt[an] - j);
+                ++nch;
+            }
+        H.n_chunks = nch;
+        // the mean frame position, summed in frame order as pack_window sums it
+        const double *fr = a.frames + (size_t)w * a.Ncap * kFrameStride;
+        double o[3] = {0.0, 0.0, 0.0};
+        for (int f = 0; f < N; ++f) for (int k = 0; k < 3; ++k) o[k] += fr[f * kFrameStride + 4 + k];
+        for (int k = 0; k < 3; ++k) a.cst[w].origin[k] = N > 0 ? o[k] / N : 0.0;
+        if (a.imu_idx) {
+            for (int k = 0; k < n_imu; ++k) { a.imu_idx[((size_t)w * a.Ncap + k) * 2] = k; a.imu_idx[((size_t)w * a.Ncap + k) * 2 + 1] = k + 1; }
+            for (int k = 0; k < H.n_prior; ++k) a.prior_frames[(size_t)w * a.Ncap + k] = k;
+        }
+    }
+}
+
+// After a solve and its post-pass, one CTA per named slot: solved inverse depths back into the tracks, the post-pass
+// flags of the landmarks into their rows (0 / 0 for the rows that did not take part, and for every row when the solve
+// ran no post-pass: flags == 0)
+__global__ void __launch_bounds__(kBwThreads) bw_writeback_kernel(BwArgs a, const BwLayout *lay, int flags) {
+    const BwLayout L = lay[blockIdx.x];
+    const int w = L.slot;
+    const size_t base = (size_t)w * a.Mcap;
+    for (int r = threadIdx.x; r < L.T; r += kBwThreads) { a.tvalid[base + r] = 0; a.tqual[base + r] = 0.0; }
+    __syncthreads();
+    const int M = a.hdr[w].M;
+    for (int lp = threadIdx.x; lp < M; lp += kBwThreads) {
+        const int row = a.lm_row[base + lp];
+        a.trho[base + row] = a.rho[base + lp];
+        if (flags) { a.tvalid[base + row] = a.valid[base + lp]; a.tqual[base + row] = a.quality[base + lp]; }
+    }
+}
+
+// quaternions (x, y, z, w), Hamilton product, q * v = rotate (resident.cu)
+__device__ void bw_qmul(const double *a, const double *b, double *o) {
+    o[0] = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1];
+    o[1] = a[3] * b[1] - a[0] * b[2] + a[1] * b[3] + a[2] * b[0];
+    o[2] = a[3] * b[2] + a[0] * b[1] - a[1] * b[0] + a[2] * b[3];
+    o[3] = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2];
+}
+__device__ void bw_qrot(const double *q, const double *v, double *o) {
+    const double x = q[0], y = q[1], z = q[2], w = q[3];
+    const double tx = 2.0 * (y * v[2] - z * v[1]), ty = 2.0 * (z * v[0] - x * v[2]), tz = 2.0 * (x * v[1] - y * v[0]);
+    o[0] = v[0] + w * tx + (y * tz - z * ty);
+    o[1] = v[1] + w * ty + (z * tx - x * tz);
+    o[2] = v[2] + w * tz + (x * ty - y * tx);
+}
+__device__ void bw_cam_pose(const double *fs, const WinConst &c, double *qc, double *pc) {
+    bw_qmul(fs, c.cam_q, qc);
+    double t[3];
+    bw_qrot(fs, c.cam_p, t);
+    for (int i = 0; i < 3; ++i) pc[i] = fs[4 + i] + t[i];
+}
+
+// Map::marginalize_frame(0) after the marginaliser, one CTA per slot (L.N, L.T: the window BEFORE the drop): a track
+// anchored in the victim is re-anchored in its next frame from the current states (track.cpp:42-49, quirk Q5), the
+// victim's observations leave their tracks, frames and IMU records shift down by one, dead tracks leave the table.
+__global__ void __launch_bounds__(kBwThreads) bw_drop_kernel(BwArgs a, const BwLayout *lay) {
+    __shared__ int sh[kBwWarps + 1];
+    const BwLayout L = lay[blockIdx.x];
+    const int w = L.slot, N = L.N, T = L.T;
+    const size_t base = (size_t)w * a.Mcap;
+    double *fr = a.frames + (size_t)w * a.Ncap * kFrameStride;
+    const WinConst &c = a.cst[w];
+    for (int r = threadIdx.x; r < T; r += kBwThreads) {
+        const uint32_t m = a.tmask[base + r];
+        double2 *z = a.tz + (base + r) * a.Ncap;
+        if ((m & 1u) && __popc(m) >= 2) {
+            const int nx = __ffs(m & ~1u) - 1;
+            double qa[4], pa[3], qn[4], pn[3];
+            bw_cam_pose(fr, c, qa, pa);
+            bw_cam_pose(fr + nx * kFrameStride, c, qn, pn);
+            const double rho = a.trho[base + r];
+            const double ray[3] = {z[0].x / rho, z[0].y / rho, 1.0 / rho};
+            double x[3], d[3], y[3];
+            bw_qrot(qa, ray, x);
+            for (int i = 0; i < 3; ++i) d[i] = x[i] + pa[i] - pn[i];
+            const double qc[4] = {-qn[0], -qn[1], -qn[2], qn[3]};
+            bw_qrot(qc, d, y);
+            a.trho[base + r] = 1.0 / y[2];
+        }
+        for (int f = 0; f + 1 < N; ++f) z[f] = z[f + 1];
+        a.tmask[base + r] = m >> 1;
+    }
+    __syncthreads();
+    const int nf = (N - 1) * kFrameStride;
+    for (int i0 = 0; i0 < nf; i0 += kBwThreads) {
+        const int i = i0 + threadIdx.x;
+        const double v = i < nf ? fr[kFrameStride + i] : 0.0;
+        __syncthreads();
+        if (i < nf) fr[i] = v;
+        __syncthreads();
+    }
+    if (L.inertial && N > 2) {
+        double *rec = a.imu_data + (size_t)w * a.Ncap * kImuStride;
+        const int ni = (N - 2) * kImuStride;
+        for (int i0 = 0; i0 < ni; i0 += kBwThreads) {
+            const int i = i0 + threadIdx.x;
+            const double v = i < ni ? rec[kImuStride + i] : 0.0;
+            __syncthreads();
+            if (i < ni) rec[i] = v;
+            __syncthreads();
+        }
+    }
+    bw_compact(a, w, T, sh);
+}
+
+// One CTA per slot: frames, then per row inverse depth, quality, id, anchor, observation count, valid -- packed at dl.off
+__global__ void __launch_bounds__(kBwThreads) bw_download_kernel(BwArgs a, const BwDl *dls, uint8_t *outb) {
+    const BwDl d = dls[blockIdx.x];
+    const int w = d.slot, N = d.N, T = d.T;
+    const size_t base = (size_t)w * a.Mcap;
+    double *fo = reinterpret_cast<double *>(outb + d.off);
+    double *ro = fo + (size_t)N * kFrameStride, *qo = ro + T;
+    int32_t *io = reinterpret_cast<int32_t *>(qo + T), *ao = io + T, *no = ao + T;
+    uint8_t *vo = reinterpret_cast<uint8_t *>(no + T);
+    const double *fr = a.frames + (size_t)w * a.Ncap * kFrameStride;
+    for (int i = threadIdx.x; i < N * kFrameStride; i += kBwThreads) fo[i] = fr[i];
+    for (int r = threadIdx.x; r < T; r += kBwThreads) {
+        const uint32_t m = a.tmask[base + r];
+        ro[r] = a.trho[base + r]; qo[r] = a.tqual[base + r];
+        io[r] = a.tid[base + r]; ao[r] = m ? __ffs(m) - 1 : -1; no[r] = __popc(m); vo[r] = a.tvalid[base + r];
+    }
+}
+
+// ------------------------------------------------------------------------ host side
+static BwArgs bw_args(Handle *h) {
+    BwArgs a{};
+    BatchWindows &b = h->bw;
+    a.hdr = h->hdr.d; a.cst = h->cst.d; a.lms = h->lms.d; a.obs = h->obs.d; a.rho = h->rho.d; a.frames = h->frames.d;
+    a.imu_data = h->imu_data.d; a.imu_idx = h->imu_idx.d; a.prior_frames = h->prior_frames.d;
+    a.tid = b.tid.d; a.tmask = b.tmask.d; a.trho = b.trho.d; a.tz = b.tz.d; a.tvalid = b.tvalid.d; a.tqual = b.tqual.d;
+    a.lm_row = b.lm_row.d; a.valid = h->valid.d; a.quality = h->quality.d;
+    a.Ncap = h->Ncap; a.Mcap = h->Mcap; a.Kcap = h->Kcap;
+    return a;
+}
+
+static int ensure_bw(Handle *h) {
+    BatchWindows &b = h->bw;
+    if (!b.slot.empty()) return 0;
+    const size_t W = h->W, M = h->Mcap;
+    TRY(alloc(h, b.tid, W * M, kDevice)); TRY(alloc(h, b.tmask, W * M, kDevice)); TRY(alloc(h, b.trho, W * M, kDevice));
+    TRY(alloc(h, b.tz, W * M * h->Ncap, kDevice)); TRY(alloc(h, b.tvalid, W * M, kDevice)); TRY(alloc(h, b.tqual, W * M, kDevice));
+    TRY(alloc(h, b.lm_row, W * M, kDevice)); TRY(alloc(h, b.named, W, kDevice));
+    b.slot.resize(W);
+    return 0;
+}
+
+// byte buffer of one call's upload, every section 8-byte aligned
+struct Packer {
+    std::vector<uint8_t> buf;
+    template <typename T>
+    size_t put(const T *p, size_t n) {
+        const size_t off = (buf.size() + 7) & ~(size_t)7;
+        buf.resize(off + sizeof(T) * n);
+        if (n) memcpy(buf.data() + off, p, sizeof(T) * n);
+        return off;
+    }
+};
+
+// the window of a slot as the checks and the launch shapes see it
+struct BwShape { int M = 0, K = 0, chunks = 0, max_obs = 0; };
+static BwShape shape_of(const BwSlot &s) {
+    BwShape r;
+    int cnt[kMaxFrames] = {};
+    for (uint32_t m : s.mask) {
+        const int p = __builtin_popcount(m);
+        if (p < 2) continue;
+        ++cnt[__builtin_ctz(m)]; ++r.M; r.K += p - 1; r.max_obs = std::max(r.max_obs, p - 1);
+    }
+    for (int a = 0; a < kMaxFrames; ++a) r.chunks += (cnt[a] + 31) / 32;
+    return r;
+}
+
+static int check_window(Handle *h, const BwSlot &s) {
+    const BwShape sh = shape_of(s);
+    if (s.N > h->Ncap) return fail(h, PVIO_B200_EINVAL, "batch_window: more frames than max_frames");
+    if ((int)s.ids.size() > h->Mcap) return fail(h, PVIO_B200_EINVAL, "batch_window: more live tracks than max_landmarks");
+    if (sh.K > h->Kcap) return fail(h, PVIO_B200_EINVAL, "batch_window: more observations than max_obs");
+    if (sh.max_obs >= 16) return fail(h, PVIO_B200_EINVAL, "batch_window: a landmark with 16 or more observations");
+    if (sh.chunks > kMaxChunks) return fail(h, PVIO_B200_EINVAL, "batch_window: too many landmark chunks");
+    return 0;
+}
+
+// the shape fields of the slot's host header (batch_shape and the marginaliser read them); the device header is the
+// re-layout kernel's
+static void host_header(Handle *h, int slot) {
+    const BwSlot &s = h->bw.slot[slot];
+    const BwShape sh = shape_of(s);
+    WinHdr &H = h->hdr.h[slot];
+    memset(&H, 0, sizeof(H));
+    H.N = s.N; H.M = sh.M; H.K = sh.K; H.use_inertial = s.inertial; H.n_imu = s.inertial ? std::max(s.N - 1, 0) : 0;
+    H.n_prior = s.inertial ? s.n_prior : 0; H.fixed_mask = s.fixed; H.n_chunks = sh.chunks;
+    h->slot_N[slot] = s.N; h->slot_M[slot] = sh.M; h->slot_K[slot] = sh.K;
+    h->perm[slot].clear(); h->perm_identity[slot] = 1;      // no caller landmark order: nothing of a former pack survives
+}
+
+static BwLayout layout_of(const Handle *h, int slot) {
+    const BwSlot &s = h->bw.slot[slot];
+    return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial};
+}
+
+static int check_slots(Handle *h, int n, const int32_t *slots, const char *what) {
+    if (n < 0 || (n > 0 && !slots)) return fail(h, PVIO_B200_EINVAL, what);
+    std::vector<uint8_t> seen(h->W, 0);
+    for (int i = 0; i < n; ++i) {
+        const int s = slots[i];
+        if (s < 0 || s >= h->W || h->bw.slot.empty() || !h->bw.slot[s].on)
+            return fail(h, PVIO_B200_EINVAL, "batch_window: slot out of range or not resident");
+        if (seen[s]) return fail(h, PVIO_B200_EINVAL, "batch_window: a slot named twice");
+        seen[s] = 1;
+    }
+    return 0;
+}
+
+// stage, upload, and return device pointers into the staged bytes
+static int upload_stage(Handle *h, const Packer &p, size_t out_bytes, uint8_t *&d_in, uint8_t *&d_out) {
+    const size_t in = (p.buf.size() + 15) & ~(size_t)15;
+    TRY(reserve(h, h->bw.stage, in + out_bytes + 16, kBoth));
+    if (!p.buf.empty()) {
+        memcpy(h->bw.stage.h, p.buf.data(), p.buf.size());
+        CK(h, cudaMemcpyAsync(h->bw.stage.d, h->bw.stage.h, p.buf.size(), cudaMemcpyHostToDevice, h->stream));
+    }
+    d_in = h->bw.stage.d;
+    d_out = h->bw.stage.d + in;
+    return 0;
+}
+
+// re-layout of the slots whose BwLayout records start at byte `off` of the upload (list of int32 slots at slots_off)
+static int relayout(Handle *h, uint8_t *d_in, size_t lay_off, size_t slots_off, int n, bool prior) {
+    if (n == 0) return 0;
+    bw_layout_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(d_in + lay_off));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    return launch_layout_tail(h, reinterpret_cast<const int32_t *>(d_in + slots_off), n, prior);
+}
+
+static int find_row(const BwSlot &s, int32_t id) {
+    const auto it = std::lower_bound(s.ids.begin(), s.ids.end(), id);
+    return (it == s.ids.end() || *it != id) ? -1 : (int)(it - s.ids.begin());
+}
+
+}  // namespace pvio
+
+using namespace pvio;
+
+extern "C" {
+
+int pvio_b200_batch_window_reset(pvio_b200_handle hh, int slot, const pvio_b200_window *w) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h || !w) return PVIO_B200_EINVAL;
+    if (slot < 0 || slot >= h->W) return fail(h, PVIO_B200_EINVAL, "batch_window_reset: slot out of range");
+    if (w->n_planes > 0 || w->n_plane_tracks > 0) return fail(h, PVIO_B200_EINVAL, "batch_window_reset: resident windows carry no planes");
+    TRY(ensure_bw(h));
+    if (w->use_inertial) TRY(ensure_inertial(h));
+    BwSlot &s = h->bw.slot[slot];
+    s = BwSlot();
+    s.on = true; s.inertial = w->use_inertial ? 1 : 0;
+    h->prior_resident[slot] = 0;
+    host_header(h, slot);
+    WinConst &C = h->cst.h[slot];
+    memset(&C, 0, sizeof(C));
+    memcpy(C.cam_q, w->cam_q_cs, 32); memcpy(C.cam_p, w->cam_p_cs, 24);
+    memcpy(C.imu_q, w->imu_q_cs, 32); memcpy(C.imu_p, w->imu_p_cs, 24);
+    memcpy(C.sic, w->sqrt_inv_cov, 32);
+    C.fx = w->fx; C.fy = w->fy; C.cauchy_a = w->cauchy_a > 0 ? w->cauchy_a : 1.0; C.plane_sic = w->plane_sqrt_inv_cov;
+    CK(h, cudaMemcpyAsync(h->cst.dslot(slot), &C, sizeof(WinConst), cudaMemcpyHostToDevice, h->stream));
+    Packer p;
+    const BwLayout L = layout_of(h, slot);
+    const size_t lay = p.put(&L, 1), sl = p.put(&slot, 1);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    TRY(relayout(h, din, lay, sl, 1, false));
+    CK(h, cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+int pvio_b200_batch_window_set_prior(pvio_b200_handle hh, int slot, int n_prior, const double *S, const double *e,
+                                     const double *state0) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    TRY(check_slots(h, 1, &slot, "batch_window_set_prior: bad slot"));
+    BwSlot &s = h->bw.slot[slot];
+    if (n_prior < 0 || (n_prior > 0 && (!S || !e || !state0))) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: null prior");
+    if (!s.inertial && n_prior > 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: the window carries no motion states");
+    if (n_prior > s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: prior over more frames than the window holds");
+    const size_t d = 15 * (size_t)n_prior;
+    if (d > 0) {
+        memcpy(h->prior_S.slot(slot), S, sizeof(double) * d * d);
+        memcpy(h->prior_e.slot(slot), e, sizeof(double) * d);
+        memcpy(h->prior_x0.slot(slot), state0, sizeof(double) * n_prior * kFrameStride);
+        CK(h, cudaMemcpyAsync(h->prior_S.dslot(slot), h->prior_S.slot(slot), sizeof(double) * d * d, cudaMemcpyHostToDevice, h->stream));
+        CK(h, cudaMemcpyAsync(h->prior_e.dslot(slot), h->prior_e.slot(slot), sizeof(double) * d, cudaMemcpyHostToDevice, h->stream));
+        CK(h, cudaMemcpyAsync(h->prior_x0.dslot(slot), h->prior_x0.slot(slot), sizeof(double) * n_prior * kFrameStride,
+                              cudaMemcpyHostToDevice, h->stream));
+    }
+    s.n_prior = n_prior;
+    h->prior_resident[slot] = n_prior;
+    host_header(h, slot);
+    Packer p;
+    const BwLayout L = layout_of(h, slot);
+    const size_t lay = p.put(&L, 1), sl = p.put(&slot, 1);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    TRY(relayout(h, din, lay, sl, 1, n_prior > 0));
+    CK(h, cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_window_edit *edits) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !edits)) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: bad edit list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = edits[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_edit: bad slot list"));
+    // every edit is applied to a copy of its slot's host mirror; nothing is staged before all of them passed
+    std::vector<BwSlot> next(n);
+    std::vector<BwEdit> recs(n);
+    std::vector<int32_t> rm;
+    std::vector<BwNew> nws;
+    std::vector<BwObs> obs;
+    std::vector<double> xs;
+    int out_ints = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_edit &E = edits[i];
+        BwSlot s = h->bw.slot[E.slot];
+        BwEdit &R = recs[i];
+        R = BwEdit{};
+        R.slot = E.slot; R.N_old = s.N; R.T_old = (int)s.ids.size(); R.frame = -1;
+        if (E.n_new_tracks < 0 || E.n_obs < 0 || E.n_remove < 0 ||
+            (E.n_new_tracks > 0 && (!E.new_frame || !E.new_z || !E.new_inv_depth)) ||
+            (E.n_obs > 0 && (!E.obs_track || !E.obs_frame || !E.obs_z)) || (E.n_remove > 0 && !E.remove))
+            return fail(h, PVIO_B200_EINVAL, "batch_window_edit: null array");
+        if (E.replace_last) {                                         // map->erase_frame(frame_num - 1)
+            if (s.N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: replace_last on an empty window");
+            if (s.N - 1 < s.n_prior) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: the newest frame is covered by the prior");
+            for (uint32_t &m : s.mask) m &= ~(1u << (s.N - 1));
+            s.fixed &= ~(1 << (s.N - 1));
+            --s.N;
+            R.replace_last = 1;
+        }
+        // removals are looked up in the table as it stands before the call (they are applied after the observations,
+        // which they make moot; a track cannot be new and removed in one edit)
+        std::vector<int32_t> removed;
+        R.rm_off = (int)rm.size();
+        for (int k = 0; k < E.n_remove; ++k) {
+            const int r = find_row(s, E.remove[k]);
+            if (r < 0 || s.mask[r] == 0u) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: unknown or dead track removed");
+            s.mask[r] = 0u;
+            rm.push_back(r);
+            removed.push_back(E.remove[k]);
+        }
+        R.n_rm = E.n_remove;
+        std::sort(removed.begin(), removed.end());
+        {   // compaction
+            size_t o = 0;
+            for (size_t r = 0; r < s.ids.size(); ++r)
+                if (s.mask[r]) { s.ids[o] = s.ids[r]; s.mask[o] = s.mask[r]; ++o; }
+            s.ids.resize(o); s.mask.resize(o);
+        }
+        if (E.state) {
+            if (s.N >= h->Ncap) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: window of more than max_frames frames");
+            const bool imu = s.inertial && s.N > 0;
+            if (imu && !E.imu_record) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: an inertial window needs the IMU record to the previous frame");
+            R.frame = s.N; R.has_imu = imu ? 1 : 0; R.x_off = (int)xs.size();
+            xs.insert(xs.end(), E.state, E.state + kFrameStride);
+            if (imu) xs.insert(xs.end(), E.imu_record, E.imu_record + kImuStride);
+            if (E.fixed) s.fixed |= 1 << s.N;
+            ++s.N;
+        }
+        R.new_off = (int)nws.size(); R.n_new = E.n_new_tracks;
+        for (int k = 0; k < E.n_new_tracks; ++k) {
+            const int f = E.new_frame[k];
+            if (f < 0 || f >= s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: track starts outside the window");
+            BwNew t{(int32_t)s.ids.size(), s.next_id, f, 0, E.new_z[2 * k], E.new_z[2 * k + 1], E.new_inv_depth[k]};
+            s.ids.push_back(s.next_id++); s.mask.push_back(1u << f);
+            nws.push_back(t);
+        }
+        R.obs_off = (int)obs.size();
+        for (int k = 0; k < E.n_obs; ++k) {
+            const int32_t id = E.obs_track[k];
+            const int f = E.obs_frame[k];
+            if (f < 0 || f >= s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: observation outside the window");
+            if (std::binary_search(removed.begin(), removed.end(), id)) continue;
+            const int r = find_row(s, id);
+            if (r < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: observation of an unknown or dead track");
+            if (f <= 31 - __builtin_clz(s.mask[r]))
+                return fail(h, PVIO_B200_EINVAL, "batch_window_edit: observations of a track arrive in increasing frame order");
+            s.mask[r] |= 1u << f;
+            obs.push_back(BwObs{r, f, E.obs_z[2 * k], E.obs_z[2 * k + 1]});
+        }
+        R.n_obs = (int)obs.size() - R.obs_off;
+        TRY(check_window(h, s));
+        R.out_off = out_ints;
+        out_ints += 1 + E.n_new_tracks;
+        next[i] = std::move(s);
+    }
+    Packer p;
+    std::vector<BwLayout> lays(n);
+    for (int i = 0; i < n; ++i) lays[i] = BwLayout{slots[i], next[i].N, (int)next[i].ids.size(), next[i].fixed, next[i].n_prior, next[i].inertial};
+    const size_t o_ed = p.put(recs.data(), n), o_lay = p.put(lays.data(), n), o_sl = p.put(slots.data(), n);
+    const size_t o_rm = p.put(rm.data(), rm.size()), o_nw = p.put(nws.data(), nws.size()), o_ob = p.put(obs.data(), obs.size());
+    const size_t o_x = p.put(xs.data(), xs.size());
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, sizeof(int32_t) * out_ints, din, dout));
+    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwEdit *>(din + o_ed),
+        reinterpret_cast<const int32_t *>(din + o_rm), reinterpret_cast<const BwNew *>(din + o_nw),
+        reinterpret_cast<const BwObs *>(din + o_ob), reinterpret_cast<const double *>(din + o_x), reinterpret_cast<int32_t *>(dout));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(relayout(h, din, o_lay, o_sl, n, false));
+    const size_t in = dout - din;
+    CK(h, cudaMemcpyAsync(h->bw.stage.h + in, dout, sizeof(int32_t) * out_ints, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    const int32_t *res = reinterpret_cast<const int32_t *>(h->bw.stage.h + in);
+    for (int i = 0; i < n; ++i) {
+        h->bw.slot[slots[i]] = std::move(next[i]);
+        host_header(h, slots[i]);
+    }
+    for (int i = 0; i < n; ++i) {
+        const int32_t *r = res + recs[i].out_off;
+        if (r[0] != (int32_t)h->bw.slot[slots[i]].ids.size())
+            return fail(h, PVIO_B200_ECUDA, "batch_window_edit: the device track table disagrees with the host's");
+        if (edits[i].new_ids) memcpy(edits[i].new_ids, r + 1, sizeof(int32_t) * edits[i].n_new_tracks);
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_solve(pvio_b200_handle hh, int n, const int32_t *slots, const pvio_b200_options *opt,
+                                 pvio_b200_summary *summaries) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    TRY(check_slots(h, n, slots, "batch_window_solve: bad slot list"));
+    if (n == 0) return 0;
+    // the trust-region chain runs over windows [0, range) and skips the unnamed ones (init_ctrl_kernel marks them
+    // finished before the first body; every kernel of the chain returns for a finished window before it reads anything
+    // else of it); the post-pass and the write-back run over the named list only
+    int range = 0;
+    for (int i = 0; i < n; ++i) {
+        if (h->bw.slot[slots[i]].N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_solve: a window without frames");
+        range = std::max(range, slots[i] + 1);
+    }
+    std::vector<uint8_t> named(range, 0);
+    std::vector<BwLayout> lays(n);
+    for (int i = 0; i < n; ++i) { named[slots[i]] = 1; lays[i] = layout_of(h, slots[i]); }
+    Packer p;
+    const size_t o_nm = p.put(named.data(), range), o_lay = p.put(lays.data(), n), o_sl = p.put(slots, n);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    CK(h, cudaEventRecord(h->ev0, h->stream));
+    TRY(run_named_solve(h, opt, range, din + o_nm));
+    CK(h, cudaEventRecord(h->ev1, h->stream));
+    const bool post = !opt || opt->run_postpass;
+    if (post) TRY(run_postpass_slots(h, n, reinterpret_cast<const int32_t *>(din + o_sl)));
+    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(din + o_lay), post ? 1 : 0);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(h->ctrl.h, h->ctrl.d, sizeof(WinCtrl) * range, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+    for (int i = 0; i < n; ++i) {
+        const WinCtrl &c = h->ctrl.h[slots[i]];
+        if (summaries) {
+            pvio_b200_summary &sm = summaries[i];
+            memset(&sm, 0, sizeof(sm));
+            sm.iterations = c.iteration; sm.accepted_steps = c.accepted; sm.termination = c.termination; sm.usable = c.usable;
+            sm.initial_cost = c.initial_cost; sm.final_cost = c.cost; sm.final_radius = c.radius; sm.final_mu = c.mu;
+            sm.solve_seconds = ms * 1e-3;
+        }
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t *slots, double *S_out, int64_t S_stride,
+                                       double *e_out, int64_t e_stride) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    TRY(check_slots(h, n, slots, "batch_window_drop_victim: bad slot list"));
+    if (n == 0) return 0;
+    std::vector<BwSlot> next(n);
+    for (int i = 0; i < n; ++i) {
+        BwSlot s = h->bw.slot[slots[i]];
+        if (!s.inertial) return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: the window must carry motion states");
+        if (s.N < 2) return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: a window needs at least two frames");
+        const int dk = 15 * (s.N - 1);
+        if (!marg_eig_fits(dk))
+            return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: window too large for the shared-memory eigen-solver (15 (N - 1) <= 165)");
+        if ((S_out && S_stride < (int64_t)dk * dk) || (e_out && e_stride < dk))
+            return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: output stride smaller than a window's prior");
+        size_t o = 0;                                                  // map.cpp:76-88 on the host mirror
+        for (size_t r = 0; r < s.ids.size(); ++r) {
+            const uint32_t m = s.mask[r] >> 1;
+            if (m) { s.ids[o] = s.ids[r]; s.mask[o] = m; ++o; }
+        }
+        s.ids.resize(o); s.mask.resize(o);
+        --s.N; s.fixed >>= 1; s.n_prior = s.N;
+        TRY(check_window(h, s));
+        next[i] = std::move(s);
+    }
+    std::vector<BwLayout> before(n), after(n);
+    for (int i = 0; i < n; ++i) {
+        before[i] = layout_of(h, slots[i]);
+        after[i] = BwLayout{slots[i], next[i].N, (int)next[i].ids.size(), next[i].fixed, next[i].n_prior, next[i].inertial};
+    }
+    Packer p;
+    const size_t o_sl = p.put(slots, n), o_b = p.put(before.data(), n), o_a = p.put(after.data(), n);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    TRY(named_marginalize_impl(h, n, slots, reinterpret_cast<const int32_t *>(din + o_sl)));
+    for (int i = 0; i < n; ++i) {
+        const size_t dk = 15 * (size_t)(h->bw.slot[slots[i]].N - 1);
+        if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.dslot(slots[i]), sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
+        if (e_out) CK(h, cudaMemcpyAsync(e_out + i * e_stride, h->prior_e.dslot(slots[i]), sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
+    }
+    bw_drop_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(din + o_b));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(relayout(h, din, o_a, o_sl, n, true));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        h->bw.slot[slots[i]] = std::move(next[i]);
+        h->prior_resident[slots[i]] = h->bw.slot[slots[i]].n_prior;
+        host_header(h, slots[i]);
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *slots, int32_t *n_frames, double *frames,
+                                    int64_t frames_stride, int32_t *n_tracks, int64_t track_stride, int32_t *track_id,
+                                    double *inv_depth, int32_t *anchor_frame, int32_t *n_observations, uint8_t *valid,
+                                    double *quality) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    TRY(check_slots(h, n, slots, "batch_window_download: bad slot list"));
+    if (n == 0) return 0;
+    std::vector<BwDl> dls(n);
+    int64_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        const BwSlot &s = h->bw.slot[slots[i]];
+        const int T = (int)s.ids.size();
+        if (frames && frames_stride < (int64_t)s.N * kFrameStride) return fail(h, PVIO_B200_EINVAL, "batch_window_download: frames_stride too small");
+        if ((track_id || inv_depth || anchor_frame || n_observations || valid || quality) && track_stride < T)
+            return fail(h, PVIO_B200_EINVAL, "batch_window_download: track_stride smaller than a slot's live tracks");
+        dls[i] = BwDl{slots[i], s.N, T, 0, off};
+        off += ((int64_t)(s.N * kFrameStride + 2 * T) * 8 + (int64_t)T * 13 + 15) & ~(int64_t)15;
+    }
+    Packer p;
+    const size_t o_dl = p.put(dls.data(), n);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, (size_t)off, din, dout));
+    bw_download_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwDl *>(din + o_dl), dout);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    const size_t in = dout - din;
+    CK(h, cudaMemcpyAsync(h->bw.stage.h + in, dout, (size_t)off, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        const int N = dls[i].N, T = dls[i].T;
+        const uint8_t *b = h->bw.stage.h + in + dls[i].off;
+        const double *fo = reinterpret_cast<const double *>(b), *ro = fo + (size_t)N * kFrameStride, *qo = ro + T;
+        const int32_t *io = reinterpret_cast<const int32_t *>(qo + T), *ao = io + T, *no = ao + T;
+        const uint8_t *vo = reinterpret_cast<const uint8_t *>(no + T);
+        const size_t t0 = (size_t)i * track_stride;
+        if (n_frames) n_frames[i] = N;
+        if (n_tracks) n_tracks[i] = T;
+        if (frames) memcpy(frames + (size_t)i * frames_stride, fo, sizeof(double) * N * kFrameStride);
+        if (track_id) memcpy(track_id + t0, io, sizeof(int32_t) * T);
+        if (inv_depth) memcpy(inv_depth + t0, ro, sizeof(double) * T);
+        if (anchor_frame) memcpy(anchor_frame + t0, ao, sizeof(int32_t) * T);
+        if (n_observations) memcpy(n_observations + t0, no, sizeof(int32_t) * T);
+        if (valid) memcpy(valid + t0, vo, T);
+        if (quality) memcpy(quality + t0, qo, sizeof(double) * T);
+    }
+    return 0;
+}
+
+}  // extern "C"

@@ -174,3 +174,176 @@ class ResidentPlayer:
         self.rw.append_frame(self.state16(f_abs), False, self.rec[f_abs - 1])
         self.seconds += time.perf_counter() - t
         self.feed(f_abs, self.run.N - 1)
+
+
+class WindowModel:
+    """Host model of one resident slot, as the map sees it: absolute frames in the window and, per live track, its
+    landmark, window frames (increasing), keypoints and inverse depth.  It applies the same edits and drops as
+    pvio_b200_batch_window_* (erase_frame / put_frame / add_keypoint / prune_tracks / marginalize_frame(0) of
+    map/map.cpp, without the re-anchoring, which needs states), and gives the window a gather would pack."""
+
+    def __init__(self):
+        self.frames, self.tracks, self.next_id = [], {}, 0
+
+    def edit(self, e, f_abs=None):
+        """apply an Edit; f_abs: the absolute id of its new frame.  Returns the new track ids."""
+        if e.replace_last:                                   # map->erase_frame(frame_num - 1)
+            last = len(self.frames) - 1
+            self.frames.pop()
+            for i in list(self.tracks):
+                t = self.tracks[i]
+                if t['frames'][-1] == last:
+                    t['frames'].pop(); t['zs'].pop()
+                if not t['frames']:
+                    del self.tracks[i]
+        if e.state is not None:
+            self.frames.append(f_abs)
+        ids = []
+        for (f, z, rho), l in zip(e.new, getattr(e, 'landmarks', [None] * len(e.new))):
+            self.tracks[self.next_id] = dict(l=l, frames=[f], zs=[np.asarray(z, dtype=float)], rho=rho)
+            ids.append(self.next_id)
+            self.next_id += 1
+        for i, f, z in e.obs:
+            if i in self.tracks:
+                self.tracks[i]['frames'].append(f); self.tracks[i]['zs'].append(np.asarray(z, dtype=float))
+        for i in e.remove:
+            del self.tracks[i]
+        return ids
+
+    def drop(self):
+        """marginalize_frame(0): the victim's keypoints leave their tracks, indices shift"""
+        self.frames.pop(0)
+        for i in list(self.tracks):
+            t = self.tracks[i]
+            if t['frames'][0] == 0:
+                t['frames'].pop(0); t['zs'].pop(0)
+            if not t['frames']:
+                del self.tracks[i]
+                continue
+            t['frames'] = [f - 1 for f in t['frames']]
+
+    def view(self):
+        """landmark -> (anchor, z_ref, obs frames, obs keypoints) of the tracks with >= 2 observations, in id order"""
+        out = {}
+        for i in sorted(self.tracks):
+            t = self.tracks[i]
+            if len(t['frames']) >= 2:
+                out[t['l']] = (t['frames'][0], t['zs'][0], list(t['frames'][1:]), [z for z in t['zs'][1:]])
+        return out
+
+
+class ModelWindows:
+    """The host models of several slots behind the interface of pvio_b200.batch_window.BatchWindows (edits, drops, the
+    live ids of a download): a BatchPlayer runs on it without a device."""
+
+    def __init__(self):
+        self.m = {}
+
+    def reset(self, slot, win):
+        self.m[slot] = WindowModel()
+
+    def set_prior(self, slot, S, e, x0):
+        pass
+
+    def edit(self, edits):
+        return [np.array(self.m[e.slot].edit(e, getattr(e, 'f_abs', None)), dtype=np.int32) for e in edits]
+
+    def drop_victim(self, slots, want=False):
+        for s in slots:
+            self.m[s].drop()
+
+    def download(self, slots, track_stride):
+        return [dict(ids=np.array(sorted(self.m[s].tracks), dtype=np.int32)) for s in slots]
+
+
+class BatchPlayer:
+    """Feeds several runs into RESIDENT batched slots (pvio_b200.batch_window.BatchWindows): run j lives in slot
+    slots[j].  Per keyframe of a slot: solve, drop the victim, then the next camera frame arrives first as a non-keyframe
+    (a perturbed state with the frame's observations) that the real keyframe replaces (replace_last), as PVIO's tracker
+    erases a non-keyframe newest frame (sliding_window_tracker.cpp:115-121).  The host model keeps, per slot, the live
+    track of each landmark (`ids`) and the window's first absolute frame (`k`)."""
+
+    def __init__(self, ba, runs, slots=None, bw=None):
+        """ba: the handle's BundleAdjustor; bw (instead of ba): any object with BatchWindows' interface (ModelWindows).
+        `model` (a ModelWindows) follows every edit and drop: the window a gather of the map would pack."""
+        from pvio_b200 import _lib
+        from pvio_b200.batch_window import BatchWindows, Edit
+        self.Edit = Edit
+        self.runs, self.bw = runs, (BatchWindows(ba) if bw is None else bw)
+        self.model = bw if isinstance(bw, ModelWindows) else ModelWindows()
+        self.slots = list(range(len(runs))) if slots is None else list(slots)
+        self.ids = [dict() for _ in runs]                  # landmark -> live track id
+        self.k = [0] * len(runs)
+        self.rec = [_lib.PackedArgs(r.w, r.guess).keep["imu"].reshape(-1, 288) for r in runs]
+        for j, r in enumerate(runs):
+            self.bw.reset(self.slots[j], r.w)
+            if self.model is not self.bw:
+                self.model.reset(self.slots[j], r.w)
+        for f in range(max(r.N for r in runs)):
+            js = [j for j, r in enumerate(runs) if f < r.N]
+            self._apply([self.frame_edit(j, f, f) for j in js], js)
+        for j, r in enumerate(runs):
+            w0, _, _ = Chain(r).window(0)                   # first window: the 1e15 gauge prior
+            x0 = np.concatenate([w0.prior_q0, w0.prior_p0, w0.prior_v0, w0.prior_bg0, w0.prior_ba0], axis=1)
+            self.bw.set_prior(self.slots[j], w0.prior_S, w0.prior_e, x0)
+
+    def state16(self, j, f):
+        g = self.runs[j].guess
+        return np.concatenate([g.q[f], g.p[f], g.v[f], g.bg[f], g.ba[f]])
+
+    def frame_edit(self, j, f_abs, f_win, replace_last=False, state=None):
+        """the edit that appends absolute frame f_abs at window index f_win, with its observations and new tracks"""
+        r = self.runs[j]
+        e = self.Edit(self.slots[j], replace_last).frame(self.state16(j, f_abs) if state is None else state, False,
+                                                         self.rec[j][f_abs - 1] if f_abs > 0 and f_win > 0 else None)
+        e.landmarks, e.f_abs = [], f_abs
+        for l, (fr, zs) in enumerate(r.tracks):
+            if f_abs in fr:
+                z = zs[fr.index(f_abs)]
+                if l in self.ids[j]:
+                    e.obs.append((self.ids[j][l], f_win, z))
+                else:
+                    e.new.append((f_win, z, r.guess.rho[l]))
+                    e.landmarks.append(l)
+        return e
+
+    def _apply(self, edits, js):
+        got = self.bw.edit(edits)
+        if self.model is not self.bw:
+            self.model.edit(edits)
+        for e, j, ids in zip(edits, js, got):
+            for l, i in zip(e.landmarks, ids):
+                self.ids[j][l] = int(i)
+
+    def refresh(self, js, track_stride):
+        """download the slots of runs js; forget the landmarks whose tracks died"""
+        out = self.bw.download([self.slots[j] for j in js], track_stride)
+        for j, d in zip(js, out):
+            live = set(int(i) for i in d["ids"])
+            self.ids[j] = {l: i for l, i in self.ids[j].items() if i in live}
+        return out
+
+    def advance(self, js, perturb=1e-3, nonkey=True):
+        """drop the victim of the runs js, then their next frame -- first as a non-keyframe that the keyframe replaces
+        (nonkey), or directly"""
+        self.bw.drop_victim([self.slots[j] for j in js])
+        if self.model is not self.bw:
+            self.model.drop_victim([self.slots[j] for j in js])
+        self.refresh(js, max(len(r.tracks) for r in self.runs))
+        for j in js:
+            self.k[j] += 1
+        if not nonkey:
+            self._apply([self.frame_edit(j, self.k[j] + self.runs[j].N - 1, self.runs[j].N - 1) for j in js], js)
+            return
+        fake = []
+        for j in js:
+            f_abs, N = self.k[j] + self.runs[j].N - 1, self.runs[j].N
+            s = self.state16(j, f_abs).copy()
+            s[4:7] += perturb
+            fake.append(self.frame_edit(j, f_abs, N - 1, state=s))
+        self._apply(fake, js)
+        for e, j in zip(fake, js):                          # the non-keyframe's new tracks die with it
+            for l in e.landmarks:
+                del self.ids[j][l]
+        real = [self.frame_edit(j, self.k[j] + self.runs[j].N - 1, self.runs[j].N - 1, replace_last=True) for j in js]
+        self._apply(real, js)
