@@ -167,11 +167,22 @@ int pvio_b200_ba_marginalize(pvio_b200_handle h, const pvio_b200_window *w, cons
 
 /* ---- resident sliding window (SURVEY 8(f) rank 1) ----------------------------------- */
 /* The window persists in the handle between keyframes instead of being rebuilt from Map / Frame / Track at every
- * solve (bundle_adjustor.cpp:75-242): the shim reports what CHANGED.  The marginalisation prior stays ON THE DEVICE:
- * pvio_b200_window_drop_victim leaves S, e and the linearisation point where the solve kernels read them.
- * One resident window per handle.  Frame arguments are window indices (0 = oldest). */
+ * solve (bundle_adjustor.cpp:75-242): the shim reports what CHANGED.  The whole window stays ON THE DEVICE, the
+ * marginalisation prior included: pvio_b200_window_drop_victim leaves S, e and the linearisation point where the solve
+ * kernels read them.  One resident window per handle.  Frame arguments are window indices (0 = oldest).
+ * These calls are the resident batched windows below, on slot 0 (each edit call is one pvio_b200_batch_window_edit),
+ * so their rules apply:
+ *  - pvio_b200_window_* and pvio_b200_batch_window_* on slot 0 are the same window.  A call that packs slot 0 ends it
+ *    (ba_solve, ba_gn_step, ba_marginalize, reprojection_error, batch_set_window(0)); then these calls return
+ *    PVIO_B200_EINVAL until pvio_b200_window_reset.
+ *  - The slot limits apply: live one-observation tracks count toward max_landmarks, a landmark has fewer than 16
+ *    observations, a window at most 96 landmark chunks.
+ *  - A rejected call changes nothing.
+ *  - A prior on a window without motion states (use_inertial == 0) is rejected.
+ * Every other call before pvio_b200_window_reset returns PVIO_B200_EINVAL.  Track ids count from 0 per reset and are never
+ * reused. */
 /* Start an empty window.  Of `constants` the scalar members are kept (extrinsics, sqrt_inv_cov, fx, fy, cauchy_a,
- * use_inertial); its arrays are ignored. */
+ * use_inertial); its arrays and plane counts are ignored. */
 int pvio_b200_window_reset(pvio_b200_handle h, const pvio_b200_window *constants);
 /* sliding_window_tracker.cpp:113-118.  state [PVIO_B200_FRAME_STRIDE]; imu_record [PVIO_B200_IMU_STRIDE]: the
  * pre-integration factor (previous frame, this frame), NULL for the first frame / a visual-only window. */
@@ -182,18 +193,21 @@ int pvio_b200_window_add_tracks(pvio_b200_handle h, int n, const int32_t *frame,
                                 const double *inv_depth, int32_t *ids_out);
 /* Track::add_keypoint (track.cpp:32-37): observations arrive in increasing frame order per track. */
 int pvio_b200_window_add_observations(pvio_b200_handle h, int n, const int32_t *track, const int32_t *frame, const double *z);
+/* Map::prune_tracks.  Removing a track that is already gone returns 0; an id never handed out, PVIO_B200_EINVAL. */
 int pvio_b200_window_remove_track(pvio_b200_handle h, int32_t track);
 /* A prior given by the caller over frames 0 .. n_prior-1 (the 1e15 gauge prior of the first window,
  * sliding_window_tracker.cpp:100-112); later priors come from pvio_b200_window_drop_victim. */
 int pvio_b200_window_set_prior(pvio_b200_handle h, int n_prior, const double *S, const double *e, const double *state0);
 /* BundleAdjustor::solve on the resident window (tracks with >= 2 observations take part); states and inverse
- * depths are updated in the handle. */
+ * depths are updated in the handle.  No landmark post-pass runs. */
 int pvio_b200_window_solve(pvio_b200_handle h, const pvio_b200_options *opt, pvio_b200_summary *summary);
 /* Map::marginalize_frame(0) (map.cpp:76-88): marginaliser -> new prior (device resident), the victim's observations
  * leave their tracks, tracks anchored in it are re-anchored from the current estimate (track.cpp:42-49). */
 int pvio_b200_window_drop_victim(pvio_b200_handle h);
-/* Read back: frames [n_frames][PVIO_B200_FRAME_STRIDE]; per queried track its inverse depth, anchor frame (-1: gone)
- * and observation count.  Any output pointer may be NULL. */
+/* Read back: frames [n_frames][PVIO_B200_FRAME_STRIDE]; per queried track its inverse depth, anchor frame and
+ * observation count.  A gone track reports anchor -1 and 0 observations, and its inverse depth is not written; an id
+ * never handed out is PVIO_B200_EINVAL.  Any output pointer may be NULL.  With frames == NULL and n_tracks == 0 the
+ * call answers n_frames without touching the device. */
 int pvio_b200_window_get(pvio_b200_handle h, int32_t *n_frames, double *frames, int n_tracks, const int32_t *tracks,
                          double *inv_depth, int32_t *anchor_frame, int32_t *n_observations);
 
@@ -246,8 +260,8 @@ int pvio_b200_batch_marginalize(pvio_b200_handle h, int n, double *S_out, int64_
 /* A slot made resident by pvio_b200_batch_window_reset holds its sequence's whole window on the device between camera
  * frames: frame states, IMU records, the prior and every live track (frame mask, fp64 keypoint per frame, inverse depth).
  * The caller sends only what changed; the packed tables the solve kernels read are rebuilt on the device exactly as
- * pvio_b200_batch_set_window would pack the window pvio_b200_window_* keeps (tracks with >= 2 observations, in id order,
- * stably sorted by anchor).  Frame arguments are window indices (0 = oldest).
+ * pvio_b200_batch_set_window would pack the window of the tracks with >= 2 observations, in id order, stably sorted by
+ * anchor.  Frame arguments are window indices (0 = oldest).  Slot 0 is also the window of pvio_b200_window_*.
  * Rules:
  *  - Every call checks all its inputs before it stages or launches anything: on PVIO_B200_EINVAL no slot has changed.
  *    Rejected: a slot out of range or not resident, a slot named twice, an unknown or dead track, observations out of
@@ -256,9 +270,10 @@ int pvio_b200_batch_marginalize(pvio_b200_handle h, int n, double *S_out, int64_
  *    landmark chunks, a drop on a window without motion states or with 15 (N - 1) > 165.
  *  - Track ids are per slot, increasing, never reused until the slot is reset; the storage of dead tracks is reused, so a
  *    sequence is limited by its live tracks only.
- *  - A resident slot changes through these calls only.  pvio_b200_batch_set_window on it, and any single-window call
- *    that packs into slot 0 (ba_solve, ba_gn_step, ba_marginalize, reprojection_error, window_*), end its residency;
- *    then these calls return PVIO_B200_EINVAL for it until it is reset.  batch_upload, batch_replicate, batch_gn_step,
+ *  - A resident slot changes through these calls (and, for slot 0, pvio_b200_window_*) only.
+ *    pvio_b200_batch_set_window on it, and any single-window call that packs into slot 0 (ba_solve, ba_gn_step,
+ *    ba_marginalize, reprojection_error), end its residency; then these calls return PVIO_B200_EINVAL for it until it
+ *    is reset.  batch_upload, batch_replicate, batch_gn_step,
  *    batch_solve, batch_marginalize and the *_host calls over a range holding a resident slot return PVIO_B200_EINVAL.
  *  - The kernel-launch count of a call does not depend on n.  An edit call makes one host -> device and one
  *    device -> host copy. */

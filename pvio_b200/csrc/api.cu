@@ -1293,7 +1293,7 @@ int pvio_b200_ba_marginalize(pvio_b200_handle hh, const pvio_b200_window *w, con
                              double *S_out, double *e_out, double *H_out, double *b_out) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h || !w || !s) return PVIO_B200_EINVAL;
-    return marginalize_impl(h, w, s, index, false, S_out, e_out, H_out, b_out);
+    return marginalize_impl(h, w, s, index, S_out, e_out, H_out, b_out);
 }
 
 int pvio_b200_batch_marginalize(pvio_b200_handle hh, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride) {

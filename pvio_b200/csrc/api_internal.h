@@ -3,10 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <algorithm>
-#include <array>
 #include <cstring>
 #include <map>
-#include <memory>
 #include <string>
 #include <tuple>
 #include <utility>
@@ -123,34 +121,12 @@ struct FmState {
     DevBuf<unsigned> h_mask;                  // pinned: its inlier mask
 };
 
-// resident.cu: the sliding window kept between keyframes
-struct ResTrack {
-    std::vector<int32_t> frames;      // window indices, increasing
-    std::vector<double> z;            // [2] per observation
-    double rho = 1.0;
-    bool alive = true;
-};
-
-struct ResidentWindow {
-    pvio_b200_window cst;             // constants (extrinsics, noise model, flags); the array members are rebuilt per call
-    std::vector<std::array<double, kFrameStride>> frames;
-    std::vector<uint8_t> fixed;
-    std::vector<std::array<double, kImuStride>> imu;      // factor k couples frames (k, k + 1)
-    std::vector<ResTrack> tracks;
-    int n_prior = 0;                  // the prior covers frames 0 .. n_prior - 1
-    bool prior_on_device = false;
-    std::vector<double> host_S, host_e, host_x0;          // a prior given by the caller (first window: the gauge prior)
-    // the view handed to pack_window
-    std::vector<int32_t> lm_anchor, lm_obs_begin, obs_frame, imu_i, imu_j, prior_frames, lm_track;
-    std::vector<double> lm_z_ref, obs_z, imu_data, st_frames, st_rho;
-    std::vector<uint8_t> lm_in_victim;
-};
-
-// batch_window.cu: the resident windows of the batched slots.  Per slot the host keeps integers only: the frame count,
-// the prior's frame count, the fixed mask, and for every live track (rows in id order) its id and frame mask; the device
-// keeps the track table (frame mask, inverse depth, fp64 keypoint per window frame, post-pass flags) and the packed window.
+// batch_window.cu: the resident windows of the batched slots; slot 0 is also the window of pvio_b200_window_*.  Per slot
+// the host keeps integers only: the frame count, the prior's frame count, the fixed mask, and for every live track (rows
+// in id order) its id and frame mask; the device keeps the track table (frame mask, inverse depth, fp64 keypoint per
+// window frame, post-pass flags) and the packed window.
 struct BwSlot {
-    bool on = false;                  // resident: the slot changes through pvio_b200_batch_window_* only
+    bool on = false;                  // resident: the slot changes through pvio_b200_batch_window_* (and window_*) only
     int N = 0, n_prior = 0, fixed = 0, inertial = 0;
     int32_t next_id = 0;
     std::vector<int32_t> ids;         // live tracks, increasing: row r of the device table holds track ids[r]
@@ -185,7 +161,6 @@ struct Handle {
     int64_t launches = 0;
     std::vector<int> prior_resident;              // per slot: frame count of the prior (S, e, x0) the marginaliser wrote on the
                                                   // device (0: none); a pack naming it with prior_S == NULL keeps it, a host prior clears it
-    std::unique_ptr<ResidentWindow> resident;     // resident.cu (null until pvio_b200_window_reset)
     DetectState detect;                           // detect.cu
     DetectBatchState detectb;                     // detect.cu: the batched detector, independent of detect
     size_t sys_set = 0;                           // elements between the two buffer sets of the reduced-system arrays (LinBufs)
@@ -339,9 +314,10 @@ int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_
 int run_postpass_slots(Handle *h, int n, const int32_t *slots);   // post-pass of the n windows of a device list
 // the frame-major table of the n windows slots[0 .. n) (device list), and Lambda = S^T S of their priors when prior
 int launch_layout_tail(Handle *h, const int32_t *slots, int n, bool prior);
-// ba_marg.cu: the marginaliser (index 0, new prior into the slots) of the n windows h_slots / d_slots (host / device
-// copies of one list)
-int named_marginalize_impl(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots);
+// ba_marg.cu: the marginaliser of windows [0, n) or of the list h_slots / d_slots (host / device copies of one list);
+// to_slots: each new prior into its window's prior arrays
+int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, const int32_t *h_slots = nullptr,
+             const int32_t *d_slots = nullptr);
 bool marg_eig_fits(int dk);
 // klt.cu
 int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int width, int height, int stride,
@@ -364,7 +340,7 @@ void klt_batch_clahe(Handle *h, const KltBatchFrame *frames, int n_frames, int t
 // detect.cu: pvio_b200_batch_detect_keypoints
 int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, double clahe_clip, int tiles_x, int tiles_y);
 // ba_marg.cu
-int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
+int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index,
                      double *S_out, double *e_out, double *H_out, double *b_out);
 int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride);
 int selftest_eig_impl(Handle *h, int n, const int32_t *dk, const double *A, const double *b, double *S_out, double *e_out);

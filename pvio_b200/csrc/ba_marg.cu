@@ -475,99 +475,71 @@ int marg_opt_in(Handle *h) {
     return 0;
 }
 
-// The marginaliser of the uploaded windows [0, n) at their device states: the vision part of all n windows, then the dense
-// tail chunk by chunk (assemble -> frame Schur complement -> eigen-solver; a window's three kernels stay in one chunk, so
-// its old prior is consumed before its new one overwrites it).  eig = false stops after the Schur complement.
+// The marginaliser of n uploaded windows at their device states: the vision part of all n windows, then the dense tail
+// chunk by chunk (assemble -> frame Schur complement -> eigen-solver; a window's three kernels stay in one chunk, so its
+// old prior is consumed before its new one overwrites it).  eig = false stops after the Schur complement.
+// The windows are [0, n), or the list h_slots / d_slots (host / device copies of one list; every kernel, the vision
+// sweeps included, then works on the listed windows only).
 // to_slots: S, e and the linearisation point (the CURRENT states of frames 1 .. N - 1) go straight into each window's own
-// prior arrays, where a later pack of the shifted window names them with prior_S == NULL; otherwise (n == 1) into the
-// scratch block of window 0.
-static int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, MargLayout &L) {
+// prior arrays, where a later pack of the shifted window names them with prior_S == NULL or a resident slot's next solve
+// reads them; otherwise (n == 1, no list) into the scratch block of window 0.
+int run_marg(Handle *h, int n, int index, bool eig, bool to_slots, const int32_t *h_slots, const int32_t *d_slots) {
     const int chunk = std::min(n, kMargChunkPerSm * h->sm_count);
-    L = marg_layout(h);
+    const MargLayout L = marg_layout(h);
     TRY(reserve(h, h->marg, L.stride * chunk, kDevice));
     // vision part: no loss, victim-seen landmarks only, mu = 0, fp64 (lin_obs_kernel<false, double> + schur_kernel<double>)
-    TRY(run_marg_vision(h, n));
+    TRY(run_marg_vision(h, n, h_slots, d_slots));
     double *buf = h->marg.d;
     MargArgs m = launch_args<MargArgs>(h);
-    m.index = index; m.buf = buf; m.L = L;
+    m.index = index; m.buf = buf; m.L = L; m.slots = d_slots;
     for (int w0 = 0; w0 < n; w0 += chunk) {
         const int cn = std::min(chunk, n - w0);
         m.w0 = w0;
         marg_assemble_kernel<<<cn, 256, 0, h->stream>>>(m);
-        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, buf, L, nullptr);
+        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, index, buf, L, d_slots);
         h->launches += 2;
         if (!eig) continue;
         int dk = 0;
-        for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[i].N - 1));
+        for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[h_slots ? h_slots[i] : i].N - 1));
         const EigLaunch el = eig_launch(dk);
-        if (to_slots)
+        if (to_slots) {        // with a list the kernel offsets each output by its slot, without one CTA c writes w0 + c
+            const int o = d_slots ? 0 : w0;
             marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring,
-                h->prior_S.dslot(w0), h->prior_S.per, h->prior_e.dslot(w0), h->prior_e.per, h->frames.dslot(w0),
-                h->prior_x0.dslot(w0), h->prior_x0.per, nullptr);
-        else
+                h->prior_S.dslot(o), h->prior_S.per, h->prior_e.dslot(o), h->prior_e.per, h->frames.dslot(o),
+                h->prior_x0.dslot(o), h->prior_x0.per, d_slots);
+        } else {
             marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring,
                 buf + L.S, L.stride, buf + L.e, L.stride, nullptr, nullptr, 0, nullptr);
+        }
         ++h->launches;
     }
     CK(h, cudaGetLastError());
     return 0;
 }
 
-// keep_on_device (index 0 only): the new prior is written straight into slot 0's prior arrays on the device (run_marg's
-// to_slots); the next solve of the shifted window names it with prior_S == NULL (pack_window) and nothing of it crosses PCIe.
-int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index, bool keep_on_device,
+int marginalize_impl(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s, int index,
                      double *S_out, double *e_out, double *H_out, double *b_out) {
     const int N = w->n_frames;
     if (index < 0 || index >= N || N < 2) return fail(h, PVIO_B200_EINVAL, "marginalize: bad frame index");
     if (!w->use_inertial) return fail(h, PVIO_B200_EINVAL, "marginalize: the window must carry motion states");
     const int dk = 15 * (N - 1);
-    if (keep_on_device && index != 0) return fail(h, PVIO_B200_EINVAL, "marginalize: the resident prior is defined for index 0");
-    const bool eig = S_out || e_out || keep_on_device;
+    const bool eig = S_out || e_out;
     if (eig && !eig_fits(dk))
         return fail(h, PVIO_B200_EINVAL, "marginalize: window too large for the shared-memory eigen-solver (15 (N - 1) <= 165)");
     TRY(pack_and_upload(h, w, s));
-    MargLayout L;
-    TRY(run_marg(h, 1, index, eig, keep_on_device, L));
+    TRY(run_marg(h, 1, index, eig, false));
+    const MargLayout L = marg_layout(h);
     const double *blk = h->marg.d;
     if (H_out) CK(h, cudaMemcpyAsync(H_out, blk + L.Hk, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
     if (b_out) CK(h, cudaMemcpyAsync(b_out, blk + L.bk, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
-    const double *dS = keep_on_device ? h->prior_S.d : blk + L.S, *de = keep_on_device ? h->prior_e.d : blk + L.e;
-    if (S_out) CK(h, cudaMemcpyAsync(S_out, dS, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
-    if (e_out) CK(h, cudaMemcpyAsync(e_out, de, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
+    if (S_out) CK(h, cudaMemcpyAsync(S_out, blk + L.S, sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
+    if (e_out) CK(h, cudaMemcpyAsync(e_out, blk + L.e, sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    if (keep_on_device) h->prior_resident[0] = N - 1;
     return 0;
 }
 
 bool marg_eig_fits(int dk) { return eig_fits(dk); }
-
-// The marginaliser of frame 0 for the n resident windows of a list (batch_window.cu: pvio_b200_batch_window_drop_victim),
-// checked by the caller: every kernel, the vision sweeps included, works on the listed windows only, each new prior into
-// its own slot.
-int named_marginalize_impl(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots) {
-    const int chunk = std::min(n, kMargChunkPerSm * h->sm_count);
-    const MargLayout L = marg_layout(h);
-    TRY(reserve(h, h->marg, L.stride * chunk, kDevice));
-    TRY(run_marg_vision(h, n, h_slots, d_slots));
-    double *buf = h->marg.d;
-    MargArgs m = launch_args<MargArgs>(h);
-    m.index = 0; m.buf = buf; m.L = L; m.slots = d_slots;
-    for (int w0 = 0; w0 < n; w0 += chunk) {
-        const int cn = std::min(chunk, n - w0);
-        m.w0 = w0;
-        marg_assemble_kernel<<<cn, 256, 0, h->stream>>>(m);
-        marg_reduce_kernel<<<cn, 256, 0, h->stream>>>(h->hdr.d, w0, 0, buf, L, d_slots);
-        int dk = 0;
-        for (int i = w0; i < w0 + cn; ++i) dk = std::max(dk, 15 * (h->hdr.h[h_slots[i]].N - 1));
-        const EigLaunch el = eig_launch(dk);
-        marg_eig_kernel<<<cn, 256, el.smem, h->stream>>>(h->hdr.d, w0, buf, L, el.ring, h->prior_S.d, h->prior_S.per,
-            h->prior_e.d, h->prior_e.per, h->frames.d, h->prior_x0.d, h->prior_x0.per, d_slots);
-        h->launches += 3;
-    }
-    CK(h, cudaGetLastError());
-    return 0;
-}
 
 // pvio_b200_batch_marginalize: every window is checked before anything is launched, so a rejected call changes nothing.
 int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride) {
@@ -582,8 +554,7 @@ int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, do
         if ((S_out && S_stride < (int64_t)dk * dk) || (e_out && e_stride < dk))
             return fail(h, PVIO_B200_EINVAL, "batch_marginalize: output stride smaller than a window's prior");
     }
-    MargLayout L;
-    TRY(run_marg(h, n, 0, true, true, L));
+    TRY(run_marg(h, n, 0, true, true));
     for (int i = 0; i < n; ++i) {          // slot i's prior arrays hold the dense dk x dk S and e at their start
         const size_t dk = 15 * (size_t)(h->hdr.h[i].N - 1);
         if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.dslot(i), sizeof(double) * dk * dk,

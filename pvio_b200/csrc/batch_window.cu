@@ -1,9 +1,12 @@
-// Resident sliding windows of the batched slots (pvio_b200_batch_window_*): the many-sequence counterpart of resident.cu.
+// Resident sliding windows of the batched slots (pvio_b200_batch_window_*), and the single resident window
+// (pvio_b200_window_*), which is slot 0 of them.  The window persists between keyframes instead of being rebuilt from
+// Map / Frame / Track at every BundleAdjustor::solve (bundle_adjustor.cpp:75-242); its bookkeeping follows map.cpp:76-88
+// and track.cpp:32-49.
 // A resident slot keeps its whole window on the device -- frame states, IMU records, the prior, and a TRACK TABLE with
 // every live track's frame mask, inverse depth and fp64 keypoint per window frame.  Per camera frame the host sends only
 // what changed (edit records); the packed tables the solve kernels read (LmRec, ObsRec, rho, WinHdr, the frame-major
-// table) are rebuilt from the track table on the device, exactly as pack_window builds them from resident.cu's
-// build_view: tracks with >= 2 observations in id order, stably sorted by anchor (their lowest frame).
+// table) are rebuilt from the track table on the device, exactly as pack_window packs the window of the tracks with
+// >= 2 observations in id order: stably sorted by anchor (their lowest frame).
 //
 // The host keeps integers only (frame count, prior size, fixed mask, the id and frame mask of every live row), enough to
 // check every call completely before anything is staged, and to know the launch shapes.  The rows of a slot's table are
@@ -255,7 +258,7 @@ __global__ void __launch_bounds__(kBwThreads) bw_writeback_kernel(BwArgs a, cons
     }
 }
 
-// quaternions (x, y, z, w), Hamilton product, q * v = rotate (resident.cu)
+// quaternions (x, y, z, w), Hamilton product, q * v = rotate: the reference's Eigen conventions (estimation/state.h)
 __device__ void bw_qmul(const double *a, const double *b, double *o) {
     o[0] = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1];
     o[1] = a[3] * b[1] - a[0] * b[2] + a[1] * b[3] + a[2] * b[0];
@@ -464,6 +467,59 @@ static int find_row(const BwSlot &s, int32_t id) {
     return (it == s.ids.end() || *it != id) ? -1 : (int)(it - s.ids.begin());
 }
 
+// BundleAdjustor::solve on the n slots of a list; post: then the landmark post-pass
+static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_options *opt, bool post,
+                       pvio_b200_summary *summaries) {
+    TRY(check_slots(h, n, slots, "batch_window_solve: bad slot list"));
+    if (n == 0) return 0;
+    // the trust-region chain runs over windows [0, range) and skips the unnamed ones (init_ctrl_kernel marks them
+    // finished before the first body; every kernel of the chain returns for a finished window before it reads anything
+    // else of it); the post-pass and the write-back run over the named list only
+    int range = 0;
+    for (int i = 0; i < n; ++i) {
+        if (h->bw.slot[slots[i]].N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_solve: a window without frames");
+        range = std::max(range, slots[i] + 1);
+    }
+    std::vector<uint8_t> named(range, 0);
+    std::vector<BwLayout> lays(n);
+    for (int i = 0; i < n; ++i) { named[slots[i]] = 1; lays[i] = layout_of(h, slots[i]); }
+    Packer p;
+    const size_t o_nm = p.put(named.data(), range), o_lay = p.put(lays.data(), n), o_sl = p.put(slots, n);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    CK(h, cudaEventRecord(h->ev0, h->stream));
+    TRY(run_named_solve(h, opt, range, din + o_nm));
+    CK(h, cudaEventRecord(h->ev1, h->stream));
+    if (post) TRY(run_postpass_slots(h, n, reinterpret_cast<const int32_t *>(din + o_sl)));
+    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(din + o_lay), post ? 1 : 0);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(h->ctrl.h, h->ctrl.d, sizeof(WinCtrl) * range, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+    for (int i = 0; i < n; ++i) {
+        const WinCtrl &c = h->ctrl.h[slots[i]];
+        if (summaries) {
+            pvio_b200_summary &sm = summaries[i];
+            memset(&sm, 0, sizeof(sm));
+            sm.iterations = c.iteration; sm.accepted_steps = c.accepted; sm.termination = c.termination; sm.usable = c.usable;
+            sm.initial_cost = c.initial_cost; sm.final_cost = c.cost; sm.final_radius = c.radius; sm.final_mu = c.mu;
+            sm.solve_seconds = ms * 1e-3;
+        }
+    }
+    return 0;
+}
+
+// slot 0 as the single resident window (pvio_b200_window_*); null, with the error set, before pvio_b200_window_reset
+static const BwSlot *window0(Handle *h) {
+    if (h->bw.slot.empty() || !h->bw.slot[0].on) {
+        fail(h, PVIO_B200_EINVAL, "window: no resident window: call pvio_b200_window_reset first");
+        return nullptr;
+    }
+    return &h->bw.slot[0];
+}
+
 }  // namespace pvio
 
 using namespace pvio;
@@ -656,46 +712,7 @@ int pvio_b200_batch_window_solve(pvio_b200_handle hh, int n, const int32_t *slot
                                  pvio_b200_summary *summaries) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    TRY(check_slots(h, n, slots, "batch_window_solve: bad slot list"));
-    if (n == 0) return 0;
-    // the trust-region chain runs over windows [0, range) and skips the unnamed ones (init_ctrl_kernel marks them
-    // finished before the first body; every kernel of the chain returns for a finished window before it reads anything
-    // else of it); the post-pass and the write-back run over the named list only
-    int range = 0;
-    for (int i = 0; i < n; ++i) {
-        if (h->bw.slot[slots[i]].N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_solve: a window without frames");
-        range = std::max(range, slots[i] + 1);
-    }
-    std::vector<uint8_t> named(range, 0);
-    std::vector<BwLayout> lays(n);
-    for (int i = 0; i < n; ++i) { named[slots[i]] = 1; lays[i] = layout_of(h, slots[i]); }
-    Packer p;
-    const size_t o_nm = p.put(named.data(), range), o_lay = p.put(lays.data(), n), o_sl = p.put(slots, n);
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
-    CK(h, cudaEventRecord(h->ev0, h->stream));
-    TRY(run_named_solve(h, opt, range, din + o_nm));
-    CK(h, cudaEventRecord(h->ev1, h->stream));
-    const bool post = !opt || opt->run_postpass;
-    if (post) TRY(run_postpass_slots(h, n, reinterpret_cast<const int32_t *>(din + o_sl)));
-    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(din + o_lay), post ? 1 : 0);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(h->ctrl.h, h->ctrl.d, sizeof(WinCtrl) * range, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaStreamSynchronize(h->stream));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-    for (int i = 0; i < n; ++i) {
-        const WinCtrl &c = h->ctrl.h[slots[i]];
-        if (summaries) {
-            pvio_b200_summary &sm = summaries[i];
-            memset(&sm, 0, sizeof(sm));
-            sm.iterations = c.iteration; sm.accepted_steps = c.accepted; sm.termination = c.termination; sm.usable = c.usable;
-            sm.initial_cost = c.initial_cost; sm.final_cost = c.cost; sm.final_radius = c.radius; sm.final_mu = c.mu;
-            sm.solve_seconds = ms * 1e-3;
-        }
-    }
-    return 0;
+    return solve_slots(h, n, slots, opt, !opt || opt->run_postpass, summaries);
 }
 
 int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t *slots, double *S_out, int64_t S_stride,
@@ -733,7 +750,7 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
     const size_t o_sl = p.put(slots, n), o_b = p.put(before.data(), n), o_a = p.put(after.data(), n);
     uint8_t *din, *dout;
     TRY(upload_stage(h, p, 0, din, dout));
-    TRY(named_marginalize_impl(h, n, slots, reinterpret_cast<const int32_t *>(din + o_sl)));
+    TRY(run_marg(h, n, 0, true, true, slots, reinterpret_cast<const int32_t *>(din + o_sl)));
     for (int i = 0; i < n; ++i) {
         const size_t dk = 15 * (size_t)(h->bw.slot[slots[i]].N - 1);
         if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.dslot(slots[i]), sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
@@ -797,6 +814,87 @@ int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *s
         if (n_observations) memcpy(n_observations + t0, no, sizeof(int32_t) * T);
         if (valid) memcpy(valid + t0, vo, T);
         if (quality) memcpy(quality + t0, qo, sizeof(double) * T);
+    }
+    return 0;
+}
+
+// ------------------------------------------------------------------------ the single resident window: slot 0
+int pvio_b200_window_reset(pvio_b200_handle hh, const pvio_b200_window *constants) {
+    if (!constants) return PVIO_B200_EINVAL;
+    pvio_b200_window c = *constants;          // the arrays of `constants` are ignored, its plane counts with them
+    c.n_planes = 0; c.n_plane_tracks = 0;
+    return pvio_b200_batch_window_reset(hh, 0, &c);
+}
+
+int pvio_b200_window_set_prior(pvio_b200_handle hh, int n_prior, const double *S, const double *e, const double *state0) {
+    return pvio_b200_batch_window_set_prior(hh, 0, n_prior, S, e, state0);
+}
+
+int pvio_b200_window_append_frame(pvio_b200_handle hh, const double *state, int fixed, const double *imu_record) {
+    if (!state) return PVIO_B200_EINVAL;
+    pvio_b200_window_edit e{};
+    e.state = state; e.fixed = fixed; e.imu_record = imu_record;
+    return pvio_b200_batch_window_edit(hh, 1, &e);
+}
+
+int pvio_b200_window_add_tracks(pvio_b200_handle hh, int n, const int32_t *frame, const double *z, const double *inv_depth, int32_t *ids_out) {
+    pvio_b200_window_edit e{};
+    e.n_new_tracks = n; e.new_frame = frame; e.new_z = z; e.new_inv_depth = inv_depth; e.new_ids = ids_out;
+    return pvio_b200_batch_window_edit(hh, 1, &e);
+}
+
+int pvio_b200_window_add_observations(pvio_b200_handle hh, int n, const int32_t *track, const int32_t *frame, const double *z) {
+    pvio_b200_window_edit e{};
+    e.n_obs = n; e.obs_track = track; e.obs_frame = frame; e.obs_z = z;
+    return pvio_b200_batch_window_edit(hh, 1, &e);
+}
+
+int pvio_b200_window_remove_track(pvio_b200_handle hh, int32_t track) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const BwSlot *s = window0(h);
+    if (!s) return PVIO_B200_EINVAL;
+    if (track < 0 || track >= s->next_id) return fail(h, PVIO_B200_EINVAL, "window_remove_track: unknown track");
+    if (find_row(*s, track) < 0) return 0;    // already gone
+    pvio_b200_window_edit e{};
+    e.n_remove = 1; e.remove = &track;
+    return pvio_b200_batch_window_edit(hh, 1, &e);
+}
+
+int pvio_b200_window_solve(pvio_b200_handle hh, const pvio_b200_options *opt, pvio_b200_summary *summary) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const int32_t slot = 0;
+    return solve_slots(h, 1, &slot, opt, false, summary);
+}
+
+int pvio_b200_window_drop_victim(pvio_b200_handle hh) {
+    const int32_t slot = 0;
+    return pvio_b200_batch_window_drop_victim(hh, 1, &slot, nullptr, 0, nullptr, 0);
+}
+
+int pvio_b200_window_get(pvio_b200_handle hh, int32_t *n_frames, double *frames, int n_tracks, const int32_t *tracks,
+                         double *inv_depth, int32_t *anchor_frame, int32_t *n_observations) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const BwSlot *s = window0(h);
+    if (!s) return PVIO_B200_EINVAL;
+    if (n_tracks > 0 && !tracks) return fail(h, PVIO_B200_EINVAL, "window_get: null track list");
+    for (int i = 0; i < n_tracks; ++i)
+        if (tracks[i] < 0 || tracks[i] >= s->next_id) return fail(h, PVIO_B200_EINVAL, "window_get: unknown track");
+    if (n_frames) *n_frames = s->N;
+    if (!frames && n_tracks <= 0) return 0;   // the frame count is the host's
+    const int T = (int)s->ids.size();
+    std::vector<double> rho(T);
+    std::vector<int32_t> anchor(T), count(T);
+    const int32_t slot = 0;
+    TRY(pvio_b200_batch_window_download(hh, 1, &slot, nullptr, frames, (int64_t)s->N * kFrameStride, nullptr, T, nullptr,
+                                        rho.data(), anchor.data(), count.data(), nullptr, nullptr));
+    for (int i = 0; i < n_tracks; ++i) {
+        const int r = find_row(*s, tracks[i]);   // a gone track: anchor -1, no observations, its inverse depth not written
+        if (r >= 0 && inv_depth) inv_depth[i] = rho[r];
+        if (anchor_frame) anchor_frame[i] = r >= 0 ? anchor[r] : -1;
+        if (n_observations) n_observations[i] = r >= 0 ? count[r] : 0;
     }
     return 0;
 }

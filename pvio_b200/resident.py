@@ -1,4 +1,4 @@
-"""Host mirror of the resident sliding window (include/pvio_b200.h, csrc/resident.cu): the window persists in the handle
+"""Host mirror of the resident sliding window (include/pvio_b200.h, csrc/batch_window.cu): the window persists in the handle
 between keyframes; the caller reports appended frames, new tracks / observations and drops the oldest frame, which
 marginalises it into a prior that stays on the device (map/map.cpp:76-88, core/sliding_window_tracker.cpp:79-125)."""
 import ctypes as C
