@@ -277,8 +277,8 @@ int pvio_b200_batch_marginalize(pvio_b200_handle h, int n, double *S_out, int64_
  *    batch_solve, batch_marginalize and the *_host calls over a range holding a resident slot return PVIO_B200_EINVAL.
  *  - The kernel-launch count of a call does not depend on n.  An edit call makes one host -> device and one
  *    device -> host copy. */
-/* Start an empty resident window in `slot`.  Of `constants` the scalar members are kept (as pvio_b200_window_reset);
- * n_planes > 0 is rejected. */
+/* Start an empty resident window in `slot`.  Of `constants` the scalar members are kept (as pvio_b200_window_reset),
+ * plane_sqrt_inv_cov among them; n_planes > 0 is rejected (planes arrive through pvio_b200_batch_window_set_planes). */
 int pvio_b200_batch_window_reset(pvio_b200_handle h, int slot, const pvio_b200_window *constants);
 /* A prior given by the caller over frames 0 .. n_prior-1 (the 1e15 gauge prior of the first window,
  * sliding_window_tracker.cpp:100-112).  S [(15 n_prior)^2] row-major, e [15 n_prior], state0 [n_prior][16]. */
@@ -312,6 +312,30 @@ typedef struct pvio_b200_window_edit {
 } pvio_b200_window_edit;           /* 120 bytes on LP64 */
 /* n edits, each naming a different resident slot. */
 int pvio_b200_batch_window_edit(pvio_b200_handle h, int n, const pvio_b200_window_edit *edits);
+/* Plane factors of a resident slot (bundle_adjustor.cpp:162-196).  Every live track has a role, -1 for a new track:
+ *  -1      a landmark (TF_VALID, not TF_PLANE): inverse-depth landmark with >= 2 observations, in the marginaliser's
+ *          victim set when anchored in frame 0;
+ *  -2      a landmark that is TF_PLANE on a plane with fewer than 20 tracks: solved like -1, never in the victim set;
+ *  p >= 0  a plane track of plane p (landmark.plane_id of a plane with >= 20 tracks): one plane-distance factor over all
+ *          its window observations, anchor included; no inverse depth is solved, never in the victim set.
+ * A record replaces the slot's planes (n_planes 0 .. 4, plane_param [n_planes][4]: normal, distance) unless n_planes is
+ * -1, then sets the role of n_set live tracks, and their inverse depth in their anchor frame where inv_depth (may be
+ * NULL) is not NaN.  Rejected: a plane count outside -1 .. 4, non-finite plane parameters, an unknown or dead track, a
+ * track named twice, a role other than -1, -2 or a plane index below the slot's plane count after the record, an
+ * infinite inverse depth, and a track left with a role of a plane the record removes.  Edits, drops and resets keep the
+ * role of every track that stays; a reset clears the planes and the roles.  One host -> device copy; the named slots
+ * are re-laid out. */
+typedef struct pvio_b200_window_planes {
+    int32_t slot;
+    int32_t n_planes;                 /* -1: keep the slot's planes; 0 .. 4: replace them */
+    const double *plane_param;        /* [n_planes][4] normal, distance */
+    int32_t n_set;
+    const int32_t *track;             /* [n_set] live track ids of the slot */
+    const int32_t *role;              /* [n_set] -1, -2 or a plane index below the slot's plane count after this record */
+    const double *inv_depth;          /* [n_set] or NULL: new inverse depth in the track's anchor frame, NaN = keep */
+} pvio_b200_window_planes;            /* 48 bytes on LP64 */
+/* n records, each naming a different resident slot. */
+int pvio_b200_batch_window_set_planes(pvio_b200_handle h, int n, const pvio_b200_window_planes *records);
 /* BundleAdjustor::solve on the named slots: the trust-region chain of pvio_b200_batch_solve (per-window termination),
  * then the landmark post-pass (unless opt->run_postpass == 0); solved states and inverse depths stay in the slots and the
  * post-pass flags in the tracks.  Slots not named keep their windows bit for bit and run no iteration (their solver

@@ -84,6 +84,11 @@ class CWindowEdit(C.Structure):
                 ("obs_frame", c_i32p), ("obs_z", c_f64p), ("n_remove", C.c_int32), ("remove", c_i32p)]
 
 
+class CWindowPlanes(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n_planes", C.c_int32), ("plane_param", c_f64p), ("n_set", C.c_int32),
+                ("track", c_i32p), ("role", c_i32p), ("inv_depth", c_f64p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -100,7 +105,7 @@ EXPORTS = [
     "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve", "pvio_b200_batch_track_keypoints",
     "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig", "pvio_b200_batch_window_reset",
     "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
-    "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download",
+    "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
 ]
 
 _lib = None

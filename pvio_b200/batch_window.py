@@ -15,6 +15,7 @@ def _argtypes(L):
     L.pvio_b200_batch_window_reset.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindow)]
     L.pvio_b200_batch_window_set_prior.argtypes = [vp, C.c_int, C.c_int, _f64p, _f64p, _f64p]
     L.pvio_b200_batch_window_edit.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowEdit)]
+    L.pvio_b200_batch_window_set_planes.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowPlanes)]
     L.pvio_b200_batch_window_solve.argtypes = [vp, C.c_int, _i32p, C.POINTER(_lib.COptions), C.POINTER(_lib.CSummary)]
     L.pvio_b200_batch_window_drop_victim.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64, _f64p, C.c_int64]
     L.pvio_b200_batch_window_download.argtypes = [vp, C.c_int, _i32p, _i32p, _f64p, C.c_int64, _i32p, C.c_int64, _i32p,
@@ -45,6 +46,25 @@ class Edit:
     def frame(self, state16, fixed=False, imu_record=None):
         self.state, self.fixed = np.ascontiguousarray(state16, dtype=np.float64), bool(fixed)
         self.imu = None if imu_record is None else np.ascontiguousarray(imu_record, dtype=np.float64)
+        return self
+
+
+# roles of a track (pvio_b200_window_planes): a landmark; a landmark kept out of the marginaliser's victim set (TF_PLANE
+# on a plane with fewer than 20 tracks); a plane index p >= 0 makes the track a plane track of plane p
+LANDMARK, SMALL_PLANE = -1, -2
+
+
+class Planes:
+    """The plane factors of one slot (pvio_b200_window_planes), built up by the caller: the slot's planes (None: keep
+    them), and per track a role (LANDMARK, SMALL_PLANE or a plane index) with an optional new inverse depth."""
+
+    def __init__(self, slot, planes=None):
+        self.slot = int(slot)
+        self.planes = None if planes is None else np.ascontiguousarray(planes, dtype=np.float64).reshape(-1, 4)
+        self.tracks, self.roles, self.rho = [], [], []
+
+    def role(self, track, role, inv_depth=np.nan):
+        self.tracks.append(int(track)); self.roles.append(int(role)); self.rho.append(float(inv_depth))
         return self
 
 
@@ -98,6 +118,25 @@ class BatchWindows:
                 r.n_remove, r.remove = len(rm), _lib._ptr(rm, C.c_int32)
         self.ba._ck(self.lib.pvio_b200_batch_window_edit(self.h, len(edits), recs))
         return [o[:len(e.new)].copy() for o, e in zip(ids, edits)]
+
+    def set_planes(self, records):
+        """Apply a list of Planes (distinct slots) in one call."""
+        keep, recs = [], (_lib.CWindowPlanes * max(len(records), 1))()
+        for i, p in enumerate(records):
+            r = recs[i]
+            r.slot = p.slot
+            if p.planes is None:
+                r.n_planes = -1
+            else:
+                keep.append(p.planes)
+                r.n_planes, r.plane_param = len(p.planes), _lib._ptr(p.planes, C.c_double)
+            if p.tracks:
+                t, ro = np.array(p.tracks, dtype=np.int32), np.array(p.roles, dtype=np.int32)
+                rho = np.array(p.rho, dtype=np.float64)
+                keep += [t, ro, rho]
+                r.n_set = len(t)
+                r.track, r.role, r.inv_depth = _lib._ptr(t, C.c_int32), _lib._ptr(ro, C.c_int32), _lib._ptr(rho, C.c_double)
+        self.ba._ck(self.lib.pvio_b200_batch_window_set_planes(self.h, len(records), recs))
 
     def solve(self, slots, max_iterations=10, max_time=1e6, alias_bias=True, postpass=True):
         s = np.ascontiguousarray(slots, dtype=np.int32)

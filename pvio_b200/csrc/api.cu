@@ -88,9 +88,17 @@ int ensure_inertial(Handle *h) {
     return 0;
 }
 
-// Plane buffers grow on demand WITHOUT losing the slots already packed into the pinned staging area
-// (the device copies are refreshed by the next upload anyway).
-static int ensure_planes(Handle *h, int T, int O) {
+// device array src -> device array dst slot by slot, the arrays differing in slot stride only (on the handle's stream)
+template <typename T>
+static int copy_slots_d2d(Handle *h, DevBuf<T> &dst, const DevBuf<T> &src) {
+    CK(h, cudaMemcpy2DAsync(dst.d, sizeof(T) * dst.per, src.d, sizeof(T) * src.per, sizeof(T) * std::min(dst.per, src.per),
+                            (size_t)h->W, cudaMemcpyDeviceToDevice, h->stream));
+    return 0;
+}
+
+// Plane buffers grow on demand WITHOUT losing any slot's tables: the slots packed into the pinned staging area, and the
+// device copies, which the resident windows (batch_window.cu) build on the device and never upload.
+int ensure_planes(Handle *h, int T, int O) {
     if (h->have_planes && T <= h->Tcap && O <= h->Ocap) return 0;
     const int Tn = std::max({T, h->Tcap, 256}), On = std::max({O, h->Ocap, 256 * 8});
     const size_t W = h->W;
@@ -108,6 +116,9 @@ static int ensure_planes(Handle *h, int T, int O) {
             copy_slot(pp, i, h->plane_param, i); copy_slot(tp, i, h->pt_plane, i); copy_slot(tb, i, h->pt_begin, i);
             copy_slot(tf, i, h->pt_frame, i); copy_slot(tz, i, h->pt_z, i);
         }
+        TRY(copy_slots_d2d(h, pp, h->plane_param)); TRY(copy_slots_d2d(h, tp, h->pt_plane));
+        TRY(copy_slots_d2d(h, tb, h->pt_begin)); TRY(copy_slots_d2d(h, tf, h->pt_frame)); TRY(copy_slots_d2d(h, tz, h->pt_z));
+        CK(h, cudaStreamSynchronize(h->stream));      // the old arrays are freed below
     }
     h->plane_param = std::move(pp); h->pt_plane = std::move(tp); h->pt_begin = std::move(tb); h->pt_frame = std::move(tf);
     h->pt_z = std::move(tz);

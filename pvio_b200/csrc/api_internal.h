@@ -122,15 +122,18 @@ struct FmState {
 };
 
 // batch_window.cu: the resident windows of the batched slots; slot 0 is also the window of pvio_b200_window_*.  Per slot
-// the host keeps integers only: the frame count, the prior's frame count, the fixed mask, and for every live track (rows
-// in id order) its id and frame mask; the device keeps the track table (frame mask, inverse depth, fp64 keypoint per
-// window frame, post-pass flags) and the packed window.
+// the host keeps integers only: the frame count, the prior's frame count, the fixed mask, the plane count, and for every
+// live track (rows in id order) its id, frame mask and role; the device keeps the track table (frame mask, role, inverse
+// depth, fp64 keypoint per window frame, post-pass flags), the plane parameters and the packed window.
+// Role of a row: -1 a landmark; -2 a landmark that stays out of the marginaliser's victim set (a plane track of a plane
+// with fewer than 20 tracks); p >= 0 a plane track of plane p: one plane-distance factor over all its observations.
 struct BwSlot {
     bool on = false;                  // resident: the slot changes through pvio_b200_batch_window_* (and window_*) only
-    int N = 0, n_prior = 0, fixed = 0, inertial = 0;
+    int N = 0, n_prior = 0, fixed = 0, inertial = 0, n_planes = 0;
     int32_t next_id = 0;
     std::vector<int32_t> ids;         // live tracks, increasing: row r of the device table holds track ids[r]
     std::vector<uint32_t> mask;       // frame mask of each row
+    std::vector<int8_t> role;         // role of each row
 };
 struct BatchWindows {
     std::vector<BwSlot> slot;                    // [W]
@@ -140,6 +143,8 @@ struct BatchWindows {
     DevBuf<double2> tz;                          // [W][Mcap][Ncap] fp64 keypoint per window frame
     DevBuf<uint8_t> tvalid;                      // [W][Mcap] post-pass result of the last solve
     DevBuf<double> tqual;                        // [W][Mcap]
+    DevBuf<int8_t> trole;                        // [W][Mcap] role of each row (BwSlot::role)
+    DevBuf<double> tplane;                       // [W][Pcap][4] plane parameters (normal, distance)
     DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
     DevBuf<uint8_t> named;                       // [W] device: 1 for the slots a solve names
     DevBuf<uint8_t> stage;                       // both sides, grown: the one upload / download of a call
@@ -308,6 +313,9 @@ int run_marg_vision(Handle *h, int n, const int32_t *h_slots = nullptr, const in
 void drop_graphs(Handle *h);
 // api.cu, for the resident batched windows (batch_window.cu)
 int ensure_inertial(Handle *h);
+// plane-table capacity of at least T plane tracks and O plane observations per window; growth keeps every slot's tables,
+// the pinned staging and the device arrays
+int ensure_planes(Handle *h, int T, int O);
 // the trust-region solve of windows [0, n); named (device, [n], may be NULL): only windows with named[w] != 0 are solved,
 // the others are marked finished before the first body and cost no iteration
 int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named);

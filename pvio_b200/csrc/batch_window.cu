@@ -8,10 +8,17 @@
 // table) are rebuilt from the track table on the device, exactly as pack_window packs the window of the tracks with
 // >= 2 observations in id order: stably sorted by anchor (their lowest frame).
 //
-// The host keeps integers only (frame count, prior size, fixed mask, the id and frame mask of every live row), enough to
-// check every call completely before anything is staged, and to know the launch shapes.  The rows of a slot's table are
-// its live tracks in id order: removals compact the table (the storage of dead tracks is reused), new tracks append.
+// The host keeps integers only (frame count, prior size, fixed mask, plane count, the id, frame mask and role of every
+// live row), enough to check every call completely before anything is staged, and to know the launch shapes.  The rows
+// of a slot's table are its live tracks in id order: removals compact the table (the storage of dead tracks is reused),
+// new tracks append.
+// Plane factors (bundle_adjustor.cpp:162-196): the role of a row (BwSlot) decides what it is in the solve.  Rows of
+// role < 0 with >= 2 observations are the landmarks (role -2 ones stay out of the marginaliser's victim set,
+// bundle_adjustor.cpp:456-457); rows of role p >= 0 are the plane tracks of plane p, packed in row (= id) order with all
+// their observations, anchor included, into the plane tables the solve kernels read (pt_plane, pt_begin, pt_frame,
+// pt_z), with the slot's plane parameters.  The caller decides the roles (pvio_b200_batch_window_set_planes).
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <vector>
 
@@ -29,8 +36,10 @@ struct BwEdit {                       // one slot's edit, applied by bw_edit_ker
 };
 struct BwNew { int32_t row, id, frame, pad; double zx, zy, rho; };
 struct BwObs { int32_t row, frame; double zx, zy; };
-struct BwLayout { int32_t slot, N, T, fixed, n_prior, inertial; };     // a slot's window as the kernels rebuild it
+struct BwLayout { int32_t slot, N, T, fixed, n_prior, inertial, n_planes, pad; };   // a slot's window as the kernels rebuild it
 struct BwDl { int32_t slot, N, T, pad; int64_t off; };                  // download: bytes into the result area
+struct BwPlanes { int32_t slot, n_planes, n_set, set_off, param_off, pad; };   // one set_planes record (n_planes < 0: keep)
+struct BwRole { int32_t row, role; double rho; };                       // rho NaN: keep the row's inverse depth
 
 struct BwArgs {
     WinHdr *hdr;
@@ -45,10 +54,15 @@ struct BwArgs {
     double2 *tz;
     uint8_t *tvalid;
     double *tqual;
+    int8_t *trole;
+    double *tplane;
     int32_t *lm_row;
     const uint8_t *valid;
     const double *quality;
-    int Ncap, Mcap, Kcap;
+    double *plane_param;                  // the plane tables of the solve (null until a slot has plane tracks)
+    int32_t *pt_plane, *pt_begin, *pt_frame;
+    float *pt_z;
+    int Ncap, Mcap, Kcap, Pcap, Tcap, Ocap;
 };
 
 constexpr int kBwThreads = 256;
@@ -80,10 +94,16 @@ __device__ int bw_compact(const BwArgs &a, int w, int T, int *sh) {
         const bool live = r < T && a.tmask[base + r] != 0u;
         int tot;
         const int d = carry + bw_block_scan(live ? 1 : 0, sh, tot);
-        int32_t id = 0; uint32_t m = 0; double rho = 0.0, q = 0.0; uint8_t v = 0;
-        if (live) { id = a.tid[base + r]; m = a.tmask[base + r]; rho = a.trho[base + r]; v = a.tvalid[base + r]; q = a.tqual[base + r]; }
+        int32_t id = 0; uint32_t m = 0; double rho = 0.0, q = 0.0; uint8_t v = 0; int8_t ro = -1;
+        if (live) {
+            id = a.tid[base + r]; m = a.tmask[base + r]; rho = a.trho[base + r]; v = a.tvalid[base + r]; q = a.tqual[base + r];
+            ro = a.trole[base + r];
+        }
         __syncthreads();
-        if (live && d != r) { a.tid[base + d] = id; a.tmask[base + d] = m; a.trho[base + d] = rho; a.tvalid[base + d] = v; a.tqual[base + d] = q; }
+        if (live && d != r) {
+            a.tid[base + d] = id; a.tmask[base + d] = m; a.trho[base + d] = rho; a.tvalid[base + d] = v; a.tqual[base + d] = q;
+            a.trole[base + d] = ro;
+        }
         __syncthreads();
         for (int f = 0; f < a.Ncap; ++f) {
             double2 z = make_double2(0.0, 0.0);
@@ -94,7 +114,7 @@ __device__ int bw_compact(const BwArgs &a, int w, int T, int *sh) {
         }
         carry += tot;
     }
-    for (int r = carry + threadIdx.x; r < T; r += kBwThreads) a.tmask[base + r] = 0u;
+    for (int r = carry + threadIdx.x; r < T; r += kBwThreads) { a.tmask[base + r] = 0u; a.trole[base + r] = -1; }
     __syncthreads();
     return carry;
 }
@@ -124,7 +144,7 @@ __global__ void __launch_bounds__(kBwThreads) bw_edit_kernel(BwArgs a, const BwE
     for (int i = threadIdx.x; i < e.n_new; i += kBwThreads) {
         const BwNew t = nw[e.new_off + i];
         const size_t R = base + t.row;
-        a.tid[R] = t.id; a.tmask[R] = 1u << t.frame; a.trho[R] = t.rho; a.tvalid[R] = 0; a.tqual[R] = 0.0;
+        a.tid[R] = t.id; a.tmask[R] = 1u << t.frame; a.trho[R] = t.rho; a.tvalid[R] = 0; a.tqual[R] = 0.0; a.trole[R] = -1;
         a.tz[R * a.Ncap + t.frame] = make_double2(t.zx, t.zy);
     }
     __syncthreads();
@@ -143,20 +163,29 @@ __global__ void __launch_bounds__(kBwThreads) bw_edit_kernel(BwArgs a, const BwE
     for (int i = threadIdx.x; i < e.n_new; i += kBwThreads) out[e.out_off + 1 + i] = a.tid[base + nw[e.new_off + i].row];
 }
 
+// the anchor of row r as a landmark (role < 0, >= 2 observations), kMaxFrames for the other rows
+__device__ __forceinline__ int bw_lm_anchor(const BwArgs &a, size_t R) {
+    const uint32_t m = a.tmask[R];
+    return (a.trole[R] < 0 && __popc(m) >= 2) ? __ffs(m) - 1 : kMaxFrames;
+}
+
 // One CTA per slot: the packed window from the track table, as pack_window builds it from build_view's window.
 __global__ void __launch_bounds__(kBwThreads) bw_layout_kernel(BwArgs a, const BwLayout *lay) {
     __shared__ int sh[kBwWarps + 1];
     __shared__ int cnt[kMaxFrames], first[kMaxFrames], run[kMaxFrames];
     __shared__ int wcnt[kBwWarps][kMaxFrames + 1];
+    __shared__ int n_pl;
     const BwLayout L = lay[blockIdx.x];
     const int w = L.slot, N = L.N, T = L.T;
     const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
     const size_t base = (size_t)w * a.Mcap;
     if (threadIdx.x < kMaxFrames) { cnt[threadIdx.x] = 0; run[threadIdx.x] = 0; }
+    if (threadIdx.x == 0) n_pl = 0;
     __syncthreads();
     for (int r = threadIdx.x; r < T; r += kBwThreads) {
-        const uint32_t m = a.tmask[base + r];
-        if (__popc(m) >= 2) atomicAdd(&cnt[__ffs(m) - 1], 1);
+        const int an = bw_lm_anchor(a, base + r);
+        if (an < kMaxFrames) atomicAdd(&cnt[an], 1);
+        else if (a.trole[base + r] >= 0) atomicAdd(&n_pl, 1);
     }
     __syncthreads();
     if (threadIdx.x == 0) { int s = 0; for (int k = 0; k < kMaxFrames; ++k) { first[k] = s; s += cnt[k]; } sh[kBwWarps] = s; }
@@ -166,8 +195,7 @@ __global__ void __launch_bounds__(kBwThreads) bw_layout_kernel(BwArgs a, const B
     // landmark order: anchor, then row (= id) -- a counting sort, stable chunk by chunk
     for (int c0 = 0; c0 < T; c0 += kBwThreads) {
         const int r = c0 + threadIdx.x;
-        const uint32_t m = r < T ? a.tmask[base + r] : 0u;
-        const int an = __popc(m) >= 2 ? __ffs(m) - 1 : kMaxFrames;
+        const int an = r < T ? bw_lm_anchor(a, base + r) : kMaxFrames;
         for (int i = threadIdx.x; i < kBwWarps * (kMaxFrames + 1); i += kBwThreads) (&wcnt[0][0])[i] = 0;
         __syncthreads();
         const unsigned peers = __match_any_sync(0xffffffffu, an);
@@ -199,7 +227,7 @@ __global__ void __launch_bounds__(kBwThreads) bw_layout_kernel(BwArgs a, const B
             const double2 *z = a.tz + (base + row) * a.Ncap;
             LmRec lr;
             lr.zrx = (float)z[an].x; lr.zry = (float)z[an].y;
-            lr.meta = lm_meta(an, an == 0 ? 1 : 0, n, seen);
+            lr.meta = lm_meta(an, (an == 0 && a.trole[base + row] != -2) ? 1 : 0, n, seen);
             lr.obs_begin = ob;
             a.lms[base + lp] = lr;
             a.rho[base + lp] = a.trho[base + row];
@@ -213,13 +241,45 @@ __global__ void __launch_bounds__(kBwThreads) bw_layout_kernel(BwArgs a, const B
         }
         carry += tot;
     }
+    // plane tracks in row order: plane index, CSR of their observations (every frame of the mask, increasing), fp32
+    // keypoints; the host grew the tables to the slot's counts before the launch
+    const int T_pl = n_pl;
+    if (T_pl > 0) {
+        const size_t pb = (size_t)w * a.Tcap, ob0 = (size_t)w * a.Ocap;
+        int t_carry = 0, o_carry = 0;
+        for (int c0 = 0; c0 < T; c0 += kBwThreads) {
+            const int r = c0 + threadIdx.x;
+            const int ro = r < T ? a.trole[base + r] : -1;
+            const uint32_t m = ro >= 0 ? a.tmask[base + r] : 0u;
+            int t_tot, o_tot;
+            const int t = t_carry + bw_block_scan(ro >= 0 ? 1 : 0, sh, t_tot);
+            const int ob = o_carry + bw_block_scan(__popc(m), sh, o_tot);
+            if (ro >= 0) {
+                a.pt_plane[pb + t] = ro;
+                a.pt_begin[pb + (size_t)w + t] = ob;          // pt_begin: Tcap + 1 entries per window
+                const double2 *z = a.tz + (base + r) * a.Ncap;
+                int k = 0;
+                for (uint32_t s = m; s; s &= s - 1) {
+                    const int f = __ffs(s) - 1;
+                    a.pt_frame[ob0 + ob + k] = f;
+                    a.pt_z[2 * (ob0 + ob + k)] = (float)z[f].x; a.pt_z[2 * (ob0 + ob + k) + 1] = (float)z[f].y;
+                    ++k;
+                }
+            }
+            t_carry += t_tot; o_carry += o_tot;
+        }
+        if (threadIdx.x == 0) a.pt_begin[pb + (size_t)w + T_pl] = o_carry;
+    }
+    if (a.plane_param)
+        for (int i = threadIdx.x; i < 4 * L.n_planes; i += kBwThreads)
+            a.plane_param[(size_t)w * a.Pcap * 4 + i] = a.tplane[(size_t)w * a.Pcap * 4 + i];
     WinHdr &H = a.hdr[w];
     for (int i = threadIdx.x; i < kMaxChunks; i += kBwThreads) { H.chunk_begin[i] = 0; H.chunk_meta[i] = 0; }
     __syncthreads();
     if (threadIdx.x == 0) {
         const int n_imu = L.inertial ? max(N - 1, 0) : 0;
         H.N = N; H.M = M; H.K = carry; H.use_inertial = L.inertial;
-        H.n_imu = n_imu; H.n_prior = L.inertial ? L.n_prior : 0; H.n_planes = 0; H.n_ptracks = 0;
+        H.n_imu = n_imu; H.n_prior = L.inertial ? L.n_prior : 0; H.n_planes = L.n_planes; H.n_ptracks = T_pl;
         H.fixed_mask = L.fixed; H.pad0 = 0; H.pad1 = 0;
         int nch = 0;
         for (int an = 0; an < N; ++an)
@@ -242,8 +302,8 @@ __global__ void __launch_bounds__(kBwThreads) bw_layout_kernel(BwArgs a, const B
 }
 
 // After a solve and its post-pass, one CTA per named slot: solved inverse depths back into the tracks, the post-pass
-// flags of the landmarks into their rows (0 / 0 for the rows that did not take part, and for every row when the solve
-// ran no post-pass: flags == 0)
+// flags of the landmarks into their rows (0 / 0 for the rows that did not take part -- plane tracks among them, as
+// ba_solve gives them no flags -- and for every row when the solve ran no post-pass: flags == 0)
 __global__ void __launch_bounds__(kBwThreads) bw_writeback_kernel(BwArgs a, const BwLayout *lay, int flags) {
     const BwLayout L = lay[blockIdx.x];
     const int w = L.slot;
@@ -255,6 +315,21 @@ __global__ void __launch_bounds__(kBwThreads) bw_writeback_kernel(BwArgs a, cons
         const int row = a.lm_row[base + lp];
         a.trho[base + row] = a.rho[base + lp];
         if (flags) { a.tvalid[base + row] = a.valid[base + lp]; a.tqual[base + row] = a.quality[base + lp]; }
+    }
+}
+
+// One CTA per set_planes record (each names a different slot): the slot's plane parameters, then the roles and inverse
+// depths of the named rows
+__global__ void __launch_bounds__(kBwThreads) bw_planes_kernel(BwArgs a, const BwPlanes *recs, const BwRole *roles,
+                                                                const double *params) {
+    const BwPlanes p = recs[blockIdx.x];
+    const int w = p.slot;
+    const size_t base = (size_t)w * a.Mcap;
+    for (int i = threadIdx.x; i < 4 * p.n_planes; i += kBwThreads) a.tplane[(size_t)w * a.Pcap * 4 + i] = params[p.param_off + i];
+    for (int i = threadIdx.x; i < p.n_set; i += kBwThreads) {
+        const BwRole r = roles[p.set_off + i];
+        a.trole[base + r.row] = (int8_t)r.role;
+        if (!isnan(r.rho)) a.trho[base + r.row] = r.rho;
     }
 }
 
@@ -357,8 +432,11 @@ static BwArgs bw_args(Handle *h) {
     a.hdr = h->hdr.d; a.cst = h->cst.d; a.lms = h->lms.d; a.obs = h->obs.d; a.rho = h->rho.d; a.frames = h->frames.d;
     a.imu_data = h->imu_data.d; a.imu_idx = h->imu_idx.d; a.prior_frames = h->prior_frames.d;
     a.tid = b.tid.d; a.tmask = b.tmask.d; a.trho = b.trho.d; a.tz = b.tz.d; a.tvalid = b.tvalid.d; a.tqual = b.tqual.d;
+    a.trole = b.trole.d; a.tplane = b.tplane.d;
     a.lm_row = b.lm_row.d; a.valid = h->valid.d; a.quality = h->quality.d;
-    a.Ncap = h->Ncap; a.Mcap = h->Mcap; a.Kcap = h->Kcap;
+    a.plane_param = h->plane_param.d; a.pt_plane = h->pt_plane.d; a.pt_begin = h->pt_begin.d; a.pt_frame = h->pt_frame.d;
+    a.pt_z = h->pt_z.d;
+    a.Ncap = h->Ncap; a.Mcap = h->Mcap; a.Kcap = h->Kcap; a.Pcap = h->Pcap; a.Tcap = h->Tcap; a.Ocap = h->Ocap;
     return a;
 }
 
@@ -368,6 +446,7 @@ static int ensure_bw(Handle *h) {
     const size_t W = h->W, M = h->Mcap;
     TRY(alloc(h, b.tid, W * M, kDevice)); TRY(alloc(h, b.tmask, W * M, kDevice)); TRY(alloc(h, b.trho, W * M, kDevice));
     TRY(alloc(h, b.tz, W * M * h->Ncap, kDevice)); TRY(alloc(h, b.tvalid, W * M, kDevice)); TRY(alloc(h, b.tqual, W * M, kDevice));
+    TRY(alloc(h, b.trole, W * M, kDevice)); TRY(alloc(h, b.tplane, W * h->Pcap * 4, kDevice));
     TRY(alloc(h, b.lm_row, W * M, kDevice)); TRY(alloc(h, b.named, W, kDevice));
     b.slot.resize(W);
     return 0;
@@ -385,13 +464,15 @@ struct Packer {
     }
 };
 
-// the window of a slot as the checks and the launch shapes see it
-struct BwShape { int M = 0, K = 0, chunks = 0, max_obs = 0; };
+// the window of a slot as the checks and the launch shapes see it; T / O: plane tracks and their observations
+struct BwShape { int M = 0, K = 0, chunks = 0, max_obs = 0, T = 0, O = 0; };
 static BwShape shape_of(const BwSlot &s) {
     BwShape r;
     int cnt[kMaxFrames] = {};
-    for (uint32_t m : s.mask) {
+    for (size_t i = 0; i < s.mask.size(); ++i) {
+        const uint32_t m = s.mask[i];
         const int p = __builtin_popcount(m);
+        if (s.role[i] >= 0) { ++r.T; r.O += p; continue; }
         if (p < 2) continue;
         ++cnt[__builtin_ctz(m)]; ++r.M; r.K += p - 1; r.max_obs = std::max(r.max_obs, p - 1);
     }
@@ -418,13 +499,21 @@ static void host_header(Handle *h, int slot) {
     memset(&H, 0, sizeof(H));
     H.N = s.N; H.M = sh.M; H.K = sh.K; H.use_inertial = s.inertial; H.n_imu = s.inertial ? std::max(s.N - 1, 0) : 0;
     H.n_prior = s.inertial ? s.n_prior : 0; H.fixed_mask = s.fixed; H.n_chunks = sh.chunks;
+    H.n_planes = s.n_planes; H.n_ptracks = sh.T;            // batch_shape: plane tracks take the full solve kernel
     h->slot_N[slot] = s.N; h->slot_M[slot] = sh.M; h->slot_K[slot] = sh.K;
     h->perm[slot].clear(); h->perm_identity[slot] = 1;      // no caller landmark order: nothing of a former pack survives
 }
 
-static BwLayout layout_of(const Handle *h, int slot) {
-    const BwSlot &s = h->bw.slot[slot];
-    return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial};
+static BwLayout layout_from(int slot, const BwSlot &s) {
+    return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial, s.n_planes, 0};
+}
+static BwLayout layout_of(const Handle *h, int slot) { return layout_from(slot, h->bw.slot[slot]); }
+
+// plane-table capacity for the windows the n slots of a call will hold, before anything of the call is staged
+static int ensure_plane_tables(Handle *h, const std::vector<BwSlot> &next) {
+    int T = 0, O = 0;
+    for (const BwSlot &s : next) { const BwShape sh = shape_of(s); T = std::max(T, sh.T); O = std::max(O, sh.O); }
+    return T > 0 ? ensure_planes(h, T, O) : 0;
 }
 
 static int check_slots(Handle *h, int n, const int32_t *slots, const char *what) {
@@ -637,8 +726,8 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
         {   // compaction
             size_t o = 0;
             for (size_t r = 0; r < s.ids.size(); ++r)
-                if (s.mask[r]) { s.ids[o] = s.ids[r]; s.mask[o] = s.mask[r]; ++o; }
-            s.ids.resize(o); s.mask.resize(o);
+                if (s.mask[r]) { s.ids[o] = s.ids[r]; s.mask[o] = s.mask[r]; s.role[o] = s.role[r]; ++o; }
+            s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
         }
         if (E.state) {
             if (s.N >= h->Ncap) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: window of more than max_frames frames");
@@ -655,7 +744,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
             const int f = E.new_frame[k];
             if (f < 0 || f >= s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: track starts outside the window");
             BwNew t{(int32_t)s.ids.size(), s.next_id, f, 0, E.new_z[2 * k], E.new_z[2 * k + 1], E.new_inv_depth[k]};
-            s.ids.push_back(s.next_id++); s.mask.push_back(1u << f);
+            s.ids.push_back(s.next_id++); s.mask.push_back(1u << f); s.role.push_back(-1);
             nws.push_back(t);
         }
         R.obs_off = (int)obs.size();
@@ -677,9 +766,10 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
         out_ints += 1 + E.n_new_tracks;
         next[i] = std::move(s);
     }
+    TRY(ensure_plane_tables(h, next));                 // observations of plane tracks may outgrow the plane tables
     Packer p;
     std::vector<BwLayout> lays(n);
-    for (int i = 0; i < n; ++i) lays[i] = BwLayout{slots[i], next[i].N, (int)next[i].ids.size(), next[i].fixed, next[i].n_prior, next[i].inertial};
+    for (int i = 0; i < n; ++i) lays[i] = layout_from(slots[i], next[i]);
     const size_t o_ed = p.put(recs.data(), n), o_lay = p.put(lays.data(), n), o_sl = p.put(slots.data(), n);
     const size_t o_rm = p.put(rm.data(), rm.size()), o_nw = p.put(nws.data(), nws.size()), o_ob = p.put(obs.data(), obs.size());
     const size_t o_x = p.put(xs.data(), xs.size());
@@ -704,6 +794,71 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
         if (r[0] != (int32_t)h->bw.slot[slots[i]].ids.size())
             return fail(h, PVIO_B200_ECUDA, "batch_window_edit: the device track table disagrees with the host's");
         if (edits[i].new_ids) memcpy(edits[i].new_ids, r + 1, sizeof(int32_t) * edits[i].n_new_tracks);
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_set_planes(pvio_b200_handle hh, int n, const pvio_b200_window_planes *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_set_planes: bad slot list"));
+    // every record is applied to a copy of its slot's host mirror; nothing is staged before all of them passed
+    std::vector<BwSlot> next(n);
+    std::vector<BwPlanes> recs(n);
+    std::vector<BwRole> roles;
+    std::vector<double> params;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_planes &R = records[i];
+        BwSlot s = h->bw.slot[R.slot];
+        if (R.n_planes < -1 || R.n_planes > h->Pcap) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: plane count outside -1 (keep) .. 4");
+        if (R.n_set < 0 || (R.n_set > 0 && (!R.track || !R.role)) || (R.n_planes > 0 && !R.plane_param))
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: null array");
+        recs[i] = BwPlanes{R.slot, std::max(R.n_planes, 0), R.n_set, (int32_t)roles.size(), (int32_t)params.size(), 0};
+        if (R.n_planes >= 0) {
+            for (int k = 0; k < 4 * R.n_planes; ++k)
+                if (!std::isfinite(R.plane_param[k])) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: non-finite plane parameters");
+            params.insert(params.end(), R.plane_param, R.plane_param + 4 * R.n_planes);
+            s.n_planes = R.n_planes;
+        }
+        std::vector<uint8_t> named(s.ids.size(), 0);
+        for (int k = 0; k < R.n_set; ++k) {
+            const int r = find_row(s, R.track[k]);
+            if (r < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: unknown or dead track");
+            if (named[r]) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: a track named twice");
+            named[r] = 1;
+            const int role = R.role[k];
+            if (role < -2 || role >= s.n_planes) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: role not -1, -2 or a plane of the slot");
+            const double rho = R.inv_depth ? R.inv_depth[k] : NAN;
+            if (std::isinf(rho)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: infinite inverse depth");
+            s.role[r] = (int8_t)role;
+            roles.push_back(BwRole{r, role, rho});
+        }
+        for (int8_t ro : s.role)
+            if (ro >= s.n_planes) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: a track keeps a plane the slot no longer has");
+        TRY(check_window(h, s));
+        next[i] = std::move(s);
+    }
+    TRY(ensure_plane_tables(h, next));
+    Packer p;
+    std::vector<BwLayout> lays(n);
+    for (int i = 0; i < n; ++i) lays[i] = layout_from(slots[i], next[i]);
+    const size_t o_rec = p.put(recs.data(), n), o_lay = p.put(lays.data(), n), o_sl = p.put(slots.data(), n);
+    const size_t o_ro = p.put(roles.data(), roles.size()), o_pa = p.put(params.data(), params.size());
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    bw_planes_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwPlanes *>(din + o_rec),
+        reinterpret_cast<const BwRole *>(din + o_ro), reinterpret_cast<const double *>(din + o_pa));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(relayout(h, din, o_lay, o_sl, n, false));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        h->bw.slot[slots[i]] = std::move(next[i]);
+        host_header(h, slots[i]);
     }
     return 0;
 }
@@ -734,9 +889,9 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
         size_t o = 0;                                                  // map.cpp:76-88 on the host mirror
         for (size_t r = 0; r < s.ids.size(); ++r) {
             const uint32_t m = s.mask[r] >> 1;
-            if (m) { s.ids[o] = s.ids[r]; s.mask[o] = m; ++o; }
+            if (m) { s.ids[o] = s.ids[r]; s.mask[o] = m; s.role[o] = s.role[r]; ++o; }
         }
-        s.ids.resize(o); s.mask.resize(o);
+        s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
         --s.N; s.fixed >>= 1; s.n_prior = s.N;
         TRY(check_window(h, s));
         next[i] = std::move(s);
@@ -744,7 +899,7 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
     std::vector<BwLayout> before(n), after(n);
     for (int i = 0; i < n; ++i) {
         before[i] = layout_of(h, slots[i]);
-        after[i] = BwLayout{slots[i], next[i].N, (int)next[i].ids.size(), next[i].fixed, next[i].n_prior, next[i].inertial};
+        after[i] = layout_from(slots[i], next[i]);
     }
     Packer p;
     const size_t o_sl = p.put(slots, n), o_b = p.put(before.data(), n), o_a = p.put(after.data(), n);

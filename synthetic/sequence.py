@@ -15,15 +15,49 @@ from . import so3, synth
 
 
 class Run:
-    def __init__(self, F=26, N=6, M=260, seed=700):
+    def __init__(self, F=26, N=6, M=260, seed=700, planes=0):
+        """planes > 0: synth.make_cfg3(planes=...) over the long run; its plane tracks follow the landmarks in `tracks`"""
         self.F, self.N = F, N
-        self.w, self.guess, self.truth = synth.make_cfg3(seed=seed, N=F, M=M, prior='none')
+        self.w, self.guess, self.truth = synth.make_cfg3(seed=seed, N=F, M=M, prior='none', planes=planes)
         w = self.w
-        self.tracks = []                      # per landmark: sorted frame list and keypoints
+        self.tracks = []                      # per track (landmarks, then plane tracks): sorted frame list and keypoints
         for l in range(w.M):
             fr = [int(w.lm_anchor[l])] + [int(f) for f in w.obs_frame[w.lm_obs_begin[l]:w.lm_obs_begin[l + 1]]]
             zs = [w.lm_z_ref[l]] + [w.obs_z[k] for k in range(w.lm_obs_begin[l], w.lm_obs_begin[l + 1])]
             self.tracks.append((fr, zs))
+        self.plane_of = [-1] * w.M            # per track: the plane a plane track was drawn on, -1 for a landmark
+        self.rho0 = list(self.guess.rho)      # per track: initial inverse depth in its first frame
+        for t in range(w.n_ptracks):          # plane points: the anchor ray meets the plane (guess pose of the anchor)
+            ks = range(int(w.pt_obs_begin[t]), int(w.pt_obs_begin[t + 1]))
+            fr, zs = [int(w.pt_obs_frame[k]) for k in ks], [w.pt_obs_z[k] for k in ks]
+            self.tracks.append((fr, zs))
+            p = int(w.pt_plane[t])
+            self.plane_of.append(p)
+            qc, pc = self.cam_pose(self.guess.q[fr[0]], self.guess.p[fr[0]])
+            u = so3.qrot(qc, np.array([zs[0][0], zs[0][1], 1.0]))
+            self.rho0.append((w.plane_normal[p] @ u) / (w.plane_distance[p] - w.plane_normal[p] @ pc))
+        self.rho0 = np.array(self.rho0)
+
+    def role(self, l, k):
+        """The role the host shim gives track l in the window of keyframe k (pvio_b200_window_planes): the plane
+        extractor casts every 11th landmark onto a plane from keyframe 3; every 7th plane track is revalidated off its
+        plane at keyframe 5 and stays a landmark; plane 1 has fewer than 20 tracks in keyframes 4 .. 7 (role -2)."""
+        n_planes, p = self.w.n_planes, self.plane_of[l]
+        if p < 0:
+            return (l // 11) % n_planes if n_planes > 0 and l % 11 == 0 and k >= 3 else -1
+        if (l - self.w.M) % 7 == 0 and k >= 5:
+            return -1
+        return -2 if p == 1 and 4 <= k < 8 else p
+
+    def planes_at(self, k):
+        """[n_planes][4] the plane parameters of keyframe k (the extractor refines them after every keyframe)"""
+        w = self.w
+        return np.concatenate([w.plane_normal, (w.plane_distance + 1e-3 * k)[:, None]], axis=1)
+
+    def revalidated_rho(self, l):
+        """the inverse depth the revalidation gives a plane track that becomes a landmark (set_landmark_point), in its
+        anchor frame at that keyframe"""
+        return 1.1 * self.rho0[l]
 
     def cam_pose(self, q, p):
         return so3.qmul(q, self.w.cam_q_cs), p + so3.qrot(q, self.w.cam_p_cs)
@@ -37,8 +71,10 @@ class Chain:
         g = run.guess
         self.q, self.p, self.v, self.bg, self.ba = g.q.copy(), g.p.copy(), g.v.copy(), g.bg.copy(), g.ba.copy()
         self.anchor = np.array([t[0][0] for t in run.tracks])
-        self.rho = g.rho.copy()
+        self.rho = run.rho0.copy()
         self.prior = None                     # dict(frames (absolute), S, e, x0 [n][16])
+        self.roles = {}                       # track -> role in the last gathered window (tracks seen there)
+        self.pt_ids = []                      # plane tracks of the last gathered window, in the order of its pt tables
 
     def _reanchor(self, l, new_anchor):
         """Track::first_frame changes when the old anchor leaves the window: the inverse depth is re-expressed in the next
@@ -55,22 +91,35 @@ class Chain:
         self.rho[l] = 1.0 / y[2]
 
     def window(self, k):
-        """Window over absolute frames [k, k + N): (Window, State, landmark ids)."""
+        """Window over absolute frames [k, k + N): (Window, State, landmark ids).  With planes (Run.role): landmarks are
+        the tracks of role < 0 with >= 2 observations (role -2: lm_in_victim = 0), plane tracks those of role >= 0 with all
+        their observations, in the order the resident slot creates them (first frame, then track); a plane track that
+        becomes a landmark takes Run.revalidated_rho."""
         run, N = self.run, self.run.N
         src = run.w
         w = dataclasses.replace(src)
         w.N = N
         w.frame_fixed = np.zeros(N, dtype=np.uint8)
         lm_ids, anchors, zref, begins, of, oz, victim, rho = [], [], [], [0], [], [], [], []
+        pts = []
         for l, (fr, zs) in enumerate(run.tracks):
             inw = [(f, z) for f, z in zip(fr, zs) if k <= f < k + N]
-            if len(inw) < 2:
+            if not inw:
+                continue
+            role, prev = run.role(l, k), self.roles.get(l, -1)
+            self.roles[l] = role
+            if len(inw) < 2 and role < 0:
                 continue
             if self.anchor[l] != inw[0][0]:
                 if self.anchor[l] < inw[0][0]:
                     self._reanchor(l, inw[0][0])
                 else:
                     continue
+            if prev >= 0 and role == -1:
+                self.rho[l] = run.revalidated_rho(l)
+            if role >= 0:
+                pts.append((fr[0], l, role, inw))
+                continue
             lm_ids.append(l)
             anchors.append(inw[0][0] - k)
             zref.append(inw[0][1])
@@ -78,7 +127,7 @@ class Chain:
                 of.append(f - k)
                 oz.append(z)
             begins.append(len(of))
-            victim.append(1 if inw[0][0] == k else 0)
+            victim.append(1 if inw[0][0] == k and role != -2 else 0)
             rho.append(self.rho[l])
         w.M, w.K = len(lm_ids), len(of)
         w.lm_anchor = np.array(anchors, dtype=np.int32)
@@ -106,7 +155,17 @@ class Chain:
             x0 = pr['x0']
             w.prior_q0, w.prior_p0, w.prior_v0 = x0[:, 0:4].copy(), x0[:, 4:7].copy(), x0[:, 7:10].copy()
             w.prior_bg0, w.prior_ba0 = x0[:, 10:13].copy(), x0[:, 13:16].copy()
-        w.n_planes, w.n_ptracks = 0, 0
+        pts.sort(key=lambda t: t[:2])
+        self.pt_ids = [t[1] for t in pts]
+        w.n_planes = src.n_planes
+        if src.n_planes > 0:
+            pl = run.planes_at(k)
+            w.plane_normal, w.plane_distance = pl[:, :3].copy(), pl[:, 3].copy()
+        w.n_ptracks = len(pts)
+        w.pt_plane = np.array([t[2] for t in pts], dtype=np.int32)
+        w.pt_obs_begin = np.concatenate([[0], np.cumsum([len(t[3]) for t in pts])]).astype(np.int32)
+        w.pt_obs_frame = np.array([f - k for t in pts for f, _ in t[3]], dtype=np.int32)
+        w.pt_obs_z = np.array([z for t in pts for _, z in t[3]]).reshape(-1, 2)
         w.validate()
         return w, st, lm_ids
 
@@ -200,7 +259,7 @@ class WindowModel:
             self.frames.append(f_abs)
         ids = []
         for (f, z, rho), l in zip(e.new, getattr(e, 'landmarks', [None] * len(e.new))):
-            self.tracks[self.next_id] = dict(l=l, frames=[f], zs=[np.asarray(z, dtype=float)], rho=rho)
+            self.tracks[self.next_id] = dict(l=l, frames=[f], zs=[np.asarray(z, dtype=float)], rho=rho, role=-1)
             ids.append(self.next_id)
             self.next_id += 1
         for i, f, z in e.obs:
@@ -222,14 +281,30 @@ class WindowModel:
                 continue
             t['frames'] = [f - 1 for f in t['frames']]
 
+    def set_planes(self, p):
+        """apply a pvio_b200.batch_window.Planes record: the roles of its tracks"""
+        for i, role in zip(p.tracks, p.roles):
+            self.tracks[i]['role'] = role
+
     def view(self):
-        """landmark -> (anchor, z_ref, obs frames, obs keypoints) of the tracks with >= 2 observations, in id order"""
+        """landmark -> (anchor, z_ref, obs frames, obs keypoints) of the tracks of role < 0 with >= 2 observations, in
+        id order"""
         out = {}
         for i in sorted(self.tracks):
             t = self.tracks[i]
-            if len(t['frames']) >= 2:
+            if t['role'] < 0 and len(t['frames']) >= 2:
                 out[t['l']] = (t['frames'][0], t['zs'][0], list(t['frames'][1:]), [z for z in t['zs'][1:]])
         return out
+
+    def victims(self):
+        """landmark -> lm_in_victim of the landmarks of view(): anchored in frame 0 and not role -2"""
+        return {t['l']: int(t['frames'][0] == 0 and t['role'] != -2) for t in self.tracks.values()
+                if t['role'] < 0 and len(t['frames']) >= 2}
+
+    def plane_view(self):
+        """the plane tracks (role >= 0) in id order: (landmark, plane, frames, keypoints)"""
+        return [(t['l'], t['role'], list(t['frames']), list(t['zs']))
+                for t in (self.tracks[i] for i in sorted(self.tracks)) if t['role'] >= 0]
 
 
 class ModelWindows:
@@ -247,6 +322,10 @@ class ModelWindows:
 
     def edit(self, edits):
         return [np.array(self.m[e.slot].edit(e, getattr(e, 'f_abs', None)), dtype=np.int32) for e in edits]
+
+    def set_planes(self, records):
+        for p in records:
+            self.m[p.slot].set_planes(p)
 
     def drop_victim(self, slots, want=False):
         for s in slots:
@@ -267,12 +346,13 @@ class BatchPlayer:
         """ba: the handle's BundleAdjustor; bw (instead of ba): any object with BatchWindows' interface (ModelWindows).
         `model` (a ModelWindows) follows every edit and drop: the window a gather of the map would pack."""
         from pvio_b200 import _lib
-        from pvio_b200.batch_window import BatchWindows, Edit
-        self.Edit = Edit
+        from pvio_b200.batch_window import BatchWindows, Edit, Planes
+        self.Edit, self.Planes = Edit, Planes
         self.runs, self.bw = runs, (BatchWindows(ba) if bw is None else bw)
         self.model = bw if isinstance(bw, ModelWindows) else ModelWindows()
         self.slots = list(range(len(runs))) if slots is None else list(slots)
         self.ids = [dict() for _ in runs]                  # landmark -> live track id
+        self.roles = [dict() for _ in runs]                # landmark -> role of its live track
         self.k = [0] * len(runs)
         self.rec = [_lib.PackedArgs(r.w, r.guess).keep["imu"].reshape(-1, 288) for r in runs]
         for j, r in enumerate(runs):
@@ -286,6 +366,7 @@ class BatchPlayer:
             w0, _, _ = Chain(r).window(0)                   # first window: the 1e15 gauge prior
             x0 = np.concatenate([w0.prior_q0, w0.prior_p0, w0.prior_v0, w0.prior_bg0, w0.prior_ba0], axis=1)
             self.bw.set_prior(self.slots[j], w0.prior_S, w0.prior_e, x0)
+        self.set_roles(list(range(len(runs))))
 
     def state16(self, j, f):
         g = self.runs[j].guess
@@ -303,7 +384,7 @@ class BatchPlayer:
                 if l in self.ids[j]:
                     e.obs.append((self.ids[j][l], f_win, z))
                 else:
-                    e.new.append((f_win, z, r.guess.rho[l]))
+                    e.new.append((f_win, z, r.rho0[l]))
                     e.landmarks.append(l)
         return e
 
@@ -314,6 +395,27 @@ class BatchPlayer:
         for e, j, ids in zip(edits, js, got):
             for l, i in zip(e.landmarks, ids):
                 self.ids[j][l] = int(i)
+                self.roles[j][l] = -1
+
+    def set_roles(self, js):
+        """the roles of keyframe self.k[j] (Run.role) and the plane parameters of the runs js with planes, in one
+        set_planes: a changed role per live track, and a plane track that becomes a landmark with its new inverse depth"""
+        recs = []
+        for j in js:
+            r = self.runs[j]
+            if r.w.n_planes == 0:
+                continue
+            k, p = self.k[j], self.Planes(self.slots[j], r.planes_at(self.k[j]))
+            for l, i in sorted(self.ids[j].items(), key=lambda t: t[1]):
+                old, new = self.roles[j].get(l, -1), r.role(l, k)
+                if new != old:
+                    p.role(i, new, r.revalidated_rho(l) if old >= 0 and new == -1 else np.nan)
+                    self.roles[j][l] = new
+            recs.append(p)
+        if recs:
+            self.bw.set_planes(recs)
+            if self.model is not self.bw:
+                self.model.set_planes(recs)
 
     def refresh(self, js, track_stride):
         """download the slots of runs js; forget the landmarks whose tracks died"""
@@ -334,6 +436,7 @@ class BatchPlayer:
             self.k[j] += 1
         if not nonkey:
             self._apply([self.frame_edit(j, self.k[j] + self.runs[j].N - 1, self.runs[j].N - 1) for j in js], js)
+            self.set_roles(js)
             return
         fake = []
         for j in js:
@@ -347,3 +450,4 @@ class BatchPlayer:
                 del self.ids[j][l]
         real = [self.frame_edit(j, self.k[j] + self.runs[j].N - 1, self.runs[j].N - 1, replace_last=True) for j in js]
         self._apply(real, js)
+        self.set_roles(js)
