@@ -45,6 +45,29 @@ static void copy_slot(DevBuf<T> &dst, size_t i, const DevBuf<T> &src, size_t j) 
     memcpy(dst.slot(i), src.slot(j), sizeof(T) * std::min(dst.per, src.per));
 }
 
+// f(t.table...) for each table of the plane-table sets t (ensure_planes pairs the grown tables with the old ones)
+template <typename F, typename... P>
+static void for_each_plane_table(F f, P &...t) {
+    f(t.plane_param...); f(t.pt_plane...); f(t.pt_begin...); f(t.pt_frame...); f(t.pt_z...);
+}
+
+// Every per-slot array the host stages in pinned memory and copies to the device slot by slot: f(array, prior) for the
+// vision arrays, then the inertial arrays and the prior (prior: its S, e and x0) when allocated, then the plane tables
+// when allocated.  Stops at the first f that returns non-zero and returns that code.  A new per-slot array needs its
+// alloc and one entry here.
+template <typename F>
+static int for_each_staged(Handle *h, F f) {
+    int rc = 0;
+    auto v = [&](auto &b, bool prior) { if (rc == 0) rc = f(b, prior); };
+    v(h->hdr, false); v(h->cst, false); v(h->obs, false); v(h->lms, false); v(h->rho, false); v(h->frames, false);
+    if (h->have_inertial) {
+        v(h->imu_idx, false); v(h->imu_data, false); v(h->prior_frames, false);
+        v(h->prior_S, true); v(h->prior_e, true); v(h->prior_x0, true);
+    }
+    if (h->have_planes) for_each_plane_table([&](auto &b) { v(b, false); }, h->planes);
+    return rc;
+}
+
 // The handle's arrays as the kernels see them (BatchArrays).  Called after every (re)allocation, which also drops the
 // cached graphs: their launches carry the old view.
 static void refresh_arrays(Handle *h) {
@@ -60,8 +83,9 @@ static void refresh_arrays(Handle *h) {
     a.acc = h->acc.d; a.aux_cost = h->aux_cost.d;
     a.imu_idx = h->imu_idx.d; a.imu_data = h->imu_data.d; a.prior_frames = h->prior_frames.d; a.prior_S = h->prior_S.d;
     a.prior_L = h->prior_L.d; a.prior_e = h->prior_e.d; a.prior_x0 = h->prior_x0.d;
-    a.plane_param = h->plane_param.d; a.pt_plane = h->pt_plane.d; a.pt_begin = h->pt_begin.d; a.pt_frame = h->pt_frame.d;
-    a.pt_z = h->pt_z.d; a.pt_J = h->pt_J.d;
+    const PlaneTables &p = h->planes;
+    a.plane_param = p.plane_param.d; a.pt_plane = p.pt_plane.d; a.pt_begin = p.pt_begin.d; a.pt_frame = p.pt_frame.d;
+    a.pt_z = p.pt_z.d; a.pt_J = h->pt_J.d;
     a.Ncap = h->Ncap; a.Mcap = h->Mcap; a.Kcap = h->Kcap; a.Pcap = h->Pcap; a.Tcap = h->Tcap; a.Ocap = h->Ocap;
     a.bufs = lin_bufs(h);
 }
@@ -105,23 +129,22 @@ int ensure_planes(Handle *h, int T, int O) {
     cudaStreamSynchronize(h->stream);
     drop_graphs(h);
     const size_t P4 = (size_t)h->Pcap * 4;
-    DevBuf<double> pp; DevBuf<int32_t> tp, tb, tf; DevBuf<float> tz;
-    TRY(alloc(h, pp, W * P4, kBoth, P4));
-    TRY(alloc(h, tp, W * Tn, kBoth, Tn));
-    TRY(alloc(h, tb, W * (Tn + 1), kBoth, Tn + 1));
-    TRY(alloc(h, tf, W * On, kBoth, On));
-    TRY(alloc(h, tz, W * On * 2, kBoth, On * 2));
+    PlaneTables next;
+    TRY(alloc(h, next.plane_param, W * P4, kBoth, P4));
+    TRY(alloc(h, next.pt_plane, W * Tn, kBoth, Tn));
+    TRY(alloc(h, next.pt_begin, W * (Tn + 1), kBoth, Tn + 1));
+    TRY(alloc(h, next.pt_frame, W * On, kBoth, On));
+    TRY(alloc(h, next.pt_z, W * On * 2, kBoth, On * 2));
     if (h->have_planes) {
-        for (size_t i = 0; i < W; ++i) {
-            copy_slot(pp, i, h->plane_param, i); copy_slot(tp, i, h->pt_plane, i); copy_slot(tb, i, h->pt_begin, i);
-            copy_slot(tf, i, h->pt_frame, i); copy_slot(tz, i, h->pt_z, i);
-        }
-        TRY(copy_slots_d2d(h, pp, h->plane_param)); TRY(copy_slots_d2d(h, tp, h->pt_plane));
-        TRY(copy_slots_d2d(h, tb, h->pt_begin)); TRY(copy_slots_d2d(h, tf, h->pt_frame)); TRY(copy_slots_d2d(h, tz, h->pt_z));
+        int rc = 0;
+        for_each_plane_table([&](auto &dst, auto &src) {
+            for (size_t i = 0; i < W; ++i) copy_slot(dst, i, src, i);
+            if (rc == 0) rc = copy_slots_d2d(h, dst, src);
+        }, next, h->planes);
+        TRY(rc);
         CK(h, cudaStreamSynchronize(h->stream));      // the old arrays are freed below
     }
-    h->plane_param = std::move(pp); h->pt_plane = std::move(tp); h->pt_begin = std::move(tb); h->pt_frame = std::move(tf);
-    h->pt_z = std::move(tz);
+    h->planes = std::move(next);
     TRY(alloc(h, h->pt_J, W * Tn * (6 * (size_t)h->Ncap + 2), kDevice));      // device scratch of solve_kernel's plane block
     h->Tcap = Tn; h->Ocap = On;
     h->have_planes = true;
@@ -205,6 +228,16 @@ __global__ void postpass_kernel(const WinHdr *hdr, const WinConst *cst, const Ob
 }
 
 // ------------------------------------------------------------------------ packing
+WinConst win_const(const pvio_b200_window *w) {
+    WinConst C;
+    memset(&C, 0, sizeof(C));
+    memcpy(C.cam_q, w->cam_q_cs, 32); memcpy(C.cam_p, w->cam_p_cs, 24);
+    memcpy(C.imu_q, w->imu_q_cs, 32); memcpy(C.imu_p, w->imu_p_cs, 24);
+    memcpy(C.sic, w->sqrt_inv_cov, 32);
+    C.fx = w->fx; C.fy = w->fy; C.cauchy_a = w->cauchy_a > 0 ? w->cauchy_a : 1.0; C.plane_sic = w->plane_sqrt_inv_cov;
+    return C;
+}
+
 static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvio_b200_state *s) {
     const int N = w->n_frames, M = w->n_landmarks, K = w->n_obs;
     if (slot < 0 || slot >= h->W) return fail(h, PVIO_B200_EINVAL, "slot out of range");
@@ -234,7 +267,8 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     }
     // prior_S == NULL names the prior the marginaliser left in this slot's device arrays (pvio_b200_batch_marginalize,
     // pvio_b200_window_drop_victim); checked before anything of the slot is overwritten
-    if (n_prior > 0 && !w->prior_S && h->prior_resident[slot] != n_prior)
+    WinSlot &ws = h->slots[slot];
+    if (n_prior > 0 && !w->prior_S && ws.prior_resident != n_prior)
         return fail(h, PVIO_B200_EINVAL, "prior_S == NULL: no device-resident prior of that size in this slot");
     if (w->n_plane_tracks < 0 || w->n_planes < 0 || w->n_planes > h->Pcap) return fail(h, PVIO_B200_EINVAL, "too many planes");
     if (w->n_plane_tracks > 0) {
@@ -250,16 +284,14 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
             if (w->pt_obs_frame[i] < 0 || w->pt_obs_frame[i] >= N) return fail(h, PVIO_B200_EINVAL, "pt_obs_frame out of range");
     }
     if (n_imu > 0 || n_prior > 0 || inertial) TRY(ensure_inertial(h));
-    if (slot < (int)h->bw.slot.size()) h->bw.slot[slot].on = false;     // a packed slot is no longer a resident window
+    ws.resident = false;                  // a packed slot is no longer a resident window
+    ws.perm.clear();                      // until the landmark order below is known
     WinHdr &H = h->hdr.h[slot];
     WinConst &C = h->cst.h[slot];
     memset(&H, 0, sizeof(H));
     H.N = N; H.M = M; H.K = K; H.use_inertial = inertial ? 1 : 0;
     for (int f = 0; f < N; ++f) if (w->frame_fixed && w->frame_fixed[f]) H.fixed_mask |= 1 << f;
-    memcpy(C.cam_q, w->cam_q_cs, 32); memcpy(C.cam_p, w->cam_p_cs, 24);
-    memcpy(C.imu_q, w->imu_q_cs, 32); memcpy(C.imu_p, w->imu_p_cs, 24);
-    memcpy(C.sic, w->sqrt_inv_cov, 32);
-    C.fx = w->fx; C.fy = w->fy; C.cauchy_a = w->cauchy_a > 0 ? w->cauchy_a : 1.0; C.plane_sic = w->plane_sqrt_inv_cov;
+    C = win_const(w);
     // frames + origin (mean frame position keeps |x_l| ~ depth in the fp32 Jacobian arithmetic)
     double *fr = h->frames.slot(slot);
     memcpy(fr, s->frames, sizeof(double) * N * kFrameStride);
@@ -267,22 +299,24 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     for (int f = 0; f < N; ++f) for (int k = 0; k < 3; ++k) o[k] += fr[f * kFrameStride + 4 + k];
     for (int k = 0; k < 3; ++k) C.origin[k] = o[k] / N;
     // landmarks sorted by anchor (the reference's first-visit order already is, bundle_adjustor.cpp:92-103)
-    std::vector<int32_t> &perm = h->perm[slot];
-    perm.resize(M);
-    std::iota(perm.begin(), perm.end(), 0);
+    std::vector<int32_t> perm;
     bool sorted = true;
     for (int l = 0; l < M; ++l) {
         const int a = w->lm_anchor[l];
         if (a < 0 || a >= N) return fail(h, PVIO_B200_EINVAL, "landmark with bad anchor");
         if (l > 0 && a < w->lm_anchor[l - 1]) sorted = false;
     }
-    if (!sorted) std::stable_sort(perm.begin(), perm.end(), [&](int a, int b) { return w->lm_anchor[a] < w->lm_anchor[b]; });
+    if (!sorted) {
+        perm.resize(M);
+        std::iota(perm.begin(), perm.end(), 0);
+        std::stable_sort(perm.begin(), perm.end(), [&](int a, int b) { return w->lm_anchor[a] < w->lm_anchor[b]; });
+    }
     ObsRec *ob = h->obs.slot(slot);
     LmRec *lm = h->lms.slot(slot);
     double *rh = h->rho.slot(slot);
     int k_out = 0, nch = 0;
     for (int lp = 0; lp < M; ++lp) {
-        const int l = perm[lp];
+        const int l = sorted ? lp : perm[lp];
         const int a = w->lm_anchor[l];
         const int b0 = w->lm_obs_begin[l], b1 = w->lm_obs_begin[l + 1];
         const int n = b1 - b0;
@@ -319,8 +353,7 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     }
     H.n_chunks = nch;
     H.K = k_out;
-    h->slot_M[slot] = M; h->slot_N[slot] = N; h->slot_K[slot] = k_out;
-    h->perm_identity[slot] = sorted ? 1 : 0;
+    ws.perm = std::move(perm);
     // inertial part
     H.n_imu = n_imu;
     H.n_prior = n_prior;
@@ -331,7 +364,7 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
         const size_t d = 15 * (size_t)n_prior;
         for (int n = 0; n < n_prior; ++n) h->prior_frames.slot(slot)[n] = w->prior_frames[n];
         if (d > 0 && w->prior_S) {          // a host prior replaces a device-resident one
-            h->prior_resident[slot] = 0;
+            ws.prior_resident = 0;
             memcpy(h->prior_S.slot(slot), w->prior_S, sizeof(double) * d * d);   // dense d x d, row-major
             memcpy(h->prior_e.slot(slot), w->prior_e, sizeof(double) * d);
             memcpy(h->prior_x0.slot(slot), w->prior_state0, sizeof(double) * n_prior * kFrameStride);
@@ -342,11 +375,12 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     if (H.n_ptracks > 0) {
         const int O = w->pt_obs_begin[H.n_ptracks];
         TRY(ensure_planes(h, H.n_ptracks, O));
-        memcpy(h->plane_param.slot(slot), w->plane_param, sizeof(double) * 4 * H.n_planes);
-        memcpy(h->pt_plane.slot(slot), w->pt_plane, sizeof(int32_t) * H.n_ptracks);
-        memcpy(h->pt_begin.slot(slot), w->pt_obs_begin, sizeof(int32_t) * (H.n_ptracks + 1));
-        memcpy(h->pt_frame.slot(slot), w->pt_obs_frame, sizeof(int32_t) * O);
-        float *z = h->pt_z.slot(slot);
+        PlaneTables &p = h->planes;
+        memcpy(p.plane_param.slot(slot), w->plane_param, sizeof(double) * 4 * H.n_planes);
+        memcpy(p.pt_plane.slot(slot), w->pt_plane, sizeof(int32_t) * H.n_ptracks);
+        memcpy(p.pt_begin.slot(slot), w->pt_obs_begin, sizeof(int32_t) * (H.n_ptracks + 1));
+        memcpy(p.pt_frame.slot(slot), w->pt_obs_frame, sizeof(int32_t) * O);
+        float *z = p.pt_z.slot(slot);
         for (int i = 0; i < 2 * O; ++i) z[i] = (float)w->pt_obs_z[i];
     }
     return 0;
@@ -364,38 +398,24 @@ static int h2d(Handle *h, DevBuf<T> &b, int w0, int n, cudaStream_t st) {
 // across the iterations of a solve: the frame-major table and Lambda = S^T S of the priors.
 static int upload_range(Handle *h, int w0, int n, cudaStream_t st) {
     if (n < 1 || w0 < 0 || w0 + n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window range");
-    TRY(h2d(h, h->hdr, w0, n, st));
-    TRY(h2d(h, h->cst, w0, n, st));
-    TRY(h2d(h, h->obs, w0, n, st));
-    TRY(h2d(h, h->lms, w0, n, st));
-    TRY(h2d(h, h->rho, w0, n, st));
-    TRY(h2d(h, h->frames, w0, n, st));
-    bool any_prior = false;
-    if (h->have_inertial) {
-        TRY(h2d(h, h->imu_idx, w0, n, st));
-        TRY(h2d(h, h->imu_data, w0, n, st));
-        TRY(h2d(h, h->prior_frames, w0, n, st));
+    TRY(for_each_staged(h, [&](auto &b, bool prior) {
+        if (!prior) return h2d(h, b, w0, n, st);
         for (int i = w0; i < w0 + n;) {      // a device-resident prior is never re-uploaded: copy the runs of the other slots
-            if (h->prior_resident[i]) { ++i; continue; }
+            if (h->slots[i].prior_resident) { ++i; continue; }
             int j = i;
-            while (j < w0 + n && !h->prior_resident[j]) ++j;
-            TRY(h2d(h, h->prior_S, i, j - i, st));
-            TRY(h2d(h, h->prior_e, i, j - i, st));
-            TRY(h2d(h, h->prior_x0, i, j - i, st));
+            while (j < w0 + n && !h->slots[j].prior_resident) ++j;
+            TRY(h2d(h, b, i, j - i, st));
             i = j;
         }
+        return 0;
+    }));
+    bool any_prior = false;
+    if (h->have_inertial) {
         for (int i = w0; i < w0 + n; ++i) any_prior |= h->hdr.h[i].n_prior > 0;
         if (any_prior) {
             prior_lambda_kernel<<<dim3(n, n < 64 ? 32 : 1), 256, 0, st>>>(h->hdr.d, h->prior_S.d, h->prior_L.d, h->Ncap, w0, nullptr);
             ++h->launches;
         }
-    }
-    if (h->have_planes) {
-        TRY(h2d(h, h->plane_param, w0, n, st));
-        TRY(h2d(h, h->pt_plane, w0, n, st));
-        TRY(h2d(h, h->pt_begin, w0, n, st));
-        TRY(h2d(h, h->pt_frame, w0, n, st));
-        TRY(h2d(h, h->pt_z, w0, n, st));
     }
     FobsArgs fa = launch_args<FobsArgs>(h);
     fa.w0 = w0;
@@ -806,16 +826,23 @@ int launch_layout_tail(Handle *h, const int32_t *slots, int n, bool prior) {
     return 0;
 }
 
+// per-landmark values of the packed window in slot i -> the caller's landmark order
+template <typename T>
+static void unpermute(const Handle *h, int i, T *dst, const T *src) {
+    const std::vector<int32_t> &perm = h->slots[i].perm;
+    const int M = h->hdr.h[i].M;
+    if (perm.empty()) memcpy(dst, src, sizeof(T) * M);
+    else for (int lp = 0; lp < M; ++lp) dst[perm[lp]] = src[lp];
+}
+
 // pinned staging -> caller arrays (landmark order un-permuted), windows [w0, w0 + n)
 static int scatter_dx(Handle *h, int w0, int n, double *dx, int64_t dx_stride, double *costs) {
     for (int i = w0; i < w0 + n; ++i) {
-        const int N = h->slot_N[i], M = h->slot_M[i];
         if (dx) {
+            const int N = h->hdr.h[i].N;
             double *o = dx + (size_t)i * dx_stride;
             memcpy(o, h->dx_pose.slot(i), sizeof(double) * N * 15);
-            const double *dl = h->dx_lm.slot(i);
-            if (h->perm_identity[i]) memcpy(o + N * 15, dl, sizeof(double) * M);
-            else { const std::vector<int32_t> &perm = h->perm[i]; for (int lp = 0; lp < M; ++lp) o[N * 15 + perm[lp]] = dl[lp]; }
+            unpermute(h, i, o + N * 15, h->dx_lm.slot(i));
         }
         if (costs) { costs[2 * i] = h->ctrl.h[i].cost; costs[2 * i + 1] = h->ctrl.h[i].cand_cost; }
         if (h->ctrl.h[i].solve_failed) return fail(h, PVIO_B200_ENUMERIC, "reduced system not positive definite");
@@ -851,21 +878,15 @@ static int download_state_async(Handle *h, int w0, int n, cudaStream_t st) {
     return d2h(h, h->ctrl, h->ctrl, w0, n, st);
 }
 
-static void fill_summary(const WinCtrl &c, pvio_b200_summary *sm) {
+void fill_summary(const WinCtrl &c, pvio_b200_summary *sm) {
     memset(sm, 0, sizeof(*sm));
     sm->iterations = c.iteration; sm->accepted_steps = c.accepted; sm->termination = c.termination; sm->usable = c.usable;
     sm->initial_cost = c.initial_cost; sm->final_cost = c.cost; sm->final_radius = c.radius; sm->final_mu = c.mu;
 }
 
 static void scatter_state(Handle *h, int i, double *frames, double *inv_depth) {
-    const int N = h->slot_N[i], M = h->slot_M[i];
-    if (frames) memcpy(frames, h->frames_out.slot(i), sizeof(double) * N * kFrameStride);
-    if (inv_depth) {
-        const double *r = h->rho_out.slot(i);
-        const std::vector<int32_t> &perm = h->perm[i];
-        if (h->perm_identity[i]) memcpy(inv_depth, r, sizeof(double) * M);
-        else for (int lp = 0; lp < M; ++lp) inv_depth[perm[lp]] = r[lp];
-    }
+    if (frames) memcpy(frames, h->frames_out.slot(i), sizeof(double) * h->hdr.h[i].N * kFrameStride);
+    if (inv_depth) unpermute(h, i, inv_depth, h->rho_out.slot(i));
 }
 
 // pinned landing area -> caller arrays of windows [w0, w0 + n): states (landmark order un-permuted) and summaries
@@ -911,6 +932,14 @@ static int ensure_pipeline_streams(Handle *h, int nsub) {
     return 0;
 }
 
+// The entry points that take packed windows (what: the one called) refuse a range [0, n) that holds a resident window.
+static int check_packed(Handle *h, int n, const char *what) {
+    for (int i = 0; i < std::min(n, h->W); ++i)
+        if (h->slots[i].resident)
+            return fail(h, PVIO_B200_EINVAL, (std::string(what) + ": the range holds a resident window (pvio_b200_batch_window_*)").c_str());
+    return 0;
+}
+
 // Upload, work and download of windows [0, n) with HOST buffers.  Below 1024 windows: one upload, the work and one
 // download on the handle's stream.  Large batches are cut into sub-batches and pipelined: sub-batch i is uploaded on
 // the copy stream, worked on compute stream i % kPipeStreams (a sub-batch is at most one wave of CTAs, so alone it runs
@@ -922,9 +951,9 @@ static int ensure_pipeline_streams(Handle *h, int nsub) {
 //   download(w0, m, st) enqueues their device -> host copies into the pinned staging on st
 //   scatter(w0, m)      hands the landed results to the caller
 template <typename Work, typename Download, typename Scatter>
-static int run_host_pipeline(Handle *h, int n, Work work, Download download, Scatter scatter) {
+static int run_host_pipeline(Handle *h, int n, const char *what, Work work, Download download, Scatter scatter) {
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
-    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "upload: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, what));
     const std::vector<int> sizes = sub_batches(n);
     const int nsub = (int)sizes.size();
     if (nsub == 1) {
@@ -1015,8 +1044,7 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
     TRY(alloc(h, h->acc, W * kAcc, kBoth)); TRY(alloc(h, h->aux_cost, W, kDevice));
     TRY(alloc(h, h->Hfull, (15 * N) * (15 * N), kBoth)); TRY(alloc(h, h->gfull, 15 * N, kBoth));
     refresh_arrays(h);
-    h->perm.resize(W); h->perm_identity.assign(W, 1); h->slot_M.assign(W, 0); h->slot_N.assign(W, 0); h->slot_K.assign(W, 0);
-    h->prior_resident.assign(W, 0);
+    h->slots.resize(W);
     {   // opt in to large dynamic shared memory ONCE per kernel with the device limit: the attribute is process-wide, so a
         // per-handle value would be overwritten by the next handle with other capacities
         const int lim = (int)prop.sharedMemPerBlockOptin - 2048;
@@ -1130,16 +1158,13 @@ int pvio_b200_batch_replicate(pvio_b200_handle hh, int n) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
-    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_replicate: the range holds a resident window (pvio_b200_batch_window_*)");
-    if (h->prior_resident[0] && h->hdr.h[0].n_prior > 0)
+    TRY(check_packed(h, n, "batch_replicate"));
+    if (h->slots[0].prior_resident && h->hdr.h[0].n_prior > 0)
         return fail(h, PVIO_B200_EINVAL, "batch_replicate: slot 0's prior is device-resident, its staging does not hold it");
     for (int i = 1; i < n; ++i) {
-        auto rep = [&](auto &b) { copy_slot(b, i, b, 0); };
-        h->prior_resident[i] = 0;          // the slot takes slot 0's host prior from the staging
-        rep(h->hdr); rep(h->cst); rep(h->obs); rep(h->lms); rep(h->rho); rep(h->frames);
-        h->perm[i] = h->perm[0]; h->perm_identity[i] = h->perm_identity[0]; h->slot_M[i] = h->slot_M[0]; h->slot_N[i] = h->slot_N[0]; h->slot_K[i] = h->slot_K[0];
-        if (h->have_inertial) { rep(h->imu_idx); rep(h->imu_data); rep(h->prior_frames); rep(h->prior_S); rep(h->prior_e); rep(h->prior_x0); }
-        if (h->have_planes) { rep(h->plane_param); rep(h->pt_plane); rep(h->pt_begin); rep(h->pt_frame); rep(h->pt_z); }
+        h->slots[i].prior_resident = 0;          // the slot takes slot 0's host prior from the staging
+        h->slots[i].perm = h->slots[0].perm;
+        for_each_staged(h, [&](auto &b, bool) { copy_slot(b, i, b, 0); return 0; });
     }
     return 0;
 }
@@ -1147,7 +1172,7 @@ int pvio_b200_batch_replicate(pvio_b200_handle hh, int n) {
 int pvio_b200_batch_upload(pvio_b200_handle hh, int n) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_upload: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, "batch_upload"));
     return upload(h, n);
 }
 
@@ -1155,7 +1180,7 @@ int pvio_b200_batch_gn_step(pvio_b200_handle hh, int n, double mu, int apply) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->n_uploaded) return fail(h, PVIO_B200_EINVAL, "windows not uploaded");
-    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_gn_step: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, "batch_gn_step"));
     StepCfg c;
     c.mu = mu; c.apply = apply; c.compute_scale = 1;
     return run_gn_step(h, n, c, batch_shape(h, 0, n, false));
@@ -1164,7 +1189,7 @@ int pvio_b200_batch_gn_step(pvio_b200_handle hh, int n, double mu, int apply) {
 int pvio_b200_batch_download(pvio_b200_handle hh, int n, double *dx, int64_t dx_stride, double *costs) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_download: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, "batch_download"));
     return download_dx(h, n, dx, dx_stride, costs);
 }
 
@@ -1172,7 +1197,7 @@ int pvio_b200_batch_download(pvio_b200_handle hh, int n, double *dx, int64_t dx_
 int pvio_b200_batch_gn_step_host(pvio_b200_handle hh, int n, double mu, double *dx, int64_t dx_stride, double *costs) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    return run_host_pipeline(h, n,
+    return run_host_pipeline(h, n, "batch_gn_step_host",
         [&](int w0, int m, cudaStream_t st) {
             StepCfg c;
             c.mu = mu; c.apply = 0; c.compute_scale = 1; c.w0 = w0; c.stream = st;
@@ -1188,7 +1213,7 @@ int pvio_b200_batch_solve(pvio_b200_handle hh, int n, const pvio_b200_options *o
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->n_uploaded) return fail(h, PVIO_B200_EINVAL, "windows not uploaded");
-    if (any_resident(h, 0, n)) return fail(h, PVIO_B200_EINVAL, "batch_solve: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, "batch_solve"));
     return run_solve_loop(h, solve_options(opt), 0, n, h->stream);
 }
 
@@ -1197,8 +1222,7 @@ int pvio_b200_batch_download_state(pvio_b200_handle hh, int n, double *frames, i
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     if (n < 1 || n > h->W) return fail(h, PVIO_B200_EINVAL, "bad window count");
-    if (any_resident(h, 0, n))
-        return fail(h, PVIO_B200_EINVAL, "batch_download_state: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, "batch_download_state"));
     TRY(download_state_async(h, 0, n, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     scatter_states(h, 0, n, frames, frames_stride, inv_depth, inv_depth_stride, summaries);
@@ -1212,7 +1236,7 @@ int pvio_b200_batch_solve_host(pvio_b200_handle hh, int n, const pvio_b200_optio
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     const SolveOptions o = solve_options(opt);
-    return run_host_pipeline(h, n,
+    return run_host_pipeline(h, n, "batch_solve_host",
         [&](int w0, int m, cudaStream_t st) { return run_solve_loop(h, o, w0, m, st ? st : h->stream); },
         [&](int w0, int m, cudaStream_t st) { return download_state_async(h, w0, m, st); },
         [&](int w0, int m) {
@@ -1271,13 +1295,8 @@ int pvio_b200_ba_solve(pvio_b200_handle hh, const pvio_b200_window *w, pvio_b200
     TRY(download_state_async(h, 0, 1, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     scatter_state(h, 0, s->frames, s->inv_depth);
-    if (post) {
-        const std::vector<int32_t> &perm = h->perm[0];
-        for (int lp = 0; lp < M; ++lp) {
-            if (valid) valid[perm[lp]] = h->valid.h[lp];
-            if (quality) quality[perm[lp]] = h->quality.h[lp];
-        }
-    }
+    if (post && valid) unpermute(h, 0, valid, h->valid.h);
+    if (post && quality) unpermute(h, 0, quality, h->quality.h);
     if (summary) {
         fill_summary(h->ctrl.h[0], summary);
         float ms = 0.f;
@@ -1310,8 +1329,7 @@ int pvio_b200_ba_marginalize(pvio_b200_handle hh, const pvio_b200_window *w, con
 int pvio_b200_batch_marginalize(pvio_b200_handle hh, int n, double *S_out, int64_t S_stride, double *e_out, int64_t e_stride) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    if (n >= 1 && n <= h->W && any_resident(h, 0, n))
-        return fail(h, PVIO_B200_EINVAL, "batch_marginalize: the range holds a resident window (pvio_b200_batch_window_*)");
+    TRY(check_packed(h, n, "batch_marginalize"));
     return batch_marginalize_impl(h, n, S_out, S_stride, e_out, e_stride);
 }
 

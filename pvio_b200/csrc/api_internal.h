@@ -121,33 +121,44 @@ struct FmState {
     DevBuf<unsigned> h_mask;                  // pinned: its inlier mask
 };
 
-// batch_window.cu: the resident windows of the batched slots; slot 0 is also the window of pvio_b200_window_*.  Per slot
-// the host keeps integers only: the frame count, the prior's frame count, the fixed mask, the plane count, and for every
-// live track (rows in id order) its id, frame mask and role; the device keeps the track table (frame mask, role, inverse
-// depth, fp64 keypoint per window frame, post-pass flags), the plane parameters and the packed window.
+// The host record of one window slot.  Its frame and landmark counts are those of the slot's host header (Handle::hdr).
+// A slot holds either a window packed from the caller's arrays (api.cu: pack_window) or a resident window
+// (batch_window.cu; slot 0 is also the window of pvio_b200_window_*).  Of a resident window the host keeps integers only:
+// the frame count, the prior's frame count, the fixed mask, the plane count, and for every live track (rows in id order)
+// its id, frame mask and role; the device keeps the track table (frame mask, role, inverse depth, fp64 keypoint per
+// window frame, post-pass flags), the plane parameters and the packed window.
 // Role of a row: -1 a landmark; -2 a landmark that stays out of the marginaliser's victim set (a plane track of a plane
 // with fewer than 20 tracks); p >= 0 a plane track of plane p: one plane-distance factor over all its observations.
-struct BwSlot {
-    bool on = false;                  // resident: the slot changes through pvio_b200_batch_window_* (and window_*) only
+struct WinSlot {
+    bool resident = false;            // the slot changes through pvio_b200_batch_window_* (and window_*) only
     int N = 0, n_prior = 0, fixed = 0, inertial = 0, n_planes = 0;
     int32_t next_id = 0;
     std::vector<int32_t> ids;         // live tracks, increasing: row r of the device table holds track ids[r]
     std::vector<uint32_t> mask;       // frame mask of each row
     std::vector<int8_t> role;         // role of each row
+    std::vector<int32_t> perm;        // packed landmark -> caller landmark; empty: the identity (always, when resident)
+    int prior_resident = 0;           // frame count of the prior (S, e, x0) the marginaliser wrote on the device (0: none);
+                                      // a pack naming it with prior_S == NULL keeps it, a host prior clears it
 };
 struct BatchWindows {
-    std::vector<BwSlot> slot;                    // [W]
     DevBuf<int32_t> tid;                         // [W][Mcap] track id of each row
     DevBuf<uint32_t> tmask;                      // [W][Mcap] frames observing it (0: free row)
     DevBuf<double> trho;                         // [W][Mcap] inverse depth in its anchor (lowest) frame
     DevBuf<double2> tz;                          // [W][Mcap][Ncap] fp64 keypoint per window frame
     DevBuf<uint8_t> tvalid;                      // [W][Mcap] post-pass result of the last solve
     DevBuf<double> tqual;                        // [W][Mcap]
-    DevBuf<int8_t> trole;                        // [W][Mcap] role of each row (BwSlot::role)
+    DevBuf<int8_t> trole;                        // [W][Mcap] role of each row (WinSlot::role)
     DevBuf<double> tplane;                       // [W][Pcap][4] plane parameters (normal, distance)
     DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
-    DevBuf<uint8_t> named;                       // [W] device: 1 for the slots a solve names
     DevBuf<uint8_t> stage;                       // both sides, grown: the one upload / download of a call
+};
+
+// the plane tables of the solve (api.cu: for_each_staged), allocated with the first window that has plane tracks and
+// grown by ensure_planes
+struct PlaneTables {
+    DevBuf<double> plane_param;
+    DevBuf<int32_t> pt_plane, pt_begin, pt_frame;
+    DevBuf<float> pt_z;
 };
 
 struct Handle {
@@ -164,8 +175,7 @@ struct Handle {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::string err;
     int64_t launches = 0;
-    std::vector<int> prior_resident;              // per slot: frame count of the prior (S, e, x0) the marginaliser wrote on the
-                                                  // device (0: none); a pack naming it with prior_S == NULL keeps it, a host prior clears it
+    std::vector<WinSlot> slots;                   // [W]
     DetectState detect;                           // detect.cu
     DetectBatchState detectb;                     // detect.cu: the batched detector, independent of detect
     size_t sys_set = 0;                           // elements between the two buffer sets of the reduced-system arrays (LinBufs)
@@ -203,14 +213,8 @@ struct Handle {
     DevBuf<int32_t> imu_idx, prior_frames;
     DevBuf<double> imu_data, prior_S, prior_L, prior_e, prior_x0;
     bool have_planes = false;
-    DevBuf<double> plane_param;
-    DevBuf<int32_t> pt_plane, pt_begin, pt_frame;
-    DevBuf<float> pt_z;
+    PlaneTables planes;
     DevBuf<double> pt_J;                          // [W][Tcap][6 Ncap + 2] scratch of the plane block of solve_kernel
-    // host bookkeeping per slot
-    std::vector<std::vector<int32_t>> perm;      // packed landmark -> caller landmark
-    std::vector<int> slot_M, slot_N, slot_K;
-    std::vector<uint8_t> perm_identity;
     int n_uploaded = 0;
     // ring of event triples around the linearise + Schur launches (roofline timing without host syncs)
     std::vector<cudaEvent_t> kev;
@@ -231,13 +235,6 @@ struct Handle {
                                                   // points, IMU records, frames) seen
     BatchWindows bw;                              // batch_window.cu (empty until the first pvio_b200_batch_window_reset)
 };
-
-// whether any of the slots [w0, w0 + n) holds a resident window (batch_window.cu)
-inline bool any_resident(const Handle *h, int w0, int n) {
-    for (int i = std::max(w0, 0); i < w0 + n && i < (int)h->bw.slot.size(); ++i)
-        if (h->bw.slot[i].on) return true;
-    return false;
-}
 
 int fail(Handle *h, int code, const char *what, cudaError_t e = cudaSuccess);
 
@@ -307,6 +304,10 @@ int reserve(Handle *h, DevBuf<T> &b, size_t n, int sides) {
 
 // api.cu: pack window into slot 0, copy it to the device, build the frame-major table
 int pack_and_upload(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s);
+// api.cu: the constants of window w as the kernels read them, origin 0
+WinConst win_const(const pvio_b200_window *w);
+// api.cu: the summary of a solve from its window's WinCtrl (solve_seconds 0)
+void fill_summary(const WinCtrl &c, pvio_b200_summary *sm);
 // api.cu: linearise + Schur of the uploaded windows [0, n) with the fp64 pipeline, no loss (the marginaliser's reprojection part)
 // h_slots / d_slots (may be NULL): host / device copies of a list of the n windows, instead of [0, n)
 int run_marg_vision(Handle *h, int n, const int32_t *h_slots = nullptr, const int32_t *d_slots = nullptr);

@@ -564,7 +564,7 @@ int batch_marginalize_impl(Handle *h, int n, double *S_out, int64_t S_stride, do
     }
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    for (int i = 0; i < n; ++i) h->prior_resident[i] = h->hdr.h[i].N - 1;
+    for (int i = 0; i < n; ++i) h->slots[i].prior_resident = h->hdr.h[i].N - 1;
     return 0;
 }
 

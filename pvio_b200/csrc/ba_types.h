@@ -112,10 +112,10 @@ struct __align__(16) LmAux {
 // handle keeps one copy, rebuilt whenever an array is reallocated; each kernel's argument struct derives from it and adds
 // only its per-launch fields.  Arrays of [W] windows; "2x": two buffer sets, set 1 at the LinBufs offset.
 struct BatchArrays {
-    const WinHdr *hdr;              // [W]
-    const WinConst *cst;            // [W]
-    const ObsRec *obs;              // [W][Kcap] landmark-major table as the shim gathers it
-    const LmRec *lms;               // [W][Mcap]
+    WinHdr *hdr;                    // [W]
+    WinConst *cst;                  // [W]
+    ObsRec *obs;                    // [W][Kcap] landmark-major table as the shim gathers it
+    LmRec *lms;                     // [W][Mcap]
     double *rho;                    // [W][Mcap] state (overwritten by the candidate on acceptance)
     double *frames;                 // [W][Ncap][16] state
     WinCtrl *ctrl;                  // [W]
@@ -151,19 +151,19 @@ struct BatchArrays {
     double *pose_scale;             // [W][15 Ncap]
     double *aux_cost;               // [W] non-vision (IMU + prior + plane) cost of the candidate
     // IMU and prior: allocated with the first window that has motion states
-    const int32_t *imu_idx;         // [W][Ncap][2] (frame_i, frame_j)
-    const double *imu_data;         // [W][Ncap][kImuStride]
-    const int32_t *prior_frames;    // [W][Ncap]
+    int32_t *imu_idx;               // [W][Ncap][2] (frame_i, frame_j)
+    double *imu_data;               // [W][Ncap][kImuStride]
+    int32_t *prior_frames;          // [W][Ncap]
     const double *prior_S;          // [W][dcap * dcap], dcap = 15 Ncap
     const double *prior_L;          // [W][dcap * dcap] Lambda = S^T S
     const double *prior_e;          // [W][dcap]
     const double *prior_x0;         // [W][Ncap][16]
     // planes: allocated with the first window that has plane tracks
-    const double *plane_param;      // [W][Pcap][4]
-    const int32_t *pt_plane;        // [W][Tcap]
-    const int32_t *pt_begin;        // [W][Tcap + 1]
-    const int32_t *pt_frame;        // [W][Ocap]
-    const float *pt_z;              // [W][Ocap][2] (observations are stored fp32 like the reprojection table)
+    double *plane_param;            // [W][Pcap][4]
+    int32_t *pt_plane;              // [W][Tcap]
+    int32_t *pt_begin;              // [W][Tcap + 1]
+    int32_t *pt_frame;              // [W][Ocap]
+    float *pt_z;                    // [W][Ocap][2] (observations are stored fp32 like the reprojection table)
     double *pt_J;                   // [W][Tcap][6 Ncap + 2] scratch: corrected Jacobian rows of the plane tracks
 };
 

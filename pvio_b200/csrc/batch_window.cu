@@ -12,7 +12,7 @@
 // live row), enough to check every call completely before anything is staged, and to know the launch shapes.  The rows
 // of a slot's table are its live tracks in id order: removals compact the table (the storage of dead tracks is reused),
 // new tracks append.
-// Plane factors (bundle_adjustor.cpp:162-196): the role of a row (BwSlot) decides what it is in the solve.  Rows of
+// Plane factors (bundle_adjustor.cpp:162-196): the role of a row (WinSlot) decides what it is in the solve.  Rows of
 // role < 0 with >= 2 observations are the landmarks (role -2 ones stay out of the marginaliser's victim set,
 // bundle_adjustor.cpp:456-457); rows of role p >= 0 are the plane tracks of plane p, packed in row (= id) order with all
 // their observations, anchor included, into the plane tables the solve kernels read (pt_plane, pt_begin, pt_frame,
@@ -41,13 +41,8 @@ struct BwDl { int32_t slot, N, T, pad; int64_t off; };                  // downl
 struct BwPlanes { int32_t slot, n_planes, n_set, set_off, param_off, pad; };   // one set_planes record (n_planes < 0: keep)
 struct BwRole { int32_t row, role; double rho; };                       // rho NaN: keep the row's inverse depth
 
-struct BwArgs {
-    WinHdr *hdr;
-    WinConst *cst;
-    LmRec *lms;
-    ObsRec *obs;
-    double *rho, *frames, *imu_data;
-    int32_t *imu_idx, *prior_frames;
+// the handle's arrays (the plane tables null until a slot has plane tracks), the track table and the post-pass results
+struct BwArgs : BatchArrays {
     int32_t *tid;
     uint32_t *tmask;
     double *trho;
@@ -59,10 +54,6 @@ struct BwArgs {
     int32_t *lm_row;
     const uint8_t *valid;
     const double *quality;
-    double *plane_param;                  // the plane tables of the solve (null until a slot has plane tracks)
-    int32_t *pt_plane, *pt_begin, *pt_frame;
-    float *pt_z;
-    int Ncap, Mcap, Kcap, Pcap, Tcap, Ocap;
 };
 
 constexpr int kBwThreads = 256;
@@ -426,29 +417,24 @@ __global__ void __launch_bounds__(kBwThreads) bw_download_kernel(BwArgs a, const
 }
 
 // ------------------------------------------------------------------------ host side
-static BwArgs bw_args(Handle *h) {
+template <>
+BwArgs launch_args<BwArgs>(const Handle *h) {
+    const BatchWindows &b = h->bw;
     BwArgs a{};
-    BatchWindows &b = h->bw;
-    a.hdr = h->hdr.d; a.cst = h->cst.d; a.lms = h->lms.d; a.obs = h->obs.d; a.rho = h->rho.d; a.frames = h->frames.d;
-    a.imu_data = h->imu_data.d; a.imu_idx = h->imu_idx.d; a.prior_frames = h->prior_frames.d;
+    static_cast<BatchArrays &>(a) = h->arrays;
     a.tid = b.tid.d; a.tmask = b.tmask.d; a.trho = b.trho.d; a.tz = b.tz.d; a.tvalid = b.tvalid.d; a.tqual = b.tqual.d;
-    a.trole = b.trole.d; a.tplane = b.tplane.d;
-    a.lm_row = b.lm_row.d; a.valid = h->valid.d; a.quality = h->quality.d;
-    a.plane_param = h->plane_param.d; a.pt_plane = h->pt_plane.d; a.pt_begin = h->pt_begin.d; a.pt_frame = h->pt_frame.d;
-    a.pt_z = h->pt_z.d;
-    a.Ncap = h->Ncap; a.Mcap = h->Mcap; a.Kcap = h->Kcap; a.Pcap = h->Pcap; a.Tcap = h->Tcap; a.Ocap = h->Ocap;
+    a.trole = b.trole.d; a.tplane = b.tplane.d; a.lm_row = b.lm_row.d; a.valid = h->valid.d; a.quality = h->quality.d;
     return a;
 }
 
 static int ensure_bw(Handle *h) {
     BatchWindows &b = h->bw;
-    if (!b.slot.empty()) return 0;
+    if (b.lm_row.n) return 0;                 // allocated last: every table is there
     const size_t W = h->W, M = h->Mcap;
     TRY(alloc(h, b.tid, W * M, kDevice)); TRY(alloc(h, b.tmask, W * M, kDevice)); TRY(alloc(h, b.trho, W * M, kDevice));
     TRY(alloc(h, b.tz, W * M * h->Ncap, kDevice)); TRY(alloc(h, b.tvalid, W * M, kDevice)); TRY(alloc(h, b.tqual, W * M, kDevice));
     TRY(alloc(h, b.trole, W * M, kDevice)); TRY(alloc(h, b.tplane, W * h->Pcap * 4, kDevice));
-    TRY(alloc(h, b.lm_row, W * M, kDevice)); TRY(alloc(h, b.named, W, kDevice));
-    b.slot.resize(W);
+    TRY(alloc(h, b.lm_row, W * M, kDevice));
     return 0;
 }
 
@@ -466,7 +452,7 @@ struct Packer {
 
 // the window of a slot as the checks and the launch shapes see it; T / O: plane tracks and their observations
 struct BwShape { int M = 0, K = 0, chunks = 0, max_obs = 0, T = 0, O = 0; };
-static BwShape shape_of(const BwSlot &s) {
+static BwShape shape_of(const WinSlot &s) {
     BwShape r;
     int cnt[kMaxFrames] = {};
     for (size_t i = 0; i < s.mask.size(); ++i) {
@@ -480,7 +466,7 @@ static BwShape shape_of(const BwSlot &s) {
     return r;
 }
 
-static int check_window(Handle *h, const BwSlot &s) {
+static int check_window(Handle *h, const WinSlot &s) {
     const BwShape sh = shape_of(s);
     if (s.N > h->Ncap) return fail(h, PVIO_B200_EINVAL, "batch_window: more frames than max_frames");
     if ((int)s.ids.size() > h->Mcap) return fail(h, PVIO_B200_EINVAL, "batch_window: more live tracks than max_landmarks");
@@ -493,26 +479,24 @@ static int check_window(Handle *h, const BwSlot &s) {
 // the shape fields of the slot's host header (batch_shape and the marginaliser read them); the device header is the
 // re-layout kernel's
 static void host_header(Handle *h, int slot) {
-    const BwSlot &s = h->bw.slot[slot];
+    const WinSlot &s = h->slots[slot];
     const BwShape sh = shape_of(s);
     WinHdr &H = h->hdr.h[slot];
     memset(&H, 0, sizeof(H));
     H.N = s.N; H.M = sh.M; H.K = sh.K; H.use_inertial = s.inertial; H.n_imu = s.inertial ? std::max(s.N - 1, 0) : 0;
     H.n_prior = s.inertial ? s.n_prior : 0; H.fixed_mask = s.fixed; H.n_chunks = sh.chunks;
     H.n_planes = s.n_planes; H.n_ptracks = sh.T;            // batch_shape: plane tracks take the full solve kernel
-    h->slot_N[slot] = s.N; h->slot_M[slot] = sh.M; h->slot_K[slot] = sh.K;
-    h->perm[slot].clear(); h->perm_identity[slot] = 1;      // no caller landmark order: nothing of a former pack survives
 }
 
-static BwLayout layout_from(int slot, const BwSlot &s) {
+static BwLayout layout_from(int slot, const WinSlot &s) {
     return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial, s.n_planes, 0};
 }
-static BwLayout layout_of(const Handle *h, int slot) { return layout_from(slot, h->bw.slot[slot]); }
+static BwLayout layout_of(const Handle *h, int slot) { return layout_from(slot, h->slots[slot]); }
 
 // plane-table capacity for the windows the n slots of a call will hold, before anything of the call is staged
-static int ensure_plane_tables(Handle *h, const std::vector<BwSlot> &next) {
+static int ensure_plane_tables(Handle *h, const std::vector<WinSlot> &next) {
     int T = 0, O = 0;
-    for (const BwSlot &s : next) { const BwShape sh = shape_of(s); T = std::max(T, sh.T); O = std::max(O, sh.O); }
+    for (const WinSlot &s : next) { const BwShape sh = shape_of(s); T = std::max(T, sh.T); O = std::max(O, sh.O); }
     return T > 0 ? ensure_planes(h, T, O) : 0;
 }
 
@@ -521,7 +505,7 @@ static int check_slots(Handle *h, int n, const int32_t *slots, const char *what)
     std::vector<uint8_t> seen(h->W, 0);
     for (int i = 0; i < n; ++i) {
         const int s = slots[i];
-        if (s < 0 || s >= h->W || h->bw.slot.empty() || !h->bw.slot[s].on)
+        if (s < 0 || s >= h->W || !h->slots[s].resident)
             return fail(h, PVIO_B200_EINVAL, "batch_window: slot out of range or not resident");
         if (seen[s]) return fail(h, PVIO_B200_EINVAL, "batch_window: a slot named twice");
         seen[s] = 1;
@@ -545,13 +529,13 @@ static int upload_stage(Handle *h, const Packer &p, size_t out_bytes, uint8_t *&
 // re-layout of the slots whose BwLayout records start at byte `off` of the upload (list of int32 slots at slots_off)
 static int relayout(Handle *h, uint8_t *d_in, size_t lay_off, size_t slots_off, int n, bool prior) {
     if (n == 0) return 0;
-    bw_layout_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(d_in + lay_off));
+    bw_layout_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwLayout *>(d_in + lay_off));
     ++h->launches;
     CK(h, cudaGetLastError());
     return launch_layout_tail(h, reinterpret_cast<const int32_t *>(d_in + slots_off), n, prior);
 }
 
-static int find_row(const BwSlot &s, int32_t id) {
+static int find_row(const WinSlot &s, int32_t id) {
     const auto it = std::lower_bound(s.ids.begin(), s.ids.end(), id);
     return (it == s.ids.end() || *it != id) ? -1 : (int)(it - s.ids.begin());
 }
@@ -566,7 +550,7 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
     // else of it); the post-pass and the write-back run over the named list only
     int range = 0;
     for (int i = 0; i < n; ++i) {
-        if (h->bw.slot[slots[i]].N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_solve: a window without frames");
+        if (h->slots[slots[i]].N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_solve: a window without frames");
         range = std::max(range, slots[i] + 1);
     }
     std::vector<uint8_t> named(range, 0);
@@ -580,33 +564,28 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
     TRY(run_named_solve(h, opt, range, din + o_nm));
     CK(h, cudaEventRecord(h->ev1, h->stream));
     if (post) TRY(run_postpass_slots(h, n, reinterpret_cast<const int32_t *>(din + o_sl)));
-    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(din + o_lay), post ? 1 : 0);
+    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwLayout *>(din + o_lay), post ? 1 : 0);
     ++h->launches;
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(h->ctrl.h, h->ctrl.d, sizeof(WinCtrl) * range, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-    for (int i = 0; i < n; ++i) {
-        const WinCtrl &c = h->ctrl.h[slots[i]];
-        if (summaries) {
-            pvio_b200_summary &sm = summaries[i];
-            memset(&sm, 0, sizeof(sm));
-            sm.iterations = c.iteration; sm.accepted_steps = c.accepted; sm.termination = c.termination; sm.usable = c.usable;
-            sm.initial_cost = c.initial_cost; sm.final_cost = c.cost; sm.final_radius = c.radius; sm.final_mu = c.mu;
-            sm.solve_seconds = ms * 1e-3;
+    if (summaries)
+        for (int i = 0; i < n; ++i) {
+            fill_summary(h->ctrl.h[slots[i]], &summaries[i]);
+            summaries[i].solve_seconds = ms * 1e-3;
         }
-    }
     return 0;
 }
 
 // slot 0 as the single resident window (pvio_b200_window_*); null, with the error set, before pvio_b200_window_reset
-static const BwSlot *window0(Handle *h) {
-    if (h->bw.slot.empty() || !h->bw.slot[0].on) {
+static const WinSlot *window0(Handle *h) {
+    if (!h->slots[0].resident) {
         fail(h, PVIO_B200_EINVAL, "window: no resident window: call pvio_b200_window_reset first");
         return nullptr;
     }
-    return &h->bw.slot[0];
+    return &h->slots[0];
 }
 
 }  // namespace pvio
@@ -622,17 +601,12 @@ int pvio_b200_batch_window_reset(pvio_b200_handle hh, int slot, const pvio_b200_
     if (w->n_planes > 0 || w->n_plane_tracks > 0) return fail(h, PVIO_B200_EINVAL, "batch_window_reset: resident windows carry no planes");
     TRY(ensure_bw(h));
     if (w->use_inertial) TRY(ensure_inertial(h));
-    BwSlot &s = h->bw.slot[slot];
-    s = BwSlot();
-    s.on = true; s.inertial = w->use_inertial ? 1 : 0;
-    h->prior_resident[slot] = 0;
+    WinSlot &s = h->slots[slot];
+    s = WinSlot();                            // nothing of a former pack or resident window survives
+    s.resident = true; s.inertial = w->use_inertial ? 1 : 0;
     host_header(h, slot);
     WinConst &C = h->cst.h[slot];
-    memset(&C, 0, sizeof(C));
-    memcpy(C.cam_q, w->cam_q_cs, 32); memcpy(C.cam_p, w->cam_p_cs, 24);
-    memcpy(C.imu_q, w->imu_q_cs, 32); memcpy(C.imu_p, w->imu_p_cs, 24);
-    memcpy(C.sic, w->sqrt_inv_cov, 32);
-    C.fx = w->fx; C.fy = w->fy; C.cauchy_a = w->cauchy_a > 0 ? w->cauchy_a : 1.0; C.plane_sic = w->plane_sqrt_inv_cov;
+    C = win_const(w);
     CK(h, cudaMemcpyAsync(h->cst.dslot(slot), &C, sizeof(WinConst), cudaMemcpyHostToDevice, h->stream));
     Packer p;
     const BwLayout L = layout_of(h, slot);
@@ -649,7 +623,7 @@ int pvio_b200_batch_window_set_prior(pvio_b200_handle hh, int slot, int n_prior,
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     TRY(check_slots(h, 1, &slot, "batch_window_set_prior: bad slot"));
-    BwSlot &s = h->bw.slot[slot];
+    WinSlot &s = h->slots[slot];
     if (n_prior < 0 || (n_prior > 0 && (!S || !e || !state0))) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: null prior");
     if (!s.inertial && n_prior > 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: the window carries no motion states");
     if (n_prior > s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: prior over more frames than the window holds");
@@ -663,8 +637,7 @@ int pvio_b200_batch_window_set_prior(pvio_b200_handle hh, int slot, int n_prior,
         CK(h, cudaMemcpyAsync(h->prior_x0.dslot(slot), h->prior_x0.slot(slot), sizeof(double) * n_prior * kFrameStride,
                               cudaMemcpyHostToDevice, h->stream));
     }
-    s.n_prior = n_prior;
-    h->prior_resident[slot] = n_prior;
+    s.n_prior = s.prior_resident = n_prior;
     host_header(h, slot);
     Packer p;
     const BwLayout L = layout_of(h, slot);
@@ -685,7 +658,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
     for (int i = 0; i < n; ++i) slots[i] = edits[i].slot;
     TRY(check_slots(h, n, slots.data(), "batch_window_edit: bad slot list"));
     // every edit is applied to a copy of its slot's host mirror; nothing is staged before all of them passed
-    std::vector<BwSlot> next(n);
+    std::vector<WinSlot> next(n);
     std::vector<BwEdit> recs(n);
     std::vector<int32_t> rm;
     std::vector<BwNew> nws;
@@ -694,7 +667,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
     int out_ints = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_window_edit &E = edits[i];
-        BwSlot s = h->bw.slot[E.slot];
+        WinSlot s = h->slots[E.slot];
         BwEdit &R = recs[i];
         R = BwEdit{};
         R.slot = E.slot; R.N_old = s.N; R.T_old = (int)s.ids.size(); R.frame = -1;
@@ -775,7 +748,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
     const size_t o_x = p.put(xs.data(), xs.size());
     uint8_t *din, *dout;
     TRY(upload_stage(h, p, sizeof(int32_t) * out_ints, din, dout));
-    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwEdit *>(din + o_ed),
+    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwEdit *>(din + o_ed),
         reinterpret_cast<const int32_t *>(din + o_rm), reinterpret_cast<const BwNew *>(din + o_nw),
         reinterpret_cast<const BwObs *>(din + o_ob), reinterpret_cast<const double *>(din + o_x), reinterpret_cast<int32_t *>(dout));
     ++h->launches;
@@ -786,12 +759,12 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
     CK(h, cudaStreamSynchronize(h->stream));
     const int32_t *res = reinterpret_cast<const int32_t *>(h->bw.stage.h + in);
     for (int i = 0; i < n; ++i) {
-        h->bw.slot[slots[i]] = std::move(next[i]);
+        h->slots[slots[i]] = std::move(next[i]);
         host_header(h, slots[i]);
     }
     for (int i = 0; i < n; ++i) {
         const int32_t *r = res + recs[i].out_off;
-        if (r[0] != (int32_t)h->bw.slot[slots[i]].ids.size())
+        if (r[0] != (int32_t)h->slots[slots[i]].ids.size())
             return fail(h, PVIO_B200_ECUDA, "batch_window_edit: the device track table disagrees with the host's");
         if (edits[i].new_ids) memcpy(edits[i].new_ids, r + 1, sizeof(int32_t) * edits[i].n_new_tracks);
     }
@@ -807,13 +780,13 @@ int pvio_b200_batch_window_set_planes(pvio_b200_handle hh, int n, const pvio_b20
     for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
     TRY(check_slots(h, n, slots.data(), "batch_window_set_planes: bad slot list"));
     // every record is applied to a copy of its slot's host mirror; nothing is staged before all of them passed
-    std::vector<BwSlot> next(n);
+    std::vector<WinSlot> next(n);
     std::vector<BwPlanes> recs(n);
     std::vector<BwRole> roles;
     std::vector<double> params;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_window_planes &R = records[i];
-        BwSlot s = h->bw.slot[R.slot];
+        WinSlot s = h->slots[R.slot];
         if (R.n_planes < -1 || R.n_planes > h->Pcap) return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: plane count outside -1 (keep) .. 4");
         if (R.n_set < 0 || (R.n_set > 0 && (!R.track || !R.role)) || (R.n_planes > 0 && !R.plane_param))
             return fail(h, PVIO_B200_EINVAL, "batch_window_set_planes: null array");
@@ -850,14 +823,14 @@ int pvio_b200_batch_window_set_planes(pvio_b200_handle hh, int n, const pvio_b20
     const size_t o_ro = p.put(roles.data(), roles.size()), o_pa = p.put(params.data(), params.size());
     uint8_t *din, *dout;
     TRY(upload_stage(h, p, 0, din, dout));
-    bw_planes_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwPlanes *>(din + o_rec),
+    bw_planes_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwPlanes *>(din + o_rec),
         reinterpret_cast<const BwRole *>(din + o_ro), reinterpret_cast<const double *>(din + o_pa));
     ++h->launches;
     CK(h, cudaGetLastError());
     TRY(relayout(h, din, o_lay, o_sl, n, false));
     CK(h, cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n; ++i) {
-        h->bw.slot[slots[i]] = std::move(next[i]);
+        h->slots[slots[i]] = std::move(next[i]);
         host_header(h, slots[i]);
     }
     return 0;
@@ -876,9 +849,9 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
     if (!h) return PVIO_B200_EINVAL;
     TRY(check_slots(h, n, slots, "batch_window_drop_victim: bad slot list"));
     if (n == 0) return 0;
-    std::vector<BwSlot> next(n);
+    std::vector<WinSlot> next(n);
     for (int i = 0; i < n; ++i) {
-        BwSlot s = h->bw.slot[slots[i]];
+        WinSlot s = h->slots[slots[i]];
         if (!s.inertial) return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: the window must carry motion states");
         if (s.N < 2) return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: a window needs at least two frames");
         const int dk = 15 * (s.N - 1);
@@ -892,7 +865,7 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
             if (m) { s.ids[o] = s.ids[r]; s.mask[o] = m; s.role[o] = s.role[r]; ++o; }
         }
         s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
-        --s.N; s.fixed >>= 1; s.n_prior = s.N;
+        --s.N; s.fixed >>= 1; s.n_prior = s.prior_resident = s.N;
         TRY(check_window(h, s));
         next[i] = std::move(s);
     }
@@ -907,18 +880,17 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
     TRY(upload_stage(h, p, 0, din, dout));
     TRY(run_marg(h, n, 0, true, true, slots, reinterpret_cast<const int32_t *>(din + o_sl)));
     for (int i = 0; i < n; ++i) {
-        const size_t dk = 15 * (size_t)(h->bw.slot[slots[i]].N - 1);
+        const size_t dk = 15 * (size_t)(h->slots[slots[i]].N - 1);
         if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.dslot(slots[i]), sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
         if (e_out) CK(h, cudaMemcpyAsync(e_out + i * e_stride, h->prior_e.dslot(slots[i]), sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
     }
-    bw_drop_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwLayout *>(din + o_b));
+    bw_drop_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwLayout *>(din + o_b));
     ++h->launches;
     CK(h, cudaGetLastError());
     TRY(relayout(h, din, o_a, o_sl, n, true));
     CK(h, cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n; ++i) {
-        h->bw.slot[slots[i]] = std::move(next[i]);
-        h->prior_resident[slots[i]] = h->bw.slot[slots[i]].n_prior;
+        h->slots[slots[i]] = std::move(next[i]);
         host_header(h, slots[i]);
     }
     return 0;
@@ -935,7 +907,7 @@ int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *s
     std::vector<BwDl> dls(n);
     int64_t off = 0;
     for (int i = 0; i < n; ++i) {
-        const BwSlot &s = h->bw.slot[slots[i]];
+        const WinSlot &s = h->slots[slots[i]];
         const int T = (int)s.ids.size();
         if (frames && frames_stride < (int64_t)s.N * kFrameStride) return fail(h, PVIO_B200_EINVAL, "batch_window_download: frames_stride too small");
         if ((track_id || inv_depth || anchor_frame || n_observations || valid || quality) && track_stride < T)
@@ -947,7 +919,7 @@ int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *s
     const size_t o_dl = p.put(dls.data(), n);
     uint8_t *din, *dout;
     TRY(upload_stage(h, p, (size_t)off, din, dout));
-    bw_download_kernel<<<n, kBwThreads, 0, h->stream>>>(bw_args(h), reinterpret_cast<const BwDl *>(din + o_dl), dout);
+    bw_download_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwDl *>(din + o_dl), dout);
     ++h->launches;
     CK(h, cudaGetLastError());
     const size_t in = dout - din;
@@ -1007,7 +979,7 @@ int pvio_b200_window_add_observations(pvio_b200_handle hh, int n, const int32_t 
 int pvio_b200_window_remove_track(pvio_b200_handle hh, int32_t track) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    const BwSlot *s = window0(h);
+    const WinSlot *s = window0(h);
     if (!s) return PVIO_B200_EINVAL;
     if (track < 0 || track >= s->next_id) return fail(h, PVIO_B200_EINVAL, "window_remove_track: unknown track");
     if (find_row(*s, track) < 0) return 0;    // already gone
@@ -1032,7 +1004,7 @@ int pvio_b200_window_get(pvio_b200_handle hh, int32_t *n_frames, double *frames,
                          double *inv_depth, int32_t *anchor_frame, int32_t *n_observations) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
-    const BwSlot *s = window0(h);
+    const WinSlot *s = window0(h);
     if (!s) return PVIO_B200_EINVAL;
     if (n_tracks > 0 && !tracks) return fail(h, PVIO_B200_EINVAL, "window_get: null track list");
     for (int i = 0; i < n_tracks; ++i)
