@@ -508,9 +508,10 @@ static int sweep_grid_x(Handle *h, int n) { return n * 2 < h->sm_count ? 16 : 1;
 // slower per step, 3 for either is within the run-to-run spread; the results do not depend on them.  The update sweep at
 // 8 CTAs / SM (64 registers) takes 0.352 ms per step, at 6 (80 registers) 0.361 ms (H100 SXM, 700 W power limit).
 constexpr int kLinWarps = 4, kLinBlocks = 4;
-// the linearise sweep may drop to 3 CTAs / SM for its fp64 shared-memory sums (lin_part_fits); 3 CTAs / SM alone was
-// measured within the run-to-run spread (above)
-constexpr int kLinPartMinBlocks = 3;
+// the linearise sweep may drop to 3 CTAs / SM for its fp64 shared-memory sums (lin_part_fits; 72 KB at cfg2, where 4 do
+// not fit).  That instantiation is compiled for the 3 CTAs it gets (168 registers instead of 128) and spends the room on
+// two rows in flight per lane (kLinPartRows); the one without the shared sums keeps one row at 4 CTAs / SM
+constexpr int kLinPartMinBlocks = 3, kLinPartRows = 2;
 constexpr int kSchurThreads = 128, kSchurBlocks = 4;
 constexpr int kUpdWarps = 4, kUpdBlocks = 8;
 
@@ -543,9 +544,10 @@ static __global__ void zero_system_kernel(PipeArgs a_in, int npairs_cap) {
 // Whether a linearise CTA that owns its window keeps the per-landmark (j.j, j.r) sums in shared memory (PipeArgs::lm_part)
 // at this shape: only when the larger layout fits and leaves at least min(kLinPartMinBlocks, the CTAs / SM without it)
 // resident (occupancy API: registers and shared memory), so that e.g. a large max_landmarks falls back to the jr records
-// instead of failing or losing more occupancy.
+// instead of failing or losing more occupancy.  k_part / k_plain: the instantiations launched with and without the
+// shared sums (the same kernel in fp64), each asked about with its own layout.
 template <typename real>
-static bool lin_part_fits(Handle *h, const void *kernel, int N, int Mp) {
+static bool lin_part_fits(Handle *h, const void *k_part, const void *k_plain, int N, int Mp) {
     const auto key = std::make_tuple((int)sizeof(real), N, Mp);
     auto it = h->lin_part.find(key);
     if (it != h->lin_part.end()) return it->second;
@@ -553,8 +555,8 @@ static bool lin_part_fits(Handle *h, const void *kernel, int N, int Mp) {
     int nb_with = 0, nb_without = 0;
     bool ok = false;
     if ((int)with <= h->smem_lim) {
-        const cudaError_t e1 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_with, kernel, kLinWarps * 32, with);
-        const cudaError_t e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_without, kernel, kLinWarps * 32, without);
+        const cudaError_t e1 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_with, k_part, kLinWarps * 32, with);
+        const cudaError_t e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_without, k_plain, kLinWarps * 32, without);
         if (e1 != cudaSuccess || e2 != cudaSuccess) cudaGetLastError();      // a failed query only means: keep jr
         else ok = nb_with >= 1 && nb_with >= std::min(nb_without, kLinPartMinBlocks);
     }
@@ -578,14 +580,16 @@ static int launch_lin(Handle *h, int n, const StepCfg &c, const BatchShape &b, b
     const int Mp = (b.M + 31) & ~31;
     if (!h->hs_double) {
         if (!loss) return fail(h, PVIO_B200_EINVAL, "the loss-free sweep runs in fp64");
-        auto k = lin_obs_kernel<true, float, kLinWarps, kLinBlocks>;
-        a.lm_part = gx == 1 && lin_part_fits<float>(h, (const void *)k, b.N, Mp) ? 1 : 0;
+        auto k_part = lin_obs_kernel<true, float, kLinWarps, kLinPartMinBlocks, kLinPartRows>;
+        auto k_plain = lin_obs_kernel<true, float, kLinWarps, kLinBlocks>;
+        a.lm_part = gx == 1 && lin_part_fits<float>(h, (const void *)k_part, (const void *)k_plain, b.N, Mp) ? 1 : 0;
+        auto k = a.lm_part ? k_part : k_plain;
         k<<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<float>(b.N, Mp, kLinWarps, a.lm_part), st>>>(a);
         LAUNCH_CK(h, "lin_obs_kernel<float>");
         if (gx > 1) { lm_finish_kernel<float><<<dim3((b.M + 127) / 128, n), 128, 0, st>>>(a); ++h->launches; LAUNCH_CK(h, "lm_finish_kernel<float>"); }
     } else {
         auto k = loss ? lin_obs_kernel<true, double, kLinWarps, 2> : lin_obs_kernel<false, double, kLinWarps, 2>;
-        a.lm_part = gx == 1 && lin_part_fits<double>(h, (const void *)k, b.N, Mp) ? 1 : 0;
+        a.lm_part = gx == 1 && lin_part_fits<double>(h, (const void *)k, (const void *)k, b.N, Mp) ? 1 : 0;
         k<<<dim3(gx, n), kLinWarps * 32, lin_smem_bytes<double>(b.N, Mp, kLinWarps, a.lm_part), st>>>(a);
         LAUNCH_CK(h, "lin_obs_kernel<double>");
         if (gx > 1) { lm_finish_kernel<double><<<dim3((b.M + 127) / 128, n), 128, 0, st>>>(a); ++h->launches; LAUNCH_CK(h, "lm_finish_kernel<double>"); }
@@ -1050,6 +1054,8 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
         const int lim = (int)prop.sharedMemPerBlockOptin - 2048;
         h->smem_lim = lim;
         CK(h, cudaFuncSetAttribute(lin_obs_kernel<true, float, kLinWarps, kLinBlocks>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+        CK(h, cudaFuncSetAttribute(lin_obs_kernel<true, float, kLinWarps, kLinPartMinBlocks, kLinPartRows>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(lin_obs_kernel<true, double, kLinWarps, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(lin_obs_kernel<false, double, kLinWarps, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(schur_kernel<float, kSchurThreads, kSchurBlocks>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));

@@ -293,6 +293,7 @@ __device__ __constant__ signed char kQSlot[32] = {0, 1, 2, 3, 4, 5, -1, 6, 7, 8,
 __device__ __forceinline__ int spair(int t, int a) { return t * (t - 1) / 2 + a; }
 
 constexpr int kRing = 4;                        // rows of the frame-major table in flight per warp (cp.async ring)
+constexpr int kLmBatch = 4;                     // landmarks per thread whose records lin_obs_kernel loads together
 
 // Walks the rows of a warp: row r lies in segment sp = (t, an), its first table entry is k0()
 struct RowCursor {
@@ -343,15 +344,16 @@ __device__ __forceinline__ void row_prefetch(RowCursor &pf, int r_end, const flo
 // (the Schur tiles then need no per-block predicate).
 // part: the per-warp partial sums [nwarps][Mp] of the CTA's shared memory (lin_obs_kernel with lm_part), each a sum
 // in frame order; summed here in warp order, which is again frame order.  nullptr: the per-block pairs in jr.
+// lr_pre: the landmark's record, already loaded by the caller (nullptr: loaded here).
 template <typename real>
 __device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N, int M, unsigned fixed, double mu, int compute_scale,
-                                          const double2 *part = nullptr, int nwarps = 0, int Mp = 0) {
+                                          const double2 *part = nullptr, int nwarps = 0, int Mp = 0, const LmRec *lr_pre = nullptr) {
     typedef typename Vec2<real>::type real2;
     const LmRec *lms = a.lms + (size_t)w * a.Mcap;
     real2 *wv = reinterpret_cast<real2 *>(a.lm_w) + (size_t)w * a.Mcap;
     int32_t *msk = a.lm_msk + (size_t)w * a.Mcap;
     if (l >= M) { wv[l] = mk2((real)0, (real)0); msk[l] = 0; return; }      // padding up to the copy granule of the Schur kernel
-    const LmRec lr = lms[l];
+    const LmRec lr = lr_pre ? *lr_pre : lms[l];
     const int n_obs = lm_nobs(lr.meta), anchor = lm_anchor(lr.meta);
     const unsigned targets = lm_mask(lr.meta);
     const bool live = n_obs > 0 && !(a.victim_only && !lm_victim(lr.meta));
@@ -442,9 +444,12 @@ __host__ __device__ inline size_t lin_smem_bytes(int N, int Mp, int warps, bool 
     return lin_smem_layout<real>(N, Mp, warps, part, &a, &b, &c, &d, &e, &f);
 }
 
-template <bool kLoss, typename real, int kWarps, int kMinBlocks>
+// kRows: rows of a piece a lane linearises per iteration (1 or 2: two independent blocks in flight against the latency
+// of the fp64 -> cvt -> MUFU chains, at the price of registers); the results do not depend on it
+template <bool kLoss, typename real, int kWarps, int kMinBlocks, int kRows = 1>
 __global__ void __launch_bounds__(kWarps * 32, kMinBlocks)
 lin_obs_kernel(PipeArgs a_in) {
+    static_assert(kRows == 1 || kRows == 2, "one or two rows per iteration");
     typedef typename Vec2<real>::type real2;
     constexpr int kThreads = kWarps * 32;
     PipeArgs a = a_in;
@@ -474,6 +479,18 @@ lin_obs_kernel(PipeArgs a_in) {
     unsigned char *skip = smem_raw + o_skip;
     double2 *part = reinterpret_cast<double2 *>(smem_raw + o_part);         // [kWarps][Mp] when lpart
 
+    // The CTA's set-up is a chain of dependent loads at the latency of a loaded memory system, with at most three CTAs per
+    // SM to hide it; so the loads that depend only on w (segment table, frame states) are issued first, ahead of the L2
+    // read-ahead, and the per-landmark loads of phase 0 and of the epilogue go out kLmBatch at a time.
+    constexpr int kSegPer = (kSegTab + kThreads - 1) / kThreads;
+    int32_t sgv[kSegPer];
+#pragma unroll
+    for (int j = 0; j < kSegPer; ++j) {
+        const int i = tid + j * kThreads;
+        sgv[j] = i < kSegTab ? a.seg[(size_t)w * kSegTab + i] : 0;
+    }
+    FrameSm f;
+    if (tid < a.Ncap) make_frame(a.frames + ((size_t)w * a.Ncap + tid) * kFrameStride, wc, f);   // stored for tid < N
     if (gridDim.x == 1) {          // everything this CTA will read from HBM, requested before the first dependent load
         l2_prefetch(a.fz + (size_t)w * a.Kcap, sizeof(float2) * (size_t)H.K, tid, kThreads);
         l2_prefetch(a.flm + (size_t)w * a.Kcap, sizeof(FLm) * (size_t)H.K, tid, kThreads);
@@ -481,8 +498,6 @@ lin_obs_kernel(PipeArgs a_in) {
         l2_prefetch(a.rho + (size_t)w * a.Mcap, sizeof(double) * (size_t)M, tid, kThreads);
     }
     if (tid < N) {
-        FrameSm f;
-        make_frame(a.frames + ((size_t)w * a.Ncap + tid) * kFrameStride, wc, f);
 #pragma unroll
         for (int i = 0; i < 9; ++i) Fs[tid * 12 + i] = f.Rwc[i];
 #pragma unroll
@@ -491,23 +506,33 @@ lin_obs_kernel(PipeArgs a_in) {
         for (int i = 0; i < 9; ++i) Rs[tid * 12 + i] = (real)f.Rwc[i];
     }
     for (int i = tid; i < (nsp + 1 + N) * kDta + 8; i += kThreads) Dta[i] = 0.0;
-    for (int i = tid; i < kSegTab; i += kThreads) sg[i] = a.seg[(size_t)w * kSegTab + i];
+#pragma unroll
+    for (int j = 0; j < kSegPer; ++j) if (tid + j * kThreads < kSegTab) sg[tid + j * kThreads] = sgv[j];
     if (lpart) for (int i = tid; i < kWarps * Mp; i += kThreads) part[i] = make_double2(0.0, 0.0);
     __syncthreads();
 
     // ---- phase 0: world points (reprojection_error_cost.h:58-60)
     const LmRec *lms = a.lms + (size_t)w * a.Mcap;
     const double *rho = a.rho + (size_t)w * a.Mcap;
-    for (int l = tid; l < Mp; l += kThreads) {
-        unsigned char sk = 1;
-        double x0 = 0.0, x1 = 0.0, x2 = 1.0;
-        real c0 = 0, c1 = 0, c2 = 0;
-        if (l < M) {
-            const LmRec lr = lms[l];
-            if (lm_nobs(lr.meta) > 0 && !(a.victim_only && !lm_victim(lr.meta))) {
-                const double *Fa = Fs + lm_anchor(lr.meta) * 12;
-                const double ir = 1.0 / rho[l];
-                const double zx = (double)lr.zrx, zy = (double)lr.zry;
+    for (int l0 = tid; l0 < Mp; l0 += kLmBatch * kThreads) {
+        LmRec lr[kLmBatch] = {};
+        double rh[kLmBatch] = {};
+#pragma unroll
+        for (int j = 0; j < kLmBatch; ++j) {
+            const int l = l0 + j * kThreads;
+            if (l < M) { lr[j] = lms[l]; rh[j] = rho[l]; }
+        }
+#pragma unroll
+        for (int j = 0; j < kLmBatch; ++j) {
+            const int l = l0 + j * kThreads;
+            if (l >= Mp) break;
+            unsigned char sk = 1;
+            double x0 = 0.0, x1 = 0.0, x2 = 1.0;
+            real c0 = 0, c1 = 0, c2 = 0;
+            if (l < M && lm_nobs(lr[j].meta) > 0 && !(a.victim_only && !lm_victim(lr[j].meta))) {
+                const double *Fa = Fs + lm_anchor(lr[j].meta) * 12;
+                const double ir = 1.0 / rh[j];
+                const double zx = (double)lr[j].zrx, zy = (double)lr[j].zry;
                 const double v0 = (Fa[0] * zx + Fa[1] * zy + Fa[2]) * ir;
                 const double v1 = (Fa[3] * zx + Fa[4] * zy + Fa[5]) * ir;
                 const double v2 = (Fa[6] * zx + Fa[7] * zy + Fa[8]) * ir;
@@ -515,9 +540,9 @@ lin_obs_kernel(PipeArgs a_in) {
                 c0 = (real)ir;          // linearize_blk forms d r / d rho from 1 / rho and the segment's baseline
                 sk = 0;
             }
+            lm_sm_store(recs + (size_t)l * kLmSm, x0, x1, x2, c0, c1, c2);
+            skip[l] = sk;
         }
-        lm_sm_store(recs + (size_t)l * kLmSm, x0, x1, x2, c0, c1, c2);
-        skip[l] = sk;
     }
     __syncthreads();
 
@@ -575,7 +600,43 @@ lin_obs_kernel(PipeArgs a_in) {
             const int e = kQSlot[lane];
             if (e >= 0) atomicAdd(&Dta[sp * kDta + e], tot);          // +sum Y^T Y, Y^T r; the epilogue applies the signs
         };
-        // the table entry of the NEXT row is requested before the current row is evaluated
+        // what one linearised block of landmark l adds, in row order: the cost, (j.j, j.r), h_t, Y^T Y and Y^T r
+        auto emit = [&](const ObsL<real> &ol, int l) {
+            if (kLoss) la.add(ol.cost); else cost_acc += ol.cost;
+            const unsigned rec = tM + (unsigned)l;
+            const real2 jj = mk2(ol.j0 * ol.j0 + ol.j1 * ol.j1, ol.j0 * ol.r0 + ol.j1 * ol.r1);
+            if (lpart) {        // the warp's own partial; a row holds a landmark at most once: no two lanes collide
+                part_add(part_w + (unsigned)l * (unsigned)sizeof(double2), make_double2((double)jj.x, (double)jj.y));
+            } else {
+                jr[rec] = jj;
+            }
+            if (need) {
+                real2 h[3];
+#pragma unroll
+                for (int p = 0; p < 3; ++p) h[p] = bfma(ol.j1, ol.Y1[p], bmul(ol.j0, ol.Y0[p]));
+                real2 *dst = reinterpret_cast<real2 *>(hs) + (size_t)rec * 3;
+                dst[0] = h[0]; dst[1] = h[1]; dst[2] = h[2];
+                const real y0[6] = {ol.Y0[0].x, ol.Y0[0].y, ol.Y0[1].x, ol.Y0[1].y, ol.Y0[2].x, ol.Y0[2].y};
+                const real y1[6] = {ol.Y1[0].x, ol.Y1[0].y, ol.Y1[1].x, ol.Y1[1].y, ol.Y1[2].x, ol.Y1[2].y};
+                // upper triangle of Y^T Y by column pairs, then Y^T r
+                q[0] = bfma(y1[0], ol.Y1[0], bfma(y0[0], ol.Y0[0], q[0]));
+                q[1] = bfma(y1[0], ol.Y1[1], bfma(y0[0], ol.Y0[1], q[1]));
+                q[2] = bfma(y1[0], ol.Y1[2], bfma(y0[0], ol.Y0[2], q[2]));
+                q[3] = bfma(y1[1], ol.Y1[0], bfma(y0[1], ol.Y0[0], q[3]));
+                q[4] = bfma(y1[1], ol.Y1[1], bfma(y0[1], ol.Y0[1], q[4]));
+                q[5] = bfma(y1[1], ol.Y1[2], bfma(y0[1], ol.Y0[2], q[5]));
+                q[6] = bfma(y1[2], ol.Y1[1], bfma(y0[2], ol.Y0[1], q[6]));
+                q[7] = bfma(y1[2], ol.Y1[2], bfma(y0[2], ol.Y0[2], q[7]));
+                q[8] = bfma(y1[3], ol.Y1[1], bfma(y0[3], ol.Y0[1], q[8]));
+                q[9] = bfma(y1[3], ol.Y1[2], bfma(y0[3], ol.Y0[2], q[9]));
+                q[10] = bfma(y1[4], ol.Y1[2], bfma(y0[4], ol.Y0[2], q[10]));
+                q[11] = bfma(y1[5], ol.Y1[2], bfma(y0[5], ol.Y0[2], q[11]));
+                q[12] = bfma(ol.r1, ol.Y1[0], bfma(ol.r0, ol.Y0[0], q[12]));
+                q[13] = bfma(ol.r1, ol.Y1[1], bfma(ol.r0, ol.Y0[1], q[13]));
+                q[14] = bfma(ol.r1, ol.Y1[2], bfma(ol.r0, ol.Y0[2], q[14]));
+            }
+        };
+        // the table entries of the NEXT row (kRows = 2: the next two rows) are requested before the current ones are evaluated
         int k = cs.k0() + lane;
         const float2 *pz = fz + k;
         const FLm *pl = flm + k;
@@ -583,56 +644,56 @@ lin_obs_kernel(PipeArgs a_in) {
         int l_nx = 0;
         if (k < seg_end) { z_nx = *pz; l_nx = *pl; }
         const int nrow = r_stop - cs.r;
-        for (int i = 0; i < nrow; ++i) {
-            const float2 z = z_nx;
-            const int l = l_nx;
-            const bool valid = k < seg_end;
-            k += 32; pz += 32; pl += 32;
-            if (i + 1 < nrow && k < seg_end) { z_nx = *pz; l_nx = *pl; }
-            if (valid) {
-                if (!(vo && skip[l])) {
-                    ObsL<real> ol;
-                    double x[3];
-                    real xf[3], ir[3];             // ir = (1 / rho, 0, 0)
-                    lm_sm_load(recs_a + (unsigned)l * kLmSm, x, xf, ir);
-                    linearize_blk<kLoss, real>(F, x[0], x[1], x[2], xf[0], xf[1], xf[2], ir[0], bt, z.x, z.y, W,
-                                               diag_w, inv_cb, ol);
-                    if (kLoss) la.add(ol.cost); else cost_acc += ol.cost;
-                    const unsigned rec = tM + (unsigned)l;
-                    const real2 jj = mk2(ol.j0 * ol.j0 + ol.j1 * ol.j1, ol.j0 * ol.r0 + ol.j1 * ol.r1);
-                    if (lpart) {        // the warp's own partial; a row holds a landmark at most once: no two lanes collide
-                        part_add(part_w + (unsigned)l * (unsigned)sizeof(double2), make_double2((double)jj.x, (double)jj.y));
-                    } else {
-                        jr[rec] = jj;
-                    }
-                    if (need) {
-                        real2 h[3];
-#pragma unroll
-                        for (int p = 0; p < 3; ++p) h[p] = bfma(ol.j1, ol.Y1[p], bmul(ol.j0, ol.Y0[p]));
-                        real2 *dst = reinterpret_cast<real2 *>(hs) + (size_t)rec * 3;
-                        dst[0] = h[0]; dst[1] = h[1]; dst[2] = h[2];
-                        const real y0[6] = {ol.Y0[0].x, ol.Y0[0].y, ol.Y0[1].x, ol.Y0[1].y, ol.Y0[2].x, ol.Y0[2].y};
-                        const real y1[6] = {ol.Y1[0].x, ol.Y1[0].y, ol.Y1[1].x, ol.Y1[1].y, ol.Y1[2].x, ol.Y1[2].y};
-                        // upper triangle of Y^T Y by column pairs, then Y^T r
-                        q[0] = bfma(y1[0], ol.Y1[0], bfma(y0[0], ol.Y0[0], q[0]));
-                        q[1] = bfma(y1[0], ol.Y1[1], bfma(y0[0], ol.Y0[1], q[1]));
-                        q[2] = bfma(y1[0], ol.Y1[2], bfma(y0[0], ol.Y0[2], q[2]));
-                        q[3] = bfma(y1[1], ol.Y1[0], bfma(y0[1], ol.Y0[0], q[3]));
-                        q[4] = bfma(y1[1], ol.Y1[1], bfma(y0[1], ol.Y0[1], q[4]));
-                        q[5] = bfma(y1[1], ol.Y1[2], bfma(y0[1], ol.Y0[2], q[5]));
-                        q[6] = bfma(y1[2], ol.Y1[1], bfma(y0[2], ol.Y0[1], q[6]));
-                        q[7] = bfma(y1[2], ol.Y1[2], bfma(y0[2], ol.Y0[2], q[7]));
-                        q[8] = bfma(y1[3], ol.Y1[1], bfma(y0[3], ol.Y0[1], q[8]));
-                        q[9] = bfma(y1[3], ol.Y1[2], bfma(y0[3], ol.Y0[2], q[9]));
-                        q[10] = bfma(y1[4], ol.Y1[2], bfma(y0[4], ol.Y0[2], q[10]));
-                        q[11] = bfma(y1[5], ol.Y1[2], bfma(y0[5], ol.Y0[2], q[11]));
-                        q[12] = bfma(ol.r1, ol.Y1[0], bfma(ol.r0, ol.Y0[0], q[12]));
-                        q[13] = bfma(ol.r1, ol.Y1[1], bfma(ol.r0, ol.Y0[1], q[13]));
-                        q[14] = bfma(ol.r1, ol.Y1[2], bfma(ol.r0, ol.Y0[2], q[14]));
+        if constexpr (kRows == 1) {
+            for (int i = 0; i < nrow; ++i) {
+                const float2 z = z_nx;
+                const int l = l_nx;
+                const bool valid = k < seg_end;
+                k += 32; pz += 32; pl += 32;
+                if (i + 1 < nrow && k < seg_end) { z_nx = *pz; l_nx = *pl; }
+                if (valid) {
+                    if (!(vo && skip[l])) {
+                        ObsL<real> ol;
+                        double x[3];
+                        real xf[3], ir[3];             // ir = (1 / rho, 0, 0)
+                        lm_sm_load(recs_a + (unsigned)l * kLmSm, x, xf, ir);
+                        linearize_blk<kLoss, real>(F, x[0], x[1], x[2], xf[0], xf[1], xf[2], ir[0], bt, z.x, z.y, W,
+                                                   diag_w, inv_cb, ol);
+                        emit(ol, l);
                     }
                 }
+                if (kLoss && (i & 3) == 3) la.fold();
             }
-            if (kLoss && (i & 3) == 3) la.fold();
+        } else {
+            // rows i and i + 1 per iteration: two independent linearisations in flight per lane, then their
+            // contributions in row order, so every sum sees the terms of the one-row loop in the same order.  Both blocks
+            // are evaluated unconditionally (a lane past the segment's end, or past an odd piece's last row, works on
+            // the record of a landmark it read earlier, or record 0) and only the live ones are emitted.
+            float2 z_nx1 = make_float2(0.f, 0.f);
+            int l_nx1 = 0;
+            if (nrow > 1 && k + 32 < seg_end) { z_nx1 = fz[k + 32]; l_nx1 = flm[k + 32]; }
+            for (int i = 0; i < nrow; i += 2) {
+                const float2 z0 = z_nx, z1 = z_nx1;
+                const int l0 = l_nx, l1 = l_nx1;
+                const bool has1 = i + 1 < nrow;
+                const bool live0 = k < seg_end && !(vo && skip[l0]);
+                const bool live1 = has1 && k + 32 < seg_end && !(vo && skip[l1]);
+                k += 64;                  // the table is addressed from k (no running pointers: registers)
+                if (i + 2 < nrow && k < seg_end) { z_nx = fz[k]; l_nx = flm[k]; }
+                if (i + 3 < nrow && k + 32 < seg_end) { z_nx1 = fz[k + 32]; l_nx1 = flm[k + 32]; }
+                ObsL<real> o0, o1;
+                double x0[3], x1[3];
+                real xf0[3], ir0[3], xf1[3], ir1[3];
+                lm_sm_load(recs_a + (unsigned)l0 * kLmSm, x0, xf0, ir0);
+                lm_sm_load(recs_a + (unsigned)l1 * kLmSm, x1, xf1, ir1);
+                linearize_blk<kLoss, real>(F, x0[0], x0[1], x0[2], xf0[0], xf0[1], xf0[2], ir0[0], bt, z0.x, z0.y, W,
+                                           diag_w, inv_cb, o0);
+                linearize_blk<kLoss, real>(F, x1[0], x1[1], x1[2], xf1[0], xf1[1], xf1[2], ir1[0], bt, z1.x, z1.y, W,
+                                           diag_w, inv_cb, o1);
+                if (live0) emit(o0, l0);
+                if (live1) emit(o1, l1);
+                if (kLoss && has1 && (i & 3) == 2) la.fold();     // after rows 3, 7, 11, ... as in the one-row loop
+            }
         }
         if (kLoss && (nrow & 3)) la.fold();         // never more than 4 factors in the product
         cs.r = r_stop; cs.seek();
@@ -650,8 +711,17 @@ lin_obs_kernel(PipeArgs a_in) {
     if (exclusive) {       // this CTA wrote every record of the window: complete the landmarks here
         const double mu = pipe_mu(a, w);
         const int compute_scale = a.loop ? (a.ctrl[w].have_scale == 0) : a.compute_scale;
-        for (int l = tid; l < ((M + 3) & ~3); l += kThreads)
-            lm_finish<real>(a, w, l, N, M, fixed, mu, compute_scale, lpart ? part : nullptr, kWarps, Mp);
+        const int Mq = (M + 3) & ~3;
+        for (int l0 = tid; l0 < Mq; l0 += kLmBatch * kThreads) {
+            LmRec lr[kLmBatch] = {};
+#pragma unroll
+            for (int j = 0; j < kLmBatch; ++j)
+                if (l0 + j * kThreads < M) lr[j] = lms[l0 + j * kThreads];
+#pragma unroll
+            for (int j = 0; j < kLmBatch; ++j)
+                if (l0 + j * kThreads < Mq)
+                    lm_finish<real>(a, w, l0 + j * kThreads, N, M, fixed, mu, compute_scale, lpart ? part : nullptr, kWarps, Mp, &lr[j]);
+        }
     }
     // direct part of the reduced system (schur_kernel subtracts the Schur sum from Hred / gred).  D(t, a) enters the
     // off-diagonal block (t, a) with a minus sign and BOTH diagonal blocks with a plus sign; its gradient part enters

@@ -27,7 +27,7 @@ def table_slots(N, M):
 
 
 def lin_bytes(N, M, K, slots, Ncap, Mcap, table_bytes=10, jr=False, nfree=None):
-    """lin_obs_kernel<true, float, 4, 4> + its lm_finish epilogue, one window: the table (table_bytes per slot), LmRec (16 B)
+    """lin_obs_kernel<true, float, ...> (either instantiation) + its lm_finish epilogue, one window: the table (table_bytes per slot), LmRec (16 B)
     and rho (8 B) per landmark read; the fp32 h record (24 B) of every (landmark, free target) written; w_l (8), mask (4),
     LmAux (32) and lm_scale (8) per landmark written; the direct and reduced system blocks written (fp64).  jr: the
     (j.j, j.r) pair (8 B) of every (landmark, target) written and read back."""
