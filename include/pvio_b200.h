@@ -356,6 +356,53 @@ int pvio_b200_batch_window_download(pvio_b200_handle h, int n, const int32_t *sl
                                     int64_t frames_stride, int32_t *n_tracks, int64_t track_stride, int32_t *track_id,
                                     double *inv_depth, int32_t *anchor_frame, int32_t *n_observations, uint8_t *valid,
                                     double *quality);
+/* The per-camera-frame half of SlidingWindowTracker::track (sliding_window_tracker.cpp:76-88) on resident slots, before
+ * the edit that appends the new frame: visual_inertial_pnp of the new frame against the slot (pnp.cpp:32-100), then
+ * Track::triangulate of the tracks born in the new frame (track.cpp:83-106).  The slot's newest frame plays
+ * map->last_frame().  The call reads the slots and writes none of them; its results feed pvio_b200_batch_window_edit.
+ *  - PnP points: an observation takes part only if its track is observed in the slot's newest frame.  Its world point
+ *    is the given one when obs_point's row is finite (the plane-cast point of a TF_PLANE track, pnp.cpp:62-83),
+ *    otherwise Track::get_landmark_point() from the slot: the anchor frame's camera pose applied to
+ *    [z_anchor; 1] / inverse depth.  A track of role -2 or p >= 0 must come with a point.  Residual blocks follow the
+ *    order of obs_track.  Extrinsics, sqrt_inv_cov and cauchy_a are the slot's; the newest frame is the constant
+ *    last frame of the IMU factor.  The solve is pvio_b200_batch_pnp_solve's kernel on a record staged as that call
+ *    stages it, so a record agrees with pvio_b200_batch_pnp_solve of the same problem in a batch of the same n to
+ *    rounding: the kernel's per-warp sums meet in shared-memory atomics, whose order can change from run to run.
+ *  - Triangulation of each new track over two views: the camera of the slot's newest frame (keypoint new_z_last) and
+ *    the camera of the new frame at the solved state (keypoint new_z), with the parallax / depth < 100 checks of
+ *    pvio_b200_triangulate.  new_inv_depth: the inverse depth in the newest slot frame (set_landmark_point), for a new
+ *    track anchored there (a keyframe edit); new_inv_depth_next: the same re-expressed in the new frame (track.cpp:42-49),
+ *    for a new track anchored in the new frame when the edit replaces the newest frame (replace_last).  Both are NaN
+ *    for an invalid track.
+ * Only tracks whose inverse depth is set (TF_VALID) should be named: a landmark point is not checked on the device.
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no output has changed.  Rejected: a slot out
+ * of range, not resident, named twice or without frames; an unknown or dead track, or one named twice in a record; a
+ * non-finite keypoint; a point row neither finite nor NaN; a missing array; an inertial record without an IMU record; a
+ * track of role -2 or p >= 0 that takes part without a point.  n == 0 is a no-op.  One host -> device copy, three
+ * kernel launches whatever n is (gather, PnP, triangulation), one device -> host copy, one synchronisation; the staging
+ * is pvio_b200_batch_pnp_solve's, grown to the largest call seen. */
+typedef struct pvio_b200_window_localize {
+    int32_t slot;
+    int32_t use_inertial;
+    const double *imu_record;   /* [PVIO_B200_IMU_STRIDE] the new frame's factor from the slot's newest frame; NULL when
+                                   !use_inertial */
+    double *state;              /* [16] in: the predicted state; out: the PnP solution */
+    int32_t n_obs;              /* the new frame's keypoints on live tracks of the slot */
+    const int32_t *obs_track;   /* [n_obs] track ids */
+    const double *obs_z;        /* [n_obs][2] normalised keypoints in the new frame */
+    const double *obs_point;    /* [n_obs][3] or NULL: a finite row is the world point; a NaN row or NULL: from the slot */
+    double *points_out;         /* [n_obs][3] or NULL: the world point used, NaN for an observation left out */
+    int32_t n_new;              /* tracks born in the new frame: keypoint in the slot's newest frame and in the new one */
+    const double *new_z_last;   /* [n_new][2] */
+    const double *new_z;        /* [n_new][2] */
+    uint8_t *new_valid;         /* [n_new] out: Track::triangulate's result (TF_VALID) */
+    double *new_inv_depth;      /* [n_new] out: inverse depth in the slot's newest frame, NaN if invalid */
+    double *new_inv_depth_next; /* [n_new] or NULL, out: the same in the new frame, NaN if invalid */
+    pvio_b200_summary *summary; /* or NULL: solve_seconds is the device time of the PnP launch */
+} pvio_b200_window_localize;    /* 120 bytes on LP64 */
+/* n records, each naming a different resident slot; opt (may be NULL) is shared. */
+int pvio_b200_batch_window_localize(pvio_b200_handle h, int n, pvio_b200_window_localize *records,
+                                    const pvio_b200_options *opt);
 
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */

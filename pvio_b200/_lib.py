@@ -89,6 +89,14 @@ class CWindowPlanes(C.Structure):
                 ("track", c_i32p), ("role", c_i32p), ("inv_depth", c_f64p)]
 
 
+class CWindowLocalize(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("use_inertial", C.c_int32), ("imu_record", c_f64p), ("state", c_f64p),
+                ("n_obs", C.c_int32), ("obs_track", c_i32p), ("obs_z", c_f64p), ("obs_point", c_f64p),
+                ("points_out", c_f64p), ("n_new", C.c_int32), ("new_z_last", c_f64p), ("new_z", c_f64p),
+                ("new_valid", c_u8p), ("new_inv_depth", c_f64p), ("new_inv_depth_next", c_f64p),
+                ("summary", C.POINTER(CSummary))]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -106,6 +114,7 @@ EXPORTS = [
     "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig", "pvio_b200_batch_window_reset",
     "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
     "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
+    "pvio_b200_batch_window_localize",
 ]
 
 _lib = None

@@ -20,6 +20,7 @@ def _argtypes(L):
     L.pvio_b200_batch_window_drop_victim.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64, _f64p, C.c_int64]
     L.pvio_b200_batch_window_download.argtypes = [vp, C.c_int, _i32p, _i32p, _f64p, C.c_int64, _i32p, C.c_int64, _i32p,
                                                   _f64p, _i32p, _i32p, _u8p, _f64p]
+    L.pvio_b200_batch_window_localize.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowLocalize), C.POINTER(_lib.COptions)]
 
 
 def _constants(win):
@@ -65,6 +66,27 @@ class Planes:
 
     def role(self, track, role, inv_depth=np.nan):
         self.tracks.append(int(track)); self.roles.append(int(role)); self.rho.append(float(inv_depth))
+        return self
+
+
+class Localize:
+    """One new camera frame of one slot (pvio_b200_window_localize), before the edit that appends it: the predicted
+    state, the IMU record from the slot's newest frame (None: a visual-only PnP), the frame's keypoints on live tracks
+    of the slot (id, z, and a world point for a plane track), and the keypoint pairs of the tracks born in the frame
+    (z in the slot's newest frame, z in the new frame)."""
+
+    def __init__(self, slot, state16, imu_record=None):
+        self.slot = int(slot)
+        self.state = np.array(state16, dtype=np.float64, copy=True)
+        self.imu = None if imu_record is None else np.ascontiguousarray(imu_record, dtype=np.float64)
+        self.obs, self.new = [], []
+
+    def observe(self, track, z, point=None):
+        self.obs.append((int(track), z, point))
+        return self
+
+    def born(self, z_last, z):
+        self.new.append((z_last, z))
         return self
 
 
@@ -137,6 +159,43 @@ class BatchWindows:
                 r.n_set = len(t)
                 r.track, r.role, r.inv_depth = _lib._ptr(t, C.c_int32), _lib._ptr(ro, C.c_int32), _lib._ptr(rho, C.c_double)
         self.ba._ck(self.lib.pvio_b200_batch_window_set_planes(self.h, len(records), recs))
+
+    def localize(self, records, max_iterations=10, initial_radius=0.0):
+        """PnP and new-track triangulation of a list of Localize (distinct slots) in one call; the slots do not change.
+        Per record a dict: state [16], summary, points [n_obs, 3] (NaN: left out of the PnP), and per new track valid,
+        inv_depth (in the slot's newest frame) and inv_depth_next (in the new frame)."""
+        keep, out, n = [], [], len(records)
+        recs, sms = (_lib.CWindowLocalize * max(n, 1))(), (_lib.CSummary * max(n, 1))()
+        p = _lib._ptr
+        for i, L in enumerate(records):
+            r = recs[i]
+            o = dict(state=L.state.copy(), points=np.zeros((len(L.obs), 3)), valid=np.zeros(len(L.new), dtype=np.uint8),
+                     inv_depth=np.zeros(len(L.new)), inv_depth_next=np.zeros(len(L.new)))
+            out.append(o)
+            r.slot, r.state, r.summary = L.slot, p(o["state"], C.c_double), C.pointer(sms[i])
+            if L.imu is not None:
+                keep.append(L.imu)
+                r.use_inertial, r.imu_record = 1, p(L.imu, C.c_double)
+            if L.obs:
+                t = np.array([b[0] for b in L.obs], dtype=np.int32)
+                z = np.ascontiguousarray([b[1] for b in L.obs], dtype=np.float64).reshape(-1, 2)
+                x = np.array([np.full(3, np.nan) if b[2] is None else b[2] for b in L.obs], dtype=np.float64).reshape(-1, 3)
+                keep += [t, z, x]
+                r.n_obs, r.obs_track, r.obs_z, r.obs_point = len(t), p(t, C.c_int32), p(z, C.c_double), p(x, C.c_double)
+                r.points_out = p(o["points"], C.c_double)
+            if L.new:
+                zl = np.ascontiguousarray([b[0] for b in L.new], dtype=np.float64).reshape(-1, 2)
+                zn = np.ascontiguousarray([b[1] for b in L.new], dtype=np.float64).reshape(-1, 2)
+                keep += [zl, zn]
+                r.n_new, r.new_z_last, r.new_z = len(zl), p(zl, C.c_double), p(zn, C.c_double)
+                r.new_valid, r.new_inv_depth = p(o["valid"], C.c_uint8), p(o["inv_depth"], C.c_double)
+                r.new_inv_depth_next = p(o["inv_depth_next"], C.c_double)
+        opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
+        self.ba._ck(self.lib.pvio_b200_batch_window_localize(self.h, n, recs, C.byref(opt)))
+        for i, o in enumerate(out):
+            o["summary"] = {k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_}
+            o["valid"] = o["valid"].astype(bool)
+        return out
 
     def solve(self, slots, max_iterations=10, max_time=1e6, alias_bias=True, postpass=True):
         s = np.ascontiguousarray(slots, dtype=np.int32)

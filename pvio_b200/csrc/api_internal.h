@@ -334,7 +334,21 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
                    int max_level, int max_iter, double eps, double clahe_clip = 0.0, int tiles_x = 0, int tiles_y = 0,
                    uint8_t *prev_eq = nullptr, uint8_t *next_eq = nullptr, uint64_t prev_id = 0, uint64_t next_id = 0, int border = 0);
 int clahe_impl(Handle *h, const uint8_t *src, int width, int height, int stride, double clip, int tiles_x, int tiles_y, uint8_t *dst);
-// pnp.cu
+// pnp.cu: one problem's record of the PnP kernel, staged in device memory (pointers into the same staging buffer)
+struct PnpArgs {
+    const double *pts;      // [n][3]
+    const double *z;        // [n][2]
+    int n, inertial, max_iter;
+    double radius0;
+    WinConst wc;            // extrinsics, sqrt_inv_cov, cauchy_a
+    double last[16];
+    const double *imu_rec;  // [288] device (null without inertial)
+    double *frame;          // [16] in/out (device)
+    double *out;            // [8] iterations, accepted, termination, usable, initial_cost, final_cost, radius, mu
+};
+static_assert(sizeof(PnpArgs) % sizeof(double) == 0, "records are staged as whole 8-byte words");
+// the PnP kernel on n records already on the device, between the events ev0 / ev1: 256 threads for n == 1, otherwise 128
+int launch_pnp(Handle *h, int n, const PnpArgs *d_recs);
 int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,
                    pvio_b200_summary *summary);
 int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,

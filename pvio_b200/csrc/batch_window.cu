@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "api_internal.h"
+#include "tri.cuh"
 
 namespace pvio {
 
@@ -413,6 +414,125 @@ __global__ void __launch_bounds__(kBwThreads) bw_download_kernel(BwArgs a, const
         const uint32_t m = a.tmask[base + r];
         ro[r] = a.trho[base + r]; qo[r] = a.tqual[base + r];
         io[r] = a.tid[base + r]; ao[r] = m ? __ffs(m) - 1 : -1; no[r] = __popc(m); vo[r] = a.tvalid[base + r];
+    }
+}
+
+// ------------------------------------------------------------------------ localize: PnP + triangulation of a new frame
+// One record of pvio_b200_batch_window_localize as staged: the observations that take part (their rows, keypoints and
+// points) at obs_off, the IMU record at imu_off (in records), the new tracks' keypoint pairs at new_off
+struct BwLoc { int32_t slot, newest, inertial, n_obs, obs_off, imu_off, n_new, new_off; };
+static_assert(sizeof(BwLoc) % sizeof(double) == 0, "records are staged as whole 8-byte words");
+
+// the staged sections of one localize call (device pointers into the PnP staging)
+struct LocArgs {
+    const BwLoc *rec;        // [n]
+    const int32_t *row;      // [n_obs] track-table row of each observation
+    const double *z;         // [n_obs][2]
+    const double *imu;       // [n_imu][kImuStride]
+    const double *nz;        // [n_new][4] keypoint in the newest slot frame, keypoint in the new frame
+    double *frames;          // [n][16] in: predicted state, out: solved
+    double *pts;             // [n_obs][3] in: the given point or NaN, out: the point used
+    double *out;             // [n][8] summary words of the PnP kernel
+    double *rho, *rho_next;  // [n_new]
+    uint8_t *valid;          // [n_new]
+    PnpArgs *args;           // [n] written by the gather kernel
+    int max_iter;
+    double radius0;
+};
+
+constexpr int kLocGatherThreads = 128, kLocTriThreads = 64;
+
+// One CTA per record: the world point of every observation without a given one (Track::get_landmark_point, the
+// arithmetic of bw_drop_kernel's re-anchoring), and the record's PnP problem with the slot's constants and newest frame.
+__global__ void __launch_bounds__(kLocGatherThreads) bw_localize_gather_kernel(BwArgs a, LocArgs L) {
+    const BwLoc r = L.rec[blockIdx.x];
+    const int w = r.slot;
+    const size_t base = (size_t)w * a.Mcap;
+    const double *fr = a.frames + (size_t)w * a.Ncap * kFrameStride;
+    const WinConst &c = a.cst[w];
+    for (int i = threadIdx.x; i < r.n_obs; i += kLocGatherThreads) {
+        const int k = r.obs_off + i;
+        double *x = L.pts + 3 * (size_t)k;
+        if (!isnan(x[0])) continue;
+        const size_t R = base + L.row[k];
+        const int an = __ffs(a.tmask[R]) - 1;
+        const double2 z = a.tz[R * a.Ncap + an];
+        const double rho = a.trho[R];
+        double qc[4], pc[3], y[3];
+        bw_cam_pose(fr + an * kFrameStride, c, qc, pc);
+        const double ray[3] = {z.x / rho, z.y / rho, 1.0 / rho};
+        bw_qrot(qc, ray, y);
+        for (int j = 0; j < 3; ++j) x[j] = y[j] + pc[j];
+    }
+    if (threadIdx.x == 0) {
+        PnpArgs p{};                      // what batch_pnp_solve_impl stages for the same problem
+        p.pts = L.pts + 3 * (size_t)r.obs_off; p.z = L.z + 2 * (size_t)r.obs_off;
+        p.n = r.n_obs; p.inertial = r.inertial; p.max_iter = L.max_iter; p.radius0 = L.radius0;
+        for (int j = 0; j < 4; ++j) { p.wc.cam_q[j] = c.cam_q[j]; p.wc.imu_q[j] = c.imu_q[j]; p.wc.sic[j] = c.sic[j]; }
+        for (int j = 0; j < 3; ++j) { p.wc.cam_p[j] = c.cam_p[j]; p.wc.imu_p[j] = c.imu_p[j]; }
+        p.wc.cauchy_a = c.cauchy_a;
+        for (int j = 0; j < kFrameStride; ++j) p.last[j] = fr[r.newest * kFrameStride + j];
+        p.imu_rec = r.inertial ? L.imu + (size_t)r.imu_off * kImuStride : nullptr;
+        p.frame = L.frames + kFrameStride * (size_t)blockIdx.x;
+        p.out = L.out + 8 * (size_t)blockIdx.x;
+        L.args[blockIdx.x] = p;
+    }
+}
+
+// the camera matrix [R | T] of a camera pose (R = q^-1, T = -R p, track.cpp:90-95), row-major 3 x 4
+__device__ void loc_camera_matrix(const double *qc, const double *pc, double *P) {
+    const double qi[4] = {-qc[0], -qc[1], -qc[2], qc[3]};
+    for (int j = 0; j < 3; ++j) {
+        const double e[3] = {j == 0 ? 1.0 : 0.0, j == 1 ? 1.0 : 0.0, j == 2 ? 1.0 : 0.0};
+        double col[3];
+        bw_qrot(qi, e, col);
+        for (int i = 0; i < 3; ++i) P[4 * i + j] = col[i];
+    }
+    double t[3];
+    bw_qrot(qi, pc, t);
+    for (int i = 0; i < 3; ++i) P[4 * i + 3] = -t[i];
+}
+
+struct LocViews {                     // the two views of a new track: the newest slot frame, then the new frame
+    const double *P0, *P1, *nz;
+    __device__ const double *P(int o) const { return o ? P1 : P0; }
+    __device__ const double *z(int o) const { return nz + 2 * o; }
+};
+
+// One CTA per record, one thread per new track: Track::triangulate over the newest slot frame and the new frame at its
+// solved state, the inverse depth in the newest slot frame (set_landmark_point) and re-expressed in the new frame
+// (track.cpp:42-49)
+__global__ void __launch_bounds__(kLocTriThreads) bw_localize_triangulate_kernel(BwArgs a, LocArgs L) {
+    const BwLoc r = L.rec[blockIdx.x];
+    if (r.n_new == 0) return;
+    const WinConst &c = a.cst[r.slot];
+    double qa[4], pa[3], qn[4], pn[3], Pa[12], Pn[12];
+    bw_cam_pose(a.frames + ((size_t)r.slot * a.Ncap + r.newest) * kFrameStride, c, qa, pa);
+    bw_cam_pose(L.frames + kFrameStride * (size_t)blockIdx.x, c, qn, pn);
+    loc_camera_matrix(qa, pa, Pa);
+    loc_camera_matrix(qn, pn, Pn);
+    const double qai[4] = {-qa[0], -qa[1], -qa[2], qa[3]}, qni[4] = {-qn[0], -qn[1], -qn[2], qn[3]};
+    for (int t = threadIdx.x; t < r.n_new; t += kLocTriThreads) {
+        const int k = r.new_off + t;
+        const double *nz = L.nz + 4 * (size_t)k;
+        double p[3], score;
+        const bool ok = tri_point_scored(LocViews{Pa, Pn, nz}, 0, 2, p, score);
+        double rho = NAN, rho_next = NAN;
+        if (ok) {
+            double d[3], y[3];
+            for (int j = 0; j < 3; ++j) d[j] = p[j] - pa[j];
+            bw_qrot(qai, d, y);
+            rho = 1.0 / y[2];
+            const double ray[3] = {nz[0] / rho, nz[1] / rho, 1.0 / rho};
+            double x[3];
+            bw_qrot(qa, ray, x);
+            for (int j = 0; j < 3; ++j) d[j] = x[j] + pa[j] - pn[j];
+            bw_qrot(qni, d, y);
+            rho_next = 1.0 / y[2];
+        }
+        L.valid[k] = ok ? 1 : 0;
+        L.rho[k] = rho;
+        L.rho_next[k] = rho_next;
     }
 }
 
@@ -941,6 +1061,132 @@ int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *s
         if (n_observations) memcpy(n_observations + t0, no, sizeof(int32_t) * T);
         if (valid) memcpy(valid + t0, vo, T);
         if (quality) memcpy(quality + t0, qo, sizeof(double) * T);
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_localize(pvio_b200_handle hh, int n, pvio_b200_window_localize *records,
+                                    const pvio_b200_options *opt) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_localize: bad slot list"));
+    // every record is checked against its slot's host mirror before anything is staged; the observations that take part
+    // are kept with the index they came from
+    std::vector<BwLoc> recs(n);
+    std::vector<int32_t> rows, from;
+    std::vector<double> zs, pts, nzs;
+    int n_imu = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_localize &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (s.N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a window without frames");
+        if (!R.state || R.n_obs < 0 || R.n_new < 0 || (R.n_obs > 0 && (!R.obs_track || !R.obs_z)) ||
+            (R.n_new > 0 && (!R.new_z_last || !R.new_z || !R.new_valid || !R.new_inv_depth)))
+            return fail(h, PVIO_B200_EINVAL, "batch_window_localize: null array");
+        if (R.use_inertial && !R.imu_record)
+            return fail(h, PVIO_B200_EINVAL, "batch_window_localize: an inertial record needs the IMU record from the newest frame");
+        BwLoc &L = recs[i];
+        L = BwLoc{R.slot, s.N - 1, R.use_inertial ? 1 : 0, 0, (int32_t)rows.size(), R.use_inertial ? n_imu++ : -1,
+                  R.n_new, (int32_t)(nzs.size() / 4)};
+        const uint32_t newest = 1u << (s.N - 1);
+        std::vector<uint8_t> named(s.ids.size(), 0);
+        for (int k = 0; k < R.n_obs; ++k) {
+            const int r = find_row(s, R.obs_track[k]);
+            if (r < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: unknown or dead track");
+            if (named[r]) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a track named twice");
+            named[r] = 1;
+            const double *z = R.obs_z + 2 * k;
+            if (!std::isfinite(z[0]) || !std::isfinite(z[1])) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: non-finite keypoint");
+            const double *x = R.obs_point ? R.obs_point + 3 * k : nullptr;
+            const bool given = x && std::isfinite(x[0]) && std::isfinite(x[1]) && std::isfinite(x[2]);
+            if (x && !given && !(std::isnan(x[0]) && std::isnan(x[1]) && std::isnan(x[2])))
+                return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a point row neither finite nor NaN");
+            if (!(s.mask[r] & newest)) continue;                              // pnp.cpp:58
+            if (!given && s.role[r] != -1)
+                return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a plane track without its plane-cast point");
+            rows.push_back(r);
+            from.push_back(k);
+            zs.insert(zs.end(), z, z + 2);
+            for (int j = 0; j < 3; ++j) pts.push_back(given ? x[j] : NAN);
+        }
+        L.n_obs = (int32_t)rows.size() - L.obs_off;
+        for (int k = 0; k < R.n_new; ++k) {
+            const double *a = R.new_z_last + 2 * k, *b = R.new_z + 2 * k;
+            if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(b[0]) || !std::isfinite(b[1]))
+                return fail(h, PVIO_B200_EINVAL, "batch_window_localize: non-finite keypoint");
+            nzs.insert(nzs.end(), {a[0], a[1], b[0], b[1]});
+        }
+    }
+    // staging (doubles): upload records | rows | z | IMU records | new keypoints | states | points; download states |
+    // points | summary words | inverse depths | re-anchored inverse depths | valid bytes; then the PnP records (device)
+    const size_t K = rows.size(), T = nzs.size() / 4, w8 = sizeof(double);
+    const size_t o_row = (size_t)n * sizeof(BwLoc) / w8, o_z = o_row + (K + 1) / 2, o_imu = o_z + 2 * K;
+    const size_t o_nz = o_imu + (size_t)n_imu * kImuStride, o_fr = o_nz + 4 * T, o_pts = o_fr + 16 * (size_t)n;
+    const size_t o_out = o_pts + 3 * K, o_rho = o_out + 8 * (size_t)n, o_next = o_rho + T, o_val = o_next + T;
+    const size_t o_args = o_val + (T + 7) / 8, words = o_args + (size_t)n * sizeof(PnpArgs) / w8;
+    TRY(reserve(h, h->pnp, words, kBoth));
+    double *st = h->pnp.h, *d = h->pnp.d;
+    memcpy(st, recs.data(), sizeof(BwLoc) * n);
+    if (K) {
+        memcpy(st + o_row, rows.data(), sizeof(int32_t) * K);
+        memcpy(st + o_z, zs.data(), w8 * 2 * K);
+        memcpy(st + o_pts, pts.data(), w8 * 3 * K);
+    }
+    if (T) memcpy(st + o_nz, nzs.data(), w8 * 4 * T);
+    for (int i = 0; i < n; ++i) {
+        memcpy(st + o_fr + 16 * (size_t)i, records[i].state, w8 * 16);
+        if (recs[i].inertial) memcpy(st + o_imu + (size_t)recs[i].imu_off * kImuStride, records[i].imu_record, w8 * kImuStride);
+    }
+    CK(h, cudaMemcpyAsync(d, st, w8 * o_out, cudaMemcpyHostToDevice, h->stream));
+    const SolveOptions so = solve_options(opt);
+    LocArgs L;
+    L.rec = reinterpret_cast<const BwLoc *>(d); L.row = reinterpret_cast<const int32_t *>(d + o_row); L.z = d + o_z;
+    L.imu = d + o_imu; L.nz = d + o_nz; L.frames = d + o_fr; L.pts = d + o_pts; L.out = d + o_out; L.rho = d + o_rho;
+    L.rho_next = d + o_next; L.valid = reinterpret_cast<uint8_t *>(d + o_val); L.args = reinterpret_cast<PnpArgs *>(d + o_args);
+    L.max_iter = so.max_iter; L.radius0 = so.radius0;
+    const BwArgs a = launch_args<BwArgs>(h);
+    bw_localize_gather_kernel<<<n, kLocGatherThreads, 0, h->stream>>>(a, L);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(launch_pnp(h, n, L.args));
+    CK(h, cudaGetLastError());
+    bw_localize_triangulate_kernel<<<n, kLocTriThreads, 0, h->stream>>>(a, L);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(st + o_fr, d + o_fr, w8 * (o_args - o_fr), cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+    const uint8_t *val = reinterpret_cast<const uint8_t *>(st + o_val);
+    size_t k = 0;
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_window_localize &R = records[i];
+        const BwLoc &L = recs[i];
+        memcpy(R.state, st + o_fr + 16 * (size_t)i, w8 * 16);
+        if (R.points_out) {
+            for (int j = 0; j < 3 * R.n_obs; ++j) R.points_out[j] = NAN;
+            for (int j = 0; j < L.n_obs; ++j, ++k) memcpy(R.points_out + 3 * from[k], st + o_pts + 3 * k, w8 * 3);
+        } else {
+            k += L.n_obs;
+        }
+        for (int t = 0; t < L.n_new; ++t) {
+            const size_t q = (size_t)L.new_off + t;
+            R.new_valid[t] = val[q];
+            R.new_inv_depth[t] = st[o_rho + q];
+            if (R.new_inv_depth_next) R.new_inv_depth_next[t] = st[o_next + q];
+        }
+        if (R.summary) {
+            const double *b = st + o_out + 8 * (size_t)i;
+            pvio_b200_summary &S = *R.summary;
+            memset(&S, 0, sizeof(S));
+            S.iterations = (int)b[0]; S.accepted_steps = (int)b[1]; S.termination = (int)b[2]; S.usable = (int)b[3];
+            S.initial_cost = b[4]; S.final_cost = b[5]; S.final_radius = b[6]; S.final_mu = b[7];
+            S.solve_seconds = ms * 1e-3;
+        }
     }
     return 0;
 }

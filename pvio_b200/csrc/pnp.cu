@@ -19,18 +19,6 @@
 
 namespace pvio {
 
-struct PnpArgs {            // one problem's record, staged in device memory (pointers into the same staging buffer)
-    const double *pts;      // [n][3]
-    const double *z;        // [n][2]
-    int n, inertial, max_iter;
-    double radius0;
-    WinConst wc;            // extrinsics, sqrt_inv_cov, cauchy_a
-    double last[16];
-    const double *imu_rec;  // [288] device (null without inertial)
-    double *frame;          // [16] in/out (device)
-    double *out;            // [8] iterations, accepted, termination, usable, initial_cost, final_cost, radius, mu
-};
-static_assert(sizeof(PnpArgs) % sizeof(double) == 0, "records are staged as whole 8-byte words");
 constexpr int kPnpRecWords = sizeof(PnpArgs) / sizeof(double);
 
 // The two instantiations of pnp_kernel.  One problem (pvio_b200_pnp_solve, or a batch of one): 256 threads, the
@@ -300,6 +288,15 @@ __global__ void __launch_bounds__(kPnpThreads, kMinCtas) pnp_kernel(const PnpArg
     }
 }
 
+int launch_pnp(Handle *h, int n, const PnpArgs *d_recs) {
+    CK(h, cudaEventRecord(h->ev0, h->stream));
+    if (n == 1) pnp_kernel<kPnpSingleThreads, 1><<<1, kPnpSingleThreads, 0, h->stream>>>(d_recs);
+    else pnp_kernel<kPnpBatchThreads, kPnpBatchCtasPerSm><<<n, kPnpBatchThreads, 0, h->stream>>>(d_recs);
+    CK(h, cudaEventRecord(h->ev1, h->stream));
+    ++h->launches;
+    return 0;
+}
+
 // n problems, frames [n][frames_stride]: every problem is checked before anything is copied; then one H2D copy of the
 // packed staging, one launch between ev0 / ev1, one D2H copy of the frames and summary words, one synchronise.
 int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
@@ -356,11 +353,7 @@ int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, dou
     }
     CK(h, cudaMemcpyAsync(d, stage, sizeof(double) * o_out, cudaMemcpyHostToDevice, h->stream));
     const PnpArgs *d_recs = reinterpret_cast<const PnpArgs *>(d);
-    CK(h, cudaEventRecord(h->ev0, h->stream));
-    if (n == 1) pnp_kernel<kPnpSingleThreads, 1><<<1, kPnpSingleThreads, 0, h->stream>>>(d_recs);
-    else pnp_kernel<kPnpBatchThreads, kPnpBatchCtasPerSm><<<n, kPnpBatchThreads, 0, h->stream>>>(d_recs);
-    CK(h, cudaEventRecord(h->ev1, h->stream));
-    ++h->launches;
+    TRY(launch_pnp(h, n, d_recs));
     // the frames + summary words come back into the pinned staging
     CK(h, cudaMemcpyAsync(stage + o_frames, d + o_frames, sizeof(double) * 24 * n, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
