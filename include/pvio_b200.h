@@ -403,6 +403,43 @@ typedef struct pvio_b200_window_localize {
 /* n records, each naming a different resident slot; opt (may be NULL) is shared. */
 int pvio_b200_batch_window_localize(pvio_b200_handle h, int n, pvio_b200_window_localize *records,
                                     const pvio_b200_options *opt);
+/* The raw IMU samples of a slot's factors, kept on the device with the factor, so that the slot re-integrates it before
+ * every solve as BundleAdjustor::solve does (bundle_adjustor.cpp:220-231): without a first-order bias correction in the
+ * factor (alias_bias), the factor follows the biases only through this re-integration.
+ *  - Which factors are re-integrated: a factor that holds samples is re-integrated before every
+ *    pvio_b200_batch_window_solve and pvio_b200_window_solve that names its slot, at the biases its first frame holds
+ *    on the device at that moment.  The new record overwrites the old one, bg0 / ba0 included, and is bit-identical to
+ *    what pvio_b200_preintegrate returns for the same samples, t_end, biases and noise.  A factor without samples keeps
+ *    the record its edit gave it.
+ *  - How samples follow their factor: drop_victim: the factor of old frame 1 leaves (map.cpp:86) and every other factor
+ *    shifts down with its frame; replace_last: the replaced frame's samples leave, the new frame's factor holds only its
+ *    edit record until a set_imu names it; pvio_b200_batch_window_reset clears every factor's samples, and so does
+ *    anything that ends the slot's residency.
+ *  - drop_victim's marginaliser reads the records of the last solve (as marginalize_frame reads the factors of the last
+ *    solve); localize is unchanged.
+ *  - Every record is checked before anything is staged: on PVIO_B200_EINVAL nothing has changed and nothing was
+ *    launched.  Rejected: a slot out of range, not resident or visual-only; a frame outside 1 .. N - 1; a (slot, frame)
+ *    pair named twice; n_samples < 1; a missing array; a non-finite sample, t_end or noise entry.
+ *  - A set_imu call makes one host -> device copy and one kernel launch whatever n is.  A solve whose named slots hold
+ *    no samples makes the launches and copies it makes without them; otherwise one more launch whatever n is, before
+ *    the trust-region chain (summary.solve_seconds still times the chain only).
+ * The device keeps, per slot and window frame, the samples, t_end and noise; its sample stride grows to the longest
+ * list seen (every slot's samples are copied across on the device). */
+typedef struct pvio_b200_window_imu {
+    int32_t slot;
+    int32_t frame;             /* window index j >= 1: the factor (j - 1, j) */
+    int32_t n_samples;         /* >= 1 (integrate() returns false on none, preintegrator.cpp:86) */
+    const double *samples;     /* [n_samples][7] t, w xyz, a xyz: frame_j->preintegration.data, as stored (after a
+                                  non-keyframe merge, sliding_window_tracker.cpp:116-117, the merged list) */
+    double t_end;              /* frame_j->image->t */
+    const double *noise_cov;   /* [4][9] cov_w, cov_a, cov_bg, cov_ba, as pvio_b200_preintegrate takes it */
+} pvio_b200_window_imu;        /* 40 bytes on LP64 */
+/* n records; a slot may be named by several records, each (slot, frame) once. */
+int pvio_b200_batch_window_set_imu(pvio_b200_handle h, int n, const pvio_b200_window_imu *records);
+/* Device -> host, one copy: records [n][records_stride], the N_i - 1 IMU records of each named slot (resident, with
+ * motion states, named once), in frame order. */
+int pvio_b200_batch_window_imu_records(pvio_b200_handle h, int n, const int32_t *slots, double *records,
+                                       int64_t records_stride);
 
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */

@@ -97,6 +97,11 @@ class CWindowLocalize(C.Structure):
                 ("summary", C.POINTER(CSummary))]
 
 
+class CWindowImu(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("frame", C.c_int32), ("n_samples", C.c_int32), ("samples", c_f64p),
+                ("t_end", C.c_double), ("noise_cov", c_f64p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -114,7 +119,7 @@ EXPORTS = [
     "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig", "pvio_b200_batch_window_reset",
     "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
     "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
-    "pvio_b200_batch_window_localize",
+    "pvio_b200_batch_window_localize", "pvio_b200_batch_window_set_imu", "pvio_b200_batch_window_imu_records",
 ]
 
 _lib = None

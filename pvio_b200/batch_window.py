@@ -21,6 +21,8 @@ def _argtypes(L):
     L.pvio_b200_batch_window_download.argtypes = [vp, C.c_int, _i32p, _i32p, _f64p, C.c_int64, _i32p, C.c_int64, _i32p,
                                                   _f64p, _i32p, _i32p, _u8p, _f64p]
     L.pvio_b200_batch_window_localize.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowLocalize), C.POINTER(_lib.COptions)]
+    L.pvio_b200_batch_window_set_imu.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowImu)]
+    L.pvio_b200_batch_window_imu_records.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64]
 
 
 def _constants(win):
@@ -88,6 +90,17 @@ class Localize:
     def born(self, z_last, z):
         self.new.append((z_last, z))
         return self
+
+
+class Imu:
+    """The raw samples of one IMU factor of one slot (pvio_b200_window_imu): window frame j >= 1 (the factor (j - 1, j)),
+    samples [K][7] (t, w xyz, a xyz), t_end (the time of frame j) and noise_cov (cov_w, cov_a, cov_bg, cov_ba, 3x3 each
+    or [4][9]).  The slot re-integrates the factor from them before every solve that names it."""
+
+    def __init__(self, slot, frame, samples, t_end, noise_cov):
+        self.slot, self.frame, self.t_end = int(slot), int(frame), float(t_end)
+        self.samples = np.ascontiguousarray(np.asarray(samples, dtype=np.float64).reshape(-1, 7))
+        self.noise = np.ascontiguousarray(np.array([np.asarray(c, dtype=np.float64).reshape(9) for c in noise_cov]))
 
 
 class BatchWindows:
@@ -196,6 +209,27 @@ class BatchWindows:
             o["summary"] = {k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_}
             o["valid"] = o["valid"].astype(bool)
         return out
+
+    def set_imu(self, records):
+        """Keep the samples of a list of Imu on the device with their factors, in one call."""
+        recs = (_lib.CWindowImu * max(len(records), 1))()
+        for r, m in zip(recs, records):
+            r.slot, r.frame, r.n_samples, r.t_end = m.slot, m.frame, len(m.samples), m.t_end
+            r.samples, r.noise_cov = _lib._ptr(m.samples, C.c_double), _lib._ptr(m.noise, C.c_double)
+        self.ba._ck(self.lib.pvio_b200_batch_window_set_imu(self.h, len(records), recs))
+
+    def imu_records(self, slots):
+        """Per slot its N - 1 IMU records [N - 1, 288] as they stand on the device (after a solve: the records it used)."""
+        s = np.ascontiguousarray(slots, dtype=np.int32)
+        n = len(s)
+        nf = np.zeros(max(n, 1), dtype=np.int32)
+        self.ba._ck(self.lib.pvio_b200_batch_window_download(self.h, n, _lib._ptr(s, C.c_int32), _lib._ptr(nf, C.c_int32),
+                                                             None, 0, None, 0, None, None, None, None, None, None))
+        stride = _lib.IMU_STRIDE * max(self.ba.max_frames - 1, 1)
+        out = np.zeros((max(n, 1), stride))
+        self.ba._ck(self.lib.pvio_b200_batch_window_imu_records(self.h, n, _lib._ptr(s, C.c_int32), _lib._ptr(out, C.c_double),
+                                                                 stride))
+        return [out[i, :_lib.IMU_STRIDE * max(int(nf[i]) - 1, 0)].reshape(-1, _lib.IMU_STRIDE).copy() for i in range(n)]
 
     def solve(self, slots, max_iterations=10, max_time=1e6, alias_bias=True, postpass=True):
         s = np.ascontiguousarray(slots, dtype=np.int32)

@@ -285,6 +285,7 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     }
     if (n_imu > 0 || n_prior > 0 || inertial) TRY(ensure_inertial(h));
     ws.resident = false;                  // a packed slot is no longer a resident window
+    ws.n_samples.clear();                 // and its IMU factors hold no samples
     ws.perm.clear();                      // until the landmark order below is known
     WinHdr &H = h->hdr.h[slot];
     WinConst &C = h->cst.h[slot];

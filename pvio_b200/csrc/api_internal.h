@@ -126,7 +126,8 @@ struct FmState {
 // (batch_window.cu; slot 0 is also the window of pvio_b200_window_*).  Of a resident window the host keeps integers only:
 // the frame count, the prior's frame count, the fixed mask, the plane count, and for every live track (rows in id order)
 // its id, frame mask and role; the device keeps the track table (frame mask, role, inverse depth, fp64 keypoint per
-// window frame, post-pass flags), the plane parameters and the packed window.
+// window frame, post-pass flags), the plane parameters and the packed window.  Of the IMU factors whose samples stay on
+// the device (pvio_b200_batch_window_set_imu) the host keeps the sample count only.
 // Role of a row: -1 a landmark; -2 a landmark that stays out of the marginaliser's victim set (a plane track of a plane
 // with fewer than 20 tracks); p >= 0 a plane track of plane p: one plane-distance factor over all its observations.
 struct WinSlot {
@@ -139,6 +140,8 @@ struct WinSlot {
     std::vector<int32_t> perm;        // packed landmark -> caller landmark; empty: the identity (always, when resident)
     int prior_resident = 0;           // frame count of the prior (S, e, x0) the marginaliser wrote on the device (0: none);
                                       // a pack naming it with prior_S == NULL keeps it, a host prior clears it
+    std::vector<int32_t> n_samples;   // resident: [Ncap] per IMU factor k (frames k, k + 1) the samples it holds on the
+                                      // device, 0: none (it keeps the record its edit gave it)
 };
 struct BatchWindows {
     DevBuf<int32_t> tid;                         // [W][Mcap] track id of each row
@@ -151,6 +154,11 @@ struct BatchWindows {
     DevBuf<double> tplane;                       // [W][Pcap][4] plane parameters (normal, distance)
     DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
     DevBuf<uint8_t> stage;                       // both sides, grown: the one upload / download of a call
+    // IMU samples of the factors named by set_imu, indexed like imu_data (factor k couples frames k, k + 1); allocated
+    // with the first set_imu, imu_s grown to the longest sample list seen
+    int Scap = 0;                                // samples per factor in imu_s
+    DevBuf<double> imu_s;                        // [W][Ncap][Scap][7] t, w xyz, a xyz
+    DevBuf<double> imu_aux;                      // [W][Ncap][37] t_end, then noise [4][9] cov_w, cov_a, cov_bg, cov_ba
 };
 
 // the plane tables of the solve (api.cu: for_each_staged), allocated with the first window that has plane tracks and

@@ -17,12 +17,17 @@
 // bundle_adjustor.cpp:456-457); rows of role p >= 0 are the plane tracks of plane p, packed in row (= id) order with all
 // their observations, anchor included, into the plane tables the solve kernels read (pt_plane, pt_begin, pt_frame,
 // pt_z), with the slot's plane parameters.  The caller decides the roles (pvio_b200_batch_window_set_planes).
+// IMU factors with samples (pvio_b200_batch_window_set_imu): a factor's raw samples, t_end and noise stay on the device
+// with it, indexed like its record (BatchWindows::imu_s / imu_aux), shift with it in a drop, and are re-integrated at
+// the biases its first frame holds on the device before every solve that names the slot (bundle_adjustor.cpp:220-231);
+// the host keeps the sample count of each factor.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <vector>
 
 #include "api_internal.h"
+#include "imu.cuh"
 #include "tri.cuh"
 
 namespace pvio {
@@ -37,10 +42,14 @@ struct BwEdit {                       // one slot's edit, applied by bw_edit_ker
 };
 struct BwNew { int32_t row, id, frame, pad; double zx, zy, rho; };
 struct BwObs { int32_t row, frame; double zx, zy; };
-struct BwLayout { int32_t slot, N, T, fixed, n_prior, inertial, n_planes, pad; };   // a slot's window as the kernels rebuild it
+struct BwLayout { int32_t slot, N, T, fixed, n_prior, inertial, n_planes, smax; };  // a slot's window as the kernels rebuild
+                                                                                    // it; smax: its longest sample list
 struct BwDl { int32_t slot, N, T, pad; int64_t off; };                  // download: bytes into the result area
 struct BwPlanes { int32_t slot, n_planes, n_set, set_off, param_off, pad; };   // one set_planes record (n_planes < 0: keep)
 struct BwRole { int32_t row, role; double rho; };                       // rho NaN: keep the row's inverse depth
+struct BwImu { int32_t slot, factor, n, off; };   // a factor with samples: n rows at row off (staged rows in set_imu,
+                                                  // rows of the sample store in a solve's work list)
+constexpr int kImuAux = 37;                                             // per factor: t_end, noise [4][9]
 
 // the handle's arrays (the plane tables null until a slot has plane tracks), the track table and the post-pass results
 struct BwArgs : BatchArrays {
@@ -55,6 +64,8 @@ struct BwArgs : BatchArrays {
     int32_t *lm_row;
     const uint8_t *valid;
     const double *quality;
+    double *imu_s, *imu_aux;
+    int Scap;
 };
 
 constexpr int kBwThreads = 256;
@@ -395,8 +406,79 @@ __global__ void __launch_bounds__(kBwThreads) bw_drop_kernel(BwArgs a, const BwL
             if (i < ni) rec[i] = v;
             __syncthreads();
         }
+        if (L.smax > 0) {                     // the samples, t_end and noise of the factors that hold some
+            double *aux = a.imu_aux + (size_t)w * a.Ncap * kImuAux;
+            const int na = (N - 2) * kImuAux;
+            for (int i0 = 0; i0 < na; i0 += kBwThreads) {
+                const int i = i0 + threadIdx.x;
+                const double v = i < na ? aux[kImuAux + i] : 0.0;
+                __syncthreads();
+                if (i < na) aux[i] = v;
+                __syncthreads();
+            }
+            // factor f + 1 -> f, rows [0, smax) of each: every chunk reads above every address an earlier chunk wrote
+            const int rs = L.smax * 7, fs = a.Scap * 7;
+            double *smp = a.imu_s + (size_t)w * a.Ncap * fs;
+            const int ns = (N - 2) * rs;
+            for (int i0 = 0; i0 < ns; i0 += kBwThreads) {
+                const int i = i0 + threadIdx.x, f = i / rs, r = i - f * rs;
+                const double v = i < ns ? smp[(size_t)(f + 1) * fs + r] : 0.0;
+                __syncthreads();
+                if (i < ns) smp[(size_t)f * fs + r] = v;
+                __syncthreads();
+            }
+        }
     }
     bw_compact(a, w, T, sh);
+}
+
+// One CTA per set_imu record: the factor's samples, t_end and noise from the upload into the slot
+__global__ void __launch_bounds__(kBwThreads) bw_set_imu_kernel(BwArgs a, const BwImu *recs, const double *smp,
+                                                                const double *aux) {
+    const BwImu r = recs[blockIdx.x];
+    const size_t F = (size_t)r.slot * a.Ncap + r.factor;
+    double *dst = a.imu_s + F * a.Scap * 7;
+    const double *src = smp + (size_t)r.off * 7;
+    for (int i = threadIdx.x; i < 7 * r.n; i += kBwThreads) dst[i] = src[i];
+    for (int i = threadIdx.x; i < kImuAux; i += kBwThreads) a.imu_aux[F * kImuAux + i] = aux[(size_t)blockIdx.x * kImuAux + i];
+}
+
+// a factor of a slot as imu_integrate_warp reads it: rows J.off .. J.off + J.n - 1 of the slots' sample store (the
+// factor's rows start at its index times Scap), t_end and noise in its aux record
+struct BwSlotFactor {
+    const BwImu &J;
+    const double *samples, *noise, *aux;
+    double *r;
+    __device__ int begin() const { return J.off; }
+    __device__ int end() const { return J.off + J.n; }
+    __device__ double t_end() const { return aux[0]; }
+    __device__ double *rec() const { return r; }
+};
+
+constexpr int kBwImuWarps = 4;
+
+// Before a solve, one warp per factor with samples of the named slots: PreIntegrator::integrate(t, bg, ba, true, true)
+// at the biases the factor's first frame holds now (frame state doubles 10 .. 15), into the slot's IMU record -- the
+// arithmetic of pvio_b200_preintegrate (imu.cuh)
+__global__ void __launch_bounds__(32 * kBwImuWarps) bw_reintegrate_kernel(BwArgs a, const BwImu *jobs, int n) {
+    __shared__ ImuWarpSm sm[kBwImuWarps];
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const int j = blockIdx.x * kBwImuWarps + wv;
+    if (j >= n) return;                                      // whole warps leave together
+    const BwImu &J = jobs[j];
+    const size_t F = (size_t)J.slot * a.Ncap + J.factor;
+    const double *x = a.frames + F * kFrameStride;
+    const double bg[3] = {x[10], x[11], x[12]}, ba[3] = {x[13], x[14], x[15]};
+    const double *aux = a.imu_aux + F * kImuAux;
+    imu_integrate_warp(sm[wv], lane, BwSlotFactor{J, a.imu_s, aux + 1, aux, a.imu_data + F * kImuStride}, bg, ba);
+}
+
+// One CTA per slot: its N - 1 IMU records at dl.off (bytes)
+__global__ void __launch_bounds__(kBwThreads) bw_imu_records_kernel(BwArgs a, const BwDl *dls, uint8_t *outb) {
+    const BwDl d = dls[blockIdx.x];
+    double *o = reinterpret_cast<double *>(outb + d.off);
+    const double *rec = a.imu_data + (size_t)d.slot * a.Ncap * kImuStride;
+    for (int i = threadIdx.x; i < (d.N - 1) * kImuStride; i += kBwThreads) o[i] = rec[i];
 }
 
 // One CTA per slot: frames, then per row inverse depth, quality, id, anchor, observation count, valid -- packed at dl.off
@@ -544,6 +626,7 @@ BwArgs launch_args<BwArgs>(const Handle *h) {
     static_cast<BatchArrays &>(a) = h->arrays;
     a.tid = b.tid.d; a.tmask = b.tmask.d; a.trho = b.trho.d; a.tz = b.tz.d; a.tvalid = b.tvalid.d; a.tqual = b.tqual.d;
     a.trole = b.trole.d; a.tplane = b.tplane.d; a.lm_row = b.lm_row.d; a.valid = h->valid.d; a.quality = h->quality.d;
+    a.imu_s = b.imu_s.d; a.imu_aux = b.imu_aux.d; a.Scap = b.Scap;
     return a;
 }
 
@@ -555,6 +638,25 @@ static int ensure_bw(Handle *h) {
     TRY(alloc(h, b.tz, W * M * h->Ncap, kDevice)); TRY(alloc(h, b.tvalid, W * M, kDevice)); TRY(alloc(h, b.tqual, W * M, kDevice));
     TRY(alloc(h, b.trole, W * M, kDevice)); TRY(alloc(h, b.tplane, W * h->Pcap * 4, kDevice));
     TRY(alloc(h, b.lm_row, W * M, kDevice));
+    return 0;
+}
+
+// the sample store for factors of up to S samples: t_end / noise allocated with the first set_imu, the samples grown to
+// the longest list seen, every slot's samples copied across to the new stride on the device
+static int ensure_imu_store(Handle *h, int S) {
+    BatchWindows &b = h->bw;
+    const size_t F = (size_t)h->W * h->Ncap;
+    if (!b.imu_aux.n) TRY(alloc(h, b.imu_aux, F * kImuAux, kDevice));
+    if (S <= b.Scap) return 0;
+    DevBuf<double> next;
+    TRY(alloc(h, next, F * S * 7, kDevice));
+    if (b.Scap > 0) {
+        CK(h, cudaMemcpy2DAsync(next.d, sizeof(double) * 7 * S, b.imu_s.d, sizeof(double) * 7 * b.Scap,
+                                sizeof(double) * 7 * b.Scap, F, cudaMemcpyDeviceToDevice, h->stream));
+        CK(h, cudaStreamSynchronize(h->stream));       // the old store is freed below
+    }
+    b.imu_s = std::move(next);
+    b.Scap = S;
     return 0;
 }
 
@@ -609,7 +711,9 @@ static void host_header(Handle *h, int slot) {
 }
 
 static BwLayout layout_from(int slot, const WinSlot &s) {
-    return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial, s.n_planes, 0};
+    int smax = 0;
+    for (int32_t c : s.n_samples) smax = std::max(smax, (int)c);
+    return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial, s.n_planes, smax};
 }
 static BwLayout layout_of(const Handle *h, int slot) { return layout_from(slot, h->slots[slot]); }
 
@@ -675,11 +779,27 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
     }
     std::vector<uint8_t> named(range, 0);
     std::vector<BwLayout> lays(n);
-    for (int i = 0; i < n; ++i) { named[slots[i]] = 1; lays[i] = layout_of(h, slots[i]); }
+    std::vector<BwImu> jobs;                  // the factors with samples: re-integrated before the chain
+    for (int i = 0; i < n; ++i) {
+        const WinSlot &s = h->slots[slots[i]];
+        named[slots[i]] = 1; lays[i] = layout_of(h, slots[i]);
+        if (s.inertial)
+            for (int k = 0; k + 1 < s.N; ++k)
+                if (s.n_samples[k] > 0)
+                    jobs.push_back(BwImu{slots[i], k, s.n_samples[k], (int32_t)(((size_t)slots[i] * h->Ncap + k) * h->bw.Scap)});
+    }
     Packer p;
     const size_t o_nm = p.put(named.data(), range), o_lay = p.put(lays.data(), n), o_sl = p.put(slots, n);
+    const size_t o_job = jobs.empty() ? 0 : p.put(jobs.data(), jobs.size());
     uint8_t *din, *dout;
     TRY(upload_stage(h, p, 0, din, dout));
+    if (!jobs.empty()) {
+        const int J = (int)jobs.size();
+        bw_reintegrate_kernel<<<(J + kBwImuWarps - 1) / kBwImuWarps, 32 * kBwImuWarps, 0, h->stream>>>(
+            launch_args<BwArgs>(h), reinterpret_cast<const BwImu *>(din + o_job), J);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+    }
     CK(h, cudaEventRecord(h->ev0, h->stream));
     TRY(run_named_solve(h, opt, range, din + o_nm));
     CK(h, cudaEventRecord(h->ev1, h->stream));
@@ -724,6 +844,7 @@ int pvio_b200_batch_window_reset(pvio_b200_handle hh, int slot, const pvio_b200_
     WinSlot &s = h->slots[slot];
     s = WinSlot();                            // nothing of a former pack or resident window survives
     s.resident = true; s.inertial = w->use_inertial ? 1 : 0;
+    s.n_samples.assign(h->Ncap, 0);
     host_header(h, slot);
     WinConst &C = h->cst.h[slot];
     C = win_const(w);
@@ -800,6 +921,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
             if (s.N - 1 < s.n_prior) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: the newest frame is covered by the prior");
             for (uint32_t &m : s.mask) m &= ~(1u << (s.N - 1));
             s.fixed &= ~(1 << (s.N - 1));
+            if (s.N >= 2) s.n_samples[s.N - 2] = 0;                   // the replaced frame's samples leave
             --s.N;
             R.replace_last = 1;
         }
@@ -830,6 +952,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
             xs.insert(xs.end(), E.state, E.state + kFrameStride);
             if (imu) xs.insert(xs.end(), E.imu_record, E.imu_record + kImuStride);
             if (E.fixed) s.fixed |= 1 << s.N;
+            if (imu) s.n_samples[s.N - 1] = 0;                          // the new factor holds its edit record only
             ++s.N;
         }
         R.new_off = (int)nws.size(); R.n_new = E.n_new_tracks;
@@ -986,6 +1109,8 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
         }
         s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
         --s.N; s.fixed >>= 1; s.n_prior = s.prior_resident = s.N;
+        s.n_samples.erase(s.n_samples.begin());                        // factor 0 leaves, the others shift with their frames
+        s.n_samples.push_back(0);
         TRY(check_window(h, s));
         next[i] = std::move(s);
     }
@@ -1188,6 +1313,97 @@ int pvio_b200_batch_window_localize(pvio_b200_handle hh, int n, pvio_b200_window
             S.solve_seconds = ms * 1e-3;
         }
     }
+    return 0;
+}
+
+int pvio_b200_batch_window_set_imu(pvio_b200_handle hh, int n, const pvio_b200_window_imu *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: bad record list");
+    if (n == 0) return 0;
+    // every record is checked before anything is staged
+    std::vector<BwImu> recs(n);
+    std::vector<std::pair<int32_t, int32_t>> pairs(n);
+    size_t rows = 0;
+    int smax = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_imu &R = records[i];
+        if (R.slot < 0 || R.slot >= h->W || !h->slots[R.slot].resident)
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: slot out of range or not resident");
+        const WinSlot &s = h->slots[R.slot];
+        if (!s.inertial) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: the window carries no motion states");
+        if (R.frame < 1 || R.frame >= s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: frame outside 1 .. N - 1");
+        if (R.n_samples < 1)
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: a factor without IMU samples (integrate() returns false, preintegrator.cpp:86)");
+        if (!R.samples || !R.noise_cov) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: null array");
+        for (int64_t k = 0; k < 7 * (int64_t)R.n_samples; ++k)
+            if (!std::isfinite(R.samples[k])) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite sample");
+        if (!std::isfinite(R.t_end)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite t_end");
+        for (int k = 0; k < 36; ++k)
+            if (!std::isfinite(R.noise_cov[k])) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite noise");
+        recs[i] = BwImu{R.slot, R.frame - 1, R.n_samples, (int32_t)rows};
+        pairs[i] = {R.slot, R.frame};
+        rows += R.n_samples;
+        smax = std::max(smax, R.n_samples);
+    }
+    std::sort(pairs.begin(), pairs.end());
+    if (std::adjacent_find(pairs.begin(), pairs.end()) != pairs.end())
+        return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: a (slot, frame) named twice");
+    if (rows > (size_t)INT32_MAX) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: too many samples in one call");
+    TRY(ensure_imu_store(h, smax));
+    Packer p;
+    const size_t o_rec = p.put(recs.data(), n);
+    const size_t o_smp = (p.buf.size() + 7) & ~(size_t)7;
+    p.buf.resize(o_smp + sizeof(double) * 7 * rows);
+    std::vector<double> aux((size_t)n * kImuAux);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_imu &R = records[i];
+        memcpy(p.buf.data() + o_smp + sizeof(double) * 7 * recs[i].off, R.samples, sizeof(double) * 7 * R.n_samples);
+        aux[(size_t)i * kImuAux] = R.t_end;
+        memcpy(&aux[(size_t)i * kImuAux + 1], R.noise_cov, sizeof(double) * 36);
+    }
+    const size_t o_aux = p.put(aux.data(), aux.size());
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, 0, din, dout));
+    bw_set_imu_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwImu *>(din + o_rec),
+        reinterpret_cast<const double *>(din + o_smp), reinterpret_cast<const double *>(din + o_aux));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) h->slots[recs[i].slot].n_samples[recs[i].factor] = recs[i].n;
+    return 0;
+}
+
+int pvio_b200_batch_window_imu_records(pvio_b200_handle hh, int n, const int32_t *slots, double *records,
+                                       int64_t records_stride) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    TRY(check_slots(h, n, slots, "batch_window_imu_records: bad slot list"));
+    if (n == 0) return 0;
+    if (!records) return fail(h, PVIO_B200_EINVAL, "batch_window_imu_records: null array");
+    std::vector<BwDl> dls(n);
+    int64_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        const WinSlot &s = h->slots[slots[i]];
+        if (!s.inertial) return fail(h, PVIO_B200_EINVAL, "batch_window_imu_records: the window carries no motion states");
+        const int64_t m = (int64_t)std::max(s.N - 1, 0) * kImuStride;
+        if (records_stride < m) return fail(h, PVIO_B200_EINVAL, "batch_window_imu_records: records_stride smaller than a slot's records");
+        dls[i] = BwDl{slots[i], std::max(s.N, 1), 0, 0, off};
+        off += m * (int64_t)sizeof(double);
+    }
+    Packer p;
+    const size_t o_dl = p.put(dls.data(), n);
+    uint8_t *din, *dout;
+    TRY(upload_stage(h, p, (size_t)off, din, dout));
+    bw_imu_records_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwDl *>(din + o_dl), dout);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    const size_t in = dout - din;
+    if (off > 0) CK(h, cudaMemcpyAsync(h->bw.stage.h + in, dout, (size_t)off, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i)
+        memcpy(records + i * records_stride, h->bw.stage.h + in + dls[i].off,
+               sizeof(double) * (size_t)(dls[i].N - 1) * kImuStride);
     return 0;
 }
 

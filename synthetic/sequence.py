@@ -327,6 +327,9 @@ class ModelWindows:
         for p in records:
             self.m[p.slot].set_planes(p)
 
+    def set_imu(self, records):
+        pass
+
     def drop_victim(self, slots, want=False):
         for s in slots:
             self.m[s].drop()
@@ -340,14 +343,17 @@ class BatchPlayer:
     slots[j].  Per keyframe of a slot: solve, drop the victim, then the next camera frame arrives first as a non-keyframe
     (a perturbed state with the frame's observations) that the real keyframe replaces (replace_last), as PVIO's tracker
     erases a non-keyframe newest frame (sliding_window_tracker.cpp:115-121).  The host model keeps, per slot, the live
-    track of each landmark (`ids`) and the window's first absolute frame (`k`)."""
+    track of each landmark (`ids`) and the window's first absolute frame (`k`).
+    With imu_samples, every frame edit with an IMU factor is followed by a set_imu with the factor's raw samples
+    (Run.truth.imu_factors), so the slots re-integrate their factors before each solve; off, the factors keep the
+    records of their edits (integrated once, at the guess biases)."""
 
-    def __init__(self, ba, runs, slots=None, bw=None):
+    def __init__(self, ba, runs, slots=None, bw=None, imu_samples=False):
         """ba: the handle's BundleAdjustor; bw (instead of ba): any object with BatchWindows' interface (ModelWindows).
         `model` (a ModelWindows) follows every edit and drop: the window a gather of the map would pack."""
         from pvio_b200 import _lib
-        from pvio_b200.batch_window import BatchWindows, Edit, Planes
-        self.Edit, self.Planes = Edit, Planes
+        from pvio_b200.batch_window import BatchWindows, Edit, Imu, Planes
+        self.Edit, self.Planes, self.Imu, self.imu_samples = Edit, Planes, Imu, imu_samples
         self.runs, self.bw = runs, (BatchWindows(ba) if bw is None else bw)
         self.model = bw if isinstance(bw, ModelWindows) else ModelWindows()
         self.slots = list(range(len(runs))) if slots is None else list(slots)
@@ -377,7 +383,7 @@ class BatchPlayer:
         r = self.runs[j]
         e = self.Edit(self.slots[j], replace_last).frame(self.state16(j, f_abs) if state is None else state, False,
                                                          self.rec[j][f_abs - 1] if f_abs > 0 and f_win > 0 else None)
-        e.landmarks, e.f_abs = [], f_abs
+        e.landmarks, e.f_abs, e.f_win = [], f_abs, f_win
         for l, (fr, zs) in enumerate(r.tracks):
             if f_abs in fr:
                 z = zs[fr.index(f_abs)]
@@ -388,10 +394,23 @@ class BatchPlayer:
                     e.landmarks.append(l)
         return e
 
+    def imu(self, j, f_win, f_abs, first=None):
+        """the Imu record of window frame f_win = absolute frame f_abs of run j: the raw samples of the factors from
+        absolute frame `first` (default f_abs - 1) to f_abs back to back -- a frame that replaces an erased
+        non-keyframe holds the merged list (sliding_window_tracker.cpp:116-117)"""
+        fs = self.runs[j].truth.imu_factors
+        first = f_abs - 1 if first is None else first
+        smp = np.concatenate([fs[g][0] for g in range(first, f_abs)])
+        return self.Imu(self.slots[j], f_win, smp, fs[f_abs - 1][1], self.runs[j].truth.imu_noise)
+
     def _apply(self, edits, js):
         got = self.bw.edit(edits)
         if self.model is not self.bw:
             self.model.edit(edits)
+        if self.imu_samples:
+            recs = [self.imu(j, e.f_win, e.f_abs) for e, j in zip(edits, js) if e.imu is not None]
+            if recs:
+                self.bw.set_imu(recs)
         for e, j, ids in zip(edits, js, got):
             for l, i in zip(e.landmarks, ids):
                 self.ids[j][l] = int(i)
