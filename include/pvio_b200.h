@@ -440,6 +440,66 @@ int pvio_b200_batch_window_set_imu(pvio_b200_handle h, int n, const pvio_b200_wi
  * motion states, named once), in frame order. */
 int pvio_b200_batch_window_imu_records(pvio_b200_handle h, int n, const int32_t *slots, double *records,
                                        int64_t records_stride);
+/* The whole per-camera-frame start of SlidingWindowTracker::track (sliding_window_tracker.cpp:75-81, 116-118) on
+ * resident inertial slots, before the frame edit; the slot's newest frame plays map->last_frame().  Per record, in the
+ * reference's order:
+ *  1. integrate the new frame's samples up to t_end at the newest frame's device biases (state doubles 10 .. 15):
+ *     bit-identical to pvio_b200_preintegrate of the same samples, biases and noise;
+ *  2. predict the new frame's state from the newest frame's device state and that record (preintegrator.cpp:102-109):
+ *     biases copied, v = v_i + g dt + q_i dv, p = p_i + g dt^2 / 2 + v_i dt + q_i dp, q = q_i dq (not normalised),
+ *     g = (0, 0, -9.80665);
+ *  3. localize from the predicted state: the PnP and the triangulation of pvio_b200_batch_window_localize, with the
+ *     same observation, point and new-track rules and the same kernels;
+ *  4. keyframe_check (:255-296): frame_i is the slot's latest keyframe -- its newest frame when newest_is_keyframe,
+ *     otherwise frame N - 2 (a slot holds at most one non-keyframe, its newest).  qij = (cam_q^* imu_q dq imu_q^*
+ *     cam_q)^* with dq the step-1 record's.  Each named track with a keypoint in frame_i adds
+ *     |apply_k(hnormalized(qij [z_i; 1])) - apply_k(z_j)| (fx, fy the slot's, cx, cy the record's): an observed track
+ *     with its keypoint in frame_i from the slot, a new track with new_z_last when frame_i is the newest frame.  Fewer
+ *     than 50 entries: a keyframe; otherwise entry m * 4 / 5 of the ascending list (exact for any m), a keyframe above
+ *     50 px, else ++skipped; skipped > 10 forces a keyframe, a keyframe resets skipped to 0;
+ *  5. when the newest frame is not a keyframe: integrate merge_samples ++ samples up to t_end at the newest frame's
+ *     biases (:116-118), bit-identical to pvio_b200_preintegrate of the concatenated list.
+ * imu_record is the factor the frame edit appends: step 1's record when the newest frame is a keyframe, otherwise step
+ * 5's.  The call reads the slots and writes none of them.  Every record is checked before anything is staged: on
+ * PVIO_B200_EINVAL no output has changed and nothing was launched.  Rejected: every localize rejection; a visual-only
+ * slot; n_samples < 1; a non-finite sample, t_end, noise entry, cx or cy; newest_is_keyframe not 0 or 1; a non-keyframe
+ * newest frame with N < 2 or without a merge list; a merge list with a keyframe newest frame; a missing array;
+ * skipped_frames NULL or negative.  n == 0 is a no-op.  One host -> device copy, five kernel launches whatever n is
+ * (integrate + predict, gather, PnP, triangulation, keyframe check), one device -> host copy, one synchronisation; the
+ * staging is localize's. */
+typedef struct pvio_b200_window_track_frame {
+    int32_t slot;
+    int32_t newest_is_keyframe;       /* 1: the slot's newest frame is a keyframe; 0: it is not (the next edit replaces it) */
+    int32_t n_samples;                /* >= 1 */
+    int32_t n_merge;                  /* newest_is_keyframe == 0: >= 1; otherwise 0 */
+    const double *samples;            /* [n_samples][7] t, w xyz, a xyz: the new frame's own samples */
+    const double *merge_samples;      /* [n_merge][7] the newest frame's own samples, or NULL with a keyframe newest frame */
+    double t_end;                     /* the new frame's time */
+    const double *noise_cov;          /* [4][9] cov_w, cov_a, cov_bg, cov_ba, as pvio_b200_preintegrate takes it */
+    double cx, cy;                    /* principal point of the camera matrix the parallax is measured with */
+    int32_t *skipped_frames;          /* in / out: the tracker's skipped-frame counter, >= 0 */
+    double *state;                    /* [16] out: the PnP solution */
+    double *predicted;                /* [16] or NULL, out: the predicted state */
+    double *imu_record;               /* [PVIO_B200_IMU_STRIDE] out: the factor of the frame edit */
+    uint8_t *keyframe;                /* out: 1 if the new frame is a keyframe */
+    double *parallax;                 /* or NULL, out: the 80th-percentile parallax in px, NaN with fewer than 50 pairs */
+    int32_t *n_parallax;              /* or NULL, out: the pairs in the parallax list */
+    int32_t n_obs;                    /* as pvio_b200_window_localize */
+    const int32_t *obs_track;
+    const double *obs_z;
+    const double *obs_point;
+    double *points_out;
+    int32_t n_new;
+    const double *new_z_last;
+    const double *new_z;
+    uint8_t *new_valid;
+    double *new_inv_depth;
+    double *new_inv_depth_next;
+    pvio_b200_summary *summary;
+} pvio_b200_window_track_frame;       /* 216 bytes on LP64 */
+/* n records, each naming a different resident slot; opt (may be NULL) is shared by the PnP solves. */
+int pvio_b200_batch_window_track_frame(pvio_b200_handle h, int n, pvio_b200_window_track_frame *records,
+                                       const pvio_b200_options *opt);
 
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */

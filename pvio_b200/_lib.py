@@ -102,6 +102,17 @@ class CWindowImu(C.Structure):
                 ("t_end", C.c_double), ("noise_cov", c_f64p)]
 
 
+class CWindowTrackFrame(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("newest_is_keyframe", C.c_int32), ("n_samples", C.c_int32), ("n_merge", C.c_int32),
+                ("samples", c_f64p), ("merge_samples", c_f64p), ("t_end", C.c_double), ("noise_cov", c_f64p),
+                ("cx", C.c_double), ("cy", C.c_double), ("skipped_frames", c_i32p), ("state", c_f64p),
+                ("predicted", c_f64p), ("imu_record", c_f64p), ("keyframe", c_u8p), ("parallax", c_f64p),
+                ("n_parallax", c_i32p), ("n_obs", C.c_int32), ("obs_track", c_i32p), ("obs_z", c_f64p),
+                ("obs_point", c_f64p), ("points_out", c_f64p), ("n_new", C.c_int32), ("new_z_last", c_f64p),
+                ("new_z", c_f64p), ("new_valid", c_u8p), ("new_inv_depth", c_f64p), ("new_inv_depth_next", c_f64p),
+                ("summary", C.POINTER(CSummary))]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -120,6 +131,7 @@ EXPORTS = [
     "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
     "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
     "pvio_b200_batch_window_localize", "pvio_b200_batch_window_set_imu", "pvio_b200_batch_window_imu_records",
+    "pvio_b200_batch_window_track_frame",
 ]
 
 _lib = None

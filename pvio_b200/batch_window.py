@@ -23,6 +23,7 @@ def _argtypes(L):
     L.pvio_b200_batch_window_localize.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowLocalize), C.POINTER(_lib.COptions)]
     L.pvio_b200_batch_window_set_imu.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowImu)]
     L.pvio_b200_batch_window_imu_records.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64]
+    L.pvio_b200_batch_window_track_frame.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowTrackFrame), C.POINTER(_lib.COptions)]
 
 
 def _constants(win):
@@ -90,6 +91,48 @@ class Localize:
     def born(self, z_last, z):
         self.new.append((z_last, z))
         return self
+
+
+class TrackFrame(Localize):
+    """One new camera frame of one inertial slot (pvio_b200_window_track_frame): its raw samples [K][7] up to t_end with
+    noise_cov (as Imu takes them), the principal point (cx, cy), whether the slot's newest frame is a keyframe, and
+    otherwise the newest frame's own samples (merge_samples); the tracker's skipped-frame counter; the keypoints as
+    Localize's observe / born.  The call integrates, predicts, solves the PnP, triangulates and checks for a keyframe."""
+
+    def __init__(self, slot, samples, t_end, noise_cov, cx, cy, newest_is_keyframe=True, merge_samples=None,
+                 skipped_frames=0):
+        super().__init__(slot, np.full(16, np.nan))
+        self.samples = np.ascontiguousarray(np.asarray(samples, dtype=np.float64).reshape(-1, 7))
+        self.t_end, self.cx, self.cy = float(t_end), float(cx), float(cy)
+        self.noise = np.ascontiguousarray(np.array([np.asarray(c, dtype=np.float64).reshape(9) for c in noise_cov]))
+        self.newest_is_keyframe = bool(newest_is_keyframe)
+        self.merge = None if merge_samples is None else np.ascontiguousarray(
+            np.asarray(merge_samples, dtype=np.float64).reshape(-1, 7))
+        self.skipped = int(skipped_frames)
+
+
+def _localize_fields(r, L, o, keep):
+    """the observation and new-track fields of a localize / track_frame ctypes record r from L, outputs into dict o"""
+    p = _lib._ptr
+    if L.obs:
+        t = np.array([b[0] for b in L.obs], dtype=np.int32)
+        z = np.ascontiguousarray([b[1] for b in L.obs], dtype=np.float64).reshape(-1, 2)
+        x = np.array([np.full(3, np.nan) if b[2] is None else b[2] for b in L.obs], dtype=np.float64).reshape(-1, 3)
+        keep += [t, z, x]
+        r.n_obs, r.obs_track, r.obs_z, r.obs_point = len(t), p(t, C.c_int32), p(z, C.c_double), p(x, C.c_double)
+        r.points_out = p(o["points"], C.c_double)
+    if L.new:
+        zl = np.ascontiguousarray([b[0] for b in L.new], dtype=np.float64).reshape(-1, 2)
+        zn = np.ascontiguousarray([b[1] for b in L.new], dtype=np.float64).reshape(-1, 2)
+        keep += [zl, zn]
+        r.n_new, r.new_z_last, r.new_z = len(zl), p(zl, C.c_double), p(zn, C.c_double)
+        r.new_valid, r.new_inv_depth = p(o["valid"], C.c_uint8), p(o["inv_depth"], C.c_double)
+        r.new_inv_depth_next = p(o["inv_depth_next"], C.c_double)
+
+
+def _localize_out(L):
+    return dict(state=L.state.copy(), points=np.zeros((len(L.obs), 3)), valid=np.zeros(len(L.new), dtype=np.uint8),
+                inv_depth=np.zeros(len(L.new)), inv_depth_next=np.zeros(len(L.new)))
 
 
 class Imu:
@@ -182,33 +225,58 @@ class BatchWindows:
         p = _lib._ptr
         for i, L in enumerate(records):
             r = recs[i]
-            o = dict(state=L.state.copy(), points=np.zeros((len(L.obs), 3)), valid=np.zeros(len(L.new), dtype=np.uint8),
-                     inv_depth=np.zeros(len(L.new)), inv_depth_next=np.zeros(len(L.new)))
+            o = _localize_out(L)
             out.append(o)
             r.slot, r.state, r.summary = L.slot, p(o["state"], C.c_double), C.pointer(sms[i])
             if L.imu is not None:
                 keep.append(L.imu)
                 r.use_inertial, r.imu_record = 1, p(L.imu, C.c_double)
-            if L.obs:
-                t = np.array([b[0] for b in L.obs], dtype=np.int32)
-                z = np.ascontiguousarray([b[1] for b in L.obs], dtype=np.float64).reshape(-1, 2)
-                x = np.array([np.full(3, np.nan) if b[2] is None else b[2] for b in L.obs], dtype=np.float64).reshape(-1, 3)
-                keep += [t, z, x]
-                r.n_obs, r.obs_track, r.obs_z, r.obs_point = len(t), p(t, C.c_int32), p(z, C.c_double), p(x, C.c_double)
-                r.points_out = p(o["points"], C.c_double)
-            if L.new:
-                zl = np.ascontiguousarray([b[0] for b in L.new], dtype=np.float64).reshape(-1, 2)
-                zn = np.ascontiguousarray([b[1] for b in L.new], dtype=np.float64).reshape(-1, 2)
-                keep += [zl, zn]
-                r.n_new, r.new_z_last, r.new_z = len(zl), p(zl, C.c_double), p(zn, C.c_double)
-                r.new_valid, r.new_inv_depth = p(o["valid"], C.c_uint8), p(o["inv_depth"], C.c_double)
-                r.new_inv_depth_next = p(o["inv_depth_next"], C.c_double)
+            _localize_fields(r, L, o, keep)
         opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
         self.ba._ck(self.lib.pvio_b200_batch_window_localize(self.h, n, recs, C.byref(opt)))
         for i, o in enumerate(out):
             o["summary"] = {k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_}
             o["valid"] = o["valid"].astype(bool)
         return out
+
+    def track_frame(self, records, max_iterations=10, initial_radius=0.0):
+        """Integrate, predict, PnP, triangulate and keyframe-check a list of TrackFrame (distinct inertial slots) in one
+        call; the slots do not change.  Per record what localize returns, plus predicted [16], imu_record [288] (the
+        factor of the frame edit), keyframe, parallax (NaN with fewer than 50 pairs), n_parallax and skipped_frames."""
+        recs, sms, out, keep = self.track_frame_records(records)
+        opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
+        self.ba._ck(self.lib.pvio_b200_batch_window_track_frame(self.h, len(records), recs, C.byref(opt)))
+        for i, o in enumerate(out):
+            o["summary"] = {k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_}
+            o["valid"] = o["valid"].astype(bool)
+            o["keyframe"], o["parallax"] = bool(o["keyframe"][0]), float(o["parallax"][0])
+            o["n_parallax"], o["skipped_frames"] = int(o["n_parallax"][0]), int(o["skipped_frames"][0])
+        return out
+
+    @staticmethod
+    def track_frame_records(records):
+        """the ctypes records of a list of TrackFrame: (records, summaries, output arrays per record, arrays to keep)"""
+        keep, out, n = [], [], len(records)
+        recs, sms = (_lib.CWindowTrackFrame * max(n, 1))(), (_lib.CSummary * max(n, 1))()
+        p = _lib._ptr
+        for i, T in enumerate(records):
+            r = recs[i]
+            o = _localize_out(T)
+            o.update(predicted=np.zeros(16), imu_record=np.zeros(_lib.IMU_STRIDE), keyframe=np.zeros(1, dtype=np.uint8),
+                     parallax=np.zeros(1), n_parallax=np.zeros(1, dtype=np.int32),
+                     skipped_frames=np.array([T.skipped], dtype=np.int32))
+            out.append(o)
+            r.slot, r.newest_is_keyframe = T.slot, 1 if T.newest_is_keyframe else 0
+            r.n_samples, r.samples, r.t_end, r.noise_cov = len(T.samples), p(T.samples, C.c_double), T.t_end, p(T.noise, C.c_double)
+            if T.merge is not None:
+                r.n_merge, r.merge_samples = len(T.merge), p(T.merge, C.c_double)
+            r.cx, r.cy = T.cx, T.cy
+            r.skipped_frames, r.state, r.predicted = p(o["skipped_frames"], C.c_int32), p(o["state"], C.c_double), p(o["predicted"], C.c_double)
+            r.imu_record, r.keyframe = p(o["imu_record"], C.c_double), p(o["keyframe"], C.c_uint8)
+            r.parallax, r.n_parallax, r.summary = p(o["parallax"], C.c_double), p(o["n_parallax"], C.c_int32), C.pointer(sms[i])
+            keep += [T.samples, T.noise] + ([] if T.merge is None else [T.merge])
+            _localize_fields(r, T, o, keep)
+        return recs, sms, out, keep
 
     def set_imu(self, records):
         """Keep the samples of a list of Imu on the device with their factors, in one call."""

@@ -618,6 +618,164 @@ __global__ void __launch_bounds__(kLocTriThreads) bw_localize_triangulate_kernel
     }
 }
 
+// ------------------------------------------------------------------------ track_frame: integrate, predict, keyframe check
+// One record of pvio_b200_batch_window_track_frame beyond its localize half (same index): its samples' t_end and noise
+// at aux_off (kImuAux doubles), frame_i of the keyframe check, the observed tracks with a keypoint in frame_i (rows and
+// new-frame keypoints at kf_off), whether the new tracks count, where its parallax list starts in the scratch
+struct BwTrack { int32_t merged, frame_i, n_kf, kf_off, use_new, par_off, skipped, aux_off; double cx, cy; };
+// one warp job of the integrate launch: record `rec`, staged sample rows [begin, end); merged: the merged list
+struct BwTrackJob { int32_t rec, begin, end, merged; };
+static_assert(sizeof(BwTrack) % sizeof(double) == 0 && sizeof(BwTrackJob) % sizeof(double) == 0,
+              "records are staged as whole 8-byte words");
+
+struct TrackArgs {
+    const BwTrack *tr;       // [n]
+    const BwTrackJob *job;   // [n_jobs]
+    const double *smp;       // [rows][7] per record merge_samples ++ samples
+    const double *aux;       // [n][kImuAux] t_end, noise
+    const int32_t *kf_row;   // [n_kf] track-table row of each observed pair
+    const double *kf_z;      // [n_kf][2] its keypoint in the new frame
+    double *rec1;            // [n][kImuStride] step-1 records (scratch; the PnP reads them through LocArgs::imu)
+    double *rec_out;         // [n][kImuStride] the edit's records
+    double *pred;            // [n][16]
+    double *kfo;             // [n][4] keyframe, parallax, pairs, skipped
+    double *par;             // parallax lists (scratch)
+    int n_jobs;
+};
+
+// a job as imu_integrate_warp reads it
+struct BwTrackFactor {
+    const BwTrackJob &J;
+    const double *samples, *noise, *aux;
+    double *r;
+    __device__ int begin() const { return J.begin; }
+    __device__ int end() const { return J.end; }
+    __device__ double t_end() const { return aux[0]; }
+    __device__ double *rec() const { return r; }
+};
+
+// One warp per job: PreIntegrator::integrate(t, bg, ba, true, true) at the biases of the slot's newest frame
+// (sliding_window_tracker.cpp:77, 118) -- the arithmetic of pvio_b200_preintegrate (imu.cuh); after the step-1 job,
+// PreIntegrator::predict (preintegrator.cpp:102-109) into the PnP's initial state
+__global__ void __launch_bounds__(32 * kBwImuWarps) bw_track_integrate_kernel(BwArgs a, LocArgs L, TrackArgs T) {
+    __shared__ ImuWarpSm sm[kBwImuWarps];
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const int j = blockIdx.x * kBwImuWarps + wv;
+    if (j >= T.n_jobs) return;                               // whole warps leave together
+    const BwTrackJob &J = T.job[j];
+    const BwLoc r = L.rec[J.rec];
+    const double *x = a.frames + ((size_t)r.slot * a.Ncap + r.newest) * kFrameStride;
+    const double bg[3] = {x[10], x[11], x[12]}, ba[3] = {x[13], x[14], x[15]};
+    const double *aux = T.aux + (size_t)T.tr[J.rec].aux_off;
+    double *rec = (J.merged ? T.rec_out : T.rec1) + (size_t)J.rec * kImuStride;
+    imu_integrate_warp(sm[wv], lane, BwTrackFactor{J, T.smp, aux + 1, aux, rec}, bg, ba);
+    if (J.merged) return;
+    __syncwarp();
+    if (!T.tr[J.rec].merged)                                 // the edit takes the step-1 record
+        for (int i = lane; i < kImuStride; i += 32) T.rec_out[(size_t)J.rec * kImuStride + i] = rec[i];
+    if (lane == 0) {
+        const double g[3] = {0.0, 0.0, -9.80665};            // PVIO_GRAVITY_NOMINAL, as ba_factors.cuh
+        const double dt = rec[0];
+        double y[16], qdv[3], qdp[3];
+        bw_qrot(x, rec + 8, qdv);
+        bw_qrot(x, rec + 5, qdp);
+        for (int k = 0; k < 3; ++k) {
+            y[7 + k] = x[7 + k] + g[k] * dt + qdv[k];
+            y[4 + k] = x[4 + k] + 0.5 * g[k] * dt * dt + x[7 + k] * dt + qdp[k];
+        }
+        bw_qmul(x, rec + 1, y);
+        for (int k = 10; k < 16; ++k) y[k] = x[k];
+        for (int k = 0; k < 16; ++k) {
+            L.frames[kFrameStride * (size_t)J.rec + k] = y[k];
+            T.pred[kFrameStride * (size_t)J.rec + k] = y[k];
+        }
+    }
+}
+
+// One CTA per record: SlidingWindowTracker::keyframe_check (sliding_window_tracker.cpp:255-296).  The parallax list goes
+// to the scratch; its entry m * 4 / 5 in ascending order is found by a radix select over the fp64 bit patterns (the
+// parallaxes are >= 0, so their bit patterns order as their values), eight 8-bit digits from the top, which returns
+// exactly the element a sort would put there for any m.
+__global__ void __launch_bounds__(kBwThreads) bw_track_keyframe_kernel(BwArgs a, LocArgs L, TrackArgs T) {
+    __shared__ int sh[kBwWarps + 1];
+    __shared__ unsigned int hist[256];
+    __shared__ unsigned long long prefix;
+    __shared__ int rank;
+    const BwTrack t = T.tr[blockIdx.x];
+    const BwLoc r = L.rec[blockIdx.x];
+    const WinConst &c = a.cst[r.slot];
+    const size_t base = (size_t)r.slot * a.Mcap;
+    const double *dq = T.rec1 + (size_t)blockIdx.x * kImuStride + 1;
+    double q[4], u[4], qij[4];
+    const double cq[4] = {-c.cam_q[0], -c.cam_q[1], -c.cam_q[2], c.cam_q[3]};
+    const double iq[4] = {-c.imu_q[0], -c.imu_q[1], -c.imu_q[2], c.imu_q[3]};
+    bw_qmul(cq, c.imu_q, q);
+    bw_qmul(q, dq, u);
+    bw_qmul(u, iq, q);
+    bw_qmul(q, c.cam_q, u);
+    qij[0] = -u[0]; qij[1] = -u[1]; qij[2] = -u[2]; qij[3] = u[3];
+    const int n_new = t.use_new ? r.n_new : 0, m = t.n_kf + n_new;
+    double *par = T.par + t.par_off;
+    for (int k = threadIdx.x; k < m; k += kBwThreads) {
+        double zi[3], zj[2];
+        if (k < t.n_kf) {
+            const double2 z = a.tz[(base + T.kf_row[t.kf_off + k]) * a.Ncap + t.frame_i];
+            zi[0] = z.x; zi[1] = z.y;
+            zj[0] = T.kf_z[2 * ((size_t)t.kf_off + k)]; zj[1] = T.kf_z[2 * ((size_t)t.kf_off + k) + 1];
+        } else {
+            const double *nz = L.nz + 4 * ((size_t)r.new_off + k - t.n_kf);
+            zi[0] = nz[0]; zi[1] = nz[1]; zj[0] = nz[2]; zj[1] = nz[3];
+        }
+        zi[2] = 1.0;
+        double y[3];
+        bw_qrot(qij, zi, y);
+        const double pix = y[0] / y[2] * c.fx + t.cx, piy = y[1] / y[2] * c.fy + t.cy;
+        const double pjx = zj[0] * c.fx + t.cx, pjy = zj[1] * c.fy + t.cy;
+        const double dx = pix - pjx, dy = piy - pjy;
+        par[k] = sqrt(dx * dx + dy * dy);
+    }
+    if (threadIdx.x == 0) { prefix = 0ull; rank = m * 4 / 5; }
+    __syncthreads();
+    if (m >= 50) {
+        unsigned long long mask = 0ull;
+        for (int shift = 56; shift >= 0; shift -= 8) {
+            hist[threadIdx.x] = 0u;
+            __syncthreads();
+            const unsigned long long pre = prefix;
+            for (int k = threadIdx.x; k < m; k += kBwThreads) {
+                const unsigned long long v = (unsigned long long)__double_as_longlong(par[k]);
+                if ((v & mask) == pre) atomicAdd(&hist[(v >> shift) & 255u], 1u);
+            }
+            __syncthreads();
+            const int cnt = (int)hist[threadIdx.x], want = rank;
+            int tot;
+            const int below = bw_block_scan(cnt, sh, tot);   // ends with a barrier: every thread has read rank / prefix
+            if (want >= below && want < below + cnt) {           // exactly one digit holds the wanted rank
+                prefix = pre | ((unsigned long long)threadIdx.x << shift);
+                rank = want - below;
+            }
+            mask |= 255ull << shift;
+            __syncthreads();
+        }
+    }
+    if (threadIdx.x == 0) {
+        int skipped = t.skipped;
+        bool kf;
+        double p = NAN;
+        if (m < 50) {
+            kf = true;
+        } else {
+            p = __longlong_as_double((long long)prefix);
+            kf = p > 50.0;
+            if (!kf) ++skipped;
+        }
+        if (skipped > 10) kf = true;
+        if (kf) skipped = 0;
+        double *o = T.kfo + 4 * (size_t)blockIdx.x;
+        o[0] = kf ? 1.0 : 0.0; o[1] = p; o[2] = m; o[3] = skipped;
+    }
+}
+
 // ------------------------------------------------------------------------ host side
 template <>
 BwArgs launch_args<BwArgs>(const Handle *h) {
@@ -817,6 +975,161 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
             summaries[i].solve_seconds = ms * 1e-3;
         }
     return 0;
+}
+
+// The localize half of a batch of records (pvio_b200_batch_window_localize, pvio_b200_batch_window_track_frame): every
+// record checked against its slot's host mirror, the observations that take part kept with the index they came from,
+// the new tracks' keypoint pairs; then the staging layout in h->pnp (doubles).  Upload: records | rows | z | IMU
+// records (imu_staged) | new keypoints | the caller's upload words (x) | states | points.  Download: states | points |
+// summary words | inverse depths | re-anchored inverse depths | valid bytes | the caller's download words (y).  Then,
+// device only: the PnP records and the caller's scratch words (s).
+struct LocPlan {
+    const char *what;
+    std::vector<BwLoc> recs;
+    std::vector<int32_t> rows, from;
+    std::vector<double> zs, pts, nzs;
+    int n_imu = 0;
+    bool imu_staged = true;
+    size_t o_row = 0, o_z = 0, o_imu = 0, o_nz = 0, o_x = 0, o_fr = 0, o_pts = 0, o_out = 0, o_rho = 0, o_next = 0;
+    size_t o_val = 0, o_y = 0, o_args = 0, o_s = 0, words = 0;
+};
+
+static int loc_fail(Handle *h, const LocPlan &P, const char *why) {
+    return fail(h, PVIO_B200_EINVAL, (std::string(P.what) + ": " + why).c_str());
+}
+
+// checks record R (imu_given: it must carry its IMU record when inertial) and appends it to the plan
+static int loc_add(Handle *h, LocPlan &P, const pvio_b200_window_localize &R, bool imu_given) {
+    const WinSlot &s = h->slots[R.slot];
+    if (s.N < 1) return loc_fail(h, P, "a window without frames");
+    if (!R.state || R.n_obs < 0 || R.n_new < 0 || (R.n_obs > 0 && (!R.obs_track || !R.obs_z)) ||
+        (R.n_new > 0 && (!R.new_z_last || !R.new_z || !R.new_valid || !R.new_inv_depth)))
+        return loc_fail(h, P, "null array");
+    if (imu_given && R.use_inertial && !R.imu_record)
+        return loc_fail(h, P, "an inertial record needs the IMU record from the newest frame");
+    P.recs.push_back(BwLoc{R.slot, s.N - 1, R.use_inertial ? 1 : 0, 0, (int32_t)P.rows.size(), R.use_inertial ? P.n_imu++ : -1,
+                           R.n_new, (int32_t)(P.nzs.size() / 4)});
+    BwLoc &L = P.recs.back();
+    const uint32_t newest = 1u << (s.N - 1);
+    std::vector<uint8_t> named(s.ids.size(), 0);
+    for (int k = 0; k < R.n_obs; ++k) {
+        const int r = find_row(s, R.obs_track[k]);
+        if (r < 0) return loc_fail(h, P, "unknown or dead track");
+        if (named[r]) return loc_fail(h, P, "a track named twice");
+        named[r] = 1;
+        const double *z = R.obs_z + 2 * k;
+        if (!std::isfinite(z[0]) || !std::isfinite(z[1])) return loc_fail(h, P, "non-finite keypoint");
+        const double *x = R.obs_point ? R.obs_point + 3 * k : nullptr;
+        const bool given = x && std::isfinite(x[0]) && std::isfinite(x[1]) && std::isfinite(x[2]);
+        if (x && !given && !(std::isnan(x[0]) && std::isnan(x[1]) && std::isnan(x[2])))
+            return loc_fail(h, P, "a point row neither finite nor NaN");
+        if (!(s.mask[r] & newest)) continue;                              // pnp.cpp:58
+        if (!given && s.role[r] != -1) return loc_fail(h, P, "a plane track without its plane-cast point");
+        P.rows.push_back(r);
+        P.from.push_back(k);
+        P.zs.insert(P.zs.end(), z, z + 2);
+        for (int j = 0; j < 3; ++j) P.pts.push_back(given ? x[j] : NAN);
+    }
+    L.n_obs = (int32_t)P.rows.size() - L.obs_off;
+    for (int k = 0; k < R.n_new; ++k) {
+        const double *a = R.new_z_last + 2 * k, *b = R.new_z + 2 * k;
+        if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(b[0]) || !std::isfinite(b[1]))
+            return loc_fail(h, P, "non-finite keypoint");
+        P.nzs.insert(P.nzs.end(), {a[0], a[1], b[0], b[1]});
+    }
+    return 0;
+}
+
+// the layout of n records with x / y / s caller words; grows h->pnp and stages the plan's sections on the host side
+static int loc_stage(Handle *h, LocPlan &P, size_t x, size_t y, size_t s) {
+    const size_t n = P.recs.size(), K = P.rows.size(), T = P.nzs.size() / 4, w8 = sizeof(double);
+    P.o_row = n * sizeof(BwLoc) / w8; P.o_z = P.o_row + (K + 1) / 2; P.o_imu = P.o_z + 2 * K;
+    P.o_nz = P.o_imu + (P.imu_staged ? (size_t)P.n_imu * kImuStride : 0); P.o_x = P.o_nz + 4 * T; P.o_fr = P.o_x + x;
+    P.o_pts = P.o_fr + 16 * n; P.o_out = P.o_pts + 3 * K; P.o_rho = P.o_out + 8 * n; P.o_next = P.o_rho + T;
+    P.o_val = P.o_next + T; P.o_y = P.o_val + (T + 7) / 8; P.o_args = P.o_y + y;
+    P.o_s = P.o_args + n * sizeof(PnpArgs) / w8; P.words = P.o_s + s;
+    TRY(reserve(h, h->pnp, P.words, kBoth));
+    double *st = h->pnp.h;
+    memcpy(st, P.recs.data(), sizeof(BwLoc) * n);
+    if (K) {
+        memcpy(st + P.o_row, P.rows.data(), sizeof(int32_t) * K);
+        memcpy(st + P.o_z, P.zs.data(), w8 * 2 * K);
+        memcpy(st + P.o_pts, P.pts.data(), w8 * 3 * K);
+    }
+    if (T) memcpy(st + P.o_nz, P.nzs.data(), w8 * 4 * T);
+    return 0;
+}
+
+// the device view of the staged plan
+static LocArgs loc_args(const Handle *h, const LocPlan &P, const pvio_b200_options *opt) {
+    double *d = h->pnp.d;
+    const SolveOptions so = solve_options(opt);
+    LocArgs L;
+    L.rec = reinterpret_cast<const BwLoc *>(d); L.row = reinterpret_cast<const int32_t *>(d + P.o_row); L.z = d + P.o_z;
+    L.imu = d + P.o_imu; L.nz = d + P.o_nz; L.frames = d + P.o_fr; L.pts = d + P.o_pts; L.out = d + P.o_out;
+    L.rho = d + P.o_rho; L.rho_next = d + P.o_next; L.valid = reinterpret_cast<uint8_t *>(d + P.o_val);
+    L.args = reinterpret_cast<PnpArgs *>(d + P.o_args);
+    L.max_iter = so.max_iter; L.radius0 = so.radius0;
+    return L;
+}
+
+// gather, PnP, triangulation: three launches whatever n is
+static int loc_launch(Handle *h, const LocArgs &L, int n) {
+    const BwArgs a = launch_args<BwArgs>(h);
+    bw_localize_gather_kernel<<<n, kLocGatherThreads, 0, h->stream>>>(a, L);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(launch_pnp(h, n, L.args));
+    CK(h, cudaGetLastError());
+    bw_localize_triangulate_kernel<<<n, kLocTriThreads, 0, h->stream>>>(a, L);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// after the download: record i's localize outputs into R
+static void loc_results(const Handle *h, const LocPlan &P, int i, size_t &k, const pvio_b200_window_localize &R, float ms) {
+    const double *st = h->pnp.h;
+    const size_t w8 = sizeof(double);
+    const uint8_t *val = reinterpret_cast<const uint8_t *>(st + P.o_val);
+    const BwLoc &L = P.recs[i];
+    memcpy(R.state, st + P.o_fr + 16 * (size_t)i, w8 * 16);
+    if (R.points_out) {
+        for (int j = 0; j < 3 * R.n_obs; ++j) R.points_out[j] = NAN;
+        for (int j = 0; j < L.n_obs; ++j, ++k) memcpy(R.points_out + 3 * P.from[k], st + P.o_pts + 3 * k, w8 * 3);
+    } else {
+        k += L.n_obs;
+    }
+    for (int t = 0; t < L.n_new; ++t) {
+        const size_t q = (size_t)L.new_off + t;
+        R.new_valid[t] = val[q];
+        R.new_inv_depth[t] = st[P.o_rho + q];
+        if (R.new_inv_depth_next) R.new_inv_depth_next[t] = st[P.o_next + q];
+    }
+    if (R.summary) {
+        const double *b = st + P.o_out + 8 * (size_t)i;
+        pvio_b200_summary &S = *R.summary;
+        memset(&S, 0, sizeof(S));
+        S.iterations = (int)b[0]; S.accepted_steps = (int)b[1]; S.termination = (int)b[2]; S.usable = (int)b[3];
+        S.initial_cost = b[4]; S.final_cost = b[5]; S.final_radius = b[6]; S.final_mu = b[7];
+        S.solve_seconds = ms * 1e-3;
+    }
+}
+
+// the localize half of a track_frame record
+static pvio_b200_window_localize localize_view(const pvio_b200_window_track_frame &R) {
+    pvio_b200_window_localize L{};
+    L.slot = R.slot; L.use_inertial = 1; L.state = R.state;
+    L.n_obs = R.n_obs; L.obs_track = R.obs_track; L.obs_z = R.obs_z; L.obs_point = R.obs_point; L.points_out = R.points_out;
+    L.n_new = R.n_new; L.new_z_last = R.new_z_last; L.new_z = R.new_z; L.new_valid = R.new_valid;
+    L.new_inv_depth = R.new_inv_depth; L.new_inv_depth_next = R.new_inv_depth_next; L.summary = R.summary;
+    return L;
+}
+
+static bool all_finite(const double *x, int64_t n) {
+    for (int64_t k = 0; k < n; ++k)
+        if (!std::isfinite(x[k])) return false;
+    return true;
 }
 
 // slot 0 as the single resident window (pvio_b200_window_*); null, with the error set, before pvio_b200_window_reset
@@ -1199,119 +1512,144 @@ int pvio_b200_batch_window_localize(pvio_b200_handle hh, int n, pvio_b200_window
     std::vector<int32_t> slots(n);
     for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
     TRY(check_slots(h, n, slots.data(), "batch_window_localize: bad slot list"));
-    // every record is checked against its slot's host mirror before anything is staged; the observations that take part
-    // are kept with the index they came from
-    std::vector<BwLoc> recs(n);
-    std::vector<int32_t> rows, from;
-    std::vector<double> zs, pts, nzs;
-    int n_imu = 0;
-    for (int i = 0; i < n; ++i) {
-        const pvio_b200_window_localize &R = records[i];
-        const WinSlot &s = h->slots[R.slot];
-        if (s.N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a window without frames");
-        if (!R.state || R.n_obs < 0 || R.n_new < 0 || (R.n_obs > 0 && (!R.obs_track || !R.obs_z)) ||
-            (R.n_new > 0 && (!R.new_z_last || !R.new_z || !R.new_valid || !R.new_inv_depth)))
-            return fail(h, PVIO_B200_EINVAL, "batch_window_localize: null array");
-        if (R.use_inertial && !R.imu_record)
-            return fail(h, PVIO_B200_EINVAL, "batch_window_localize: an inertial record needs the IMU record from the newest frame");
-        BwLoc &L = recs[i];
-        L = BwLoc{R.slot, s.N - 1, R.use_inertial ? 1 : 0, 0, (int32_t)rows.size(), R.use_inertial ? n_imu++ : -1,
-                  R.n_new, (int32_t)(nzs.size() / 4)};
-        const uint32_t newest = 1u << (s.N - 1);
-        std::vector<uint8_t> named(s.ids.size(), 0);
-        for (int k = 0; k < R.n_obs; ++k) {
-            const int r = find_row(s, R.obs_track[k]);
-            if (r < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: unknown or dead track");
-            if (named[r]) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a track named twice");
-            named[r] = 1;
-            const double *z = R.obs_z + 2 * k;
-            if (!std::isfinite(z[0]) || !std::isfinite(z[1])) return fail(h, PVIO_B200_EINVAL, "batch_window_localize: non-finite keypoint");
-            const double *x = R.obs_point ? R.obs_point + 3 * k : nullptr;
-            const bool given = x && std::isfinite(x[0]) && std::isfinite(x[1]) && std::isfinite(x[2]);
-            if (x && !given && !(std::isnan(x[0]) && std::isnan(x[1]) && std::isnan(x[2])))
-                return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a point row neither finite nor NaN");
-            if (!(s.mask[r] & newest)) continue;                              // pnp.cpp:58
-            if (!given && s.role[r] != -1)
-                return fail(h, PVIO_B200_EINVAL, "batch_window_localize: a plane track without its plane-cast point");
-            rows.push_back(r);
-            from.push_back(k);
-            zs.insert(zs.end(), z, z + 2);
-            for (int j = 0; j < 3; ++j) pts.push_back(given ? x[j] : NAN);
-        }
-        L.n_obs = (int32_t)rows.size() - L.obs_off;
-        for (int k = 0; k < R.n_new; ++k) {
-            const double *a = R.new_z_last + 2 * k, *b = R.new_z + 2 * k;
-            if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(b[0]) || !std::isfinite(b[1]))
-                return fail(h, PVIO_B200_EINVAL, "batch_window_localize: non-finite keypoint");
-            nzs.insert(nzs.end(), {a[0], a[1], b[0], b[1]});
-        }
-    }
-    // staging (doubles): upload records | rows | z | IMU records | new keypoints | states | points; download states |
-    // points | summary words | inverse depths | re-anchored inverse depths | valid bytes; then the PnP records (device)
-    const size_t K = rows.size(), T = nzs.size() / 4, w8 = sizeof(double);
-    const size_t o_row = (size_t)n * sizeof(BwLoc) / w8, o_z = o_row + (K + 1) / 2, o_imu = o_z + 2 * K;
-    const size_t o_nz = o_imu + (size_t)n_imu * kImuStride, o_fr = o_nz + 4 * T, o_pts = o_fr + 16 * (size_t)n;
-    const size_t o_out = o_pts + 3 * K, o_rho = o_out + 8 * (size_t)n, o_next = o_rho + T, o_val = o_next + T;
-    const size_t o_args = o_val + (T + 7) / 8, words = o_args + (size_t)n * sizeof(PnpArgs) / w8;
-    TRY(reserve(h, h->pnp, words, kBoth));
+    // every record is checked against its slot's host mirror before anything is staged
+    LocPlan P;
+    P.what = "batch_window_localize";
+    for (int i = 0; i < n; ++i) TRY(loc_add(h, P, records[i], true));
+    TRY(loc_stage(h, P, 0, 0, 0));
     double *st = h->pnp.h, *d = h->pnp.d;
-    memcpy(st, recs.data(), sizeof(BwLoc) * n);
-    if (K) {
-        memcpy(st + o_row, rows.data(), sizeof(int32_t) * K);
-        memcpy(st + o_z, zs.data(), w8 * 2 * K);
-        memcpy(st + o_pts, pts.data(), w8 * 3 * K);
-    }
-    if (T) memcpy(st + o_nz, nzs.data(), w8 * 4 * T);
+    const size_t w8 = sizeof(double);
     for (int i = 0; i < n; ++i) {
-        memcpy(st + o_fr + 16 * (size_t)i, records[i].state, w8 * 16);
-        if (recs[i].inertial) memcpy(st + o_imu + (size_t)recs[i].imu_off * kImuStride, records[i].imu_record, w8 * kImuStride);
+        memcpy(st + P.o_fr + 16 * (size_t)i, records[i].state, w8 * 16);
+        if (P.recs[i].inertial)
+            memcpy(st + P.o_imu + (size_t)P.recs[i].imu_off * kImuStride, records[i].imu_record, w8 * kImuStride);
     }
-    CK(h, cudaMemcpyAsync(d, st, w8 * o_out, cudaMemcpyHostToDevice, h->stream));
-    const SolveOptions so = solve_options(opt);
-    LocArgs L;
-    L.rec = reinterpret_cast<const BwLoc *>(d); L.row = reinterpret_cast<const int32_t *>(d + o_row); L.z = d + o_z;
-    L.imu = d + o_imu; L.nz = d + o_nz; L.frames = d + o_fr; L.pts = d + o_pts; L.out = d + o_out; L.rho = d + o_rho;
-    L.rho_next = d + o_next; L.valid = reinterpret_cast<uint8_t *>(d + o_val); L.args = reinterpret_cast<PnpArgs *>(d + o_args);
-    L.max_iter = so.max_iter; L.radius0 = so.radius0;
-    const BwArgs a = launch_args<BwArgs>(h);
-    bw_localize_gather_kernel<<<n, kLocGatherThreads, 0, h->stream>>>(a, L);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    TRY(launch_pnp(h, n, L.args));
-    CK(h, cudaGetLastError());
-    bw_localize_triangulate_kernel<<<n, kLocTriThreads, 0, h->stream>>>(a, L);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(st + o_fr, d + o_fr, w8 * (o_args - o_fr), cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(d, st, w8 * P.o_out, cudaMemcpyHostToDevice, h->stream));
+    TRY(loc_launch(h, loc_args(h, P, opt), n));
+    CK(h, cudaMemcpyAsync(st + P.o_fr, d + P.o_fr, w8 * (P.o_args - P.o_fr), cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-    const uint8_t *val = reinterpret_cast<const uint8_t *>(st + o_val);
     size_t k = 0;
+    for (int i = 0; i < n; ++i) loc_results(h, P, i, k, records[i], ms);
+    return 0;
+}
+
+int pvio_b200_batch_window_track_frame(pvio_b200_handle hh, int n, pvio_b200_window_track_frame *records,
+                                       const pvio_b200_options *opt) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_track_frame: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_track_frame: bad slot list"));
+    // every record is checked before anything is staged: its localize half as localize checks it, then the rest
+    LocPlan P;
+    P.what = "batch_window_track_frame";
+    P.imu_staged = false;                     // the step-1 records are computed on the device
+    std::vector<BwTrack> trs(n);
+    std::vector<BwTrackJob> jobs;
+    std::vector<int32_t> kf_row;
+    std::vector<double> kf_z;
+    size_t rows = 0, par = 0;
     for (int i = 0; i < n; ++i) {
-        pvio_b200_window_localize &R = records[i];
-        const BwLoc &L = recs[i];
-        memcpy(R.state, st + o_fr + 16 * (size_t)i, w8 * 16);
-        if (R.points_out) {
-            for (int j = 0; j < 3 * R.n_obs; ++j) R.points_out[j] = NAN;
-            for (int j = 0; j < L.n_obs; ++j, ++k) memcpy(R.points_out + 3 * from[k], st + o_pts + 3 * k, w8 * 3);
-        } else {
-            k += L.n_obs;
+        const pvio_b200_window_track_frame &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (!s.inertial) return loc_fail(h, P, "the window carries no motion states");
+        TRY(loc_add(h, P, localize_view(R), false));
+        if (!R.samples || !R.noise_cov || !R.imu_record || !R.keyframe || !R.skipped_frames) return loc_fail(h, P, "null array");
+        if (R.n_samples < 1)
+            return loc_fail(h, P, "a frame without IMU samples (integrate() returns false, preintegrator.cpp:86)");
+        if (R.newest_is_keyframe != 0 && R.newest_is_keyframe != 1) return loc_fail(h, P, "newest_is_keyframe not 0 or 1");
+        const bool merged = R.newest_is_keyframe == 0;
+        if (merged && s.N < 2) return loc_fail(h, P, "a non-keyframe newest frame without a keyframe before it");
+        if (merged && (R.n_merge < 1 || !R.merge_samples)) return loc_fail(h, P, "a non-keyframe newest frame without its samples");
+        if (!merged && (R.n_merge != 0 || R.merge_samples)) return loc_fail(h, P, "a merge list with a keyframe newest frame");
+        if (!all_finite(R.samples, 7 * (int64_t)R.n_samples) || (merged && !all_finite(R.merge_samples, 7 * (int64_t)R.n_merge)))
+            return loc_fail(h, P, "non-finite sample");
+        if (!std::isfinite(R.t_end) || !all_finite(R.noise_cov, 36) || !std::isfinite(R.cx) || !std::isfinite(R.cy))
+            return loc_fail(h, P, "non-finite t_end, noise or principal point");
+        if (*R.skipped_frames < 0) return loc_fail(h, P, "negative skipped_frames");
+        BwTrack &t = trs[i];
+        t = BwTrack{merged ? 1 : 0, merged ? s.N - 2 : s.N - 1, 0, (int32_t)kf_row.size(), merged ? 0 : 1, 0,
+                    *R.skipped_frames, (int32_t)i * kImuAux, R.cx, R.cy};
+        const uint32_t fi = 1u << t.frame_i;
+        for (int k = 0; k < R.n_obs; ++k) {                    // loc_add found every track live and named once
+            const int r = find_row(s, R.obs_track[k]);
+            if (!(s.mask[r] & fi)) continue;
+            kf_row.push_back(r);
+            kf_z.insert(kf_z.end(), R.obs_z + 2 * k, R.obs_z + 2 * k + 2);
         }
-        for (int t = 0; t < L.n_new; ++t) {
-            const size_t q = (size_t)L.new_off + t;
-            R.new_valid[t] = val[q];
-            R.new_inv_depth[t] = st[o_rho + q];
-            if (R.new_inv_depth_next) R.new_inv_depth_next[t] = st[o_next + q];
-        }
-        if (R.summary) {
-            const double *b = st + o_out + 8 * (size_t)i;
-            pvio_b200_summary &S = *R.summary;
-            memset(&S, 0, sizeof(S));
-            S.iterations = (int)b[0]; S.accepted_steps = (int)b[1]; S.termination = (int)b[2]; S.usable = (int)b[3];
-            S.initial_cost = b[4]; S.final_cost = b[5]; S.final_radius = b[6]; S.final_mu = b[7];
-            S.solve_seconds = ms * 1e-3;
-        }
+        t.n_kf = (int32_t)kf_row.size() - t.kf_off;
+        t.par_off = (int32_t)par;
+        par += t.n_kf + (t.use_new ? R.n_new : 0);
+        const size_t b = rows + (merged ? R.n_merge : 0), e = b + R.n_samples;
+        if (e > (size_t)INT32_MAX || par > (size_t)INT32_MAX) return loc_fail(h, P, "too many samples or pairs in one call");
+        jobs.push_back(BwTrackJob{i, (int32_t)b, (int32_t)e, 0});
+        if (merged) jobs.push_back(BwTrackJob{i, (int32_t)rows, (int32_t)e, 1});
+        rows = e;
+    }
+    // the caller's words: upload track records | jobs | observed pairs' rows | their keypoints | samples | t_end and
+    // noise; download the edit's IMU records | predicted states | keyframe words; scratch step-1 records | parallaxes
+    const size_t w8 = sizeof(double), J = jobs.size(), Kf = kf_row.size();
+    const size_t x_tr = 0, x_job = x_tr + n * sizeof(BwTrack) / w8, x_row = x_job + J * sizeof(BwTrackJob) / w8;
+    const size_t x_z = x_row + (Kf + 1) / 2, x_smp = x_z + 2 * Kf, x_aux = x_smp + 7 * rows, x = x_aux + (size_t)n * kImuAux;
+    const size_t y_rec = 0, y_pred = y_rec + (size_t)n * kImuStride, y_kf = y_pred + 16 * (size_t)n, y = y_kf + 4 * (size_t)n;
+    const size_t s_rec = 0, s_par = s_rec + (size_t)n * kImuStride, sw = s_par + par;
+    TRY(loc_stage(h, P, x, y, sw));
+    double *st = h->pnp.h, *d = h->pnp.d, *sx = st + P.o_x;
+    memcpy(sx + x_tr, trs.data(), sizeof(BwTrack) * n);
+    memcpy(sx + x_job, jobs.data(), sizeof(BwTrackJob) * J);
+    if (Kf) {
+        memcpy(sx + x_row, kf_row.data(), sizeof(int32_t) * Kf);
+        memcpy(sx + x_z, kf_z.data(), w8 * 2 * Kf);
+    }
+    for (int i = 0; i < n; ++i) {
+        double *a = sx + x_aux + (size_t)i * kImuAux;
+        a[0] = records[i].t_end;
+        memcpy(a + 1, records[i].noise_cov, w8 * 36);
+    }
+    for (const BwTrackJob &j : jobs) {                          // merge_samples ++ samples, back to back per record
+        if (j.merged) continue;
+        const pvio_b200_window_track_frame &R = records[j.rec];
+        memcpy(sx + x_smp + 7 * (size_t)j.begin, R.samples, w8 * 7 * R.n_samples);
+        if (trs[j.rec].merged) memcpy(sx + x_smp + 7 * ((size_t)j.begin - R.n_merge), R.merge_samples, w8 * 7 * R.n_merge);
+    }
+    CK(h, cudaMemcpyAsync(d, st, w8 * P.o_out, cudaMemcpyHostToDevice, h->stream));
+    const LocArgs L = loc_args(h, P, opt);
+    TrackArgs T;
+    double *dx = d + P.o_x, *dy = d + P.o_y, *ds = d + P.o_s;
+    T.tr = reinterpret_cast<const BwTrack *>(dx + x_tr); T.job = reinterpret_cast<const BwTrackJob *>(dx + x_job);
+    T.kf_row = reinterpret_cast<const int32_t *>(dx + x_row); T.kf_z = dx + x_z; T.smp = dx + x_smp; T.aux = dx + x_aux;
+    T.rec_out = dy + y_rec; T.pred = dy + y_pred; T.kfo = dy + y_kf; T.rec1 = ds + s_rec; T.par = ds + s_par;
+    T.n_jobs = (int)J;
+    LocArgs Li = L;
+    Li.imu = T.rec1;                          // the PnP reads the step-1 records (imu_off = record index)
+    const BwArgs a = launch_args<BwArgs>(h);
+    bw_track_integrate_kernel<<<(int)((J + kBwImuWarps - 1) / kBwImuWarps), 32 * kBwImuWarps, 0, h->stream>>>(a, Li, T);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(loc_launch(h, Li, n));
+    bw_track_keyframe_kernel<<<n, kBwThreads, 0, h->stream>>>(a, Li, T);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(st + P.o_fr, d + P.o_fr, w8 * (P.o_args - P.o_fr), cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+    size_t k = 0;
+    const double *sy = st + P.o_y;
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_window_track_frame &R = records[i];
+        loc_results(h, P, i, k, localize_view(R), ms);
+        memcpy(R.imu_record, sy + y_rec + (size_t)i * kImuStride, w8 * kImuStride);
+        if (R.predicted) memcpy(R.predicted, sy + y_pred + 16 * (size_t)i, w8 * 16);
+        const double *o = sy + y_kf + 4 * (size_t)i;
+        *R.keyframe = o[0] != 0.0 ? 1 : 0;
+        if (R.parallax) *R.parallax = o[1];
+        if (R.n_parallax) *R.n_parallax = (int32_t)o[2];
+        *R.skipped_frames = (int32_t)o[3];
     }
     return 0;
 }
