@@ -200,6 +200,18 @@ def _ptr(a, ctype):
     return a.ctypes.data_as(C.POINTER(ctype))
 
 
+def window_constants(win):
+    """A CWindow holding only the constants of win (use_inertial, extrinsics, noise model, intrinsics); no arrays."""
+    cw = CWindow()
+    cw.use_inertial = 1 if win.use_inertial else 0
+    cw.cam_q_cs[:] = list(win.cam_q_cs); cw.cam_p_cs[:] = list(win.cam_p_cs)
+    cw.imu_q_cs[:] = list(win.imu_q_cs); cw.imu_p_cs[:] = list(win.imu_p_cs)
+    cw.sqrt_inv_cov[:] = list(np.asarray(win.sqrt_inv_cov, dtype=np.float64).reshape(4))
+    cw.fx, cw.fy, cw.cauchy_a = win.K_fx, win.K_fy, win.cauchy_a
+    cw.plane_sqrt_inv_cov = getattr(win, "plane_sqrt_inv_cov", 0.0)
+    return cw
+
+
 class PackedArgs:
     """Keeps the contiguous NumPy arrays alive while a CWindow / CState points into them."""
 
@@ -210,16 +222,9 @@ class PackedArgs:
             k[name] = np.ascontiguousarray(a, dtype=dt)
             return k[name]
 
-        cw = CWindow()
+        cw = window_constants(win)
         cw.n_frames, cw.n_landmarks, cw.n_obs = win.N, win.M, win.K
-        cw.use_inertial = 1 if win.use_inertial else 0
         cw.frame_fixed = _ptr(arr("fixed", win.frame_fixed, np.uint8), C.c_uint8)
-        cw.cam_q_cs[:] = list(win.cam_q_cs)
-        cw.cam_p_cs[:] = list(win.cam_p_cs)
-        cw.imu_q_cs[:] = list(win.imu_q_cs)
-        cw.imu_p_cs[:] = list(win.imu_p_cs)
-        cw.sqrt_inv_cov[:] = list(np.asarray(win.sqrt_inv_cov, dtype=np.float64).reshape(4))
-        cw.fx, cw.fy, cw.cauchy_a = win.K_fx, win.K_fy, win.cauchy_a
         cw.lm_anchor = _ptr(arr("anchor", win.lm_anchor, np.int32), C.c_int32)
         cw.lm_z_ref = _ptr(arr("zref", win.lm_z_ref, np.float64), C.c_double)
         cw.lm_obs_begin = _ptr(arr("ob", win.lm_obs_begin, np.int32), C.c_int32)
@@ -253,7 +258,6 @@ class PackedArgs:
             cw.prior_e = _ptr(arr("pe", win.prior_e, np.float64), C.c_double)
             cw.prior_state0 = _ptr(arr("px0", x0, np.float64), C.c_double)
         cw.n_planes = win.n_planes
-        cw.plane_sqrt_inv_cov = win.plane_sqrt_inv_cov
         cw.n_plane_tracks = win.n_ptracks
         if win.n_ptracks > 0:
             pp = np.concatenate([win.plane_normal, win.plane_distance[:, None]], axis=1)

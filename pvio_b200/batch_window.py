@@ -26,15 +26,7 @@ def _argtypes(L):
     L.pvio_b200_batch_window_track_frame.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowTrackFrame), C.POINTER(_lib.COptions)]
 
 
-def _constants(win):
-    cw = _lib.CWindow()
-    cw.use_inertial = 1 if win.use_inertial else 0
-    cw.cam_q_cs[:] = list(win.cam_q_cs); cw.cam_p_cs[:] = list(win.cam_p_cs)
-    cw.imu_q_cs[:] = list(win.imu_q_cs); cw.imu_p_cs[:] = list(win.imu_p_cs)
-    cw.sqrt_inv_cov[:] = list(np.asarray(win.sqrt_inv_cov, dtype=np.float64).reshape(4))
-    cw.fx, cw.fy, cw.cauchy_a = win.K_fx, win.K_fy, win.cauchy_a
-    cw.plane_sqrt_inv_cov = getattr(win, "plane_sqrt_inv_cov", 0.0)
-    return cw
+_constants = _lib.window_constants            # the CWindow a reset takes: the window's constants only
 
 
 class Edit:

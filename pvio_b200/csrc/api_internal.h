@@ -153,7 +153,8 @@ struct BatchWindows {
     DevBuf<int8_t> trole;                        // [W][Mcap] role of each row (WinSlot::role)
     DevBuf<double> tplane;                       // [W][Pcap][4] plane parameters (normal, distance)
     DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
-    DevBuf<uint8_t> stage;                       // both sides, grown: the one upload / download of a call
+    DevBuf<uint8_t> stage;                       // both sides, grown: every call's staging (batch_window.cu: Stage) --
+                                                 // upload | in/out | download | device-only scratch
     // IMU samples of the factors named by set_imu, indexed like imu_data (factor k couples frames k, k + 1); allocated
     // with the first set_imu, imu_s grown to the longest sample list seen
     int Scap = 0;                                // samples per factor in imu_s
@@ -239,8 +240,8 @@ struct Handle {
     KltBatchState kltb;                           // klt.cu: the batched tracker, independent of klt
     DevBuf<double> marg;                          // ba_marg.cu: scratch blocks of the marginaliser's dense kernels
     FmState fm;
-    DevBuf<double> pnp;                           // pnp.cu: both sides, grown on demand to the largest batch (records,
-                                                  // points, IMU records, frames) seen
+    DevBuf<double> pnp;                           // pnp.cu's own: both sides, grown on demand to the largest batch
+                                                  // (records, points, IMU records, frames) seen
     BatchWindows bw;                              // batch_window.cu (empty until the first pvio_b200_batch_window_reset)
 };
 

@@ -47,8 +47,11 @@ struct BwLayout { int32_t slot, N, T, fixed, n_prior, inertial, n_planes, smax; 
 struct BwDl { int32_t slot, N, T, pad; int64_t off; };                  // download: bytes into the result area
 struct BwPlanes { int32_t slot, n_planes, n_set, set_off, param_off, pad; };   // one set_planes record (n_planes < 0: keep)
 struct BwRole { int32_t row, role; double rho; };                       // rho NaN: keep the row's inverse depth
-struct BwImu { int32_t slot, factor, n, off; };   // a factor with samples: n rows at row off (staged rows in set_imu,
-                                                  // rows of the sample store in a solve's work list)
+struct BwImu {                                    // a factor with samples: n rows at row off (staged rows in set_imu,
+    int32_t slot, factor, n, off;                 // rows of the sample store in a solve's work list)
+    __device__ int begin() const { return off; }
+    __device__ int end() const { return off + n; }
+};
 constexpr int kImuAux = 37;                                             // per factor: t_end, noise [4][9]
 
 // the handle's arrays (the plane tables null until a slot has plane tracks), the track table and the post-pass results
@@ -356,6 +359,37 @@ __device__ void bw_cam_pose(const double *fs, const WinConst &c, double *qc, dou
     bw_qrot(fs, c.cam_p, t);
     for (int i = 0; i < 3; ++i) pc[i] = fs[4 + i] + t[i];
 }
+// the world point at inverse depth rho along keypoint (zx, zy) of the camera at pose (qc, pc) (Track::get_landmark_point)
+__device__ __forceinline__ void bw_world_point(const double *qc, const double *pc, double zx, double zy, double rho,
+                                               double *x) {
+    const double ray[3] = {zx / rho, zy / rho, 1.0 / rho};
+    double y[3];
+    bw_qrot(qc, ray, y);
+    for (int i = 0; i < 3; ++i) x[i] = y[i] + pc[i];
+}
+// the inverse depth of world point x in the camera at pose (qc, pc)
+__device__ __forceinline__ double bw_inv_depth(const double *qc, const double *pc, const double *x) {
+    const double qi[4] = {-qc[0], -qc[1], -qc[2], qc[3]};
+    double d[3], y[3];
+    for (int i = 0; i < 3; ++i) d[i] = x[i] - pc[i];
+    bw_qrot(qi, d, y);
+    return 1.0 / y[2];
+}
+
+// rows [0, n) of p down by one row over the CTA, chunk by chunk, each chunk read completely before it is written (every
+// chunk reads above every address an earlier chunk wrote).  kW > 0: rows of kW doubles back to back; kW == 0: rows of w
+// doubles at stride s.
+template <int kW>
+__device__ __forceinline__ void bw_shift_down(double *p, int n, int w = kW, int s = kW) {
+    const int ne = n * w;
+    for (int i0 = 0; i0 < ne; i0 += kBwThreads) {
+        const int i = i0 + threadIdx.x, f = kW ? 0 : i / w, r = i - f * w;
+        const double v = i < ne ? p[kW ? (size_t)(kW + i) : (size_t)(f + 1) * s + r] : 0.0;
+        __syncthreads();
+        if (i < ne) p[kW ? (size_t)i : (size_t)f * s + r] = v;
+        __syncthreads();
+    }
+}
 
 // Map::marginalize_frame(0) after the marginaliser, one CTA per slot (L.N, L.T: the window BEFORE the drop): a track
 // anchored in the victim is re-anchored in its next frame from the current states (track.cpp:42-49, quirk Q5), the
@@ -375,58 +409,22 @@ __global__ void __launch_bounds__(kBwThreads) bw_drop_kernel(BwArgs a, const BwL
             double qa[4], pa[3], qn[4], pn[3];
             bw_cam_pose(fr, c, qa, pa);
             bw_cam_pose(fr + nx * kFrameStride, c, qn, pn);
-            const double rho = a.trho[base + r];
-            const double ray[3] = {z[0].x / rho, z[0].y / rho, 1.0 / rho};
-            double x[3], d[3], y[3];
-            bw_qrot(qa, ray, x);
-            for (int i = 0; i < 3; ++i) d[i] = x[i] + pa[i] - pn[i];
-            const double qc[4] = {-qn[0], -qn[1], -qn[2], qn[3]};
-            bw_qrot(qc, d, y);
-            a.trho[base + r] = 1.0 / y[2];
+            double x[3];
+            bw_world_point(qa, pa, z[0].x, z[0].y, a.trho[base + r], x);
+            a.trho[base + r] = bw_inv_depth(qn, pn, x);
         }
         for (int f = 0; f + 1 < N; ++f) z[f] = z[f + 1];
         a.tmask[base + r] = m >> 1;
     }
     __syncthreads();
-    const int nf = (N - 1) * kFrameStride;
-    for (int i0 = 0; i0 < nf; i0 += kBwThreads) {
-        const int i = i0 + threadIdx.x;
-        const double v = i < nf ? fr[kFrameStride + i] : 0.0;
-        __syncthreads();
-        if (i < nf) fr[i] = v;
-        __syncthreads();
-    }
+    bw_shift_down<kFrameStride>(fr, N - 1);
     if (L.inertial && N > 2) {
-        double *rec = a.imu_data + (size_t)w * a.Ncap * kImuStride;
-        const int ni = (N - 2) * kImuStride;
-        for (int i0 = 0; i0 < ni; i0 += kBwThreads) {
-            const int i = i0 + threadIdx.x;
-            const double v = i < ni ? rec[kImuStride + i] : 0.0;
-            __syncthreads();
-            if (i < ni) rec[i] = v;
-            __syncthreads();
-        }
+        bw_shift_down<kImuStride>(a.imu_data + (size_t)w * a.Ncap * kImuStride, N - 2);
         if (L.smax > 0) {                     // the samples, t_end and noise of the factors that hold some
-            double *aux = a.imu_aux + (size_t)w * a.Ncap * kImuAux;
-            const int na = (N - 2) * kImuAux;
-            for (int i0 = 0; i0 < na; i0 += kBwThreads) {
-                const int i = i0 + threadIdx.x;
-                const double v = i < na ? aux[kImuAux + i] : 0.0;
-                __syncthreads();
-                if (i < na) aux[i] = v;
-                __syncthreads();
-            }
-            // factor f + 1 -> f, rows [0, smax) of each: every chunk reads above every address an earlier chunk wrote
-            const int rs = L.smax * 7, fs = a.Scap * 7;
-            double *smp = a.imu_s + (size_t)w * a.Ncap * fs;
-            const int ns = (N - 2) * rs;
-            for (int i0 = 0; i0 < ns; i0 += kBwThreads) {
-                const int i = i0 + threadIdx.x, f = i / rs, r = i - f * rs;
-                const double v = i < ns ? smp[(size_t)(f + 1) * fs + r] : 0.0;
-                __syncthreads();
-                if (i < ns) smp[(size_t)f * fs + r] = v;
-                __syncthreads();
-            }
+            bw_shift_down<kImuAux>(a.imu_aux + (size_t)w * a.Ncap * kImuAux, N - 2);
+            // factor f + 1 -> f, rows [0, smax) of each
+            const int fs = a.Scap * 7;
+            bw_shift_down<0>(a.imu_s + (size_t)w * a.Ncap * fs, N - 2, L.smax * 7, fs);
         }
     }
     bw_compact(a, w, T, sh);
@@ -443,14 +441,15 @@ __global__ void __launch_bounds__(kBwThreads) bw_set_imu_kernel(BwArgs a, const 
     for (int i = threadIdx.x; i < kImuAux; i += kBwThreads) a.imu_aux[F * kImuAux + i] = aux[(size_t)blockIdx.x * kImuAux + i];
 }
 
-// a factor of a slot as imu_integrate_warp reads it: rows J.off .. J.off + J.n - 1 of the slots' sample store (the
-// factor's rows start at its index times Scap), t_end and noise in its aux record
-struct BwSlotFactor {
-    const BwImu &J;
+// a factor as imu_integrate_warp reads it: the sample rows [J.begin(), J.end()) of a job, t_end in aux[0], the noise at
+// aux + 1, its record r.  The rows are read from the job where imu_integrate_warp asks for them.
+template <typename Job>
+struct BwFactor {
+    const Job &J;
     const double *samples, *noise, *aux;
     double *r;
-    __device__ int begin() const { return J.off; }
-    __device__ int end() const { return J.off + J.n; }
+    __device__ int begin() const { return J.begin(); }
+    __device__ int end() const { return J.end(); }
     __device__ double t_end() const { return aux[0]; }
     __device__ double *rec() const { return r; }
 };
@@ -470,7 +469,7 @@ __global__ void __launch_bounds__(32 * kBwImuWarps) bw_reintegrate_kernel(BwArgs
     const double *x = a.frames + F * kFrameStride;
     const double bg[3] = {x[10], x[11], x[12]}, ba[3] = {x[13], x[14], x[15]};
     const double *aux = a.imu_aux + F * kImuAux;
-    imu_integrate_warp(sm[wv], lane, BwSlotFactor{J, a.imu_s, aux + 1, aux, a.imu_data + F * kImuStride}, bg, ba);
+    imu_integrate_warp(sm[wv], lane, BwFactor<BwImu>{J, a.imu_s, aux + 1, aux, a.imu_data + F * kImuStride}, bg, ba);
 }
 
 // One CTA per slot: its N - 1 IMU records at dl.off (bytes)
@@ -481,21 +480,32 @@ __global__ void __launch_bounds__(kBwThreads) bw_imu_records_kernel(BwArgs a, co
     for (int i = threadIdx.x; i < (d.N - 1) * kImuStride; i += kBwThreads) o[i] = rec[i];
 }
 
-// One CTA per slot: frames, then per row inverse depth, quality, id, anchor, observation count, valid -- packed at dl.off
+// one slot's record of pvio_b200_batch_window_download at byte b: its N frames, then per row of its T rows inverse depth,
+// quality, id, anchor, observation count, valid; bytes: the record's size, rounded up to 16
+struct BwDlRec {
+    double *fo, *ro, *qo;
+    int32_t *io, *ao, *no;
+    uint8_t *vo;
+    __host__ __device__ BwDlRec(uint8_t *b, int N, int T)
+        : fo(reinterpret_cast<double *>(b)), ro(fo + (size_t)N * kFrameStride), qo(ro + T),
+          io(reinterpret_cast<int32_t *>(qo + T)), ao(io + T), no(ao + T), vo(reinterpret_cast<uint8_t *>(no + T)) {}
+    __host__ __device__ static int64_t bytes(int N, int T) {
+        return ((int64_t)(N * kFrameStride + 2 * T) * 8 + (int64_t)T * 13 + 15) & ~(int64_t)15;
+    }
+};
+
+// One CTA per slot: its download record at dl.off
 __global__ void __launch_bounds__(kBwThreads) bw_download_kernel(BwArgs a, const BwDl *dls, uint8_t *outb) {
     const BwDl d = dls[blockIdx.x];
     const int w = d.slot, N = d.N, T = d.T;
     const size_t base = (size_t)w * a.Mcap;
-    double *fo = reinterpret_cast<double *>(outb + d.off);
-    double *ro = fo + (size_t)N * kFrameStride, *qo = ro + T;
-    int32_t *io = reinterpret_cast<int32_t *>(qo + T), *ao = io + T, *no = ao + T;
-    uint8_t *vo = reinterpret_cast<uint8_t *>(no + T);
+    const BwDlRec o(outb + d.off, N, T);
     const double *fr = a.frames + (size_t)w * a.Ncap * kFrameStride;
-    for (int i = threadIdx.x; i < N * kFrameStride; i += kBwThreads) fo[i] = fr[i];
+    for (int i = threadIdx.x; i < N * kFrameStride; i += kBwThreads) o.fo[i] = fr[i];
     for (int r = threadIdx.x; r < T; r += kBwThreads) {
         const uint32_t m = a.tmask[base + r];
-        ro[r] = a.trho[base + r]; qo[r] = a.tqual[base + r];
-        io[r] = a.tid[base + r]; ao[r] = m ? __ffs(m) - 1 : -1; no[r] = __popc(m); vo[r] = a.tvalid[base + r];
+        o.ro[r] = a.trho[base + r]; o.qo[r] = a.tqual[base + r];
+        o.io[r] = a.tid[base + r]; o.ao[r] = m ? __ffs(m) - 1 : -1; o.no[r] = __popc(m); o.vo[r] = a.tvalid[base + r];
     }
 }
 
@@ -540,11 +550,9 @@ __global__ void __launch_bounds__(kLocGatherThreads) bw_localize_gather_kernel(B
         const int an = __ffs(a.tmask[R]) - 1;
         const double2 z = a.tz[R * a.Ncap + an];
         const double rho = a.trho[R];
-        double qc[4], pc[3], y[3];
+        double qc[4], pc[3];
         bw_cam_pose(fr + an * kFrameStride, c, qc, pc);
-        const double ray[3] = {z.x / rho, z.y / rho, 1.0 / rho};
-        bw_qrot(qc, ray, y);
-        for (int j = 0; j < 3; ++j) x[j] = y[j] + pc[j];
+        bw_world_point(qc, pc, z.x, z.y, rho, x);
     }
     if (threadIdx.x == 0) {
         PnpArgs p{};                      // what batch_pnp_solve_impl stages for the same problem
@@ -593,7 +601,6 @@ __global__ void __launch_bounds__(kLocTriThreads) bw_localize_triangulate_kernel
     bw_cam_pose(L.frames + kFrameStride * (size_t)blockIdx.x, c, qn, pn);
     loc_camera_matrix(qa, pa, Pa);
     loc_camera_matrix(qn, pn, Pn);
-    const double qai[4] = {-qa[0], -qa[1], -qa[2], qa[3]}, qni[4] = {-qn[0], -qn[1], -qn[2], qn[3]};
     for (int t = threadIdx.x; t < r.n_new; t += kLocTriThreads) {
         const int k = r.new_off + t;
         const double *nz = L.nz + 4 * (size_t)k;
@@ -601,16 +608,10 @@ __global__ void __launch_bounds__(kLocTriThreads) bw_localize_triangulate_kernel
         const bool ok = tri_point_scored(LocViews{Pa, Pn, nz}, 0, 2, p, score);
         double rho = NAN, rho_next = NAN;
         if (ok) {
-            double d[3], y[3];
-            for (int j = 0; j < 3; ++j) d[j] = p[j] - pa[j];
-            bw_qrot(qai, d, y);
-            rho = 1.0 / y[2];
-            const double ray[3] = {nz[0] / rho, nz[1] / rho, 1.0 / rho};
+            rho = bw_inv_depth(qa, pa, p);
             double x[3];
-            bw_qrot(qa, ray, x);
-            for (int j = 0; j < 3; ++j) d[j] = x[j] + pa[j] - pn[j];
-            bw_qrot(qni, d, y);
-            rho_next = 1.0 / y[2];
+            bw_world_point(qa, pa, nz[0], nz[1], rho, x);
+            rho_next = bw_inv_depth(qn, pn, x);
         }
         L.valid[k] = ok ? 1 : 0;
         L.rho[k] = rho;
@@ -623,8 +624,12 @@ __global__ void __launch_bounds__(kLocTriThreads) bw_localize_triangulate_kernel
 // at aux_off (kImuAux doubles), frame_i of the keyframe check, the observed tracks with a keypoint in frame_i (rows and
 // new-frame keypoints at kf_off), whether the new tracks count, where its parallax list starts in the scratch
 struct BwTrack { int32_t merged, frame_i, n_kf, kf_off, use_new, par_off, skipped, aux_off; double cx, cy; };
-// one warp job of the integrate launch: record `rec`, staged sample rows [begin, end); merged: the merged list
-struct BwTrackJob { int32_t rec, begin, end, merged; };
+// one warp job of the integrate launch: record `rec`, staged sample rows [b, e); merged: the merged list
+struct BwTrackJob {
+    int32_t rec, b, e, merged;
+    __device__ int begin() const { return b; }
+    __device__ int end() const { return e; }
+};
 static_assert(sizeof(BwTrack) % sizeof(double) == 0 && sizeof(BwTrackJob) % sizeof(double) == 0,
               "records are staged as whole 8-byte words");
 
@@ -643,17 +648,6 @@ struct TrackArgs {
     int n_jobs;
 };
 
-// a job as imu_integrate_warp reads it
-struct BwTrackFactor {
-    const BwTrackJob &J;
-    const double *samples, *noise, *aux;
-    double *r;
-    __device__ int begin() const { return J.begin; }
-    __device__ int end() const { return J.end; }
-    __device__ double t_end() const { return aux[0]; }
-    __device__ double *rec() const { return r; }
-};
-
 // One warp per job: PreIntegrator::integrate(t, bg, ba, true, true) at the biases of the slot's newest frame
 // (sliding_window_tracker.cpp:77, 118) -- the arithmetic of pvio_b200_preintegrate (imu.cuh); after the step-1 job,
 // PreIntegrator::predict (preintegrator.cpp:102-109) into the PnP's initial state
@@ -668,7 +662,7 @@ __global__ void __launch_bounds__(32 * kBwImuWarps) bw_track_integrate_kernel(Bw
     const double bg[3] = {x[10], x[11], x[12]}, ba[3] = {x[13], x[14], x[15]};
     const double *aux = T.aux + (size_t)T.tr[J.rec].aux_off;
     double *rec = (J.merged ? T.rec_out : T.rec1) + (size_t)J.rec * kImuStride;
-    imu_integrate_warp(sm[wv], lane, BwTrackFactor{J, T.smp, aux + 1, aux, rec}, bg, ba);
+    imu_integrate_warp(sm[wv], lane, BwFactor<BwTrackJob>{J, T.smp, aux + 1, aux, rec}, bg, ba);
     if (J.merged) return;
     __syncwarp();
     if (!T.tr[J.rec].merged)                                 // the edit takes the step-1 record
@@ -818,15 +812,54 @@ static int ensure_imu_store(Handle *h, int S) {
     return 0;
 }
 
-// byte buffer of one call's upload, every section 8-byte aligned
-struct Packer {
-    std::vector<uint8_t> buf;
+// One call's staging in BatchWindows::stage.  Sections are declared by kind and size, then laid out kind after kind in
+// the order of Kind, each 8-byte aligned, so that the call copies upload + in/out to the device in one copy and in/out +
+// download back in one copy; scratch stays on the device.
+struct Stage {
+    enum Kind { kUp, kInOut, kDown, kScratch, kKinds };
     template <typename T>
-    size_t put(const T *p, size_t n) {
-        const size_t off = (buf.size() + 7) & ~(size_t)7;
-        buf.resize(off + sizeof(T) * n);
-        if (n) memcpy(buf.data() + off, p, sizeof(T) * n);
-        return off;
+    struct Sec { int i; };
+    struct Entry { Kind kind; size_t bytes; const void *src; size_t off; };
+    std::vector<Entry> secs;
+    size_t end[kKinds] = {};                  // after place: the end of each kind's sections
+    uint8_t *hp = nullptr, *dp = nullptr;
+
+    // n elements of kind k; src (n elements, or null): what place copies into the section
+    template <typename T>
+    Sec<T> add(Kind k, size_t n, const T *src = nullptr) {
+        secs.push_back(Entry{k, sizeof(T) * n, src, 0});
+        return Sec<T>{(int)secs.size() - 1};
+    }
+    template <typename T>
+    Sec<T> up(const std::vector<T> &v) { return add(kUp, v.size(), v.data()); }
+    template <typename T>
+    T *host(Sec<T> s) const { return reinterpret_cast<T *>(hp + secs[s.i].off); }
+    template <typename T>
+    T *dev(Sec<T> s) const { return reinterpret_cast<T *>(dp + secs[s.i].off); }
+
+    // lays the sections out, grows BatchWindows::stage to them and copies the sources into its host side; upload_now:
+    // then uploads (a call that fills host sections itself uploads after that)
+    int place(Handle *h, bool upload_now = false) {
+        size_t o = 0;
+        for (int k = 0; k < kKinds; ++k) {
+            for (Entry &e : secs)
+                if (e.kind == k) { e.off = o; o += (e.bytes + 7) & ~(size_t)7; }
+            end[k] = o;
+        }
+        TRY(reserve(h, h->bw.stage, o, kBoth));
+        hp = h->bw.stage.h; dp = h->bw.stage.d;
+        for (const Entry &e : secs)
+            if (e.src && e.bytes) memcpy(hp + e.off, e.src, e.bytes);
+        return upload_now ? upload(h) : 0;
+    }
+    int upload(Handle *h) const {
+        if (end[kInOut] > 0) CK(h, cudaMemcpyAsync(dp, hp, end[kInOut], cudaMemcpyHostToDevice, h->stream));
+        return 0;
+    }
+    int download(Handle *h) const {
+        if (end[kDown] > end[kUp])
+            CK(h, cudaMemcpyAsync(hp + end[kUp], dp + end[kUp], end[kDown] - end[kUp], cudaMemcpyDeviceToHost, h->stream));
+        return 0;
     }
 };
 
@@ -868,12 +901,49 @@ static void host_header(Handle *h, int slot) {
     H.n_planes = s.n_planes; H.n_ptracks = sh.T;            // batch_shape: plane tracks take the full solve kernel
 }
 
-static BwLayout layout_from(int slot, const WinSlot &s) {
+static BwLayout layout_of(int slot, const WinSlot &s) {
     int smax = 0;
     for (int32_t c : s.n_samples) smax = std::max(smax, (int)c);
     return BwLayout{slot, s.N, (int)s.ids.size(), s.fixed, s.n_prior, s.inertial, s.n_planes, smax};
 }
-static BwLayout layout_of(const Handle *h, int slot) { return layout_from(slot, h->slots[slot]); }
+
+// the rows of a mirror whose frame mask, shifted down by `shift` frames, is not 0, in order, with their shifted masks
+static void compact_rows(WinSlot &s, int shift) {
+    size_t o = 0;
+    for (size_t r = 0; r < s.ids.size(); ++r) {
+        const uint32_t m = s.mask[r] >> shift;
+        if (m) { s.ids[o] = s.ids[r]; s.mask[o] = m; s.role[o] = s.role[r]; ++o; }
+    }
+    s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
+}
+
+// the re-layout of a call's slots to their new mirrors next[]: their BwLayouts and the slot list go with the call's
+// upload; launch rebuilds the packed windows once the call's own kernels are queued
+struct Relayout {
+    std::vector<BwLayout> lays;
+    Stage::Sec<BwLayout> lay;
+    Stage::Sec<int32_t> slots;
+    Relayout(Stage &S, const int32_t *sl, const std::vector<WinSlot> &next) : lays(next.size()) {
+        for (size_t i = 0; i < next.size(); ++i) lays[i] = layout_of(sl[i], next[i]);
+        lay = S.up(lays);
+        slots = S.add(Stage::kUp, next.size(), sl);
+    }
+    int launch(Handle *h, const Stage &S, bool prior) const {
+        const int n = (int)lays.size();
+        bw_layout_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(lay));
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        return launch_layout_tail(h, S.dev(slots), n, prior);
+    }
+};
+
+// the mirrors of a call that has run into their slots, with their host headers
+static void commit(Handle *h, const int32_t *slots, std::vector<WinSlot> &next) {
+    for (size_t i = 0; i < next.size(); ++i) {
+        h->slots[slots[i]] = std::move(next[i]);
+        host_header(h, slots[i]);
+    }
+}
 
 // plane-table capacity for the windows the n slots of a call will hold, before anything of the call is staged
 static int ensure_plane_tables(Handle *h, const std::vector<WinSlot> &next) {
@@ -893,28 +963,6 @@ static int check_slots(Handle *h, int n, const int32_t *slots, const char *what)
         seen[s] = 1;
     }
     return 0;
-}
-
-// stage, upload, and return device pointers into the staged bytes
-static int upload_stage(Handle *h, const Packer &p, size_t out_bytes, uint8_t *&d_in, uint8_t *&d_out) {
-    const size_t in = (p.buf.size() + 15) & ~(size_t)15;
-    TRY(reserve(h, h->bw.stage, in + out_bytes + 16, kBoth));
-    if (!p.buf.empty()) {
-        memcpy(h->bw.stage.h, p.buf.data(), p.buf.size());
-        CK(h, cudaMemcpyAsync(h->bw.stage.d, h->bw.stage.h, p.buf.size(), cudaMemcpyHostToDevice, h->stream));
-    }
-    d_in = h->bw.stage.d;
-    d_out = h->bw.stage.d + in;
-    return 0;
-}
-
-// re-layout of the slots whose BwLayout records start at byte `off` of the upload (list of int32 slots at slots_off)
-static int relayout(Handle *h, uint8_t *d_in, size_t lay_off, size_t slots_off, int n, bool prior) {
-    if (n == 0) return 0;
-    bw_layout_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwLayout *>(d_in + lay_off));
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    return launch_layout_tail(h, reinterpret_cast<const int32_t *>(d_in + slots_off), n, prior);
 }
 
 static int find_row(const WinSlot &s, int32_t id) {
@@ -940,29 +988,30 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
     std::vector<BwImu> jobs;                  // the factors with samples: re-integrated before the chain
     for (int i = 0; i < n; ++i) {
         const WinSlot &s = h->slots[slots[i]];
-        named[slots[i]] = 1; lays[i] = layout_of(h, slots[i]);
+        named[slots[i]] = 1; lays[i] = layout_of(slots[i], s);
         if (s.inertial)
             for (int k = 0; k + 1 < s.N; ++k)
                 if (s.n_samples[k] > 0)
                     jobs.push_back(BwImu{slots[i], k, s.n_samples[k], (int32_t)(((size_t)slots[i] * h->Ncap + k) * h->bw.Scap)});
     }
-    Packer p;
-    const size_t o_nm = p.put(named.data(), range), o_lay = p.put(lays.data(), n), o_sl = p.put(slots, n);
-    const size_t o_job = jobs.empty() ? 0 : p.put(jobs.data(), jobs.size());
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
+    Stage S;
+    const auto nm = S.up(named);
+    const auto lay = S.up(lays);
+    const auto sl = S.add(Stage::kUp, n, slots);
+    const auto job = S.up(jobs);
+    TRY(S.place(h, true));
     if (!jobs.empty()) {
         const int J = (int)jobs.size();
         bw_reintegrate_kernel<<<(J + kBwImuWarps - 1) / kBwImuWarps, 32 * kBwImuWarps, 0, h->stream>>>(
-            launch_args<BwArgs>(h), reinterpret_cast<const BwImu *>(din + o_job), J);
+            launch_args<BwArgs>(h), S.dev(job), J);
         ++h->launches;
         CK(h, cudaGetLastError());
     }
     CK(h, cudaEventRecord(h->ev0, h->stream));
-    TRY(run_named_solve(h, opt, range, din + o_nm));
+    TRY(run_named_solve(h, opt, range, S.dev(nm)));
     CK(h, cudaEventRecord(h->ev1, h->stream));
-    if (post) TRY(run_postpass_slots(h, n, reinterpret_cast<const int32_t *>(din + o_sl)));
-    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwLayout *>(din + o_lay), post ? 1 : 0);
+    if (post) TRY(run_postpass_slots(h, n, S.dev(sl)));
+    bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(lay), post ? 1 : 0);
     ++h->launches;
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(h->ctrl.h, h->ctrl.d, sizeof(WinCtrl) * range, cudaMemcpyDeviceToHost, h->stream));
@@ -979,19 +1028,13 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
 
 // The localize half of a batch of records (pvio_b200_batch_window_localize, pvio_b200_batch_window_track_frame): every
 // record checked against its slot's host mirror, the observations that take part kept with the index they came from,
-// the new tracks' keypoint pairs; then the staging layout in h->pnp (doubles).  Upload: records | rows | z | IMU
-// records (imu_staged) | new keypoints | the caller's upload words (x) | states | points.  Download: states | points |
-// summary words | inverse depths | re-anchored inverse depths | valid bytes | the caller's download words (y).  Then,
-// device only: the PnP records and the caller's scratch words (s).
+// the new tracks' keypoint pairs
 struct LocPlan {
     const char *what;
     std::vector<BwLoc> recs;
     std::vector<int32_t> rows, from;
     std::vector<double> zs, pts, nzs;
     int n_imu = 0;
-    bool imu_staged = true;
-    size_t o_row = 0, o_z = 0, o_imu = 0, o_nz = 0, o_x = 0, o_fr = 0, o_pts = 0, o_out = 0, o_rho = 0, o_next = 0;
-    size_t o_val = 0, o_y = 0, o_args = 0, o_s = 0, words = 0;
 };
 
 static int loc_fail(Handle *h, const LocPlan &P, const char *why) {
@@ -1040,35 +1083,37 @@ static int loc_add(Handle *h, LocPlan &P, const pvio_b200_window_localize &R, bo
     return 0;
 }
 
-// the layout of n records with x / y / s caller words; grows h->pnp and stages the plan's sections on the host side
-static int loc_stage(Handle *h, LocPlan &P, size_t x, size_t y, size_t s) {
-    const size_t n = P.recs.size(), K = P.rows.size(), T = P.nzs.size() / 4, w8 = sizeof(double);
-    P.o_row = n * sizeof(BwLoc) / w8; P.o_z = P.o_row + (K + 1) / 2; P.o_imu = P.o_z + 2 * K;
-    P.o_nz = P.o_imu + (P.imu_staged ? (size_t)P.n_imu * kImuStride : 0); P.o_x = P.o_nz + 4 * T; P.o_fr = P.o_x + x;
-    P.o_pts = P.o_fr + 16 * n; P.o_out = P.o_pts + 3 * K; P.o_rho = P.o_out + 8 * n; P.o_next = P.o_rho + T;
-    P.o_val = P.o_next + T; P.o_y = P.o_val + (T + 7) / 8; P.o_args = P.o_y + y;
-    P.o_s = P.o_args + n * sizeof(PnpArgs) / w8; P.words = P.o_s + s;
-    TRY(reserve(h, h->pnp, P.words, kBoth));
-    double *st = h->pnp.h;
-    memcpy(st, P.recs.data(), sizeof(BwLoc) * n);
-    if (K) {
-        memcpy(st + P.o_row, P.rows.data(), sizeof(int32_t) * K);
-        memcpy(st + P.o_z, P.zs.data(), w8 * 2 * K);
-        memcpy(st + P.o_pts, P.pts.data(), w8 * 3 * K);
-    }
-    if (T) memcpy(st + P.o_nz, P.nzs.data(), w8 * 4 * T);
-    return 0;
+// the staged sections of a plan: upload records | rows | keypoints | IMU records | new pairs; in/out states (in: the
+// prediction, out: solved) | points (in: the given point or NaN, out: the point used); download summary words |
+// inverse depths | re-anchored inverse depths | valid bytes; device only the PnP records
+struct LocSecs {
+    Stage::Sec<BwLoc> rec;
+    Stage::Sec<int32_t> row;
+    Stage::Sec<double> z, imu, nz, frames, pts, out, rho, next;
+    Stage::Sec<uint8_t> valid;
+    Stage::Sec<PnpArgs> args;
+};
+
+// imu: the IMU records of the inertial records are staged (the caller fills them)
+static LocSecs loc_stage(Stage &S, const LocPlan &P, bool imu) {
+    const size_t n = P.recs.size(), T = P.nzs.size() / 4;
+    LocSecs s;
+    s.rec = S.up(P.recs); s.row = S.up(P.rows); s.z = S.up(P.zs);
+    s.imu = S.add<double>(Stage::kUp, imu ? (size_t)P.n_imu * kImuStride : 0); s.nz = S.up(P.nzs);
+    s.frames = S.add<double>(Stage::kInOut, 16 * n); s.pts = S.add(Stage::kInOut, P.pts.size(), P.pts.data());
+    s.out = S.add<double>(Stage::kDown, 8 * n); s.rho = S.add<double>(Stage::kDown, T);
+    s.next = S.add<double>(Stage::kDown, T); s.valid = S.add<uint8_t>(Stage::kDown, T);
+    s.args = S.add<PnpArgs>(Stage::kScratch, n);
+    return s;
 }
 
-// the device view of the staged plan
-static LocArgs loc_args(const Handle *h, const LocPlan &P, const pvio_b200_options *opt) {
-    double *d = h->pnp.d;
+// the device view of the placed plan
+static LocArgs loc_args(const Stage &S, const LocSecs &s, const pvio_b200_options *opt) {
     const SolveOptions so = solve_options(opt);
     LocArgs L;
-    L.rec = reinterpret_cast<const BwLoc *>(d); L.row = reinterpret_cast<const int32_t *>(d + P.o_row); L.z = d + P.o_z;
-    L.imu = d + P.o_imu; L.nz = d + P.o_nz; L.frames = d + P.o_fr; L.pts = d + P.o_pts; L.out = d + P.o_out;
-    L.rho = d + P.o_rho; L.rho_next = d + P.o_next; L.valid = reinterpret_cast<uint8_t *>(d + P.o_val);
-    L.args = reinterpret_cast<PnpArgs *>(d + P.o_args);
+    L.rec = S.dev(s.rec); L.row = S.dev(s.row); L.z = S.dev(s.z); L.imu = S.dev(s.imu); L.nz = S.dev(s.nz);
+    L.frames = S.dev(s.frames); L.pts = S.dev(s.pts); L.out = S.dev(s.out); L.rho = S.dev(s.rho);
+    L.rho_next = S.dev(s.next); L.valid = S.dev(s.valid); L.args = S.dev(s.args);
     L.max_iter = so.max_iter; L.radius0 = so.radius0;
     return L;
 }
@@ -1088,26 +1133,25 @@ static int loc_launch(Handle *h, const LocArgs &L, int n) {
 }
 
 // after the download: record i's localize outputs into R
-static void loc_results(const Handle *h, const LocPlan &P, int i, size_t &k, const pvio_b200_window_localize &R, float ms) {
-    const double *st = h->pnp.h;
+static void loc_results(const Stage &S, const LocSecs &s, const LocPlan &P, int i, size_t &k,
+                        const pvio_b200_window_localize &R, float ms) {
     const size_t w8 = sizeof(double);
-    const uint8_t *val = reinterpret_cast<const uint8_t *>(st + P.o_val);
     const BwLoc &L = P.recs[i];
-    memcpy(R.state, st + P.o_fr + 16 * (size_t)i, w8 * 16);
+    memcpy(R.state, S.host(s.frames) + 16 * (size_t)i, w8 * 16);
     if (R.points_out) {
         for (int j = 0; j < 3 * R.n_obs; ++j) R.points_out[j] = NAN;
-        for (int j = 0; j < L.n_obs; ++j, ++k) memcpy(R.points_out + 3 * P.from[k], st + P.o_pts + 3 * k, w8 * 3);
+        for (int j = 0; j < L.n_obs; ++j, ++k) memcpy(R.points_out + 3 * P.from[k], S.host(s.pts) + 3 * k, w8 * 3);
     } else {
         k += L.n_obs;
     }
     for (int t = 0; t < L.n_new; ++t) {
         const size_t q = (size_t)L.new_off + t;
-        R.new_valid[t] = val[q];
-        R.new_inv_depth[t] = st[P.o_rho + q];
-        if (R.new_inv_depth_next) R.new_inv_depth_next[t] = st[P.o_next + q];
+        R.new_valid[t] = S.host(s.valid)[q];
+        R.new_inv_depth[t] = S.host(s.rho)[q];
+        if (R.new_inv_depth_next) R.new_inv_depth_next[t] = S.host(s.next)[q];
     }
     if (R.summary) {
-        const double *b = st + P.o_out + 8 * (size_t)i;
+        const double *b = S.host(s.out) + 8 * (size_t)i;
         pvio_b200_summary &S = *R.summary;
         memset(&S, 0, sizeof(S));
         S.iterations = (int)b[0]; S.accepted_steps = (int)b[1]; S.termination = (int)b[2]; S.usable = (int)b[3];
@@ -1154,21 +1198,18 @@ int pvio_b200_batch_window_reset(pvio_b200_handle hh, int slot, const pvio_b200_
     if (w->n_planes > 0 || w->n_plane_tracks > 0) return fail(h, PVIO_B200_EINVAL, "batch_window_reset: resident windows carry no planes");
     TRY(ensure_bw(h));
     if (w->use_inertial) TRY(ensure_inertial(h));
-    WinSlot &s = h->slots[slot];
-    s = WinSlot();                            // nothing of a former pack or resident window survives
-    s.resident = true; s.inertial = w->use_inertial ? 1 : 0;
-    s.n_samples.assign(h->Ncap, 0);
-    host_header(h, slot);
+    std::vector<WinSlot> next(1);             // nothing of a former pack or resident window survives
+    next[0].resident = true; next[0].inertial = w->use_inertial ? 1 : 0;
+    next[0].n_samples.assign(h->Ncap, 0);
     WinConst &C = h->cst.h[slot];
     C = win_const(w);
     CK(h, cudaMemcpyAsync(h->cst.dslot(slot), &C, sizeof(WinConst), cudaMemcpyHostToDevice, h->stream));
-    Packer p;
-    const BwLayout L = layout_of(h, slot);
-    const size_t lay = p.put(&L, 1), sl = p.put(&slot, 1);
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
-    TRY(relayout(h, din, lay, sl, 1, false));
+    Stage S;
+    const Relayout lay(S, &slot, next);
+    TRY(S.place(h, true));
+    TRY(lay.launch(h, S, false));
     CK(h, cudaStreamSynchronize(h->stream));
+    commit(h, &slot, next);
     return 0;
 }
 
@@ -1177,7 +1218,7 @@ int pvio_b200_batch_window_set_prior(pvio_b200_handle hh, int slot, int n_prior,
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     TRY(check_slots(h, 1, &slot, "batch_window_set_prior: bad slot"));
-    WinSlot &s = h->slots[slot];
+    const WinSlot &s = h->slots[slot];
     if (n_prior < 0 || (n_prior > 0 && (!S || !e || !state0))) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: null prior");
     if (!s.inertial && n_prior > 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: the window carries no motion states");
     if (n_prior > s.N) return fail(h, PVIO_B200_EINVAL, "batch_window_set_prior: prior over more frames than the window holds");
@@ -1191,15 +1232,14 @@ int pvio_b200_batch_window_set_prior(pvio_b200_handle hh, int slot, int n_prior,
         CK(h, cudaMemcpyAsync(h->prior_x0.dslot(slot), h->prior_x0.slot(slot), sizeof(double) * n_prior * kFrameStride,
                               cudaMemcpyHostToDevice, h->stream));
     }
-    s.n_prior = s.prior_resident = n_prior;
-    host_header(h, slot);
-    Packer p;
-    const BwLayout L = layout_of(h, slot);
-    const size_t lay = p.put(&L, 1), sl = p.put(&slot, 1);
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
-    TRY(relayout(h, din, lay, sl, 1, n_prior > 0));
+    std::vector<WinSlot> next(1, s);
+    next[0].n_prior = next[0].prior_resident = n_prior;
+    Stage st;
+    const Relayout lay(st, &slot, next);
+    TRY(st.place(h, true));
+    TRY(lay.launch(h, st, n_prior > 0));
     CK(h, cudaStreamSynchronize(h->stream));
+    commit(h, &slot, next);
     return 0;
 }
 
@@ -1251,12 +1291,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
         }
         R.n_rm = E.n_remove;
         std::sort(removed.begin(), removed.end());
-        {   // compaction
-            size_t o = 0;
-            for (size_t r = 0; r < s.ids.size(); ++r)
-                if (s.mask[r]) { s.ids[o] = s.ids[r]; s.mask[o] = s.mask[r]; s.role[o] = s.role[r]; ++o; }
-            s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
-        }
+        compact_rows(s, 0);
         if (E.state) {
             if (s.N >= h->Ncap) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: window of more than max_frames frames");
             const bool imu = s.inertial && s.N > 0;
@@ -1296,28 +1331,23 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
         next[i] = std::move(s);
     }
     TRY(ensure_plane_tables(h, next));                 // observations of plane tracks may outgrow the plane tables
-    Packer p;
-    std::vector<BwLayout> lays(n);
-    for (int i = 0; i < n; ++i) lays[i] = layout_from(slots[i], next[i]);
-    const size_t o_ed = p.put(recs.data(), n), o_lay = p.put(lays.data(), n), o_sl = p.put(slots.data(), n);
-    const size_t o_rm = p.put(rm.data(), rm.size()), o_nw = p.put(nws.data(), nws.size()), o_ob = p.put(obs.data(), obs.size());
-    const size_t o_x = p.put(xs.data(), xs.size());
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, sizeof(int32_t) * out_ints, din, dout));
-    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwEdit *>(din + o_ed),
-        reinterpret_cast<const int32_t *>(din + o_rm), reinterpret_cast<const BwNew *>(din + o_nw),
-        reinterpret_cast<const BwObs *>(din + o_ob), reinterpret_cast<const double *>(din + o_x), reinterpret_cast<int32_t *>(dout));
+    Stage S;
+    const auto ed = S.up(recs);
+    const auto nw = S.up(nws);
+    const auto ob = S.up(obs);
+    const auto x = S.up(xs);
+    const auto rmv = S.up(rm), out = S.add<int32_t>(Stage::kDown, out_ints);
+    const Relayout lay(S, slots.data(), next);
+    TRY(S.place(h, true));
+    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(ed), S.dev(rmv), S.dev(nw), S.dev(ob),
+                                                    S.dev(x), S.dev(out));
     ++h->launches;
     CK(h, cudaGetLastError());
-    TRY(relayout(h, din, o_lay, o_sl, n, false));
-    const size_t in = dout - din;
-    CK(h, cudaMemcpyAsync(h->bw.stage.h + in, dout, sizeof(int32_t) * out_ints, cudaMemcpyDeviceToHost, h->stream));
+    TRY(lay.launch(h, S, false));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(h->stream));
-    const int32_t *res = reinterpret_cast<const int32_t *>(h->bw.stage.h + in);
-    for (int i = 0; i < n; ++i) {
-        h->slots[slots[i]] = std::move(next[i]);
-        host_header(h, slots[i]);
-    }
+    const int32_t *res = S.host(out);
+    commit(h, slots.data(), next);
     for (int i = 0; i < n; ++i) {
         const int32_t *r = res + recs[i].out_off;
         if (r[0] != (int32_t)h->slots[slots[i]].ids.size())
@@ -1372,23 +1402,18 @@ int pvio_b200_batch_window_set_planes(pvio_b200_handle hh, int n, const pvio_b20
         next[i] = std::move(s);
     }
     TRY(ensure_plane_tables(h, next));
-    Packer p;
-    std::vector<BwLayout> lays(n);
-    for (int i = 0; i < n; ++i) lays[i] = layout_from(slots[i], next[i]);
-    const size_t o_rec = p.put(recs.data(), n), o_lay = p.put(lays.data(), n), o_sl = p.put(slots.data(), n);
-    const size_t o_ro = p.put(roles.data(), roles.size()), o_pa = p.put(params.data(), params.size());
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
-    bw_planes_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwPlanes *>(din + o_rec),
-        reinterpret_cast<const BwRole *>(din + o_ro), reinterpret_cast<const double *>(din + o_pa));
+    Stage S;
+    const auto rec = S.up(recs);
+    const auto ro = S.up(roles);
+    const auto pa = S.up(params);
+    const Relayout lay(S, slots.data(), next);
+    TRY(S.place(h, true));
+    bw_planes_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(rec), S.dev(ro), S.dev(pa));
     ++h->launches;
     CK(h, cudaGetLastError());
-    TRY(relayout(h, din, o_lay, o_sl, n, false));
+    TRY(lay.launch(h, S, false));
     CK(h, cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < n; ++i) {
-        h->slots[slots[i]] = std::move(next[i]);
-        host_header(h, slots[i]);
-    }
+    commit(h, slots.data(), next);
     return 0;
 }
 
@@ -1415,42 +1440,31 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
             return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: window too large for the shared-memory eigen-solver (15 (N - 1) <= 165)");
         if ((S_out && S_stride < (int64_t)dk * dk) || (e_out && e_stride < dk))
             return fail(h, PVIO_B200_EINVAL, "batch_window_drop_victim: output stride smaller than a window's prior");
-        size_t o = 0;                                                  // map.cpp:76-88 on the host mirror
-        for (size_t r = 0; r < s.ids.size(); ++r) {
-            const uint32_t m = s.mask[r] >> 1;
-            if (m) { s.ids[o] = s.ids[r]; s.mask[o] = m; s.role[o] = s.role[r]; ++o; }
-        }
-        s.ids.resize(o); s.mask.resize(o); s.role.resize(o);
+        compact_rows(s, 1);                                            // map.cpp:76-88 on the host mirror
         --s.N; s.fixed >>= 1; s.n_prior = s.prior_resident = s.N;
         s.n_samples.erase(s.n_samples.begin());                        // factor 0 leaves, the others shift with their frames
         s.n_samples.push_back(0);
         TRY(check_window(h, s));
         next[i] = std::move(s);
     }
-    std::vector<BwLayout> before(n), after(n);
-    for (int i = 0; i < n; ++i) {
-        before[i] = layout_of(h, slots[i]);
-        after[i] = layout_from(slots[i], next[i]);
-    }
-    Packer p;
-    const size_t o_sl = p.put(slots, n), o_b = p.put(before.data(), n), o_a = p.put(after.data(), n);
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
-    TRY(run_marg(h, n, 0, true, true, slots, reinterpret_cast<const int32_t *>(din + o_sl)));
+    std::vector<BwLayout> before(n);
+    for (int i = 0; i < n; ++i) before[i] = layout_of(slots[i], h->slots[slots[i]]);
+    Stage S;
+    const auto b = S.up(before);
+    const Relayout lay(S, slots, next);
+    TRY(S.place(h, true));
+    TRY(run_marg(h, n, 0, true, true, slots, S.dev(lay.slots)));
     for (int i = 0; i < n; ++i) {
         const size_t dk = 15 * (size_t)(h->slots[slots[i]].N - 1);
         if (S_out) CK(h, cudaMemcpyAsync(S_out + i * S_stride, h->prior_S.dslot(slots[i]), sizeof(double) * dk * dk, cudaMemcpyDeviceToHost, h->stream));
         if (e_out) CK(h, cudaMemcpyAsync(e_out + i * e_stride, h->prior_e.dslot(slots[i]), sizeof(double) * dk, cudaMemcpyDeviceToHost, h->stream));
     }
-    bw_drop_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwLayout *>(din + o_b));
+    bw_drop_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(b));
     ++h->launches;
     CK(h, cudaGetLastError());
-    TRY(relayout(h, din, o_a, o_sl, n, true));
+    TRY(lay.launch(h, S, true));
     CK(h, cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < n; ++i) {
-        h->slots[slots[i]] = std::move(next[i]);
-        host_header(h, slots[i]);
-    }
+    commit(h, slots, next);
     return 0;
 }
 
@@ -1471,34 +1485,30 @@ int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *s
         if ((track_id || inv_depth || anchor_frame || n_observations || valid || quality) && track_stride < T)
             return fail(h, PVIO_B200_EINVAL, "batch_window_download: track_stride smaller than a slot's live tracks");
         dls[i] = BwDl{slots[i], s.N, T, 0, off};
-        off += ((int64_t)(s.N * kFrameStride + 2 * T) * 8 + (int64_t)T * 13 + 15) & ~(int64_t)15;
+        off += BwDlRec::bytes(s.N, T);
     }
-    Packer p;
-    const size_t o_dl = p.put(dls.data(), n);
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, (size_t)off, din, dout));
-    bw_download_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwDl *>(din + o_dl), dout);
+    Stage S;
+    const auto dl = S.up(dls);
+    const auto out = S.add<uint8_t>(Stage::kDown, (size_t)off);
+    TRY(S.place(h, true));
+    bw_download_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(dl), S.dev(out));
     ++h->launches;
     CK(h, cudaGetLastError());
-    const size_t in = dout - din;
-    CK(h, cudaMemcpyAsync(h->bw.stage.h + in, dout, (size_t)off, cudaMemcpyDeviceToHost, h->stream));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n; ++i) {
         const int N = dls[i].N, T = dls[i].T;
-        const uint8_t *b = h->bw.stage.h + in + dls[i].off;
-        const double *fo = reinterpret_cast<const double *>(b), *ro = fo + (size_t)N * kFrameStride, *qo = ro + T;
-        const int32_t *io = reinterpret_cast<const int32_t *>(qo + T), *ao = io + T, *no = ao + T;
-        const uint8_t *vo = reinterpret_cast<const uint8_t *>(no + T);
+        const BwDlRec o(S.host(out) + dls[i].off, N, T);
         const size_t t0 = (size_t)i * track_stride;
         if (n_frames) n_frames[i] = N;
         if (n_tracks) n_tracks[i] = T;
-        if (frames) memcpy(frames + (size_t)i * frames_stride, fo, sizeof(double) * N * kFrameStride);
-        if (track_id) memcpy(track_id + t0, io, sizeof(int32_t) * T);
-        if (inv_depth) memcpy(inv_depth + t0, ro, sizeof(double) * T);
-        if (anchor_frame) memcpy(anchor_frame + t0, ao, sizeof(int32_t) * T);
-        if (n_observations) memcpy(n_observations + t0, no, sizeof(int32_t) * T);
-        if (valid) memcpy(valid + t0, vo, T);
-        if (quality) memcpy(quality + t0, qo, sizeof(double) * T);
+        if (frames) memcpy(frames + (size_t)i * frames_stride, o.fo, sizeof(double) * N * kFrameStride);
+        if (track_id) memcpy(track_id + t0, o.io, sizeof(int32_t) * T);
+        if (inv_depth) memcpy(inv_depth + t0, o.ro, sizeof(double) * T);
+        if (anchor_frame) memcpy(anchor_frame + t0, o.ao, sizeof(int32_t) * T);
+        if (n_observations) memcpy(n_observations + t0, o.no, sizeof(int32_t) * T);
+        if (valid) memcpy(valid + t0, o.vo, T);
+        if (quality) memcpy(quality + t0, o.qo, sizeof(double) * T);
     }
     return 0;
 }
@@ -1516,22 +1526,23 @@ int pvio_b200_batch_window_localize(pvio_b200_handle hh, int n, pvio_b200_window
     LocPlan P;
     P.what = "batch_window_localize";
     for (int i = 0; i < n; ++i) TRY(loc_add(h, P, records[i], true));
-    TRY(loc_stage(h, P, 0, 0, 0));
-    double *st = h->pnp.h, *d = h->pnp.d;
+    Stage S;
+    const LocSecs s = loc_stage(S, P, true);
+    TRY(S.place(h));
     const size_t w8 = sizeof(double);
     for (int i = 0; i < n; ++i) {
-        memcpy(st + P.o_fr + 16 * (size_t)i, records[i].state, w8 * 16);
+        memcpy(S.host(s.frames) + 16 * (size_t)i, records[i].state, w8 * 16);
         if (P.recs[i].inertial)
-            memcpy(st + P.o_imu + (size_t)P.recs[i].imu_off * kImuStride, records[i].imu_record, w8 * kImuStride);
+            memcpy(S.host(s.imu) + (size_t)P.recs[i].imu_off * kImuStride, records[i].imu_record, w8 * kImuStride);
     }
-    CK(h, cudaMemcpyAsync(d, st, w8 * P.o_out, cudaMemcpyHostToDevice, h->stream));
-    TRY(loc_launch(h, loc_args(h, P, opt), n));
-    CK(h, cudaMemcpyAsync(st + P.o_fr, d + P.o_fr, w8 * (P.o_args - P.o_fr), cudaMemcpyDeviceToHost, h->stream));
+    TRY(S.upload(h));
+    TRY(loc_launch(h, loc_args(S, s, opt), n));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(h->stream));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, h->ev0, h->ev1);
     size_t k = 0;
-    for (int i = 0; i < n; ++i) loc_results(h, P, i, k, records[i], ms);
+    for (int i = 0; i < n; ++i) loc_results(S, s, P, i, k, records[i], ms);
     return 0;
 }
 
@@ -1547,7 +1558,6 @@ int pvio_b200_batch_window_track_frame(pvio_b200_handle hh, int n, pvio_b200_win
     // every record is checked before anything is staged: its localize half as localize checks it, then the rest
     LocPlan P;
     P.what = "batch_window_track_frame";
-    P.imu_staged = false;                     // the step-1 records are computed on the device
     std::vector<BwTrack> trs(n);
     std::vector<BwTrackJob> jobs;
     std::vector<int32_t> kf_row;
@@ -1590,62 +1600,57 @@ int pvio_b200_batch_window_track_frame(pvio_b200_handle hh, int n, pvio_b200_win
         if (merged) jobs.push_back(BwTrackJob{i, (int32_t)rows, (int32_t)e, 1});
         rows = e;
     }
-    // the caller's words: upload track records | jobs | observed pairs' rows | their keypoints | samples | t_end and
-    // noise; download the edit's IMU records | predicted states | keyframe words; scratch step-1 records | parallaxes
-    const size_t w8 = sizeof(double), J = jobs.size(), Kf = kf_row.size();
-    const size_t x_tr = 0, x_job = x_tr + n * sizeof(BwTrack) / w8, x_row = x_job + J * sizeof(BwTrackJob) / w8;
-    const size_t x_z = x_row + (Kf + 1) / 2, x_smp = x_z + 2 * Kf, x_aux = x_smp + 7 * rows, x = x_aux + (size_t)n * kImuAux;
-    const size_t y_rec = 0, y_pred = y_rec + (size_t)n * kImuStride, y_kf = y_pred + 16 * (size_t)n, y = y_kf + 4 * (size_t)n;
-    const size_t s_rec = 0, s_par = s_rec + (size_t)n * kImuStride, sw = s_par + par;
-    TRY(loc_stage(h, P, x, y, sw));
-    double *st = h->pnp.h, *d = h->pnp.d, *sx = st + P.o_x;
-    memcpy(sx + x_tr, trs.data(), sizeof(BwTrack) * n);
-    memcpy(sx + x_job, jobs.data(), sizeof(BwTrackJob) * J);
-    if (Kf) {
-        memcpy(sx + x_row, kf_row.data(), sizeof(int32_t) * Kf);
-        memcpy(sx + x_z, kf_z.data(), w8 * 2 * Kf);
-    }
+    // the localize sections without IMU records (the PnP reads the step-1 records, imu_off = record index); upload
+    // track records | jobs | observed pairs' rows | their keypoints | merge_samples ++ samples | t_end and noise,
+    // download the edit's IMU records | predicted states | keyframe words, scratch step-1 records | parallaxes
+    const size_t w8 = sizeof(double), J = jobs.size();
+    Stage S;
+    const LocSecs s = loc_stage(S, P, false);
+    const auto tr = S.up(trs);
+    const auto job = S.up(jobs);
+    const auto kr = S.up(kf_row);
+    const auto kz = S.up(kf_z), smp = S.add<double>(Stage::kUp, 7 * rows), aux = S.add<double>(Stage::kUp, (size_t)n * kImuAux);
+    const auto rec_out = S.add<double>(Stage::kDown, (size_t)n * kImuStride), pred = S.add<double>(Stage::kDown, 16 * (size_t)n);
+    const auto kfo = S.add<double>(Stage::kDown, 4 * (size_t)n);
+    const auto rec1 = S.add<double>(Stage::kScratch, (size_t)n * kImuStride), pars = S.add<double>(Stage::kScratch, par);
+    TRY(S.place(h));
     for (int i = 0; i < n; ++i) {
-        double *a = sx + x_aux + (size_t)i * kImuAux;
+        double *a = S.host(aux) + (size_t)i * kImuAux;
         a[0] = records[i].t_end;
         memcpy(a + 1, records[i].noise_cov, w8 * 36);
     }
     for (const BwTrackJob &j : jobs) {                          // merge_samples ++ samples, back to back per record
         if (j.merged) continue;
         const pvio_b200_window_track_frame &R = records[j.rec];
-        memcpy(sx + x_smp + 7 * (size_t)j.begin, R.samples, w8 * 7 * R.n_samples);
-        if (trs[j.rec].merged) memcpy(sx + x_smp + 7 * ((size_t)j.begin - R.n_merge), R.merge_samples, w8 * 7 * R.n_merge);
+        memcpy(S.host(smp) + 7 * (size_t)j.b, R.samples, w8 * 7 * R.n_samples);
+        if (trs[j.rec].merged) memcpy(S.host(smp) + 7 * ((size_t)j.b - R.n_merge), R.merge_samples, w8 * 7 * R.n_merge);
     }
-    CK(h, cudaMemcpyAsync(d, st, w8 * P.o_out, cudaMemcpyHostToDevice, h->stream));
-    const LocArgs L = loc_args(h, P, opt);
+    TRY(S.upload(h));
     TrackArgs T;
-    double *dx = d + P.o_x, *dy = d + P.o_y, *ds = d + P.o_s;
-    T.tr = reinterpret_cast<const BwTrack *>(dx + x_tr); T.job = reinterpret_cast<const BwTrackJob *>(dx + x_job);
-    T.kf_row = reinterpret_cast<const int32_t *>(dx + x_row); T.kf_z = dx + x_z; T.smp = dx + x_smp; T.aux = dx + x_aux;
-    T.rec_out = dy + y_rec; T.pred = dy + y_pred; T.kfo = dy + y_kf; T.rec1 = ds + s_rec; T.par = ds + s_par;
+    T.tr = S.dev(tr); T.job = S.dev(job); T.kf_row = S.dev(kr); T.kf_z = S.dev(kz); T.smp = S.dev(smp); T.aux = S.dev(aux);
+    T.rec_out = S.dev(rec_out); T.pred = S.dev(pred); T.kfo = S.dev(kfo); T.rec1 = S.dev(rec1); T.par = S.dev(pars);
     T.n_jobs = (int)J;
-    LocArgs Li = L;
-    Li.imu = T.rec1;                          // the PnP reads the step-1 records (imu_off = record index)
+    LocArgs L = loc_args(S, s, opt);
+    L.imu = T.rec1;
     const BwArgs a = launch_args<BwArgs>(h);
-    bw_track_integrate_kernel<<<(int)((J + kBwImuWarps - 1) / kBwImuWarps), 32 * kBwImuWarps, 0, h->stream>>>(a, Li, T);
+    bw_track_integrate_kernel<<<(int)((J + kBwImuWarps - 1) / kBwImuWarps), 32 * kBwImuWarps, 0, h->stream>>>(a, L, T);
     ++h->launches;
     CK(h, cudaGetLastError());
-    TRY(loc_launch(h, Li, n));
-    bw_track_keyframe_kernel<<<n, kBwThreads, 0, h->stream>>>(a, Li, T);
+    TRY(loc_launch(h, L, n));
+    bw_track_keyframe_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T);
     ++h->launches;
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(st + P.o_fr, d + P.o_fr, w8 * (P.o_args - P.o_fr), cudaMemcpyDeviceToHost, h->stream));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(h->stream));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, h->ev0, h->ev1);
     size_t k = 0;
-    const double *sy = st + P.o_y;
     for (int i = 0; i < n; ++i) {
         pvio_b200_window_track_frame &R = records[i];
-        loc_results(h, P, i, k, localize_view(R), ms);
-        memcpy(R.imu_record, sy + y_rec + (size_t)i * kImuStride, w8 * kImuStride);
-        if (R.predicted) memcpy(R.predicted, sy + y_pred + 16 * (size_t)i, w8 * 16);
-        const double *o = sy + y_kf + 4 * (size_t)i;
+        loc_results(S, s, P, i, k, localize_view(R), ms);
+        memcpy(R.imu_record, S.host(rec_out) + (size_t)i * kImuStride, w8 * kImuStride);
+        if (R.predicted) memcpy(R.predicted, S.host(pred) + 16 * (size_t)i, w8 * 16);
+        const double *o = S.host(kfo) + 4 * (size_t)i;
         *R.keyframe = o[0] != 0.0 ? 1 : 0;
         if (R.parallax) *R.parallax = o[1];
         if (R.n_parallax) *R.n_parallax = (int32_t)o[2];
@@ -1674,11 +1679,9 @@ int pvio_b200_batch_window_set_imu(pvio_b200_handle hh, int n, const pvio_b200_w
         if (R.n_samples < 1)
             return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: a factor without IMU samples (integrate() returns false, preintegrator.cpp:86)");
         if (!R.samples || !R.noise_cov) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: null array");
-        for (int64_t k = 0; k < 7 * (int64_t)R.n_samples; ++k)
-            if (!std::isfinite(R.samples[k])) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite sample");
+        if (!all_finite(R.samples, 7 * (int64_t)R.n_samples)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite sample");
         if (!std::isfinite(R.t_end)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite t_end");
-        for (int k = 0; k < 36; ++k)
-            if (!std::isfinite(R.noise_cov[k])) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite noise");
+        if (!all_finite(R.noise_cov, 36)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: non-finite noise");
         recs[i] = BwImu{R.slot, R.frame - 1, R.n_samples, (int32_t)rows};
         pairs[i] = {R.slot, R.frame};
         rows += R.n_samples;
@@ -1689,22 +1692,19 @@ int pvio_b200_batch_window_set_imu(pvio_b200_handle hh, int n, const pvio_b200_w
         return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: a (slot, frame) named twice");
     if (rows > (size_t)INT32_MAX) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: too many samples in one call");
     TRY(ensure_imu_store(h, smax));
-    Packer p;
-    const size_t o_rec = p.put(recs.data(), n);
-    const size_t o_smp = (p.buf.size() + 7) & ~(size_t)7;
-    p.buf.resize(o_smp + sizeof(double) * 7 * rows);
-    std::vector<double> aux((size_t)n * kImuAux);
+    Stage S;
+    const auto rec = S.up(recs);
+    const auto smp = S.add<double>(Stage::kUp, 7 * rows), aux = S.add<double>(Stage::kUp, (size_t)n * kImuAux);
+    TRY(S.place(h));
     for (int i = 0; i < n; ++i) {
         const pvio_b200_window_imu &R = records[i];
-        memcpy(p.buf.data() + o_smp + sizeof(double) * 7 * recs[i].off, R.samples, sizeof(double) * 7 * R.n_samples);
-        aux[(size_t)i * kImuAux] = R.t_end;
-        memcpy(&aux[(size_t)i * kImuAux + 1], R.noise_cov, sizeof(double) * 36);
+        memcpy(S.host(smp) + 7 * (size_t)recs[i].off, R.samples, sizeof(double) * 7 * R.n_samples);
+        double *a = S.host(aux) + (size_t)i * kImuAux;
+        a[0] = R.t_end;
+        memcpy(a + 1, R.noise_cov, sizeof(double) * 36);
     }
-    const size_t o_aux = p.put(aux.data(), aux.size());
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, 0, din, dout));
-    bw_set_imu_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwImu *>(din + o_rec),
-        reinterpret_cast<const double *>(din + o_smp), reinterpret_cast<const double *>(din + o_aux));
+    TRY(S.upload(h));
+    bw_set_imu_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(rec), S.dev(smp), S.dev(aux));
     ++h->launches;
     CK(h, cudaGetLastError());
     CK(h, cudaStreamSynchronize(h->stream));
@@ -1729,19 +1729,17 @@ int pvio_b200_batch_window_imu_records(pvio_b200_handle hh, int n, const int32_t
         dls[i] = BwDl{slots[i], std::max(s.N, 1), 0, 0, off};
         off += m * (int64_t)sizeof(double);
     }
-    Packer p;
-    const size_t o_dl = p.put(dls.data(), n);
-    uint8_t *din, *dout;
-    TRY(upload_stage(h, p, (size_t)off, din, dout));
-    bw_imu_records_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), reinterpret_cast<const BwDl *>(din + o_dl), dout);
+    Stage S;
+    const auto dl = S.up(dls);
+    const auto out = S.add<uint8_t>(Stage::kDown, (size_t)off);
+    TRY(S.place(h, true));
+    bw_imu_records_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(dl), S.dev(out));
     ++h->launches;
     CK(h, cudaGetLastError());
-    const size_t in = dout - din;
-    if (off > 0) CK(h, cudaMemcpyAsync(h->bw.stage.h + in, dout, (size_t)off, cudaMemcpyDeviceToHost, h->stream));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n; ++i)
-        memcpy(records + i * records_stride, h->bw.stage.h + in + dls[i].off,
-               sizeof(double) * (size_t)(dls[i].N - 1) * kImuStride);
+        memcpy(records + i * records_stride, S.host(out) + dls[i].off, sizeof(double) * (size_t)(dls[i].N - 1) * kImuStride);
     return 0;
 }
 

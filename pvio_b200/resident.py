@@ -24,14 +24,7 @@ class ResidentWindow:
         L.pvio_b200_window_solve.argtypes = [C.c_void_p, C.POINTER(_lib.COptions), C.POINTER(_lib.CSummary)]
         L.pvio_b200_window_drop_victim.argtypes = [C.c_void_p]
         L.pvio_b200_window_get.argtypes = [C.c_void_p, i32p, f64p, C.c_int, i32p, f64p, i32p, i32p]
-        cw = _lib.CWindow()
-        cw.use_inertial = 1 if win.use_inertial else 0
-        cw.cam_q_cs[:] = list(win.cam_q_cs); cw.cam_p_cs[:] = list(win.cam_p_cs)
-        cw.imu_q_cs[:] = list(win.imu_q_cs); cw.imu_p_cs[:] = list(win.imu_p_cs)
-        cw.sqrt_inv_cov[:] = list(np.asarray(win.sqrt_inv_cov, dtype=np.float64).reshape(4))
-        cw.fx, cw.fy, cw.cauchy_a = win.K_fx, win.K_fy, win.cauchy_a
-        cw.plane_sqrt_inv_cov = getattr(win, "plane_sqrt_inv_cov", 0.0)
-        ba._ck(L.pvio_b200_window_reset(self.h, C.byref(cw)))
+        ba._ck(L.pvio_b200_window_reset(self.h, C.byref(_lib.window_constants(win))))
 
     def append_frame(self, state16, fixed=False, imu_record=None):
         s = np.ascontiguousarray(state16, dtype=np.float64)
