@@ -62,9 +62,12 @@ def scharr_deriv(img):
 
 
 def build_pyramid(img, max_level):
+    """buildOpticalFlowPyramid's levels: it halves first and drops the NEW level when it is not larger than the window
+    (a 160 x 120 frame keeps 80 x 60 and 40 x 30 and drops 20 x 15)."""
     levels = [np.ascontiguousarray(img, dtype=np.uint8)]
     for _ in range(max_level):
-        if min(levels[-1].shape) <= WIN:      # buildOpticalFlowPyramid stops when the level gets too small
+        h, w = levels[-1].shape
+        if (w + 1) // 2 <= WIN or (h + 1) // 2 <= WIN:
             break
         levels.append(pyr_down(levels[-1]))
     return levels
@@ -106,9 +109,15 @@ def _patch(P, ix, iy, iw, shift):
     return _descale(a * iw[0] + b * iw[1] + c * iw[2] + d * iw[3], shift)
 
 
+# why a point was lost (return_reasons): its window at level 0 lies outside the frame, its level-0 gradient matrix fails
+# the min-eigenvalue test, it left the frame while iterating at level 0, or its final error window lies outside
+TRACKED, LOST_OUTSIDE, LOST_MIN_EIG, LOST_ITERATING, LOST_ERR_WINDOW = range(5)
+
+
 def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, next_pts_init, max_level=3, max_iter=30, eps=0.01,
-                             min_eig_threshold=1e-4):
-    """Returns (next_pts float32 [n,2], status uint8 [n], err float32 [n])."""
+                             min_eig_threshold=1e-4, return_reasons=False):
+    """Returns (next_pts float32 [n,2], status uint8 [n], err float32 [n]) (+ the reason of each status, int [n],
+    with return_reasons)."""
     f32 = np.float32
     pyr_i, pyr_j = build_pyramid(prev, max_level), build_pyramid(nxt, max_level)
     max_level = min(len(pyr_i), len(pyr_j)) - 1
@@ -117,6 +126,7 @@ def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, next_pts_init, max_level=3, ma
     nxt_pts = np.array(next_pts_init, dtype=f32, copy=True)
     status = np.ones(n, dtype=np.uint8)
     err = np.zeros(n, dtype=f32)
+    reason = np.zeros(n, dtype=np.int32)
     max_iter = min(max(max_iter, 0), 100)
     eps2 = min(max(eps, 0.0), 10.0) ** 2
     half = f32((WIN - 1) * 0.5)
@@ -138,6 +148,7 @@ def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, next_pts_init, max_level=3, ma
                 if level == 0:
                     status[k] = 0
                     err[k] = 0
+                    reason[k] = LOST_OUTSIDE
                 continue
             a, b = f32(prev_pt[0] - f32(ipx)), f32(prev_pt[1] - f32(ipy))
             iw = _weights(a, b)
@@ -152,6 +163,7 @@ def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, next_pts_init, max_level=3, ma
             if min_eig < min_eig_threshold or D < np.finfo(np.float32).eps:
                 if level == 0:
                     status[k] = 0
+                    reason[k] = LOST_MIN_EIG
                 continue
             D = f32(1.0) / D
             next_pt = next_pt - half
@@ -161,6 +173,7 @@ def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, next_pts_init, max_level=3, ma
                 if inx < -WIN or inx >= cols or iny < -WIN or iny >= rows:
                     if level == 0:
                         status[k] = 0
+                        reason[k] = LOST_ITERATING
                     break
                 a, b = f32(next_pt[0] - f32(inx)), f32(next_pt[1] - f32(iny))
                 iwj = _weights(a, b)
@@ -181,9 +194,10 @@ def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, next_pts_init, max_level=3, ma
                 inx, iny = int(np.floor(npnt[0])), int(np.floor(npnt[1]))
                 if inx < -WIN or inx >= cols or iny < -WIN or iny >= rows:
                     status[k] = 0
+                    reason[k] = LOST_ERR_WINDOW
                     continue
                 a, b = f32(npnt[0] - f32(inx)), f32(npnt[1] - f32(iny))
                 iwj = _weights(a, b)
                 diff = _patch(Jp, inx, iny, iwj, W_BITS - 5) - Iw
                 err[k] = f32(np.sum(np.abs(diff)).astype(f32) * f32(1.0 / (32 * WIN * WIN)))
-    return nxt_pts, status, err
+    return (nxt_pts, status, err, reason) if return_reasons else (nxt_pts, status, err)

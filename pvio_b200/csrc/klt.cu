@@ -14,6 +14,7 @@
 #include <cstring>
 #include <vector>
 #include "api_internal.h"
+#include "klt_border.cuh"
 
 namespace pvio {
 
@@ -35,11 +36,6 @@ struct KltLevels {
     int w[kMaxLevels], h[kMaxLevels];
     int n;
 };
-
-__device__ __forceinline__ int reflect101(int i, int n) {
-    i = i < 0 ? -i : i;
-    return i >= n ? 2 * (n - 1) - i : i;
-}
 
 // ---- CLAHE (cv::createCLAHE(clip, tiles)->apply, opencv_image.cpp:138-143; algorithm: OpenCV imgproc/clahe.cpp,
 // restated in oracle/clahe_oracle.py which is pinned bit for bit against cv2).  Image sizes that are multiples
@@ -150,7 +146,9 @@ static int clahe_device(Handle *h, const uint8_t *src, uint8_t *dst, uint8_t *lu
     return 0;
 }
 
-// kBatch: level `level` of frame blockIdx.z of frames[] (frames with fewer levels exit) instead of the arguments
+// kBatch: level `level` of frame blockIdx.z of frames[] (frames with fewer levels exit) instead of the arguments.
+// The taps 2x - 2 .. 2x + 2 of a dw = (sw + 1) / 2 wide level reach -2 and at most 2 dw <= sw + 1: one fold brings them
+// inside whenever sw >= 3 (reflect101_once), and klt_levels only builds a level from one of at least 43 px.
 template <bool kBatch>
 __global__ void pyrdown_kernel(const uint8_t *src, int sw, int sh, uint8_t *dst, int dw, int dh, const KltBatchFrame *frames,
                                int level) {
@@ -166,10 +164,10 @@ __global__ void pyrdown_kernel(const uint8_t *src, int sw, int sh, uint8_t *dst,
     int acc = 0;
 #pragma unroll
     for (int dy = -2; dy <= 2; ++dy) {
-        const uint8_t *row = src + (size_t)reflect101(2 * y + dy, sh) * sw;
+        const uint8_t *row = src + (size_t)reflect101_once(2 * y + dy, sh) * sw;
         int r = 0;
 #pragma unroll
-        for (int dx = -2; dx <= 2; ++dx) r += k[dx + 2] * row[reflect101(2 * x + dx, sw)];
+        for (int dx = -2; dx <= 2; ++dx) r += k[dx + 2] * row[reflect101_once(2 * x + dx, sw)];
         acc += k[dy + 2] * r;
     }
     dst[(size_t)y * dw + x] = (uint8_t)((acc + 128) >> 8);
@@ -395,7 +393,7 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
                    const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points,
                    int max_level, int max_iter, double eps, double clahe_clip, int tiles_x, int tiles_y,
                    uint8_t *prev_eq, uint8_t *next_eq, uint64_t prev_id, uint64_t next_id, int border) {
-    if (width < 2 || height < 2 || stride < width || n_points < 0 || max_level < 0 || max_level >= kMaxLevels || border < 0)
+    if (width < kKltMinFrame || height < kKltMinFrame || stride < width || n_points < 0 || max_level < 0 || max_level >= kMaxLevels || border < 0)
         return fail(h, PVIO_B200_EINVAL, "klt: bad arguments");
     const bool do_clahe = clahe_clip > 0.0;
     if (do_clahe && (tiles_x < 1 || tiles_y < 1 || width % tiles_x || height % tiles_y))
@@ -512,7 +510,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
         if ((size_t)a.slot >= taken.size()) taken.resize(a.slot + 1, 0);
         if (taken[a.slot]) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: a slot appears twice");
         taken[a.slot] = 1;
-        if (a.width < 2 || a.height < 2 || a.stride < a.width || !a.prev_id || !a.next_id)
+        if (a.width < kKltMinFrame || a.height < kKltMinFrame || a.stride < a.width || !a.prev_id || !a.next_id)
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad shape, stride or frame id");
         if (do_clahe && (a.width % tiles_x || a.height % tiles_y))
             return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");

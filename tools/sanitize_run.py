@@ -24,6 +24,12 @@ print('reproj err', ba.compute_reprojection_error(w, st))
 prev, nxt, pts, _ = synth.make_klt_pair(size=(160, 120), n_points=20)
 p, s_, e_ = klt.track_keypoints(ba, prev, nxt, pts)
 print('klt', int(s_.sum()))
+# LK windows folding at a 22-px level (176 x 176, level 3) and on a frame narrower than the window, points beyond the edge
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
+from test_klt_oracle_edges import edge_case
+for size in ((176, 176), (12, 12)):
+    ep, en, epts, einit, _ = edge_case(size)
+    print('klt edges', size, int(klt.track_keypoints(ba, ep, en, epts, einit, raw=True)[1].sum()))
 # PnP, IMU pre-integration, triangulation, Lie self-test, batched device-side solve
 from pvio_b200 import pnp, imu, triangulate as tri
 d = synth.make_pnp()
