@@ -59,19 +59,18 @@ struct KltPyramids {
 // capacity changes.
 struct KltState : KltPyramids {
     int cap_pts = 0;
-    DevBuf<float> pts;                        // [5][cap_pts] both sides: prev [2] | next [2] | err
-    DevBuf<uint8_t> status;                   // [cap_pts] both sides
+    DevBuf<uint8_t> stage;                    // both sides, grown: descriptors and points | positions, errors, status
     DevBuf<uint8_t> raw[2];                   // pre-CLAHE level-0 images (raw entry point only)
     DevBuf<uint8_t> lut;                      // [tiles][256] CLAHE look-up tables
     DevBuf<uint8_t> img;                      // pinned staging for both level-0 images
 };
 
-// one frame a batched call equalises or downsamples on the device (klt.cu: batch_track_impl, detect.cu:
-// batch_detect_impl): its raw pixels, CLAHE into level 0 of `pyr`, then pyrDown level by level
+// one frame the tracker or the detector equalises or downsamples on the device (klt.cu, detect.cu), as the CLAHE and
+// pyrDown kernels read it: its raw pixels, CLAHE into level 0 of `pyr`, then pyrDown level by level
 struct KltBatchFrame {
     const uint8_t *raw;                       // level-0 pixels as uploaded (raw when CLAHE runs)
     uint8_t *lut;                             // [tiles][256] its CLAHE tables
-    uint8_t *pyr;                             // its pyramid (the detector: level 0 only, in its scratch)
+    uint8_t *pyr;                             // its pyramid (the detector and clahe_impl: level 0 only)
     int levels, tw, th, clip;
     float lut_scale;
     int w[kMaxLevels], h[kMaxLevels];
@@ -98,7 +97,7 @@ struct DetectState {
     DevBuf<float> resp;
     DevBuf<unsigned long long> keys;
     DevBuf<unsigned long long> keys_sorted;   // both sides
-    DevBuf<int> counters;                     // both sides: [0] max response bits, [1] candidate count
+    DevBuf<uint8_t> stage;                    // both sides: the frame's descriptors and counters (detect.cu: DetectStage)
     DevBuf<uint8_t> cub_tmp;
 };
 
@@ -112,8 +111,7 @@ struct DetectBatchState {
 
 // fmat.cu: RANSAC buffers, grown to the largest point count / iteration budget seen
 struct FmState {
-    DevBuf<float> pts;                        // [2][n][2] p then q, both sides
-    DevBuf<int> sched;                        // [s][7], both sides
+    DevBuf<uint8_t> stage;                    // both sides: problem, mask job, counts | p, q | schedule [s][7] (fmat.cu: FmStage)
     DevBuf<int> counts;                       // [s][4] nmodels, count / median bits of each model, both sides
     DevBuf<double> F;                         // [s][3][9]
     DevBuf<unsigned> masks;                   // [s][3][words]
@@ -364,7 +362,6 @@ int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, dou
                          const pvio_b200_options *opt, pvio_b200_summary *summaries);
 // klt.cu / detect.cu
 const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int height, double clahe_clip);
-int klt_clahe_device(Handle *h, const uint8_t *d_src, uint8_t *d_dst, uint8_t *d_lut, int width, int height, double clip, int tiles_x, int tiles_y);
 // klt.cu, used by detect.cu: cv::CLAHE's per-tile constants of a w x h frame, and CLAHE of n_frames frames (frames in
 // device memory; each equalises raw into level 0 of pyr) as 2 launches whose grids cover max_w x max_h
 void klt_clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_y, int &tw, int &th, int &clip, float &lut_scale);

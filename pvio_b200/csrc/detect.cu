@@ -46,7 +46,7 @@ struct DetectResult {
     unsigned corner[kMaxCorners];             // the GFTT corners in order, as pixel indices y * w + x
 };
 
-// one frame of a batched call, as the kernels read it
+// one frame as the kernels read it (the single call: frame 0 of one)
 struct DetectBatchFrame {
     const uint8_t *img;                       // the equalised frame (a cached level 0, uploaded pixels, or CLAHE output)
     float *resp;                              // [h][w] Harris response
@@ -60,19 +60,24 @@ struct DetectBatchFrame {
     int n_pre, gw, gh, hbits;                 // min-distance grid gw x gh; Poisson hash table of 2^hbits cells
 };
 
+// the single call's staging (DetectState::stage, both sides): its frame, the frame CLAHE equalises, zeroed counters
+struct DetectStage {
+    DetectBatchFrame frame;
+    KltBatchFrame clahe;
+    int counters[2];                          // [0] max response bits, [1] candidate count
+};
+
 // one thread per pixel; the (kTX + 2) x (kTY + 2) tile of the three products in shared memory.  Every operation is a
 // separately rounded fp32 operation except the one fused multiply-add of the Sobel-x column pass (this file is
-// compiled with -fmad=false).  kBatch: frame blockIdx.z of frames[] instead of the arguments (blocks outside a smaller
-// frame exit).
-template <bool kBatch>
-__global__ void __launch_bounds__(kTX *kTY) harris_response_kernel(const uint8_t *img, int w, int h, float k, float *resp, int *max_bits,
-                                                                   const DetectBatchFrame *frames) {
+// compiled with -fmad=false).  The frame is frames[blockIdx.z] (blocks outside a smaller frame exit).
+__global__ void __launch_bounds__(kTX *kTY) harris_response_kernel(float k, const DetectBatchFrame *frames) {
     __shared__ float cxx[kTY + 2][kTX + 2], cxy[kTY + 2][kTX + 2], cyy[kTY + 2][kTX + 2];
-    if constexpr (kBatch) {
-        const DetectBatchFrame &f = frames[blockIdx.z];
-        img = f.img; w = f.w; h = f.h; resp = f.resp; max_bits = f.counters;
-        if ((int)blockIdx.x * kTX >= w || (int)blockIdx.y * kTY >= h) return;     // block-uniform
-    }
+    const DetectBatchFrame &f = frames[blockIdx.z];
+    const uint8_t *img = f.img;
+    float *resp = f.resp;
+    int *max_bits = f.counters;
+    const int w = f.w, h = f.h;
+    if ((int)blockIdx.x * kTX >= w || (int)blockIdx.y * kTY >= h) return;     // block-uniform
     const int x0 = blockIdx.x * kTX, y0 = blockIdx.y * kTY, tid = threadIdx.y * kTX + threadIdx.x;
     // the box filter's border pixel is the product AT the mirror pixel: evaluate the products at reflected coordinates
     for (int e = tid; e < (kTY + 2) * (kTX + 2); e += kTX * kTY) {
@@ -119,14 +124,14 @@ __global__ void __launch_bounds__(kTX *kTY) harris_response_kernel(const uint8_t
     if (r > 0.0f) atomicMax(max_bits, __float_as_int(r));       // positive floats order like their bit patterns
 }
 
-// kBatch: frame blockIdx.z of frames[] instead of the arguments; its keys go to its own segment
-template <bool kBatch>
-__global__ void nms_compact_kernel(const float *resp, int w, int h, double quality, const int *max_bits, unsigned long long *keys,
-                                   int *count, int cap, const DetectBatchFrame *frames) {
-    if constexpr (kBatch) {
-        const DetectBatchFrame &f = frames[blockIdx.z];
-        resp = f.resp; w = f.w; h = f.h; max_bits = f.counters; keys = f.keys; count = f.counters + 1; cap = f.cap;
-    }
+// The frame is frames[blockIdx.z]; its keys go to its own segment
+__global__ void nms_compact_kernel(double quality, const DetectBatchFrame *frames) {
+    const DetectBatchFrame &f = frames[blockIdx.z];
+    const float *resp = f.resp;
+    const int *max_bits = f.counters;
+    unsigned long long *keys = f.keys;
+    int *count = f.counters + 1;
+    const int w = f.w, h = f.h, cap = f.cap;
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x < 1 || y < 1 || x >= w - 1 || y >= h - 1) return;      // goodFeaturesToTrack visits interior pixels only
     const float mx = __int_as_float(*max_bits);
@@ -221,7 +226,7 @@ int ensure(Handle *h, int w, int hgt) {
     TRY(reserve(h, d.resp, px, kDevice));
     TRY(reserve(h, d.keys, d.cap, kDevice));
     TRY(reserve(h, d.keys_sorted, d.cap, kBoth));
-    TRY(reserve(h, d.counters, 2, kBoth));
+    TRY(reserve(h, d.stage, sizeof(DetectStage), kBoth));
     TRY(reserve(h, d.cub_tmp, d.cub_bytes, kDevice));
     return 0;
 }
@@ -568,10 +573,8 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     CK(h, cudaMemcpyAsync(ds, hs, o_up, cudaMemcpyHostToDevice, st));
     const DetectBatchFrame *d_frm = reinterpret_cast<const DetectBatchFrame *>(ds + o_frm);
     if (n_eq > 0) klt_batch_clahe(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_eq, tiles_x, tiles_y, eq_w, eq_h);
-    harris_response_kernel<true><<<dim3((max_w + kTX - 1) / kTX, (max_h + kTY - 1) / kTY, n), dim3(kTX, kTY), 0, st>>>(
-        nullptr, 0, 0, 0.04f, nullptr, nullptr, d_frm);
-    nms_compact_kernel<true><<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n), dim3(32, 8), 0, st>>>(
-        nullptr, 0, 0, 1.0e-3, nullptr, nullptr, nullptr, 0, d_frm);
+    harris_response_kernel<<<dim3((max_w + kTX - 1) / kTX, (max_h + kTY - 1) / kTY, n), dim3(kTX, kTY), 0, st>>>(0.04f, d_frm);
+    nms_compact_kernel<<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n), dim3(32, 8), 0, st>>>(1.0e-3, d_frm);
     h->launches += 2;
     size_t tmp = cub_bytes;
     CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(
@@ -627,29 +630,35 @@ extern "C" int pvio_b200_detect_keypoints(pvio_b200_handle hh, uint64_t frame_id
     TRY(ensure(h, width, height));
     DetectState &d = h->detect;
     const size_t px = (size_t)width * height;
+    DetectStage &S = *reinterpret_cast<DetectStage *>(d.stage.h);
+    DetectStage *dS = reinterpret_cast<DetectStage *>(d.stage.d);
+    memset(&S, 0, sizeof(S));
     const uint8_t *src = klt_cached_level0(h, frame_id, width, height, clahe_clip);
+    const bool clahe = !src && clahe_clip > 0.0;
     if (!src) {
         if (!image || stride < width) return fail(h, PVIO_B200_EINVAL, "detect_keypoints: frame not cached and no pixels given");
         for (int y = 0; y < height; ++y) memcpy(d.img.h + (size_t)y * width, image + (size_t)y * stride, width);
-        if (clahe_clip > 0.0) {
+        if (clahe) {
             TRY(reserve(h, d.lut, (size_t)tiles_x * tiles_y * 256, kDevice));
-            CK(h, cudaMemcpyAsync(d.raw.d, d.img.h, px, cudaMemcpyHostToDevice, h->stream));
-            TRY(klt_clahe_device(h, d.raw.d, d.img.d, d.lut.d, width, height, clahe_clip, tiles_x, tiles_y));
-        } else {
-            CK(h, cudaMemcpyAsync(d.img.d, d.img.h, px, cudaMemcpyHostToDevice, h->stream));
+            KltBatchFrame &K = S.clahe;
+            K.raw = d.raw.d; K.lut = d.lut.d; K.pyr = d.img.d;
+            K.levels = 1; K.w[0] = width; K.h[0] = height;
+            klt_clahe_params(width, height, clahe_clip, tiles_x, tiles_y, K.tw, K.th, K.clip, K.lut_scale);
         }
+        CK(h, cudaMemcpyAsync(clahe ? d.raw.d : d.img.d, d.img.h, px, cudaMemcpyHostToDevice, h->stream));
         src = d.img.d;
     }
-    int *counters = d.counters.d;
-    CK(h, cudaMemsetAsync(counters, 0, sizeof(int) * 2, h->stream));
-    harris_response_kernel<false><<<dim3((width + kTX - 1) / kTX, (height + kTY - 1) / kTY), dim3(kTX, kTY), 0, h->stream>>>(
-        src, width, height, 0.04f, d.resp.d, counters, nullptr);
-    nms_compact_kernel<false><<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, h->stream>>>(
-        d.resp.d, width, height, 1.0e-3, counters, d.keys.d, counters + 1, d.cap, nullptr);
+    DetectBatchFrame &F = S.frame;
+    F.img = src; F.resp = d.resp.d; F.keys = d.keys.d; F.counters = dS->counters;
+    F.w = width; F.h = height; F.cap = d.cap;
+    CK(h, cudaMemcpyAsync(dS, &S, sizeof(S), cudaMemcpyHostToDevice, h->stream));
+    if (clahe) klt_batch_clahe(h, &dS->clahe, 1, tiles_x, tiles_y, width, height);
+    harris_response_kernel<<<dim3((width + kTX - 1) / kTX, (height + kTY - 1) / kTY), dim3(kTX, kTY), 0, h->stream>>>(0.04f, &dS->frame);
+    nms_compact_kernel<<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, h->stream>>>(1.0e-3, &dS->frame);
     h->launches += 2;
-    CK(h, cudaMemcpyAsync(d.counters.h, counters, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(S.counters, dS->counters, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
-    const int n = std::min(d.counters.h[1], d.cap);
+    const int n = std::min(S.counters[1], d.cap);
     std::vector<float> corners;
     if (n > 0) {
         size_t tmp = d.cub_bytes;

@@ -280,25 +280,21 @@ __device__ __forceinline__ float fm_error(const double *F, float2 m1, float2 m2)
 
 constexpr int kWarpsPerCta = 4;
 
-// One warp per iteration of the schedule.  lmeds == 0: counts[it] = {nmodels, inliers of model 0, 1, 2}, masks[it][k][nw];
-// lmeds == 1 (n < 32): counts[it] = {nmodels, float bits of the median error of model 0, 1, 2}.
-// kBatch: problem blockIdx.y of probs[] instead of the arguments; its survivor and iteration counts come from the
-// schedule kernel, and it runs LMedS below 15 survivors as the single call does.
-template <bool kBatch>
-__global__ void __launch_bounds__(32 * kWarpsPerCta) fm_hypotheses_kernel(const float2 *p, const float2 *q, int n, const int *sched,
-                                                                          int iters, float thr2, int lmeds, int nw, int *counts,
-                                                                          double *Fout, unsigned *masks,
-                                                                          const FmBatchProblem *probs) {
+// One warp per iteration of the schedule of problem probs[blockIdx.y], whose match and iteration counts are P.surv (the
+// schedule kernel's or the single call's).  RANSAC (n >= 15): counts[it] = {nmodels, inliers of model 0, 1, 2},
+// masks[it][k][nw]; LMedS (n < 15): counts[it] = {nmodels, float bits of the median error of model 0, 1, 2}.
+__global__ void __launch_bounds__(32 * kWarpsPerCta) fm_hypotheses_kernel(float thr2, const FmBatchProblem *probs) {
     __shared__ double sF[kWarpsPerCta][3][9];
     __shared__ int sN[kWarpsPerCta];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int it = blockIdx.x * kWarpsPerCta + warp;
-    if constexpr (kBatch) {
-        const FmBatchProblem &P = probs[blockIdx.y];
-        n = P.surv[0]; iters = P.surv[1];       // iters == 0 below 8 survivors
-        p = P.p; q = P.q; sched = P.sched; counts = P.counts; Fout = P.F; masks = P.masks;
-        lmeds = n < 15 ? 1 : 0; nw = (n + 31) / 32;
-    }
+    const FmBatchProblem &P = probs[blockIdx.y];
+    const int n = P.surv[0], iters = P.surv[1], lmeds = n < 15 ? 1 : 0, nw = (n + 31) / 32;    // iters == 0 below 8 survivors
+    const float2 *p = P.p, *q = P.q;
+    const int *sched = P.sched;
+    int *counts = P.counts;
+    double *Fout = P.F;
+    unsigned *masks = P.masks;
     if (it >= iters) return;
     if (lane == 0) {
         int idx[7];
@@ -343,22 +339,21 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta) fm_hypotheses_kernel(const 
     }
 }
 
-// mask of one model under one threshold (LMedS: the inliers of the best model under sigma; n == 7: not needed).
-// kBatch: the job jobs[blockIdx.y] instead of the arguments; a RANSAC job copies the mask fm_hypotheses_kernel stored.
-template <bool kBatch>
-__global__ void fm_mask_kernel(const float2 *p, const float2 *q, int n, const double *Fm, float thr2, unsigned *mask,
-                               const FmMaskJob *jobs) {
+// the mask of the job jobs[blockIdx.y]: LMedS, the inliers of the best model under sigma; RANSAC, a copy of the mask
+// fm_hypotheses_kernel stored (n == 7: not needed)
+__global__ void fm_mask_kernel(const FmMaskJob *jobs) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if constexpr (kBatch) {
-        const FmMaskJob &J = jobs[blockIdx.y];
-        if ((i >> 5) * 32 >= J.n) return;       // whole warps
-        mask = J.out;
-        if (J.src) {
-            if ((threadIdx.x & 31) == 0) mask[i >> 5] = J.src[i >> 5];
-            return;
-        }
-        p = J.p; q = J.q; n = J.n; Fm = J.F; thr2 = J.thr2;
+    const FmMaskJob &J = jobs[blockIdx.y];
+    if ((i >> 5) * 32 >= J.n) return;       // whole warps
+    unsigned *mask = J.out;
+    if (J.src) {
+        if ((threadIdx.x & 31) == 0) mask[i >> 5] = J.src[i >> 5];
+        return;
     }
+    const float2 *p = J.p, *q = J.q;
+    const double *Fm = J.F;
+    const float thr2 = J.thr2;
+    const int n = J.n;
     double F[9];
     for (int k = 0; k < 9; ++k) F[k] = Fm[k];
     bool in = false;
@@ -396,12 +391,20 @@ __global__ void __launch_bounds__(32) fm_schedule_kernel(const FmBatchProblem *p
     P.surv[0] = s; P.surv[1] = have;
 }
 
+// the single call's staging (FmState::stage, both sides), followed by the matches p[n], q[n] (float2) and the schedule
+// [iterations][7]; the mask job is written after the replay and read in place
+struct FmStage {
+    FmBatchProblem prob;
+    FmMaskJob job;
+    int surv[2];                              // matches, iterations that have a subset
+};
+static_assert(sizeof(FmStage) % sizeof(float2) == 0, "the matches follow the record");
+
 // room for n points and s iterations: at least 1024 points and 1000 iterations, grown on demand
 int fm_reserve(Handle *h, int n, int s) {
     FmState &f = h->fm;
     const size_t cn = std::max(n, 1024), cs = std::max(s, 1000), cw = (cn + 31) / 32;
-    TRY(reserve(h, f.pts, 4 * cn, kBoth));
-    TRY(reserve(h, f.sched, 7 * cs, kBoth));
+    TRY(reserve(h, f.stage, sizeof(FmStage) + sizeof(float2) * 2 * cn + sizeof(int) * 7 * cs, kBoth));
     TRY(reserve(h, f.counts, 4 * cs, kBoth));
     TRY(reserve(h, f.F, 27 * cs, kDevice));
     TRY(reserve(h, f.masks, 3 * cs * cw, kDevice));
@@ -486,11 +489,15 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
     const int budget = seven ? 1 : ransac ? max_iters : fm_lmeds_iters(confidence, max_iters);
     TRY(fm_reserve(h, n, budget));
     FmState &f = h->fm;
-    std::memcpy(f.pts.h, p, sizeof(float) * 2 * n);
-    std::memcpy(f.pts.h + 2 * n, q, sizeof(float) * 2 * n);
+    FmStage &S = *reinterpret_cast<FmStage *>(f.stage.h);
+    FmStage *dS = reinterpret_cast<FmStage *>(f.stage.d);
+    float *hp = reinterpret_cast<float *>(&S + 1);
+    int *sched = reinterpret_cast<int *>(hp + 4 * n);
+    std::memcpy(hp, p, sizeof(float) * 2 * n);
+    std::memcpy(hp + 2 * n, q, sizeof(float) * 2 * n);
     int have = budget;                        // iterations that have a subset
     if (seven) {
-        for (int i = 0; i < 7; ++i) f.sched.h[i] = i;
+        for (int i = 0; i < 7; ++i) sched[i] = i;
     } else if (schedule) {
         if (n_schedule < 1) return fail(h, PVIO_B200_EINVAL, "find_fundamental_mask: empty schedule");
         have = std::min(budget, n_schedule);
@@ -499,24 +506,26 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
             for (int i = 0; i < 7; ++i) {
                 const int v = schedule[7 * it + i];
                 if (v < 0 || v >= n) return fail(h, PVIO_B200_EINVAL, "find_fundamental_mask: schedule index out of range");
-                f.sched.h[7 * it + i] = v;
+                sched[7 * it + i] = v;
             }
         }
     } else {
-        have = cv_schedule(p, q, n, budget, ransac ? 10000 : 1000, f.sched.h);
+        have = cv_schedule(p, q, n, budget, ransac ? 10000 : 1000, sched);
     }
     if (have == 0) {                          // getSubset failed at iteration 0: run() returns false, the mask stays as created
         std::memset(mask, 0, n);
         return finish(0);
     }
+    // the problem as the batched tracker's kernel reads it: n matches, `have` iterations.  The kernel runs the LMedS
+    // branch for n == 7 too (the call draws no schedule then); the replay of n == 7 reads counts[0] only, which both
+    // branches write alike, and its mask is all ones.
     cudaStream_t st = h->stream;
     const int nw = (n + 31) / 32;
-    float2 *dp = (float2 *)f.pts.d, *dq = (float2 *)(f.pts.d + 2 * n);
-    CK(h, cudaMemcpyAsync(f.pts.d, f.pts.h, sizeof(float) * 4 * n, cudaMemcpyHostToDevice, st));
-    CK(h, cudaMemcpyAsync(f.sched.d, f.sched.h, sizeof(int) * 7 * have, cudaMemcpyHostToDevice, st));
-    const float thr2 = (float)(threshold * threshold);
-    fm_hypotheses_kernel<false><<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>(
-        dp, dq, n, f.sched.d, have, thr2, (!ransac && !seven) ? 1 : 0, nw, f.counts.d, f.F.d, f.masks.d, nullptr);
+    float2 *dp = reinterpret_cast<float2 *>(dS + 1), *dq = dp + n;
+    S.prob = FmBatchProblem{nullptr, nullptr, nullptr, dp, dq, reinterpret_cast<int *>(dq + n), f.counts.d, f.F.d, f.masks.d, dS->surv, n, have};
+    S.surv[0] = n; S.surv[1] = have;
+    CK(h, cudaMemcpyAsync(dS, &S, sizeof(FmStage) + sizeof(float2) * 2 * n + sizeof(int) * 7 * have, cudaMemcpyHostToDevice, st));
+    fm_hypotheses_kernel<<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>((float)(threshold * threshold), &dS->prob);
     h->launches++;
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(f.counts.h, f.counts.d, sizeof(int) * 4 * have, cudaMemcpyDeviceToHost, st));
@@ -530,8 +539,10 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
         return finish(0);
     }
     if (!ransac && !seven) {
-        fm_mask_kernel<false><<<(n + 31) / 32, 32, 0, st>>>(dp, dq, n, f.F.d + (size_t)(3 * best_it + best_k) * 9, thr_lmeds,
-                                                            f.masks.d, nullptr);
+        S.job = FmMaskJob{dp, dq, f.F.d + (size_t)(3 * best_it + best_k) * 9, nullptr, f.masks.d, thr_lmeds, n};
+        FmMaskJob *d_job = nullptr;           // read in place from the pinned staging (mapped: unified addressing)
+        CK(h, cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_job), &S.job, 0));
+        fm_mask_kernel<<<nw, 32, 0, st>>>(d_job);
         h->launches++;
         CK(h, cudaGetLastError());
     }
@@ -555,14 +566,13 @@ void fm_batch_schedule(Handle *h, const FmBatchProblem *probs, int n, int max_it
 
 // every iteration of every pair in one launch: blockIdx.y is the pair, warps beyond its schedule exit at once
 void fm_batch_hypotheses(Handle *h, const FmBatchProblem *probs, int n, int max_budget, float thr2) {
-    fm_hypotheses_kernel<true><<<dim3((max_budget + kWarpsPerCta - 1) / kWarpsPerCta, n), 32 * kWarpsPerCta, 0, h->stream>>>(
-        nullptr, nullptr, 0, nullptr, 0, thr2, 0, 0, nullptr, nullptr, nullptr, probs);
+    fm_hypotheses_kernel<<<dim3((max_budget + kWarpsPerCta - 1) / kWarpsPerCta, n), 32 * kWarpsPerCta, 0, h->stream>>>(thr2, probs);
     h->launches++;
 }
 
 // every winner's mask in one launch: one warp per mask word, blockIdx.y the pair
 void fm_batch_masks(Handle *h, const FmMaskJob *jobs, int n, int max_words) {
-    fm_mask_kernel<true><<<dim3((max_words + 3) / 4, n), 128, 0, h->stream>>>(nullptr, nullptr, 0, nullptr, 0.f, nullptr, jobs);
+    fm_mask_kernel<<<dim3((max_words + 3) / 4, n), 128, 0, h->stream>>>(jobs);
     h->launches++;
 }
 

@@ -22,14 +22,6 @@ constexpr int kWin = 21;
 constexpr int kWBits = 14;
 constexpr int kKltWarps = 4;
 
-// 20-pixel border rejection of OpenCvImage::track_keypoints (opencv_image.cpp:106-108) on the device
-__global__ void klt_border_kernel(const float *pts, uint8_t *status, int n, int w, int h, int border) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float x = pts[2 * i], y = pts[2 * i + 1];
-    if (x < (float)border || x >= (float)(w - border) || y < (float)border || y >= (float)(h - border)) status[i] = 0;
-}
-
 struct KltLevels {
     const uint8_t *I[kMaxLevels];
     const uint8_t *J[kMaxLevels];
@@ -42,17 +34,16 @@ struct KltLevels {
 // of the tile grid only.  Kernel 1: one CTA per tile -- histogram in shared memory, clip + redistribute, prefix
 // sum, LUT = cvRound(cdf * 255 / area).  Kernel 2: one thread per pixel, bilinear blend of the four neighbouring
 // tiles' LUTs in OpenCV's float32 operation order (explicit _rn intrinsics: no FMA contraction).
-// kBatch: frame blockIdx.y of frames[] (lut kernel) / blockIdx.z (apply kernel) instead of the arguments.
-template <bool kBatch>
-__global__ void __launch_bounds__(256) clahe_lut_kernel(const uint8_t *src, int w, int tw, int th, int tiles_x,
-                                                        int clip, float lut_scale, uint8_t *lut, const KltBatchFrame *frames) {
+// The frame is frames[blockIdx.y] (lut kernel) / frames[blockIdx.z] (apply kernel).
+__global__ void __launch_bounds__(256) clahe_lut_kernel(int tiles_x, const KltBatchFrame *frames) {
     __shared__ int hist[256];
     __shared__ int wsum[8];
     __shared__ int total_clipped;
-    if constexpr (kBatch) {
-        const KltBatchFrame &f = frames[blockIdx.y];
-        src = f.raw; w = f.w[0]; tw = f.tw; th = f.th; clip = f.clip; lut_scale = f.lut_scale; lut = f.lut;
-    }
+    const KltBatchFrame &fr = frames[blockIdx.y];
+    const uint8_t *src = fr.raw;
+    uint8_t *lut = fr.lut;
+    const int w = fr.w[0], tw = fr.tw, th = fr.th, clip = fr.clip;
+    const float lut_scale = fr.lut_scale;
     const int t = blockIdx.x, tx = t % tiles_x, ty = t / tiles_x, tid = threadIdx.x;
     hist[tid] = 0;
     __syncthreads();
@@ -90,14 +81,12 @@ __global__ void __launch_bounds__(256) clahe_lut_kernel(const uint8_t *src, int 
     lut[(size_t)t * 256 + tid] = (uint8_t)min(max(__float2int_rn(f), 0), 255);
 }
 
-template <bool kBatch>
-__global__ void clahe_apply_kernel(const uint8_t *src, int w, int h, int tw, int th, int tiles_x, int tiles_y,
-                                   const uint8_t *lut, uint8_t *dst, const KltBatchFrame *frames) {
+__global__ void clahe_apply_kernel(int tiles_x, int tiles_y, const KltBatchFrame *frames) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    if constexpr (kBatch) {
-        const KltBatchFrame &f = frames[blockIdx.z];
-        src = f.raw; w = f.w[0]; h = f.h[0]; tw = f.tw; th = f.th; lut = f.lut; dst = f.pyr;
-    }
+    const KltBatchFrame &f = frames[blockIdx.z];
+    const uint8_t *src = f.raw, *lut = f.lut;
+    uint8_t *dst = f.pyr;
+    const int w = f.w[0], h = f.h[0], tw = f.tw, th = f.th;
     if (x >= w || y >= h) return;
     const float inv_tw = __fdiv_rn(1.0f, (float)tw), inv_th = __fdiv_rn(1.0f, (float)th);
     const float txf = __fsub_rn(__fmul_rn((float)x, inv_tw), 0.5f), tyf = __fsub_rn(__fmul_rn((float)y, inv_th), 0.5f);
@@ -124,41 +113,23 @@ void klt_clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_
     lut_scale = 255.0f / (float)area;
 }
 
-// CLAHE of the frames of a batched call, each into level 0 of its f.pyr
+// CLAHE of n_frames frames (in device memory), each into level 0 of its f.pyr
 void klt_batch_clahe(Handle *h, const KltBatchFrame *frames, int n_frames, int tiles_x, int tiles_y, int max_w, int max_h) {
-    clahe_lut_kernel<true><<<dim3((unsigned)(tiles_x * tiles_y), n_frames), 256, 0, h->stream>>>(nullptr, 0, 0, 0, tiles_x, 0, 0.f,
-                                                                                               nullptr, frames);
-    clahe_apply_kernel<true><<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n_frames), dim3(32, 8), 0, h->stream>>>(
-        nullptr, 0, 0, 0, 0, tiles_x, tiles_y, nullptr, nullptr, frames);
+    clahe_lut_kernel<<<dim3((unsigned)(tiles_x * tiles_y), n_frames), 256, 0, h->stream>>>(tiles_x, frames);
+    clahe_apply_kernel<<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n_frames), dim3(32, 8), 0, h->stream>>>(tiles_x, tiles_y, frames);
     h->launches += 2;
 }
 
-// device-resident CLAHE of a w x h image (row stride w)
-static int clahe_device(Handle *h, const uint8_t *src, uint8_t *dst, uint8_t *lut, int w, int hgt, double clip_limit,
-                        int tiles_x, int tiles_y) {
-    int tw, th, clip;
-    float lut_scale;
-    klt_clahe_params(w, hgt, clip_limit, tiles_x, tiles_y, tw, th, clip, lut_scale);
-    clahe_lut_kernel<false><<<tiles_x * tiles_y, 256, 0, h->stream>>>(src, w, tw, th, tiles_x, clip, lut_scale, lut, nullptr);
-    dim3 b(32, 8), g((w + 31) / 32, (hgt + 7) / 8);
-    clahe_apply_kernel<false><<<g, b, 0, h->stream>>>(src, w, hgt, tw, th, tiles_x, tiles_y, lut, dst, nullptr);
-    h->launches += 2;
-    return 0;
-}
-
-// kBatch: level `level` of frame blockIdx.z of frames[] (frames with fewer levels exit) instead of the arguments.
+// Level `level` of frame frames[blockIdx.z] (frames with fewer levels exit).
 // The taps 2x - 2 .. 2x + 2 of a dw = (sw + 1) / 2 wide level reach -2 and at most 2 dw <= sw + 1: one fold brings them
 // inside whenever sw >= 3 (reflect101_once), and klt_levels only builds a level from one of at least 43 px.
-template <bool kBatch>
-__global__ void pyrdown_kernel(const uint8_t *src, int sw, int sh, uint8_t *dst, int dw, int dh, const KltBatchFrame *frames,
-                               int level) {
+__global__ void pyrdown_kernel(const KltBatchFrame *frames, int level) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    if constexpr (kBatch) {
-        const KltBatchFrame &f = frames[blockIdx.z];
-        if (level >= f.levels) return;
-        src = f.pyr + f.off[level - 1]; sw = f.w[level - 1]; sh = f.h[level - 1];
-        dst = f.pyr + f.off[level]; dw = f.w[level]; dh = f.h[level];
-    }
+    const KltBatchFrame &f = frames[blockIdx.z];
+    if (level >= f.levels) return;
+    const uint8_t *src = f.pyr + f.off[level - 1];
+    uint8_t *dst = f.pyr + f.off[level];
+    const int sw = f.w[level - 1], sh = f.h[level - 1], dw = f.w[level], dh = f.h[level];
     if (x >= dw || y >= dh) return;
     const int k[5] = {1, 4, 6, 4, 1};
     int acc = 0;
@@ -189,13 +160,11 @@ __device__ __forceinline__ void bilinear_weights(float a, float b, int &w00, int
 
 __device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
 
-// kBatch: the points of all pairs of a batched call; point pt belongs to pair pair_of[pt], whose pyramids are
-// pairs[pair_of[pt]] (in device memory) instead of L, and the border test of that pair's frame size (border > 0) runs
-// here rather than in klt_border_kernel.
-template <bool kBatch>
+// Point pt belongs to pair pair_of[pt], whose pyramids are pairs[pair_of[pt]] (in device memory); with border > 0 the
+// 20-pixel border rejection of OpenCvImage::track_keypoints (opencv_image.cpp:106-108) on that pair's frame size follows.
 __global__ void __launch_bounds__(32 * kKltWarps)
-klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points,
-                 int max_iter, double eps2, float min_eig_thr, const KltLevels *pairs, const int *pair_of, int border) {
+klt_track_kernel(const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points, int max_iter, double eps2,
+                 float min_eig_thr, const KltLevels *pairs, const int *pair_of, int border) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int pt = blockIdx.x * kKltWarps + warp;
     __shared__ int Ipatch[kKltWarps][24 * 24];
@@ -203,7 +172,7 @@ klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *s
     __shared__ short IWin[kKltWarps][kWin * kWin];
     __shared__ short dIWin[kKltWarps][kWin * kWin * 2];
     if (pt >= n_points) return;
-    const KltLevels &Lv = kBatch ? pairs[pair_of[pt]] : L;
+    const KltLevels &Lv = pairs[pair_of[pt]];
     const float px0 = prev_pts[2 * pt], py0 = prev_pts[2 * pt + 1];
     float nx = next_pts[2 * pt], ny = next_pts[2 * pt + 1];      // OPTFLOW_USE_INITIAL_FLOW
     bool st = true;
@@ -327,7 +296,7 @@ klt_track_kernel(KltLevels L, const float *prev_pts, float *next_pts, uint8_t *s
     if (lane == 0) {
         next_pts[2 * pt] = nx; next_pts[2 * pt + 1] = ny;
         bool keep = st;
-        if (kBatch && border > 0) {           // klt_border_kernel's test on the pair's level-0 size
+        if (border > 0) {
             const int w = Lv.w[0], h = Lv.h[0];
             if (nx < (float)border || nx >= (float)(w - border) || ny < (float)border || ny >= (float)(h - border)) keep = false;
         }
@@ -375,6 +344,61 @@ static void klt_lookup(const KltPyramids &k, uint64_t prev_id, uint64_t next_id,
     slot[0] = sp; slot[1] = sn;
 }
 
+namespace {
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+}  // namespace
+
+// The pyramids of n_frames new frames (frames: host copies of the descriptors at d_frames): CLAHE into level 0, or
+// without CLAHE a device copy of the raw pixels into level 0 unless they were uploaded there; then one pyrDown launch per
+// level over every frame (grid z)
+static int klt_build_pyramids(Handle *h, const KltBatchFrame *frames, const KltBatchFrame *d_frames, int n_frames, bool clahe,
+                              int tiles_x, int tiles_y) {
+    int levels = 1, lw[kMaxLevels] = {}, lh[kMaxLevels] = {};
+    for (int j = 0; j < n_frames; ++j) {
+        const KltBatchFrame &f = frames[j];
+        levels = std::max(levels, f.levels);
+        for (int l = 0; l < f.levels; ++l) { lw[l] = std::max(lw[l], f.w[l]); lh[l] = std::max(lh[l], f.h[l]); }
+        if (!clahe && f.raw != f.pyr)
+            CK(h, cudaMemcpyAsync(f.pyr, f.raw, (size_t)f.w[0] * f.h[0], cudaMemcpyDeviceToDevice, h->stream));
+    }
+    if (clahe) klt_batch_clahe(h, d_frames, n_frames, tiles_x, tiles_y, lw[0], lh[0]);
+    for (int l = 1; l < levels; ++l) {
+        pyrdown_kernel<<<dim3((lw[l] + 31) / 32, (lh[l] + 7) / 8, n_frames), dim3(32, 8), 0, h->stream>>>(d_frames, l);
+        ++h->launches;
+    }
+    return 0;
+}
+
+// LK + border over n_pts points of the pairs `pairs` (every array in device memory)
+static void klt_lk(Handle *h, const KltLevels *pairs, const int *pair_of, const float *prev_pts, float *next_pts, uint8_t *status,
+                   float *err, size_t n_pts, int max_iter, double eps, int border) {
+    const int mi = std::min(std::max(max_iter, 0), 100);
+    const double e = std::min(std::max(eps, 0.0), 10.0);
+    klt_track_kernel<<<(unsigned)((n_pts + kKltWarps - 1) / kKltWarps), 32 * kKltWarps, 0, h->stream>>>(
+        prev_pts, next_pts, status, err, (int)n_pts, mi, e * e, 1e-4f, pairs, pair_of, border);
+    ++h->launches;
+}
+
+// the descriptor of the pair s.pyr[slot[0]] (prev), s.pyr[slot[1]] (next) as klt_track_kernel reads it
+static KltLevels klt_pair(const KltPyramids &s, const int slot[2]) {
+    KltLevels L{};
+    L.n = s.levels;
+    for (int l = 0; l < s.levels; ++l) {
+        L.I[l] = s.pyr[slot[0]].d + s.off[l]; L.J[l] = s.pyr[slot[1]].d + s.off[l];
+        L.w[l] = s.lw[l]; L.h[l] = s.lh[l];
+    }
+    return L;
+}
+
+// the descriptor of a new frame whose pyramid is s.pyr[i]: its pixels at raw, its CLAHE tables at lut (clip > 0)
+static KltBatchFrame klt_frame(const KltPyramids &s, int i, const uint8_t *raw, uint8_t *lut, double clip, int tiles_x, int tiles_y) {
+    KltBatchFrame F{};
+    F.raw = raw; F.lut = lut; F.pyr = s.pyr[i].d; F.levels = s.levels;
+    for (int l = 0; l < s.levels; ++l) { F.w[l] = s.lw[l]; F.h[l] = s.lh[l]; F.off[l] = s.off[l]; }
+    if (clip > 0.0) klt_clahe_params(s.w, s.h, clip, tiles_x, tiles_y, F.tw, F.th, F.clip, F.lut_scale);
+    return F;
+}
+
 static int klt_prepare(Handle *h, int w, int hgt, int max_level, int n_points) {
     KltState &k = h->klt;
     if (k.w != w || k.h != hgt || k.levels != max_level + 1 || k.cap_pts < n_points) {   // (drops the image cache)
@@ -383,12 +407,14 @@ static int klt_prepare(Handle *h, int w, int hgt, int max_level, int n_points) {
         k.cap_pts = std::max(n_points, 1024);
     }
     for (auto &p : k.pyr) TRY(reserve(h, p, k.off[k.levels], kDevice));
-    TRY(reserve(h, k.pts, 5 * (size_t)k.cap_pts, kBoth));
-    TRY(reserve(h, k.status, k.cap_pts, kBoth));
     TRY(reserve(h, k.img, (size_t)2 * w * hgt, kPinned));
     return 0;
 }
 
+// The single call: one pair of the cache h->klt.  Its pair descriptor, the descriptors of the frames it uploads, a zero
+// pair index per point and the points go to the device in one copy; each new frame's pixels are copied into level 0 of
+// its pyramid (raw[i] with CLAHE).  The pyramids are built one frame at a time, so the launches of a call tell how many
+// it built; one D2H copy brings positions, errors and status back.
 int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int width, int height, int stride,
                    const float *prev_pts, float *next_pts, uint8_t *status, float *err, int n_points,
                    int max_level, int max_iter, double eps, double clahe_clip, int tiles_x, int tiles_y,
@@ -402,72 +428,61 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
     max_level = klt_levels(width, height, max_level) - 1;
     TRY(klt_prepare(h, width, height, max_level, n_points));
     KltState &k = h->klt;
-    const size_t img_bytes = (size_t)width * height, cap = k.cap_pts;
-    float *h_pts = k.pts.h, *d_prev = k.pts.d, *d_next = k.pts.d + 2 * cap, *d_err = k.pts.d + 4 * cap;
+    const size_t img_bytes = (size_t)width * height, n = n_points;
     int slot[2];
     bool have[2];
     klt_lookup(k, prev_id, next_id, clahe_clip, slot, have);
     const int sp = slot[0], sn = slot[1];
     if ((!have[0] && !prev) || (!have[1] && !next)) return fail(h, PVIO_B200_EINVAL, "klt: image not cached and no pixels given");
-    const uint8_t *src[2] = {prev, next};
-    for (int i = 0; i < 2; ++i) {
-        if (have[i]) continue;
-        for (int y = 0; y < height; ++y) memcpy(k.img.h + i * img_bytes + (size_t)y * width, src[i] + (size_t)y * stride, width);
-    }
-    memcpy(h_pts, prev_pts, sizeof(float) * 2 * n_points);
-    memcpy(h_pts + 2 * cap, next_pts, sizeof(float) * 2 * n_points);
     if (do_clahe) {
-        // raw frames -> device, CLAHE on the device into level 0 of the pyramids (opencv_image.cpp:138-143)
         for (auto &r : k.raw) TRY(reserve(h, r, img_bytes, kDevice));
         TRY(reserve(h, k.lut, (size_t)tiles_x * tiles_y * 256, kDevice));
     }
+
+    // staging (both sides): upload [0, o_err) | download [o_next, o)
+    size_t o = 0;
+    const size_t o_lv = o;   o = align256(o + sizeof(KltLevels));
+    const size_t o_frm = o;  o = align256(o + sizeof(KltBatchFrame) * 2);
+    const size_t o_pof = o;  o = align256(o + sizeof(int) * n);
+    const size_t o_prev = o; o = align256(o + sizeof(float) * 2 * n);
+    const size_t o_next = o; o = align256(o + sizeof(float) * 2 * n);          // guesses in, positions out
+    const size_t o_err = o;  o = align256(o + sizeof(float) * n);
+    const size_t o_st = o;   o += n;
+    TRY(reserve(h, k.stage, o, kBoth));
+    uint8_t *hs = k.stage.h, *ds = k.stage.d;
+    *reinterpret_cast<KltLevels *>(hs + o_lv) = klt_pair(k, slot);
+    memset(hs + o_pof, 0, sizeof(int) * n);
+    memcpy(hs + o_prev, prev_pts, sizeof(float) * 2 * n);
+    memcpy(hs + o_next, next_pts, sizeof(float) * 2 * n);
+    KltBatchFrame *frm = reinterpret_cast<KltBatchFrame *>(hs + o_frm);
+    const uint8_t *src[2] = {prev, next};
+    int nf = 0;
     for (int i = 0; i < 2; ++i) {
         if (have[i]) continue;
-        uint8_t *P = k.pyr[slot[i]].d;
-        if (do_clahe) {
-            CK(h, cudaMemcpyAsync(k.raw[i].d, k.img.h + i * img_bytes, img_bytes, cudaMemcpyHostToDevice, h->stream));
-            clahe_device(h, k.raw[i].d, P, k.lut.d, width, height, clahe_clip, tiles_x, tiles_y);
-        } else {
-            CK(h, cudaMemcpyAsync(P, k.img.h + i * img_bytes, img_bytes, cudaMemcpyHostToDevice, h->stream));
-        }
-        for (int l = 1; l <= max_level; ++l) {
-            dim3 b(32, 8), g((k.lw[l] + 31) / 32, (k.lh[l] + 7) / 8);
-            pyrdown_kernel<false><<<g, b, 0, h->stream>>>(P + k.off[l - 1], k.lw[l - 1], k.lh[l - 1], P + k.off[l], k.lw[l], k.lh[l],
-                                                           nullptr, 0);
-            ++h->launches;
-        }
+        uint8_t *img = k.img.h + i * img_bytes;
+        for (int y = 0; y < height; ++y) memcpy(img + (size_t)y * width, src[i] + (size_t)y * stride, width);
+        uint8_t *dst = do_clahe ? k.raw[i].d : k.pyr[slot[i]].d;     // without CLAHE: straight into level 0
+        frm[nf++] = klt_frame(k, slot[i], dst, k.lut.d, clahe_clip, tiles_x, tiles_y);
+        CK(h, cudaMemcpyAsync(dst, img, img_bytes, cudaMemcpyHostToDevice, h->stream));
     }
+    CK(h, cudaMemcpyAsync(ds, hs, o_err, cudaMemcpyHostToDevice, h->stream));
+    const KltBatchFrame *d_frm = reinterpret_cast<const KltBatchFrame *>(ds + o_frm);
+    for (int j = 0; j < nf; ++j) TRY(klt_build_pyramids(h, frm + j, d_frm + j, 1, do_clahe, tiles_x, tiles_y));
     k.pyr_id[sp] = prev_id; k.pyr_clahe[sp] = clahe_clip;
     k.pyr_id[sn] = next_id; k.pyr_clahe[sn] = clahe_clip;
-    CK(h, cudaMemcpyAsync(d_prev, h_pts, sizeof(float) * 2 * n_points, cudaMemcpyHostToDevice, h->stream));
-    CK(h, cudaMemcpyAsync(d_next, h_pts + 2 * cap, sizeof(float) * 2 * n_points, cudaMemcpyHostToDevice, h->stream));
-    KltLevels L;
-    L.n = max_level + 1;
-    for (int l = 0; l <= max_level; ++l) {
-        L.I[l] = k.pyr[sp].d + k.off[l]; L.J[l] = k.pyr[sn].d + k.off[l];
-        L.w[l] = k.lw[l]; L.h[l] = k.lh[l];
-    }
-    const int mi = std::min(std::max(max_iter, 0), 100);
-    const double e = std::min(std::max(eps, 0.0), 10.0);
-    klt_track_kernel<false><<<(n_points + kKltWarps - 1) / kKltWarps, 32 * kKltWarps, 0, h->stream>>>(
-        L, d_prev, d_next, k.status.d, d_err, n_points, mi, e * e, 1e-4f, nullptr, nullptr, 0);
-    ++h->launches;
-    if (border > 0) {
-        klt_border_kernel<<<(n_points + 127) / 128, 128, 0, h->stream>>>(d_next, k.status.d, n_points, width, height, border);
-        ++h->launches;
-    }
-    CK(h, cudaMemcpyAsync(h_pts + 2 * cap, d_next, sizeof(float) * 2 * n_points, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaMemcpyAsync(h_pts + 4 * cap, d_err, sizeof(float) * n_points, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaMemcpyAsync(k.status.h, k.status.d, n_points, cudaMemcpyDeviceToHost, h->stream));
+    klt_lk(h, reinterpret_cast<const KltLevels *>(ds + o_lv), reinterpret_cast<const int *>(ds + o_pof),
+           reinterpret_cast<const float *>(ds + o_prev), reinterpret_cast<float *>(ds + o_next), ds + o_st,
+           reinterpret_cast<float *>(ds + o_err), n, max_iter, eps, border);
+    CK(h, cudaMemcpyAsync(hs + o_next, ds + o_next, o - o_next, cudaMemcpyDeviceToHost, h->stream));
     if (do_clahe && (prev_eq || next_eq)) {
         CK(h, cudaMemcpyAsync(k.img.h, k.pyr[sp].d, img_bytes, cudaMemcpyDeviceToHost, h->stream));
         CK(h, cudaMemcpyAsync(k.img.h + img_bytes, k.pyr[sn].d, img_bytes, cudaMemcpyDeviceToHost, h->stream));
     }
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    memcpy(next_pts, h_pts + 2 * cap, sizeof(float) * 2 * n_points);
-    if (err) memcpy(err, h_pts + 4 * cap, sizeof(float) * n_points);
-    memcpy(status, k.status.h, n_points);
+    memcpy(next_pts, hs + o_next, sizeof(float) * 2 * n);
+    if (err) memcpy(err, hs + o_err, sizeof(float) * n);
+    memcpy(status, hs + o_st, n);
     if (do_clahe && prev_eq) memcpy(prev_eq, k.img.h, img_bytes);
     if (do_clahe && next_eq) memcpy(next_eq, k.img.h + img_bytes, img_bytes);
     return 0;
@@ -483,7 +498,6 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
 namespace {
 constexpr int kMaxBatchPairs = 32767;         // grid y / z limits: one block row per pair, per new frame
 constexpr int kFmIters = 1000;                // findFundamentalMat's maxIters, as pvio_b200_track_keypoints passes it
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 }  // namespace
 
 int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_level, int max_iter, double eps,
@@ -535,7 +549,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     if (taken.size() > B.slots.size()) B.slots.resize(taken.size());
     std::vector<int> budget(n);
     size_t n_frames = 0, pix_bytes = 0, budget_sum = 0, words_sum = 0, mask_words = 0;
-    int max_budget = 0, max_words = 0, max_levels = 1, lvw[kMaxLevels] = {}, lvh[kMaxLevels] = {};
+    int max_budget = 0, max_words = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_klt_pair &a = pairs[i];
         const Plan &pl = plan[i];
@@ -549,8 +563,6 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
             if (pl.have[side]) continue;
             ++n_frames;
             pix_bytes += align256((size_t)a.width * a.height);
-            max_levels = std::max(max_levels, s.levels);
-            for (int l = 0; l < s.levels; ++l) { lvw[l] = std::max(lvw[l], s.lw[l]); lvh[l] = std::max(lvh[l], s.lh[l]); }
         }
         const int np = a.n_points, nw = (np + 31) / 32;
         budget[i] = np < 8 ? 0 : np < 15 ? lmeds_iters : std::max(fm_iters, lmeds_iters);
@@ -597,26 +609,13 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
         const pvio_b200_klt_pair &a = pairs[i];
         const Plan &pl = plan[i];
         KltPyramids &s = B.slots[a.slot];
-        KltLevels &L = lv[i];
-        memset(&L, 0, sizeof(L));
-        L.n = s.levels;
-        for (int l = 0; l < s.levels; ++l) {
-            L.I[l] = s.pyr[pl.slot[0]].d + s.off[l]; L.J[l] = s.pyr[pl.slot[1]].d + s.off[l];
-            L.w[l] = s.lw[l]; L.h[l] = s.lh[l];
-        }
+        lv[i] = klt_pair(s, pl.slot);
         const uint8_t *src[2] = {a.prev, a.next};
         for (int side = 0; side < 2; ++side) {
             if (pl.have[side]) continue;
             uint8_t *dst = hs + o_pix + pix;
             for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, src[side] + (size_t)y * a.stride, a.width);
-            KltBatchFrame &F = frm[f];
-            memset(&F, 0, sizeof(F));
-            F.raw = ds + o_pix + pix;
-            F.lut = dc + c_lut + f * tiles * 256;
-            F.pyr = s.pyr[pl.slot[side]].d;
-            F.levels = s.levels;
-            for (int l = 0; l < s.levels; ++l) { F.w[l] = s.lw[l]; F.h[l] = s.lh[l]; F.off[l] = s.off[l]; }
-            if (do_clahe) klt_clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, F.tw, F.th, F.clip, F.lut_scale);
+            frm[f] = klt_frame(s, pl.slot[side], ds + o_pix + pix, dc + c_lut + f * tiles * 256, clahe_clip, tiles_x, tiles_y);
             pix += align256((size_t)a.width * a.height);
             ++f;
         }
@@ -648,32 +647,12 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
 
     cudaStream_t st = h->stream;
     CK(h, cudaMemcpyAsync(ds, hs, o_err, cudaMemcpyHostToDevice, st));
-    const KltBatchFrame *d_frm = reinterpret_cast<const KltBatchFrame *>(ds + o_frm);
-    const dim3 b2(32, 8);
-    if (n_frames > 0) {
-        const int nf = (int)n_frames;
-        if (do_clahe) {
-            klt_batch_clahe(h, d_frm, nf, tiles_x, tiles_y, lvw[0], lvh[0]);
-        } else {
-            for (size_t j = 0; j < n_frames; ++j)
-                CK(h, cudaMemcpyAsync(frm[j].pyr, frm[j].raw, (size_t)frm[j].w[0] * frm[j].h[0], cudaMemcpyDeviceToDevice, st));
-        }
-        for (int l = 1; l < max_levels; ++l) {
-            pyrdown_kernel<true><<<dim3((lvw[l] + 31) / 32, (lvh[l] + 7) / 8, nf), b2, 0, st>>>(nullptr, 0, 0, nullptr, 0, 0, d_frm, l);
-            ++h->launches;
-        }
-    }
-    float *d_next = reinterpret_cast<float *>(ds + o_next);
-    uint8_t *d_status = ds + o_st;
-    if (n_pts > 0) {
-        const int mi = std::min(std::max(max_iter, 0), 100);
-        const double e = std::min(std::max(eps, 0.0), 10.0);
-        klt_track_kernel<true><<<(unsigned)((n_pts + kKltWarps - 1) / kKltWarps), 32 * kKltWarps, 0, st>>>(
-            KltLevels{}, reinterpret_cast<const float *>(ds + o_prev), d_next, d_status, reinterpret_cast<float *>(ds + o_err),
-            (int)n_pts, mi, e * e, 1e-4f, reinterpret_cast<const KltLevels *>(ds + o_lv), reinterpret_cast<const int *>(ds + o_pof),
-            border);
-        ++h->launches;
-    }
+    if (n_frames > 0)
+        TRY(klt_build_pyramids(h, frm, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_frames, do_clahe, tiles_x, tiles_y));
+    if (n_pts > 0)
+        klt_lk(h, reinterpret_cast<const KltLevels *>(ds + o_lv), reinterpret_cast<const int *>(ds + o_pof),
+               reinterpret_cast<const float *>(ds + o_prev), reinterpret_cast<float *>(ds + o_next), ds + o_st,
+               reinterpret_cast<float *>(ds + o_err), n_pts, max_iter, eps, border);
     const FmBatchProblem *d_fmp = reinterpret_cast<const FmBatchProblem *>(ds + o_fmp);
     if (max_budget > 0) {
         fm_batch_schedule(h, d_fmp, n, fm_iters, lmeds_iters);
@@ -759,22 +738,22 @@ const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int he
     for (int i = 0; i < 2; ++i) if (k.pyr_id[i] == frame_id && k.pyr_clahe[i] == clahe_clip) return k.pyr[i].d;
     return nullptr;
 }
-// CLAHE of a device image into a device image (the detector's own upload path)
-int klt_clahe_device(Handle *h, const uint8_t *d_src, uint8_t *d_dst, uint8_t *d_lut, int width, int height, double clip, int tiles_x, int tiles_y) {
-    clahe_device(h, d_src, d_dst, d_lut, width, height, clip, tiles_x, tiles_y);
-    return 0;
-}
 
 // stand-alone CLAHE of one host image (dst row stride = width)
 int clahe_impl(Handle *h, const uint8_t *src, int width, int height, int stride, double clip, int tiles_x, int tiles_y, uint8_t *dst) {
     if (width < 1 || height < 1 || stride < width || clip <= 0.0 || tiles_x < 1 || tiles_y < 1 || width % tiles_x || height % tiles_y)
         return fail(h, PVIO_B200_EINVAL, "clahe: bad arguments (the image size must be a multiple of the tile grid)");
-    const size_t bytes = (size_t)width * height;
+    const size_t bytes = (size_t)width * height, o_frm = align256(2 * bytes + (size_t)tiles_x * tiles_y * 256);
     DevBuf<uint8_t> buf;
-    TRY(alloc(h, buf, 2 * bytes + (size_t)tiles_x * tiles_y * 256, kDevice));
+    TRY(alloc(h, buf, o_frm + sizeof(KltBatchFrame), kDevice));
     uint8_t *d = buf.d;
+    KltBatchFrame F{};                        // the image as one frame of one level
+    F.raw = d; F.pyr = d + bytes; F.lut = d + 2 * bytes;
+    F.levels = 1; F.w[0] = width; F.h[0] = height;
+    klt_clahe_params(width, height, clip, tiles_x, tiles_y, F.tw, F.th, F.clip, F.lut_scale);
     CK(h, cudaMemcpy2DAsync(d, width, src, stride, width, height, cudaMemcpyHostToDevice, h->stream));
-    clahe_device(h, d, d + bytes, d + 2 * bytes, width, height, clip, tiles_x, tiles_y);
+    CK(h, cudaMemcpyAsync(d + o_frm, &F, sizeof(F), cudaMemcpyHostToDevice, h->stream));
+    klt_batch_clahe(h, reinterpret_cast<const KltBatchFrame *>(d + o_frm), 1, tiles_x, tiles_y, width, height);
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(dst, d + bytes, bytes, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
