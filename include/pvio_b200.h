@@ -669,6 +669,64 @@ typedef struct pvio_b200_detect_request {
 int pvio_b200_batch_detect_keypoints(pvio_b200_handle h, int n, const pvio_b200_detect_request *requests,
                                      double clahe_clip, int tiles_x, int tiles_y);
 
+/* ---- lens distortion ------------------------------------------------------------------- */
+/* The undistortion PVIO's dataset readers run on every raw frame before CLAHE:
+ *  PVIO_B200_LENS_RADTAN       cv::undistort(img, out, K, D) with K and D as cv::Mat_<float> (EurocDatasetReader::read_image,
+ *                              pvio-pc/src/euroc_dataset_reader.cpp:70-74; OpenCvImage::correct_distortion,
+ *                              pvio-extra/src/pvio/extra/opencv_image.cpp:162-175): coefficients k1 k2 p1 p2, new camera
+ *                              matrix K.  fx, fy, cx, cy and the coefficients are first rounded to float32.
+ *  PVIO_B200_LENS_EQUIDISTANT  ImageUndistorter (pvio-extra/include/pvio/extra/image_undistorter.h:28-95, as
+ *                              tum_dataset_reader.cpp:71-81 uses it): distort_pixel in double, a float map converted by
+ *                              cv::convertMaps to CV_16SC2, cv::remap(INTER_LINEAR, BORDER_CONSTANT).  Coefficients k1..k4.
+ * The undistorted frame has the raw frame's shape.  Both are a bilinear remap with OpenCV's fixed-point weights, bit for
+ * bit what OpenCV gives. */
+#define PVIO_B200_LENS_RADTAN 1
+#define PVIO_B200_LENS_EQUIDISTANT 2
+
+/* Host only (no device, no handle): the map of one lens for width x height frames, built in fp64 on the host as OpenCV
+ * builds it (cv::undistort's 4096-pixel stripes included).  fx_fy_cx_cy [4], coeffs [4] as above.  Out: OpenCV's CV_16SC2
+ * pair, m1 int16 [height][width][2] the integer source pixel (x, y), m2 uint16 [height][width] the fraction index
+ * (v & 31) * 32 + (u & 31) of the 1/32-pixel coordinates (u, v).  PVIO_B200_EINVAL for an unknown model, width or height
+ * below 8 or above 32767 (cv::remap's limit), a parameter that is not finite, fx <= 0 or fy <= 0, or a map coordinate
+ * that is not finite. */
+int pvio_b200_undistort_map(int model, int width, int height, const double *fx_fy_cx_cy, const double *coeffs,
+                            int16_t *m1, uint16_t *m2);
+
+/* The lens of one sequence slot of pvio_b200_batch_track_keypoints. */
+typedef struct pvio_b200_lens {
+    int32_t slot;                  /* a sequence slot of pvio_b200_batch_track_keypoints, 0 .. 65535                  */
+    int32_t model;                 /* 0 none (clears the slot's lens), PVIO_B200_LENS_RADTAN, PVIO_B200_LENS_EQUIDISTANT */
+    int32_t width, height;         /* the raw frame's shape; the undistorted frame has the same shape                */
+    double fx, fy, cx, cy;
+    double coeffs[4];              /* radtan: k1 k2 p1 p2; equidistant: k1 k2 k3 k4                                   */
+} pvio_b200_lens;                  /* 80 bytes on LP64 */
+
+/* Sets (or, model 0, clears) the lens of n slots, once per sequence.  Each slot's map is built on the host
+ * (pvio_b200_undistort_map) and kept on the device, one map per slot at 6 bytes per pixel: 2.2 MB for 752 x 480, so 528
+ * slots hold 1.1 GB.  Slots never share a map.  From then on a frame that pvio_b200_batch_track_keypoints or
+ * pvio_b200_batch_detect_keypoints uploads for a slot with a lens is the RAW frame: it is undistorted on the device
+ * before CLAHE, and the results are bit for bit those of the same call on frames undistorted by OpenCV.  Frames read
+ * from a slot's cache are used as cached (already undistorted).  A tracker pair whose slot has a lens must have the
+ * lens's shape.  Setting or clearing a lens drops the slot's two cached frames.  Slots are created on demand; a lens
+ * outlives the tracker's rebuild of its slot on a shape change.  Every record is checked, and every map built, before a
+ * slot changes: PVIO_B200_EINVAL for each rejection of pvio_b200_undistort_map, a slot out of range or a slot named
+ * twice.  n == 0 is a no-op. */
+int pvio_b200_batch_set_lens(pvio_b200_handle h, int n, const pvio_b200_lens *records);
+
+/* One frame of pvio_b200_batch_undistort. */
+typedef struct pvio_b200_undistort_request {
+    int32_t slot;                  /* a slot with a lens                                                              */
+    int32_t width, height, stride; /* the lens's shape; stride >= width                                               */
+    const uint8_t *src;            /* the raw frame                                                                   */
+    uint8_t *dst;                  /* [height][width] out: the undistorted frame                                      */
+} pvio_b200_undistort_request;     /* 32 bytes on LP64 */
+
+/* The undistorted frames of n slots (several requests may name one slot), for callers that need the image itself: one
+ * upload, one kernel launch, one download.  The call reads no cache and changes none.  Every request is checked first:
+ * PVIO_B200_EINVAL for a slot out of range or without a lens, a shape other than the lens's, stride < width, or a NULL
+ * pointer; no output has changed then. */
+int pvio_b200_batch_undistort(pvio_b200_handle h, int n, const pvio_b200_undistort_request *requests);
+
 /* CLAHE of one frame (same kernels); dst is [height][width]. */
 int pvio_b200_clahe(pvio_b200_handle h, const uint8_t *src, int width, int height, int stride, double clip_limit,
                     int tiles_x, int tiles_y, uint8_t *dst);

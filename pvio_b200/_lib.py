@@ -113,6 +113,17 @@ class CWindowTrackFrame(C.Structure):
                 ("summary", C.POINTER(CSummary))]
 
 
+class CLens(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+                ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+                ("coeffs", C.c_double * 4)]
+
+
+class CUndistortRequest(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32),
+                ("src", c_u8p), ("dst", c_u8p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -131,7 +142,7 @@ EXPORTS = [
     "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
     "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
     "pvio_b200_batch_window_localize", "pvio_b200_batch_window_set_imu", "pvio_b200_batch_window_imu_records",
-    "pvio_b200_batch_window_track_frame",
+    "pvio_b200_batch_window_track_frame", "pvio_b200_undistort_map", "pvio_b200_batch_set_lens", "pvio_b200_batch_undistort",
 ]
 
 _lib = None
@@ -186,6 +197,10 @@ def load():
     lib.pvio_b200_batch_track_keypoints.argtypes = [vp, C.c_int, C.POINTER(CKltPair), C.c_int, C.c_int, C.c_double,
                                                     C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
     lib.pvio_b200_batch_detect_keypoints.argtypes = [vp, C.c_int, C.POINTER(CDetectRequest), C.c_double, C.c_int, C.c_int]
+    lib.pvio_b200_undistort_map.argtypes = [C.c_int, C.c_int, C.c_int, c_f64p, c_f64p, C.POINTER(C.c_int16),
+                                            C.POINTER(C.c_uint16)]
+    lib.pvio_b200_batch_set_lens.argtypes = [vp, C.c_int, C.POINTER(CLens)]
+    lib.pvio_b200_batch_undistort.argtypes = [vp, C.c_int, C.POINTER(CUndistortRequest)]
     lib.pvio_b200_klt_track.argtypes = [vp, c_u8p, c_u8p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p,
                                         C.c_int, C.c_int, C.c_int, C.c_double]
     for name in EXPORTS:

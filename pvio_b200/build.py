@@ -13,6 +13,16 @@ FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c
          "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
+def _extra(name):
+    """per-file flags: OpenCV's float rounding on the device (no contraction); undistort.cu's host-side map builder
+    without fused multiply-adds, which GCC forms by default where the target has them (aarch64)"""
+    if name.endswith(("klt.cu", "detect.cu", "fmat.cu")):
+        return ["-fmad=false"]
+    if name.endswith("undistort.cu"):
+        return ["-Xcompiler", "-ffp-contract=off"]
+    return []
+
+
 def _stale(target, deps):
     if not os.path.exists(target):
         return True
@@ -38,7 +48,7 @@ def build(force=False, verbose=False, defines=(), out=None):
 
     def cc(job):
         src, obj = job
-        extra = ["-fmad=false"] if src.endswith(("klt.cu", "detect.cu", "fmat.cu")) else []   # OpenCV's float rounding: no contraction
+        extra = _extra(src)
         r = subprocess.run([NVCC] + FLAGS + extra + ["-c", src, "-o", obj], capture_output=True, text=True)
         return src, r
 
@@ -66,7 +76,7 @@ def _build_variant(defines, out):
     objs = []
     for s in sorted(f for f in os.listdir(CSRC) if f.endswith(".cu")):
         obj = os.path.join(odir, s[:-3] + ".o")
-        extra = ["-fmad=false"] if s in ("klt.cu", "detect.cu", "fmat.cu") else []
+        extra = _extra(s)
         ref = os.path.join(CSRC, s[:-3] + ".o")
         names = [d.split("=")[0] for d in defines]
         text = open(os.path.join(CSRC, s)).read()

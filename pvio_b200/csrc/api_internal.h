@@ -65,10 +65,14 @@ struct KltState : KltPyramids {
     DevBuf<uint8_t> img;                      // pinned staging for both level-0 images
 };
 
-// one frame the tracker or the detector equalises or downsamples on the device (klt.cu, detect.cu), as the CLAHE and
-// pyrDown kernels read it: its raw pixels, CLAHE into level 0 of `pyr`, then pyrDown level by level
+// one frame the tracker or the detector undistorts, equalises or downsamples on the device (klt.cu, detect.cu,
+// undistort.cu), as the remap, CLAHE and pyrDown kernels read it: with a lens the uploaded pixels remapped into raw,
+// then CLAHE from raw into level 0 of `pyr`, then pyrDown level by level
 struct KltBatchFrame {
-    const uint8_t *raw;                       // level-0 pixels as uploaded (raw when CLAHE runs)
+    const uint8_t *lens_src;                  // with a lens: the uploaded frame, remapped into raw through m1 / m2
+    const short2 *m1;                         //   (its slot's map, SlotLens); nullptr: no lens
+    const uint16_t *m2;
+    uint8_t *raw;                             // level-0 pixels before CLAHE: as uploaded, or the remap's output
     uint8_t *lut;                             // [tiles][256] its CLAHE tables
     uint8_t *pyr;                             // its pyramid (the detector and clahe_impl: level 0 only)
     int levels, tw, th, clip;
@@ -78,10 +82,22 @@ struct KltBatchFrame {
 };
 constexpr int kMaxBatchSlot = 65535;          // the sequence slots of the batched calls: 0 .. kMaxBatchSlot
 
+// undistort.cu: the lens of one sequence slot (pvio_b200_batch_set_lens) -- OpenCV's CV_16SC2 map pair, 6 bytes per pixel
+// on the device: [h][w] short2 integer source pixel, then [h][w] uint16 fraction index.  Kept apart from the slot's
+// pyramids, so the tracker's shape-change rebuild of a slot leaves its lens alone.
+struct SlotLens {
+    int w = 0, h = 0, model = 0;              // model 0: no lens
+    DevBuf<uint8_t> map;
+    const short2 *m1() const { return reinterpret_cast<const short2 *>(map.d); }
+    const uint16_t *m2() const { return reinterpret_cast<const uint16_t *>(map.d + (size_t)4 * w * h); }
+};
+
 // the batched tracker (pvio_b200_batch_track_keypoints): one pyramid cache per sequence slot, grown on demand, and
 // the buffers of one call, grown to the largest call seen
 struct KltBatchState {
     std::vector<KltPyramids> slots;
+    std::vector<SlotLens> lens;               // per slot, grown on demand by pvio_b200_batch_set_lens
+    DevBuf<uint8_t> ustage;                   // both sides: pvio_b200_batch_undistort's descriptors and frames
     DevBuf<uint8_t> stage;                    // both sides: uploaded descriptors, frames and points | downloaded results |
                                               // winners' masks; host side only: the mask jobs the device reads in place
     DevBuf<uint8_t> scratch;                  // device: CLAHE tables, RANSAC matches, schedules, counts, models, masks
@@ -366,6 +382,11 @@ const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int he
 // device memory; each equalises raw into level 0 of pyr) as 2 launches whose grids cover max_w x max_h
 void klt_clahe_params(int w, int hgt, double clip_limit, int tiles_x, int tiles_y, int &tw, int &th, int &clip, float &lut_scale);
 void klt_batch_clahe(Handle *h, const KltBatchFrame *frames, int n_frames, int tiles_x, int tiles_y, int max_w, int max_h);
+// undistort.cu: the map of one lens (pvio_b200_undistort_map); the lens of a slot, or nullptr; the remap of n_frames
+// frames (descriptors in device memory, each with lens_src, m1, m2, raw and w[0] x h[0]) as 1 launch covering max_w x max_h
+int undistort_map_host(int model, int width, int height, const double *p, const double *c, int16_t *m1, uint16_t *m2);
+const SlotLens *slot_lens(const KltBatchState &B, int slot);
+void undistort_frames(Handle *h, const KltBatchFrame *frames, int n_frames, int max_w, int max_h);
 // detect.cu: pvio_b200_batch_detect_keypoints
 int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, double clahe_clip, int tiles_x, int tiles_y);
 // ba_marg.cu

@@ -237,6 +237,9 @@ int ensure(Handle *h, int w, int hgt) {
 // CLAHE over the uploaded frames (2 launches, clahe_clip > 0 only); Harris and NMS over every frame, grid z = frame
 // (2); a segmented descending radix sort of each frame's keys, whose segment ends are read on the device (1);
 // detect_select_kernel, one CTA per frame running both greedy passes (1); one D2H copy of the results, a synchronise.
+// An uploaded frame whose slot has a lens (pvio_b200_batch_set_lens) is raw: it is remapped first (1 launch over every
+// such frame, undistort.cu) into the detector's scratch, which CLAHE (or, without CLAHE, Harris) reads.  These frames
+// come first among the CLAHE descriptors, so the remap's grid covers them alone.
 constexpr int kMinDist = 20;                  // GFTT's minDistance, and the cell of its grid (lround(20))
 constexpr int kCellEmpty = -(1 << 30);        // x of an empty min-distance slot: farther than 20 px from every pixel
 constexpr unsigned long long kHashEmpty = ~0ull;
@@ -423,6 +426,7 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     const bool do_clahe = clahe_clip > 0.0;
     const KltBatchState &B = h->kltb;
     std::vector<const uint8_t *> cached(n, nullptr);
+    std::vector<const SlotLens *> lens(n, nullptr);
     for (int i = 0; i < n; ++i) {
         const pvio_b200_detect_request &a = reqs[i];
         if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: slot out of range");
@@ -440,12 +444,15 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
         if (a.stride < a.width) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: bad stride");
         if (do_clahe && (tiles_x < 1 || tiles_y < 1 || a.width % tiles_x || a.height % tiles_y))
             return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
+        lens[i] = slot_lens(B, a.slot);
+        if (lens[i] && (lens[i]->w != a.width || lens[i]->h != a.height))
+            return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: the frame shape differs from the slot's lens");
     }
 
     // sizes: per frame its key segment, the existing points its Poisson walks can meet (cells [-2, cx + 2] x
     // [-2, cy + 3] around the cells of its pixels), its working area; the staging and the scratch of the call
     struct Plan {
-        size_t pix_off, eq_off, resp_off, work, work_off;
+        size_t pix_off, eq_off, und_off, resp_off, work, work_off;
         int cap, key_off, n_pre, gw, gh, hbits;
         double gs, cxmax, cymax;
     };
@@ -454,8 +461,8 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
         const double fx = std::floor(x / P.gs), fy = std::floor(y / P.gs);
         return fx >= -2.0 && fx <= P.cxmax + 2.0 && fy >= -2.0 && fy <= P.cymax + 3.0;
     };
-    size_t n_keys = 0, n_pre = 0, pix_bytes = 0, eq_bytes = 0, resp_bytes = 0, smem = 0;
-    int n_eq = 0, max_w = 0, max_h = 0, eq_w = 0, eq_h = 0;
+    size_t n_keys = 0, n_pre = 0, pix_bytes = 0, eq_bytes = 0, und_bytes = 0, resp_bytes = 0, smem = 0;
+    int n_eq = 0, n_lens = 0, max_w = 0, max_h = 0, eq_w = 0, eq_h = 0, und_w = 0, und_h = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_detect_request &a = reqs[i];
         Plan &P = plan[i];
@@ -487,8 +494,15 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
                 ++n_eq;
                 eq_w = std::max(eq_w, a.width); eq_h = std::max(eq_h, a.height);
             }
+            if (lens[i]) {
+                P.und_off = und_bytes;
+                und_bytes += align256(px);
+                ++n_lens;
+                und_w = std::max(und_w, a.width); und_h = std::max(und_h, a.height);
+            }
         }
     }
+    const int n_kf = do_clahe ? n_eq : n_lens;     // frames CLAHE or the remap read: those with a lens first
     if (n_keys > (size_t)INT_MAX) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: too many pixels in one call");
     size_t work_bytes = 0;
     for (auto &P : plan)
@@ -497,13 +511,14 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     // staging (both sides): upload [0, o_up) | download [o_res, o)
     size_t o = 0;
     const size_t o_frm = o; o = align256(o + sizeof(DetectBatchFrame) * n);
-    const size_t o_kf = o;  o = align256(o + sizeof(KltBatchFrame) * n_eq);
+    const size_t o_kf = o;  o = align256(o + sizeof(KltBatchFrame) * n_kf);
     const size_t o_cnt = o; o = align256(o + sizeof(int) * 2 * n);
     const size_t o_pre = o; o = align256(o + sizeof(double2) * n_pre);
     const size_t o_pix = o; o += pix_bytes;
     const size_t o_up = o;  o = align256(o);
     const size_t o_res = o; o = align256(o + sizeof(DetectResult) * n);
-    // device scratch: responses | keys | sorted keys | equalised frames | CLAHE tables | working areas | sort temporaries
+    // device scratch: responses | keys | sorted keys | equalised frames | CLAHE tables | working areas | sort temporaries |
+    // undistorted frames
     const size_t tiles = do_clahe ? (size_t)tiles_x * tiles_y : 0;
     auto begin_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{nullptr});
     auto end_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{nullptr});
@@ -518,6 +533,7 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     const size_t c_lut = c;    c = align256(c + tiles * 256 * n_eq);
     const size_t c_work = c;   c += work_bytes;
     const size_t c_cub = c;    c = align256(c + cub_bytes);
+    const size_t c_und = c;    c += und_bytes;
     DetectBatchState &D = h->detectb;
     TRY(reserve(h, D.stage, o, kBoth));
     TRY(reserve(h, D.scratch, c, kDevice));
@@ -528,7 +544,7 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     double2 *pre = reinterpret_cast<double2 *>(hs + o_pre);
     memset(hs + o_cnt, 0, sizeof(int) * 2 * n);
     size_t p = 0;
-    int q = 0;
+    int q_lens = 0, q_plain = n_lens;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_detect_request &a = reqs[i];
         const Plan &P = plan[i];
@@ -536,18 +552,26 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
         if (!img) {
             uint8_t *dst = hs + o_pix + P.pix_off;
             for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, a.image + (size_t)y * a.stride, a.width);
-            img = ds + o_pix + P.pix_off;
-            if (do_clahe) {                   // raw pixels: CLAHE into the detector's scratch
+            uint8_t *up = ds + o_pix + P.pix_off;
+            img = up;
+            if (do_clahe || lens[i]) {        // raw pixels: remap and / or CLAHE into the detector's scratch
+                const int q = lens[i] ? q_lens++ : q_plain++;
                 KltBatchFrame &K = kf[q];
                 memset(&K, 0, sizeof(K));
-                K.raw = img;
-                K.lut = dc + c_lut + (size_t)q * tiles * 256;
-                K.pyr = dc + c_eq + P.eq_off;
+                K.raw = up;
+                if (lens[i]) {
+                    K.lens_src = up; K.m1 = lens[i]->m1(); K.m2 = lens[i]->m2();
+                    K.raw = dc + c_und + P.und_off;
+                }
                 K.levels = 1;
                 K.w[0] = a.width; K.h[0] = a.height;
-                klt_clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, K.tw, K.th, K.clip, K.lut_scale);
-                img = K.pyr;
-                ++q;
+                img = K.raw;
+                if (do_clahe) {
+                    K.lut = dc + c_lut + (size_t)q * tiles * 256;
+                    K.pyr = dc + c_eq + P.eq_off;
+                    klt_clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, K.tw, K.th, K.clip, K.lut_scale);
+                    img = K.pyr;
+                }
             }
         }
         DetectBatchFrame &F = frm[i];
@@ -572,6 +596,7 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     cudaStream_t st = h->stream;
     CK(h, cudaMemcpyAsync(ds, hs, o_up, cudaMemcpyHostToDevice, st));
     const DetectBatchFrame *d_frm = reinterpret_cast<const DetectBatchFrame *>(ds + o_frm);
+    if (n_lens > 0) undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_lens, und_w, und_h);
     if (n_eq > 0) klt_batch_clahe(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_eq, tiles_x, tiles_y, eq_w, eq_h);
     harris_response_kernel<<<dim3((max_w + kTX - 1) / kTX, (max_h + kTY - 1) / kTY, n), dim3(kTX, kTY), 0, st>>>(0.04f, d_frm);
     nms_compact_kernel<<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n), dim3(32, 8), 0, st>>>(1.0e-3, d_frm);

@@ -391,7 +391,7 @@ static KltLevels klt_pair(const KltPyramids &s, const int slot[2]) {
 }
 
 // the descriptor of a new frame whose pyramid is s.pyr[i]: its pixels at raw, its CLAHE tables at lut (clip > 0)
-static KltBatchFrame klt_frame(const KltPyramids &s, int i, const uint8_t *raw, uint8_t *lut, double clip, int tiles_x, int tiles_y) {
+static KltBatchFrame klt_frame(const KltPyramids &s, int i, uint8_t *raw, uint8_t *lut, double clip, int tiles_x, int tiles_y) {
     KltBatchFrame F{};
     F.raw = raw; F.lut = lut; F.pyr = s.pyr[i].d; F.levels = s.levels;
     for (int l = 0; l < s.levels; ++l) { F.w[l] = s.lw[l]; F.h[l] = s.lh[l]; F.off[l] = s.off[l]; }
@@ -495,6 +495,10 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
 // sample schedule drawn on the device (1); every RANSAC iteration of every pair (1); one D2H copy of the results and a
 // synchronise; the host replays each pair as fm_ransac_impl does; one launch writes every winner's mask, one D2H copy,
 // a synchronise.  Without CLAHE each new frame is copied into level 0 of its pyramid (a device copy per frame).
+// A new frame of a slot with a lens (pvio_b200_batch_set_lens) is uploaded raw and remapped first (1 launch over every
+// such frame, undistort.cu): into a scratch frame that CLAHE reads, or without CLAHE straight into level 0 of its
+// pyramid in place of its device copy.  These frames come first in the descriptor array, so the remap's grid covers
+// them alone.
 namespace {
 constexpr int kMaxBatchPairs = 32767;         // grid y / z limits: one block row per pair, per new frame
 constexpr int kFmIters = 1000;                // findFundamentalMat's maxIters, as pvio_b200_track_keypoints passes it
@@ -528,6 +532,9 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad shape, stride or frame id");
         if (do_clahe && (a.width % tiles_x || a.height % tiles_y))
             return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
+        const SlotLens *L = slot_lens(B, a.slot);
+        if (L && (L->w != a.width || L->h != a.height))
+            return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: the frame shape differs from the slot's lens");
         if (a.n_points < 0 || (a.n_points > 0 && (!a.prev_pts || !a.next_pts || !a.status)))
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad points");
         Plan &pl = plan[i];
@@ -548,8 +555,8 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     const int lmeds_iters = fm_lmeds_iters(conf, fm_iters);
     if (taken.size() > B.slots.size()) B.slots.resize(taken.size());
     std::vector<int> budget(n);
-    size_t n_frames = 0, pix_bytes = 0, budget_sum = 0, words_sum = 0, mask_words = 0;
-    int max_budget = 0, max_words = 0;
+    size_t n_frames = 0, pix_bytes = 0, budget_sum = 0, words_sum = 0, mask_words = 0, n_lens = 0, und_bytes = 0;
+    int max_budget = 0, max_words = 0, lens_w = 0, lens_h = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_klt_pair &a = pairs[i];
         const Plan &pl = plan[i];
@@ -563,6 +570,11 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
             if (pl.have[side]) continue;
             ++n_frames;
             pix_bytes += align256((size_t)a.width * a.height);
+            if (slot_lens(B, a.slot)) {
+                ++n_lens;
+                if (do_clahe) und_bytes += align256((size_t)a.width * a.height);
+                lens_w = std::max(lens_w, a.width); lens_h = std::max(lens_h, a.height);
+            }
         }
         const int np = a.n_points, nw = (np + 31) / 32;
         budget[i] = np < 8 ? 0 : np < 15 ? lmeds_iters : std::max(fm_iters, lmeds_iters);
@@ -589,13 +601,15 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     const size_t o_cnt = o;  o = align256(o + sizeof(int) * 4 * budget_sum);
     const size_t o_mw = o;   o = align256(o + sizeof(unsigned) * words_sum);
     const size_t o_job = o;  o = align256(o + sizeof(FmMaskJob) * n);
-    // device scratch: CLAHE tables | survivors p, q | schedules | models | per-iteration masks
+    // device scratch: CLAHE tables | survivors p, q | schedules | models | per-iteration masks | undistorted frames
+    // (CLAHE's input)
     size_t c = 0;
     const size_t c_lut = c;   c = align256(c + tiles * 256 * n_frames);
     const size_t c_pq = c;    c = align256(c + sizeof(float2) * 2 * n_pts);
     const size_t c_sched = c; c = align256(c + sizeof(int) * 7 * budget_sum);
     const size_t c_F = c;     c = align256(c + sizeof(double) * 27 * budget_sum);
     const size_t c_masks = c; c = align256(c + sizeof(unsigned) * mask_words);
+    const size_t c_und = c;   c += und_bytes;
     TRY(reserve(h, B.stage, o, kBoth));
     TRY(reserve(h, B.scratch, std::max<size_t>(c, 256), kDevice));
     uint8_t *hs = B.stage.h, *ds = B.stage.d, *dc = B.scratch.d;
@@ -604,20 +618,27 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     KltBatchFrame *frm = reinterpret_cast<KltBatchFrame *>(hs + o_frm);
     int *pof = reinterpret_cast<int *>(hs + o_pof);
     float *h_prev = reinterpret_cast<float *>(hs + o_prev), *h_next = reinterpret_cast<float *>(hs + o_next);
-    size_t p = 0, f = 0, pix = 0, bsum = 0, msum = 0;
+    size_t p = 0, f_lens = 0, f_plain = n_lens, pix = 0, und = 0, bsum = 0, msum = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_klt_pair &a = pairs[i];
         const Plan &pl = plan[i];
         KltPyramids &s = B.slots[a.slot];
+        const SlotLens *L = slot_lens(B, a.slot);
         lv[i] = klt_pair(s, pl.slot);
         const uint8_t *src[2] = {a.prev, a.next};
         for (int side = 0; side < 2; ++side) {
             if (pl.have[side]) continue;
             uint8_t *dst = hs + o_pix + pix;
             for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, src[side] + (size_t)y * a.stride, a.width);
-            frm[f] = klt_frame(s, pl.slot[side], ds + o_pix + pix, dc + c_lut + f * tiles * 256, clahe_clip, tiles_x, tiles_y);
+            const size_t f = L ? f_lens++ : f_plain++;
+            uint8_t *raw = ds + o_pix + pix;
+            if (L) raw = do_clahe ? dc + c_und + und : s.pyr[pl.slot[side]].d;    // remapped: CLAHE's input, or level 0
+            frm[f] = klt_frame(s, pl.slot[side], raw, dc + c_lut + f * tiles * 256, clahe_clip, tiles_x, tiles_y);
+            if (L) {
+                frm[f].lens_src = ds + o_pix + pix; frm[f].m1 = L->m1(); frm[f].m2 = L->m2();
+                if (do_clahe) und += align256((size_t)a.width * a.height);
+            }
             pix += align256((size_t)a.width * a.height);
-            ++f;
         }
         s.pyr_id[pl.slot[0]] = a.prev_id; s.pyr_clahe[pl.slot[0]] = clahe_clip;
         s.pyr_id[pl.slot[1]] = a.next_id; s.pyr_clahe[pl.slot[1]] = clahe_clip;
@@ -647,6 +668,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
 
     cudaStream_t st = h->stream;
     CK(h, cudaMemcpyAsync(ds, hs, o_err, cudaMemcpyHostToDevice, st));
+    if (n_lens > 0) undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_lens, lens_w, lens_h);
     if (n_frames > 0)
         TRY(klt_build_pyramids(h, frm, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_frames, do_clahe, tiles_x, tiles_y));
     if (n_pts > 0)
