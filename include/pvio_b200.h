@@ -669,6 +669,59 @@ typedef struct pvio_b200_detect_request {
 int pvio_b200_batch_detect_keypoints(pvio_b200_handle h, int n, const pvio_b200_detect_request *requests,
                                      double clahe_clip, int tiles_x, int tiles_y);
 
+/* ---- two-view initialisation ------------------------------------------------------------- */
+/* The two-view step of Initializer::init_sfm (pvio/src/pvio/core/initializer.cpp:102-161) that seeds a sequence: the
+ * match-count and parallax gates, find_homography_matrix and find_essential_matrix (Ransac<> of utility/ransac.h,
+ * threshold 0.7 / fx), decompose_homography and decompose_essential, and triangulate_from_rt_scored over the 8 pose
+ * candidates.  status is the first of init_sfm's early returns that applies, in its order: */
+#define PVIO_B200_TWO_VIEW_OK 0
+#define PVIO_B200_TWO_VIEW_FEW_MATCHES 1      /* n_matches < min_matches, or n_matches < 5                      */
+#define PVIO_B200_TWO_VIEW_LOW_PARALLAX 2     /* mean parallax (pixels) < min_parallax                          */
+#define PVIO_B200_TWO_VIEW_PURE_ROTATION 3    /* decompose_homography found a pure rotation                     */
+#define PVIO_B200_TWO_VIEW_FEW_TRIANGULATED 4 /* the chosen candidate triangulates fewer than min_triangulation */
+
+/* One problem of pvio_b200_batch_two_view: the matches of frames i and j of one sequence.  Every output may be NULL. */
+typedef struct pvio_b200_two_view {
+    int32_t n_matches;
+    int32_t seed;                  /* Config::random(); PVIO's default 648                                            */
+    const double *p1, *p2;         /* [n][2] normalised keypoints of frames i and j (initializer.cpp:117-127)         */
+    double fx, fy;                 /* frame i's focal lengths: the parallax in pixels and the threshold 0.7 / fx      */
+    int32_t min_matches;           /* Config::initializer_min_matches (50)                                            */
+    int32_t min_triangulation;     /* Config::initializer_min_triangulation (20)                                      */
+    double min_parallax;           /* Config::initializer_min_parallax (10)                                           */
+    double confidence;             /* 0.999                                                                           */
+    int32_t max_iteration;         /* 1000                                                                            */
+    int32_t *info;                 /* [10] out: status, H inliers, H iterations run, H winning iteration,             */
+                                   /* E inliers, E iterations run, E winning iteration, E winning model,              */
+                                   /* chosen candidate (0..7 in init_sfm's Rs / Ts order), triangulated count;        */
+                                   /* winners and candidate -1 when there are none                                    */
+    double *parallax;              /* out: the mean parallax                                                          */
+    double *H, *E;                 /* [9] out, row-major: the two RANSACs' models (0 without a winner)                */
+    double *R, *T;                 /* [9], [3] out: init_R, init_T (the chosen candidate)                             */
+    uint8_t *h_mask, *e_mask;      /* [n] out: the inlier masks of the two winners                                    */
+    double *points;                /* [n][3] out: the chosen candidate's points in frame i (0 where not triangulated) */
+    uint8_t *point_status;         /* [n] out: init_point_status                                                      */
+    int32_t *h_schedule;           /* [max_iteration][4] out: the H RANSAC's sample schedule                          */
+    int32_t *e_schedule;           /* [max_iteration][5] out: the E RANSAC's sample schedule                          */
+    int32_t *h_counts;             /* [max_iteration] out: the inliers of each iteration's homography                 */
+    int32_t *e_counts;             /* [max_iteration][11] out: each iteration's model count, then each model's inliers */
+} pvio_b200_two_view;              /* 184 bytes on LP64 */
+
+/* init_sfm's two-view step for n sequences in one call.  Both RANSACs evaluate every iteration of their sample schedule
+ * (drawn on the device as Ransac::solve draws it, from a LotBox seeded with `seed`) and the serial acceptance rule,
+ * early stop included, is replayed on the host: each problem gets the serial loop's result for that schedule.  One
+ * deviation: the E models of one iteration are taken in ascending order of their action-matrix eigenvalue (the reference
+ * takes Eigen's real-Schur order), which matters only when two models of one iteration tie on the winning count.
+ * decompose_essential's SVD leaves the sign of T and the order of R1, R2 to rounding (an essential matrix has two equal
+ * singular values); here T's component of largest magnitude is positive and R1 has the larger trace.  The
+ * RANSACs and the triangulation run whatever the gates say, except below 5 matches; the diagnostic outputs (schedules,
+ * counts) are written for the iterations evaluated, none below 5 matches.
+ * Every record is checked before anything is staged: PVIO_B200_EINVAL, with no output changed, for n < 0, n > 65535,
+ * a negative n_matches or one above 2^24, more than 2^31 - 1 matches in all, NULL keypoints with n_matches > 0, fx or
+ * fy not positive, confidence not positive, max_iteration < 1 or a negative minimum.  n == 0 is a no-op.  A call is 4
+ * kernel launches and 2 synchronisations whatever n is; its buffers grow to the largest call and are then reused. */
+int pvio_b200_batch_two_view(pvio_b200_handle h, int n, const pvio_b200_two_view *records);
+
 /* ---- lens distortion ------------------------------------------------------------------- */
 /* The undistortion PVIO's dataset readers run on every raw frame before CLAHE:
  *  PVIO_B200_LENS_RADTAN       cv::undistort(img, out, K, D) with K and D as cv::Mat_<float> (EurocDatasetReader::read_image,

@@ -124,6 +124,15 @@ class CUndistortRequest(C.Structure):
                 ("src", c_u8p), ("dst", c_u8p)]
 
 
+class CTwoView(C.Structure):
+    _fields_ = [("n_matches", C.c_int32), ("seed", C.c_int32), ("p1", c_f64p), ("p2", c_f64p), ("fx", C.c_double),
+                ("fy", C.c_double), ("min_matches", C.c_int32), ("min_triangulation", C.c_int32),
+                ("min_parallax", C.c_double), ("confidence", C.c_double), ("max_iteration", C.c_int32), ("info", c_i32p),
+                ("parallax", c_f64p), ("H", c_f64p), ("E", c_f64p), ("R", c_f64p), ("T", c_f64p), ("h_mask", c_u8p),
+                ("e_mask", c_u8p), ("points", c_f64p), ("point_status", c_u8p), ("h_schedule", c_i32p),
+                ("e_schedule", c_i32p), ("h_counts", c_i32p), ("e_counts", c_i32p)]
+
+
 EXPORTS = [
     "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
     "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
@@ -143,6 +152,7 @@ EXPORTS = [
     "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
     "pvio_b200_batch_window_localize", "pvio_b200_batch_window_set_imu", "pvio_b200_batch_window_imu_records",
     "pvio_b200_batch_window_track_frame", "pvio_b200_undistort_map", "pvio_b200_batch_set_lens", "pvio_b200_batch_undistort",
+    "pvio_b200_batch_two_view",
 ]
 
 _lib = None
@@ -201,6 +211,7 @@ def load():
                                             C.POINTER(C.c_uint16)]
     lib.pvio_b200_batch_set_lens.argtypes = [vp, C.c_int, C.POINTER(CLens)]
     lib.pvio_b200_batch_undistort.argtypes = [vp, C.c_int, C.POINTER(CUndistortRequest)]
+    lib.pvio_b200_batch_two_view.argtypes = [vp, C.c_int, C.POINTER(CTwoView)]
     lib.pvio_b200_klt_track.argtypes = [vp, c_u8p, c_u8p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p,
                                         C.c_int, C.c_int, C.c_int, C.c_double]
     for name in EXPORTS:

@@ -135,6 +135,13 @@ struct FmState {
     DevBuf<unsigned> h_mask;                  // pinned: its inlier mask
 };
 
+// twoview.cu: the buffers of pvio_b200_batch_two_view, grown to the largest call seen
+struct TwoViewState {
+    DevBuf<uint8_t> stage;                    // both sides: problems, keypoints (uploaded) | results (downloaded)
+    DevBuf<int> counts;                       // both sides: sample schedules and per-iteration inlier counts of both RANSACs
+    DevBuf<uint8_t> scratch;                  // device: lots, models of every iteration, parallax, candidate scores
+};
+
 // The host record of one window slot.  Its frame and landmark counts are those of the slot's host header (Handle::hdr).
 // A slot holds either a window packed from the caller's arrays (api.cu: pack_window) or a resident window
 // (batch_window.cu; slot 0 is also the window of pvio_b200_window_*).  Of a resident window the host keeps integers only:
@@ -257,6 +264,7 @@ struct Handle {
     DevBuf<double> pnp;                           // pnp.cu's own: both sides, grown on demand to the largest batch
                                                   // (records, points, IMU records, frames) seen
     BatchWindows bw;                              // batch_window.cu (empty until the first pvio_b200_batch_window_reset)
+    TwoViewState tv;                              // twoview.cu
 };
 
 int fail(Handle *h, int code, const char *what, cudaError_t e = cudaSuccess);
@@ -428,6 +436,8 @@ float fm_replay(const int *counts, int n, int have, int max_iters, double confid
 void fm_batch_schedule(Handle *h, const FmBatchProblem *probs, int n, int max_iters, int lmeds_iters);
 void fm_batch_hypotheses(Handle *h, const FmBatchProblem *probs, int n, int max_budget, float thr2);
 void fm_batch_masks(Handle *h, const FmMaskJob *jobs, int n, int max_words);
+// twoview.cu: pvio_b200_batch_two_view
+int batch_two_view_impl(Handle *h, int n, const pvio_b200_two_view *recs);
 // selftest.cu
 int selftest_lie_impl(Handle *h, int n, const double *w_in, double *out);
 

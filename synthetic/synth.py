@@ -663,3 +663,41 @@ def make_fm_matches(seed=652, n=300, outlier_frac=0.2, noise=0.3, planar=False, 
     if no:
         x2[:no] += r.uniform(-40, 40, (no, 2))
     return x1.astype(np.float32), x2.astype(np.float32)
+
+
+def make_two_view(seed=660, n=150, outlier_frac=0.0, noise_px=0.5, kind="general", cal=EUROC):
+    """Frames i and j of init_sfm's two-view step (initializer.cpp:117-127): n world points seen from two camera poses,
+    Gaussian pixel noise, the first int(outlier_frac n) matches of frame j displaced by 20 to 80 pixels.
+    kind: 'general' (depths 3..12 m, a 1 m baseline), 'plane' (every point on one tilted plane), 'rotation' (no
+    translation), 'small' (a 2 cm baseline and a
+    small rotation: too little parallax).  Returns a dict: p1, p2 [n][2] normalised keypoints,
+    fx, fy, R, t (x_j = R x_i + t), X [n][3] the points in frame i."""
+    r = np.random.default_rng(seed)
+    fx, fy = cal["K"][0], cal["K"][1]
+    X = np.stack([r.uniform(-4, 4, n), r.uniform(-3, 3, n), r.uniform(3, 12, n)], 1)
+    if kind == "plane":
+        X[:, 2] = 7.0 + 0.3 * X[:, 0] - 0.2 * X[:, 1]
+    w = r.normal(0, 0.08, 3) * (0.05 if kind == "small" else 1.0)
+    R = _rodrigues(w)
+    b = {"general": 1.0, "plane": 1.0, "rotation": 0.0, "small": 0.02}[kind]
+    d = r.normal(0, 1, 3)
+    d[2] *= 0.3
+    t = b * d / np.linalg.norm(d)
+    Xj = X @ R.T + t
+    p1 = X[:, :2] / X[:, 2:]
+    p2 = Xj[:, :2] / Xj[:, 2:]
+    px = np.array([fx, fy])
+    p1 = p1 + r.normal(0, noise_px, p1.shape) / px
+    p2 = p2 + r.normal(0, noise_px, p2.shape) / px
+    no = int(outlier_frac * n)
+    if no:
+        off = r.uniform(20, 80, (no, 2)) * r.choice([-1, 1], (no, 2))
+        p2[:no] += off / px
+    return dict(p1=p1, p2=p2, fx=fx, fy=fy, R=R, t=t, X=X)
+
+
+def _rodrigues(w):
+    th = np.linalg.norm(w)
+    k = w / th
+    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    return np.eye(3) + np.sin(th) * Kx + (1 - np.cos(th)) * Kx @ Kx
