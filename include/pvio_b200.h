@@ -506,7 +506,9 @@ int pvio_b200_sync(pvio_b200_handle h);
 int pvio_b200_timer_start(pvio_b200_handle h);
 int pvio_b200_timer_stop(pvio_b200_handle h, float *ms);
 /* device-side time (ms) of the linearise + Schur stage from CUDA events around its launches: which = 0 the most recent
- * stage, 1 the mean stage since the last reset, 2 / 3 the mean of the linearise / Schur kernel alone, -1 reset */
+ * stage, 1 the mean stage since the last reset, 2 / 3 the mean of the linearise / Schur kernel alone, -1 reset.  Always
+ * the whole batch's: when batch_gn_step runs it as overlapping sub-batches, 2 ends with the batch's last linearise sweep
+ * and 3 is the Schur time left after it (DESIGN §7) */
 int pvio_b200_last_kernel_ms(pvio_b200_handle h, int which, float *ms);
 
 /* ---- visual-inertial PnP (SURVEY 8f rank 2) ------------------------------------------------ */

@@ -201,6 +201,9 @@ def load():
     lib.pvio_b200_timer_start.argtypes = [vp]
     lib.pvio_b200_timer_stop.argtypes = [vp, c_f32p]
     lib.pvio_b200_last_kernel_ms.argtypes = [vp, C.c_int, c_f32p]
+    # internal, not in the header: force batch_gn_step's sub-batch count (tests/test_gpu_step_split.py, tools/)
+    lib.pvio_b200_internal_set_step_split.argtypes = [vp, C.c_int]
+    lib.pvio_b200_internal_set_step_split.restype = C.c_int
     lib.pvio_b200_pnp_solve.argtypes = [vp, C.POINTER(CPnpProblem), c_f64p, C.POINTER(COptions), C.POINTER(CSummary)]
     lib.pvio_b200_batch_pnp_solve.argtypes = [vp, C.c_int, C.POINTER(CPnpProblem), c_f64p, C.c_int64,
                                               C.POINTER(COptions), C.POINTER(CSummary)]

@@ -703,15 +703,86 @@ static int launch_aux_cost(Handle *h, int n, const StepCfg &c, const BatchShape 
     return 0;
 }
 
-// One plain Gauss-Newton iteration (fixed mu, step beta * dx_gn): linearise, Schur, solve, back-substitution +
-// candidate in one sweep, non-vision cost + optional acceptance.  5 launches.
+// One plain Gauss-Newton iteration (fixed mu, step beta * dx_gn): linearise, Schur, solve (which also clears the
+// window's step scalars), back-substitution + candidate in one sweep, non-vision cost + optional acceptance.  5 launches.
 static int run_gn_step(Handle *h, int n, const StepCfg &c, const BatchShape &b) {
-    cudaStream_t st = c.stream ? c.stream : h->stream;
     TRY(run_linearize(h, n, c, b));
     TRY(run_solve(h, n, c, b));
-    CK(h, cudaMemsetAsync(h->acc.d + (size_t)kAcc * c.w0, 0, sizeof(double) * kAcc * n, st));
     TRY(launch_update<0>(h, n, c, b, sweep_grid_x(h, n)));
     TRY(launch_aux_cost(h, n, c, b));
+    return 0;
+}
+
+// The second stream of the split step shares the handle's aux stream (the latency path only captures through it)
+static int aux_stream(Handle *h) {
+    if (h->stream_aux) return 0;
+    CK(h, cudaStreamCreateWithFlags(&h->stream_aux, cudaStreamNonBlocking));
+    CK(h, cudaEventCreateWithFlags(&h->ev_aux_fork, cudaEventDisableTiming));
+    CK(h, cudaEventCreateWithFlags(&h->ev_aux_join, cudaEventDisableTiming));
+    return 0;
+}
+
+// Sub-batches of the plain batched step (run_gn_step_split).  Each sweep launch drains the whole grid before the next
+// sweep of the same windows may start: a sweep's last wave and the next sweep's first CTAs leave most SMs idle.  Cutting
+// the batch into contiguous sub-batches on two streams lets one sub-batch's CTAs fill what the other's tail leaves.
+// Measured on an H100 SXM (700 W, cfg2, DESIGN §9): 2 parts take 1.253 instead of 1.345 ms per step at 4096 windows,
+// 0.653 instead of 0.732 at 2048 and 0.372 instead of 0.386 at 1024; 4 parts are no faster at 4096 and slower below;
+// 3 parts are slower everywhere (two of them share a stream, so that stream's sweeps wait for each other).
+constexpr int kStepParts = 2, kStepPartsMax = 4, kStepSplitMinPerSm = 7;
+
+static int gn_step_parts(Handle *h, int n) {
+    // every part keeps the launch shapes of the whole batch: one CTA per window in the sweeps (sweep_grid_x) and the
+    // lean solve kernel (run_solve) -- at least max(SMs, 64) windows
+    const int most = std::min(kStepPartsMax, n / std::max(h->sm_count, 64));
+    const int want = h->step_parts > 0 ? h->step_parts : (n >= kStepSplitMinPerSm * h->sm_count ? kStepParts : 1);
+    return std::max(1, std::min(want, most));
+}
+
+// run_gn_step over `parts` contiguous sub-batches of equal size (+-1), on the handle's stream (even parts) and the aux
+// stream (odd parts), issued breadth first: lin(0), lin(1), ..., Schur(0), Schur(1), ...  Every window runs the same
+// kernels with the same arguments as in the unsplit step (b is the whole batch's shape), so the results are bit-identical.  The aux stream
+// joins the handle's stream before the call returns.  The stage times (last_kernel_ms) stay those of the whole batch:
+// from before the first linearise launch to the end of the last linearise (Schur) sweep of any sub-batch, taken on a
+// third stream that waits for both compute streams, so that no compute launch waits for a timing event.
+static int run_gn_step_split(Handle *h, int n, const StepCfg &c0, const BatchShape &b, int parts) {
+    TRY(aux_stream(h));
+    if (!h->stream_mark) {
+        CK(h, cudaStreamCreateWithFlags(&h->stream_mark, cudaStreamNonBlocking));
+        for (auto &e : h->ev_stage) CK(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    if (h->kev.empty()) {
+        h->kev.resize(3 * 256);
+        for (auto &e : h->kev) CK(h, cudaEventCreate(&e));
+    }
+    const int slot = (h->kev_count % 256) * 3;
+    cudaStream_t st[2] = {h->stream, h->stream_aux};
+    int w0[kStepPartsMax + 1];
+    for (int k = 0; k <= parts; ++k) w0[k] = (int)((int64_t)n * k / parts);
+    StepCfg c[kStepPartsMax];
+    for (int k = 0; k < parts; ++k) { c[k] = c0; c[k].w0 = w0[k]; c[k].stream = st[k & 1]; }
+    auto m = [&](int k) { return w0[k + 1] - w0[k]; };
+    auto mark = [&](cudaEvent_t e) {         // e: once every launch so far on both streams has finished
+        for (int s = 0; s < 2; ++s) {
+            CK(h, cudaEventRecord(h->ev_stage[s], st[s]));
+            CK(h, cudaStreamWaitEvent(h->stream_mark, h->ev_stage[s], 0));
+        }
+        CK(h, cudaEventRecord(e, h->stream_mark));
+        return 0;
+    };
+    CK(h, cudaEventRecord(h->kev[slot], h->stream));
+    CK(h, cudaEventRecord(h->ev_aux_fork, h->stream));
+    CK(h, cudaStreamWaitEvent(h->stream_aux, h->ev_aux_fork, 0));
+    for (int k = 0; k < parts; ++k) TRY(launch_lin(h, m(k), c[k], b, true, false, false));
+    TRY(mark(h->kev[slot + 1]));
+    for (int k = 0; k < parts; ++k) TRY(launch_schur(h, m(k), c[k], b, false));
+    TRY(mark(h->kev[slot + 2]));
+    ++h->kev_count;
+    for (int k = 0; k < parts; ++k) TRY(run_solve(h, m(k), c[k], b));
+    for (int k = 0; k < parts; ++k) TRY(launch_update<0>(h, m(k), c[k], b, 1));
+    for (int k = 0; k < parts; ++k) TRY(launch_aux_cost(h, m(k), c[k], b));
+    CK(h, cudaEventRecord(h->ev_aux_join, h->stream_aux));
+    CK(h, cudaStreamWaitEvent(h->stream, h->ev_aux_join, 0));
+    CK(h, cudaStreamWaitEvent(h->stream, h->kev[slot + 2], 0));   // last_kernel_ms synchronises the handle's stream only
     return 0;
 }
 
@@ -774,11 +845,7 @@ static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaS
         const int64_t l0 = h->launches;
         cudaGraph_t g = nullptr;
         cudaGraphExec_t ge = nullptr;
-        if (!h->stream_aux) {
-            CK(h, cudaStreamCreateWithFlags(&h->stream_aux, cudaStreamNonBlocking));
-            CK(h, cudaEventCreateWithFlags(&h->ev_aux_fork, cudaEventDisableTiming));
-            CK(h, cudaEventCreateWithFlags(&h->ev_aux_join, cudaEventDisableTiming));
-        }
+        TRY(aux_stream(h));
         c.fork_aux = 1;                // a second branch of the graph (captured through h->stream_aux)
         CK(h, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
         h->capturing = true;
@@ -1095,6 +1162,7 @@ void pvio_b200_destroy(pvio_b200_handle hh) {
     for (auto &st : h->stream_c) cudaStreamDestroy(st);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->stream_aux) { cudaStreamDestroy(h->stream_aux); cudaEventDestroy(h->ev_aux_fork); cudaEventDestroy(h->ev_aux_join); }
+    if (h->stream_mark) { cudaStreamDestroy(h->stream_mark); for (auto &e : h->ev_stage) cudaEventDestroy(e); }
     cudaStreamDestroy(h->stream);
     delete h;                        // frees every buffer (DevBuf)
 }
@@ -1134,7 +1202,8 @@ int pvio_b200_timer_stop(pvio_b200_handle hh, float *ms) {
 
 // Device time of the linearise + Schur stage from the CUDA events recorded around its launches:
 // which = 0 the most recent stage; 1 the MEAN stage over the launches since the last reset (at most the latest 256);
-// 2 / 3 the mean of the linearise / the Schur kernel alone; -1 resets the accumulation.
+// 2 / 3 the mean of the linearise / the Schur kernel alone; -1 resets the accumulation.  A split step (run_gn_step_split)
+// records the same three events for the whole batch.
 int pvio_b200_last_kernel_ms(pvio_b200_handle hh, int which, float *ms) {
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
@@ -1190,7 +1259,18 @@ int pvio_b200_batch_gn_step(pvio_b200_handle hh, int n, double mu, int apply) {
     TRY(check_packed(h, n, "batch_gn_step"));
     StepCfg c;
     c.mu = mu; c.apply = apply; c.compute_scale = 1;
-    return run_gn_step(h, n, c, batch_shape(h, 0, n, false));
+    const BatchShape b = batch_shape(h, 0, n, false);
+    const int parts = gn_step_parts(h, n);
+    return parts > 1 ? run_gn_step_split(h, n, c, b, parts) : run_gn_step(h, n, c, b);
+}
+
+// Not in the public header: the sub-batch count of batch_gn_step forced (parts > 0, at most 4, fewer when the batch is
+// too small to keep the launch shapes) or chosen from the batch (0).  For the bit-identity tests and the tuning tools.
+int pvio_b200_internal_set_step_split(pvio_b200_handle hh, int parts) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h || parts < 0 || parts > kStepPartsMax) return PVIO_B200_EINVAL;
+    h->step_parts = parts;
+    return 0;
 }
 
 int pvio_b200_batch_download(pvio_b200_handle hh, int n, double *dx, int64_t dx_stride, double *costs) {

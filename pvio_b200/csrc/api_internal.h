@@ -200,7 +200,11 @@ struct Handle {
     std::vector<cudaStream_t> stream_c;                        // compute streams of the pipelined host path
     cudaEvent_t ev_fork = nullptr;
     cudaStream_t stream_aux = nullptr;                         // second branch of the captured single-window solve (api.cu: iteration_body)
-    cudaEvent_t ev_aux_fork = nullptr, ev_aux_join = nullptr;
+    cudaEvent_t ev_aux_fork = nullptr, ev_aux_join = nullptr;  //   and the second stream of the split batched step
+    cudaStream_t stream_mark = nullptr;                        // stage-time events of the split batched step (api.cu:
+    cudaEvent_t ev_stage[2] = {nullptr, nullptr};              //   run_gn_step_split), recorded once both streams are done
+    int step_parts = 0;                                        // batch_gn_step's sub-batches: 0 chosen from the batch (api.cu:
+                                                               //   gn_step_parts); > 0 forced by the internal entry point
     std::vector<cudaEvent_t> ev_up, ev_done, ev_down;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::string err;

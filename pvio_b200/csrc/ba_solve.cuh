@@ -961,6 +961,8 @@ static __device__ __forceinline__ void solve_body(const SolveArgs &a) {
             ctrl.fresh = 1;
         }
     }
+    // plain step: clear the scalars the back-substitution sweep adds to (in the loop it stores them, ba_update.cuh)
+    if (!a.loop && tid < kAcc) a.acc[(size_t)w * kAcc + tid] = 0.0;
     SOLVE_STAMP(9);
 }
 
