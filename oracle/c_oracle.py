@@ -44,7 +44,7 @@ def gn_step(win, st, mu=1e-8):
     pa = L.PackedArgs(win, st)
     dx = np.zeros(15 * win.N + win.M)
     c0, c1 = C.c_double(), C.c_double()
-    rc = lib.ba_oracle_gn_step(C.byref(pa.cw), C.byref(pa.cs), mu, L._ptr(dx, C.c_double), C.byref(c0), C.byref(c1))
+    rc = lib.ba_oracle_gn_step(C.byref(pa.cw), C.byref(pa.cs), mu, L.ptr(dx), C.byref(c0), C.byref(c1))
     assert rc == 0
     return dict(dx=dx, cost=c0.value, new_cost=c1.value)
 
@@ -64,8 +64,7 @@ def marginalize(win, st, index=0):
     pa = L.PackedArgs(win, st)
     d = 15 * (win.N - 1)
     S, e, H, b = np.zeros((d, d)), np.zeros(d), np.zeros((d, d)), np.zeros(d)
-    rc = lib.ba_oracle_marginalize(C.byref(pa.cw), C.byref(pa.cs), index, L._ptr(S, C.c_double), L._ptr(e, C.c_double),
-                                   L._ptr(H, C.c_double), L._ptr(b, C.c_double))
+    rc = lib.ba_oracle_marginalize(C.byref(pa.cw), C.byref(pa.cs), index, L.ptr(S), L.ptr(e), L.ptr(H), L.ptr(b))
     assert rc == 0
     return S, e, H, b
 
@@ -82,10 +81,7 @@ def batch(kind, win, st, n_windows, n_threads=0, mu=1e-8, max_iter=10, index=0, 
     iters = np.zeros(n_windows, dtype=np.int64) if k == 1 else None
     fcost = np.zeros(n_windows) if k == 1 else None
     used = lib.ba_oracle_batch(k, n_windows, n_threads, C.byref(pa.cw), C.byref(pa.cs), C.byref(opt), mu, index,
-                               L._ptr(dx, C.c_double) if dx is not None else None,
-                               L._ptr(costs, C.c_double) if costs is not None else None,
-                               iters.ctypes.data_as(C.POINTER(C.c_int64)) if iters is not None else None,
-                               L._ptr(fcost, C.c_double) if fcost is not None else None)
+                               L.ptr(dx), L.ptr(costs), L.ptr(iters), L.ptr(fcost))
     units = int(iters.sum()) if k == 1 else n_windows
     return (used, units, dict(dx=dx, costs=costs, iters=iters, final_costs=fcost)) if want else (used, units)
 

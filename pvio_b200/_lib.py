@@ -1,4 +1,6 @@
-"""ctypes loader for libpvio_b200.so (the C-ABI in include/pvio_b200.h).
+"""ctypes binding of libpvio_b200.so (the C-ABI in include/pvio_b200.h): the header's constants, its structs as ctypes
+classes, one signature table that load() applies to every entry point, and the typed pointer helpers.  This is the
+only module that declares the ABI; tests/test_abi_bindings.py holds it to the header.
 
 There is NO CPU fallback: if the shared library is missing or no CUDA device is present the
 product path raises.  The library is built in-tree by `python -m pvio_b200.build`
@@ -13,8 +15,15 @@ LIB_PATH = os.path.join(_HERE, "libpvio_b200.so")
 if os.environ.get("PVIO_B200_TUNE_LIB"):        # tools/ only: a tuning build of the same sources (pvio_b200.build, defines=...)
     LIB_PATH = os.environ["PVIO_B200_TUNE_LIB"]
 
-IMU_STRIDE = 288
+# ---- the header's constants (PVIO_B200_<name>) ----------------------------------------------------------------------
+OK, ENODEV, EINVAL, ENOMEM, ECUDA, ENUMERIC = 0, -1, -2, -3, -4, -5
 FRAME_STRIDE = 16
+IMU_STRIDE = 288
+IMU_DT, IMU_DQ, IMU_DP, IMU_DV, IMU_SQRT_INV_COV = 0, 1, 5, 8, 11
+IMU_DQ_DBG, IMU_DP_DBG, IMU_DP_DBA, IMU_DV_DBG, IMU_DV_DBA, IMU_BG0, IMU_BA0 = 236, 245, 254, 263, 272, 281, 284
+TERM_CONVERGENCE, TERM_NO_CONVERGENCE, TERM_FAILURE = 0, 1, 2
+TWO_VIEW_OK, TWO_VIEW_FEW_MATCHES, TWO_VIEW_LOW_PARALLAX, TWO_VIEW_PURE_ROTATION, TWO_VIEW_FEW_TRIANGULATED = 0, 1, 2, 3, 4
+LENS_RADTAN, LENS_EQUIDISTANT = 1, 2
 
 c_i32p = C.POINTER(C.c_int32)
 c_u8p = C.POINTER(C.c_uint8)
@@ -133,33 +142,97 @@ class CTwoView(C.Structure):
                 ("e_schedule", c_i32p), ("h_counts", c_i32p), ("e_counts", c_i32p)]
 
 
-EXPORTS = [
-    "pvio_b200_create", "pvio_b200_destroy", "pvio_b200_last_error", "pvio_b200_kernel_launches",
-    "pvio_b200_version", "pvio_b200_ba_solve", "pvio_b200_ba_gn_step", "pvio_b200_ba_marginalize",
-    "pvio_b200_reprojection_error", "pvio_b200_batch_set_window", "pvio_b200_batch_replicate",
-    "pvio_b200_batch_upload", "pvio_b200_batch_gn_step", "pvio_b200_batch_download",
-    "pvio_b200_batch_gn_step_host", "pvio_b200_sync", "pvio_b200_timer_start", "pvio_b200_timer_stop",
-    "pvio_b200_last_kernel_ms", "pvio_b200_klt_track", "pvio_b200_pnp_solve", "pvio_b200_preintegrate",
-    "pvio_b200_triangulate", "pvio_b200_klt_track_raw", "pvio_b200_clahe", "pvio_b200_batch_solve",
-    "pvio_b200_batch_download_state", "pvio_b200_batch_solve_host", "pvio_b200_selftest_lie", "pvio_b200_klt_track_cached",
-    "pvio_b200_window_reset", "pvio_b200_window_append_frame", "pvio_b200_window_add_tracks",
-    "pvio_b200_window_add_observations", "pvio_b200_window_remove_track", "pvio_b200_window_set_prior",
-    "pvio_b200_window_solve", "pvio_b200_window_drop_victim", "pvio_b200_window_get", "pvio_b200_detect_keypoints",
-    "pvio_b200_find_fundamental_mask", "pvio_b200_track_keypoints", "pvio_b200_fm_sample_schedule",
-    "pvio_b200_batch_marginalize", "pvio_b200_batch_pnp_solve", "pvio_b200_batch_track_keypoints",
-    "pvio_b200_batch_detect_keypoints", "pvio_b200_selftest_eig", "pvio_b200_batch_window_reset",
-    "pvio_b200_batch_window_set_prior", "pvio_b200_batch_window_edit", "pvio_b200_batch_window_solve",
-    "pvio_b200_batch_window_drop_victim", "pvio_b200_batch_window_download", "pvio_b200_batch_window_set_planes",
-    "pvio_b200_batch_window_localize", "pvio_b200_batch_window_set_imu", "pvio_b200_batch_window_imu_records",
-    "pvio_b200_batch_window_track_frame", "pvio_b200_undistort_map", "pvio_b200_batch_set_lens", "pvio_b200_batch_undistort",
-    "pvio_b200_batch_two_view",
-]
+# ---- the signature table: name -> (restype, argtypes), in the header's order -----------------------------------------
+_int, _i32, _i64, _u64, _f64, _h = C.c_int, C.c_int32, C.c_int64, C.c_uint64, C.c_double, C.c_void_p
+_P = C.POINTER
+_intp = _P(C.c_int)
+SIGNATURES = {
+    "pvio_b200_create": (_int, [_int, _int, _int, _int, _int, _P(_h)]),
+    "pvio_b200_destroy": (None, [_h]),
+    "pvio_b200_last_error": (C.c_char_p, [_h]),
+    "pvio_b200_kernel_launches": (_i64, [_h]),
+    "pvio_b200_version": (C.c_char_p, []),
+    "pvio_b200_ba_solve": (_int, [_h, _P(CWindow), _P(CState), _P(COptions), _P(CSummary), c_u8p, c_f64p]),
+    "pvio_b200_ba_gn_step": (_int, [_h, _P(CWindow), _P(CState), _f64, c_f64p, c_f64p, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_ba_marginalize": (_int, [_h, _P(CWindow), _P(CState), _int, c_f64p, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_window_reset": (_int, [_h, _P(CWindow)]),
+    "pvio_b200_window_append_frame": (_int, [_h, c_f64p, _int, c_f64p]),
+    "pvio_b200_window_add_tracks": (_int, [_h, _int, c_i32p, c_f64p, c_f64p, c_i32p]),
+    "pvio_b200_window_add_observations": (_int, [_h, _int, c_i32p, c_i32p, c_f64p]),
+    "pvio_b200_window_remove_track": (_int, [_h, _i32]),
+    "pvio_b200_window_set_prior": (_int, [_h, _int, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_window_solve": (_int, [_h, _P(COptions), _P(CSummary)]),
+    "pvio_b200_window_drop_victim": (_int, [_h]),
+    "pvio_b200_window_get": (_int, [_h, c_i32p, c_f64p, _int, c_i32p, c_f64p, c_i32p, c_i32p]),
+    "pvio_b200_reprojection_error": (_int, [_h, _P(CWindow), _P(CState), c_f64p]),
+    "pvio_b200_batch_set_window": (_int, [_h, _int, _P(CWindow), _P(CState)]),
+    "pvio_b200_batch_replicate": (_int, [_h, _int]),
+    "pvio_b200_batch_upload": (_int, [_h, _int]),
+    "pvio_b200_batch_gn_step": (_int, [_h, _int, _f64, _int]),
+    "pvio_b200_batch_download": (_int, [_h, _int, c_f64p, _i64, c_f64p]),
+    "pvio_b200_batch_gn_step_host": (_int, [_h, _int, _f64, c_f64p, _i64, c_f64p]),
+    "pvio_b200_batch_solve": (_int, [_h, _int, _P(COptions)]),
+    "pvio_b200_batch_download_state": (_int, [_h, _int, c_f64p, _i64, c_f64p, _i64, _P(CSummary)]),
+    "pvio_b200_batch_solve_host": (_int, [_h, _int, _P(COptions), c_f64p, _i64, c_f64p, _i64, _P(CSummary)]),
+    "pvio_b200_batch_marginalize": (_int, [_h, _int, c_f64p, _i64, c_f64p, _i64]),
+    "pvio_b200_batch_window_reset": (_int, [_h, _int, _P(CWindow)]),
+    "pvio_b200_batch_window_set_prior": (_int, [_h, _int, _int, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_batch_window_edit": (_int, [_h, _int, _P(CWindowEdit)]),
+    "pvio_b200_batch_window_set_planes": (_int, [_h, _int, _P(CWindowPlanes)]),
+    "pvio_b200_batch_window_solve": (_int, [_h, _int, c_i32p, _P(COptions), _P(CSummary)]),
+    "pvio_b200_batch_window_drop_victim": (_int, [_h, _int, c_i32p, c_f64p, _i64, c_f64p, _i64]),
+    "pvio_b200_batch_window_download": (_int, [_h, _int, c_i32p, c_i32p, c_f64p, _i64, c_i32p, _i64, c_i32p, c_f64p,
+                                               c_i32p, c_i32p, c_u8p, c_f64p]),
+    "pvio_b200_batch_window_localize": (_int, [_h, _int, _P(CWindowLocalize), _P(COptions)]),
+    "pvio_b200_batch_window_set_imu": (_int, [_h, _int, _P(CWindowImu)]),
+    "pvio_b200_batch_window_imu_records": (_int, [_h, _int, c_i32p, c_f64p, _i64]),
+    "pvio_b200_batch_window_track_frame": (_int, [_h, _int, _P(CWindowTrackFrame), _P(COptions)]),
+    "pvio_b200_sync": (_int, [_h]),
+    "pvio_b200_timer_start": (_int, [_h]),
+    "pvio_b200_timer_stop": (_int, [_h, c_f32p]),
+    "pvio_b200_last_kernel_ms": (_int, [_h, _int, c_f32p]),
+    "pvio_b200_pnp_solve": (_int, [_h, _P(CPnpProblem), c_f64p, _P(COptions), _P(CSummary)]),
+    "pvio_b200_batch_pnp_solve": (_int, [_h, _int, _P(CPnpProblem), c_f64p, _i64, _P(COptions), _P(CSummary)]),
+    "pvio_b200_klt_track_raw": (_int, [_h, c_u8p, c_u8p, _int, _int, _int, c_f32p, c_f32p, c_u8p, c_f32p, _int, _int,
+                                       _int, _f64, _f64, _int, _int, c_u8p, c_u8p]),
+    "pvio_b200_klt_track_cached": (_int, [_h, _u64, c_u8p, _u64, c_u8p, _int, _int, _int, c_f32p, c_f32p, c_u8p, c_f32p,
+                                          _int, _int, _int, _f64, _f64, _int, _int, _int]),
+    "pvio_b200_detect_keypoints": (_int, [_h, _u64, c_u8p, _int, _int, _int, _f64, _int, _int, c_f64p, _int, _f64, _int,
+                                          c_f64p, _intp, c_f32p, _intp]),
+    "pvio_b200_find_fundamental_mask": (_int, [_h, _int, c_f32p, c_f32p, _f64, _f64, _int, c_i32p, _int, c_u8p, c_f64p,
+                                               c_i32p]),
+    "pvio_b200_fm_sample_schedule": (_int, [_int, c_f32p, c_f32p, _int, c_i32p]),
+    "pvio_b200_track_keypoints": (_int, [_h, _u64, c_u8p, _u64, c_u8p, _int, _int, _int, c_f32p, c_f32p, c_u8p, _int,
+                                         _int, _int, _f64, _f64, _int, _int, _int, _f64, _f64]),
+    "pvio_b200_batch_track_keypoints": (_int, [_h, _int, _P(CKltPair), _int, _int, _f64, _f64, _int, _int, _int, _f64,
+                                               _f64]),
+    "pvio_b200_batch_detect_keypoints": (_int, [_h, _int, _P(CDetectRequest), _f64, _int, _int]),
+    "pvio_b200_batch_two_view": (_int, [_h, _int, _P(CTwoView)]),
+    "pvio_b200_undistort_map": (_int, [_int, _int, _int, c_f64p, c_f64p, _P(C.c_int16), _P(C.c_uint16)]),
+    "pvio_b200_batch_set_lens": (_int, [_h, _int, _P(CLens)]),
+    "pvio_b200_batch_undistort": (_int, [_h, _int, _P(CUndistortRequest)]),
+    "pvio_b200_clahe": (_int, [_h, c_u8p, _int, _int, _int, _f64, _int, _int, c_u8p]),
+    "pvio_b200_preintegrate": (_int, [_h, _int, c_i32p, c_f64p, c_f64p, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_triangulate": (_int, [_h, _int, c_f64p, _int, c_i32p, c_i32p, c_f64p, c_f64p, c_u8p, c_f64p]),
+    "pvio_b200_selftest_lie": (_int, [_h, _int, c_f64p, c_f64p]),
+    "pvio_b200_selftest_eig": (_int, [_h, _int, c_i32p, c_f64p, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_klt_track": (_int, [_h, c_u8p, c_u8p, _int, _int, _int, c_f32p, c_f32p, c_u8p, c_f32p, _int, _int, _int,
+                                   _f64]),
+}
+EXPORTS = list(SIGNATURES)          # the header's entry points
+# not in the header: force batch_gn_step's sub-batch count (tests/test_gpu_step_split.py, tools/step_overlap.py)
+SIGNATURES["pvio_b200_internal_set_step_split"] = (_int, [_h, _int])
+# tuning builds only (-DPVIO_SOLVE_STAMPS / -DPVIO_MARG_STAMPS, loaded through PVIO_B200_TUNE_LIB): bound when present
+TUNING_SIGNATURES = {
+    "pvio_b200_debug_solve_stamps": (_int, [_P(C.c_longlong)]),
+    "pvio_b200_debug_marg_stamps": (_int, [_P(C.c_longlong)]),
+}
 
 _lib = None
 
 
 def load():
-    """Load the shared library (raises if it was not built: no fallback)."""
+    """Load the shared library and declare every entry point (raises if it was not built: no fallback)."""
     global _lib
     if _lib is not None:
         return _lib
@@ -167,66 +240,84 @@ def load():
         raise RuntimeError(f"{LIB_PATH} is missing: run `python -m pvio_b200.build` (nvcc, sm_90a). "
                            "pvio_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    vp = C.c_void_p
-    lib.pvio_b200_create.argtypes = [C.c_int] * 5 + [C.POINTER(vp)]
-    lib.pvio_b200_create.restype = C.c_int
-    lib.pvio_b200_destroy.argtypes = [vp]
-    lib.pvio_b200_destroy.restype = None
-    lib.pvio_b200_last_error.argtypes = [vp]
-    lib.pvio_b200_last_error.restype = C.c_char_p
-    lib.pvio_b200_kernel_launches.argtypes = [vp]
-    lib.pvio_b200_kernel_launches.restype = C.c_int64
-    lib.pvio_b200_version.restype = C.c_char_p
-    lib.pvio_b200_ba_solve.argtypes = [vp, C.POINTER(CWindow), C.POINTER(CState), C.POINTER(COptions),
-                                       C.POINTER(CSummary), c_u8p, c_f64p]
-    lib.pvio_b200_ba_gn_step.argtypes = [vp, C.POINTER(CWindow), C.POINTER(CState), C.c_double, c_f64p, c_f64p,
-                                         c_f64p, c_f64p, c_f64p]
-    lib.pvio_b200_ba_marginalize.argtypes = [vp, C.POINTER(CWindow), C.POINTER(CState), C.c_int, c_f64p, c_f64p,
-                                             c_f64p, c_f64p]
-    lib.pvio_b200_reprojection_error.argtypes = [vp, C.POINTER(CWindow), C.POINTER(CState), c_f64p]
-    lib.pvio_b200_batch_set_window.argtypes = [vp, C.c_int, C.POINTER(CWindow), C.POINTER(CState)]
-    lib.pvio_b200_batch_replicate.argtypes = [vp, C.c_int]
-    lib.pvio_b200_batch_upload.argtypes = [vp, C.c_int]
-    lib.pvio_b200_batch_gn_step.argtypes = [vp, C.c_int, C.c_double, C.c_int]
-    lib.pvio_b200_batch_download.argtypes = [vp, C.c_int, c_f64p, C.c_int64, c_f64p]
-    lib.pvio_b200_batch_gn_step_host.argtypes = [vp, C.c_int, C.c_double, c_f64p, C.c_int64, c_f64p]
-    lib.pvio_b200_batch_solve.argtypes = [vp, C.c_int, C.POINTER(COptions)]
-    lib.pvio_b200_batch_download_state.argtypes = [vp, C.c_int, c_f64p, C.c_int64, c_f64p, C.c_int64, C.POINTER(CSummary)]
-    lib.pvio_b200_batch_solve_host.argtypes = [vp, C.c_int, C.POINTER(COptions), c_f64p, C.c_int64, c_f64p, C.c_int64,
-                                               C.POINTER(CSummary)]
-    lib.pvio_b200_batch_marginalize.argtypes = [vp, C.c_int, c_f64p, C.c_int64, c_f64p, C.c_int64]
-    lib.pvio_b200_selftest_lie.argtypes = [vp, C.c_int, c_f64p, c_f64p]
-    lib.pvio_b200_selftest_eig.argtypes = [vp, C.c_int, c_i32p, c_f64p, c_f64p, c_f64p, c_f64p]
-    lib.pvio_b200_sync.argtypes = [vp]
-    lib.pvio_b200_timer_start.argtypes = [vp]
-    lib.pvio_b200_timer_stop.argtypes = [vp, c_f32p]
-    lib.pvio_b200_last_kernel_ms.argtypes = [vp, C.c_int, c_f32p]
-    # internal, not in the header: force batch_gn_step's sub-batch count (tests/test_gpu_step_split.py, tools/)
-    lib.pvio_b200_internal_set_step_split.argtypes = [vp, C.c_int]
-    lib.pvio_b200_internal_set_step_split.restype = C.c_int
-    lib.pvio_b200_pnp_solve.argtypes = [vp, C.POINTER(CPnpProblem), c_f64p, C.POINTER(COptions), C.POINTER(CSummary)]
-    lib.pvio_b200_batch_pnp_solve.argtypes = [vp, C.c_int, C.POINTER(CPnpProblem), c_f64p, C.c_int64,
-                                              C.POINTER(COptions), C.POINTER(CSummary)]
-    lib.pvio_b200_batch_track_keypoints.argtypes = [vp, C.c_int, C.POINTER(CKltPair), C.c_int, C.c_int, C.c_double,
-                                                    C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
-    lib.pvio_b200_batch_detect_keypoints.argtypes = [vp, C.c_int, C.POINTER(CDetectRequest), C.c_double, C.c_int, C.c_int]
-    lib.pvio_b200_undistort_map.argtypes = [C.c_int, C.c_int, C.c_int, c_f64p, c_f64p, C.POINTER(C.c_int16),
-                                            C.POINTER(C.c_uint16)]
-    lib.pvio_b200_batch_set_lens.argtypes = [vp, C.c_int, C.POINTER(CLens)]
-    lib.pvio_b200_batch_undistort.argtypes = [vp, C.c_int, C.POINTER(CUndistortRequest)]
-    lib.pvio_b200_batch_two_view.argtypes = [vp, C.c_int, C.POINTER(CTwoView)]
-    lib.pvio_b200_klt_track.argtypes = [vp, c_u8p, c_u8p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p,
-                                        C.c_int, C.c_int, C.c_int, C.c_double]
-    for name in EXPORTS:
+    for name, (restype, argtypes) in SIGNATURES.items():
         fn = getattr(lib, name)
-        if fn.restype is C.c_int and name not in ("pvio_b200_create",):
-            fn.restype = C.c_int
+        fn.restype, fn.argtypes = restype, argtypes
+    for name, (restype, argtypes) in TUNING_SIGNATURES.items():
+        if hasattr(lib, name):
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 
 
+# ---- typed pointers ---------------------------------------------------------------------------------------------------
+_CTYPE = {np.dtype(np.float64): C.c_double, np.dtype(np.float32): C.c_float, np.dtype(np.int64): C.c_int64,
+          np.dtype(np.int32): C.c_int32, np.dtype(np.int16): C.c_int16, np.dtype(np.uint16): C.c_uint16,
+          np.dtype(np.uint8): C.c_uint8}
+
+
+def ptr(a):
+    """A pointer to the data of array `a`, typed by its dtype (None: NULL).  Raises on an array that is not
+    C-contiguous; never copies."""
+    if a is None:
+        return None
+    if not a.flags.c_contiguous:
+        raise ValueError(f"a {a.dtype} array of shape {a.shape} is not C-contiguous")
+    ct = _CTYPE.get(a.dtype)
+    if ct is None:
+        raise TypeError(f"no C type for a {a.dtype} array")
+    return a.ctypes.data_as(C.POINTER(ct))
+
+
 def _ptr(a, ctype):
-    return a.ctypes.data_as(C.POINTER(ctype))
+    """ptr(a) for callers that name the element type; raises TypeError when a's dtype is not that type."""
+    if a is not None and _CTYPE.get(a.dtype) is not ctype:
+        raise TypeError(f"a {a.dtype} array is not a {ctype.__name__} array")
+    return ptr(a)
+
+
+def set_ptrs(rec, **arrays):
+    """Point the pointer fields of struct `rec` at the arrays (None: NULL), each through ptr(); raises TypeError when
+    an array's dtype is not the field's declared element type (ctypes refuses the assignment).  Returns rec."""
+    for name, a in arrays.items():
+        try:
+            setattr(rec, name, ptr(a))
+        except TypeError as e:
+            raise TypeError(f"{type(rec).__name__}.{name} does not take a {a.dtype} array: {e}") from None
+    return rec
+
+
+def check_rows(a, n, stride, name):
+    """Raises unless `a` is a C-contiguous float64 [n, stride] array: a caller's output buffer of a strided call."""
+    if a.dtype != np.float64 or not a.flags.c_contiguous or a.shape != (n, stride):
+        raise ValueError(f"{name} must be a C-contiguous float64 array of shape {(n, stride)}, "
+                         f"not {a.dtype} {a.shape}{'' if a.flags.c_contiguous else ' (strided)'}")
+
+
+def summary(sm):
+    """A CSummary as a dict of its fields."""
+    return {k: getattr(sm, k) for k, _ in CSummary._fields_}
+
+
+def imu_records(dt, dq, dp, dv, sqrt_inv_cov, dq_dbg, dp_dbg, dp_dba, dv_dbg, dv_dba, bg0=None, ba0=None):
+    """IMU factor records [n, IMU_STRIDE] in the header's layout (PVIO_B200_IMU_*) from the PreIntegrator outputs of n
+    factors: dt [n], dq [n, 4] (x, y, z, w), dp, dv [n, 3], sqrt_inv_cov [n, 15, 15], the five bias Jacobians [n, 3, 3],
+    and the bias linearisation point bg0, ba0 [n, 3] (None: left 0)."""
+    n = np.size(dt)
+    rec = np.zeros((n, IMU_STRIDE))
+    rec[:, IMU_DT] = dt
+    rec[:, IMU_DQ:IMU_DQ + 4] = dq
+    rec[:, IMU_DP:IMU_DP + 3] = dp
+    rec[:, IMU_DV:IMU_DV + 3] = dv
+    rec[:, IMU_SQRT_INV_COV:IMU_SQRT_INV_COV + 225] = np.asarray(sqrt_inv_cov).reshape(n, 225)
+    for o, m in ((IMU_DQ_DBG, dq_dbg), (IMU_DP_DBG, dp_dbg), (IMU_DP_DBA, dp_dba), (IMU_DV_DBG, dv_dbg),
+                 (IMU_DV_DBA, dv_dba)):
+        rec[:, o:o + 9] = np.asarray(m).reshape(n, 9)
+    if bg0 is not None:
+        rec[:, IMU_BG0:IMU_BG0 + 3] = bg0
+        rec[:, IMU_BA0:IMU_BA0 + 3] = ba0
+    return rec
 
 
 def window_constants(win):
@@ -253,51 +344,30 @@ class PackedArgs:
 
         cw = window_constants(win)
         cw.n_frames, cw.n_landmarks, cw.n_obs = win.N, win.M, win.K
-        cw.frame_fixed = _ptr(arr("fixed", win.frame_fixed, np.uint8), C.c_uint8)
-        cw.lm_anchor = _ptr(arr("anchor", win.lm_anchor, np.int32), C.c_int32)
-        cw.lm_z_ref = _ptr(arr("zref", win.lm_z_ref, np.float64), C.c_double)
-        cw.lm_obs_begin = _ptr(arr("ob", win.lm_obs_begin, np.int32), C.c_int32)
-        cw.lm_in_victim = _ptr(arr("victim", win.lm_in_victim if len(win.lm_in_victim) == win.M
-                                   else np.zeros(win.M), np.uint8), C.c_uint8)
-        cw.obs_frame = _ptr(arr("of", win.obs_frame, np.int32), C.c_int32)
-        cw.obs_z = _ptr(arr("oz", win.obs_z, np.float64), C.c_double)
+        set_ptrs(cw, frame_fixed=arr("fixed", win.frame_fixed, np.uint8), lm_anchor=arr("anchor", win.lm_anchor, np.int32),
+                 lm_z_ref=arr("zref", win.lm_z_ref, np.float64), lm_obs_begin=arr("ob", win.lm_obs_begin, np.int32),
+                 lm_in_victim=arr("victim", win.lm_in_victim if len(win.lm_in_victim) == win.M else np.zeros(win.M),
+                                  np.uint8),
+                 obs_frame=arr("of", win.obs_frame, np.int32), obs_z=arr("oz", win.obs_z, np.float64))
         cw.n_imu = win.n_imu if win.use_inertial else 0
         if cw.n_imu > 0:
-            rec = np.zeros((win.n_imu, IMU_STRIDE))
-            rec[:, 0] = win.imu_dt
-            rec[:, 1:5] = win.imu_dq
-            rec[:, 5:8] = win.imu_dp
-            rec[:, 8:11] = win.imu_dv
-            rec[:, 11:236] = win.imu_sqrt_inv_cov.reshape(win.n_imu, 225)
-            rec[:, 236:245] = win.imu_dq_dbg.reshape(win.n_imu, 9)
-            rec[:, 245:254] = win.imu_dp_dbg.reshape(win.n_imu, 9)
-            rec[:, 254:263] = win.imu_dp_dba.reshape(win.n_imu, 9)
-            rec[:, 263:272] = win.imu_dv_dbg.reshape(win.n_imu, 9)
-            rec[:, 272:281] = win.imu_dv_dba.reshape(win.n_imu, 9)
-            rec[:, 281:284] = win.imu_bg0
-            rec[:, 284:287] = win.imu_ba0
-            cw.imu_data = _ptr(arr("imu", rec, np.float64), C.c_double)
-            cw.imu_frame_i = _ptr(arr("imui", win.imu_frame_i, np.int32), C.c_int32)
-            cw.imu_frame_j = _ptr(arr("imuj", win.imu_frame_j, np.int32), C.c_int32)
+            rec = imu_records(win.imu_dt, win.imu_dq, win.imu_dp, win.imu_dv, win.imu_sqrt_inv_cov, win.imu_dq_dbg,
+                              win.imu_dp_dbg, win.imu_dp_dba, win.imu_dv_dbg, win.imu_dv_dba, win.imu_bg0, win.imu_ba0)
+            set_ptrs(cw, imu_data=arr("imu", rec, np.float64), imu_frame_i=arr("imui", win.imu_frame_i, np.int32),
+                     imu_frame_j=arr("imuj", win.imu_frame_j, np.int32))
         cw.n_prior = win.n_prior if win.use_inertial else 0
         if cw.n_prior > 0:
             x0 = np.concatenate([win.prior_q0, win.prior_p0, win.prior_v0, win.prior_bg0, win.prior_ba0], axis=1)
-            cw.prior_frames = _ptr(arr("pf", win.prior_frames, np.int32), C.c_int32)
-            cw.prior_S = _ptr(arr("pS", win.prior_S, np.float64), C.c_double)
-            cw.prior_e = _ptr(arr("pe", win.prior_e, np.float64), C.c_double)
-            cw.prior_state0 = _ptr(arr("px0", x0, np.float64), C.c_double)
+            set_ptrs(cw, prior_frames=arr("pf", win.prior_frames, np.int32), prior_S=arr("pS", win.prior_S, np.float64),
+                     prior_e=arr("pe", win.prior_e, np.float64), prior_state0=arr("px0", x0, np.float64))
         cw.n_planes = win.n_planes
         cw.n_plane_tracks = win.n_ptracks
         if win.n_ptracks > 0:
             pp = np.concatenate([win.plane_normal, win.plane_distance[:, None]], axis=1)
-            cw.plane_param = _ptr(arr("pp", pp, np.float64), C.c_double)
-            cw.pt_plane = _ptr(arr("ptp", win.pt_plane, np.int32), C.c_int32)
-            cw.pt_obs_begin = _ptr(arr("ptb", win.pt_obs_begin, np.int32), C.c_int32)
-            cw.pt_obs_frame = _ptr(arr("ptf", win.pt_obs_frame, np.int32), C.c_int32)
-            cw.pt_obs_z = _ptr(arr("ptz", win.pt_obs_z, np.float64), C.c_double)
+            set_ptrs(cw, plane_param=arr("pp", pp, np.float64), pt_plane=arr("ptp", win.pt_plane, np.int32),
+                     pt_obs_begin=arr("ptb", win.pt_obs_begin, np.int32),
+                     pt_obs_frame=arr("ptf", win.pt_obs_frame, np.int32), pt_obs_z=arr("ptz", win.pt_obs_z, np.float64))
         self.cw = cw
         frames = np.concatenate([st.q, st.p, st.v, st.bg, st.ba], axis=1)
-        cs = CState()
-        cs.frames = _ptr(arr("frames", frames, np.float64), C.c_double)
-        cs.inv_depth = _ptr(arr("rho", np.array(st.rho, dtype=np.float64, copy=True), np.float64), C.c_double)
-        self.cs = cs
+        self.cs = set_ptrs(CState(), frames=arr("frames", frames, np.float64),
+                           inv_depth=arr("rho", np.array(st.rho, dtype=np.float64, copy=True), np.float64))

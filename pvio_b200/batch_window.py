@@ -7,25 +7,6 @@ import numpy as np
 
 from . import _lib
 
-_i32p, _f64p, _u8p = C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_uint8)
-
-
-def _argtypes(L):
-    vp = C.c_void_p
-    L.pvio_b200_batch_window_reset.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindow)]
-    L.pvio_b200_batch_window_set_prior.argtypes = [vp, C.c_int, C.c_int, _f64p, _f64p, _f64p]
-    L.pvio_b200_batch_window_edit.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowEdit)]
-    L.pvio_b200_batch_window_set_planes.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowPlanes)]
-    L.pvio_b200_batch_window_solve.argtypes = [vp, C.c_int, _i32p, C.POINTER(_lib.COptions), C.POINTER(_lib.CSummary)]
-    L.pvio_b200_batch_window_drop_victim.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64, _f64p, C.c_int64]
-    L.pvio_b200_batch_window_download.argtypes = [vp, C.c_int, _i32p, _i32p, _f64p, C.c_int64, _i32p, C.c_int64, _i32p,
-                                                  _f64p, _i32p, _i32p, _u8p, _f64p]
-    L.pvio_b200_batch_window_localize.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowLocalize), C.POINTER(_lib.COptions)]
-    L.pvio_b200_batch_window_set_imu.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowImu)]
-    L.pvio_b200_batch_window_imu_records.argtypes = [vp, C.c_int, _i32p, _f64p, C.c_int64]
-    L.pvio_b200_batch_window_track_frame.argtypes = [vp, C.c_int, C.POINTER(_lib.CWindowTrackFrame), C.POINTER(_lib.COptions)]
-
-
 _constants = _lib.window_constants            # the CWindow a reset takes: the window's constants only
 
 
@@ -105,21 +86,20 @@ class TrackFrame(Localize):
 
 def _localize_fields(r, L, o, keep):
     """the observation and new-track fields of a localize / track_frame ctypes record r from L, outputs into dict o"""
-    p = _lib._ptr
     if L.obs:
         t = np.array([b[0] for b in L.obs], dtype=np.int32)
         z = np.ascontiguousarray([b[1] for b in L.obs], dtype=np.float64).reshape(-1, 2)
         x = np.array([np.full(3, np.nan) if b[2] is None else b[2] for b in L.obs], dtype=np.float64).reshape(-1, 3)
         keep += [t, z, x]
-        r.n_obs, r.obs_track, r.obs_z, r.obs_point = len(t), p(t, C.c_int32), p(z, C.c_double), p(x, C.c_double)
-        r.points_out = p(o["points"], C.c_double)
+        r.n_obs = len(t)
+        _lib.set_ptrs(r, obs_track=t, obs_z=z, obs_point=x, points_out=o["points"])
     if L.new:
         zl = np.ascontiguousarray([b[0] for b in L.new], dtype=np.float64).reshape(-1, 2)
         zn = np.ascontiguousarray([b[1] for b in L.new], dtype=np.float64).reshape(-1, 2)
         keep += [zl, zn]
-        r.n_new, r.new_z_last, r.new_z = len(zl), p(zl, C.c_double), p(zn, C.c_double)
-        r.new_valid, r.new_inv_depth = p(o["valid"], C.c_uint8), p(o["inv_depth"], C.c_double)
-        r.new_inv_depth_next = p(o["inv_depth_next"], C.c_double)
+        r.n_new = len(zl)
+        _lib.set_ptrs(r, new_z_last=zl, new_z=zn, new_valid=o["valid"], new_inv_depth=o["inv_depth"],
+                      new_inv_depth_next=o["inv_depth_next"])
 
 
 def _localize_out(L):
@@ -142,7 +122,6 @@ class BatchWindows:
     def __init__(self, ba):
         """ba: a BundleAdjustor (owns the device handle and its max_windows slots)."""
         self.ba, self.lib, self.h = ba, ba.lib, ba.h
-        _argtypes(self.lib)
 
     def reset(self, slot, win):
         """Start an empty resident window in `slot`; `win` carries the constants (its arrays are not used)."""
@@ -151,8 +130,8 @@ class BatchWindows:
     def set_prior(self, slot, S, e, state0):
         S = np.ascontiguousarray(S, dtype=np.float64); e = np.ascontiguousarray(e, dtype=np.float64)
         x0 = np.ascontiguousarray(state0, dtype=np.float64).reshape(-1, 16)
-        self.ba._ck(self.lib.pvio_b200_batch_window_set_prior(self.h, int(slot), len(x0), _lib._ptr(S, C.c_double),
-                                                              _lib._ptr(e, C.c_double), _lib._ptr(x0, C.c_double)))
+        self.ba._ck(self.lib.pvio_b200_batch_window_set_prior(self.h, int(slot), len(x0), _lib.ptr(S), _lib.ptr(e),
+                                                              _lib.ptr(x0)))
 
     def edit(self, edits):
         """Apply a list of Edit (distinct slots) in one call; returns the new track ids of each edit."""
@@ -162,9 +141,9 @@ class BatchWindows:
             r = recs[i]
             r.slot, r.replace_last = e.slot, 1 if e.replace_last else 0
             if e.state is not None:
-                keep.append(e.state); r.state = _lib._ptr(e.state, C.c_double); r.fixed = 1 if e.fixed else 0
-                if e.imu is not None:
-                    keep.append(e.imu); r.imu_record = _lib._ptr(e.imu, C.c_double)
+                keep += [e.state, e.imu]
+                _lib.set_ptrs(r, state=e.state, imu_record=e.imu)
+                r.fixed = 1 if e.fixed else 0
             out = np.zeros(max(len(e.new), 1), dtype=np.int32)
             ids.append(out)
             if e.new:
@@ -173,19 +152,19 @@ class BatchWindows:
                 rho = np.array([t[2] for t in e.new], dtype=np.float64)
                 keep += [f, z, rho]
                 r.n_new_tracks = len(e.new)
-                r.new_frame, r.new_z = _lib._ptr(f, C.c_int32), _lib._ptr(z, C.c_double)
-                r.new_inv_depth, r.new_ids = _lib._ptr(rho, C.c_double), _lib._ptr(out, C.c_int32)
+                _lib.set_ptrs(r, new_frame=f, new_z=z, new_inv_depth=rho, new_ids=out)
             if e.obs:
                 t = np.array([o[0] for o in e.obs], dtype=np.int32)
                 f = np.array([o[1] for o in e.obs], dtype=np.int32)
                 z = np.ascontiguousarray([o[2] for o in e.obs], dtype=np.float64).reshape(-1, 2)
                 keep += [t, f, z]
                 r.n_obs = len(e.obs)
-                r.obs_track, r.obs_frame, r.obs_z = _lib._ptr(t, C.c_int32), _lib._ptr(f, C.c_int32), _lib._ptr(z, C.c_double)
+                _lib.set_ptrs(r, obs_track=t, obs_frame=f, obs_z=z)
             if e.remove:
                 rm = np.array(e.remove, dtype=np.int32)
                 keep.append(rm)
-                r.n_remove, r.remove = len(rm), _lib._ptr(rm, C.c_int32)
+                r.n_remove = len(rm)
+                _lib.set_ptrs(r, remove=rm)
         self.ba._ck(self.lib.pvio_b200_batch_window_edit(self.h, len(edits), recs))
         return [o[:len(e.new)].copy() for o, e in zip(ids, edits)]
 
@@ -199,13 +178,14 @@ class BatchWindows:
                 r.n_planes = -1
             else:
                 keep.append(p.planes)
-                r.n_planes, r.plane_param = len(p.planes), _lib._ptr(p.planes, C.c_double)
+                r.n_planes = len(p.planes)
+                _lib.set_ptrs(r, plane_param=p.planes)
             if p.tracks:
                 t, ro = np.array(p.tracks, dtype=np.int32), np.array(p.roles, dtype=np.int32)
                 rho = np.array(p.rho, dtype=np.float64)
                 keep += [t, ro, rho]
                 r.n_set = len(t)
-                r.track, r.role, r.inv_depth = _lib._ptr(t, C.c_int32), _lib._ptr(ro, C.c_int32), _lib._ptr(rho, C.c_double)
+                _lib.set_ptrs(r, track=t, role=ro, inv_depth=rho)
         self.ba._ck(self.lib.pvio_b200_batch_window_set_planes(self.h, len(records), recs))
 
     def localize(self, records, max_iterations=10, initial_radius=0.0):
@@ -214,20 +194,19 @@ class BatchWindows:
         inv_depth (in the slot's newest frame) and inv_depth_next (in the new frame)."""
         keep, out, n = [], [], len(records)
         recs, sms = (_lib.CWindowLocalize * max(n, 1))(), (_lib.CSummary * max(n, 1))()
-        p = _lib._ptr
         for i, L in enumerate(records):
             r = recs[i]
             o = _localize_out(L)
             out.append(o)
-            r.slot, r.state, r.summary = L.slot, p(o["state"], C.c_double), C.pointer(sms[i])
-            if L.imu is not None:
-                keep.append(L.imu)
-                r.use_inertial, r.imu_record = 1, p(L.imu, C.c_double)
+            r.slot, r.summary = L.slot, C.pointer(sms[i])
+            keep.append(L.imu)
+            _lib.set_ptrs(r, state=o["state"], imu_record=L.imu)
+            r.use_inertial = 0 if L.imu is None else 1
             _localize_fields(r, L, o, keep)
         opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
         self.ba._ck(self.lib.pvio_b200_batch_window_localize(self.h, n, recs, C.byref(opt)))
         for i, o in enumerate(out):
-            o["summary"] = {k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_}
+            o["summary"] = _lib.summary(sms[i])
             o["valid"] = o["valid"].astype(bool)
         return out
 
@@ -239,7 +218,7 @@ class BatchWindows:
         opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
         self.ba._ck(self.lib.pvio_b200_batch_window_track_frame(self.h, len(records), recs, C.byref(opt)))
         for i, o in enumerate(out):
-            o["summary"] = {k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_}
+            o["summary"] = _lib.summary(sms[i])
             o["valid"] = o["valid"].astype(bool)
             o["keyframe"], o["parallax"] = bool(o["keyframe"][0]), float(o["parallax"][0])
             o["n_parallax"], o["skipped_frames"] = int(o["n_parallax"][0]), int(o["skipped_frames"][0])
@@ -250,7 +229,6 @@ class BatchWindows:
         """the ctypes records of a list of TrackFrame: (records, summaries, output arrays per record, arrays to keep)"""
         keep, out, n = [], [], len(records)
         recs, sms = (_lib.CWindowTrackFrame * max(n, 1))(), (_lib.CSummary * max(n, 1))()
-        p = _lib._ptr
         for i, T in enumerate(records):
             r = recs[i]
             o = _localize_out(T)
@@ -259,13 +237,12 @@ class BatchWindows:
                      skipped_frames=np.array([T.skipped], dtype=np.int32))
             out.append(o)
             r.slot, r.newest_is_keyframe = T.slot, 1 if T.newest_is_keyframe else 0
-            r.n_samples, r.samples, r.t_end, r.noise_cov = len(T.samples), p(T.samples, C.c_double), T.t_end, p(T.noise, C.c_double)
-            if T.merge is not None:
-                r.n_merge, r.merge_samples = len(T.merge), p(T.merge, C.c_double)
-            r.cx, r.cy = T.cx, T.cy
-            r.skipped_frames, r.state, r.predicted = p(o["skipped_frames"], C.c_int32), p(o["state"], C.c_double), p(o["predicted"], C.c_double)
-            r.imu_record, r.keyframe = p(o["imu_record"], C.c_double), p(o["keyframe"], C.c_uint8)
-            r.parallax, r.n_parallax, r.summary = p(o["parallax"], C.c_double), p(o["n_parallax"], C.c_int32), C.pointer(sms[i])
+            r.n_samples, r.n_merge, r.t_end = len(T.samples), 0 if T.merge is None else len(T.merge), T.t_end
+            r.cx, r.cy, r.summary = T.cx, T.cy, C.pointer(sms[i])
+            _lib.set_ptrs(r, samples=T.samples, merge_samples=T.merge, noise_cov=T.noise,
+                          skipped_frames=o["skipped_frames"], state=o["state"], predicted=o["predicted"],
+                          imu_record=o["imu_record"], keyframe=o["keyframe"], parallax=o["parallax"],
+                          n_parallax=o["n_parallax"])
             keep += [T.samples, T.noise] + ([] if T.merge is None else [T.merge])
             _localize_fields(r, T, o, keep)
         return recs, sms, out, keep
@@ -275,7 +252,7 @@ class BatchWindows:
         recs = (_lib.CWindowImu * max(len(records), 1))()
         for r, m in zip(recs, records):
             r.slot, r.frame, r.n_samples, r.t_end = m.slot, m.frame, len(m.samples), m.t_end
-            r.samples, r.noise_cov = _lib._ptr(m.samples, C.c_double), _lib._ptr(m.noise, C.c_double)
+            _lib.set_ptrs(r, samples=m.samples, noise_cov=m.noise)
         self.ba._ck(self.lib.pvio_b200_batch_window_set_imu(self.h, len(records), recs))
 
     def imu_records(self, slots):
@@ -283,31 +260,30 @@ class BatchWindows:
         s = np.ascontiguousarray(slots, dtype=np.int32)
         n = len(s)
         nf = np.zeros(max(n, 1), dtype=np.int32)
-        self.ba._ck(self.lib.pvio_b200_batch_window_download(self.h, n, _lib._ptr(s, C.c_int32), _lib._ptr(nf, C.c_int32),
-                                                             None, 0, None, 0, None, None, None, None, None, None))
+        self.ba._ck(self.lib.pvio_b200_batch_window_download(self.h, n, _lib.ptr(s), _lib.ptr(nf), None, 0, None, 0,
+                                                             None, None, None, None, None, None))
         stride = _lib.IMU_STRIDE * max(self.ba.max_frames - 1, 1)
         out = np.zeros((max(n, 1), stride))
-        self.ba._ck(self.lib.pvio_b200_batch_window_imu_records(self.h, n, _lib._ptr(s, C.c_int32), _lib._ptr(out, C.c_double),
-                                                                 stride))
+        self.ba._ck(self.lib.pvio_b200_batch_window_imu_records(self.h, n, _lib.ptr(s), _lib.ptr(out), stride))
         return [out[i, :_lib.IMU_STRIDE * max(int(nf[i]) - 1, 0)].reshape(-1, _lib.IMU_STRIDE).copy() for i in range(n)]
 
     def solve(self, slots, max_iterations=10, max_time=1e6, alias_bias=True, postpass=True):
         s = np.ascontiguousarray(slots, dtype=np.int32)
         opt = _lib.COptions(max_iterations, max_time, 1 if alias_bias else 0, 1 if postpass else 0, 0.0)
         sm = (_lib.CSummary * max(len(s), 1))()
-        self.ba._ck(self.lib.pvio_b200_batch_window_solve(self.h, len(s), _lib._ptr(s, C.c_int32), C.byref(opt), sm))
-        return [{k: getattr(sm[i], k) for k, _ in _lib.CSummary._fields_} for i in range(len(s))]
+        self.ba._ck(self.lib.pvio_b200_batch_window_solve(self.h, len(s), _lib.ptr(s), C.byref(opt), sm))
+        return [_lib.summary(sm[i]) for i in range(len(s))]
 
     def drop_victim(self, slots, want=False, max_frames=None):
         """Map::marginalize_frame(0) on the slots; want: also return each slot's new prior (S, e)."""
         s = np.ascontiguousarray(slots, dtype=np.int32)
         if not want:
-            self.ba._ck(self.lib.pvio_b200_batch_window_drop_victim(self.h, len(s), _lib._ptr(s, C.c_int32), None, 0, None, 0))
+            self.ba._ck(self.lib.pvio_b200_batch_window_drop_victim(self.h, len(s), _lib.ptr(s), None, 0, None, 0))
             return None
         d = 15 * ((max_frames or self.ba.max_frames) - 1)
         S = np.zeros((max(len(s), 1), d * d)); e = np.zeros((max(len(s), 1), d))
-        self.ba._ck(self.lib.pvio_b200_batch_window_drop_victim(self.h, len(s), _lib._ptr(s, C.c_int32), _lib._ptr(S, C.c_double),
-                                                                d * d, _lib._ptr(e, C.c_double), d))
+        self.ba._ck(self.lib.pvio_b200_batch_window_drop_victim(self.h, len(s), _lib.ptr(s), _lib.ptr(S), d * d,
+                                                                _lib.ptr(e), d))
         return S, e
 
     def download(self, slots, track_stride):
@@ -319,10 +295,9 @@ class BatchWindows:
         T = max(int(track_stride), 1)
         ids = np.zeros((max(n, 1), T), dtype=np.int32); rho = np.zeros((max(n, 1), T)); an = np.zeros_like(ids)
         cnt = np.zeros_like(ids); val = np.zeros((max(n, 1), T), dtype=np.uint8); q = np.zeros((max(n, 1), T))
-        p = _lib._ptr
-        self.ba._ck(self.lib.pvio_b200_batch_window_download(
-            self.h, n, p(s, C.c_int32), p(nf, C.c_int32), p(fr, C.c_double), fs, p(nt, C.c_int32), T, p(ids, C.c_int32),
-            p(rho, C.c_double), p(an, C.c_int32), p(cnt, C.c_int32), p(val, C.c_uint8), p(q, C.c_double)))
+        p = _lib.ptr
+        self.ba._ck(self.lib.pvio_b200_batch_window_download(self.h, n, p(s), p(nf), p(fr), fs, p(nt), T, p(ids), p(rho),
+                                                             p(an), p(cnt), p(val), p(q)))
         out = []
         for i in range(n):
             N, k = int(nf[i]), int(nt[i])

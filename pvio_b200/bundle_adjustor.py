@@ -57,11 +57,11 @@ class BundleAdjustor:
         valid = np.zeros(max(win.M, 1), dtype=np.uint8)
         quality = np.zeros(max(win.M, 1))
         self._ck(self.lib.pvio_b200_ba_solve(self.h, C.byref(pa.cw), C.byref(pa.cs), C.byref(opt), C.byref(sm),
-                                             _lib._ptr(valid, C.c_uint8), _lib._ptr(quality, C.c_double)))
+                                             _lib.ptr(valid), _lib.ptr(quality)))
         fr = pa.keep["frames"]
         out = State(fr[:, 0:4].copy(), fr[:, 4:7].copy(), fr[:, 7:10].copy(), fr[:, 10:13].copy(),
                     fr[:, 13:16].copy(), pa.keep["rho"].copy())
-        summ = {k: getattr(sm, k) for k, _ in _lib.CSummary._fields_}
+        summ = _lib.summary(sm)
         summ["valid"] = valid[:win.M].astype(bool)
         summ["quality"] = quality[:win.M]
         return out, summ
@@ -76,8 +76,8 @@ class BundleAdjustor:
         H = np.zeros((D, D)) if want_system else None
         g = np.zeros(D) if want_system else None
         self._ck(self.lib.pvio_b200_ba_gn_step(
-            self.h, C.byref(pa.cw), C.byref(pa.cs), mu, _lib._ptr(dx, C.c_double), C.byref(cost), C.byref(new_cost),
-            _lib._ptr(H, C.c_double) if want_system else None, _lib._ptr(g, C.c_double) if want_system else None))
+            self.h, C.byref(pa.cw), C.byref(pa.cs), mu, _lib.ptr(dx), C.byref(cost), C.byref(new_cost), _lib.ptr(H),
+            _lib.ptr(g)))
         out = dict(dx=dx, cost=cost.value, new_cost=new_cost.value)
         if want_system:
             out.update(Hred=H, gred=g)
@@ -91,8 +91,7 @@ class BundleAdjustor:
         H = np.zeros((d, d)) if want_info else None
         b = np.zeros(d) if want_info else None
         self._ck(self.lib.pvio_b200_ba_marginalize(
-            self.h, C.byref(pa.cw), C.byref(pa.cs), index, _lib._ptr(S, C.c_double), _lib._ptr(e, C.c_double),
-            _lib._ptr(H, C.c_double) if want_info else None, _lib._ptr(b, C.c_double) if want_info else None))
+            self.h, C.byref(pa.cw), C.byref(pa.cs), index, _lib.ptr(S), _lib.ptr(e), _lib.ptr(H), _lib.ptr(b)))
         return (S, e, H, b) if want_info else (S, e)
 
     def compute_reprojection_error(self, win, st):
@@ -126,8 +125,7 @@ class BundleAdjustor:
             return None
         dmax = 15 * (self.max_frames - 1)
         S, e = np.zeros((n, dmax * dmax)), np.zeros((n, dmax))
-        self._ck(self.lib.pvio_b200_batch_marginalize(self.h, n, _lib._ptr(S, C.c_double), dmax * dmax,
-                                                      _lib._ptr(e, C.c_double), dmax))
+        self._ck(self.lib.pvio_b200_batch_marginalize(self.h, n, _lib.ptr(S), dmax * dmax, _lib.ptr(e), dmax))
         out = []
         for i in range(n):
             d = 15 * (self._slot_frames[i] - 1)
@@ -143,15 +141,15 @@ class BundleAdjustor:
     def batch_download(self, n, stride):
         dx = np.zeros((n, stride))
         costs = np.zeros((n, 2))
-        self._ck(self.lib.pvio_b200_batch_download(self.h, n, _lib._ptr(dx, C.c_double), stride,
-                                                   _lib._ptr(costs, C.c_double)))
+        self._ck(self.lib.pvio_b200_batch_download(self.h, n, _lib.ptr(dx), stride, _lib.ptr(costs)))
         return dx, costs
 
     def batch_gn_step_host(self, n, stride, mu=1e-8, dx=None, costs=None):
         dx = np.zeros((n, stride)) if dx is None else dx
         costs = np.zeros((n, 2)) if costs is None else costs
-        self._ck(self.lib.pvio_b200_batch_gn_step_host(self.h, n, mu, _lib._ptr(dx, C.c_double), stride,
-                                                       _lib._ptr(costs, C.c_double)))
+        _lib.check_rows(dx, n, stride, "dx")
+        _lib.check_rows(costs, n, 2, "costs")
+        self._ck(self.lib.pvio_b200_batch_gn_step_host(self.h, n, mu, _lib.ptr(dx), stride, _lib.ptr(costs)))
         return dx, costs
 
     def batch_solve(self, n, max_iterations=10, max_time=0.0, alias_bias=True, initial_radius=0.0):
@@ -164,25 +162,27 @@ class BundleAdjustor:
         frames = np.zeros((n, N * 16))
         rho = np.zeros((n, max(M, 1)))
         sm = (_lib.CSummary * n)()
-        self._ck(self.lib.pvio_b200_batch_download_state(self.h, n, _lib._ptr(frames, C.c_double), N * 16,
-                                                         _lib._ptr(rho, C.c_double), max(M, 1), sm))
-        return frames.reshape(n, N, 16), rho[:, :M], [{k: getattr(x, k) for k, _ in _lib.CSummary._fields_} for x in sm]
+        self._ck(self.lib.pvio_b200_batch_download_state(self.h, n, _lib.ptr(frames), N * 16, _lib.ptr(rho), max(M, 1),
+                                                         sm))
+        return frames.reshape(n, N, 16), rho[:, :M], [_lib.summary(x) for x in sm]
 
     def batch_solve_host(self, n, N, M, max_iterations=10, alias_bias=True, frames=None, rho=None):
         """upload + solve + download through host buffers (the end-to-end call bench.py times)."""
         frames = np.zeros((n, N * 16)) if frames is None else frames
         rho = np.zeros((n, max(M, 1))) if rho is None else rho
+        _lib.check_rows(frames, n, N * 16, "frames")
+        _lib.check_rows(rho, n, max(M, 1), "rho")
         opt = _lib.COptions(max_iterations, 0.0, 1 if alias_bias else 0, 0, 0.0)
         sm = (_lib.CSummary * n)()
-        self._ck(self.lib.pvio_b200_batch_solve_host(self.h, n, C.byref(opt), _lib._ptr(frames, C.c_double), N * 16,
-                                                     _lib._ptr(rho, C.c_double), max(M, 1), sm))
+        self._ck(self.lib.pvio_b200_batch_solve_host(self.h, n, C.byref(opt), _lib.ptr(frames), N * 16, _lib.ptr(rho),
+                                                     max(M, 1), sm))
         return frames, rho, sm
 
     def selftest_lie(self, w):
         """Device expmap / logmap / right_jacobian / Plus on rotation vectors w [n, 3] -> [n, 32] (see the header)."""
         w = np.ascontiguousarray(w, dtype=np.float64)
         out = np.zeros((len(w), 32))
-        self._ck(self.lib.pvio_b200_selftest_lie(self.h, len(w), _lib._ptr(w, C.c_double), _lib._ptr(out, C.c_double)))
+        self._ck(self.lib.pvio_b200_selftest_lie(self.h, len(w), _lib.ptr(w), _lib.ptr(out)))
         return out
 
     def selftest_eig(self, problems):
@@ -191,8 +191,8 @@ class BundleAdjustor:
         A = np.concatenate([np.ascontiguousarray(a, dtype=np.float64).ravel() for a, _ in problems])
         b = np.concatenate([np.asarray(v, dtype=np.float64) for _, v in problems])
         S, e = np.zeros_like(A), np.zeros_like(b)
-        self._ck(self.lib.pvio_b200_selftest_eig(self.h, len(dk), _lib._ptr(dk, C.c_int32), _lib._ptr(A, C.c_double),
-                                                 _lib._ptr(b, C.c_double), _lib._ptr(S, C.c_double), _lib._ptr(e, C.c_double)))
+        self._ck(self.lib.pvio_b200_selftest_eig(self.h, len(dk), _lib.ptr(dk), _lib.ptr(A), _lib.ptr(b), _lib.ptr(S),
+                                                 _lib.ptr(e)))
         out, oa, ob = [], 0, 0
         for d in dk:
             out.append((S[oa:oa + d * d].reshape(d, d), e[ob:ob + d]))

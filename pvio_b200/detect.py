@@ -18,13 +18,10 @@ def detect_keypoints(ba, image, keypoints=(), keypoint_distance=25.0, clahe_clip
     out = np.zeros((max_out, 2))
     gftt = np.zeros((1000, 2), dtype=np.float32)
     n, ng = C.c_int(), C.c_int()
-    fn = ba.lib.pvio_b200_detect_keypoints
-    fn.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int,
-                   C.POINTER(C.c_double), C.c_int, C.c_double, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int),
-                   C.POINTER(C.c_float), C.POINTER(C.c_int)]
-    ba._ck(fn(ba.h, int(frame_id), None if img is None else _lib._ptr(img, C.c_uint8), w, h, w, float(clahe_clip),
-              clahe_tiles[0], clahe_tiles[1], _lib._ptr(ex, C.c_double) if len(ex) else None, len(ex), float(keypoint_distance),
-              max_out, _lib._ptr(out, C.c_double), C.byref(n), _lib._ptr(gftt, C.c_float), C.byref(ng)))
+    ba._ck(ba.lib.pvio_b200_detect_keypoints(ba.h, int(frame_id), _lib.ptr(img), w, h, w, float(clahe_clip), clahe_tiles[0],
+                                             clahe_tiles[1], _lib.ptr(ex) if len(ex) else None, len(ex),
+                                             float(keypoint_distance), max_out, _lib.ptr(out), C.byref(n), _lib.ptr(gftt),
+                                             C.byref(ng)))
     return (out[:n.value].copy(), gftt[:ng.value].copy()) if want_gftt else out[:n.value].copy()
 
 
@@ -45,15 +42,11 @@ def pack_requests(requests, want_gftt=False):
         c = cr[i]
         c.slot, c.width, c.height, c.stride = int(d["slot"]), w, h, w
         c.frame_id = int(d.get("frame_id", 0))
-        c.image = None if img is None else _lib._ptr(img, C.c_uint8)
-        c.existing = _lib._ptr(ex, C.c_double) if len(ex) else None
         c.n_existing = len(ex)
         c.max_out = max_out
         c.keypoint_distance = float(d.get("keypoint_distance", 25.0))
-        c.keypoints_out = _lib._ptr(out, C.c_double)
-        c.n_out = _lib._ptr(cnt, C.c_int32)
-        c.gftt_out = None if gftt is None else _lib._ptr(gftt, C.c_float)
-        c.n_gftt = C.cast(cnt.ctypes.data + 4, C.POINTER(C.c_int32))
+        _lib.set_ptrs(c, image=img, existing=ex if len(ex) else None, keypoints_out=out, n_out=cnt[:1], gftt_out=gftt,
+                      n_gftt=cnt[1:])
         keep += [img, ex, out, cnt, gftt]
         outs.append((out, cnt, gftt))
     return cr, outs, keep

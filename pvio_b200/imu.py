@@ -1,7 +1,5 @@
 """Host-side mirror of PreIntegrator::integrate (pvio/src/pvio/estimation/preintegrator.cpp:85-98) over
 the C ABI: batches of independent IMU factors, one warp each on the device (csrc/imu.cu)."""
-import ctypes as C
-
 import numpy as np
 
 from . import _lib
@@ -19,9 +17,6 @@ def preintegrate(ba, factors, noise_cov):
     bias = np.ascontiguousarray(np.array([np.concatenate([f[2], f[3]]) for f in factors], dtype=np.float64))
     noise = np.ascontiguousarray(np.array([np.asarray(c, dtype=np.float64).reshape(9) for c in noise_cov]))
     rec = np.zeros((n, _lib.IMU_STRIDE))
-    fn = ba.lib.pvio_b200_preintegrate
-    fn.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_double),
-                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
-    ba._ck(fn(ba.h, n, _lib._ptr(begin, C.c_int32), _lib._ptr(samples, C.c_double), _lib._ptr(t_end, C.c_double),
-              _lib._ptr(bias, C.c_double), _lib._ptr(noise, C.c_double), _lib._ptr(rec, C.c_double)))
+    ba._ck(ba.lib.pvio_b200_preintegrate(ba.h, n, _lib.ptr(begin), _lib.ptr(samples), _lib.ptr(t_end), _lib.ptr(bias),
+                                         _lib.ptr(noise), _lib.ptr(rec)))
     return rec

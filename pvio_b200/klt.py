@@ -2,8 +2,6 @@
 over the C-ABI: pyramidal LK on the GPU (pvio_b200_klt_track) followed by the reference's 20-px
 border rejection (:106) and the F-matrix RANSAC of :121-129 (pvio_b200_find_fundamental_mask;
 track_keypoints(..., ransac=True) is the whole OpenCvImage::track_keypoints)."""
-import ctypes as C
-
 import numpy as np
 
 from . import _lib
@@ -14,9 +12,7 @@ def clahe(ba, img, clip_limit=6.0, tiles=(8, 8)):
     img = np.ascontiguousarray(img, dtype=np.uint8)
     h, w = img.shape
     out = np.zeros_like(img)
-    fn = ba.lib.pvio_b200_clahe
-    fn.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_uint8)]
-    ba._ck(fn(ba.h, _lib._ptr(img, C.c_uint8), w, h, w, float(clip_limit), tiles[0], tiles[1], _lib._ptr(out, C.c_uint8)))
+    ba._ck(ba.lib.pvio_b200_clahe(ba.h, _lib.ptr(img), w, h, w, float(clip_limit), tiles[0], tiles[1], _lib.ptr(out)))
     return out
 
 
@@ -40,17 +36,12 @@ def track_keypoints(ba, prev_img, next_img, curr_keypoints, next_keypoints=None,
     status = np.zeros(max(n, 1), dtype=np.uint8)
     err = np.zeros(max(n, 1), dtype=np.float32)
     if clahe_clip > 0:
-        fn = ba.lib.pvio_b200_klt_track_raw
-        fn.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float),
-                       C.POINTER(C.c_float), C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.c_int, C.c_int, C.c_int, C.c_double,
-                       C.c_double, C.c_int, C.c_int, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8)]
-        rc = fn(ba.h, _lib._ptr(prev_img, C.c_uint8), _lib._ptr(next_img, C.c_uint8), w, h, w,
-                _lib._ptr(cur, C.c_float), _lib._ptr(nxt, C.c_float), _lib._ptr(status, C.c_uint8),
-                _lib._ptr(err, C.c_float), n, max_level, max_iter, eps, float(clahe_clip), clahe_tiles[0], clahe_tiles[1], None, None)
+        rc = ba.lib.pvio_b200_klt_track_raw(ba.h, _lib.ptr(prev_img), _lib.ptr(next_img), w, h, w, _lib.ptr(cur),
+                                            _lib.ptr(nxt), _lib.ptr(status), _lib.ptr(err), n, max_level, max_iter, eps,
+                                            float(clahe_clip), clahe_tiles[0], clahe_tiles[1], None, None)
     else:
-        rc = ba.lib.pvio_b200_klt_track(ba.h, _lib._ptr(prev_img, C.c_uint8), _lib._ptr(next_img, C.c_uint8), w, h, w,
-                                        _lib._ptr(cur, C.c_float), _lib._ptr(nxt, C.c_float), _lib._ptr(status, C.c_uint8),
-                                        _lib._ptr(err, C.c_float), n, max_level, max_iter, eps)
+        rc = ba.lib.pvio_b200_klt_track(ba.h, _lib.ptr(prev_img), _lib.ptr(next_img), w, h, w, _lib.ptr(cur), _lib.ptr(nxt),
+                                        _lib.ptr(status), _lib.ptr(err), n, max_level, max_iter, eps)
     ba._ck(rc)
     status, err = status[:n], err[:n]
     if not raw:
@@ -70,14 +61,10 @@ def _track_cached(ba, prev_img, next_img, curr_keypoints, next_keypoints, max_le
     n = len(cur)
     status = np.zeros(max(n, 1), dtype=np.uint8)
     err = np.zeros(max(n, 1), dtype=np.float32)
-    fn = ba.lib.pvio_b200_klt_track_cached
-    fn.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint8), C.c_uint64, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int,
-                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.c_int, C.c_int,
-                   C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int]
-    ptr = lambda a: None if a is None else _lib._ptr(a, C.c_uint8)
-    ba._ck(fn(ba.h, prev_id, ptr(imgs[0]), next_id, ptr(imgs[1]), w, h, w, _lib._ptr(cur, C.c_float), _lib._ptr(nxt, C.c_float),
-              _lib._ptr(status, C.c_uint8), _lib._ptr(err, C.c_float), n, max_level, max_iter, eps, float(clahe_clip),
-              clahe_tiles[0], clahe_tiles[1], int(border)))
+    p = _lib.ptr
+    ba._ck(ba.lib.pvio_b200_klt_track_cached(ba.h, prev_id, p(imgs[0]), next_id, p(imgs[1]), w, h, w, p(cur), p(nxt),
+                                             p(status), p(err), n, max_level, max_iter, eps, float(clahe_clip),
+                                             clahe_tiles[0], clahe_tiles[1], int(border)))
     return nxt, status[:n], err[:n]
 
 
@@ -92,12 +79,9 @@ def find_fundamental_mask(ba, p, q, threshold=1.0, confidence=0.99, max_iters=10
     F = np.zeros(9)
     info = np.zeros(4, dtype=np.int32)
     sch = None if schedule is None else np.ascontiguousarray(schedule, dtype=np.int32).reshape(-1, 7)
-    fn = ba.lib.pvio_b200_find_fundamental_mask
-    fn.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_double, C.c_double, C.c_int,
-                   C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_uint8), C.POINTER(C.c_double), C.POINTER(C.c_int32)]
-    ba._ck(fn(ba.h, n, _lib._ptr(p, C.c_float), _lib._ptr(q, C.c_float), float(threshold), float(confidence), int(max_iters),
-              None if sch is None else _lib._ptr(sch, C.c_int32), 0 if sch is None else len(sch),
-              _lib._ptr(mask, C.c_uint8), _lib._ptr(F, C.c_double), _lib._ptr(info, C.c_int32)))
+    ba._ck(ba.lib.pvio_b200_find_fundamental_mask(ba.h, n, _lib.ptr(p), _lib.ptr(q), float(threshold), float(confidence),
+                                                  int(max_iters), _lib.ptr(sch), 0 if sch is None else len(sch),
+                                                  _lib.ptr(mask), _lib.ptr(F), _lib.ptr(info)))
     out = (mask[:n], F.reshape(3, 3))
     if return_info:
         out += ({"iterations": int(info[0]), "best_iteration": int(info[1]), "best_model": int(info[2]),
@@ -118,14 +102,11 @@ def track_keypoints_ransac(ba, prev_img, next_img, curr_keypoints, next_keypoint
         np.array(next_keypoints, dtype=np.float32, copy=True).reshape(-1, 2)
     n = len(cur)
     status = np.zeros(max(n, 1), dtype=np.uint8)
-    fn = ba.lib.pvio_b200_track_keypoints
-    fn.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint8), C.c_uint64, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int,
-                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, C.c_double,
-                   C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
-    ptr = lambda a: None if a is None else _lib._ptr(a, C.c_uint8)
-    ba._ck(fn(ba.h, prev_id, ptr(imgs[0]), next_id, ptr(imgs[1]), w, h, w, _lib._ptr(cur, C.c_float), _lib._ptr(nxt, C.c_float),
-              _lib._ptr(status, C.c_uint8), n, max_level, max_iter, eps, float(clahe_clip), clahe_tiles[0], clahe_tiles[1],
-              int(border), float(ransac_threshold), float(ransac_confidence)))
+    p = _lib.ptr
+    ba._ck(ba.lib.pvio_b200_track_keypoints(ba.h, prev_id, p(imgs[0]), next_id, p(imgs[1]), w, h, w, p(cur), p(nxt),
+                                            p(status), n, max_level, max_iter, eps, float(clahe_clip), clahe_tiles[0],
+                                            clahe_tiles[1], int(border), float(ransac_threshold),
+                                            float(ransac_confidence)))
     return nxt, status[:n]
 
 
@@ -149,11 +130,8 @@ def pack_pairs(pairs):
         c = cp[i]
         c.slot, c.width, c.height, c.stride = int(d["slot"]), w, h, w
         c.prev_id, c.next_id = int(d["prev_id"]), int(d["next_id"])
-        c.prev = None if imgs[0] is None else _lib._ptr(imgs[0], C.c_uint8)
-        c.next = None if imgs[1] is None else _lib._ptr(imgs[1], C.c_uint8)
         c.n_points = m
-        c.prev_pts, c.next_pts = _lib._ptr(cur, C.c_float), _lib._ptr(nxt, C.c_float)
-        c.status, c.err, c.info = _lib._ptr(status, C.c_uint8), _lib._ptr(err, C.c_float), _lib._ptr(info, C.c_int32)
+        _lib.set_ptrs(c, prev=imgs[0], next=imgs[1], prev_pts=cur, next_pts=nxt, status=status, err=err, info=info)
         keep += [imgs, cur, nxt, status, err, info]
         outs.append((nxt, status[:m], err[:m], info))
     return cp, outs, keep

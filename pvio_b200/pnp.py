@@ -9,13 +9,8 @@ from . import _lib
 
 def imu_record(imu):
     """PreIntegrator outputs (dict as pvio_b200.so3.PreIntegrator.integrate returns) -> [288] record."""
-    rec = np.zeros(_lib.IMU_STRIDE)
-    rec[0] = imu['dt']
-    rec[1:5], rec[5:8], rec[8:11] = imu['dq'], imu['dp'], imu['dv']
-    rec[11:236] = np.asarray(imu['sqrt_inv_cov']).reshape(225)
-    for k, o in (('dq_dbg', 236), ('dp_dbg', 245), ('dp_dba', 254), ('dv_dbg', 263), ('dv_dba', 272)):
-        rec[o:o + 9] = np.asarray(imu[k]).reshape(9)
-    return rec
+    return _lib.imu_records(imu['dt'], imu['dq'], imu['dp'], imu['dv'], imu['sqrt_inv_cov'], imu['dq_dbg'], imu['dp_dbg'],
+                            imu['dp_dba'], imu['dv_dbg'], imu['dv_dba'])[0]
 
 
 def _fill_problem(pb, keep, last_frame, imu, points, z, cam_q, cam_p, imu_q, imu_p, sqrt_inv_cov, use_inertial,
@@ -27,16 +22,11 @@ def _fill_problem(pb, keep, last_frame, imu, points, z, cam_q, cam_p, imu_q, imu
     rec = imu_record(imu) if use_inertial else np.zeros(_lib.IMU_STRIDE)
     keep += [pts, zz, last, rec]
     pb.n_points, pb.use_inertial = len(pts), 1 if use_inertial else 0
-    pb.points, pb.z = _lib._ptr(pts, C.c_double), _lib._ptr(zz, C.c_double)
     pb.cam_q_cs[:], pb.cam_p_cs[:] = list(cam_q), list(cam_p)
     pb.imu_q_cs[:], pb.imu_p_cs[:] = list(imu_q), list(imu_p)
     pb.sqrt_inv_cov[:] = list(np.asarray(sqrt_inv_cov, dtype=np.float64).reshape(4))
     pb.cauchy_a = cauchy_a
-    pb.last_frame, pb.imu_data = _lib._ptr(last, C.c_double), _lib._ptr(rec, C.c_double)
-
-
-def _summary(sm):
-    return {k: getattr(sm, k) for k, _ in _lib.CSummary._fields_}
+    _lib.set_ptrs(pb, points=pts, z=zz, last_frame=last, imu_data=rec)
 
 
 def visual_inertial_pnp(ba, frame, last_frame, imu, points, z, cam_q, cam_p, imu_q, imu_p, sqrt_inv_cov,
@@ -49,8 +39,8 @@ def visual_inertial_pnp(ba, frame, last_frame, imu, points, z, cam_q, cam_p, imu
     out = np.array(frame, dtype=np.float64, copy=True)
     opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
     sm = _lib.CSummary()
-    ba._ck(ba.lib.pvio_b200_pnp_solve(ba.h, C.byref(pb), _lib._ptr(out, C.c_double), C.byref(opt), C.byref(sm)))
-    return out, _summary(sm)
+    ba._ck(ba.lib.pvio_b200_pnp_solve(ba.h, C.byref(pb), _lib.ptr(out), C.byref(opt), C.byref(sm)))
+    return out, _lib.summary(sm)
 
 
 def batch_visual_inertial_pnp(ba, problems, max_iterations=10, initial_radius=0.0):
@@ -67,6 +57,5 @@ def batch_visual_inertial_pnp(ba, problems, max_iterations=10, initial_radius=0.
         frames[i] = d['frame']
     opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
     sms = (_lib.CSummary * max(n, 1))()
-    ba._ck(ba.lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib._ptr(frames, C.c_double), _lib.FRAME_STRIDE,
-                                            C.byref(opt), sms))
-    return frames, [_summary(sms[i]) for i in range(n)]
+    ba._ck(ba.lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib.ptr(frames), _lib.FRAME_STRIDE, C.byref(opt), sms))
+    return frames, [_lib.summary(sms[i]) for i in range(n)]

@@ -13,39 +13,25 @@ class ResidentWindow:
         """ba: a BundleAdjustor (owns the device handle); win: any Window carrying the constants (extrinsics, noise model,
         use_inertial) -- its arrays are not used."""
         self.ba, self.lib, self.h = ba, ba.lib, ba.h
-        L = self.lib
-        i32p, f64p = C.POINTER(C.c_int32), C.POINTER(C.c_double)
-        L.pvio_b200_window_reset.argtypes = [C.c_void_p, C.POINTER(_lib.CWindow)]
-        L.pvio_b200_window_append_frame.argtypes = [C.c_void_p, f64p, C.c_int, f64p]
-        L.pvio_b200_window_add_tracks.argtypes = [C.c_void_p, C.c_int, i32p, f64p, f64p, i32p]
-        L.pvio_b200_window_add_observations.argtypes = [C.c_void_p, C.c_int, i32p, i32p, f64p]
-        L.pvio_b200_window_remove_track.argtypes = [C.c_void_p, C.c_int32]
-        L.pvio_b200_window_set_prior.argtypes = [C.c_void_p, C.c_int, f64p, f64p, f64p]
-        L.pvio_b200_window_solve.argtypes = [C.c_void_p, C.POINTER(_lib.COptions), C.POINTER(_lib.CSummary)]
-        L.pvio_b200_window_drop_victim.argtypes = [C.c_void_p]
-        L.pvio_b200_window_get.argtypes = [C.c_void_p, i32p, f64p, C.c_int, i32p, f64p, i32p, i32p]
-        ba._ck(L.pvio_b200_window_reset(self.h, C.byref(_lib.window_constants(win))))
+        ba._ck(self.lib.pvio_b200_window_reset(self.h, C.byref(_lib.window_constants(win))))
 
     def append_frame(self, state16, fixed=False, imu_record=None):
         s = np.ascontiguousarray(state16, dtype=np.float64)
         rec = None if imu_record is None else np.ascontiguousarray(imu_record, dtype=np.float64)
-        self.ba._ck(self.lib.pvio_b200_window_append_frame(self.h, _lib._ptr(s, C.c_double), 1 if fixed else 0,
-                                                           None if rec is None else _lib._ptr(rec, C.c_double)))
+        self.ba._ck(self.lib.pvio_b200_window_append_frame(self.h, _lib.ptr(s), 1 if fixed else 0, _lib.ptr(rec)))
 
     def add_tracks(self, frames, z, inv_depth):
         n = len(frames)
         f = np.ascontiguousarray(frames, dtype=np.int32); zz = np.ascontiguousarray(z, dtype=np.float64).reshape(-1, 2)
         r = np.ascontiguousarray(inv_depth, dtype=np.float64); ids = np.zeros(max(n, 1), dtype=np.int32)
-        self.ba._ck(self.lib.pvio_b200_window_add_tracks(self.h, n, _lib._ptr(f, C.c_int32), _lib._ptr(zz, C.c_double),
-                                                         _lib._ptr(r, C.c_double), _lib._ptr(ids, C.c_int32)))
+        self.ba._ck(self.lib.pvio_b200_window_add_tracks(self.h, n, _lib.ptr(f), _lib.ptr(zz), _lib.ptr(r), _lib.ptr(ids)))
         return ids[:n]
 
     def add_observations(self, tracks, frames, z):
         n = len(tracks)
         t = np.ascontiguousarray(tracks, dtype=np.int32); f = np.ascontiguousarray(frames, dtype=np.int32)
         zz = np.ascontiguousarray(z, dtype=np.float64).reshape(-1, 2)
-        self.ba._ck(self.lib.pvio_b200_window_add_observations(self.h, n, _lib._ptr(t, C.c_int32), _lib._ptr(f, C.c_int32),
-                                                               _lib._ptr(zz, C.c_double)))
+        self.ba._ck(self.lib.pvio_b200_window_add_observations(self.h, n, _lib.ptr(t), _lib.ptr(f), _lib.ptr(zz)))
 
     def remove_track(self, track):
         self.ba._ck(self.lib.pvio_b200_window_remove_track(self.h, int(track)))
@@ -53,14 +39,13 @@ class ResidentWindow:
     def set_prior(self, S, e, state0):
         S = np.ascontiguousarray(S, dtype=np.float64); e = np.ascontiguousarray(e, dtype=np.float64)
         x0 = np.ascontiguousarray(state0, dtype=np.float64).reshape(-1, 16)
-        self.ba._ck(self.lib.pvio_b200_window_set_prior(self.h, len(x0), _lib._ptr(S, C.c_double), _lib._ptr(e, C.c_double),
-                                                        _lib._ptr(x0, C.c_double)))
+        self.ba._ck(self.lib.pvio_b200_window_set_prior(self.h, len(x0), _lib.ptr(S), _lib.ptr(e), _lib.ptr(x0)))
 
     def solve(self, max_iterations=10, max_time=1e6, alias_bias=True):
         opt = _lib.COptions(max_iterations, max_time, 1 if alias_bias else 0, 0, 0.0)
         sm = _lib.CSummary()
         self.ba._ck(self.lib.pvio_b200_window_solve(self.h, C.byref(opt), C.byref(sm)))
-        return {k: getattr(sm, k) for k, _ in _lib.CSummary._fields_}
+        return _lib.summary(sm)
 
     def drop_victim(self):
         self.ba._ck(self.lib.pvio_b200_window_drop_victim(self.h))
@@ -72,7 +57,6 @@ class ResidentWindow:
         fr = np.zeros((max(n.value, 1), 16))
         t = np.ascontiguousarray(tracks, dtype=np.int32)
         rho = np.zeros(max(len(t), 1)); an = np.zeros(max(len(t), 1), dtype=np.int32); cnt = np.zeros(max(len(t), 1), dtype=np.int32)
-        self.ba._ck(self.lib.pvio_b200_window_get(self.h, C.byref(n), _lib._ptr(fr, C.c_double), len(t),
-                                                  _lib._ptr(t, C.c_int32) if len(t) else None, _lib._ptr(rho, C.c_double),
-                                                  _lib._ptr(an, C.c_int32), _lib._ptr(cnt, C.c_int32)))
+        self.ba._ck(self.lib.pvio_b200_window_get(self.h, C.byref(n), _lib.ptr(fr), len(t), _lib.ptr(t) if len(t) else None,
+                                                  _lib.ptr(rho), _lib.ptr(an), _lib.ptr(cnt)))
         return fr[:n.value], rho[:len(t)], an[:len(t)], cnt[:len(t)]

@@ -1,6 +1,4 @@
 """Host-side mirror of Track::triangulate (pvio/src/pvio/map/track.cpp:83-106) over the C ABI: a batch of tracks."""
-import ctypes as C
-
 import numpy as np
 
 from . import _lib
@@ -15,9 +13,6 @@ def triangulate(ba, P, begin, obs_frame, obs_z):
     z = np.ascontiguousarray(obs_z, dtype=np.float64).reshape(-1, 2)
     n = len(begin) - 1
     pts, valid, score = np.zeros((n, 3)), np.zeros(n, dtype=np.uint8), np.zeros(n)
-    fn = ba.lib.pvio_b200_triangulate
-    fn.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
-                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_uint8), C.POINTER(C.c_double)]
-    ba._ck(fn(ba.h, len(P), _lib._ptr(P, C.c_double), n, _lib._ptr(begin, C.c_int32), _lib._ptr(fr, C.c_int32),
-              _lib._ptr(z, C.c_double), _lib._ptr(pts, C.c_double), _lib._ptr(valid, C.c_uint8), _lib._ptr(score, C.c_double)))
+    ba._ck(ba.lib.pvio_b200_triangulate(ba.h, len(P), _lib.ptr(P), n, _lib.ptr(begin), _lib.ptr(fr), _lib.ptr(z),
+                                        _lib.ptr(pts), _lib.ptr(valid), _lib.ptr(score)))
     return pts, valid.astype(bool), score

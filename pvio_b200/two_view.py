@@ -1,18 +1,17 @@
 """Host mirror of the two-view step of Initializer::init_sfm (pvio/src/pvio/core/initializer.cpp:102-161) over the
 C-ABI (pvio_b200_batch_two_view): both RANSACs, both decompositions and the scored choice of pose on the device."""
-import ctypes as C
-
 import numpy as np
 
 from . import _lib
 
-STATUS = ("ok", "few_matches", "low_parallax", "pure_rotation", "few_triangulated")
+STATUS = {_lib.TWO_VIEW_OK: "ok", _lib.TWO_VIEW_FEW_MATCHES: "few_matches", _lib.TWO_VIEW_LOW_PARALLAX: "low_parallax",
+          _lib.TWO_VIEW_PURE_ROTATION: "pure_rotation", _lib.TWO_VIEW_FEW_TRIANGULATED: "few_triangulated"}
 
 
 def batch_two_view(ba, problems, diagnostics=False):
     """problems: dicts with p1, p2 ([n][2] normalised keypoints of frames i and j), fx, fy, and optional min_matches
     (50), min_parallax (10), min_triangulation (20), seed (648), confidence (0.999), max_iteration (1000).
-    Returns one dict per problem: status (an index into STATUS), parallax, H, E, h_inliers, h_iterations, h_best_it,
+    Returns one dict per problem: status (a key of STATUS), parallax, H, E, h_inliers, h_iterations, h_best_it,
     e_inliers, e_iterations, e_best_it, e_best_model, candidate, triangulated, R, T, h_mask, e_mask, points,
     point_status; with diagnostics also h_schedule, e_schedule, h_counts, e_counts."""
     n = len(problems)
@@ -29,13 +28,11 @@ def batch_two_view(ba, problems, diagnostics=False):
                      h_counts=np.zeros(it, np.int32), e_counts=np.zeros((it, 11), np.int32))
         r = recs[i]
         r.n_matches, r.seed = m, int(d.get("seed", 648))
-        r.p1, r.p2 = _lib._ptr(p1, C.c_double), _lib._ptr(p2, C.c_double)
         r.fx, r.fy = float(d["fx"]), float(d["fy"])
         r.min_matches, r.min_triangulation = int(d.get("min_matches", 50)), int(d.get("min_triangulation", 20))
         r.min_parallax, r.confidence = float(d.get("min_parallax", 10.0)), float(d.get("confidence", 0.999))
         r.max_iteration = it
-        for k, a in o.items():
-            setattr(r, k, a.ctypes.data_as(type(getattr(r, k))))
+        _lib.set_ptrs(r, p1=p1, p2=p2, **o)
         keep += [p1, p2]
         outs.append(o)
     ba._ck(ba.lib.pvio_b200_batch_two_view(ba.h, n, recs))

@@ -3,13 +3,11 @@
 (pvio-extra/include/pvio/extra/image_undistorter.h:28-95), bit for bit.  A lens is set once per sequence slot of the
 batched tracker; the batched tracker and detector then take that slot's raw frames (klt.batch_track_keypoints and
 detect.batch_detect_keypoints are unchanged)."""
-import ctypes as C
-
 import numpy as np
 
 from . import _lib
 
-NONE, RADTAN, EQUIDISTANT = 0, 1, 2
+NONE, RADTAN, EQUIDISTANT = 0, _lib.LENS_RADTAN, _lib.LENS_EQUIDISTANT
 
 
 def undistort_map(model, width, height, K, coeffs):
@@ -21,8 +19,8 @@ def undistort_map(model, width, height, K, coeffs):
     c = np.ascontiguousarray(coeffs, dtype=np.float64).reshape(4)
     m1 = np.zeros((height, width, 2), np.int16)
     m2 = np.zeros((height, width), np.uint16)
-    rc = lib.pvio_b200_undistort_map(int(model), int(width), int(height), _lib._ptr(p, C.c_double),
-                                     _lib._ptr(c, C.c_double), _lib._ptr(m1, C.c_int16), _lib._ptr(m2, C.c_uint16))
+    rc = lib.pvio_b200_undistort_map(int(model), int(width), int(height), _lib.ptr(p), _lib.ptr(c), _lib.ptr(m1),
+                                     _lib.ptr(m2))
     if rc != 0:
         raise ValueError(f"pvio_b200_undistort_map rejected the lens ({rc})")
     return m1, m2
@@ -59,7 +57,7 @@ def batch_undistort(ba, requests):
         out = np.zeros((h, w), np.uint8)
         r = arr[i]
         r.slot, r.width, r.height, r.stride = int(d["slot"]), w, h, w
-        r.src, r.dst = _lib._ptr(img, C.c_uint8), _lib._ptr(out, C.c_uint8)
+        _lib.set_ptrs(r, src=img, dst=out)
         keep.append(img)
         outs.append(out)
     ba._ck(ba.lib.pvio_b200_batch_undistort(ba.h, n, arr))

@@ -102,16 +102,13 @@ def test_golden_vectors():
 def test_library_sample_schedule_equals_the_oracle():
     """Host side of pvio_b200_find_fundamental_mask (no GPU): the subsets the library draws are the oracle's, i.e. OpenCV's
     (the oracle's RANSAC masks equal cv2's iteration for iteration only if the schedule does)."""
-    import ctypes as C
     from pvio_b200 import _lib
     lib = _lib.load()
     fn = lib.pvio_b200_fm_sample_schedule
-    fn.argtypes = [C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int32)]
-    fn.restype = C.c_int
     for seed, n in [(1, 15), (2, 60), (3, 400), (4, 9)]:
         p, q = synth.make_fm_matches(seed, n, 0.2)
         out = np.zeros((300, 7), dtype=np.int32)
-        got = fn(n, _lib._ptr(p, C.c_float), _lib._ptr(q, C.c_float), 300, _lib._ptr(out, C.c_int32))
+        got = fn(n, _lib.ptr(p), _lib.ptr(q), 300, _lib.ptr(out))
         assert got == 300
         assert np.array_equal(out, fo.sample_schedule(p, q, 300, 10000 if n >= 15 else 1000))
-    assert fn(5, _lib._ptr(p, C.c_float), _lib._ptr(q, C.c_float), 10, _lib._ptr(out, C.c_int32)) < 0
+    assert fn(5, _lib.ptr(p), _lib.ptr(q), 10, _lib.ptr(out)) < 0

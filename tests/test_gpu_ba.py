@@ -8,6 +8,7 @@ import pytest
 
 from oracle import ba_oracle as bo
 from synthetic import synth
+from pvio_b200._lib import TERM_FAILURE
 from pvio_b200.bundle_adjustor import BundleAdjustor
 
 pytestmark = pytest.mark.gpu
@@ -604,7 +605,7 @@ def test_failed_linear_solve_is_retried_with_larger_mu_and_ends_in_failure(ba):
         wb.obs_z = wb.obs_z.copy()
         wb.obs_z[3, 0] = np.nan
         out, summ = ba.solve(wb, st, max_iterations=10, postpass=False)     # 9 retries (1e-8 -> 10) fit into 10 + 2 bodies
-        assert summ['termination'] == 2 and summ['usable'] == 0 and summ['accepted_steps'] == 0      # PVIO_B200_TERM_FAILURE
+        assert summ['termination'] == TERM_FAILURE and summ['usable'] == 0 and summ['accepted_steps'] == 0
         assert summ['final_mu'] > 1.0
         assert np.array_equal(out.p, st.p) and np.array_equal(out.q, st.q) and np.array_equal(out.rho, st.rho)
         # the handle is intact: the healthy window solves as before

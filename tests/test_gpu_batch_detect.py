@@ -9,9 +9,9 @@ import pytest
 
 from pvio_b200 import _lib, klt
 from pvio_b200.detect import batch_detect_keypoints, detect_keypoints, pack_requests
+from pvio_b200._lib import EINVAL
 from synthetic import synth
 
-EINVAL = -2
 
 
 def test_detect_request_layout_matches_header():
@@ -251,9 +251,9 @@ def test_rejected_calls_change_nothing():
         assert outs[1][1][0] == len(full[1]) and np.array_equal(outs[1][0][:len(full[1])], full[1])
         n = C.c_int()
         out = np.zeros((5, 2))
-        rc = b.lib.pvio_b200_detect_keypoints(b.h, 0, _lib._ptr(np.ascontiguousarray(B), C.c_uint8), B.shape[1], B.shape[0],
-                                              B.shape[1], C.c_double(6.0), 8, 8, _lib._ptr(np.ascontiguousarray(pts[::4], dtype=np.float64), C.c_double),
-                                              len(pts[::4]), C.c_double(25.0), 5, _lib._ptr(out, C.c_double), C.byref(n), None, None)
+        rc = b.lib.pvio_b200_detect_keypoints(b.h, 0, _lib.ptr(np.ascontiguousarray(B)), B.shape[1], B.shape[0],
+                                              B.shape[1], 6.0, 8, 8, _lib.ptr(np.ascontiguousarray(pts[::4], dtype=np.float64)),
+                                              len(pts[::4]), 25.0, 5, _lib.ptr(out), C.byref(n), None, None)
         assert rc == EINVAL and n.value == len(full[0]) and np.array_equal(out, full[0][:5])
         del keep
     finally:

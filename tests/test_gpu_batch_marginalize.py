@@ -9,12 +9,13 @@ import pytest
 from oracle import ba_oracle as bo
 from synthetic import synth
 from synthetic.sequence import Run, Chain
+from pvio_b200 import _lib
 from pvio_b200.bundle_adjustor import BundleAdjustor, PvioB200Error
 from pvio_b200.window import State
 
 pytestmark = pytest.mark.gpu
 
-EINVAL = r"error -2\b"
+EINVAL = rf"error {_lib.EINVAL}\b"
 
 
 def _rel(a, b):

@@ -10,10 +10,10 @@ from oracle import pnp_oracle as po
 from synthetic import synth
 from pvio_b200 import _lib, pnp
 from pvio_b200.bundle_adjustor import BundleAdjustor
+from pvio_b200._lib import EINVAL
 
 pytestmark = pytest.mark.gpu
 
-EINVAL = -2
 COST_TOL, STATE_TOL = 1e-9, 1e-8      # the bars of test_gpu_pnp.py
 
 
@@ -152,7 +152,7 @@ def test_rejections_leave_everything_untouched(ba, spoil):
     frames = np.full((7, 16), 12345.0)
     sms = (_lib.CSummary * 7)()
     opt = _lib.COptions(10, 1e6, 1, 0, 0.0)
-    rc = ba.lib.pvio_b200_batch_pnp_solve(ba.h, 7, pbs, _lib._ptr(frames, C.c_double), stride, C.byref(opt), sms)
+    rc = ba.lib.pvio_b200_batch_pnp_solve(ba.h, 7, pbs, _lib.ptr(frames), stride, C.byref(opt), sms)
     assert rc == EINVAL
     assert np.all(frames == 12345.0)
     assert all(sms[i].iterations == 0 for i in range(7))
@@ -176,7 +176,7 @@ def test_buffer_growth_strided_frames_no_summaries():
         for i, d in enumerate(large):
             frames[i, :16] = d['frame']
         opt = _lib.COptions(10, 1e6, 1, 0, 0.0)
-        rc = b.lib.pvio_b200_batch_pnp_solve(b.h, len(large), pbs, _lib._ptr(frames, C.c_double), stride,
+        rc = b.lib.pvio_b200_batch_pnp_solve(b.h, len(large), pbs, _lib.ptr(frames), stride,
                                              C.byref(opt), None)
         assert rc == 0
         assert np.all(frames[:, 16:] == -7.0)                       # the padding of each row is not touched

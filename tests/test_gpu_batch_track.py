@@ -8,9 +8,9 @@ import numpy as np
 import pytest
 
 from pvio_b200 import _lib, klt
+from pvio_b200._lib import EINVAL
 from synthetic import synth
 
-EINVAL = -2
 METHOD = {None: 0, "ransac": 1, "lmeds": 2, "7point": 3}
 
 

@@ -5,6 +5,7 @@ import dataclasses
 import numpy as np
 import pytest
 
+from pvio_b200 import _lib
 from pvio_b200.batch_window import BatchWindows, Edit
 from pvio_b200.bundle_adjustor import BundleAdjustor, PvioB200Error
 from pvio_b200.window import State
@@ -12,7 +13,7 @@ from synthetic import synth
 from synthetic.sequence import BatchPlayer, Chain, Run
 
 pytestmark = pytest.mark.gpu
-EINVAL = "error -2"
+EINVAL = f"error {_lib.EINVAL}"
 
 
 def _feed_window(bw, slot, w, st):
@@ -205,7 +206,7 @@ def _solve_with_flags(one, w, st):
     valid = np.zeros(max(w.M, 1), dtype=np.uint8)
     quality = np.zeros(max(w.M, 1))
     one._ck(one.lib.pvio_b200_ba_solve(one.h, C.byref(pa.cw), C.byref(pa.cs), C.byref(opt), C.byref(sm),
-                                       _lib._ptr(valid, C.c_uint8), _lib._ptr(quality, C.c_double)))
+                                       _lib.ptr(valid), _lib.ptr(quality)))
     return None, sm, valid[:w.M], quality[:w.M]
 
 

@@ -11,11 +11,11 @@ from oracle import imu_oracle
 from pvio_b200 import _lib, imu
 from pvio_b200.batch_window import BatchWindows, Imu
 from pvio_b200.bundle_adjustor import BundleAdjustor, PvioB200Error
+from pvio_b200._lib import EINVAL
 from synthetic import synth
 from synthetic.sequence import BatchPlayer, Chain, Run
 
 pytestmark = pytest.mark.gpu
-EINVAL = -2
 SEQ_TOL = 2e-6
 
 
@@ -210,7 +210,6 @@ def test_samples_follow_drops_replacements_and_growth():
     # window_solve on slot 0
     sm = _lib.CSummary()
     opt = _lib.COptions(3, 1e6, 1, 0, 0.0)
-    ba.lib.pvio_b200_window_solve.argtypes = [C.c_void_p, C.POINTER(_lib.COptions), C.POINTER(_lib.CSummary)]
     check([0], lambda: ba._ck(ba.lib.pvio_b200_window_solve(ba.h, C.byref(opt), C.byref(sm))))
     # slot 2: a non-keyframe with samples, replaced by a frame without a set_imu: the replaced samples leave, the new
     # factor keeps its edit record
@@ -303,8 +302,8 @@ def test_rejections_change_nothing():
         keep.extend([s, nz])
         r = _lib.CWindowImu()
         r.slot, r.frame, r.n_samples, r.t_end = slot, frame, len(s) if n is None else n, t_end if spoil != "t_end" else np.inf
-        r.samples = _lib._ptr(s, C.c_double) if samples else None
-        r.noise_cov = _lib._ptr(nz, C.c_double) if noise else None
+        r.samples = _lib.ptr(s) if samples else None
+        r.noise_cov = _lib.ptr(nz) if noise else None
         return r
 
     def arr(*rs):

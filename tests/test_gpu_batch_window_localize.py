@@ -13,11 +13,11 @@ from pvio_b200 import _lib, triangulate
 from pvio_b200.pnp import imu_record
 from pvio_b200.batch_window import Edit, Localize
 from pvio_b200.bundle_adjustor import BundleAdjustor, PvioB200Error
+from pvio_b200._lib import EINVAL
 from synthetic import so3
 from synthetic.sequence import BatchPlayer, Run
 
 pytestmark = pytest.mark.gpu
-EINVAL = -2
 COST_TOL, STATE_TOL = 1e-9, 1e-8          # the bars of test_gpu_pnp.py
 SEQ_TOL = 2e-6                            # the bar of the resident sequence tests
 
@@ -90,17 +90,17 @@ def _host_pnp(ba, problems, max_iterations=10):
         rec = L.imu if L.imu is not None else np.zeros(_lib.IMU_STRIDE)
         keep += [x, z, lf, rec]
         pb.n_points, pb.use_inertial = len(x), 0 if L.imu is None else 1
-        pb.points, pb.z = _lib._ptr(x, C.c_double), _lib._ptr(z, C.c_double)
+        pb.points, pb.z = _lib.ptr(x), _lib.ptr(z)
         pb.cam_q_cs[:], pb.cam_p_cs[:] = list(w.cam_q_cs), list(w.cam_p_cs)
         pb.imu_q_cs[:], pb.imu_p_cs[:] = list(w.imu_q_cs), list(w.imu_p_cs)
         pb.sqrt_inv_cov[:] = list(np.asarray(w.sqrt_inv_cov, dtype=np.float64).reshape(4))
         pb.cauchy_a = w.cauchy_a
-        pb.last_frame, pb.imu_data = _lib._ptr(lf, C.c_double), _lib._ptr(rec, C.c_double)
+        pb.last_frame, pb.imu_data = _lib.ptr(lf), _lib.ptr(rec)
         frames[i] = L.state
     opt = _lib.COptions(max_iterations, 1e6, 1, 0, 0.0)
     sms = (_lib.CSummary * n)()
-    ba._ck(ba.lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib._ptr(frames, C.c_double), 16, C.byref(opt), sms))
-    return frames, [{k: getattr(sms[i], k) for k, _ in _lib.CSummary._fields_} for i in range(n)]
+    ba._ck(ba.lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib.ptr(frames), 16, C.byref(opt), sms))
+    return frames, [_lib.summary(sms[i]) for i in range(n)]
 
 
 def _cam_matrix(run, x16):
@@ -317,13 +317,13 @@ def _spoil_dead(recs, keep, player):
     t = np.ctypeslib.as_array(recs[1].obs_track, shape=(recs[1].n_obs,)).copy()
     t[0] = player.dead[1][0]                              # a removed track of the slot
     keep.append(t)
-    recs[1].obs_track = _lib._ptr(t, C.c_int32)
+    recs[1].obs_track = _lib.ptr(t)
 
 
 def _spoil_unknown(recs, keep, player):
     t = np.array([10 ** 6], dtype=np.int32)
     keep.append(t)
-    recs[1].obs_track = _lib._ptr(t, C.c_int32)
+    recs[1].obs_track = _lib.ptr(t)
     recs[1].n_obs = 1
 
 
@@ -331,21 +331,21 @@ def _spoil_track_twice(recs, keep, player):
     t = np.ctypeslib.as_array(recs[1].obs_track, shape=(recs[1].n_obs,)).copy()
     t[3] = t[2]
     keep.append(t)
-    recs[1].obs_track = _lib._ptr(t, C.c_int32)
+    recs[1].obs_track = _lib.ptr(t)
 
 
 def _spoil_z(recs, keep, player):
     z = np.ctypeslib.as_array(recs[1].obs_z, shape=(recs[1].n_obs, 2)).copy()
     z[4, 1] = np.inf
     keep.append(z)
-    recs[1].obs_z = _lib._ptr(z, C.c_double)
+    recs[1].obs_z = _lib.ptr(z)
 
 
 def _spoil_new_z(recs, keep, player):
     z = np.ctypeslib.as_array(recs[0].new_z, shape=(recs[0].n_new, 2)).copy()
     z[0, 0] = np.nan
     keep.append(z)
-    recs[0].new_z = _lib._ptr(z, C.c_double)
+    recs[0].new_z = _lib.ptr(z)
 
 
 def _spoil_null(recs, keep, player):
@@ -363,7 +363,7 @@ def _spoil_imu(recs, keep, player):
 def _spoil_plane_point(recs, keep, player):
     x = np.full((recs[1].n_obs, 3), np.nan)               # the plane run without its plane-cast points
     keep.append(x)
-    recs[1].obs_point = _lib._ptr(x, C.c_double)
+    recs[1].obs_point = _lib.ptr(x)
 
 
 SPOILERS = [_spoil_slot, _spoil_not_resident, _spoil_no_frames, _spoil_twice, _spoil_dead, _spoil_unknown,
@@ -390,13 +390,13 @@ def test_rejections_change_no_output(setup, spoil):
         sm = _lib.CSummary()
         sm.iterations = 777
         o["sm"] = sm
-        r.slot, r.use_inertial, r.imu_record = L.slot, 1, _lib._ptr(L.imu, C.c_double)
-        r.state = _lib._ptr(o["state"], C.c_double)
-        r.n_obs, r.obs_track, r.obs_z, r.obs_point = len(t), _lib._ptr(t, C.c_int32), _lib._ptr(z, C.c_double), _lib._ptr(x, C.c_double)
-        r.points_out = _lib._ptr(o["points"], C.c_double)
-        r.n_new, r.new_z_last, r.new_z = len(zl), _lib._ptr(zl, C.c_double), _lib._ptr(zn, C.c_double)
-        r.new_valid, r.new_inv_depth = _lib._ptr(o["valid"], C.c_uint8), _lib._ptr(o["rho"], C.c_double)
-        r.new_inv_depth_next, r.summary = _lib._ptr(o["nxt"], C.c_double), C.pointer(sm)
+        r.slot, r.use_inertial, r.imu_record = L.slot, 1, _lib.ptr(L.imu)
+        r.state = _lib.ptr(o["state"])
+        r.n_obs, r.obs_track, r.obs_z, r.obs_point = len(t), _lib.ptr(t), _lib.ptr(z), _lib.ptr(x)
+        r.points_out = _lib.ptr(o["points"])
+        r.n_new, r.new_z_last, r.new_z = len(zl), _lib.ptr(zl), _lib.ptr(zn)
+        r.new_valid, r.new_inv_depth = _lib.ptr(o["valid"]), _lib.ptr(o["rho"])
+        r.new_inv_depth_next, r.summary = _lib.ptr(o["nxt"]), C.pointer(sm)
     assert recs[0].n_new > 0 and recs[1].n_obs > 5
     spoil(recs, keep, player)
     before = _downloads(player.bw, [0, 1, 2, 3, 5], 400)

@@ -15,7 +15,7 @@ from synthetic import synth
 from synthetic.sequence import BatchPlayer, Chain, Run
 
 pytestmark = pytest.mark.gpu
-EINVAL = "error -2"
+EINVAL = f"error {_lib.EINVAL}"
 SUMMARY_KEYS = ("iterations", "accepted_steps", "termination", "initial_cost", "final_cost", "final_radius", "final_mu")
 
 

@@ -2,8 +2,6 @@
 the new frame's samples, predict its state, PnP + triangulation as localize, the keyframe check, and the merged record
 after a non-keyframe -- with the slot's newest frame as map->last_frame().  Checked against pvio_b200_preintegrate,
 tracker_oracle.predict, localize and tracker_oracle.keyframe_check, and along whole sequences against a host twin."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -11,11 +9,11 @@ from oracle import lie, tracker_oracle
 from pvio_b200 import _lib, imu
 from pvio_b200.batch_window import BatchWindows, Edit, Localize, TrackFrame
 from pvio_b200.bundle_adjustor import BundleAdjustor, PvioB200Error
+from pvio_b200._lib import EINVAL
 from synthetic.sequence import BatchPlayer, Run
 from test_gpu_batch_window_localize import _downloads, _given_point, _near_threshold, _cam_matrix, _same_download
 
 pytestmark = pytest.mark.gpu
-EINVAL = -2
 SEQ_TOL = 2e-6
 CX, CY = 376.0, 240.0
 
@@ -250,10 +248,10 @@ def test_no_slot_changes(setup):
     assert all(np.array_equal(_bits(a), _bits(b)) for a, b in zip(imu_before, p.bw.imu_records([0, 1, 2, 3])))
 
 
-def _arr(keep, a, t):
+def _arr(keep, a):
     a = np.ascontiguousarray(a)
     keep.append(a)
-    return _lib._ptr(a, t)
+    return _lib.ptr(a)
 
 
 def _sp_visual(r, keep):
@@ -267,7 +265,7 @@ def _sp_no_samples(r, keep):
 def _sp_sample(r, keep):
     s = np.ctypeslib.as_array(r.samples, shape=(r.n_samples, 7)).copy()
     s[3, 4] = np.nan
-    r.samples = _arr(keep, s, C.c_double)
+    r.samples = _arr(keep, s)
 
 
 def _sp_t_end(r, keep):
@@ -277,7 +275,7 @@ def _sp_t_end(r, keep):
 def _sp_noise(r, keep):
     n = np.ctypeslib.as_array(r.noise_cov, shape=(36,)).copy()
     n[30] = np.nan
-    r.noise_cov = _arr(keep, n, C.c_double)
+    r.noise_cov = _arr(keep, n)
 
 
 def _sp_cx(r, keep):
@@ -301,13 +299,13 @@ def _sp_skipped_null(r, keep):
 
 
 def _sp_skipped_negative(r, keep):
-    r.skipped_frames = _arr(keep, np.array([-1], dtype=np.int32), C.c_int32)
+    r.skipped_frames = _arr(keep, np.array([-1], dtype=np.int32))
 
 
 def _sp_unknown_track(r, keep):
     t = np.ctypeslib.as_array(r.obs_track, shape=(r.n_obs,)).copy()
     t[0] = 10 ** 6
-    r.obs_track = _arr(keep, t, C.c_int32)
+    r.obs_track = _arr(keep, t)
 
 
 def _sp_record_null(r, keep):

@@ -19,7 +19,6 @@ from test_klt_oracle_edges import PARAMS, SIZES, assert_lk_parity, cv_lk, edge_c
 
 pytestmark = pytest.mark.gpu
 PAD = 13                                    # the padded frames' row stride is width + PAD; the padding holds 0xAB
-U8, F32 = C.POINTER(C.c_uint8), C.POINTER(C.c_float)
 
 
 @pytest.fixture(scope="module")
@@ -36,8 +35,7 @@ def _padded(img):
     return buf
 
 
-def _p(a, t=C.c_uint8):
-    return None if a is None else a.ctypes.data_as(C.POINTER(t))
+_p = _lib.ptr
 
 
 # ---- LK at the edges --------------------------------------------------------------------------------------------
@@ -54,10 +52,10 @@ def test_edge_points_match_cv2_and_oracle(ba, size):
 def test_frames_under_twelve_pixels_are_rejected(ba):
     """Below 12 px the window's reads would fold more than twice: such frames are refused, unlike cv2, which tracks them."""
     prev, nxt, pts, init, _ = edge_case((12, 12))
-    rc = ba.lib.pvio_b200_klt_track(ba.h, _p(prev[:, :11].copy()), _p(nxt[:, :11].copy()), 11, 12, 11, _p(pts, C.c_float),
-                                    _p(init.copy(), C.c_float), _p(np.zeros(len(pts), np.uint8)),
-                                    _p(np.zeros(len(pts), np.float32), C.c_float), len(pts), 3, 30, C.c_double(0.01))
-    assert rc == -2
+    rc = ba.lib.pvio_b200_klt_track(ba.h, _p(prev[:, :11].copy()), _p(nxt[:, :11].copy()), 11, 12, 11, _p(pts),
+                                    _p(init.copy()), _p(np.zeros(len(pts), np.uint8)),
+                                    _p(np.zeros(len(pts), np.float32)), len(pts), 3, 30, 0.01)
+    assert rc == _lib.EINVAL
 
 
 @pytest.mark.parametrize("name,value", PARAMS, ids=[f"{n}={v}" for n, v in PARAMS])
@@ -80,11 +78,8 @@ def _track_raw(ba, prev, nxt, pts, clip, tiles, stride=None):
     out = cur.copy()
     st, err = np.zeros(len(cur), np.uint8), np.zeros(len(cur), np.float32)
     eq = [np.zeros((h, w), np.uint8) for _ in range(2)]
-    fn = ba.lib.pvio_b200_klt_track_raw
-    fn.argtypes = [C.c_void_p, U8, U8, C.c_int, C.c_int, C.c_int, F32, F32, U8, F32, C.c_int, C.c_int, C.c_int, C.c_double,
-                   C.c_double, C.c_int, C.c_int, U8, U8]
-    ba._ck(fn(ba.h, _p(prev), _p(nxt), w, h, stride or w, _p(cur, C.c_float), _p(out, C.c_float), _p(st), _p(err, C.c_float),
-              len(cur), 3, 30, 0.01, float(clip), tiles[0], tiles[1], _p(eq[0]), _p(eq[1])))
+    ba._ck(ba.lib.pvio_b200_klt_track_raw(ba.h, _p(prev), _p(nxt), w, h, stride or w, _p(cur), _p(out), _p(st), _p(err),
+                                          len(cur), 3, 30, 0.01, float(clip), tiles[0], tiles[1], _p(eq[0]), _p(eq[1])))
     return out, st, err, eq[0], eq[1]
 
 
@@ -131,27 +126,19 @@ def test_every_strided_entry_point_equals_the_contiguous_call(ba):
     def lk(stride, name):
         a, b = (pp, pn) if stride else (prev, nxt)
         out, st, err = init.copy(), np.zeros(n, np.uint8), np.zeros(n, np.float32)
-        args = (_p(pts, C.c_float), _p(out, C.c_float), _p(st), _p(err, C.c_float), n, 3, 30, 0.01)
+        args = (_p(pts), _p(out), _p(st), _p(err), n, 3, 30, 0.01)
         s = stride or w
         ids = (11, 12) if stride else (21, 22)          # distinct ids: the strided call must not hit the cache
         if name == "klt_track":
-            fn = ba.lib.pvio_b200_klt_track
-            fn.argtypes = [C.c_void_p, U8, U8, C.c_int, C.c_int, C.c_int, F32, F32, U8, F32, C.c_int, C.c_int, C.c_int,
-                           C.c_double]
-            ba._ck(fn(ba.h, _p(a), _p(b), w, h, s, *args))
+            ba._ck(ba.lib.pvio_b200_klt_track(ba.h, _p(a), _p(b), w, h, s, *args))
             return out, st, err
         if name == "klt_track_cached":
-            fn = ba.lib.pvio_b200_klt_track_cached
-            fn.argtypes = [C.c_void_p, C.c_uint64, U8, C.c_uint64, U8, C.c_int, C.c_int, C.c_int, F32, F32, U8, F32, C.c_int,
-                           C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int]
-            ba._ck(fn(ba.h, ids[0], _p(a), ids[1], _p(b), w, h, s, *args, 6.0, 8, 8, 20))
+            ba._ck(ba.lib.pvio_b200_klt_track_cached(ba.h, ids[0], _p(a), ids[1], _p(b), w, h, s, *args, 6.0, 8, 8,
+                                                     20))
             return out, st, err
         assert name == "track_keypoints"
-        fn = ba.lib.pvio_b200_track_keypoints
-        fn.argtypes = [C.c_void_p, C.c_uint64, U8, C.c_uint64, U8, C.c_int, C.c_int, C.c_int, F32, F32, U8, C.c_int, C.c_int,
-                       C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
-        ba._ck(fn(ba.h, ids[0] + 100, _p(a), ids[1] + 100, _p(b), w, h, s, _p(pts, C.c_float), _p(out, C.c_float), _p(st), n,
-                  3, 30, 0.01, 6.0, 8, 8, 20, 1.0, 0.99))
+        ba._ck(ba.lib.pvio_b200_track_keypoints(ba.h, ids[0] + 100, _p(a), ids[1] + 100, _p(b), w, h, s, _p(pts), _p(out),
+                                                _p(st), n, 3, 30, 0.01, 6.0, 8, 8, 20, 1.0, 0.99))
         return out, st
 
     for name in ("klt_track", "klt_track_cached", "track_keypoints"):
@@ -162,20 +149,15 @@ def test_every_strided_entry_point_equals_the_contiguous_call(ba):
     assert all(np.array_equal(x, y) for x, y in zip(want, got)), "klt_track_raw"
 
     out = np.zeros_like(prev)
-    fn = ba.lib.pvio_b200_clahe
-    fn.argtypes = [C.c_void_p, U8, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, U8]
-    ba._ck(fn(ba.h, _p(pp), w, h, w + PAD, 6.0, 8, 8, _p(out)))
+    ba._ck(ba.lib.pvio_b200_clahe(ba.h, _p(pp), w, h, w + PAD, 6.0, 8, 8, _p(out)))
     assert np.array_equal(out, klt.clahe(ba, prev)), "clahe"
 
     existing = np.ascontiguousarray(pts[::3], np.float64)
     kp = np.zeros((2048, 2))
     gftt = np.zeros((1000, 2), np.float32)
     n_out, n_g = C.c_int(), C.c_int()
-    fn = ba.lib.pvio_b200_detect_keypoints
-    fn.argtypes = [C.c_void_p, C.c_uint64, U8, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_double),
-                   C.c_int, C.c_double, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int), F32, C.POINTER(C.c_int)]
-    ba._ck(fn(ba.h, 0, _p(pn), w, h, w + PAD, 6.0, 8, 8, _p(existing, C.c_double), len(existing), 25.0, 2048,
-              _p(kp, C.c_double), C.byref(n_out), _p(gftt, C.c_float), C.byref(n_g)))
+    ba._ck(ba.lib.pvio_b200_detect_keypoints(ba.h, 0, _p(pn), w, h, w + PAD, 6.0, 8, 8, _p(existing), len(existing), 25.0,
+                                             2048, _p(kp), C.byref(n_out), _p(gftt), C.byref(n_g)))
     want_kp, want_g = detect_keypoints(ba, nxt, existing, keypoint_distance=25.0, clahe_clip=6.0, want_gftt=True)
     assert np.array_equal(kp[:n_out.value], want_kp) and np.array_equal(gftt[:n_g.value], want_g), "detect_keypoints"
     assert n_out.value > 20

@@ -4,18 +4,16 @@ too little parallax; 0 to 1000 matches; 0 to 50 % outliers.  The device's sample
 exactly; the homography counts must equal the oracle's on every iteration; the essential counts too, except on
 iterations the oracle flags as borderline (an eigenvalue with 1e-11 < |imag| < 1e-9, or a match within 1e-9 relative
 of the threshold), at most 1 % of them; the final answer must equal the serial loop's."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from oracle import twoview_oracle as tv
 from pvio_b200 import _lib
 from pvio_b200.two_view import batch_two_view, two_view
+from pvio_b200._lib import EINVAL
 from synthetic import synth
 
 pytestmark = pytest.mark.gpu
-EINVAL = -2
 
 SCENES = [
     dict(seed=40, n=150, outlier_frac=0.0, kind="general"),
@@ -153,10 +151,10 @@ def test_rejected_calls_change_nothing(ba):
         p1 = np.ascontiguousarray(d["p1"])
         p2 = np.ascontiguousarray(d["p2"])
         for r, src in zip(recs, (d, b)):
-            r.n_matches, r.seed, r.p1, r.p2 = 100, 648, _lib._ptr(p1, C.c_double), _lib._ptr(p2, C.c_double)
+            r.n_matches, r.seed, r.p1, r.p2 = 100, 648, _lib.ptr(p1), _lib.ptr(p2)
             r.fx, r.fy, r.min_matches, r.min_triangulation = src["fx"], d["fy"], 50, src.get("min_triangulation", 20)
             r.min_parallax, r.confidence, r.max_iteration = 10.0, src.get("confidence", 0.999), src.get("max_iteration", 1000)
-            r.info = _lib._ptr(info, C.c_int32)
+            r.info = _lib.ptr(info)
         assert ba.lib.pvio_b200_batch_two_view(ba.h, 2, recs) == EINVAL
         assert np.all(info == 77)
     recs = (_lib.CTwoView * 1)()
@@ -174,7 +172,7 @@ def test_rejected_calls_change_nothing(ba):
     assert ba.lib.pvio_b200_batch_two_view(ba.h, 65536, many) == EINVAL
     big = (_lib.CTwoView * 128)()
     for r in big:
-        r.n_matches, r.p1, r.p2 = 1 << 24, _lib._ptr(p1, C.c_double), _lib._ptr(p1, C.c_double)
+        r.n_matches, r.p1, r.p2 = 1 << 24, _lib.ptr(p1), _lib.ptr(p1)
         r.fx, r.fy, r.confidence, r.max_iteration = 400.0, 400.0, 0.9, 10
     assert ba.lib.pvio_b200_batch_two_view(ba.h, 128, big) == EINVAL
     big[0].n_matches = (1 << 24) + 1

@@ -2,8 +2,6 @@
 batched tracker and detector).  The undistorted frames equal cv2.undistort (radtan, K and D as float32, as
 EurocDatasetReader::read_image) and the oracle's equidistant remap (ImageUndistorter) bit for bit; the tracker and the
 detector on raw frames of slots with a lens equal the same calls, without lenses, on frames undistorted on the host."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -11,10 +9,10 @@ from oracle import undistort_oracle as uo
 from pvio_b200 import _lib, klt
 from pvio_b200.detect import batch_detect_keypoints, pack_requests
 from pvio_b200.undistort import EQUIDISTANT, NONE, RADTAN, batch_undistort, pack_lenses, set_lens
+from pvio_b200._lib import EINVAL
 from synthetic import synth
 
 cv2 = pytest.importorskip("cv2")
-EINVAL = -2
 
 EUROC = {"model": RADTAN, "width": 752, "height": 480, "K": (458.654, 457.296, 367.215, 248.375),
          "coeffs": (-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05)}
@@ -190,7 +188,7 @@ def test_rejections_change_nothing():
             arr = (_lib.CUndistortRequest * 1)()
             r = arr[0]
             r.slot, r.width, r.height, r.stride = 2, small.shape[1], small.shape[0], small.shape[1]
-            r.src, r.dst = _lib._ptr(img, C.c_uint8), _lib._ptr(out, C.c_uint8)
+            r.src, r.dst = _lib.ptr(img), _lib.ptr(out)
             edit(r)
             assert b.lib.pvio_b200_batch_undistort(b.h, 1, arr) == EINVAL
             assert (out == 77).all()

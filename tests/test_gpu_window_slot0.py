@@ -4,6 +4,7 @@ before a reset) under the slot rules (slot limits, a rejected call changes nothi
 import numpy as np
 import pytest
 
+from pvio_b200 import _lib
 from pvio_b200 import resident
 from pvio_b200.batch_window import BatchWindows, Edit
 from pvio_b200.bundle_adjustor import BundleAdjustor, PvioB200Error
@@ -12,7 +13,7 @@ from synthetic import synth
 from synthetic.sequence import ResidentPlayer, Run
 
 pytestmark = pytest.mark.gpu
-EINVAL = "error -2"
+EINVAL = f"error {_lib.EINVAL}"
 
 
 class Slot0Window:

@@ -13,10 +13,10 @@ import pytest
 from oracle import undistort_oracle as uo
 from pvio_b200 import _lib
 from pvio_b200.undistort import EQUIDISTANT, RADTAN, undistort_map
+from pvio_b200._lib import EINVAL
 
 cv2 = pytest.importorskip("cv2")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EINVAL = -2
 
 # (K = fx, fy, cx, cy), (k1, k2, p1, p2), width, height
 RADTAN_LENSES = {
@@ -104,8 +104,8 @@ def _rc(model, w, h, K, D, m1=True, m2=True):
     c = np.ascontiguousarray(D, dtype=np.float64)
     a = np.zeros((max(h, 1), max(w, 1), 2), np.int16)
     b = np.zeros((max(h, 1), max(w, 1)), np.uint16)
-    return lib.pvio_b200_undistort_map(model, w, h, _lib._ptr(p, C.c_double), _lib._ptr(c, C.c_double),
-                                       _lib._ptr(a, C.c_int16) if m1 else None, _lib._ptr(b, C.c_uint16) if m2 else None)
+    return lib.pvio_b200_undistort_map(model, w, h, _lib.ptr(p), _lib.ptr(c),
+                                       _lib.ptr(a) if m1 else None, _lib.ptr(b) if m2 else None)
 
 
 def test_library_map_rejections():

@@ -83,9 +83,6 @@ def main():
     def timed_loop(n, reps):
         """one handle per sequence, its frame 2 cached by track_keypoints; single pvio_b200_detect_keypoints calls"""
         fn = lib.pvio_b200_detect_keypoints
-        fn.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int,
-                       C.POINTER(C.c_double), C.c_int, C.c_double, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int),
-                       C.POINTER(C.c_float), C.POINTER(C.c_int)]
         hs = [BundleAdjustor(max_windows=1, max_frames=4, max_landmarks=16, max_obs=64) for _ in range(n)]
         try:
             bufs = []
@@ -102,8 +99,8 @@ def main():
                 for i in range(n):
                     ex, out, cnt, (h, w) = bufs[i]
                     t0 = time.perf_counter()
-                    hs[i]._ck(fn(hs[i].h, 2, None, w, h, w, *CLAHE, _lib._ptr(ex, C.c_double), len(ex), 25.0, 2048,
-                                 _lib._ptr(out, C.c_double), C.byref(cnt), None, None))
+                    hs[i]._ck(fn(hs[i].h, 2, None, w, h, w, *CLAHE, _lib.ptr(ex), len(ex), 25.0, 2048,
+                                 _lib.ptr(out), C.byref(cnt), None, None))
                     t += time.perf_counter() - t0
                 if r >= 1:
                     wall.append(t * 1e3)

@@ -76,7 +76,7 @@ def main():
         sms = (_lib.CSummary * n)()
 
         def batch():
-            ba._ck(lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib._ptr(frames, C.c_double), 16, C.byref(opt), sms))
+            ba._ck(lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib.ptr(frames), 16, C.byref(opt), sms))
             return sms[0].solve_seconds * 1e3
         kern, wall = timed(batch, init, frames, args.reps)
         its = [sms[i].iterations for i in range(n)]
@@ -88,7 +88,7 @@ def main():
             def loop():
                 k = 0.0
                 for i in range(n):
-                    ba._ck(lib.pvio_b200_pnp_solve(ba.h, C.byref(pbs[i]), _lib._ptr(frames[i], C.c_double),
+                    ba._ck(lib.pvio_b200_pnp_solve(ba.h, C.byref(pbs[i]), _lib.ptr(frames[i]),
                                                    C.byref(opt), C.byref(sm1)))
                     k += sm1.solve_seconds * 1e3
                 return k
@@ -103,13 +103,13 @@ def main():
         n = args.profile_n
         pbs, keep, init = packed(n)
         frames = init.copy()
-        lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib._ptr(frames, C.c_double), 16, C.byref(opt), None)
+        lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib.ptr(frames), 16, C.byref(opt), None)
         torch.cuda.synchronize()
         reps = 5
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(reps):
                 frames[:] = init
-                ba._ck(lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib._ptr(frames, C.c_double), 16, C.byref(opt),
+                ba._ck(lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib.ptr(frames), 16, C.byref(opt),
                                                      None))
             torch.cuda.synchronize()
         for e in prof.key_averages():

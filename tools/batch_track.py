@@ -12,7 +12,6 @@ Wall times are host clocks around the C call alone (every call ends in a synchro
 outside the timed region.  Medians of --reps calls after 3 warm-up calls.
 """
 import argparse
-import ctypes as C
 import json
 import os
 import sys
@@ -67,7 +66,7 @@ def main():
                  for i in range(n)]
         klt.batch_track_keypoints(ba, pairs, *ARGS[:3], clahe_clip=6.0)
         cp, outs, keep = klt.pack_pairs(pairs)
-        frame_ptr = [[_lib._ptr(np.ascontiguousarray(f), C.c_uint8) for f in k["frames"]] for k in kinds]
+        frame_ptr = [[_lib.ptr(np.ascontiguousarray(f)) for f in k["frames"]] for k in kinds]
 
         def step(k):                        # call k: frame k (cached) -> frame k + 1 (new, raw)
             for i in range(n):
@@ -93,9 +92,6 @@ def main():
     def timed_loop(n, reps):
         """one handle per sequence, single pvio_b200_track_keypoints calls over the same steady-state pairs"""
         fn = lib.pvio_b200_track_keypoints
-        fn.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint8), C.c_uint64, C.POINTER(C.c_uint8), C.c_int, C.c_int,
-                       C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint8), C.c_int, C.c_int,
-                       C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double]
         hs = [BundleAdjustor(max_windows=1, max_frames=4, max_landmarks=16, max_obs=64) for _ in range(n)]
         try:
             bufs = []
@@ -104,8 +100,8 @@ def main():
                 frames = [np.ascontiguousarray(f) for f in kd["frames"]]
                 nxt = kd["init"].copy()
                 st = np.zeros(500, np.uint8)
-                bufs.append((frames, [_lib._ptr(f, C.c_uint8) for f in frames], _lib._ptr(kd["pts"], C.c_float), nxt,
-                             _lib._ptr(nxt, C.c_float), st, _lib._ptr(st, C.c_uint8), kd["shape"]))
+                bufs.append((frames, [_lib.ptr(f) for f in frames], _lib.ptr(kd["pts"]), nxt,
+                             _lib.ptr(nxt), st, _lib.ptr(st), kd["shape"]))
             for i in range(n):                  # frame 1 -> 2 with both frames given: frame 2 is cached
                 frames, fp, pp, nxt, np_, st, sp, (h, w) = bufs[i]
                 hs[i]._ck(fn(hs[i].h, 1, fp[0], 2, fp[1], w, h, w, pp, np_, sp, 500, *ARGS))

@@ -16,7 +16,6 @@ Wall times are host clocks around the work of one call (every call ends in a syn
 after 3 warm-up calls.
 """
 import argparse
-import ctypes as C
 import json
 import os
 import sys
@@ -76,8 +75,8 @@ def main():
         klt.batch_track_keypoints(ba, pairs, *ARGS[:3], clahe_clip=6.0)
         cp, outs, keep = klt.pack_pairs(pairs)
         dst = [np.zeros((480, 752), np.uint8) for _ in range(n)] if not lens else None
-        raw_ptr = [[_lib._ptr(f, C.c_uint8) for f in k["frames"]] for k in kinds]
-        dst_ptr = [_lib._ptr(d, C.c_uint8) for d in dst] if dst else None
+        raw_ptr = [[_lib.ptr(f) for f in k["frames"]] for k in kinds]
+        dst_ptr = [_lib.ptr(d) for d in dst] if dst else None
 
         def step(k):                        # call k: frame k (cached) -> frame k + 1 (new, raw)
             for i in range(n):

@@ -87,15 +87,15 @@ def host_path(ba, player, recs):
         keep += [x, z, last]
         pb = pbs[j]
         pb.n_points, pb.use_inertial = len(x), 1
-        pb.points, pb.z = _lib._ptr(x, C.c_double), _lib._ptr(z, C.c_double)
+        pb.points, pb.z = _lib.ptr(x), _lib.ptr(z)
         pb.cam_q_cs[:], pb.cam_p_cs[:] = list(w.cam_q_cs), list(w.cam_p_cs)
         pb.imu_q_cs[:], pb.imu_p_cs[:] = list(w.imu_q_cs), list(w.imu_p_cs)
         pb.sqrt_inv_cov[:] = list(np.asarray(w.sqrt_inv_cov, dtype=np.float64).reshape(4))
         pb.cauchy_a = w.cauchy_a
-        pb.last_frame, pb.imu_data = _lib._ptr(last, C.c_double), _lib._ptr(L.imu, C.c_double)
+        pb.last_frame, pb.imu_data = _lib.ptr(last), _lib.ptr(L.imu)
         frames[j] = L.state
     opt = _lib.COptions(10, 1e6, 1, 0, 0.0)
-    ba._ck(ba.lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib._ptr(frames, C.c_double), 16, C.byref(opt), None))
+    ba._ck(ba.lib.pvio_b200_batch_pnp_solve(ba.h, n, pbs, _lib.ptr(frames), 16, C.byref(opt), None))
     Ps, z, fr = [], [], []
     for j, ((L, _), d) in enumerate(zip(recs, ds)):
         run = player.runs[j]

@@ -1,12 +1,12 @@
 """Phase times of solve_kernel on the cfg3 / cfg4 / cfg2 single window (tuning build with -DPVIO_SOLVE_STAMPS):
     python -c "from pvio_b200 import build as b; b.build(defines=['PVIO_SOLVE_STAMPS'], out='tools/_variants/libpvio_stamps.so')"
     PVIO_B200_TUNE_LIB=$PWD/tools/_variants/libpvio_stamps.so python tools/solve_stamps.py"""
-import ctypes as C
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 from synthetic import synth
+from pvio_b200 import _lib
 from pvio_b200.bundle_adjustor import BundleAdjustor
 
 NAMES = ["init+T", "vision blocks", "imu_factor_raw", "imu whiten+accumulate", "prior r, S^T r", "prior H, g", "planes",
@@ -17,9 +17,7 @@ for name, maker in (("cfg3", synth.make_cfg3), ("cfg4", synth.make_cfg4), ("cfg2
     for _ in range(3):
         ba.gn_step(w, s)
     st = np.zeros(16, dtype=np.int64)
-    fn = ba.lib.pvio_b200_debug_solve_stamps
-    fn.argtypes = [C.POINTER(C.c_longlong)]
-    assert fn(st.ctypes.data_as(C.POINTER(C.c_longlong))) == 0
+    assert ba.lib.pvio_b200_debug_solve_stamps(_lib.ptr(st)) == 0
     d = np.diff(st[:10])
     print(name, "total cycles", int(st[9] - st[0]), "=", round((st[9] - st[0]) / 1.965e3, 1), "us at 1.965 GHz")
     for n, v in zip(NAMES[1:], d):
