@@ -671,6 +671,50 @@ typedef struct pvio_b200_detect_request {
 int pvio_b200_batch_detect_keypoints(pvio_b200_handle h, int n, const pvio_b200_detect_request *requests,
                                      double clahe_clip, int tiles_x, int tiles_y);
 
+/* One camera frame of pvio_b200_batch_feature_track: the next frame of one sequence. */
+typedef struct pvio_b200_feature_frame {
+    int32_t slot;                  /* a sequence slot of pvio_b200_batch_track_keypoints, 0 .. 65535, distinct        */
+    int32_t width, height, stride;
+    uint64_t frame_id;             /* the frame's id within the sequence, != 0                                        */
+    const uint8_t *image;          /* raw pixels (undistorted on the device when the slot has a lens)                 */
+    double fx, fy, cx, cy;         /* the frame's K                                                                   */
+    int32_t map_frames;            /* the tracker map's frame_num() before this frame is put (0: a new sequence)      */
+    int32_t max_keypoints;         /* capacity of keypoints / prev_index (see the bound below)                       */
+    const double *predict_q;       /* [4] x, y, z, w: delta_key_q of frame.cpp:98; NULL: no prediction              */
+    double *keypoints;             /* [max_keypoints][2] out: the frame's keypoints, normalised (Frame::keypoints)    */
+    int32_t *prev_index;           /* [max_keypoints] out: the previous frame's keypoint each one continues, or -1   */
+    int32_t *n_keypoints;          /* out: their number                                                               */
+    int32_t *counts;               /* [4] out, may be NULL: kept after LK and the border test, after F-RANSAC, after */
+                                   /* the track-length thinning, and the number of new detections                    */
+    int32_t *info;                 /* [4] out, may be NULL: as pvio_b200_klt_pair::info                               */
+} pvio_b200_feature_frame;         /* 120 bytes on LP64 */
+
+/* The per-frame step of FeatureTracker::work (feature_tracker.cpp:77-99) for n sequences in one call: Frame::track_keypoints
+ * of the previous frame into this one (frame.cpp:88-138) -- the initial guesses, pvio_b200_batch_track_keypoints' LK,
+ * border test and F-RANSAC, then the track-length-ordered Poisson-disk thinning -- followed by Frame::detect_keypoints
+ * (frame.cpp:72-86) on the new frame.  Each slot keeps its newest frame's keypoints on the device, so nothing but the
+ * new pixels goes up and the new keypoints come down.  The options are pvio_b200_batch_track_keypoints' plus
+ * keypoint_distance (Config::feature_tracker_min_keypoint_distance, > 0).
+ * Slot rules:
+ *  - map_frames == 0 starts the sequence: the slot drops its keypoints, and the frame is only equalised, cached and
+ *    detected, as the reference does for a map's first frame.
+ *  - map_frames > 0 continues it: the slot's newest frame must still be in its pyramid cache (same shape and
+ *    clahe_clip); a request whose frame another call has evicted is rejected, as is a frame_id equal to that frame's.
+ *  - A slot named twice is rejected.
+ *  - max_keypoints below cells + 2000 is rejected, cells = (floor(w / (r / sqrt 2)) + 1) (floor(h / (r / sqrt 2)) + 1)
+ *    with r = keypoint_distance: the thinned keypoints are at least r apart (at most one per cell), and at most 1000
+ *    untracked survivors and 1000 detections are added.
+ *  - Every request is checked before anything is staged: on PVIO_B200_EINVAL no output and no slot has changed.
+ *  - pvio_b200_batch_track_keypoints and pvio_b200_batch_detect_keypoints leave a slot's keypoints alone (they may
+ *    evict its frames).
+ * A keypoint's track length is min(frames since it was detected + 1, map_frames); keypoints the previous frame detected
+ * have no track yet and skip the thinning.  n == 0 is a no-op.  With clahe_clip > 0 the launches, copies and
+ * synchronisations of a call do not depend on n (DESIGN.md §4.7f). */
+int pvio_b200_batch_feature_track(pvio_b200_handle h, int n, const pvio_b200_feature_frame *frames,
+                                  int max_level, int max_iter, double eps, double clahe_clip,
+                                  int tiles_x, int tiles_y, int border,
+                                  double ransac_threshold, double ransac_confidence, double keypoint_distance);
+
 /* ---- two-view initialisation ------------------------------------------------------------- */
 /* The two-view step of Initializer::init_sfm (pvio/src/pvio/core/initializer.cpp:102-161) that seeds a sequence: the
  * match-count and parallax gates, find_homography_matrix and find_essential_matrix (Ransac<> of utility/ransac.h,

@@ -86,6 +86,14 @@ class CDetectRequest(C.Structure):
                 ("gftt_out", c_f32p), ("n_gftt", c_i32p)]
 
 
+class CFeatureFrame(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32),
+                ("frame_id", C.c_uint64), ("image", c_u8p), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double),
+                ("cy", C.c_double), ("map_frames", C.c_int32), ("max_keypoints", C.c_int32), ("predict_q", c_f64p),
+                ("keypoints", c_f64p), ("prev_index", c_i32p), ("n_keypoints", c_i32p), ("counts", c_i32p),
+                ("info", c_i32p)]
+
+
 class CWindowEdit(C.Structure):
     _fields_ = [("slot", C.c_int32), ("replace_last", C.c_int32), ("state", c_f64p), ("fixed", C.c_int32),
                 ("imu_record", c_f64p), ("n_new_tracks", C.c_int32), ("new_frame", c_i32p), ("new_z", c_f64p),
@@ -207,6 +215,8 @@ SIGNATURES = {
     "pvio_b200_batch_track_keypoints": (_int, [_h, _int, _P(CKltPair), _int, _int, _f64, _f64, _int, _int, _int, _f64,
                                                _f64]),
     "pvio_b200_batch_detect_keypoints": (_int, [_h, _int, _P(CDetectRequest), _f64, _int, _int]),
+    "pvio_b200_batch_feature_track": (_int, [_h, _int, _P(CFeatureFrame), _int, _int, _f64, _f64, _int, _int, _int, _f64,
+                                             _f64, _f64]),
     "pvio_b200_batch_two_view": (_int, [_h, _int, _P(CTwoView)]),
     "pvio_b200_undistort_map": (_int, [_int, _int, _int, c_f64p, c_f64p, _P(C.c_int16), _P(C.c_uint16)]),
     "pvio_b200_batch_set_lens": (_int, [_h, _int, _P(CLens)]),

@@ -1516,6 +1516,15 @@ int pvio_b200_batch_track_keypoints(pvio_b200_handle hh, int n, const pvio_b200_
                             ransac_confidence);
 }
 
+int pvio_b200_batch_feature_track(pvio_b200_handle hh, int n, const pvio_b200_feature_frame *frames, int max_level, int max_iter,
+                                  double eps, double clahe_clip, int tiles_x, int tiles_y, int border,
+                                  double ransac_threshold, double ransac_confidence, double keypoint_distance) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const KltBatchOptions o{max_level, max_iter, eps, clahe_clip, tiles_x, tiles_y, border, ransac_threshold, ransac_confidence};
+    return batch_feature_track_impl(h, n, frames, o, keypoint_distance);
+}
+
 int pvio_b200_batch_detect_keypoints(pvio_b200_handle hh, int n, const pvio_b200_detect_request *requests, double clahe_clip,
                                      int tiles_x, int tiles_y) {
     Handle *h = reinterpret_cast<Handle *>(hh);

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <algorithm>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
 #include <tuple>
@@ -92,15 +93,31 @@ struct SlotLens {
     const uint16_t *m2() const { return reinterpret_cast<const uint16_t *>(map.d + (size_t)4 * w * h); }
 };
 
+// feature_track.cu: the keypoints of a slot's newest frame (pvio_b200_batch_feature_track), double-buffered so that a
+// call reads buf[cur] and writes buf[1 - cur].  Each buffer: [cap] double2 normalised keypoint, then [cap] int32 birth
+// (the number of the frame that detected it).
+struct SlotKeypoints {
+    DevBuf<uint8_t> buf[2];
+    size_t cap[2] = {0, 0};                   // keypoints each buffer holds
+    int cur = 0, n = 0;                       // newest buffer, its keypoint count
+    bool live = false;                        // a sequence was started in this slot (map_frames == 0)
+    int frame_no = 0;                         // the number of the newest frame (births count in these)
+    uint64_t frame_id = 0;                    // its id in the slot's pyramid cache
+    double fx = 0, fy = 0, cx = 0, cy = 0;    // its K
+};
+
 // the batched tracker (pvio_b200_batch_track_keypoints): one pyramid cache per sequence slot, grown on demand, and
 // the buffers of one call, grown to the largest call seen
 struct KltBatchState {
     std::vector<KltPyramids> slots;
+    std::vector<SlotKeypoints> kps;           // per slot, grown on demand by pvio_b200_batch_feature_track
     std::vector<SlotLens> lens;               // per slot, grown on demand by pvio_b200_batch_set_lens
     DevBuf<uint8_t> ustage;                   // both sides: pvio_b200_batch_undistort's descriptors and frames
     DevBuf<uint8_t> stage;                    // both sides: uploaded descriptors, frames and points | downloaded results |
                                               // winners' masks; host side only: the mask jobs the device reads in place
     DevBuf<uint8_t> scratch;                  // device: CLAHE tables, RANSAC matches, schedules, counts, models, masks
+    DevBuf<uint8_t> fstage;                   // feature_track.cu, both sides: descriptors (uploaded) | outputs (downloaded)
+    DevBuf<uint8_t> fscratch;                 // feature_track.cu, device: thinning, detection and commit working areas
 };
 
 // detect.cu: per-image-shape buffers of the corner detector
@@ -411,6 +428,45 @@ int marg_opt_in(Handle *h);        // the eigen-solver's dynamic shared memory, 
 int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_level, int max_iter, double eps,
                      double clahe_clip, int tiles_x, int tiles_y, int border, double ransac_threshold,
                      double ransac_confidence);
+// klt.cu: the stages of a batched tracker call, shared by pvio_b200_batch_track_keypoints and
+// pvio_b200_batch_feature_track.  One pair of such a call:
+struct KltBatchItem {
+    int slot, width, height, stride, n_points;
+    uint64_t prev_id, next_id;                // prev_id 0: no previous frame and no points; the next frame is only cached
+    const uint8_t *prev, *next;
+    const float *prev_pts, *next_pts;         // host [n_points][2]; unused when the points are written on the device
+};
+struct KltBatchOptions {
+    int max_level, max_iter;
+    double eps, clahe_clip;
+    int tiles_x, tiles_y, border;
+    double ransac_threshold, ransac_confidence;
+};
+// points written on the device: called once the staging is uploaded, with the call's device arrays of LK inputs and
+// initial guesses ([n][2], pair i's points from KltBatchResults::first[i]) and the pair of each point
+struct KltDevicePoints {
+    std::function<int(Handle *, float *prev_pts, float *next_pts, const int *pair_of)> write_points;
+};
+// what the stages leave: LK + border results (host copies, or device arrays when the points were written on the
+// device), and per pair its F-RANSAC outcome: mask = the winner's mask words on the device (fm_batch_masks has been
+// launched; bit k: the k-th point with a nonzero status), clear = RANSAC ran and kept nothing, info as
+// pvio_b200_klt_pair::info
+struct KltBatchResults {
+    const float *next = nullptr, *err = nullptr;
+    const uint8_t *status = nullptr;
+    std::vector<size_t> first;
+    std::vector<const unsigned *> mask;
+    std::vector<uint8_t> clear;
+    std::vector<int32_t> info;
+    size_t o_mw = 0, words = 0;               // the mask words: offset in KltBatchState::stage, count
+};
+// Checks every pair, then uploads, builds the pyramids, runs LK, the schedules and the hypotheses, synchronises once,
+// replays each pair on the host and launches the winners' masks.  dev == nullptr: the points come from the items.
+int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchOptions &opt, const KltDevicePoints *dev,
+                    KltBatchResults &res);
+// feature_track.cu: pvio_b200_batch_feature_track
+int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
+                             double keypoint_distance);
 // fmat.cu
 int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double threshold, double confidence, int max_iters,
                    const int32_t *schedule, int n_schedule, uint8_t *mask, double *F_out, int32_t *info);

@@ -28,6 +28,7 @@
 
 #include "api_internal.h"
 #include "imu.cuh"
+#include "quat.cuh"
 #include "tri.cuh"
 
 namespace pvio {
@@ -339,20 +340,6 @@ __global__ void __launch_bounds__(kBwThreads) bw_planes_kernel(BwArgs a, const B
     }
 }
 
-// quaternions (x, y, z, w), Hamilton product, q * v = rotate: the reference's Eigen conventions (estimation/state.h)
-__device__ void bw_qmul(const double *a, const double *b, double *o) {
-    o[0] = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1];
-    o[1] = a[3] * b[1] - a[0] * b[2] + a[1] * b[3] + a[2] * b[0];
-    o[2] = a[3] * b[2] + a[0] * b[1] - a[1] * b[0] + a[2] * b[3];
-    o[3] = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2];
-}
-__device__ void bw_qrot(const double *q, const double *v, double *o) {
-    const double x = q[0], y = q[1], z = q[2], w = q[3];
-    const double tx = 2.0 * (y * v[2] - z * v[1]), ty = 2.0 * (z * v[0] - x * v[2]), tz = 2.0 * (x * v[1] - y * v[0]);
-    o[0] = v[0] + w * tx + (y * tz - z * ty);
-    o[1] = v[1] + w * ty + (z * tx - x * tz);
-    o[2] = v[2] + w * tz + (x * ty - y * tx);
-}
 __device__ void bw_cam_pose(const double *fs, const WinConst &c, double *qc, double *pc) {
     bw_qmul(fs, c.cam_q, qc);
     double t[3];

@@ -30,6 +30,7 @@
 #include <thrust/iterator/transform_iterator.h>
 
 #include "api_internal.h"
+#include "detect.cuh"
 
 namespace pvio {
 namespace {
@@ -37,28 +38,6 @@ namespace {
 __device__ __forceinline__ int refl(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 constexpr int kTX = 32, kTY = 16;
-constexpr int kMaxCorners = 1000;             // GFTTDetector::create(1000, ...)
-
-// the per-request results of a batched call (batch_detect_impl), downloaded in one copy
-struct DetectResult {
-    int n_gftt, pad;
-    unsigned mask[(kMaxCorners + 31) / 32];   // bit j: corner j passes the Poisson filter and the 20-pixel border
-    unsigned corner[kMaxCorners];             // the GFTT corners in order, as pixel indices y * w + x
-};
-
-// one frame as the kernels read it (the single call: frame 0 of one)
-struct DetectBatchFrame {
-    const uint8_t *img;                       // the equalised frame (a cached level 0, uploaded pixels, or CLAHE output)
-    float *resp;                              // [h][w] Harris response
-    unsigned long long *keys, *sorted;        // its segment of the candidate keys, unsorted / sorted descending
-    int *counters;                            // [2] max response bits, candidate count
-    const double2 *pre;                       // [n_pre] the existing keypoints a corner's Poisson walk can meet, in order
-    uint8_t *work;                            // the select kernel's working area in global memory, or nullptr: on chip
-    DetectResult *res;
-    double gs, r2;                            // Poisson cell size r / sqrt(2) and r^2
-    int w, h, cap, key_off;                   // key_off: the segment's first key
-    int n_pre, gw, gh, hbits;                 // min-distance grid gw x gh; Poisson hash table of 2^hbits cells
-};
 
 // the single call's staging (DetectState::stage, both sides): its frame, the frame CLAHE equalises, zeroed counters
 struct DetectStage {
@@ -242,32 +221,13 @@ int ensure(Handle *h, int w, int hgt) {
 // come first among the CLAHE descriptors, so the remap's grid covers them alone.
 constexpr int kMinDist = 20;                  // GFTT's minDistance, and the cell of its grid (lround(20))
 constexpr int kCellEmpty = -(1 << 30);        // x of an empty min-distance slot: farther than 20 px from every pixel
-constexpr unsigned long long kHashEmpty = ~0ull;
-constexpr double kCellLimit = 1073741824.0;   // 2^30: the Poisson cell indices the host pass forms without int overflow
 constexpr int kSelectThreads = 128;
-constexpr size_t kSelectSmem = 96 * 1024;     // larger working areas go to global memory
 constexpr int kMaxBatchDetect = 65535;        // grid z: one layer per frame
 
 // min_distance_select's distance test: float dx^2 + dy^2 against 20^2
 __device__ __forceinline__ bool md_close(int x, int y, int px, int py) {
     const float dx = (float)x - (float)px, dy = (float)y - (float)py;
     return dx * dx + dy * dy < 400.0f;
-}
-
-// Poisson cells (ix, iy) >= (-2, -2) as hash keys; never kHashEmpty
-__device__ __forceinline__ unsigned long long cell_key(long long ix, long long iy) {
-    return ((unsigned long long)(ix + 8) << 32) | (unsigned long long)(iy + 8);
-}
-__device__ __forceinline__ unsigned long long hash_slot(unsigned long long key, int hbits) {
-    return (key * 0x9E3779B97F4A7C15ull) >> (64 - hbits);
-}
-__device__ int hash_find(const unsigned long long *hk, const int *hv, int hbits, unsigned long long key) {
-    const unsigned long long m = (1ull << hbits) - 1;
-    for (unsigned long long s = hash_slot(key, hbits);; s = (s + 1) & m) {
-        const unsigned long long k = hk[s];
-        if (k == key) return hv[s];
-        if (k == kHashEmpty) return -1;
-    }
 }
 
 // The two greedy passes of pvio_b200_detect_keypoints (min_distance_select, PoissonFilter, the border) for frame
@@ -283,9 +243,8 @@ __device__ int hash_find(const unsigned long long *hk, const int *hv, int hbits,
 //                 resolved in lane order (the host's order) with shuffles: lane k is accepted if it passed and no
 //                 accepted earlier lane of the chunk is closer than 20 px.  Within 20 px means within the 3 x 3 cells
 //                 the host examines, so the two tests agree.  Stops at 1000 corners.
-//   Poisson       corner by corner: lane t examines cell t + 1 of the reference's walk over the 5 x 5 block (which
-//                 skips the block's first cell and examines the one past its end), then a vote; an accepted corner
-//                 overwrites its cell and is kept if it lies inside the 20-px border.
+//   Poisson       corner by corner, poisson_insert (detect.cuh); a taken corner is kept if it lies inside the 20-px
+//                 border.
 __global__ void __launch_bounds__(kSelectThreads) detect_select_kernel(const DetectBatchFrame *frames) {
     extern __shared__ __align__(16) uint8_t smem[];
     const DetectBatchFrame &f = frames[blockIdx.x];
@@ -303,9 +262,13 @@ __global__ void __launch_bounds__(kSelectThreads) detect_select_kernel(const Det
     __syncthreads();
     const unsigned long long hm = hcap - 1;
     const double gs = f.gs;
-    for (int i = tid; i < f.n_pre; i += kSelectThreads) {          // the last preset of a cell holds it: the largest index
+    const int n_pre = f.pre_count ? *f.pre_count : f.n_pre;
+    for (int i = tid; i < n_pre; i += kSelectThreads) {             // the last preset of a cell holds it: the largest index
         const double2 p = f.pre[i];
-        const unsigned long long key = cell_key((long long)floor(p.x / gs), (long long)floor(p.y / gs));
+        // only presets in cells [-2, cxmax + 2] x [-2, cymax + 3] can meet a corner's walk: the others stay out
+        const double fx = floor(p.x / gs), fy = floor(p.y / gs);
+        if (!(fx >= -2.0 && fx <= f.cxmax + 2.0 && fy >= -2.0 && fy <= f.cymax + 3.0)) continue;
+        const unsigned long long key = cell_key((long long)fx, (long long)fy);
         for (unsigned long long s = hash_slot(key, f.hbits);; s = (s + 1) & hm) {
             const unsigned long long k = atomicCAS(&hk[s], kHashEmpty, key);
             if (k == kHashEmpty || k == key) { atomicMax(&hv[s], i); break; }
@@ -370,35 +333,18 @@ __global__ void __launch_bounds__(kSelectThreads) detect_select_kernel(const Det
 
     // PoissonDiskFilter against the presets, then the 20-pixel border (opencv_image.cpp:69-84)
     const double r2 = f.r2;
+    const double2 *pre = f.pre;
+    auto point = [pre, corners, n_pre](int v) {
+        return v < n_pre ? pre[v] : make_double2((double)corners[v - n_pre].x, (double)corners[v - n_pre].y);
+    };
     unsigned word = 0;
     for (int i = 0; i < ng; ++i) {
         const double x = corners[i].x, y = corners[i].y;
-        const double fx = floor(x / gs), fy = floor(y / gs);
-        // beyond 2^30 (or a NaN radius) the host's cell arithmetic overflows and its walk meets no point: no test
-        const bool regular = fx <= kCellLimit && fy <= kCellLimit;
-        bool near = false;
-        if (regular && lane < 25) {
-            const int t = lane + 1;
-            const int v = hash_find(hk, hv, f.hbits, cell_key((long long)fx - 2 + t % 5, (long long)fy - 2 + t / 5));
-            if (v >= 0) {
-                const double px = v < f.n_pre ? f.pre[v].x : (double)corners[v - f.n_pre].x;
-                const double py = v < f.n_pre ? f.pre[v].y : (double)corners[v - f.n_pre].y;
-                const double dx = x - px, dy = y - py;
-                near = dx * dx + dy * dy < r2;
-            }
-        }
-        const bool take = !__any_sync(0xffffffffu, near);
+        const bool take = poisson_insert(hk, hv, f.hbits, gs, r2, x, y, n_pre + i, point);
         if (lane == 0) {
-            if (take && regular) {
-                const unsigned long long key = cell_key((long long)fx, (long long)fy);
-                unsigned long long s = hash_slot(key, f.hbits);
-                while (hk[s] != kHashEmpty && hk[s] != key) s = (s + 1) & hm;
-                hk[s] = key; hv[s] = f.n_pre + i;
-            }
             if (take && !(x < 20 || y < 20 || x >= w - 20 || y >= hgt - 20)) word |= 1u << (i & 31);
             if ((i & 31) == 31 || i == ng - 1) { res->mask[i >> 5] = word; word = 0; }
         }
-        __syncwarp();
     }
 }
 
@@ -418,6 +364,57 @@ struct SegEnd {
 inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 }  // namespace
+
+DetectPlan detect_plan(int w, int hgt, double keypoint_distance, int n_pre) {
+    DetectPlan P;
+    P.cap = candidate_cap((size_t)w * hgt);
+    P.gs = keypoint_distance / std::sqrt(2.0);                      // PoissonFilter's cell size
+    P.cxmax = std::min(std::floor((w - 1) / P.gs), kCellLimit);
+    P.cymax = std::min(std::floor((hgt - 1) / P.gs), kCellLimit);
+    P.n_pre = n_pre;
+    P.gw = (w + kMinDist - 1) / kMinDist;
+    P.gh = (hgt + kMinDist - 1) / kMinDist;
+    P.hbits = 1;
+    while (((size_t)1 << P.hbits) < 2 * ((size_t)n_pre + kMaxCorners)) ++P.hbits;
+    P.work = align256(sizeof(int4) * P.gw * P.gh + sizeof(float2) * kMaxCorners + 12 * ((size_t)1 << P.hbits));
+    return P;
+}
+
+void detect_apply_plan(const DetectPlan &P, int w, int hgt, double keypoint_distance, DetectBatchFrame &F) {
+    F.gs = P.gs; F.r2 = keypoint_distance * keypoint_distance;
+    F.cxmax = P.cxmax; F.cymax = P.cymax;
+    F.w = w; F.h = hgt; F.cap = P.cap;
+    F.n_pre = P.n_pre; F.gw = P.gw; F.gh = P.gh; F.hbits = P.hbits;
+}
+
+int detect_sort_bytes(Handle *h, int n, size_t n_keys, size_t &bytes) {
+    auto begin_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{nullptr});
+    auto end_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{nullptr});
+    bytes = 0;
+    CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(nullptr, bytes, (const unsigned long long *)nullptr,
+                                                            (unsigned long long *)nullptr, (int)n_keys, n, begin_it, end_it, 0, 64));
+    return 0;
+}
+
+int detect_run(Handle *h, const DetectBatchFrame *d_frm, int n, int max_w, int max_h, const unsigned long long *keys,
+               unsigned long long *sorted, size_t n_keys, uint8_t *sort_tmp, size_t sort_bytes, size_t smem) {
+    cudaStream_t st = h->stream;
+    harris_response_kernel<<<dim3((max_w + kTX - 1) / kTX, (max_h + kTY - 1) / kTY, n), dim3(kTX, kTY), 0, st>>>(0.04f, d_frm);
+    nms_compact_kernel<<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n), dim3(32, 8), 0, st>>>(1.0e-3, d_frm);
+    h->launches += 2;
+    size_t tmp = sort_bytes;
+    CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(
+              sort_tmp, tmp, keys, sorted, (int)n_keys, n,
+              thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{d_frm}),
+              thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{d_frm}), 0, 64, st));
+    ++h->launches;
+    if (smem > 48 * 1024)
+        CK(h, cudaFuncSetAttribute(detect_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    detect_select_kernel<<<n, kSelectThreads, smem, st>>>(d_frm);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    return 0;
+}
 
 int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, double clahe_clip, int tiles_x, int tiles_y) {
     if (n < 0 || n > kMaxBatchDetect) return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: bad request count");
@@ -449,38 +446,22 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
             return fail(h, PVIO_B200_EINVAL, "batch_detect_keypoints: the frame shape differs from the slot's lens");
     }
 
-    // sizes: per frame its key segment, the existing points its Poisson walks can meet (cells [-2, cx + 2] x
-    // [-2, cy + 3] around the cells of its pixels), its working area; the staging and the scratch of the call
-    struct Plan {
-        size_t pix_off, eq_off, und_off, resp_off, work, work_off;
-        int cap, key_off, n_pre, gw, gh, hbits;
-        double gs, cxmax, cymax;
+    // sizes: per frame its key segment and its working area; the staging and the scratch of the call
+    struct Plan : DetectPlan {
+        size_t pix_off, eq_off, und_off, resp_off, work_off;
+        int key_off;
     };
     std::vector<Plan> plan(n);
-    auto keep = [](const Plan &P, double x, double y) {
-        const double fx = std::floor(x / P.gs), fy = std::floor(y / P.gs);
-        return fx >= -2.0 && fx <= P.cxmax + 2.0 && fy >= -2.0 && fy <= P.cymax + 3.0;
-    };
     size_t n_keys = 0, n_pre = 0, pix_bytes = 0, eq_bytes = 0, und_bytes = 0, resp_bytes = 0, smem = 0;
     int n_eq = 0, n_lens = 0, max_w = 0, max_h = 0, eq_w = 0, eq_h = 0, und_w = 0, und_h = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_detect_request &a = reqs[i];
         Plan &P = plan[i];
+        static_cast<DetectPlan &>(P) = detect_plan(a.width, a.height, a.keypoint_distance, a.n_existing);
         const size_t px = (size_t)a.width * a.height;
-        P.cap = candidate_cap(px);
         P.key_off = (int)std::min<size_t>(n_keys, INT_MAX);
         n_keys += P.cap;
-        P.gs = a.keypoint_distance / std::sqrt(2.0);                // PoissonFilter's cell size
-        P.cxmax = std::min(std::floor((a.width - 1) / P.gs), kCellLimit);
-        P.cymax = std::min(std::floor((a.height - 1) / P.gs), kCellLimit);
-        P.n_pre = 0;
-        for (int j = 0; j < a.n_existing; ++j) P.n_pre += keep(P, a.existing[2 * j], a.existing[2 * j + 1]);
         n_pre += P.n_pre;
-        P.gw = (a.width + kMinDist - 1) / kMinDist;
-        P.gh = (a.height + kMinDist - 1) / kMinDist;
-        P.hbits = 1;
-        while (((size_t)1 << P.hbits) < 2 * ((size_t)P.n_pre + kMaxCorners)) ++P.hbits;
-        P.work = align256(sizeof(int4) * P.gw * P.gh + sizeof(float2) * kMaxCorners + 12 * ((size_t)1 << P.hbits));
         if (P.work <= kSelectSmem) smem = std::max(smem, P.work);
         P.resp_off = resp_bytes;
         resp_bytes += align256(sizeof(float) * px);
@@ -520,11 +501,8 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     // device scratch: responses | keys | sorted keys | equalised frames | CLAHE tables | working areas | sort temporaries |
     // undistorted frames
     const size_t tiles = do_clahe ? (size_t)tiles_x * tiles_y : 0;
-    auto begin_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{nullptr});
-    auto end_it = thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{nullptr});
     size_t cub_bytes = 0;
-    CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(nullptr, cub_bytes, (const unsigned long long *)nullptr,
-                                                            (unsigned long long *)nullptr, (int)n_keys, n, begin_it, end_it, 0, 64));
+    TRY(detect_sort_bytes(h, n, n_keys, cub_bytes));
     size_t c = 0;
     const size_t c_resp = c;   c += resp_bytes;
     const size_t c_keys = c;   c = align256(c + sizeof(unsigned long long) * n_keys);
@@ -582,15 +560,11 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
         F.sorted = reinterpret_cast<unsigned long long *>(dc + c_sorted) + P.key_off;
         F.counters = reinterpret_cast<int *>(ds + o_cnt) + 2 * i;
         F.pre = reinterpret_cast<const double2 *>(ds + o_pre) + p;
-        for (int j = 0; j < a.n_existing; ++j) {
-            const double x = a.existing[2 * j], y = a.existing[2 * j + 1];
-            if (keep(P, x, y)) pre[p++] = make_double2(x, y);
-        }
+        for (int j = 0; j < a.n_existing; ++j) pre[p++] = make_double2(a.existing[2 * j], a.existing[2 * j + 1]);
         F.work = P.work > smem ? dc + c_work + P.work_off : nullptr;
         F.res = reinterpret_cast<DetectResult *>(ds + o_res) + i;
-        F.gs = P.gs; F.r2 = a.keypoint_distance * a.keypoint_distance;
-        F.w = a.width; F.h = a.height; F.cap = P.cap; F.key_off = P.key_off;
-        F.n_pre = P.n_pre; F.gw = P.gw; F.gh = P.gh; F.hbits = P.hbits;
+        detect_apply_plan(P, a.width, a.height, a.keypoint_distance, F);
+        F.key_off = P.key_off;
     }
 
     cudaStream_t st = h->stream;
@@ -598,20 +572,8 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     const DetectBatchFrame *d_frm = reinterpret_cast<const DetectBatchFrame *>(ds + o_frm);
     if (n_lens > 0) undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_lens, und_w, und_h);
     if (n_eq > 0) klt_batch_clahe(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_eq, tiles_x, tiles_y, eq_w, eq_h);
-    harris_response_kernel<<<dim3((max_w + kTX - 1) / kTX, (max_h + kTY - 1) / kTY, n), dim3(kTX, kTY), 0, st>>>(0.04f, d_frm);
-    nms_compact_kernel<<<dim3((max_w + 31) / 32, (max_h + 7) / 8, n), dim3(32, 8), 0, st>>>(1.0e-3, d_frm);
-    h->launches += 2;
-    size_t tmp = cub_bytes;
-    CK(h, cub::DeviceSegmentedRadixSort::SortKeysDescending(
-              dc + c_cub, tmp, reinterpret_cast<const unsigned long long *>(dc + c_keys), reinterpret_cast<unsigned long long *>(dc + c_sorted),
-              (int)n_keys, n, thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegBegin{d_frm}),
-              thrust::make_transform_iterator(thrust::make_counting_iterator(0), SegEnd{d_frm}), 0, 64, st));
-    ++h->launches;
-    if (smem > 48 * 1024)
-        CK(h, cudaFuncSetAttribute(detect_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    detect_select_kernel<<<n, kSelectThreads, smem, st>>>(d_frm);
-    ++h->launches;
-    CK(h, cudaGetLastError());
+    TRY(detect_run(h, d_frm, n, max_w, max_h, reinterpret_cast<const unsigned long long *>(dc + c_keys),
+                   reinterpret_cast<unsigned long long *>(dc + c_sorted), n_keys, dc + c_cub, cub_bytes, smem));
     CK(h, cudaMemcpyAsync(hs + o_res, ds + o_res, sizeof(DetectResult) * n, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
 

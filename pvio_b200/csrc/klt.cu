@@ -12,6 +12,7 @@
 // because status flags are compared bit-exactly with cv2.
 #include <algorithm>
 #include <cstring>
+#include <functional>
 #include <vector>
 #include "api_internal.h"
 #include "klt_border.cuh"
@@ -509,7 +510,61 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
                      double ransac_confidence) {
     if (n < 0 || n > kMaxBatchPairs) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad pair count");
     if (n == 0) return 0;
-    if (!pairs || max_level < 0 || max_level >= kMaxLevels || border < 0 || !(clahe_clip >= 0.0))
+    if (!pairs) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad arguments");
+    std::vector<KltBatchItem> items(n);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_klt_pair &a = pairs[i];
+        if (!a.prev_id) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad shape, stride or frame id");
+        if (a.n_points > 0 && !a.status) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad points");
+        items[i] = KltBatchItem{a.slot, a.width, a.height, a.stride, a.n_points, a.prev_id, a.next_id, a.prev, a.next,
+                                a.prev_pts, a.next_pts};
+    }
+    const KltBatchOptions o{max_level, max_iter, eps, clahe_clip, tiles_x, tiles_y, border, ransac_threshold, ransac_confidence};
+    KltBatchResults r;
+    TRY(klt_batch_track(h, n, items.data(), o, nullptr, r));
+    bool any_job = false;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_klt_pair &a = pairs[i];
+        const int np = a.n_points;
+        if (np > 0) {
+            memcpy(a.next_pts, r.next + 2 * r.first[i], sizeof(float) * 2 * np);
+            memcpy(a.status, r.status + r.first[i], np);
+            if (a.err) memcpy(a.err, r.err + r.first[i], sizeof(float) * np);
+            if (r.clear[i]) memset(a.status, 0, np);     // getSubset gave up at once, or no model won: the mask is all zero
+        }
+        any_job |= r.mask[i] != nullptr;
+    }
+    if (any_job) {
+        KltBatchState &B = h->kltb;
+        unsigned *h_mw = reinterpret_cast<unsigned *>(B.stage.h + r.o_mw);
+        CK(h, cudaMemcpyAsync(h_mw, B.stage.d + r.o_mw, sizeof(unsigned) * r.words, cudaMemcpyDeviceToHost, h->stream));
+        CK(h, cudaStreamSynchronize(h->stream));
+        for (int i = 0; i < n; ++i) {
+            const pvio_b200_klt_pair &a = pairs[i];
+            if (!r.mask[i]) continue;
+            const unsigned *m = h_mw + (r.mask[i] - reinterpret_cast<const unsigned *>(B.stage.d + r.o_mw));
+            for (int j = 0, k = 0; j < a.n_points; ++j) {
+                if (!a.status[j]) continue;
+                if (!((m[k >> 5] >> (k & 31)) & 1u)) a.status[j] = 0;
+                ++k;
+            }
+        }
+    }
+    for (int i = 0; i < n; ++i)
+        if (pairs[i].info) memcpy(pairs[i].info, &r.info[4 * (size_t)i], sizeof(int32_t) * 4);
+    return 0;
+}
+
+int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchOptions &opt, const KltDevicePoints *dev,
+                    KltBatchResults &res) {
+    const int max_level = opt.max_level, max_iter = opt.max_iter, tiles_x = opt.tiles_x, tiles_y = opt.tiles_y;
+    const int border = opt.border;
+    const double eps = opt.eps, clahe_clip = opt.clahe_clip;
+    res.first.assign(n, 0);
+    res.mask.assign(n, nullptr);
+    res.clear.assign(n, 0);
+    res.info.assign(4 * (size_t)n, 0);
+    if (max_level < 0 || max_level >= kMaxLevels || border < 0 || !(clahe_clip >= 0.0))
         return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad arguments");
     const bool do_clahe = clahe_clip > 0.0;
     if (do_clahe && (tiles_x < 1 || tiles_y < 1)) return fail(h, PVIO_B200_EINVAL, "clahe: bad tile grid");
@@ -523,25 +578,26 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     const KltPyramids empty;
     size_t n_pts = 0;
     for (int i = 0; i < n; ++i) {
-        const pvio_b200_klt_pair &a = pairs[i];
+        const KltBatchItem &a = pairs[i];
         if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: slot out of range");
         if ((size_t)a.slot >= taken.size()) taken.resize(a.slot + 1, 0);
         if (taken[a.slot]) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: a slot appears twice");
         taken[a.slot] = 1;
-        if (a.width < kKltMinFrame || a.height < kKltMinFrame || a.stride < a.width || !a.prev_id || !a.next_id)
+        if (a.width < kKltMinFrame || a.height < kKltMinFrame || a.stride < a.width || !a.next_id)
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad shape, stride or frame id");
         if (do_clahe && (a.width % tiles_x || a.height % tiles_y))
             return fail(h, PVIO_B200_EINVAL, "clahe: the image size must be a multiple of the tile grid");
         const SlotLens *L = slot_lens(B, a.slot);
         if (L && (L->w != a.width || L->h != a.height))
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: the frame shape differs from the slot's lens");
-        if (a.n_points < 0 || (a.n_points > 0 && (!a.prev_pts || !a.next_pts || !a.status)))
+        if (a.n_points < 0 || (a.n_points > 0 && !dev && (!a.prev_pts || !a.next_pts)) || (a.n_points > 0 && !a.prev_id))
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad points");
         Plan &pl = plan[i];
         pl.levels = klt_levels(a.width, a.height, max_level);
         const KltPyramids *c = (size_t)a.slot < B.slots.size() ? &B.slots[a.slot] : nullptr;
         pl.rebuild = !c || c->w != a.width || c->h != a.height || c->levels != pl.levels;
         klt_lookup(pl.rebuild ? empty : *c, a.prev_id, a.next_id, clahe_clip, pl.slot, pl.have);
+        if (!a.prev_id) pl.have[0] = true;    // no previous frame: the next frame is only cached
         if ((!pl.have[0] && !a.prev) || (!pl.have[1] && !a.next))
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: image not cached in its slot and no pixels given");
         n_pts += a.n_points;
@@ -549,7 +605,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     if (n_pts > ((size_t)1 << 28)) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: too many points");
 
     // the slots: grown on demand, rebuilt on a shape change; per pair its RANSAC budget (iterations reserved)
-    double thr = ransac_threshold, conf = ransac_confidence;
+    double thr = opt.ransac_threshold, conf = opt.ransac_confidence;
     int fm_iters = kFmIters;
     fm_options(thr, conf, fm_iters);
     const int lmeds_iters = fm_lmeds_iters(conf, fm_iters);
@@ -558,7 +614,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     size_t n_frames = 0, pix_bytes = 0, budget_sum = 0, words_sum = 0, mask_words = 0, n_lens = 0, und_bytes = 0;
     int max_budget = 0, max_words = 0, lens_w = 0, lens_h = 0;
     for (int i = 0; i < n; ++i) {
-        const pvio_b200_klt_pair &a = pairs[i];
+        const KltBatchItem &a = pairs[i];
         const Plan &pl = plan[i];
         KltPyramids &s = B.slots[a.slot];
         if (pl.rebuild) {
@@ -620,7 +676,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     float *h_prev = reinterpret_cast<float *>(hs + o_prev), *h_next = reinterpret_cast<float *>(hs + o_next);
     size_t p = 0, f_lens = 0, f_plain = n_lens, pix = 0, und = 0, bsum = 0, msum = 0;
     for (int i = 0; i < n; ++i) {
-        const pvio_b200_klt_pair &a = pairs[i];
+        const KltBatchItem &a = pairs[i];
         const Plan &pl = plan[i];
         KltPyramids &s = B.slots[a.slot];
         const SlotLens *L = slot_lens(B, a.slot);
@@ -640,12 +696,15 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
             }
             pix += align256((size_t)a.width * a.height);
         }
-        s.pyr_id[pl.slot[0]] = a.prev_id; s.pyr_clahe[pl.slot[0]] = clahe_clip;
+        if (a.prev_id) { s.pyr_id[pl.slot[0]] = a.prev_id; s.pyr_clahe[pl.slot[0]] = clahe_clip; }
         s.pyr_id[pl.slot[1]] = a.next_id; s.pyr_clahe[pl.slot[1]] = clahe_clip;
         const int np = a.n_points;
+        res.first[i] = p;
         if (np > 0) {
-            memcpy(h_prev + 2 * p, a.prev_pts, sizeof(float) * 2 * np);
-            memcpy(h_next + 2 * p, a.next_pts, sizeof(float) * 2 * np);
+            if (!dev) {
+                memcpy(h_prev + 2 * p, a.prev_pts, sizeof(float) * 2 * np);
+                memcpy(h_next + 2 * p, a.next_pts, sizeof(float) * 2 * np);
+            }
             std::fill(pof + p, pof + p + np, i);
         }
         FmBatchProblem &P = fmp[i];
@@ -667,7 +726,11 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
     }
 
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(ds, hs, o_err, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(ds, hs, dev ? o_prev : o_err, cudaMemcpyHostToDevice, st));
+    if (dev && n_pts > 0) {
+        TRY(dev->write_points(h, reinterpret_cast<float *>(ds + o_prev), reinterpret_cast<float *>(ds + o_next),
+                              reinterpret_cast<const int *>(ds + o_pof)));
+    }
     if (n_lens > 0) undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_lens, lens_w, lens_h);
     if (n_frames > 0)
         TRY(klt_build_pyramids(h, frm, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_frames, do_clahe, tiles_x, tiles_y));
@@ -681,27 +744,25 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
         fm_batch_hypotheses(h, d_fmp, n, max_budget, (float)(thr * thr));
     }
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(hs + o_next, ds + o_next, o_mw - o_next, cudaMemcpyDeviceToHost, st));
+    // with the points on the device, only what the replay reads comes back
+    const size_t o_down = dev ? o_surv : o_next;
+    CK(h, cudaMemcpyAsync(hs + o_down, ds + o_down, o_mw - o_down, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
 
-    // LK results out; each pair's replay (opencv_image.cpp:112-129: findFundamentalMat over >= 8 survivors)
-    const float *r_next = reinterpret_cast<const float *>(hs + o_next), *r_err = reinterpret_cast<const float *>(hs + o_err);
-    const uint8_t *r_st = hs + o_st;
+    // each pair's replay (opencv_image.cpp:112-129: findFundamentalMat over >= 8 survivors)
     const int *r_surv = reinterpret_cast<const int *>(hs + o_surv), *r_cnt = reinterpret_cast<const int *>(hs + o_cnt);
     FmMaskJob *jobs = reinterpret_cast<FmMaskJob *>(hs + o_job);
-    std::vector<int32_t> info(4 * (size_t)n);
+    res.next = reinterpret_cast<const float *>(dev ? ds + o_next : hs + o_next);
+    res.err = reinterpret_cast<const float *>(dev ? ds + o_err : hs + o_err);
+    res.status = dev ? ds + o_st : hs + o_st;
+    res.o_mw = o_mw;
+    res.words = words_sum;
     bool any_job = false;
-    p = 0; bsum = 0;
+    bsum = 0;
     size_t wsum = 0;
     for (int i = 0; i < n; ++i) {
-        const pvio_b200_klt_pair &a = pairs[i];
-        const int np = a.n_points;
-        if (np > 0) {
-            memcpy(a.next_pts, r_next + 2 * p, sizeof(float) * 2 * np);
-            memcpy(a.status, r_st + p, np);
-            if (a.err) memcpy(a.err, r_err + p, sizeof(float) * np);
-        }
-        int32_t *inf = &info[4 * (size_t)i];
+        const int np = pairs[i].n_points;
+        int32_t *inf = &res.info[4 * (size_t)i];
         inf[0] = 0; inf[1] = -1; inf[2] = -1; inf[3] = 0;
         FmMaskJob &J = jobs[i];
         memset(&J, 0, sizeof(J));
@@ -716,12 +777,12 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
                 J.out = reinterpret_cast<unsigned *>(ds + o_mw) + wsum;
                 if (s >= 15) J.src = P.masks + (size_t)(3 * bi + bk) * ((s + 31) / 32);
                 else { J.F = P.F + (size_t)(3 * bi + bk) * 9; J.thr2 = thr_lmeds; }
+                res.mask[i] = J.out;
                 any_job = true;
             } else {
-                memset(a.status, 0, np);     // getSubset gave up at once, or no model won: the mask is all zero
+                res.clear[i] = 1;             // getSubset gave up at once, or no model won: the mask is all zero
             }
         }
-        p += np;
         bsum += budget[i];
         wsum += (np + 31) / 32;
     }
@@ -730,25 +791,7 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
         CK(h, cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_jobs), jobs, 0));
         fm_batch_masks(h, d_jobs, n, max_words);
         CK(h, cudaGetLastError());
-        CK(h, cudaMemcpyAsync(hs + o_mw, ds + o_mw, sizeof(unsigned) * words_sum, cudaMemcpyDeviceToHost, st));
-        CK(h, cudaStreamSynchronize(st));
-        const unsigned *r_mw = reinterpret_cast<const unsigned *>(hs + o_mw);
-        wsum = 0;
-        for (int i = 0; i < n; ++i) {
-            const pvio_b200_klt_pair &a = pairs[i];
-            if (jobs[i].n > 0) {
-                const unsigned *m = r_mw + wsum;
-                for (int j = 0, r = 0; j < a.n_points; ++j) {
-                    if (!a.status[j]) continue;
-                    if (!((m[r >> 5] >> (r & 31)) & 1u)) a.status[j] = 0;
-                    ++r;
-                }
-            }
-            wsum += (a.n_points + 31) / 32;
-        }
     }
-    for (int i = 0; i < n; ++i)
-        if (pairs[i].info) memcpy(pairs[i].info, &info[4 * (size_t)i], sizeof(int32_t) * 4);
     return 0;
 }
 
