@@ -500,6 +500,60 @@ typedef struct pvio_b200_window_track_frame {
 /* n records, each naming a different resident slot; opt (may be NULL) is shared by the PnP solves. */
 int pvio_b200_batch_window_track_frame(pvio_b200_handle h, int n, pvio_b200_window_track_frame *records,
                                        const pvio_b200_options *opt);
+/* Plane detection on resident slots, from each slot's own track table: per record one Ransac<3, PlaneState,
+ * PlaneSolver, PlaneEvaluator> (utility/ransac.h) over the points of its candidate tracks, then the inliers' plane.
+ *  - mode PVIO_B200_PLANE_EXTRACT is PlaneExtractor::work (plane_extractor.cpp:40-81): a candidate's point is
+ *    Track::get_landmark_point() from the slot row (the arithmetic of pvio_b200_batch_window_localize); threshold 0.03;
+ *    the RANSAC runs on 3 or more points.
+ *  - mode PVIO_B200_PLANE_REFIT is Plane::update_parameter(true) (plane.cpp:64-114): a candidate's point is
+ *    Track::try_triangulate over the row's observations in the window (track.cpp:61-81: [R | T] per observing frame,
+ *    R = q_cam^*, T = -R p_cam, the parallax / depth < 100 checks of pvio_b200_triangulate); threshold 0.05; fewer than
+ *    50 points run no RANSAC (plane.cpp:74).  A track whose triangulation fails, or that has fewer than two window
+ *    observations, is left out (the reference pushes an uninitialised point, plane.cpp:69-72).
+ *  - Candidates: the caller's track ids in the caller's order, which is the RANSAC's index space: Map order for an
+ *    extraction (not id order: Map::recycle_track swaps with the back), plane->tracks order (id order) for a refit.  The
+ *    caller applies the rules only the map knows: TF_VALID, !TF_PLANE, life >= 10 and quality < 2.0 for an extraction
+ *    (plane_extractor.cpp:45-47); TF_VALID and life >= 15 for a refit (plane.cpp:67).  The device applies
+ *    PlaneExtractor::enough_baseline (plane_extractor.cpp:197-200): Track::compute_baseline over the row's observing
+ *    frames in window order from their body positions (state doubles 4 .. 6), and the row's inverse depth.
+ *  - Everything else is PVIO's: seed 0, confidence 0.999, 1000 iterations (every one evaluated, the serial acceptance
+ *    rule replayed on the host, as pvio_b200_batch_two_view), accepted on more than 30 inliers.  PlaneSolver:
+ *    n = (p2 - p0) x (p1 - p0), Eigen's stableNormalize (a zero cross product stays zero and then counts every point),
+ *    d = p0 . n; an inlier has |p . n - d| <= threshold.
+ *  - plane [7]: normal, distance, reference point.  Accepted: the inliers' centroid (summed serially in candidate order)
+ *    is the reference point, the covariance's eigenvector of smallest eigenvalue the normal, d = n . centroid
+ *    (plane_extractor.cpp:58-77, plane.cpp:78-97); the normal's sign is fixed: d >= 0, and its component of largest
+ *    magnitude positive when d == 0 (the reference leaves the sign to Eigen's QR iterations).  A rejected refit returns
+ *    the winning iteration's raw model, which the reference assigns whatever the count (plane.cpp:77), with a NaN
+ *    reference point.  Otherwise all NaN.
+ * The call reads the slots and writes none of them.  Every record is checked before anything is staged: on
+ * PVIO_B200_EINVAL no output has changed and nothing was launched.  Rejected: more than 65535 records; a slot out of
+ * range or not resident; a mode other than the two; n_tracks < 0; a missing array; an unknown or dead track, or one named
+ * twice in a record.  A slot may be named by several records.  n == 0 is a no-op.  One host -> device copy, three
+ * kernel launches whatever n is (gather and schedule, hypotheses, finish), a download of the counts and one
+ * synchronisation, the replay, one more host -> device copy of the records, one device -> host copy of the results and
+ * one synchronisation; the staging is the slots' (pvio_b200_batch_window_*), grown to the largest call seen. */
+#define PVIO_B200_PLANE_EXTRACT 0
+#define PVIO_B200_PLANE_REFIT 1
+#define PVIO_B200_PLANE_ACCEPTED 0   /* more than 30 inliers                                          */
+#define PVIO_B200_PLANE_FEW_POINTS 1 /* fewer used points than the mode's minimum: no RANSAC          */
+#define PVIO_B200_PLANE_REJECTED 2   /* 30 inliers or fewer                                           */
+typedef struct pvio_b200_window_plane_ransac {
+    int32_t slot;
+    int32_t mode;               /* PVIO_B200_PLANE_EXTRACT or PVIO_B200_PLANE_REFIT */
+    int32_t n_tracks;
+    const int32_t *tracks;      /* [n_tracks] candidate track ids of the slot, in the caller's order */
+    int32_t *info;              /* [5] out: status, points that entered the RANSAC, inliers, iterations run, winning
+                                   iteration (-1: none) */
+    double *plane;              /* [7] out: normal, distance, reference point */
+    uint8_t *used;              /* [n_tracks] out: 1 if the candidate's point entered the RANSAC */
+    uint8_t *inlier;            /* [n_tracks] out: 1 if it is an inlier of the winning model */
+    double *points;             /* [n_tracks][3] or NULL, out: the point used, NaN where the track was left out */
+    int32_t *schedule;          /* [1000][3] or NULL, out: the sample drawn for every evaluated iteration (indices into
+                                   the used points), -1 without a RANSAC */
+    int32_t *counts;            /* [1000] or NULL, out: every evaluated iteration's inlier count, -1 without a RANSAC */
+} pvio_b200_window_plane_ransac; /* 80 bytes on LP64 */
+int pvio_b200_batch_window_plane_ransac(pvio_b200_handle h, int n, const pvio_b200_window_plane_ransac *records);
 
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */

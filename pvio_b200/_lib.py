@@ -24,6 +24,8 @@ IMU_DQ_DBG, IMU_DP_DBG, IMU_DP_DBA, IMU_DV_DBG, IMU_DV_DBA, IMU_BG0, IMU_BA0 = 2
 TERM_CONVERGENCE, TERM_NO_CONVERGENCE, TERM_FAILURE = 0, 1, 2
 TWO_VIEW_OK, TWO_VIEW_FEW_MATCHES, TWO_VIEW_LOW_PARALLAX, TWO_VIEW_PURE_ROTATION, TWO_VIEW_FEW_TRIANGULATED = 0, 1, 2, 3, 4
 LENS_RADTAN, LENS_EQUIDISTANT = 1, 2
+PLANE_EXTRACT, PLANE_REFIT = 0, 1
+PLANE_ACCEPTED, PLANE_FEW_POINTS, PLANE_REJECTED = 0, 1, 2
 
 c_i32p = C.POINTER(C.c_int32)
 c_u8p = C.POINTER(C.c_uint8)
@@ -130,6 +132,12 @@ class CWindowTrackFrame(C.Structure):
                 ("summary", C.POINTER(CSummary))]
 
 
+class CWindowPlaneRansac(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("mode", C.c_int32), ("n_tracks", C.c_int32), ("tracks", c_i32p), ("info", c_i32p),
+                ("plane", c_f64p), ("used", c_u8p), ("inlier", c_u8p), ("points", c_f64p), ("schedule", c_i32p),
+                ("counts", c_i32p)]
+
+
 class CLens(C.Structure):
     _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
@@ -195,6 +203,7 @@ SIGNATURES = {
     "pvio_b200_batch_window_set_imu": (_int, [_h, _int, _P(CWindowImu)]),
     "pvio_b200_batch_window_imu_records": (_int, [_h, _int, c_i32p, c_f64p, _i64]),
     "pvio_b200_batch_window_track_frame": (_int, [_h, _int, _P(CWindowTrackFrame), _P(COptions)]),
+    "pvio_b200_batch_window_plane_ransac": (_int, [_h, _int, _P(CWindowPlaneRansac)]),
     "pvio_b200_sync": (_int, [_h]),
     "pvio_b200_timer_start": (_int, [_h]),
     "pvio_b200_timer_stop": (_int, [_h, c_f32p]),

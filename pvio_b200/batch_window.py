@@ -107,6 +107,18 @@ def _localize_out(L):
                 inv_depth=np.zeros(len(L.new)), inv_depth_next=np.zeros(len(L.new)))
 
 
+class PlaneRansac:
+    """One plane RANSAC on one slot (pvio_b200_window_plane_ransac): mode EXTRACT (PlaneExtractor::work, the candidates'
+    landmark points) or REFIT (Plane::update_parameter(true), the candidates triangulated over their window views), and
+    the candidate track ids in the caller's order (Map order for an extraction, plane->tracks order for a refit)."""
+
+    EXTRACT, REFIT = _lib.PLANE_EXTRACT, _lib.PLANE_REFIT
+
+    def __init__(self, slot, mode, tracks):
+        self.slot, self.mode = int(slot), int(mode)
+        self.tracks = np.ascontiguousarray(tracks, dtype=np.int32).reshape(-1)
+
+
 class Imu:
     """The raw samples of one IMU factor of one slot (pvio_b200_window_imu): window frame j >= 1 (the factor (j - 1, j)),
     samples [K][7] (t, w xyz, a xyz), t_end (the time of frame j) and noise_cov (cov_w, cov_a, cov_bg, cov_ba, 3x3 each
@@ -246,6 +258,32 @@ class BatchWindows:
             keep += [T.samples, T.noise] + ([] if T.merge is None else [T.merge])
             _localize_fields(r, T, o, keep)
         return recs, sms, out, keep
+
+    def plane_ransac(self, records, schedules=False):
+        """Run a list of PlaneRansac in one call (a slot may be named by several); the slots do not change.  Per record
+        a dict: status (PLANE_ACCEPTED, PLANE_FEW_POINTS or PLANE_REJECTED), n_points, inliers, iterations, best_it,
+        normal [3], distance, reference [3], and per candidate used, inlier (bool) and point [3] (NaN: left out).
+        schedules: also the sample schedule [1000, 3] and every iteration's inlier count [1000] (-1 without a RANSAC)."""
+        n = len(records)
+        recs, out = (_lib.CWindowPlaneRansac * max(n, 1))(), []
+        for r, P in zip(recs, records):
+            m = len(P.tracks)
+            o = dict(info=np.zeros(5, dtype=np.int32), plane=np.zeros(7), used=np.zeros(m, dtype=np.uint8),
+                     inlier=np.zeros(m, dtype=np.uint8), points=np.zeros((m, 3)), tracks=P.tracks)
+            if schedules:
+                o.update(schedule=np.zeros((1000, 3), dtype=np.int32), counts=np.zeros(1000, dtype=np.int32))
+            out.append(o)
+            r.slot, r.mode, r.n_tracks = P.slot, P.mode, m
+            _lib.set_ptrs(r, tracks=P.tracks, info=o["info"], plane=o["plane"], used=o["used"], inlier=o["inlier"],
+                          points=o["points"], schedule=o.get("schedule"), counts=o.get("counts"))
+        self.ba._ck(self.lib.pvio_b200_batch_window_plane_ransac(self.h, n, recs))
+        for o in out:
+            i, p = o.pop("info"), o.pop("plane")
+            o.pop("tracks")
+            o.update(status=int(i[0]), n_points=int(i[1]), inliers=int(i[2]), iterations=int(i[3]), best_it=int(i[4]),
+                     normal=p[:3].copy(), distance=float(p[3]), reference=p[4:].copy(),
+                     used=o["used"].astype(bool), inlier=o["inlier"].astype(bool))
+        return out
 
     def set_imu(self, records):
         """Keep the samples of a list of Imu on the device with their factors, in one call."""

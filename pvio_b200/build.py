@@ -17,7 +17,8 @@ def _extra(name):
     """per-file flags: OpenCV's float rounding and the reference's uncontracted fp64 on the device (no contraction);
     undistort.cu's host-side map builder without fused multiply-adds, which GCC forms by default where the target has
     them (aarch64)"""
-    if name.endswith(("klt.cu", "detect.cu", "fmat.cu", "twoview.cu", "feature_track.cu")):
+    if name.endswith(("klt.cu", "detect.cu", "fmat.cu", "twoview.cu", "feature_track.cu",
+                             "plane_ransac.cu")):
         return ["-fmad=false"]
     if name.endswith("undistort.cu"):
         return ["-Xcompiler", "-ffp-contract=off"]

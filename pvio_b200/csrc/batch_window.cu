@@ -27,8 +27,8 @@
 #include <vector>
 
 #include "api_internal.h"
+#include "batch_window.cuh"
 #include "imu.cuh"
-#include "quat.cuh"
 #include "tri.cuh"
 
 namespace pvio {
@@ -54,42 +54,6 @@ struct BwImu {                                    // a factor with samples: n ro
     __device__ int end() const { return off + n; }
 };
 constexpr int kImuAux = 37;                                             // per factor: t_end, noise [4][9]
-
-// the handle's arrays (the plane tables null until a slot has plane tracks), the track table and the post-pass results
-struct BwArgs : BatchArrays {
-    int32_t *tid;
-    uint32_t *tmask;
-    double *trho;
-    double2 *tz;
-    uint8_t *tvalid;
-    double *tqual;
-    int8_t *trole;
-    double *tplane;
-    int32_t *lm_row;
-    const uint8_t *valid;
-    const double *quality;
-    double *imu_s, *imu_aux;
-    int Scap;
-};
-
-constexpr int kBwThreads = 256;
-constexpr int kBwWarps = kBwThreads / 32;
-
-// exclusive scan of one int per thread over the CTA (kBwThreads); total: the sum
-__device__ int bw_block_scan(int v, int *sh, int &total) {
-    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) sh[wv] = x;
-    __syncthreads();
-    if (threadIdx.x == 0) { int s = 0; for (int k = 0; k < kBwWarps; ++k) { const int t = sh[k]; sh[k] = s; s += t; } sh[kBwWarps] = s; }
-    __syncthreads();
-    const int r = sh[wv] + x - v;
-    total = sh[kBwWarps];
-    __syncthreads();
-    return r;
-}
 
 // stable compaction of rows [0, T) of window w to the rows whose frame mask is not 0; returns the live count.  A row only
 // moves down, chunk by chunk: each chunk is read completely before it is written.
@@ -340,20 +304,6 @@ __global__ void __launch_bounds__(kBwThreads) bw_planes_kernel(BwArgs a, const B
     }
 }
 
-__device__ void bw_cam_pose(const double *fs, const WinConst &c, double *qc, double *pc) {
-    bw_qmul(fs, c.cam_q, qc);
-    double t[3];
-    bw_qrot(fs, c.cam_p, t);
-    for (int i = 0; i < 3; ++i) pc[i] = fs[4 + i] + t[i];
-}
-// the world point at inverse depth rho along keypoint (zx, zy) of the camera at pose (qc, pc) (Track::get_landmark_point)
-__device__ __forceinline__ void bw_world_point(const double *qc, const double *pc, double zx, double zy, double rho,
-                                               double *x) {
-    const double ray[3] = {zx / rho, zy / rho, 1.0 / rho};
-    double y[3];
-    bw_qrot(qc, ray, y);
-    for (int i = 0; i < 3; ++i) x[i] = y[i] + pc[i];
-}
 // the inverse depth of world point x in the camera at pose (qc, pc)
 __device__ __forceinline__ double bw_inv_depth(const double *qc, const double *pc, const double *x) {
     const double qi[4] = {-qc[0], -qc[1], -qc[2], qc[3]};
@@ -533,13 +483,7 @@ __global__ void __launch_bounds__(kLocGatherThreads) bw_localize_gather_kernel(B
         const int k = r.obs_off + i;
         double *x = L.pts + 3 * (size_t)k;
         if (!isnan(x[0])) continue;
-        const size_t R = base + L.row[k];
-        const int an = __ffs(a.tmask[R]) - 1;
-        const double2 z = a.tz[R * a.Ncap + an];
-        const double rho = a.trho[R];
-        double qc[4], pc[3];
-        bw_cam_pose(fr + an * kFrameStride, c, qc, pc);
-        bw_world_point(qc, pc, z.x, z.y, rho, x);
+        bw_landmark_point(a, base + L.row[k], fr, c, x);
     }
     if (threadIdx.x == 0) {
         PnpArgs p{};                      // what batch_pnp_solve_impl stages for the same problem
@@ -554,20 +498,6 @@ __global__ void __launch_bounds__(kLocGatherThreads) bw_localize_gather_kernel(B
         p.out = L.out + 8 * (size_t)blockIdx.x;
         L.args[blockIdx.x] = p;
     }
-}
-
-// the camera matrix [R | T] of a camera pose (R = q^-1, T = -R p, track.cpp:90-95), row-major 3 x 4
-__device__ void loc_camera_matrix(const double *qc, const double *pc, double *P) {
-    const double qi[4] = {-qc[0], -qc[1], -qc[2], qc[3]};
-    for (int j = 0; j < 3; ++j) {
-        const double e[3] = {j == 0 ? 1.0 : 0.0, j == 1 ? 1.0 : 0.0, j == 2 ? 1.0 : 0.0};
-        double col[3];
-        bw_qrot(qi, e, col);
-        for (int i = 0; i < 3; ++i) P[4 * i + j] = col[i];
-    }
-    double t[3];
-    bw_qrot(qi, pc, t);
-    for (int i = 0; i < 3; ++i) P[4 * i + 3] = -t[i];
 }
 
 struct LocViews {                     // the two views of a new track: the newest slot frame, then the new frame
@@ -799,57 +729,6 @@ static int ensure_imu_store(Handle *h, int S) {
     return 0;
 }
 
-// One call's staging in BatchWindows::stage.  Sections are declared by kind and size, then laid out kind after kind in
-// the order of Kind, each 8-byte aligned, so that the call copies upload + in/out to the device in one copy and in/out +
-// download back in one copy; scratch stays on the device.
-struct Stage {
-    enum Kind { kUp, kInOut, kDown, kScratch, kKinds };
-    template <typename T>
-    struct Sec { int i; };
-    struct Entry { Kind kind; size_t bytes; const void *src; size_t off; };
-    std::vector<Entry> secs;
-    size_t end[kKinds] = {};                  // after place: the end of each kind's sections
-    uint8_t *hp = nullptr, *dp = nullptr;
-
-    // n elements of kind k; src (n elements, or null): what place copies into the section
-    template <typename T>
-    Sec<T> add(Kind k, size_t n, const T *src = nullptr) {
-        secs.push_back(Entry{k, sizeof(T) * n, src, 0});
-        return Sec<T>{(int)secs.size() - 1};
-    }
-    template <typename T>
-    Sec<T> up(const std::vector<T> &v) { return add(kUp, v.size(), v.data()); }
-    template <typename T>
-    T *host(Sec<T> s) const { return reinterpret_cast<T *>(hp + secs[s.i].off); }
-    template <typename T>
-    T *dev(Sec<T> s) const { return reinterpret_cast<T *>(dp + secs[s.i].off); }
-
-    // lays the sections out, grows BatchWindows::stage to them and copies the sources into its host side; upload_now:
-    // then uploads (a call that fills host sections itself uploads after that)
-    int place(Handle *h, bool upload_now = false) {
-        size_t o = 0;
-        for (int k = 0; k < kKinds; ++k) {
-            for (Entry &e : secs)
-                if (e.kind == k) { e.off = o; o += (e.bytes + 7) & ~(size_t)7; }
-            end[k] = o;
-        }
-        TRY(reserve(h, h->bw.stage, o, kBoth));
-        hp = h->bw.stage.h; dp = h->bw.stage.d;
-        for (const Entry &e : secs)
-            if (e.src && e.bytes) memcpy(hp + e.off, e.src, e.bytes);
-        return upload_now ? upload(h) : 0;
-    }
-    int upload(Handle *h) const {
-        if (end[kInOut] > 0) CK(h, cudaMemcpyAsync(dp, hp, end[kInOut], cudaMemcpyHostToDevice, h->stream));
-        return 0;
-    }
-    int download(Handle *h) const {
-        if (end[kDown] > end[kUp])
-            CK(h, cudaMemcpyAsync(hp + end[kUp], dp + end[kUp], end[kDown] - end[kUp], cudaMemcpyDeviceToHost, h->stream));
-        return 0;
-    }
-};
-
 // the window of a slot as the checks and the launch shapes see it; T / O: plane tracks and their observations
 struct BwShape { int M = 0, K = 0, chunks = 0, max_obs = 0, T = 0, O = 0; };
 static BwShape shape_of(const WinSlot &s) {
@@ -950,11 +829,6 @@ static int check_slots(Handle *h, int n, const int32_t *slots, const char *what)
         seen[s] = 1;
     }
     return 0;
-}
-
-static int find_row(const WinSlot &s, int32_t id) {
-    const auto it = std::lower_bound(s.ids.begin(), s.ids.end(), id);
-    return (it == s.ids.end() || *it != id) ? -1 : (int)(it - s.ids.begin());
 }
 
 // BundleAdjustor::solve on the n slots of a list; post: then the landmark post-pass

@@ -1,0 +1,150 @@
+// The pieces of the resident batched windows (batch_window.cu) that other calls on the slots share: the kernels' view of
+// the track table, the CTA scan, the camera pose and world point of a slot row, the staging of a call, and the row of a
+// track id in a slot's host mirror.  Used by batch_window.cu and plane_ransac.cu.
+#pragma once
+
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
+#include "api_internal.h"
+#include "quat.cuh"
+
+namespace pvio {
+
+// the handle's arrays (the plane tables null until a slot has plane tracks), the track table and the post-pass results
+struct BwArgs : BatchArrays {
+    int32_t *tid;
+    uint32_t *tmask;
+    double *trho;
+    double2 *tz;
+    uint8_t *tvalid;
+    double *tqual;
+    int8_t *trole;
+    double *tplane;
+    int32_t *lm_row;
+    const uint8_t *valid;
+    const double *quality;
+    double *imu_s, *imu_aux;
+    int Scap;
+};
+
+constexpr int kBwThreads = 256;
+constexpr int kBwWarps = kBwThreads / 32;
+
+// exclusive scan of one int per thread over the CTA (kBwThreads); total: the sum
+__device__ inline int bw_block_scan(int v, int *sh, int &total) {
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) sh[wv] = x;
+    __syncthreads();
+    if (threadIdx.x == 0) { int s = 0; for (int k = 0; k < kBwWarps; ++k) { const int t = sh[k]; sh[k] = s; s += t; } sh[kBwWarps] = s; }
+    __syncthreads();
+    const int r = sh[wv] + x - v;
+    total = sh[kBwWarps];
+    __syncthreads();
+    return r;
+}
+
+// the kernels' view of the handle's arrays and the track table
+template <>
+BwArgs launch_args<BwArgs>(const Handle *h);
+
+__device__ inline void bw_cam_pose(const double *fs, const WinConst &c, double *qc, double *pc) {
+    bw_qmul(fs, c.cam_q, qc);
+    double t[3];
+    bw_qrot(fs, c.cam_p, t);
+    for (int i = 0; i < 3; ++i) pc[i] = fs[4 + i] + t[i];
+}
+// the world point at inverse depth rho along keypoint (zx, zy) of the camera at pose (qc, pc) (Track::get_landmark_point)
+__device__ __forceinline__ void bw_world_point(const double *qc, const double *pc, double zx, double zy, double rho,
+                                               double *x) {
+    const double ray[3] = {zx / rho, zy / rho, 1.0 / rho};
+    double y[3];
+    bw_qrot(qc, ray, y);
+    for (int i = 0; i < 3; ++i) x[i] = y[i] + pc[i];
+}
+// Track::get_landmark_point() of track-table row R of the slot whose frames are fr: its anchor (lowest) frame's camera
+// pose applied to the anchor keypoint at the row's inverse depth
+__device__ __forceinline__ void bw_landmark_point(const BwArgs &a, size_t R, const double *fr, const WinConst &c, double *x) {
+    const int an = __ffs(a.tmask[R]) - 1;
+    const double2 z = a.tz[R * a.Ncap + an];
+    const double rho = a.trho[R];
+    double qc[4], pc[3];
+    bw_cam_pose(fr + an * kFrameStride, c, qc, pc);
+    bw_world_point(qc, pc, z.x, z.y, rho, x);
+}
+// the camera matrix [R | T] of a camera pose (R = q^-1, T = -R p, track.cpp:90-95), row-major 3 x 4
+__device__ inline void loc_camera_matrix(const double *qc, const double *pc, double *P) {
+    const double qi[4] = {-qc[0], -qc[1], -qc[2], qc[3]};
+    for (int j = 0; j < 3; ++j) {
+        const double e[3] = {j == 0 ? 1.0 : 0.0, j == 1 ? 1.0 : 0.0, j == 2 ? 1.0 : 0.0};
+        double col[3];
+        bw_qrot(qi, e, col);
+        for (int i = 0; i < 3; ++i) P[4 * i + j] = col[i];
+    }
+    double t[3];
+    bw_qrot(qi, pc, t);
+    for (int i = 0; i < 3; ++i) P[4 * i + 3] = -t[i];
+}
+
+// One call's staging in BatchWindows::stage.  Sections are declared by kind and size, then laid out kind after kind in
+// the order of Kind, each 8-byte aligned, so that the call copies upload + in/out to the device in one copy and in/out +
+// download back in one copy; scratch stays on the device.
+struct Stage {
+    enum Kind { kUp, kInOut, kDown, kScratch, kKinds };
+    template <typename T>
+    struct Sec { int i; };
+    struct Entry { Kind kind; size_t bytes; const void *src; size_t off; };
+    std::vector<Entry> secs;
+    size_t end[kKinds] = {};                  // after place: the end of each kind's sections
+    uint8_t *hp = nullptr, *dp = nullptr;
+
+    // n elements of kind k; src (n elements, or null): what place copies into the section
+    template <typename T>
+    Sec<T> add(Kind k, size_t n, const T *src = nullptr) {
+        secs.push_back(Entry{k, sizeof(T) * n, src, 0});
+        return Sec<T>{(int)secs.size() - 1};
+    }
+    template <typename T>
+    Sec<T> up(const std::vector<T> &v) { return add(kUp, v.size(), v.data()); }
+    template <typename T>
+    T *host(Sec<T> s) const { return reinterpret_cast<T *>(hp + secs[s.i].off); }
+    template <typename T>
+    T *dev(Sec<T> s) const { return reinterpret_cast<T *>(dp + secs[s.i].off); }
+
+    // lays the sections out, grows BatchWindows::stage to them and copies the sources into its host side; upload_now:
+    // then uploads (a call that fills host sections itself uploads after that)
+    int place(Handle *h, bool upload_now = false) {
+        size_t o = 0;
+        for (int k = 0; k < kKinds; ++k) {
+            for (Entry &e : secs)
+                if (e.kind == k) { e.off = o; o += (e.bytes + 7) & ~(size_t)7; }
+            end[k] = o;
+        }
+        TRY(reserve(h, h->bw.stage, o, kBoth));
+        hp = h->bw.stage.h; dp = h->bw.stage.d;
+        for (const Entry &e : secs)
+            if (e.src && e.bytes) memcpy(hp + e.off, e.src, e.bytes);
+        return upload_now ? upload(h) : 0;
+    }
+    int upload(Handle *h) const {
+        if (end[kInOut] > 0) CK(h, cudaMemcpyAsync(dp, hp, end[kInOut], cudaMemcpyHostToDevice, h->stream));
+        return 0;
+    }
+    int download(Handle *h) const {
+        if (end[kDown] > end[kUp])
+            CK(h, cudaMemcpyAsync(hp + end[kUp], dp + end[kUp], end[kDown] - end[kUp], cudaMemcpyDeviceToHost, h->stream));
+        return 0;
+    }
+};
+
+// the row of track `id` in a slot's host mirror, -1 for an unknown or dead track
+inline int find_row(const WinSlot &s, int32_t id) {
+    const auto it = std::lower_bound(s.ids.begin(), s.ids.end(), id);
+    return (it == s.ids.end() || *it != id) ? -1 : (int)(it - s.ids.begin());
+}
+
+}  // namespace pvio

@@ -15,10 +15,19 @@ from . import so3, synth
 
 
 class Run:
-    def __init__(self, F=26, N=6, M=260, seed=700, planes=0):
-        """planes > 0: synth.make_cfg3(planes=...) over the long run; its plane tracks follow the landmarks in `tracks`"""
-        self.F, self.N = F, N
-        self.w, self.guess, self.truth = synth.make_cfg3(seed=seed, N=F, M=M, prior='none', planes=planes)
+    def __init__(self, F=26, N=6, M=260, seed=700, planes=0, tracks_per_plane=40, plane_landmarks=False):
+        """planes > 0: synth.make_cfg3(planes=..., tracks_per_plane=...) over the long run; its plane tracks follow the
+        landmarks in `tracks`.  plane_landmarks: those tracks stay ordinary landmarks (role -1) whose points lie on the
+        known planes -- what a plane extractor finds before any track is a plane track -- drawn within 6 m and with
+        0.05 px of keypoint noise, and the run starts from its true states, so that the solved points of those tracks
+        stay within the extractor's 3 cm of the plane"""
+        self.F, self.N, self.plane_landmarks = F, N, plane_landmarks
+        self.w, self.guess, self.truth = synth.make_cfg3(seed=seed, N=F, M=M, prior='none', planes=planes,
+                                                         tracks_per_plane=tracks_per_plane,
+                                                         plane_noise_px=0.05 if plane_landmarks else None,
+                                                         plane_range=(1.0, 6.0) if plane_landmarks else (1.0, 15.0))
+        if plane_landmarks:
+            self.guess = self.truth.copy()
         w = self.w
         self.tracks = []                      # per track (landmarks, then plane tracks): sorted frame list and keypoints
         for l in range(w.M):
@@ -41,8 +50,11 @@ class Run:
     def role(self, l, k):
         """The role the host shim gives track l in the window of keyframe k (pvio_b200_window_planes): the plane
         extractor casts every 11th landmark onto a plane from keyframe 3; every 7th plane track is revalidated off its
-        plane at keyframe 5 and stays a landmark; plane 1 has fewer than 20 tracks in keyframes 4 .. 7 (role -2)."""
+        plane at keyframe 5 and stays a landmark; plane 1 has fewer than 20 tracks in keyframes 4 .. 7 (role -2).  With
+        plane_landmarks every track is a landmark."""
         n_planes, p = self.w.n_planes, self.plane_of[l]
+        if self.plane_landmarks:
+            return -1
         if p < 0:
             return (l // 11) % n_planes if n_planes > 0 and l % 11 == 0 and k >= 3 else -1
         if (l - self.w.M) % 7 == 0 and k >= 5:

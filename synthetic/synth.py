@@ -216,10 +216,11 @@ def gauge_prior(w, st):
 
 
 def make_cfg3(seed=649, N=9, M=300, cal=EUROC, planes=0, tracks_per_plane=40, prior='synthetic',
-              kf_dt=0.25, imu_hz=200.0, depth_mix=None):
+              kf_dt=0.25, imu_hz=200.0, depth_mix=None, plane_noise_px=None, plane_range=(1.0, 15.0)):
     """BASELINE config 3 (planes=0) / config 4 (planes=2, TUM-VI calibration): full window
     with reprojection + IMU pre-integration + marginalisation prior (+ plane factors).
-    depth_mix: landmark depths (see _depth_ranges)."""
+    depth_mix: landmark depths (see _depth_ranges).  plane_noise_px: the keypoint noise (px) of the plane tracks,
+    None: the calibration's; plane_range: the distances from the first camera at which plane tracks are drawn"""
     rng = np.random.default_rng(seed)
     w = _base_window(cal, N, use_inertial=True)
     R_wb0 = R_WC0 @ so3.qmat(w.cam_q_cs).T
@@ -287,7 +288,7 @@ def make_cfg3(seed=649, N=9, M=300, cal=EUROC, planes=0, tracks_per_plane=40, pr
     # planes: floor (z = -1.4) and a wall ahead (x = 7), plane tracks seen in 2..N frames
     if planes > 0:
         fx, fy = cal['K'][0], cal['K'][1]
-        s = np.sqrt(cal['noise_px2'])
+        s = np.sqrt(cal['noise_px2']) if plane_noise_px is None else plane_noise_px
         defs = [(np.array([0., 0., 1.]), -1.4), (np.array([1., 0., 0.]), 7.0)][:planes]
         w.n_planes = len(defs)
         w.plane_normal = np.array([d[0] for d in defs])
@@ -307,7 +308,7 @@ def make_cfg3(seed=649, N=9, M=300, cal=EUROC, planes=0, tracks_per_plane=40, pr
                 if abs(den) < 1e-3:
                     continue
                 lam = (dist - nrm @ pc) / den
-                if lam < 1.0 or lam > 15.0:
+                if lam < plane_range[0] or lam > plane_range[1]:
                     continue
                 x = pc + lam * ray
                 zs, ok = [], True
