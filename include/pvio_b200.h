@@ -554,6 +554,101 @@ typedef struct pvio_b200_window_plane_ransac {
     int32_t *counts;            /* [1000] or NULL, out: every evaluated iteration's inlier count, -1 without a RANSAC */
 } pvio_b200_window_plane_ransac; /* 80 bytes on LP64 */
 int pvio_b200_batch_window_plane_ransac(pvio_b200_handle h, int n, const pvio_b200_window_plane_ransac *records);
+/* The link between a resident slot's newest frame and the tracker slot of pvio_b200_batch_feature_track that holds that
+ * frame's keypoints: which keypoint each live track has there.  With the link set, pvio_b200_batch_window_mirror_frame
+ * takes the next camera frame straight from the tracker slot.  A record replaces the slot's link: the tracker slot, the
+ * tracker frame_id of the slot's newest window frame, (track, keypoint index) pairs for the live tracks observed in that
+ * frame (the other tracks have no keypoint there), whether that frame is a keyframe, and the tracker's skipped-frame
+ * counter (sliding_window_tracker.cpp:286).  A shim calls it after seating an initialised window (every frame a
+ * keyframe, initializer.cpp:91-98) and after any host edit that writes the newest frame.
+ * What keeps or clears a link: removal-only edits (prune_tracks), solve, set_planes, set_imu, set_prior and drop_victim
+ * keep it, and each row keeps its keypoint index through the compactions; reset clears it, and so does every other edit
+ * (replace_last, a new frame, new tracks, observations added from the host).  A link names the tracker slot's current
+ * sequence: once batch_feature_track restarts the slot (map_frames == 0), mirror_frame rejects the slot until
+ * set_keypoints links it again, even where frame ids repeat.
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no slot has changed.  Rejected: a slot out of
+ * range, not resident, without frames or named twice; a tracker slot outside 0 .. 65535; frame_id 0 or not one of the
+ * tracker slot's two newest frames (of its current sequence); n < 0; a missing array; an unknown or dead track, one not observed in the newest frame, or one named twice; a keypoint index below 0 or
+ * named twice; newest_is_keyframe not 0 or 1; a negative skipped_frames.  n == 0 is a no-op.  One host -> device copy,
+ * one kernel launch whatever n is, one synchronisation. */
+typedef struct pvio_b200_window_keypoints {
+    int32_t slot;
+    int32_t tracker_slot;             /* the slot of pvio_b200_batch_feature_track holding the newest frame's keypoints */
+    uint64_t frame_id;                /* that frame's id in the tracker slot, != 0 */
+    int32_t n;
+    const int32_t *track;             /* [n] live track ids observed in the newest frame */
+    const int32_t *keypoint;          /* [n] their keypoint index in that frame */
+    int32_t newest_is_keyframe;       /* 0 or 1 */
+    int32_t skipped_frames;           /* >= 0 */
+} pvio_b200_window_keypoints;         /* 48 bytes on LP64 */
+int pvio_b200_batch_window_set_keypoints(pvio_b200_handle h, int n, const pvio_b200_window_keypoints *records);
+/* SlidingWindowTracker::mirror_frame (sliding_window_tracker.cpp:52-73), then the whole per-camera-frame start of
+ * SlidingWindowTracker::track (:75-121) and the frame edit, on linked resident inertial slots, right after
+ * pvio_b200_batch_feature_track advanced their tracker slots.  The host mirrors no keypoint.  Per record:
+ *  1. mirror: the new frame's keypoints kj in order; prev_index[kj] = ki with a row at ki continues that row's track; a
+ *     ki without a row is a new-track candidate (keypoint z_i[ki] in the newest frame, z_j[kj] in the new one); -1 is a
+ *     fresh detection and stays without a track.  The PnP observations and the parallax list follow kj
+ *     (frame->keypoint_num() order, pnp.cpp:56, :269); the candidates follow ki (mirror_frame creates tracks walking
+ *     frame i, :66-71), and the slot's next ids go to the valid ones in that order.
+ *  2. track_frame's steps with these lists and its kernels: integrate and predict from the newest frame, PnP,
+ *     triangulation of the candidates, keyframe check, the merged record behind a non-keyframe newest frame.  PnP
+ *     points: a row of role -1 always takes part, from the slot or from its given point; a row of role -2 or p >= 0
+ *     only with a given point (the plane-cast point, pnp.cpp:62-85), otherwise it is left out.  The one difference from
+ *     track_frame: every continued track and every candidate enters the parallax list (keyframe_check walks every
+ *     track of frame j, :269-277), not only those the PnP uses.  The merge list behind a non-keyframe newest frame is
+ *     the newest factor's samples, which the slot keeps (keep_samples of the call that appended that frame).
+ *  3. the frame edit: replace_last when the slot's newest frame is not a keyframe; the new frame at the PnP state with
+ *     the edit's IMU record, not fixed; an observation in the new frame for every continued track (a track observed in
+ *     the replaced frame only ends with it, and its keypoint stays without a track); every valid candidate a new track
+ *     anchored in the newest frame (new_inv_depth) with its observation in the new frame, or anchored in the new frame
+ *     (new_inv_depth_next) after replace_last.  keep_samples: the new factor keeps its samples (the merged list after a
+ *     non-keyframe) as pvio_b200_batch_window_set_imu would.  The slot's link moves to the new frame with the keyframe
+ *     decision and the skipped-frame counter.
+ * Outputs: state, predicted, imu_record, keyframe, parallax, n_parallax, skipped_frames and summary as track_frame;
+ * kp_track [n_keypoints of the new frame]: the track each keypoint now observes, or -1; counts [4]: continued tracks,
+ * PnP observations, new-track candidates, new tracks added.
+ * Every record is checked before anything is changed: on PVIO_B200_EINVAL no slot, no tracker slot and no output has
+ * changed.  Rejected: every track_frame rejection that applies (a slot out of range, not resident, visual-only, named
+ * twice; n_samples < 1; a non-finite sample, t_end, noise entry, cx or cy; a missing array); an unknown or dead given
+ * track, one named twice, a non-finite given point; a slot without a link; a tracker slot not the link's, named twice,
+ * or restarted since the link, or whose previous frame is not the slot's newest frame (a frontend that skipped frames, feature_tracker.cpp:70-75:
+ * the shim falls back to track_frame + edit + set_keypoints); max_keypoints below the tracker's keypoint count;
+ * keep_samples not 0 or 1; a non-keyframe newest frame with N < 2 or whose factor holds no samples; a window that the
+ * new frame would take past max_frames; and, after the mirror, a window that would exceed max_landmarks or max_obs if
+ * every candidate turned out valid.  n == 0 is a no-op.  The kernel launches do not depend on n: mirror, integrate +
+ * predict, gather, PnP, triangulation, keyframe check, a download of the counts and the continued rows and one
+ * synchronisation, the capacity check, then append, edit, re-layout, the kept samples (when a record keeps them),
+ * the link, one download of the results and a second synchronisation.  Growing the device sample store (a kept list
+ * longer than any kept before, done before anything is staged) or the plane tables (after the capacity check) adds a
+ * device copy and a synchronisation each. */
+typedef struct pvio_b200_window_mirror {
+    int32_t slot;
+    int32_t tracker_slot;             /* the tracker slot just advanced by pvio_b200_batch_feature_track */
+    int32_t n_samples;                /* >= 1 */
+    int32_t keep_samples;             /* 1: the new factor keeps its samples on the device (as set_imu) */
+    const double *samples;            /* [n_samples][7] t, w xyz, a xyz: the new frame's own samples */
+    double t_end;                     /* the new frame's time */
+    const double *noise_cov;          /* [4][9] cov_w, cov_a, cov_bg, cov_ba */
+    double cx, cy;                    /* principal point of the camera matrix the parallax is measured with */
+    int32_t n_given;
+    const int32_t *given_track;       /* [n_given] live track ids with a given world point */
+    const double *given_point;        /* [n_given][3] */
+    int32_t max_keypoints;            /* capacity of kp_track, >= the new frame's keypoint count */
+    int32_t *kp_track;                /* [max_keypoints] out */
+    int32_t *counts;                  /* [4] or NULL, out */
+    double *state;                    /* [16] out: the PnP solution */
+    double *predicted;                /* [16] or NULL, out */
+    double *imu_record;               /* [PVIO_B200_IMU_STRIDE] or NULL, out: the factor of the frame edit */
+    uint8_t *keyframe;                /* out: 1 if the new frame is a keyframe */
+    double *parallax;                 /* or NULL, out */
+    int32_t *n_parallax;              /* or NULL, out */
+    int32_t *skipped_frames;          /* or NULL, out: the counter after this frame */
+    pvio_b200_summary *summary;       /* or NULL */
+} pvio_b200_window_mirror;            /* 168 bytes on LP64 */
+/* n records, each naming a different resident slot and a different tracker slot; opt (may be NULL) is shared by the
+ * PnP solves. */
+int pvio_b200_batch_window_mirror_frame(pvio_b200_handle h, int n, pvio_b200_window_mirror *records,
+                                        const pvio_b200_options *opt);
 
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */

@@ -138,6 +138,20 @@ class CWindowPlaneRansac(C.Structure):
                 ("counts", c_i32p)]
 
 
+class CWindowKeypoints(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("frame_id", C.c_uint64), ("n", C.c_int32),
+                ("track", c_i32p), ("keypoint", c_i32p), ("newest_is_keyframe", C.c_int32), ("skipped_frames", C.c_int32)]
+
+
+class CWindowMirror(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("n_samples", C.c_int32), ("keep_samples", C.c_int32),
+                ("samples", c_f64p), ("t_end", C.c_double), ("noise_cov", c_f64p), ("cx", C.c_double), ("cy", C.c_double),
+                ("n_given", C.c_int32), ("given_track", c_i32p), ("given_point", c_f64p), ("max_keypoints", C.c_int32),
+                ("kp_track", c_i32p), ("counts", c_i32p), ("state", c_f64p), ("predicted", c_f64p),
+                ("imu_record", c_f64p), ("keyframe", c_u8p), ("parallax", c_f64p), ("n_parallax", c_i32p),
+                ("skipped_frames", c_i32p), ("summary", C.POINTER(CSummary))]
+
+
 class CLens(C.Structure):
     _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
@@ -204,6 +218,8 @@ SIGNATURES = {
     "pvio_b200_batch_window_imu_records": (_int, [_h, _int, c_i32p, c_f64p, _i64]),
     "pvio_b200_batch_window_track_frame": (_int, [_h, _int, _P(CWindowTrackFrame), _P(COptions)]),
     "pvio_b200_batch_window_plane_ransac": (_int, [_h, _int, _P(CWindowPlaneRansac)]),
+    "pvio_b200_batch_window_set_keypoints": (_int, [_h, _int, _P(CWindowKeypoints)]),
+    "pvio_b200_batch_window_mirror_frame": (_int, [_h, _int, _P(CWindowMirror), _P(COptions)]),
     "pvio_b200_sync": (_int, [_h]),
     "pvio_b200_timer_start": (_int, [_h]),
     "pvio_b200_timer_stop": (_int, [_h, c_f32p]),

@@ -130,6 +130,19 @@ class Imu:
         self.noise = np.ascontiguousarray(np.array([np.asarray(c, dtype=np.float64).reshape(9) for c in noise_cov]))
 
 
+class Mirror:
+    """One new camera frame of one linked inertial slot (pvio_b200_window_mirror), right after batch_feature_track
+    advanced its tracker slot: the raw samples [K][7] up to t_end with noise_cov, the principal point, whether the new
+    factor keeps its samples, and the given world points {track id: point [3]} of plane tracks."""
+
+    def __init__(self, slot, tracker_slot, samples, t_end, noise_cov, cx, cy, keep_samples=True, given=None):
+        self.slot, self.tracker_slot = int(slot), int(tracker_slot)
+        self.samples = np.ascontiguousarray(np.asarray(samples, dtype=np.float64).reshape(-1, 7))
+        self.t_end, self.cx, self.cy, self.keep = float(t_end), float(cx), float(cy), bool(keep_samples)
+        self.noise = np.ascontiguousarray(np.array([np.asarray(c, dtype=np.float64).reshape(9) for c in noise_cov]))
+        self.given = dict(given or {})
+
+
 class BatchWindows:
     def __init__(self, ba):
         """ba: a BundleAdjustor (owns the device handle and its max_windows slots)."""
@@ -257,6 +270,53 @@ class BatchWindows:
                           n_parallax=o["n_parallax"])
             keep += [T.samples, T.noise] + ([] if T.merge is None else [T.merge])
             _localize_fields(r, T, o, keep)
+        return recs, sms, out, keep
+
+    def set_keypoints(self, slot, tracker_slot, frame_id, pairs, newest_is_keyframe=True, skipped_frames=0):
+        """Link `slot`'s newest frame to frame `frame_id` of tracker slot `tracker_slot`: pairs {track id: keypoint
+        index in that frame} for the live tracks observed there."""
+        t = np.array(list(pairs), dtype=np.int32)
+        k = np.array([pairs[i] for i in pairs], dtype=np.int32)
+        r = _lib.CWindowKeypoints()
+        r.slot, r.tracker_slot, r.frame_id, r.n = int(slot), int(tracker_slot), int(frame_id), len(t)
+        r.newest_is_keyframe, r.skipped_frames = 1 if newest_is_keyframe else 0, int(skipped_frames)
+        _lib.set_ptrs(r, track=t, keypoint=k)
+        self.ba._ck(self.lib.pvio_b200_batch_window_set_keypoints(self.h, 1, C.byref(r)))
+
+    def mirror_frame(self, records, max_keypoints, max_iterations=10, initial_radius=0.0):
+        """mirror_frame + track_frame + the frame edit of a list of Mirror (distinct slots and tracker slots) in one
+        call.  Per record a dict: kp_track [max_keypoints] (the track of each new-frame keypoint, -1: none; only the
+        tracker's keypoint count is written), counts [4] (continued, PnP observations, candidates, new tracks), state,
+        predicted, imu_record, keyframe, parallax, n_parallax, skipped_frames, summary."""
+        recs, sms, out, keep = self.mirror_records(records, max_keypoints)
+        opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
+        self.ba._ck(self.lib.pvio_b200_batch_window_mirror_frame(self.h, len(records), recs, C.byref(opt)))
+        for i, o in enumerate(out):
+            o["summary"] = _lib.summary(sms[i])
+            o["keyframe"], o["parallax"] = bool(o["keyframe"][0]), float(o["parallax"][0])
+            o["n_parallax"], o["skipped_frames"] = int(o["n_parallax"][0]), int(o["skipped_frames"][0])
+        return out
+
+    @staticmethod
+    def mirror_records(records, max_keypoints):
+        """the ctypes records of a list of Mirror: (records, summaries, output arrays per record, arrays to keep)"""
+        keep, out, n = [], [], len(records)
+        recs, sms = (_lib.CWindowMirror * max(n, 1))(), (_lib.CSummary * max(n, 1))()
+        for i, M in enumerate(records):
+            r = recs[i]
+            o = dict(kp_track=np.full(max_keypoints, -7, dtype=np.int32), counts=np.zeros(4, dtype=np.int32),
+                     state=np.zeros(16), predicted=np.zeros(16), imu_record=np.zeros(_lib.IMU_STRIDE),
+                     keyframe=np.zeros(1, dtype=np.uint8), parallax=np.zeros(1), n_parallax=np.zeros(1, dtype=np.int32),
+                     skipped_frames=np.zeros(1, dtype=np.int32))
+            out.append(o)
+            r.slot, r.tracker_slot, r.n_samples, r.keep_samples = M.slot, M.tracker_slot, len(M.samples), int(M.keep)
+            r.t_end, r.cx, r.cy, r.max_keypoints, r.summary = M.t_end, M.cx, M.cy, int(max_keypoints), C.pointer(sms[i])
+            gt = np.array(list(M.given), dtype=np.int32)
+            gp = np.ascontiguousarray([M.given[t] for t in M.given], dtype=np.float64).reshape(-1, 3)
+            r.n_given = len(gt)
+            keep += [M.samples, M.noise, gt, gp]
+            _lib.set_ptrs(r, samples=M.samples, noise_cov=M.noise, given_track=gt if len(gt) else None,
+                          given_point=gp if len(gt) else None, **{k: o[k] for k in o})
         return recs, sms, out, keep
 
     def plane_ransac(self, records, schedules=False):

@@ -95,7 +95,9 @@ struct SlotLens {
 
 // feature_track.cu: the keypoints of a slot's newest frame (pvio_b200_batch_feature_track), double-buffered so that a
 // call reads buf[cur] and writes buf[1 - cur].  Each buffer: [cap] double2 normalised keypoint, then [cap] int32 birth
-// (the number of the frame that detected it).
+// (the number of the frame that detected it), then [cap] int32 prev_index (the keypoint of the frame before that it
+// continues, or -1).  Right after a call buf[1 - cur] still holds the previous frame's keypoints: the link that
+// pvio_b200_batch_window_mirror_frame reads (batch_window.cu).
 struct SlotKeypoints {
     DevBuf<uint8_t> buf[2];
     size_t cap[2] = {0, 0};                   // keypoints each buffer holds
@@ -103,7 +105,14 @@ struct SlotKeypoints {
     bool live = false;                        // a sequence was started in this slot (map_frames == 0)
     int frame_no = 0;                         // the number of the newest frame (births count in these)
     uint64_t frame_id = 0;                    // its id in the slot's pyramid cache
+    uint64_t prev_frame_id = 0;               // the previous frame's id, 0: none (the newest frame started the sequence)
+    uint32_t gen = 0;                         // sequences started in the slot (map_frames == 0): a window link names one
+    int prev_n = 0;                           // the previous frame's keypoint count (in buf[1 - cur])
     double fx = 0, fy = 0, cx = 0, cy = 0;    // its K
+    static size_t bytes(size_t cap) { return (sizeof(double2) + 2 * sizeof(int)) * cap; }
+    double2 *z(int b) const { return reinterpret_cast<double2 *>(buf[b].d); }
+    int *birth(int b) const { return reinterpret_cast<int *>(buf[b].d + sizeof(double2) * cap[b]); }
+    int *prev(int b) const { return birth(b) + cap[b]; }
 };
 
 // the batched tracker (pvio_b200_batch_track_keypoints): one pyramid cache per sequence slot, grown on demand, and
@@ -180,6 +189,15 @@ struct WinSlot {
                                       // a pack naming it with prior_S == NULL keeps it, a host prior clears it
     std::vector<int32_t> n_samples;   // resident: [Ncap] per IMU factor k (frames k, k + 1) the samples it holds on the
                                       // device, 0: none (it keeps the record its edit gave it)
+    // the link of the newest frame to a tracker slot (pvio_b200_batch_window_set_keypoints / mirror_frame); the device
+    // keeps each row's keypoint index in that frame (BatchWindows::tkp)
+    bool link = false;
+    int link_tracker = -1;            // the tracker slot
+    uint64_t link_frame = 0;          // the tracker's frame id of the newest frame
+    uint32_t link_gen = 0;            // the tracker slot's sequence (SlotKeypoints::gen): frame ids restart with it
+    int link_kmax = -1;               // the largest keypoint index a row holds, -1: none
+    int newest_kf = 1;                // the newest frame is a keyframe
+    int skipped = 0;                  // the tracker's skipped-frame counter (sliding_window_tracker.cpp:286)
 };
 struct BatchWindows {
     DevBuf<int32_t> tid;                         // [W][Mcap] track id of each row
@@ -191,6 +209,8 @@ struct BatchWindows {
     DevBuf<int8_t> trole;                        // [W][Mcap] role of each row (WinSlot::role)
     DevBuf<double> tplane;                       // [W][Pcap][4] plane parameters (normal, distance)
     DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
+    DevBuf<int32_t> tkp;                         // [W][Mcap] keypoint index of each row in the newest frame, -1: none
+                                                 // (meaningful while the slot's link is set, WinSlot::link)
     DevBuf<uint8_t> stage;                       // both sides, grown: every call's staging (batch_window.cu: Stage) --
                                                  // upload | in/out | download | device-only scratch
     // IMU samples of the factors named by set_imu, indexed like imu_data (factor k couples frames k, k + 1); allocated

@@ -65,15 +65,15 @@ __device__ int bw_compact(const BwArgs &a, int w, int T, int *sh) {
         const bool live = r < T && a.tmask[base + r] != 0u;
         int tot;
         const int d = carry + bw_block_scan(live ? 1 : 0, sh, tot);
-        int32_t id = 0; uint32_t m = 0; double rho = 0.0, q = 0.0; uint8_t v = 0; int8_t ro = -1;
+        int32_t id = 0, kp = -1; uint32_t m = 0; double rho = 0.0, q = 0.0; uint8_t v = 0; int8_t ro = -1;
         if (live) {
             id = a.tid[base + r]; m = a.tmask[base + r]; rho = a.trho[base + r]; v = a.tvalid[base + r]; q = a.tqual[base + r];
-            ro = a.trole[base + r];
+            ro = a.trole[base + r]; kp = a.tkp[base + r];
         }
         __syncthreads();
         if (live && d != r) {
             a.tid[base + d] = id; a.tmask[base + d] = m; a.trho[base + d] = rho; a.tvalid[base + d] = v; a.tqual[base + d] = q;
-            a.trole[base + d] = ro;
+            a.trole[base + d] = ro; a.tkp[base + d] = kp;
         }
         __syncthreads();
         for (int f = 0; f < a.Ncap; ++f) {
@@ -85,7 +85,7 @@ __device__ int bw_compact(const BwArgs &a, int w, int T, int *sh) {
         }
         carry += tot;
     }
-    for (int r = carry + threadIdx.x; r < T; r += kBwThreads) { a.tmask[base + r] = 0u; a.trole[base + r] = -1; }
+    for (int r = carry + threadIdx.x; r < T; r += kBwThreads) { a.tmask[base + r] = 0u; a.trole[base + r] = -1; a.tkp[base + r] = -1; }
     __syncthreads();
     return carry;
 }
@@ -687,6 +687,237 @@ __global__ void __launch_bounds__(kBwThreads) bw_track_keyframe_kernel(BwArgs a,
     }
 }
 
+// ------------------------------------------------------------------------ set_keypoints / mirror_frame: the tracker link
+// one set_keypoints record: the slot's T rows, its n (row, keypoint) pairs at off
+struct BwKeys { int32_t slot, T, n, off; };
+
+// One CTA per set_keypoints record: every row without a keypoint in the newest frame, then the named ones
+__global__ void __launch_bounds__(kBwThreads) bw_set_keypoints_kernel(BwArgs a, const BwKeys *recs, const int2 *pairs) {
+    const BwKeys k = recs[blockIdx.x];
+    const size_t base = (size_t)k.slot * a.Mcap;
+    for (int r = threadIdx.x; r < k.T; r += kBwThreads) a.tkp[base + r] = -1;
+    __syncthreads();
+    for (int i = threadIdx.x; i < k.n; i += kBwThreads) { const int2 p = pairs[k.off + i]; a.tkp[base + p.x] = p.y; }
+}
+
+// One record of pvio_b200_batch_window_mirror_frame as staged.  Its lists start at kp_off, the earlier records' new-frame
+// keypoint counts summed (each list holds at most one entry per new-frame keypoint): PnP observations, new-track
+// candidates, parallax pairs, continued rows, kp_track, the edit's new tracks and observations.
+struct BwMirror {
+    const double2 *zi, *zj;           // the tracker slot's previous frame (the slot's newest) and new frame
+    const int32_t *prev;              // the new frame's prev_index
+    int32_t slot, T, n_i, n_j;        // live rows; keypoints of the two frames
+    int32_t tab_off, kp_off, g_off, n_g;          // keypoint tables (2 n_i ints); given points (rows ascending)
+    int32_t rm_off, merge_row, n_merge, replace;  // row map (T ints); the merge list's staged rows
+    int32_t N_old, next_id, pad0, pad1;
+};
+static_assert(sizeof(BwMirror) % sizeof(double) == 0, "records are staged as whole 8-byte words");
+
+// the device view of a mirror_frame call: the mirror's records and lists, and the sections of track_frame's kernels
+// (LocArgs, TrackArgs) and bw_edit_kernel it writes
+struct MirArgs {
+    const BwMirror *rec;
+    BwLoc *loc;              // [n] n_obs, n_new written by the mirror
+    BwTrack *tr;             // [n] n_kf written by the mirror
+    int32_t *tab;            // row of each keypoint of frame i (-1: none), then the new-frame keypoint continuing it
+    const int32_t *grow;     // given points: rows, ascending per record
+    const double *gpt;       //   [3] each
+    int32_t *row;            // LocArgs::row
+    double *z, *pts, *nz;    // LocArgs::z, pts, nz
+    int32_t *kf_row;         // TrackArgs::kf_row
+    double *kf_z, *smp;      // TrackArgs::kf_z, smp (the merge rows are copied from the slot)
+    int2 *cont;              // continued tracks in new-frame order: (row, kj)
+    int32_t *cand;           // the new-frame keypoint of each candidate
+    int32_t *rmap;           // row after the edit's compaction, -1: the track ends with the replaced frame
+    int32_t *lrow;           // row after the edit of each new-frame keypoint, -1: none
+    int32_t *kp;             // kp_track
+    int32_t *cnt;            // [n][4] continued, PnP observations, candidates, new tracks
+    const int32_t *eout;     // bw_edit_kernel's results (live rows at each edit's out_off)
+    int32_t *live;           // [n] live rows after the edit (downloaded)
+    BwEdit *ed;              // [n] host-filled but for n_new, n_obs
+    BwNew *nw;
+    BwObs *ob;
+    double *x;               // [n][16 + kImuStride] the edit's state and IMU record
+    BwLayout *lay;           // [n] the re-layout's records, T written by the append
+};
+constexpr int kMirX = kFrameStride + kImuStride;
+
+// One CTA per record: SlidingWindowTracker::mirror_frame (sliding_window_tracker.cpp:52-73) into the lists track_frame's
+// kernels read.  The slot's keypoint -> row table of the newest frame (frame i) and, for each keypoint of frame i, the
+// new-frame keypoint kj continuing it; then the continued tracks in kj order (the PnP observations, the parallax pairs
+// with a keypoint in frame_i) and the candidates in ki order; the merge list from the slot's newest factor.
+__global__ void __launch_bounds__(kBwThreads) bw_mirror_kernel(BwArgs a, MirArgs M) {
+    __shared__ int sh[kBwWarps + 1];
+    const BwMirror r = M.rec[blockIdx.x];
+    const BwLoc lc = M.loc[blockIdx.x];
+    const BwTrack tk = M.tr[blockIdx.x];
+    const size_t base = (size_t)r.slot * a.Mcap;
+    int *row_of = M.tab + r.tab_off, *kj_of = row_of + r.n_i;
+    for (int k = threadIdx.x; k < r.n_i; k += kBwThreads) { row_of[k] = -1; kj_of[k] = -1; }
+    __syncthreads();
+    for (int q = threadIdx.x; q < r.T; q += kBwThreads) {
+        const int k = a.tkp[base + q];
+        if (k >= 0) row_of[k] = q;
+    }
+    for (int kj = threadIdx.x; kj < r.n_j; kj += kBwThreads) {
+        const int ki = r.prev[kj];
+        if (ki >= 0) kj_of[ki] = kj;
+    }
+    __syncthreads();
+    const uint32_t fi = 1u << tk.frame_i;
+    int nc = 0, np = 0, nk = 0;
+    for (int c0 = 0; c0 < r.n_j; c0 += kBwThreads) {
+        const int kj = c0 + threadIdx.x;
+        const int ki = kj < r.n_j ? r.prev[kj] : -1;
+        const int row = ki >= 0 ? row_of[ki] : -1;
+        int g = -1;
+        bool pnp = false, kf = false;
+        if (row >= 0) {
+            int lo = 0, hi = r.n_g;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (M.grow[r.g_off + mid] < row) lo = mid + 1; else hi = mid;
+            }
+            if (lo < r.n_g && M.grow[r.g_off + lo] == row) g = r.g_off + lo;
+            pnp = a.trole[base + row] == -1 || g >= 0;
+            kf = (a.tmask[base + row] & fi) != 0u;
+        }
+        int tc, tp, tq;
+        const int ic = nc + bw_block_scan(row >= 0 ? 1 : 0, sh, tc);
+        const int ip = np + bw_block_scan(pnp ? 1 : 0, sh, tp);
+        const int iq = nk + bw_block_scan(kf ? 1 : 0, sh, tq);
+        if (row >= 0) {
+            const double2 z = r.zj[kj];
+            M.cont[r.kp_off + ic] = make_int2(row, kj);
+            if (pnp) {
+                const size_t k = (size_t)lc.obs_off + ip;
+                M.row[k] = row;
+                M.z[2 * k] = z.x; M.z[2 * k + 1] = z.y;
+                for (int j = 0; j < 3; ++j) M.pts[3 * k + j] = g >= 0 ? M.gpt[3 * (size_t)g + j] : NAN;
+            }
+            if (kf) {
+                const size_t k = (size_t)tk.kf_off + iq;
+                M.kf_row[k] = row;
+                M.kf_z[2 * k] = z.x; M.kf_z[2 * k + 1] = z.y;
+            }
+        }
+        nc += tc; np += tp; nk += tq;
+    }
+    int nn = 0;
+    for (int c0 = 0; c0 < r.n_i; c0 += kBwThreads) {
+        const int ki = c0 + threadIdx.x;
+        const int kj = ki < r.n_i ? kj_of[ki] : -1;
+        const bool cand = kj >= 0 && row_of[ki] < 0;
+        int tn;
+        const int in = nn + bw_block_scan(cand ? 1 : 0, sh, tn);
+        if (cand) {
+            const size_t k = (size_t)lc.new_off + in;
+            const double2 zi = r.zi[ki], zj = r.zj[kj];
+            M.nz[4 * k] = zi.x; M.nz[4 * k + 1] = zi.y; M.nz[4 * k + 2] = zj.x; M.nz[4 * k + 3] = zj.y;
+            M.cand[k] = kj;
+        }
+        nn += tn;
+    }
+    if (r.n_merge > 0) {                      // the newest factor's samples: factor N - 2 of the slot
+        const double *src = a.imu_s + ((size_t)r.slot * a.Ncap + r.N_old - 2) * a.Scap * 7;
+        for (int i = threadIdx.x; i < 7 * r.n_merge; i += kBwThreads) M.smp[7 * (size_t)r.merge_row + i] = src[i];
+    }
+    if (threadIdx.x == 0) {
+        M.loc[blockIdx.x].n_obs = np; M.loc[blockIdx.x].n_new = nn; M.tr[blockIdx.x].n_kf = nk;
+        int *c = M.cnt + 4 * (size_t)blockIdx.x;
+        c[0] = nc; c[1] = np; c[2] = nn; c[3] = 0;
+    }
+}
+
+// One CTA per record, after track_frame's kernels: the frame edit in bw_edit_kernel's layout.  replace_last follows the
+// slot's newest frame; the continued tracks that outlive it observe the new frame (kj order); the valid candidates (ki
+// order) become the slot's next ids, anchored in the newest frame with their observation in the new one, or anchored in
+// the new frame after replace_last.  kp_track, the rows of the new frame's keypoints after the edit, the edit's state
+// and IMU record, the re-layout's row count.
+__global__ void __launch_bounds__(kBwThreads) bw_mirror_append_kernel(BwArgs a, LocArgs L, TrackArgs T, MirArgs M) {
+    __shared__ int sh[kBwWarps + 1];
+    const int b = blockIdx.x;
+    const BwMirror r = M.rec[b];
+    const BwLoc lc = M.loc[b];
+    const BwEdit e = M.ed[b];
+    const int nc = M.cnt[4 * b];
+    const size_t base = (size_t)r.slot * a.Mcap;
+    const int fnew = e.frame;
+    int32_t *rmap = M.rmap + r.rm_off, *lrow = M.lrow + r.kp_off, *kp = M.kp + r.kp_off;
+    const uint32_t keep = r.replace ? ~(1u << (r.N_old - 1)) : ~0u;
+    int kept = 0;
+    for (int c0 = 0; c0 < r.T; c0 += kBwThreads) {
+        const int q = c0 + threadIdx.x;
+        const bool live = q < r.T && (a.tmask[base + q] & keep) != 0u;
+        int tot;
+        const int d = kept + bw_block_scan(live ? 1 : 0, sh, tot);
+        if (q < r.T) rmap[q] = live ? d : -1;
+        kept += tot;
+    }
+    for (int kj = threadIdx.x; kj < r.n_j; kj += kBwThreads) { lrow[kj] = -1; kp[kj] = -1; }
+    __syncthreads();
+    int no = 0;
+    for (int c0 = 0; c0 < nc; c0 += kBwThreads) {
+        const int i = c0 + threadIdx.x;
+        int row = -1, kj = 0, id = -1;
+        if (i < nc) {
+            const int2 c = M.cont[r.kp_off + i];
+            row = rmap[c.x]; kj = c.y; id = a.tid[base + c.x];
+        }
+        int tot;
+        const int o = no + bw_block_scan(row >= 0 ? 1 : 0, sh, tot);
+        if (row >= 0) {
+            const double2 z = r.zj[kj];
+            M.ob[e.obs_off + o] = BwObs{row, fnew, z.x, z.y};
+            lrow[kj] = row; kp[kj] = id;
+        }
+        no += tot;
+    }
+    int nv = 0;
+    for (int c0 = 0; c0 < lc.n_new; c0 += kBwThreads) {
+        const int t = c0 + threadIdx.x;
+        const bool v = t < lc.n_new && L.valid[lc.new_off + t] != 0;
+        int tot;
+        const int k = nv + bw_block_scan(v ? 1 : 0, sh, tot);
+        if (v) {
+            const size_t q = (size_t)lc.new_off + t;
+            const double *nz = M.nz + 4 * q;
+            const int row = kept + k, kj = M.cand[q];
+            if (r.replace) {
+                M.nw[e.new_off + k] = BwNew{row, r.next_id + k, fnew, 0, nz[2], nz[3], L.rho_next[q]};
+            } else {
+                M.nw[e.new_off + k] = BwNew{row, r.next_id + k, fnew - 1, 0, nz[0], nz[1], L.rho[q]};
+                M.ob[e.obs_off + no + k] = BwObs{row, fnew, nz[2], nz[3]};
+            }
+            lrow[kj] = row; kp[kj] = r.next_id + k;
+        }
+        nv += tot;
+    }
+    double *x = M.x + (size_t)b * kMirX;
+    for (int i = threadIdx.x; i < kFrameStride; i += kBwThreads) x[i] = L.frames[(size_t)b * kFrameStride + i];
+    for (int i = threadIdx.x; i < kImuStride; i += kBwThreads) x[kFrameStride + i] = T.rec_out[(size_t)b * kImuStride + i];
+    if (threadIdx.x == 0) {
+        M.ed[b].n_new = nv;
+        M.ed[b].n_obs = no + (r.replace ? 0 : nv);
+        M.cnt[4 * b + 3] = nv;
+        M.lay[b].T = kept + nv;
+    }
+}
+
+// One CTA per record, after the edit's compaction: the slot's keypoint index of every row in the new frame
+__global__ void __launch_bounds__(kBwThreads) bw_mirror_link_kernel(BwArgs a, MirArgs M) {
+    const BwMirror r = M.rec[blockIdx.x];
+    const size_t base = (size_t)r.slot * a.Mcap;
+    const int T = M.lay[blockIdx.x].T;
+    if (threadIdx.x == 0) M.live[blockIdx.x] = M.eout[M.ed[blockIdx.x].out_off];
+    for (int q = threadIdx.x; q < T; q += kBwThreads) a.tkp[base + q] = -1;
+    __syncthreads();
+    for (int kj = threadIdx.x; kj < r.n_j; kj += kBwThreads) {
+        const int row = M.lrow[r.kp_off + kj];
+        if (row >= 0) a.tkp[base + row] = kj;
+    }
+}
+
 // ------------------------------------------------------------------------ host side
 template <>
 BwArgs launch_args<BwArgs>(const Handle *h) {
@@ -695,7 +926,7 @@ BwArgs launch_args<BwArgs>(const Handle *h) {
     static_cast<BatchArrays &>(a) = h->arrays;
     a.tid = b.tid.d; a.tmask = b.tmask.d; a.trho = b.trho.d; a.tz = b.tz.d; a.tvalid = b.tvalid.d; a.tqual = b.tqual.d;
     a.trole = b.trole.d; a.tplane = b.tplane.d; a.lm_row = b.lm_row.d; a.valid = h->valid.d; a.quality = h->quality.d;
-    a.imu_s = b.imu_s.d; a.imu_aux = b.imu_aux.d; a.Scap = b.Scap;
+    a.imu_s = b.imu_s.d; a.imu_aux = b.imu_aux.d; a.Scap = b.Scap; a.tkp = b.tkp.d;
     return a;
 }
 
@@ -706,6 +937,7 @@ static int ensure_bw(Handle *h) {
     TRY(alloc(h, b.tid, W * M, kDevice)); TRY(alloc(h, b.tmask, W * M, kDevice)); TRY(alloc(h, b.trho, W * M, kDevice));
     TRY(alloc(h, b.tz, W * M * h->Ncap, kDevice)); TRY(alloc(h, b.tvalid, W * M, kDevice)); TRY(alloc(h, b.tqual, W * M, kDevice));
     TRY(alloc(h, b.trole, W * M, kDevice)); TRY(alloc(h, b.tplane, W * h->Pcap * 4, kDevice));
+    TRY(alloc(h, b.tkp, W * M, kDevice));
     TRY(alloc(h, b.lm_row, W * M, kDevice));
     return 0;
 }
@@ -1046,6 +1278,32 @@ static const WinSlot *window0(Handle *h) {
     return &h->slots[0];
 }
 
+// the host mirror of a slot after its mirror_frame record: replace_last when the newest frame is not a keyframe, the new
+// frame (its factor holding n_kept samples), an observation there for each continued row (rows of s) that outlives the
+// replaced frame, n_new new tracks with the slot's next ids
+static WinSlot mirror_next(const WinSlot &s0, const std::vector<int> &rows, int n_new, int n_kept) {
+    WinSlot s = s0;
+    const bool replace = !s.newest_kf;
+    if (replace) {
+        for (uint32_t &m : s.mask) m &= ~(1u << (s.N - 1));
+        s.fixed &= ~(1 << (s.N - 1));
+        s.n_samples[s.N - 2] = 0;
+        --s.N;
+    }
+    const int f = s.N;
+    for (int r : rows)
+        if (s.mask[r]) s.mask[r] |= 1u << f;
+    compact_rows(s, 0);
+    s.n_samples[f - 1] = n_kept;
+    ++s.N;
+    for (int k = 0; k < n_new; ++k) {
+        s.ids.push_back(s.next_id++);
+        s.mask.push_back(replace ? 1u << f : (1u << (f - 1)) | (1u << f));
+        s.role.push_back(-1);
+    }
+    return s;
+}
+
 }  // namespace pvio
 
 using namespace pvio;
@@ -1130,6 +1388,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
             (E.n_new_tracks > 0 && (!E.new_frame || !E.new_z || !E.new_inv_depth)) ||
             (E.n_obs > 0 && (!E.obs_track || !E.obs_frame || !E.obs_z)) || (E.n_remove > 0 && !E.remove))
             return fail(h, PVIO_B200_EINVAL, "batch_window_edit: null array");
+        if (E.replace_last || E.state || E.n_new_tracks > 0 || E.n_obs > 0) s.link = false;   // the newest frame changes
         if (E.replace_last) {                                         // map->erase_frame(frame_num - 1)
             if (s.N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: replace_last on an empty window");
             if (s.N - 1 < s.n_prior) return fail(h, PVIO_B200_EINVAL, "batch_window_edit: the newest frame is covered by the prior");
@@ -1601,6 +1860,325 @@ int pvio_b200_batch_window_imu_records(pvio_b200_handle hh, int n, const int32_t
     CK(h, cudaStreamSynchronize(h->stream));
     for (int i = 0; i < n; ++i)
         memcpy(records + i * records_stride, S.host(out) + dls[i].off, sizeof(double) * (size_t)(dls[i].N - 1) * kImuStride);
+    return 0;
+}
+
+int pvio_b200_batch_window_set_keypoints(pvio_b200_handle hh, int n, const pvio_b200_window_keypoints *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_set_keypoints: bad slot list"));
+    std::vector<BwKeys> ks(n);
+    std::vector<int2> pairs;
+    std::vector<int> kmax(n, -1);
+    std::vector<uint32_t> gens(n, 0);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_keypoints &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (s.N < 1) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: a window without frames");
+        if (R.tracker_slot < 0 || R.tracker_slot > kMaxBatchSlot)
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: tracker slot out of range");
+        if (!R.frame_id) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: frame id 0");
+        const KltBatchState &B = h->kltb;
+        const SlotKeypoints *K = (size_t)R.tracker_slot < B.kps.size() ? &B.kps[R.tracker_slot] : nullptr;
+        if (!K || !K->live || (R.frame_id != K->frame_id && R.frame_id != K->prev_frame_id))
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: the frame is not one of the tracker slot's two newest");
+        gens[i] = K->gen;
+        if (R.n < 0 || (R.n > 0 && (!R.track || !R.keypoint))) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: null array");
+        if (R.newest_is_keyframe != 0 && R.newest_is_keyframe != 1)
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: newest_is_keyframe not 0 or 1");
+        if (R.skipped_frames < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: negative skipped_frames");
+        ks[i] = BwKeys{R.slot, (int32_t)s.ids.size(), R.n, (int32_t)pairs.size()};
+        const uint32_t newest = 1u << (s.N - 1);
+        std::vector<uint8_t> named(s.ids.size(), 0);
+        std::vector<int32_t> kps(R.keypoint, R.keypoint + R.n);
+        for (int k = 0; k < R.n; ++k) {
+            const int r = find_row(s, R.track[k]);
+            if (r < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: unknown or dead track");
+            if (!(s.mask[r] & newest)) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: a track not observed in the newest frame");
+            if (named[r]) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: a track named twice");
+            named[r] = 1;
+            if (R.keypoint[k] < 0) return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: negative keypoint index");
+            pairs.push_back(make_int2(r, R.keypoint[k]));
+            kmax[i] = std::max(kmax[i], (int)R.keypoint[k]);
+        }
+        std::sort(kps.begin(), kps.end());
+        if (std::adjacent_find(kps.begin(), kps.end()) != kps.end())
+            return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: a keypoint named twice");
+    }
+    Stage S;
+    const auto k = S.up(ks);
+    const auto p = S.up(pairs);
+    TRY(S.place(h, true));
+    bw_set_keypoints_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(k), S.dev(p));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_keypoints &R = records[i];
+        WinSlot &s = h->slots[R.slot];
+        s.link = true; s.link_tracker = R.tracker_slot; s.link_frame = R.frame_id; s.link_kmax = kmax[i]; s.link_gen = gens[i];
+        s.newest_kf = R.newest_is_keyframe; s.skipped = R.skipped_frames;
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_mirror_frame(pvio_b200_handle hh, int n, pvio_b200_window_mirror *records,
+                                        const pvio_b200_options *opt) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_mirror_frame: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_mirror_frame: bad slot list"));
+    auto bad = [h](const char *why) {
+        return fail(h, PVIO_B200_EINVAL, (std::string("batch_window_mirror_frame: ") + why).c_str());
+    };
+    // every record is checked against its slot's host mirror and its tracker slot before anything is staged
+    const KltBatchState &B = h->kltb;
+    std::vector<BwMirror> mir(n);
+    std::vector<BwLoc> locs(n);
+    std::vector<BwTrack> trs(n);
+    std::vector<BwEdit> eds(n);
+    std::vector<BwTrackJob> jobs;
+    std::vector<BwImu> kimu;                  // the factors that keep their samples, as set_imu stages them
+    std::vector<double> kaux, gpt;
+    std::vector<int32_t> grow;
+    std::vector<WinSlot> next(n);             // the slots' windows after the call, but for their row counts
+    std::vector<uint8_t> taken;
+    std::vector<const SlotKeypoints *> kps(n);
+    size_t kp = 0, tab = 0, rm = 0, rows = 0;
+    int smax = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_mirror &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (!s.inertial) return bad("the window carries no motion states");
+        if (s.N < 1) return bad("a window without frames");
+        if (!s.link) return bad("the slot has no link to a tracker slot (set_keypoints)");
+        if (R.tracker_slot != s.link_tracker) return bad("not the tracker slot of the slot's link");
+        if ((size_t)R.tracker_slot >= taken.size()) taken.resize(R.tracker_slot + 1, 0);
+        if (taken[R.tracker_slot]) return bad("a tracker slot named twice");
+        taken[R.tracker_slot] = 1;
+        const SlotKeypoints *K = (size_t)R.tracker_slot < B.kps.size() ? &B.kps[R.tracker_slot] : nullptr;
+        if (!K || !K->live || K->gen != s.link_gen || K->prev_frame_id == 0 || K->prev_frame_id != s.link_frame ||
+            s.link_kmax >= K->prev_n)
+            return bad("the tracker slot's previous frame is not the slot's newest frame");
+        kps[i] = K;
+        if (!R.samples || !R.noise_cov || !R.kp_track || !R.state || !R.keyframe) return bad("null array");
+        if (R.max_keypoints < K->n) return bad("max_keypoints below the tracker's keypoint count");
+        if (R.n_samples < 1) return bad("a frame without IMU samples (integrate() returns false, preintegrator.cpp:86)");
+        if (R.keep_samples != 0 && R.keep_samples != 1) return bad("keep_samples not 0 or 1");
+        if (!all_finite(R.samples, 7 * (int64_t)R.n_samples)) return bad("non-finite sample");
+        if (!std::isfinite(R.t_end) || !all_finite(R.noise_cov, 36) || !std::isfinite(R.cx) || !std::isfinite(R.cy))
+            return bad("non-finite t_end, noise or principal point");
+        const bool merged = !s.newest_kf;
+        if (merged && s.N < 2) return bad("a non-keyframe newest frame without a keyframe before it");
+        if (merged && s.N - 1 < s.n_prior) return bad("the newest frame is covered by the prior");
+        const int n_merge = merged ? s.n_samples[s.N - 2] : 0;
+        if (merged && n_merge < 1) return bad("a non-keyframe newest frame whose factor holds no samples");
+        if (!merged && s.N >= h->Ncap) return bad("window of more than max_frames frames");
+        if (R.n_given < 0 || (R.n_given > 0 && (!R.given_track || !R.given_point))) return bad("null array");
+        std::vector<std::pair<int, int>> given;
+        std::vector<uint8_t> named(s.ids.size(), 0);
+        for (int k = 0; k < R.n_given; ++k) {
+            const int r = find_row(s, R.given_track[k]);
+            if (r < 0) return bad("unknown or dead track");
+            if (named[r]) return bad("a track named twice");
+            named[r] = 1;
+            if (!all_finite(R.given_point + 3 * k, 3)) return bad("non-finite given point");
+            given.push_back({r, k});
+        }
+        std::sort(given.begin(), given.end());
+        const int T = (int)s.ids.size(), fnew = merged ? s.N - 1 : s.N;
+        const size_t first = rows;            // the call's sample rows: merge list ++ own samples per record
+        mir[i] = BwMirror{K->z(1 - K->cur), K->z(K->cur), K->prev(K->cur), R.slot, T, K->prev_n, K->n, (int32_t)tab,
+                          (int32_t)kp, (int32_t)grow.size(), R.n_given, (int32_t)rm, (int32_t)first, n_merge,
+                          merged ? 1 : 0, s.N, s.next_id, 0, 0};
+        for (const auto &g : given) {
+            grow.push_back(g.first);
+            gpt.insert(gpt.end(), R.given_point + 3 * g.second, R.given_point + 3 * g.second + 3);
+        }
+        locs[i] = BwLoc{R.slot, s.N - 1, 1, 0, (int32_t)kp, i, 0, (int32_t)kp};
+        trs[i] = BwTrack{merged ? 1 : 0, merged ? s.N - 2 : s.N - 1, 0, (int32_t)kp, merged ? 0 : 1, (int32_t)kp,
+                         s.skipped, (int32_t)i * kImuAux, R.cx, R.cy};
+        eds[i] = BwEdit{R.slot, s.N, T, merged ? 1 : 0, 0, 0, fnew, 1, i * kMirX, 0, (int32_t)kp, 0, (int32_t)kp,
+                        (int32_t)(kp + i)};
+        const size_t b = first + n_merge, e = b + R.n_samples;
+        jobs.push_back(BwTrackJob{i, (int32_t)b, (int32_t)e, 0});
+        if (merged) jobs.push_back(BwTrackJob{i, (int32_t)first, (int32_t)e, 1});
+        rows = e;
+        const int n_list = n_merge + R.n_samples;
+        if (R.keep_samples) {
+            kimu.push_back(BwImu{R.slot, fnew - 1, n_list, (int32_t)first});
+            kaux.push_back(R.t_end);
+            kaux.insert(kaux.end(), R.noise_cov, R.noise_cov + 36);
+            smax = std::max(smax, n_list);
+        }
+        next[i] = mirror_next(s, {}, 0, R.keep_samples ? n_list : 0);
+        kp += K->n; tab += 2 * (size_t)K->prev_n; rm += T;
+        if (rows > (size_t)INT32_MAX || kp + n > (size_t)INT32_MAX || tab > (size_t)INT32_MAX)
+            return bad("too many samples or keypoints in one call");
+    }
+
+    if (!kimu.empty()) TRY(ensure_imu_store(h, smax));   // the kept lists' room, before anything is staged
+
+    // staging: upload records | track_frame's records, jobs, samples, t_end and noise | given points | edit records |
+    // kept factors | re-layout; download counts | continued rows (the capacity check), then the results; device only
+    // the mirror's tables and lists, the localize sections, the edit's lists
+    const size_t w8 = sizeof(double);
+    Stage S;
+    const auto mr = S.up(mir);
+    const auto lo = S.up(locs);
+    const auto tr = S.up(trs);
+    const auto job = S.up(jobs);
+    const auto smp = S.add<double>(Stage::kUp, 7 * rows), aux = S.add<double>(Stage::kUp, (size_t)n * kImuAux);
+    const auto gr = S.up(grow);
+    const auto gp = S.up(gpt);
+    const auto ed = S.up(eds);
+    const auto kim = S.up(kimu);
+    const auto kax = S.up(kaux);
+    const Relayout lay(S, slots.data(), next);
+    const auto cnt = S.add<int32_t>(Stage::kDown, 4 * (size_t)n);
+    const auto live = S.add<int32_t>(Stage::kDown, n);
+    const auto frames = S.add<double>(Stage::kDown, 16 * (size_t)n), out = S.add<double>(Stage::kDown, 8 * (size_t)n);
+    const auto rec_out = S.add<double>(Stage::kDown, (size_t)n * kImuStride), pred = S.add<double>(Stage::kDown, 16 * (size_t)n);
+    const auto kfo = S.add<double>(Stage::kDown, 4 * (size_t)n);
+    const auto kpt = S.add<int32_t>(Stage::kDown, kp);
+    // the continued rows: downloaded once, for the capacity check
+    const auto cont = S.add<int2>(Stage::kScratch, kp);
+    const auto eout = S.add<int32_t>(Stage::kScratch, kp + n);
+    const auto tabs = S.add<int32_t>(Stage::kScratch, tab), rmap = S.add<int32_t>(Stage::kScratch, rm);
+    const auto lrow = S.add<int32_t>(Stage::kScratch, kp), cand = S.add<int32_t>(Stage::kScratch, kp);
+    const auto row = S.add<int32_t>(Stage::kScratch, kp), kf_row = S.add<int32_t>(Stage::kScratch, kp);
+    const auto z = S.add<double>(Stage::kScratch, 2 * kp), pts = S.add<double>(Stage::kScratch, 3 * kp);
+    const auto nz = S.add<double>(Stage::kScratch, 4 * kp), kf_z = S.add<double>(Stage::kScratch, 2 * kp);
+    const auto rho = S.add<double>(Stage::kScratch, kp), rho_next = S.add<double>(Stage::kScratch, kp);
+    const auto valid = S.add<uint8_t>(Stage::kScratch, kp);
+    const auto par = S.add<double>(Stage::kScratch, kp), rec1 = S.add<double>(Stage::kScratch, (size_t)n * kImuStride);
+    const auto args = S.add<PnpArgs>(Stage::kScratch, n);
+    const auto nw = S.add<BwNew>(Stage::kScratch, kp);
+    const auto ob = S.add<BwObs>(Stage::kScratch, kp);
+    const auto xs = S.add<double>(Stage::kScratch, (size_t)n * kMirX);
+    TRY(S.place(h));
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_mirror &R = records[i];
+        memcpy(S.host(smp) + 7 * ((size_t)mir[i].merge_row + mir[i].n_merge), R.samples, w8 * 7 * R.n_samples);
+        double *a = S.host(aux) + (size_t)i * kImuAux;
+        a[0] = R.t_end;
+        memcpy(a + 1, R.noise_cov, w8 * 36);
+    }
+    TRY(S.upload(h));
+    const SolveOptions so = solve_options(opt);
+    LocArgs L;
+    L.rec = S.dev(lo); L.row = S.dev(row); L.z = S.dev(z); L.imu = S.dev(rec1); L.nz = S.dev(nz);
+    L.frames = S.dev(frames); L.pts = S.dev(pts); L.out = S.dev(out); L.rho = S.dev(rho); L.rho_next = S.dev(rho_next);
+    L.valid = S.dev(valid); L.args = S.dev(args); L.max_iter = so.max_iter; L.radius0 = so.radius0;
+    TrackArgs T;
+    T.tr = S.dev(tr); T.job = S.dev(job); T.kf_row = S.dev(kf_row); T.kf_z = S.dev(kf_z); T.smp = S.dev(smp);
+    T.aux = S.dev(aux); T.rec_out = S.dev(rec_out); T.pred = S.dev(pred); T.kfo = S.dev(kfo); T.rec1 = S.dev(rec1);
+    T.par = S.dev(par); T.n_jobs = (int)jobs.size();
+    MirArgs M;
+    M.rec = S.dev(mr); M.loc = S.dev(lo); M.tr = S.dev(tr); M.tab = S.dev(tabs); M.grow = S.dev(gr); M.gpt = S.dev(gp);
+    M.row = S.dev(row); M.z = S.dev(z); M.pts = S.dev(pts); M.nz = S.dev(nz); M.kf_row = S.dev(kf_row);
+    M.kf_z = S.dev(kf_z); M.smp = S.dev(smp); M.cont = S.dev(cont); M.cand = S.dev(cand); M.rmap = S.dev(rmap);
+    M.lrow = S.dev(lrow); M.kp = S.dev(kpt); M.cnt = S.dev(cnt); M.ed = S.dev(ed); M.nw = S.dev(nw); M.ob = S.dev(ob);
+    M.x = S.dev(xs); M.lay = S.dev(lay.lay); M.eout = S.dev(eout); M.live = S.dev(live);
+    // mirror, then track_frame's five kernels on its lists
+    BwArgs a = launch_args<BwArgs>(h);
+    bw_mirror_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    const int J = (int)jobs.size();
+    bw_track_integrate_kernel<<<(J + kBwImuWarps - 1) / kBwImuWarps, 32 * kBwImuWarps, 0, h->stream>>>(a, L, T);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(loc_launch(h, L, n));
+    bw_track_keyframe_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(S.download(h, cnt, cnt));
+    TRY(S.download(h, cont, cont));
+    CK(h, cudaStreamSynchronize(h->stream));
+
+    // capacity: the windows as they would be if every candidate turned out valid
+    std::vector<WinSlot> most(n);
+    for (int i = 0; i < n; ++i) {
+        const int32_t *c = S.host(cnt) + 4 * (size_t)i;
+        const int2 *cr = S.host(cont) + mir[i].kp_off;
+        std::vector<int> rws(c[0]);
+        for (int k = 0; k < c[0]; ++k) rws[k] = cr[k].x;
+        most[i] = mirror_next(h->slots[slots[i]], rws, c[2], 0);
+        TRY(check_window(h, most[i]));
+    }
+    TRY(ensure_plane_tables(h, most));        // observations of plane tracks may outgrow the plane tables
+
+    // append: the edit, the re-layout, the kept samples, the link
+    a = launch_args<BwArgs>(h);
+    bw_mirror_append_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T, M);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(a, S.dev(ed), nullptr, S.dev(nw), S.dev(ob), S.dev(xs), S.dev(eout));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(lay.launch(h, S, false));
+    if (!kimu.empty()) {
+        bw_set_imu_kernel<<<(int)kimu.size(), kBwThreads, 0, h->stream>>>(a, S.dev(kim), S.dev(smp), S.dev(kax));
+        ++h->launches;
+        CK(h, cudaGetLastError());
+    }
+    bw_mirror_link_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(S.download(h));
+    CK(h, cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+
+    // the host mirrors from kp_track: continued tracks hold ids below the slot's next id, new tracks the next ids
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_mirror &R = records[i];
+        const WinSlot &s = h->slots[slots[i]];
+        const int32_t *k = S.host(kpt) + mir[i].kp_off;
+        std::vector<int> rws;
+        int n_new = 0, kmax = -1;
+        for (int j = 0; j < mir[i].n_j; ++j) {
+            if (k[j] < 0) continue;
+            kmax = j;
+            if (k[j] < s.next_id) rws.push_back(find_row(s, k[j])); else ++n_new;
+        }
+        const double *o = S.host(kfo) + 4 * (size_t)i;
+        next[i] = mirror_next(s, rws, n_new, R.keep_samples ? mir[i].n_merge + R.n_samples : 0);
+        next[i].link_frame = kps[i]->frame_id; next[i].link_kmax = kmax; next[i].link_gen = kps[i]->gen;
+        next[i].newest_kf = o[0] != 0.0 ? 1 : 0; next[i].skipped = (int)o[3];
+    }
+    commit(h, slots.data(), next);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_mirror &R = records[i];
+        if (S.host(live)[i] != (int32_t)h->slots[slots[i]].ids.size())
+            return fail(h, PVIO_B200_ECUDA, "batch_window_mirror_frame: the device track table disagrees with the host's");
+        memcpy(R.kp_track, S.host(kpt) + mir[i].kp_off, sizeof(int32_t) * mir[i].n_j);
+        if (R.counts) memcpy(R.counts, S.host(cnt) + 4 * (size_t)i, sizeof(int32_t) * 4);
+        memcpy(R.state, S.host(frames) + 16 * (size_t)i, w8 * 16);
+        if (R.predicted) memcpy(R.predicted, S.host(pred) + 16 * (size_t)i, w8 * 16);
+        if (R.imu_record) memcpy(R.imu_record, S.host(rec_out) + (size_t)i * kImuStride, w8 * kImuStride);
+        const double *o = S.host(kfo) + 4 * (size_t)i;
+        *R.keyframe = o[0] != 0.0 ? 1 : 0;
+        if (R.parallax) *R.parallax = o[1];
+        if (R.n_parallax) *R.n_parallax = (int32_t)o[2];
+        if (R.skipped_frames) *R.skipped_frames = (int32_t)o[3];
+        if (R.summary) {
+            const double *b = S.host(out) + 8 * (size_t)i;
+            pvio_b200_summary &sm = *R.summary;
+            memset(&sm, 0, sizeof(sm));
+            sm.iterations = (int)b[0]; sm.accepted_steps = (int)b[1]; sm.termination = (int)b[2]; sm.usable = (int)b[3];
+            sm.initial_cost = b[4]; sm.final_cost = b[5]; sm.final_radius = b[6]; sm.final_mu = b[7];
+            sm.solve_seconds = ms * 1e-3;
+        }
+    }
     return 0;
 }
 

@@ -27,6 +27,7 @@ struct BwArgs : BatchArrays {
     const double *quality;
     double *imu_s, *imu_aux;
     int Scap;
+    int32_t *tkp;
 };
 
 constexpr int kBwThreads = 256;
@@ -137,6 +138,13 @@ struct Stage {
     int download(Handle *h) const {
         if (end[kDown] > end[kUp])
             CK(h, cudaMemcpyAsync(hp + end[kUp], dp + end[kUp], end[kDown] - end[kUp], cudaMemcpyDeviceToHost, h->stream));
+        return 0;
+    }
+    // sections a .. b (declared in that order, one kind) back to the host in one copy
+    template <typename A, typename B>
+    int download(Handle *h, Sec<A> a, Sec<B> b) const {
+        const size_t o = secs[a.i].off, e = secs[b.i].off + secs[b.i].bytes;
+        if (e > o) CK(h, cudaMemcpyAsync(hp + o, dp + o, e - o, cudaMemcpyDeviceToHost, h->stream));
         return 0;
     }
 };

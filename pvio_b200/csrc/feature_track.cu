@@ -46,6 +46,7 @@ struct FtSeq {
     double gs, r2;                            // Poisson cell size r / sqrt(2), r^2
     int use_q, n_prev, first, prev_no;        // first: its first point in the tracker's arrays; prev_no: the previous
     int map_frames, out_cap, hbits, w;        //   frame's number (births count in these)
+    int *prev_next;                           // the slot's other buffer: this frame's prev_index
 };
 
 // the F-RANSAC outcome of one sequence (uploaded after the replay)
@@ -151,7 +152,7 @@ __global__ void __launch_bounds__(kThinThreads) ft_thin_kernel(const FtSeq *seqs
             const double2 z = make_double2((x - s.kn[2]) / s.kn[0], (y - s.kn[3]) / s.kn[1]);
             s.pre[j] = make_double2(z.x * s.kn[0] + s.kn[2], z.y * s.kn[1] + s.kn[3]);
             if (j < s.out_cap) {                  // always, by the capacity bound; the host reports a breach
-                s.z_next[j] = z; s.birth_next[j] = s.birth_prev[k];
+                s.z_next[j] = z; s.birth_next[j] = s.birth_prev[k]; s.prev_next[j] = k;
                 s.out_z[j] = z; s.out_prev[j] = k;
             }
         }
@@ -176,7 +177,7 @@ __global__ void ft_commit_kernel(const FtSeq *seqs, const DetectResult *res) {
             const unsigned idx = R.corner[j], y = idx / (unsigned)s.w, x = idx - y * (unsigned)s.w;
             const double2 z = make_double2(((double)x - s.kn[2]) / s.kn[0], ((double)y - s.kn[3]) / s.kn[1]);
             if (i < s.out_cap) {
-                s.z_next[i] = z; s.birth_next[i] = s.prev_no + 1;
+                s.z_next[i] = z; s.birth_next[i] = s.prev_no + 1; s.prev_next[i] = -1;
                 s.out_z[i] = z; s.out_prev[i] = -1;
             }
         }
@@ -302,7 +303,7 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
         const int b = 1 - K.cur;
         const size_t need = std::max<size_t>(plan[i].out_cap, 1024);
         if (K.cap[b] < (size_t)plan[i].out_cap) {
-            TRY(alloc(h, K.buf[b], (sizeof(double2) + sizeof(int)) * need, kDevice));
+            TRY(alloc(h, K.buf[b], SlotKeypoints::bytes(need), kDevice));
             K.cap[b] = need;
         }
     }
@@ -317,10 +318,11 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
         FtSeq &S = seq[i];
         memset(&S, 0, sizeof(S));
         const int cb = K.cur, nb = 1 - K.cur;
-        S.z_prev = reinterpret_cast<const double2 *>(K.buf[cb].d);
-        S.birth_prev = reinterpret_cast<const int *>(K.buf[cb].d + sizeof(double2) * K.cap[cb]);
-        S.z_next = reinterpret_cast<double2 *>(K.buf[nb].d);
-        S.birth_next = reinterpret_cast<int *>(K.buf[nb].d + sizeof(double2) * K.cap[nb]);
+        S.z_prev = K.z(cb);
+        S.birth_prev = K.birth(cb);
+        S.z_next = K.z(nb);
+        S.birth_next = K.birth(nb);
+        S.prev_next = K.prev(nb);
         S.pre = reinterpret_cast<double2 *>(dc + c_pre) + pre;
         S.out_z = reinterpret_cast<double2 *>(ds + o_out + P.out_off);
         S.out_prev = reinterpret_cast<int *>(ds + o_out + P.out_off + sizeof(double2) * P.out_cap);
@@ -408,6 +410,9 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
         if (a.counts) memcpy(a.counts, hd + 1, sizeof(int32_t) * 4);
         if (a.info) memcpy(a.info, &r.info[4 * (size_t)i], sizeof(int32_t) * 4);
         SlotKeypoints &K = B.kps[a.slot];
+        K.prev_frame_id = a.map_frames > 0 ? K.frame_id : 0;     // map_frames == 0: the link to the previous frame goes
+        K.prev_n = a.map_frames > 0 ? K.n : 0;
+        if (a.map_frames == 0) ++K.gen;
         K.cur = 1 - K.cur;
         K.n = w;
         K.live = true;
