@@ -649,6 +649,54 @@ typedef struct pvio_b200_window_mirror {
  * PnP solves. */
 int pvio_b200_batch_window_mirror_frame(pvio_b200_handle h, int n, pvio_b200_window_mirror *records,
                                         const pvio_b200_options *opt);
+/* Snapshots: a live sequence saved to host memory and restored into any slot of any handle, so that it can outlive its
+ * handle, move to another handle or device, or be forked or rolled back.  A record names a window slot, a tracker slot
+ * of pvio_b200_batch_feature_track, or both (-1: none).  The blob holds the source-of-truth state only, compacted to
+ * what is used: the window's constants (with the origin its solves use), counts, fixed mask, next id, prior size, keyframe flag and skipped-frame
+ * counter; per live track its id, frame mask, role, inverse depth, post-pass flags, keypoint index in the newest frame
+ * and fp64 keypoint per window frame; the frame states, IMU records, prior (S, e, state0), the factors' samples, t_end
+ * and noise, the plane parameters; of the tracker slot the keypoints of its two newest frames (keypoint, birth,
+ * prev_index; newest first), its counters, frame ids and K, and the pyramid of its newest frame with its CLAHE clip.
+ * Packed tables (the solve's landmark and observation records, the frame-major table, the prior's Lambda, the plane
+ * tables) are rebuilt on restore.  A blob names no slot, pointer, capacity or sequence generation, its padding is zero,
+ * so save -> restore -> save gives the same bytes in any slot of any handle.
+ *  - save: a resident window slot and / or a live tracker slot.  data == NULL asks for the size only (no device work);
+ *    otherwise capacity must hold `size` bytes.  size is written on success.  The window's link to a tracker slot is
+ *    saved only when the record names that tracker slot too and the link still names one of its two newest frames
+ *    (of its current sequence) with every keypoint index inside that frame's keypoints, as mirror_frame needs it;
+ *    otherwise the blob holds no link (every keypoint index -1), and such a blob restores unlinked.
+ *  - restore: capacity is the blob's byte count.  A record restores the parts it names (the blob must hold them) and
+ *    skips the others.  The window part replaces the target slot as a reset followed by seating the state; the tracker
+ *    part replaces the target tracker slot, starts a new sequence there (a window linked to it before must be linked
+ *    again) with only its newest frame cached.  The link comes back only when both parts are restored, re-pointed at the
+ *    target tracker slot; otherwise the window comes back unlinked and pvio_b200_batch_window_set_keypoints links it.
+ *  - Not restored: the tracker slot's lens (configuration: set it with pvio_b200_batch_set_lens on the target, as at the
+ *    start of a sequence), its older pyramid, the single-call tracker and detector caches.  A blob restored into a handle
+ *    of the other precision (fp32 or fp64 Jacobians) solves with that handle's pipeline.
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no slot, tracker slot or output has changed.
+ * Rejected: n < 0; a record naming neither part; a slot out of range (save: not resident); a tracker slot outside
+ * 0 .. 65535 (save: not live); a slot or a tracker slot named twice; save capacity below the size; a restore blob with
+ * the wrong magic or version, a declared size other than its byte count, a part the record names but the blob lacks,
+ * or contents out of range: more frames than max_frames, more live tracks than max_landmarks, the observation, chunk and
+ * 16-observation limits of the other calls, ids not strictly increasing or not below the next id, a frame mask 0 or
+ * outside the window's frames, a role not -1, -2 or a plane of the blob, a prior over more frames than the window or on
+ * a visual-only window, samples on a visual-only window, a keypoint index or prev_index outside its keypoint count, a
+ * pyramid shape the tracker would not build.  Buffers grow as the other calls grow them.
+ * Launches, whatever n is: save one pack kernel, one device -> host copy, one synchronisation; restore one host ->
+ * device copy, one unpack kernel, the re-layout of the window slots and the write-back of their saved origins (4
+ * launches, when a record restores a window) and one synchronisation.  A restored window solves, drops and edits
+ * exactly as its source would have. */
+#define PVIO_B200_SNAPSHOT_MAGIC 1314084432  /* "PVSN" as a little-endian uint32 */
+#define PVIO_B200_SNAPSHOT_VERSION 1
+typedef struct pvio_b200_window_snapshot {
+    int32_t slot;                     /* window slot, or -1 */
+    int32_t tracker_slot;             /* tracker slot of pvio_b200_batch_feature_track, or -1 */
+    uint8_t *data;                    /* save: room for capacity bytes, NULL: size query only; restore: the saved bytes */
+    int64_t capacity;                 /* bytes at data */
+    int64_t size;                     /* save, out: the bytes the record needs / wrote */
+} pvio_b200_window_snapshot;          /* 32 bytes on LP64 */
+int pvio_b200_batch_window_save(pvio_b200_handle h, int n, pvio_b200_window_snapshot *records);
+int pvio_b200_batch_window_restore(pvio_b200_handle h, int n, const pvio_b200_window_snapshot *records);
 
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */

@@ -26,6 +26,7 @@ TWO_VIEW_OK, TWO_VIEW_FEW_MATCHES, TWO_VIEW_LOW_PARALLAX, TWO_VIEW_PURE_ROTATION
 LENS_RADTAN, LENS_EQUIDISTANT = 1, 2
 PLANE_EXTRACT, PLANE_REFIT = 0, 1
 PLANE_ACCEPTED, PLANE_FEW_POINTS, PLANE_REJECTED = 0, 1, 2
+SNAPSHOT_MAGIC, SNAPSHOT_VERSION = 1314084432, 1
 
 c_i32p = C.POINTER(C.c_int32)
 c_u8p = C.POINTER(C.c_uint8)
@@ -152,6 +153,11 @@ class CWindowMirror(C.Structure):
                 ("skipped_frames", c_i32p), ("summary", C.POINTER(CSummary))]
 
 
+class CWindowSnapshot(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("data", c_u8p), ("capacity", C.c_int64),
+                ("size", C.c_int64)]
+
+
 class CLens(C.Structure):
     _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
@@ -220,6 +226,8 @@ SIGNATURES = {
     "pvio_b200_batch_window_plane_ransac": (_int, [_h, _int, _P(CWindowPlaneRansac)]),
     "pvio_b200_batch_window_set_keypoints": (_int, [_h, _int, _P(CWindowKeypoints)]),
     "pvio_b200_batch_window_mirror_frame": (_int, [_h, _int, _P(CWindowMirror), _P(COptions)]),
+    "pvio_b200_batch_window_save": (_int, [_h, _int, _P(CWindowSnapshot)]),
+    "pvio_b200_batch_window_restore": (_int, [_h, _int, _P(CWindowSnapshot)]),
     "pvio_b200_sync": (_int, [_h]),
     "pvio_b200_timer_start": (_int, [_h]),
     "pvio_b200_timer_stop": (_int, [_h, c_f32p]),

@@ -384,6 +384,42 @@ class BatchWindows:
                                                                 _lib.ptr(e), d))
         return S, e
 
+    def save(self, slots, tracker_slots=None):
+        """Save each sequence to host memory: per record a window slot (-1: none) and, from tracker_slots (None: none),
+        a tracker slot of batch_feature_track (-1: none).  Returns one blob (bytes) per record, which restore() seats in
+        any slot of any handle."""
+        recs, n = self._snapshots(slots, tracker_slots)
+        self.ba._ck(self.lib.pvio_b200_batch_window_save(self.h, n, recs))          # data NULL: the sizes
+        bufs = [np.zeros(recs[i].size, dtype=np.uint8) for i in range(n)]
+        for i, b in enumerate(bufs):
+            recs[i].data, recs[i].capacity = _lib.ptr(b), len(b)
+        self.ba._ck(self.lib.pvio_b200_batch_window_save(self.h, n, recs))
+        return [b.tobytes() for b in bufs]
+
+    def restore(self, slots, blobs, tracker_slots=None):
+        """Restore blobs of save(): record i seats blobs[i]'s window in slots[i] and its tracker part in
+        tracker_slots[i] (-1 or None: that part is skipped).  The link between them comes back only when both are
+        restored; a restored tracker slot needs its lens set again (batch_set_lens) if it had one."""
+        recs, n = self._snapshots(slots, tracker_slots)
+        arrs = [np.frombuffer(b, dtype=np.uint8) for b in blobs]
+        if len(arrs) != n:
+            raise ValueError("one blob per record")
+        for i, a in enumerate(arrs):
+            recs[i].data, recs[i].capacity = _lib.ptr(a), len(a)
+        self.ba._ck(self.lib.pvio_b200_batch_window_restore(self.h, n, recs))
+
+    @staticmethod
+    def _snapshots(slots, tracker_slots):
+        """the pvio_b200_window_snapshot records of a save / restore call, and their count"""
+        slots = [-1 if s is None else int(s) for s in slots]
+        ts = [-1] * len(slots) if tracker_slots is None else [-1 if t is None else int(t) for t in tracker_slots]
+        if len(ts) != len(slots):
+            raise ValueError("one tracker slot per record")
+        recs = (_lib.CWindowSnapshot * max(len(slots), 1))()
+        for r, s, t in zip(recs, slots, ts):
+            r.slot, r.tracker_slot = s, t
+        return recs, len(slots)
+
     def download(self, slots, track_stride):
         """Per slot a dict: frames [N, 16], and per live track in id order: id, inv_depth, anchor, n_obs, valid, quality."""
         s = np.ascontiguousarray(slots, dtype=np.int32)

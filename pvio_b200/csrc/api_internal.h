@@ -425,6 +425,10 @@ int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, co
                    pvio_b200_summary *summary);
 int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
                          const pvio_b200_options *opt, pvio_b200_summary *summaries);
+// klt.cu: the level count of a width x height frame's pyramid for maxLevel max_level; the level sizes and offsets of an
+// empty cache for w x hgt frames with `levels` levels
+int klt_levels(int width, int height, int max_level);
+void klt_layout(KltPyramids &k, int w, int hgt, int levels);
 // klt.cu / detect.cu
 const uint8_t *klt_cached_level0(Handle *h, uint64_t frame_id, int width, int height, double clahe_clip);
 // klt.cu, used by detect.cu: cv::CLAHE's per-tile constants of a w x h frame, and CLAHE of n_frames frames (frames in

@@ -308,7 +308,7 @@ klt_track_kernel(const float *prev_pts, float *next_pts, uint8_t *status, float 
 
 // cv::buildOpticalFlowPyramid halves first and drops the NEW level if it is not larger than the window: the number of
 // levels (level 0 included) a width x height frame gets for maxLevel max_level
-static int klt_levels(int width, int height, int max_level) {
+int klt_levels(int width, int height, int max_level) {
     int levels = 1, lw = width, lh = height;
     while (levels <= max_level) {
         lw = (lw + 1) / 2; lh = (lh + 1) / 2;
@@ -319,7 +319,7 @@ static int klt_levels(int width, int height, int max_level) {
 }
 
 // the level sizes and offsets of an empty cache for w x hgt frames with `levels` levels
-static void klt_layout(KltPyramids &k, int w, int hgt, int levels) {
+void klt_layout(KltPyramids &k, int w, int hgt, int levels) {
     k.w = w; k.h = hgt; k.levels = levels;
     size_t off = 0;
     int lw = w, lh = hgt;
