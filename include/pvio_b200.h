@@ -649,6 +649,71 @@ typedef struct pvio_b200_window_mirror {
  * PnP solves. */
 int pvio_b200_batch_window_mirror_frame(pvio_b200_handle h, int n, pvio_b200_window_mirror *records,
                                         const pvio_b200_options *opt);
+/* One new camera frame of linked resident inertial slots in one call: what pvio_b200_batch_feature_track with a
+ * host-given predict_q followed by pvio_b200_batch_window_mirror_frame with the same samples gives, with the IMU
+ * keypoint prediction of FeatureTracker::work (feature_tracker.cpp:77-91, frame.cpp:98) made on the device.
+ * Lockstep is assumed: the tracker slot's newest frame is the window slot's newest frame (the frontend's latest
+ * optimised frame), so the re-prediction loop of feature_tracker.cpp:57-76 is empty.  Per record:
+ *  1. PreIntegrator::integrate over samples at the biases of the slot's newest frame, then predict from that frame's
+ *     state (post-solve when the slot was solved after the previous frame): `predicted`, the feature tracker's
+ *     latest_state (:87-90), from which a shim's Core::predict_pose propagates.
+ *  2. delta_key_q = (cam_q^* imu_q dq imu_q^* cam_q)^* from that integration's dq and the slot constants' extrinsics,
+ *     each product in Eigen's scalar order, uncontracted; written to predict_q when given.
+ *  3. batch_feature_track's frame with that prediction on tracker_slot (map_frames > 0), then mirror_frame's steps with
+ *     the new frame's keypoints; the PnP starts from the state of step 1.
+ * samples are the list mirror_frame takes: the frame's preintegration.data after the prepend rule of
+ * feature_tracker.cpp:78-84, which the caller applies (it holds the previous frame's samples).
+ * Rejected: every batch_feature_track and mirror_frame rejection that applies (the tracker slot is checked as it stands
+ * before the call: its newest frame must be the slot's newest frame), a visual-only slot, map_frames == 0 (a sequence
+ * start goes through batch_feature_track), fx or fy other than the slot constants' (the reference's Frame::K serves
+ * both), and, after the gather, more keypoints than the bound or mirror_frame's capacity check.  A rejected call
+ * changes no window slot, no tracker slot and no output; the tracker slot's host state (newest buffer, counts, frame
+ * ids, counters) commits only after the capacity check.  Its one side effect: the tracker slot's older cached pyramid,
+ * which no call reads, may have been evicted.
+ * Launches, copies and synchronisations do not depend on n: batch_feature_track's and mirror_frame's together plus two
+ * launches (the step-1 integration ahead of the feature stages, the delta_key_q composition), with one host -> device
+ * copy more (the new frames into the mirror's records) and one device -> host copy fewer (counts and continued rows
+ * in one).  n == 0 is a no-op. */
+typedef struct pvio_b200_window_camera {
+    int32_t slot;                     /* resident inertial slot, linked to tracker_slot */
+    int32_t tracker_slot;             /* its tracker slot of pvio_b200_batch_feature_track */
+    uint64_t frame_id;                /* the new frame's id, != 0 */
+    int32_t width, height, stride;
+    int32_t map_frames;               /* > 0: the tracker map's frame_num() before this frame is put */
+    const uint8_t *image;             /* raw pixels */
+    double fx, fy, cx, cy;            /* the frame's K; fx, fy as the slot constants' */
+    int32_t max_keypoints;            /* capacity of kp_track, keypoints, prev_index: >= cells + 2000 */
+    int32_t n_samples;                /* >= 1 */
+    const double *samples;            /* [n_samples][7] t, w xyz, a xyz: the frame's samples after the prepend rule */
+    double t_end;                     /* the new frame's time */
+    const double *noise_cov;          /* [4][9] cov_w, cov_a, cov_bg, cov_ba */
+    int32_t keep_samples;             /* 1: the new factor keeps its samples on the device (as set_imu) */
+    int32_t n_given;
+    const int32_t *given_track;       /* [n_given] live track ids with a given (plane-cast) world point */
+    const double *given_point;        /* [n_given][3] */
+    int32_t *n_keypoints;             /* out: the new frame's keypoint count */
+    int32_t *kp_track;                /* [max_keypoints] out, as mirror_frame */
+    int32_t *counts;                  /* [4] or NULL, out, as mirror_frame */
+    double *state;                    /* [16] out: the PnP solution */
+    double *predicted;                /* [16] or NULL, out: step 1's state */
+    double *imu_record;               /* [PVIO_B200_IMU_STRIDE] or NULL, out: the factor of the frame edit */
+    uint8_t *keyframe;                /* out */
+    double *parallax;                 /* or NULL, out */
+    int32_t *n_parallax;              /* or NULL, out */
+    int32_t *skipped_frames;          /* or NULL, out */
+    pvio_b200_summary *summary;       /* or NULL */
+    double *keypoints;                /* [max_keypoints][2] or NULL, out: as batch_feature_track */
+    int32_t *prev_index;              /* [max_keypoints] or NULL, out: as batch_feature_track */
+    int32_t *feature_counts;          /* [4] or NULL, out: batch_feature_track's counts */
+    int32_t *info;                    /* [4] or NULL, out: batch_feature_track's info */
+    double *predict_q;                /* [4] or NULL, out: the delta_key_q used, x y z w */
+} pvio_b200_window_camera;            /* 256 bytes on LP64 */
+/* n records, each naming a different resident slot and a different tracker slot; the tracker options are
+ * pvio_b200_batch_feature_track's, opt (may be NULL) is shared by the PnP solves. */
+int pvio_b200_batch_window_track_camera(pvio_b200_handle h, int n, pvio_b200_window_camera *records, int max_level,
+                                        int max_iter, double eps, double clahe_clip, int tiles_x, int tiles_y,
+                                        int border, double ransac_threshold, double ransac_confidence,
+                                        double keypoint_distance, const pvio_b200_options *opt);
 /* Snapshots: a live sequence saved to host memory and restored into any slot of any handle, so that it can outlive its
  * handle, move to another handle or device, or be forked or rolled back.  A record names a window slot, a tracker slot
  * of pvio_b200_batch_feature_track, or both (-1: none).  The blob holds the source-of-truth state only, compacted to

@@ -153,6 +153,19 @@ class CWindowMirror(C.Structure):
                 ("skipped_frames", c_i32p), ("summary", C.POINTER(CSummary))]
 
 
+class CWindowCamera(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("frame_id", C.c_uint64), ("width", C.c_int32),
+                ("height", C.c_int32), ("stride", C.c_int32), ("map_frames", C.c_int32), ("image", c_u8p),
+                ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+                ("max_keypoints", C.c_int32), ("n_samples", C.c_int32), ("samples", c_f64p), ("t_end", C.c_double),
+                ("noise_cov", c_f64p), ("keep_samples", C.c_int32), ("n_given", C.c_int32), ("given_track", c_i32p),
+                ("given_point", c_f64p), ("n_keypoints", c_i32p), ("kp_track", c_i32p), ("counts", c_i32p),
+                ("state", c_f64p), ("predicted", c_f64p), ("imu_record", c_f64p), ("keyframe", c_u8p),
+                ("parallax", c_f64p), ("n_parallax", c_i32p), ("skipped_frames", c_i32p),
+                ("summary", C.POINTER(CSummary)), ("keypoints", c_f64p), ("prev_index", c_i32p),
+                ("feature_counts", c_i32p), ("info", c_i32p), ("predict_q", c_f64p)]
+
+
 class CWindowSnapshot(C.Structure):
     _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("data", c_u8p), ("capacity", C.c_int64),
                 ("size", C.c_int64)]
@@ -226,6 +239,8 @@ SIGNATURES = {
     "pvio_b200_batch_window_plane_ransac": (_int, [_h, _int, _P(CWindowPlaneRansac)]),
     "pvio_b200_batch_window_set_keypoints": (_int, [_h, _int, _P(CWindowKeypoints)]),
     "pvio_b200_batch_window_mirror_frame": (_int, [_h, _int, _P(CWindowMirror), _P(COptions)]),
+    "pvio_b200_batch_window_track_camera": (_int, [_h, _int, _P(CWindowCamera), _int, _int, _f64, _f64, _int, _int, _int,
+                                                   _f64, _f64, _f64, _P(COptions)]),
     "pvio_b200_batch_window_save": (_int, [_h, _int, _P(CWindowSnapshot)]),
     "pvio_b200_batch_window_restore": (_int, [_h, _int, _P(CWindowSnapshot)]),
     "pvio_b200_sync": (_int, [_h]),

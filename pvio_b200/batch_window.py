@@ -143,6 +143,27 @@ class Mirror:
         self.given = dict(given or {})
 
 
+class Camera(Mirror):
+    """One new camera frame of one linked inertial slot (pvio_b200_window_camera) for track_camera: the raw image
+    (uint8 [h, w]) with frame_id, K (fx, fy, cx, cy; fx, fy as the slot's) and map_frames (> 0) for the tracker slot,
+    and the Mirror fields; samples are the frame's list after the prepend rule of feature_tracker.cpp:78-84."""
+
+    def __init__(self, slot, tracker_slot, frame_id, image, K, map_frames, samples, t_end, noise_cov,
+                 keep_samples=True, given=None):
+        super().__init__(slot, tracker_slot, samples, t_end, noise_cov, K[2], K[3], keep_samples, given)
+        self.frame_id, self.map_frames = int(frame_id), int(map_frames)
+        self.image = np.ascontiguousarray(image, dtype=np.uint8)
+        self.K = tuple(float(v) for v in K)
+
+
+def _mirror_out(max_keypoints):
+    """the output arrays of one mirror_frame record (kp_track filled with -7, the rest zero)"""
+    return dict(kp_track=np.full(max_keypoints, -7, dtype=np.int32), counts=np.zeros(4, dtype=np.int32),
+                state=np.zeros(16), predicted=np.zeros(16), imu_record=np.zeros(_lib.IMU_STRIDE),
+                keyframe=np.zeros(1, dtype=np.uint8), parallax=np.zeros(1), n_parallax=np.zeros(1, dtype=np.int32),
+                skipped_frames=np.zeros(1, dtype=np.int32))
+
+
 class BatchWindows:
     def __init__(self, ba):
         """ba: a BundleAdjustor (owns the device handle and its max_windows slots)."""
@@ -297,6 +318,51 @@ class BatchWindows:
             o["n_parallax"], o["skipped_frames"] = int(o["n_parallax"][0]), int(o["skipped_frames"][0])
         return out
 
+    def track_camera(self, records, max_keypoints, keypoint_distance=20.0, max_level=3, max_iter=30, eps=0.01,
+                     clahe_clip=6.0, clahe_tiles=(8, 8), border=20, ransac_threshold=1.0, ransac_confidence=0.99,
+                     max_iterations=10, initial_radius=0.0):
+        """batch_feature_track with the IMU prediction made on the device, then mirror_frame, of a list of Camera
+        (distinct slots and tracker slots) in one call.  Per record mirror_frame's dict plus n_keypoints, keypoints
+        [n_keypoints][2], prev_index [n_keypoints], feature_counts [4], info [4] and predict_q [4] (the delta_key_q
+        used)."""
+        recs, sms, out, keep = self.camera_records(records, max_keypoints)
+        opt = _lib.COptions(max_iterations, 1e6, 1, 0, initial_radius)
+        self.ba._ck(self.lib.pvio_b200_batch_window_track_camera(
+            self.h, len(records), recs, int(max_level), int(max_iter), float(eps), float(clahe_clip),
+            int(clahe_tiles[0]), int(clahe_tiles[1]), int(border), float(ransac_threshold), float(ransac_confidence),
+            float(keypoint_distance), C.byref(opt)))
+        for i, o in enumerate(out):
+            m = int(o["n_keypoints"][0])
+            o["n_keypoints"], o["keypoints"], o["prev_index"] = m, o["keypoints"][:m], o["prev_index"][:m]
+            o["summary"] = _lib.summary(sms[i])
+            o["keyframe"], o["parallax"] = bool(o["keyframe"][0]), float(o["parallax"][0])
+            o["n_parallax"], o["skipped_frames"] = int(o["n_parallax"][0]), int(o["skipped_frames"][0])
+        return out
+
+    @staticmethod
+    def camera_records(records, max_keypoints):
+        """the ctypes records of a list of Camera: (records, summaries, output arrays per record, arrays to keep)"""
+        keep, out, n = [], [], len(records)
+        recs, sms = (_lib.CWindowCamera * max(n, 1))(), (_lib.CSummary * max(n, 1))()
+        for i, M in enumerate(records):
+            r = recs[i]
+            o = _mirror_out(max_keypoints)
+            o.update(n_keypoints=np.full(1, -7, dtype=np.int32), keypoints=np.full((max_keypoints, 2), -7.0),
+                     prev_index=np.full(max_keypoints, -7, dtype=np.int32), feature_counts=np.zeros(4, dtype=np.int32),
+                     info=np.zeros(4, dtype=np.int32), predict_q=np.zeros(4))
+            out.append(o)
+            h, w = M.image.shape
+            r.slot, r.tracker_slot, r.frame_id, r.width, r.height, r.stride = M.slot, M.tracker_slot, M.frame_id, w, h, w
+            r.map_frames, (r.fx, r.fy, r.cx, r.cy), r.max_keypoints = M.map_frames, M.K, int(max_keypoints)
+            r.n_samples, r.t_end, r.keep_samples, r.summary = len(M.samples), M.t_end, int(M.keep), C.pointer(sms[i])
+            gt = np.array(list(M.given), dtype=np.int32)
+            gp = np.ascontiguousarray([M.given[t] for t in M.given], dtype=np.float64).reshape(-1, 3)
+            r.n_given = len(gt)
+            keep += [M.image, M.samples, M.noise, gt, gp]
+            _lib.set_ptrs(r, image=M.image, samples=M.samples, noise_cov=M.noise, given_track=gt if len(gt) else None,
+                          given_point=gp if len(gt) else None, **{k: o[k] for k in o})
+        return recs, sms, out, keep
+
     @staticmethod
     def mirror_records(records, max_keypoints):
         """the ctypes records of a list of Mirror: (records, summaries, output arrays per record, arrays to keep)"""
@@ -304,10 +370,7 @@ class BatchWindows:
         recs, sms = (_lib.CWindowMirror * max(n, 1))(), (_lib.CSummary * max(n, 1))()
         for i, M in enumerate(records):
             r = recs[i]
-            o = dict(kp_track=np.full(max_keypoints, -7, dtype=np.int32), counts=np.zeros(4, dtype=np.int32),
-                     state=np.zeros(16), predicted=np.zeros(16), imu_record=np.zeros(_lib.IMU_STRIDE),
-                     keyframe=np.zeros(1, dtype=np.uint8), parallax=np.zeros(1), n_parallax=np.zeros(1, dtype=np.int32),
-                     skipped_frames=np.zeros(1, dtype=np.int32))
+            o = _mirror_out(max_keypoints)
             out.append(o)
             r.slot, r.tracker_slot, r.n_samples, r.keep_samples = M.slot, M.tracker_slot, len(M.samples), int(M.keep)
             r.t_end, r.cx, r.cy, r.max_keypoints, r.summary = M.t_end, M.cx, M.cy, int(max_keypoints), C.pointer(sms[i])

@@ -99,8 +99,10 @@ struct SlotLens {
 // continues, or -1).  Right after a call buf[1 - cur] still holds the previous frame's keypoints: the link that
 // pvio_b200_batch_window_mirror_frame reads (batch_window.cu).
 struct SlotKeypoints {
-    DevBuf<uint8_t> buf[2];
-    size_t cap[2] = {0, 0};                   // keypoints each buffer holds
+    DevBuf<uint8_t> buf[3];                   // buf[2]: pvio_b200_batch_window_track_camera writes the new frame here and
+                                              // swaps it with buf[1 - cur] when the call commits, so that a rejected
+                                              // call leaves the previous frame's keypoints as they were
+    size_t cap[3] = {0, 0, 0};                // keypoints each buffer holds
     int cur = 0, n = 0;                       // newest buffer, its keypoint count
     bool live = false;                        // a sequence was started in this slot (map_frames == 0)
     int frame_no = 0;                         // the number of the newest frame (births count in these)
@@ -488,9 +490,34 @@ struct KltBatchResults {
 // replays each pair on the host and launches the winners' masks.  dev == nullptr: the points come from the items.
 int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchOptions &opt, const KltDevicePoints *dev,
                     KltBatchResults &res);
-// feature_track.cu: pvio_b200_batch_feature_track
+// feature_track.cu: pvio_b200_batch_feature_track, and its stages, which pvio_b200_batch_window_track_camera shares:
+// ft_check checks every request (outputs: keypoints, prev_index and n_keypoints must be given); ft_run stages,
+// launches and synchronises without changing any slot's keypoints; ft_finish writes the outputs and makes each slot's
+// newest frame the new one.
 int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
                              double keypoint_distance);
+// the device inputs of delta_key_q (frame.cpp:98), composed before the initial guesses: sequence i's step-1 IMU record
+// (delta q at +1) and the constants of its window slot
+struct FtPredict {
+    const double *rec;                        // [n][kImuStride]
+    const WinConst *cst;                      // the handle's window constants
+    const int32_t *slot;                      // sequence i's window slot at slot[i * slot_stride]
+    int slot_stride;
+    double *q_out;                            // [n][4] the delta_key_q written
+};
+struct FtRun {
+    std::vector<int> n_prev, out_cap;         // ft_check: keypoints of the previous frame, the output bound
+    std::vector<int> count, prev_no;          // ft_run: the new frame's keypoints, the previous frame's number
+    std::vector<size_t> out_off;
+    const uint8_t *head = nullptr, *out = nullptr;   // the downloaded counts and outputs
+    bool staged = false;                      // the new frames go to each slot's buf[2] (SlotKeypoints), not buf[1 - cur]
+    KltBatchResults r;
+};
+int ft_check(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
+             double keypoint_distance, bool outputs, FtRun &run);
+int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
+           double keypoint_distance, const FtPredict *pred, FtRun &run);
+int ft_finish(Handle *h, int n, const pvio_b200_feature_frame *frames, const FtRun &run);
 // fmat.cu
 int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double threshold, double confidence, int max_iters,
                    const int32_t *schedule, int n_schedule, uint8_t *mask, double *F_out, int32_t *info);

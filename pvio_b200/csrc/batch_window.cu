@@ -27,6 +27,7 @@
 #include <cstddef>
 #include <cstring>
 #include <memory>
+#include <optional>
 #include <vector>
 
 #include "api_internal.h"
@@ -2191,78 +2192,96 @@ int pvio_b200_batch_window_set_keypoints(pvio_b200_handle hh, int n, const pvio_
     return 0;
 }
 
-int pvio_b200_batch_window_mirror_frame(pvio_b200_handle hh, int n, pvio_b200_window_mirror *records,
-                                        const pvio_b200_options *opt) {
-    Handle *h = reinterpret_cast<Handle *>(hh);
-    if (!h) return PVIO_B200_EINVAL;
-    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_mirror_frame: bad record list");
-    if (n == 0) return 0;
-    std::vector<int32_t> slots(n);
-    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
-    TRY(check_slots(h, n, slots.data(), "batch_window_mirror_frame: bad slot list"));
-    auto bad = [h](const char *why) {
-        return fail(h, PVIO_B200_EINVAL, (std::string("batch_window_mirror_frame: ") + why).c_str());
-    };
-    // every record is checked against its slot's host mirror and its tracker slot before anything is staged
-    const KltBatchState &B = h->kltb;
-    std::vector<BwMirror> mir(n);
-    std::vector<BwLoc> locs(n);
-    std::vector<BwTrack> trs(n);
-    std::vector<BwEdit> eds(n);
-    std::vector<BwTrackJob> jobs;
+// ------------------------------------------------------------------------ mirror_frame's stages
+// A record's tracker slot as the mirror reads it: frame i (the slot's newest) and the new frame j with its prev_index.
+// n_j bounds the new frame's keypoints when the staging is laid out (track_camera lays it out before they exist) and
+// is their count when the mirror runs.
+struct MirView { const double2 *zi, *zj; const int32_t *prev; int n_i, n_j; };
+
+// One call of pvio_b200_batch_window_mirror_frame, or the mirror half of pvio_b200_batch_window_track_camera: the
+// checked records, their staging and the device views of track_frame's kernels.  Both calls run add for every record,
+// stage, then front, launch or their own split of it, check, append and commit.
+struct MirCall {
+    const char *what;
+    std::vector<int32_t> slots;
+    std::vector<BwMirror> mir;
+    std::vector<BwLoc> locs;
+    std::vector<BwTrack> trs;
+    std::vector<BwEdit> eds;
+    std::vector<BwTrackJob> jobs;             // per record its step-1 job, then its merged job (split: all step-1 first)
     std::vector<BwImu> kimu;                  // the factors that keep their samples, as set_imu stages them
     std::vector<double> kaux, gpt;
     std::vector<int32_t> grow;
-    std::vector<WinSlot> next(n);             // the slots' windows after the call, but for their row counts
+    std::vector<WinSlot> next;                // the slots' windows after the call, but for their row counts
     std::vector<uint8_t> taken;
-    std::vector<const SlotKeypoints *> kps(n);
     size_t kp = 0, tab = 0, rm = 0, rows = 0;
-    int smax = 0;
-    for (int i = 0; i < n; ++i) {
-        const pvio_b200_window_mirror &R = records[i];
+    int smax = 0, n1 = 0;                     // n1: the step-1 jobs (split)
+
+    Stage S;
+    Stage::Sec<BwMirror> mr;
+    Stage::Sec<BwLoc> lo;
+    Stage::Sec<BwTrack> tr;
+    Stage::Sec<BwTrackJob> job;
+    Stage::Sec<double> pq, smp, aux, gp, kax, frames, out, rec_out, pred, kfo, z, pts, nz, kf_z, rho, rho_next, par, rec1, xs;
+    Stage::Sec<int32_t> gr, cnt, live, kpt, eout, tabs, rmap, lrow, cand, row, kf_row;
+    Stage::Sec<BwEdit> ed;
+    Stage::Sec<BwImu> kim;
+    Stage::Sec<int2> cont;
+    Stage::Sec<uint8_t> valid;
+    Stage::Sec<PnpArgs> args;
+    Stage::Sec<BwNew> nw;
+    Stage::Sec<BwObs> ob;
+    std::optional<Relayout> lay;
+    LocArgs L;
+    TrackArgs T;
+    MirArgs M;
+
+    MirCall(const char *w, int n) : what(w), mir(n), locs(n), trs(n), eds(n), next(n) {}
+    int bad(Handle *h, const char *why) const { return fail(h, PVIO_B200_EINVAL, (std::string(what) + ": " + why).c_str()); }
+
+    // Record i checked against its slot's host mirror; tracker_why: the caller's verdict on the tracker slot (null:
+    // usable), checked after the link.  Returns null or why the record is rejected.
+    const char *add(Handle *h, int i, const pvio_b200_window_mirror &R, const MirView &v, const char *tracker_why,
+                    bool split) {
         const WinSlot &s = h->slots[R.slot];
-        if (!s.inertial) return bad("the window carries no motion states");
-        if (s.N < 1) return bad("a window without frames");
-        if (!s.link) return bad("the slot has no link to a tracker slot (set_keypoints)");
-        if (R.tracker_slot != s.link_tracker) return bad("not the tracker slot of the slot's link");
+        if (!s.inertial) return "the window carries no motion states";
+        if (s.N < 1) return "a window without frames";
+        if (!s.link) return "the slot has no link to a tracker slot (set_keypoints)";
+        if (R.tracker_slot != s.link_tracker) return "not the tracker slot of the slot's link";
         if ((size_t)R.tracker_slot >= taken.size()) taken.resize(R.tracker_slot + 1, 0);
-        if (taken[R.tracker_slot]) return bad("a tracker slot named twice");
+        if (taken[R.tracker_slot]) return "a tracker slot named twice";
         taken[R.tracker_slot] = 1;
-        const SlotKeypoints *K = (size_t)R.tracker_slot < B.kps.size() ? &B.kps[R.tracker_slot] : nullptr;
-        if (!K || !K->live || K->gen != s.link_gen || K->prev_frame_id == 0 || K->prev_frame_id != s.link_frame ||
-            s.link_kmax >= K->prev_n)
-            return bad("the tracker slot's previous frame is not the slot's newest frame");
-        kps[i] = K;
-        if (!R.samples || !R.noise_cov || !R.kp_track || !R.state || !R.keyframe) return bad("null array");
-        if (R.max_keypoints < K->n) return bad("max_keypoints below the tracker's keypoint count");
-        if (R.n_samples < 1) return bad("a frame without IMU samples (integrate() returns false, preintegrator.cpp:86)");
-        if (R.keep_samples != 0 && R.keep_samples != 1) return bad("keep_samples not 0 or 1");
-        if (!all_finite(R.samples, 7 * (int64_t)R.n_samples)) return bad("non-finite sample");
+        if (tracker_why) return tracker_why;
+        if (!R.samples || !R.noise_cov || !R.kp_track || !R.state || !R.keyframe) return "null array";
+        if (R.max_keypoints < v.n_j) return "max_keypoints below the tracker's keypoint count";
+        if (R.n_samples < 1) return "a frame without IMU samples (integrate() returns false, preintegrator.cpp:86)";
+        if (R.keep_samples != 0 && R.keep_samples != 1) return "keep_samples not 0 or 1";
+        if (!all_finite(R.samples, 7 * (int64_t)R.n_samples)) return "non-finite sample";
         if (!std::isfinite(R.t_end) || !all_finite(R.noise_cov, 36) || !std::isfinite(R.cx) || !std::isfinite(R.cy))
-            return bad("non-finite t_end, noise or principal point");
+            return "non-finite t_end, noise or principal point";
         const bool merged = !s.newest_kf;
-        if (merged && s.N < 2) return bad("a non-keyframe newest frame without a keyframe before it");
-        if (merged && s.N - 1 < s.n_prior) return bad("the newest frame is covered by the prior");
+        if (merged && s.N < 2) return "a non-keyframe newest frame without a keyframe before it";
+        if (merged && s.N - 1 < s.n_prior) return "the newest frame is covered by the prior";
         const int n_merge = merged ? s.n_samples[s.N - 2] : 0;
-        if (merged && n_merge < 1) return bad("a non-keyframe newest frame whose factor holds no samples");
-        if (!merged && s.N >= h->Ncap) return bad("window of more than max_frames frames");
-        if (R.n_given < 0 || (R.n_given > 0 && (!R.given_track || !R.given_point))) return bad("null array");
+        if (merged && n_merge < 1) return "a non-keyframe newest frame whose factor holds no samples";
+        if (!merged && s.N >= h->Ncap) return "window of more than max_frames frames";
+        if (R.n_given < 0 || (R.n_given > 0 && (!R.given_track || !R.given_point))) return "null array";
         std::vector<std::pair<int, int>> given;
         std::vector<uint8_t> named(s.ids.size(), 0);
         for (int k = 0; k < R.n_given; ++k) {
             const int r = find_row(s, R.given_track[k]);
-            if (r < 0) return bad("unknown or dead track");
-            if (named[r]) return bad("a track named twice");
+            if (r < 0) return "unknown or dead track";
+            if (named[r]) return "a track named twice";
             named[r] = 1;
-            if (!all_finite(R.given_point + 3 * k, 3)) return bad("non-finite given point");
+            if (!all_finite(R.given_point + 3 * k, 3)) return "non-finite given point";
             given.push_back({r, k});
         }
         std::sort(given.begin(), given.end());
         const int T = (int)s.ids.size(), fnew = merged ? s.N - 1 : s.N;
         const size_t first = rows;            // the call's sample rows: merge list ++ own samples per record
-        mir[i] = BwMirror{K->z(1 - K->cur), K->z(K->cur), K->prev(K->cur), R.slot, T, K->prev_n, K->n, (int32_t)tab,
-                          (int32_t)kp, (int32_t)grow.size(), R.n_given, (int32_t)rm, (int32_t)first, n_merge,
-                          merged ? 1 : 0, s.N, s.next_id, 0, 0};
+        slots.push_back(R.slot);
+        mir[i] = BwMirror{v.zi, v.zj, v.prev, R.slot, T, v.n_i, v.n_j, (int32_t)tab, (int32_t)kp, (int32_t)grow.size(),
+                          R.n_given, (int32_t)rm, (int32_t)first, n_merge, merged ? 1 : 0, s.N, s.next_id, 0, 0};
         for (const auto &g : given) {
             grow.push_back(g.first);
             gpt.insert(gpt.end(), R.given_point + 3 * g.second, R.given_point + 3 * g.second + 3);
@@ -2273,7 +2292,11 @@ int pvio_b200_batch_window_mirror_frame(pvio_b200_handle hh, int n, pvio_b200_wi
         eds[i] = BwEdit{R.slot, s.N, T, merged ? 1 : 0, 0, 0, fnew, 1, i * kMirX, 0, (int32_t)kp, 0, (int32_t)kp,
                         (int32_t)(kp + i)};
         const size_t b = first + n_merge, e = b + R.n_samples;
-        jobs.push_back(BwTrackJob{i, (int32_t)b, (int32_t)e, 0});
+        if (split) {
+            jobs.insert(jobs.begin() + n1++, BwTrackJob{i, (int32_t)b, (int32_t)e, 0});
+        } else {
+            jobs.push_back(BwTrackJob{i, (int32_t)b, (int32_t)e, 0});
+        }
         if (merged) jobs.push_back(BwTrackJob{i, (int32_t)first, (int32_t)e, 1});
         rows = e;
         const int n_list = n_merge + R.n_samples;
@@ -2284,167 +2307,319 @@ int pvio_b200_batch_window_mirror_frame(pvio_b200_handle hh, int n, pvio_b200_wi
             smax = std::max(smax, n_list);
         }
         next[i] = mirror_next(s, {}, 0, R.keep_samples ? n_list : 0);
-        kp += K->n; tab += 2 * (size_t)K->prev_n; rm += T;
-        if (rows > (size_t)INT32_MAX || kp + n > (size_t)INT32_MAX || tab > (size_t)INT32_MAX)
-            return bad("too many samples or keypoints in one call");
+        kp += v.n_j; tab += 2 * (size_t)v.n_i; rm += T;
+        if (rows > (size_t)INT32_MAX || kp + mir.size() > (size_t)INT32_MAX || tab > (size_t)INT32_MAX)
+            return "too many samples or keypoints in one call";
+        return nullptr;
     }
-
-    if (!kimu.empty()) TRY(ensure_imu_store(h, smax));   // the kept lists' room, before anything is staged
 
     // staging: upload records | track_frame's records, jobs, samples, t_end and noise | given points | edit records |
     // kept factors | re-layout; download counts | continued rows (the capacity check), then the results; device only
-    // the mirror's tables and lists, the localize sections, the edit's lists
-    const size_t w8 = sizeof(double);
-    Stage S;
-    const auto mr = S.up(mir);
-    const auto lo = S.up(locs);
-    const auto tr = S.up(trs);
-    const auto job = S.up(jobs);
-    const auto smp = S.add<double>(Stage::kUp, 7 * rows), aux = S.add<double>(Stage::kUp, (size_t)n * kImuAux);
-    const auto gr = S.up(grow);
-    const auto gp = S.up(gpt);
-    const auto ed = S.up(eds);
-    const auto kim = S.up(kimu);
-    const auto kax = S.up(kaux);
-    const Relayout lay(S, slots.data(), next);
-    const auto cnt = S.add<int32_t>(Stage::kDown, 4 * (size_t)n);
-    const auto live = S.add<int32_t>(Stage::kDown, n);
-    const auto frames = S.add<double>(Stage::kDown, 16 * (size_t)n), out = S.add<double>(Stage::kDown, 8 * (size_t)n);
-    const auto rec_out = S.add<double>(Stage::kDown, (size_t)n * kImuStride), pred = S.add<double>(Stage::kDown, 16 * (size_t)n);
-    const auto kfo = S.add<double>(Stage::kDown, 4 * (size_t)n);
-    const auto kpt = S.add<int32_t>(Stage::kDown, kp);
-    // the continued rows: downloaded once, for the capacity check
-    const auto cont = S.add<int2>(Stage::kScratch, kp);
-    const auto eout = S.add<int32_t>(Stage::kScratch, kp + n);
-    const auto tabs = S.add<int32_t>(Stage::kScratch, tab), rmap = S.add<int32_t>(Stage::kScratch, rm);
-    const auto lrow = S.add<int32_t>(Stage::kScratch, kp), cand = S.add<int32_t>(Stage::kScratch, kp);
-    const auto row = S.add<int32_t>(Stage::kScratch, kp), kf_row = S.add<int32_t>(Stage::kScratch, kp);
-    const auto z = S.add<double>(Stage::kScratch, 2 * kp), pts = S.add<double>(Stage::kScratch, 3 * kp);
-    const auto nz = S.add<double>(Stage::kScratch, 4 * kp), kf_z = S.add<double>(Stage::kScratch, 2 * kp);
-    const auto rho = S.add<double>(Stage::kScratch, kp), rho_next = S.add<double>(Stage::kScratch, kp);
-    const auto valid = S.add<uint8_t>(Stage::kScratch, kp);
-    const auto par = S.add<double>(Stage::kScratch, kp), rec1 = S.add<double>(Stage::kScratch, (size_t)n * kImuStride);
-    const auto args = S.add<PnpArgs>(Stage::kScratch, n);
-    const auto nw = S.add<BwNew>(Stage::kScratch, kp);
-    const auto ob = S.add<BwObs>(Stage::kScratch, kp);
-    const auto xs = S.add<double>(Stage::kScratch, (size_t)n * kMirX);
-    TRY(S.place(h));
-    for (int i = 0; i < n; ++i) {
-        const pvio_b200_window_mirror &R = records[i];
-        memcpy(S.host(smp) + 7 * ((size_t)mir[i].merge_row + mir[i].n_merge), R.samples, w8 * 7 * R.n_samples);
-        double *a = S.host(aux) + (size_t)i * kImuAux;
-        a[0] = R.t_end;
-        memcpy(a + 1, R.noise_cov, w8 * 36);
+    // the mirror's tables and lists, the localize sections, the edit's lists.  camera (track_camera): the continued rows are a
+    // download section right after the counts, so that one copy brings both back (they then come back with the
+    // results too), and the delta_key_q of every record comes back; otherwise they are device scratch, downloaded on
+    // their own (mirror_frame).  Uploads everything.
+    int stage(Handle *h, const pvio_b200_window_mirror *records, const pvio_b200_options *opt, bool camera) {
+        const int n = (int)mir.size();
+        if (!kimu.empty()) TRY(ensure_imu_store(h, smax));   // the kept lists' room, before anything is staged
+        const size_t w8 = sizeof(double);
+        mr = S.up(mir);
+        lo = S.up(locs);
+        tr = S.up(trs);
+        job = S.up(jobs);
+        smp = S.add<double>(Stage::kUp, 7 * rows); aux = S.add<double>(Stage::kUp, (size_t)n * kImuAux);
+        gr = S.up(grow);
+        gp = S.up(gpt);
+        ed = S.up(eds);
+        kim = S.up(kimu);
+        kax = S.up(kaux);
+        lay.emplace(S, slots.data(), next);
+        cnt = S.add<int32_t>(Stage::kDown, 4 * (size_t)n);
+        cont = S.add<int2>(camera ? Stage::kDown : Stage::kScratch, kp);
+        live = S.add<int32_t>(Stage::kDown, n);
+        frames = S.add<double>(Stage::kDown, 16 * (size_t)n); out = S.add<double>(Stage::kDown, 8 * (size_t)n);
+        rec_out = S.add<double>(Stage::kDown, (size_t)n * kImuStride); pred = S.add<double>(Stage::kDown, 16 * (size_t)n);
+        kfo = S.add<double>(Stage::kDown, 4 * (size_t)n);
+        kpt = S.add<int32_t>(Stage::kDown, kp);
+        if (camera) pq = S.add<double>(Stage::kDown, 4 * (size_t)n);
+        eout = S.add<int32_t>(Stage::kScratch, kp + n);
+        tabs = S.add<int32_t>(Stage::kScratch, tab); rmap = S.add<int32_t>(Stage::kScratch, rm);
+        lrow = S.add<int32_t>(Stage::kScratch, kp); cand = S.add<int32_t>(Stage::kScratch, kp);
+        row = S.add<int32_t>(Stage::kScratch, kp); kf_row = S.add<int32_t>(Stage::kScratch, kp);
+        z = S.add<double>(Stage::kScratch, 2 * kp); pts = S.add<double>(Stage::kScratch, 3 * kp);
+        nz = S.add<double>(Stage::kScratch, 4 * kp); kf_z = S.add<double>(Stage::kScratch, 2 * kp);
+        rho = S.add<double>(Stage::kScratch, kp); rho_next = S.add<double>(Stage::kScratch, kp);
+        valid = S.add<uint8_t>(Stage::kScratch, kp);
+        par = S.add<double>(Stage::kScratch, kp); rec1 = S.add<double>(Stage::kScratch, (size_t)n * kImuStride);
+        args = S.add<PnpArgs>(Stage::kScratch, n);
+        nw = S.add<BwNew>(Stage::kScratch, kp);
+        ob = S.add<BwObs>(Stage::kScratch, kp);
+        xs = S.add<double>(Stage::kScratch, (size_t)n * kMirX);
+        S.pow2 = camera;                      // laid out for output bounds that change from frame to frame
+        TRY(S.place(h));
+        for (int i = 0; i < n; ++i) {
+            const pvio_b200_window_mirror &R = records[i];
+            memcpy(S.host(smp) + 7 * ((size_t)mir[i].merge_row + mir[i].n_merge), R.samples, w8 * 7 * R.n_samples);
+            double *a = S.host(aux) + (size_t)i * kImuAux;
+            a[0] = R.t_end;
+            memcpy(a + 1, R.noise_cov, w8 * 36);
+        }
+        TRY(S.upload(h));
+        const SolveOptions so = solve_options(opt);
+        L.rec = S.dev(lo); L.row = S.dev(row); L.z = S.dev(z); L.imu = S.dev(rec1); L.nz = S.dev(nz);
+        L.frames = S.dev(frames); L.pts = S.dev(pts); L.out = S.dev(out); L.rho = S.dev(rho); L.rho_next = S.dev(rho_next);
+        L.valid = S.dev(valid); L.args = S.dev(args); L.max_iter = so.max_iter; L.radius0 = so.radius0;
+        T.tr = S.dev(tr); T.job = S.dev(job); T.kf_row = S.dev(kf_row); T.kf_z = S.dev(kf_z); T.smp = S.dev(smp);
+        T.aux = S.dev(aux); T.rec_out = S.dev(rec_out); T.pred = S.dev(pred); T.kfo = S.dev(kfo); T.rec1 = S.dev(rec1);
+        T.par = S.dev(par); T.n_jobs = (int)jobs.size();
+        M.rec = S.dev(mr); M.loc = S.dev(lo); M.tr = S.dev(tr); M.tab = S.dev(tabs); M.grow = S.dev(gr); M.gpt = S.dev(gp);
+        M.row = S.dev(row); M.z = S.dev(z); M.pts = S.dev(pts); M.nz = S.dev(nz); M.kf_row = S.dev(kf_row);
+        M.kf_z = S.dev(kf_z); M.smp = S.dev(smp); M.cont = S.dev(cont); M.cand = S.dev(cand); M.rmap = S.dev(rmap);
+        M.lrow = S.dev(lrow); M.kp = S.dev(kpt); M.cnt = S.dev(cnt); M.ed = S.dev(ed); M.nw = S.dev(nw); M.ob = S.dev(ob);
+        M.x = S.dev(xs); M.lay = S.dev(lay->lay); M.eout = S.dev(eout); M.live = S.dev(live);
+        return 0;
     }
-    TRY(S.upload(h));
-    const SolveOptions so = solve_options(opt);
-    LocArgs L;
-    L.rec = S.dev(lo); L.row = S.dev(row); L.z = S.dev(z); L.imu = S.dev(rec1); L.nz = S.dev(nz);
-    L.frames = S.dev(frames); L.pts = S.dev(pts); L.out = S.dev(out); L.rho = S.dev(rho); L.rho_next = S.dev(rho_next);
-    L.valid = S.dev(valid); L.args = S.dev(args); L.max_iter = so.max_iter; L.radius0 = so.radius0;
-    TrackArgs T;
-    T.tr = S.dev(tr); T.job = S.dev(job); T.kf_row = S.dev(kf_row); T.kf_z = S.dev(kf_z); T.smp = S.dev(smp);
-    T.aux = S.dev(aux); T.rec_out = S.dev(rec_out); T.pred = S.dev(pred); T.kfo = S.dev(kfo); T.rec1 = S.dev(rec1);
-    T.par = S.dev(par); T.n_jobs = (int)jobs.size();
-    MirArgs M;
-    M.rec = S.dev(mr); M.loc = S.dev(lo); M.tr = S.dev(tr); M.tab = S.dev(tabs); M.grow = S.dev(gr); M.gpt = S.dev(gp);
-    M.row = S.dev(row); M.z = S.dev(z); M.pts = S.dev(pts); M.nz = S.dev(nz); M.kf_row = S.dev(kf_row);
-    M.kf_z = S.dev(kf_z); M.smp = S.dev(smp); M.cont = S.dev(cont); M.cand = S.dev(cand); M.rmap = S.dev(rmap);
-    M.lrow = S.dev(lrow); M.kp = S.dev(kpt); M.cnt = S.dev(cnt); M.ed = S.dev(ed); M.nw = S.dev(nw); M.ob = S.dev(ob);
-    M.x = S.dev(xs); M.lay = S.dev(lay.lay); M.eout = S.dev(eout); M.live = S.dev(live);
-    // mirror, then track_frame's five kernels on its lists
-    BwArgs a = launch_args<BwArgs>(h);
-    bw_mirror_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    const int J = (int)jobs.size();
-    bw_track_integrate_kernel<<<(J + kBwImuWarps - 1) / kBwImuWarps, 32 * kBwImuWarps, 0, h->stream>>>(a, L, T);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    TRY(loc_launch(h, L, n));
-    bw_track_keyframe_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    TRY(S.download(h, cnt, cnt));
-    TRY(S.download(h, cont, cont));
-    CK(h, cudaStreamSynchronize(h->stream));
 
-    // capacity: the windows as they would be if every candidate turned out valid
-    std::vector<WinSlot> most(n);
-    for (int i = 0; i < n; ++i) {
-        const int32_t *c = S.host(cnt) + 4 * (size_t)i;
-        const int2 *cr = S.host(cont) + mir[i].kp_off;
-        std::vector<int> rws(c[0]);
-        for (int k = 0; k < c[0]; ++k) rws[k] = cr[k].x;
-        most[i] = mirror_next(h->slots[slots[i]], rws, c[2], 0);
-        TRY(check_window(h, most[i]));
-    }
-    TRY(ensure_plane_tables(h, most));        // observations of plane tracks may outgrow the plane tables
-
-    // append: the edit, the re-layout, the kept samples, the link
-    a = launch_args<BwArgs>(h);
-    bw_mirror_append_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T, M);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(a, S.dev(ed), nullptr, S.dev(nw), S.dev(ob), S.dev(xs), S.dev(eout));
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    TRY(lay.launch(h, S, false));
-    if (!kimu.empty()) {
-        bw_set_imu_kernel<<<(int)kimu.size(), kBwThreads, 0, h->stream>>>(a, S.dev(kim), S.dev(smp), S.dev(kax));
+    // bw_track_integrate_kernel on jobs [j0, j0 + nj); at least one CTA, so that the launches do not depend on the jobs
+    int integrate(Handle *h, int j0, int nj) {
+        TrackArgs t = T;
+        t.job = T.job + j0;
+        t.n_jobs = nj;
+        bw_track_integrate_kernel<<<std::max((nj + kBwImuWarps - 1) / kBwImuWarps, 1), 32 * kBwImuWarps, 0, h->stream>>>(
+            launch_args<BwArgs>(h), L, t);
         ++h->launches;
         CK(h, cudaGetLastError());
+        return 0;
     }
-    bw_mirror_link_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
-    ++h->launches;
-    CK(h, cudaGetLastError());
-    TRY(S.download(h));
-    CK(h, cudaStreamSynchronize(h->stream));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev0, h->ev1);
 
-    // the host mirrors from kp_track: continued tracks hold ids below the slot's next id, new tracks the next ids
+    // mirror, then track_frame's kernels on its lists; integrate_jobs: the integrate launch's jobs from j0
+    int launch(Handle *h, int j0) {
+        const int n = (int)mir.size();
+        const BwArgs a = launch_args<BwArgs>(h);
+        bw_mirror_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        TRY(integrate(h, j0, (int)jobs.size() - j0));
+        TRY(loc_launch(h, L, n));
+        bw_track_keyframe_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        return 0;
+    }
+
+    // the counts and continued rows down, a synchronisation, and the capacity: the windows as they would be if every
+    // candidate turned out valid
+    int check(Handle *h, bool camera) {
+        const int n = (int)mir.size();
+        if (camera) {
+            TRY(S.download(h, cnt, cont));
+        } else {
+            TRY(S.download(h, cnt, cnt));
+            TRY(S.download(h, cont, cont));
+        }
+        CK(h, cudaStreamSynchronize(h->stream));
+        std::vector<WinSlot> most(n);
+        for (int i = 0; i < n; ++i) {
+            const int32_t *c = S.host(cnt) + 4 * (size_t)i;
+            const int2 *cr = S.host(cont) + mir[i].kp_off;
+            std::vector<int> rws(c[0]);
+            for (int k = 0; k < c[0]; ++k) rws[k] = cr[k].x;
+            most[i] = mirror_next(h->slots[slots[i]], rws, c[2], 0);
+            TRY(check_window(h, most[i]));
+        }
+        return ensure_plane_tables(h, most);  // observations of plane tracks may outgrow the plane tables
+    }
+
+    // append: the edit, the re-layout, the kept samples, the link; the results down and a synchronisation
+    int append(Handle *h) {
+        const int n = (int)mir.size();
+        const BwArgs a = launch_args<BwArgs>(h);
+        bw_mirror_append_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L, T, M);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        bw_edit_kernel<<<n, kBwThreads, 0, h->stream>>>(a, S.dev(ed), nullptr, S.dev(nw), S.dev(ob), S.dev(xs), S.dev(eout));
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        TRY(lay->launch(h, S, false));
+        if (!kimu.empty()) {
+            bw_set_imu_kernel<<<(int)kimu.size(), kBwThreads, 0, h->stream>>>(a, S.dev(kim), S.dev(smp), S.dev(kax));
+            ++h->launches;
+            CK(h, cudaGetLastError());
+        }
+        bw_mirror_link_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        TRY(S.download(h));
+        CK(h, cudaStreamSynchronize(h->stream));
+        return 0;
+    }
+
+    // the host mirrors from kp_track (continued tracks hold ids below the slot's next id, new tracks the next ids) with
+    // the link to each tracker slot's new frame, committed; then the outputs
+    int commit_out(Handle *h, pvio_b200_window_mirror *records, const uint64_t *frame_id, const uint32_t *gen) {
+        const int n = (int)mir.size();
+        const size_t w8 = sizeof(double);
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+        for (int i = 0; i < n; ++i) {
+            const pvio_b200_window_mirror &R = records[i];
+            const WinSlot &s = h->slots[slots[i]];
+            const int32_t *k = S.host(kpt) + mir[i].kp_off;
+            std::vector<int> rws;
+            int n_new = 0, kmax = -1;
+            for (int j = 0; j < mir[i].n_j; ++j) {
+                if (k[j] < 0) continue;
+                kmax = j;
+                if (k[j] < s.next_id) rws.push_back(find_row(s, k[j])); else ++n_new;
+            }
+            const double *o = S.host(kfo) + 4 * (size_t)i;
+            next[i] = mirror_next(s, rws, n_new, R.keep_samples ? mir[i].n_merge + R.n_samples : 0);
+            next[i].link_frame = frame_id[i]; next[i].link_kmax = kmax; next[i].link_gen = gen[i];
+            next[i].newest_kf = o[0] != 0.0 ? 1 : 0; next[i].skipped = (int)o[3];
+        }
+        commit(h, slots.data(), next);
+        for (int i = 0; i < n; ++i) {
+            const pvio_b200_window_mirror &R = records[i];
+            if (S.host(live)[i] != (int32_t)h->slots[slots[i]].ids.size())
+                return fail(h, PVIO_B200_ECUDA, (std::string(what) + ": the device track table disagrees with the host's").c_str());
+            memcpy(R.kp_track, S.host(kpt) + mir[i].kp_off, sizeof(int32_t) * mir[i].n_j);
+            if (R.counts) memcpy(R.counts, S.host(cnt) + 4 * (size_t)i, sizeof(int32_t) * 4);
+            memcpy(R.state, S.host(frames) + 16 * (size_t)i, w8 * 16);
+            if (R.predicted) memcpy(R.predicted, S.host(pred) + 16 * (size_t)i, w8 * 16);
+            if (R.imu_record) memcpy(R.imu_record, S.host(rec_out) + (size_t)i * kImuStride, w8 * kImuStride);
+            const double *o = S.host(kfo) + 4 * (size_t)i;
+            *R.keyframe = o[0] != 0.0 ? 1 : 0;
+            if (R.parallax) *R.parallax = o[1];
+            if (R.n_parallax) *R.n_parallax = (int32_t)o[2];
+            if (R.skipped_frames) *R.skipped_frames = (int32_t)o[3];
+            if (R.summary) {
+                const double *b = S.host(out) + 8 * (size_t)i;
+                pvio_b200_summary &sm = *R.summary;
+                memset(&sm, 0, sizeof(sm));
+                sm.iterations = (int)b[0]; sm.accepted_steps = (int)b[1]; sm.termination = (int)b[2]; sm.usable = (int)b[3];
+                sm.initial_cost = b[4]; sm.final_cost = b[5]; sm.final_radius = b[6]; sm.final_mu = b[7];
+                sm.solve_seconds = ms * 1e-3;
+            }
+        }
+        return 0;
+    }
+};
+
+int pvio_b200_batch_window_mirror_frame(pvio_b200_handle hh, int n, pvio_b200_window_mirror *records,
+                                        const pvio_b200_options *opt) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_mirror_frame: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_mirror_frame: bad slot list"));
+    // every record is checked against its slot's host mirror and its tracker slot before anything is staged
+    const KltBatchState &B = h->kltb;
+    MirCall C("batch_window_mirror_frame", n);
+    std::vector<uint64_t> fid(n);
+    std::vector<uint32_t> gen(n);
     for (int i = 0; i < n; ++i) {
         const pvio_b200_window_mirror &R = records[i];
-        const WinSlot &s = h->slots[slots[i]];
-        const int32_t *k = S.host(kpt) + mir[i].kp_off;
-        std::vector<int> rws;
-        int n_new = 0, kmax = -1;
-        for (int j = 0; j < mir[i].n_j; ++j) {
-            if (k[j] < 0) continue;
-            kmax = j;
-            if (k[j] < s.next_id) rws.push_back(find_row(s, k[j])); else ++n_new;
-        }
-        const double *o = S.host(kfo) + 4 * (size_t)i;
-        next[i] = mirror_next(s, rws, n_new, R.keep_samples ? mir[i].n_merge + R.n_samples : 0);
-        next[i].link_frame = kps[i]->frame_id; next[i].link_kmax = kmax; next[i].link_gen = kps[i]->gen;
-        next[i].newest_kf = o[0] != 0.0 ? 1 : 0; next[i].skipped = (int)o[3];
+        const WinSlot &s = h->slots[R.slot];
+        const SlotKeypoints *K = R.tracker_slot >= 0 && (size_t)R.tracker_slot < B.kps.size() ? &B.kps[R.tracker_slot] : nullptr;
+        const bool ok = K && K->live && K->gen == s.link_gen && K->prev_frame_id != 0 && K->prev_frame_id == s.link_frame &&
+                        s.link_kmax < K->prev_n;
+        MirView v{};
+        if (ok) v = MirView{K->z(1 - K->cur), K->z(K->cur), K->prev(K->cur), K->prev_n, K->n};
+        if (const char *why = C.add(h, i, R, v, ok ? nullptr : "the tracker slot's previous frame is not the slot's newest frame",
+                                    false))
+            return C.bad(h, why);
+        fid[i] = K->frame_id; gen[i] = K->gen;
     }
-    commit(h, slots.data(), next);
+    TRY(C.stage(h, records, opt, false));
+    TRY(C.launch(h, 0));
+    TRY(C.check(h, false));
+    TRY(C.append(h));
+    return C.commit_out(h, records, fid.data(), gen.data());
+}
+
+int pvio_b200_batch_window_track_camera(pvio_b200_handle hh, int n, pvio_b200_window_camera *records, int max_level,
+                                        int max_iter, double eps, double clahe_clip, int tiles_x, int tiles_y,
+                                        int border, double ransac_threshold, double ransac_confidence,
+                                        double keypoint_distance, const pvio_b200_options *opt) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    if (n < 0 || (n > 0 && !records)) return fail(h, PVIO_B200_EINVAL, "batch_window_track_camera: bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_track_camera: bad slot list"));
+    // every record is checked, as feature_track and as mirror_frame (against the tracker slot before it advances), before
+    // anything is staged
+    const KltBatchOptions ko{max_level, max_iter, eps, clahe_clip, tiles_x, tiles_y, border, ransac_threshold,
+                             ransac_confidence};
+    std::vector<pvio_b200_feature_frame> ff(n);
+    std::vector<pvio_b200_window_mirror> mr(n);
     for (int i = 0; i < n; ++i) {
-        const pvio_b200_window_mirror &R = records[i];
-        if (S.host(live)[i] != (int32_t)h->slots[slots[i]].ids.size())
-            return fail(h, PVIO_B200_ECUDA, "batch_window_mirror_frame: the device track table disagrees with the host's");
-        memcpy(R.kp_track, S.host(kpt) + mir[i].kp_off, sizeof(int32_t) * mir[i].n_j);
-        if (R.counts) memcpy(R.counts, S.host(cnt) + 4 * (size_t)i, sizeof(int32_t) * 4);
-        memcpy(R.state, S.host(frames) + 16 * (size_t)i, w8 * 16);
-        if (R.predicted) memcpy(R.predicted, S.host(pred) + 16 * (size_t)i, w8 * 16);
-        if (R.imu_record) memcpy(R.imu_record, S.host(rec_out) + (size_t)i * kImuStride, w8 * kImuStride);
-        const double *o = S.host(kfo) + 4 * (size_t)i;
-        *R.keyframe = o[0] != 0.0 ? 1 : 0;
-        if (R.parallax) *R.parallax = o[1];
-        if (R.n_parallax) *R.n_parallax = (int32_t)o[2];
-        if (R.skipped_frames) *R.skipped_frames = (int32_t)o[3];
-        if (R.summary) {
-            const double *b = S.host(out) + 8 * (size_t)i;
-            pvio_b200_summary &sm = *R.summary;
-            memset(&sm, 0, sizeof(sm));
-            sm.iterations = (int)b[0]; sm.accepted_steps = (int)b[1]; sm.termination = (int)b[2]; sm.usable = (int)b[3];
-            sm.initial_cost = b[4]; sm.final_cost = b[5]; sm.final_radius = b[6]; sm.final_mu = b[7];
-            sm.solve_seconds = ms * 1e-3;
-        }
+        const pvio_b200_window_camera &R = records[i];
+        ff[i] = pvio_b200_feature_frame{R.tracker_slot, R.width, R.height, R.stride, R.frame_id, R.image, R.fx, R.fy,
+                                        R.cx, R.cy, R.map_frames, R.max_keypoints, nullptr, R.keypoints, R.prev_index,
+                                        R.n_keypoints, R.feature_counts, R.info};
+        mr[i] = pvio_b200_window_mirror{R.slot, R.tracker_slot, R.n_samples, R.keep_samples, R.samples, R.t_end,
+                                        R.noise_cov, R.cx, R.cy, R.n_given, R.given_track, R.given_point,
+                                        R.max_keypoints, R.kp_track, R.counts, R.state, R.predicted, R.imu_record,
+                                        R.keyframe, R.parallax, R.n_parallax, R.skipped_frames, R.summary};
     }
-    return 0;
+    MirCall C("batch_window_track_camera", n);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_camera &R = records[i];
+        if (!h->slots[R.slot].inertial) return C.bad(h, "the window carries no motion states");
+        if (R.map_frames == 0) return C.bad(h, "map_frames 0 (a sequence start goes through batch_feature_track)");
+        if (!R.n_keypoints) return C.bad(h, "null array");
+        if (R.fx != h->cst.h[R.slot].fx || R.fy != h->cst.h[R.slot].fy) return C.bad(h, "fx, fy not the slot's");
+    }
+    FtRun run;
+    run.staged = true;
+    TRY(ft_check(h, n, ff.data(), ko, keypoint_distance, false, run));
+    const KltBatchState &B = h->kltb;
+    std::vector<uint64_t> fid(n);
+    std::vector<uint32_t> gen(n);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_camera &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        const SlotKeypoints &K = B.kps[R.tracker_slot];     // ft_check found it live with its newest frame cached
+        const bool ok = K.gen == s.link_gen && K.frame_id == s.link_frame && s.link_kmax < K.n;
+        const MirView v{K.z(K.cur), nullptr, nullptr, K.n, run.out_cap[i]};
+        if (const char *why = C.add(h, i, mr[i], v, ok ? nullptr : "the tracker slot's newest frame is not the slot's newest frame",
+                                    true))
+            return C.bad(h, why);
+        fid[i] = R.frame_id; gen[i] = K.gen;
+    }
+
+    // the mirror's staging, laid out for every new frame's output bound and uploaded; the step-1 integration and
+    // prediction from each slot's newest frame; the feature stages with delta_key_q composed from it on the device
+    TRY(C.stage(h, mr.data(), opt, true));
+    TRY(C.integrate(h, 0, C.n1));
+    static_assert(offsetof(BwLoc, slot) == 0 && sizeof(BwLoc) % sizeof(int32_t) == 0,
+                  "ft_predict_kernel reads each record's window slot from the staged BwLoc records");
+    const FtPredict pred{C.S.dev(C.rec1), launch_args<BwArgs>(h).cst, &C.S.dev(C.lo)->slot,
+                         (int)(sizeof(BwLoc) / sizeof(int32_t)), C.S.dev(C.pq)};
+    TRY(ft_run(h, n, ff.data(), ko, keypoint_distance, &pred, run));
+    for (int i = 0; i < n; ++i)
+        if (run.count[i] > run.out_cap[i]) return C.bad(h, "more keypoints than the stated bound");
+
+    // the new frames into the mirror's records; mirror, track_frame's kernels, the capacity check, the append; then the
+    // tracker slots and the window slots commit
+    for (int i = 0; i < n; ++i) {
+        const SlotKeypoints &K = B.kps[records[i].tracker_slot];
+        BwMirror &m = C.S.host(C.mr)[i];
+        m.zj = K.z(2); m.prev = K.prev(2); m.n_j = run.count[i];
+        C.mir[i] = m;
+    }
+    TRY(C.S.upload(h, C.mr));
+    TRY(C.launch(h, C.n1));
+    TRY(C.check(h, true));
+    TRY(C.append(h));
+    TRY(ft_finish(h, n, ff.data(), run));
+    for (int i = 0; i < n; ++i)
+        if (records[i].predict_q) memcpy(records[i].predict_q, C.S.host(C.pq) + 4 * (size_t)i, sizeof(double) * 4);
+    return C.commit_out(h, mr.data(), fid.data(), gen.data());
 }
 
 int pvio_b200_batch_window_save(pvio_b200_handle hh, int n, pvio_b200_window_snapshot *records) {

@@ -102,6 +102,7 @@ struct Stage {
     std::vector<Entry> secs;
     size_t end[kKinds] = {};                  // after place: the end of each kind's sections
     uint8_t *hp = nullptr, *dp = nullptr;
+    bool pow2 = false;                        // grow BatchWindows::stage to a power of two (sizes that vary per call)
 
     // n elements of kind k; src (n elements, or null): what place copies into the section
     template <typename T>
@@ -125,7 +126,10 @@ struct Stage {
                 if (e.kind == k) { e.off = o; o += (e.bytes + 7) & ~(size_t)7; }
             end[k] = o;
         }
-        TRY(reserve(h, h->bw.stage, o, kBoth));
+        size_t want = o;
+        if (pow2)
+            for (want = 4096; want < o; want <<= 1) {}
+        TRY(reserve(h, h->bw.stage, want, kBoth));
         hp = h->bw.stage.h; dp = h->bw.stage.d;
         for (const Entry &e : secs)
             if (e.src && e.bytes) memcpy(hp + e.off, e.src, e.bytes);
@@ -138,6 +142,13 @@ struct Stage {
     int download(Handle *h) const {
         if (end[kDown] > end[kUp])
             CK(h, cudaMemcpyAsync(hp + end[kUp], dp + end[kUp], end[kDown] - end[kUp], cudaMemcpyDeviceToHost, h->stream));
+        return 0;
+    }
+    // one upload section again, after the host has rewritten it
+    template <typename A>
+    int upload(Handle *h, Sec<A> a) const {
+        if (secs[a.i].bytes)
+            CK(h, cudaMemcpyAsync(dp + secs[a.i].off, hp + secs[a.i].off, secs[a.i].bytes, cudaMemcpyHostToDevice, h->stream));
         return 0;
     }
     // sections a .. b (declared in that order, one kind) back to the host in one copy

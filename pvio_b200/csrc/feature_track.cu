@@ -186,22 +186,40 @@ __global__ void ft_commit_kernel(const FtSeq *seqs, const DetectResult *res) {
     if (lane == 0) { s.head[0] = ns + m; s.head[4] = m; }
 }
 
+// track_camera's prediction: delta_key_q of frame.cpp:98, (cam_q^* imu_q dq imu_q^* cam_q)^* with the extrinsics of the
+// sequence's window slot and dq of its step-1 IMU record, each product eigen_qmul (uncontracted: this unit is built
+// with -fmad=false), written into the staged FtSeq before ft_guess_kernel reads it
+__global__ void ft_predict_kernel(FtSeq *seqs, int n, FtPredict p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const WinConst &c = p.cst[p.slot[(size_t)i * p.slot_stride]];
+    const double *dq = p.rec + (size_t)i * kImuStride + 1;
+    const double cq[4] = {-c.cam_q[0], -c.cam_q[1], -c.cam_q[2], c.cam_q[3]};
+    const double iq[4] = {-c.imu_q[0], -c.imu_q[1], -c.imu_q[2], c.imu_q[3]};
+    double u[4], v[4];
+    eigen_qmul(cq, c.imu_q, u);
+    eigen_qmul(u, dq, v);
+    eigen_qmul(v, iq, u);
+    eigen_qmul(u, c.cam_q, v);
+    const double q[4] = {-v[0], -v[1], -v[2], v[3]};
+    for (int k = 0; k < 4; ++k) { seqs[i].q[k] = q[k]; p.q_out[4 * (size_t)i + k] = q[k]; }
+    seqs[i].use_q = 1;
+}
+
 }  // namespace
 
-// Every request is checked first.  Then: the tracker's stages (klt_batch_track) with the points written by
-// ft_guess_kernel right after its upload; after its replay one H2D copy (masks' outcome, detector descriptors, zeroed
-// counters), ft_thin_kernel, the detector's 4 launches, ft_commit_kernel, one D2H copy of every output, a synchronise;
-// then each slot's buffers swap.
-int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
-                             double keypoint_distance) {
-    if (n < 0 || n > kMaxFeatureFrames) return fail(h, PVIO_B200_EINVAL, "batch_feature_track: bad frame count");
-    if (n == 0) return 0;
+// Every request is checked, and each gets its previous frame's keypoint count and its output bound.  outputs: the
+// keypoints, prev_index and n_keypoints arrays are required.
+int ft_check(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
+             double keypoint_distance, bool outputs, FtRun &run) {
+    if (n < 1 || n > kMaxFeatureFrames) return fail(h, PVIO_B200_EINVAL, "batch_feature_track: bad frame count");
     if (!frames || !(keypoint_distance > 0.0) || !std::isfinite(keypoint_distance))
         return fail(h, PVIO_B200_EINVAL, "batch_feature_track: bad arguments");
     KltBatchState &B = h->kltb;
     const double gs = keypoint_distance / std::sqrt(2.0);
     std::vector<uint8_t> taken;
-    std::vector<int> n_prev(n, 0);
+    std::vector<int> &n_prev = run.n_prev;
+    n_prev.assign(n, 0);
     for (int i = 0; i < n; ++i) {
         const pvio_b200_feature_frame &a = frames[i];
         if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_feature_track: slot out of range");
@@ -209,7 +227,7 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
         if (taken[a.slot]) return fail(h, PVIO_B200_EINVAL, "batch_feature_track: a slot appears twice");
         taken[a.slot] = 1;
         if (a.width < kKltMinFrame || a.height < kKltMinFrame || a.stride < a.width || !a.frame_id || !a.image ||
-            a.map_frames < 0 || !a.keypoints || !a.prev_index || !a.n_keypoints)
+            a.map_frames < 0 || (outputs && (!a.keypoints || !a.prev_index || !a.n_keypoints)))
             return fail(h, PVIO_B200_EINVAL, "batch_feature_track: bad shape, stride, frame id, pixels or outputs");
         if (!(a.fx != 0.0 && a.fy != 0.0 && std::isfinite(a.fx) && std::isfinite(a.fy) && std::isfinite(a.cx) &&
               std::isfinite(a.cy)))
@@ -228,6 +246,21 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
         n_prev[i] = K->n;
     }
     if (taken.size() > B.kps.size()) B.kps.resize(taken.size());
+    run.out_cap.resize(n);
+    for (int i = 0; i < n; ++i)
+        run.out_cap[i] = (int)std::min<long long>(frames[i].max_keypoints, (long long)n_prev[i] + kMaxCorners);
+    return 0;
+}
+
+// The tracker's stages (klt_batch_track) with the points written by ft_guess_kernel right after its upload (pred, when
+// given: after ft_predict_kernel has written each sequence's delta_key_q); after its replay one H2D copy (masks'
+// outcome, detector descriptors, zeroed counters), ft_thin_kernel, the detector's 4 launches, ft_commit_kernel, one D2H
+// copy of every output, a synchronise.  No slot's keypoints change.
+int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
+           double keypoint_distance, const FtPredict *pred, FtRun &run) {
+    KltBatchState &B = h->kltb;
+    const double gs = keypoint_distance / std::sqrt(2.0);
+    const std::vector<int> &n_prev = run.n_prev;
 
     // the tracker's pairs: a new sequence has no previous frame and no points
     std::vector<KltBatchItem> items(n);
@@ -251,7 +284,7 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
     for (int i = 0; i < n; ++i) {
         const pvio_b200_feature_frame &a = frames[i];
         Plan &P = plan[i];
-        P.out_cap = (int)std::min<long long>(a.max_keypoints, (long long)n_prev[i] + kMaxCorners);
+        P.out_cap = run.out_cap[i];
         P.out_off = out_bytes;
         out_bytes += align256((sizeof(double2) + sizeof(int)) * (size_t)P.out_cap);
         P.hbits = 1;
@@ -300,8 +333,9 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
     // each slot's other buffer holds this frame's keypoints
     for (int i = 0; i < n; ++i) {
         SlotKeypoints &K = B.kps[frames[i].slot];
-        const int b = 1 - K.cur;
-        const size_t need = std::max<size_t>(plan[i].out_cap, 1024);
+        const int b = run.staged ? 2 : 1 - K.cur;
+        // the staged buffer rotates through all three: sized for the stated bound, so each is allocated once
+        const size_t need = std::max<size_t>(run.staged ? frames[i].max_keypoints : plan[i].out_cap, 1024);
         if (K.cap[b] < (size_t)plan[i].out_cap) {
             TRY(alloc(h, K.buf[b], SlotKeypoints::bytes(need), kDevice));
             K.cap[b] = need;
@@ -317,7 +351,7 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
         const SlotKeypoints &K = B.kps[a.slot];
         FtSeq &S = seq[i];
         memset(&S, 0, sizeof(S));
-        const int cb = K.cur, nb = 1 - K.cur;
+        const int cb = K.cur, nb = run.staged ? 2 : 1 - K.cur;
         S.z_prev = K.z(cb);
         S.birth_prev = K.birth(cb);
         S.z_next = K.z(nb);
@@ -344,13 +378,18 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
     cudaStream_t st = h->stream;
     const FtSeq *d_seq = reinterpret_cast<const FtSeq *>(ds + o_seq);
     CK(h, cudaMemcpyAsync(ds + o_seq, hs + o_seq, o_fm - o_seq, cudaMemcpyHostToDevice, st));
+    if (pred) {
+        ft_predict_kernel<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<FtSeq *>(ds + o_seq), n, *pred);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+    }
     KltDevicePoints dev;
     dev.write_points = [&](Handle *hh, float *prev_pts, float *next_pts, const int *pair_of) -> int {
         ft_guess_kernel<<<(unsigned)((pre + 255) / 256), 256, 0, st>>>(d_seq, pair_of, prev_pts, next_pts, (int)pre);
         ++hh->launches;
         return 0;
     };
-    KltBatchResults r;
+    KltBatchResults &r = run.r;
     TRY(klt_batch_track(h, n, items.data(), opt, &dev, r));
 
     // after the replay: each sequence's F-RANSAC outcome and detector descriptor, on the frame just cached
@@ -394,33 +433,59 @@ int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *fr
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(hs + o_head, ds + o_head, o - o_head, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
+    run.count.resize(n);
+    run.out_off.resize(n);
+    run.prev_no.resize(n);
+    run.head = hs + o_head;
+    run.out = hs + o_out;
+    for (int i = 0; i < n; ++i) {
+        run.count[i] = reinterpret_cast<const int *>(hs + o_head)[8 * i];
+        run.out_off[i] = plan[i].out_off;
+        run.prev_no[i] = seq[i].prev_no;
+    }
+    return 0;
+}
 
-    // outputs, and each slot's newest frame is now this one
+// The outputs (keypoints and prev_index where given), and each slot's newest frame is now this one
+int ft_finish(Handle *h, int n, const pvio_b200_feature_frame *frames, const FtRun &run) {
+    KltBatchState &B = h->kltb;
     bool overflow = false;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_feature_frame &a = frames[i];
-        const Plan &P = plan[i];
-        const int *hd = reinterpret_cast<const int *>(hs + o_head) + 8 * i;
-        const int m = hd[0];
-        overflow |= m > P.out_cap;
-        const int w = std::min(m, P.out_cap);
-        memcpy(a.keypoints, hs + o_out + P.out_off, sizeof(double2) * w);
-        memcpy(a.prev_index, hs + o_out + P.out_off + sizeof(double2) * P.out_cap, sizeof(int) * w);
+        const int *hd = reinterpret_cast<const int *>(run.head) + 8 * i;
+        const int m = hd[0], cap = run.out_cap[i];
+        overflow |= m > cap;
+        const int w = std::min(m, cap);
+        if (a.keypoints) memcpy(a.keypoints, run.out + run.out_off[i], sizeof(double2) * w);
+        if (a.prev_index) memcpy(a.prev_index, run.out + run.out_off[i] + sizeof(double2) * cap, sizeof(int) * w);
         *a.n_keypoints = m;
         if (a.counts) memcpy(a.counts, hd + 1, sizeof(int32_t) * 4);
-        if (a.info) memcpy(a.info, &r.info[4 * (size_t)i], sizeof(int32_t) * 4);
+        if (a.info) memcpy(a.info, &run.r.info[4 * (size_t)i], sizeof(int32_t) * 4);
         SlotKeypoints &K = B.kps[a.slot];
         K.prev_frame_id = a.map_frames > 0 ? K.frame_id : 0;     // map_frames == 0: the link to the previous frame goes
         K.prev_n = a.map_frames > 0 ? K.n : 0;
         if (a.map_frames == 0) ++K.gen;
+        if (run.staged) {
+            std::swap(K.buf[1 - K.cur], K.buf[2]);
+            std::swap(K.cap[1 - K.cur], K.cap[2]);
+        }
         K.cur = 1 - K.cur;
         K.n = w;
         K.live = true;
-        K.frame_no = seq[i].prev_no + 1;
+        K.frame_no = run.prev_no[i] + 1;
         K.frame_id = a.frame_id;
         K.fx = a.fx; K.fy = a.fy; K.cx = a.cx; K.cy = a.cy;
     }
     return overflow ? fail(h, PVIO_B200_EINVAL, "batch_feature_track: more keypoints than the stated bound") : 0;
+}
+
+int batch_feature_track_impl(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBatchOptions &opt,
+                             double keypoint_distance) {
+    if (n == 0) return 0;
+    FtRun run;
+    TRY(ft_check(h, n, frames, opt, keypoint_distance, true, run));
+    TRY(ft_run(h, n, frames, opt, keypoint_distance, nullptr, run));
+    return ft_finish(h, n, frames, run);
 }
 
 }  // namespace pvio
