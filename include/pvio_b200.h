@@ -763,6 +763,76 @@ typedef struct pvio_b200_window_snapshot {
 int pvio_b200_batch_window_save(pvio_b200_handle h, int n, pvio_b200_window_snapshot *records);
 int pvio_b200_batch_window_restore(pvio_b200_handle h, int n, const pvio_b200_window_snapshot *records);
 
+/* IMU stream slots: the IMU side of PVIO::Core for many sequences, one stream slot per sequence (slots 0 .. 65535,
+ * independent of window and tracker slots).  A record gives a sequence's new events in arrival order, each a row
+ * (kind, t, x, y, z): a gyroscope reading (rad/s), an accelerometer reading (m/s^2) or a camera timestamp (x, y, z
+ * unused).  The call restates, event by event, Core::track_gyroscope / track_accelerometer (core.cpp:59-107), the frame
+ * enqueue of Core::track_camera (:109-127), Core::track_imu (:129-141) and Core::predict_pose (:143-164) with
+ * propagate_state (:32-39), and applies FeatureTracker::work's prepend rule (feature_tracker.cpp:78-84) to each frame
+ * it releases, against the previously released frame's list, which the slot keeps.
+ *  - poses: each consumed event's OutputPose, q = state.q * output_q and p = state.p + state.q * output_p (q xyzw, p),
+ *    the slot's latest state propagated over its kept samples with t <= the event's t; all zero while the slot has no
+ *    latest state.
+ *  - released frames: when a sample releases pending camera frames (track_imu's else branch), each frame's timestamp
+ *    frame_t[k], its row count frame_rows[k] and its rows, back to back in rows ([t, w xyz, a xyz]) with the prepend
+ *    rule applied: the list pvio_b200_window_camera / pvio_b200_window_mirror take as samples.
+ *  - Lockstep rule (the reference's frontend runs asynchronously; this makes it deterministic): a record's events are
+ *    consumed up to and including the first event that releases a frame, and n_consumed says how many.  The caller
+ *    runs the released frames through the frontend (pvio_b200_batch_window_track_camera, or batch_feature_track before
+ *    initialisation), then calls again with the rest and the new latest state.  The releasing event's own pose uses
+ *    the latest state from before the release (the frontend has only just been handed the frame).
+ *  - Latest state: state_op PVIO_B200_IMU_STREAM_SET gives the slot a new latest state before the events, the 16-double
+ *    `predicted` of track_camera / mirror_frame / track_frame with its frame time; CLEAR removes it
+ *    (feature_tracker.cpp:74); KEEP leaves it.  The next pose computed with a new state first drops the kept samples with
+ *    t <= state_time, as predict_pose does.
+ *    While the slot has no state, each release drops the kept samples with t <= the released frame's time: the next
+ *    state is that frame's or a later one's (DESIGN 4.7h).
+ *  - Size query: a call in which any record's rows is NULL writes need_frames / need_rows of every record and does
+ *    nothing else.  need_rows bounds the released rows: unreleased samples + queued accelerometer readings + the
+ *    record's accelerometer readings + need_frames (pending frames + the record's camera events).
+ *  - Deviation from the reference: a gyroscope or accelerometer time below that stream's previous one is rejected (the
+ *    reference's output then depends on the order of its unsorted sample queue).
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no stream slot and no output has changed.
+ * Rejected: n < 0; a slot out of range, named twice or never reset; n_events < 0; a NULL events or poses with events;
+ * an unknown kind, state_op or a value that is not finite; a gyroscope or accelerometer time below that stream's
+ * previous one; a SET state with a NULL state, or older than a frame released while the slot had no state; a queue that
+ * could exceed PVIO_B200_IMU_STREAM_MAX_QUEUE entries (its size plus the record's readings that could enter it: the
+ * reference's queues grow without bound on a gyroscope stream with no accelerometer and on samples before the first
+ * camera frame); max_frames or max_rows below need_frames / need_rows.
+ * Launches, whatever n is: one host -> device copy, one kernel (one thread per record), one device -> host copy, one
+ * synchronisation; a call that grows the slots' queues first copies them into the larger buffers.  fp64, no fused
+ * multiply-adds, Eigen's scalar evaluation order (DESIGN 4.7h).
+ * reset: n stream slots (each once) emptied, latest state cleared, with their output extrinsic (Config
+ * output_to_body_rotation [4] xyzw / translation [3] per slot). */
+#define PVIO_B200_IMU_EVENT_GYROSCOPE 0
+#define PVIO_B200_IMU_EVENT_ACCELEROMETER 1
+#define PVIO_B200_IMU_EVENT_CAMERA 2
+#define PVIO_B200_IMU_STREAM_KEEP 0
+#define PVIO_B200_IMU_STREAM_SET 1
+#define PVIO_B200_IMU_STREAM_CLEAR 2
+#define PVIO_B200_IMU_STREAM_MAX_QUEUE 65536
+typedef struct pvio_b200_imu_stream_record {
+    int32_t slot;
+    int32_t n_events;
+    const double *events;             /* [n_events][5] kind, t, x, y, z */
+    int32_t state_op;                 /* PVIO_B200_IMU_STREAM_KEEP / SET / CLEAR, applied before the events */
+    double state_time;                /* SET: the state's frame time */
+    const double *state;              /* SET: [16] q xyzw, p, v, bg, ba */
+    double *poses;                    /* out [n_events][7] q xyzw, p: the first n_consumed rows */
+    int32_t max_frames;               /* room at frame_t / frame_rows */
+    int64_t max_rows;                 /* rows of room at rows */
+    double *frame_t;                  /* out [max_frames] */
+    int32_t *frame_rows;              /* out [max_frames] */
+    double *rows;                     /* out [max_rows][7] t, w xyz, a xyz; NULL: size query */
+    int32_t n_consumed;               /* out */
+    int32_t n_frames;                 /* out: frames released */
+    int32_t need_frames;              /* out: the room the record needs */
+    int64_t need_rows;                /* out */
+} pvio_b200_imu_stream_record;        /* 112 bytes on LP64 */
+int pvio_b200_batch_imu_stream_reset(pvio_b200_handle h, int n, const int32_t *slots, const double *output_q,
+                                     const double *output_p);
+int pvio_b200_batch_imu_stream(pvio_b200_handle h, int n, pvio_b200_imu_stream_record *records);
+
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */
 int pvio_b200_timer_start(pvio_b200_handle h);

@@ -27,6 +27,9 @@ LENS_RADTAN, LENS_EQUIDISTANT = 1, 2
 PLANE_EXTRACT, PLANE_REFIT = 0, 1
 PLANE_ACCEPTED, PLANE_FEW_POINTS, PLANE_REJECTED = 0, 1, 2
 SNAPSHOT_MAGIC, SNAPSHOT_VERSION = 1314084432, 1
+IMU_EVENT_GYROSCOPE, IMU_EVENT_ACCELEROMETER, IMU_EVENT_CAMERA = 0, 1, 2
+IMU_STREAM_KEEP, IMU_STREAM_SET, IMU_STREAM_CLEAR = 0, 1, 2
+IMU_STREAM_MAX_QUEUE = 65536
 
 c_i32p = C.POINTER(C.c_int32)
 c_u8p = C.POINTER(C.c_uint8)
@@ -171,6 +174,13 @@ class CWindowSnapshot(C.Structure):
                 ("size", C.c_int64)]
 
 
+class CImuStreamRecord(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n_events", C.c_int32), ("events", c_f64p), ("state_op", C.c_int32),
+                ("state_time", C.c_double), ("state", c_f64p), ("poses", c_f64p), ("max_frames", C.c_int32),
+                ("max_rows", C.c_int64), ("frame_t", c_f64p), ("frame_rows", c_i32p), ("rows", c_f64p),
+                ("n_consumed", C.c_int32), ("n_frames", C.c_int32), ("need_frames", C.c_int32), ("need_rows", C.c_int64)]
+
+
 class CLens(C.Structure):
     _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
@@ -243,6 +253,8 @@ SIGNATURES = {
                                                    _f64, _f64, _f64, _P(COptions)]),
     "pvio_b200_batch_window_save": (_int, [_h, _int, _P(CWindowSnapshot)]),
     "pvio_b200_batch_window_restore": (_int, [_h, _int, _P(CWindowSnapshot)]),
+    "pvio_b200_batch_imu_stream_reset": (_int, [_h, _int, c_i32p, c_f64p, c_f64p]),
+    "pvio_b200_batch_imu_stream": (_int, [_h, _int, _P(CImuStreamRecord)]),
     "pvio_b200_sync": (_int, [_h]),
     "pvio_b200_timer_start": (_int, [_h]),
     "pvio_b200_timer_stop": (_int, [_h, c_f32p]),

@@ -18,7 +18,7 @@ def _extra(name):
     undistort.cu's host-side map builder without fused multiply-adds, which GCC forms by default where the target has
     them (aarch64)"""
     if name.endswith(("klt.cu", "detect.cu", "fmat.cu", "twoview.cu", "feature_track.cu",
-                             "plane_ransac.cu")):
+                             "plane_ransac.cu", "imu_stream.cu")):
         return ["-fmad=false"]
     if name.endswith("undistort.cu"):
         return ["-Xcompiler", "-ffp-contract=off"]

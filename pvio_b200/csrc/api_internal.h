@@ -170,6 +170,29 @@ struct TwoViewState {
     DevBuf<uint8_t> scratch;                  // device: lots, models of every iteration, parallax, candidate scores
 };
 
+// imu_stream.cu: the IMU stream slots (pvio_b200_batch_imu_stream).  The device keeps each slot's queues ([slot][Qcap]
+// rows, live at [head, head + n) and moved to the front at the start of every call) and its ImuStreamSlot header; the
+// host keeps what checking a record needs: the queue sizes after the last call, the last reading time of each stream,
+// whether the slot has a latest state, and the newest frame released without one.
+struct ImuStreamHost {
+    bool set = false;                 // reset at least once
+    bool has_state = false;
+    double last_g = 0, last_a = 0;    // last gyroscope / accelerometer time (valid once n_g / n_a readings were seen)
+    bool seen_g = false, seen_a = false;
+    double t_drop = 0;                // newest frame time released without a state (samples up to it are dropped)
+    bool dropped = false;
+    int64_t g = 0, a = 0, s = 0, f = 0, k = 0;   // queue sizes: gyroscope, accelerometer, unreleased samples, pending
+                                                 // frames, kept samples
+};
+struct ImuStreams {
+    int slots = 0;                    // slots allocated on the device
+    int qcap = 0;                     // rows per queue per slot
+    std::vector<ImuStreamHost> host;
+    DevBuf<uint8_t> hdr;              // [slots] ImuStreamSlot (imu_stream.cu)
+    DevBuf<double> g, a, s, f, k;     // [slots][qcap][4 / 4 / 7 / 1 / 7]
+    DevBuf<uint8_t> stage;            // both sides: records and events (uploaded) | outputs (downloaded)
+};
+
 // The host record of one window slot.  Its frame and landmark counts are those of the slot's host header (Handle::hdr).
 // A slot holds either a window packed from the caller's arrays (api.cu: pack_window) or a resident window
 // (batch_window.cu; slot 0 is also the window of pvio_b200_window_*).  Of a resident window the host keeps integers only:
@@ -308,6 +331,7 @@ struct Handle {
                                                   // (records, points, IMU records, frames) seen
     BatchWindows bw;                              // batch_window.cu (empty until the first pvio_b200_batch_window_reset)
     TwoViewState tv;                              // twoview.cu
+    ImuStreams imus;                              // imu_stream.cu
 };
 
 int fail(Handle *h, int code, const char *what, cudaError_t e = cudaSuccess);

@@ -1,0 +1,532 @@
+// IMU stream slots (pvio_b200_batch_imu_stream): the IMU side of PVIO::Core for many sequences -- gyroscope and
+// accelerometer synchronisation (core.cpp:59-107), the sorting of samples into pending camera frames (:129-141), the
+// prepend rule of each released frame's sample list (feature_tracker.cpp:78-84) and the IMU-rate pose (:143-164 with
+// propagate_state :32-39).  One thread per record: a sequence's events are a serial state machine.
+//
+// A sequence's poses are prefixes of one propagation chain from its latest state over its kept samples, which are in
+// time order (the gyroscope and accelerometer times are checked to be non-decreasing, so the samples' accelerometer
+// times are too).  So the chain is extended event by event instead of recomputed from the state per event, as
+// predict_pose does; an event earlier than the chain's last sample restarts it from the state.  Both are the same
+// operations in the same order, so the same bits.  Compiled with -fmad=false: the arithmetic is Eigen's scalar
+// evaluation order without contraction (DESIGN 4.7h).
+#include <cmath>
+#include "api_internal.h"
+#include "ba_math.cuh"
+#include "quat.cuh"
+
+namespace pvio {
+
+namespace {
+
+constexpr double kGravityNominal = 9.80665;           // PVIO_GRAVITY_NOMINAL, common.h:62
+constexpr int kMinQcap = 16;
+
+// one stream slot on the device: output extrinsic, latest state, the previously released frame's last row, and where
+// each queue's live rows are in the slot's part of ImuStreams::g / a / s / f / k
+struct ImuStreamSlot {
+    double q_ob[4], p_ob[3];
+    double state_t, state[16];
+    double prev_t, prev_row[6];       // the previously released frame: its time, its list's last row (w xyz, a xyz)
+    int32_t has_state, has_prev, prev_nonempty;
+    int32_t drop_pending;             // a state was set and no pose has read it yet: the kept samples up to its time go at
+                                      // the next pose, as predict_pose pops them (core.cpp:149-151)
+    int32_t g0, gn, a0, an, s0, sn, nfront, f0, fn, k0, kn, pad2;   // head and size of each queue; nfront: the leading
+                                                                     // unreleased samples given to the front frame
+};
+
+struct ImuStreamRec {                 // one record as staged
+    int32_t slot, n_events, state_op, pad;
+    double state_t, state[16];
+    int64_t ev, pose, frame, row;     // first event / pose row / frame / sample row of the record in the call's arrays
+    int32_t frame_cap, row_cap;       // the record's room for frames and rows (need_frames / need_rows)
+};
+
+struct ImuStreamOut {                 // one record's results, downloaded
+    int32_t n_consumed, n_frames, n_rows, overflow;
+    int32_t g, a, s, f, k, pad[3];    // queue sizes after the call
+};
+
+struct ImuStreamArgs {
+    ImuStreamSlot *hdr;
+    double *g, *a, *s, *f, *k;
+    int qcap;
+    const ImuStreamRec *recs;
+    const double *events;             // [*][5]
+    ImuStreamOut *outs;
+    double *poses, *frame_t, *rows;   // [*][7], [*], [*][7]
+    int32_t *frame_rows;
+    int n;
+};
+
+__device__ inline void copy_rows(double *q, int w, int from, int n) {
+    for (int j = 0; j < n * w; ++j) q[j] = q[from * w + j];
+}
+
+__global__ void __launch_bounds__(128) imu_stream_kernel(ImuStreamArgs A) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= A.n) return;
+    const ImuStreamRec &R = A.recs[i];
+    ImuStreamSlot &S = A.hdr[R.slot];
+    const size_t qb = (size_t)R.slot * A.qcap;
+    double *G = A.g + qb * 4, *Ac = A.a + qb * 4, *Sm = A.s + qb * 7, *F = A.f + qb, *K = A.k + qb * 7;
+    // each queue's live rows to the front: the call's growth bound then fits in qcap
+    copy_rows(G, 4, S.g0, S.gn);
+    copy_rows(Ac, 4, S.a0, S.an);
+    copy_rows(Sm, 7, S.s0, S.sn);
+    copy_rows(F, 1, S.f0, S.fn);
+    copy_rows(K, 7, S.k0, S.kn);
+    int g0 = 0, gn = S.gn, a0 = 0, an = S.an, s0 = 0, sn = S.sn, nfront = S.nfront, f0 = 0, fn = S.fn, k0 = 0, kn = S.kn;
+
+    if (R.state_op == PVIO_B200_IMU_STREAM_SET) {
+        S.has_state = 1;
+        S.state_t = R.state_t;
+        for (int j = 0; j < 16; ++j) S.state[j] = R.state[j];
+        S.drop_pending = 1;
+    } else if (R.state_op == PVIO_B200_IMU_STREAM_CLEAR) {
+        S.has_state = 0;
+        S.drop_pending = 0;
+    }
+    const bool has_state = S.has_state != 0;
+    const double state_t = S.state_t;
+
+    ImuStreamOut &O = A.outs[i];
+    double *ft = A.frame_t + R.frame, *rows = A.rows + R.row * 7;
+    int32_t *frows = A.frame_rows + R.frame;
+    int nf = 0, nr = 0, overflow = 0;
+
+    // the propagation chain: c kept samples (from k0) applied to the latest state
+    int c = 0;
+    bool chain = false;
+    double ct = 0, cq[4], cp[3], cv[3];
+
+    // Core::track_imu: keep the sample for predict_pose, queue it, give queued samples to the front frame and release
+    // frames that a later sample has passed
+    auto track_imu = [&](double t, const double *w, const double *acc) -> bool {
+        if (!(has_state && t <= state_t)) {            // the event's pose pops it before any use (:149-151)
+            double *r = K + (k0 + kn) * 7;
+            r[0] = t;
+            for (int j = 0; j < 3; ++j) { r[1 + j] = w[j]; r[4 + j] = acc[j]; }
+            ++kn;
+        }
+        double *r = Sm + (s0 + sn) * 7;
+        r[0] = t;
+        for (int j = 0; j < 3; ++j) { r[1 + j] = w[j]; r[4 + j] = acc[j]; }
+        ++sn;
+        bool released = false;
+        while (sn > nfront && fn > 0) {
+            const double tf = F[f0];
+            if (Sm[(s0 + nfront) * 7] <= tf) { ++nfront; continue; }
+            // release the front frame: its samples, with the prepend rule against the previous frame's list
+            const bool prepend = S.has_prev && S.prev_nonempty && (nfront == 0 || Sm[s0 * 7] - S.prev_t > 1.0e-5);
+            const int cnt = nfront + (prepend ? 1 : 0);
+            if (nf >= R.frame_cap || nr + cnt > R.row_cap) { overflow = 1; return released; }
+            double *o = rows + (size_t)nr * 7;
+            if (prepend) {
+                o[0] = S.prev_t;
+                for (int j = 0; j < 6; ++j) o[1 + j] = S.prev_row[j];
+                o += 7;
+            }
+            for (int j = 0; j < nfront * 7; ++j) o[j] = Sm[s0 * 7 + j];
+            if (cnt > 0) {
+                const double *last = rows + (size_t)(nr + cnt - 1) * 7;
+                for (int j = 0; j < 6; ++j) S.prev_row[j] = last[1 + j];
+            }
+            S.has_prev = 1;
+            S.prev_nonempty = cnt > 0;
+            S.prev_t = tf;
+            ft[nf] = tf;
+            frows[nf] = cnt;
+            ++nf;
+            nr += cnt;
+            s0 += nfront; sn -= nfront; nfront = 0;
+            ++f0; --fn;
+            if (!has_state) {                          // the next state is this frame's or a later one's
+                while (kn > 0 && K[k0 * 7] <= tf) { ++k0; --kn; }
+                chain = false;
+            }
+            released = true;
+        }
+        return released;
+    };
+
+    auto restart = [&]() {
+        c = 0;
+        ct = state_t;
+        for (int j = 0; j < 4; ++j) cq[j] = S.state[j];
+        for (int j = 0; j < 3; ++j) { cp[j] = S.state[4 + j]; cv[j] = S.state[7 + j]; }
+        chain = true;
+    };
+
+    // Core::predict_pose at t, into pose row o
+    auto predict = [&](double t, double *o) {
+        if (!has_state) {
+            for (int j = 0; j < 7; ++j) o[j] = 0.0;
+            return;
+        }
+        if (S.drop_pending) {                            // predict_pose :149-151
+            while (kn > 0 && K[k0 * 7] <= state_t) { ++k0; --kn; }
+            S.drop_pending = 0;
+            chain = false;
+        }
+        if (!chain || (c > 0 && K[(k0 + c - 1) * 7] > t)) restart();
+        const double *bg = S.state + 10, *ba = S.state + 13;
+        for (; c < kn && K[(k0 + c) * 7] <= t; ++c) {   // propagate_state, core.cpp:32-39
+            const double *r = K + (k0 + c) * 7;
+            const double dt = r[0] - ct;
+            const double d[3] = {r[4] - ba[0], r[5] - ba[1], r[6] - ba[2]};
+            double ra[3];
+            bw_qrot(cq, d, ra);
+            const double acc[3] = {0.0 + ra[0], 0.0 + ra[1], -kGravityNominal + ra[2]};
+            const double hdt = 0.5 * dt * dt;
+            for (int j = 0; j < 3; ++j) {
+                cp[j] = cp[j] + dt * cv[j] + hdt * acc[j];
+                cv[j] = cv[j] + dt * acc[j];
+            }
+            const double u[3] = {(r[1] - bg[0]) * dt, (r[2] - bg[1]) * dt, (r[3] - bg[2]) * dt};
+            double e[4], qn[4];
+            expmap(u, e);
+            eigen_qmul(cq, e, qn);
+            const double nrm = sqrt(qn[0] * qn[0] + qn[1] * qn[1] + qn[2] * qn[2] + qn[3] * qn[3]);
+            for (int j = 0; j < 4; ++j) cq[j] = qn[j] / nrm;
+            ct = r[0];
+        }
+        double q[4], rp[3];
+        eigen_qmul(cq, S.q_ob, q);                       // :158-159
+        bw_qrot(cq, S.p_ob, rp);
+        for (int j = 0; j < 4; ++j) o[j] = q[j];
+        for (int j = 0; j < 3; ++j) o[4 + j] = cp[j] + rp[j];
+    };
+
+    int consumed = 0;
+    for (int e = 0; e < R.n_events; ++e) {
+        const double *ev = A.events + (size_t)(R.ev + e) * 5;
+        const int kind = (int)ev[0];
+        const double t = ev[1], v[3] = {ev[2], ev[3], ev[4]};
+        bool released = false;
+        if (kind == PVIO_B200_IMU_EVENT_GYROSCOPE) {                // Core::track_gyroscope
+            if (an > 0) {
+                if (t < Ac[a0 * 4]) {
+                    g0 = 0; gn = 0;
+                } else {
+                    while (an > 0 && t >= Ac[a0 * 4]) {
+                        const double *ac = Ac + a0 * 4, *g = G + g0 * 4;
+                        const double lambda = (ac[0] - g[0]) / (t - g[0]);
+                        const double w[3] = {g[1] + lambda * (v[0] - g[1]), g[2] + lambda * (v[1] - g[2]),
+                                             g[3] + lambda * (v[2] - g[3])};
+                        released |= track_imu(ac[0], w, ac + 1);
+                        ++a0; --an;
+                    }
+                    if (an > 0)
+                        while (gn > 0 && G[g0 * 4] < t) { ++g0; --gn; }
+                }
+            }
+            double *g = G + (g0 + gn) * 4;
+            g[0] = t; g[1] = v[0]; g[2] = v[1]; g[3] = v[2];
+            ++gn;
+        } else if (kind == PVIO_B200_IMU_EVENT_ACCELEROMETER) {     // Core::track_accelerometer
+            if (gn > 0 && t >= G[g0 * 4]) {
+                const double tb = G[(g0 + gn - 1) * 4];
+                if (t > tb) {
+                    g0 += gn - 1; gn = 1;
+                    double *a = Ac + (a0 + an) * 4;
+                    a[0] = t; a[1] = v[0]; a[2] = v[1]; a[3] = v[2];
+                    ++an;
+                } else if (t == tb) {
+                    g0 += gn - 1; gn = 1;
+                    released = track_imu(t, G + g0 * 4 + 1, v);
+                } else {
+                    while (t >= G[(g0 + 1) * 4]) { ++g0; --gn; }
+                    const double *g = G + g0 * 4, *g1 = g + 4;
+                    const double lambda = (t - g[0]) / (g1[0] - g[0]);
+                    const double w[3] = {g[1] + lambda * (g1[1] - g[1]), g[2] + lambda * (g1[2] - g[2]),
+                                         g[3] + lambda * (g1[3] - g[3])};
+                    released = track_imu(t, w, v);
+                }
+            }
+        } else {                                                    // Core::track_camera: the frame waits for samples
+            F[f0 + fn] = t;
+            ++fn;
+        }
+        predict(t, A.poses + (size_t)(R.pose + e) * 7);
+        consumed = e + 1;
+        if (released || overflow) break;
+    }
+
+    S.g0 = g0; S.gn = gn; S.a0 = a0; S.an = an; S.s0 = s0; S.sn = sn; S.nfront = nfront;
+    S.f0 = f0; S.fn = fn; S.k0 = k0; S.kn = kn;
+    O.n_consumed = consumed; O.n_frames = nf; O.n_rows = nr; O.overflow = overflow;
+    O.g = gn; O.a = an; O.s = sn; O.f = fn; O.k = kn;
+}
+
+// reset: slot list and headers staged back to back
+__global__ void imu_stream_reset_kernel(int n, const int32_t *slots, const ImuStreamSlot *src, ImuStreamSlot *hdr) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) hdr[slots[i]] = src[i];
+}
+
+size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// device queues for `slots` slots of at least `qcap` rows each; growth keeps every slot's queues and header
+int ensure_streams(Handle *h, int slots, int qcap) {
+    ImuStreams &M = h->imus;
+    if (slots <= M.slots && qcap <= M.qcap) return 0;
+    const int ns = slots <= M.slots ? M.slots : std::max(slots, std::min(std::max(2 * M.slots, 64), kMaxBatchSlot + 1));
+    int nq = std::max(M.qcap, kMinQcap);
+    while (nq < qcap) nq *= 2;
+    CK(h, cudaStreamSynchronize(h->stream));
+    DevBuf<uint8_t> hdr;
+    TRY(alloc(h, hdr, sizeof(ImuStreamSlot) * ns, kDevice));
+    if (M.slots) CK(h, cudaMemcpyAsync(hdr.d, M.hdr.d, sizeof(ImuStreamSlot) * M.slots, cudaMemcpyDeviceToDevice, h->stream));
+    DevBuf<double> *qs[5] = {&M.g, &M.a, &M.s, &M.f, &M.k};
+    const int width[5] = {4, 4, 7, 1, 7};
+    DevBuf<double> grown[5];
+    for (int q = 0; q < 5; ++q) {
+        TRY(alloc(h, grown[q], (size_t)ns * nq * width[q], kDevice));
+        if (M.slots)
+            CK(h, cudaMemcpy2DAsync(grown[q].d, sizeof(double) * nq * width[q], qs[q]->d, sizeof(double) * M.qcap * width[q],
+                                    sizeof(double) * M.qcap * width[q], M.slots, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    CK(h, cudaStreamSynchronize(h->stream));
+    M.hdr = std::move(hdr);
+    for (int q = 0; q < 5; ++q) *qs[q] = std::move(grown[q]);
+    M.slots = ns;
+    M.qcap = nq;
+    return 0;
+}
+
+bool finite_all(const double *v, int n) {
+    for (int j = 0; j < n; ++j)
+        if (!std::isfinite(v[j])) return false;
+    return true;
+}
+
+int stream_reset_impl(Handle *h, int n, const int32_t *slots, const double *oq, const double *op) {
+    if (n < 0) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: bad slot count");
+    if (n == 0) return 0;
+    if (!slots || !oq || !op) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: bad arguments");
+    std::vector<uint8_t> taken;
+    int top = 0;
+    for (int i = 0; i < n; ++i) {
+        const int s = slots[i];
+        if (s < 0 || s > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: slot out of range");
+        if ((size_t)s >= taken.size()) taken.resize(s + 1, 0);
+        if (taken[s]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: a slot appears twice");
+        taken[s] = 1;
+        if (!finite_all(oq + 4 * i, 4) || !finite_all(op + 3 * i, 3))
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: an extrinsic value is not finite");
+        top = std::max(top, s + 1);
+    }
+    ImuStreams &M = h->imus;
+    TRY(ensure_streams(h, top, kMinQcap));
+    const size_t o_hdr = align256(sizeof(int32_t) * n);
+    TRY(reserve(h, M.stage, o_hdr + sizeof(ImuStreamSlot) * n, kBoth));
+    memcpy(M.stage.h, slots, sizeof(int32_t) * n);
+    ImuStreamSlot *hs = reinterpret_cast<ImuStreamSlot *>(M.stage.h + o_hdr);
+    for (int i = 0; i < n; ++i) {
+        ImuStreamSlot z{};
+        for (int j = 0; j < 4; ++j) z.q_ob[j] = oq[4 * i + j];
+        for (int j = 0; j < 3; ++j) z.p_ob[j] = op[3 * i + j];
+        hs[i] = z;
+    }
+    cudaStream_t st = h->stream;
+    CK(h, cudaMemcpyAsync(M.stage.d, M.stage.h, o_hdr + sizeof(ImuStreamSlot) * n, cudaMemcpyHostToDevice, st));
+    imu_stream_reset_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, reinterpret_cast<const int32_t *>(M.stage.d),
+                                                             reinterpret_cast<const ImuStreamSlot *>(M.stage.d + o_hdr),
+                                                             reinterpret_cast<ImuStreamSlot *>(M.hdr.d));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaStreamSynchronize(st));
+    if ((size_t)top > M.host.size()) M.host.resize(top);
+    for (int i = 0; i < n; ++i) {
+        M.host[slots[i]] = ImuStreamHost{};
+        M.host[slots[i]].set = true;
+    }
+    return 0;
+}
+
+// what checking a record finds: its queue bounds and its room
+struct StreamNeed {
+    int64_t frames = 0, rows = 0, queue = 0;
+};
+
+int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
+    if (n < 0) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: bad record count");
+    if (n == 0) return 0;
+    if (!recs) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: bad arguments");
+    ImuStreams &M = h->imus;
+    std::vector<uint8_t> taken;
+    std::vector<StreamNeed> need(n);
+    bool query = false;
+    int64_t total_ev = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_record &r = recs[i];
+        if (r.slot < 0 || r.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: slot out of range");
+        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
+        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: a slot appears twice");
+        taken[r.slot] = 1;
+        if ((size_t)r.slot >= M.host.size() || !M.host[r.slot].set)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: the slot was never reset");
+        const ImuStreamHost &S = M.host[r.slot];
+        if (r.n_events < 0 || (r.n_events > 0 && (!r.events || !r.poses)))
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: bad event count or pointer");
+        if (r.state_op < PVIO_B200_IMU_STREAM_KEEP || r.state_op > PVIO_B200_IMU_STREAM_CLEAR)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: unknown state_op");
+        if (r.state_op == PVIO_B200_IMU_STREAM_SET) {
+            if (!r.state || !std::isfinite(r.state_time) || !finite_all(r.state, 16))
+                return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: a SET state is missing or not finite");
+            if (S.dropped && r.state_time < S.t_drop)
+                return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: the state is older than a frame released without one");
+        }
+        int64_t ng = 0, na = 0, nc = 0;
+        bool seen_g = S.seen_g, seen_a = S.seen_a;
+        double last_g = S.last_g, last_a = S.last_a;
+        for (int e = 0; e < r.n_events; ++e) {
+            const double *ev = r.events + (size_t)e * 5;
+            if (!finite_all(ev, 5)) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: an event value is not finite");
+            const double t = ev[1];
+            if (ev[0] == PVIO_B200_IMU_EVENT_GYROSCOPE) {
+                if (seen_g && t < last_g) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: a gyroscope time decreases");
+                seen_g = true; last_g = t; ++ng;
+            } else if (ev[0] == PVIO_B200_IMU_EVENT_ACCELEROMETER) {
+                if (seen_a && t < last_a) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: an accelerometer time decreases");
+                seen_a = true; last_a = t; ++na;
+            } else if (ev[0] == PVIO_B200_IMU_EVENT_CAMERA) {
+                ++nc;
+            } else {
+                return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: unknown event kind");
+            }
+        }
+        StreamNeed &d = need[i];
+        d.frames = S.f + nc;
+        d.rows = S.s + S.a + na + d.frames;
+        d.queue = std::max({S.g + ng, S.a + na, S.s + S.a + na, S.f + nc, S.k + S.a + na});
+        if (d.queue > PVIO_B200_IMU_STREAM_MAX_QUEUE)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: a queue could exceed PVIO_B200_IMU_STREAM_MAX_QUEUE");
+        if (!r.rows) query = true;
+        total_ev += r.n_events;
+    }
+    if (query) {
+        for (int i = 0; i < n; ++i) { recs[i].need_frames = (int32_t)need[i].frames; recs[i].need_rows = need[i].rows; }
+        return 0;
+    }
+    int64_t total_f = 0, total_r = 0, qcap = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_record &r = recs[i];
+        if (r.max_frames < need[i].frames || r.max_rows < need[i].rows || (need[i].frames > 0 && (!r.frame_t || !r.frame_rows)))
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: max_frames / max_rows below need_frames / need_rows");
+        total_f += need[i].frames;
+        total_r += need[i].rows;
+        qcap = std::max(qcap, need[i].queue);
+    }
+    TRY(ensure_streams(h, M.slots, (int)qcap));
+
+    // staging: records | events (uploaded) || outputs | poses | frame times | rows | frame row counts (downloaded)
+    size_t o = 0;
+    const size_t o_rec = o; o = align256(o + sizeof(ImuStreamRec) * n);
+    const size_t o_ev = o; o = align256(o + sizeof(double) * 5 * total_ev);
+    const size_t up = o;
+    const size_t o_out = o; o = align256(o + sizeof(ImuStreamOut) * n);
+    const size_t o_pose = o; o += sizeof(double) * 7 * total_ev;
+    const size_t o_ft = o; o += sizeof(double) * total_f;
+    const size_t o_rows = o; o += sizeof(double) * 7 * total_r;
+    const size_t o_fr = o; o += sizeof(int32_t) * total_f;
+    TRY(reserve(h, M.stage, o, kBoth));
+    uint8_t *hs = M.stage.h, *ds = M.stage.d;
+    ImuStreamRec *hr = reinterpret_cast<ImuStreamRec *>(hs + o_rec);
+    double *hev = reinterpret_cast<double *>(hs + o_ev);
+    int64_t ev = 0, fr = 0, row = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_record &r = recs[i];
+        ImuStreamRec R{};
+        R.slot = r.slot; R.n_events = r.n_events; R.state_op = r.state_op;
+        if (r.state_op == PVIO_B200_IMU_STREAM_SET) {
+            R.state_t = r.state_time;
+            memcpy(R.state, r.state, sizeof(R.state));
+        }
+        R.ev = ev; R.pose = ev; R.frame = fr; R.row = row;
+        R.frame_cap = (int32_t)need[i].frames; R.row_cap = (int32_t)need[i].rows;
+        hr[i] = R;
+        if (r.n_events) memcpy(hev + ev * 5, r.events, sizeof(double) * 5 * r.n_events);
+        ev += r.n_events; fr += need[i].frames; row += need[i].rows;
+    }
+    ImuStreamArgs A;
+    A.hdr = reinterpret_cast<ImuStreamSlot *>(M.hdr.d);
+    A.g = M.g.d; A.a = M.a.d; A.s = M.s.d; A.f = M.f.d; A.k = M.k.d;
+    A.qcap = M.qcap;
+    A.recs = reinterpret_cast<const ImuStreamRec *>(ds + o_rec);
+    A.events = reinterpret_cast<const double *>(ds + o_ev);
+    A.outs = reinterpret_cast<ImuStreamOut *>(ds + o_out);
+    A.poses = reinterpret_cast<double *>(ds + o_pose);
+    A.frame_t = reinterpret_cast<double *>(ds + o_ft);
+    A.rows = reinterpret_cast<double *>(ds + o_rows);
+    A.frame_rows = reinterpret_cast<int32_t *>(ds + o_fr);
+    A.n = n;
+    cudaStream_t st = h->stream;
+    CK(h, cudaMemcpyAsync(ds, hs, up, cudaMemcpyHostToDevice, st));
+    imu_stream_kernel<<<(n + 127) / 128, 128, 0, st>>>(A);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaMemcpyAsync(hs + up, ds + up, o - up, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaStreamSynchronize(st));
+
+    // Internal invariant: the host bounds (need_frames / need_rows) hold every release, so overflow is never set.  Were
+    // it set, the kernel would already have changed the call's slots without the host's record of them following, so
+    // every slot of the call is marked unset: later calls on them are rejected until they are reset.
+    const ImuStreamOut *outs = reinterpret_cast<const ImuStreamOut *>(hs + o_out);
+    for (int i = 0; i < n; ++i)
+        if (outs[i].overflow) {
+            for (int j = 0; j < n; ++j) M.host[recs[j].slot].set = false;
+            return fail(h, PVIO_B200_ECUDA, "batch_imu_stream: a record's releases exceeded its bound (internal "
+                                            "error); the call's slots must be reset");
+        }
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_imu_stream_record &r = recs[i];
+        const ImuStreamRec &R = hr[i];
+        const ImuStreamOut &O = outs[i];
+        memcpy(r.poses, hs + o_pose + sizeof(double) * 7 * R.pose, sizeof(double) * 7 * O.n_consumed);
+        const double *ft = reinterpret_cast<const double *>(hs + o_ft) + R.frame;
+        if (O.n_frames) {
+            memcpy(r.frame_t, ft, sizeof(double) * O.n_frames);
+            memcpy(r.frame_rows, reinterpret_cast<const int32_t *>(hs + o_fr) + R.frame, sizeof(int32_t) * O.n_frames);
+        }
+        if (O.n_rows) memcpy(r.rows, hs + o_rows + sizeof(double) * 7 * R.row, sizeof(double) * 7 * O.n_rows);
+        r.n_consumed = O.n_consumed;
+        r.n_frames = O.n_frames;
+        r.need_frames = (int32_t)need[i].frames;
+        r.need_rows = need[i].rows;
+        ImuStreamHost &S = M.host[r.slot];
+        if (r.state_op == PVIO_B200_IMU_STREAM_SET) S.has_state = true;
+        if (r.state_op == PVIO_B200_IMU_STREAM_CLEAR) S.has_state = false;
+        for (int e = 0; e < O.n_consumed; ++e) {
+            const double *evr = r.events + (size_t)e * 5;
+            if (evr[0] == PVIO_B200_IMU_EVENT_GYROSCOPE) { S.seen_g = true; S.last_g = evr[1]; }
+            if (evr[0] == PVIO_B200_IMU_EVENT_ACCELEROMETER) { S.seen_a = true; S.last_a = evr[1]; }
+        }
+        if (!S.has_state)
+            for (int k = 0; k < O.n_frames; ++k) {
+                S.t_drop = S.dropped ? std::max(S.t_drop, ft[k]) : ft[k];
+                S.dropped = true;
+            }
+        S.g = O.g; S.a = O.a; S.s = O.s; S.f = O.f; S.k = O.k;
+    }
+    return 0;
+}
+
+}  // namespace
+
+}  // namespace pvio
+
+using namespace pvio;
+
+extern "C" int pvio_b200_batch_imu_stream_reset(pvio_b200_handle hh, int n, const int32_t *slots, const double *output_q,
+                                                const double *output_p) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return stream_reset_impl(h, n, slots, output_q, output_p);
+}
+
+extern "C" int pvio_b200_batch_imu_stream(pvio_b200_handle hh, int n, pvio_b200_imu_stream_record *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return stream_impl(h, n, records);
+}

@@ -1,0 +1,77 @@
+"""IMU stream slots of many sequences (include/pvio_b200.h "IMU stream slots", csrc/imu_stream.cu): per sequence the
+IMU side of PVIO::Core on the device -- raw gyroscope and accelerometer readings synchronised into samples, samples
+sorted into camera frames (with the prepend rule of the frontend applied), and the IMU-rate pose from the latest state
+the caller feeds back."""
+import numpy as np
+
+from . import _lib
+
+GYROSCOPE, ACCELEROMETER, CAMERA = _lib.IMU_EVENT_GYROSCOPE, _lib.IMU_EVENT_ACCELEROMETER, _lib.IMU_EVENT_CAMERA
+KEEP, SET, CLEAR = _lib.IMU_STREAM_KEEP, _lib.IMU_STREAM_SET, _lib.IMU_STREAM_CLEAR
+
+
+class StreamRecord:
+    """One sequence's part of a push (pvio_b200_imu_stream_record): its stream slot, its new events as rows
+    (kind, t, x, y, z) in arrival order, and optionally a new latest state (set_state: the 16-double `predicted` of
+    track_camera with its frame time) or its removal (clear_state), applied before the events."""
+
+    def __init__(self, slot, events=()):
+        self.slot = int(slot)
+        self.events = np.ascontiguousarray(np.asarray(events, dtype=np.float64).reshape(-1, 5))
+        self.state_op, self.state_time, self.state = KEEP, 0.0, None
+
+    def set_state(self, t, state16):
+        self.state_op, self.state_time = SET, float(t)
+        self.state = np.ascontiguousarray(state16, dtype=np.float64).reshape(16)
+        return self
+
+    def clear_state(self):
+        self.state_op, self.state = CLEAR, None
+        return self
+
+
+class ImuStream:
+    def __init__(self, ba):
+        """ba: a BundleAdjustor (owns the device handle); stream slots are independent of its window slots."""
+        self.ba, self.lib, self.h = ba, ba.lib, ba.h
+
+    def reset(self, slots, output_q=None, output_p=None):
+        """Empty each slot and clear its latest state; output_q [n, 4] xyzw / output_p [n, 3]: the output extrinsic
+        (Config output_to_body_rotation / translation), identity when None."""
+        s = np.ascontiguousarray(slots, dtype=np.int32).reshape(-1)
+        n = len(s)
+        q = np.tile([0.0, 0.0, 0.0, 1.0], (n, 1)) if output_q is None else output_q
+        p = np.zeros((n, 3)) if output_p is None else output_p
+        q = np.ascontiguousarray(np.broadcast_to(np.asarray(q, dtype=np.float64), (n, 4)))
+        p = np.ascontiguousarray(np.broadcast_to(np.asarray(p, dtype=np.float64), (n, 3)))
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream_reset(self.h, n, _lib.ptr(s), _lib.ptr(q), _lib.ptr(p)))
+
+    def push(self, records):
+        """One call over a list of StreamRecord (distinct slots).  Per record a dict: n_consumed (the events used, up to
+        and including the first that released a frame), poses [n_consumed, 7] (q xyzw, p), frames: a list of
+        (t, samples [k, 7]) for the released camera frames, samples as pvio_b200_window_camera takes them."""
+        n = len(records)
+        recs = (_lib.CImuStreamRecord * max(n, 1))()
+        poses = []
+        for r, rec in zip(recs, records):
+            p = np.zeros((max(len(rec.events), 1), 7))
+            poses.append(p)
+            r.slot, r.n_events, r.state_op, r.state_time = rec.slot, len(rec.events), rec.state_op, rec.state_time
+            _lib.set_ptrs(r, events=rec.events, state=rec.state, poses=p, rows=None)
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream(self.h, n, recs))          # rows NULL: the sizes
+        ft, fr, rows = [], [], []
+        for r in recs[:n]:
+            ft.append(np.zeros(max(r.need_frames, 1)))
+            fr.append(np.zeros(max(r.need_frames, 1), dtype=np.int32))
+            rows.append(np.zeros((max(r.need_rows, 1), 7)))
+            r.max_frames, r.max_rows = r.need_frames, r.need_rows
+            _lib.set_ptrs(r, frame_t=ft[-1], frame_rows=fr[-1], rows=rows[-1])
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream(self.h, n, recs))
+        out = []
+        for i, r in enumerate(recs[:n]):
+            frames, o = [], 0
+            for k in range(r.n_frames):
+                frames.append((float(ft[i][k]), rows[i][o:o + fr[i][k]].copy()))
+                o += int(fr[i][k])
+            out.append(dict(n_consumed=int(r.n_consumed), poses=poses[i][:r.n_consumed].copy(), frames=frames))
+        return out
