@@ -1197,6 +1197,17 @@ int pvio_b200_selftest_lie(pvio_b200_handle h, int n, const double *w, double *o
  * Not part of the reference interface. */
 int pvio_b200_selftest_eig(pvio_b200_handle h, int n, const int32_t *dk, const double *A, const double *b, double *S_out,
                            double *e_out);
+/* Device self-test of the reduced-system Cholesky solve of the Gauss-Newton step: n systems in one launch, one CTA per
+ * system, packed as the solve kernels pack a window's reduced system (4 x 4 tiles, D padded to 4 nb with identity rows).
+ * System i: D[i] unknowns, a D[i] x D[i] symmetric row-major matrix A_i (its lower triangle is read) and a right-hand
+ * side b_i, stored back to back in A and b.  mode 0: the factorisation of the batched visual-only kernel (64 threads);
+ * 1: the one the single-window kernel chooses for the block count (256 threads); 2: its tiled fallback, forced.
+ * Out: x_i (same layout as b; 0 where the factorisation failed) and ok_i = 1 where every pivot was positive and finite.
+ * PVIO_B200_EINVAL for n < 1, an unknown mode, a D[i] < 1, a system that needs more shared memory than the mode's
+ * production kernel gets (48 KB for mode 0, 220 KB otherwise) or, in mode 1, more than 64 block rows.
+ * Not part of the reference interface. */
+int pvio_b200_selftest_chol(pvio_b200_handle h, int n, int mode, const int32_t *D, const double *A, const double *b,
+                            double *x_out, int32_t *ok_out);
 
 /* ---- KLT ----------------------------------------------------------------------------- */
 /* Pyramidal Lucas-Kanade with OpenCV's semantics: winSize 21x21, maxLevel levels above

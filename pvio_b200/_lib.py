@@ -286,6 +286,7 @@ SIGNATURES = {
     "pvio_b200_triangulate": (_int, [_h, _int, c_f64p, _int, c_i32p, c_i32p, c_f64p, c_f64p, c_u8p, c_f64p]),
     "pvio_b200_selftest_lie": (_int, [_h, _int, c_f64p, c_f64p]),
     "pvio_b200_selftest_eig": (_int, [_h, _int, c_i32p, c_f64p, c_f64p, c_f64p, c_f64p]),
+    "pvio_b200_selftest_chol": (_int, [_h, _int, _int, c_i32p, c_f64p, c_f64p, c_f64p, c_i32p]),
     "pvio_b200_klt_track": (_int, [_h, c_u8p, c_u8p, _int, _int, _int, c_f32p, c_f32p, c_u8p, c_f32p, _int, _int, _int,
                                    _f64]),
 }

@@ -200,6 +200,19 @@ class BundleAdjustor:
             ob += d
         return out
 
+    CHOL_MODES = {"narrow": 0, "wide": 1, "wide-tiled": 2}
+
+    def selftest_chol(self, systems, mode):
+        """The reduced-system Cholesky solve on [(A, b)] in one launch (see the header); mode: one of CHOL_MODES.
+        -> ([x], ok [n] bool)"""
+        D = np.array([len(b) for _, b in systems], dtype=np.int32)
+        A = np.concatenate([np.ascontiguousarray(a, dtype=np.float64).ravel() for a, _ in systems])
+        b = np.concatenate([np.asarray(v, dtype=np.float64) for _, v in systems])
+        x, ok = np.zeros_like(b), np.zeros(len(D), dtype=np.int32)
+        self._ck(self.lib.pvio_b200_selftest_chol(self.h, len(D), self.CHOL_MODES[mode], _lib.ptr(D), _lib.ptr(A),
+                                                  _lib.ptr(b), _lib.ptr(x), _lib.ptr(ok)))
+        return np.split(x, np.cumsum(D)[:-1]), ok.astype(bool)
+
     def sync(self):
         self._ck(self.lib.pvio_b200_sync(self.h))
 

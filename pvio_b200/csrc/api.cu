@@ -1138,6 +1138,7 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
         CK(h, cudaFuncSetAttribute(update_obs_kernel<double, kUpdWarps, 4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
         CK(h, cudaFuncSetAttribute(solve_kernel_visual, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024));
+        TRY(selftest_chol_opt_in(h));
         TRY(marg_opt_in(h));
     }
     init_ctrl_kernel<<<(int)W, 32, 0, h->stream>>>(h->ctrl.d, 1e-8, 1e4, 10, 0.0, 0);
@@ -1550,6 +1551,13 @@ int pvio_b200_selftest_eig(pvio_b200_handle hh, int n, const int32_t *dk, const 
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h || !dk || !A || !b || !S_out || !e_out) return PVIO_B200_EINVAL;
     return selftest_eig_impl(h, n, dk, A, b, S_out, e_out);
+}
+
+int pvio_b200_selftest_chol(pvio_b200_handle hh, int n, int mode, const int32_t *D, const double *A, const double *b,
+                            double *x_out, int32_t *ok_out) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h || !D || !A || !b || !x_out || !ok_out) return PVIO_B200_EINVAL;
+    return selftest_chol_impl(h, n, mode, D, A, b, x_out, ok_out);
 }
 
 #ifdef PVIO_SOLVE_STAMPS

@@ -575,5 +575,8 @@ void fm_batch_masks(Handle *h, const FmMaskJob *jobs, int n, int max_words);
 int batch_two_view_impl(Handle *h, int n, const pvio_b200_two_view *recs);
 // selftest.cu
 int selftest_lie_impl(Handle *h, int n, const double *w_in, double *out);
+int selftest_chol_opt_in(Handle *h);
+int selftest_chol_impl(Handle *h, int n, int mode, const int32_t *Ds, const double *A, const double *b, double *x_out,
+                       int32_t *ok_out);
 
 }  // namespace pvio
