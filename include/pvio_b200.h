@@ -833,6 +833,44 @@ int pvio_b200_batch_imu_stream_reset(pvio_b200_handle h, int n, const int32_t *s
                                      const double *output_p);
 int pvio_b200_batch_imu_stream(pvio_b200_handle h, int n, pvio_b200_imu_stream_record *records);
 
+/* Snapshots of IMU stream slots: save a stream slot to host memory and restore it into any stream slot of any handle,
+ * to move a live sequence to another handle or GPU, fork it, or roll it back.  A blob is the slot's whole state between
+ * two calls: the output extrinsic; the latest state with its time and whether a pose still has to drop the kept samples
+ * up to it; the previously released frame's time and last row (the prepend rule reads them); the leading unreleased
+ * samples given to the front frame; the last gyroscope and accelerometer times and the newest frame released without a
+ * state (what rejecting a later record reads); and the live rows of the gyroscope, accelerometer, unreleased-sample,
+ * pending-frame and kept-sample queues, oldest first.  What the caller holds itself (events it has not yet passed, a
+ * `predicted` it has not yet fed back) is not in it.  A blob names no slot, pointer or queue capacity, its padding is
+ * zero, so save -> restore -> save gives the same bytes in any stream slot of any handle.  Separate from the window
+ * blobs of pvio_b200_batch_window_save: a sequence moved with its window and tracker slots takes both.
+ *  - save: stream slots that were reset (and not marked unset by the internal-error path of batch_imu_stream).
+ *    data == NULL asks for the size only (no device work); otherwise capacity must hold `size` bytes.  size is written
+ *    on success.
+ *  - restore: capacity is the blob's byte count.  The target slot takes the blob's state and counts as reset; its
+ *    queues and the handle's stream slots grow as batch_imu_stream grows them.  One blob restored into several slots
+ *    of one call forks the sequence.
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no stream slot and no output has changed.
+ * Rejected: n < 0; a slot out of range or named twice (save: never reset); save capacity below the size; a restore blob
+ * with the wrong magic or version, a declared size other than its byte count or than its counts imply, a queue count
+ * above PVIO_B200_IMU_STREAM_MAX_QUEUE, more leading samples than unreleased ones, a flag outside 0 / 1, a pending drop
+ * without a state, a non-empty previous list without a previous frame, a state older than a frame released without
+ * one, a value that is not finite, times that decrease within the gyroscope, accelerometer, unreleased-sample or
+ * kept-sample queue, a queued reading newer than its stream's last time, or a non-empty queue of a stream never seen.
+ * Launches, whatever n is: save one host -> device copy of the records, one pack kernel, one device -> host copy, one
+ * synchronisation; restore one host -> device copy, one unpack kernel, one synchronisation (a restore that grows the
+ * stream slots or their queues first copies them into the larger buffers). */
+#define PVIO_B200_IMU_STREAM_SNAPSHOT_MAGIC 1397315152  /* "PVIS" as a little-endian uint32 */
+#define PVIO_B200_IMU_STREAM_SNAPSHOT_VERSION 1
+typedef struct pvio_b200_imu_stream_snapshot {
+    int32_t slot;                     /* stream slot */
+    int32_t pad;                      /* 0 */
+    uint8_t *data;                    /* save: room for capacity bytes, NULL: size query only; restore: the saved bytes */
+    int64_t capacity;                 /* bytes at data */
+    int64_t size;                     /* save, out: the bytes the record needs / wrote */
+} pvio_b200_imu_stream_snapshot;      /* 32 bytes on LP64 */
+int pvio_b200_batch_imu_stream_save(pvio_b200_handle h, int n, pvio_b200_imu_stream_snapshot *records);
+int pvio_b200_batch_imu_stream_restore(pvio_b200_handle h, int n, const pvio_b200_imu_stream_snapshot *records);
+
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */
 int pvio_b200_timer_start(pvio_b200_handle h);

@@ -30,6 +30,7 @@ SNAPSHOT_MAGIC, SNAPSHOT_VERSION = 1314084432, 1
 IMU_EVENT_GYROSCOPE, IMU_EVENT_ACCELEROMETER, IMU_EVENT_CAMERA = 0, 1, 2
 IMU_STREAM_KEEP, IMU_STREAM_SET, IMU_STREAM_CLEAR = 0, 1, 2
 IMU_STREAM_MAX_QUEUE = 65536
+IMU_STREAM_SNAPSHOT_MAGIC, IMU_STREAM_SNAPSHOT_VERSION = 1397315152, 1
 
 c_i32p = C.POINTER(C.c_int32)
 c_u8p = C.POINTER(C.c_uint8)
@@ -181,6 +182,10 @@ class CImuStreamRecord(C.Structure):
                 ("n_consumed", C.c_int32), ("n_frames", C.c_int32), ("need_frames", C.c_int32), ("need_rows", C.c_int64)]
 
 
+class CImuStreamSnapshot(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("pad", C.c_int32), ("data", c_u8p), ("capacity", C.c_int64), ("size", C.c_int64)]
+
+
 class CLens(C.Structure):
     _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
@@ -255,6 +260,8 @@ SIGNATURES = {
     "pvio_b200_batch_window_restore": (_int, [_h, _int, _P(CWindowSnapshot)]),
     "pvio_b200_batch_imu_stream_reset": (_int, [_h, _int, c_i32p, c_f64p, c_f64p]),
     "pvio_b200_batch_imu_stream": (_int, [_h, _int, _P(CImuStreamRecord)]),
+    "pvio_b200_batch_imu_stream_save": (_int, [_h, _int, _P(CImuStreamSnapshot)]),
+    "pvio_b200_batch_imu_stream_restore": (_int, [_h, _int, _P(CImuStreamSnapshot)]),
     "pvio_b200_sync": (_int, [_h]),
     "pvio_b200_timer_start": (_int, [_h]),
     "pvio_b200_timer_stop": (_int, [_h, c_f32p]),

@@ -512,6 +512,274 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
     return 0;
 }
 
+// ------------------------------------------------------------ snapshots (pvio_b200_batch_imu_stream_save / restore)
+// A blob: StreamSnapHead, then the live rows of the five queues back to back in queue order (gyroscope [n0][4],
+// accelerometer [n1][4], unreleased samples [n2][7], pending frame stamps [n3], kept samples [n4][7]), oldest first.
+// The head's first part is the host record (written by the host), `dev` the slot's device header (written by the pack
+// kernel).  No slot, head offset, Qcap or pointer, so save -> restore -> save gives the same bytes in any stream slot.
+struct StreamSnapDev {
+    double q_ob[4], p_ob[3];
+    double state_t, state[16];
+    double prev_t, prev_row[6];
+    int32_t has_state, drop_pending, has_prev, prev_nonempty, nfront, pad;
+};
+struct StreamSnapHead {
+    uint32_t magic, version;
+    int64_t size;                     // bytes of the blob
+    int32_t n[5];                     // rows of each queue
+    int32_t seen_g, seen_a, dropped;  // ImuStreamHost
+    double last_g, last_a, t_drop;
+    StreamSnapDev dev;
+};
+static_assert(sizeof(StreamSnapHead) == 344 && offsetof(StreamSnapHead, dev) == 72 && sizeof(StreamSnapDev) == 272,
+              "the head has no implicit padding; the queue sections start 8-byte aligned");
+constexpr int kSnapThreads = 128;
+
+// row width of queue q (g, a, s, f, k)
+__host__ __device__ inline int queue_width(int q) { return q < 2 ? 4 : q == 3 ? 1 : 7; }
+
+__host__ __device__ inline int64_t stream_snap_size(const int32_t *n) {
+    int64_t s = sizeof(StreamSnapHead);
+    for (int q = 0; q < 5; ++q) s += sizeof(double) * queue_width(q) * (int64_t)n[q];
+    return s;
+}
+
+struct StreamSnapRec {                // one record of a save or restore call: its stream slot, its blob's byte offset
+    int32_t slot, pad;                // in the call's area
+    int64_t at;
+};
+struct StreamSnapArgs {
+    ImuStreamSlot *hdr;
+    double *q[5];                     // g, a, s, f, k
+    int qcap;
+    const StreamSnapRec *recs;
+    uint8_t *area;
+};
+
+// n doubles from src to dst by the CTA; returns dst + n
+__device__ __forceinline__ double *snap_rows(double *dst, const double *src, int n) {
+    for (int j = threadIdx.x; j < n; j += kSnapThreads) dst[j] = src[j];
+    return dst + n;
+}
+
+// One CTA per save record: the slot's device header into the blob's head and each queue's live rows [head, head + n)
+// into its section.  The host writes the rest of the head.
+__global__ void __launch_bounds__(kSnapThreads) imu_stream_pack_kernel(StreamSnapArgs A) {
+    const StreamSnapRec &R = A.recs[blockIdx.x];
+    const ImuStreamSlot &S = A.hdr[R.slot];
+    uint8_t *blob = A.area + R.at;
+    const size_t qb = (size_t)R.slot * A.qcap;
+    double *dst = reinterpret_cast<double *>(blob + sizeof(StreamSnapHead));
+    dst = snap_rows(dst, A.q[0] + (qb + S.g0) * 4, S.gn * 4);
+    dst = snap_rows(dst, A.q[1] + (qb + S.a0) * 4, S.an * 4);
+    dst = snap_rows(dst, A.q[2] + (qb + S.s0) * 7, S.sn * 7);
+    dst = snap_rows(dst, A.q[3] + (qb + S.f0), S.fn);
+    snap_rows(dst, A.q[4] + (qb + S.k0) * 7, S.kn * 7);
+    if (threadIdx.x == 0) {
+        StreamSnapDev &d = reinterpret_cast<StreamSnapHead *>(blob)->dev;
+        for (int j = 0; j < 4; ++j) d.q_ob[j] = S.q_ob[j];
+        for (int j = 0; j < 3; ++j) d.p_ob[j] = S.p_ob[j];
+        d.state_t = S.state_t;
+        for (int j = 0; j < 16; ++j) d.state[j] = S.state[j];
+        d.prev_t = S.prev_t;
+        for (int j = 0; j < 6; ++j) d.prev_row[j] = S.prev_row[j];
+        d.has_state = S.has_state; d.drop_pending = S.drop_pending; d.has_prev = S.has_prev;
+        d.prev_nonempty = S.prev_nonempty; d.nfront = S.nfront; d.pad = 0;
+    }
+}
+
+// One CTA per restore record: each queue's rows to the front of the target slot (heads 0), then its header.
+__global__ void __launch_bounds__(kSnapThreads) imu_stream_unpack_kernel(StreamSnapArgs A) {
+    const StreamSnapRec &R = A.recs[blockIdx.x];
+    const uint8_t *blob = A.area + R.at;
+    const StreamSnapHead &H = *reinterpret_cast<const StreamSnapHead *>(blob);
+    const double *src = reinterpret_cast<const double *>(blob + sizeof(StreamSnapHead));
+    const size_t qb = (size_t)R.slot * A.qcap;
+    snap_rows(A.q[0] + qb * 4, src, H.n[0] * 4);
+    src += H.n[0] * 4;
+    snap_rows(A.q[1] + qb * 4, src, H.n[1] * 4);
+    src += H.n[1] * 4;
+    snap_rows(A.q[2] + qb * 7, src, H.n[2] * 7);
+    src += H.n[2] * 7;
+    snap_rows(A.q[3] + qb, src, H.n[3]);
+    src += H.n[3];
+    snap_rows(A.q[4] + qb * 7, src, H.n[4] * 7);
+    if (threadIdx.x == 0) {
+        const StreamSnapDev &d = H.dev;
+        ImuStreamSlot S{};
+        for (int j = 0; j < 4; ++j) S.q_ob[j] = d.q_ob[j];
+        for (int j = 0; j < 3; ++j) S.p_ob[j] = d.p_ob[j];
+        S.state_t = d.state_t;
+        for (int j = 0; j < 16; ++j) S.state[j] = d.state[j];
+        S.prev_t = d.prev_t;
+        for (int j = 0; j < 6; ++j) S.prev_row[j] = d.prev_row[j];
+        S.has_state = d.has_state; S.drop_pending = d.drop_pending; S.has_prev = d.has_prev;
+        S.prev_nonempty = d.prev_nonempty; S.nfront = d.nfront;
+        S.gn = H.n[0]; S.an = H.n[1]; S.sn = H.n[2]; S.fn = H.n[3]; S.kn = H.n[4];
+        A.hdr[R.slot] = S;
+    }
+}
+
+StreamSnapArgs snap_args(Handle *h, const uint8_t *stage_d, size_t o_area) {
+    ImuStreams &M = h->imus;
+    StreamSnapArgs A;
+    A.hdr = reinterpret_cast<ImuStreamSlot *>(M.hdr.d);
+    A.q[0] = M.g.d; A.q[1] = M.a.d; A.q[2] = M.s.d; A.q[3] = M.f.d; A.q[4] = M.k.d;
+    A.qcap = M.qcap;
+    A.recs = reinterpret_cast<const StreamSnapRec *>(stage_d);
+    A.area = const_cast<uint8_t *>(stage_d) + o_area;
+    return A;
+}
+
+int stream_save_impl(Handle *h, int n, pvio_b200_imu_stream_snapshot *recs) {
+    if (n < 0 || (n > 0 && !recs)) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: bad record list");
+    if (n == 0) return 0;
+    ImuStreams &M = h->imus;
+    std::vector<uint8_t> taken;
+    std::vector<int64_t> size(n), at(n, -1);
+    int64_t area = 0;
+    int packed = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_snapshot &r = recs[i];
+        if (r.slot < 0 || r.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: slot out of range");
+        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
+        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: a slot appears twice");
+        taken[r.slot] = 1;
+        if ((size_t)r.slot >= M.host.size() || !M.host[r.slot].set)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: the slot was never reset");
+        const ImuStreamHost &S = M.host[r.slot];
+        const int32_t cnt[5] = {(int32_t)S.g, (int32_t)S.a, (int32_t)S.s, (int32_t)S.f, (int32_t)S.k};
+        size[i] = stream_snap_size(cnt);
+        if (!r.data) continue;
+        if (r.capacity < size[i]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: capacity below the record's size");
+        at[i] = area;
+        area += (int64_t)align256(size[i]);
+        ++packed;
+    }
+    if (packed) {
+        // staging: records (uploaded) | blobs (downloaded)
+        const size_t o_area = align256(sizeof(StreamSnapRec) * packed);
+        TRY(reserve(h, M.stage, o_area + area, kBoth));
+        StreamSnapRec *hr = reinterpret_cast<StreamSnapRec *>(M.stage.h);
+        for (int i = 0, j = 0; i < n; ++i)
+            if (at[i] >= 0) hr[j++] = StreamSnapRec{recs[i].slot, 0, at[i]};
+        cudaStream_t st = h->stream;
+        CK(h, cudaMemcpyAsync(M.stage.d, M.stage.h, sizeof(StreamSnapRec) * packed, cudaMemcpyHostToDevice, st));
+        imu_stream_pack_kernel<<<packed, kSnapThreads, 0, st>>>(snap_args(h, M.stage.d, o_area));
+        ++h->launches;
+        CK(h, cudaGetLastError());
+        CK(h, cudaMemcpyAsync(M.stage.h + o_area, M.stage.d + o_area, area, cudaMemcpyDeviceToHost, st));
+        CK(h, cudaStreamSynchronize(st));
+        for (int i = 0; i < n; ++i) {
+            if (at[i] < 0) continue;
+            const ImuStreamHost &S = M.host[recs[i].slot];
+            uint8_t *out = recs[i].data;
+            memcpy(out, M.stage.h + o_area + at[i], size[i]);
+            StreamSnapHead H;
+            memcpy(&H, out, sizeof(H));
+            H.magic = PVIO_B200_IMU_STREAM_SNAPSHOT_MAGIC;
+            H.version = PVIO_B200_IMU_STREAM_SNAPSHOT_VERSION;
+            H.size = size[i];
+            H.n[0] = (int32_t)S.g; H.n[1] = (int32_t)S.a; H.n[2] = (int32_t)S.s; H.n[3] = (int32_t)S.f; H.n[4] = (int32_t)S.k;
+            H.seen_g = S.seen_g; H.seen_a = S.seen_a; H.dropped = S.dropped;
+            H.last_g = S.last_g; H.last_a = S.last_a; H.t_drop = S.t_drop;
+            memcpy(out, &H, sizeof(H));
+        }
+    }
+    for (int i = 0; i < n; ++i) recs[i].size = size[i];
+    return 0;
+}
+
+// why a blob cannot be restored, or nullptr
+const char *stream_snap_check(const uint8_t *data, int64_t bytes, StreamSnapHead &H) {
+    if (!data || bytes < (int64_t)sizeof(StreamSnapHead)) return "a blob shorter than its head";
+    memcpy(&H, data, sizeof(H));
+    if (H.magic != PVIO_B200_IMU_STREAM_SNAPSHOT_MAGIC || H.version != PVIO_B200_IMU_STREAM_SNAPSHOT_VERSION)
+        return "not a stream slot blob of this version";
+    for (int q = 0; q < 5; ++q)
+        if (H.n[q] < 0 || H.n[q] > PVIO_B200_IMU_STREAM_MAX_QUEUE) return "a queue count out of range";
+    const StreamSnapDev &d = H.dev;
+    if (d.nfront < 0 || d.nfront > H.n[2]) return "nfront above the unreleased samples";
+    if (H.size != bytes || H.size != stream_snap_size(H.n)) return "the declared size is not the blob's";
+    const int32_t flags[7] = {H.seen_g, H.seen_a, H.dropped, d.has_state, d.drop_pending, d.has_prev, d.prev_nonempty};
+    for (int32_t f : flags)
+        if (f != 0 && f != 1) return "a flag outside 0 / 1";
+    if (d.pad != 0) return "a padding field not zero";
+    if (d.drop_pending && !d.has_state) return "drop_pending without a state";
+    if (d.prev_nonempty && !d.has_prev) return "prev_nonempty without a previous frame";
+    const double head_v[3] = {H.last_g, H.last_a, H.t_drop};
+    if (!finite_all(head_v, 3) || !finite_all(d.q_ob, 4) || !finite_all(d.p_ob, 3) || !finite_all(&d.state_t, 1) ||
+        !finite_all(d.state, 16) || !finite_all(&d.prev_t, 1) || !finite_all(d.prev_row, 6))
+        return "a head value is not finite";
+    if (d.has_state && H.dropped && H.t_drop > d.state_t) return "the state is older than a frame released without one";
+    const double *v = reinterpret_cast<const double *>(data + sizeof(StreamSnapHead));
+    const bool seen[5] = {H.seen_g != 0, H.seen_a != 0, H.seen_g && H.seen_a, true, H.seen_g && H.seen_a};
+    for (int q = 0; q < 5; ++q) {
+        const int w = queue_width(q);
+        if (!finite_all(v, w * H.n[q])) return "a queue value is not finite";
+        if (H.n[q] > 0 && !seen[q]) return "a non-empty queue of a stream never seen";
+        for (int r = 1; r < H.n[q] && q != 3; ++r)
+            if (v[r * w] < v[(r - 1) * w]) return "a queue's times decrease";
+        if (H.n[q] > 0 && q < 2 && v[(H.n[q] - 1) * w] > (q == 0 ? H.last_g : H.last_a))
+            return "a queued reading newer than its stream's last";
+        v += (size_t)w * H.n[q];
+    }
+    return nullptr;
+}
+
+int stream_restore_impl(Handle *h, int n, const pvio_b200_imu_stream_snapshot *recs) {
+    if (n < 0 || (n > 0 && !recs)) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_restore: bad record list");
+    if (n == 0) return 0;
+    ImuStreams &M = h->imus;
+    std::vector<uint8_t> taken;
+    std::vector<StreamSnapHead> heads(n);
+    int top = 0, qcap = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_snapshot &r = recs[i];
+        if (r.slot < 0 || r.slot > kMaxBatchSlot)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_restore: slot out of range");
+        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
+        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_restore: a slot appears twice");
+        taken[r.slot] = 1;
+        if (const char *why = stream_snap_check(r.data, r.capacity, heads[i]))
+            return fail(h, PVIO_B200_EINVAL, (std::string("batch_imu_stream_restore: ") + why).c_str());
+        top = std::max(top, r.slot + 1);
+        for (int q = 0; q < 5; ++q) qcap = std::max(qcap, heads[i].n[q]);
+    }
+    TRY(ensure_streams(h, top, qcap));
+
+    // staging: records | blobs, uploaded
+    const size_t o_area = align256(sizeof(StreamSnapRec) * n);
+    size_t area = 0;
+    for (int i = 0; i < n; ++i) area += align256(heads[i].size);
+    TRY(reserve(h, M.stage, o_area + area, kBoth));
+    StreamSnapRec *hr = reinterpret_cast<StreamSnapRec *>(M.stage.h);
+    size_t at = 0;
+    for (int i = 0; i < n; ++i) {
+        hr[i] = StreamSnapRec{recs[i].slot, 0, (int64_t)at};
+        memcpy(M.stage.h + o_area + at, recs[i].data, heads[i].size);
+        at += align256(heads[i].size);
+    }
+    cudaStream_t st = h->stream;
+    CK(h, cudaMemcpyAsync(M.stage.d, M.stage.h, o_area + area, cudaMemcpyHostToDevice, st));
+    imu_stream_unpack_kernel<<<n, kSnapThreads, 0, st>>>(snap_args(h, M.stage.d, o_area));
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaStreamSynchronize(st));
+    if ((size_t)top > M.host.size()) M.host.resize(top);
+    for (int i = 0; i < n; ++i) {
+        const StreamSnapHead &H = heads[i];
+        ImuStreamHost &S = M.host[recs[i].slot];
+        S.set = true;
+        S.has_state = H.dev.has_state;
+        S.seen_g = H.seen_g; S.last_g = H.last_g;
+        S.seen_a = H.seen_a; S.last_a = H.last_a;
+        S.dropped = H.dropped; S.t_drop = H.t_drop;
+        S.g = H.n[0]; S.a = H.n[1]; S.s = H.n[2]; S.f = H.n[3]; S.k = H.n[4];
+    }
+    return 0;
+}
+
 }  // namespace
 
 }  // namespace pvio
@@ -529,4 +797,16 @@ extern "C" int pvio_b200_batch_imu_stream(pvio_b200_handle hh, int n, pvio_b200_
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     return stream_impl(h, n, records);
+}
+
+extern "C" int pvio_b200_batch_imu_stream_save(pvio_b200_handle hh, int n, pvio_b200_imu_stream_snapshot *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return stream_save_impl(h, n, records);
+}
+
+extern "C" int pvio_b200_batch_imu_stream_restore(pvio_b200_handle hh, int n, const pvio_b200_imu_stream_snapshot *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return stream_restore_impl(h, n, records);
 }

@@ -75,3 +75,33 @@ class ImuStream:
                 o += int(fr[i][k])
             out.append(dict(n_consumed=int(r.n_consumed), poses=poses[i][:r.n_consumed].copy(), frames=frames))
         return out
+
+    def save(self, slots):
+        """Save each stream slot to host memory.  Returns one blob (bytes) per slot, which restore() seats in any stream
+        slot of any handle."""
+        recs, n = self._snapshots(slots)
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream_save(self.h, n, recs))     # data NULL: the sizes
+        bufs = [np.zeros(recs[i].size, dtype=np.uint8) for i in range(n)]
+        for i, b in enumerate(bufs):
+            recs[i].data, recs[i].capacity = _lib.ptr(b), len(b)
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream_save(self.h, n, recs))
+        return [b.tobytes() for b in bufs]
+
+    def restore(self, slots, blobs):
+        """Restore blobs of save(): slot i takes blobs[i] and counts as reset.  One blob in several slots forks it."""
+        recs, n = self._snapshots(slots)
+        arrs = [np.frombuffer(b, dtype=np.uint8) for b in blobs]
+        if len(arrs) != n:
+            raise ValueError("one blob per slot")
+        for i, a in enumerate(arrs):
+            recs[i].data, recs[i].capacity = _lib.ptr(a), len(a)
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream_restore(self.h, n, recs))
+
+    @staticmethod
+    def _snapshots(slots):
+        """the pvio_b200_imu_stream_snapshot records of a save / restore call, and their count"""
+        slots = [int(s) for s in slots]
+        recs = (_lib.CImuStreamSnapshot * max(len(slots), 1))()
+        for r, s in zip(recs, slots):
+            r.slot = s
+        return recs, len(slots)
