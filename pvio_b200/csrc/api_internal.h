@@ -125,8 +125,9 @@ struct KltBatchState {
     std::vector<SlotLens> lens;               // per slot, grown on demand by pvio_b200_batch_set_lens
     DevBuf<uint8_t> ustage;                   // both sides: pvio_b200_batch_undistort's descriptors and frames
     DevBuf<uint8_t> stage;                    // both sides: uploaded descriptors, frames and points | downloaded results |
-                                              // winners' masks; host side only: the mask jobs the device reads in place
-    DevBuf<uint8_t> scratch;                  // device: CLAHE tables, RANSAC matches, schedules, counts, models, masks
+                                              // winners' masks | the mask jobs the device reads in place (klt.cu)
+    DevBuf<uint8_t> scratch;                  // device: CLAHE tables, RANSAC matches, schedules, models, masks (and the
+                                              // LK arrays of points written on the device)
     DevBuf<uint8_t> fstage;                   // feature_track.cu, both sides: descriptors (uploaded) | outputs (downloaded)
     DevBuf<uint8_t> fscratch;                 // feature_track.cu, device: thinning, detection and commit working areas
 };
@@ -153,20 +154,17 @@ struct DetectBatchState {
                                               // sort temporaries, select working areas that do not fit on chip
 };
 
-// fmat.cu: RANSAC buffers, grown to the largest point count / iteration budget seen
+// fmat.cu: the buffers of the single F-matrix RANSAC call, grown to powers of two
 struct FmState {
-    DevBuf<uint8_t> stage;                    // both sides: problem, mask job, counts | p, q | schedule [s][7] (fmat.cu: FmStage)
-    DevBuf<int> counts;                       // [s][4] nmodels, count / median bits of each model, both sides
-    DevBuf<double> F;                         // [s][3][9]
-    DevBuf<unsigned> masks;                   // [s][3][words]
-    DevBuf<double> h_F;                       // pinned: the winning model
-    DevBuf<unsigned> h_mask;                  // pinned: its inlier mask
+    DevBuf<uint8_t> stage;                    // both sides: problem, matches, schedule | counts, the winner and its mask |
+                                              // the mask job the device reads in place
+    DevBuf<uint8_t> scratch;                  // device: the models and masks of every iteration
 };
 
 // twoview.cu: the buffers of pvio_b200_batch_two_view, grown to the largest call seen
 struct TwoViewState {
-    DevBuf<uint8_t> stage;                    // both sides: problems, keypoints (uploaded) | results (downloaded)
-    DevBuf<int> counts;                       // both sides: sample schedules and per-iteration inlier counts of both RANSACs
+    DevBuf<uint8_t> stage;                    // both sides: problems, keypoints (uploaded) | sample schedules and
+                                              // per-iteration inlier counts of both RANSACs, results (downloaded)
     DevBuf<uint8_t> scratch;                  // device: lots, models of every iteration, parallax, candidate scores
 };
 
@@ -236,8 +234,8 @@ struct BatchWindows {
     DevBuf<int32_t> lm_row;                      // [W][Mcap] packed landmark -> row
     DevBuf<int32_t> tkp;                         // [W][Mcap] keypoint index of each row in the newest frame, -1: none
                                                  // (meaningful while the slot's link is set, WinSlot::link)
-    DevBuf<uint8_t> stage;                       // both sides, grown: every call's staging (batch_window.cu: Stage) --
-                                                 // upload | in/out | download | device-only scratch
+    DevBuf<uint8_t> stage;                       // both sides, grown: every call's staging (Stage)
+    DevBuf<uint8_t> scratch;                     // device, grown: every call's scratch sections
     // IMU samples of the factors named by set_imu, indexed like imu_data (factor k couples frames k, k + 1); allocated
     // with the first set_imu, imu_s grown to the longest sample list seen
     int Scap = 0;                                // samples per factor in imu_s
@@ -327,8 +325,7 @@ struct Handle {
     KltBatchState kltb;                           // klt.cu: the batched tracker, independent of klt
     DevBuf<double> marg;                          // ba_marg.cu: scratch blocks of the marginaliser's dense kernels
     FmState fm;
-    DevBuf<double> pnp;                           // pnp.cu's own: both sides, grown on demand to the largest batch
-                                                  // (records, points, IMU records, frames) seen
+    DevBuf<uint8_t> pnp;                          // pnp.cu's own staging: both sides, grown to powers of two
     BatchWindows bw;                              // batch_window.cu (empty until the first pvio_b200_batch_window_reset)
     TwoViewState tv;                              // twoview.cu
     ImuStreams imus;                              // imu_stream.cu
@@ -400,6 +397,103 @@ int reserve(Handle *h, DevBuf<T> &b, size_t n, int sides) {
     return n <= b.n ? 0 : alloc(h, b, n, sides);
 }
 
+// x rounded up to the 256-byte boundary every staging section starts on; also for sub-blocks inside a section (per-frame
+// pixel blocks and the like)
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// One batched call's staging.  Sections are declared by kind and size, then laid out kind after kind in the order of Kind,
+// each on a 256-byte boundary (the largest alignment a kernel needs of one).  Upload, in/out, download and mapped sections
+// go to the staging buffer (both sides), in that order, so that the call copies upload + in/out to the device in one copy
+// and in/out + download back in one copy; the device reads mapped sections in place from pinned memory (unified
+// addressing), and nothing copies them.  Scratch sections go to the scratch buffer (device only), which a call that
+// declares none may leave out.
+struct Stage {
+    enum Kind { kUp, kInOut, kDown, kMapped, kScratch, kKinds };
+    template <typename T>
+    struct Sec { int i; };
+    struct Entry { Kind kind; size_t bytes; const void *src; size_t off; };
+    DevBuf<uint8_t> *buf, *scratch;
+    std::vector<Entry> secs;
+    size_t end[kKinds] = {};                  // after place: the end of each kind's sections in its buffer
+    uint8_t *hp = nullptr, *dp = nullptr, *sp = nullptr;
+    bool pow2 = false;                        // grow the buffers to powers of two (sizes that vary per call)
+
+    explicit Stage(DevBuf<uint8_t> &stage, DevBuf<uint8_t> *scratch_buf = nullptr) : buf(&stage), scratch(scratch_buf) {}
+
+    // n elements of kind k; src (n elements, or null): what place copies into the section
+    template <typename T>
+    Sec<T> add(Kind k, size_t n, const T *src = nullptr) {
+        secs.push_back(Entry{k, sizeof(T) * n, src, 0});
+        return Sec<T>{(int)secs.size() - 1};
+    }
+    template <typename T>
+    Sec<T> up(const std::vector<T> &v) { return add(kUp, v.size(), v.data()); }
+    template <typename T>
+    T *host(Sec<T> s) const { return reinterpret_cast<T *>(hp + secs[s.i].off); }
+    template <typename T>
+    T *dev(Sec<T> s) const { return reinterpret_cast<T *>((secs[s.i].kind == kScratch ? sp : dp) + secs[s.i].off); }
+
+    // lays the sections out, grows the buffers to them and copies the sources into the staging's host side; upload_now:
+    // then uploads (a call that fills host sections itself uploads after that)
+    int place(Handle *h, bool upload_now = false) {
+        size_t o = 0;
+        for (int k = 0; k < kKinds; ++k) {
+            if (k == kScratch) o = 0;
+            for (Entry &e : secs)
+                if (e.kind == k) { e.off = o; o += align256(e.bytes); }
+            end[k] = o;
+        }
+        if (end[kScratch] > 0 && !scratch) return fail(h, PVIO_B200_EINVAL, "internal error: scratch without a buffer");
+        TRY(reserve(h, *buf, grown(end[kMapped]), kBoth));
+        if (scratch) TRY(reserve(h, *scratch, grown(end[kScratch]), kDevice));
+        hp = buf->h; dp = buf->d; sp = scratch ? scratch->d : nullptr;
+        for (const Entry &e : secs)
+            if (e.src && e.bytes) memcpy(hp + e.off, e.src, e.bytes);
+        return upload_now ? upload(h) : 0;
+    }
+    int upload(Handle *h) const { return copy(h, 0, end[kInOut], true); }
+    int download(Handle *h) const { return copy(h, end[kUp], end[kDown], false); }
+    // sections a .. b (a laid out first, both in the staging buffer) in one copy: to the device after the host has
+    // rewritten them, or back to the host
+    template <typename A, typename B>
+    int upload(Handle *h, Sec<A> a, Sec<B> b) const { return copy(h, secs[a.i].off, last(b), true); }
+    template <typename A>
+    int upload(Handle *h, Sec<A> a) const { return upload(h, a, a); }
+    template <typename A, typename B>
+    int download(Handle *h, Sec<A> a, Sec<B> b) const { return copy(h, secs[a.i].off, last(b), false); }
+
+  private:
+    size_t grown(size_t n) const {
+        size_t w = n;
+        if (pow2 && n > 0)
+            for (w = 4096; w < n; w <<= 1) {}
+        return w;
+    }
+    template <typename B>
+    size_t last(Sec<B> b) const { return secs[b.i].off + secs[b.i].bytes; }
+    // bytes [o, e) of the staging buffer to the device (up) or back to the host
+    int copy(Handle *h, size_t o, size_t e, bool up) const {
+        if (e > o) CK(h, up ? cudaMemcpyAsync(dp + o, hp + o, e - o, cudaMemcpyHostToDevice, h->stream)
+                            : cudaMemcpyAsync(hp + o, dp + o, e - o, cudaMemcpyDeviceToHost, h->stream));
+        return 0;
+    }
+};
+
+// Slot s of a batched call whose slots must be distinct sequence slots (0 .. kMaxBatchSlot), marked in taken (grown to
+// it); null, or why it cannot be taken: out of range, or named before (the text `twice`)
+inline const char *take_slot(std::vector<uint8_t> &taken, int s, const char *twice = "a slot appears twice") {
+    if (s < 0 || s > kMaxBatchSlot) return "slot out of range";
+    if ((size_t)s >= taken.size()) taken.resize(s + 1, 0);
+    if (taken[s]) return twice;
+    taken[s] = 1;
+    return nullptr;
+}
+// the same for call `call`: 0, or PVIO_B200_EINVAL with the message "<call>: <why>"
+inline int take_slot(Handle *h, std::vector<uint8_t> &taken, int s, const char *call) {
+    const char *why = take_slot(taken, s);
+    return why ? fail(h, PVIO_B200_EINVAL, (std::string(call) + ": " + why).c_str()) : 0;
+}
+
 // api.cu: pack window into slot 0, copy it to the device, build the frame-major table
 int pack_and_upload(Handle *h, const pvio_b200_window *w, const pvio_b200_state *s);
 // api.cu: the constants of window w as the kernels read them, origin 0
@@ -447,6 +541,8 @@ struct PnpArgs {
 static_assert(sizeof(PnpArgs) % sizeof(double) == 0, "records are staged as whole 8-byte words");
 // the PnP kernel on n records already on the device, between the events ev0 / ev1: 256 threads for n == 1, otherwise 128
 int launch_pnp(Handle *h, int n, const PnpArgs *d_recs);
+// the summary of one problem from the kernel's 8 words PnpArgs::out, with the launch's time ms
+void pnp_summary(const double *out, float ms, pvio_b200_summary *s);
 int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,
                    pvio_b200_summary *summary);
 int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
@@ -508,7 +604,9 @@ struct KltBatchResults {
     std::vector<const unsigned *> mask;
     std::vector<uint8_t> clear;
     std::vector<int32_t> info;
-    size_t o_mw = 0, words = 0;               // the mask words: offset in KltBatchState::stage, count
+    unsigned *mw = nullptr;                   // the mask words (`words` of them) in KltBatchState::stage: host side,
+    const unsigned *d_mw = nullptr;           //   device side
+    size_t words = 0;
 };
 // Checks every pair, then uploads, builds the pyramids, runs LK, the schedules and the hypotheses, synchronises once,
 // replays each pair on the host and launches the winners' masks.  dev == nullptr: the points come from the items.

@@ -1092,7 +1092,7 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
                 if (s.n_samples[k] > 0)
                     jobs.push_back(BwImu{slots[i], k, s.n_samples[k], (int32_t)(((size_t)slots[i] * h->Ncap + k) * h->bw.Scap)});
     }
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto nm = S.up(named);
     const auto lay = S.up(lays);
     const auto sl = S.add(Stage::kUp, n, slots);
@@ -1248,14 +1248,7 @@ static void loc_results(const Stage &S, const LocSecs &s, const LocPlan &P, int 
         R.new_inv_depth[t] = S.host(s.rho)[q];
         if (R.new_inv_depth_next) R.new_inv_depth_next[t] = S.host(s.next)[q];
     }
-    if (R.summary) {
-        const double *b = S.host(s.out) + 8 * (size_t)i;
-        pvio_b200_summary &S = *R.summary;
-        memset(&S, 0, sizeof(S));
-        S.iterations = (int)b[0]; S.accepted_steps = (int)b[1]; S.termination = (int)b[2]; S.usable = (int)b[3];
-        S.initial_cost = b[4]; S.final_cost = b[5]; S.final_radius = b[6]; S.final_mu = b[7];
-        S.solve_seconds = ms * 1e-3;
-    }
+    if (R.summary) pnp_summary(S.host(s.out) + 8 * (size_t)i, ms, R.summary);
 }
 
 // the localize half of a track_frame record
@@ -1589,7 +1582,7 @@ int pvio_b200_batch_window_reset(pvio_b200_handle hh, int slot, const pvio_b200_
     WinConst &C = h->cst.h[slot];
     C = win_const(w);
     CK(h, cudaMemcpyAsync(h->cst.dslot(slot), &C, sizeof(WinConst), cudaMemcpyHostToDevice, h->stream));
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const Relayout lay(S, &slot, next);
     TRY(S.place(h, true));
     TRY(lay.launch(h, S, false));
@@ -1619,7 +1612,7 @@ int pvio_b200_batch_window_set_prior(pvio_b200_handle hh, int slot, int n_prior,
     }
     std::vector<WinSlot> next(1, s);
     next[0].n_prior = next[0].prior_resident = n_prior;
-    Stage st;
+    Stage st(h->bw.stage, &h->bw.scratch);
     const Relayout lay(st, &slot, next);
     TRY(st.place(h, true));
     TRY(lay.launch(h, st, n_prior > 0));
@@ -1717,7 +1710,7 @@ int pvio_b200_batch_window_edit(pvio_b200_handle hh, int n, const pvio_b200_wind
         next[i] = std::move(s);
     }
     TRY(ensure_plane_tables(h, next));                 // observations of plane tracks may outgrow the plane tables
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto ed = S.up(recs);
     const auto nw = S.up(nws);
     const auto ob = S.up(obs);
@@ -1788,7 +1781,7 @@ int pvio_b200_batch_window_set_planes(pvio_b200_handle hh, int n, const pvio_b20
         next[i] = std::move(s);
     }
     TRY(ensure_plane_tables(h, next));
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto rec = S.up(recs);
     const auto ro = S.up(roles);
     const auto pa = S.up(params);
@@ -1835,7 +1828,7 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
     }
     std::vector<BwLayout> before(n);
     for (int i = 0; i < n; ++i) before[i] = layout_of(slots[i], h->slots[slots[i]]);
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto b = S.up(before);
     const Relayout lay(S, slots, next);
     TRY(S.place(h, true));
@@ -1873,7 +1866,7 @@ int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *s
         dls[i] = BwDl{slots[i], s.N, T, 0, off};
         off += BwDlRec::bytes(s.N, T);
     }
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto dl = S.up(dls);
     const auto out = S.add<uint8_t>(Stage::kDown, (size_t)off);
     TRY(S.place(h, true));
@@ -1912,7 +1905,7 @@ int pvio_b200_batch_window_localize(pvio_b200_handle hh, int n, pvio_b200_window
     LocPlan P;
     P.what = "batch_window_localize";
     for (int i = 0; i < n; ++i) TRY(loc_add(h, P, records[i], true));
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const LocSecs s = loc_stage(S, P, true);
     TRY(S.place(h));
     const size_t w8 = sizeof(double);
@@ -1990,7 +1983,7 @@ int pvio_b200_batch_window_track_frame(pvio_b200_handle hh, int n, pvio_b200_win
     // track records | jobs | observed pairs' rows | their keypoints | merge_samples ++ samples | t_end and noise,
     // download the edit's IMU records | predicted states | keyframe words, scratch step-1 records | parallaxes
     const size_t w8 = sizeof(double), J = jobs.size();
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const LocSecs s = loc_stage(S, P, false);
     const auto tr = S.up(trs);
     const auto job = S.up(jobs);
@@ -2078,7 +2071,7 @@ int pvio_b200_batch_window_set_imu(pvio_b200_handle hh, int n, const pvio_b200_w
         return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: a (slot, frame) named twice");
     if (rows > (size_t)INT32_MAX) return fail(h, PVIO_B200_EINVAL, "batch_window_set_imu: too many samples in one call");
     TRY(ensure_imu_store(h, smax));
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto rec = S.up(recs);
     const auto smp = S.add<double>(Stage::kUp, 7 * rows), aux = S.add<double>(Stage::kUp, (size_t)n * kImuAux);
     TRY(S.place(h));
@@ -2115,7 +2108,7 @@ int pvio_b200_batch_window_imu_records(pvio_b200_handle hh, int n, const int32_t
         dls[i] = BwDl{slots[i], std::max(s.N, 1), 0, 0, off};
         off += m * (int64_t)sizeof(double);
     }
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto dl = S.up(dls);
     const auto out = S.add<uint8_t>(Stage::kDown, (size_t)off);
     TRY(S.place(h, true));
@@ -2175,7 +2168,7 @@ int pvio_b200_batch_window_set_keypoints(pvio_b200_handle hh, int n, const pvio_
         if (std::adjacent_find(kps.begin(), kps.end()) != kps.end())
             return fail(h, PVIO_B200_EINVAL, "batch_window_set_keypoints: a keypoint named twice");
     }
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto k = S.up(ks);
     const auto p = S.up(pairs);
     TRY(S.place(h, true));
@@ -2216,6 +2209,7 @@ struct MirCall {
     std::vector<uint8_t> taken;
     size_t kp = 0, tab = 0, rm = 0, rows = 0;
     int smax = 0, n1 = 0;                     // n1: the step-1 jobs (split)
+    bool cam = false;                         // staged for track_camera (stage)
 
     Stage S;
     Stage::Sec<BwMirror> mr;
@@ -2236,7 +2230,8 @@ struct MirCall {
     TrackArgs T;
     MirArgs M;
 
-    MirCall(const char *w, int n) : what(w), mir(n), locs(n), trs(n), eds(n), next(n) {}
+    MirCall(Handle *h, const char *w, int n)
+        : what(w), mir(n), locs(n), trs(n), eds(n), next(n), S(h->bw.stage, &h->bw.scratch) {}
     int bad(Handle *h, const char *why) const { return fail(h, PVIO_B200_EINVAL, (std::string(what) + ": " + why).c_str()); }
 
     // Record i checked against its slot's host mirror; tracker_why: the caller's verdict on the tracker slot (null:
@@ -2248,9 +2243,7 @@ struct MirCall {
         if (s.N < 1) return "a window without frames";
         if (!s.link) return "the slot has no link to a tracker slot (set_keypoints)";
         if (R.tracker_slot != s.link_tracker) return "not the tracker slot of the slot's link";
-        if ((size_t)R.tracker_slot >= taken.size()) taken.resize(R.tracker_slot + 1, 0);
-        if (taken[R.tracker_slot]) return "a tracker slot named twice";
-        taken[R.tracker_slot] = 1;
+        if (const char *why = take_slot(taken, R.tracker_slot, "a tracker slot named twice")) return why;
         if (tracker_why) return tracker_why;
         if (!R.samples || !R.noise_cov || !R.kp_track || !R.state || !R.keyframe) return "null array";
         if (R.max_keypoints < v.n_j) return "max_keypoints below the tracker's keypoint count";
@@ -2315,10 +2308,10 @@ struct MirCall {
 
     // staging: upload records | track_frame's records, jobs, samples, t_end and noise | given points | edit records |
     // kept factors | re-layout; download counts | continued rows (the capacity check), then the results; device only
-    // the mirror's tables and lists, the localize sections, the edit's lists.  camera (track_camera): the continued rows are a
-    // download section right after the counts, so that one copy brings both back (they then come back with the
-    // results too), and the delta_key_q of every record comes back; otherwise they are device scratch, downloaded on
-    // their own (mirror_frame).  Uploads everything.
+    // the mirror's tables and lists, the localize sections, the edit's lists.  camera (track_camera): the continued rows
+    // are the section right after the counts, so that one copy brings both back (they then come back with the results
+    // too), and the delta_key_q of every record comes back; otherwise they are the last section, after the results'
+    // range, downloaded on their own (mirror_frame).  Uploads everything.
     int stage(Handle *h, const pvio_b200_window_mirror *records, const pvio_b200_options *opt, bool camera) {
         const int n = (int)mir.size();
         if (!kimu.empty()) TRY(ensure_imu_store(h, smax));   // the kept lists' room, before anything is staged
@@ -2334,14 +2327,16 @@ struct MirCall {
         kim = S.up(kimu);
         kax = S.up(kaux);
         lay.emplace(S, slots.data(), next);
+        cam = camera;
         cnt = S.add<int32_t>(Stage::kDown, 4 * (size_t)n);
-        cont = S.add<int2>(camera ? Stage::kDown : Stage::kScratch, kp);
+        if (camera) cont = S.add<int2>(Stage::kDown, kp);
         live = S.add<int32_t>(Stage::kDown, n);
         frames = S.add<double>(Stage::kDown, 16 * (size_t)n); out = S.add<double>(Stage::kDown, 8 * (size_t)n);
         rec_out = S.add<double>(Stage::kDown, (size_t)n * kImuStride); pred = S.add<double>(Stage::kDown, 16 * (size_t)n);
         kfo = S.add<double>(Stage::kDown, 4 * (size_t)n);
         kpt = S.add<int32_t>(Stage::kDown, kp);
         if (camera) pq = S.add<double>(Stage::kDown, 4 * (size_t)n);
+        else cont = S.add<int2>(Stage::kDown, kp);
         eout = S.add<int32_t>(Stage::kScratch, kp + n);
         tabs = S.add<int32_t>(Stage::kScratch, tab); rmap = S.add<int32_t>(Stage::kScratch, rm);
         lrow = S.add<int32_t>(Stage::kScratch, kp); cand = S.add<int32_t>(Stage::kScratch, kp);
@@ -2449,7 +2444,7 @@ struct MirCall {
         bw_mirror_link_kernel<<<n, kBwThreads, 0, h->stream>>>(a, M);
         ++h->launches;
         CK(h, cudaGetLastError());
-        TRY(S.download(h));
+        TRY(cam ? S.download(h) : S.download(h, cnt, kpt));
         CK(h, cudaStreamSynchronize(h->stream));
         return 0;
     }
@@ -2516,7 +2511,7 @@ int pvio_b200_batch_window_mirror_frame(pvio_b200_handle hh, int n, pvio_b200_wi
     TRY(check_slots(h, n, slots.data(), "batch_window_mirror_frame: bad slot list"));
     // every record is checked against its slot's host mirror and its tracker slot before anything is staged
     const KltBatchState &B = h->kltb;
-    MirCall C("batch_window_mirror_frame", n);
+    MirCall C(h, "batch_window_mirror_frame", n);
     std::vector<uint64_t> fid(n);
     std::vector<uint32_t> gen(n);
     for (int i = 0; i < n; ++i) {
@@ -2566,7 +2561,7 @@ int pvio_b200_batch_window_track_camera(pvio_b200_handle hh, int n, pvio_b200_wi
                                         R.max_keypoints, R.kp_track, R.counts, R.state, R.predicted, R.imu_record,
                                         R.keyframe, R.parallax, R.n_parallax, R.skipped_frames, R.summary};
     }
-    MirCall C("batch_window_track_camera", n);
+    MirCall C(h, "batch_window_track_camera", n);
     for (int i = 0; i < n; ++i) {
         const pvio_b200_window_camera &R = records[i];
         if (!h->slots[R.slot].inertial) return C.bad(h, "the window carries no motion states");
@@ -2703,7 +2698,7 @@ int pvio_b200_batch_window_save(pvio_b200_handle hh, int n, pvio_b200_window_sna
         area += H.size - offs[i].dev0;
     }
     if (!recs.empty()) {
-        Stage S;
+        Stage S(h->bw.stage, &h->bw.scratch);
         const auto rc = S.up(recs);
         const auto fc = S.up(facs);
         const auto out = S.add<uint8_t>(Stage::kDown, (size_t)area);
@@ -2912,7 +2907,7 @@ int pvio_b200_batch_window_restore(pvio_b200_handle hh, int n, const pvio_b200_w
         r.n[0] = R.tracker_slot >= 0 ? H.n[0] : 0; r.n[1] = R.tracker_slot >= 0 ? H.n[1] : 0;
         area += H.size;
     }
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto blob = S.add<uint8_t>(Stage::kUp, (size_t)area);
     const auto rc = S.up(recs);
     const auto fc = S.up(facs);

@@ -1,11 +1,10 @@
 // The pieces of the resident batched windows (batch_window.cu) that other calls on the slots share: the kernels' view of
-// the track table, the CTA scan, the camera pose and world point of a slot row, the staging of a call, and the row of a
-// track id in a slot's host mirror.  Used by batch_window.cu and plane_ransac.cu.
+// the track table, the CTA scan, the camera pose and world point of a slot row, and the row of a track id in a slot's
+// host mirror.  Used by batch_window.cu and plane_ransac.cu; their calls stage through Stage (api_internal.h) in
+// BatchWindows::stage and BatchWindows::scratch.
 #pragma once
 
 #include <algorithm>
-#include <cstring>
-#include <vector>
 
 #include "api_internal.h"
 #include "quat.cuh"
@@ -90,75 +89,6 @@ __device__ inline void loc_camera_matrix(const double *qc, const double *pc, dou
     bw_qrot(qi, pc, t);
     for (int i = 0; i < 3; ++i) P[4 * i + 3] = -t[i];
 }
-
-// One call's staging in BatchWindows::stage.  Sections are declared by kind and size, then laid out kind after kind in
-// the order of Kind, each 8-byte aligned, so that the call copies upload + in/out to the device in one copy and in/out +
-// download back in one copy; scratch stays on the device.
-struct Stage {
-    enum Kind { kUp, kInOut, kDown, kScratch, kKinds };
-    template <typename T>
-    struct Sec { int i; };
-    struct Entry { Kind kind; size_t bytes; const void *src; size_t off; };
-    std::vector<Entry> secs;
-    size_t end[kKinds] = {};                  // after place: the end of each kind's sections
-    uint8_t *hp = nullptr, *dp = nullptr;
-    bool pow2 = false;                        // grow BatchWindows::stage to a power of two (sizes that vary per call)
-
-    // n elements of kind k; src (n elements, or null): what place copies into the section
-    template <typename T>
-    Sec<T> add(Kind k, size_t n, const T *src = nullptr) {
-        secs.push_back(Entry{k, sizeof(T) * n, src, 0});
-        return Sec<T>{(int)secs.size() - 1};
-    }
-    template <typename T>
-    Sec<T> up(const std::vector<T> &v) { return add(kUp, v.size(), v.data()); }
-    template <typename T>
-    T *host(Sec<T> s) const { return reinterpret_cast<T *>(hp + secs[s.i].off); }
-    template <typename T>
-    T *dev(Sec<T> s) const { return reinterpret_cast<T *>(dp + secs[s.i].off); }
-
-    // lays the sections out, grows BatchWindows::stage to them and copies the sources into its host side; upload_now:
-    // then uploads (a call that fills host sections itself uploads after that)
-    int place(Handle *h, bool upload_now = false) {
-        size_t o = 0;
-        for (int k = 0; k < kKinds; ++k) {
-            for (Entry &e : secs)
-                if (e.kind == k) { e.off = o; o += (e.bytes + 7) & ~(size_t)7; }
-            end[k] = o;
-        }
-        size_t want = o;
-        if (pow2)
-            for (want = 4096; want < o; want <<= 1) {}
-        TRY(reserve(h, h->bw.stage, want, kBoth));
-        hp = h->bw.stage.h; dp = h->bw.stage.d;
-        for (const Entry &e : secs)
-            if (e.src && e.bytes) memcpy(hp + e.off, e.src, e.bytes);
-        return upload_now ? upload(h) : 0;
-    }
-    int upload(Handle *h) const {
-        if (end[kInOut] > 0) CK(h, cudaMemcpyAsync(dp, hp, end[kInOut], cudaMemcpyHostToDevice, h->stream));
-        return 0;
-    }
-    int download(Handle *h) const {
-        if (end[kDown] > end[kUp])
-            CK(h, cudaMemcpyAsync(hp + end[kUp], dp + end[kUp], end[kDown] - end[kUp], cudaMemcpyDeviceToHost, h->stream));
-        return 0;
-    }
-    // one upload section again, after the host has rewritten it
-    template <typename A>
-    int upload(Handle *h, Sec<A> a) const {
-        if (secs[a.i].bytes)
-            CK(h, cudaMemcpyAsync(dp + secs[a.i].off, hp + secs[a.i].off, secs[a.i].bytes, cudaMemcpyHostToDevice, h->stream));
-        return 0;
-    }
-    // sections a .. b (declared in that order, one kind) back to the host in one copy
-    template <typename A, typename B>
-    int download(Handle *h, Sec<A> a, Sec<B> b) const {
-        const size_t o = secs[a.i].off, e = secs[b.i].off + secs[b.i].bytes;
-        if (e > o) CK(h, cudaMemcpyAsync(hp + o, dp + o, e - o, cudaMemcpyDeviceToHost, h->stream));
-        return 0;
-    }
-};
 
 // the row of track `id` in a slot's host mirror, -1 for an unknown or dead track
 inline int find_row(const WinSlot &s, int32_t id) {

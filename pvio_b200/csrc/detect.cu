@@ -361,8 +361,6 @@ struct SegEnd {
     }
 };
 
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 }  // namespace
 
 DetectPlan detect_plan(int w, int hgt, double keypoint_distance, int n_pre) {
@@ -489,38 +487,34 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
     for (auto &P : plan)
         if (P.work > smem) { P.work_off = work_bytes; work_bytes += P.work; }
 
-    // staging (both sides): upload [0, o_up) | download [o_res, o)
-    size_t o = 0;
-    const size_t o_frm = o; o = align256(o + sizeof(DetectBatchFrame) * n);
-    const size_t o_kf = o;  o = align256(o + sizeof(KltBatchFrame) * n_kf);
-    const size_t o_cnt = o; o = align256(o + sizeof(int) * 2 * n);
-    const size_t o_pre = o; o = align256(o + sizeof(double2) * n_pre);
-    const size_t o_pix = o; o += pix_bytes;
-    const size_t o_up = o;  o = align256(o);
-    const size_t o_res = o; o = align256(o + sizeof(DetectResult) * n);
+    // staging: frame descriptors, remap / CLAHE descriptors, counters, presets, pixels (uploaded) | results (downloaded);
     // device scratch: responses | keys | sorted keys | equalised frames | CLAHE tables | working areas | sort temporaries |
     // undistorted frames
     const size_t tiles = do_clahe ? (size_t)tiles_x * tiles_y : 0;
     size_t cub_bytes = 0;
     TRY(detect_sort_bytes(h, n, n_keys, cub_bytes));
-    size_t c = 0;
-    const size_t c_resp = c;   c += resp_bytes;
-    const size_t c_keys = c;   c = align256(c + sizeof(unsigned long long) * n_keys);
-    const size_t c_sorted = c; c = align256(c + sizeof(unsigned long long) * n_keys);
-    const size_t c_eq = c;     c += eq_bytes;
-    const size_t c_lut = c;    c = align256(c + tiles * 256 * n_eq);
-    const size_t c_work = c;   c += work_bytes;
-    const size_t c_cub = c;    c = align256(c + cub_bytes);
-    const size_t c_und = c;    c += und_bytes;
     DetectBatchState &D = h->detectb;
-    TRY(reserve(h, D.stage, o, kBoth));
-    TRY(reserve(h, D.scratch, c, kDevice));
+    Stage S(D.stage, &D.scratch);
+    const auto sFrm = S.add<DetectBatchFrame>(Stage::kUp, n);
+    const auto sKf = S.add<KltBatchFrame>(Stage::kUp, n_kf);
+    const auto sCnt = S.add<int>(Stage::kUp, 2 * n);
+    const auto sPre = S.add<double2>(Stage::kUp, n_pre);
+    const auto sPix = S.add<uint8_t>(Stage::kUp, pix_bytes);
+    const auto sRes = S.add<DetectResult>(Stage::kDown, n);
+    const auto sResp = S.add<uint8_t>(Stage::kScratch, resp_bytes);
+    const auto sKeys = S.add<unsigned long long>(Stage::kScratch, n_keys);
+    const auto sSorted = S.add<unsigned long long>(Stage::kScratch, n_keys);
+    const auto sEq = S.add<uint8_t>(Stage::kScratch, eq_bytes);
+    const auto sLut = S.add<uint8_t>(Stage::kScratch, tiles * 256 * n_eq);
+    const auto sWork = S.add<uint8_t>(Stage::kScratch, work_bytes);
+    const auto sCub = S.add<uint8_t>(Stage::kScratch, cub_bytes);
+    const auto sUnd = S.add<uint8_t>(Stage::kScratch, und_bytes);
+    TRY(S.place(h));
 
-    uint8_t *hs = D.stage.h, *ds = D.stage.d, *dc = D.scratch.d;
-    DetectBatchFrame *frm = reinterpret_cast<DetectBatchFrame *>(hs + o_frm);
-    KltBatchFrame *kf = reinterpret_cast<KltBatchFrame *>(hs + o_kf);
-    double2 *pre = reinterpret_cast<double2 *>(hs + o_pre);
-    memset(hs + o_cnt, 0, sizeof(int) * 2 * n);
+    DetectBatchFrame *frm = S.host(sFrm);
+    KltBatchFrame *kf = S.host(sKf);
+    double2 *pre = S.host(sPre);
+    memset(S.host(sCnt), 0, sizeof(int) * 2 * n);
     size_t p = 0;
     int q_lens = 0, q_plain = n_lens;
     for (int i = 0; i < n; ++i) {
@@ -528,9 +522,9 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
         const Plan &P = plan[i];
         const uint8_t *img = cached[i];
         if (!img) {
-            uint8_t *dst = hs + o_pix + P.pix_off;
+            uint8_t *dst = S.host(sPix) + P.pix_off;
             for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, a.image + (size_t)y * a.stride, a.width);
-            uint8_t *up = ds + o_pix + P.pix_off;
+            uint8_t *up = S.dev(sPix) + P.pix_off;
             img = up;
             if (do_clahe || lens[i]) {        // raw pixels: remap and / or CLAHE into the detector's scratch
                 const int q = lens[i] ? q_lens++ : q_plain++;
@@ -539,14 +533,14 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
                 K.raw = up;
                 if (lens[i]) {
                     K.lens_src = up; K.m1 = lens[i]->m1(); K.m2 = lens[i]->m2();
-                    K.raw = dc + c_und + P.und_off;
+                    K.raw = S.dev(sUnd) + P.und_off;
                 }
                 K.levels = 1;
                 K.w[0] = a.width; K.h[0] = a.height;
                 img = K.raw;
                 if (do_clahe) {
-                    K.lut = dc + c_lut + (size_t)q * tiles * 256;
-                    K.pyr = dc + c_eq + P.eq_off;
+                    K.lut = S.dev(sLut) + (size_t)q * tiles * 256;
+                    K.pyr = S.dev(sEq) + P.eq_off;
                     klt_clahe_params(a.width, a.height, clahe_clip, tiles_x, tiles_y, K.tw, K.th, K.clip, K.lut_scale);
                     img = K.pyr;
                 }
@@ -555,30 +549,28 @@ int batch_detect_impl(Handle *h, int n, const pvio_b200_detect_request *reqs, do
         DetectBatchFrame &F = frm[i];
         memset(&F, 0, sizeof(F));
         F.img = img;
-        F.resp = reinterpret_cast<float *>(dc + c_resp + P.resp_off);
-        F.keys = reinterpret_cast<unsigned long long *>(dc + c_keys) + P.key_off;
-        F.sorted = reinterpret_cast<unsigned long long *>(dc + c_sorted) + P.key_off;
-        F.counters = reinterpret_cast<int *>(ds + o_cnt) + 2 * i;
-        F.pre = reinterpret_cast<const double2 *>(ds + o_pre) + p;
+        F.resp = reinterpret_cast<float *>(S.dev(sResp) + P.resp_off);
+        F.keys = S.dev(sKeys) + P.key_off;
+        F.sorted = S.dev(sSorted) + P.key_off;
+        F.counters = S.dev(sCnt) + 2 * i;
+        F.pre = S.dev(sPre) + p;
         for (int j = 0; j < a.n_existing; ++j) pre[p++] = make_double2(a.existing[2 * j], a.existing[2 * j + 1]);
-        F.work = P.work > smem ? dc + c_work + P.work_off : nullptr;
-        F.res = reinterpret_cast<DetectResult *>(ds + o_res) + i;
+        F.work = P.work > smem ? S.dev(sWork) + P.work_off : nullptr;
+        F.res = S.dev(sRes) + i;
         detect_apply_plan(P, a.width, a.height, a.keypoint_distance, F);
         F.key_off = P.key_off;
     }
 
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(ds, hs, o_up, cudaMemcpyHostToDevice, st));
-    const DetectBatchFrame *d_frm = reinterpret_cast<const DetectBatchFrame *>(ds + o_frm);
-    if (n_lens > 0) undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_lens, und_w, und_h);
-    if (n_eq > 0) klt_batch_clahe(h, reinterpret_cast<const KltBatchFrame *>(ds + o_kf), n_eq, tiles_x, tiles_y, eq_w, eq_h);
-    TRY(detect_run(h, d_frm, n, max_w, max_h, reinterpret_cast<const unsigned long long *>(dc + c_keys),
-                   reinterpret_cast<unsigned long long *>(dc + c_sorted), n_keys, dc + c_cub, cub_bytes, smem));
-    CK(h, cudaMemcpyAsync(hs + o_res, ds + o_res, sizeof(DetectResult) * n, cudaMemcpyDeviceToHost, st));
+    TRY(S.upload(h));
+    if (n_lens > 0) undistort_frames(h, S.dev(sKf), n_lens, und_w, und_h);
+    if (n_eq > 0) klt_batch_clahe(h, S.dev(sKf), n_eq, tiles_x, tiles_y, eq_w, eq_h);
+    TRY(detect_run(h, S.dev(sFrm), n, max_w, max_h, S.dev(sKeys), S.dev(sSorted), n_keys, S.dev(sCub), cub_bytes, smem));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(st));
 
     // per request: the corners, and the keypoints the mask keeps, in order
-    const DetectResult *rr = reinterpret_cast<const DetectResult *>(hs + o_res);
+    const DetectResult *rr = S.host(sRes);
     bool overflow = false;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_detect_request &a = reqs[i];

@@ -61,8 +61,6 @@ inline size_t thin_work_bytes(int n, int hbits) {
     return a16(sizeof(int2) * n) + a16((size_t)n) + 12 * ((size_t)1 << hbits);
 }
 
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 __global__ void ft_guess_kernel(const FtSeq *seqs, const int *pair_of, float *prev_pts, float *next_pts, int n_pts) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n_pts) return;
@@ -222,10 +220,7 @@ int ft_check(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltB
     n_prev.assign(n, 0);
     for (int i = 0; i < n; ++i) {
         const pvio_b200_feature_frame &a = frames[i];
-        if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_feature_track: slot out of range");
-        if ((size_t)a.slot >= taken.size()) taken.resize(a.slot + 1, 0);
-        if (taken[a.slot]) return fail(h, PVIO_B200_EINVAL, "batch_feature_track: a slot appears twice");
-        taken[a.slot] = 1;
+        TRY(take_slot(h, taken, a.slot, "batch_feature_track"));
         if (a.width < kKltMinFrame || a.height < kKltMinFrame || a.stride < a.width || !a.frame_id || !a.image ||
             a.map_frames < 0 || (outputs && (!a.keypoints || !a.prev_index || !a.n_keypoints)))
             return fail(h, PVIO_B200_EINVAL, "batch_feature_track: bad shape, stride, frame id, pixels or outputs");
@@ -310,26 +305,25 @@ int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBat
     size_t sort_bytes = 0;
     TRY(detect_sort_bytes(h, n, n_keys, sort_bytes));
 
-    // staging (both sides): upload 1 [0, o_fm) | upload 2 [o_fm, o_head) | download [o_head, o)
-    size_t o = 0;
-    const size_t o_seq = o;  o = align256(o + sizeof(FtSeq) * n);
-    const size_t o_fm = o;   o = align256(o + sizeof(FtFm) * n);
-    const size_t o_det = o;  o = align256(o + sizeof(DetectBatchFrame) * n);
-    const size_t o_cnt = o;  o = align256(o + sizeof(int) * 2 * n);
-    const size_t o_head = o; o = align256(o + sizeof(int) * 8 * n);
-    const size_t o_out = o;  o += out_bytes;
-    // device scratch: presets | thinning areas | responses | keys | sorted keys | select areas | sort temporaries | results
-    size_t c = 0;
-    const size_t c_pre = c;    c = align256(c + sizeof(double2) * n_pre);
-    const size_t c_thin = c;   c += thin_work;
-    const size_t c_resp = c;   c += resp_bytes;
-    const size_t c_keys = c;   c = align256(c + sizeof(unsigned long long) * n_keys);
-    const size_t c_sorted = c; c = align256(c + sizeof(unsigned long long) * n_keys);
-    const size_t c_work = c;   c += det_work;
-    const size_t c_sort = c;   c = align256(c + sort_bytes);
-    const size_t c_res = c;    c = align256(c + sizeof(DetectResult) * n);
-    TRY(reserve(h, B.fstage, o, kBoth));
-    TRY(reserve(h, B.fscratch, c, kDevice));
+    // staging: sequences (uploaded first) | F-RANSAC outcomes, detector descriptors, counters (uploaded after the replay) |
+    // heads, outputs (downloaded); device scratch: presets | thinning areas | responses | keys | sorted keys | select
+    // areas | sort temporaries | results
+    Stage stage(B.fstage, &B.fscratch);
+    const auto sSeq = stage.add<FtSeq>(Stage::kUp, n);
+    const auto sFm = stage.add<FtFm>(Stage::kUp, n);
+    const auto sDet = stage.add<DetectBatchFrame>(Stage::kUp, n);
+    const auto sCnt = stage.add<int>(Stage::kUp, 2 * n);
+    const auto sHead = stage.add<int>(Stage::kDown, 8 * n);
+    const auto sOut = stage.add<uint8_t>(Stage::kDown, out_bytes);
+    const auto sPre = stage.add<double2>(Stage::kScratch, n_pre);
+    const auto sThin = stage.add<uint8_t>(Stage::kScratch, thin_work);
+    const auto sResp = stage.add<uint8_t>(Stage::kScratch, resp_bytes);
+    const auto sKeys = stage.add<unsigned long long>(Stage::kScratch, n_keys);
+    const auto sSorted = stage.add<unsigned long long>(Stage::kScratch, n_keys);
+    const auto sWork = stage.add<uint8_t>(Stage::kScratch, det_work);
+    const auto sSort = stage.add<uint8_t>(Stage::kScratch, sort_bytes);
+    const auto sRes = stage.add<DetectResult>(Stage::kScratch, n);
+    TRY(stage.place(h));
     // each slot's other buffer holds this frame's keypoints
     for (int i = 0; i < n; ++i) {
         SlotKeypoints &K = B.kps[frames[i].slot];
@@ -342,8 +336,7 @@ int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBat
         }
     }
 
-    uint8_t *hs = B.fstage.h, *ds = B.fstage.d, *dc = B.fscratch.d;
-    FtSeq *seq = reinterpret_cast<FtSeq *>(hs + o_seq);
+    FtSeq *seq = stage.host(sSeq);
     size_t pre = 0, dwork = 0;                // pre: the call's points
     for (int i = 0; i < n; ++i) {
         const pvio_b200_feature_frame &a = frames[i];
@@ -357,11 +350,11 @@ int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBat
         S.z_next = K.z(nb);
         S.birth_next = K.birth(nb);
         S.prev_next = K.prev(nb);
-        S.pre = reinterpret_cast<double2 *>(dc + c_pre) + pre;
-        S.out_z = reinterpret_cast<double2 *>(ds + o_out + P.out_off);
-        S.out_prev = reinterpret_cast<int *>(ds + o_out + P.out_off + sizeof(double2) * P.out_cap);
-        S.head = reinterpret_cast<int *>(ds + o_head) + 8 * i;
-        S.work = P.work > thin_smem ? dc + c_thin + P.work_off : nullptr;
+        S.pre = stage.dev(sPre) + pre;
+        S.out_z = reinterpret_cast<double2 *>(stage.dev(sOut) + P.out_off);
+        S.out_prev = reinterpret_cast<int *>(stage.dev(sOut) + P.out_off + sizeof(double2) * P.out_cap);
+        S.head = stage.dev(sHead) + 8 * i;
+        S.work = P.work > thin_smem ? stage.dev(sThin) + P.work_off : nullptr;
         S.kp[0] = K.fx; S.kp[1] = K.fy; S.kp[2] = K.cx; S.kp[3] = K.cy;
         S.kn[0] = a.fx; S.kn[1] = a.fy; S.kn[2] = a.cx; S.kn[3] = a.cy;
         S.use_q = a.predict_q != nullptr;
@@ -376,10 +369,10 @@ int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBat
     }
 
     cudaStream_t st = h->stream;
-    const FtSeq *d_seq = reinterpret_cast<const FtSeq *>(ds + o_seq);
-    CK(h, cudaMemcpyAsync(ds + o_seq, hs + o_seq, o_fm - o_seq, cudaMemcpyHostToDevice, st));
+    const FtSeq *d_seq = stage.dev(sSeq);
+    TRY(stage.upload(h, sSeq));
     if (pred) {
-        ft_predict_kernel<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<FtSeq *>(ds + o_seq), n, *pred);
+        ft_predict_kernel<<<(n + 127) / 128, 128, 0, st>>>(stage.dev(sSeq), n, *pred);
         ++h->launches;
         CK(h, cudaGetLastError());
     }
@@ -393,9 +386,9 @@ int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBat
     TRY(klt_batch_track(h, n, items.data(), opt, &dev, r));
 
     // after the replay: each sequence's F-RANSAC outcome and detector descriptor, on the frame just cached
-    FtFm *fm = reinterpret_cast<FtFm *>(hs + o_fm);
-    DetectBatchFrame *det = reinterpret_cast<DetectBatchFrame *>(hs + o_det);
-    memset(hs + o_cnt, 0, sizeof(int) * 2 * n);
+    FtFm *fm = stage.host(sFm);
+    DetectBatchFrame *det = stage.host(sDet);
+    memset(stage.host(sCnt), 0, sizeof(int) * 2 * n);
     dwork = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_feature_frame &a = frames[i];
@@ -408,38 +401,37 @@ int ft_run(Handle *h, int n, const pvio_b200_feature_frame *frames, const KltBat
         DetectBatchFrame &F = det[i];
         memset(&F, 0, sizeof(F));
         F.img = img;
-        F.resp = reinterpret_cast<float *>(dc + c_resp + P.resp_off);
-        F.keys = reinterpret_cast<unsigned long long *>(dc + c_keys) + P.key_off;
-        F.sorted = reinterpret_cast<unsigned long long *>(dc + c_sorted) + P.key_off;
-        F.counters = reinterpret_cast<int *>(ds + o_cnt) + 2 * i;
+        F.resp = reinterpret_cast<float *>(stage.dev(sResp) + P.resp_off);
+        F.keys = stage.dev(sKeys) + P.key_off;
+        F.sorted = stage.dev(sSorted) + P.key_off;
+        F.counters = stage.dev(sCnt) + 2 * i;
         F.pre = seq[i].pre;
         F.pre_count = seq[i].head + 5;
-        F.work = P.det.work > det_smem ? dc + c_work + dwork : nullptr;
+        F.work = P.det.work > det_smem ? stage.dev(sWork) + dwork : nullptr;
         if (P.det.work > det_smem) dwork += P.det.work;
-        F.res = reinterpret_cast<DetectResult *>(dc + c_res) + i;
+        F.res = stage.dev(sRes) + i;
         detect_apply_plan(P.det, a.width, a.height, keypoint_distance, F);
         F.key_off = P.key_off;
     }
-    CK(h, cudaMemcpyAsync(ds + o_fm, hs + o_fm, o_head - o_fm, cudaMemcpyHostToDevice, st));
+    TRY(stage.upload(h, sFm, sCnt));
     if (thin_smem > 48 * 1024)
         CK(h, cudaFuncSetAttribute(ft_thin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)thin_smem));
-    ft_thin_kernel<<<n, kThinThreads, thin_smem, st>>>(d_seq, reinterpret_cast<const FtFm *>(ds + o_fm), r.next, r.status);
+    ft_thin_kernel<<<n, kThinThreads, thin_smem, st>>>(d_seq, stage.dev(sFm), r.next, r.status);
     ++h->launches;
-    TRY(detect_run(h, reinterpret_cast<const DetectBatchFrame *>(ds + o_det), n, max_w, max_h,
-                   reinterpret_cast<const unsigned long long *>(dc + c_keys), reinterpret_cast<unsigned long long *>(dc + c_sorted),
-                   n_keys, dc + c_sort, sort_bytes, det_smem));
-    ft_commit_kernel<<<n, 32, 0, st>>>(d_seq, reinterpret_cast<const DetectResult *>(dc + c_res));
+    TRY(detect_run(h, stage.dev(sDet), n, max_w, max_h, stage.dev(sKeys), stage.dev(sSorted), n_keys, stage.dev(sSort),
+                   sort_bytes, det_smem));
+    ft_commit_kernel<<<n, 32, 0, st>>>(d_seq, stage.dev(sRes));
     ++h->launches;
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(hs + o_head, ds + o_head, o - o_head, cudaMemcpyDeviceToHost, st));
+    TRY(stage.download(h));
     CK(h, cudaStreamSynchronize(st));
     run.count.resize(n);
     run.out_off.resize(n);
     run.prev_no.resize(n);
-    run.head = hs + o_head;
-    run.out = hs + o_out;
+    run.head = reinterpret_cast<const uint8_t *>(stage.host(sHead));
+    run.out = stage.host(sOut);
     for (int i = 0; i < n; ++i) {
-        run.count[i] = reinterpret_cast<const int *>(hs + o_head)[8 * i];
+        run.count[i] = stage.host(sHead)[8 * i];
         run.out_off[i] = plan[i].out_off;
         run.prev_no[i] = seq[i].prev_no;
     }

@@ -391,28 +391,6 @@ __global__ void __launch_bounds__(32) fm_schedule_kernel(const FmBatchProblem *p
     P.surv[0] = s; P.surv[1] = have;
 }
 
-// the single call's staging (FmState::stage, both sides), followed by the matches p[n], q[n] (float2) and the schedule
-// [iterations][7]; the mask job is written after the replay and read in place
-struct FmStage {
-    FmBatchProblem prob;
-    FmMaskJob job;
-    int surv[2];                              // matches, iterations that have a subset
-};
-static_assert(sizeof(FmStage) % sizeof(float2) == 0, "the matches follow the record");
-
-// room for n points and s iterations: at least 1024 points and 1000 iterations, grown on demand
-int fm_reserve(Handle *h, int n, int s) {
-    FmState &f = h->fm;
-    const size_t cn = std::max(n, 1024), cs = std::max(s, 1000), cw = (cn + 31) / 32;
-    TRY(reserve(h, f.stage, sizeof(FmStage) + sizeof(float2) * 2 * cn + sizeof(int) * 7 * cs, kBoth));
-    TRY(reserve(h, f.counts, 4 * cs, kBoth));
-    TRY(reserve(h, f.F, 27 * cs, kDevice));
-    TRY(reserve(h, f.masks, 3 * cs * cw, kDevice));
-    TRY(reserve(h, f.h_F, 9, kPinned));
-    TRY(reserve(h, f.h_mask, cw, kPinned));
-    return 0;
-}
-
 }  // namespace
 
 // host-only: the subsets OpenCV would draw (exported as pvio_b200_fm_sample_schedule)
@@ -487,17 +465,30 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
     fm_options(threshold, confidence, max_iters);
     const bool seven = n == 7, ransac = n >= 15;
     const int budget = seven ? 1 : ransac ? max_iters : fm_lmeds_iters(confidence, max_iters);
-    TRY(fm_reserve(h, n, budget));
-    FmState &f = h->fm;
-    FmStage &S = *reinterpret_cast<FmStage *>(f.stage.h);
-    FmStage *dS = reinterpret_cast<FmStage *>(f.stage.d);
-    float *hp = reinterpret_cast<float *>(&S + 1);
-    int *sched = reinterpret_cast<int *>(hp + 4 * n);
+    // staging: the problem, its survivor and iteration counts, the matches p[n], q[n] and the schedule [budget][7]
+    // (uploaded) | counts [budget][4], the winning model and its mask (downloaded) | the mask job, written after the replay
+    // and read in place; device scratch: the models [budget][3][9] and masks [budget][3][words] of every iteration
+    const int nw = (n + 31) / 32;
+    Stage S(h->fm.stage, &h->fm.scratch);
+    S.pow2 = true;
+    const auto prob = S.add<FmBatchProblem>(Stage::kUp, 1);
+    const auto surv = S.add<int>(Stage::kUp, 2);
+    const auto pq = S.add<float2>(Stage::kUp, 2 * (size_t)n);
+    const auto sched = S.add<int>(Stage::kUp, 7 * (size_t)budget);
+    const auto counts = S.add<int>(Stage::kDown, 4 * (size_t)budget);
+    const auto win_F = S.add<double>(Stage::kDown, 9);
+    const auto win_mask = S.add<unsigned>(Stage::kDown, nw);
+    const auto job = S.add<FmMaskJob>(Stage::kMapped, 1);
+    const auto F = S.add<double>(Stage::kScratch, 27 * (size_t)budget);
+    const auto masks = S.add<unsigned>(Stage::kScratch, 3 * (size_t)budget * nw);
+    TRY(S.place(h));
+    float *hp = reinterpret_cast<float *>(S.host(pq));
+    int *hs = S.host(sched);
     std::memcpy(hp, p, sizeof(float) * 2 * n);
     std::memcpy(hp + 2 * n, q, sizeof(float) * 2 * n);
     int have = budget;                        // iterations that have a subset
     if (seven) {
-        for (int i = 0; i < 7; ++i) sched[i] = i;
+        for (int i = 0; i < 7; ++i) hs[i] = i;
     } else if (schedule) {
         if (n_schedule < 1) return fail(h, PVIO_B200_EINVAL, "find_fundamental_mask: empty schedule");
         have = std::min(budget, n_schedule);
@@ -506,11 +497,11 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
             for (int i = 0; i < 7; ++i) {
                 const int v = schedule[7 * it + i];
                 if (v < 0 || v >= n) return fail(h, PVIO_B200_EINVAL, "find_fundamental_mask: schedule index out of range");
-                sched[7 * it + i] = v;
+                hs[7 * it + i] = v;
             }
         }
     } else {
-        have = cv_schedule(p, q, n, budget, ransac ? 10000 : 1000, sched);
+        have = cv_schedule(p, q, n, budget, ransac ? 10000 : 1000, hs);
     }
     if (have == 0) {                          // getSubset failed at iteration 0: run() returns false, the mask stays as created
         std::memset(mask, 0, n);
@@ -520,41 +511,42 @@ int fm_ransac_impl(Handle *h, int n, const float *p, const float *q, double thre
     // branch for n == 7 too (the call draws no schedule then); the replay of n == 7 reads counts[0] only, which both
     // branches write alike, and its mask is all ones.
     cudaStream_t st = h->stream;
-    const int nw = (n + 31) / 32;
-    float2 *dp = reinterpret_cast<float2 *>(dS + 1), *dq = dp + n;
-    S.prob = FmBatchProblem{nullptr, nullptr, nullptr, dp, dq, reinterpret_cast<int *>(dq + n), f.counts.d, f.F.d, f.masks.d, dS->surv, n, have};
-    S.surv[0] = n; S.surv[1] = have;
-    CK(h, cudaMemcpyAsync(dS, &S, sizeof(FmStage) + sizeof(float2) * 2 * n + sizeof(int) * 7 * have, cudaMemcpyHostToDevice, st));
-    fm_hypotheses_kernel<<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>((float)(threshold * threshold), &dS->prob);
+    float2 *dp = S.dev(pq), *dq = dp + n;
+    *S.host(prob) = FmBatchProblem{nullptr, nullptr, nullptr, dp, dq, S.dev(sched), S.dev(counts), S.dev(F), S.dev(masks),
+                                   S.dev(surv), n, have};
+    S.host(surv)[0] = n; S.host(surv)[1] = have;
+    TRY(S.upload(h));
+    fm_hypotheses_kernel<<<(have + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, st>>>((float)(threshold * threshold), S.dev(prob));
     h->launches++;
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(f.counts.h, f.counts.d, sizeof(int) * 4 * have, cudaMemcpyDeviceToHost, st));
+    TRY(S.download(h, counts, counts));
     CK(h, cudaStreamSynchronize(st));
 
-    const float thr_lmeds = fm_replay(f.counts.h, n, have, max_iters, confidence, inf);
+    const float thr_lmeds = fm_replay(S.host(counts), n, have, max_iters, confidence, inf);
     const int best_it = inf[1], best_k = inf[2];
     if (seven) std::memset(mask, 1, n);       // fundam.cpp: the mask of the 7-point / 8-point call is all ones
     if (best_it < 0) {
         if (!seven) std::memset(mask, 0, n);
         return finish(0);
     }
+    const double *best_F = S.dev(F) + (size_t)(3 * best_it + best_k) * 9;
     if (!ransac && !seven) {
-        S.job = FmMaskJob{dp, dq, f.F.d + (size_t)(3 * best_it + best_k) * 9, nullptr, f.masks.d, thr_lmeds, n};
+        *S.host(job) = FmMaskJob{dp, dq, best_F, nullptr, S.dev(masks), thr_lmeds, n};
         FmMaskJob *d_job = nullptr;           // read in place from the pinned staging (mapped: unified addressing)
-        CK(h, cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_job), &S.job, 0));
+        CK(h, cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_job), S.host(job), 0));
         fm_mask_kernel<<<nw, 32, 0, st>>>(d_job);
         h->launches++;
         CK(h, cudaGetLastError());
     }
-    CK(h, cudaMemcpyAsync(f.h_F.h, f.F.d + (size_t)(3 * best_it + best_k) * 9, sizeof(double) * 9, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(S.host(win_F), best_F, sizeof(double) * 9, cudaMemcpyDeviceToHost, st));
     if (!seven) {
-        const unsigned *src = ransac ? f.masks.d + (size_t)(3 * best_it + best_k) * nw : f.masks.d;
-        CK(h, cudaMemcpyAsync(f.h_mask.h, src, sizeof(unsigned) * nw, cudaMemcpyDeviceToHost, st));
+        const unsigned *src = ransac ? S.dev(masks) + (size_t)(3 * best_it + best_k) * nw : S.dev(masks);
+        CK(h, cudaMemcpyAsync(S.host(win_mask), src, sizeof(unsigned) * nw, cudaMemcpyDeviceToHost, st));
     }
     CK(h, cudaStreamSynchronize(st));
     if (!seven)
-        for (int i = 0; i < n; ++i) mask[i] = (f.h_mask.h[i >> 5] >> (i & 31)) & 1u;
-    if (F_out) std::memcpy(F_out, f.h_F.h, 9 * sizeof(double));
+        for (int i = 0; i < n; ++i) mask[i] = (S.host(win_mask)[i >> 5] >> (i & 31)) & 1u;
+    if (F_out) std::memcpy(F_out, S.host(win_F), 9 * sizeof(double));
     return finish(0);
 }
 

@@ -264,8 +264,6 @@ __global__ void imu_stream_reset_kernel(int n, const int32_t *slots, const ImuSt
     if (i < n) hdr[slots[i]] = src[i];
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // device queues for `slots` slots of at least `qcap` rows each; growth keeps every slot's queues and header
 int ensure_streams(Handle *h, int slots, int qcap) {
     ImuStreams &M = h->imus;
@@ -308,20 +306,18 @@ int stream_reset_impl(Handle *h, int n, const int32_t *slots, const double *oq, 
     int top = 0;
     for (int i = 0; i < n; ++i) {
         const int s = slots[i];
-        if (s < 0 || s > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: slot out of range");
-        if ((size_t)s >= taken.size()) taken.resize(s + 1, 0);
-        if (taken[s]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: a slot appears twice");
-        taken[s] = 1;
+        TRY(take_slot(h, taken, s, "batch_imu_stream_reset"));
         if (!finite_all(oq + 4 * i, 4) || !finite_all(op + 3 * i, 3))
             return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_reset: an extrinsic value is not finite");
         top = std::max(top, s + 1);
     }
     ImuStreams &M = h->imus;
     TRY(ensure_streams(h, top, kMinQcap));
-    const size_t o_hdr = align256(sizeof(int32_t) * n);
-    TRY(reserve(h, M.stage, o_hdr + sizeof(ImuStreamSlot) * n, kBoth));
-    memcpy(M.stage.h, slots, sizeof(int32_t) * n);
-    ImuStreamSlot *hs = reinterpret_cast<ImuStreamSlot *>(M.stage.h + o_hdr);
+    Stage S(M.stage);
+    const auto sl = S.add(Stage::kUp, n, slots);
+    const auto hdr = S.add<ImuStreamSlot>(Stage::kUp, n);
+    TRY(S.place(h));
+    ImuStreamSlot *hs = S.host(hdr);
     for (int i = 0; i < n; ++i) {
         ImuStreamSlot z{};
         for (int j = 0; j < 4; ++j) z.q_ob[j] = oq[4 * i + j];
@@ -329,10 +325,8 @@ int stream_reset_impl(Handle *h, int n, const int32_t *slots, const double *oq, 
         hs[i] = z;
     }
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(M.stage.d, M.stage.h, o_hdr + sizeof(ImuStreamSlot) * n, cudaMemcpyHostToDevice, st));
-    imu_stream_reset_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, reinterpret_cast<const int32_t *>(M.stage.d),
-                                                             reinterpret_cast<const ImuStreamSlot *>(M.stage.d + o_hdr),
-                                                             reinterpret_cast<ImuStreamSlot *>(M.hdr.d));
+    TRY(S.upload(h));
+    imu_stream_reset_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, S.dev(sl), S.dev(hdr), reinterpret_cast<ImuStreamSlot *>(M.hdr.d));
     ++h->launches;
     CK(h, cudaGetLastError());
     CK(h, cudaStreamSynchronize(st));
@@ -360,10 +354,7 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
     int64_t total_ev = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_imu_stream_record &r = recs[i];
-        if (r.slot < 0 || r.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: slot out of range");
-        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
-        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: a slot appears twice");
-        taken[r.slot] = 1;
+        TRY(take_slot(h, taken, r.slot, "batch_imu_stream"));
         if ((size_t)r.slot >= M.host.size() || !M.host[r.slot].set)
             return fail(h, PVIO_B200_EINVAL, "batch_imu_stream: the slot was never reset");
         const ImuStreamHost &S = M.host[r.slot];
@@ -421,19 +412,17 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
     TRY(ensure_streams(h, M.slots, (int)qcap));
 
     // staging: records | events (uploaded) || outputs | poses | frame times | rows | frame row counts (downloaded)
-    size_t o = 0;
-    const size_t o_rec = o; o = align256(o + sizeof(ImuStreamRec) * n);
-    const size_t o_ev = o; o = align256(o + sizeof(double) * 5 * total_ev);
-    const size_t up = o;
-    const size_t o_out = o; o = align256(o + sizeof(ImuStreamOut) * n);
-    const size_t o_pose = o; o += sizeof(double) * 7 * total_ev;
-    const size_t o_ft = o; o += sizeof(double) * total_f;
-    const size_t o_rows = o; o += sizeof(double) * 7 * total_r;
-    const size_t o_fr = o; o += sizeof(int32_t) * total_f;
-    TRY(reserve(h, M.stage, o, kBoth));
-    uint8_t *hs = M.stage.h, *ds = M.stage.d;
-    ImuStreamRec *hr = reinterpret_cast<ImuStreamRec *>(hs + o_rec);
-    double *hev = reinterpret_cast<double *>(hs + o_ev);
+    Stage stage(M.stage);
+    const auto rec = stage.add<ImuStreamRec>(Stage::kUp, n);
+    const auto evs = stage.add<double>(Stage::kUp, 5 * total_ev);
+    const auto out = stage.add<ImuStreamOut>(Stage::kDown, n);
+    const auto pose = stage.add<double>(Stage::kDown, 7 * total_ev);
+    const auto ft = stage.add<double>(Stage::kDown, total_f);
+    const auto rws = stage.add<double>(Stage::kDown, 7 * total_r);
+    const auto frw = stage.add<int32_t>(Stage::kDown, total_f);
+    TRY(stage.place(h));
+    ImuStreamRec *hr = stage.host(rec);
+    double *hev = stage.host(evs);
     int64_t ev = 0, fr = 0, row = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_imu_stream_record &r = recs[i];
@@ -453,26 +442,26 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
     A.hdr = reinterpret_cast<ImuStreamSlot *>(M.hdr.d);
     A.g = M.g.d; A.a = M.a.d; A.s = M.s.d; A.f = M.f.d; A.k = M.k.d;
     A.qcap = M.qcap;
-    A.recs = reinterpret_cast<const ImuStreamRec *>(ds + o_rec);
-    A.events = reinterpret_cast<const double *>(ds + o_ev);
-    A.outs = reinterpret_cast<ImuStreamOut *>(ds + o_out);
-    A.poses = reinterpret_cast<double *>(ds + o_pose);
-    A.frame_t = reinterpret_cast<double *>(ds + o_ft);
-    A.rows = reinterpret_cast<double *>(ds + o_rows);
-    A.frame_rows = reinterpret_cast<int32_t *>(ds + o_fr);
+    A.recs = stage.dev(rec);
+    A.events = stage.dev(evs);
+    A.outs = stage.dev(out);
+    A.poses = stage.dev(pose);
+    A.frame_t = stage.dev(ft);
+    A.rows = stage.dev(rws);
+    A.frame_rows = stage.dev(frw);
     A.n = n;
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(ds, hs, up, cudaMemcpyHostToDevice, st));
+    TRY(stage.upload(h));
     imu_stream_kernel<<<(n + 127) / 128, 128, 0, st>>>(A);
     ++h->launches;
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(hs + up, ds + up, o - up, cudaMemcpyDeviceToHost, st));
+    TRY(stage.download(h));
     CK(h, cudaStreamSynchronize(st));
 
     // Internal invariant: the host bounds (need_frames / need_rows) hold every release, so overflow is never set.  Were
     // it set, the kernel would already have changed the call's slots without the host's record of them following, so
     // every slot of the call is marked unset: later calls on them are rejected until they are reset.
-    const ImuStreamOut *outs = reinterpret_cast<const ImuStreamOut *>(hs + o_out);
+    const ImuStreamOut *outs = stage.host(out);
     for (int i = 0; i < n; ++i)
         if (outs[i].overflow) {
             for (int j = 0; j < n; ++j) M.host[recs[j].slot].set = false;
@@ -483,13 +472,13 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
         pvio_b200_imu_stream_record &r = recs[i];
         const ImuStreamRec &R = hr[i];
         const ImuStreamOut &O = outs[i];
-        memcpy(r.poses, hs + o_pose + sizeof(double) * 7 * R.pose, sizeof(double) * 7 * O.n_consumed);
-        const double *ft = reinterpret_cast<const double *>(hs + o_ft) + R.frame;
+        memcpy(r.poses, stage.host(pose) + 7 * R.pose, sizeof(double) * 7 * O.n_consumed);
+        const double *ftr = stage.host(ft) + R.frame;
         if (O.n_frames) {
-            memcpy(r.frame_t, ft, sizeof(double) * O.n_frames);
-            memcpy(r.frame_rows, reinterpret_cast<const int32_t *>(hs + o_fr) + R.frame, sizeof(int32_t) * O.n_frames);
+            memcpy(r.frame_t, ftr, sizeof(double) * O.n_frames);
+            memcpy(r.frame_rows, stage.host(frw) + R.frame, sizeof(int32_t) * O.n_frames);
         }
-        if (O.n_rows) memcpy(r.rows, hs + o_rows + sizeof(double) * 7 * R.row, sizeof(double) * 7 * O.n_rows);
+        if (O.n_rows) memcpy(r.rows, stage.host(rws) + 7 * R.row, sizeof(double) * 7 * O.n_rows);
         r.n_consumed = O.n_consumed;
         r.n_frames = O.n_frames;
         r.need_frames = (int32_t)need[i].frames;
@@ -504,7 +493,7 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
         }
         if (!S.has_state)
             for (int k = 0; k < O.n_frames; ++k) {
-                S.t_drop = S.dropped ? std::max(S.t_drop, ft[k]) : ft[k];
+                S.t_drop = S.dropped ? std::max(S.t_drop, ftr[k]) : ftr[k];
                 S.dropped = true;
             }
         S.g = O.g; S.a = O.a; S.s = O.s; S.f = O.f; S.k = O.k;
@@ -620,14 +609,14 @@ __global__ void __launch_bounds__(kSnapThreads) imu_stream_unpack_kernel(StreamS
     }
 }
 
-StreamSnapArgs snap_args(Handle *h, const uint8_t *stage_d, size_t o_area) {
+StreamSnapArgs snap_args(Handle *h, const StreamSnapRec *recs, uint8_t *area) {
     ImuStreams &M = h->imus;
     StreamSnapArgs A;
     A.hdr = reinterpret_cast<ImuStreamSlot *>(M.hdr.d);
     A.q[0] = M.g.d; A.q[1] = M.a.d; A.q[2] = M.s.d; A.q[3] = M.f.d; A.q[4] = M.k.d;
     A.qcap = M.qcap;
-    A.recs = reinterpret_cast<const StreamSnapRec *>(stage_d);
-    A.area = const_cast<uint8_t *>(stage_d) + o_area;
+    A.recs = recs;
+    A.area = area;
     return A;
 }
 
@@ -641,10 +630,7 @@ int stream_save_impl(Handle *h, int n, pvio_b200_imu_stream_snapshot *recs) {
     int packed = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_imu_stream_snapshot &r = recs[i];
-        if (r.slot < 0 || r.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: slot out of range");
-        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
-        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: a slot appears twice");
-        taken[r.slot] = 1;
+        TRY(take_slot(h, taken, r.slot, "batch_imu_stream_save"));
         if ((size_t)r.slot >= M.host.size() || !M.host[r.slot].set)
             return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_save: the slot was never reset");
         const ImuStreamHost &S = M.host[r.slot];
@@ -658,23 +644,25 @@ int stream_save_impl(Handle *h, int n, pvio_b200_imu_stream_snapshot *recs) {
     }
     if (packed) {
         // staging: records (uploaded) | blobs (downloaded)
-        const size_t o_area = align256(sizeof(StreamSnapRec) * packed);
-        TRY(reserve(h, M.stage, o_area + area, kBoth));
-        StreamSnapRec *hr = reinterpret_cast<StreamSnapRec *>(M.stage.h);
+        Stage stage(M.stage);
+        const auto rc = stage.add<StreamSnapRec>(Stage::kUp, packed);
+        const auto blobs = stage.add<uint8_t>(Stage::kDown, area);
+        TRY(stage.place(h));
+        StreamSnapRec *hr = stage.host(rc);
         for (int i = 0, j = 0; i < n; ++i)
             if (at[i] >= 0) hr[j++] = StreamSnapRec{recs[i].slot, 0, at[i]};
         cudaStream_t st = h->stream;
-        CK(h, cudaMemcpyAsync(M.stage.d, M.stage.h, sizeof(StreamSnapRec) * packed, cudaMemcpyHostToDevice, st));
-        imu_stream_pack_kernel<<<packed, kSnapThreads, 0, st>>>(snap_args(h, M.stage.d, o_area));
+        TRY(stage.upload(h));
+        imu_stream_pack_kernel<<<packed, kSnapThreads, 0, st>>>(snap_args(h, stage.dev(rc), stage.dev(blobs)));
         ++h->launches;
         CK(h, cudaGetLastError());
-        CK(h, cudaMemcpyAsync(M.stage.h + o_area, M.stage.d + o_area, area, cudaMemcpyDeviceToHost, st));
+        TRY(stage.download(h));
         CK(h, cudaStreamSynchronize(st));
         for (int i = 0; i < n; ++i) {
             if (at[i] < 0) continue;
             const ImuStreamHost &S = M.host[recs[i].slot];
             uint8_t *out = recs[i].data;
-            memcpy(out, M.stage.h + o_area + at[i], size[i]);
+            memcpy(out, stage.host(blobs) + at[i], size[i]);
             StreamSnapHead H;
             memcpy(&H, out, sizeof(H));
             H.magic = PVIO_B200_IMU_STREAM_SNAPSHOT_MAGIC;
@@ -736,11 +724,7 @@ int stream_restore_impl(Handle *h, int n, const pvio_b200_imu_stream_snapshot *r
     int top = 0, qcap = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_imu_stream_snapshot &r = recs[i];
-        if (r.slot < 0 || r.slot > kMaxBatchSlot)
-            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_restore: slot out of range");
-        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
-        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_restore: a slot appears twice");
-        taken[r.slot] = 1;
+        TRY(take_slot(h, taken, r.slot, "batch_imu_stream_restore"));
         if (const char *why = stream_snap_check(r.data, r.capacity, heads[i]))
             return fail(h, PVIO_B200_EINVAL, (std::string("batch_imu_stream_restore: ") + why).c_str());
         top = std::max(top, r.slot + 1);
@@ -749,20 +733,22 @@ int stream_restore_impl(Handle *h, int n, const pvio_b200_imu_stream_snapshot *r
     TRY(ensure_streams(h, top, qcap));
 
     // staging: records | blobs, uploaded
-    const size_t o_area = align256(sizeof(StreamSnapRec) * n);
     size_t area = 0;
     for (int i = 0; i < n; ++i) area += align256(heads[i].size);
-    TRY(reserve(h, M.stage, o_area + area, kBoth));
-    StreamSnapRec *hr = reinterpret_cast<StreamSnapRec *>(M.stage.h);
+    Stage stage(M.stage);
+    const auto rc = stage.add<StreamSnapRec>(Stage::kUp, n);
+    const auto blobs = stage.add<uint8_t>(Stage::kUp, area);
+    TRY(stage.place(h));
+    StreamSnapRec *hr = stage.host(rc);
     size_t at = 0;
     for (int i = 0; i < n; ++i) {
         hr[i] = StreamSnapRec{recs[i].slot, 0, (int64_t)at};
-        memcpy(M.stage.h + o_area + at, recs[i].data, heads[i].size);
+        memcpy(stage.host(blobs) + at, recs[i].data, heads[i].size);
         at += align256(heads[i].size);
     }
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(M.stage.d, M.stage.h, o_area + area, cudaMemcpyHostToDevice, st));
-    imu_stream_unpack_kernel<<<n, kSnapThreads, 0, st>>>(snap_args(h, M.stage.d, o_area));
+    TRY(stage.upload(h));
+    imu_stream_unpack_kernel<<<n, kSnapThreads, 0, st>>>(snap_args(h, stage.dev(rc), stage.dev(blobs)));
     ++h->launches;
     CK(h, cudaGetLastError());
     CK(h, cudaStreamSynchronize(st));

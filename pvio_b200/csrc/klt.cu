@@ -345,10 +345,6 @@ static void klt_lookup(const KltPyramids &k, uint64_t prev_id, uint64_t next_id,
     slot[0] = sp; slot[1] = sn;
 }
 
-namespace {
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-}  // namespace
-
 // The pyramids of n_frames new frames (frames: host copies of the descriptors at d_frames): CLAHE into level 0, or
 // without CLAHE a device copy of the raw pixels into level 0 unless they were uploaded there; then one pyrDown launch per
 // level over every frame (grid z)
@@ -440,22 +436,20 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
         TRY(reserve(h, k.lut, (size_t)tiles_x * tiles_y * 256, kDevice));
     }
 
-    // staging (both sides): upload [0, o_err) | download [o_next, o)
-    size_t o = 0;
-    const size_t o_lv = o;   o = align256(o + sizeof(KltLevels));
-    const size_t o_frm = o;  o = align256(o + sizeof(KltBatchFrame) * 2);
-    const size_t o_pof = o;  o = align256(o + sizeof(int) * n);
-    const size_t o_prev = o; o = align256(o + sizeof(float) * 2 * n);
-    const size_t o_next = o; o = align256(o + sizeof(float) * 2 * n);          // guesses in, positions out
-    const size_t o_err = o;  o = align256(o + sizeof(float) * n);
-    const size_t o_st = o;   o += n;
-    TRY(reserve(h, k.stage, o, kBoth));
-    uint8_t *hs = k.stage.h, *ds = k.stage.d;
-    *reinterpret_cast<KltLevels *>(hs + o_lv) = klt_pair(k, slot);
-    memset(hs + o_pof, 0, sizeof(int) * n);
-    memcpy(hs + o_prev, prev_pts, sizeof(float) * 2 * n);
-    memcpy(hs + o_next, next_pts, sizeof(float) * 2 * n);
-    KltBatchFrame *frm = reinterpret_cast<KltBatchFrame *>(hs + o_frm);
+    // staging: pair descriptor, frame descriptors, pair indices, points (uploaded) | initial guesses in, positions out |
+    // errors, status (downloaded)
+    Stage S(k.stage);
+    const auto lv = S.add<KltLevels>(Stage::kUp, 1);
+    const auto fr = S.add<KltBatchFrame>(Stage::kUp, 2);
+    const auto pof = S.add<int>(Stage::kUp, n);
+    const auto pp = S.add(Stage::kUp, 2 * n, prev_pts);
+    const auto np = S.add(Stage::kInOut, 2 * n, next_pts);
+    const auto er = S.add<float>(Stage::kDown, n);
+    const auto stat = S.add<uint8_t>(Stage::kDown, n);
+    TRY(S.place(h));
+    *S.host(lv) = klt_pair(k, slot);
+    memset(S.host(pof), 0, sizeof(int) * n);
+    KltBatchFrame *frm = S.host(fr);
     const uint8_t *src[2] = {prev, next};
     int nf = 0;
     for (int i = 0; i < 2; ++i) {
@@ -466,24 +460,21 @@ int klt_track_impl(Handle *h, const uint8_t *prev, const uint8_t *next, int widt
         frm[nf++] = klt_frame(k, slot[i], dst, k.lut.d, clahe_clip, tiles_x, tiles_y);
         CK(h, cudaMemcpyAsync(dst, img, img_bytes, cudaMemcpyHostToDevice, h->stream));
     }
-    CK(h, cudaMemcpyAsync(ds, hs, o_err, cudaMemcpyHostToDevice, h->stream));
-    const KltBatchFrame *d_frm = reinterpret_cast<const KltBatchFrame *>(ds + o_frm);
-    for (int j = 0; j < nf; ++j) TRY(klt_build_pyramids(h, frm + j, d_frm + j, 1, do_clahe, tiles_x, tiles_y));
+    TRY(S.upload(h));
+    for (int j = 0; j < nf; ++j) TRY(klt_build_pyramids(h, frm + j, S.dev(fr) + j, 1, do_clahe, tiles_x, tiles_y));
     k.pyr_id[sp] = prev_id; k.pyr_clahe[sp] = clahe_clip;
     k.pyr_id[sn] = next_id; k.pyr_clahe[sn] = clahe_clip;
-    klt_lk(h, reinterpret_cast<const KltLevels *>(ds + o_lv), reinterpret_cast<const int *>(ds + o_pof),
-           reinterpret_cast<const float *>(ds + o_prev), reinterpret_cast<float *>(ds + o_next), ds + o_st,
-           reinterpret_cast<float *>(ds + o_err), n, max_iter, eps, border);
-    CK(h, cudaMemcpyAsync(hs + o_next, ds + o_next, o - o_next, cudaMemcpyDeviceToHost, h->stream));
+    klt_lk(h, S.dev(lv), S.dev(pof), S.dev(pp), S.dev(np), S.dev(stat), S.dev(er), n, max_iter, eps, border);
+    TRY(S.download(h));
     if (do_clahe && (prev_eq || next_eq)) {
         CK(h, cudaMemcpyAsync(k.img.h, k.pyr[sp].d, img_bytes, cudaMemcpyDeviceToHost, h->stream));
         CK(h, cudaMemcpyAsync(k.img.h + img_bytes, k.pyr[sn].d, img_bytes, cudaMemcpyDeviceToHost, h->stream));
     }
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
-    memcpy(next_pts, hs + o_next, sizeof(float) * 2 * n);
-    if (err) memcpy(err, hs + o_err, sizeof(float) * n);
-    memcpy(status, hs + o_st, n);
+    memcpy(next_pts, S.host(np), sizeof(float) * 2 * n);
+    if (err) memcpy(err, S.host(er), sizeof(float) * n);
+    memcpy(status, S.host(stat), n);
     if (do_clahe && prev_eq) memcpy(prev_eq, k.img.h, img_bytes);
     if (do_clahe && next_eq) memcpy(next_eq, k.img.h + img_bytes, img_bytes);
     return 0;
@@ -535,14 +526,12 @@ int batch_track_impl(Handle *h, int n, const pvio_b200_klt_pair *pairs, int max_
         any_job |= r.mask[i] != nullptr;
     }
     if (any_job) {
-        KltBatchState &B = h->kltb;
-        unsigned *h_mw = reinterpret_cast<unsigned *>(B.stage.h + r.o_mw);
-        CK(h, cudaMemcpyAsync(h_mw, B.stage.d + r.o_mw, sizeof(unsigned) * r.words, cudaMemcpyDeviceToHost, h->stream));
+        CK(h, cudaMemcpyAsync(r.mw, r.d_mw, sizeof(unsigned) * r.words, cudaMemcpyDeviceToHost, h->stream));
         CK(h, cudaStreamSynchronize(h->stream));
         for (int i = 0; i < n; ++i) {
             const pvio_b200_klt_pair &a = pairs[i];
             if (!r.mask[i]) continue;
-            const unsigned *m = h_mw + (r.mask[i] - reinterpret_cast<const unsigned *>(B.stage.d + r.o_mw));
+            const unsigned *m = r.mw + (r.mask[i] - r.d_mw);
             for (int j = 0, k = 0; j < a.n_points; ++j) {
                 if (!a.status[j]) continue;
                 if (!((m[k >> 5] >> (k & 31)) & 1u)) a.status[j] = 0;
@@ -579,10 +568,7 @@ int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchO
     size_t n_pts = 0;
     for (int i = 0; i < n; ++i) {
         const KltBatchItem &a = pairs[i];
-        if (a.slot < 0 || a.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: slot out of range");
-        if ((size_t)a.slot >= taken.size()) taken.resize(a.slot + 1, 0);
-        if (taken[a.slot]) return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: a slot appears twice");
-        taken[a.slot] = 1;
+        TRY(take_slot(h, taken, a.slot, "batch_track_keypoints"));
         if (a.width < kKltMinFrame || a.height < kKltMinFrame || a.stride < a.width || !a.next_id)
             return fail(h, PVIO_B200_EINVAL, "batch_track_keypoints: bad shape, stride or frame id");
         if (do_clahe && (a.width % tiles_x || a.height % tiles_y))
@@ -641,39 +627,38 @@ int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchO
         max_words = std::max(max_words, nw);
     }
 
-    // staging (both sides): upload [o_lv, o_err) | download [o_next, o_mw) | masks [o_mw, o_job) | jobs (host side)
+    // staging: pair descriptors, RANSAC problems, frame descriptors, pair indices, pixels, LK inputs (uploaded) | initial
+    // guesses in, positions out | errors, status, survivors, counts (downloaded) and the winners' mask words (downloaded
+    // by the caller) | mask jobs (read in place).  Points written on the device leave LK's inputs and outputs in scratch.
+    // Scratch: CLAHE tables | survivors p, q | schedules | models | per-iteration masks | undistorted frames (CLAHE's
+    // input)
     const size_t tiles = do_clahe ? (size_t)tiles_x * tiles_y : 0;
-    size_t o = 0;
-    const size_t o_lv = o;   o = align256(o + sizeof(KltLevels) * n);
-    const size_t o_fmp = o;  o = align256(o + sizeof(FmBatchProblem) * n);
-    const size_t o_frm = o;  o = align256(o + sizeof(KltBatchFrame) * n_frames);
-    const size_t o_pof = o;  o = align256(o + sizeof(int) * n_pts);
-    const size_t o_pix = o;  o += pix_bytes;
-    const size_t o_prev = o; o = align256(o + sizeof(float) * 2 * n_pts);
-    const size_t o_next = o; o = align256(o + sizeof(float) * 2 * n_pts);          // guesses in, positions out
-    const size_t o_err = o;  o = align256(o + sizeof(float) * n_pts);
-    const size_t o_st = o;   o = align256(o + n_pts);
-    const size_t o_surv = o; o = align256(o + sizeof(int) * 2 * n);
-    const size_t o_cnt = o;  o = align256(o + sizeof(int) * 4 * budget_sum);
-    const size_t o_mw = o;   o = align256(o + sizeof(unsigned) * words_sum);
-    const size_t o_job = o;  o = align256(o + sizeof(FmMaskJob) * n);
-    // device scratch: CLAHE tables | survivors p, q | schedules | models | per-iteration masks | undistorted frames
-    // (CLAHE's input)
-    size_t c = 0;
-    const size_t c_lut = c;   c = align256(c + tiles * 256 * n_frames);
-    const size_t c_pq = c;    c = align256(c + sizeof(float2) * 2 * n_pts);
-    const size_t c_sched = c; c = align256(c + sizeof(int) * 7 * budget_sum);
-    const size_t c_F = c;     c = align256(c + sizeof(double) * 27 * budget_sum);
-    const size_t c_masks = c; c = align256(c + sizeof(unsigned) * mask_words);
-    const size_t c_und = c;   c += und_bytes;
-    TRY(reserve(h, B.stage, o, kBoth));
-    TRY(reserve(h, B.scratch, std::max<size_t>(c, 256), kDevice));
-    uint8_t *hs = B.stage.h, *ds = B.stage.d, *dc = B.scratch.d;
-    KltLevels *lv = reinterpret_cast<KltLevels *>(hs + o_lv);
-    FmBatchProblem *fmp = reinterpret_cast<FmBatchProblem *>(hs + o_fmp);
-    KltBatchFrame *frm = reinterpret_cast<KltBatchFrame *>(hs + o_frm);
-    int *pof = reinterpret_cast<int *>(hs + o_pof);
-    float *h_prev = reinterpret_cast<float *>(hs + o_prev), *h_next = reinterpret_cast<float *>(hs + o_next);
+    Stage S(B.stage, &B.scratch);
+    const auto sLv = S.add<KltLevels>(Stage::kUp, n);
+    const auto sFmp = S.add<FmBatchProblem>(Stage::kUp, n);
+    const auto sFrm = S.add<KltBatchFrame>(Stage::kUp, n_frames);
+    const auto sPof = S.add<int>(Stage::kUp, n_pts);
+    const auto sPix = S.add<uint8_t>(Stage::kUp, pix_bytes);
+    const auto sPrev = S.add<float>(dev ? Stage::kScratch : Stage::kUp, 2 * n_pts);
+    const auto sNext = S.add<float>(dev ? Stage::kScratch : Stage::kInOut, 2 * n_pts);
+    const auto sErr = S.add<float>(dev ? Stage::kScratch : Stage::kDown, n_pts);
+    const auto sSt = S.add<uint8_t>(dev ? Stage::kScratch : Stage::kDown, n_pts);
+    const auto sSurv = S.add<int>(Stage::kDown, 2 * n);
+    const auto sCnt = S.add<int>(Stage::kDown, 4 * budget_sum);
+    const auto sMw = S.add<unsigned>(Stage::kDown, words_sum);
+    const auto sJob = S.add<FmMaskJob>(Stage::kMapped, n);
+    const auto sLut = S.add<uint8_t>(Stage::kScratch, tiles * 256 * n_frames);
+    const auto sPq = S.add<float2>(Stage::kScratch, 2 * n_pts);
+    const auto sSched = S.add<int>(Stage::kScratch, 7 * budget_sum);
+    const auto sF = S.add<double>(Stage::kScratch, 27 * budget_sum);
+    const auto sMasks = S.add<unsigned>(Stage::kScratch, mask_words);
+    const auto sUnd = S.add<uint8_t>(Stage::kScratch, und_bytes);
+    TRY(S.place(h));
+    KltLevels *lv = S.host(sLv);
+    FmBatchProblem *fmp = S.host(sFmp);
+    KltBatchFrame *frm = S.host(sFrm);
+    int *pof = S.host(sPof);
+    float *h_prev = S.host(sPrev), *h_next = S.host(sNext);
     size_t p = 0, f_lens = 0, f_plain = n_lens, pix = 0, und = 0, bsum = 0, msum = 0;
     for (int i = 0; i < n; ++i) {
         const KltBatchItem &a = pairs[i];
@@ -684,14 +669,14 @@ int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchO
         const uint8_t *src[2] = {a.prev, a.next};
         for (int side = 0; side < 2; ++side) {
             if (pl.have[side]) continue;
-            uint8_t *dst = hs + o_pix + pix;
+            uint8_t *dst = S.host(sPix) + pix;
             for (int y = 0; y < a.height; ++y) memcpy(dst + (size_t)y * a.width, src[side] + (size_t)y * a.stride, a.width);
             const size_t f = L ? f_lens++ : f_plain++;
-            uint8_t *raw = ds + o_pix + pix;
-            if (L) raw = do_clahe ? dc + c_und + und : s.pyr[pl.slot[side]].d;    // remapped: CLAHE's input, or level 0
-            frm[f] = klt_frame(s, pl.slot[side], raw, dc + c_lut + f * tiles * 256, clahe_clip, tiles_x, tiles_y);
+            uint8_t *raw = S.dev(sPix) + pix;
+            if (L) raw = do_clahe ? S.dev(sUnd) + und : s.pyr[pl.slot[side]].d;    // remapped: CLAHE's input, or level 0
+            frm[f] = klt_frame(s, pl.slot[side], raw, S.dev(sLut) + f * tiles * 256, clahe_clip, tiles_x, tiles_y);
             if (L) {
-                frm[f].lens_src = ds + o_pix + pix; frm[f].m1 = L->m1(); frm[f].m2 = L->m2();
+                frm[f].lens_src = S.dev(sPix) + pix; frm[f].m1 = L->m1(); frm[f].m2 = L->m2();
                 if (do_clahe) und += align256((size_t)a.width * a.height);
             }
             pix += align256((size_t)a.width * a.height);
@@ -708,16 +693,16 @@ int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchO
             std::fill(pof + p, pof + p + np, i);
         }
         FmBatchProblem &P = fmp[i];
-        P.prev_pts = reinterpret_cast<const float *>(ds + o_prev) + 2 * p;
-        P.next_pts = reinterpret_cast<const float *>(ds + o_next) + 2 * p;
-        P.status = ds + o_st + p;
-        P.p = reinterpret_cast<float2 *>(dc + c_pq) + p;
-        P.q = reinterpret_cast<float2 *>(dc + c_pq) + n_pts + p;
-        P.sched = reinterpret_cast<int *>(dc + c_sched) + 7 * bsum;
-        P.counts = reinterpret_cast<int *>(ds + o_cnt) + 4 * bsum;
-        P.F = reinterpret_cast<double *>(dc + c_F) + 27 * bsum;
-        P.masks = reinterpret_cast<unsigned *>(dc + c_masks) + msum;
-        P.surv = reinterpret_cast<int *>(ds + o_surv) + 2 * i;
+        P.prev_pts = S.dev(sPrev) + 2 * p;
+        P.next_pts = S.dev(sNext) + 2 * p;
+        P.status = S.dev(sSt) + p;
+        P.p = S.dev(sPq) + p;
+        P.q = S.dev(sPq) + n_pts + p;
+        P.sched = S.dev(sSched) + 7 * bsum;
+        P.counts = S.dev(sCnt) + 4 * bsum;
+        P.F = S.dev(sF) + 27 * bsum;
+        P.masks = S.dev(sMasks) + msum;
+        P.surv = S.dev(sSurv) + 2 * i;
         P.n_pts = np;
         P.budget = budget[i];
         p += np;
@@ -726,36 +711,30 @@ int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchO
     }
 
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(ds, hs, dev ? o_prev : o_err, cudaMemcpyHostToDevice, st));
-    if (dev && n_pts > 0) {
-        TRY(dev->write_points(h, reinterpret_cast<float *>(ds + o_prev), reinterpret_cast<float *>(ds + o_next),
-                              reinterpret_cast<const int *>(ds + o_pof)));
-    }
-    if (n_lens > 0) undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_lens, lens_w, lens_h);
-    if (n_frames > 0)
-        TRY(klt_build_pyramids(h, frm, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), (int)n_frames, do_clahe, tiles_x, tiles_y));
+    TRY(S.upload(h));
+    if (dev && n_pts > 0) TRY(dev->write_points(h, S.dev(sPrev), S.dev(sNext), S.dev(sPof)));
+    if (n_lens > 0) undistort_frames(h, S.dev(sFrm), (int)n_lens, lens_w, lens_h);
+    if (n_frames > 0) TRY(klt_build_pyramids(h, frm, S.dev(sFrm), (int)n_frames, do_clahe, tiles_x, tiles_y));
     if (n_pts > 0)
-        klt_lk(h, reinterpret_cast<const KltLevels *>(ds + o_lv), reinterpret_cast<const int *>(ds + o_pof),
-               reinterpret_cast<const float *>(ds + o_prev), reinterpret_cast<float *>(ds + o_next), ds + o_st,
-               reinterpret_cast<float *>(ds + o_err), n_pts, max_iter, eps, border);
-    const FmBatchProblem *d_fmp = reinterpret_cast<const FmBatchProblem *>(ds + o_fmp);
+        klt_lk(h, S.dev(sLv), S.dev(sPof), S.dev(sPrev), S.dev(sNext), S.dev(sSt), S.dev(sErr), n_pts, max_iter, eps, border);
+    const FmBatchProblem *d_fmp = S.dev(sFmp);
     if (max_budget > 0) {
         fm_batch_schedule(h, d_fmp, n, fm_iters, lmeds_iters);
         fm_batch_hypotheses(h, d_fmp, n, max_budget, (float)(thr * thr));
     }
     CK(h, cudaGetLastError());
     // with the points on the device, only what the replay reads comes back
-    const size_t o_down = dev ? o_surv : o_next;
-    CK(h, cudaMemcpyAsync(hs + o_down, ds + o_down, o_mw - o_down, cudaMemcpyDeviceToHost, st));
+    TRY(dev ? S.download(h, sSurv, sCnt) : S.download(h, sNext, sCnt));
     CK(h, cudaStreamSynchronize(st));
 
     // each pair's replay (opencv_image.cpp:112-129: findFundamentalMat over >= 8 survivors)
-    const int *r_surv = reinterpret_cast<const int *>(hs + o_surv), *r_cnt = reinterpret_cast<const int *>(hs + o_cnt);
-    FmMaskJob *jobs = reinterpret_cast<FmMaskJob *>(hs + o_job);
-    res.next = reinterpret_cast<const float *>(dev ? ds + o_next : hs + o_next);
-    res.err = reinterpret_cast<const float *>(dev ? ds + o_err : hs + o_err);
-    res.status = dev ? ds + o_st : hs + o_st;
-    res.o_mw = o_mw;
+    const int *r_surv = S.host(sSurv), *r_cnt = S.host(sCnt);
+    FmMaskJob *jobs = S.host(sJob);
+    res.next = dev ? S.dev(sNext) : S.host(sNext);
+    res.err = dev ? S.dev(sErr) : S.host(sErr);
+    res.status = dev ? S.dev(sSt) : S.host(sSt);
+    res.mw = S.host(sMw);
+    res.d_mw = S.dev(sMw);
     res.words = words_sum;
     bool any_job = false;
     bsum = 0;
@@ -774,7 +753,7 @@ int klt_batch_track(Handle *h, int n, const KltBatchItem *pairs, const KltBatchO
             if (have > 0 && bi >= 0) {
                 const FmBatchProblem &P = fmp[i];
                 J.p = P.p; J.q = P.q; J.n = s;
-                J.out = reinterpret_cast<unsigned *>(ds + o_mw) + wsum;
+                J.out = S.dev(sMw) + wsum;
                 if (s >= 15) J.src = P.masks + (size_t)(3 * bi + bk) * ((s + 31) / 32);
                 else { J.F = P.F + (size_t)(3 * bi + bk) * 9; J.thr2 = thr_lmeds; }
                 res.mask[i] = J.out;

@@ -270,7 +270,7 @@ int batch_window_plane_ransac_impl(Handle *h, int n, const pvio_b200_window_plan
     const size_t C = rows.size(), I = (size_t)n * kIters;
     // upload records | rows; download (after the hypotheses) points used | counts | schedules, (after the finish)
     // used | inlier | candidate points | planes; device only the compacted points, lots, compacted indices and mask
-    Stage S;
+    Stage S(h->bw.stage, &h->bw.scratch);
     const auto sRec = S.up(plan);
     const auto sRow = S.up(rows);
     const auto sNu = S.add<int>(Stage::kDown, n);
@@ -290,16 +290,11 @@ int batch_window_plane_ransac_impl(Handle *h, int n, const pvio_b200_window_plan
     A.pts = S.dev(sPts); A.lots = S.dev(sLots); A.cidx = S.dev(sCidx); A.cmask = S.dev(sMask);
     A.used = S.dev(sUsed); A.inl = S.dev(sInl); A.cpt = S.dev(sCpt); A.plane = S.dev(sPl);
     cudaStream_t st = h->stream;
-    // device -> host of the sections [first, last]: they are laid out back to back
-    auto down = [&](const void *first_h, const void *first_d, const void *end_d) {
-        const size_t bytes = (const uint8_t *)end_d - (const uint8_t *)first_d;
-        return cudaMemcpyAsync(const_cast<void *>(first_h), first_d, bytes, cudaMemcpyDeviceToHost, st);
-    };
     pr_gather_kernel<<<n, kBwThreads, 0, st>>>(launch_args<BwArgs>(h), A);
     pr_hypothesis_kernel<<<dim3((kIters + kPrWarps - 1) / kPrWarps, n), 32 * kPrWarps, 0, st>>>(A);
     h->launches += 2;
     CK(h, cudaGetLastError());
-    CK(h, down(S.host(sNu), S.dev(sNu), want_sched ? (const void *)(S.dev(sSch) + 3 * I) : (const void *)(S.dev(sCnt) + I)));
+    TRY(S.download(h, sNu, want_sched ? sSch : sCnt));
     CK(h, cudaStreamSynchronize(st));
 
     std::vector<int> res(4 * (size_t)n);
@@ -312,11 +307,11 @@ int batch_window_plane_ransac_impl(Handle *h, int n, const pvio_b200_window_plan
         PrRec &R = S.host(sRec)[k];
         R.best_it = rk[2]; R.inliers = rk[0];
     }
-    CK(h, cudaMemcpyAsync(S.dev(sRec), S.host(sRec), sizeof(PrRec) * n, cudaMemcpyHostToDevice, st));
+    TRY(S.upload(h, sRec));
     pr_finish_kernel<<<n, kBwThreads, 0, st>>>(A);
     ++h->launches;
     CK(h, cudaGetLastError());
-    CK(h, down(S.host(sUsed), S.dev(sUsed), S.dev(sPl) + 8 * (size_t)n));
+    TRY(S.download(h, sUsed, sPl));
     CK(h, cudaStreamSynchronize(st));
 
     for (int k = 0; k < n; ++k) {

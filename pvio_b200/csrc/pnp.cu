@@ -298,7 +298,7 @@ int launch_pnp(Handle *h, int n, const PnpArgs *d_recs) {
 }
 
 // n problems, frames [n][frames_stride]: every problem is checked before anything is copied; then one H2D copy of the
-// packed staging, one launch between ev0 / ev1, one D2H copy of the frames and summary words, one synchronise.
+// staging, one launch between ev0 / ev1, one D2H copy of the frames and summary words, one synchronise.
 int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, double *frames, int64_t frames_stride,
                          const pvio_b200_options *opt, pvio_b200_summary *summaries) {
     if (n < 0) return fail(h, PVIO_B200_EINVAL, "pnp: negative problem count");
@@ -313,26 +313,29 @@ int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, dou
         n_pts += pb.n_points;
         n_imu += pb.use_inertial ? 1 : 0;
     }
-    // staging layout (doubles): records [n][kPnpRecWords] | points [n_pts][3] and z [n_pts][2], problem after problem |
-    // IMU records [n_imu][kImuStride] of the inertial problems | frames [n][16] | summary words [n][8]
-    const size_t o_pts = (size_t)n * kPnpRecWords, o_z = o_pts + 3 * n_pts, o_imu = o_z + 2 * n_pts;
-    const size_t o_frames = o_imu + n_imu * kImuStride, o_out = o_frames + (size_t)16 * n, words = o_out + (size_t)8 * n;
-    // this runs on every frame: grown to the largest batch seen, no allocation in the steady state
-    TRY(reserve(h, h->pnp, std::max<size_t>(words, (size_t)kPnpRecWords + 5 * 512 + kImuStride + 24), kBoth));
-    double *d = h->pnp.d, *stage = h->pnp.h;
-    PnpArgs *recs = reinterpret_cast<PnpArgs *>(stage);
+    // staging: records | points [n_pts][3] and z [n_pts][2], problem after problem | IMU records of the inertial
+    // problems (uploaded) || frames (both ways) || summary words (downloaded).  This runs on every frame: grown to powers
+    // of two, no allocation in the steady state.
+    Stage S(h->pnp);
+    S.pow2 = true;
+    const auto recs = S.add<PnpArgs>(Stage::kUp, n);
+    const auto pts = S.add<double>(Stage::kUp, 3 * n_pts), z = S.add<double>(Stage::kUp, 2 * n_pts);
+    const auto imu = S.add<double>(Stage::kUp, n_imu * kImuStride);
+    const auto frs = S.add<double>(Stage::kInOut, 16 * (size_t)n);
+    const auto out = S.add<double>(Stage::kDown, 8 * (size_t)n);
+    TRY(S.place(h));
     const SolveOptions o = solve_options(opt);
     size_t p = 0, k = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_pnp_problem &pb = pbs[i];
         const int m = pb.n_points;
-        PnpArgs &a = recs[i];
+        PnpArgs &a = S.host(recs)[i];
         memset(&a, 0, sizeof(a));
         if (m > 0) {
-            memcpy(stage + o_pts + 3 * p, pb.points, sizeof(double) * 3 * m);
-            memcpy(stage + o_z + 2 * p, pb.z, sizeof(double) * 2 * m);
+            memcpy(S.host(pts) + 3 * p, pb.points, sizeof(double) * 3 * m);
+            memcpy(S.host(z) + 2 * p, pb.z, sizeof(double) * 2 * m);
         }
-        a.pts = d + o_pts + 3 * p; a.z = d + o_z + 2 * p;
+        a.pts = S.dev(pts) + 3 * p; a.z = S.dev(z) + 2 * p;
         a.n = m; a.inertial = pb.use_inertial ? 1 : 0;
         a.max_iter = o.max_iter;
         a.radius0 = o.radius0;
@@ -342,37 +345,36 @@ int batch_pnp_solve_impl(Handle *h, int n, const pvio_b200_pnp_problem *pbs, dou
         a.wc.cauchy_a = pb.cauchy_a > 0 ? pb.cauchy_a : 1.0;
         memcpy(a.last, pb.last_frame, sizeof(double) * 16);
         if (a.inertial) {
-            memcpy(stage + o_imu + k * kImuStride, pb.imu_data, sizeof(double) * kImuStride);
-            a.imu_rec = d + o_imu + k * kImuStride;
+            memcpy(S.host(imu) + k * kImuStride, pb.imu_data, sizeof(double) * kImuStride);
+            a.imu_rec = S.dev(imu) + k * kImuStride;
             ++k;
         }
-        memcpy(stage + o_frames + 16 * (size_t)i, frames + frames_stride * i, sizeof(double) * 16);
-        a.frame = d + o_frames + 16 * (size_t)i;
-        a.out = d + o_out + 8 * (size_t)i;
+        memcpy(S.host(frs) + 16 * (size_t)i, frames + frames_stride * i, sizeof(double) * 16);
+        a.frame = S.dev(frs) + 16 * (size_t)i;
+        a.out = S.dev(out) + 8 * (size_t)i;
         p += m;
     }
-    CK(h, cudaMemcpyAsync(d, stage, sizeof(double) * o_out, cudaMemcpyHostToDevice, h->stream));
-    const PnpArgs *d_recs = reinterpret_cast<const PnpArgs *>(d);
-    TRY(launch_pnp(h, n, d_recs));
-    // the frames + summary words come back into the pinned staging
-    CK(h, cudaMemcpyAsync(stage + o_frames, d + o_frames, sizeof(double) * 24 * n, cudaMemcpyDeviceToHost, h->stream));
+    TRY(S.upload(h));
+    TRY(launch_pnp(h, n, S.dev(recs)));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(h->stream));
     CK(h, cudaGetLastError());
     float ms = 0.f;
     if (summaries) cudaEventElapsedTime(&ms, h->ev0, h->ev1);
     for (int i = 0; i < n; ++i) {
-        memcpy(frames + frames_stride * i, stage + o_frames + 16 * (size_t)i, sizeof(double) * 16);
-        if (!summaries) continue;
-        const double *back = stage + o_out + 8 * (size_t)i;
-        pvio_b200_summary *summary = summaries + i;
-        memset(summary, 0, sizeof(*summary));
-        summary->iterations = (int)back[0]; summary->accepted_steps = (int)back[1];
-        summary->termination = (int)back[2]; summary->usable = (int)back[3];
-        summary->initial_cost = back[4]; summary->final_cost = back[5];
-        summary->final_radius = back[6]; summary->final_mu = back[7];
-        summary->solve_seconds = ms * 1e-3;
+        memcpy(frames + frames_stride * i, S.host(frs) + 16 * (size_t)i, sizeof(double) * 16);
+        if (summaries) pnp_summary(S.host(out) + 8 * (size_t)i, ms, summaries + i);
     }
     return 0;
+}
+
+void pnp_summary(const double *out, float ms, pvio_b200_summary *s) {
+    memset(s, 0, sizeof(*s));
+    s->iterations = (int)out[0]; s->accepted_steps = (int)out[1];
+    s->termination = (int)out[2]; s->usable = (int)out[3];
+    s->initial_cost = out[4]; s->final_cost = out[5];
+    s->final_radius = out[6]; s->final_mu = out[7];
+    s->solve_seconds = ms * 1e-3;
 }
 
 int pnp_solve_impl(Handle *h, const pvio_b200_pnp_problem *pb, double *frame, const pvio_b200_options *opt,

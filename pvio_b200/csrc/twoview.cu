@@ -864,7 +864,6 @@ int batch_two_view_impl(Handle *h, int n, const pvio_b200_two_view *recs) {
     TRY(tv_check(h, n, recs));
     if (n == 0) return 0;
     cudaSetDevice(h->device);
-    TwoViewState &S = h->tv;
     std::vector<int> off(n + 1, 0);
     int I = 1;
     bool want_sched = false;
@@ -874,23 +873,25 @@ int batch_two_view_impl(Handle *h, int n, const pvio_b200_two_view *recs) {
         want_sched |= recs[k].h_schedule || recs[k].e_schedule;
     }
     const size_t total = (size_t)off[n], tot1 = std::max<size_t>(total, 1), rows = (size_t)n * I;
-    auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    // staging: problems | p1 | p2 (uploaded) | outputs | masks and point status | points (downloaded)
-    const size_t oProb = 0, oP1 = al(sizeof(TvProb) * n), oP2 = oP1 + al(16 * tot1), oOut = oP2 + al(16 * tot1),
-                 oMask = oOut + al(sizeof(TvOut) * n), oPts = oMask + al(3 * tot1), stage_bytes = oPts + al(24 * tot1);
-    // counts (both sides): schedules H, E | counts H, E
-    const size_t cSh = 0, cSe = cSh + 4 * rows, cCh = cSe + 5 * rows, cCe = cCh + rows, cnt_ints = cCe + 11 * rows;
-    // device scratch: lots | H models | E models | parallax | scores | score flags
-    const size_t sLots = 0, sHm = al(4 * tot1), sEm = sHm + al(72 * rows), sPar = sEm + al(720 * rows), sSc = sPar + al(8 * tot1),
-                 sOk = sSc + al(64 * tot1), scratch_bytes = sOk + al(8 * tot1);
-    TRY(reserve(h, S.stage, stage_bytes, kBoth));
-    TRY(reserve(h, S.counts, cnt_ints, kBoth));
-    TRY(reserve(h, S.scratch, scratch_bytes, kDevice));
+    // staging: problems | p1 | p2 (uploaded) | schedules H, E | counts H, E | outputs | masks and point status | points
+    // (downloaded); device scratch: lots | H models | E models | parallax | scores | score flags
+    Stage S(h->tv.stage, &h->tv.scratch);
+    const auto prob = S.add<TvProb>(Stage::kUp, n);
+    const auto p1 = S.add<double>(Stage::kUp, 2 * tot1), p2 = S.add<double>(Stage::kUp, 2 * tot1);
+    const auto sh = S.add<int>(Stage::kDown, 4 * rows), se = S.add<int>(Stage::kDown, 5 * rows);
+    const auto ch = S.add<int>(Stage::kDown, rows), ce = S.add<int>(Stage::kDown, 11 * rows);
+    const auto out = S.add<TvOut>(Stage::kDown, n);
+    const auto mask = S.add<uint8_t>(Stage::kDown, 3 * tot1);
+    const auto pts = S.add<double>(Stage::kDown, 3 * tot1);
+    const auto lots = S.add<int>(Stage::kScratch, tot1);
+    const auto hm = S.add<double>(Stage::kScratch, 9 * rows), em = S.add<double>(Stage::kScratch, 90 * rows);
+    const auto par = S.add<double>(Stage::kScratch, tot1), sco = S.add<double>(Stage::kScratch, 8 * tot1);
+    const auto ok = S.add<uint8_t>(Stage::kScratch, 8 * tot1);
+    TRY(S.place(h));
 
-    uint8_t *hs = S.stage.h, *ds = S.stage.d;
-    TvProb *hp = reinterpret_cast<TvProb *>(hs + oProb), *dp = reinterpret_cast<TvProb *>(ds + oProb);
-    double *h1 = reinterpret_cast<double *>(hs + oP1), *h2 = reinterpret_cast<double *>(hs + oP2);
-    const double2 *d1 = reinterpret_cast<const double2 *>(ds + oP1), *d2 = reinterpret_cast<const double2 *>(ds + oP2);
+    TvProb *hp = S.host(prob), *dp = S.dev(prob);
+    double *h1 = S.host(p1), *h2 = S.host(p2);
+    const double2 *d1 = reinterpret_cast<const double2 *>(S.dev(p1)), *d2 = reinterpret_cast<const double2 *>(S.dev(p2));
     for (int k = 0; k < n; ++k) {
         const pvio_b200_two_view &r = recs[k];
         const double thr = 0.7 / r.fx;
@@ -909,50 +910,46 @@ int batch_two_view_impl(Handle *h, int n, const pvio_b200_two_view *recs) {
         }
     }
     TvScratch sc{};
-    uint8_t *dsc = S.scratch.d;
-    int *dc = S.counts.d;
     sc.I = I;
-    sc.lots = reinterpret_cast<int *>(dsc + sLots);
-    sc.sched_h = dc + cSh; sc.sched_e = dc + cSe; sc.cnt_h = dc + cCh; sc.cnt_e = dc + cCe;
-    sc.Hm = reinterpret_cast<double *>(dsc + sHm); sc.Em = reinterpret_cast<double *>(dsc + sEm);
-    sc.par = reinterpret_cast<double *>(dsc + sPar); sc.sc = reinterpret_cast<double *>(dsc + sSc); sc.ok = dsc + sOk;
-    sc.out = reinterpret_cast<TvOut *>(ds + oOut);
-    sc.hmask = ds + oMask; sc.emask = ds + oMask + tot1; sc.pstat = ds + oMask + 2 * tot1;
-    sc.pts = reinterpret_cast<double *>(ds + oPts);
+    sc.lots = S.dev(lots);
+    sc.sched_h = S.dev(sh); sc.sched_e = S.dev(se); sc.cnt_h = S.dev(ch); sc.cnt_e = S.dev(ce);
+    sc.Hm = S.dev(hm); sc.Em = S.dev(em);
+    sc.par = S.dev(par); sc.sc = S.dev(sco); sc.ok = S.dev(ok);
+    sc.out = S.dev(out);
+    sc.hmask = S.dev(mask); sc.emask = S.dev(mask) + tot1; sc.pstat = S.dev(mask) + 2 * tot1;
+    sc.pts = S.dev(pts);
 
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(ds, hs, oOut, cudaMemcpyHostToDevice, st));
+    TRY(S.upload(h));
     tv_schedule_kernel<<<(n + 63) / 64, 64, 0, st>>>(dp, n, sc);
     const dim3 grid((I + kTvWarps - 1) / kTvWarps, n);
     tv_homography_kernel<<<grid, 32 * kTvWarps, 0, st>>>(dp, sc);
     tv_essential_kernel<<<grid, 32 * kTvWarps, 0, st>>>(dp, sc);
     h->launches += 3;
     CK(h, cudaGetLastError());
-    const size_t c0 = want_sched ? cSh : cCh;
-    CK(h, cudaMemcpyAsync(S.counts.h + c0, dc + c0, sizeof(int) * (cnt_ints - c0), cudaMemcpyDeviceToHost, st));
+    TRY(S.download(h, want_sched ? sh : ch, ce));
     CK(h, cudaStreamSynchronize(st));
 
-    const int *hc = S.counts.h;
     std::vector<int> res(8 * n);
     for (int k = 0; k < n; ++k) {
         TvProb &P = hp[k];
         int *rk = &res[8 * k];
         rk[0] = rk[1] = rk[4] = rk[5] = 0; rk[2] = rk[3] = rk[6] = rk[7] = -1;
         if (P.iters == 0) continue;
-        ransac_replay(hc + cCh + (size_t)k * I, 1, true, P.n, P.iters, recs[k].confidence, rk);
-        ransac_replay(hc + cCe + (size_t)k * I * 11, 11, false, P.n, P.iters, recs[k].confidence, rk + 4);
+        ransac_replay(S.host(ch) + (size_t)k * I, 1, true, P.n, P.iters, recs[k].confidence, rk);
+        ransac_replay(S.host(ce) + (size_t)k * I * 11, 11, false, P.n, P.iters, recs[k].confidence, rk + 4);
         P.h_it = rk[2]; P.e_it = rk[6]; P.e_k = rk[7];
     }
-    CK(h, cudaMemcpyAsync(ds, hs, sizeof(TvProb) * n, cudaMemcpyHostToDevice, st));
+    TRY(S.upload(h, prob));
     tv_finish_kernel<<<n, kFinishThreads, 0, st>>>(dp, sc);
     ++h->launches;
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(hs + oOut, ds + oOut, stage_bytes - oOut, cudaMemcpyDeviceToHost, st));
+    TRY(S.download(h, out, pts));
     CK(h, cudaStreamSynchronize(st));
 
-    const TvOut *ho = reinterpret_cast<const TvOut *>(hs + oOut);
-    const uint8_t *hm = hs + oMask;
-    const double *hpts = reinterpret_cast<const double *>(hs + oPts);
+    const TvOut *ho = S.host(out);
+    const uint8_t *hmk = S.host(mask);
+    const double *hpts = S.host(pts);
     for (int k = 0; k < n; ++k) {
         const pvio_b200_two_view &r = recs[k];
         const TvOut &O = ho[k];
@@ -967,15 +964,15 @@ int batch_two_view_impl(Handle *h, int n, const pvio_b200_two_view *recs) {
         if (r.E) std::memcpy(r.E, O.E, sizeof(O.E));
         if (r.R) std::memcpy(r.R, O.R, sizeof(O.R));
         if (r.T) std::memcpy(r.T, O.T, sizeof(O.T));
-        if (r.h_mask && nk) std::memcpy(r.h_mask, hm + o, nk);
-        if (r.e_mask && nk) std::memcpy(r.e_mask, hm + tot1 + o, nk);
-        if (r.point_status && nk) std::memcpy(r.point_status, hm + 2 * tot1 + o, nk);
+        if (r.h_mask && nk) std::memcpy(r.h_mask, hmk + o, nk);
+        if (r.e_mask && nk) std::memcpy(r.e_mask, hmk + tot1 + o, nk);
+        if (r.point_status && nk) std::memcpy(r.point_status, hmk + 2 * tot1 + o, nk);
         if (r.points && nk) std::memcpy(r.points, hpts + 3 * (size_t)o, sizeof(double) * 3 * nk);
         const size_t rb = (size_t)k * I;
-        if (r.h_schedule && Ik) std::memcpy(r.h_schedule, hc + cSh + 4 * rb, sizeof(int) * 4 * Ik);
-        if (r.e_schedule && Ik) std::memcpy(r.e_schedule, hc + cSe + 5 * rb, sizeof(int) * 5 * Ik);
-        if (r.h_counts && Ik) std::memcpy(r.h_counts, hc + cCh + rb, sizeof(int) * Ik);
-        if (r.e_counts && Ik) std::memcpy(r.e_counts, hc + cCe + 11 * rb, sizeof(int) * 11 * Ik);
+        if (r.h_schedule && Ik) std::memcpy(r.h_schedule, S.host(sh) + 4 * rb, sizeof(int) * 4 * Ik);
+        if (r.e_schedule && Ik) std::memcpy(r.e_schedule, S.host(se) + 5 * rb, sizeof(int) * 5 * Ik);
+        if (r.h_counts && Ik) std::memcpy(r.h_counts, S.host(ch) + rb, sizeof(int) * Ik);
+        if (r.e_counts && Ik) std::memcpy(r.e_counts, S.host(ce) + 11 * rb, sizeof(int) * 11 * Ik);
     }
     return 0;
 }

@@ -143,8 +143,6 @@ __global__ void undistort_kernel(const KltBatchFrame *frames) {
     f.raw[i] = (uint8_t)((sum + 512) >> 10);
 }
 
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 }  // namespace
 
 int undistort_map_host(int model, int width, int height, const double *p, const double *c, int16_t *m1, uint16_t *m2) {
@@ -177,10 +175,7 @@ int set_lens_impl(Handle *h, int n, const pvio_b200_lens *recs) {
     std::vector<std::vector<uint8_t>> maps(n);
     for (int i = 0; i < n; ++i) {
         const pvio_b200_lens &r = recs[i];
-        if (r.slot < 0 || r.slot > kMaxBatchSlot) return fail(h, PVIO_B200_EINVAL, "batch_set_lens: slot out of range");
-        if ((size_t)r.slot >= taken.size()) taken.resize(r.slot + 1, 0);
-        if (taken[r.slot]) return fail(h, PVIO_B200_EINVAL, "batch_set_lens: a slot appears twice");
-        taken[r.slot] = 1;
+        TRY(take_slot(h, taken, r.slot, "batch_set_lens"));
         if (r.model == 0) continue;
         if (r.width < 8 || r.height < 8 || r.width > kMaxMapSide || r.height > kMaxMapSide)
             return fail(h, PVIO_B200_EINVAL, "batch_set_lens: bad frame shape");
@@ -233,35 +228,34 @@ int batch_undistort_impl(Handle *h, int n, const pvio_b200_undistort_request *re
         pix_bytes += align256((size_t)a.width * a.height);
         max_w = std::max(max_w, a.width); max_h = std::max(max_h, a.height);
     }
-    // staging (both sides): upload descriptors and raw frames [0, o_dst) | download undistorted frames [o_dst, o)
-    size_t o = 0;
-    const size_t o_frm = o; o = align256(o + sizeof(KltBatchFrame) * n);
-    const size_t o_src = o; o += pix_bytes;
-    const size_t o_dst = o; o += pix_bytes;
-    TRY(reserve(h, B.ustage, o, kBoth));
-    uint8_t *hs = B.ustage.h, *ds = B.ustage.d;
-    KltBatchFrame *frm = reinterpret_cast<KltBatchFrame *>(hs + o_frm);
+    // staging: descriptors and raw frames (uploaded) | undistorted frames (downloaded), one 256-byte aligned block per frame
+    Stage S(B.ustage);
+    const auto frm = S.add<KltBatchFrame>(Stage::kUp, n);
+    const auto src = S.add<uint8_t>(Stage::kUp, pix_bytes);
+    const auto dst = S.add<uint8_t>(Stage::kDown, pix_bytes);
+    TRY(S.place(h));
     size_t pix = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_undistort_request &a = reqs[i];
         const SlotLens &L = *slot_lens(B, a.slot);
-        for (int y = 0; y < a.height; ++y) memcpy(hs + o_src + pix + (size_t)y * a.width, a.src + (size_t)y * a.stride, a.width);
-        KltBatchFrame &F = frm[i];
+        for (int y = 0; y < a.height; ++y)
+            memcpy(S.host(src) + pix + (size_t)y * a.width, a.src + (size_t)y * a.stride, a.width);
+        KltBatchFrame &F = S.host(frm)[i];
         memset(&F, 0, sizeof(F));
-        F.lens_src = ds + o_src + pix; F.raw = ds + o_dst + pix; F.m1 = L.m1(); F.m2 = L.m2();
+        F.lens_src = S.dev(src) + pix; F.raw = S.dev(dst) + pix; F.m1 = L.m1(); F.m2 = L.m2();
         F.levels = 1; F.w[0] = a.width; F.h[0] = a.height;
         pix += align256((size_t)a.width * a.height);
     }
     cudaStream_t st = h->stream;
-    CK(h, cudaMemcpyAsync(ds, hs, o_dst, cudaMemcpyHostToDevice, st));
-    undistort_frames(h, reinterpret_cast<const KltBatchFrame *>(ds + o_frm), n, max_w, max_h);
+    TRY(S.upload(h));
+    undistort_frames(h, S.dev(frm), n, max_w, max_h);
     CK(h, cudaGetLastError());
-    CK(h, cudaMemcpyAsync(hs + o_dst, ds + o_dst, pix_bytes, cudaMemcpyDeviceToHost, st));
+    TRY(S.download(h));
     CK(h, cudaStreamSynchronize(st));
     pix = 0;
     for (int i = 0; i < n; ++i) {
         const pvio_b200_undistort_request &a = reqs[i];
-        memcpy(a.dst, hs + o_dst + pix, (size_t)a.width * a.height);
+        memcpy(a.dst, S.host(dst) + pix, (size_t)a.width * a.height);
         pix += align256((size_t)a.width * a.height);
     }
     return 0;

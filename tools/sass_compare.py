@@ -1,6 +1,7 @@
 """Compares the SASS of kernels in two builds (objects or shared libraries), ignoring register numbering (with the
-operand-reuse flags that follow it) and the offsets of kernel parameters in the constant bank: a refactor that must not
-change what a kernel executes passes.
+operand-reuse flags that follow it), the offsets of kernel parameters in the constant bank and the hash nvcc gives a
+file's anonymous namespace (it changes with any edit to the file): a refactor that must not change what a kernel
+executes passes.
 
     python tools/sass_compare.py OLD.o NEW.o [KERNEL_REGEX ...]
 
@@ -13,6 +14,7 @@ CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
 _REG = re.compile(r"\b(U?R\d+|U?P[0-6])\b")
 _CBANK = re.compile(r"c\[0x0\]\[0x[0-9a-f]+\]")
 _ADDR = re.compile(r"/\*[0-9a-f]{4,}\*/")
+_ANON = re.compile(r"_GLOBAL__N__[0-9a-f]+_")
 
 
 def kernels(path):
@@ -21,7 +23,7 @@ def kernels(path):
     for line in out.splitlines():
         m = re.match(r"\s*Function : (\S+)", line)
         if m:
-            name = m.group(1)
+            name = _ANON.sub("_GLOBAL__N__", m.group(1))
             funcs[name] = []
             continue
         if name and "/*" in line and ";" in line:
