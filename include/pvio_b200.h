@@ -348,6 +348,31 @@ int pvio_b200_batch_window_solve(pvio_b200_handle h, int n, const int32_t *slots
  * S_out [n][S_stride], e_out [n][e_stride] (may be NULL): the new priors, as pvio_b200_batch_marginalize returns them. */
 int pvio_b200_batch_window_drop_victim(pvio_b200_handle h, int n, const int32_t *slots, double *S_out, int64_t S_stride,
                                        double *e_out, int64_t e_stride);
+/* The covariance of each named slot's window at its current state (after a solve: the solved state) with its IMU records
+ * as they stand: the inverse of H = J^T J of every residual block the solve adds (prior; reprojection and plane blocks
+ * with the Cauchy corrector; IMU), in the solve's local coordinates, without the trust-region regulariser, over the free
+ * coordinates of the solve.  The landmarks are eliminated exactly; the gauge is the window's own (its prior).
+ *  - cov: the joint covariance of the named frames, 15 coordinates per frame [dtheta dp dv dbg dba], in the order named;
+ *    0 in the rows and columns a frame does not have (the pose of a FF_FIX_POSE frame, v / bg / ba of a visual-only
+ *    window).
+ *  - inv_depth_var: Var(rho) of each named track; NaN for a plane track or a track with one observation.
+ *  - status: PVIO_B200_OK, or PVIO_B200_ENUMERIC when the scaled H over the free frame coordinates is not positive
+ *    definite; then every output of the record is NaN, and the call still succeeds.
+ * Rejected (PVIO_B200_EINVAL, no output changed): a slot out of range, not resident, named twice or without frames; a
+ * frame out of range or named twice; an unknown or repeated track; a missing array; a record asking for nothing.  The
+ * call changes no slot; it makes one host -> device copy, four kernel launches whatever n is, one device -> host copy and
+ * one synchronisation. */
+typedef struct pvio_b200_window_covariance {
+    int32_t slot;
+    int32_t n_frames;         /* 0 .. N frames, window indices, distinct                      */
+    const int32_t *frames;
+    double *cov;              /* [(15 n_frames)^2] row-major, frames in the order named       */
+    int32_t n_tracks;         /* 0 .. live tracks                                             */
+    const int32_t *tracks;    /* live track ids of the slot, distinct                         */
+    double *inv_depth_var;    /* [n_tracks]                                                   */
+    int32_t status;           /* out: PVIO_B200_OK or PVIO_B200_ENUMERIC                      */
+} pvio_b200_window_covariance; /* 56 bytes on LP64 */
+int pvio_b200_batch_window_covariance(pvio_b200_handle h, int n, pvio_b200_window_covariance *records);
 /* Device -> host in one copy, per named slot i: n_frames [n], frames [n][frames_stride] ([N][16]), n_tracks [n] (live
  * tracks), and for each live track in id order at [i * track_stride + r]: id, inverse depth, anchor frame, observation
  * count, and the post-pass valid / quality of the last solve (0 / 0 for a track that did not take part in it).  Any

@@ -143,6 +143,11 @@ class CWindowPlaneRansac(C.Structure):
                 ("counts", c_i32p)]
 
 
+class CWindowCovariance(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n_frames", C.c_int32), ("frames", c_i32p), ("cov", c_f64p), ("n_tracks", C.c_int32),
+                ("tracks", c_i32p), ("inv_depth_var", c_f64p), ("status", C.c_int32)]
+
+
 class CWindowKeypoints(C.Structure):
     _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("frame_id", C.c_uint64), ("n", C.c_int32),
                 ("track", c_i32p), ("keypoint", c_i32p), ("newest_is_keyframe", C.c_int32), ("skipped_frames", C.c_int32)]
@@ -245,6 +250,7 @@ SIGNATURES = {
     "pvio_b200_batch_window_set_planes": (_int, [_h, _int, _P(CWindowPlanes)]),
     "pvio_b200_batch_window_solve": (_int, [_h, _int, c_i32p, _P(COptions), _P(CSummary)]),
     "pvio_b200_batch_window_drop_victim": (_int, [_h, _int, c_i32p, c_f64p, _i64, c_f64p, _i64]),
+    "pvio_b200_batch_window_covariance": (_int, [_h, _int, _P(CWindowCovariance)]),
     "pvio_b200_batch_window_download": (_int, [_h, _int, c_i32p, c_i32p, c_f64p, _i64, c_i32p, _i64, c_i32p, c_f64p,
                                                c_i32p, c_i32p, c_u8p, c_f64p]),
     "pvio_b200_batch_window_localize": (_int, [_h, _int, _P(CWindowLocalize), _P(COptions)]),

@@ -447,6 +447,27 @@ class BatchWindows:
                                                                 _lib.ptr(e), d))
         return S, e
 
+    def covariance(self, slots, frames, tracks):
+        """The covariance of each named slot's window at its current state, in the solve's local coordinates: per slot
+        frames[i] (window indices) and tracks[i] (live track ids).  Per record a dict: cov [15 k, 15 k] (the named frames'
+        joint block, [dtheta dp dv dbg dba] per frame; 0 where a frame has no such coordinate), inv_depth_var [len(tracks)]
+        (NaN for a plane track or a track with one observation) and status (OK, or ENUMERIC with every output NaN)."""
+        n = len(slots)
+        recs, out = (_lib.CWindowCovariance * max(n, 1))(), []
+        for r, s, f, t in zip(recs, slots, frames, tracks):
+            f = np.ascontiguousarray(f, dtype=np.int32).reshape(-1)
+            t = np.ascontiguousarray(t, dtype=np.int32).reshape(-1)
+            o = dict(frames=f, tracks=t, cov=np.zeros((15 * len(f), 15 * len(f))), inv_depth_var=np.zeros(len(t)))
+            out.append(o)
+            r.slot, r.n_frames, r.n_tracks = int(s), len(f), len(t)
+            _lib.set_ptrs(r, frames=f if len(f) else None, cov=o["cov"] if len(f) else None,
+                          tracks=t if len(t) else None, inv_depth_var=o["inv_depth_var"] if len(t) else None)
+        self.ba._ck(self.lib.pvio_b200_batch_window_covariance(self.h, n, recs))
+        for r, o in zip(recs, out):
+            del o["frames"], o["tracks"]
+            o["status"] = int(r.status)
+        return out
+
     def save(self, slots, tracker_slots=None):
         """Save each sequence to host memory: per record a window slot (-1: none) and, from tracker_slots (None: none),
         a tracker slot of batch_feature_track (-1: none).  Returns one blob (bytes) per record, which restore() seats in

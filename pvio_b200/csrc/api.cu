@@ -12,6 +12,7 @@
 #include "ba_linearize.cuh"
 #include "ba_schur.cuh"
 #include "ba_solve.cuh"
+#include "ba_cov.cuh"
 #include "ba_tr.cuh"
 #include "ba_update.cuh"
 
@@ -450,6 +451,7 @@ struct StepCfg {
     int fork_aux = 0;              // latency path: the non-vision candidate cost runs beside the candidate's linearisation sweep
     cudaStream_t stream = nullptr; // nullptr: the handle's stream
     const int32_t *slots = nullptr;// device list of the windows of the sweeps (PipeArgs::slots); nullptr: [w0, w0 + n)
+    int one_cta = 0;               // sweeps: one CTA per window whatever n (sweep_grid_x otherwise)
 };
 
 // what the windows [w0, w0 + n) need from the launch: worst case over the batch
@@ -569,7 +571,7 @@ static bool lin_part_fits(Handle *h, const void *k_part, const void *k_plain, in
 // speculative sweep of the trust-region loop over the CANDIDATE, into the window's other buffer set (ba_tr.cuh).
 static int launch_lin(Handle *h, int n, const StepCfg &c, const BatchShape &b, bool loss, bool victim_only, bool spec) {
     cudaStream_t st = c.stream ? c.stream : h->stream;
-    const int gx = sweep_grid_x(h, n);
+    const int gx = c.one_cta ? 1 : sweep_grid_x(h, n);
     PipeArgs a = pipe_args(h, c);
     a.victim_only = victim_only ? 1 : 0;
     a.spec = spec ? 1 : 0;
@@ -601,7 +603,7 @@ static int launch_lin(Handle *h, int n, const StepCfg &c, const BatchShape &b, b
 
 static int launch_schur(Handle *h, int n, const StepCfg &c, const BatchShape &b, bool victim_only) {
     cudaStream_t st = c.stream ? c.stream : h->stream;
-    const int gx = sweep_grid_x(h, n);
+    const int gx = c.one_cta ? 1 : sweep_grid_x(h, n);
     PipeArgs a = pipe_args(h, c);
     a.victim_only = victim_only ? 1 : 0;
     const int sgx = std::min(gx, std::max(1, (b.M + kSlab - 1) / kSlab));
@@ -638,6 +640,33 @@ int run_marg_vision(Handle *h, int n, const int32_t *h_slots, const int32_t *d_s
     c.mu = 0.0; c.compute_scale = 1; c.slots = d_slots;
     const BatchShape b = batch_shape(h, 0, n, false, h_slots);
     return run_linearize(h, n, c, b, false, true);
+}
+
+size_t cov_smem_bytes(const WinHdr &H) { return solve_smem_one(H, false); }
+
+int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L) {
+    // the solve's linearisation at the state (with the loss, either pipeline), mu = 0 in the landmark pivots; one CTA
+    // per window so that the launch count does not depend on n
+    StepCfg c;
+    c.mu = 0.0; c.compute_scale = 1; c.slots = d_slots; c.one_cta = 1;
+    const BatchShape b = batch_shape(h, 0, n, false, h_slots);
+    TRY(launch_lin(h, n, c, b, true, false, false));
+    TRY(launch_schur(h, n, c, b, false));
+    CovArgs a;
+    static_cast<SolveArgs &>(a) = launch_args<SolveArgs>(h);
+    a.alias_bias = 0; a.Hfull = nullptr; a.gfull = nullptr; a.compute_scale = 1; a.w0 = 0; a.mu_override = 0.0; a.loop = 0;
+    a.recs = L.recs; a.frames = L.frames; a.lms = L.lms; a.n_lm = L.n_lm;
+    a.cov = L.cov; a.var = L.var; a.status = L.status; a.sig = L.sig; a.sig_xi = L.sig_xi;
+    size_t smem = 0;
+    for (int i = 0; i < n; ++i) smem = std::max(smem, cov_smem_bytes(h->hdr.h[h_slots[i]]));
+    cov_kernel<<<n, 256, smem, h->stream>>>(a);
+    LAUNCH_CK(h, "cov_kernel");
+    const int blocks = std::max(1, (L.n_lm + kCovLmWarps - 1) / kCovLmWarps);
+    if (h->hs_double) cov_lm_kernel<double><<<blocks, 32 * kCovLmWarps, 0, h->stream>>>(a);
+    else cov_lm_kernel<float><<<blocks, 32 * kCovLmWarps, 0, h->stream>>>(a);
+    LAUNCH_CK(h, "cov_lm_kernel");
+    h->launches += 2;
+    return 0;
 }
 
 static int run_solve(Handle *h, int n, const StepCfg &c, const BatchShape &b) {
@@ -1138,6 +1167,7 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
         CK(h, cudaFuncSetAttribute(update_obs_kernel<double, kUpdWarps, 4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
         CK(h, cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
         CK(h, cudaFuncSetAttribute(solve_kernel_visual, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024));
+        CK(h, cudaFuncSetAttribute(cov_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
         TRY(selftest_chol_opt_in(h));
         TRY(marg_opt_in(h));
     }

@@ -503,6 +503,20 @@ void fill_summary(const WinCtrl &c, pvio_b200_summary *sm);
 // api.cu: linearise + Schur of the uploaded windows [0, n) with the fp64 pipeline, no loss (the marginaliser's reprojection part)
 // h_slots / d_slots (may be NULL): host / device copies of a list of the n windows, instead of [0, n)
 int run_marg_vision(Handle *h, int n, const int32_t *h_slots = nullptr, const int32_t *d_slots = nullptr);
+// api.cu: the covariance of the n windows of a slot list (host / device copies h_slots / d_slots): the solve's
+// linearise + Schur sweeps at the state with mu = 0, then cov_kernel and cov_lm_kernel (ba_cov.cuh) on the staged records.
+// Four launches whatever n is.
+struct CovLaunch {
+    const CovRec *recs;
+    const int32_t *frames;
+    const CovLm *lms;
+    int n_lm;
+    double *cov, *var;
+    int32_t *status;
+    double *sig, *sig_xi;
+};
+int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L);
+size_t cov_smem_bytes(const WinHdr &H);   // dynamic shared memory of cov_kernel for a window of this header
 void drop_graphs(Handle *h);
 // api.cu, for the resident batched windows (batch_window.cu)
 int ensure_inertial(Handle *h);

@@ -10,6 +10,7 @@
 //     scalars of the trust-region step.
 // Everything here is fp64: it is O(D^3/6) flops on a D <= 210 system, off the HBM-bound path.
 #pragma once
+#include <type_traits>
 #include "ba_factors.cuh"
 #include "ba_lin.cuh"
 #include "ba_tr.cuh"
@@ -31,9 +32,16 @@ constexpr int kSolveImuSlab = 15 * 30 + 16;     // raw J + r per factor
 constexpr int kImuRound = 8;                    // IMU factors linearised concurrently by solve_kernel
 constexpr int kImuJx = 15 * 32;                 // whitened Jacobian + residual column of one factor, row pitch 32
 
-template <bool kFull>
+// Cov = NoCov: the reduced-system solve of solve_kernel / solve_kernel_visual.  Otherwise the body of the covariance
+// kernel (ba_cov.cuh): window Cov::window(a), and once the system is assembled -- without regulariser, scaling or constant
+// blocks -- Cov::finish takes over.
+struct NoCov {};
+template <bool kFull, class Cov = NoCov>
 static __device__ __forceinline__ void solve_body(const SolveArgs &a) {
-    const int w = blockIdx.x + a.w0;
+    constexpr bool kCov = !std::is_same<Cov, NoCov>::value;
+    int w;
+    if constexpr (kCov) w = Cov::window(a);
+    else w = blockIdx.x + a.w0;
     const WinHdr &H = a.hdr[w];
     const WinConst &wc = a.cst[w];
     const int N = H.N;
@@ -494,6 +502,11 @@ static __device__ __forceinline__ void solve_body(const SolveArgs &a) {
             const int fi = i / stride;
             go[(compact ? __fns(freem, 0, fi + 1) : fi) * 15 + (i % stride)] = g[i];
         }
+    }
+    if constexpr (kCov) {
+        __syncthreads();
+        Cov::finish(a, w, N, stride, D, nb, A, hcorr, gu, xs, T, scr, &flag_sm);
+        return;
     }
     SOLVE_STAMP(6);
     // ---- Jacobi scale, LM diagonal, constant blocks

@@ -167,4 +167,12 @@ struct BatchArrays {
     double *pt_J;                   // [W][Tcap][6 Ncap + 2] scratch: corrected Jacobian rows of the plane tracks
 };
 
+// One record of a covariance call (pvio_b200_batch_window_covariance, ba_cov.cuh) and one of its named tracks
+struct CovRec {
+    int32_t slot, n_frames, frames_off, pad;   // frames_off: ints into the call's frame list
+    int64_t cov_off;                           // doubles into the call's frame blocks: (15 n_frames)^2
+    int64_t sig_off;                           // doubles into the call's Sigma_delta scratch: (stride N)^2
+};
+struct CovLm { int32_t rec, slot, lm, pad; };  // lm: the track's landmark in the packed window, -1: none (variance NaN)
+
 }  // namespace pvio

@@ -1847,6 +1847,90 @@ int pvio_b200_batch_window_drop_victim(pvio_b200_handle hh, int n, const int32_t
     return 0;
 }
 
+// the landmark index of every row of a slot in its packed window (rows of role < 0 with >= 2 observations, stably by
+// anchor, as bw_layout_kernel orders them), -1 for the other rows
+static std::vector<int32_t> landmark_of_rows(const WinSlot &s) {
+    const int T = (int)s.ids.size();
+    std::vector<int32_t> lm(T, -1);
+    int k = 0;
+    for (int a = 0; a < kMaxFrames; ++a)
+        for (int r = 0; r < T; ++r)
+            if (s.role[r] < 0 && __builtin_popcount(s.mask[r]) >= 2 && __builtin_ctz(s.mask[r]) == a) lm[r] = k++;
+    return lm;
+}
+
+int pvio_b200_batch_window_covariance(pvio_b200_handle hh, int n, pvio_b200_window_covariance *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const char *what = "batch_window_covariance";
+    auto bad = [&](const char *why) { return fail(h, PVIO_B200_EINVAL, (std::string(what) + ": " + why).c_str()); };
+    if (n < 0 || (n > 0 && !records)) return bad("bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n), frames;
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_covariance: bad slot list"));
+    // every record checked against its slot's host mirror before anything is staged
+    std::vector<CovRec> recs(n);
+    std::vector<CovLm> lms;
+    int64_t cov_n = 0, sig_n = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_covariance &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (s.N < 1) return bad("a window without frames");
+        if (R.n_frames < 0 || R.n_frames > s.N || R.n_tracks < 0 || R.n_tracks > (int)s.ids.size())
+            return bad("a frame or track count out of range");
+        if (R.n_frames == 0 && R.n_tracks == 0) return bad("a record asking for nothing");
+        if (R.n_frames > 0 && (!R.frames || !R.cov)) return bad("frames or cov missing");
+        if (R.n_tracks > 0 && (!R.tracks || !R.inv_depth_var)) return bad("tracks or inv_depth_var missing");
+        uint32_t seen = 0;
+        for (int k = 0; k < R.n_frames; ++k) {
+            const int f = R.frames[k];
+            if (f < 0 || f >= s.N) return bad("a frame out of range");
+            if ((seen >> f) & 1u) return bad("a frame named twice");
+            seen |= 1u << f;
+        }
+        if (cov_smem_bytes(h->hdr.h[R.slot]) > 220 * 1024) return bad("reduced system too large for shared memory");
+        const std::vector<int32_t> lm = R.n_tracks > 0 ? landmark_of_rows(s) : std::vector<int32_t>();
+        std::vector<uint8_t> taken(s.ids.size(), 0);
+        for (int k = 0; k < R.n_tracks; ++k) {
+            const auto it = std::lower_bound(s.ids.begin(), s.ids.end(), R.tracks[k]);      // rows are in id order
+            if (it == s.ids.end() || *it != R.tracks[k]) return bad("a track that is not live in its slot");
+            const size_t r = it - s.ids.begin();
+            if (taken[r]) return bad("a track named twice");
+            taken[r] = 1;
+            lms.push_back(CovLm{i, R.slot, lm[r], 0});
+        }
+        const int64_t D = (s.inertial ? 15 : 6) * (int64_t)s.N;
+        recs[i] = CovRec{R.slot, R.n_frames, (int32_t)frames.size(), 0, cov_n, sig_n};
+        frames.insert(frames.end(), R.frames, R.frames + R.n_frames);
+        cov_n += 225 * (int64_t)R.n_frames * R.n_frames;
+        sig_n += D * D;
+    }
+    const int n_lm = (int)lms.size();
+    Stage S(h->bw.stage, &h->bw.scratch);
+    const auto rec = S.up(recs);
+    const auto fr = S.up(frames);
+    const auto lmv = S.up(lms);
+    const auto sl = S.add(Stage::kUp, n, slots.data());
+    const auto cov = S.add<double>(Stage::kDown, (size_t)cov_n), var = S.add<double>(Stage::kDown, (size_t)n_lm);
+    const auto st = S.add<int32_t>(Stage::kDown, n);
+    const auto sig = S.add<double>(Stage::kScratch, (size_t)sig_n);
+    const auto sxi = S.add<double>(Stage::kScratch, (size_t)n * h->Ncap * h->Ncap * 36);
+    TRY(S.place(h, true));
+    TRY(run_covariance(h, n, slots.data(), S.dev(sl),
+                       CovLaunch{S.dev(rec), S.dev(fr), S.dev(lmv), n_lm, S.dev(cov), S.dev(var), S.dev(st), S.dev(sig), S.dev(sxi)}));
+    TRY(S.download(h));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0, t = 0; i < n; ++i) {
+        pvio_b200_window_covariance &R = records[i];
+        if (R.n_frames > 0) memcpy(R.cov, S.host(cov) + recs[i].cov_off, sizeof(double) * 225 * R.n_frames * R.n_frames);
+        if (R.n_tracks > 0) memcpy(R.inv_depth_var, S.host(var) + t, sizeof(double) * R.n_tracks);
+        t += R.n_tracks;
+        R.status = S.host(st)[i];
+    }
+    return 0;
+}
+
 int pvio_b200_batch_window_download(pvio_b200_handle hh, int n, const int32_t *slots, int32_t *n_frames, double *frames,
                                     int64_t frames_stride, int32_t *n_tracks, int64_t track_stride, int32_t *track_id,
                                     double *inv_depth, int32_t *anchor_frame, int32_t *n_observations, uint8_t *valid,
