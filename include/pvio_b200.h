@@ -896,6 +896,74 @@ typedef struct pvio_b200_imu_stream_snapshot {
 int pvio_b200_batch_imu_stream_save(pvio_b200_handle h, int n, pvio_b200_imu_stream_snapshot *records);
 int pvio_b200_batch_imu_stream_restore(pvio_b200_handle h, int n, const pvio_b200_imu_stream_snapshot *records);
 
+/* The covariance of a stream slot's latest state, for the IMU-rate pose's covariance (pvio_b200_batch_imu_stream_predict).
+ * Coordinates are those of pvio_b200_batch_window_covariance: [dtheta dp dv dbg dba], q perturbed on the right,
+ * q (x) exp(dtheta).  A record seeds its slot's current latest state, whose time must be state_time:
+ *  - PVIO_B200_IMU_STREAM_COV_DIRECT: cov is that state's covariance.
+ *  - PVIO_B200_IMU_STREAM_COV_FACTOR: the state is the `predicted` of track_camera / mirror_frame / track_frame
+ *    (PreIntegrator::predict from the window's newest frame through the new frame's factor), cov is the covariance of
+ *    that source frame (pvio_b200_batch_window_covariance after the solve) and imu_record the factor returned with
+ *    `predicted`.  The device forms Phi cov Phi^T + Psi Sigma_d Psi^T: Phi the Jacobian of predict(integrate) with
+ *    respect to the source state, its bias columns through the record's dq_dbg .. dv_dba; Sigma_d = (U^T U)^-1 with U the
+ *    record's sqrt_inv_cov (upper triangular; its strict lower part is not read); Psi = diag(I, R, R, I, I), so the
+ *    factor's bias random walk enters the predicted biases.  R, the source rotation, is that of q_state (x) dq^-1.
+ * noise_cov [4][9] (cov_w, cov_a, cov_bg, cov_ba, 3 x 3 row-major) is what predict propagates with.  The device keeps the
+ * symmetrised matrix.  A seed holds until the slot's latest state changes: any later SET record (even of the same
+ * state), CLEAR, pvio_b200_batch_imu_stream_reset or pvio_b200_batch_imu_stream_restore of the slot drops it.  Seeds are
+ * not part of the stream blobs: after a restore the caller seeds the slot again.
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no seed has changed.
+ * Rejected: n < 0; a slot out of range, named twice or never reset; a slot without a latest state or whose state time
+ * is not state_time; an unknown mode; a NULL cov, noise_cov or (FACTOR) imu_record; a value that is not finite; a cov
+ * that is not symmetric to 1e-12 of its largest entry or has a negative diagonal; (FACTOR) a zero diagonal in
+ * sqrt_inv_cov.
+ * Launches, whatever n is: one host -> device copy, one kernel (one warp per record), one synchronisation. */
+#define PVIO_B200_IMU_STREAM_COV_DIRECT 0
+#define PVIO_B200_IMU_STREAM_COV_FACTOR 1
+typedef struct pvio_b200_imu_stream_cov_seed {
+    int32_t slot;
+    int32_t mode;                     /* PVIO_B200_IMU_STREAM_COV_DIRECT / FACTOR */
+    double state_time;                /* the slot's latest-state time */
+    const double *cov;                /* [225] row-major: the state's (DIRECT) or the source frame's (FACTOR) */
+    const double *imu_record;         /* FACTOR: [PVIO_B200_IMU_STRIDE] the factor returned with `predicted` */
+    const double *noise_cov;          /* [4][9] cov_w, cov_a, cov_bg, cov_ba */
+} pvio_b200_imu_stream_cov_seed;      /* 40 bytes on LP64 */
+int pvio_b200_batch_imu_stream_set_covariance(pvio_b200_handle h, int n, const pvio_b200_imu_stream_cov_seed *records);
+
+/* The IMU-rate pose of stream slots at any times, with its covariance; changes no slot.  Per record, n_times
+ * non-decreasing times; for each time t:
+ *  - poses: the OutputPose the slot's predict_pose(t) gives as the slot stands, bit for bit (the latest state propagated
+ *    with propagate_state over the kept samples with t_k <= t, then the output extrinsic).  A state that no pose has
+ *    read yet skips, rather than drops, the kept samples up to its time.
+ *  - states (or NULL): the propagated body state [16] q xyzw, p, v, bg, ba.
+ *  - state_cov (or NULL): the seeded covariance propagated to first order along the same chain.  The sample at t_k drives
+ *    the interval (t_{k-1}, t_k]; PreIntegrator::increment's noise discretisation: cov_w / max(dt, 1e-7) through
+ *    dt Jr((w - bg) dt) into dtheta, cov_a / max(dt, 1e-7) through dt R and dt^2 R / 2 into dv and dp, cov_bg dt and
+ *    cov_ba dt into the bias blocks.
+ *  - pose_cov (or NULL): [dtheta_out dp_out] of the OutputPose, q_out = q q_ob and p_out = p + q p_ob perturbed as q:
+ *    dtheta_out = R_ob^T dtheta, dp_out = dp - R hat(p_ob) dtheta.
+ *  - status: PVIO_B200_OK; PVIO_B200_IMU_STREAM_NO_STATE (no latest state: zero poses and states, NaN covariances);
+ *    PVIO_B200_IMU_STREAM_NO_COVARIANCE (no seed for the current state: poses and states, NaN covariances).
+ * Covariance outputs are exactly symmetric.
+ * Every record is checked before anything is staged: on PVIO_B200_EINVAL no output has changed.
+ * Rejected: n < 0; a slot out of range, named twice or never reset; n_times < 0; a NULL times or poses with n_times > 0;
+ * a time that is not finite; decreasing times.
+ * Launches, whatever n is: one host -> device copy, one kernel (one warp per record), one device -> host copy, one
+ * synchronisation. */
+#define PVIO_B200_IMU_STREAM_NO_STATE 1
+#define PVIO_B200_IMU_STREAM_NO_COVARIANCE 2
+typedef struct pvio_b200_imu_stream_predict {
+    int32_t slot;
+    int32_t n_times;
+    const double *times;              /* [n_times], non-decreasing */
+    double *poses;                    /* out [n_times][7] q xyzw, p */
+    double *states;                   /* out [n_times][16] or NULL */
+    double *pose_cov;                 /* out [n_times][36] or NULL */
+    double *state_cov;                /* out [n_times][225] or NULL */
+    int32_t status;                   /* out */
+    int32_t pad;
+} pvio_b200_imu_stream_predict;       /* 56 bytes on LP64 */
+int pvio_b200_batch_imu_stream_predict(pvio_b200_handle h, int n, pvio_b200_imu_stream_predict *records);
+
 int pvio_b200_sync(pvio_b200_handle h);
 /* CUDA-event timing on the handle's stream (bench.py): start / stop return ms. */
 int pvio_b200_timer_start(pvio_b200_handle h);

@@ -31,6 +31,8 @@ IMU_EVENT_GYROSCOPE, IMU_EVENT_ACCELEROMETER, IMU_EVENT_CAMERA = 0, 1, 2
 IMU_STREAM_KEEP, IMU_STREAM_SET, IMU_STREAM_CLEAR = 0, 1, 2
 IMU_STREAM_MAX_QUEUE = 65536
 IMU_STREAM_SNAPSHOT_MAGIC, IMU_STREAM_SNAPSHOT_VERSION = 1397315152, 1
+IMU_STREAM_COV_DIRECT, IMU_STREAM_COV_FACTOR = 0, 1
+IMU_STREAM_NO_STATE, IMU_STREAM_NO_COVARIANCE = 1, 2
 
 c_i32p = C.POINTER(C.c_int32)
 c_u8p = C.POINTER(C.c_uint8)
@@ -191,6 +193,16 @@ class CImuStreamSnapshot(C.Structure):
     _fields_ = [("slot", C.c_int32), ("pad", C.c_int32), ("data", c_u8p), ("capacity", C.c_int64), ("size", C.c_int64)]
 
 
+class CImuStreamCovSeed(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("mode", C.c_int32), ("state_time", C.c_double), ("cov", c_f64p),
+                ("imu_record", c_f64p), ("noise_cov", c_f64p)]
+
+
+class CImuStreamPredict(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n_times", C.c_int32), ("times", c_f64p), ("poses", c_f64p), ("states", c_f64p),
+                ("pose_cov", c_f64p), ("state_cov", c_f64p), ("status", C.c_int32), ("pad", C.c_int32)]
+
+
 class CLens(C.Structure):
     _fields_ = [("slot", C.c_int32), ("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
@@ -268,6 +280,8 @@ SIGNATURES = {
     "pvio_b200_batch_imu_stream": (_int, [_h, _int, _P(CImuStreamRecord)]),
     "pvio_b200_batch_imu_stream_save": (_int, [_h, _int, _P(CImuStreamSnapshot)]),
     "pvio_b200_batch_imu_stream_restore": (_int, [_h, _int, _P(CImuStreamSnapshot)]),
+    "pvio_b200_batch_imu_stream_set_covariance": (_int, [_h, _int, _P(CImuStreamCovSeed)]),
+    "pvio_b200_batch_imu_stream_predict": (_int, [_h, _int, _P(CImuStreamPredict)]),
     "pvio_b200_sync": (_int, [_h]),
     "pvio_b200_timer_start": (_int, [_h]),
     "pvio_b200_timer_stop": (_int, [_h, c_f32p]),

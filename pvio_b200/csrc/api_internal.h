@@ -182,12 +182,20 @@ struct ImuStreamHost {
     int64_t g = 0, a = 0, s = 0, f = 0, k = 0;   // queue sizes: gyroscope, accelerometer, unreleased samples, pending
                                                  // frames, kept samples
 };
+// The latest state's covariance seed of one stream slot (pvio_b200_batch_imu_stream_set_covariance).  gen counts the
+// changes of the slot's latest state (SET and CLEAR records, reset, restore); the seed holds while seed_gen == gen.
+struct ImuStreamCovHost {
+    int64_t gen = 0, seed_gen = -1;
+    double state_t = 0;               // the latest state's time (while ImuStreamHost::has_state)
+};
 struct ImuStreams {
     int slots = 0;                    // slots allocated on the device
     int qcap = 0;                     // rows per queue per slot
     std::vector<ImuStreamHost> host;
+    std::vector<ImuStreamCovHost> cov_host;   // sized with host
     DevBuf<uint8_t> hdr;              // [slots] ImuStreamSlot (imu_stream.cu)
     DevBuf<double> g, a, s, f, k;     // [slots][qcap][4 / 4 / 7 / 1 / 7]
+    DevBuf<double> cov;               // [slots][kStreamCovStride] the seeded covariance, noise_cov and state time
     DevBuf<uint8_t> stage;            // both sides: records and events (uploaded) | outputs (downloaded)
 };
 

@@ -20,6 +20,7 @@ namespace {
 
 constexpr double kGravityNominal = 9.80665;           // PVIO_GRAVITY_NOMINAL, common.h:62
 constexpr int kMinQcap = 16;
+constexpr int kStreamCovStride = 264;                 // ImuStreams::cov per slot: P [225], noise_cov [36], state time, pad
 
 // one stream slot on the device: output extrinsic, latest state, the previously released frame's last row, and where
 // each queue's live rows are in the slot's part of ImuStreams::g / a / s / f / k
@@ -275,6 +276,13 @@ int ensure_streams(Handle *h, int slots, int qcap) {
     DevBuf<uint8_t> hdr;
     TRY(alloc(h, hdr, sizeof(ImuStreamSlot) * ns, kDevice));
     if (M.slots) CK(h, cudaMemcpyAsync(hdr.d, M.hdr.d, sizeof(ImuStreamSlot) * M.slots, cudaMemcpyDeviceToDevice, h->stream));
+    DevBuf<double> cov;
+    if (ns > M.slots) {
+        TRY(alloc(h, cov, (size_t)ns * kStreamCovStride, kDevice));
+        if (M.slots)
+            CK(h, cudaMemcpyAsync(cov.d, M.cov.d, sizeof(double) * kStreamCovStride * M.slots, cudaMemcpyDeviceToDevice,
+                                  h->stream));
+    }
     DevBuf<double> *qs[5] = {&M.g, &M.a, &M.s, &M.f, &M.k};
     const int width[5] = {4, 4, 7, 1, 7};
     DevBuf<double> grown[5];
@@ -286,6 +294,7 @@ int ensure_streams(Handle *h, int slots, int qcap) {
     }
     CK(h, cudaStreamSynchronize(h->stream));
     M.hdr = std::move(hdr);
+    if (ns > M.slots) M.cov = std::move(cov);
     for (int q = 0; q < 5; ++q) *qs[q] = std::move(grown[q]);
     M.slots = ns;
     M.qcap = nq;
@@ -331,9 +340,11 @@ int stream_reset_impl(Handle *h, int n, const int32_t *slots, const double *oq, 
     CK(h, cudaGetLastError());
     CK(h, cudaStreamSynchronize(st));
     if ((size_t)top > M.host.size()) M.host.resize(top);
+    M.cov_host.resize(M.host.size());
     for (int i = 0; i < n; ++i) {
         M.host[slots[i]] = ImuStreamHost{};
         M.host[slots[i]].set = true;
+        ++M.cov_host[slots[i]].gen;
     }
     return 0;
 }
@@ -486,6 +497,10 @@ int stream_impl(Handle *h, int n, pvio_b200_imu_stream_record *recs) {
         ImuStreamHost &S = M.host[r.slot];
         if (r.state_op == PVIO_B200_IMU_STREAM_SET) S.has_state = true;
         if (r.state_op == PVIO_B200_IMU_STREAM_CLEAR) S.has_state = false;
+        if (r.state_op != PVIO_B200_IMU_STREAM_KEEP) {       // the seed of the previous state no longer holds
+            ++M.cov_host[r.slot].gen;
+            M.cov_host[r.slot].state_t = r.state_time;
+        }
         for (int e = 0; e < O.n_consumed; ++e) {
             const double *evr = r.events + (size_t)e * 5;
             if (evr[0] == PVIO_B200_IMU_EVENT_GYROSCOPE) { S.seen_g = true; S.last_g = evr[1]; }
@@ -753,8 +768,12 @@ int stream_restore_impl(Handle *h, int n, const pvio_b200_imu_stream_snapshot *r
     CK(h, cudaGetLastError());
     CK(h, cudaStreamSynchronize(st));
     if ((size_t)top > M.host.size()) M.host.resize(top);
+    M.cov_host.resize(M.host.size());
     for (int i = 0; i < n; ++i) {
         const StreamSnapHead &H = heads[i];
+        ImuStreamCovHost &C = M.cov_host[recs[i].slot];
+        ++C.gen;
+        C.state_t = H.dev.state_t;
         ImuStreamHost &S = M.host[recs[i].slot];
         S.set = true;
         S.has_state = H.dev.has_state;
@@ -766,6 +785,472 @@ int stream_restore_impl(Handle *h, int n, const pvio_b200_imu_stream_snapshot *r
     return 0;
 }
 
+
+// ------------------------------------------------------------ covariance (pvio_b200_batch_imu_stream_set_covariance / predict)
+// A slot's seed (ImuStreams::cov) is the covariance of its latest state in [dtheta dp dv dbg dba], q perturbed on the
+// right, with the noise_cov the prediction propagates with.  Both kernels run one warp per record on 15 x 15 matrices in
+// shared memory (row-major).
+constexpr int kCovWarps = 4;                          // records per CTA
+
+struct StreamSeedRec {                // one set_covariance record as staged
+    int32_t slot, mode;
+    double state_t;
+    double cov[225];
+    double imu[PVIO_B200_IMU_STRIDE];  // FACTOR: the factor of the prediction
+    double noise[36];
+};
+
+// C = A B (bt: A B^T), 15 x 15, by the warp's lanes
+__device__ void warp_mm15(const double *A, const double *B, double *C, bool bt, int lane) {
+    for (int e = lane; e < 225; e += 32) {
+        const int i = e / 15, j = e % 15;
+        double s = 0.0;
+        for (int m = 0; m < 15; ++m) s += A[i * 15 + m] * (bt ? B[j * 15 + m] : B[m * 15 + j]);
+        C[e] = s;
+    }
+    __syncwarp();
+}
+
+// 3 x 3 block (bi, bj) of the 15 x 15 M set to s X (X row-major 3 x 3, or the identity when null)
+__device__ void put_block(double *M, int bi, int bj, const double *X, double s = 1.0) {
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) M[(3 * bi + r) * 15 + 3 * bj + c] = X ? s * X[3 * r + c] : (r == c ? s : 0.0);
+}
+
+// One warp per record.  DIRECT: the symmetrised cov.  FACTOR: Phi Sigma_src Phi^T + Psi Sigma_d Psi^T (header), with
+// Sigma_d = U^-1 U^-T from the factor's upper-triangular U = sqrt_inv_cov.
+__global__ void __launch_bounds__(32 * kCovWarps) imu_stream_seed_kernel(int n, const StreamSeedRec *recs,
+                                                                         const ImuStreamSlot *hdr, double *cov) {
+    __shared__ double sm[kCovWarps][4][225];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * kCovWarps + w;
+    if (i >= n) return;
+    const StreamSeedRec &R = recs[i];
+    double *A = sm[w][0], *B = sm[w][1], *C = sm[w][2], *D = sm[w][3];
+    for (int e = lane; e < 225; e += 32) {
+        const int r = e / 15, c = e % 15;
+        A[e] = 0.5 * (R.cov[r * 15 + c] + R.cov[c * 15 + r]);
+        B[e] = 0.0;
+        D[e] = 0.0;
+    }
+    __syncwarp();
+    if (R.mode == PVIO_B200_IMU_STREAM_COV_FACTOR) {
+        const double *rec = R.imu, *dq = rec + PVIO_B200_IMU_DQ, T = rec[PVIO_B200_IMU_DT];
+        double qs[4], Rs[9], dR[9];
+        {
+            double ci[4];
+            quat_conj(dq, ci);
+            quat_mul(hdr[R.slot].state, ci, qs);
+            quat_to_mat(qs, Rs);
+            quat_to_mat(dq, dR);
+        }
+        if (lane == 0) {                                 // Phi into B
+            double H[9], X[9], Xt[9];
+            for (int r = 0; r < 3; ++r)
+                for (int c = 0; c < 3; ++c) Xt[3 * r + c] = dR[3 * c + r];
+            put_block(B, 0, 0, Xt);
+            put_block(B, 0, 3, rec + PVIO_B200_IMU_DQ_DBG);
+            hat(rec + PVIO_B200_IMU_DP, H);
+            mat3_mul(Rs, H, X);
+            put_block(B, 1, 0, X, -1.0);
+            put_block(B, 1, 1, nullptr);
+            put_block(B, 1, 2, nullptr, T);
+            mat3_mul(Rs, rec + PVIO_B200_IMU_DP_DBG, X);
+            put_block(B, 1, 3, X);
+            mat3_mul(Rs, rec + PVIO_B200_IMU_DP_DBA, X);
+            put_block(B, 1, 4, X);
+            hat(rec + PVIO_B200_IMU_DV, H);
+            mat3_mul(Rs, H, X);
+            put_block(B, 2, 0, X, -1.0);
+            put_block(B, 2, 2, nullptr);
+            mat3_mul(Rs, rec + PVIO_B200_IMU_DV_DBG, X);
+            put_block(B, 2, 3, X);
+            mat3_mul(Rs, rec + PVIO_B200_IMU_DV_DBA, X);
+            put_block(B, 2, 4, X);
+            put_block(B, 3, 3, nullptr);
+            put_block(B, 4, 4, nullptr);
+        }
+        __syncwarp();
+        warp_mm15(B, A, C, false, lane);                 // Phi Sigma_src
+        warp_mm15(C, B, A, true, lane);                  // .. Phi^T, into A
+        if (lane < 15) {                                 // column `lane` of U^-1 into C, by back substitution
+            const double *U = rec + PVIO_B200_IMU_SQRT_INV_COV;
+            const int j = lane;
+            for (int r = 14; r > j; --r) C[r * 15 + j] = 0.0;
+            C[j * 15 + j] = 1.0 / U[j * 15 + j];
+            for (int r = j - 1; r >= 0; --r) {
+                double s = 0.0;
+                for (int m = r + 1; m <= j; ++m) s += U[r * 15 + m] * C[m * 15 + j];
+                C[r * 15 + j] = -s / U[r * 15 + r];
+            }
+        }
+        __syncwarp();
+        warp_mm15(C, C, D, true, lane);                  // Sigma_d = U^-1 U^-T
+        if (lane == 0) {                                 // Psi into B
+            for (int e = 0; e < 225; ++e) B[e] = 0.0;
+            put_block(B, 0, 0, nullptr);
+            put_block(B, 1, 1, Rs);
+            put_block(B, 2, 2, Rs);
+            put_block(B, 3, 3, nullptr);
+            put_block(B, 4, 4, nullptr);
+        }
+        __syncwarp();
+        warp_mm15(B, D, C, false, lane);                 // Psi Sigma_d
+        warp_mm15(C, B, D, true, lane);                  // .. Psi^T, into D
+    }
+    double *out = cov + (size_t)R.slot * kStreamCovStride;
+    for (int e = lane; e < 225; e += 32) {
+        const int r = e / 15, c = e % 15;
+        out[e] = 0.5 * ((A[e] + D[e]) + (A[c * 15 + r] + D[c * 15 + r]));
+    }
+    for (int e = lane; e < 36; e += 32) out[225 + e] = R.noise[e];
+    if (lane == 0) { out[261] = R.state_t; out[262] = out[263] = 0.0; }
+}
+
+struct StreamPredRec {                // one predict record as staged
+    int32_t slot, n_times, has_cov, pad;
+    int64_t t_at;                     // its first time in the call's times
+    int64_t pose_at, state_at, pcov_at, scov_at;   // its first row in each output section; -1: not asked
+};
+struct StreamPredArgs {
+    const ImuStreamSlot *hdr;
+    const double *k, *cov;
+    int qcap;
+    const StreamPredRec *recs;
+    const double *times;
+    double *poses, *states, *pcov, *scov;         // [*][7], [*][16], [*][36], [*][225]
+    int n;
+};
+constexpr int kStepVals = 96;         // per warp: one step's F and noise blocks, the emit's blocks, the seed's noise_cov
+
+// One warp per record.  Every lane runs the pose chain of imu_stream_kernel's predict (the same operations in the same
+// order, so the same bits); lane 0 writes each step's blocks of F and of the noise, and the lanes propagate P:
+// F = I + [theta: E^T, -dt Jr at bg; p: -dt^2/2 R hat(a), dt I at v, -dt^2/2 R at ba; v: -dt R hat(a), -dt R at ba],
+// P <- F P F^T as two column passes (Y = F P, then F Y^T) that each touch only the theta, p and v rows, then the exact
+// symmetrisation plus the noise.  Outputs as the chain passes each requested time.
+__global__ void __launch_bounds__(32 * kCovWarps) imu_stream_predict_kernel(StreamPredArgs A) {
+    __shared__ double sm[kCovWarps][2][225];
+    __shared__ double sv[kCovWarps][kStepVals];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * kCovWarps + w;
+    if (i >= A.n) return;
+    const StreamPredRec &R = A.recs[i];
+    const ImuStreamSlot &S = A.hdr[R.slot];
+    const bool has_state = S.has_state != 0, has_cov = has_state && R.has_cov;
+    double *P = sm[w][0], *Y = sm[w][1], *V = sv[w];
+    // V: [0] R, [9] R hat(a), [18] E^T, [27] dt Jr, [36] Nw, [45] Na (3 x 3 each), [54] dt, [55] R_ob, [64] R hat(p_ob),
+    // [73] noise_cov bg, [82] ba
+    double *Rv = V, *Mv = V + 9, *Et = V + 18, *Jv = V + 27, *Nw = V + 36, *Na = V + 45, *Rob = V + 55, *Kp = V + 64;
+    const double *seed = A.cov + (size_t)R.slot * kStreamCovStride;
+    if (has_cov) {
+        for (int e = lane; e < 225; e += 32) P[e] = seed[e];
+        if (lane < 18) V[73 + lane] = seed[225 + 18 + lane];
+        if (lane == 0) quat_to_mat(S.q_ob, Rob);
+    }
+    __syncwarp();
+    const double *K = A.k + ((size_t)R.slot * A.qcap + S.k0) * 7;
+    const int kn = S.kn;
+    const double state_t = S.state_t;
+    int c = 0;
+    if (has_state && S.drop_pending)                    // predict_pose :149-151, skipped: the call changes no slot
+        while (c < kn && K[c * 7] <= state_t) ++c;
+    double ct = state_t, cq[4], cp[3], cv[3];
+    for (int j = 0; j < 4; ++j) cq[j] = S.state[j];
+    for (int j = 0; j < 3; ++j) { cp[j] = S.state[4 + j]; cv[j] = S.state[7 + j]; }
+    const double *bg = S.state + 10, *ba = S.state + 13;
+    const double nan = __longlong_as_double(0x7ff8000000000000LL);
+    for (int q = 0; q < R.n_times; ++q) {
+        const double t = A.times[R.t_at + q];
+        for (; has_state && c < kn && K[c * 7] <= t; ++c) {   // propagate_state, core.cpp:32-39
+            const double *r = K + c * 7;
+            const double dt = r[0] - ct;
+            const double d[3] = {r[4] - ba[0], r[5] - ba[1], r[6] - ba[2]};
+            double ra[3];
+            bw_qrot(cq, d, ra);
+            const double acc[3] = {0.0 + ra[0], 0.0 + ra[1], -kGravityNominal + ra[2]};
+            const double hdt = 0.5 * dt * dt;
+            if (has_cov && lane == 0) {                  // the step's blocks, at the old rotation
+                double H[9], Jr[9], X[9];
+                const double u[3] = {(r[1] - bg[0]) * dt, (r[2] - bg[1]) * dt, (r[3] - bg[2]) * dt};
+                quat_to_mat(cq, Rv);
+                hat(d, H);
+                mat3_mul(Rv, H, Mv);
+                double e[4], Em[9];
+                expmap(u, e);
+                quat_to_mat(e, Em);
+                for (int a = 0; a < 3; ++a)
+                    for (int b = 0; b < 3; ++b) Et[3 * a + b] = Em[3 * b + a];
+                right_jacobian(u, Jr);
+                for (int j = 0; j < 9; ++j) Jv[j] = dt * Jr[j];
+                const double inv_dt = 1.0 / fmax(dt, 1.0e-7);
+                mat3_mul(Jv, seed + 225, X);             // dt Jr cov_w (dt Jr)^T / max(dt, 1e-7)
+                for (int a = 0; a < 3; ++a)
+                    for (int b = 0; b < 3; ++b)
+                        Nw[3 * a + b] = (X[3 * a] * Jv[3 * b] + X[3 * a + 1] * Jv[3 * b + 1] + X[3 * a + 2] * Jv[3 * b + 2]) * inv_dt;
+                mat3_mul(Rv, seed + 234, X);             // R cov_a R^T / max(dt, 1e-7)
+                for (int a = 0; a < 3; ++a)
+                    for (int b = 0; b < 3; ++b)
+                        Na[3 * a + b] = (X[3 * a] * Rv[3 * b] + X[3 * a + 1] * Rv[3 * b + 1] + X[3 * a + 2] * Rv[3 * b + 2]) * inv_dt;
+                V[54] = dt;
+            }
+            for (int j = 0; j < 3; ++j) {
+                cp[j] = cp[j] + dt * cv[j] + hdt * acc[j];
+                cv[j] = cv[j] + dt * acc[j];
+            }
+            const double u[3] = {(r[1] - bg[0]) * dt, (r[2] - bg[1]) * dt, (r[3] - bg[2]) * dt};
+            double e[4], qn[4];
+            expmap(u, e);
+            eigen_qmul(cq, e, qn);
+            const double nrm = sqrt(qn[0] * qn[0] + qn[1] * qn[1] + qn[2] * qn[2] + qn[3] * qn[3]);
+            for (int j = 0; j < 4; ++j) cq[j] = qn[j] / nrm;
+            ct = r[0];
+            if (!has_cov) continue;
+            __syncwarp();
+            for (int pass = 0; pass < 2; ++pass) {       // Y = F P (columns of P), then P = F Y^T (rows of Y)
+                const double *src = pass ? Y : P;
+                double *dst = pass ? P : Y;
+                if (lane < 15) {
+                    const int so = pass ? 15 * lane : lane, ss = pass ? 1 : 15;    // the vector's start and stride
+                    double x[15];
+                    for (int j = 0; j < 15; ++j) x[j] = src[so + ss * j];
+                    const double h2 = 0.5 * V[54] * V[54], t1 = V[54];
+                    double o[9];
+                    for (int a = 0; a < 3; ++a) {
+                        double th = Et[3 * a] * x[0] + Et[3 * a + 1] * x[1] + Et[3 * a + 2] * x[2];
+                        th = th - (Jv[3 * a] * x[9] + Jv[3 * a + 1] * x[10] + Jv[3 * a + 2] * x[11]);
+                        const double mt = Mv[3 * a] * x[0] + Mv[3 * a + 1] * x[1] + Mv[3 * a + 2] * x[2];
+                        const double rb = Rv[3 * a] * x[12] + Rv[3 * a + 1] * x[13] + Rv[3 * a + 2] * x[14];
+                        o[a] = th;
+                        o[3 + a] = x[3 + a] - h2 * mt + t1 * x[6 + a] - h2 * rb;
+                        o[6 + a] = x[6 + a] - t1 * mt - t1 * rb;
+                    }
+                    const int dso = lane, dss = 15;      // written as column `lane`
+                    for (int j = 0; j < 9; ++j) dst[dso + dss * j] = o[j];
+                    for (int j = 9; j < 15; ++j) dst[dso + dss * j] = x[j];
+                }
+                __syncwarp();
+            }
+            for (int e = lane; e < 225; e += 32) {       // symmetrise and add the noise, each pair by one lane
+                const int a = e / 15, b = e % 15;
+                if (a > b) continue;
+                const int ba_ = a / 3, bb = b / 3, k3 = 3 * (a % 3) + b % 3;
+                const double dt = V[54];
+                double nz = 0.0;
+                if (ba_ == 0 && bb == 0) nz = Nw[k3];
+                else if (ba_ == 1 && bb == 1) nz = 0.25 * dt * dt * dt * dt * Na[k3];
+                else if (ba_ == 1 && bb == 2) nz = 0.5 * dt * dt * dt * Na[k3];
+                else if (ba_ == 2 && bb == 2) nz = dt * dt * Na[k3];
+                else if (ba_ == 3 && bb == 3) nz = V[73 + k3] * dt;
+                else if (ba_ == 4 && bb == 4) nz = V[82 + k3] * dt;
+                const double v = 0.5 * (P[a * 15 + b] + P[b * 15 + a]) + nz;
+                P[a * 15 + b] = v;
+                P[b * 15 + a] = v;
+            }
+            __syncwarp();
+        }
+        // outputs at t
+        if (lane == 0) {
+            double *o = A.poses + (R.pose_at + q) * 7;
+            if (!has_state) {
+                for (int j = 0; j < 7; ++j) o[j] = 0.0;
+            } else {
+                double qo[4], rp[3];
+                eigen_qmul(cq, S.q_ob, qo);              // :158-159
+                bw_qrot(cq, S.p_ob, rp);
+                for (int j = 0; j < 4; ++j) o[j] = qo[j];
+                for (int j = 0; j < 3; ++j) o[4 + j] = cp[j] + rp[j];
+            }
+            if (R.state_at >= 0) {
+                double *st = A.states + (R.state_at + q) * 16;
+                for (int j = 0; j < 4; ++j) st[j] = has_state ? cq[j] : 0.0;
+                for (int j = 0; j < 3; ++j) {
+                    st[4 + j] = has_state ? cp[j] : 0.0;
+                    st[7 + j] = has_state ? cv[j] : 0.0;
+                    st[10 + j] = has_state ? bg[j] : 0.0;
+                    st[13 + j] = has_state ? ba[j] : 0.0;
+                }
+            }
+            if (has_cov && R.pcov_at >= 0) {             // R hat(p_ob)
+                double Rc[9], H[9];
+                quat_to_mat(cq, Rc);
+                hat(S.p_ob, H);
+                mat3_mul(Rc, H, Kp);
+            }
+        }
+        if (R.scov_at >= 0) {
+            double *o = A.scov + (R.scov_at + q) * 225;
+            for (int e = lane; e < 225; e += 32) o[e] = has_cov ? P[e] : nan;
+        }
+        if (R.pcov_at >= 0) {
+            double *o = A.pcov + (R.pcov_at + q) * 36;
+            if (has_cov) {
+                __syncwarp();
+                // J = [[R_ob^T, 0], [-R hat(p_ob), I]] over [dtheta dp]; Y <- J P[0:6, 0:6] J^T, then exactly symmetric
+                for (int e = lane; e < 36; e += 32) {
+                    const int a = e / 6, b = e % 6;
+                    double ja[6], jb[6];
+                    for (int m = 0; m < 3; ++m) {
+                        ja[m] = a < 3 ? Rob[3 * m + a] : -Kp[3 * (a - 3) + m];
+                        ja[3 + m] = a < 3 ? 0.0 : (a - 3 == m ? 1.0 : 0.0);
+                        jb[m] = b < 3 ? Rob[3 * m + b] : -Kp[3 * (b - 3) + m];
+                        jb[3 + m] = b < 3 ? 0.0 : (b - 3 == m ? 1.0 : 0.0);
+                    }
+                    double s = 0.0;
+                    for (int m = 0; m < 6; ++m) {
+                        double r = 0.0;
+                        for (int k2 = 0; k2 < 6; ++k2) r += P[m * 15 + k2] * jb[k2];
+                        s += ja[m] * r;
+                    }
+                    Y[e] = s;
+                }
+                __syncwarp();
+                for (int e = lane; e < 36; e += 32) o[e] = 0.5 * (Y[e] + Y[(e % 6) * 6 + e / 6]);
+                __syncwarp();
+            } else {
+                for (int e = lane; e < 36; e += 32) o[e] = nan;
+            }
+        }
+    }
+}
+
+// why record r cannot seed its slot, or nullptr
+const char *seed_check(const ImuStreams &M, const pvio_b200_imu_stream_cov_seed &r) {
+    if (!M.host[r.slot].has_state) return "the slot has no latest state";
+    if (r.state_time != M.cov_host[r.slot].state_t) return "state_time is not the slot's latest-state time";
+    if (r.mode != PVIO_B200_IMU_STREAM_COV_DIRECT && r.mode != PVIO_B200_IMU_STREAM_COV_FACTOR) return "unknown mode";
+    const bool factor = r.mode == PVIO_B200_IMU_STREAM_COV_FACTOR;
+    if (!r.cov || !r.noise_cov || (factor && !r.imu_record)) return "a missing array";
+    if (!std::isfinite(r.state_time) || !finite_all(r.cov, 225) || !finite_all(r.noise_cov, 36) ||
+        (factor && !finite_all(r.imu_record, PVIO_B200_IMU_BG0)))
+        return "a value that is not finite";
+    double big = 0.0;
+    for (int e = 0; e < 225; ++e) big = std::max(big, std::fabs(r.cov[e]));
+    for (int a = 0; a < 15; ++a) {
+        if (r.cov[a * 16] < 0) return "a negative diagonal in cov";
+        for (int b = a + 1; b < 15; ++b)
+            if (std::fabs(r.cov[a * 15 + b] - r.cov[b * 15 + a]) > 1e-12 * big) return "cov is not symmetric";
+    }
+    if (factor)
+        for (int a = 0; a < 15; ++a)
+            if (r.imu_record[PVIO_B200_IMU_SQRT_INV_COV + a * 16] == 0.0) return "a zero diagonal in sqrt_inv_cov";
+    return nullptr;
+}
+
+int stream_set_covariance_impl(Handle *h, int n, const pvio_b200_imu_stream_cov_seed *recs) {
+    if (n < 0 || (n > 0 && !recs)) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_set_covariance: bad record list");
+    if (n == 0) return 0;
+    ImuStreams &M = h->imus;
+    std::vector<uint8_t> taken;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_cov_seed &r = recs[i];
+        TRY(take_slot(h, taken, r.slot, "batch_imu_stream_set_covariance"));
+        if ((size_t)r.slot >= M.host.size() || !M.host[r.slot].set)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_set_covariance: the slot was never reset");
+        if (const char *why = seed_check(M, r))
+            return fail(h, PVIO_B200_EINVAL, (std::string("batch_imu_stream_set_covariance: ") + why).c_str());
+    }
+    Stage stage(M.stage);
+    const auto rc = stage.add<StreamSeedRec>(Stage::kUp, n);
+    TRY(stage.place(h));
+    StreamSeedRec *hr = stage.host(rc);
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_cov_seed &r = recs[i];
+        StreamSeedRec &R = hr[i];
+        R.slot = r.slot;
+        R.mode = r.mode;
+        R.state_t = r.state_time;
+        memcpy(R.cov, r.cov, sizeof(R.cov));
+        if (r.mode == PVIO_B200_IMU_STREAM_COV_FACTOR) memcpy(R.imu, r.imu_record, sizeof(R.imu));
+        else memset(R.imu, 0, sizeof(R.imu));
+        memcpy(R.noise, r.noise_cov, sizeof(R.noise));
+    }
+    cudaStream_t st = h->stream;
+    TRY(stage.upload(h));
+    imu_stream_seed_kernel<<<(n + kCovWarps - 1) / kCovWarps, 32 * kCovWarps, 0, st>>>(
+        n, stage.dev(rc), reinterpret_cast<const ImuStreamSlot *>(M.hdr.d), M.cov.d);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    CK(h, cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i) M.cov_host[recs[i].slot].seed_gen = M.cov_host[recs[i].slot].gen;
+    return 0;
+}
+
+int stream_predict_impl(Handle *h, int n, pvio_b200_imu_stream_predict *recs) {
+    if (n < 0 || (n > 0 && !recs)) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_predict: bad record list");
+    if (n == 0) return 0;
+    ImuStreams &M = h->imus;
+    std::vector<uint8_t> taken;
+    int64_t nt = 0, ns = 0, npc = 0, nsc = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_predict &r = recs[i];
+        TRY(take_slot(h, taken, r.slot, "batch_imu_stream_predict"));
+        if ((size_t)r.slot >= M.host.size() || !M.host[r.slot].set)
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_predict: the slot was never reset");
+        if (r.n_times < 0 || (r.n_times > 0 && (!r.times || !r.poses)))
+            return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_predict: bad time count or pointer");
+        if (!finite_all(r.times, r.n_times)) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_predict: a time is not finite");
+        for (int k = 1; k < r.n_times; ++k)
+            if (r.times[k] < r.times[k - 1]) return fail(h, PVIO_B200_EINVAL, "batch_imu_stream_predict: the times decrease");
+        nt += r.n_times;
+        ns += r.states ? r.n_times : 0;
+        npc += r.pose_cov ? r.n_times : 0;
+        nsc += r.state_cov ? r.n_times : 0;
+    }
+    // staging: records | times (uploaded) || poses | states | pose covariances | state covariances (downloaded)
+    Stage stage(M.stage);
+    const auto rc = stage.add<StreamPredRec>(Stage::kUp, n);
+    const auto tm = stage.add<double>(Stage::kUp, nt);
+    const auto po = stage.add<double>(Stage::kDown, 7 * nt);
+    const auto sto = stage.add<double>(Stage::kDown, 16 * ns);
+    const auto pc = stage.add<double>(Stage::kDown, 36 * npc);
+    const auto sc = stage.add<double>(Stage::kDown, 225 * nsc);
+    TRY(stage.place(h));
+    StreamPredRec *hr = stage.host(rc);
+    std::vector<int32_t> status(n);
+    int64_t at = 0, as = 0, apc = 0, asc = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_imu_stream_predict &r = recs[i];
+        const ImuStreamCovHost &C = M.cov_host[r.slot];
+        const bool has_state = M.host[r.slot].has_state, has_cov = has_state && C.seed_gen == C.gen;
+        status[i] = !has_state ? PVIO_B200_IMU_STREAM_NO_STATE : has_cov ? PVIO_B200_OK : PVIO_B200_IMU_STREAM_NO_COVARIANCE;
+        StreamPredRec R{};
+        R.slot = r.slot; R.n_times = r.n_times; R.has_cov = has_cov;
+        R.t_at = at; R.pose_at = at;
+        R.state_at = r.states ? as : -1;
+        R.pcov_at = r.pose_cov ? apc : -1;
+        R.scov_at = r.state_cov ? asc : -1;
+        hr[i] = R;
+        if (r.n_times) memcpy(stage.host(tm) + at, r.times, sizeof(double) * r.n_times);
+        at += r.n_times;
+        as += r.states ? r.n_times : 0;
+        apc += r.pose_cov ? r.n_times : 0;
+        asc += r.state_cov ? r.n_times : 0;
+    }
+    StreamPredArgs A;
+    A.hdr = reinterpret_cast<const ImuStreamSlot *>(M.hdr.d);
+    A.k = M.k.d; A.cov = M.cov.d; A.qcap = M.qcap;
+    A.recs = stage.dev(rc); A.times = stage.dev(tm);
+    A.poses = stage.dev(po); A.states = stage.dev(sto); A.pcov = stage.dev(pc); A.scov = stage.dev(sc);
+    A.n = n;
+    cudaStream_t st = h->stream;
+    TRY(stage.upload(h));
+    imu_stream_predict_kernel<<<(n + kCovWarps - 1) / kCovWarps, 32 * kCovWarps, 0, st>>>(A);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(stage.download(h));
+    CK(h, cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_imu_stream_predict &r = recs[i];
+        const StreamPredRec &R = hr[i];
+        const size_t k = r.n_times;
+        if (k) memcpy(r.poses, stage.host(po) + 7 * R.pose_at, sizeof(double) * 7 * k);
+        if (k && r.states) memcpy(r.states, stage.host(sto) + 16 * R.state_at, sizeof(double) * 16 * k);
+        if (k && r.pose_cov) memcpy(r.pose_cov, stage.host(pc) + 36 * R.pcov_at, sizeof(double) * 36 * k);
+        if (k && r.state_cov) memcpy(r.state_cov, stage.host(sc) + 225 * R.scov_at, sizeof(double) * 225 * k);
+        r.status = status[i];
+    }
+    return 0;
+}
 }  // namespace
 
 }  // namespace pvio
@@ -795,4 +1280,17 @@ extern "C" int pvio_b200_batch_imu_stream_restore(pvio_b200_handle hh, int n, co
     Handle *h = reinterpret_cast<Handle *>(hh);
     if (!h) return PVIO_B200_EINVAL;
     return stream_restore_impl(h, n, records);
+}
+
+extern "C" int pvio_b200_batch_imu_stream_set_covariance(pvio_b200_handle hh, int n,
+                                                         const pvio_b200_imu_stream_cov_seed *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return stream_set_covariance_impl(h, n, records);
+}
+
+extern "C" int pvio_b200_batch_imu_stream_predict(pvio_b200_handle hh, int n, pvio_b200_imu_stream_predict *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    return stream_predict_impl(h, n, records);
 }

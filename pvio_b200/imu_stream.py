@@ -8,6 +8,7 @@ from . import _lib
 
 GYROSCOPE, ACCELEROMETER, CAMERA = _lib.IMU_EVENT_GYROSCOPE, _lib.IMU_EVENT_ACCELEROMETER, _lib.IMU_EVENT_CAMERA
 KEEP, SET, CLEAR = _lib.IMU_STREAM_KEEP, _lib.IMU_STREAM_SET, _lib.IMU_STREAM_CLEAR
+NO_STATE, NO_COVARIANCE = _lib.IMU_STREAM_NO_STATE, _lib.IMU_STREAM_NO_COVARIANCE
 
 
 class StreamRecord:
@@ -96,6 +97,59 @@ class ImuStream:
         for i, a in enumerate(arrs):
             recs[i].data, recs[i].capacity = _lib.ptr(a), len(a)
         self.ba._ck(self.lib.pvio_b200_batch_imu_stream_restore(self.h, n, recs))
+
+    def set_covariance(self, slots, state_times, covs, noise_cov, imu_records=None):
+        """Give each slot's current latest state (its time state_times[i]) a covariance [15, 15] in [dtheta dp dv dbg dba],
+        q perturbed on the right.  noise_cov [4, 9] (cov_w, cov_a, cov_bg, cov_ba), or one per slot: what predict()
+        propagates with.  imu_records None (or a None entry): covs[i] is the state's own.  Otherwise imu_records[i] is the
+        [288] factor returned with the `predicted` state and covs[i] the covariance of the frame it was predicted from.
+        The seed holds until the slot's latest state changes."""
+        slots = [int(s) for s in slots]
+        n = len(slots)
+        recs = (_lib.CImuStreamCovSeed * max(n, 1))()
+        keep = []
+        noise = np.broadcast_to(np.asarray(noise_cov, dtype=np.float64).reshape(-1, 36), (n, 36))
+        for i, r in enumerate(recs[:n]):
+            rec = None if imu_records is None else imu_records[i]
+            c = np.ascontiguousarray(covs[i], dtype=np.float64).reshape(225)
+            nz = np.ascontiguousarray(noise[i])
+            ir = None if rec is None else np.ascontiguousarray(rec, dtype=np.float64).reshape(_lib.IMU_STRIDE)
+            keep += [c, nz, ir]
+            r.slot, r.state_time = slots[i], float(state_times[i])
+            r.mode = _lib.IMU_STREAM_COV_DIRECT if ir is None else _lib.IMU_STREAM_COV_FACTOR
+            _lib.set_ptrs(r, cov=c, noise_cov=nz, imu_record=ir)
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream_set_covariance(self.h, n, recs))
+
+    def predict(self, slots, times, states=False, covariances=True):
+        """The IMU-rate pose of each slot at its non-decreasing times (times[i], one list per slot); changes no slot.
+        Per slot a dict: status (0, NO_STATE or NO_COVARIANCE), poses [k, 7] (q xyzw, p) as the stream gives them,
+        with states: states [k, 16]; with covariances: pose_cov [k, 6, 6] ([dtheta dp] of the pose) and state_cov
+        [k, 15, 15], NaN without a seed."""
+        slots = [int(s) for s in slots]
+        n = len(slots)
+        recs = (_lib.CImuStreamPredict * max(n, 1))()
+        outs = []
+        for i, r in enumerate(recs[:n]):
+            t = np.ascontiguousarray(times[i], dtype=np.float64).reshape(-1)
+            k = len(t)
+            o = dict(times=t, poses=np.zeros((max(k, 1), 7)), states=np.zeros((max(k, 1), 16)) if states else None,
+                     pose_cov=np.zeros((max(k, 1), 6, 6)) if covariances else None,
+                     state_cov=np.zeros((max(k, 1), 15, 15)) if covariances else None)
+            outs.append(o)
+            r.slot, r.n_times = slots[i], k
+            _lib.set_ptrs(r, times=t if k else None, poses=o["poses"], states=o["states"], pose_cov=o["pose_cov"],
+                          state_cov=o["state_cov"])
+        self.ba._ck(self.lib.pvio_b200_batch_imu_stream_predict(self.h, n, recs))
+        res = []
+        for r, o in zip(recs[:n], outs):
+            k = len(o["times"])
+            d = dict(status=int(r.status), poses=o["poses"][:k])
+            if states:
+                d["states"] = o["states"][:k]
+            if covariances:
+                d["pose_cov"], d["state_cov"] = o["pose_cov"][:k], o["state_cov"][:k]
+            res.append(d)
+        return res
 
     @staticmethod
     def _snapshots(slots):
