@@ -373,6 +373,38 @@ typedef struct pvio_b200_window_covariance {
     int32_t status;           /* out: PVIO_B200_OK or PVIO_B200_ENUMERIC                      */
 } pvio_b200_window_covariance; /* 56 bytes on LP64 */
 int pvio_b200_batch_window_covariance(pvio_b200_handle h, int n, pvio_b200_window_covariance *records);
+/* The map of each named slot at its current state: per row (a named track, or every live track in id order) its id,
+ * its world point Track::get_landmark_point() -- the anchor (lowest) frame's camera pose applied to [z_anchor; 1] / rho,
+ * a plane track at the inverse depth set_planes gave it -- its role (-1, -2 or the plane index), and optionally the
+ * point's 3 x 3 covariance and the track's Var(rho): the covariance of pvio_b200_batch_window_covariance (the anchor
+ * frame's pose, rho and their cross-covariance, which that call does not return) propagated to first order through
+ * Track::get_landmark_point().
+ *  - point_cov / inv_depth_var: for the rows the solve treats as landmarks (role < 0, >= 2 observations); NaN for a
+ *    plane track or a track with one observation.  inv_depth_var equals pvio_b200_batch_window_covariance's bit for
+ *    bit.  point_cov NULL: no covariance and no covariance launches for the record (inv_depth_var must be NULL too).
+ *  - status: PVIO_B200_OK, or PVIO_B200_ENUMERIC when the slot's scaled H is not positive definite (as the covariance
+ *    call defines it): then every point_cov and inv_depth_var of the record is NaN; the points are still written.
+ * Rejected (PVIO_B200_EINVAL, no output changed): a slot out of range, not resident, named twice or without frames; a
+ * track count below -1 or above the live tracks; an unknown or repeated track; a capacity smaller than the slot's live
+ * tracks (n_tracks == -1); a missing array.  The call changes no slot.  Points only: one host -> device copy, one kernel
+ * launch, one device -> host copy and one synchronisation; with covariances four launches more (the covariance call's
+ * linearise and Schur sweeps and cov_kernel over the slots that ask, and a landmark kernel), whatever n is.  With
+ * n_tracks == -1 the host does no per-track work: the rows are those of the slot's mirror. */
+typedef struct pvio_b200_window_landmarks {
+    int32_t slot;
+    int32_t n_tracks;         /* -1: every live track of the slot in id order; else 0 .. live tracks, named below     */
+    const int32_t *tracks;    /* [n_tracks] live track ids of the slot, distinct (ignored when n_tracks == -1)        */
+    int32_t capacity;         /* rows the outputs hold when n_tracks == -1                                             */
+    int32_t *track_id;        /* out [rows] (may be NULL)                                                              */
+    double *point;            /* out [rows][3] world point                                                             */
+    int32_t *role;            /* out [rows] -1, -2 or the plane index (may be NULL); int32_t like the roles
+                                 pvio_b200_window_planes takes                                                        */
+    double *point_cov;        /* out [rows][9] row-major, or NULL: no covariance                                       */
+    double *inv_depth_var;    /* out [rows] (may be NULL)                                                              */
+    int32_t n_rows;           /* out: rows written                                                                     */
+    int32_t status;           /* out: PVIO_B200_OK or PVIO_B200_ENUMERIC                                               */
+} pvio_b200_window_landmarks; /* 72 bytes on LP64 */
+int pvio_b200_batch_window_landmarks(pvio_b200_handle h, int n, pvio_b200_window_landmarks *records);
 /* Device -> host in one copy, per named slot i: n_frames [n], frames [n][frames_stride] ([N][16]), n_tracks [n] (live
  * tracks), and for each live track in id order at [i * track_stride + r]: id, inverse depth, anchor frame, observation
  * count, and the post-pass valid / quality of the last solve (0 / 0 for a track that did not take part in it).  Any

@@ -150,6 +150,12 @@ class CWindowCovariance(C.Structure):
                 ("tracks", c_i32p), ("inv_depth_var", c_f64p), ("status", C.c_int32)]
 
 
+class CWindowLandmarks(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n_tracks", C.c_int32), ("tracks", c_i32p), ("capacity", C.c_int32),
+                ("track_id", c_i32p), ("point", c_f64p), ("role", c_i32p), ("point_cov", c_f64p),
+                ("inv_depth_var", c_f64p), ("n_rows", C.c_int32), ("status", C.c_int32)]
+
+
 class CWindowKeypoints(C.Structure):
     _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("frame_id", C.c_uint64), ("n", C.c_int32),
                 ("track", c_i32p), ("keypoint", c_i32p), ("newest_is_keyframe", C.c_int32), ("skipped_frames", C.c_int32)]
@@ -263,6 +269,7 @@ SIGNATURES = {
     "pvio_b200_batch_window_solve": (_int, [_h, _int, c_i32p, _P(COptions), _P(CSummary)]),
     "pvio_b200_batch_window_drop_victim": (_int, [_h, _int, c_i32p, c_f64p, _i64, c_f64p, _i64]),
     "pvio_b200_batch_window_covariance": (_int, [_h, _int, _P(CWindowCovariance)]),
+    "pvio_b200_batch_window_landmarks": (_int, [_h, _int, _P(CWindowLandmarks)]),
     "pvio_b200_batch_window_download": (_int, [_h, _int, c_i32p, c_i32p, c_f64p, _i64, c_i32p, _i64, c_i32p, c_f64p,
                                                c_i32p, c_i32p, c_u8p, c_f64p]),
     "pvio_b200_batch_window_localize": (_int, [_h, _int, _P(CWindowLocalize), _P(COptions)]),

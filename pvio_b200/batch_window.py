@@ -468,6 +468,38 @@ class BatchWindows:
             o["status"] = int(r.status)
         return out
 
+    def landmarks(self, slots, tracks=None, covariance=False, capacity=None):
+        """The map of each named slot at its current state: per record the rows of tracks[i] (live track ids), or of every
+        live track in id order when tracks (or tracks[i]) is None.  Per record a dict: ids [rows], point [rows, 3]
+        (Track::get_landmark_point()), role [rows] (-1, -2 or the plane index) and status; with covariance also point_cov
+        [rows, 3, 3] and inv_depth_var [rows], NaN for a plane track or a track with one observation, and NaN throughout
+        when status is ENUMERIC.  capacity: rows reserved for an all-tracks record (None: the handle's max_landmarks)."""
+        n = len(slots)
+        cap = int(self.ba.max_landmarks if capacity is None else capacity)
+        recs, out = (_lib.CWindowLandmarks * max(n, 1))(), []
+        for i, (r, s) in enumerate(zip(recs, slots)):
+            t = None if tracks is None else tracks[i]
+            if t is not None:
+                t = np.ascontiguousarray(t, dtype=np.int32).reshape(-1)
+            rows = cap if t is None else len(t)
+            o = dict(tracks=t, ids=np.zeros(rows, dtype=np.int32), point=np.zeros((rows, 3)),
+                     role=np.zeros(rows, dtype=np.int32))
+            if covariance:
+                o["point_cov"], o["inv_depth_var"] = np.zeros((rows, 3, 3)), np.zeros(rows)
+            out.append(o)
+            r.slot, r.n_tracks, r.capacity = int(s), -1 if t is None else len(t), rows
+            _lib.set_ptrs(r, tracks=t if t is not None and len(t) else None, track_id=o["ids"], point=o["point"],
+                          role=o["role"], point_cov=o.get("point_cov"), inv_depth_var=o.get("inv_depth_var"))
+        self.ba._ck(self.lib.pvio_b200_batch_window_landmarks(self.h, n, recs))
+        for r, o in zip(recs, out):
+            del o["tracks"]
+            k = int(r.n_rows)
+            for key in ("ids", "point", "role", "point_cov", "inv_depth_var"):
+                if key in o:
+                    o[key] = o[key][:k]
+            o["status"] = int(r.status)
+        return out
+
     def save(self, slots, tracker_slots=None):
         """Save each sequence to host memory: per record a window slot (-1: none) and, from tracker_slots (None: none),
         a tracker slot of batch_feature_track (-1: none).  Returns one blob (bytes) per record, which restore() seats in

@@ -26,6 +26,7 @@ class BundleAdjustor:
             raise PvioB200Error(f"pvio_b200_create failed ({rc}) {msg}: a CUDA device is required, there is no CPU fallback")
         self.max_windows = max_windows
         self.max_frames = max_frames
+        self.max_landmarks = max_landmarks
         self._keep = {}
         self._slot_frames = {}          # frame count of the window packed into each slot by batch_set / batch_replicate
 

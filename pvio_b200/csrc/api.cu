@@ -644,7 +644,16 @@ int run_marg_vision(Handle *h, int n, const int32_t *h_slots, const int32_t *d_s
 
 size_t cov_smem_bytes(const WinHdr &H) { return solve_smem_one(H, false); }
 
-int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L) {
+static CovArgs cov_args(Handle *h, const CovLaunch &L) {
+    CovArgs a;
+    static_cast<SolveArgs &>(a) = launch_args<SolveArgs>(h);
+    a.alias_bias = 0; a.Hfull = nullptr; a.gfull = nullptr; a.compute_scale = 1; a.w0 = 0; a.mu_override = 0.0; a.loop = 0;
+    a.recs = L.recs; a.frames = L.frames; a.lms = L.lms; a.n_lm = L.n_lm;
+    a.cov = L.cov; a.var = L.var; a.status = L.status; a.sig = L.sig; a.sig_xi = L.sig_xi;
+    return a;
+}
+
+int run_cov_system(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L) {
     // the solve's linearisation at the state (with the loss, either pipeline), mu = 0 in the landmark pivots; one CTA
     // per window so that the launch count does not depend on n
     StepCfg c;
@@ -652,20 +661,23 @@ int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_sl
     const BatchShape b = batch_shape(h, 0, n, false, h_slots);
     TRY(launch_lin(h, n, c, b, true, false, false));
     TRY(launch_schur(h, n, c, b, false));
-    CovArgs a;
-    static_cast<SolveArgs &>(a) = launch_args<SolveArgs>(h);
-    a.alias_bias = 0; a.Hfull = nullptr; a.gfull = nullptr; a.compute_scale = 1; a.w0 = 0; a.mu_override = 0.0; a.loop = 0;
-    a.recs = L.recs; a.frames = L.frames; a.lms = L.lms; a.n_lm = L.n_lm;
-    a.cov = L.cov; a.var = L.var; a.status = L.status; a.sig = L.sig; a.sig_xi = L.sig_xi;
+    const CovArgs a = cov_args(h, L);
     size_t smem = 0;
     for (int i = 0; i < n; ++i) smem = std::max(smem, cov_smem_bytes(h->hdr.h[h_slots[i]]));
     cov_kernel<<<n, 256, smem, h->stream>>>(a);
     LAUNCH_CK(h, "cov_kernel");
+    ++h->launches;
+    return 0;
+}
+
+int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L) {
+    TRY(run_cov_system(h, n, h_slots, d_slots, L));
+    const CovArgs a = cov_args(h, L);
     const int blocks = std::max(1, (L.n_lm + kCovLmWarps - 1) / kCovLmWarps);
     if (h->hs_double) cov_lm_kernel<double><<<blocks, 32 * kCovLmWarps, 0, h->stream>>>(a);
     else cov_lm_kernel<float><<<blocks, 32 * kCovLmWarps, 0, h->stream>>>(a);
     LAUNCH_CK(h, "cov_lm_kernel");
-    h->launches += 2;
+    ++h->launches;
     return 0;
 }
 

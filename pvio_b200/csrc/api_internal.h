@@ -524,6 +524,9 @@ struct CovLaunch {
     double *sig, *sig_xi;
 };
 int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L);
+// the first three of those launches: Sigma_xi of every frame pair in L.sig_xi and each record's status, for a landmark
+// kernel of the caller's (batch_window.cu: pvio_b200_batch_window_landmarks)
+int run_cov_system(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L);
 size_t cov_smem_bytes(const WinHdr &H);   // dynamic shared memory of cov_kernel for a window of this header
 void drop_graphs(Handle *h);
 // api.cu, for the resident batched windows (batch_window.cu)

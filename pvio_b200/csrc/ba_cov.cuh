@@ -131,8 +131,11 @@ __device__ __forceinline__ void CovBody::finish(const SolveArgs &sa, int w, int 
 
 constexpr int kCovLmWarps = 4;
 
-// One warp per named track.  h_l over the free frames: the landmark's Schur records (the anchor's materialised when the
-// anchor is free, zero blocks for the free frames that do not see it); constant frames take no part (Sigma_xi is 0 there).
+// One warp per named track.  bw_landmark_cov_kernel (batch_window.cu) forms the same Var(rho) through ba_cov_lm.cuh,
+// which restates this body operation for operation so that both calls give the same bits: a change to the arithmetic
+// here must be made there too (tests/test_gpu_batch_window_landmarks.py checks the two for bit equality).
+// h_l over the free frames: the landmark's Schur records (the anchor's materialised when the anchor is free, zero
+// blocks for the free frames that do not see it); constant frames take no part (Sigma_xi is 0 there).
 template <typename real>
 static __global__ void __launch_bounds__(32 * kCovLmWarps) cov_lm_kernel(CovArgs a) {
     __shared__ double u_sm[kCovLmWarps][6 * kMaxFrames];

@@ -30,7 +30,10 @@
 #include <optional>
 #include <vector>
 
+#include <math_constants.h>
+
 #include "api_internal.h"
+#include "ba_cov_lm.cuh"
 #include "batch_window.cuh"
 #include "imu.cuh"
 #include "klt_border.cuh"
@@ -1563,6 +1566,127 @@ static SnapRec snap_rec(const SnapHead &H, const SnapOff &o, int slot, int64_t b
     return r;
 }
 
+// ---- pvio_b200_batch_window_landmarks: every row's world point, and for the rows the solve treats as landmarks the
+// point's covariance from the covariance call's Sigma_xi and the landmark's Schur records
+struct BwLmk {
+    int32_t slot, n_rows, T;      // rows written; live rows of the slot
+    int32_t rows_off;             // ints into the call's row list; -1: rows [0, n_rows) of the slot (every live track)
+    int32_t out_off;              // rows into the call's points
+    int32_t cov, cov_off, pad;    // index among the records with a covariance (-1: none); rows into its outputs
+};
+struct LmkArgs {
+    const BwLmk *rec;             // [n]
+    const int32_t *rows;          // the named rows of every record
+    const int32_t *cov_rec;       // [n_cov] the record of each covariance record
+    double *pts;                  // out: [rows][3]
+    int32_t *role;                // out: [rows]
+    int32_t *lm_of;               // scratch: [n_cov][Mcap] the packed landmark of each row of the slot, -1: none
+    const int32_t *status;        // [n_cov] cov_kernel's status
+    const double *sig_xi;         // [n_cov][Ncap][Ncap][36] Sigma_xi of every frame pair (cov_kernel)
+    double *pcov, *var;           // out: [cov rows][9], [cov rows]
+};
+constexpr int kLmkWarps = 4;
+
+// One CTA per record: Track::get_landmark_point() of every row; for a record with a covariance, the packed landmark of
+// every row of its slot (bw_layout_kernel's lm_row inverted) for bw_landmark_cov_kernel
+__global__ void __launch_bounds__(kBwThreads) bw_landmark_point_kernel(BwArgs a, LmkArgs L) {
+    const BwLmk r = L.rec[blockIdx.x];
+    const int w = r.slot;
+    const size_t base = (size_t)w * a.Mcap;
+    const double *fr = a.frames + (size_t)w * a.Ncap * kFrameStride;
+    const WinConst &c = a.cst[w];
+    for (int k = threadIdx.x; k < r.n_rows; k += kBwThreads) {
+        const int row = r.rows_off < 0 ? k : L.rows[r.rows_off + k];
+        bw_landmark_point(a, base + row, fr, c, L.pts + 3 * ((size_t)r.out_off + k));
+        L.role[r.out_off + k] = a.trole[base + row];
+    }
+    if (r.cov < 0) return;
+    int32_t *lm = L.lm_of + (size_t)r.cov * a.Mcap;
+    for (int q = threadIdx.x; q < r.T; q += kBwThreads) lm[q] = -1;
+    __syncthreads();
+    for (int lp = threadIdx.x; lp < a.hdr[w].M; lp += kBwThreads) lm[a.lm_row[base + lp]] = lp;
+}
+
+// row i of X_l = [[x]x, I]
+__device__ __forceinline__ void lmk_xrow(const double *x, int i, double *o) {
+    o[0] = i == 1 ? x[2] : (i == 2 ? -x[1] : 0.0);
+    o[1] = i == 0 ? -x[2] : (i == 2 ? x[0] : 0.0);
+    o[2] = i == 0 ? x[1] : (i == 1 ? -x[0] : 0.0);
+    o[3] = i == 0 ? 1.0 : 0.0; o[4] = i == 1 ? 1.0 : 0.0; o[5] = i == 2 ? 1.0 : 0.0;
+}
+
+// One warp per row of a record with a covariance (grid: covariance records x row blocks).  Var(rho) as cov_lm_kernel
+// forms it (ba_cov_lm.cuh), C = Cov(xi_a, rho) = -(Sigma_xi h_l)_a / H_ll from the same products, then
+//   Sigma_x = X Sigma_aa X^T - X C c^T - c C^T X^T + c c^T Var(rho),  X = [[x - o]x, I], c = -(x - c_a) / rho,
+// o the window's origin, about which frame_T takes xi,
+// the upper triangle on six lanes, mirrored (exactly symmetric).  NaN for a row that is not a landmark of the solve and
+// for every row of a record whose factorisation failed.
+template <typename real>
+__global__ void __launch_bounds__(32 * kLmkWarps) bw_landmark_cov_kernel(BwArgs a, LmkArgs L) {
+    __shared__ double u_sm[kLmkWarps][6 * kMaxFrames];
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const int crec = blockIdx.x;                     // the covariance record
+    const BwLmk r = L.rec[L.cov_rec[crec]];
+    const int k = blockIdx.y * kLmkWarps + wv;
+    if (k >= r.n_rows) return;
+    const int w = r.slot;
+    const size_t base = (size_t)w * a.Mcap;
+    const int row = r.rows_off < 0 ? k : L.rows[r.rows_off + k];
+    const int lm = L.lm_of[(size_t)crec * a.Mcap + row];
+    double *P = L.pcov + 9 * ((size_t)r.cov_off + k);
+    double *V = L.var + r.cov_off + k;
+    if (lm < 0 || L.status[crec] != PVIO_B200_OK) {
+        if (lane < 9) P[lane] = CUDART_NAN;
+        if (lane == 0) *V = CUDART_NAN;
+        return;
+    }
+    const int N = a.hdr[w].N;
+    const unsigned fixed = (unsigned)a.hdr[w].fixed_mask & ((1u << N) - 1u);
+    const real *hs = reinterpret_cast<const real *>(a.hs) + (size_t)w * a.Ncap * a.Mcap * 6;
+    double *u = u_sm[wv];
+    cov_lm_h(hs, a.Mcap, lm, N, fixed, lane, u);
+    __syncwarp();
+    const double *X = L.sig_xi + (size_t)crec * a.Ncap * a.Ncap * 36;
+    const int an = __ffs(a.tmask[base + row]) - 1;
+    double srow = 0.0;
+    const double q = cov_lm_quad<true>(u, X, N, lane, an, srow);
+    const double hll = a.lm_aux[base + lm].hll;
+    const double var = cov_lm_var(hll, q);
+    double C[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) C[i] = -__shfl_sync(0xffffffffu, srow, (6 * an + i) & 31) / hll;
+    const double2 z = a.tz[(base + row) * a.Ncap + an];
+    const double rho = a.trho[base + row];
+    double qc[4], pc[3], x[3];
+    bw_cam_pose(a.frames + ((size_t)w * a.Ncap + an) * kFrameStride, a.cst[w], qc, pc);
+    bw_world_point(qc, pc, z.x, z.y, rho, x);
+    const double cl[3] = {-(x[0] - pc[0]) / rho, -(x[1] - pc[1]) / rho, -(x[2] - pc[2]) / rho};
+    const double *o = a.cst[w].origin;                  // xi is taken about the window's origin (frame_T)
+    const double xo[3] = {x[0] - o[0], x[1] - o[1], x[2] - o[2]};
+    if (lane < 6) {
+        const int i = lane < 3 ? 0 : (lane < 5 ? 1 : 2), j = lane < 3 ? lane : (lane < 5 ? lane - 2 : 2);
+        double Xi[6], Xj[6];
+        lmk_xrow(xo, i, Xi);
+        lmk_xrow(xo, j, Xj);
+        const double *S = X + ((size_t)an * N + an) * 36;
+        double s = 0.0, bi = 0.0, bj = 0.0;
+#pragma unroll
+        for (int m = 0; m < 6; ++m) {
+            double t = 0.0;
+#pragma unroll
+            for (int n = 0; n < 6; ++n) t += S[m * 6 + n] * Xj[n];
+            s += Xi[m] * t;
+            bi += Xi[m] * C[m];
+            bj += Xj[m] * C[m];
+        }
+        const double cli = i == 0 ? cl[0] : (i == 1 ? cl[1] : cl[2]), clj = j == 0 ? cl[0] : (j == 1 ? cl[1] : cl[2]);
+        const double v = s - bi * clj - cli * bj + cli * clj * var;
+        P[3 * i + j] = v;
+        P[3 * j + i] = v;
+    }
+    if (lane == 0) *V = var;
+}
+
 }  // namespace pvio
 
 using namespace pvio;
@@ -1927,6 +2051,113 @@ int pvio_b200_batch_window_covariance(pvio_b200_handle hh, int n, pvio_b200_wind
         if (R.n_tracks > 0) memcpy(R.inv_depth_var, S.host(var) + t, sizeof(double) * R.n_tracks);
         t += R.n_tracks;
         R.status = S.host(st)[i];
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_landmarks(pvio_b200_handle hh, int n, pvio_b200_window_landmarks *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const char *what = "batch_window_landmarks";
+    auto bad = [&](const char *why) { return fail(h, PVIO_B200_EINVAL, (std::string(what) + ": " + why).c_str()); };
+    if (n < 0 || (n > 0 && !records)) return bad("bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_landmarks: bad slot list"));
+    // every record checked against its slot's host mirror before anything is staged; the all-tracks mode takes its rows
+    // from the mirror's size, with no per-track work
+    std::vector<BwLmk> recs(n);
+    std::vector<int32_t> rows, cov_slots, cov_rec;
+    std::vector<CovRec> crecs;
+    int32_t n_pts = 0, n_cov_rows = 0, max_cov_rows = 0;
+    int64_t sig_n = 0;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_landmarks &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        const int T = (int)s.ids.size();
+        if (s.N < 1) return bad("a window without frames");
+        if (R.n_tracks < -1 || R.n_tracks > T) return bad("a track count out of range");
+        const bool all = R.n_tracks == -1;
+        const int nr = all ? T : R.n_tracks;
+        if (all && R.capacity < T) return bad("capacity smaller than the slot's live tracks");
+        if (!all && nr > 0 && !R.tracks) return bad("tracks missing");
+        if (nr > 0 && !R.point) return bad("point missing");
+        if (R.inv_depth_var && !R.point_cov) return bad("inv_depth_var without point_cov");
+        const bool cov = R.point_cov != nullptr;
+        if (cov && cov_smem_bytes(h->hdr.h[R.slot]) > 220 * 1024) return bad("reduced system too large for shared memory");
+        BwLmk &L = recs[i];
+        L = BwLmk{R.slot, nr, T, all ? -1 : (int32_t)rows.size(), n_pts, cov ? (int32_t)cov_slots.size() : -1, n_cov_rows, 0};
+        if (!all) {
+            std::vector<uint8_t> taken(T, 0);
+            for (int k = 0; k < nr; ++k) {
+                const int r = find_row(s, R.tracks[k]);
+                if (r < 0) return bad("a track that is not live in its slot");
+                if (taken[r]) return bad("a track named twice");
+                taken[r] = 1;
+                rows.push_back(r);
+            }
+        }
+        n_pts += nr;
+        if (cov) {
+            const int64_t D = (s.inertial ? 15 : 6) * (int64_t)s.N;
+            crecs.push_back(CovRec{R.slot, 0, 0, 0, 0, sig_n});
+            cov_slots.push_back(R.slot);
+            cov_rec.push_back(i);
+            n_cov_rows += nr;
+            max_cov_rows = std::max(max_cov_rows, nr);
+            sig_n += D * D;
+        }
+    }
+    const int n_cov = (int)cov_slots.size();
+    Stage S(h->bw.stage, &h->bw.scratch);
+    const auto rec = S.up(recs);
+    const auto rw = S.up(rows);
+    const auto crc = S.up(cov_rec);
+    const auto cr = S.up(crecs);
+    const auto csl = S.up(cov_slots);
+    const auto pts = S.add<double>(Stage::kDown, 3 * (size_t)n_pts);
+    const auto rol = S.add<int32_t>(Stage::kDown, (size_t)n_pts);
+    const auto pcov = S.add<double>(Stage::kDown, 9 * (size_t)n_cov_rows), var = S.add<double>(Stage::kDown, (size_t)n_cov_rows);
+    const auto st = S.add<int32_t>(Stage::kDown, n_cov);
+    const auto lmo = S.add<int32_t>(Stage::kScratch, (size_t)n_cov * h->Mcap);
+    const auto sig = S.add<double>(Stage::kScratch, (size_t)sig_n);
+    const auto sxi = S.add<double>(Stage::kScratch, (size_t)n_cov * h->Ncap * h->Ncap * 36);
+    TRY(S.place(h, true));
+    const LmkArgs L{S.dev(rec), S.dev(rw), S.dev(crc), S.dev(pts), S.dev(rol), S.dev(lmo), S.dev(st), S.dev(sxi), S.dev(pcov), S.dev(var)};
+    const BwArgs a = launch_args<BwArgs>(h);
+    bw_landmark_point_kernel<<<n, kBwThreads, 0, h->stream>>>(a, L);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    if (n_cov > 0) {
+        TRY(run_cov_system(h, n_cov, cov_slots.data(), S.dev(csl),
+                           CovLaunch{S.dev(cr), nullptr, nullptr, 0, nullptr, nullptr, S.dev(st), S.dev(sig), S.dev(sxi)}));
+        const dim3 grid(n_cov, std::max(1, (max_cov_rows + kLmkWarps - 1) / kLmkWarps));
+        if (h->hs_double) bw_landmark_cov_kernel<double><<<grid, 32 * kLmkWarps, 0, h->stream>>>(a, L);
+        else bw_landmark_cov_kernel<float><<<grid, 32 * kLmkWarps, 0, h->stream>>>(a, L);
+        ++h->launches;
+        CK(h, cudaGetLastError());
+    }
+    TRY(S.download(h));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_window_landmarks &R = records[i];
+        const BwLmk &L = recs[i];
+        const WinSlot &s = h->slots[R.slot];
+        const size_t nr = L.n_rows;
+        if (nr > 0) memcpy(R.point, S.host(pts) + 3 * (size_t)L.out_off, sizeof(double) * 3 * nr);
+        if (R.role && nr > 0) memcpy(R.role, S.host(rol) + L.out_off, sizeof(int32_t) * nr);
+        if (R.track_id && nr > 0) {
+            if (L.rows_off < 0) memcpy(R.track_id, s.ids.data(), sizeof(int32_t) * nr);
+            else memcpy(R.track_id, records[i].tracks, sizeof(int32_t) * nr);
+        }
+        R.status = PVIO_B200_OK;
+        if (L.cov >= 0) {
+            if (nr > 0) memcpy(R.point_cov, S.host(pcov) + 9 * (size_t)L.cov_off, sizeof(double) * 9 * nr);
+            if (R.inv_depth_var && nr > 0) memcpy(R.inv_depth_var, S.host(var) + L.cov_off, sizeof(double) * nr);
+            R.status = S.host(st)[L.cov];
+        }
+        R.n_rows = (int32_t)nr;
     }
     return 0;
 }
