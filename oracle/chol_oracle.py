@@ -56,6 +56,41 @@ def refined_solve(A, b, rounds=4):
     return x * s
 
 
+def _two_sum(a, b):
+    """s, e with s = fl(a + b) and s + e = a + b exactly (Knuth), elementwise"""
+    s = a + b
+    z = s - a
+    return s, (a - (s - z)) + (b - z)
+
+
+def dd_identity_residual(A, X):
+    """I - A X for square A, X, every entry summed in double-double (Ogita, Rump and Oishi's Sum2 over the exact
+    products of TwoProduct): as accurate as a sum in twice the working precision, then rounded"""
+    n = A.shape[0]
+    s, c = np.eye(n), np.zeros((n, n))
+    for k in range(n):
+        p, pe = two_product(A[:, k:k + 1], X[k:k + 1, :])
+        s, t = _two_sum(s, -p)
+        c -= pe
+        c += t
+    return s + c
+
+
+def refined_inverse(A, rounds=4):
+    """A^-1 of a symmetric positive definite A by refinement as refined_solve does it (in the power-of-two diagonal
+    scaling A_s = S A S, A^-1 = S A_s^-1 S exactly), for all columns at once, with the residual I - A_s Y in
+    double-double (dd_identity_residual) in place of the exactly rounded one"""
+    A = np.asarray(A, float)
+    if A.shape[0] == 0:
+        return np.zeros((0, 0))
+    s = pow2_scaling(A)
+    As = A * s[:, None] * s[None, :]
+    Y = np.linalg.solve(As, np.eye(len(s)))
+    for _ in range(rounds):
+        Y = Y + np.linalg.solve(As, dd_identity_residual(As, Y))
+    return Y * s[:, None] * s[None, :]
+
+
 def backward_error(A, x, b):
     """componentwise backward error max_i |b - A x|_i / (|A| |x| + |b|)_i with the exactly rounded residual"""
     A, x, b = np.asarray(A, float), np.asarray(x, float), np.asarray(b, float)

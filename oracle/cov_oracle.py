@@ -11,15 +11,14 @@ def covariance(win, st, frames, tracks, refine=False):
     (ba_oracle.normal_equations, no regulariser) over ba_oracle.free_mask, taken densely.  frames: window indices,
     their joint block [15 k, 15 k] with zero rows / columns for the coordinates that are not free; tracks: landmark
     indices of `win` (None or < 0: not a landmark), their inverse-depth variances (NaN for None or a landmark without free coordinate).
-    refine: solve the identity's columns with chol_oracle.refined_solve (exactly rounded residual refinement), for
-    ill-conditioned windows, instead of one factorisation.  Returns (cov, var, Sigma) with Sigma over the free
-    coordinates in local-coordinate order."""
+    refine: the inverse by residual refinement (chol_oracle.refined_inverse), for ill-conditioned windows, instead of
+    one factorisation.  Returns (cov, var, Sigma) with Sigma over the free coordinates in local-coordinate order."""
     H, _, _ = ba_oracle.normal_equations(win, st)
     free = ba_oracle.free_mask(win)
     idx = np.flatnonzero(free)
     Hf = H[np.ix_(idx, idx)]
     if refine:
-        Sig = np.column_stack([chol_oracle.refined_solve(Hf, e) for e in np.eye(len(idx))])
+        Sig = chol_oracle.refined_inverse(Hf)
         Sig = 0.5 * (Sig + Sig.T)
     else:
         Sig = np.linalg.inv(Hf)

@@ -457,6 +457,7 @@ struct StepCfg {
 // what the windows [w0, w0 + n) need from the launch: worst case over the batch
 struct BatchShape {
     int N = 1, M = 1, nfree = 1, D = 0;
+    int N_inertial = 0;               // the largest window with motion states (0: none)
     bool inertial = false, planes = false;
     size_t solve_smem_full = 0, solve_smem_lean = 0;
 };
@@ -475,24 +476,32 @@ static size_t solve_smem_one(const WinHdr &H, bool lean) {
     return sizeof(double) * ((nb + 1) * (nb + 2) / 2 * 18 + 4 * Dp + (size_t)H.N * 36 + scr);   // tiles of kTP = 18 doubles (ba_solve.cuh)
 }
 
-static BatchShape batch_shape(Handle *h, int w0, int n, bool by_capacity, const int32_t *h_slots = nullptr) {
+// named: windows k with named[k] == 0 are skipped (a solve of named resident slots: the others take no part in it)
+static BatchShape batch_shape(Handle *h, int w0, int n, bool by_capacity, const int32_t *h_slots = nullptr,
+                              const uint8_t *named = nullptr) {
     BatchShape b;
     for (int k = w0; k < w0 + n; ++k) {
+        if (named && !named[k]) continue;
         const WinHdr &H = h->hdr.h[h_slots ? h_slots[k - w0] : k];
         b.N = std::max(b.N, H.N); b.M = std::max(b.M, H.M);
         const unsigned allm = (1u << H.N) - 1u, freem = ~(unsigned)H.fixed_mask & allm;
         b.nfree = std::max(b.nfree, __builtin_popcount(freem));
         b.inertial |= H.use_inertial != 0;
+        if (H.use_inertial) b.N_inertial = std::max(b.N_inertial, H.N);
         b.planes |= H.n_ptracks > 0;
         b.solve_smem_full = std::max(b.solve_smem_full, solve_smem_one(H, false));
         b.solve_smem_lean = std::max(b.solve_smem_lean, solve_smem_one(H, true));
     }
-    if (by_capacity) {                 // graph-cached launches: shapes depend on the frame count (part of the graph key) only
+    if (by_capacity) {                 // graph-cached launches: shapes depend on the frame counts (part of the graph key) only
         b.M = h->Mcap; b.nfree = b.N;
         WinHdr H;
         memset(&H, 0, sizeof(H));
-        H.N = b.N; H.use_inertial = b.inertial ? 1 : 0; H.n_prior = b.inertial ? b.N : 0;
+        H.N = b.N;                     // a visual window of the largest size, an inertial one of the largest inertial size
         b.solve_smem_full = solve_smem_one(H, false);
+        if (b.inertial) {
+            H.N = b.N_inertial; H.use_inertial = 1; H.n_prior = b.N_inertial;
+            b.solve_smem_full = std::max(b.solve_smem_full, solve_smem_one(H, false));
+        }
     }
     return b;
 }
@@ -864,11 +873,12 @@ static int iteration_body(Handle *h, int n, const StepCfg &c, const BatchShape &
 // bodies.  For the latency path (a few windows from window 0) the sequence is captured once into a CUDA graph keyed by
 // (n, max_iter, flags) with capacity-sized launch shapes, and replayed: ONE launch per solve, no device -> host traffic
 // inside.  The graphs bake in w0 = 0.
-static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaStream_t st, bool init = true) {
+static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaStream_t st, bool init = true,
+                          const uint8_t *named = nullptr) {
     StepCfg c;
     c.mu = -1.0; c.loop = 1; c.alias_bias = o.alias_bias; c.compute_scale = 0; c.w0 = w0; c.stream = st;
     const bool graphable = w0 == 0 && n * 2 < h->sm_count;
-    const BatchShape b = batch_shape(h, w0, n, graphable);
+    const BatchShape b = batch_shape(h, w0, n, graphable, nullptr, named);
     const int bodies = o.max_iter + 2;               // spare bodies absorb retries of a failed linear solve (mu *= 10)
     if (init) {
         init_ctrl_kernel<<<n, 32, 0, st>>>(h->ctrl.d, 1e-8, o.radius0, o.max_iter, o.max_time, w0);
@@ -879,7 +889,7 @@ static int run_solve_loop(Handle *h, const SolveOptions &o, int w0, int n, cudaS
         for (int it = 0; it < bodies; ++it) TRY(iteration_body(h, n, c, b, it == 0));
         return 0;
     }
-    const Handle::GraphKey key(1, n, o.max_iter, (o.alias_bias ? 1 : 0) | (b.inertial ? 2 : 0) | (b.planes ? 4 : 0) | (h->hs_double ? 8 : 0) | (b.N << 4));
+    const Handle::GraphKey key(1, n, o.max_iter, (o.alias_bias ? 1 : 0) | (b.inertial ? 2 : 0) | (b.planes ? 4 : 0) | (h->hs_double ? 8 : 0) | (b.N << 4) | (b.N_inertial << 9));
     auto it = h->graphs.find(key);
     if (it == h->graphs.end()) {
         if (h->graphs.size() >= 16) drop_graphs(h);
@@ -918,12 +928,12 @@ static int run_postpass(Handle *h, int n, bool want_flags, double *err_acc, cons
 
 int run_postpass_slots(Handle *h, int n, const int32_t *slots) { return run_postpass(h, n, true, nullptr, slots); }
 
-int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named) {
+int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named, const uint8_t *named_h) {
     const SolveOptions o = solve_options(opt);
     init_ctrl_kernel<<<n, 32, 0, h->stream>>>(h->ctrl.d, 1e-8, o.radius0, o.max_iter, o.max_time, 0, named);
     ++h->launches;
     LAUNCH_CK(h, "init_ctrl_kernel");
-    return run_solve_loop(h, o, 0, n, h->stream, false);
+    return run_solve_loop(h, o, 0, n, h->stream, false, named_h);
 }
 
 int launch_layout_tail(Handle *h, const int32_t *slots, int n, bool prior) {
@@ -1152,7 +1162,9 @@ int pvio_b200_create(int device, int max_windows, int max_frames, int max_landma
     TRY(alloc(h, h->valid, W * M, kBoth, M)); TRY(alloc(h, h->quality, W * M, kBoth, M));
     // the reduced-system outputs of the linearise kernel (Hred, Hdd, gdir, gred, cost_vis: refresh_arrays) live in ONE
     // allocation so that the multi-CTA-per-window mode (atomic accumulation) needs a single memset per launch
-    h->sys_set = W * (npc * 36 + N * 36 + N * 6 + N * 6 + 1);   // set 1 of each array lies sys_set elements behind set 0
+    // set 1 of each array lies sys_set elements behind set 0, an even count: the Schur kernel pulls a window's Hred and
+    // gred of either set by bulk copies, which need 16-byte aligned addresses (W cost_vis entries make the sum odd for odd W)
+    h->sys_set = (W * (npc * 36 + N * 36 + N * 6 + N * 6 + 1) + 1) & ~(size_t)1;
     TRY(alloc(h, h->Hred, 2 * h->sys_set, kDevice));
     TRY(alloc(h, h->acc, W * kAcc, kBoth)); TRY(alloc(h, h->aux_cost, W, kDevice));
     TRY(alloc(h, h->Hfull, (15 * N) * (15 * N), kBoth)); TRY(alloc(h, h->gfull, 15 * N, kBoth));

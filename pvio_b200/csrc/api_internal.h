@@ -535,8 +535,9 @@ int ensure_inertial(Handle *h);
 // the pinned staging and the device arrays
 int ensure_planes(Handle *h, int T, int O);
 // the trust-region solve of windows [0, n); named (device, [n], may be NULL): only windows with named[w] != 0 are solved,
-// the others are marked finished before the first body and cost no iteration
-int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named);
+// the others are marked finished before the first body and cost no iteration; named_h: the same on the host (the
+// launches are shaped for the named windows only)
+int run_named_solve(Handle *h, const pvio_b200_options *opt, int n, const uint8_t *named, const uint8_t *named_h);
 int run_postpass_slots(Handle *h, int n, const int32_t *slots);   // post-pass of the n windows of a device list
 // the frame-major table of the n windows slots[0 .. n) (device list), and Lambda = S^T S of their priors when prior
 int launch_layout_tail(Handle *h, const int32_t *slots, int n, bool prior);

@@ -1109,7 +1109,7 @@ static int solve_slots(Handle *h, int n, const int32_t *slots, const pvio_b200_o
         CK(h, cudaGetLastError());
     }
     CK(h, cudaEventRecord(h->ev0, h->stream));
-    TRY(run_named_solve(h, opt, range, S.dev(nm)));
+    TRY(run_named_solve(h, opt, range, S.dev(nm), named.data()));
     CK(h, cudaEventRecord(h->ev1, h->stream));
     if (post) TRY(run_postpass_slots(h, n, S.dev(sl)));
     bw_writeback_kernel<<<n, kBwThreads, 0, h->stream>>>(launch_args<BwArgs>(h), S.dev(lay), post ? 1 : 0);

@@ -49,3 +49,69 @@ def test_landmark_formula_is_the_diagonal_of_the_inverse(k):
     assert np.array_equal(c2, cov[np.ix_(cols, cols)])
     if not w.use_inertial:
         assert w.frame_fixed.sum() == 2
+
+
+def _mp_spd_inverse(A):
+    """the inverse of a symmetric positive definite matrix of mpf entries (lists of rows) by Cholesky, at the working
+    mpmath precision: L L^T = A, W = L^-1 row by row, A^-1 = W^T W"""
+    import mpmath as mp
+    n = len(A)
+    L = [[mp.mpf(0)] * n for _ in range(n)]
+    for j in range(n):
+        Lj = L[j]
+        Lj[j] = mp.sqrt(A[j][j] - mp.fdot(Lj[:j], Lj[:j]))
+        for i in range(j + 1, n):
+            L[i][j] = (A[i][j] - mp.fdot(L[i][:j], Lj[:j])) / Lj[j]
+    W = [[mp.mpf(0)] * n for _ in range(n)]
+    for i in range(n):
+        W[i][i] = 1 / L[i][i]
+        for j in range(i):
+            W[i][j] = -mp.fdot(L[i][j:i], [W[k][j] for k in range(j, i)]) / L[i][i]
+    cols = [[W[k][j] for k in range(n)] for j in range(n)]
+    X = [[None] * n for _ in range(n)]
+    for i in range(n):
+        for j in range(i, n):
+            X[i][j] = X[j][i] = mp.fdot(cols[i][j:], cols[j][j:])
+    return X
+
+
+@pytest.mark.parametrize("case", ["inertial N 11", "visual N 16"])
+def test_refined_reference_matches_a_50_digit_inverse(case):
+    """the largest windows of test_gpu_batch_window_covariance_shapes.py (40 landmarks): the free-coordinate Schur
+    complement of the fp64 H formed and inverted in 50 digits, and Var(rho_l) = 1 / H_ll + h_l^T Sigma_ff h_l / H_ll^2
+    from it; cov_oracle.covariance(refine=True) agrees to 1e-12 on every frame block (relative to sqrt(C_ii C_jj)) and
+    every Var(rho), so that the GPU bars measure the kernels and not the reference"""
+    import mpmath as mp
+    if case.startswith("inertial"):
+        w, st = synth.make_cfg3(seed=1211, N=11, M=40)[:2]
+    else:
+        w, st = synth.make_cfg2(seed=1016, N=16, M=40)[:2]
+    H = ba_oracle.normal_equations(w, st)[0]
+    free = ba_oracle.free_mask(w)
+    n = 15 * w.N
+    ff, fl = np.flatnonzero(free[:n]), n + np.flatnonzero(free[n:])
+    with mp.workdps(50):
+        S = [[mp.mpf(x) for x in row] for row in H[np.ix_(ff, ff)].tolist()]
+        coup = []
+        for c in fl:                                     # S = H_ff - sum_l h_l h_l^T / H_ll (H_ll is diagonal)
+            nz = np.flatnonzero(H[ff, c])
+            h = [mp.mpf(H[ff[i], c]) for i in nz]
+            hll = mp.mpf(H[c, c])
+            coup.append((nz, h, hll))
+            for a, i in enumerate(nz):
+                hi = h[a] / hll
+                for b, j in enumerate(nz):
+                    S[i][j] -= hi * h[b]
+        X = _mp_spd_inverse(S)
+        var = [1 / hll + mp.fsum(h[a] * h[b] * X[i][j] for a, i in enumerate(nz) for b, j in enumerate(nz)) / hll ** 2
+               for nz, h, hll in coup]
+        Xf = np.array([[float(x) for x in row] for row in X])
+        vf = np.array([float(v) for v in var])
+    cov, v_ref, _ = cov_oracle.covariance(w, st, list(range(w.N)), list(range(w.M)), refine=True)
+    sub = cov[np.ix_(ff, ff)]
+    d = np.sqrt(np.diag(Xf))
+    e_cov = float(np.max(np.abs(sub - Xf) / np.outer(d, d)))
+    e_var = float(np.max(np.abs(v_ref[fl - n] - vf) / vf))
+    print(f"{case}: {len(ff)} frame coordinates, {len(fl)} landmarks, frames {e_cov:.3g}, Var(rho) {e_var:.3g}")
+    assert np.all(cov[~free[:n]] == 0)
+    assert e_cov < 1e-12 and e_var < 1e-12, (e_cov, e_var)

@@ -39,7 +39,7 @@ def _tracks(w, planes=True):
 def _feed(bw, slot, w, st, tracks, skip_obs_frame=None):
     """the window fed frame by frame into a slot (and its prior and planes when inertial); returns id -> track"""
     bw.reset(slot, w)
-    rec = _lib.PackedArgs(w, st).keep["imu"].reshape(-1, 288) if w.use_inertial else None
+    rec = _lib.PackedArgs(w, st).keep["imu"].reshape(-1, 288) if (w.use_inertial and w.N > 1) else None
     model = {}
     for f in range(w.N):
         e = Edit(slot).frame(np.concatenate([st.q[f], st.p[f], st.v[f], st.bg[f], st.ba[f]]), bool(w.frame_fixed[f]),
