@@ -405,6 +405,42 @@ typedef struct pvio_b200_window_landmarks {
     int32_t status;           /* out: PVIO_B200_OK or PVIO_B200_ENUMERIC                                               */
 } pvio_b200_window_landmarks; /* 72 bytes on LP64 */
 int pvio_b200_batch_window_landmarks(pvio_b200_handle h, int n, pvio_b200_window_landmarks *records);
+/* The state of each named inertial slot at any times inside its window, from the solved frames and the IMU samples its
+ * factors keep on the device (pvio_b200_batch_window_set_imu, track_camera / mirror_frame with keep_samples).  Factor k
+ * couples window frames k and k + 1; its samples s_0 .. s_{m-1} start at frame k's time (or up to 1e-5 s after it) and
+ * its t_end is frame k + 1's time.
+ *  - A time t is taken by the largest k whose factor holds samples and whose s_0.t <= t, when t <= that factor's t_end
+ *    or factor k + 1 holds samples too (the last increment then runs past t_end, over the gap before s_0 of k + 1).
+ *    Then  x(t) = PreIntegrator::predict(frame k's current state, delta),  delta = PreIntegrator::integrate(t, bg_k,
+ *    ba_k) over the factor's samples at or before t (the last one up to t), at frame k's current biases: the arithmetic
+ *    of pvio_b200_preintegrate and of the re-integration before a solve.  At t = s_0.t the state is frame k's, bit for
+ *    bit; at t = t_end, delta is the factor's full re-integration.
+ *  - This is a forward propagation from the preceding frame, not an interpolation between frames k and k + 1: at frame
+ *    k + 1 the trajectory jumps by the factor's residual at the solution.
+ *  - frame: the window frame k used; -1 for a time no factor with samples covers (before the first sample, past a
+ *    factor's t_end, over a factor without samples, after the newest frame: pvio_b200_batch_imu_stream_predict's
+ *    job).  Such a row has a zero state and a NaN covariance; it is not a rejection.
+ *  - state_cov (NULL: no covariance launches): Phi Sigma_k Phi^T + Psi Sigma_delta(t) Psi^T in the coordinates of
+ *    pvio_b200_batch_window_covariance ([dtheta dp dv dbg dba], q perturbed on the right), Sigma_k frame k's marginal
+ *    covariance as that call defines it, Phi and Psi those of pvio_b200_batch_imu_stream_set_covariance's FACTOR seed,
+ *    Sigma_delta(t) the partial integration's covariance itself; exactly symmetric.  status: PVIO_B200_ENUMERIC when the
+ *    slot's scaled H is not positive definite, with every covariance of the record NaN (the states are still written).
+ * Rejected (PVIO_B200_EINVAL, no output changed): n < 0; a slot out of range, not resident, visual-only or named twice;
+ * n_times < 0; times, states or frame NULL when n_times > 0; a time that is not finite or that decreases.  The call
+ * changes no slot.  Whatever n is: one host -> device copy, one kernel launch, one device -> host copy and one
+ * synchronisation; with covariances three launches more (the covariance call's linearise and Schur sweeps and
+ * cov_kernel over the records that ask for one). */
+typedef struct pvio_b200_window_trajectory {
+    int32_t slot;             /* resident inertial slot                                       */
+    int32_t n_times;          /* >= 0                                                         */
+    const double *times;      /* [n_times] finite, non-decreasing                             */
+    double *states;           /* out [n_times][16] q xyzw, p, v, bg, ba                       */
+    double *state_cov;        /* out [n_times][225] or NULL: no covariance launches           */
+    int32_t *frame;           /* out [n_times]: the window frame k used, -1: t not covered    */
+    int32_t status;           /* out: PVIO_B200_OK or PVIO_B200_ENUMERIC                      */
+    int32_t pad;
+} pvio_b200_window_trajectory; /* 48 bytes on LP64 */
+int pvio_b200_batch_window_trajectory(pvio_b200_handle h, int n, pvio_b200_window_trajectory *records);
 /* Device -> host in one copy, per named slot i: n_frames [n], frames [n][frames_stride] ([N][16]), n_tracks [n] (live
  * tracks), and for each live track in id order at [i * track_stride + r]: id, inverse depth, anchor frame, observation
  * count, and the post-pass valid / quality of the last solve (0 / 0 for a track that did not take part in it).  Any

@@ -156,6 +156,11 @@ class CWindowLandmarks(C.Structure):
                 ("inv_depth_var", c_f64p), ("n_rows", C.c_int32), ("status", C.c_int32)]
 
 
+class CWindowTrajectory(C.Structure):
+    _fields_ = [("slot", C.c_int32), ("n_times", C.c_int32), ("times", c_f64p), ("states", c_f64p), ("state_cov", c_f64p),
+                ("frame", c_i32p), ("status", C.c_int32), ("pad", C.c_int32)]
+
+
 class CWindowKeypoints(C.Structure):
     _fields_ = [("slot", C.c_int32), ("tracker_slot", C.c_int32), ("frame_id", C.c_uint64), ("n", C.c_int32),
                 ("track", c_i32p), ("keypoint", c_i32p), ("newest_is_keyframe", C.c_int32), ("skipped_frames", C.c_int32)]
@@ -270,6 +275,7 @@ SIGNATURES = {
     "pvio_b200_batch_window_drop_victim": (_int, [_h, _int, c_i32p, c_f64p, _i64, c_f64p, _i64]),
     "pvio_b200_batch_window_covariance": (_int, [_h, _int, _P(CWindowCovariance)]),
     "pvio_b200_batch_window_landmarks": (_int, [_h, _int, _P(CWindowLandmarks)]),
+    "pvio_b200_batch_window_trajectory": (_int, [_h, _int, _P(CWindowTrajectory)]),
     "pvio_b200_batch_window_download": (_int, [_h, _int, c_i32p, c_i32p, c_f64p, _i64, c_i32p, _i64, c_i32p, c_f64p,
                                                c_i32p, c_i32p, c_u8p, c_f64p]),
     "pvio_b200_batch_window_localize": (_int, [_h, _int, _P(CWindowLocalize), _P(COptions)]),

@@ -500,6 +500,32 @@ class BatchWindows:
             o["status"] = int(r.status)
         return out
 
+    def trajectory(self, slots, times, covariance=False):
+        """The state of each named inertial slot at the sorted times[i], forward from the window frame before each time
+        through the part of that frame's IMU factor's kept samples up to it (pvio_b200_batch_window_trajectory).  Per
+        record a dict: states [n, 16] (q xyzw, p, v, bg, ba), frame [n] (the window frame used, -1: a time no factor
+        with samples covers, with a zero state) and status; with covariance also state_cov [n, 15, 15] in the
+        coordinates of covariance(), NaN for an uncovered time and throughout when status is ENUMERIC."""
+        n = len(slots)
+        if len(times) != n:
+            raise ValueError("one time list per slot")
+        recs, out = (_lib.CWindowTrajectory * max(n, 1))(), []
+        for r, s, t in zip(recs, slots, times):
+            t = np.ascontiguousarray(t, dtype=np.float64).reshape(-1)
+            k = len(t)
+            o = dict(times=t, states=np.zeros((k, 16)), frame=np.zeros(k, dtype=np.int32))
+            if covariance:
+                o["state_cov"] = np.zeros((k, 15, 15))
+            out.append(o)
+            r.slot, r.n_times = int(s), k
+            _lib.set_ptrs(r, times=t if k else None, states=o["states"] if k else None, frame=o["frame"] if k else None,
+                          state_cov=o.get("state_cov") if k else None)
+        self.ba._ck(self.lib.pvio_b200_batch_window_trajectory(self.h, n, recs))
+        for r, o in zip(recs, out):
+            del o["times"]
+            o["status"] = int(r.status)
+        return out
+
     def save(self, slots, tracker_slots=None):
         """Save each sequence to host memory: per record a window slot (-1: none) and, from tracker_slots (None: none),
         a tracker slot of batch_feature_track (-1: none).  Returns one blob (bytes) per record, which restore() seats in

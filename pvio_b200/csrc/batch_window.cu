@@ -36,6 +36,7 @@
 #include "ba_cov_lm.cuh"
 #include "batch_window.cuh"
 #include "imu.cuh"
+#include "imu_factor_cov.cuh"
 #include "klt_border.cuh"
 #include "tri.cuh"
 
@@ -401,6 +402,22 @@ struct BwFactor {
 
 constexpr int kBwImuWarps = 4;
 
+// PreIntegrator::predict (preintegrator.cpp:102-109): the state y [16] a factor of length dt and delta (dq, dp, dv)
+// reaches from the state x [16]; the biases carry over
+__device__ __forceinline__ void bw_imu_predict(const double *x, double dt, const double *dq, const double *dp,
+                                               const double *dv, double *y) {
+    const double g[3] = {0.0, 0.0, -9.80665};                // PVIO_GRAVITY_NOMINAL, as ba_factors.cuh
+    double qdv[3], qdp[3];
+    bw_qrot(x, dv, qdv);
+    bw_qrot(x, dp, qdp);
+    for (int k = 0; k < 3; ++k) {
+        y[7 + k] = x[7 + k] + g[k] * dt + qdv[k];
+        y[4 + k] = x[4 + k] + 0.5 * g[k] * dt * dt + x[7 + k] * dt + qdp[k];
+    }
+    bw_qmul(x, dq, y);
+    for (int k = 10; k < 16; ++k) y[k] = x[k];
+}
+
 // Before a solve, one warp per factor with samples of the named slots: PreIntegrator::integrate(t, bg, ba, true, true)
 // at the biases the factor's first frame holds now (frame state doubles 10 .. 15), into the slot's IMU record -- the
 // arithmetic of pvio_b200_preintegrate (imu.cuh)
@@ -593,17 +610,8 @@ __global__ void __launch_bounds__(32 * kBwImuWarps) bw_track_integrate_kernel(Bw
     if (!T.tr[J.rec].merged)                                 // the edit takes the step-1 record
         for (int i = lane; i < kImuStride; i += 32) T.rec_out[(size_t)J.rec * kImuStride + i] = rec[i];
     if (lane == 0) {
-        const double g[3] = {0.0, 0.0, -9.80665};            // PVIO_GRAVITY_NOMINAL, as ba_factors.cuh
-        const double dt = rec[0];
-        double y[16], qdv[3], qdp[3];
-        bw_qrot(x, rec + 8, qdv);
-        bw_qrot(x, rec + 5, qdp);
-        for (int k = 0; k < 3; ++k) {
-            y[7 + k] = x[7 + k] + g[k] * dt + qdv[k];
-            y[4 + k] = x[4 + k] + 0.5 * g[k] * dt * dt + x[7 + k] * dt + qdp[k];
-        }
-        bw_qmul(x, rec + 1, y);
-        for (int k = 10; k < 16; ++k) y[k] = x[k];
+        double y[16];
+        bw_imu_predict(x, rec[0], rec + 1, rec + 5, rec + 8, y);
         for (int k = 0; k < 16; ++k) {
             L.frames[kFrameStride * (size_t)J.rec + k] = y[k];
             T.pred[kFrameStride * (size_t)J.rec + k] = y[k];
@@ -1687,6 +1695,146 @@ __global__ void __launch_bounds__(32 * kLmkWarps) bw_landmark_cov_kernel(BwArgs 
     if (lane == 0) *V = var;
 }
 
+// ---- pvio_b200_batch_window_trajectory: the state at any time inside the window, forward from the preceding frame
+// through the part of its IMU factor's kept samples up to that time, and its covariance
+struct BwTraj {
+    int32_t slot, N, n_times, cov;    // cov: index among the records with a covariance (-1: none asked; -2: asked, but
+                                      // no factor holds samples)
+    int64_t t_off;                    // rows into the call's times, states and frames
+    int64_t cov_off;                  // doubles into the covariance scratch: the joint block of the frames that own a
+                                      // factor with samples (CovRec::cov_off)
+    int64_t scov_off;                 // rows into the call's state covariances
+    int32_t ns[kMaxFrames];           // samples of factor k (frames k, k + 1), 0: none
+};
+static_assert(sizeof(BwTraj) % sizeof(double) == 0, "records are staged as whole 8-byte words");
+struct TrajArgs {
+    const BwTraj *rec;                // [n]
+    const double *times;              // [rows]
+    double *states;                   // out: [rows][16]
+    int32_t *frame;                   // out: [rows]
+    double *scov;                     // out: [cov rows][225]
+    const double *jcov;               // cov_kernel's joint blocks (scratch)
+    const int32_t *status;            // [n_cov] cov_kernel's status
+    int covs;                         // 1: the per-warp covariance scratch is laid out
+};
+// per warp of bw_trajectory_kernel: the chain, the emitted copy, then (with covariances) four 15 x 15 matrices
+__host__ __device__ constexpr size_t traj_warp_bytes(bool covs) { return 2 * sizeof(ImuWarpSm) + (covs ? 4 * 225 * 8 : 0); }
+
+// the first of the n sorted times t[i] that is >= x (upper: > x)
+__device__ __forceinline__ int traj_bound(const double *t, int n, double x, bool upper) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int m = (lo + hi) >> 1;
+        if (upper ? t[m] <= x : t[m] < x) lo = m + 1;
+        else hi = m;
+    }
+    return lo;
+}
+
+// queries [q0, q1) of record r, which no factor takes: frame -1, a zero state, a NaN covariance.  One warp.
+__device__ __forceinline__ void none_rows(const TrajArgs &T, const BwTraj &r, int lane, int q0, int q1, bool cov) {
+    for (int q = q0; q < q1; ++q) {
+        const size_t row = r.t_off + q;
+        if (lane < 16) T.states[16 * row + lane] = 0.0;
+        if (lane == 0) T.frame[row] = -1;
+        if (cov)
+            for (int e = lane; e < 225; e += 32) T.scov[225 * ((size_t)r.scov_off + q) + e] = CUDART_NAN;
+    }
+}
+
+// One CTA per record, one warp per factor k with samples (warp k).  The warp's queries are the times t >= s_0.t of its
+// factor and below s_0.t of the next factor with samples (so k is the largest such factor whose s_0.t <= t), found by
+// binary search; it takes those at most its t_end, or all of them when factor k + 1 holds samples.  It walks its
+// samples once, as imu_integrate_warp does (imu_step_warp), and emits each query as the walk passes it: the increment
+// of the last sample at or before t, over t - s_j.t, goes onto a copy of the chain, which is what imu_integrate_warp
+// gives for the samples at or before t with t_end = t.  Then PreIntegrator::predict from frame k's state, and with a
+// covariance Phi Sigma_k Phi^T + Psi Sigma_delta Psi^T (imu_factor_propagate), Sigma_delta the partial increment's
+// covariance itself.  Times no warp takes (before the first sample, past a factor's t_end, over a factor without
+// samples) get frame -1, a zero state and a NaN covariance: warp 0 writes those before the earliest s_0.t, each warp
+// those past its t_end.
+__global__ void __launch_bounds__(32 * (kMaxFrames - 1)) bw_trajectory_kernel(BwArgs a, TrajArgs T) {
+    extern __shared__ __align__(16) unsigned char traj_sm[];
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const BwTraj &r = T.rec[blockIdx.x];
+    const int nf = r.N - 1, nq = r.n_times;
+    const double *tq = T.times + r.t_off;
+    const size_t F0 = (size_t)r.slot * a.Ncap;
+    auto s0 = [&](int k) { return a.imu_s[(F0 + k) * a.Scap * 7]; };
+    const bool cov = r.cov != -1;                           // -2: covariances asked, no factor holds samples
+    const bool cov_ok = r.cov >= 0 && T.status[r.cov] == PVIO_B200_OK;
+    if (wv == 0) {
+        double lo = CUDART_INF;
+        for (int j = 0; j < nf; ++j)
+            if (r.ns[j] > 0) lo = fmin(lo, s0(j));
+        none_rows(T, r, lane, 0, traj_bound(tq, nq, lo, false), cov);
+    }
+    const int k = wv;
+    if (k >= nf || r.ns[k] == 0) return;
+    const size_t F = F0 + k;
+    const double lo = s0(k);
+    double hi = CUDART_INF;
+    for (int j = k + 1; j < nf; ++j)
+        if (r.ns[j] > 0) hi = fmin(hi, s0(j));
+    const double *aux = a.imu_aux + F * kImuAux, t_end = aux[0];
+    const int q0 = traj_bound(tq, nq, lo, false), q1 = max(q0, traj_bound(tq, nq, hi, false));
+    const int q2 = (k + 1 < nf && r.ns[k + 1] > 0) ? q1 : min(q1, max(q0, traj_bound(tq, nq, t_end, true)));
+    none_rows(T, r, lane, q2, q1, cov);
+    if (q0 >= q2) return;
+    unsigned char *base = traj_sm + (size_t)wv * traj_warp_bytes(T.covs);
+    ImuWarpSm &S = *reinterpret_cast<ImuWarpSm *>(base), &E = *reinterpret_cast<ImuWarpSm *>(base + sizeof(ImuWarpSm));
+    double *A = reinterpret_cast<double *>(base + 2 * sizeof(ImuWarpSm)), *B = A + 225, *C = B + 225, *D = C + 225;
+    const double *x = a.frames + F * kFrameStride;
+    const double bg[3] = {x[10], x[11], x[12]}, ba[3] = {x[13], x[14], x[15]};
+    const double *smp = a.imu_s + F * a.Scap * 7, *noise = aux + 1;
+    const int m = r.ns[k];
+    // Sigma_k: frame k's diagonal block of the joint covariance of the frames that own a factor with samples
+    unsigned has = 0;
+    for (int j = 0; j < nf; ++j) has |= (r.ns[j] > 0 ? 1u : 0u) << j;
+    const int K15 = 15 * __popc(has), p15 = 15 * __popc(has & ((1u << k) - 1u));
+    const double *Sk = T.jcov + r.cov_off + (size_t)p15 * K15 + p15;
+    imu_reset_warp(S, lane);
+    int q = q0;
+    for (int j = 0; j < m && q < q2; ++j) {
+        const double *d = smp + (size_t)j * 7;
+        const bool last = j + 1 == m;
+        const double t_next = last ? t_end : smp[(size_t)(j + 1) * 7];
+        for (; q < q2 && (last || tq[q] < t_next); ++q) {   // the queries whose last sample is s_j
+            imu_copy_warp(S, E, lane);
+            imu_step_warp(E, lane, d, tq[q] - d[0], bg, ba, noise);
+            const size_t row = r.t_off + q;
+            if (lane == 0) {
+                bw_imu_predict(x, E.tsum, E.q, E.p, E.v, T.states + 16 * row);
+                T.frame[row] = k;
+            }
+            if (!cov) continue;
+            double *out = T.scov + 225 * (size_t)(r.scov_off + q);
+            if (!cov_ok) {
+                for (int e = lane; e < 225; e += 32) out[e] = CUDART_NAN;
+                continue;
+            }
+            for (int e = lane; e < 225; e += 32) {
+                const int i = e / 15, c = e % 15;
+                A[e] = 0.5 * (Sk[(size_t)i * K15 + c] + Sk[(size_t)c * K15 + i]);
+                D[e] = (i < 9 && c < 9) ? E.C[i * 9 + c]
+                     : (i >= 9 && i < 12 && c >= 9 && c < 12) ? E.cbg[(i - 9) * 3 + c - 9]
+                     : (i >= 12 && c >= 12) ? E.cba[(i - 12) * 3 + c - 12] : 0.0;
+            }
+            __syncwarp();
+            double Rs[9], dR[9];
+            quat_to_mat(x, Rs);
+            quat_to_mat(E.q, dR);
+            const ImuFactorJac f{E.tsum, E.p, E.v, E.dq_dbg, E.dp_dbg, E.dp_dba, E.dv_dbg, E.dv_dba};
+            imu_factor_propagate(A, B, C, D, f, Rs, dR, lane);
+            for (int e = lane; e < 225; e += 32) {
+                const int i = e / 15, c = e % 15;
+                out[e] = 0.5 * ((A[e] + D[e]) + (A[c * 15 + i] + D[c * 15 + i]));
+            }
+            __syncwarp();
+        }
+        if (!last && q < q2) imu_step_warp(S, lane, d, t_next - d[0], bg, ba, noise);
+    }
+}
+
 }  // namespace pvio
 
 using namespace pvio;
@@ -2158,6 +2306,101 @@ int pvio_b200_batch_window_landmarks(pvio_b200_handle hh, int n, pvio_b200_windo
             R.status = S.host(st)[L.cov];
         }
         R.n_rows = (int32_t)nr;
+    }
+    return 0;
+}
+
+int pvio_b200_batch_window_trajectory(pvio_b200_handle hh, int n, pvio_b200_window_trajectory *records) {
+    Handle *h = reinterpret_cast<Handle *>(hh);
+    if (!h) return PVIO_B200_EINVAL;
+    const char *what = "batch_window_trajectory";
+    auto bad = [&](const char *why) { return fail(h, PVIO_B200_EINVAL, (std::string(what) + ": " + why).c_str()); };
+    if (n < 0 || (n > 0 && !records)) return bad("bad record list");
+    if (n == 0) return 0;
+    std::vector<int32_t> slots(n);
+    for (int i = 0; i < n; ++i) slots[i] = records[i].slot;
+    TRY(check_slots(h, n, slots.data(), "batch_window_trajectory: bad slot list"));
+    // every record checked before anything is staged
+    std::vector<BwTraj> recs(n);
+    std::vector<double> times;
+    std::vector<int32_t> cov_slots, frames;
+    std::vector<CovRec> crecs;
+    int64_t rows = 0, cov_rows = 0, jcov_n = 0, sig_n = 0;
+    int warps = 1;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_trajectory &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (!s.inertial) return bad("a visual-only slot");
+        if (R.n_times < 0) return bad("a negative time count");
+        if (R.n_times > 0 && (!R.times || !R.states || !R.frame)) return bad("times, states or frame missing");
+        for (int q = 0; q < R.n_times; ++q) {
+            if (!std::isfinite(R.times[q])) return bad("a time that is not finite");
+            if (q > 0 && R.times[q] < R.times[q - 1]) return bad("times that decrease");
+        }
+        BwTraj &T = recs[i];
+        T = BwTraj{};
+        T.slot = R.slot; T.N = s.N; T.n_times = R.n_times; T.cov = -1; T.t_off = rows; T.scov_off = cov_rows;
+        std::vector<int32_t> owners;
+        for (int k = 0; k + 1 < s.N; ++k) {
+            T.ns[k] = s.n_samples.empty() ? 0 : s.n_samples[k];
+            if (T.ns[k] > 0) owners.push_back(k);
+        }
+        warps = std::max(warps, s.N - 1);
+        if (R.state_cov && !owners.empty()) {        // Sigma_k of the frames that own a factor with samples
+            if (cov_smem_bytes(h->hdr.h[R.slot]) > 220 * 1024) return bad("reduced system too large for shared memory");
+            const int64_t K15 = 15 * (int64_t)owners.size(), D = 15 * (int64_t)s.N;
+            T.cov = (int32_t)cov_slots.size(); T.cov_off = jcov_n;
+            crecs.push_back(CovRec{R.slot, (int32_t)owners.size(), (int32_t)frames.size(), 0, jcov_n, sig_n});
+            frames.insert(frames.end(), owners.begin(), owners.end());
+            cov_slots.push_back(R.slot);
+            jcov_n += K15 * K15;
+            sig_n += D * D;
+        }
+        if (R.state_cov) {
+            if (T.cov < 0) T.cov = -2;               // NaN rows only: no factor holds samples
+            cov_rows += R.n_times;
+        }
+        times.insert(times.end(), R.times, R.times + R.n_times);
+        rows += R.n_times;
+    }
+    const int n_cov = (int)cov_slots.size();
+    const bool any_cov = cov_rows > 0;
+    Stage S(h->bw.stage, &h->bw.scratch);
+    const auto rec = S.up(recs);
+    const auto tm = S.up(times);
+    const auto cr = S.up(crecs);
+    const auto fr = S.up(frames);
+    const auto csl = S.up(cov_slots);
+    const auto sto = S.add<double>(Stage::kDown, 16 * (size_t)rows);
+    const auto fro = S.add<int32_t>(Stage::kDown, (size_t)rows);
+    const auto sco = S.add<double>(Stage::kDown, 225 * (size_t)cov_rows);
+    const auto st = S.add<int32_t>(Stage::kDown, n_cov);
+    const auto jc = S.add<double>(Stage::kScratch, (size_t)jcov_n);
+    const auto sig = S.add<double>(Stage::kScratch, (size_t)sig_n);
+    const auto sxi = S.add<double>(Stage::kScratch, (size_t)n_cov * h->Ncap * h->Ncap * 36);
+    TRY(S.place(h, true));
+    if (n_cov > 0)
+        TRY(run_cov_system(h, n_cov, cov_slots.data(), S.dev(csl),
+                           CovLaunch{S.dev(cr), S.dev(fr), nullptr, 0, S.dev(jc), nullptr, S.dev(st), S.dev(sig), S.dev(sxi)}));
+    const TrajArgs T{S.dev(rec), S.dev(tm), S.dev(sto), S.dev(fro), S.dev(sco), S.dev(jc), S.dev(st), any_cov ? 1 : 0};
+    const size_t smem = warps * traj_warp_bytes(any_cov);
+    if (smem > 48 * 1024)
+        CK(h, cudaFuncSetAttribute(bw_trajectory_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    bw_trajectory_kernel<<<n, 32 * warps, smem, h->stream>>>(launch_args<BwArgs>(h), T);
+    ++h->launches;
+    CK(h, cudaGetLastError());
+    TRY(S.download(h));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_window_trajectory &R = records[i];
+        const BwTraj &T = recs[i];
+        const size_t nq = R.n_times;
+        if (nq > 0) {
+            memcpy(R.states, S.host(sto) + 16 * (size_t)T.t_off, sizeof(double) * 16 * nq);
+            memcpy(R.frame, S.host(fro) + T.t_off, sizeof(int32_t) * nq);
+            if (R.state_cov) memcpy(R.state_cov, S.host(sco) + 225 * (size_t)T.scov_off, sizeof(double) * 225 * nq);
+        }
+        R.status = T.cov >= 0 ? S.host(st)[T.cov] : PVIO_B200_OK;
     }
     return 0;
 }

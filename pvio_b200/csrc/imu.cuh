@@ -51,6 +51,127 @@ static __device__ void sqrt_inv_block(const double *C, int n, int ld, double *U,
     }
 }
 
+// PreIntegrator::reset (:25-30): the warp's chain state S to the empty increment
+__device__ __forceinline__ void imu_reset_warp(ImuWarpSm &S, int lane) {
+    for (int i = lane; i < 81; i += 32) S.C[i] = 0.0;
+    if (lane < 9) { S.cbg[lane] = 0.0; S.cba[lane] = 0.0; S.dq_dbg[lane] = 0.0; S.dp_dbg[lane] = 0.0; S.dp_dba[lane] = 0.0;
+                    S.dv_dbg[lane] = 0.0; S.dv_dba[lane] = 0.0; }
+    if (lane == 0) { S.q[0] = S.q[1] = S.q[2] = 0.0; S.q[3] = 1.0; S.tsum = 0.0;
+                     for (int k = 0; k < 3; ++k) { S.p[k] = 0.0; S.v[k] = 0.0; } }
+    __syncwarp();
+}
+
+// the warp's chain state S into D: everything imu_step_warp carries from one sample to the next
+__device__ __forceinline__ void imu_copy_warp(const ImuWarpSm &S, ImuWarpSm &D, int lane) {
+    for (int i = lane; i < 81; i += 32) D.C[i] = S.C[i];
+    if (lane < 9) { D.cbg[lane] = S.cbg[lane]; D.cba[lane] = S.cba[lane]; D.dq_dbg[lane] = S.dq_dbg[lane];
+                    D.dp_dbg[lane] = S.dp_dbg[lane]; D.dp_dba[lane] = S.dp_dba[lane]; D.dv_dbg[lane] = S.dv_dbg[lane];
+                    D.dv_dba[lane] = S.dv_dba[lane]; }
+    if (lane == 0) { for (int k = 0; k < 4; ++k) D.q[k] = S.q[k];
+                     for (int k = 0; k < 3; ++k) { D.p[k] = S.p[k]; D.v[k] = S.v[k]; }
+                     D.tsum = S.tsum; }
+    __syncwarp();
+}
+
+// PreIntegrator::increment (:39-81) of one sample d ([7] t, w xyz, a xyz) over dt, on the warp's chain state S; noise
+// [4][9] cov_w, cov_a, cov_bg, cov_ba.  imu_integrate_warp runs it per sample; the trajectory kernel (batch_window.cu)
+// runs it on a copy of the chain to stop the integration at a query time, so both give the same bits.
+__device__ __forceinline__ void imu_step_warp(ImuWarpSm &S, int lane, const double *d, double dt, const double bg[3],
+                                              const double ba[3], const double *noise) {
+    const double w[3] = {d[1] - bg[0], d[2] - bg[1], d[3] - bg[2]};                       // :42-43
+    const double acc[3] = {d[4] - ba[0], d[5] - ba[1], d[6] - ba[2]};
+    if (lane == 0) {
+        const double th[3] = {w[0] * dt, w[1] * dt, w[2] * dt};
+        double qi[4], qc[4], Ha[9];
+        expmap(th, qi);
+        quat_conj(qi, qc);
+        quat_to_mat(qc, S.Ri);
+        right_jacobian(th, S.Jr);
+        quat_to_mat(S.q, S.Rd);
+        hat(acc, Ha);
+        mat3_mul(S.Rd, Ha, S.M);
+        mat3_vec(S.Rd, acc, S.Ra);
+        S.dt = dt;
+    }
+    __syncwarp();
+    // noise blocks: Nw = Jr cov_w Jr^T, Na = Rd cov_a Rd^T (lanes 0-8, 9-17)
+    if (lane < 18) {
+        const double *X = lane < 9 ? S.Jr : S.Rd, *Q = noise + (lane < 9 ? 0 : 9);
+        const int e = lane % 9, i = e / 3, j = e % 3;
+        double sacc = 0.0;
+        for (int k = 0; k < 3; ++k)
+            for (int m = 0; m < 3; ++m) sacc += X[i * 3 + k] * Q[k * 3 + m] * X[j * 3 + m];
+        (lane < 9 ? S.Nw : S.Na)[e] = sacc;
+    }
+    // T = A C with A = [[Ri, 0, 0], [Pq, I, dt I], [Vq, 0, I]], Vq = -dt M, Pq = -dt^2/2 M   (:46-51)
+    for (int e = lane; e < 81; e += 32) {
+        const int r = e / 9, c = e % 9;
+        double t = 0.0;
+        if (r < 3) { for (int k = 0; k < 3; ++k) t += S.Ri[r * 3 + k] * S.C[k * 9 + c]; }
+        else if (r < 6) {
+            for (int k = 0; k < 3; ++k) t += S.M[(r - 3) * 3 + k] * S.C[k * 9 + c];
+            t = -0.5 * dt * dt * t + S.C[r * 9 + c] + dt * S.C[(r + 3) * 9 + c];
+        } else {
+            for (int k = 0; k < 3; ++k) t += S.M[(r - 6) * 3 + k] * S.C[k * 9 + c];
+            t = -dt * t + S.C[r * 9 + c];
+        }
+        S.T[e] = t;
+    }
+    __syncwarp();
+    // C = T A^T + B Q B^T   (:53-65)
+    const double inv_dt = 1.0 / fmax(dt, 1.0e-7);
+    for (int e = lane; e < 81; e += 32) {
+        const int r = e / 9, c = e % 9;
+        double t = 0.0;
+        if (c < 3) { for (int k = 0; k < 3; ++k) t += S.T[r * 9 + k] * S.Ri[c * 3 + k]; }
+        else if (c < 6) {
+            for (int k = 0; k < 3; ++k) t += S.T[r * 9 + k] * S.M[(c - 3) * 3 + k];
+            t = -0.5 * dt * dt * t + S.T[r * 9 + c] + dt * S.T[r * 9 + c + 3];
+        } else {
+            for (int k = 0; k < 3; ++k) t += S.T[r * 9 + k] * S.M[(c - 6) * 3 + k];
+            t = -dt * t + S.T[r * 9 + c];
+        }
+        const int rb = r / 3, cb = c / 3, ri = r % 3, ci = c % 3;
+        double nz = 0.0;
+        if (rb == 0 && cb == 0) nz = dt * dt * inv_dt * S.Nw[ri * 3 + ci];
+        else if (rb == 1 && cb == 1) nz = 0.25 * dt * dt * dt * dt * inv_dt * S.Na[ri * 3 + ci];
+        else if (rb == 2 && cb == 2) nz = dt * dt * inv_dt * S.Na[ri * 3 + ci];
+        else if (rb + cb == 3 && rb != 0 && cb != 0) nz = 0.5 * dt * dt * dt * inv_dt * S.Na[ri * 3 + ci];
+        S.C[e] = t + nz;
+    }
+    // bias Jacobians (:71-75: dp first, then dv, then dq, each from the OLD values) and bias covariances (:66-67)
+    double n_dp_dbg = 0.0, n_dp_dba = 0.0, n_dv_dbg = 0.0, n_dv_dba = 0.0, n_dq_dbg = 0.0;
+    if (lane < 9) {
+        const int i = lane / 3, j = lane % 3;
+        double mq = 0.0, rq = 0.0;
+        for (int k = 0; k < 3; ++k) { mq += S.M[i * 3 + k] * S.dq_dbg[k * 3 + j]; rq += S.Ri[i * 3 + k] * S.dq_dbg[k * 3 + j]; }
+        n_dp_dbg = S.dp_dbg[lane] + dt * S.dv_dbg[lane] - 0.5 * dt * dt * mq;
+        n_dp_dba = S.dp_dba[lane] + dt * S.dv_dba[lane] - 0.5 * dt * dt * S.Rd[lane];
+        n_dv_dbg = S.dv_dbg[lane] - dt * mq;
+        n_dv_dba = S.dv_dba[lane] - dt * S.Rd[lane];
+        n_dq_dbg = rq - dt * S.Jr[lane];
+        S.cbg[lane] += noise[18 + lane] * dt;
+        S.cba[lane] += noise[27 + lane] * dt;
+    }
+    __syncwarp();
+    if (lane < 9) { S.dp_dbg[lane] = n_dp_dbg; S.dp_dba[lane] = n_dp_dba; S.dv_dbg[lane] = n_dv_dbg; S.dv_dba[lane] = n_dv_dba;
+                    S.dq_dbg[lane] = n_dq_dbg; }
+    if (lane == 0) {                                                                      // :78-81
+        S.tsum += dt;
+        for (int k = 0; k < 3; ++k) {
+            S.p[k] += dt * S.v[k] + 0.5 * dt * dt * S.Ra[k];
+            S.v[k] += dt * S.Ra[k];
+        }
+        const double th[3] = {w[0] * dt, w[1] * dt, w[2] * dt};
+        double qi[4], qn[4];
+        expmap(th, qi);
+        quat_mul(S.q, qi, qn);
+        const double nrm = sqrt(qn[0] * qn[0] + qn[1] * qn[1] + qn[2] * qn[2] + qn[3] * qn[3]);
+        for (int k = 0; k < 4; ++k) S.q[k] = qn[k] / nrm;
+    }
+    __syncwarp();
+}
+
 // One factor on one warp (S: the warp's shared scratch); bg / ba the biases of the factor's first frame.  F describes
 // the factor where the kernel keeps it: F.samples ([*][7] t, w xyz, a xyz) rows F.begin() .. F.end() - 1 (at least
 // one), the last integrated up to F.t_end(); F.noise [4][9] cov_w, cov_a, cov_bg, cov_ba; F.rec() the record
@@ -58,109 +179,12 @@ static __device__ void sqrt_inv_block(const double *C, int n, int ld, double *U,
 template <typename Factor>
 __device__ __forceinline__ void imu_integrate_warp(ImuWarpSm &S, int lane, const Factor &F, const double bg[3],
                                                    const double ba[3]) {
-    for (int i = lane; i < 81; i += 32) S.C[i] = 0.0;
-    if (lane < 9) { S.cbg[lane] = 0.0; S.cba[lane] = 0.0; S.dq_dbg[lane] = 0.0; S.dp_dbg[lane] = 0.0; S.dp_dba[lane] = 0.0;
-                    S.dv_dbg[lane] = 0.0; S.dv_dba[lane] = 0.0; }
-    if (lane == 0) { S.q[0] = S.q[1] = S.q[2] = 0.0; S.q[3] = 1.0; S.tsum = 0.0;
-                     for (int k = 0; k < 3; ++k) { S.p[k] = 0.0; S.v[k] = 0.0; } }
-    __syncwarp();
+    imu_reset_warp(S, lane);
     const int b0 = F.begin(), b1 = F.end();
     for (int s = b0; s < b1; ++s) {
         const double *d = F.samples + (size_t)s * 7;
         const double t_next = (s + 1 < b1) ? F.samples[(size_t)(s + 1) * 7] : F.t_end();      // :89-92
-        const double dt = t_next - d[0];
-        const double w[3] = {d[1] - bg[0], d[2] - bg[1], d[3] - bg[2]};                       // :42-43
-        const double acc[3] = {d[4] - ba[0], d[5] - ba[1], d[6] - ba[2]};
-        if (lane == 0) {
-            const double th[3] = {w[0] * dt, w[1] * dt, w[2] * dt};
-            double qi[4], qc[4], Ha[9];
-            expmap(th, qi);
-            quat_conj(qi, qc);
-            quat_to_mat(qc, S.Ri);
-            right_jacobian(th, S.Jr);
-            quat_to_mat(S.q, S.Rd);
-            hat(acc, Ha);
-            mat3_mul(S.Rd, Ha, S.M);
-            mat3_vec(S.Rd, acc, S.Ra);
-            S.dt = dt;
-        }
-        __syncwarp();
-        // noise blocks: Nw = Jr cov_w Jr^T, Na = Rd cov_a Rd^T (lanes 0-8, 9-17)
-        if (lane < 18) {
-            const double *X = lane < 9 ? S.Jr : S.Rd, *Q = F.noise + (lane < 9 ? 0 : 9);
-            const int e = lane % 9, i = e / 3, j = e % 3;
-            double sacc = 0.0;
-            for (int k = 0; k < 3; ++k)
-                for (int m = 0; m < 3; ++m) sacc += X[i * 3 + k] * Q[k * 3 + m] * X[j * 3 + m];
-            (lane < 9 ? S.Nw : S.Na)[e] = sacc;
-        }
-        // T = A C with A = [[Ri, 0, 0], [Pq, I, dt I], [Vq, 0, I]], Vq = -dt M, Pq = -dt^2/2 M   (:46-51)
-        for (int e = lane; e < 81; e += 32) {
-            const int r = e / 9, c = e % 9;
-            double t = 0.0;
-            if (r < 3) { for (int k = 0; k < 3; ++k) t += S.Ri[r * 3 + k] * S.C[k * 9 + c]; }
-            else if (r < 6) {
-                for (int k = 0; k < 3; ++k) t += S.M[(r - 3) * 3 + k] * S.C[k * 9 + c];
-                t = -0.5 * dt * dt * t + S.C[r * 9 + c] + dt * S.C[(r + 3) * 9 + c];
-            } else {
-                for (int k = 0; k < 3; ++k) t += S.M[(r - 6) * 3 + k] * S.C[k * 9 + c];
-                t = -dt * t + S.C[r * 9 + c];
-            }
-            S.T[e] = t;
-        }
-        __syncwarp();
-        // C = T A^T + B Q B^T   (:53-65)
-        const double inv_dt = 1.0 / fmax(dt, 1.0e-7);
-        for (int e = lane; e < 81; e += 32) {
-            const int r = e / 9, c = e % 9;
-            double t = 0.0;
-            if (c < 3) { for (int k = 0; k < 3; ++k) t += S.T[r * 9 + k] * S.Ri[c * 3 + k]; }
-            else if (c < 6) {
-                for (int k = 0; k < 3; ++k) t += S.T[r * 9 + k] * S.M[(c - 3) * 3 + k];
-                t = -0.5 * dt * dt * t + S.T[r * 9 + c] + dt * S.T[r * 9 + c + 3];
-            } else {
-                for (int k = 0; k < 3; ++k) t += S.T[r * 9 + k] * S.M[(c - 6) * 3 + k];
-                t = -dt * t + S.T[r * 9 + c];
-            }
-            const int rb = r / 3, cb = c / 3, ri = r % 3, ci = c % 3;
-            double nz = 0.0;
-            if (rb == 0 && cb == 0) nz = dt * dt * inv_dt * S.Nw[ri * 3 + ci];
-            else if (rb == 1 && cb == 1) nz = 0.25 * dt * dt * dt * dt * inv_dt * S.Na[ri * 3 + ci];
-            else if (rb == 2 && cb == 2) nz = dt * dt * inv_dt * S.Na[ri * 3 + ci];
-            else if (rb + cb == 3 && rb != 0 && cb != 0) nz = 0.5 * dt * dt * dt * inv_dt * S.Na[ri * 3 + ci];
-            S.C[e] = t + nz;
-        }
-        // bias Jacobians (:71-75: dp first, then dv, then dq, each from the OLD values) and bias covariances (:66-67)
-        double n_dp_dbg = 0.0, n_dp_dba = 0.0, n_dv_dbg = 0.0, n_dv_dba = 0.0, n_dq_dbg = 0.0;
-        if (lane < 9) {
-            const int i = lane / 3, j = lane % 3;
-            double mq = 0.0, rq = 0.0;
-            for (int k = 0; k < 3; ++k) { mq += S.M[i * 3 + k] * S.dq_dbg[k * 3 + j]; rq += S.Ri[i * 3 + k] * S.dq_dbg[k * 3 + j]; }
-            n_dp_dbg = S.dp_dbg[lane] + dt * S.dv_dbg[lane] - 0.5 * dt * dt * mq;
-            n_dp_dba = S.dp_dba[lane] + dt * S.dv_dba[lane] - 0.5 * dt * dt * S.Rd[lane];
-            n_dv_dbg = S.dv_dbg[lane] - dt * mq;
-            n_dv_dba = S.dv_dba[lane] - dt * S.Rd[lane];
-            n_dq_dbg = rq - dt * S.Jr[lane];
-            S.cbg[lane] += F.noise[18 + lane] * dt;
-            S.cba[lane] += F.noise[27 + lane] * dt;
-        }
-        __syncwarp();
-        if (lane < 9) { S.dp_dbg[lane] = n_dp_dbg; S.dp_dba[lane] = n_dp_dba; S.dv_dbg[lane] = n_dv_dbg; S.dv_dba[lane] = n_dv_dba;
-                        S.dq_dbg[lane] = n_dq_dbg; }
-        if (lane == 0) {                                                                      // :78-81
-            S.tsum += dt;
-            for (int k = 0; k < 3; ++k) {
-                S.p[k] += dt * S.v[k] + 0.5 * dt * dt * S.Ra[k];
-                S.v[k] += dt * S.Ra[k];
-            }
-            const double th[3] = {w[0] * dt, w[1] * dt, w[2] * dt};
-            double qi[4], qn[4];
-            expmap(th, qi);
-            quat_mul(S.q, qi, qn);
-            const double nrm = sqrt(qn[0] * qn[0] + qn[1] * qn[1] + qn[2] * qn[2] + qn[3] * qn[3]);
-            for (int k = 0; k < 4; ++k) S.q[k] = qn[k] / nrm;
-        }
-        __syncwarp();
+        imu_step_warp(S, lane, d, t_next - d[0], bg, ba, F.noise);
     }
     // ---- record
     double *rec = F.rec();

@@ -12,6 +12,7 @@
 #include <cmath>
 #include "api_internal.h"
 #include "ba_math.cuh"
+#include "imu_factor_cov.cuh"
 #include "quat.cuh"
 
 namespace pvio {
@@ -800,25 +801,8 @@ struct StreamSeedRec {                // one set_covariance record as staged
     double noise[36];
 };
 
-// C = A B (bt: A B^T), 15 x 15, by the warp's lanes
-__device__ void warp_mm15(const double *A, const double *B, double *C, bool bt, int lane) {
-    for (int e = lane; e < 225; e += 32) {
-        const int i = e / 15, j = e % 15;
-        double s = 0.0;
-        for (int m = 0; m < 15; ++m) s += A[i * 15 + m] * (bt ? B[j * 15 + m] : B[m * 15 + j]);
-        C[e] = s;
-    }
-    __syncwarp();
-}
-
-// 3 x 3 block (bi, bj) of the 15 x 15 M set to s X (X row-major 3 x 3, or the identity when null)
-__device__ void put_block(double *M, int bi, int bj, const double *X, double s = 1.0) {
-    for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) M[(3 * bi + r) * 15 + 3 * bj + c] = X ? s * X[3 * r + c] : (r == c ? s : 0.0);
-}
-
-// One warp per record.  DIRECT: the symmetrised cov.  FACTOR: Phi Sigma_src Phi^T + Psi Sigma_d Psi^T (header), with
-// Sigma_d = U^-1 U^-T from the factor's upper-triangular U = sqrt_inv_cov.
+// One warp per record.  DIRECT: the symmetrised cov.  FACTOR: Phi Sigma_src Phi^T + Psi Sigma_d Psi^T
+// (imu_factor_propagate), with Sigma_d = U^-1 U^-T from the factor's upper-triangular U = sqrt_inv_cov.
 __global__ void __launch_bounds__(32 * kCovWarps) imu_stream_seed_kernel(int n, const StreamSeedRec *recs,
                                                                          const ImuStreamSlot *hdr, double *cov) {
     __shared__ double sm[kCovWarps][4][225];
@@ -830,12 +814,11 @@ __global__ void __launch_bounds__(32 * kCovWarps) imu_stream_seed_kernel(int n, 
     for (int e = lane; e < 225; e += 32) {
         const int r = e / 15, c = e % 15;
         A[e] = 0.5 * (R.cov[r * 15 + c] + R.cov[c * 15 + r]);
-        B[e] = 0.0;
         D[e] = 0.0;
     }
     __syncwarp();
     if (R.mode == PVIO_B200_IMU_STREAM_COV_FACTOR) {
-        const double *rec = R.imu, *dq = rec + PVIO_B200_IMU_DQ, T = rec[PVIO_B200_IMU_DT];
+        const double *rec = R.imu, *dq = rec + PVIO_B200_IMU_DQ;
         double qs[4], Rs[9], dR[9];
         {
             double ci[4];
@@ -844,35 +827,6 @@ __global__ void __launch_bounds__(32 * kCovWarps) imu_stream_seed_kernel(int n, 
             quat_to_mat(qs, Rs);
             quat_to_mat(dq, dR);
         }
-        if (lane == 0) {                                 // Phi into B
-            double H[9], X[9], Xt[9];
-            for (int r = 0; r < 3; ++r)
-                for (int c = 0; c < 3; ++c) Xt[3 * r + c] = dR[3 * c + r];
-            put_block(B, 0, 0, Xt);
-            put_block(B, 0, 3, rec + PVIO_B200_IMU_DQ_DBG);
-            hat(rec + PVIO_B200_IMU_DP, H);
-            mat3_mul(Rs, H, X);
-            put_block(B, 1, 0, X, -1.0);
-            put_block(B, 1, 1, nullptr);
-            put_block(B, 1, 2, nullptr, T);
-            mat3_mul(Rs, rec + PVIO_B200_IMU_DP_DBG, X);
-            put_block(B, 1, 3, X);
-            mat3_mul(Rs, rec + PVIO_B200_IMU_DP_DBA, X);
-            put_block(B, 1, 4, X);
-            hat(rec + PVIO_B200_IMU_DV, H);
-            mat3_mul(Rs, H, X);
-            put_block(B, 2, 0, X, -1.0);
-            put_block(B, 2, 2, nullptr);
-            mat3_mul(Rs, rec + PVIO_B200_IMU_DV_DBG, X);
-            put_block(B, 2, 3, X);
-            mat3_mul(Rs, rec + PVIO_B200_IMU_DV_DBA, X);
-            put_block(B, 2, 4, X);
-            put_block(B, 3, 3, nullptr);
-            put_block(B, 4, 4, nullptr);
-        }
-        __syncwarp();
-        warp_mm15(B, A, C, false, lane);                 // Phi Sigma_src
-        warp_mm15(C, B, A, true, lane);                  // .. Phi^T, into A
         if (lane < 15) {                                 // column `lane` of U^-1 into C, by back substitution
             const double *U = rec + PVIO_B200_IMU_SQRT_INV_COV;
             const int j = lane;
@@ -886,17 +840,10 @@ __global__ void __launch_bounds__(32 * kCovWarps) imu_stream_seed_kernel(int n, 
         }
         __syncwarp();
         warp_mm15(C, C, D, true, lane);                  // Sigma_d = U^-1 U^-T
-        if (lane == 0) {                                 // Psi into B
-            for (int e = 0; e < 225; ++e) B[e] = 0.0;
-            put_block(B, 0, 0, nullptr);
-            put_block(B, 1, 1, Rs);
-            put_block(B, 2, 2, Rs);
-            put_block(B, 3, 3, nullptr);
-            put_block(B, 4, 4, nullptr);
-        }
-        __syncwarp();
-        warp_mm15(B, D, C, false, lane);                 // Psi Sigma_d
-        warp_mm15(C, B, D, true, lane);                  // .. Psi^T, into D
+        const ImuFactorJac f{rec[PVIO_B200_IMU_DT], rec + PVIO_B200_IMU_DP, rec + PVIO_B200_IMU_DV,
+                             rec + PVIO_B200_IMU_DQ_DBG, rec + PVIO_B200_IMU_DP_DBG, rec + PVIO_B200_IMU_DP_DBA,
+                             rec + PVIO_B200_IMU_DV_DBG, rec + PVIO_B200_IMU_DV_DBA};
+        imu_factor_propagate(A, B, C, D, f, Rs, dR, lane);
     }
     double *out = cov + (size_t)R.slot * kStreamCovStride;
     for (int e = lane; e < 225; e += 32) {
