@@ -345,6 +345,13 @@ __device__ __forceinline__ void row_prefetch(RowCursor &pf, int r_end, const flo
 // part: the per-warp partial sums [nwarps][Mp] of the CTA's shared memory (lin_obs_kernel with lm_part), each a sum
 // in frame order; summed here in warp order, which is again frame order.  nullptr: the per-block pairs in jr.
 // lr_pre: the landmark's record, already loaded by the caller (nullptr: loaded here).
+// the whole 32-byte record in two 16-byte stores (three 8-byte ones would touch each of its sectors three times)
+__device__ __forceinline__ void lm_aux_store(LmAux *p, double hll_reg, double gl, double hll) {
+    double2 *q = reinterpret_cast<double2 *>(p);
+    q[0] = make_double2(hll_reg, gl);
+    q[1] = make_double2(hll, 0.0);
+}
+
 template <typename real>
 __device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N, int M, unsigned fixed, double mu, int compute_scale,
                                           const double2 *part = nullptr, int nwarps = 0, int Mp = 0, const LmRec *lr_pre = nullptr) {
@@ -360,7 +367,7 @@ __device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N
     LmAux *aux = a.lm_aux + (size_t)w * a.Mcap;
     if (!live) {
         wv[l] = mk2((real)0, (real)0); msk[l] = 0;
-        if (!a.victim_only) { aux[l].hll_reg = 1.0; aux[l].gl = 0.0; aux[l].hll = 0.0; }
+        if (!a.victim_only) lm_aux_store(aux + l, 1.0, 0.0, 0.0);
         return;
     }
     real *hs = reinterpret_cast<real *>(a.hs) + (size_t)w * a.Ncap * a.Mcap * 6;
@@ -385,7 +392,7 @@ __device__ __forceinline__ void lm_finish(const PipeArgs &a, int w, int l, int N
     const double hreg = hll + (mu > 0.0 ? lm_reg(hll, sc, mu) : 0.0);
     const double wl = 1.0 / hreg;
     const bool finite = isfinite(wl);
-    aux[l].hll_reg = hreg; aux[l].gl = gl; aux[l].hll = hll;
+    lm_aux_store(aux + l, hreg, gl, hll);
     const real wr = finite ? (real)wl : (real)0;
     wv[l] = mk2(wr, wr * (real)gl);
     msk[l] = finite ? (int)(targets | (1u << anchor)) : 0;
@@ -745,13 +752,13 @@ lin_obs_kernel(PipeArgs a_in) {
         if (exclusive) { Hdd_o[e] = d; Hred_o[pair_idx(f, f) * 36 + ij] = d; }
         else if (d != 0.0) { atomicAdd(&Hdd_o[e], d); atomicAdd(&Hred_o[pair_idx(f, f) * 36 + ij], d); }
     }
+    int fo = 1;                                                     // sq grows with e: fo only moves on (at most N - 2 steps)
     for (int e = tid; e < nsp * 36; e += kThreads) {                // off-diagonal blocks (f > g): -D(f, g)
         const int sq = e / 36, ij = e - sq * 36, i = ij / 6, j = ij - i * 6;
-        int f = 1;
-        while ((f + 1) * f / 2 <= sq) ++f;
-        const int g = sq - f * (f - 1) / 2;
+        while ((fo + 1) * fo / 2 <= sq) ++fo;
+        const int g = sq - fo * (fo - 1) / 2;
         const double v = -Dta[sq * kDta + (i <= j ? sym6(i, j) : sym6(j, i))];
-        if (exclusive) Hred_o[pair_idx(f, g) * 36 + ij] = v; else if (v != 0.0) atomicAdd(&Hred_o[pair_idx(f, g) * 36 + ij], v);
+        if (exclusive) Hred_o[pair_idx(fo, g) * 36 + ij] = v; else if (v != 0.0) atomicAdd(&Hred_o[pair_idx(fo, g) * 36 + ij], v);
     }
     for (int e = tid; e < N * 6; e += kThreads) {                   // gradients
         const double d = Ddg[(e / 6) * kDta + 21 + e % 6];
