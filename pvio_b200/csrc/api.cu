@@ -285,11 +285,11 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
             if (w->pt_obs_frame[i] < 0 || w->pt_obs_frame[i] >= N) return fail(h, PVIO_B200_EINVAL, "pt_obs_frame out of range");
     }
     if (n_imu > 0 || n_prior > 0 || inertial) TRY(ensure_inertial(h));
-    ws.resident = false;                  // a packed slot is no longer a resident window
-    ws.n_samples.clear();                 // and its IMU factors hold no samples
-    ws.perm.clear();                      // until the landmark order below is known
-    WinHdr &H = h->hdr.h[slot];
-    WinConst &C = h->cst.h[slot];
+    // the slot's header and bookkeeping are replaced only once the whole window is accepted: batch_shape sizes the
+    // launches and scatter_dx the downloads of the windows already uploaded by them, so a rejected window (e.g. one
+    // that needs a 97th chunk) must leave them as they were
+    WinHdr H;
+    WinConst C;
     memset(&H, 0, sizeof(H));
     H.N = N; H.M = M; H.K = K; H.use_inertial = inertial ? 1 : 0;
     for (int f = 0; f < N; ++f) if (w->frame_fixed && w->frame_fixed[f]) H.fixed_mask |= 1 << f;
@@ -355,7 +355,6 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
     }
     H.n_chunks = nch;
     H.K = k_out;
-    ws.perm = std::move(perm);
     // inertial part
     H.n_imu = n_imu;
     H.n_prior = n_prior;
@@ -385,6 +384,11 @@ static int pack_window(Handle *h, int slot, const pvio_b200_window *w, const pvi
         float *z = p.pt_z.slot(slot);
         for (int i = 0; i < 2 * O; ++i) z[i] = (float)w->pt_obs_z[i];
     }
+    h->hdr.h[slot] = H;
+    h->cst.h[slot] = C;
+    ws.resident = false;                  // a packed slot is no longer a resident window
+    ws.n_samples.clear();                 // and its IMU factors hold no samples
+    ws.perm = std::move(perm);
     return 0;
 }
 
@@ -493,7 +497,10 @@ static BatchShape batch_shape(Handle *h, int w0, int n, bool by_capacity, const 
         b.solve_smem_lean = std::max(b.solve_smem_lean, solve_smem_one(H, true));
     }
     if (by_capacity) {                 // graph-cached launches: shapes depend on the frame counts (part of the graph key) only
-        b.M = h->Mcap; b.nfree = b.N;
+        // sized for the most landmarks any window can hold (pack_window, batch_window: kMaxChunks chunks), not for the
+        // capacity: a max_landmarks above that would ask the linearise and update sweeps for more shared memory than the
+        // device has, although no window can use it
+        b.M = std::min(h->Mcap, kMaxChunks * kChunk); b.nfree = b.N;
         WinHdr H;
         memset(&H, 0, sizeof(H));
         H.N = b.N;                     // a visual window of the largest size, an inertial one of the largest inertial size
