@@ -97,7 +97,7 @@ struct SlotLens {
 // call reads buf[cur] and writes buf[1 - cur].  Each buffer: [cap] double2 normalised keypoint, then [cap] int32 birth
 // (the number of the frame that detected it), then [cap] int32 prev_index (the keypoint of the frame before that it
 // continues, or -1).  Right after a call buf[1 - cur] still holds the previous frame's keypoints: the link that
-// pvio_b200_batch_window_mirror_frame reads (batch_window.cu).
+// pvio_b200_batch_window_mirror_frame reads (bw_frame.cu).
 struct SlotKeypoints {
     DevBuf<uint8_t> buf[3];                   // buf[2]: pvio_b200_batch_window_track_camera writes the new frame here and
                                               // swaps it with buf[1 - cur] when the call commits, so that a rejected
@@ -376,6 +376,14 @@ inline SolveOptions solve_options(const pvio_b200_options *opt) {
 
 #define TRY(x) do { int rc__ = (x); if (rc__ != 0) return rc__; } while (0)
 
+// right after a launch of `kernel`: counts it (Handle::launches), then 0, or PVIO_B200_ECUDA with the message
+// "launch of <kernel>: <error>" when the launch failed
+inline int launched(Handle *h, const char *kernel) {
+    ++h->launches;
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(h, PVIO_B200_ECUDA, (std::string("launch of ") + kernel).c_str(), e);
+}
+
 // The one allocation routine of the library.  n elements on the given sides (MemSides), per elements per window slot.
 // A buffer being replaced may still be in use by queued work, so the handle's stream is synchronised before it is freed.
 // Every allocation is zeroed: device memory in stream order on the handle's stream (which every kernel of the handle
@@ -525,7 +533,7 @@ struct CovLaunch {
 };
 int run_covariance(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L);
 // the first three of those launches: Sigma_xi of every frame pair in L.sig_xi and each record's status, for a landmark
-// kernel of the caller's (batch_window.cu: pvio_b200_batch_window_landmarks)
+// kernel of the caller's (bw_query.cu: pvio_b200_batch_window_landmarks)
 int run_cov_system(Handle *h, int n, const int32_t *h_slots, const int32_t *d_slots, const CovLaunch &L);
 size_t cov_smem_bytes(const WinHdr &H);   // dynamic shared memory of cov_kernel for a window of this header
 void drop_graphs(Handle *h);

@@ -131,7 +131,7 @@ __device__ __forceinline__ void CovBody::finish(const SolveArgs &sa, int w, int 
 
 constexpr int kCovLmWarps = 4;
 
-// One warp per named track.  bw_landmark_cov_kernel (batch_window.cu) forms the same Var(rho) through ba_cov_lm.cuh,
+// One warp per named track.  bw_landmark_cov_kernel (bw_query.cu) forms the same Var(rho) through ba_cov_lm.cuh,
 // which restates this body operation for operation so that both calls give the same bits: a change to the arithmetic
 // here must be made there too (tests/test_gpu_batch_window_landmarks.py checks the two for bit equality).
 // h_l over the free frames: the landmark's Schur records (the anchor's materialised when the anchor is free, zero

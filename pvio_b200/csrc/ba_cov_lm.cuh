@@ -1,5 +1,5 @@
 // The per-landmark arithmetic of cov_lm_kernel (ba_cov.cuh), one warp per landmark: h_l in xi coordinates from the
-// Schur records, and h_l^T Sigma_xi h_l.  bw_landmark_cov_kernel (batch_window.cu: the world points' covariance of
+// Schur records, and h_l^T Sigma_xi h_l.  bw_landmark_cov_kernel (bw_query.cu: the world points' covariance of
 // pvio_b200_batch_window_landmarks) forms Var(rho) with it, so that both calls give the same bits: the floating-point
 // operations here are cov_lm_kernel's, in the same order.  cov_lm_kernel keeps its own copy of them: through these
 // helpers nvcc lays out its address arithmetic differently, and its SASS is held to what it was.

@@ -74,7 +74,7 @@ __device__ __forceinline__ void imu_copy_warp(const ImuWarpSm &S, ImuWarpSm &D, 
 }
 
 // PreIntegrator::increment (:39-81) of one sample d ([7] t, w xyz, a xyz) over dt, on the warp's chain state S; noise
-// [4][9] cov_w, cov_a, cov_bg, cov_ba.  imu_integrate_warp runs it per sample; the trajectory kernel (batch_window.cu)
+// [4][9] cov_w, cov_a, cov_bg, cov_ba.  imu_integrate_warp runs it per sample; the trajectory kernel (bw_query.cu)
 // runs it on a copy of the chain to stop the integration at a query time, so both give the same bits.
 __device__ __forceinline__ void imu_step_warp(ImuWarpSm &S, int lane, const double *d, double dt, const double bg[3],
                                               const double ba[3], const double *noise) {

@@ -6,7 +6,7 @@
 // with Phi the Jacobian of PreIntegrator::predict (preintegrator.cpp:102-109) in the source state, through the factor's
 // bias Jacobians, and Psi its Jacobian in the factor's delta.  Shared by the FACTOR seed of the IMU stream slots
 // (imu_stream_seed_kernel, imu_stream.cu), which forms Sigma_d from the factor's sqrt_inv_cov, and the trajectory of
-// the resident slots (bw_trajectory_kernel, batch_window.cu), which takes a partial integration's delta.cov directly.
+// the resident slots (bw_trajectory_kernel, bw_query.cu), which takes a partial integration's delta.cov directly.
 // One warp, 15 x 15 row-major matrices in shared memory.
 #pragma once
 #include "ba_math.cuh"

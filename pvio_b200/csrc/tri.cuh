@@ -1,5 +1,5 @@
 // Multi-view DLT triangulation of one track (stereo.h:67-75, 104-128), shared by pvio_b200_triangulate (tri.cu) and the
-// triangulation of new tracks in pvio_b200_batch_window_localize (batch_window.cu).
+// triangulation of new tracks in pvio_b200_batch_window_localize (bw_frame.cu).
 // The reference takes the last right singular vector of the 2n x 4 matrix A (JacobiSVD); here one thread per
 // track accumulates the 4 x 4 Gram matrix A^T A in fp64 and takes its eigenvector of smallest eigenvalue by
 // cyclic Jacobi rotations -- the same vector up to sign (every use below is sign invariant); sigma_4^2 against
