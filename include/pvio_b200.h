@@ -441,6 +441,42 @@ typedef struct pvio_b200_window_trajectory {
     int32_t pad;
 } pvio_b200_window_trajectory; /* 48 bytes on LP64 */
 int pvio_b200_batch_window_trajectory(pvio_b200_handle h, int n, pvio_b200_window_trajectory *records);
+/* The smoothed state of each named inertial slot at any times inside its window: each state conditioned on both solved
+ * frames around it, so that the trajectory meets frame k + 1 instead of jumping there.  The records, the factor each
+ * time is taken by, the rejections, the ENUMERIC rule and "frame -1" are exactly those of
+ * pvio_b200_batch_window_trajectory; the call changes no slot.  For a time t that factor k takes (frames k, k + 1,
+ * samples s_0 .. s_{m-1}, t_end = frame k + 1's time), at frame k's current biases:
+ *  - Delta(t), Sigma(t): the forward call's partial increment and its covariance, block-diagonal C(t) (9 x 9, [dtheta
+ *    dp dv], rotation perturbed on the right), cbg(t), cba(t); e(t) its 15-dimensional error [dtheta dp dv | dbg dba].
+ *    Delta(T), Sigma(T): the whole factor's re-integration, which the forward call reaches at t_end.
+ *  - Phi(t2, t1): the transition of e along the chain, the product of the per-sample 9 x 9 A = [[exp(w dt)^T, 0, 0],
+ *    [-dt^2/2 R hat(a), I, dt I], [-dt R hat(a), 0, I]] that pre-integration applies to C (R the chain's rotation at
+ *    the step's start), the identity on the bias blocks.  From a t inside sample j's interval the chain runs the rest
+ *    of sample j over [t, s_{j+1}] (or [t, t_end]), from the partial increment's rotation, then the whole samples.
+ *  - Delta*: the increment PreIntegrator::predict maps from frame k onto frame k + 1 exactly, T = Delta(T)'s dt:
+ *    q_k^-1 q_{k+1};  R_k^T (p_{k+1} - p_k - v_k T - g T^2 / 2);  R_k^T (v_{k+1} - v_k - g T);  b_{k+1} - b_k.
+ *    r = Delta* (-) Delta(T) (15): r_theta = log(Delta_q(T)^-1 Delta*_q), the other parts differences.
+ *  - Cov(e(t), e(T)) = Sigma(t) Phi(T, t)^T for t <= t_end; in the gap past t_end (<= 1e-5 s, which the forward rules
+ *    give to factor k) Phi(t, T) Sigma(T), Phi(t, T) the last sample's step from t_end on to t.
+ *  - K(t) = Cov(e(t), e(T)) Sigma(T)^-1;  Delta_s(t) = Delta(t) (+) K r (rotation on the right, the rest added);
+ *    x_s(t) = PreIntegrator::predict(frame k, Delta_s(t)) with the bias part of K r added to frame k's biases (the
+ *    Brownian bridge between b_k and b_{k+1}).
+ *  - At t = s_0.t the state is frame k's, bit for bit; at t = t_end it is frame k + 1's to rounding; when r = 0 it is
+ *    the forward state.
+ *  - state_cov: J Sigma_{k,k+1} J^T + Psi Sigma_c(t) Psi^T, exactly symmetric, in the coordinates of
+ *    pvio_b200_batch_window_covariance.  Sigma_{k,k+1} is the 30 x 30 joint covariance of frames k and k + 1 as that
+ *    call defines it; Sigma_c(t) = Sigma(t) - K(t) Cov(e(T), e(t)); J = [dx_s/dx_k, dx_s/dx_{k+1}] to first order with
+ *    K(t) held fixed and Delta(t), Delta(T) moving with frame k's biases through their bias Jacobians:
+ *    Phi + Psi G K dr/dx_k and Psi G K dr/dx_{k+1}, with Phi and Psi those of
+ *    pvio_b200_batch_imu_stream_set_covariance's FACTOR seed at Delta_s(t) (its dq_dbg carried through
+ *    exp(u_theta)^T, u = K r) and G = diag(Jr(u_theta), I) the Jacobian of (+).
+ *  - frame -2: the factor's Sigma(T) is not positive definite, taken as a pivot of its Cholesky factor (as
+ *    pre-integration's sqrt_inv_cov forms it) at or below 1e-10 times its diagonal entry.  A one-sample factor is the
+ *    known case: its C(T) has rank 6.  Such a row has a zero state and a NaN covariance; it is not a rejection.
+ * Whatever n is: one host -> device copy, one kernel launch, one device -> host copy and one synchronisation; with
+ * covariances three launches more (the covariance call's linearise and Schur sweeps and cov_kernel, over the frames
+ * k and k + 1 of every factor with samples). */
+int pvio_b200_batch_window_smoothed_trajectory(pvio_b200_handle h, int n, pvio_b200_window_trajectory *records);
 /* Device -> host in one copy, per named slot i: n_frames [n], frames [n][frames_stride] ([N][16]), n_tracks [n] (live
  * tracks), and for each live track in id order at [i * track_stride + r]: id, inverse depth, anchor frame, observation
  * count, and the post-pass valid / quality of the last solve (0 / 0 for a track that did not take part in it).  Any

@@ -276,6 +276,7 @@ SIGNATURES = {
     "pvio_b200_batch_window_covariance": (_int, [_h, _int, _P(CWindowCovariance)]),
     "pvio_b200_batch_window_landmarks": (_int, [_h, _int, _P(CWindowLandmarks)]),
     "pvio_b200_batch_window_trajectory": (_int, [_h, _int, _P(CWindowTrajectory)]),
+    "pvio_b200_batch_window_smoothed_trajectory": (_int, [_h, _int, _P(CWindowTrajectory)]),
     "pvio_b200_batch_window_download": (_int, [_h, _int, c_i32p, c_i32p, c_f64p, _i64, c_i32p, _i64, c_i32p, c_f64p,
                                                c_i32p, c_i32p, c_u8p, c_f64p]),
     "pvio_b200_batch_window_localize": (_int, [_h, _int, _P(CWindowLocalize), _P(COptions)]),

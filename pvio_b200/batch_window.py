@@ -500,12 +500,16 @@ class BatchWindows:
             o["status"] = int(r.status)
         return out
 
-    def trajectory(self, slots, times, covariance=False):
+    def trajectory(self, slots, times, covariance=False, smoothed=False):
         """The state of each named inertial slot at the sorted times[i], forward from the window frame before each time
         through the part of that frame's IMU factor's kept samples up to it (pvio_b200_batch_window_trajectory).  Per
         record a dict: states [n, 16] (q xyzw, p, v, bg, ba), frame [n] (the window frame used, -1: a time no factor
         with samples covers, with a zero state) and status; with covariance also state_cov [n, 15, 15] in the
-        coordinates of covariance(), NaN for an uncovered time and throughout when status is ENUMERIC."""
+        coordinates of covariance(), NaN for an uncovered time and throughout when status is ENUMERIC.
+        smoothed: each state conditioned on both solved frames around it instead, meeting the next frame rather than
+        jumping there (pvio_b200_batch_window_smoothed_trajectory); the same dicts, and frame -2 (a zero state, a NaN
+        covariance) for the times of a factor whose increment covariance is not positive definite, as a one-sample
+        factor's is not."""
         n = len(slots)
         if len(times) != n:
             raise ValueError("one time list per slot")
@@ -520,7 +524,8 @@ class BatchWindows:
             r.slot, r.n_times = int(s), k
             _lib.set_ptrs(r, times=t if k else None, states=o["states"] if k else None, frame=o["frame"] if k else None,
                           state_cov=o.get("state_cov") if k else None)
-        self.ba._ck(self.lib.pvio_b200_batch_window_trajectory(self.h, n, recs))
+        call = self.lib.pvio_b200_batch_window_smoothed_trajectory if smoothed else self.lib.pvio_b200_batch_window_trajectory
+        self.ba._ck(call(self.h, n, recs))
         for r, o in zip(recs, out):
             del o["times"]
             o["status"] = int(r.status)

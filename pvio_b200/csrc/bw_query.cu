@@ -181,96 +181,597 @@ __device__ __forceinline__ void none_rows(const TrajArgs &T, const BwTraj &r, in
     }
 }
 
-// One CTA per record, one warp per factor k with samples (warp k).  The warp's queries are the times t >= s_0.t of its
-// factor and below s_0.t of the next factor with samples (so k is the largest such factor whose s_0.t <= t), found by
-// binary search; it takes those at most its t_end, or all of them when factor k + 1 holds samples.  It walks its
-// samples once, as imu_integrate_warp does (imu_step_warp), and emits each query as the walk passes it: the increment
-// of the last sample at or before t, over t - s_j.t, goes onto a copy of the chain, which is what imu_integrate_warp
-// gives for the samples at or before t with t_end = t.  Then PreIntegrator::predict from frame k's state, and with a
-// covariance Phi Sigma_k Phi^T + Psi Sigma_delta Psi^T (imu_factor_propagate), Sigma_delta the partial increment's
-// covariance itself.  Times no warp takes (before the first sample, past a factor's t_end, over a factor without
-// samples) get frame -1, a zero state and a NaN covariance: warp 0 writes those before the earliest s_0.t, each warp
-// those past its t_end.
-__global__ void __launch_bounds__(32 * (kMaxFrames - 1)) bw_trajectory_kernel(BwArgs a, TrajArgs T) {
-    extern __shared__ __align__(16) unsigned char traj_sm[];
-    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
-    const BwTraj &r = T.rec[blockIdx.x];
+// The factor k one warp serves and its queries, shared by both trajectory kernels: the times t >= s_0.t of factor k
+// and below s_0.t of the next factor with samples (so k is the largest such factor whose s_0.t <= t), found by binary
+// search; it takes those at most its t_end, or all of them when factor k + 1 holds samples.  The warp writes the rows
+// past its t_end that no factor takes (frame -1), and with `first` those before the earliest s_0.t.  False: the warp
+// has no queries.
+struct TrajFac {
+    int k, m, q0, q2;                 // factor, samples, queries [q0, q2)
+    size_t F;                         // frame k of the slot
+    const double *x, *smp, *noise;    // frame k's state, the samples, the noise [4][9]
+    double t_end, bg[3], ba[3];
+};
+__device__ __forceinline__ bool traj_factor(const BwArgs &a, const TrajArgs &T, const BwTraj &r, int k, bool first,
+                                            int lane, bool cov, TrajFac &f) {
     const int nf = r.N - 1, nq = r.n_times;
     const double *tq = T.times + r.t_off;
     const size_t F0 = (size_t)r.slot * a.Ncap;
-    auto s0 = [&](int k) { return a.imu_s[(F0 + k) * a.Scap * 7]; };
-    const bool cov = r.cov != -1;                           // -2: covariances asked, no factor holds samples
-    const bool cov_ok = r.cov >= 0 && T.status[r.cov] == PVIO_B200_OK;
-    if (wv == 0) {
+    auto s0 = [&](int j) { return a.imu_s[(F0 + j) * a.Scap * 7]; };
+    if (first) {
         double lo = CUDART_INF;
         for (int j = 0; j < nf; ++j)
             if (r.ns[j] > 0) lo = fmin(lo, s0(j));
         none_rows(T, r, lane, 0, traj_bound(tq, nq, lo, false), cov);
     }
-    const int k = wv;
-    if (k >= nf || r.ns[k] == 0) return;
-    const size_t F = F0 + k;
+    if (k >= nf || r.ns[k] == 0) return false;
+    f.k = k; f.m = r.ns[k]; f.F = F0 + k;
     const double lo = s0(k);
     double hi = CUDART_INF;
     for (int j = k + 1; j < nf; ++j)
         if (r.ns[j] > 0) hi = fmin(hi, s0(j));
-    const double *aux = a.imu_aux + F * kImuAux, t_end = aux[0];
-    const int q0 = traj_bound(tq, nq, lo, false), q1 = max(q0, traj_bound(tq, nq, hi, false));
-    const int q2 = (k + 1 < nf && r.ns[k + 1] > 0) ? q1 : min(q1, max(q0, traj_bound(tq, nq, t_end, true)));
-    none_rows(T, r, lane, q2, q1, cov);
-    if (q0 >= q2) return;
+    const double *aux = a.imu_aux + f.F * kImuAux;
+    f.t_end = aux[0];
+    f.noise = aux + 1;
+    f.q0 = traj_bound(tq, nq, lo, false);
+    const int q1 = max(f.q0, traj_bound(tq, nq, hi, false));
+    f.q2 = (k + 1 < nf && r.ns[k + 1] > 0) ? q1 : min(q1, max(f.q0, traj_bound(tq, nq, f.t_end, true)));
+    none_rows(T, r, lane, f.q2, q1, cov);
+    f.x = a.frames + f.F * kFrameStride;
+    f.smp = a.imu_s + f.F * a.Scap * 7;
+    for (int c = 0; c < 3; ++c) { f.bg[c] = f.x[10 + c]; f.ba[c] = f.x[13 + c]; }
+    return f.q0 < f.q2;
+}
+
+// The forward walk of a factor's samples, as imu_integrate_warp walks them (imu_step_warp), emitting each query as the
+// walk passes it: the increment of the last sample at or before t, over t - s_j.t, goes onto a copy E of the chain S,
+// which is what imu_integrate_warp gives for the samples at or before t with t_end = t; then emit(q).  knot(j) sees
+// the chain at s_j.t before sample j is stepped.  ToEnd: walk every sample, leaving the full re-integration in S;
+// otherwise stop after the last query.
+template <bool ToEnd, typename Knot, typename Emit>
+__device__ __forceinline__ void traj_walk(ImuWarpSm &S, ImuWarpSm &E, const TrajFac &f, const double *tq, int lane,
+                                          Knot knot, Emit emit) {
+    imu_reset_warp(S, lane);
+    int q = f.q0;
+    for (int j = 0; j < f.m && (ToEnd || q < f.q2); ++j) {
+        const double *d = f.smp + (size_t)j * 7;
+        const bool last = j + 1 == f.m;
+        const double t_next = last ? f.t_end : f.smp[(size_t)(j + 1) * 7];
+        knot(j);
+        for (; q < f.q2 && (last || tq[q] < t_next); ++q) {   // the queries whose last sample is s_j
+            imu_copy_warp(S, E, lane);
+            imu_step_warp(E, lane, d, tq[q] - d[0], f.bg, f.ba, f.noise);
+            emit(q);
+        }
+        if (ToEnd || (!last && q < f.q2)) imu_step_warp(S, lane, d, t_next - d[0], f.bg, f.ba, f.noise);
+    }
+}
+
+// One CTA per record, one warp per factor k with samples (warp k), each walking its samples once (traj_factor,
+// traj_walk).  Each query's state is PreIntegrator::predict from frame k's state, and with a covariance Phi Sigma_k
+// Phi^T + Psi Sigma_delta Psi^T (imu_factor_propagate), Sigma_delta the partial increment's covariance itself.  Times
+// no warp takes (before the first sample, past a factor's t_end, over a factor without samples) get frame -1, a zero
+// state and a NaN covariance: warp 0 writes those before the earliest s_0.t, each warp those past its t_end.
+__global__ void __launch_bounds__(32 * (kMaxFrames - 1)) bw_trajectory_kernel(BwArgs a, TrajArgs T) {
+    extern __shared__ __align__(16) unsigned char traj_sm[];
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const BwTraj &r = T.rec[blockIdx.x];
+    const int nf = r.N - 1;
+    const double *tq = T.times + r.t_off;
+    const bool cov = r.cov != -1;                           // -2: covariances asked, no factor holds samples
+    const bool cov_ok = r.cov >= 0 && T.status[r.cov] == PVIO_B200_OK;
+    TrajFac f;
+    if (!traj_factor(a, T, r, wv, wv == 0, lane, cov, f)) return;
+    const int k = f.k;
     unsigned char *base = traj_sm + (size_t)wv * traj_warp_bytes(T.covs);
     ImuWarpSm &S = *reinterpret_cast<ImuWarpSm *>(base), &E = *reinterpret_cast<ImuWarpSm *>(base + sizeof(ImuWarpSm));
     double *A = reinterpret_cast<double *>(base + 2 * sizeof(ImuWarpSm)), *B = A + 225, *C = B + 225, *D = C + 225;
-    const double *x = a.frames + F * kFrameStride;
-    const double bg[3] = {x[10], x[11], x[12]}, ba[3] = {x[13], x[14], x[15]};
-    const double *smp = a.imu_s + F * a.Scap * 7, *noise = aux + 1;
-    const int m = r.ns[k];
+    const double *x = f.x;
     // Sigma_k: frame k's diagonal block of the joint covariance of the frames that own a factor with samples
     unsigned has = 0;
     for (int j = 0; j < nf; ++j) has |= (r.ns[j] > 0 ? 1u : 0u) << j;
     const int K15 = 15 * __popc(has), p15 = 15 * __popc(has & ((1u << k) - 1u));
     const double *Sk = T.jcov + r.cov_off + (size_t)p15 * K15 + p15;
-    imu_reset_warp(S, lane);
-    int q = q0;
-    for (int j = 0; j < m && q < q2; ++j) {
-        const double *d = smp + (size_t)j * 7;
-        const bool last = j + 1 == m;
-        const double t_next = last ? t_end : smp[(size_t)(j + 1) * 7];
-        for (; q < q2 && (last || tq[q] < t_next); ++q) {   // the queries whose last sample is s_j
-            imu_copy_warp(S, E, lane);
-            imu_step_warp(E, lane, d, tq[q] - d[0], bg, ba, noise);
+    traj_walk<false>(S, E, f, tq, lane, [](int) {}, [&](int q) {
+        const size_t row = r.t_off + q;
+        if (lane == 0) {
+            bw_imu_predict(x, E.tsum, E.q, E.p, E.v, T.states + 16 * row);
+            T.frame[row] = k;
+        }
+        if (!cov) return;
+        double *out = T.scov + 225 * (size_t)(r.scov_off + q);
+        if (!cov_ok) {
+            for (int e = lane; e < 225; e += 32) out[e] = CUDART_NAN;
+            return;
+        }
+        for (int e = lane; e < 225; e += 32) {
+            const int i = e / 15, c = e % 15;
+            A[e] = 0.5 * (Sk[(size_t)i * K15 + c] + Sk[(size_t)c * K15 + i]);
+            D[e] = (i < 9 && c < 9) ? E.C[i * 9 + c]
+                 : (i >= 9 && i < 12 && c >= 9 && c < 12) ? E.cbg[(i - 9) * 3 + c - 9]
+                 : (i >= 12 && c >= 12) ? E.cba[(i - 12) * 3 + c - 12] : 0.0;
+        }
+        __syncwarp();
+        double Rs[9], dR[9];
+        quat_to_mat(x, Rs);
+        quat_to_mat(E.q, dR);
+        const ImuFactorJac fj{E.tsum, E.p, E.v, E.dq_dbg, E.dp_dbg, E.dp_dba, E.dv_dbg, E.dv_dba};
+        imu_factor_propagate(A, B, C, D, fj, Rs, dR, lane);
+        for (int e = lane; e < 225; e += 32) {
+            const int i = e / 15, c = e % 15;
+            out[e] = 0.5 * ((A[e] + D[e]) + (A[c * 15 + i] + D[c * 15 + i]));
+        }
+        __syncwarp();
+    });
+}
+
+// ---- pvio_b200_batch_window_smoothed_trajectory: the state at t conditioned on both frames around it (the header's
+// definition).  Per query the forward walk keeps the partial increment Delta(t) in global scratch (kTrajSnap doubles:
+// C, cbg, cba, the five bias Jacobians, q, p, v, dt), and per knot the chain's rotation at s_j (4 doubles).
+constexpr int kTrajSnap = 156;
+struct TrajSmooth {
+    double *snap;                     // [rows][kTrajSnap]
+    double *knot;                     // [records][kMaxFrames - 1][Scap][4]
+};
+
+// one step's transition A = [[Ri, 0, 0], [-dt^2/2 M, I, dt I], [-dt M, 0, I]] over dt of sample d from rotation q, as
+// imu_step_warp forms Ri and M.  Lane 0.
+struct TrajA { double Ri[9], M[9], dt; };
+__device__ __forceinline__ void traj_a(TrajA &A, const double *d, const double *q, double dt, const double *bg,
+                                       const double *ba) {
+    const double th[3] = {(d[1] - bg[0]) * dt, (d[2] - bg[1]) * dt, (d[3] - bg[2]) * dt};
+    const double acc[3] = {d[4] - ba[0], d[5] - ba[1], d[6] - ba[2]};
+    double qi[4], qc[4], Rd[9], Ha[9];
+    expmap(th, qi);
+    quat_conj(qi, qc);
+    quat_to_mat(qc, A.Ri);
+    quat_to_mat(q, Rd);
+    hat(acc, Ha);
+    mat3_mul(Rd, Ha, A.M);
+    A.dt = dt;
+}
+// entry (r, c) of A^T X (xt: of A^T X^T), X 9 x 9 row-major
+__device__ __forceinline__ double traj_at(const TrajA &A, const double *X, int r, int c, bool xt) {
+    auto x = [&](int i, int j) { return xt ? X[j * 9 + i] : X[i * 9 + j]; };
+    const double dt = A.dt;
+    if (r >= 6) return dt * x(r - 3, c) + x(r, c);
+    if (r >= 3) return x(r, c);
+    double s = 0.0, m = 0.0;
+    for (int k = 0; k < 3; ++k) {
+        s += A.Ri[k * 3 + r] * x(k, c);
+        m += A.M[k * 3 + r] * (0.5 * dt * dt * x(3 + k, c) + dt * x(6 + k, c));
+    }
+    return s - m;
+}
+// Y = A^T X (xt: A^T X^T), by the warp's lanes; Y must not alias X
+__device__ __forceinline__ void traj_at_warp(const TrajA &A, const double *X, double *Y, bool xt, int lane) {
+    for (int e = lane; e < 81; e += 32) Y[e] = traj_at(A, X, e / 9, e % 9, xt);
+    __syncwarp();
+}
+// y = A^T v (9).  One lane.
+__device__ __forceinline__ void traj_at_vec(const TrajA &A, const double *v, double *y) {
+    const double dt = A.dt;
+    for (int r = 0; r < 3; ++r) {
+        double s = 0.0, m = 0.0;
+        for (int k = 0; k < 3; ++k) {
+            s += A.Ri[k * 3 + r] * v[k];
+            m += A.M[k * 3 + r] * (0.5 * dt * dt * v[3 + k] + dt * v[6 + k]);
+        }
+        y[r] = s - m;
+    }
+    for (int r = 3; r < 6; ++r) y[r] = v[r];
+    for (int r = 6; r < 9; ++r) y[r] = dt * v[r - 3] + v[r];
+}
+// C = A B (n x n, row-major; A, B with leading dimension n), by the warp's lanes
+__device__ __forceinline__ void traj_mm(const double *A, const double *B, double *C, int n, int lane) {
+    for (int e = lane; e < n * n; e += 32) {
+        const int i = e / n, j = e % n;
+        double s = 0.0;
+        for (int m = 0; m < n; ++m) s += A[i * n + m] * B[m * n + j];
+        C[e] = s;
+    }
+    __syncwarp();
+}
+
+// per warp of bw_smoothed_trajectory_kernel
+struct TrajSmSm {
+    ImuWarpSm S, E;                   // the chain (after the walk: Delta(T)), a query's partial increment
+    TrajA A;                          // the step the backward pass is at
+    double r[15], lam[15];            // the residual; Sigma(T)^-1 r carried back to the pass's knot (bias parts fixed)
+    double u[15], Gu[9], Eu[9];       // a query's K r; Jr(u_theta) and R(exp(u_theta))
+    double U9[81], Ub[18];            // sqrt_inv_block of C(T), cbg(T), cba(T)
+    double Rk[9], Jri[9];             // R(q_k), Jr(r_theta)^-1
+    double dqs[4], dps[3], dvs[3], dqdbg[9];      // a query's Delta_s, its dq_dbg carried through exp(u_theta)
+    int pd;                           // Sigma(T) positive definite
+};
+struct TrajSmCov {                    // with covariances
+    double L[81], W[81];              // Phi^T C(T)^-1 and Phi^T C(T)^-1 Phi at the pass's knot
+    double Cb[18];                    // cbg(T)^-1, cba(T)^-1
+    double X[4][81];                  // 9 x 9 scratch
+    double Dk[225], P[4][225];        // dr/dx_k; 15 x 15 scratch
+};
+__host__ __device__ constexpr size_t traj_smooth_bytes(bool covs) {
+    return sizeof(TrajSmSm) + (covs ? sizeof(TrajSmCov) : 0);
+}
+
+// rows 0-2 of the 15 x 15 P by G (null: unchanged), rows 3-5 and 6-8 by R: P <- diag(G, R, R, I, I) P.  Lane per column.
+__device__ __forceinline__ void traj_rows(double *P, const double *G, const double *R, int lane) {
+    if (lane < 15) {
+        double t[9];
+        for (int i = 0; i < 9; ++i) t[i] = P[i * 15 + lane];
+        for (int b = G ? 0 : 1; b < 3; ++b) {
+            const double *X = b == 0 ? G : R;
+            for (int i = 0; i < 3; ++i)
+                P[(3 * b + i) * 15 + lane] = X[3 * i] * t[3 * b] + X[3 * i + 1] * t[3 * b + 1] + X[3 * i + 2] * t[3 * b + 2];
+        }
+    }
+    __syncwarp();
+}
+// columns 0-2 of the 15 x 15 P by G (null: unchanged), columns 3-5 and 6-8 by R^T: P <- P diag(G, R^T, R^T, I, I).
+// Lane per row.
+__device__ __forceinline__ void traj_cols(double *P, const double *G, const double *R, int lane) {
+    if (lane < 15) {
+        double t[9];
+        double *row = P + lane * 15;
+        for (int i = 0; i < 9; ++i) t[i] = row[i];
+        for (int b = G ? 0 : 1; b < 3; ++b)
+            for (int c = 0; c < 3; ++c)
+                row[3 * b + c] = b == 0 ? t[0] * G[c] + t[1] * G[3 + c] + t[2] * G[6 + c]
+                                        : t[3 * b] * R[3 * c] + t[3 * b + 1] * R[3 * c + 1] + t[3 * b + 2] * R[3 * c + 2];
+    }
+    __syncwarp();
+}
+
+// One CTA of one warp per (record, factor k with samples): grid (records, factors).  The forward walk of
+// bw_trajectory_kernel runs to t_end (traj_walk<true>), keeping each query's partial increment and each knot's
+// rotation in global scratch; then r and sqrt_inv_block of Sigma(T) (frame -2 for every query when Sigma(T) is not
+// positive definite), and a backward adjoint pass over the knots that carries lam = Phi^T Sigma(T)^-1 r, and with
+// covariances L = Phi^T C(T)^-1 and W = Phi^T C(T)^-1 Phi, one step per sample, emitting each query as it reaches it:
+//   K r = C(t) A_t^T lam,  K = C(t) A_t^T L,  Sigma_c = C(t) - C(t) A_t^T W A_t C(t)
+// with A_t the rest of the query's sample from t (bias blocks: cbg(t) cbg(T)^-1); past t_end K = A the last sample
+// from t_end on to t.  Then the state is predict(x_k, Delta(t) (+) K r) with the bias part of K r added, and the
+// covariance J Sigma_{k,k+1} J^T + Psi Sigma_c Psi^T (the header's definition), exactly symmetric.  Linear in samples
+// plus queries; shared memory does not grow with either.
+__global__ void __launch_bounds__(32) bw_smoothed_trajectory_kernel(BwArgs a, TrajArgs T, TrajSmooth Z) {
+    extern __shared__ __align__(16) unsigned char traj_sm[];
+    const int lane = threadIdx.x;
+    const BwTraj &r = T.rec[blockIdx.x];
+    const int nf = r.N - 1;
+    const double *tq = T.times + r.t_off;
+    const bool cov = r.cov != -1;
+    const bool cov_ok = r.cov >= 0 && T.status[r.cov] == PVIO_B200_OK;
+    TrajFac f;
+    if (!traj_factor(a, T, r, blockIdx.y, blockIdx.y == 0, lane, cov, f)) return;
+    TrajSmSm &W = *reinterpret_cast<TrajSmSm *>(traj_sm);
+    TrajSmCov &V = *reinterpret_cast<TrajSmCov *>(traj_sm + sizeof(TrajSmSm));
+    ImuWarpSm &S = W.S, &E = W.E;
+    const int k = f.k;
+    const double *x = f.x, *x1 = x + kFrameStride;
+    double *kq = Z.knot + ((size_t)blockIdx.x * (kMaxFrames - 1) + k) * a.Scap * 4;
+    traj_walk<true>(S, E, f, tq, lane, [&](int j) { if (lane < 4) kq[4 * j + lane] = S.q[lane]; }, [&](int q) {
+        double *z = Z.snap + (size_t)(r.t_off + q) * kTrajSnap;
+        for (int e = lane; e < 81; e += 32) z[e] = E.C[e];
+        if (lane < 9) {
+            z[81 + lane] = E.cbg[lane]; z[90 + lane] = E.cba[lane]; z[99 + lane] = E.dq_dbg[lane];
+            z[108 + lane] = E.dp_dbg[lane]; z[117 + lane] = E.dp_dba[lane]; z[126 + lane] = E.dv_dbg[lane];
+            z[135 + lane] = E.dv_dba[lane];
+        }
+        if (lane < 4) z[144 + lane] = E.q[lane];
+        if (lane < 3) { z[148 + lane] = E.p[lane]; z[151 + lane] = E.v[lane]; }
+        if (lane == 0) z[154] = E.tsum;
+        __syncwarp();
+    });
+    // ---- r = Delta* (-) Delta(T) and the factors of Sigma(T)
+    const double Tt = S.tsum;
+    double dsp[3], dsv[3], dsq[4];                           // Delta* (lane 0)
+    if (lane == 0) {
+        const double g[3] = {0.0, 0.0, -9.80665};            // as bw_imu_predict
+        double qc[4], qe[4], y[3];
+        quat_to_mat(x, W.Rk);
+        quat_conj(x, qc);
+        quat_mul(qc, x1, dsq);
+        quat_conj(S.q, qc);
+        quat_mul(qc, dsq, qe);
+        logmap(qe, W.r);
+        for (int c = 0; c < 3; ++c) y[c] = x1[4 + c] - x[4 + c] - x[7 + c] * Tt - 0.5 * g[c] * Tt * Tt;
+        mat3_tvec(W.Rk, y, dsp);
+        for (int c = 0; c < 3; ++c) y[c] = x1[7 + c] - x[7 + c] - g[c] * Tt;
+        mat3_tvec(W.Rk, y, dsv);
+        for (int c = 0; c < 3; ++c) {
+            W.r[3 + c] = dsp[c] - S.p[c];
+            W.r[6 + c] = dsv[c] - S.v[c];
+            W.r[9 + c] = x1[10 + c] - x[10 + c];
+            W.r[12 + c] = x1[13 + c] - x[13 + c];
+        }
+        sqrt_inv_block(S.C, 9, 9, W.U9, 9);
+    } else if (lane == 1) {
+        sqrt_inv_block(S.cbg, 3, 3, W.Ub, 3);
+    } else if (lane == 2) {
+        sqrt_inv_block(S.cba, 3, 3, W.Ub + 9, 3);
+    }
+    __syncwarp();
+    if (lane == 0) {            // every pivot R_jj^2 = U_jj^-2 above 1e-10 C_jj (a one-sample factor's C(T) has rank 6)
+        bool pd = true;
+        for (int j = 0; j < 15; ++j) {
+            const double u = j < 9 ? W.U9[j * 10] : W.Ub[(j - 9) / 3 * 9 + (j % 3) * 4];
+            const double c = j < 9 ? S.C[j * 10] : (j < 12 ? S.cbg : S.cba)[(j % 3) * 4];
+            pd = pd && u > 0.0 && u < CUDART_INF && u * u * c * 1e-10 < 1.0;
+        }
+        W.pd = pd;
+    }
+    __syncwarp();
+    if (!W.pd) {                                             // no smoother: frame -2
+        for (int q = f.q0; q < f.q2; ++q) {
             const size_t row = r.t_off + q;
-            if (lane == 0) {
-                bw_imu_predict(x, E.tsum, E.q, E.p, E.v, T.states + 16 * row);
-                T.frame[row] = k;
+            if (lane < 16) T.states[16 * row + lane] = 0.0;
+            if (lane == 0) T.frame[row] = -2;
+            if (cov)
+                for (int e = lane; e < 225; e += 32) T.scov[225 * ((size_t)r.scov_off + q) + e] = CUDART_NAN;
+        }
+        return;
+    }
+    const bool cv = cov && cov_ok;
+    if (lane == 0) {                                         // lam = Sigma(T)^-1 r
+        double y[9];
+        for (int i = 0; i < 9; ++i) {
+            double s = 0.0;
+            for (int j = i; j < 9; ++j) s += W.U9[i * 9 + j] * W.r[j];
+            y[i] = s;
+        }
+        for (int i = 0; i < 9; ++i) {
+            double s = 0.0;
+            for (int j = 0; j <= i; ++j) s += W.U9[j * 9 + i] * y[j];
+            W.lam[i] = s;
+        }
+        for (int b = 0; b < 2; ++b) {
+            const double *U = W.Ub + 9 * b, *rb = W.r + 9 + 3 * b;
+            for (int i = 0; i < 3; ++i) {
+                double s = 0.0;
+                for (int j = i; j < 3; ++j) s += U[i * 3 + j] * rb[j];
+                y[i] = s;
             }
-            if (!cov) continue;
-            double *out = T.scov + 225 * (size_t)(r.scov_off + q);
-            if (!cov_ok) {
-                for (int e = lane; e < 225; e += 32) out[e] = CUDART_NAN;
-                continue;
+            for (int i = 0; i < 3; ++i) {
+                double s = 0.0;
+                for (int j = 0; j <= i; ++j) s += U[j * 3 + i] * y[j];
+                W.lam[9 + 3 * b + i] = s;
             }
-            for (int e = lane; e < 225; e += 32) {
+        }
+        double J[9];
+        right_jacobian(W.r, J);
+        mat3_inv(J, W.Jri);
+    }
+    __syncwarp();
+    if (cv) {
+        for (int e = lane; e < 81; e += 32) {                // L = W = C(T)^-1 = U^T U
+            const int i = e / 9, j = e % 9;
+            double s = 0.0;
+            for (int m = 0; m <= min(i, j); ++m) s += W.U9[m * 9 + i] * W.U9[m * 9 + j];
+            V.L[e] = s;
+            V.W[e] = s;
+        }
+        if (lane < 18) {
+            const double *U = W.Ub + 9 * (lane / 9);
+            const int i = (lane % 9) / 3, j = lane % 3;
+            double s = 0.0;
+            for (int m = 0; m <= min(i, j); ++m) s += U[m * 3 + i] * U[m * 3 + j];
+            V.Cb[lane] = s;
+        }
+        for (int e = lane; e < 225; e += 32) V.Dk[e] = 0.0;
+        __syncwarp();
+        if (lane == 0) {                                     // dr/dx_k
+            double Er[9], Rq[9], X[9], Y[9], qe[4];
+            expmap(W.r, qe);
+            quat_to_mat(qe, Er);
+            quat_to_mat(dsq, Rq);
+            for (int i = 0; i < 3; ++i)
+                for (int j = 0; j < 3; ++j) Y[3 * i + j] = Rq[3 * j + i];
+            mat3_mul(W.Jri, Y, X);
+            put_block(V.Dk, 0, 0, X, -1.0);
+            mat3_mul_tn(Er, S.dq_dbg, Y);
+            mat3_mul(W.Jri, Y, X);
+            put_block(V.Dk, 0, 3, X, -1.0);
+            for (int i = 0; i < 3; ++i)
+                for (int j = 0; j < 3; ++j) Y[3 * i + j] = W.Rk[3 * j + i];
+            hat(dsp, X);
+            put_block(V.Dk, 1, 0, X);
+            put_block(V.Dk, 1, 1, Y, -1.0);
+            put_block(V.Dk, 1, 2, Y, -Tt);
+            put_block(V.Dk, 1, 3, S.dp_dbg, -1.0);
+            put_block(V.Dk, 1, 4, S.dp_dba, -1.0);
+            hat(dsv, X);
+            put_block(V.Dk, 2, 0, X);
+            put_block(V.Dk, 2, 2, Y, -1.0);
+            put_block(V.Dk, 2, 3, S.dv_dbg, -1.0);
+            put_block(V.Dk, 2, 4, S.dv_dba, -1.0);
+            put_block(V.Dk, 3, 3, nullptr, -1.0);
+            put_block(V.Dk, 4, 4, nullptr, -1.0);
+        }
+        __syncwarp();
+    }
+    // Sigma_{k,k+1}: frames k and k + 1 in the joint block of the frames {k, k + 1 : factor k holds samples}
+    unsigned has = 0;
+    for (int j = 0; j < nf; ++j) has |= (r.ns[j] > 0 ? 3u : 0u) << j;
+    const int K15 = 15 * __popc(has), p15 = 15 * __popc(has & ((1u << k) - 1u));
+    const double *Sj = T.jcov + r.cov_off + (size_t)p15 * K15 + p15;
+    auto sjoint = [&](int i, int c) { return 0.5 * (Sj[(size_t)i * K15 + c] + Sj[(size_t)c * K15 + i]); };
+
+    // one query: row q, its partial increment z; gap: past t_end
+    auto emit = [&](int q, bool gap) {
+        const size_t row = r.t_off + q;
+        const double *z = Z.snap + row * kTrajSnap, *Ct = z;
+        if (lane == 0) {
+            double *u = W.u;
+            if (gap) {                                       // K r = A r (bias part r)
+                double mr[3];
+                mat3_vec(W.A.M, W.r, mr);
+                mat3_vec(W.A.Ri, W.r, u);
+                const double dt = W.A.dt;
+                for (int c = 0; c < 3; ++c) {
+                    u[3 + c] = -0.5 * dt * dt * mr[c] + W.r[3 + c] + dt * W.r[6 + c];
+                    u[6 + c] = -dt * mr[c] + W.r[6 + c];
+                    u[9 + c] = W.r[9 + c];
+                    u[12 + c] = W.r[12 + c];
+                }
+            } else {                                         // K r = C(t) A_t^T lam, cbg(t) lam_bg, cba(t) lam_ba
+                double lt[9];
+                traj_at_vec(W.A, W.lam, lt);
+                for (int i = 0; i < 9; ++i) {
+                    double s = 0.0;
+                    for (int j = 0; j < 9; ++j) s += Ct[i * 9 + j] * lt[j];
+                    u[i] = s;
+                }
+                for (int i = 0; i < 6; ++i) {
+                    const double *Cb = z + 81 + 9 * (i / 3);
+                    const int ib = i % 3;
+                    u[9 + i] = Cb[ib * 3] * W.lam[9 + i - ib] + Cb[ib * 3 + 1] * W.lam[10 + i - ib] +
+                               Cb[ib * 3 + 2] * W.lam[11 + i - ib];
+                }
+            }
+            // Delta_s = Delta(t) (+) u: the rotation on the right (exactly Delta(t)'s when u_theta = 0)
+            double qe[4];
+            expmap(u, qe);
+            quat_to_mat(qe, W.Eu);
+            right_jacobian(u, W.Gu);
+            if (u[0] == 0.0 && u[1] == 0.0 && u[2] == 0.0)
+                for (int c = 0; c < 4; ++c) W.dqs[c] = z[144 + c];
+            else quat_mul(z + 144, qe, W.dqs);
+            for (int c = 0; c < 3; ++c) { W.dps[c] = z[148 + c] + u[3 + c]; W.dvs[c] = z[151 + c] + u[6 + c]; }
+            double *y = T.states + 16 * row;
+            bw_imu_predict(x, z[154], W.dqs, W.dps, W.dvs, y);
+            for (int c = 0; c < 6; ++c) y[10 + c] = x[10 + c] + u[9 + c];
+            T.frame[row] = k;
+            mat3_mul_tn(W.Eu, z + 99, W.dqdbg);
+        }
+        __syncwarp();
+        if (!cov) return;
+        double *out = T.scov + 225 * (size_t)(r.scov_off + q);
+        if (!cov_ok) {
+            for (int e = lane; e < 225; e += 32) out[e] = CUDART_NAN;
+            return;
+        }
+        double (*X)[81] = V.X;
+        // K9 into X[1], Sigma_c's 9 x 9 block into X[3]
+        if (gap) {
+            for (int e = lane; e < 81; e += 32) X[0][e] = e / 9 == e % 9 ? 1.0 : 0.0;
+            __syncwarp();
+            traj_at_warp(W.A, X[0], X[2], false, lane);     // A^T
+            for (int e = lane; e < 81; e += 32) X[1][e] = X[2][(e % 9) * 9 + e / 9];
+            __syncwarp();
+            traj_mm(X[1], S.C, X[0], 9, lane);              // A C(T)
+            traj_mm(X[0], X[2], X[3], 9, lane);             // .. A^T
+            for (int e = lane; e < 81; e += 32) X[3][e] = Ct[e] - X[3][e];
+        } else {
+            traj_at_warp(W.A, V.L, X[0], false, lane);      // L(t)
+            traj_mm(Ct, X[0], X[1], 9, lane);               // K9
+            traj_at_warp(W.A, V.W, X[0], false, lane);      // A^T W
+            traj_at_warp(W.A, X[0], X[2], true, lane);      // W(t)^T
+            for (int e = lane; e < 81; e += 32) X[0][e] = X[2][(e % 9) * 9 + e / 9];
+            __syncwarp();
+            traj_mm(X[0], Ct, X[2], 9, lane);               // W(t) C(t)
+            traj_mm(Ct, X[2], X[0], 9, lane);               // C(t) W(t) C(t)
+            for (int e = lane; e < 81; e += 32) X[3][e] = Ct[e] - X[0][e];
+        }
+        __syncwarp();
+        double *P0 = V.P[0], *P1 = V.P[1], *P2 = V.P[2], *P3 = V.P[3];
+        for (int e = lane; e < 225; e += 32) {               // K into P0, Sigma_c into P1 (block diagonal)
+            const int i = e / 15, c = e % 15;
+            double kv = 0.0, sv = 0.0;
+            if (i < 9 && c < 9) { kv = X[1][i * 9 + c]; sv = X[3][i * 9 + c]; }
+            else if (i >= 9 && c >= 9 && (i - 9) / 3 == (c - 9) / 3) {
+                const int b = (i - 9) / 3, ib = (i - 9) % 3, cb = (c - 9) % 3;
+                const double *Cb = z + 81 + 9 * b, *CT = b == 0 ? S.cbg : S.cba, *Ci = V.Cb + 9 * b;
+                if (gap) { kv = ib == cb ? 1.0 : 0.0; sv = Cb[ib * 3 + cb] - CT[ib * 3 + cb]; }
+                else {
+                    double ki[3];
+                    for (int m = 0; m < 3; ++m)
+                        ki[m] = Cb[ib * 3] * Ci[m] + Cb[ib * 3 + 1] * Ci[3 + m] + Cb[ib * 3 + 2] * Ci[6 + m];
+                    kv = ki[cb];
+                    sv = Cb[ib * 3 + cb] - (ki[0] * Cb[cb] + ki[1] * Cb[3 + cb] + ki[2] * Cb[6 + cb]);
+                }
+            }
+            P0[e] = kv;
+            P1[e] = sv;
+        }
+        __syncwarp();
+        // J_k = Phi + Psi G K dr/dx_k into P3, J_k1 = Psi G K dr/dx_k1 into P2
+        warp_mm15(P0, V.Dk, P2, false, lane);
+        traj_rows(P2, W.Gu, W.Rk, lane);
+        double dR[9];
+        quat_to_mat(W.dqs, dR);
+        const ImuFactorJac fj{z[154], W.dps, W.dvs, W.dqdbg, z + 108, z + 117, z + 126, z + 135};
+        imu_factor_phi(P3, fj, W.Rk, dR, lane);
+        for (int e = lane; e < 225; e += 32) P3[e] += P2[e];
+        __syncwarp();
+        for (int e = lane; e < 225; e += 32) P2[e] = P0[e];
+        __syncwarp();
+        traj_cols(P2, W.Jri, W.Rk, lane);
+        traj_rows(P2, W.Gu, W.Rk, lane);
+        // J Sigma_{k,k+1} J^T + Psi Sigma_c Psi^T
+        double acc[8];
+        for (int h = 0; h < 2; ++h) {
+            for (int e = lane; e < 225; e += 32) {           // J_k Sigma_{k,h} + J_k1 Sigma_{k+1,h}
                 const int i = e / 15, c = e % 15;
-                A[e] = 0.5 * (Sk[(size_t)i * K15 + c] + Sk[(size_t)c * K15 + i]);
-                D[e] = (i < 9 && c < 9) ? E.C[i * 9 + c]
-                     : (i >= 9 && i < 12 && c >= 9 && c < 12) ? E.cbg[(i - 9) * 3 + c - 9]
-                     : (i >= 12 && c >= 12) ? E.cba[(i - 12) * 3 + c - 12] : 0.0;
+                double s = 0.0;
+                for (int m = 0; m < 15; ++m)
+                    s += P3[i * 15 + m] * sjoint(m, 15 * h + c) + P2[i * 15 + m] * sjoint(15 + m, 15 * h + c);
+                P0[e] = s;
             }
             __syncwarp();
-            double Rs[9], dR[9];
-            quat_to_mat(x, Rs);
-            quat_to_mat(E.q, dR);
-            const ImuFactorJac f{E.tsum, E.p, E.v, E.dq_dbg, E.dp_dbg, E.dp_dba, E.dv_dbg, E.dv_dba};
-            imu_factor_propagate(A, B, C, D, f, Rs, dR, lane);
-            for (int e = lane; e < 225; e += 32) {
+            const double *Jh = h == 0 ? P3 : P2;
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+                const int e = lane + 32 * g;
+                if (e >= 225) continue;
                 const int i = e / 15, c = e % 15;
-                out[e] = 0.5 * ((A[e] + D[e]) + (A[c * 15 + i] + D[c * 15 + i]));
+                double s = 0.0;
+                for (int m = 0; m < 15; ++m) s += P0[i * 15 + m] * Jh[c * 15 + m];
+                acc[g] = h == 0 ? s : acc[g] + s;
             }
             __syncwarp();
         }
-        if (!last && q < q2) imu_step_warp(S, lane, d, t_next - d[0], bg, ba, noise);
+        traj_rows(P1, nullptr, W.Rk, lane);
+        traj_cols(P1, nullptr, W.Rk, lane);
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+            const int e = lane + 32 * g;
+            if (e < 225) P0[e] = acc[g] + P1[e];
+        }
+        __syncwarp();
+        for (int e = lane; e < 225; e += 32) out[e] = 0.5 * (P0[e] + P0[(e % 15) * 15 + e / 15]);
+        __syncwarp();
+    };
+
+    // ---- the backward pass: the queries past t_end, then per sample from the last down
+    int q = f.q2 - 1;
+    for (; q >= f.q0 && tq[q] > f.t_end; --q) {
+        if (lane == 0) traj_a(W.A, f.smp + (size_t)(f.m - 1) * 7, S.q, tq[q] - f.t_end, f.bg, f.ba);
+        __syncwarp();
+        emit(q, true);
+    }
+    for (int j = f.m - 1; j >= 0 && q >= f.q0; --j) {
+        const double *d = f.smp + (size_t)j * 7;
+        const double t_next = j + 1 < f.m ? f.smp[(size_t)(j + 1) * 7] : f.t_end;
+        for (; q >= f.q0 && tq[q] >= d[0]; --q) {            // the rest of sample j from t
+            if (lane == 0) traj_a(W.A, d, Z.snap + (size_t)(r.t_off + q) * kTrajSnap + 144, t_next - tq[q], f.bg, f.ba);
+            __syncwarp();
+            emit(q, false);
+        }
+        if (j == 0 || q < f.q0) break;
+        if (lane == 0) {                                     // the whole sample j: lam <- A_j^T lam
+            traj_a(W.A, d, kq + 4 * j, t_next - d[0], f.bg, f.ba);
+            double y[9];
+            traj_at_vec(W.A, W.lam, y);
+            for (int i = 0; i < 9; ++i) W.lam[i] = y[i];
+        }
+        __syncwarp();
+        if (cv) {                                            // L <- A^T L, W <- A^T W A
+            traj_at_warp(W.A, V.L, V.X[0], false, lane);
+            for (int e = lane; e < 81; e += 32) V.L[e] = V.X[0][e];
+            traj_at_warp(W.A, V.W, V.X[0], false, lane);
+            traj_at_warp(W.A, V.X[0], V.X[1], true, lane);
+            for (int e = lane; e < 81; e += 32) V.W[e] = V.X[1][(e % 9) * 9 + e / 9];
+            __syncwarp();
+        }
     }
 }
 
@@ -327,6 +828,94 @@ struct CovPlan {
 }  // namespace pvio
 
 using namespace pvio;
+
+// pvio_b200_batch_window_trajectory and (smooth) pvio_b200_batch_window_smoothed_trajectory: one validation, staging
+// and download
+static int trajectory_call(pvio_b200_handle hh, int n, pvio_b200_window_trajectory *records, bool smooth) {
+    BwCall C(hh, smooth ? "batch_window_smoothed_trajectory" : "batch_window_trajectory");
+    if (!C.open(n, records)) return C.rc;
+    Handle *h = C.h;
+    // every record checked before anything is staged
+    std::vector<BwTraj> recs(n);
+    std::vector<double> times;
+    CovPlan P;
+    int64_t rows = 0, cov_rows = 0;
+    int warps = 1;
+    for (int i = 0; i < n; ++i) {
+        const pvio_b200_window_trajectory &R = records[i];
+        const WinSlot &s = h->slots[R.slot];
+        if (!s.inertial) return C.bad("a visual-only slot");
+        if (R.n_times < 0) return C.bad("a negative time count");
+        if (R.n_times > 0 && (!R.times || !R.states || !R.frame)) return C.bad("times, states or frame missing");
+        for (int q = 0; q < R.n_times; ++q) {
+            if (!std::isfinite(R.times[q])) return C.bad("a time that is not finite");
+            if (q > 0 && R.times[q] < R.times[q - 1]) return C.bad("times that decrease");
+        }
+        BwTraj &T = recs[i];
+        T = BwTraj{};
+        T.slot = R.slot; T.N = s.N; T.n_times = R.n_times; T.cov = -1; T.t_off = rows; T.scov_off = cov_rows;
+        std::vector<int32_t> owners;                 // the frames that own a factor with samples (smooth: and the
+        for (int k = 0; k + 1 < s.N; ++k) {          // frames after them)
+            T.ns[k] = s.n_samples.empty() ? 0 : s.n_samples[k];
+            if (T.ns[k] > 0 && (owners.empty() || owners.back() != k)) owners.push_back(k);
+            if (T.ns[k] > 0 && smooth) owners.push_back(k + 1);
+        }
+        warps = std::max(warps, s.N - 1);
+        if (R.state_cov && !owners.empty()) {        // their joint block
+            T.cov_off = P.cov_n;
+            T.cov = P.add(h, R.slot, (int)owners.size(), owners.data());
+            if (T.cov < 0) return C.bad("reduced system too large for shared memory");
+        }
+        if (R.state_cov) {
+            if (T.cov < 0) T.cov = -2;               // NaN rows only: no factor holds samples
+            cov_rows += R.n_times;
+        }
+        times.insert(times.end(), R.times, R.times + R.n_times);
+        rows += R.n_times;
+    }
+    const bool any_cov = cov_rows > 0;
+    Stage S(h->bw.stage, &h->bw.scratch);
+    const auto rec = S.up(recs);
+    const auto tm = S.up(times);
+    P.stage(S, h, Stage::kScratch);
+    const auto sto = S.add<double>(Stage::kDown, 16 * (size_t)rows);
+    const auto fro = S.add<int32_t>(Stage::kDown, (size_t)rows);
+    const auto sco = S.add<double>(Stage::kDown, 225 * (size_t)cov_rows);
+    const auto snap = S.add<double>(Stage::kScratch, smooth ? kTrajSnap * (size_t)rows : 0);
+    const auto knot = S.add<double>(Stage::kScratch, smooth ? (size_t)n * (kMaxFrames - 1) * h->bw.Scap * 4 : 0);
+    TRY(S.place(h, true));
+    TRY(P.run(h, S));
+    const TrajArgs T{S.dev(rec), S.dev(tm), S.dev(sto), S.dev(fro), S.dev(sco), S.dev(P.cov), S.dev(P.st), any_cov ? 1 : 0};
+    if (smooth) {
+        const size_t smem = traj_smooth_bytes(any_cov);
+        if (smem > 48 * 1024)
+            CK(h, cudaFuncSetAttribute(bw_smoothed_trajectory_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        bw_smoothed_trajectory_kernel<<<dim3(n, warps), 32, smem, h->stream>>>(launch_args<BwArgs>(h), T,
+                                                                             TrajSmooth{S.dev(snap), S.dev(knot)});
+        TRY(launched(h, "bw_smoothed_trajectory_kernel"));
+    } else {
+        const size_t smem = warps * traj_warp_bytes(any_cov);
+        if (smem > 48 * 1024)
+            CK(h, cudaFuncSetAttribute(bw_trajectory_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        bw_trajectory_kernel<<<n, 32 * warps, smem, h->stream>>>(launch_args<BwArgs>(h), T);
+        TRY(launched(h, "bw_trajectory_kernel"));
+    }
+    TRY(S.download(h));
+    CK(h, cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; ++i) {
+        pvio_b200_window_trajectory &R = records[i];
+        const BwTraj &T = recs[i];
+        const size_t nq = R.n_times;
+        if (nq > 0) {
+            memcpy(R.states, S.host(sto) + 16 * (size_t)T.t_off, sizeof(double) * 16 * nq);
+            memcpy(R.frame, S.host(fro) + T.t_off, sizeof(int32_t) * nq);
+            if (R.state_cov) memcpy(R.state_cov, S.host(sco) + 225 * (size_t)T.scov_off, sizeof(double) * 225 * nq);
+        }
+        R.status = T.cov >= 0 ? S.host(P.st)[T.cov] : PVIO_B200_OK;
+    }
+    return 0;
+}
+
 
 extern "C" {
 
@@ -474,76 +1063,11 @@ int pvio_b200_batch_window_landmarks(pvio_b200_handle hh, int n, pvio_b200_windo
 }
 
 int pvio_b200_batch_window_trajectory(pvio_b200_handle hh, int n, pvio_b200_window_trajectory *records) {
-    BwCall C(hh, "batch_window_trajectory");
-    if (!C.open(n, records)) return C.rc;
-    Handle *h = C.h;
-    // every record checked before anything is staged
-    std::vector<BwTraj> recs(n);
-    std::vector<double> times;
-    CovPlan P;
-    int64_t rows = 0, cov_rows = 0;
-    int warps = 1;
-    for (int i = 0; i < n; ++i) {
-        const pvio_b200_window_trajectory &R = records[i];
-        const WinSlot &s = h->slots[R.slot];
-        if (!s.inertial) return C.bad("a visual-only slot");
-        if (R.n_times < 0) return C.bad("a negative time count");
-        if (R.n_times > 0 && (!R.times || !R.states || !R.frame)) return C.bad("times, states or frame missing");
-        for (int q = 0; q < R.n_times; ++q) {
-            if (!std::isfinite(R.times[q])) return C.bad("a time that is not finite");
-            if (q > 0 && R.times[q] < R.times[q - 1]) return C.bad("times that decrease");
-        }
-        BwTraj &T = recs[i];
-        T = BwTraj{};
-        T.slot = R.slot; T.N = s.N; T.n_times = R.n_times; T.cov = -1; T.t_off = rows; T.scov_off = cov_rows;
-        std::vector<int32_t> owners;
-        for (int k = 0; k + 1 < s.N; ++k) {
-            T.ns[k] = s.n_samples.empty() ? 0 : s.n_samples[k];
-            if (T.ns[k] > 0) owners.push_back(k);
-        }
-        warps = std::max(warps, s.N - 1);
-        if (R.state_cov && !owners.empty()) {        // Sigma_k of the frames that own a factor with samples
-            T.cov_off = P.cov_n;
-            T.cov = P.add(h, R.slot, (int)owners.size(), owners.data());
-            if (T.cov < 0) return C.bad("reduced system too large for shared memory");
-        }
-        if (R.state_cov) {
-            if (T.cov < 0) T.cov = -2;               // NaN rows only: no factor holds samples
-            cov_rows += R.n_times;
-        }
-        times.insert(times.end(), R.times, R.times + R.n_times);
-        rows += R.n_times;
-    }
-    const bool any_cov = cov_rows > 0;
-    Stage S(h->bw.stage, &h->bw.scratch);
-    const auto rec = S.up(recs);
-    const auto tm = S.up(times);
-    P.stage(S, h, Stage::kScratch);
-    const auto sto = S.add<double>(Stage::kDown, 16 * (size_t)rows);
-    const auto fro = S.add<int32_t>(Stage::kDown, (size_t)rows);
-    const auto sco = S.add<double>(Stage::kDown, 225 * (size_t)cov_rows);
-    TRY(S.place(h, true));
-    TRY(P.run(h, S));
-    const TrajArgs T{S.dev(rec), S.dev(tm), S.dev(sto), S.dev(fro), S.dev(sco), S.dev(P.cov), S.dev(P.st), any_cov ? 1 : 0};
-    const size_t smem = warps * traj_warp_bytes(any_cov);
-    if (smem > 48 * 1024)
-        CK(h, cudaFuncSetAttribute(bw_trajectory_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    bw_trajectory_kernel<<<n, 32 * warps, smem, h->stream>>>(launch_args<BwArgs>(h), T);
-    TRY(launched(h, "bw_trajectory_kernel"));
-    TRY(S.download(h));
-    CK(h, cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < n; ++i) {
-        pvio_b200_window_trajectory &R = records[i];
-        const BwTraj &T = recs[i];
-        const size_t nq = R.n_times;
-        if (nq > 0) {
-            memcpy(R.states, S.host(sto) + 16 * (size_t)T.t_off, sizeof(double) * 16 * nq);
-            memcpy(R.frame, S.host(fro) + T.t_off, sizeof(int32_t) * nq);
-            if (R.state_cov) memcpy(R.state_cov, S.host(sco) + 225 * (size_t)T.scov_off, sizeof(double) * 225 * nq);
-        }
-        R.status = T.cov >= 0 ? S.host(P.st)[T.cov] : PVIO_B200_OK;
-    }
-    return 0;
+    return trajectory_call(hh, n, records, false);
+}
+
+int pvio_b200_batch_window_smoothed_trajectory(pvio_b200_handle hh, int n, pvio_b200_window_trajectory *records) {
+    return trajectory_call(hh, n, records, true);
 }
 
 }  // extern "C"

@@ -37,14 +37,13 @@ struct ImuFactorJac {
     const double *dp, *dv, *dq_dbg, *dp_dbg, *dp_dba, *dv_dbg, *dv_dba;
 };
 
-// In: A = Sigma_src, D = Sigma_d; Rs = R(q_src), dR = R(delta q).  Out: A = Phi Sigma_src Phi^T, D = Psi Sigma_d Psi^T
-// (the caller adds and symmetrises them); B and C are scratch.
-static __device__ __forceinline__ void imu_factor_propagate(double *A, double *B, double *C, double *D,
-                                                            const ImuFactorJac &f, const double Rs[9],
-                                                            const double dR[9], int lane) {
+// Phi into B (15 x 15, zeroed here): the Jacobian of PreIntegrator::predict in the source state, through the factor's
+// bias Jacobians; Rs = R(q_src), dR = R(delta q)
+static __device__ __forceinline__ void imu_factor_phi(double *B, const ImuFactorJac &f, const double Rs[9],
+                                                      const double dR[9], int lane) {
     for (int e = lane; e < 225; e += 32) B[e] = 0.0;
     __syncwarp();
-    if (lane == 0) {                                 // Phi into B
+    if (lane == 0) {
         double H[9], X[9], Xt[9];
         for (int r = 0; r < 3; ++r)
             for (int c = 0; c < 3; ++c) Xt[3 * r + c] = dR[3 * c + r];
@@ -71,6 +70,14 @@ static __device__ __forceinline__ void imu_factor_propagate(double *A, double *B
         put_block(B, 4, 4, nullptr);
     }
     __syncwarp();
+}
+
+// In: A = Sigma_src, D = Sigma_d; Rs = R(q_src), dR = R(delta q).  Out: A = Phi Sigma_src Phi^T, D = Psi Sigma_d Psi^T
+// (the caller adds and symmetrises them); B and C are scratch.
+static __device__ __forceinline__ void imu_factor_propagate(double *A, double *B, double *C, double *D,
+                                                            const ImuFactorJac &f, const double Rs[9],
+                                                            const double dR[9], int lane) {
+    imu_factor_phi(B, f, Rs, dR, lane);              // Phi into B
     warp_mm15(B, A, C, false, lane);                 // Phi Sigma_src
     warp_mm15(C, B, A, true, lane);                  // .. Phi^T, into A
     if (lane == 0) {                                 // Psi into B
