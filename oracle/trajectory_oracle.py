@@ -14,6 +14,13 @@ def _holds(f):
     return f[0] is not None and len(f[0]) > 0
 
 
+def noise_of(noise, k):
+    """factor k's noise (cov_w, cov_a, cov_bg, cov_ba): noise is one such tuple for every factor, or a list of one per
+    factor (None for a factor without samples)"""
+    per_factor = len(noise) > 0 and (noise[0] is None or np.ndim(noise[0]) == 3)
+    return noise[k] if per_factor else noise
+
+
 def factor_of(t, factors):
     """the factor k that takes time t: the largest k holding samples with s_0.t <= t, when t <= its t_end or factor
     k + 1 holds samples too; -1 when none does"""
@@ -69,7 +76,8 @@ def propagate(x_k, d, Sig_k):
 
 
 def trajectory(times, frames, factors, noise, Sig=None):
-    """frames [N][16] the window's states; factors as above; noise (cov_w, cov_a, cov_bg, cov_ba); Sig: per frame its
+    """frames [N][16] the window's states; factors as above; noise (cov_w, cov_a, cov_bg, cov_ba), or one such tuple per
+    factor (noise_of); Sig: per frame its
     15 x 15 marginal covariance (None: no covariances).  Returns (frame [n], states [n][16], covs [n][15][15] or None):
     frame -1 with a zero state and a NaN covariance for a time no factor takes."""
     n = len(times)
@@ -80,7 +88,7 @@ def trajectory(times, frames, factors, noise, Sig=None):
         if k < 0:
             continue
         x = np.asarray(frames[k], dtype=np.float64)
-        d = delta(factors[k][0], t, x[10:13], x[13:16], noise)
+        d = delta(factors[k][0], t, x[10:13], x[13:16], noise_of(noise, k))
         fr[i], st[i] = k, sco.predict(x, d)
         if Sig is not None:
             cov[i] = propagate(x, d, Sig[k])

@@ -13,7 +13,7 @@ import numpy as np
 from oracle import imu_oracle
 from oracle import imu_stream_cov_oracle as sco
 from oracle import lie
-from oracle.trajectory_oracle import delta, factor_of
+from oracle.trajectory_oracle import delta, factor_of, noise_of
 
 _G = sco.GRAVITY
 
@@ -84,12 +84,28 @@ def cross_cov(samples, t, t_end, bg, ba, noise):
     P = np.block([[S, S], [S, S]])
     j = int(np.flatnonzero(s[:, 0] <= t)[-1])
     knots = list(s[:, 0]) + [float(t_end)]
+    kq = _knot_rotations(s, bg) if np.all(np.diff(s[:, 0]) > 0) else None
     q, t0 = d["dq"], t
     for i in range(j, len(s)):
         P = _aug_step(P, q, s[i], knots[i + 1] - t0, bg, ba, nz)
         if i + 1 < len(s):
-            q, t0 = delta(s, knots[i + 1], bg, ba, noise)["dq"], knots[i + 1]
+            q = delta(s, knots[i + 1], bg, ba, noise)["dq"] if kq is None else kq[i + 1]
+            t0 = knots[i + 1]
     return P[0:15, 15:30]
+
+
+def _knot_rotations(s, bg):
+    """delta(s, s_i.t, bg, ...)["dq"] for every sample i of strictly increasing times, in one pass instead of one
+    prefix integration per knot: imu_oracle.integrate's rotation chain over samples 0 .. i - 1, then the zero-length
+    step of sample i that closes a prefix ending at s_i.t -- the same operations in the same order, so the same bits"""
+    bg = np.asarray(bg, dtype=np.float64)
+    dq, out = np.array([0.0, 0.0, 0.0, 1.0]), []
+    for i in range(len(s)):
+        w = s[i, 1:4] - bg
+        out.append(lie.qnormalized(lie.qmul(dq, lie.expmap(w * (s[i, 0] - s[i, 0])))))
+        if i + 1 < len(s):
+            dq = lie.qnormalized(lie.qmul(dq, lie.expmap(w * (s[i + 1, 0] - s[i, 0]))))
+    return out
 
 
 def gain(samples, t, t_end, bg, ba, noise):
@@ -157,7 +173,7 @@ def jacobians(x_k, x_k1, d, dT, K):
 
 
 def smoothed(times, frames, factors, noise, Sig_joint=None):
-    """frames, factors, noise as trajectory(); Sig_joint: the 15 N x 15 N joint covariance of the window's frames (None:
+    """frames, factors, noise as trajectory() (one tuple, or one per factor); Sig_joint: the 15 N x 15 N joint covariance of the window's frames (None:
     no covariances).  Returns (frame [n], states [n][16], covs [n][15][15] or None): frame as trajectory() gives it, or
     -2 with a zero state and a NaN covariance when the factor's Sigma(T) is not positive definite."""
     n = len(times)
@@ -168,7 +184,7 @@ def smoothed(times, frames, factors, noise, Sig_joint=None):
         if k < 0:
             continue
         x, x1 = np.asarray(frames[k], dtype=np.float64), np.asarray(frames[k + 1], dtype=np.float64)
-        g = gain(factors[k][0], t, factors[k][1], x[10:13], x[13:16], noise)
+        g = gain(factors[k][0], t, factors[k][1], x[10:13], x[13:16], noise_of(noise, k))
         if g is None:
             fr[i] = -2
             continue
